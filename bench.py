@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - HSTU training sequences/sec (BASELINE.json metric) on N B200s of one node.
+"""bench.py - HSTU training sequences/sec (BASELINE.json metric) on N H100s of one node.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
@@ -10,7 +10,7 @@ embedding gather -> 4 HSTU blocks -> final LN -> tied logits + CE -> backward ->
 
 One JSON line on stdout (rank 0):  value = whole-job sequences/s with the batch already resident in HBM;
 e2e = the same through the public nn.Module API with pinned-host inputs copied H2D and the loss read back D2H every
-step; roofline = the HSTU block stack (fwd+bwd, 4 layers) against the measured bf16 peak; cpu_baseline = the oracle port
+step; roofline = the HSTU block stack (fwd+bwd, 4 layers) against the dense bf16 peak; cpu_baseline = the oracle port
 of the reference's CPU-eager path on this box's host cores (bounded sample).
 """
 from __future__ import annotations
@@ -57,6 +57,8 @@ def parse():
     ap.add_argument("--skip-cpu", action="store_true")
     ap.add_argument("--skip-eager", action="store_true")
     ap.add_argument("--skip-roofline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps write the last step's loss and updated parameters to DIR/<name>.npy")
     args = ap.parse_args()
     c = CONFIGS[args.config]
     CFG.clear(); CFG.update(c["model"])
@@ -175,7 +177,7 @@ def cpu_arm(batch, L, seconds, steps=None, warmup=1):
 
 def cuda_eager_arm(batch, L, dev, steps, warmup=2):
     """The reference's algorithm as plain PyTorch eager ON THE SAME GPU (oracle restatement, torch.autocast(bf16), dropout 0, Adam):
-    the "beat this on the same box" number of BASELINE.md section 2.2 - the reference ships no kernel of its own."""
+    the "beat this on the same box" number - the reference ships no kernel of its own."""
     from oracle import hstu as oh
     from genrec_b200.hstu import HSTU
     torch.manual_seed(0)
@@ -360,6 +362,8 @@ def run_ours(args, rank, world, local_rank):
     clocks = sampler.stop() if rank == 0 else None
     ms_e2e, wall_e2e, pct_e2e = timed(load_host, sync_each=True)
     final_loss = float(loss_static.detach().float().item())
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, loss_static, model)
 
     # ---- roofline of the HSTU block stack (fwd+bwd), device-timed inside a graph
     roof = None
@@ -398,7 +402,7 @@ def run_ours(args, rank, world, local_rank):
                                      f"{'all-reduce, ' if world > 1 else ''}Adam)", name=args.config,
                             global_batch=gb, batch_per_gpu=B, seq_len=L, parallelism=f"dp{world}",
                             cuda_graph=used_graph, dp_mode=opt.dp_mode,
-                            l2="per-step working set (activations + logits, > 1 GB) exceeds the 126 MB L2; no explicit flush",
+                            l2="per-step working set (activations + logits, > 1 GB) exceeds the 50 MB L2; no explicit flush",
                             final_loss=final_loss, ms_per_step_pct=pct_dev),
                 e2e=dict(value=gb * K / (ms_e2e * 1e-3), unit=UNIT, h2d_bytes_per_step=h2d, d2h_bytes_per_step=4,
                          ms_per_step=ms_e2e / K, wall_ms_per_step=wall_e2e / K, ms_per_step_pct=pct_e2e),
@@ -406,22 +410,37 @@ def run_ours(args, rank, world, local_rank):
     emit(line)
 
 
-# DRAM bytes (dram__bytes_read.sum + dram__bytes_write.sum) of the block stack's kernels for one fwd+bwd, from the committed ncu
-# capture of the same command (profiles/*_step_dram_traffic.txt, scripts/step_traffic.py); keyed by (B, L, D, layers)
-TRAFFIC_NCU = {(128, 200, 128, 4): 2.023e9,      # profiles/r2_step_cfg2_dram_traffic.txt
-               (32, 2048, 256, 8): 38.780e9}     # profiles/r2_step_cfg3_dram_traffic.txt
+DUMP_MAX_ELEMS = (16 << 20) - 1   # all arrays together: 64 MB of float32 with the loss
+
+
+def dump_outputs(out_dir, loss, model):
+    """What the timed training step hands its caller after the last timed step: the loss and every parameter as Adam left it
+    (float32 .npy files, keyed by parameter name).  When the parameters exceed DUMP_MAX_ELEMS elements in all, every tensor is
+    written as a sample of its elements in proportion to its size, at the same seeded indices on every run."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray(loss.detach().float().cpu().numpy(), dtype=np.float32))
+    params = list(model.named_parameters())
+    total = sum(p.numel() for _, p in params)
+    for name, p in params:
+        flat = p.detach().float().reshape(-1).cpu()
+        keep = flat.numel() if total <= DUMP_MAX_ELEMS else max(1, flat.numel() * DUMP_MAX_ELEMS // total)
+        if keep < flat.numel():
+            idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            flat = flat[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), flat.numpy().astype(np.float32).reshape(p.shape if keep == p.numel() else (-1,)))
 
 
 def block_roofline(model, B, L, dev, K):
     """fwd+bwd of the HSTU block stack alone (no embedding / head / optimizer): algorithmic FLOPs (SURVEY.md section 8d:
-    72 L D^2 + 6 D L (L+1) per sequence-layer) / CUDA-event time, vs the measured dense bf16 peak."""
+    72 L D^2 + 6 D L (L+1) per sequence-layer) / CUDA-event time, vs the dense bf16 peak."""
     D, nl = CFG["embed_dim"], CFG["num_blocks"]
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak, which = (peaks["bf16_tflops"], "measured (burst)") if "bf16_tflops" in peaks else (1590.0, "fallback")
+    peak, which = (peaks["bf16_tflops"], "measured (burst)") if "bf16_tflops" in peaks else (989.0, "H100 SXM data sheet, dense bf16 at 700 W")
     ids, ts, _ = synth_batch(B, L, CFG["num_items"], 7)
     ids, ts = ids.to(dev), ts.to(dev)
     x0 = torch.randn(B, L, D, device=dev)
@@ -464,11 +483,8 @@ def block_roofline(model, B, L, dev, K):
     model.zero_grad(set_to_none=False)
     flops = (72 * L * D * D + 6 * D * L * (L + 1)) * B * nl
     ach = flops / (ms * 1e-3) / 1e12
-    # DRAM bytes (read + write) of the block stack's kernels for one fwd+bwd at the default geometry, summed from the ncu
-    # captures profiles/r2_step_cfg{2,3}_dram_traffic.txt (scripts/step_traffic.py); not re-measured here (needs a profiler)
-    traffic = TRAFFIC_NCU.get((B, L, D, nl))
     return dict(bound="tensor", kernel="hstu_block_stack_fwd_bwd", achieved=ach, peak=peak, unit="TFLOP/s", frac=ach / peak,
-                peak_source=which, traffic=traffic, traffic_unit="bytes per launch (ncu dram__bytes_read.sum + dram__bytes_write.sum)",
+                peak_source=which,
                 algorithmic_bytes_per_launch=(10 * L * D + 9 * L) * B * nl, ms_per_launch=ms, flops_per_launch=flops,
                 unit_of_work=f"{nl} layers x B={B} sequences x L={L}")
 

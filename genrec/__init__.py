@@ -1,5 +1,5 @@
 """Import-path shim: ``genrec.models.{hstu,sasrec,rqvae}`` and ``genrec.data.{amazon_hstu,amazon_sasrec}`` resolve to the
-B200-native modules in ``genrec_b200`` so that the reference's gin files (``import genrec.data.amazon_hstu`` /
+H100-native modules in ``genrec_b200`` so that the reference's gin files (``import genrec.data.amazon_hstu`` /
 ``import genrec.models.hstu``, config/hstu/amazon.gin:5-6) and trainers find the hot path under the names they already use.
 
 This package does NOT shadow the rest of the reference: every level extends its ``__path__`` over all ``genrec`` directories on

@@ -1,4 +1,4 @@
-"""genrec_b200 - B200-native (sm_100a) implementation of the sequential-attention hot path of phonism/genrec.
+"""genrec_b200 - H100-native (sm_90a) implementation of the sequential-attention hot path of phonism/genrec.
 
 Public surface (mirrors the reference's import paths through the thin ``genrec`` shim package at the repo root):
     genrec_b200.hstu    HSTU, HSTULayer, RelativePositionBias, TemporalBias

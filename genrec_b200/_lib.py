@@ -1,6 +1,6 @@
 """ctypes binding of include/genrec_b200.h - the reference-side stub a genrec maintainer would add (INTEGRATION.md).
 
-There is NO fallback: if the shared library is missing or the device is not sm_100, importing callers get a
+There is NO fallback: if the shared library is missing or the device is not sm_90, importing callers get a
 RuntimeError that says how to build.  Nothing here touches ``oracle/``.
 """
 from __future__ import annotations
@@ -72,8 +72,8 @@ SIGNATURES = {
     "grb_collate_jagged": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_embed_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int,
                                   c_float, c_u64, c_void_p, c_void_p]),
-    "grb_embed_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int, c_float,
-                                   c_u64, c_void_p, c_void_p]),
+    "grb_embed_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int, c_float,
+                                   c_u64, c_void_p, c_void_p, c_void_p]),
     "grb_head_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "grb_head_loss_forward_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_int, c_int, c_int,
                                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -134,7 +134,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"genrec_b200: {LIB_PATH} is missing.  Build it with `python -m genrec_b200.build` "
-            "(nvcc, sm_100a).  There is no CPU or PyTorch fallback for this path.")
+            "(nvcc, sm_90a).  There is no CPU or PyTorch fallback for this path.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)
@@ -164,7 +164,7 @@ def stream_ptr(device) -> int:
 def require_cuda(*tensors: Optional[torch.Tensor]) -> None:
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("genrec_b200 ops run on CUDA (sm_100a) tensors only - there is no CPU fallback; "
+            raise RuntimeError("genrec_b200 ops run on CUDA (sm_90a) tensors only - there is no CPU fallback; "
                                f"got a tensor on {t.device}")
 
 

@@ -1,6 +1,6 @@
-"""Build recipe for the sm_100a C-ABI library (in-tree: genrec_b200/libgenrec_b200.so).
+"""Build recipe for the sm_90a C-ABI library (in-tree: genrec_b200/libgenrec_b200.so).
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels to the GPU box with the repo snapshot.
+nvcc cross-compiles without a GPU.  The .so is a build product (git-ignored); build() makes it in the package directory.
 """
 from __future__ import annotations
 
@@ -14,7 +14,7 @@ LIB = os.path.join(HERE, "libgenrec_b200.so")
 # --use_fast_math: flush-to-zero + approximate div/sqrt.  Without .ftz every ex2.approx / rcp.approx in the SiLU, softmax and
 # cross-entropy inner loops carries a 3-instruction denormal fix-up (FSETP + 2 predicated FMUL); the operands are bf16-rounded
 # activations, so denormal inputs carry no information here.
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

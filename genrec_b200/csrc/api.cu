@@ -5,6 +5,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <map>
 #include <mutex>
 #include <utility>
@@ -12,7 +13,7 @@
 #include "attn_hstu.cuh"
 #include "attn_sasrec.cuh"
 #include "attn_t5.cuh"
-#include "attn_tc.cuh"
+#include "attn_buckets.cuh"
 #include "beam.cuh"
 #include "common.cuh"
 #include "dp_adam.cuh"
@@ -22,7 +23,6 @@
 #include "rq_argmin.cuh"
 #include "tc_gemm.cuh"
 #include "tc_ce.cuh"
-#include "tc_ffn.cuh"
 #include "tc_tn_group.cuh"
 #include <cstdlib>
 
@@ -69,27 +69,50 @@ int sm_count() {     // per device ordinal: a process may drive several GPUs
     if (n[dev] == 0) {
         int v = 0;
         cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-        n[dev] = v > 0 ? v : 148;
+        n[dev] = v > 0 ? v : 132;
     }
     return n[dev];
 }
-// GRB_CE = store : G' stored, dE by the TN GEMM (round-1 schedule; always at D = 256)
-//          exact : no [T, C] tensor, two class sweeps (the exponent shift is the exact row maximum)
-//          (default) : no [T, C] tensor, ONE class sweep (shift = max(probe-tile maximum, target logit), see tc_ce.cuh)
-int ce_mode_env() {
-    static const int v = [] {
-        const char* e = getenv("GRB_CE");
-        if (e && !strcmp(e, "store")) return (int)CE_STORE_G;
-        if (e && (!strcmp(e, "exact") || !strcmp(e, "keep"))) return (int)CE_KEEP_G;
-        return (int)CE_ONE_SWEEP;
-    }();
-    return v;
-}
-bool ce_store_forced() { return ce_mode_env() == CE_STORE_G; }
 int row_grid(int T) {
     int need = (T + ROW_THREADS / 32 - 1) / (ROW_THREADS / 32);
     int cap = sm_count() * 8;
     return need < cap ? (need < 1 ? 1 : need) : cap;
+}
+int row_bwd_grid(int T) {
+    const int need = (T + ROW_THREADS / 32 - 1) / (ROW_THREADS / 32), cap = sm_count() * 3;
+    return need < cap ? (need < 1 ? 1 : need) : cap;
+}
+// grids of the column-sum kernels (their partial scratch is sized from them)
+dim3 colsum_grid(int T, int N) {
+    const int cx = (N + 255) / 256, maxy = (T + 63) / 64;
+    int cy = (4 * sm_count() + cx - 1) / cx;
+    cy = cy > maxy ? maxy : cy;
+    return dim3(cx, cy < 1 ? 1 : cy);
+}
+dim3 cast_colsum_grid(int T, int D) {
+    const int cx = (D + 127) / 128, maxy = (T + 31) / 32;
+    int cy = (8 * sm_count() + cx - 1) / cx;
+    cy = cy > maxy ? maxy : cy;
+    return dim3(cx, cy < 1 ? 1 : cy);
+}
+size_t attn_dw_part_floats(int B, int L, int H) { return (size_t)2 * H * B * ((L + ATT_BLK - 1) / ATT_BLK) * 64; }
+// the ordered sum of the per-CTA partials a kernel left in `part` (common.cuh det_store, layout [group][member][W]): group g,
+// element i -> out[g / gpo][(g % gpo) * gstride + i * estride] when that index < len[g / gpo]
+struct DetOut {
+    float* out;
+    int len;
+};
+int det_finish(const float* part, int ngroups, int nmembers, int W, int gpo, int gstride, int estride, std::initializer_list<DetOut> outs,
+               cudaStream_t st) {
+    DetFinishArgs f;
+    memset(&f, 0, sizeof(f));
+    f.part = part; f.ngroups = ngroups; f.nmembers = nmembers; f.W = W; f.gpo = gpo; f.gstride = gstride; f.estride = estride;
+    int k = 0;
+    for (const DetOut& o : outs) { f.out[k] = o.out; f.len[k] = o.len; ++k; }
+    const unsigned blocks = (unsigned)(((size_t)ngroups * W * 32 + 255) / 256);
+    launch_k(det_finish_kernel, blocks, 256, 0, st, f);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
 }
 int splitk_for(int M, int N, int K) {
     int tiles = ((M + GEMM_BM - 1) / GEMM_BM) * ((N + GEMM_BN - 1) / GEMM_BN);
@@ -100,7 +123,7 @@ int splitk_for(int M, int N, int K) {
 }
 
 
-// ---- GEMM dispatch: tcgen05/TMA path (default) or the first-generation mma.sync path (GRB_GEMM=mma, kept as an on-device
+// ---- GEMM dispatch: wgmma/TMA path (default) or the first-generation mma.sync path (GRB_GEMM=mma, kept as an on-device
 //      cross-check).  Operand majors: *_MN = 0 -> K contiguous, 1 -> M/N contiguous (see tc_gemm.cuh / gemm.cuh).
 bool use_tc() {
     static int v = -1;
@@ -155,10 +178,10 @@ cudaError_t gemm_tn_atomic(const bf16* A, const bf16* B, float* out, int M, int 
     if (use_tc()) return launch_tc_gemm<1, 1>(A, B, M, N, K, lda, ldb, tn_splits(M, N, K), TcEpiAtomicF32{out, N, 1.f}, nullptr, nullptr, 0, sm_count(), st);
     return launch_gemm<1, 1>(A, B, M, N, K, lda, ldb, splitk_for(M, N, K), EpiAtomicF32{out, N, 1.f}, st);
 }
-// out[M,N] bf16 (leading dim ldo) = A[M,K] B[N,K]^T   (NT)
-cudaError_t gemm_nt_bf16(const bf16* A, const bf16* B, bf16* out, int ldo, int M, int N, int K, cudaStream_t st) {
-    if (use_tc()) return launch_tc_gemm<0, 0>(A, B, M, N, K, K, K, 1, TcEpiBf16{}, out, nullptr, ldo, sm_count(), st);
-    return launch_gemm<0, 0>(A, B, M, N, K, K, K, 1, EpiBf16{out, ldo}, st);
+// out[M,N] fp32 (leading dim ldo, a multiple of 4) = A[M,K] B[N,K]^T   (NT)
+cudaError_t gemm_nt_f32(const bf16* A, const bf16* B, float* out, int ldo, int M, int N, int K, cudaStream_t st) {
+    if (use_tc()) return launch_tc_gemm<0, 0>(A, B, M, N, K, K, K, 1, TcEpiF32{nullptr, ldo, 1.f}, out, nullptr, ldo, sm_count(), st);
+    return launch_gemm<0, 0>(A, B, M, N, K, K, K, 1, EpiF32Scalar{out, ldo, N}, st);
 }
 // out[M,N] fp32 (leading dim N, any parity) = A B^T   (NT)
 cudaError_t gemm_nt_f32_plain(const bf16* A, const bf16* B, float* out, int M, int N, int K, cudaStream_t st) {
@@ -192,10 +215,19 @@ LayerSaved carve_saved(void* base, size_t T, size_t D) {
 }
 struct LayerWork {
     bf16 *dyb, *dz1, *dO, *dzp;
-    float *dxn, *dx1, *dq_acc;
+    float *dxn, *dx1;
+    // scratch of the ordered cross-CTA sums: weight-gradient split-K tiles, bias column sums, LayerNorm and bias-table gradients
+    float *part_tn, *part_colsum, *part_cast, *part_ln, *part_attn;
     size_t bytes;
 };
-LayerWork carve_work(void* base, size_t T, size_t D) {
+void layer_tn_specs(TnSpec (&specs)[3], const bf16* dyb, const bf16* hact, const bf16* dz1, const bf16* xn, const bf16* dzp, const bf16* xb,
+                    float* dw2, float* dw1, float* dwp, int T, int D) {
+    specs[0] = {dyb, hact, dw2, D, 4 * D, T, D, 4 * D, 4 * D};   // dW2 += dyb^T h
+    specs[1] = {dz1, xn, dw1, 4 * D, D, T, 4 * D, D, D};         // dW1 += dz1^T xn
+    specs[2] = {dzp, xb, dwp, 4 * D, D, T, 4 * D, D, D};         // dWp += dzp^T xb
+}
+LayerWork carve_work(void* base, const grb_hstu_dims* d) {
+    const size_t T = (size_t)d->B * d->L, D = d->D;
     LayerWork w;
     size_t off = 0;
     char* b = static_cast<char*>(base);
@@ -206,7 +238,14 @@ LayerWork carve_work(void* base, size_t T, size_t D) {
     w.dx1 = (float*)take(T * D * 4);
     w.dO = (bf16*)take(T * D * 2);
     w.dzp = (bf16*)take(T * 4 * D * 2);
-    w.dq_acc = (float*)take(T * D * 4);
+    TnSpec specs[3];
+    layer_tn_specs(specs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, (int)T, (int)D);
+    w.part_tn = (float*)take(tn_part_floats(specs, 3, sm_count()) * 4);
+    const dim3 cg = colsum_grid((int)T, 4 * (int)D), kg = cast_colsum_grid((int)T, (int)D);
+    w.part_colsum = (float*)take((size_t)cg.x * cg.y * 256 * 4);
+    w.part_cast = (float*)take((size_t)kg.x * kg.y * 128 * 4);
+    w.part_ln = (float*)take((size_t)4 * row_grid((int)T) * D * 4);
+    w.part_attn = (float*)take(attn_dw_part_floats(d->B, d->L, d->H) * 4);
     w.bytes = off;
     return w;
 }
@@ -338,8 +377,7 @@ int join_pending(cudaStream_t st) {
 bool use_side_stream() {
     static int v = -1;
     if (v < 0) {
-        // dQ and dK/dV side by side: +1.6 % step throughput at cfg-2 (1.786 -> 1.758 ms) once the weight-gradient GEMMs had moved
-        // off the critical path; GRB_SIDE_STREAM=0 serialises them again
+        // dQ and dK/dV side by side (the two backward kernels are independent); GRB_SIDE_STREAM=0 serialises them
         const char* e = getenv("GRB_SIDE_STREAM");
         v = (e && strcmp(e, "0") == 0) ? 0 : 1;
     }
@@ -366,6 +404,8 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
     }
     size_t smem_k = sizeof(AttSmemKV<DH>) + posb + (size_t)4 * (a.bias.ntime + 1 + (a.bias.pos_uniform ? 0 : a.bias.npos + 1)) * 32 * sizeof(float);
     const bool has_time = a.bias.wtime != nullptr && a.bias.ntime > 0, pos_uni = a.bias.pos_uniform != 0;
+    const int nmem = (int)(grid.x * grid.z), ngroups = has_time && a.dwtime ? 2 * a.H : a.H;
+    GRB_REQUIRE((pos_uni || a.bias.npos <= 64) && a.bias.ntime <= 64, "attention backward: at most 64 position / time buckets");
     auto go = [&](auto kern) -> int {
         GRB_TRY(set_smem(kern, smem_k));
         launch_k(kern, grid, ATT_THREADS, smem_k, st, a, (int)posb);
@@ -375,104 +415,15 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
     else if (has_time) GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, true, false>));
     else if (pos_uni) GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, false, true>));
     else GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, false, false>));
+    if (a.dw_part) {
+        // groups h < H: position buckets of head h ; H + h: time buckets of head h ; element = bucket
+        float* pos_out = a.dwpos + (pos_uni ? (size_t)a.bias.pos_bucket0 * a.H : 0);
+        const int pos_len = pos_uni ? a.H : a.bias.npos * a.H;
+        if (ngroups > a.H) GRB_TRY(det_finish(a.dw_part, ngroups, nmem, 64, a.H, 1, a.H, {{pos_out, pos_len}, {a.dwtime, a.bias.ntime * a.H}}, st));
+        else GRB_TRY(det_finish(a.dw_part, ngroups, nmem, 64, a.H, 1, a.H, {{pos_out, pos_len}}, st));
+    }
     GRB_CUDA(cudaGetLastError());
     if (forked) GRB_CUDA(cudaStreamWaitEvent(st, ss.join, 0));
-    return 0;
-}
-
-// ---- tcgen05 attention path (attn_tc.cuh): the default whenever the position buckets are uniform (the reference's behaviour)
-//      and head_dim is 32 or 64.  GRB_ATTN=mma selects the first-generation mma.sync kernels (they need the bias_index matrix).
-// GRB_ATTN = tc | mma | auto (default).  auto: the tcgen05 kernels for seq_len > 256, the mma.sync kernels below - measured on
-// B200 (scripts/bench_attn.py): with 128-row tiles and one thread per TMEM lane a 200-token sequence leaves 40 % of the lanes idle and a
-// CTA lives for only a handful of tiles, so the 64-row mma.sync kernels (5 CTAs per SM) are still ahead there; from ~512 tokens on
-// the tcgen05 path wins and needs no [B, L, L] index.  Read on every call so that a test can flip it.
-int attn_mode() {
-    const char* e = getenv("GRB_ATTN");
-    if (e && strcmp(e, "mma") == 0) return 0;
-    if (e && strcmp(e, "tc") == 0) return 1;
-    return 2;
-}
-bool attn_tc_possible(const grb_hstu_dims* d, const grb_hstu_seq* s);
-bool use_attn_tc(const grb_hstu_dims* d, const grb_hstu_seq* s) {
-    const int mode = attn_mode();
-    if (mode == 0 || (mode == 2 && d->L <= 256 && s->bias_index != nullptr)) return false;
-    return attn_tc_possible(d, s);
-}
-bool attn_tc_possible(const grb_hstu_dims* d, const grb_hstu_seq* s) {
-    const int dh = d->D / d->H;
-    return s->pos_uniform && (dh == 32 || dh == 64) && d->D % 64 == 0 && s->pad != nullptr && s->time_thr != nullptr &&
-           (s->timestamps == nullptr || !s->has_time || (s->rel32 != nullptr && s->wide != nullptr));
-}
-HstuTcArgs make_tc_args(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s) {
-    HstuTcArgs a;
-    memset(&a, 0, sizeof(a));
-    const bool has_time = time_table != nullptr && s->has_time && s->timestamps != nullptr && d->ntime > 0;
-    a.ts = has_time ? reinterpret_cast<const long long*>(s->timestamps) : nullptr;
-    a.rel32 = has_time ? s->rel32 : nullptr;
-    a.wide = s->wide;
-    a.pad = s->pad;
-    a.thr64 = reinterpret_cast<const long long*>(s->time_thr);
-    a.wpos = pos_table + (size_t)s->pos_bucket0 * d->H;
-    a.wtime = has_time ? time_table : nullptr;
-    a.ntime = has_time ? d->ntime : 0;
-    a.B = d->B; a.L = d->L; a.H = d->H; a.D = d->D;
-    return a;
-}
-int launch_attn_tc_fwd(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s, const bf16* P, bf16* O,
-                       cudaStream_t st) {
-    const int D = d->D, dh = D / d->H;
-    const size_t T = (size_t)d->B * d->L;
-    HstuTcArgs a = make_tc_args(d, pos_table, time_table, s);
-    a.o = O; a.ldo = D;
-    CUtensorMap tmP;
-    if (!make_tmap_bf16(&tmP, P, T, 4 * (size_t)D, 4 * (size_t)D, 64, 128)) return fail(GRB_EINVAL, "tensor map creation failed (attention P)");
-    const int nqt = (d->L + 127) / 128;
-    const unsigned grid = (unsigned)((D / 64) * d->B * nqt);
-    if (dh == 32) {
-        const size_t smem = AtcFwdSmem<32>::kBytes + 1024;
-        GRB_TRY(set_smem(hstu_attn_tc_fwd_kernel<32>, smem));
-        launch_k(hstu_attn_tc_fwd_kernel<32>, grid, ATC_THREADS, smem, st, tmP, a, nqt);
-    } else {
-        const size_t smem = AtcFwdSmem<64>::kBytes + 1024;
-        GRB_TRY(set_smem(hstu_attn_tc_fwd_kernel<64>, smem));
-        launch_k(hstu_attn_tc_fwd_kernel<64>, grid, ATC_THREADS, smem, st, tmP, a, nqt);
-    }
-    GRB_CUDA(cudaGetLastError());
-    return 0;
-}
-// dzp columns V, Q, K <- gradients w.r.t. the pre-activations ; dq_acc: [T, D] fp32 scratch
-int launch_attn_tc_bwd(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s, const bf16* P,
-                       const bf16* zp, const bf16* dO, bf16* dzp, float* dwpos, float* dwtime, float* dq_acc, cudaStream_t st) {
-    const int D = d->D, dh = D / d->H;
-    const size_t T = (size_t)d->B * d->L;
-    HstuTcArgs a = make_tc_args(d, pos_table, time_table, s);
-    a.zk = zp ? zp + 3 * D : nullptr; a.zv = zp ? zp + D : nullptr; a.ldz = 4 * D;
-    a.dk = dzp + 3 * D; a.dv = dzp + D; a.lddz = 4 * D;
-    a.dq_acc = dq_acc;
-    a.dwpos = dwpos + (size_t)s->pos_bucket0 * d->H;
-    a.dwtime = a.wtime ? dwtime : nullptr;
-    GRB_REQUIRE(a.wtime == nullptr || dwtime != nullptr, "time_table gradient pointer is null");
-    CUtensorMap tmP, tmDO;
-    if (!make_tmap_bf16(&tmP, P, T, 4 * (size_t)D, 4 * (size_t)D, 64, 128) || !make_tmap_bf16(&tmDO, dO, T, D, D, 64, 128))
-        return fail(GRB_EINVAL, "tensor map creation failed (attention backward)");
-    GRB_CUDA(cudaMemsetAsync(dq_acc, 0, T * D * sizeof(float), st));
-    const int nqt = (d->L + 127) / 128;
-    const unsigned grid = (unsigned)((D / 64) * d->B * nqt);
-    if (dh == 32) {
-        const size_t smem = AtcBwdSmem<32>::kBytes + 1024;
-        GRB_TRY(set_smem(hstu_attn_tc_bwd_kernel<32>, smem));
-        launch_k(hstu_attn_tc_bwd_kernel<32>, grid, ATC_THREADS, smem, st, tmP, tmDO, a, nqt);
-    } else {
-        const size_t smem = AtcBwdSmem<64>::kBytes + 1024;
-        GRB_TRY(set_smem(hstu_attn_tc_bwd_kernel<64>, smem));
-        launch_k(hstu_attn_tc_bwd_kernel<64>, grid, ATC_THREADS, smem, st, tmP, tmDO, a, nqt);
-    }
-    GRB_CUDA(cudaGetLastError());
-    size_t blocks = (T * (D / 8) + 255) / 256;
-    if (blocks > (size_t)sm_count() * 8) blocks = (size_t)sm_count() * 8;
-    launch_k(hstu_dq_finish_kernel, (unsigned)blocks, 256, 0, st, (const float*)dq_acc, zp ? zp + 2 * D : (const bf16*)nullptr, 4 * D, dzp + 2 * D,
-             4 * D, T, D);
-    GRB_CUDA(cudaGetLastError());
     return 0;
 }
 
@@ -484,9 +435,7 @@ int launch_row(Kern k, const Args& a, int T, cudaStream_t st) {
 }
 template <int NP, class Args, class Kern>
 int launch_row_bwd(Kern k, const Args& a, int T, cudaStream_t st) {
-    int need = (T + ROW_THREADS / 32 - 1) / (ROW_THREADS / 32);
-    int cap = sm_count() * 3;
-    launch_k(k, need < cap ? (need < 1 ? 1 : need) : cap, ROW_THREADS, 0, st, a);
+    launch_k(k, row_bwd_grid(T), ROW_THREADS, 0, st, a);
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -515,34 +464,22 @@ int cast_bf16(const float* in, bf16* out, size_t n, int D, const Dropout& drop, 
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
-int cast_colsum(const float* in, bf16* out, int T, int D, const Dropout& drop, float* colsum_out, cudaStream_t st) {
+// part (nullable): cast_colsum_grid(T, D).x * .y * 128 floats of scratch for the ordered sum; without it one atomic add per CTA
+int cast_colsum(const float* in, bf16* out, int T, int D, const Dropout& drop, float* colsum_out, float* part, cudaStream_t st) {
     GRB_REQUIRE(D > 0 && D % 4 == 0, "cast needs rows of a multiple-of-4 length D");
-    int cx = (D + 127) / 128;
-    int cy = (8 * sm_count() + cx - 1) / cx;
-    int maxy = (T + 31) / 32;
-    if (cy > maxy) cy = maxy;
-    if (cy < 1) cy = 1;
-    launch_k(cast_colsum_f32_bf16_kernel, dim3(cx, cy), 256, 0, st, in, out, T, D, drop, colsum_out);
+    const dim3 grid = cast_colsum_grid(T, D);
+    launch_k(cast_colsum_f32_bf16_kernel, grid, 256, 0, st, in, out, T, D, drop, colsum_out, part);
     GRB_CUDA(cudaGetLastError());
+    if (part) GRB_TRY(det_finish(part, grid.x, grid.y, 128, grid.x, 128, 1, {{colsum_out, D}}, st));
     return 0;
 }
-// GRB_FFN_FUSED=1 routes the forward FFN through the single fused kernel of tc_ffn.cuh.  Off by default: at cfg-2 it
-// measures 47 us per layer against 43 us for the two separate GEMM launches (its 16 epilogue warps walk the phases of a
-// chunk in lock-step); it is the first building block of the fused layer kernel and is kept bit-compatible and tested.
-// Read on every call so that a test can flip it.
-bool ffn_fused() {
-    const char* e = getenv("GRB_FFN_FUSED");
-    return e != nullptr && e[0] == '1';
-}
-int colsum(const bf16* in, int T, int N, int ld, float* out, cudaStream_t st) {
+// part (nullable): colsum_grid(T, N).x * .y * 256 floats of scratch for the ordered sum; without it one atomic add per CTA
+int colsum(const bf16* in, int T, int N, int ld, float* out, float* part, cudaStream_t st) {
     if (N % 8 != 0 || ld % 8 != 0) return fail(GRB_EINVAL, "colsum needs N and ld to be multiples of 8");
-    int cx = (N + 255) / 256;
-    int cy = (4 * sm_count() + cx - 1) / cx;
-    int maxy = (T + 63) / 64;
-    if (cy > maxy) cy = maxy;
-    if (cy < 1) cy = 1;
-    launch_k(colsum_bf16_kernel, dim3(cx, cy), 256, 0, st, in, T, N, ld, out);
+    const dim3 grid = colsum_grid(T, N);
+    launch_k(colsum_bf16_kernel, grid, 256, 0, st, in, T, N, ld, out, part);
     GRB_CUDA(cudaGetLastError());
+    if (part) GRB_TRY(det_finish(part, grid.x, grid.y, 256, grid.x, 256, 1, {{out, N}}, st));
     return 0;
 }
 
@@ -561,7 +498,7 @@ int grb_check_device(int ordinal) {
     cudaDeviceProp prop;
     cudaError_t e = cudaGetDeviceProperties(&prop, ordinal);
     if (e != cudaSuccess) return fail(GRB_ENODEV, "cudaGetDeviceProperties(%d): %s", ordinal, cudaGetErrorString(e));
-    if (prop.major != 10) return fail(GRB_ENODEV, "device %d is sm_%d%d; this library is built for sm_100a only", ordinal, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail(GRB_ENODEV, "device %d is sm_%d%d; this library is built for sm_90a only", ordinal, prop.major, prop.minor);
     return 0;
 }
 
@@ -571,7 +508,7 @@ size_t grb_hstu_layer_saved_bytes(const grb_hstu_dims* d) {
 }
 size_t grb_hstu_layer_workspace_bytes(const grb_hstu_dims* d) {
     if (check_dims(d)) return 0;
-    return carve_work(nullptr, (size_t)d->B * d->L, d->D).bytes;
+    return carve_work(nullptr, d).bytes;
 }
 
 int grb_hstu_layer_forward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const float* x,
@@ -580,9 +517,8 @@ int grb_hstu_layer_forward(const grb_hstu_dims* d, const grb_hstu_layer_params* 
     GRB_REQUIRE(p && s && x && y && saved, "null argument");
     GRB_REQUIRE(p->proj_w && p->proj_b && p->pos_table && p->ln1_g && p->ln1_b && p->ffn1_w && p->ffn1_b && p->ffn2_w &&
                     p->ffn2_b && p->ln2_g && p->ln2_b, "null parameter pointer");
-    const bool attn_tc = use_attn_tc(d, s);
-    GRB_REQUIRE(attn_tc || s->bias_index, "null sequence metadata: the mma.sync attention path needs bias_index");
-    GRB_REQUIRE(attn_tc || (s->ld_index >= d->L && s->ld_index % 8 == 0 && aligned16(s->bias_index)),
+    GRB_REQUIRE(s->bias_index, "null sequence metadata: the attention kernels need bias_index");
+    GRB_REQUIRE((s->ld_index >= d->L && s->ld_index % 8 == 0 && aligned16(s->bias_index)),
                 "bias_index pitch must be a multiple of 8 and >= L");
     GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(saved) && aligned16(p->proj_w) && aligned16(p->ffn1_w) && aligned16(p->ffn2_w),
                 "buffers must be 16-byte aligned");
@@ -599,9 +535,7 @@ int grb_hstu_layer_forward(const grb_hstu_dims* d, const grb_hstu_layer_params* 
     }
     // 3. O = silu(Q K^T + bias) V, causal + key padding                                      (hstu.py:244-267)
     GRB_TRY(join_pending(st));   // a bias-index matrix built on the side stream (deferred schedule) must be complete
-    if (attn_tc) {
-        GRB_TRY(launch_attn_tc_fwd(d, p->pos_table, p->time_table, s, sv.P, sv.O, st));
-    } else {
+    {
         HstuAttnArgs a = make_attn_args(d, p, s, sv);
         if (D / d->H == 32) GRB_TRY(launch_hstu_attn_fwd<32>(a, st));
         else GRB_TRY(launch_hstu_attn_fwd<64>(a, st));
@@ -611,15 +545,6 @@ int grb_hstu_layer_forward(const grb_hstu_dims* d, const grb_hstu_layer_params* 
         LnGateFwdArgs a{sv.O, D, sv.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, sv.x1, sv.xn, sv.st1, sv.st2, T, D, 1e-5f,
                         make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_GATE), d->seed_dev)};
         GRB_ROW_DISPATCH(D, ln_gate_fwd_kernel, a, T, st);
-    }
-    // 5 + 6 in one kernel (tc_ffn.cuh): h is written once for the backward and never re-read in the forward
-    if (use_tc() && ffn_fused() && (D == 64 || D == 128)) {
-        FfnEpiArgs ea{p->ffn1_b, p->ffn2_b, sv.x1, sv.z1, y,
-                      make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_HID), d->seed_dev),
-                      make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_OUT), d->seed_dev)};
-        if (D == 64) GRB_CUDA(launch_tc_ffn_fwd<1>(sv.xn, (const bf16*)p->ffn1_w, (const bf16*)p->ffn2_w, sv.hact, T, ea, sm_count(), st));
-        else GRB_CUDA(launch_tc_ffn_fwd<2>(sv.xn, (const bf16*)p->ffn1_w, (const bf16*)p->ffn2_w, sv.hact, T, ea, sm_count(), st));
-        return 0;
     }
     // 5. h = drop(silu(xn W1^T + b1))                                                        (hstu.py:210-212)
     {
@@ -644,14 +569,14 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int T = d->B * d->L, D = d->D;
     LayerSaved sv = carve_saved(const_cast<void*>(saved), T, D);
-    LayerWork w = carve_work(workspace, T, D);
+    LayerWork w = carve_work(workspace, d);
     const Dropout nodrop = make_dropout(0.f, 0, 0);
     const Dropout drop_out = make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_OUT), d->seed_dev);
     const Dropout drop_hid = make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_HID), d->seed_dev);
     const Dropout drop_gate = make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_GATE), d->seed_dev);
 
     // FFN second linear
-    GRB_TRY(cast_colsum(dy, w.dyb, T, D, drop_out, g->ffn2_b, st));   // dyb = bf16(dropmask(dy)) ; db2 += column sums
+    GRB_TRY(cast_colsum(dy, w.dyb, T, D, drop_out, g->ffn2_b, w.part_cast, st));   // dyb = bf16(dropmask(dy)) ; db2 += column sums
     {
         if (!use_tc()) GRB_CUDA(gemm_tn_atomic(w.dyb, sv.hact, g->ffn2_w, D, 4 * D, T, D, 4 * D, st));  // dW2[D,4D] += dyb^T h
     }
@@ -661,8 +586,9 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
     // FFN first linear
     // bias gradients are off the critical path too: with deferred weight gradients the column sums run beside the main chain
     auto colsum_maybe_deferred = [&](const bf16* in, float* out) -> int {
-        if (use_tc() && g_defer_on) return defer_run(st, [&](cudaStream_t side) -> int { return colsum(in, T, 4 * D, 4 * D, out, side); });
-        return colsum(in, T, 4 * D, 4 * D, out, st);
+        if (use_tc() && g_defer_on)
+            return defer_run(st, [&](cudaStream_t side) -> int { return colsum(in, T, 4 * D, 4 * D, out, w.part_colsum, side); });
+        return colsum(in, T, 4 * D, 4 * D, out, w.part_colsum, st);
     };
     GRB_TRY(colsum_maybe_deferred(w.dz1, g->ffn1_b));
     {
@@ -674,20 +600,20 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
     // LN2 + residual + gate + LN1
     {
         LnGateBwdArgs a{dy, w.dxn, sv.x1, sv.st1, sv.st2, sv.O, D, sv.P, 4 * D, sv.zp, 4 * D, p->ln1_g, p->ln1_b, p->ln2_g,
-                        w.dx1, w.dO, D, w.dzp, 4 * D, g->ln1_g, g->ln1_b, g->ln2_g, g->ln2_b, T, D, drop_gate};
+                        w.dx1, w.dO, D, w.dzp, 4 * D, g->ln1_g, g->ln1_b, g->ln2_g, g->ln2_b, T, D, drop_gate, w.part_ln};
         GRB_ROW_DISPATCH(D, ln_gate_bwd_kernel, a, T, st);
+        GRB_TRY(det_finish(w.part_ln, 4, row_grid(T), D, 1, 0, 1, {{a.dg1, D}, {a.db1, D}, {a.dg2, D}, {a.db2, D}}, st));
     }
     // attention backward -> gradients w.r.t. the V, Q, K pre-activations
-    if (use_attn_tc(d, s)) {
-        GRB_TRY(launch_attn_tc_bwd(d, p->pos_table, p->time_table, s, sv.P, sv.zp, w.dO, w.dzp, g->pos_table, g->time_table, w.dq_acc, st));
-    } else {
-        GRB_REQUIRE(s->bias_index, "null sequence metadata: the mma.sync attention path needs bias_index");
+    {
+        GRB_REQUIRE(s->bias_index, "null sequence metadata: the attention kernels need bias_index");
         HstuAttnArgs a = make_attn_args(d, p, s, sv);
         a.d_o = w.dO; a.lddo = D;
         a.zq = sv.zp + 2 * D; a.zk = sv.zp + 3 * D; a.zv = sv.zp + D; a.ldz = 4 * D;
         a.dq = w.dzp + 2 * D; a.dk = w.dzp + 3 * D; a.dv = w.dzp + D; a.lddq = 4 * D;
         a.dwpos = g->pos_table + (s->pos_uniform ? (size_t)s->pos_bucket0 * d->H : 0);
         a.dwtime = g->time_table;
+        a.dw_part = w.part_attn;
         GRB_REQUIRE(a.bias.wtime == nullptr || g->time_table != nullptr, "time_table gradient pointer is null");
         if (D / d->H == 32) GRB_TRY(launch_hstu_attn_bwd<32>(a, st));
         else GRB_TRY(launch_hstu_attn_bwd<64>(a, st));
@@ -702,16 +628,15 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
     }
     if (use_tc()) {
         // the three weight gradients of the layer in ONE grouped launch: dW2 += dyb^T h, dW1 += dz1^T xn, dWp += dzp^T xb
-        TnSpec specs[3] = {{w.dyb, sv.hact, g->ffn2_w, D, 4 * D, T, D, 4 * D, 4 * D},
-                           {w.dz1, sv.xn, g->ffn1_w, 4 * D, D, T, 4 * D, D, D},
-                           {w.dzp, sv.xb, g->proj_w, 4 * D, D, T, 4 * D, D, D}};
+        TnSpec specs[3];
+        layer_tn_specs(specs, w.dyb, sv.hact, w.dz1, sv.xn, w.dzp, sv.xb, g->ffn2_w, g->ffn1_w, g->proj_w, T, D);
         if (g_defer_on) {
             GRB_TRY(defer_run(st, [&](cudaStream_t side) -> int {
-                GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), side));
+                GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, side));
                 return 0;
             }));
         } else {
-            GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), st));
+            GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, st));
         }
     }
     (void)nodrop;
@@ -756,7 +681,7 @@ int grb_hstu_seq_prepare(const int64_t* timestamps, const uint8_t* pad, int B, i
 int grb_hstu_bucket_bytes_debug(const grb_hstu_seq* s, int B, int L, int ntime, uint8_t* out, void* stream) {
     GRB_REQUIRE(s && out && s->pad && s->time_thr, "null argument");
     GRB_REQUIRE(B > 0 && L > 0 && B <= 65535 && ntime >= 0 && ntime <= 64, "bad shape");
-    HstuTcArgs a;
+    HstuBucketArgs a;
     memset(&a, 0, sizeof(a));
     const bool has_time = s->timestamps != nullptr && s->has_time && ntime > 0;
     GRB_REQUIRE(!has_time || (s->rel32 && s->wide), "rel32 / wide missing: call grb_hstu_seq_prepare first");
@@ -773,27 +698,57 @@ int grb_hstu_bucket_bytes_debug(const grb_hstu_seq* s, int B, int L, int ntime, 
 
 size_t grb_hstu_attention_scratch_bytes(const grb_hstu_dims* d) {
     if (check_dims(d)) return 0;
-    return align_up((size_t)d->B * d->L * d->D * sizeof(float));
+    return align_up(attn_dw_part_floats(d->B, d->L, d->H) * sizeof(float));   // the bias-table gradient partials
 }
+namespace {
+HstuAttnArgs make_attn_args_p(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s, const bf16* P) {
+    grb_hstu_layer_params p;
+    memset(&p, 0, sizeof(p));
+    p.pos_table = pos_table;
+    p.time_table = time_table;
+    LayerSaved sv;
+    memset(&sv, 0, sizeof(sv));
+    sv.P = const_cast<bf16*>(P);
+    return make_attn_args(d, &p, s, sv);
+}
+}  // namespace
+
 int grb_hstu_attention_forward(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s,
                                const void* P_bf16, void* O_bf16, void* stream) {
     GRB_TRY(check_dims(d));
     GRB_REQUIRE(pos_table && s && P_bf16 && O_bf16, "null argument");
-    GRB_REQUIRE(attn_tc_possible(d, s), "the stand-alone attention entry points run the tcgen05 path: uniform position buckets, head_dim 32/64, "
-                                        "pad / time_thr (and rel32 / wide with timestamps) required");
+    GRB_REQUIRE(s->bias_index && s->ld_index >= d->L && s->ld_index % 8 == 0 && aligned16(s->bias_index),
+                "the attention kernels need bias_index (pitch a multiple of 8 and >= L)");
     GRB_REQUIRE(aligned16(P_bf16) && aligned16(O_bf16), "buffers must be 16-byte aligned");
-    return launch_attn_tc_fwd(d, pos_table, time_table, s, (const bf16*)P_bf16, (bf16*)O_bf16, static_cast<cudaStream_t>(stream));
+    HstuAttnArgs a = make_attn_args_p(d, pos_table, time_table, s, (const bf16*)P_bf16);
+    a.o = (bf16*)O_bf16;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (d->D / d->H == 32) return launch_hstu_attn_fwd<32>(a, st);
+    return launch_hstu_attn_fwd<64>(a, st);
 }
 int grb_hstu_attention_backward(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s,
                                 const void* P_bf16, const void* zp_bf16, const void* dO_bf16, void* dzp_bf16, float* dpos_table,
                                 float* dtime_table, void* scratch, void* stream) {
     GRB_TRY(check_dims(d));
     GRB_REQUIRE(pos_table && s && P_bf16 && dO_bf16 && dzp_bf16 && dpos_table && scratch, "null argument");
-    GRB_REQUIRE(attn_tc_possible(d, s), "the stand-alone attention entry points run the tcgen05 path");
+    GRB_REQUIRE(s->bias_index && s->ld_index >= d->L && s->ld_index % 8 == 0 && aligned16(s->bias_index),
+                "the attention kernels need bias_index (pitch a multiple of 8 and >= L)");
     GRB_REQUIRE(aligned16(P_bf16) && aligned16(dO_bf16) && aligned16(dzp_bf16) && aligned16(scratch) && (zp_bf16 == nullptr || aligned16(zp_bf16)),
                 "buffers must be 16-byte aligned");
-    return launch_attn_tc_bwd(d, pos_table, time_table, s, (const bf16*)P_bf16, (const bf16*)zp_bf16, (const bf16*)dO_bf16, (bf16*)dzp_bf16,
-                              dpos_table, dtime_table, (float*)scratch, static_cast<cudaStream_t>(stream));
+    HstuAttnArgs a = make_attn_args_p(d, pos_table, time_table, s, (const bf16*)P_bf16);
+    a.dw_part = static_cast<float*>(scratch);
+    GRB_REQUIRE(a.bias.wtime == nullptr || dtime_table != nullptr, "time_table gradient pointer is null");
+    const int D = d->D;
+    const bf16* zp = (const bf16*)zp_bf16;
+    bf16* dzp = (bf16*)dzp_bf16;
+    a.d_o = (const bf16*)dO_bf16; a.lddo = D;
+    a.zq = zp ? zp + 2 * D : nullptr; a.zk = zp ? zp + 3 * D : nullptr; a.zv = zp ? zp + D : nullptr; a.ldz = 4 * D;
+    a.dq = dzp + 2 * D; a.dk = dzp + 3 * D; a.dv = dzp + D; a.lddq = 4 * D;
+    a.dwpos = dpos_table + (s->pos_uniform ? (size_t)s->pos_bucket0 * d->H : 0);
+    a.dwtime = dtime_table;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (D / d->H == 32) return launch_hstu_attn_bwd<32>(a, st);
+    return launch_hstu_attn_bwd<64>(a, st);
 }
 
 int grb_collate_jagged(const int64_t* items, const int64_t* stamps, const int64_t* offsets, const int64_t* targets, int B, int L,
@@ -819,15 +774,23 @@ int grb_embed_forward(const int64_t* ids, const float* table, const float* pos_t
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
-int grb_embed_backward(const int64_t* ids, const float* dx, float* dtable, float* dpos_table, int B, int L, int D, float scale,
-                       int mask_pad_rows, float dropout_p, uint64_t seed, const uint64_t* seed_dev, void* stream) {
-    GRB_REQUIRE(ids && dx && dtable, "null argument");
-    GRB_REQUIRE(D % 4 == 0 && aligned16(dx) && aligned16(dtable) && (dpos_table == nullptr || aligned16(dpos_table)),
+int grb_embed_backward(const int64_t* ids, const int64_t* order, const float* dx, float* dtable, float* dpos_table, int B, int L, int D,
+                       float scale, int mask_pad_rows, float dropout_p, uint64_t seed, const uint64_t* seed_dev, float* scratch, void* stream) {
+    GRB_REQUIRE(ids && order && dx && dtable && scratch, "null argument");
+    GRB_REQUIRE(D <= 128 * EMB_MAX_CH, "embedding backward supports D <= %d", 128 * EMB_MAX_CH);
+    GRB_REQUIRE(D % 4 == 0 && aligned16(dx) && aligned16(dtable) && aligned16(scratch) && (dpos_table == nullptr || aligned16(dpos_table)),
                 "embedding backward needs D %% 4 == 0 and 16-byte aligned buffers");
     EmbedBwdArgs a{reinterpret_cast<const long long*>(ids), dx, dtable, dpos_table, B * L, L, D, scale, mask_pad_rows,
-                   make_dropout(dropout_p, seed, SITE_EMBED, seed_dev)};
-    launch_k(embed_bwd_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
+                   make_dropout(dropout_p, seed, SITE_EMBED, seed_dev), reinterpret_cast<const long long*>(order)};
+    const EmbedPieceArgs pa{a, scratch};
+    launch_k(embed_bwd_piece_kernel, row_grid((B * L + 31) / 32), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), pa);
     GRB_CUDA(cudaGetLastError());
+    launch_k(embed_bwd_run_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), pa);
+    GRB_CUDA(cudaGetLastError());
+    if (dpos_table) {
+        launch_k(embed_bwd_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
+        GRB_CUDA(cudaGetLastError());
+    }
     return 0;
 }
 
@@ -835,12 +798,14 @@ int grb_embed_backward(const int64_t* ids, const float* dx, float* dtable, float
 namespace {
 struct HeadWork {
     bf16* xf; float* stf; bf16* logits; float* dxf; float* scal;  // scal[0] = inv_count
-    bf16* xs; float* row_sums; float2* row_stats;                  // fused CE: x / sum_row, per-row sums of G', {max, target logit}
-    float* col_shift;                                              // fused CE: exponent shift of every token for the class-stationary dE pass
-    void* ce_scratch;
+    float* logits32;                                               // stored schedule: fp32 logits (the CE reads them, the bf16 buffer takes the gradient)
+    float* row_loss;                                               // per-token loss, summed in a fixed order
+    float* shift;                                                  // fused schedule: per-token log2-domain softmax shift
+    float *part_ln, *part_tn;                                      // scratch of the ordered cross-CTA sums (LayerNorm, stored-schedule dE)
     int ldl;
     size_t bytes;
 };
+bool head_fused(int D) { return use_tc() && (D == 64 || D == 128); }
 HeadWork carve_head(void* base, size_t T, size_t D, size_t C) {
     HeadWork h;
     size_t off = 0;
@@ -851,12 +816,15 @@ HeadWork carve_head(void* base, size_t T, size_t D, size_t C) {
     h.stf = (float*)take(T * 2 * 4);
     h.dxf = (float*)take(T * D * 4);
     h.scal = (float*)take(64);
-    h.xs = (bf16*)take(T * D * 2);
-    h.row_sums = (float*)take(4 * T * 4);   // [2][T] sums of G' per class half, then [2][T] target-logit partials (one-sweep CE)
-    h.row_stats = (float2*)take(T * 8);
-    h.col_shift = (float*)take(((T + 127) / 128) * 128 * 4);
-    h.ce_scratch = take(ce_scratch_bytes((int)T));
-    h.logits = (bf16*)take(T * (size_t)h.ldl * 2);
+    // D <= 128: the fused kernels (tc_ce.cuh) never form the [T, C] logits; D = 256 (and GRB_GEMM=mma) store them
+    const bool fused = head_fused((int)D);
+    h.logits = fused ? nullptr : (bf16*)take(T * (size_t)h.ldl * 2);
+    h.logits32 = fused ? nullptr : (float*)take(T * (size_t)h.ldl * 4);
+    h.row_loss = (float*)take(T * 4);
+    h.shift = (float*)take(T * 4);
+    h.part_ln = (float*)take((size_t)2 * row_bwd_grid((int)T) * D * 4);
+    const TnSpec spec{nullptr, nullptr, nullptr, (int)C, (int)D, (int)T, h.ldl, (int)D, (int)D};
+    h.part_tn = fused ? nullptr : (float*)take(tn_part_floats(&spec, 1, sm_count()) * 4);
     h.bytes = off;
     return h;
 }
@@ -874,12 +842,8 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     HeadWork h = carve_head(workspace, T, D, C);
     // the target count (one CTA, latency-bound) depends on the targets only: with the deferred schedule it runs beside the final
-    // LayerNorm and is joined before the fused CE kernel
+    // LayerNorm and is joined before the CE kernel
     const bool count_aside = g_defer_on;
-    // D <= 128: no [T, C] tensor reaches HBM - dX' accumulates in TMEM beside the CE sweep and dE comes from a class-stationary pass
-    // that recomputes G.  D = 256 (or GRB_CE=store): G' is stored and dE is a TN GEMM.
-    const bool keep_g = use_tc() && D <= 128 && want_grad && !ce_store_forced();
-    const int ce_mode = keep_g ? ce_mode_env() : (int)CE_STORE_G;
     auto count = [&](cudaStream_t s_) -> int {
         launch_k(ce_count_kernel, 1, 1024, 0, s_, reinterpret_cast<const long long*>(targets), T, h.scal, loss);
         GRB_CUDA(cudaGetLastError());
@@ -892,65 +856,54 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
     }
     if (count_aside) GRB_TRY(join_pending(st));
     else GRB_TRY(count(st));
-    bool fused_dx = false;
-    if (use_tc()) {
-        // fused: logits are never materialised; (D <= 128) h.dxf = G' E, and h.logits receives G' only when a dE GEMM needs it
-        const long long* tg = reinterpret_cast<const long long*>(targets);                                  // (hstu.py:137-146)
-        const bf16* tb = (const bf16*)table_bf16;
-        if (D == 64) GRB_CUDA(launch_tc_ce<1>(h.xf, tb, h.logits, ce_mode, T, C, h.ldl, tg, h.scal, h.row_sums, h.row_stats, h.dxf, &fused_dx, h.ce_scratch, sm_count(), st));
-        else if (D == 128) GRB_CUDA(launch_tc_ce<2>(h.xf, tb, h.logits, ce_mode, T, C, h.ldl, tg, h.scal, h.row_sums, h.row_stats, h.dxf, &fused_dx, h.ce_scratch, sm_count(), st));
-        else GRB_CUDA(launch_tc_ce<4>(h.xf, tb, h.logits, CE_STORE_G, T, C, h.ldl, tg, h.scal, h.row_sums, h.row_stats, h.dxf, &fused_dx, h.ce_scratch, sm_count(), st));
-    } else {
-    GRB_CUDA(gemm_nt_bf16(h.xf, (const bf16*)table_bf16, h.logits, h.ldl, T, C, D, st));  // logits = xf E^T   (hstu.py:137)
-    if (h.ldl / 8 <= 256 * 8)
-        launch_k(ce_fwd_bwd_vec_kernel<8>, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, loss, want_grad ? 1 : 0);
-    else
-        launch_k(ce_fwd_bwd_kernel, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, loss, want_grad ? 1 : 0);
-    GRB_CUDA(cudaGetLastError());
-    }
-    if (use_tc()) {
-        // normalisation pass of the fused CE (rowwise.cuh ce_finish_kernel): loss, and - with gradients - dxf, x / sum_row, the one-hot
-        // term of dE.  Without the dX fusion (D = 256) dxf' = G' E comes from a GEMM first.
-        if (want_grad && !fused_dx) GRB_CUDA(gemm_nn_f32(h.logits, (const bf16*)table_bf16, h.dxf, nullptr, 1.f, T, D, C, h.ldl, D, st));
-        CeFinishArgs fa{h.row_sums, h.row_stats, ce_mode == CE_ONE_SWEEP ? h.row_sums + (size_t)2 * T : nullptr,
-                        reinterpret_cast<const long long*>(targets), h.scal, h.xf, (const bf16*)table_bf16,
-                        want_grad ? h.dxf : nullptr, (want_grad && !keep_g) ? h.xs : nullptr, keep_g ? h.col_shift : nullptr,
-                        want_grad ? dtable : nullptr, loss, T, D};
-        launch_k(ce_finish_kernel, row_grid(T), ROW_THREADS, 0, st, fa);
+    if (head_fused(D)) {
+        // loss, dxf and the per-token shifts in one row-stationary pass; dE in a class-stationary pass (a weight gradient: off the
+        // critical path with the deferred schedule)                                                      (hstu.py:137-146)
+        CeArgs ca{reinterpret_cast<const long long*>(targets), h.scal, T, C, want_grad ? h.dxf : nullptr, h.shift, h.row_loss, dtable};
+        if (D == 64) GRB_CUDA(launch_tc_ce<64>(h.xf, (const bf16*)table_bf16, ca, st));
+        else GRB_CUDA(launch_tc_ce<128>(h.xf, (const bf16*)table_bf16, ca, st));
+        launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
         GRB_CUDA(cudaGetLastError());
-    }
+        if (!want_grad) return 0;
+        auto table_grad = [&](cudaStream_t s_) -> int {
+            if (D == 64) GRB_CUDA(launch_ce_table<64>(h.xf, (const bf16*)table_bf16, ca, s_));
+            else GRB_CUDA(launch_ce_table<128>(h.xf, (const bf16*)table_bf16, ca, s_));
+            return 0;
+        };
+        if (g_defer_on) GRB_TRY(defer_run(st, table_grad));
+        else GRB_TRY(table_grad(st));
+    } else {
+    GRB_CUDA(gemm_nt_f32(h.xf, (const bf16*)table_bf16, h.logits32, h.ldl, T, C, D, st));  // logits = xf E^T   (hstu.py:137)
+    if (h.ldl / 8 <= 256 * 8)
+        launch_k(ce_fwd_bwd_vec_kernel<8>, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0,
+                 (const float*)h.logits32);
+    else
+        launch_k(ce_fwd_bwd_kernel, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0,
+                 (const float*)h.logits32);
+    GRB_CUDA(cudaGetLastError());
+    launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
+    GRB_CUDA(cudaGetLastError());
     if (!want_grad) return 0;
-    {
-        if (!use_tc()) GRB_CUDA(gemm_nn_f32(h.logits, (const bf16*)table_bf16, h.dxf, nullptr, 1.f, T, D, C, h.ldl, D, st));  // dxf = dlogits E
-    }
-    {
-        if (keep_g) {
-            // dE[C,D] += G^T xf with G recomputed class block by class block (tc_ce.cuh CE_ACCUM_T); off the critical path like the
-            // other weight gradients
-            auto accum = [&](cudaStream_t s_) -> int {
-                if (D == 64) GRB_CUDA(launch_tc_ce_accum_t<1>(h.xf, (const bf16*)table_bf16, h.col_shift, dtable, T, C, sm_count(), s_));
-                else GRB_CUDA(launch_tc_ce_accum_t<2>(h.xf, (const bf16*)table_bf16, h.col_shift, dtable, T, C, sm_count(), s_));
+    GRB_CUDA(gemm_nn_f32(h.logits, (const bf16*)table_bf16, h.dxf, nullptr, 1.f, T, D, C, h.ldl, D, st));  // dxf = dlogits E
+    // dE[C,D] += dlogits^T xf: a weight gradient, off the critical path with the deferred schedule
+    if (use_tc()) {
+        TnSpec spec{h.logits, h.xf, dtable, C, D, T, h.ldl, D, D};
+        if (g_defer_on) {
+            GRB_TRY(defer_run(st, [&](cudaStream_t side) -> int {
+                GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, side));
                 return 0;
-            };
-            if (g_defer_on) GRB_TRY(defer_run(st, accum));
-            else GRB_TRY(accum(st));
-        } else if (use_tc()) {
-            TnSpec spec{h.logits, h.xs, dtable, C, D, T, h.ldl, D, D};  // dE[C,D] += G'^T (xf / sum_row) = dlogits^T xf
-            if (g_defer_on) {
-                GRB_TRY(defer_run(st, [&](cudaStream_t side) -> int {
-                    GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), side));
-                    return 0;
-                }));
-            } else {
-                GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), st));
-            }
+            }));
         } else {
-            GRB_CUDA(gemm_tn_atomic(h.logits, h.xf, dtable, C, D, T, h.ldl, D, st));
+            GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, st));
         }
+    } else {
+        GRB_CUDA(gemm_tn_atomic(h.logits, h.xf, dtable, C, D, T, h.ldl, D, st));
+    }
     }
     {
-        LnBwdArgs a{h.dxf, x, h.stf, ln_g, nullptr, dx, dln_g, dln_b, T, D};
+        LnBwdArgs a{h.dxf, x, h.stf, ln_g, nullptr, dx, dln_g, dln_b, T, D, h.part_ln};
         GRB_ROW_BWD_DISPATCH(D, ln_bwd_kernel, a, T, st);
+        GRB_TRY(det_finish(h.part_ln, 2, row_bwd_grid(T), D, 1, 0, 1, {{a.dg, D}, {a.db, D}}, st));
     }
     return 0;
 }
@@ -1063,7 +1016,7 @@ int grb_linear_backward(const void* dy_bf16, const void* w_bf16, const void* x_b
     GRB_REQUIRE(dy_bf16 && w_bf16, "null argument");
     GRB_REQUIRE(T > 0 && N % 8 == 0 && K % 8 == 0, "N and K must be multiples of 8");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (db) GRB_TRY(colsum((const bf16*)dy_bf16, T, N, N, db, st));
+    if (db) GRB_TRY(colsum((const bf16*)dy_bf16, T, N, N, db, nullptr, st));
     if (dw) {
         GRB_REQUIRE(x_bf16, "x is null");
         GRB_CUDA(gemm_tn_atomic((const bf16*)dy_bf16, (const bf16*)x_bf16, dw, N, K, T, N, K, st));

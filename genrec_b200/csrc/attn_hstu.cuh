@@ -27,8 +27,7 @@ constexpr int ATT_THREADS = 128;  // 4 warps x 16 rows
 constexpr int ATT_MAX_BUCKETS = 64;
 // Diagonal tiles that lie wholly below L also take the guard-free straight-line path: their masked (above-diagonal) cells are
 // computed and come out as exact zeros through the sentinel index, which costs up to half a tile of wasted work but lets
-// the scheduler interleave all 32 score chains of a lane.  Measured at cfg-2: 1.923 -> 1.889 ms per step.  (-DGRB_ATT_DIAG_FULL=0
-// restores the per-warp triangular skipping.)
+// the scheduler interleave all 32 score chains of a lane.  (-DGRB_ATT_DIAG_FULL=0 restores the per-warp triangular skipping.)
 #ifndef GRB_ATT_DIAG_FULL
 #define GRB_ATT_DIAG_FULL 1
 #endif
@@ -59,6 +58,7 @@ struct HstuAttnArgs {
     bf16* dq; bf16* dk; bf16* dv; int lddq;                       // gradients w.r.t. pre-activations (or activations if z null)
     float* dwpos;   // [npos, H]  accumulated (atomicAdd)
     float* dwtime;  // [ntime, H] accumulated
+    float* dw_part; // nullable: [2H][B * key tiles][64] scratch for the ordered cross-CTA sum of dwpos / dwtime (det_finish_kernel)
 };
 
 GRB_DEVINL int time_bucket_dev(long long dt, const long long* thr, int ntime) {
@@ -583,31 +583,43 @@ __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 3 : 2) hstu_attn_bwd_d
         }
     }
 
-    // bias-table gradients
+    // bias-table gradients: per-CTA sums, added across the CTAs of a head in (sequence, key tile) order when dw_part is given
+    __shared__ float s_pos[ATT_THREADS / 32];
     if (pos_uniform) {
         pos_acc = warp_sum(pos_acc);
-        if (lane == 0 && pos_acc != 0.f) atomicAdd(a.dwpos + a.bias.pos_bucket0 * a.H + h, pos_acc);
+        if (lane == 0) s_pos[warp] = pos_acc;
     }
     __syncthreads();
-    if (!pos_uniform) {
-        for (int bk = warp; bk < npos; bk += 4) {
-            float v = 0.f;
-#pragma unroll
-            for (int w = 0; w < 4; ++w) v += hist_p[(w * (npos + 1) + bk) * 32 + lane];
-            if (!__any_sync(0xffffffffu, v != 0.f)) continue;   // most bins of a tile are empty: skip their reductions
-            v = warp_sum(v);
-            if (lane == 0 && v != 0.f) atomicAdd(a.dwpos + bk * a.H + h, v);
+    const int member = b * gridDim.x + kt, nmem = gridDim.x * gridDim.z;
+    auto pos_sum = [&](int) {
+        float v = 0.f;
+        for (int w = 0; w < ATT_THREADS / 32; ++w) v += s_pos[w];
+        return v;
+    };
+    auto pos_bin = [&](int bk) {
+        float v = 0.f;
+        for (int w = 0; w < 4; ++w)
+            for (int l = 0; l < 32; ++l) v += hist_p[(w * (npos + 1) + bk) * 32 + l];
+        return v;
+    };
+    auto time_bin = [&](int bk) {
+        float v = 0.f;
+        for (int w = 0; w < 4; ++w)
+            for (int l = 0; l < 32; ++l) v += hist_t[(w * nt_bins + bk) * 32 + l];
+        return v;
+    };
+    if (a.dw_part) {
+        if (pos_uniform) det_store(a.dw_part, h, member, nmem, 64, 1, pos_sum);
+        else det_store(a.dw_part, h, member, nmem, 64, npos, pos_bin);
+        if (has_time && a.dwtime) det_store(a.dw_part, a.H + h, member, nmem, 64, ntime, time_bin);
+    } else {
+        if (pos_uniform) {
+            if (tid == 0) atomicAdd(a.dwpos + a.bias.pos_bucket0 * a.H + h, pos_sum(0));
+        } else {
+            for (int bk = tid; bk < npos; bk += ATT_THREADS) atomicAdd(a.dwpos + bk * a.H + h, pos_bin(bk));
         }
-    }
-    if (has_time && a.dwtime) {
-        for (int bk = warp; bk < ntime; bk += 4) {
-            float v = 0.f;
-#pragma unroll
-            for (int w = 0; w < 4; ++w) v += hist_t[(w * nt_bins + bk) * 32 + lane];
-            if (!__any_sync(0xffffffffu, v != 0.f)) continue;   // a tile touches ~10 of the 64 time buckets
-            v = warp_sum(v);
-            if (lane == 0 && v != 0.f) atomicAdd(a.dwtime + bk * a.H + h, v);
-        }
+        if (has_time && a.dwtime)
+            for (int bk = tid; bk < ntime; bk += ATT_THREADS) atomicAdd(a.dwtime + bk * a.H + h, time_bin(bk));
     }
 }
 

@@ -5,7 +5,7 @@
 //   out    = dropout(softmax(scores)) v                                                               transformer.py:153-156
 //
 // TIGER's sequences are short (encoder 1 + 20 items x 3 tokens, decoder <= 4, head_dim 64) and the op is a few GFLOP per step, so
-// this is an FP32 CUDA-core kernel with bf16 inputs / outputs (the tensors the tcgen05 projection GEMMs produce and consume):
+// this is an FP32 CUDA-core kernel with bf16 inputs / outputs (the tensors the wgmma projection GEMMs produce and consume):
 // a CTA owns 32 query rows of one (batch, head); thread (row r, key quarter kq) walks the keys kq, kq + 4, ... of every 64-key
 // tile with its own online-softmax state; the four states of a row are merged with shuffles.  Rectangular (cross-attention) and
 // non-causal (encoder) shapes are the general case; the relative-position bucket of every delta = j - i is a host-made table.

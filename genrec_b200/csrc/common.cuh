@@ -1,4 +1,4 @@
-// genrec_b200 - shared device helpers (sm_100a).
+// genrec_b200 - shared device helpers (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -20,7 +20,7 @@ typedef __nv_bfloat16 bf16;
 // has started (and therefore passed its own wait), so the next kernel's CTAs fill SMs as this grid's last wave drains
 // and never compete with CTAs of this grid that are still to be scheduled; look-ahead is exactly one kernel.  Data
 // ordering stays the stream's own (each dependent waits for full completion of this grid) - only launch latency and
-// the per-CTA prologue (barrier init, TMEM allocation, descriptor prefetch) move off the critical path.
+// the per-CTA prologue (barrier init, descriptor prefetch) move off the critical path.
 GRB_DEVINL void pdl_wait() {
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -211,7 +211,7 @@ GRB_DEVINL void mma_bf16_z(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, u
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1), "f"(0.f));
 }
 
-// Fragment address helpers (lane -> row/col of the 8x8 matrix row this lane points at), see DESIGN.md "mma.sync fragments".
+// Fragment address helpers (lane -> row/col of the 8x8 matrix row this lane points at), see the PTX ISA, mma.m16n8k16 fragment layouts.
 // A operand, smem tile stored [m][k] (k contiguous): non-transposed ldmatrix.
 GRB_DEVINL int lane_a_row(int lane) { return (lane & 7) + ((lane >> 3) & 1) * 8; }
 GRB_DEVINL int lane_a_col(int lane) { return (lane >> 4) * 8; }
@@ -220,5 +220,40 @@ GRB_DEVINL int lane_b_row(int lane) { return (lane & 7) + (lane >> 4) * 8; }
 GRB_DEVINL int lane_b_col(int lane) { return ((lane >> 3) & 1) * 8; }
 // B operand, smem tile stored [k][n] (n contiguous): transposed ldmatrix, two n-tiles per x4  (== lane_a_row/col).
 // A operand, smem tile stored [k][m] (m contiguous): transposed ldmatrix                      (== lane_b_row/col with row=k, col=m).
+
+
+// ----------------------------------------------------------------------------- deterministic cross-CTA sums
+// Float atomics from many CTAs add in whatever order the CTAs finish, so the last bits of a gradient (and through Adam the
+// parameters) would change from run to run.  The cross-CTA reductions of the training step are split in two instead: each CTA
+// stores its partials to scratch from the caller's workspace (det_store, layout [group][member][W]), and det_finish_kernel,
+// launched right after on the same stream, sums them in a fixed order and adds the result once.  Entry points without a
+// workspace keep one atomic add per CTA.
+template <class F>
+GRB_DEVINL void det_store(float* part, int group, int member, int nmembers, int W, int n, F vals) {
+    float* dst = part + ((size_t)group * nmembers + member) * W;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = vals(i);
+}
+struct DetFinishArgs {
+    const float* part;
+    int ngroups, nmembers, W;
+    int gpo, gstride, estride;   // group g, element i -> out[g / gpo][(g % gpo) * gstride + i * estride], kept when that index < len
+    float* out[4];
+    int len[4];
+};
+// one warp per (group, element): lane l sums members l, l + 32, ... in order, then a fixed butterfly
+__global__ void __launch_bounds__(256) det_finish_kernel(DetFinishArgs a) {
+    pdl_wait();
+    const int w = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+    const int g = w / a.W, i = w % a.W;
+    if (g >= a.ngroups) return;
+    const int k = g / a.gpo, idx = (g % a.gpo) * a.gstride + i * a.estride;
+    if (idx >= a.len[k]) return;
+    const float* p = a.part + (size_t)g * a.nmembers * a.W + i;
+    float s = 0.f;
+#pragma unroll 4
+    for (int m = lane; m < a.nmembers; m += 32) s += p[(size_t)m * a.W];
+    s = warp_sum(s);
+    if (lane == 0) atomicAdd(a.out[k] + idx, s);   // one add per element and launch
+}
 
 }  // namespace grb

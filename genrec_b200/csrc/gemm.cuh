@@ -1,5 +1,5 @@
 // genrec_b200 - generic bf16 tensor-core GEMM with fused epilogues (first-generation path: cp.async + ldmatrix +
-// mma.sync.m16n8k16; the tcgen05/TMA kernels in tc_*.cu replace it on the hot GEMMs).
+// mma.sync.m16n8k16; the wgmma/TMA kernels in tc_*.cuh replace it on the hot GEMMs).
 //
 //   C[M,N] (+)= opA(A) * opB(B),  fp32 accumulate
 //     AMODE 0 : A stored [M][K], K contiguous          AMODE 1 : A stored [K][M], M contiguous (i.e. A^T given)

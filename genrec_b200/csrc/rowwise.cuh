@@ -99,9 +99,10 @@ struct LnGateBwdArgs {
     float* dx1;                    // [T,D] fp32
     bf16* dO; int lddo;            // [T,D]
     bf16* dzu; int lddz;           // [T, ...] grad wrt U pre-activation
-    float *dg1, *db1, *dg2, *db2;  // accumulated (atomicAdd)
+    float *dg1, *db1, *dg2, *db2;  // accumulated
     int T, D;
     Dropout drop;
+    float* part;                   // nullable: [4][gridDim.x][D] scratch for the ordered cross-CTA sum (det_finish_kernel)
 };
 template <int NP>
 __global__ void __launch_bounds__(ROW_THREADS) ln_gate_bwd_kernel(LnGateBwdArgs a) {
@@ -187,7 +188,7 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_gate_bwd_kernel(LnGateBwdArgs 
             *reinterpret_cast<uint32_t*>(a.dO + (size_t)row * a.lddo + c) = pack_bf16(d0, d1);
         }
     }
-    // CTA reduction of the four parameter-gradient vectors, then one atomicAdd per column per CTA
+    // CTA reduction of the four parameter-gradient vectors, then the ordered cross-CTA sum
 #pragma unroll
     for (int p = 0; p < NP; ++p)
 #pragma unroll
@@ -198,12 +199,15 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_gate_bwd_kernel(LnGateBwdArgs 
         }
     __syncthreads();
     float* outs[4] = {a.dg1, a.db1, a.dg2, a.db2};
-    for (int i = threadIdx.x; i < 4 * a.D; i += ROW_THREADS) {
-        int which = i / a.D, c = i % a.D;
-        float s = 0.f;
+    for (int which = 0; which < 4; ++which) {
+        auto colsum = [&](int c) {
+            float s = 0.f;
 #pragma unroll
-        for (int w = 0; w < ROW_THREADS / 32; ++w) s += red[which][w][c];
-        atomicAdd(outs[which] + c, s);
+            for (int w = 0; w < ROW_THREADS / 32; ++w) s += red[which][w][c];
+            return s;
+        };
+        if (a.part) det_store(a.part, which, blockIdx.x, gridDim.x, a.D, a.D, colsum);
+        else for (int c = threadIdx.x; c < a.D; c += ROW_THREADS) atomicAdd(outs[which] + c, colsum(c));
     }
 }
 
@@ -245,6 +249,7 @@ struct LnBwdArgs {
     const float* res;  // nullable, added to dx
     float* dx; float *dg, *db;
     int T, D;
+    float* part;       // nullable: [2][gridDim.x][D] scratch for the ordered cross-CTA sum (det_finish_kernel)
 };
 template <int NP>
 __global__ void __launch_bounds__(ROW_THREADS) ln_bwd_kernel(LnBwdArgs a) {
@@ -292,12 +297,15 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_bwd_kernel(LnBwdArgs a) {
             red[0][wib][c] = adg[p][e]; red[1][wib][c] = adb[p][e];
         }
     __syncthreads();
-    for (int i = threadIdx.x; i < 2 * a.D; i += ROW_THREADS) {
-        int which = i / a.D, c = i % a.D;
-        float s = 0.f;
+    for (int which = 0; which < 2; ++which) {
+        auto colsum = [&](int c) {
+            float s = 0.f;
 #pragma unroll
-        for (int w = 0; w < ROW_THREADS / 32; ++w) s += red[which][w][c];
-        atomicAdd((which ? a.db : a.dg) + c, s);
+            for (int w = 0; w < ROW_THREADS / 32; ++w) s += red[which][w][c];
+            return s;
+        };
+        if (a.part) det_store(a.part, which, blockIdx.x, gridDim.x, a.D, a.D, colsum);
+        else for (int c = threadIdx.x; c < a.D; c += ROW_THREADS) atomicAdd((which ? a.db : a.dg) + c, colsum(c));
     }
 }
 
@@ -331,7 +339,7 @@ __global__ void cast_f32_bf16_kernel(const float* __restrict__ in, bf16* __restr
 // out_bf16[r, c] = bf16(dropmask(in[r, c]))  and  colsum[c] += sum_r out_bf16[r, c]   (the cast of dy and the bias gradient
 // of the layer's last linear in one pass).  grid (ceil(D / 128), chunks) ; block 256 = 8 row lanes x 32 threads of 4 columns.
 __global__ void __launch_bounds__(256) cast_colsum_f32_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, int T, int D,
-                                                                  Dropout drop, float* __restrict__ colsum) {
+                                                                  Dropout drop, float* __restrict__ colsum, float* __restrict__ part) {
     pdl_wait();
     drop.resolve();
     __shared__ float red[8][128];
@@ -364,17 +372,20 @@ __global__ void __launch_bounds__(256) cast_colsum_f32_bf16_kernel(const float* 
 #pragma unroll
     for (int k = 0; k < 4; ++k) red[ty][4 * tx + k] = s[k];
     __syncthreads();
-    if (threadIdx.x < 128) {
+    auto sum8 = [&](int i) {
         float t = 0.f;
 #pragma unroll
-        for (int w = 0; w < 8; ++w) t += red[w][threadIdx.x];
-        const int cc = blockIdx.x * 128 + threadIdx.x;
-        if (cc < D) atomicAdd(colsum + cc, t);
-    }
+        for (int w = 0; w < 8; ++w) t += red[w][i];
+        return t;
+    };
+    const int nc = min(128, D - (int)blockIdx.x * 128);
+    if (part) det_store(part, blockIdx.x, blockIdx.y, gridDim.y, 128, nc, sum8);
+    else if (threadIdx.x < nc) atomicAdd(colsum + blockIdx.x * 128 + threadIdx.x, sum8(threadIdx.x));
 }
 // out[c] += sum_r in[r, c]   in: bf16 [T, ld] (ld % 8 == 0), columns [0, N) ; grid (ceil(N/256), chunks) ;
 // block 256 = 32 column groups of 8 (one 16-byte load each) x 8 row lanes, 4 rows in flight per thread
-__global__ void __launch_bounds__(256) colsum_bf16_kernel(const bf16* __restrict__ in, int T, int N, int ld, float* __restrict__ out) {
+__global__ void __launch_bounds__(256) colsum_bf16_kernel(const bf16* __restrict__ in, int T, int N, int ld, float* __restrict__ out,
+                                                         float* __restrict__ part) {
     pdl_wait();
     __shared__ float red[8][256];
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
@@ -413,11 +424,15 @@ __global__ void __launch_bounds__(256) colsum_bf16_kernel(const bf16* __restrict
 #pragma unroll
     for (int k = 0; k < 8; ++k) red[ty][8 * tx + k] = s[k];
     __syncthreads();
-    float t = 0.f;
+    auto sum8 = [&](int i) {
+        float t = 0.f;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) t += red[w][threadIdx.x];
-    const int cc = blockIdx.x * 256 + threadIdx.x;
-    if (cc < N) atomicAdd(out + cc, t);
+        for (int w = 0; w < 8; ++w) t += red[w][i];
+        return t;
+    };
+    const int nc = min(256, N - (int)blockIdx.x * 256);
+    if (part) det_store(part, blockIdx.x, blockIdx.y, gridDim.y, 256, nc, sum8);
+    else if ((int)threadIdx.x < nc) atomicAdd(out + blockIdx.x * 256 + threadIdx.x, sum8(threadIdx.x));
 }
 
 // ------------------------------------------------------------------------------------------------ embedding
@@ -457,11 +472,12 @@ __global__ void __launch_bounds__(ROW_THREADS) embed_fwd_kernel(EmbedArgs a) {
         }
     }
 }
-// dE[ids[t],:] += scale * dropmask(dx[t,:]) for ids[t] != 0 (padding_idx) ; dpos[t % L,:] += dropmask(dx[t,:])
+// dpos[t % L,:] += dropmask(dx[t,:])   (the table rows: embed_bwd_piece_kernel + embed_bwd_run_kernel)
 struct EmbedBwdArgs {
     const long long* ids; const float* dx; float* dE; float* dpos;
     int T, L, D; float scale; int mask_pad_rows;
     Dropout drop;
+    const long long* order;   // token indices sorted by id (stable)
 };
 __global__ void __launch_bounds__(ROW_THREADS) embed_bwd_kernel(EmbedBwdArgs a) {
     pdl_wait();
@@ -469,15 +485,100 @@ __global__ void __launch_bounds__(ROW_THREADS) embed_bwd_kernel(EmbedBwdArgs a) 
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int nw = gridDim.x * (ROW_THREADS / 32);
     for (int row = blockIdx.x * (ROW_THREADS / 32) + wib; row < a.T; row += nw) {
-        long long id = a.ids[row];
-        if (id == 0 && (a.mask_pad_rows || !a.dpos)) continue;
+        const long long id = a.ids[row];
+        if (a.mask_pad_rows && id == 0) continue;
         // four columns per lane and one 16-byte vector reduction per destination (D % 4 == 0, rows 16-byte aligned)
         for (int c = 4 * lane; c < a.D; c += 128) {
             float4 v = *reinterpret_cast<const float4*>(a.dx + (size_t)row * a.D + c);
             a.drop.apply2(v.x, v.y, row, c);
             a.drop.apply2(v.z, v.w, row, c + 2);
-            if (id != 0) red_add_v4(a.dE + (size_t)id * a.D + c, v.x * a.scale, v.y * a.scale, v.z * a.scale, v.w * a.scale);
-            if (a.dpos && !(a.mask_pad_rows && id == 0)) red_add_v4(a.dpos + (size_t)(row % a.L) * a.D + c, v.x, v.y, v.z, v.w);
+            red_add_v4(a.dpos + (size_t)(row % a.L) * a.D + c, v.x, v.y, v.z, v.w);
+        }
+    }
+}
+
+// dE[id,:] += sum over the tokens t with ids[t] == id, in token order, of scale * dropmask(dx[t,:]), with a summation order that does
+// not depend on timing.  a.order lists the tokens sorted by id (stable) and is cut into fixed pieces of 32 positions:
+//   pass 1 (one warp per piece): the tokens of every id run inside the piece are summed in order -> piece[first position][:]
+//   pass 2 (one warp per id run): the run's pieces are summed in order and added to dE once
+struct EmbedPieceArgs {
+    EmbedBwdArgs e;
+    float* piece;   // [T, D] fp32 scratch, rows indexed by sorted position
+};
+// (the warp-wide shuffles / ballots sit outside the column loops: with D = 64 half of the lanes own no column)
+constexpr int EMB_MAX_CH = 2;   // float4 columns per lane: D <= 256
+__global__ void __launch_bounds__(ROW_THREADS) embed_bwd_piece_kernel(EmbedPieceArgs a) {
+    pdl_wait();
+    a.e.drop.resolve();
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const int nw = gridDim.x * (ROW_THREADS / 32);
+    const int npieces = (a.e.T + 31) / 32;
+    for (int k = blockIdx.x * (ROW_THREADS / 32) + wib; k < npieces; k += nw) {
+        const int q = k * 32 + lane;
+        const int rowq = q < a.e.T ? (int)a.e.order[q] : 0;
+        const long long idq = q < a.e.T ? a.e.ids[rowq] : -1;
+        const int cnt = min(32, a.e.T - k * 32);
+        float4 s[EMB_MAX_CH];
+#pragma unroll
+        for (int h = 0; h < EMB_MAX_CH; ++h) s[h] = make_float4(0.f, 0.f, 0.f, 0.f);
+        int start = 0;
+        for (int j = 0; j < cnt; ++j) {
+            const int row = __shfl_sync(0xffffffffu, rowq, j);
+            const long long id = __shfl_sync(0xffffffffu, idq, j);
+            const long long next = __shfl_sync(0xffffffffu, idq, (j + 1) & 31);
+            const bool last = j + 1 == cnt || next != id;
+#pragma unroll
+            for (int h = 0; h < EMB_MAX_CH; ++h) {
+                const int c = 4 * lane + 128 * h;
+                if (c >= a.e.D) continue;
+                float4 v = *reinterpret_cast<const float4*>(a.e.dx + (size_t)row * a.e.D + c);
+                a.e.drop.apply2(v.x, v.y, row, c);
+                a.e.drop.apply2(v.z, v.w, row, c + 2);
+                s[h].x += v.x * a.e.scale; s[h].y += v.y * a.e.scale; s[h].z += v.z * a.e.scale; s[h].w += v.w * a.e.scale;
+                if (last) {
+                    *reinterpret_cast<float4*>(a.piece + (size_t)(k * 32 + start) * a.e.D + c) = s[h];
+                    s[h] = make_float4(0.f, 0.f, 0.f, 0.f);
+                }
+            }
+            if (last) start = j + 1;
+        }
+    }
+}
+__global__ void __launch_bounds__(ROW_THREADS) embed_bwd_run_kernel(EmbedPieceArgs a) {
+    pdl_wait();
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const int nw = gridDim.x * (ROW_THREADS / 32);
+    const int T = a.e.T;
+    for (int p = blockIdx.x * (ROW_THREADS / 32) + wib; p < T; p += nw) {
+        const long long id = a.e.ids[a.e.order[p]];
+        if (id == 0 || (p > 0 && a.e.ids[a.e.order[p - 1]] == id)) continue;
+        float4 s[EMB_MAX_CH];
+#pragma unroll
+        for (int h = 0; h < EMB_MAX_CH; ++h) {
+            const int c = 4 * lane + 128 * h;
+            s[h] = c < a.e.D ? *reinterpret_cast<const float4*>(a.piece + (size_t)p * a.e.D + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        // the further pieces of the run start at the piece boundaries 32 k > p whose first token still has this id
+        for (int k0 = p / 32 + 1; k0 * 32 < T; k0 += 32) {
+            const int k = k0 + lane;
+            const bool match = k * 32 < T && a.e.ids[a.e.order[k * 32]] == id;
+            const unsigned miss = ~__ballot_sync(0xffffffffu, match);
+            const int cnt = miss ? __ffs(miss) - 1 : 32;
+            for (int j = 0; j < cnt; ++j) {
+#pragma unroll
+                for (int h = 0; h < EMB_MAX_CH; ++h) {
+                    const int c = 4 * lane + 128 * h;
+                    if (c >= a.e.D) continue;
+                    const float4 v = *reinterpret_cast<const float4*>(a.piece + (size_t)(k0 + j) * 32 * a.e.D + c);
+                    s[h].x += v.x; s[h].y += v.y; s[h].z += v.z; s[h].w += v.w;
+                }
+            }
+            if (cnt < 32) break;
+        }
+#pragma unroll
+        for (int h = 0; h < EMB_MAX_CH; ++h) {
+            const int c = 4 * lane + 128 * h;
+            if (c < a.e.D) red_add_v4(a.e.dE + (size_t)id * a.e.D + c, s[h].x, s[h].y, s[h].z, s[h].w);
         }
     }
 }
@@ -511,23 +612,28 @@ __global__ void ce_count_kernel(const long long* __restrict__ tg, int T, float* 
 }
 // one CTA per row: loss += (lse - logit[target]) * inv_count ; logits <- (softmax - onehot) * inv_count  (0 for ignored rows)
 // pad columns [C, ld) are written with zeros.   (hstu.py:141-146, ignore_index = 0, class 0 stays in the denominator)
+// src32 (nullable, [T, ld] fp32): the logits are read from there instead of `logits`, which then only receives the gradient -
+// fp32 logits keep the softmax exact when a row spans tens of nats (bf16 rounds a logit of 60 by 0.25).
 __global__ void __launch_bounds__(256) ce_fwd_bwd_kernel(bf16* __restrict__ logits, int ld, int C, const long long* __restrict__ tg,
-                                                        const float* __restrict__ inv_count, float* __restrict__ loss,
-                                                        int write_grad) {
+                                                        const float* __restrict__ inv_count, float* __restrict__ row_loss,
+                                                        int write_grad, const float* __restrict__ src32) {
     pdl_wait();
     __shared__ float red[8];
     __shared__ float bc[2];
     const int row = blockIdx.x, tid = threadIdx.x;
     bf16* lr = logits + (size_t)row * ld;
+    const float* sr = src32 ? src32 + (size_t)row * ld : nullptr;
+    auto logit = [&](int c) { return sr ? sr[c] : __bfloat162float(lr[c]); };
     const long long t = tg[row];
     const float ic = *inv_count;
     if (t == 0) {
+        if (tid == 0) row_loss[row] = 0.f;
         if (write_grad)
             for (int c = tid; c < ld; c += 256) lr[c] = __float2bfloat16(0.f);
         return;
     }
     float m = -INFINITY;
-    for (int c = tid; c < C; c += 256) m = fmaxf(m, __bfloat162float(lr[c]));
+    for (int c = tid; c < C; c += 256) m = fmaxf(m, logit(c));
     m = warp_max(m);
     if ((tid & 31) == 0) red[tid >> 5] = m;
     __syncthreads();
@@ -539,7 +645,7 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_kernel(bf16* __restrict__ logi
     __syncthreads();
     m = bc[0];
     float s = 0.f;
-    for (int c = tid; c < C; c += 256) s += __expf(__bfloat162float(lr[c]) - m);
+    for (int c = tid; c < C; c += 256) s += __expf(logit(c) - m);
     s = warp_sum(s);
     __syncthreads();
     if ((tid & 31) == 0) red[tid >> 5] = s;
@@ -549,7 +655,7 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_kernel(bf16* __restrict__ logi
         for (int w = 0; w < 8; ++w) ss += red[w];
         bc[1] = ss;
         float lse = m + logf(ss);
-        atomicAdd(loss, (lse - __bfloat162float(lr[t])) * ic);
+        row_loss[row] = (lse - logit((int)t)) * ic;
     }
     __syncthreads();
     if (!write_grad) return;
@@ -557,7 +663,7 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_kernel(bf16* __restrict__ logi
     for (int c = tid; c < ld; c += 256) {
         float gvl = 0.f;
         if (c < C) {
-            gvl = __expf(__bfloat162float(lr[c]) - m) * inv_s;
+            gvl = __expf(logit(c) - m) * inv_s;
             if (c == (int)t) gvl -= 1.f;
             gvl *= ic;
         }
@@ -565,12 +671,28 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_kernel(bf16* __restrict__ logi
     }
 }
 
+// loss += sum of the per-row losses, in a fixed order (one CTA of 1024 threads: strided partial sums, then a fixed tree)
+__global__ void __launch_bounds__(1024) ce_loss_sum_kernel(const float* __restrict__ row_loss, int T, float* __restrict__ loss) {
+    pdl_wait();
+    __shared__ float red[32];
+    float s = 0.f;
+    for (int i = threadIdx.x; i < T; i += 1024) s += row_loss[i];
+    s = warp_sum(s);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        s = warp_sum(red[threadIdx.x]);
+        if (threadIdx.x == 0) *loss += s;
+    }
+}
+
 // Register-resident variant: the whole row (<= 256 x NCH x 8 logits) is read ONCE with 16-byte loads; exp(x - max) is
 // evaluated once per logit and kept in registers for the gradient pass; the row is written ONCE.
-// HBM traffic = 1 read + 1 write of the logits; ~10 instructions per logit.
+// HBM traffic = 1 read + 1 write of the logits; ~10 instructions per logit.  src32: as in ce_fwd_bwd_kernel.
 template <int NCH>
 __global__ void __launch_bounds__(256) ce_fwd_bwd_vec_kernel(bf16* __restrict__ logits, int ld, int C, const long long* __restrict__ tg,
-                                                            const float* __restrict__ inv_count, float* __restrict__ loss, int write_grad) {
+                                                            const float* __restrict__ inv_count, float* __restrict__ row_loss, int write_grad,
+                                                            const float* __restrict__ src32) {
     pdl_wait();
     __shared__ float red[8];
     __shared__ float bc[3];
@@ -580,6 +702,7 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_vec_kernel(bf16* __restrict__ 
     const int t = (int)tg[row];
     const float ic = *inv_count;
     if (t == 0) {
+        if (tid == 0) row_loss[row] = 0.f;
         if (write_grad)
             for (int c = tid; c < nchunks; c += 256) lr[c] = make_uint4(0u, 0u, 0u, 0u);
         return;
@@ -590,13 +713,20 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_vec_kernel(bf16* __restrict__ 
     for (int i = 0; i < NCH; ++i) {
         const int c = tid + i * 256;
         if (c < nchunks) {
-            const uint4 q = lr[c];
-            const uint32_t u[4] = {q.x, q.y, q.z, q.w};
+            if (src32) {
+                const float4* sr = reinterpret_cast<const float4*>(src32 + (size_t)row * ld) + 2 * c;
+                const float4 f0 = sr[0], f1 = sr[1];
+                e[i][0] = f0.x; e[i][1] = f0.y; e[i][2] = f0.z; e[i][3] = f0.w;
+                e[i][4] = f1.x; e[i][5] = f1.y; e[i][6] = f1.z; e[i][7] = f1.w;
+            } else {
+                const uint4 q = lr[c];
+                const uint32_t u[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                float2 f = unpack_bf16(u[k]);
-                e[i][2 * k] = f.x;
-                e[i][2 * k + 1] = f.y;
+                for (int k = 0; k < 4; ++k) {
+                    float2 f = unpack_bf16(u[k]);
+                    e[i][2 * k] = f.x;
+                    e[i][2 * k + 1] = f.y;
+                }
             }
             if (c * 8 + 8 > C) {   // the single partial chunk: pad columns do not take part
 #pragma unroll
@@ -650,7 +780,7 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_vec_kernel(bf16* __restrict__ 
     }
     __syncthreads();
     const float stot = bc[1];
-    if (own) atomicAdd(loss, (m + logf(stot) - tlogit) * ic);
+    if (own) row_loss[row] = (m + logf(stot) - tlogit) * ic;
     if (!write_grad) return;
     const float sc = ic / stot;
 #pragma unroll
@@ -719,7 +849,7 @@ __global__ void cast_flat_f32_bf16_kernel(const float* __restrict__ in, bf16* __
 // fp32-accurate GEMM on the bf16 tensor path: x = hi + mid + lo with three bf16 terms (24 mantissa bits together); the product
 // of two such numbers keeps the six terms of weight >= 2^-16 (hi*hi, hi*mid, mid*hi, hi*lo, lo*hi, mid*mid).  Laying the terms
 // out along K,   A' = [hi | hi | mid | hi | lo | mid]   B' = [hi | mid | hi | lo | hi | mid]   (K' = 6 K),
-// turns the sum of the six partial GEMMs into ONE ordinary GEMM with fp32 accumulation in TMEM.
+// turns the sum of the six partial GEMMs into ONE ordinary GEMM with fp32 accumulation.
 // out [rows, 6 K] bf16 ; operand 0 = A layout, 1 = B layout.
 __global__ void __launch_bounds__(256) split3_f32_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, size_t rows, int K, int operand) {
     pdl_wait();
@@ -801,79 +931,5 @@ __global__ void __launch_bounds__(256) collate_jagged_kernel(const long long* __
     if (out_ts != nullptr) out_ts[e] = (p < pad || stamps == nullptr) ? 0 : stamps[(hi - n) + (p - pad)];
 }
 
-
-// ------------------------------------------------------------------------------------------------ fused CE: normalisation pass
-// The fused CE kernel (tc_ce.cuh) leaves G' = exp(s - max) / count unnormalised and reports, per row, the sum of G' over each
-// class half, the row max and the target logit.  With rs = 1 / sum_c exp(s_c - max) (so that G = G' rs is the softmax / count):
-//   loss    += (max + log sum exp - logit[target]) / count
-//   dxf      = dxf' rs - E[target] / count                 (dxf' = G' E from the CE kernel or the GEMM)
-//   xs       = bf16(x rs)                                   -> a dE GEMM over the stored G' computes G'^T xs = G^T x, or
-//   col_shift = log2e * logsumexp - log2(1 / count)         -> the class-stationary pass (tc_ce.cuh CE_ACCUM_T) recomputes G from it
-//   dE[target] -= x / count                                 (the one-hot term of dE, a 16-byte-vector scatter)
-// One warp per token row; rows with target 0 (ignore_index) get rs = 0 and contribute nothing.
-struct CeFinishArgs {
-    const float* row_sums;       // [2][T]
-    const float2* row_stats;     // [T] {exponent shift (the row max, or the one-sweep kernel's estimate), target logit}
-    const float* tl_parts;       // nullable [2][T]: the target logit as two per-half partials (one-sweep kernel) instead of row_stats.y
-    const long long* targets;    // [T]
-    const float* inv_count;
-    const bf16* xf;              // [T, D]
-    const bf16* table;           // [C, D] bf16 mirror of the tied embedding table
-    float* dxf;                  // [T, D] in: G' E, out: d loss / d xf   (nullable: loss only)
-    bf16* xs;                    // [T, D] out (nullable)
-    float* col_shift;            // [ceil(T / 128) * 128] out (nullable); +inf for ignored rows and the padding
-    float* dtable;               // [C, D] += (nullable)
-    float* loss;                 // += (zeroed by ce_count_kernel)
-    int T, D;
-};
-__global__ void __launch_bounds__(ROW_THREADS) ce_finish_kernel(CeFinishArgs a) {
-    pdl_wait();
-    __shared__ float s_loss[ROW_THREADS / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int wpb = ROW_THREADS / 32;
-    const float ic = *a.inv_count;
-    float lsum = 0.f;
-    for (int row = blockIdx.x * wpb + warp; row < a.T; row += gridDim.x * wpb) {
-        const int t = (int)a.targets[row];
-        const float icr = t != 0 ? ic : 0.f;
-        const float gs = a.row_sums[row] + a.row_sums[(size_t)a.T + row];        // = sum_c exp(s_c - max) * icr
-        const float rs = (icr > 0.f && gs > 0.f) ? icr / gs : 0.f;                // 1 / sum_c exp(s_c - max)
-        if (lane == 0) {
-            const float2 st = a.row_stats[row];
-            const float tlog = a.tl_parts ? a.tl_parts[row] + a.tl_parts[(size_t)a.T + row] : st.y;
-            const bool live = icr > 0.f && gs > 0.f;
-            if (live) lsum += (st.x + __logf(gs / icr) - tlog) * icr;
-            if (a.col_shift) a.col_shift[row] = live ? st.x * 1.4426950408889634f + __log2f(gs / icr) - __log2f(icr) : INFINITY;
-        }
-        const bf16* x = a.xf + (size_t)row * a.D;
-        const bf16* e = a.table + (size_t)t * a.D;
-        for (int c = lane * 4; c < a.D; c += 128) {
-            const uint2 xu = *reinterpret_cast<const uint2*>(x + c);
-            const float2 x0 = unpack_bf16(xu.x), x1 = unpack_bf16(xu.y);
-            if (a.xs) {
-                uint2 o;
-                o.x = pack_bf16(x0.x * rs, x0.y * rs); o.y = pack_bf16(x1.x * rs, x1.y * rs);
-                *reinterpret_cast<uint2*>(a.xs + (size_t)row * a.D + c) = o;
-            }
-            if (a.dxf) {
-                float4 d = *reinterpret_cast<float4*>(a.dxf + (size_t)row * a.D + c);
-                const uint2 eu = *reinterpret_cast<const uint2*>(e + c);
-                const float2 e0 = unpack_bf16(eu.x), e1 = unpack_bf16(eu.y);
-                d.x = d.x * rs - icr * e0.x; d.y = d.y * rs - icr * e0.y; d.z = d.z * rs - icr * e1.x; d.w = d.w * rs - icr * e1.y;
-                *reinterpret_cast<float4*>(a.dxf + (size_t)row * a.D + c) = d;
-            }
-            if (a.dtable && icr > 0.f) red_add_v4(a.dtable + (size_t)t * a.D + c, -icr * x0.x, -icr * x0.y, -icr * x1.x, -icr * x1.y);
-        }
-    }
-    if (a.col_shift && blockIdx.x == 0)
-        for (int i = a.T + threadIdx.x; i < ((a.T + 127) / 128) * 128; i += ROW_THREADS) a.col_shift[i] = INFINITY;
-    if (lane == 0) s_loss[warp] = lsum;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float tot = 0.f;
-        for (int w = 0; w < wpb; ++w) tot += s_loss[w];
-        if (tot != 0.f) atomicAdd(a.loss, tot);
-    }
-}
 
 }  // namespace grb

@@ -318,13 +318,11 @@ __global__ void __launch_bounds__(RQ_THREADS) rq_residual_argmin_split_kernel(Rq
 // catalogue size (N = 12,101) additionally by one serial chain of 3 x 256 (or 64) codes per thread on a third of the SMs.
 // This variant is the distance "GEMM" on the CUDA cores: a CTA owns 128 item rows; the residual tile and the level's codebook sit
 // TRANSPOSED in shared memory (rT[d][row], cT[d][code]); thread (rg, cg) accumulates an 8-row x 16-code block of dot products in
-// registers - per d: 2 + 4 LDS.128 feed 64 packed FFMA2 = 128 fma (the 3-register FFMA issues every second clock per SM
-// sub-partition: ~37 TFLOP/s; fma.rn.f32x2 does two per issue).  Every (row, code) dot product is still ONE fmaf chain over d = 0 .. D-1
+// registers - per d: 2 + 4 LDS.128 feed 128 FFMA.  Every (row, code) dot product is still ONE fmaf chain over d = 0 .. D-1
 // and the distance is still (|r|^2 + |c|^2) - 2 r.c with strict '<' over ascending code indices, so ids are bit-identical to the
 // kernels above (tests/test_rq_gpu.py).  The 16 threads that share a row meet through 4 shuffle steps (lower index wins ties).
 // Outputs in the reference's [N, D, levels] layout are staged per tile and written as one contiguous span.
-constexpr int RQT_ROWS = 128;             // rows per CTA (64 rows / 128 threads / two CTAs per SM measured slower without the auxiliary
-                                          // outputs: 1.78 vs 1.58 ms at N = 2^20 - every CTA transposes the level's codebook for itself)
+constexpr int RQT_ROWS = 128;             // rows per CTA: every CTA transposes the level's codebook for itself, so fewer, larger tiles
 constexpr int RQT_THREADS = 256;          // 16 code groups x 16 row groups
 constexpr int RQT_RLD = RQT_ROWS + 4;     // row pitch of the transposed residual tile (floats); +4 keeps the float4 loads 16-byte aligned
 template <int D>
@@ -387,13 +385,11 @@ __global__ void __launch_bounds__(RQT_THREADS, 1) rq_residual_argmin_tile_kernel
         for (int i = 0; i < 8; ++i) { best[i] = INFINITY; best_k[i] = 0; }
         // rows of this thread: rg*8 + {0..7}; codes per 256-code pass: q*64 + cg*4 + {0..3}, q = 0..3
         for (int kb = 0; kb < a.K; kb += 256) {
-            // packed FP32 FMA (fma.rn.f32x2 -> FFMA2): two neighbouring codes per instruction, the row value broadcast to both
-            // halves; each half is an IEEE fma, so every dot product is still one fmaf chain over d
-            unsigned long long acc[8][8];
+            float acc[8][16];
 #pragma unroll
             for (int i = 0; i < 8; ++i)
 #pragma unroll
-                for (int j = 0; j < 8; ++j) acc[i][j] = 0ull;
+                for (int j = 0; j < 16; ++j) acc[i][j] = 0.f;
 #pragma unroll 2
             for (int d = 0; d < D; ++d) {
                 const float* rrow = rT + d * RQT_RLD + rg * 8;
@@ -401,16 +397,15 @@ __global__ void __launch_bounds__(RQT_THREADS, 1) rq_residual_argmin_tile_kernel
                 const float4 a0 = *reinterpret_cast<const float4*>(rrow);
                 const float4 a1 = *reinterpret_cast<const float4*>(rrow + 4);
                 const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-                unsigned long long a2[8];
-#pragma unroll
-                for (int i = 0; i < 8; ++i) asm("mov.b64 %0, {%1, %1};" : "=l"(a2[i]) : "f"(av[i]));
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {
-                    const ulonglong2 b = *reinterpret_cast<const ulonglong2*>(crow + q * 64 + cg * 4);   // codes (k, k+1), (k+2, k+3)
+                    const float4 b = *reinterpret_cast<const float4*>(crow + q * 64 + cg * 4);   // codes k .. k+3
 #pragma unroll
                     for (int i = 0; i < 8; ++i) {
-                        asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc[i][2 * q]) : "l"(a2[i]), "l"(b.x));
-                        asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc[i][2 * q + 1]) : "l"(a2[i]), "l"(b.y));
+                        acc[i][4 * q] = fmaf(av[i], b.x, acc[i][4 * q]);
+                        acc[i][4 * q + 1] = fmaf(av[i], b.y, acc[i][4 * q + 1]);
+                        acc[i][4 * q + 2] = fmaf(av[i], b.z, acc[i][4 * q + 2]);
+                        acc[i][4 * q + 3] = fmaf(av[i], b.w, acc[i][4 * q + 3]);
                     }
                 }
             }
@@ -420,9 +415,7 @@ __global__ void __launch_bounds__(RQT_THREADS, 1) rq_residual_argmin_tile_kernel
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {            // ascending code index inside the thread: q-major, then the 4 of a chunk
                     const int k = kb + (j >> 2) * 64 + cg * 4 + (j & 3);
-                    const unsigned long long pr = acc[i][j >> 1];
-                    const float dot = __uint_as_float((j & 1) ? (unsigned)(pr >> 32) : (unsigned)(pr & 0xffffffffull));
-                    const float dist = (x2 + cn[k]) - 2.f * dot;
+                    const float dist = (x2 + cn[k]) - 2.f * acc[i][j];
                     if (dist < best[i]) { best[i] = dist; best_k[i] = k; }
                 }
             }

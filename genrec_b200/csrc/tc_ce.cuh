@@ -1,617 +1,389 @@
-// genrec_b200 - fused tied-embedding logits + cross-entropy: loss, d(loss)/d(logits) AND d(loss)/d(x) on tcgen05.
+// genrec_b200 - fused tied-embedding logits + cross-entropy on wgmma: loss, d(loss)/d(x) and d(loss)/d(table) without ever
+// writing a [tokens, classes] tensor.  D = 64 or 128 (the table rows fit one shared-memory tile).
 //
-// Replaces `logits = x @ E^T ; loss = cross_entropy(logits, targets, ignore_index=0)` (genrec/models/hstu.py:137-146), the
-// autograd softmax-backward and the `dlogits @ E` GEMM.  The [T, C] logits tensor is never written: one CTA owns a block
-// of 128 token rows (token tile resident in shared memory) and sweeps the C classes twice with the same TMA -> tcgen05.mma
-// pipeline, the embedding table streaming from L2:
-//   sweep 0 : S = X E_n^T in TMEM  ->  per-row running MAX + the target logit, one thread per (row, 32 columns) - no exponentials
-//   sweep 1 : S recomputed         ->  G' = exp(S - max) * inv_count (UNNORMALISED: the row sum is only known once this sweep
-//                                      has seen every class) + the row sum  ->  bf16, 128B-swizzled staging tile
-//   Every logit therefore costs ONE exponential (the kernel is MUFU-bound: the first version spent one per sweep).  The
-//   normalisation 1 / sum_row commutes with both products that consume G': ce_finish_kernel scales dX' = G' E by it, subtracts the
-//   one-hot term, and hands the dE GEMM x / sum_row instead of x.
-//                                      -> TMA store to dlogits (consumed by the dE = G^T X GEMM)
-//                                      -> (D <= 128) the SAME staging tile is the K-major A operand of a second MMA
-//                                         dX[128, D] += G_tile E_n, whose B operand is the E_n tile already in shared memory
-//                                         read through an MN-major descriptor; dX accumulates in TMEM over all classes.
-// HBM sees one bf16 write of dlogits (620 MB at cfg-2) and one fp32 write of dX; the K = D recompute is cheap (D <= 256).
-//
-// Load balance: T/128 row blocks rarely divide by the SM count (200 blocks on 148 SMs = 2 rounds at 68 % occupancy), so a
-// work item is HALF the class range of a row block: items (2b, 2b+1) always run in the same round on neighbouring CTAs
-// (the grid is persistent and even-sized), exchange their per-row (max, sum, target-logit) partials through global memory
-// with a release/acquire flag after sweep 0, and each finishes sweep 1 on its own half; dX partials meet in a pre-zeroed
-// fp32 buffer through 16-byte vector reductions.  400 half-items on 148 CTAs = 2.7 rounds of half the length.
+//   ce_rows_kernel   (row-stationary, one CTA per 128 token rows): the token tile X [128 x D] stays in shared memory while the
+//                    table streams through a TMA ring in 64-class tiles.  Sweep 1: S = X E^T (wgmma, register accumulators),
+//                    online row maximum / exponent sum and the target logit -> per-row loss and the row's log2-domain shift.
+//                    Sweep 2: S again, G = (softmax - onehot) / count in registers, converted in place to the bf16 A operand of
+//                    dX += G E (wgmma with A from registers, the same table tile read MN-major) -> dX [T, D] fp32, written once.
+//   ce_table_kernel  (class-stationary, one CTA per 64 classes): the table tile stays resident while the token tiles stream;
+//                    S^T = E X^T, G^T from the saved row shifts, dE += G^T X, the two consumer warpgroups take alternate token
+//                    tiles and their sums are added in a fixed order -> dE [C, D] += once per element.
+// Every sum runs in a fixed order, so the results do not depend on timing.
 #pragma once
 #include "tc_gemm.cuh"
 
 namespace grb {
 
-constexpr int CE_EPI_WARPS = 16;                 // 4 per TMEM sub-partition, one 32-column quarter of the class tile each
-constexpr int CE_THREADS = 64 + 32 * CE_EPI_WARPS;   // TMA, MMA, epilogue warps
-GRB_DEVINL void ce_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(32 * CE_EPI_WARPS) : "memory"); }
-
-template <int KB>
-constexpr int ce_smem_bytes() {   // fused dX (KB <= 2) keeps the table slices of three class tiles alive: 3 * KB ring slots
-    return KB * TC_TILE_BYTES + (KB <= 2 ? 3 * KB : 5) * TC_TILE_BYTES + 2 * 32768 + 12 * 128 * 4 + 1024 + 256;
-}
-
-// Kernel modes.  CE_STORE_G and CE_KEEP_G are the row-stationary CE pass (token rows resident, classes streaming) with / without the
-// bf16 G' tile going to HBM; CE_ACCUM_T is the same pipeline with the operands exchanged (a block of 128 CLASS rows resident, the token
-// tiles streaming, the exponent shift a per-COLUMN array): its "dX" accumulator is dE[class, :] = sum_tokens G[token, class] x[token, :],
-// so the tied-table gradient needs no [T, C] tensor in HBM either - it recomputes S once more instead (K = D is cheap).
-// CE_ONE_SWEEP is CE_KEEP_G without the statistics sweep: the exponent shift of a row only has to be NEAR its maximum, not equal to it
-// (the normalisation by the row sum happens later, in ce_finish_kernel), so the kernel takes
-//     shift = max( max over the first class tile ,  logit of the row's target class )
-// - the first term from ONE probe tile that both halves of a row block compute (bit-identical, no exchange between the halves), the
-// second a 128-term dot product per row.  shift <= the row maximum, so nothing underflows that the exact shift would keep; the result
-// is exact as long as no class beats BOTH the target and 128 probe classes by more than ~98 nats (fp32 / bf16 range of
-// exp(s - shift) / count) - a token whose own loss exceeds 98 nats.  Beyond that the row's G' overflows to inf and loss and gradients
-// come out inf / NaN: loud, never silently wrong; GRB_CE=exact selects the two-sweep mode, which has no such limit.
-// One S recompute and one epilogue pass less: a third of the kernel's tensor and element-wise work.
-enum { CE_STORE_G = 0, CE_KEEP_G = 1, CE_ACCUM_T = 2, CE_ONE_SWEEP = 3 };
-
-struct CeShape {
-    int T, C, ldl;       // rows of the resident operand, rows of the streaming operand, leading dimension of dlogits (multiple of 8, >= C)
-    int num_m, num_n;
-    int n_half;          // class tiles [0, n_half) belong to half 0, [n_half, num_n) to half 1
-    int nsplit;          // CE_ACCUM_T: work items per resident block (each sweeps 1/nsplit of the streaming tiles); 2 otherwise
-    float4* stats;       // [2 * num_m][128] {max, sum, target logit, -}  partials published after sweep 0
-    unsigned* flags;     // [2 * num_m] zero before launch
-};
-GRB_DEVINL void red_add_v4_ce(float* addr, float a, float b, float c, float d) {
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-// tcgen05.mma with the A operand in tensor memory (lane = row, one 32-bit column = two consecutive bf16 along K)
-GRB_DEVINL void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 64] (+)= A[smem desc, K-major] * B[smem desc]; TB = 1: B is MN-major
+template <int TB>
+GRB_DEVINL void wgmma_m64n64k16_ss(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, %35;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TB));
 }
-GRB_DEVINL void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
+// D[64 x 64] (+)= A[registers, 64 x 16 bf16] * B[smem desc]; TB = 1: B is MN-major
+template <int TB>
+GRB_DEVINL void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]),
-        "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %37, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, %38;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate), "n"(TB));
 }
-GRB_DEVINL void st_release_u32(unsigned* p, unsigned v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-GRB_DEVINL unsigned ld_acquire_u32(const unsigned* p) {
-    unsigned v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
+// D[64 x 128] (+)= A[registers, 64 x 16 bf16] * B[smem desc]; TB = 1: B is MN-major
+template <int TB>
+GRB_DEVINL void wgmma_m64n128k16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %69, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1, %70;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate), "n"(TB));
 }
 
-template <int MODE>
-GRB_DEVINL void ce_item(int w, const CeShape& sh, int& blk, int& nb, int& ne) {
-    if (MODE == CE_ACCUM_T) {
-        blk = w / sh.nsplit;
-        const int p = w - blk * sh.nsplit;
-        nb = (int)((long long)p * sh.num_n / sh.nsplit);
-        ne = (int)((long long)(p + 1) * sh.num_n / sh.nsplit);
-    } else {
-        blk = w >> 1;
-        nb = (w & 1) ? sh.n_half : 0;
-        ne = (w & 1) ? sh.num_n : sh.n_half;
+template <int D>
+GRB_DEVINL void wgmma_rs_d(float (&d)[D / 2], const uint32_t (&a)[4], uint64_t bdesc) {
+    if constexpr (D == 64) wgmma_m64n64k16_rs<1>(d, a, bdesc, 1u);
+    else wgmma_m64n128k16_rs<1>(d, a, bdesc, 1u);
+}
+
+constexpr int CE_THREADS = 384;           // producer warpgroup + 2 consumer warpgroups
+constexpr int CE_STAGES = 4;
+constexpr float CE_L2E = 1.4426950408889634f;
+
+struct CeArgs {
+    const long long* tg;        // [T] targets (0 = ignored)
+    const float* inv_count;     // device scalar: 1 / #(targets != 0)
+    int T, C;
+    float* dx;                  // [T, D] fp32 out (nullable: loss only)
+    float* shift;               // [T] out of ce_rows_kernel, in of ce_table_kernel: log2(sum_c 2^(S_c log2e)) (the log2-domain lse)
+    float* row_loss;            // [T] out
+    float* dtable;              // [C, D] += (ce_table_kernel)
+};
+
+template <int D>
+struct CeSmem {
+    static constexpr int XB = D / 64;                  // 64-column boxes
+    static constexpr int ROW_TILE = XB * 128 * 128;    // [128 rows][D] bf16
+    static constexpr int CLS_TILE = XB * 64 * 128;     // [64 rows][D] bf16
+    static constexpr int ROWS_BYTES = ROW_TILE + CE_STAGES * CLS_TILE + 1024 + 256;
+    static constexpr int TABLE_BYTES = CLS_TILE + CE_STAGES * CLS_TILE + 1024 + 256;
+};
+
+// S[64 x 64] = A (64 rows of a K-major tile, D wide) * B^T (64 rows of a K-major tile); box b of A at a_addr + b * a_box
+template <int D>
+GRB_DEVINL void ce_scores(float (&S)[32], uint32_t a_addr, int a_box, uint32_t b_addr) {
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < D / 16; ++kk)
+        wgmma_m64n64k16_ss<0>(S, wgmma_desc(a_addr + (kk >> 2) * a_box + (kk & 3) * 32, 16, 1024),
+                              wgmma_desc(b_addr + (kk >> 2) * 8192 + (kk & 3) * 32, 16, 1024), kk > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+}
+// acc[64 x D] += G (registers, 64 x 64 along K) * B (a [64 k-rows][D] K-major tile read MN-major: N = D contiguous)
+template <int D>
+GRB_DEVINL void ce_accumulate(float (&acc)[D / 2], const float (&G)[32], uint32_t b_addr) {
+    uint32_t a[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        a[kk][0] = pack_bf16(G[8 * kk], G[8 * kk + 1]);
+        a[kk][1] = pack_bf16(G[8 * kk + 2], G[8 * kk + 3]);
+        a[kk][2] = pack_bf16(G[8 * kk + 4], G[8 * kk + 5]);
+        a[kk][3] = pack_bf16(G[8 * kk + 6], G[8 * kk + 7]);
     }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs_d<D>(acc, a[kk], wgmma_desc(b_addr + kk * 2048, 8192, 1024));
+    wgmma_commit();
+    wgmma_wait<0>();
 }
 
-template <int KB, int MODE>  // k-blocks of 64: D = 64 * KB
+template <int D>
 __global__ void __launch_bounds__(CE_THREADS, 1)
-    tc_ce_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmE, const __grid_constant__ CUtensorMap tmG,
-                 CeShape sh, const long long* __restrict__ targets, const float* __restrict__ inv_count,
-                 float* __restrict__ row_sums /* [2][T]: sum_c G'[row, c] of each class half */,
-                 float2* __restrict__ row_stats /* [T]: {row max, target logit} */,
-                 const float* __restrict__ col_shift /* CE_ACCUM_T: [num_n * 128] exponent shift of each streaming row (+inf = skip) */,
-                 const bf16* __restrict__ table /* CE_ONE_SWEEP: the class table [C, D] (rows gathered for the target logits) */,
-                 float* __restrict__ dx_out /* [T, 64*KB] fp32 +=, written only when the second MMA is compiled in (KB <= 2) */) {
-    constexpr bool FUSE_DX = KB <= 2;
-    static_assert(MODE == CE_STORE_G || FUSE_DX, "without the G' store the second MMA is the only consumer of the tile");
-    constexpr int SWEEPS = (MODE == CE_ACCUM_T || MODE == CE_ONE_SWEEP) ? 1 : 2;
-    constexpr bool ONE = MODE == CE_ONE_SWEEP;
-    constexpr int NS = KB <= 2 ? 3 * KB : 5;
-    constexpr int D = 64 * KB;
+    ce_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmE, CeArgs a) {
+    using SM = CeSmem<D>;
     extern __shared__ unsigned char ce_smem_raw[];
-    unsigned char* base = ce_smem_raw + ((1024u - (smem_u32(ce_smem_raw) & 1023u)) & 1023u)   /* offset from the __shared__ array: keeps the shared address space (LDS / STS) */;
-    unsigned char* sX = base;                                   // KB x 16 KB, resident per row block
-    unsigned char* sE = sX + KB * TC_TILE_BYTES;                // ring of table slices [128 classes][64 d]
-    unsigned char* sOut0 = sE + NS * TC_TILE_BYTES;             // 2 x 32 KB staging (G tiles)
-    float* s_part = reinterpret_cast<float*>(sOut0 + 2 * 32768);  // [4 column quarters][{max, sum, target logit}][128 rows]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(s_part) + 12 * 128 * 4);
-    uint64_t* efull = bars;                 // [NS]   TMA -> MMA
-    uint64_t* eempty = bars + NS;           // [NS]   MMA -> TMA
-    uint64_t* tfull = bars + 2 * NS;        // [2]    S accumulator ready
-    uint64_t* tempty = bars + 2 * NS + 2;   // [2]    S accumulator drained
-    uint64_t* xfull = bars + 2 * NS + 4;    // [1]
-    uint64_t* xempty = bars + 2 * NS + 5;   // [1]
-    uint64_t* gfull = bars + 2 * NS + 6;    // [2]    G staging tile written (epilogue -> MMA)
-    uint64_t* gempty = bars + 2 * NS + 8;   // [2]    second MMA has read the staging tile
-    uint64_t* dxfull = bars + 2 * NS + 10;  // [1]    dX accumulator complete
-    uint64_t* dxempty = bars + 2 * NS + 11; // [1]    dX accumulator drained
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * NS + 12);
-
+    unsigned char* base = ce_smem_raw + ((1024u - (smem_u32(ce_smem_raw) & 1023u)) & 1023u);
+    unsigned char* sX = base;
+    unsigned char* sE = base + SM::ROW_TILE;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sE + CE_STAGES * SM::CLS_TILE);
+    uint64_t* full = bars;
+    uint64_t* empty = bars + CE_STAGES;
+    uint64_t* xfull = bars + 2 * CE_STAGES;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (warp == 0 && lane == 0) {
+    const int row0 = blockIdx.x * 128;
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmX);
         tma_prefetch_desc(&tmE);
-        if (MODE == CE_STORE_G) tma_prefetch_desc(&tmG);
-        for (int s = 0; s < NS; ++s) { mbar_init(&efull[s], 1); mbar_init(&eempty[s], 1); }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&tfull[a], 1); mbar_init(&tempty[a], CE_EPI_WARPS);
-            mbar_init(&gfull[a], MODE == CE_STORE_G ? 1 : CE_EPI_WARPS); mbar_init(&gempty[a], 1);
-        }
+        for (int s = 0; s < CE_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         mbar_init(xfull, 1);
-        mbar_init(xempty, 1);
-        mbar_init(dxfull, 1);
-        mbar_init(dxempty, CE_EPI_WARPS);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_wait();  // prologue above overlaps the previous kernel's tail
-    const uint32_t tmem_dx = tmem_base + 256;
-    // CE_KEEP_G / CE_ACCUM_T: the G tile never touches shared memory - the epilogue packs it to bf16 pairs in tensor memory (2 x 64
-    // columns) and the second MMA takes its A operand from there.  With both operands in shared memory that MMA alone would read
-    // 96 KB per class tile (two N = 64 instructions re-reading A); the kernel is bound by shared-memory bandwidth, not by the tensor pipe.
-    const uint32_t tmem_g = tmem_base + 384;
-    const int num_items = (MODE == CE_ACCUM_T ? sh.nsplit : 2) * sh.num_m;
+    pdl_wait();
+    const int ntile = (a.C + 63) / 64;
+    const int sweeps = a.dx ? 2 : 1;
 
-    if (warp == 0) {
-        // ===================================================================== TMA producer
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0, xphase = 0;
-            for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
-                int blk, nb, ne;
-                ce_item<MODE>(w, sh, blk, nb, ne);
-                const int ntile = ne - nb;
-                mbar_wait(xempty, xphase ^ 1);
-                mbar_expect_tx(xfull, KB * TC_TILE_BYTES);
-                for (int kb = 0; kb < KB; ++kb) tma_load_2d(sX + kb * TC_TILE_BYTES, &tmX, kb * 64, blk * 128, xfull);
-                xphase ^= 1;
-                for (int tile = ONE ? -1 : 0; tile < SWEEPS * ntile; ++tile) {
-                    const int n0 = tile < 0 ? 0 : (nb + tile % ntile) * 128;      // tile -1: the probe (class tile 0) of CE_ONE_SWEEP
-                    for (int kb = 0; kb < KB; ++kb) {
-                        mbar_wait(&eempty[stage], phase ^ 1);
-                        mbar_expect_tx(&efull[stage], TC_TILE_BYTES);
-                        tma_load_2d(sE + stage * TC_TILE_BYTES, &tmE, kb * 64, n0, &efull[stage]);
-                        if (++stage == NS) { stage = 0; phase ^= 1; }
-                    }
+    if (warp < 4) {
+        if (warp == 0 && lane == 0) {
+            mbar_expect_tx(xfull, SM::ROW_TILE);
+            for (int b = 0; b < SM::XB; ++b) tma_load_2d(sX + b * 16384, &tmX, b * 64, row0, xfull);
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int sw = 0; sw < sweeps; ++sw)
+                for (int j = 0; j < ntile; ++j) {
+                    mbar_wait(&empty[stage], phase ^ 1);
+                    mbar_expect_tx(&full[stage], SM::CLS_TILE);
+                    for (int b = 0; b < SM::XB; ++b) tma_load_2d(sE + stage * SM::CLS_TILE + b * 8192, &tmE, b * 64, j * 64, &full[stage]);
+                    if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
                 }
-            }
         }
-    } else if (warp == 1) {
-        // ===================================================================== MMA issuer
-        if (lane == 0) {
-            constexpr uint32_t idesc1 = umma_idesc(128, 128, 0, 0);   // S  = X   E_n^T  (both K-major)
-            constexpr uint32_t idesc2 = umma_idesc(128, 64, 0, 1);    // dX += G   E_n    (A K-major staging, B MN-major table slice)
-            int stage = 0; uint32_t phase = 0, xphase = 0;
-            int acc = 0; uint32_t acc_phase = 0;
-            int gbuf = 0; uint32_t gphase = 0, dxphase = 0;
-            // dX += G(n) E_n : reads staging buffer `buf` (two 64-class halves) and the KB ring slices that held tile n
-            auto gemm2 = [&](int first_stage, int buf, bool first) {
-                if (MODE != CE_STORE_G) {
-                    // A = G tile in tensor memory; B = the KB adjacent ring slices of this class tile read MN-major as ONE [128 k][64 KB n]
-                    // operand (the next 64-wide n block is one slice = TC_TILE_BYTES away; a tile never wraps the ring: NS = 3 KB)
-                    constexpr uint32_t idesc2t = umma_idesc(128, 64 * KB, 0, 1);
-                    const uint32_t b_addr = smem_u32(sE + first_stage * TC_TILE_BYTES);
+        return;
+    }
+    // consumer warpgroup g: tile rows 64 g .. 64 g + 63 ; this thread: rows r[0], r[1] = r[0] + 8, columns 8 j + 2 q + {0, 1}
+    const int g = (warp >> 2) - 1, w = warp & 3, q = lane & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    int row[2], tgt[2];
+    float ic[2];
+    const float inv = *a.inv_count;
 #pragma unroll
-                    for (int k = 0; k < 8; ++k)   // 128 classes = 8 k-steps of 16 = 8 packed columns each
-                        umma_bf16_ts(tmem_dx, tmem_g + buf * 64 + k * 8, umma_desc(b_addr + k * 2048, TC_TILE_BYTES, 1024), idesc2t,
-                                     (first && k == 0) ? 0u : 1u);
+    for (int i = 0; i < 2; ++i) {
+        row[i] = row0 + 64 * g + 16 * w + (lane >> 2) + 8 * i;
+        tgt[i] = row[i] < a.T ? (int)a.tg[row[i]] : 0;
+        ic[i] = tgt[i] != 0 ? inv : 0.f;
+    }
+    mbar_wait(xfull, 0);
+    const uint32_t xa = smem_u32(sX) + g * 8192;
+    int stage = 0;
+    uint32_t phase = 0;
+    float m[2] = {-INFINITY, -INFINITY}, s[2] = {0.f, 0.f}, tl[2] = {0.f, 0.f};
+    for (int j = 0; j < ntile; ++j) {
+        mbar_wait(&full[stage], phase);
+        float S[32];
+        ce_scores<D>(S, xa, 16384, smem_u32(sE + stage * SM::CLS_TILE));
+        if (leader) mbar_arrive(&empty[stage]);
+        if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
 #pragma unroll
-                    for (int kb = 0; kb < KB; ++kb) umma_commit(&eempty[first_stage + kb]);
-                    umma_commit(&gempty[buf]);
-                    return;
+        for (int i = 0; i < 2; ++i) {
+            float mx = -INFINITY;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int col = j * 64 + 8 * jj + 2 * q + c;
+                    float& v = S[jj * 4 + i * 2 + c];
+                    if (col >= a.C) v = -INFINITY;
+                    if (col == tgt[i]) tl[i] = v;
+                    mx = fmaxf(mx, v);
                 }
-                const uint32_t a_addr = smem_u32(sOut0 + buf * 32768);
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float mn = fmaxf(m[i], mx);
+            float acc = s[i] * ex2_fast((m[i] - mn) * CE_L2E);
 #pragma unroll
-                for (int kb = 0; kb < KB; ++kb) {
-                    int st = first_stage + kb;
-                    if (st >= NS) st -= NS;
-                    const uint32_t b_addr = smem_u32(sE + st * TC_TILE_BYTES);
+            for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-                    for (int k = 0; k < 8; ++k) {   // 128 classes = 8 k-steps of 16: staging half k/4, 32 B per step inside the row
-                        const uint64_t ad = umma_desc(a_addr + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024);
-                        const uint64_t bd = umma_desc(b_addr + k * 2048, 16, 1024);   // 16 class-rows of 128 B per step
-                        umma_bf16(tmem_dx + kb * 64, ad, bd, idesc2, (first && k == 0) ? 0u : 1u);
-                    }
-                    umma_commit(&eempty[st]);      // this slice of the table is no longer needed
-                }
-                umma_commit(&gempty[buf]);
-            };
-            for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
-                int blk_, nb_, ne_;
-                ce_item<MODE>(w, sh, blk_, nb_, ne_);
-                const int ntile = ne_ - nb_;
-                mbar_wait(xfull, xphase);
-                xphase ^= 1;
-                tc_fence_after();
-                int prev_stage = -1, prev_buf = 0;
-                bool first_g = true;
-                for (int tile = ONE ? -1 : 0; tile < SWEEPS * ntile; ++tile) {
-                    const bool sweep1 = MODE == CE_ACCUM_T || (ONE ? tile >= 0 : tile >= ntile);
-                    mbar_wait(&tempty[acc], acc_phase ^ 1);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + acc * 128;
-                    const int tile_stage = stage;
-                    for (int kb = 0; kb < KB; ++kb) {
-                        mbar_wait(&efull[stage], phase);
-                        tc_fence_after();
-                        const uint32_t a_addr = smem_u32(sX + kb * TC_TILE_BYTES);
-                        const uint32_t b_addr = smem_u32(sE + stage * TC_TILE_BYTES);
+                for (int c = 0; c < 2; ++c) acc += ex2_fast((S[jj * 4 + i * 2 + c] - mn) * CE_L2E);
+            s[i] = acc;
+            m[i] = mn;
+        }
+    }
+    float shift[2];
 #pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma_bf16(d_tmem, umma_desc(a_addr + k * 32, 16, 1024), umma_desc(b_addr + k * 32, 16, 1024), idesc1,
-                                      (kb > 0 || k > 0) ? 1u : 0u);
-                        if (!(FUSE_DX && sweep1)) umma_commit(&eempty[stage]);   // sweep 1 keeps the slice for the dX MMA
-                        if (++stage == NS) { stage = 0; phase ^= 1; }
-                    }
-                    umma_commit(&tfull[acc]);
-                    if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-                    if (FUSE_DX && sweep1) {
-                        if (prev_stage >= 0) {   // dX MMA of the PREVIOUS class tile, once its G tile has been staged
-                            if (first_g) { mbar_wait(dxempty, dxphase ^ 1); tc_fence_after(); }
-                            mbar_wait(&gfull[prev_buf], gphase);
-                            tc_fence_after();
-                            gemm2(prev_stage, prev_buf, first_g);
-                            first_g = false;
-                            if (prev_buf == 1) gphase ^= 1;
-                        }
-                        prev_stage = tile_stage;
-                        prev_buf = gbuf;
-                        gbuf ^= 1;
-                    }
+    for (int i = 0; i < 2; ++i) {
+        s[i] += __shfl_xor_sync(0xffffffffu, s[i], 1);
+        s[i] += __shfl_xor_sync(0xffffffffu, s[i], 2);
+        tl[i] += __shfl_xor_sync(0xffffffffu, tl[i], 1);
+        tl[i] += __shfl_xor_sync(0xffffffffu, tl[i], 2);
+        shift[i] = m[i] * CE_L2E + __log2f(s[i]);
+        if (q == 0 && row[i] < a.T) {
+            a.row_loss[row[i]] = tgt[i] != 0 ? (m[i] + __logf(s[i]) - tl[i]) * ic[i] : 0.f;
+            a.shift[row[i]] = shift[i];
+        }
+    }
+    if (!a.dx) return;
+    float dx[D / 2];
+#pragma unroll
+    for (int k = 0; k < D / 2; ++k) dx[k] = 0.f;
+    for (int j = 0; j < ntile; ++j) {
+        mbar_wait(&full[stage], phase);
+        float S[32];
+        const uint32_t e_addr = smem_u32(sE + stage * SM::CLS_TILE);
+        ce_scores<D>(S, xa, 16384, e_addr);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int col = j * 64 + 8 * jj + 2 * q + c;
+                    float& v = S[jj * 4 + i * 2 + c];
+                    float gv = col < a.C ? ex2_fast(v * CE_L2E - shift[i]) * ic[i] : 0.f;
+                    if (col == tgt[i]) gv -= ic[i];
+                    v = gv;
                 }
-                if (FUSE_DX && ntile > 0) {
-                    if (first_g) { mbar_wait(dxempty, dxphase ^ 1); tc_fence_after(); }
-                    mbar_wait(&gfull[prev_buf], gphase);
-                    tc_fence_after();
-                    gemm2(prev_stage, prev_buf, first_g);
-                    if (prev_buf == 1) gphase ^= 1;
-                    umma_commit(dxfull);
-                    dxphase ^= 1;
-                }
-                umma_commit(xempty);  // every MMA that reads this row block has retired -> the producer may overwrite sX
+        ce_accumulate<D>(dx, S, e_addr);
+        if (leader) mbar_arrive(&empty[stage]);
+        if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
+    }
+#pragma unroll
+    for (int jj = 0; jj < D / 8; ++jj)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+            if (row[i] < a.T)
+                *reinterpret_cast<float2*>(a.dx + (size_t)row[i] * D + 8 * jj + 2 * q) = make_float2(dx[jj * 4 + i * 2], dx[jj * 4 + i * 2 + 1]);
+}
+
+template <int D>
+__global__ void __launch_bounds__(CE_THREADS, 1)
+    ce_table_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmE, CeArgs a) {
+    using SM = CeSmem<D>;
+    extern __shared__ unsigned char ce_smem_raw[];
+    unsigned char* base = ce_smem_raw + ((1024u - (smem_u32(ce_smem_raw) & 1023u)) & 1023u);
+    unsigned char* sE = base;
+    unsigned char* sX = base + SM::CLS_TILE;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sX + CE_STAGES * SM::CLS_TILE);
+    uint64_t* full = bars;
+    uint64_t* empty = bars + CE_STAGES;
+    uint64_t* efull = bars + 2 * CE_STAGES;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int cls0 = blockIdx.x * 64;
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tmX);
+        tma_prefetch_desc(&tmE);
+        for (int s = 0; s < CE_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+        mbar_init(efull, 1);
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_wait();
+    const int ntt = (a.T + 63) / 64;
+    const int g = (warp >> 2) - 1, w = warp & 3, q = lane & 3;
+    float acc[D / 2];
+    if (warp < 4) {
+        if (warp == 0 && lane == 0) {
+            mbar_expect_tx(efull, SM::CLS_TILE);
+            for (int b = 0; b < SM::XB; ++b) tma_load_2d(sE + b * 8192, &tmE, b * 64, cls0, efull);
+            // token tile tt -> stage tt % CE_STAGES; consumer warpgroup tt % 2 owns it (CE_STAGES is even)
+            for (int tt = 0; tt < ntt; ++tt) {
+                const int stage = tt % CE_STAGES;
+                mbar_wait(&empty[stage], ((tt / CE_STAGES) & 1) ^ 1);
+                mbar_expect_tx(&full[stage], SM::CLS_TILE);
+                for (int b = 0; b < SM::XB; ++b) tma_load_2d(sX + stage * SM::CLS_TILE + b * 8192, &tmX, b * 64, tt * 64, &full[stage]);
             }
         }
     } else {
-        // ===================================================================== epilogue (16 warps)
-        const int sub = warp & 3, cq = (warp - 2) >> 2;   // TMEM sub-partition ; 32-column quarter of the class tile
-        const int r = sub * 32 + lane;
-        int acc = 0; uint32_t acc_phase = 0;
-        int gbuf = 0; uint32_t gphase = 0, dxphase = 0, xphase_e = 0;
-        const float ic = MODE == CE_ACCUM_T ? 0.f : *inv_count;
-        for (int w = blockIdx.x; w < num_items; w += gridDim.x) {
-            int blk, nb, ne;
-            ce_item<MODE>(w, sh, blk, nb, ne);
-            const int half = w & 1;
-            const int row = blk * 128 + r;
-            float gshift = 0.f, g_sum = 0.f;   // exponent shift of this row ; sum of this thread's G' entries (this half, this quarter)
-            if (ONE) { mbar_wait(xfull, xphase_e); xphase_e ^= 1; }   // the epilogue reads the token tile itself (row norms)
-            int t = 0;
-            float tl = 0.f;
-            if (MODE != CE_ACCUM_T) {
-            t = row < sh.T ? (int)targets[row] : 0;
-            const float icr = t != 0 ? ic : 0.f;   // ignore_index = 0 (and rows past the end)
-            float m_run = -INFINITY;
-            // ------------------------------------------------------------------ sweep 0: statistics (CE_ONE_SWEEP: the probe tile only)
-            for (int n = ONE ? 0 : nb; n < (ONE ? 1 : ne); ++n) {
-                mbar_wait(&tfull[acc], acc_phase);
-                tc_fence_after();
-                {
-                    float v[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(sub * 32) << 16) + (uint32_t)(acc * 128 + cq * 32), v);
-                    // the accumulator is in registers: hand it back to the MMA warp before the element-wise work
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tempty[acc]);
-                    const int col0 = n * 128 + cq * 32;
-                    if (col0 + 32 > sh.C) {
+        const bool leader = (threadIdx.x & 127) == 0;
+        int cls[2];
 #pragma unroll
-                        for (int i = 0; i < 32; ++i)
-                            if (col0 + i >= sh.C) v[i] = -INFINITY;
-                    }
-                    if (!ONE && (unsigned)(t - col0) < 32u) {
+        for (int i = 0; i < 2; ++i) cls[i] = cls0 + 16 * w + (lane >> 2) + 8 * i;
+        const float inv = *a.inv_count;
 #pragma unroll
-                        for (int i = 0; i < 32; ++i)
-                            if (i == t - col0) tl = v[i];
-                    }
-                    float cm = v[0];
+        for (int k = 0; k < D / 2; ++k) acc[k] = 0.f;
+        mbar_wait(efull, 0);
+        const uint32_t ea = smem_u32(sE) + 0;
+        for (int tt = g; tt < ntt; tt += 2) {
+            const int stage = tt % CE_STAGES;
+            // this thread's 16 token columns: shift, target, 1 / count
+            float sh[16], icc[16];
+            int tg[16];
 #pragma unroll
-                    for (int i = 1; i < 32; ++i) cm = fmaxf(cm, v[i]);
-                    m_run = fmaxf(m_run, cm);
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int t = tt * 64 + 8 * jj + 2 * q + c;
+                    const bool ok = t < a.T;
+                    tg[jj * 2 + c] = ok ? (int)a.tg[t] : 0;
+                    sh[jj * 2 + c] = ok ? a.shift[t] : 0.f;
+                    icc[jj * 2 + c] = tg[jj * 2 + c] != 0 ? inv : 0.f;
                 }
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-            // combine the four column quarters of every row (this half of the classes) ...
-            s_part[(cq * 3 + 0) * 128 + r] = m_run;
-            s_part[(cq * 3 + 2) * 128 + r] = tl;
-            if (ONE) {
-                // this quarter's 32 terms of x_row . E[target]: x from the resident token tile (16-byte chunk j of a row sits at
-                // j ^ (row & 7) inside its 128-byte swizzle row), E[target] from global memory (L2-resident table)
-                float dot = 0.f;
-                if (cq * 32 < D) {
-                    const bf16* erow = table + (size_t)t * D + cq * 32;
-                    const unsigned char* xrow = sX + (cq >> 1) * TC_TILE_BYTES + r * 128;
+            mbar_wait(&full[stage], (tt / CE_STAGES) & 1);
+            const uint32_t x_addr = smem_u32(sX + stage * SM::CLS_TILE);
+            float S[32];
+            ce_scores<D>(S, ea + 0, 8192, x_addr);   // S^T: rows = this warpgroup's... all 64 classes, columns = 64 tokens
 #pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        const uint4 xu = *reinterpret_cast<const uint4*>(xrow + ((((cq & 1) * 4 + c) ^ (r & 7)) << 4));
-                        const uint4 eu = *reinterpret_cast<const uint4*>(erow + c * 8);
-                        const float2 x0 = unpack_bf16(xu.x), x1 = unpack_bf16(xu.y), x2 = unpack_bf16(xu.z), x3 = unpack_bf16(xu.w);
-                        const float2 e0 = unpack_bf16(eu.x), e1 = unpack_bf16(eu.y), e2 = unpack_bf16(eu.z), e3 = unpack_bf16(eu.w);
-                        dot = fmaf(x0.x, e0.x, dot); dot = fmaf(x0.y, e0.y, dot); dot = fmaf(x1.x, e1.x, dot); dot = fmaf(x1.y, e1.y, dot);
-                        dot = fmaf(x2.x, e2.x, dot); dot = fmaf(x2.y, e2.y, dot); dot = fmaf(x3.x, e3.x, dot); dot = fmaf(x3.y, e3.y, dot);
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        float& v = S[jj * 4 + i * 2 + c];
+                        const int k = jj * 2 + c;
+                        float gv = ex2_fast(v * CE_L2E - sh[k]) * icc[k];
+                        if (cls[i] == tg[k]) gv -= icc[k];
+                        v = gv;
                     }
-                }
-                s_part[(cq * 3 + 1) * 128 + r] = dot;
-            }
-            ce_bar_sync();
-            float mh = -INFINITY, tlh = 0.f;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                mh = fmaxf(mh, s_part[(q * 3 + 0) * 128 + r]);
-                tlh += s_part[(q * 3 + 2) * 128 + r];
-            }
-            if (ONE) {
-                const float tdot = (s_part[1 * 128 + r] + s_part[4 * 128 + r]) + (s_part[7 * 128 + r] + s_part[10 * 128 + r]);
-                const float mm = fmaxf(mh, tdot);
-                gshift = mm * kLog2e - __log2f(icr);
-                if (half == 0 && cq == 0 && row < sh.T) row_stats[row] = make_float2(mm, 0.f);
-                tl = 0.f;
-            } else {
-            // ... publish them, and pick up the partner item's maximum: both halves must scale their exponentials alike, their dX'
-            // partials and G' tiles are summed
-            if (cq == 0) sh.stats[(size_t)w * 128 + r] = make_float4(mh, 0.f, tlh, 0.f);
-            __threadfence();
-            ce_bar_sync();
-            if (warp == 2 && lane == 0) {
-                st_release_u32(sh.flags + w, 1u);
-                while (ld_acquire_u32(sh.flags + (w ^ 1)) == 0u) { }
-            }
-            ce_bar_sync();
-            const float4 pp = __ldcg(sh.stats + (size_t)(w ^ 1) * 128 + r);
-            const float mm = fmaxf(mh, pp.x);
-            gshift = mm * kLog2e - __log2f(icr);               // icr == 0 (ignored row) -> +inf -> every entry of G' is 2^-inf = 0
-            if (half == 0 && cq == 0 && row < sh.T) row_stats[row] = make_float2(mm, tlh + pp.z);
-            }
-            }
-            // ------------------------------------------------------------------ sweep 1: gradient tiles
-            if (MODE == CE_STORE_G && warp == 2 && lane == 0) tma_store_wait_read();  // both staging buffers are free of pending bulk stores
-            if (MODE != CE_ACCUM_T) ce_bar_sync();             // (also: everybody has read s_part)
-            for (int n = nb; n < ne; ++n) {
-                if (MODE == CE_ACCUM_T && n + 1 < ne)   // next tile's shifts -> L1 while this tile is processed
-                    asm volatile("prefetch.global.L1 [%0];" ::"l"(col_shift + (n + 1) * 128 + cq * 32));
-                mbar_wait(&tfull[acc], acc_phase);
-                tc_fence_after();
-                if (FUSE_DX) { mbar_wait(&gempty[gbuf], gphase ^ 1); tc_fence_after(); }   // the dX MMA that read this G buffer two tiles ago is done
-                unsigned char* sOut = sOut0 + gbuf * 32768;
-                {
-                    float v[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(sub * 32) << 16) + (uint32_t)(acc * 128 + cq * 32), v);
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tempty[acc]);   // accumulator drained (it lives in registers now)
-                    const int col0 = n * 128 + cq * 32;
-                    if (ONE && (unsigned)(t - col0) < 32u) {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i)
-                            if (i == t - col0) tl = v[i];
-                    }
-                    if (MODE == CE_ACCUM_T) {   // the shift belongs to the streaming (token) row = this tile's column
-                        const float4* cs = reinterpret_cast<const float4*>(col_shift + col0);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float4 s4 = __ldg(cs + j);
-                            v[4 * j] = ex2_fast(fmaf(v[4 * j], kLog2e, -s4.x));
-                            v[4 * j + 1] = ex2_fast(fmaf(v[4 * j + 1], kLog2e, -s4.y));
-                            v[4 * j + 2] = ex2_fast(fmaf(v[4 * j + 2], kLog2e, -s4.z));
-                            v[4 * j + 3] = ex2_fast(fmaf(v[4 * j + 3], kLog2e, -s4.w));
-                        }
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) v[i] = ex2_fast(fmaf(v[i], kLog2e, -gshift));   // exp(s - max) * (1/count), folded into the exponent
-                    }
-                    if (col0 + 32 > sh.C) {
-#pragma unroll
-                        for (int i = 0; i < 32; ++i)
-                            if (col0 + i >= sh.C) v[i] = 0.f;
-                    }
-                    if (MODE != CE_ACCUM_T) {   // row sum of G' (four partial chains keep the adds off the critical path)
-                        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll
-                        for (int i = 0; i < 32; i += 4) { a0 += v[i]; a1 += v[i + 1]; a2 += v[i + 2]; a3 += v[i + 3]; }
-                        g_sum += (a0 + a1) + (a2 + a3);
-                    }
-                    if (MODE != CE_STORE_G) {
-                        uint32_t pk[16];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) pk[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
-                        tmem_st16(tmem_g + ((uint32_t)(sub * 32) << 16) + (uint32_t)(gbuf * 64 + cq * 16), pk);
-                    } else {
-                    unsigned char* dst = sOut + (cq >> 1) * 16384 + r * 128;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        uint4 u;
-                        u.x = pack_bf16(v[8 * j], v[8 * j + 1]); u.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
-                        u.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]); u.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
-                        *reinterpret_cast<uint4*>(dst + ((((cq & 1) * 4 + j) ^ (r & 7)) << 4)) = u;
-                    }
-                    }
-                }
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-                if (MODE != CE_STORE_G) {
-                    // each warp hands its 32 x 32 piece of the G tile to the MMA warp on its own: no CTA-wide barrier per class tile
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&gfull[gbuf]);
-                } else {
-                fence_proxy_async();   // generic-proxy smem writes -> visible to TMA and to tcgen05.mma (async proxy)
-                ce_bar_sync();
-                if (warp == 2 && lane == 0) {
-                    if (FUSE_DX) mbar_arrive(&gfull[gbuf]);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        if (n * 128 + h * 64 < sh.ldl) tma_store_2d(&tmG, sOut + h * 16384, n * 128 + h * 64, blk * 128);
-                    tma_store_commit();
-                    tma_store_wait_read1();
-                }
-                ce_bar_sync();   // the staging buffer written two tiles ago has been read by its bulk store
-                }
-                if (gbuf == 1) gphase ^= 1;
-                gbuf ^= 1;
-            }
-            // row sums of this half -> global (four quarters combined through shared memory; slot 1 of s_part is free now)
-            if (MODE != CE_ACCUM_T) {
-                s_part[(cq * 3 + 1) * 128 + r] = g_sum;
-                if (ONE) s_part[(cq * 3 + 2) * 128 + r] = tl;
-                ce_bar_sync();
-                if (cq == 0 && row < sh.T) {
-                    row_sums[(size_t)half * sh.T + row] = (s_part[1 * 128 + r] + s_part[4 * 128 + r]) + (s_part[7 * 128 + r] + s_part[10 * 128 + r]);
-                    if (ONE)   // target logit of this half's classes (0 when the target lives in the other half)
-                        row_sums[(size_t)(2 + half) * sh.T + row] = (s_part[2 * 128 + r] + s_part[5 * 128 + r]) + (s_part[8 * 128 + r] + s_part[11 * 128 + r]);
-                }
-                if (ONE) ce_bar_sync();   // the next item's probe reuses slots 1 and 2 of s_part
-            }
-            if (FUSE_DX && ne > nb) {
-                // ------------------------------------------------------------------ dX' partial of this half: TMEM -> += fp32 global
-                mbar_wait(dxfull, dxphase);
-                dxphase ^= 1;
-                tc_fence_after();
-                if (cq * 32 < D) {
-                    float v[32];
-                    tmem_ld32(tmem_dx + ((uint32_t)(sub * 32) << 16) + (uint32_t)(cq * 32), v);
-                    if (row < sh.T) {
-                        float* dst = dx_out + (size_t)row * D + cq * 32;
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) red_add_v4_ce(dst + 4 * j, v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    }
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(dxempty);
-            }
+            ce_accumulate<D>(acc, S, x_addr);
+            if (leader) mbar_arrive(&empty[stage]);
         }
-        if (MODE == CE_STORE_G && warp == 2 && lane == 0) tma_store_wait_read();
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
+    // warpgroup 2 hands its sum to warpgroup 1 through shared memory (the X ring is free by now); fixed order: wg1 + wg2
+    float* red = reinterpret_cast<float*>(sX);
+    asm volatile("bar.sync 1, 384;" ::: "memory");
+    if (g == 1) {
+#pragma unroll
+        for (int k = 0; k < D / 2; ++k) red[(size_t)k * 128 + (threadIdx.x & 127)] = acc[k];
+    }
+    asm volatile("bar.sync 1, 384;" ::: "memory");
+    if (g == 0) {
+#pragma unroll
+        for (int jj = 0; jj < D / 8; ++jj)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int c = cls0 + 16 * w + (lane >> 2) + 8 * i;
+                const int k = jj * 4 + i * 2;
+                const float v0 = acc[k] + red[(size_t)k * 128 + (threadIdx.x & 127)];
+                const float v1 = acc[k + 1] + red[(size_t)(k + 1) * 128 + (threadIdx.x & 127)];
+                if (c < a.C) {
+                    float* dst = a.dtable + (size_t)c * D + 8 * jj + 2 * q;
+                    atomicAdd(dst, v0);          // one add per element and launch
+                    atomicAdd(dst + 1, v1);
+                }
+            }
     }
 }
 
-// X [T, D] bf16, E [C, D] bf16 -> row_sums [2][T], row_stats [T] {max, target logit}, (D <= 128) dx' [T, D] fp32 = G' E with
-// G' = exp(s - rowmax) * inv_count, and - store_g - G' [T, ldl] bf16 (columns >= C zeroed) for a dE GEMM.  Returns through *fused_dx
-// whether dx' was produced.  ce_finish_kernel (rowwise.cuh) turns these into the loss, d loss / d x and the operands of the dE pass.
-inline size_t ce_scratch_bytes(int T) { return (size_t)2 * ((T + 127) / 128) * (128 * sizeof(float4) + sizeof(unsigned)) + 256; }
-template <int KB, int MODE>
-inline cudaError_t ce_set_attr() {
-    static bool attr_set_dev[64] = {false};
-    int attr_dev = 0;
-    cudaGetDevice(&attr_dev);
-    bool& attr_set = attr_set_dev[attr_dev & 63];   // the attribute is per device
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(tc_ce_kernel<KB, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, ce_smem_bytes<KB>());
-        if (e != cudaSuccess) return e;
-        attr_set = true;
-    }
-    return cudaSuccess;
+template <int D>
+inline cudaError_t ce_set_smem() {
+    static bool attr_set[64] = {false};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (attr_set[dev & 63]) return cudaSuccess;
+    cudaError_t e = cudaFuncSetAttribute(ce_rows_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, CeSmem<D>::ROWS_BYTES);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(ce_table_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, CeSmem<D>::TABLE_BYTES);
+    if (e == cudaSuccess) attr_set[dev & 63] = true;
+    return e;
 }
-// scratch: ce_scratch_bytes(T) bytes of device memory (partials + flags); dx must hold [T, D] fp32 and is zero-filled here
-// mode: CE_STORE_G, CE_KEEP_G or CE_ONE_SWEEP (the latter two need D <= 128; row_sums must be [4][T] for CE_ONE_SWEEP: sums of the two
-// halves, then their target-logit partials)
-template <int KB>
-inline cudaError_t launch_tc_ce(const bf16* X, const bf16* E, bf16* G, int mode, int T, int C, int ldl, const long long* targets,
-                                const float* inv_count, float* row_sums, float2* row_stats, float* dx, bool* fused_dx, void* scratch,
-                                int num_sms, cudaStream_t st) {
-    CUtensorMap tmX, tmE, tmG;
-    const int D = 64 * KB;
-    if (KB > 2) mode = CE_STORE_G;
-    const bool store_g = mode == CE_STORE_G;
-    bool ok = make_tmap_bf16(&tmX, X, T, D, D, 64, 128) && make_tmap_bf16(&tmE, E, C, D, D, 64, 128) && make_tmap(&tmG, G, false, T, ldl, ldl, 64, 128);
-    if (!ok) return cudaErrorInvalidValue;
-    CeShape sh;
-    sh.T = T; sh.C = C; sh.ldl = ldl;
-    sh.num_m = (T + 127) / 128;
-    sh.num_n = (C + 127) / 128;
-    sh.n_half = (sh.num_n + 1) / 2;
-    sh.nsplit = 2;
-    sh.stats = reinterpret_cast<float4*>(scratch);
-    sh.flags = reinterpret_cast<unsigned*>(reinterpret_cast<unsigned char*>(scratch) + (size_t)2 * sh.num_m * 128 * sizeof(float4));
-    cudaError_t me = cudaSuccess;
-    if (mode != CE_ONE_SWEEP) me = cudaMemsetAsync(sh.flags, 0, (size_t)2 * sh.num_m * sizeof(unsigned), st);
-    if (me != cudaSuccess) return me;
-    *fused_dx = KB <= 2;
-    if (KB <= 2) {
-        me = cudaMemsetAsync(dx, 0, (size_t)T * D * sizeof(float), st);
-        if (me != cudaSuccess) return me;
-    }
-    // the two halves of a row block spin on each other: both must be resident at the same time -> even, persistent grid
-    int grid = 2 * sh.num_m < num_sms ? 2 * sh.num_m : (num_sms & ~1);
-    if (store_g) {
-        me = ce_set_attr<KB, CE_STORE_G>();
-        if (me != cudaSuccess) return me;
-        launch_k(tc_ce_kernel<KB, CE_STORE_G>, grid, CE_THREADS, ce_smem_bytes<KB>(), st, tmX, tmE, tmG, sh, targets, inv_count, row_sums,
-                 row_stats, (const float*)nullptr, E, dx);
-    } else if (mode == CE_ONE_SWEEP) {
-        constexpr int M = KB <= 2 ? CE_ONE_SWEEP : CE_STORE_G;
-        me = ce_set_attr<KB, M>();
-        if (me != cudaSuccess) return me;
-        grid = 2 * sh.num_m < num_sms ? 2 * sh.num_m : num_sms;     // no exchange between the halves: any grid will do
-        launch_k(tc_ce_kernel<KB, M>, grid, CE_THREADS, ce_smem_bytes<KB>(), st, tmX, tmE, tmG, sh, targets, inv_count, row_sums, row_stats,
-                 (const float*)nullptr, E, dx);
-    } else {
-        constexpr int M = KB <= 2 ? CE_KEEP_G : CE_STORE_G;
-        me = ce_set_attr<KB, M>();
-        if (me != cudaSuccess) return me;
-        launch_k(tc_ce_kernel<KB, M>, grid, CE_THREADS, ce_smem_bytes<KB>(), st, tmX, tmE, tmG, sh, targets, inv_count, row_sums, row_stats,
-                 (const float*)nullptr, E, dx);
-    }
+// loss per row, shift per row and (a.dx != null) d loss / d xf
+template <int D>
+inline cudaError_t launch_tc_ce(const bf16* xf, const bf16* table, const CeArgs& a, cudaStream_t st) {
+    CUtensorMap tmX, tmE;
+    if (!make_tmap_bf16(&tmX, xf, a.T, D, D, 64, 128) || !make_tmap_bf16(&tmE, table, a.C, D, D, 64, 64)) return cudaErrorInvalidValue;
+    cudaError_t e = ce_set_smem<D>();
+    if (e != cudaSuccess) return e;
+    launch_k(ce_rows_kernel<D>, (a.T + 127) / 128, CE_THREADS, CeSmem<D>::ROWS_BYTES, st, tmX, tmE, a);
     return cudaGetLastError();
 }
-
-// dE [C, D] fp32 += G^T X without G in HBM (CE_ACCUM_T): G[t, c] = 2^(s_tc log2e - col_shift[t]) with s = X E^T recomputed, col_shift
-// [ceil(T/128)*128] = log2e * logsumexp_t - log2(inv_count_t) from ce_finish_kernel (+inf for ignored tokens and the padding).
-// One work item = a block of 128 classes x 1/nsplit of the token tiles; its accumulator leaves through 16-byte vector reductions.
-inline int ce_accum_nsplit(int num_m, int num_n, int num_sms) {
-    int best = 1; long long best_cost = -1;
-    for (int ns = 1; ns <= 16 && ns <= num_n; ++ns) {
-        const long long rounds = ((long long)num_m * ns + num_sms - 1) / num_sms;
-        const long long cost = rounds * ((num_n + ns - 1) / ns + 2);   // +2: resident load and accumulator flush of every item
-        if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = ns; }
-    }
-    return best;
-}
-template <int KB>
-inline cudaError_t launch_tc_ce_accum_t(const bf16* X, const bf16* E, const float* col_shift, float* dE, int T, int C, int num_sms,
-                                        cudaStream_t st) {
-    static_assert(KB <= 2, "second MMA needs D <= 128");
-    CUtensorMap tmRes, tmStream;
-    const int D = 64 * KB;
-    bool ok = make_tmap_bf16(&tmRes, E, C, D, D, 64, 128) && make_tmap_bf16(&tmStream, X, T, D, D, 64, 128);
-    if (!ok) return cudaErrorInvalidValue;
-    CeShape sh;
-    sh.T = C; sh.C = T; sh.ldl = 0;            // resident rows = classes, streaming rows = tokens
-    sh.num_m = (C + 127) / 128;
-    sh.num_n = (T + 127) / 128;
-    sh.n_half = 0;
-    sh.nsplit = ce_accum_nsplit(sh.num_m, sh.num_n, num_sms);
-    sh.stats = nullptr; sh.flags = nullptr;
-    cudaError_t me = ce_set_attr<KB, CE_ACCUM_T>();
-    if (me != cudaSuccess) return me;
-    const int items = sh.num_m * sh.nsplit;
-    const int grid = items < num_sms ? items : num_sms;
-    launch_k(tc_ce_kernel<KB, CE_ACCUM_T>, grid, CE_THREADS, ce_smem_bytes<KB>(), st, tmRes, tmStream, tmStream, sh, (const long long*)nullptr,
-             (const float*)nullptr, (float*)nullptr, (float2*)nullptr, col_shift, (const bf16*)nullptr, dE);
+// a.dtable += d loss / d table, from the shifts launch_tc_ce left
+template <int D>
+inline cudaError_t launch_ce_table(const bf16* xf, const bf16* table, const CeArgs& a, cudaStream_t st) {
+    CUtensorMap tmX, tmE;
+    if (!make_tmap_bf16(&tmX, xf, a.T, D, D, 64, 64) || !make_tmap_bf16(&tmE, table, a.C, D, D, 64, 64)) return cudaErrorInvalidValue;
+    cudaError_t e = ce_set_smem<D>();
+    if (e != cudaSuccess) return e;
+    launch_k(ce_table_kernel<D>, (a.C + 63) / 64, CE_THREADS, CeSmem<D>::TABLE_BYTES, st, tmX, tmE, a);
     return cudaGetLastError();
 }
 

@@ -1,17 +1,18 @@
-// genrec_b200 - Blackwell-native GEMM: TMA (cp.async.bulk.tensor, 128B swizzle) -> shared memory -> tcgen05.mma
-// (single-thread issue, fp32 accumulators in TMEM, double-buffered) -> tcgen05.ld epilogue with fused element-wise work.
+// genrec_b200 - Hopper GEMM: TMA (cp.async.bulk.tensor, 128B swizzle) -> shared-memory ring (mbarrier pipeline) -> wgmma
+// (fp32 accumulators in registers) -> shared-memory accumulator tile -> fused element-wise epilogue -> TMA stores.
 //
 //   C[M,N] (+)= opA(A) * opB(B)          bf16 operands, fp32 accumulate
 //     A_MN = 0 : A stored [M][K] (K contiguous)        A_MN = 1 : A stored [K][M] (M contiguous)
 //     B_MN = 0 : B stored [N][K] (K contiguous)        B_MN = 1 : B stored [K][N] (N contiguous)
-//   Both majors map straight onto UMMA shared-memory descriptors (K-major / MN-major canonical SWIZZLE_128B layouts),
-//   so no operand is ever transposed in memory.
+//   Both majors map straight onto wgmma shared-memory descriptors (K-major / MN-major canonical SWIZZLE_128B layouts, the
+//   MN-major ones through the instruction's transpose bits), so no operand is ever transposed in memory.
 //
-// Persistent kernel, one CTA per SM, 320 threads:
-//   warp 0    : TMA producer (one elected lane)      - ring of TC_STAGES x (A 16 KB + B 16 KB)
-//   warp 1    : TMEM allocator + MMA issuer (one lane): 4 x tcgen05.mma (K = 16 each) per 64-wide k-block
-//   warps 2-9 : epilogue; warp w owns TMEM lanes 32*(w%4)..+31 = 32 rows of the 128 x 128 tile and, by (w-2)/4, one
-//               64-column half of it (two warps per TMEM sub-partition so the element-wise work has 8 warps to run on)
+// Persistent kernel, one CTA per SM, 384 threads:
+//   warp 0        : TMA producer (one elected lane)      - ring of TC_STAGES x (A 16 KB + B 16 KB)
+//   warps 1-3     : idle (they complete the producer warpgroup so that the consumers are aligned warpgroups)
+//   warpgroups 1-2: consumers; warpgroup g issues m64n128k16 wgmma for rows 64*g .. 64*g+63 of the 128 x 128 tile, parks the
+//                   accumulators in shared memory and runs the epilogue on them: its warp w owns 32 rows and one 64-column
+//                   half of the tile (the same row / column split for every epilogue functor below)
 // Work item = (m tile, n tile, k split).  Split-K partial sums go out through an atomic epilogue.
 #pragma once
 #include <cuda.h>
@@ -20,14 +21,14 @@
 
 namespace grb {
 
-constexpr int TC_EPI_WARPS = 8;    // 2 per TMEM sub-partition: each converts 4 / (TC_EPI_WARPS / 4) 32-column chunks of the tile
-constexpr int TC_EPI_CPW = 4 / (TC_EPI_WARPS / 4);   // chunks per warp (16 warps measured slower here: register spills)
-static_assert(TC_EPI_CPW == 2, "a warp's 2 x 32 columns are one 64-column bf16 store box");
-constexpr int TC_BM = 128, TC_BN = 128, TC_BK = 64, TC_STAGES = 3, TC_THREADS = 64 + 32 * TC_EPI_WARPS;  // TMA, MMA, epilogue warps
+constexpr int TC_EPI_WARPS = 8;    // 4 per consumer warpgroup: each converts TC_EPI_CPW 32-column chunks of 32 rows
+constexpr int TC_EPI_CPW = 2;
+constexpr int TC_BM = 128, TC_BN = 128, TC_BK = 64, TC_STAGES = 3, TC_THREADS = 128 + 32 * TC_EPI_WARPS;  // producer WG + 2 consumer WGs
 constexpr int TC_TILE_BYTES = TC_BM * TC_BK * 2;  // 16 KB per operand per stage
 constexpr int TC_STAGE_OUT_BYTES = 64 * 1024;   // epilogue staging: 2 x bf16 [128x128] or 1 x fp32 [128x128], 128B-swizzled boxes
-constexpr int TC_SMEM_BYTES = 2 * TC_STAGES * TC_TILE_BYTES + 2 * TC_STAGE_OUT_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-constexpr int TC_TMEM_COLS = 2 * TC_BN;           // two accumulators
+constexpr int TC_ACC_BYTES = TC_BM * TC_BN * 4;  // fp32 accumulator tile
+// 3 x 32 KB ring + 64 KB output staging + 64 KB accumulator tile = 224 KB of the 227 KB a Hopper block may use
+constexpr int TC_SMEM_BYTES = 2 * TC_STAGES * TC_TILE_BYTES + TC_STAGE_OUT_BYTES + TC_ACC_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 
 // ------------------------------------------------------------------------------------------------ PTX wrappers
 GRB_DEVINL void mbar_init(uint64_t* bar, uint32_t count) {
@@ -67,66 +68,98 @@ GRB_DEVINL void tma_store_2d(const CUtensorMap* tmap, const void* smem_src, int 
 }
 GRB_DEVINL void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 GRB_DEVINL void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-GRB_DEVINL void tma_store_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 GRB_DEVINL void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-GRB_DEVINL void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(32 * TC_EPI_WARPS) : "memory"); }   // the epilogue warps only
 GRB_DEVINL void tma_prefetch_desc(const CUtensorMap* tmap) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
 }
-GRB_DEVINL void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// the 128 threads of consumer warpgroup g (named barriers 2 and 3; 0 is __syncthreads)
+GRB_DEVINL void wg_bar_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory"); }
+
+GRB_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+GRB_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+GRB_DEVINL void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-GRB_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-GRB_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-GRB_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-GRB_DEVINL void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 128] (+)= A[smem desc, 64 x 16] * B[smem desc, 16 x 128]; TA / TB = 1: the operand is MN-major (transposed)
+template <int TA, int TB>
+GRB_DEVINL void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier once every tcgen05.mma issued so far by this thread has completed
-GRB_DEVINL void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-GRB_DEVINL void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t* r = reinterpret_cast<uint32_t*>(v);
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,"
-        "%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
-// Shared-memory matrix descriptor, SWIZZLE_128B, sm_100 (version = 1).  Tile base must be 1024-byte aligned; `byte_off`
+// Shared-memory matrix descriptor, SWIZZLE_128B (sm_90 layout type 1).  Tile base must be 1024-byte aligned; `byte_off`
 // selects the k-slice inside it.   K-major : rows of 128 B (64 bf16 along K), 8-row groups SBO = 1024 B apart.
 //                                  MN-major: k-rows of 128 B (64 bf16 along MN), 8-k groups SBO = 1024 B apart, the next
 //                                            64-wide MN block LBO bytes away.
-GRB_DEVINL uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+GRB_DEVINL uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;  // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;  // SWIZZLE_128B
     return d;
 }
-// Instruction descriptor for kind::f16, bf16 x bf16 -> f32
-GRB_DEVINL constexpr uint32_t umma_idesc(int M, int N, int a_mn, int b_mn) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) |
-           ((uint32_t)(M >> 4) << 24);
+
+// One consumer warpgroup's share of a work item: rows 64*g .. +63 of the 128 x 128 tile over k-blocks kb0 .. kb1-1 of the ring.
+// Each stage is released to the producer once the wgmma reading it has retired (one MMA batch stays in flight).
+template <int A_MN, int B_MN, int STAGES>
+GRB_DEVINL void tc_mainloop(float (&acc)[64], const unsigned char* sA, const unsigned char* sB, uint64_t* full_bar, uint64_t* empty_bar,
+                            int kb0, int kb1, int g, int& stage, uint32_t& phase) {
+    const bool leader = (threadIdx.x & 127) == 0;
+    int prev = -1;
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;   // the first wgmma overwrites them; this only ends their live range at the previous epilogue
+    for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(sA + stage * TC_TILE_BYTES) + g * (TC_TILE_BYTES / 2);  // 64 rows (K-major) or one 64-wide M box
+        const uint32_t b_addr = smem_u32(sB + stage * TC_TILE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k) {
+            // K-major: +32 B per 16-wide k-slice inside the 128 B swizzle row ; MN-major: +16 k-rows = 2048 B
+            const uint64_t ad = A_MN == 0 ? wgmma_desc(a_addr + k * 32, 16, 1024) : wgmma_desc(a_addr + k * 2048, TC_TILE_BYTES / 2, 1024);
+            const uint64_t bd = B_MN == 0 ? wgmma_desc(b_addr + k * 32, 16, 1024) : wgmma_desc(b_addr + k * 2048, TC_TILE_BYTES / 2, 1024);
+            wgmma_m64n128k16<A_MN, B_MN>(acc, ad, bd, (kb > kb0 || k > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+}
+
+// Accumulator tile in shared memory: fp32 [128 rows][128 cols], 16-byte chunk j of row r stored at chunk (j ^ (r & 7)), so that
+// both the fragment stores below and the row-per-thread reads of the epilogue are free of bank conflicts.
+GRB_DEVINL void tc_acc_store(float* sAcc, const float (&acc)[64], int g) {
+    const int t = threadIdx.x & 127, w = t >> 5, lane = t & 31;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int r = g * 64 + w * 16 + (lane >> 2) + 8 * i;       // wgmma D fragment: row, column pair 8 j + 2 (lane % 4)
+            const int c = 8 * j + 2 * (lane & 3);
+            float* dst = sAcc + r * TC_BN + (((c >> 2) ^ (r & 7)) << 2) + (c & 3);
+            *reinterpret_cast<float2*>(dst) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+        }
+    }
+}
+// columns c*32 .. c*32+31 of row r
+GRB_DEVINL void tc_acc_load32(const float* sAcc, int r, int c, float (&v)[32]) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const float4 f = *reinterpret_cast<const float4*>(sAcc + r * TC_BN + (((c * 8 + j) ^ (r & 7)) << 2));
+        v[4 * j] = f.x; v[4 * j + 1] = f.y; v[4 * j + 2] = f.z; v[4 * j + 3] = f.w;
+    }
 }
 
 struct TcGemmShape {
@@ -146,18 +179,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC0,
                    const __grid_constant__ CUtensorMap tmC1, TcGemmShape sh, Epi epi) {
     extern __shared__ unsigned char tc_smem_raw[];
-    // 1024-byte aligned operand ring, then barriers
+    // 1024-byte aligned operand ring, output staging, accumulator tile, then barriers
     unsigned char* base = tc_smem_raw + ((1024u - (smem_u32(tc_smem_raw) & 1023u)) & 1023u)   /* offset from the __shared__ array: keeps the shared address space (LDS / STS) */;
     unsigned char* sA = base;
     unsigned char* sB = base + TC_STAGES * TC_TILE_BYTES;
-    unsigned char* sOut0 = base + 2 * TC_STAGES * TC_TILE_BYTES;  // 2 x 64 KB staging (double-buffered), 1024-aligned
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sOut0 + 2 * TC_STAGE_OUT_BYTES);
+    unsigned char* sOut = base + 2 * TC_STAGES * TC_TILE_BYTES;
+    float* sAcc = reinterpret_cast<float*>(sOut + TC_STAGE_OUT_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sOut + TC_STAGE_OUT_BYTES + TC_ACC_BYTES);
     uint64_t* full_bar = bars;                       // [TC_STAGES]  TMA -> MMA
-    uint64_t* empty_bar = bars + TC_STAGES;          // [TC_STAGES]  MMA -> TMA
-    uint64_t* tfull_bar = bars + 2 * TC_STAGES;      // [2]          MMA -> epilogue
-    uint64_t* tempty_bar = bars + 2 * TC_STAGES + 2; // [2]          epilogue -> MMA
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * TC_STAGES + 4);
-    uint64_t* zfull_bar = bars + 2 * TC_STAGES + 5;  // [2]          TMA -> epilogue (auxiliary operand tile, Epi::kAux)
+    uint64_t* empty_bar = bars + TC_STAGES;          // [TC_STAGES]  MMA -> TMA (one arrive per consumer warpgroup)
+    uint64_t* zempty_bar = bars + 2 * TC_STAGES;     // epilogue -> TMA: the auxiliary tile has been read (Epi::kAux)
+    uint64_t* zfull_bar = bars + 2 * TC_STAGES + 1;  // TMA -> epilogue: auxiliary operand tile landed
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     epi.prepare();
@@ -167,31 +199,22 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < TC_STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], 2);
         }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&tfull_bar[a], 1);
-            mbar_init(&tempty_bar[a], TC_EPI_WARPS);  // one arrive per epilogue warp
-            mbar_init(&zfull_bar[a], 1);
-        }
+        mbar_init(zempty_bar, TC_EPI_WARPS);  // one arrive per epilogue warp
+        mbar_init(zfull_bar, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, TC_TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_wait();  // prologue above overlaps the previous kernel's tail
 
     const int num_work = sh.num_m * sh.num_n * sh.splits;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ===================================================================== TMA producer
-        if (lane == 0) {
+        if (warp == 0 && lane == 0) {
             int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
+            uint32_t phase = 0, zphase = 0;
             for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
                 const int split = w % sh.splits;
                 const int tile = w / sh.splits;
@@ -219,64 +242,38 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                     if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
                 }
                 if constexpr (Epi::kAux) {
-                    // auxiliary element-wise operand of this tile -> the unused half of the tile's staging buffer, as soon as
-                    // the epilogue that last used that buffer (two tiles ago) has drained it
-                    mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                    unsigned char* z_dst = sOut0 + acc * TC_STAGE_OUT_BYTES + 32768;
-                    mbar_expect_tx(&zfull_bar[acc], 32768);
-                    tma_load_2d(z_dst, &tmC1, n0, m0, &zfull_bar[acc]);                  // box {64 cols, 128 rows}
-                    tma_load_2d(z_dst + 16384, &tmC1, n0 + 64, m0, &zfull_bar[acc]);
-                    if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+                    // auxiliary element-wise operand of this tile -> the half of the staging buffer a single bf16 output leaves
+                    // free, as soon as the epilogue of the previous tile has read it
+                    mbar_wait(zempty_bar, zphase ^ 1);
+                    unsigned char* z_dst = sOut + 32768;
+                    mbar_expect_tx(zfull_bar, 32768);
+                    tma_load_2d(z_dst, &tmC1, n0, m0, zfull_bar);                  // box {64 cols, 128 rows}
+                    tma_load_2d(z_dst + 16384, &tmC1, n0 + 64, m0, zfull_bar);
+                    zphase ^= 1;
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================================================================== MMA issuer
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc(TC_BM, TC_BN, A_MN, B_MN);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-                const int split = w % sh.splits;
-                const int kb0 = split * sh.kblocks_per_split;
-                const int kb1 = min(sh.kblocks_total, kb0 + sh.kblocks_per_split);
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);  // epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * TC_BN;
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(sA + stage * TC_TILE_BYTES);
-                    const uint32_t b_addr = smem_u32(sB + stage * TC_TILE_BYTES);
-#pragma unroll
-                    for (int k = 0; k < TC_BK / 16; ++k) {
-                        // K-major: +32 B per 16-wide k-slice inside the 128 B swizzle row ; MN-major: +16 k-rows = 2048 B
-                        const uint64_t ad = A_MN == 0 ? umma_desc(a_addr + k * 32, 16, 1024) : umma_desc(a_addr + k * 2048, TC_TILE_BYTES / 2, 1024);
-                        const uint64_t bd = B_MN == 0 ? umma_desc(b_addr + k * 32, 16, 1024) : umma_desc(b_addr + k * 2048, TC_TILE_BYTES / 2, 1024);
-                        umma_bf16(d_tmem, ad, bd, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs retire
-                    if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tfull_bar[acc]);        // accumulator complete
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
             }
         }
     } else {
-        // ===================================================================== epilogue (warps 2..9)
-        const int sub = warp & 3;         // TMEM sub-partition this warp may access: lanes 32*sub .. 32*sub+31
-        const int cq = (warp - 2) >> 2;     // which 32-column chunk of the tile this warp converts
-        int acc = 0;
-        uint32_t acc_phase = 0;
+        // ===================================================================== consumers: MMA + epilogue
+        const int g = (warp >> 2) - 1;             // consumer warpgroup: tile rows 64 g .. 64 g + 63
+        const int wi = warp & 3;
+        const int sub = g * 2 + (wi & 1);          // 32-row slab of the tile this warp converts
+        const int cq = wi >> 1;                    // which 64-column half of the tile this warp converts
+        int stage = 0;
+        uint32_t phase = 0, zphase = 0;
+        float acc[64];
         for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
+            const int split = w % sh.splits;
             const int tile = w / sh.splits;
             const int m0 = (tile / sh.num_n) * TC_BM, n0 = (tile % sh.num_n) * TC_BN;
-            const int r = sub * 32 + lane;  // row inside the tile == TMEM lane
+            const int kb0 = split * sh.kblocks_per_split;
+            const int kb1 = min(sh.kblocks_total, kb0 + sh.kblocks_per_split);
+            tc_mainloop<A_MN, B_MN, TC_STAGES>(acc, sA, sB, full_bar, empty_bar, kb0, kb1, g, stage, phase);
+            wg_bar_sync(g);                        // the previous tile's epilogue of this warpgroup has read sAcc
+            tc_acc_store(sAcc, acc, g);
+            wg_bar_sync(g);
+            const int r = sub * 32 + lane;  // row inside the tile
             const int row = m0 + r;
-            // operands of the fused element-wise work that do not depend on the MMA (residual rows, saved pre-activations)
-            // are fetched BEFORE waiting for the accumulator, so their latency hides behind the tensor-core work
             float pre[Epi::kPre ? TC_EPI_CPW : 1][Epi::kPre ? 32 : 1];
             if constexpr (Epi::kPre) {
 #pragma unroll
@@ -287,18 +284,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                 }
             }
             if constexpr (Epi::kOut != 0) {
-                if (lane == 0) tma_store_wait_read1();   // this warp's store from two tiles ago has finished reading its staging piece
+                if (lane == 0) tma_store_wait_read();   // this warp's store of the previous tile has finished reading its staging piece
                 __syncwarp();
             }
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            unsigned char* sOut = sOut0 + acc * TC_STAGE_OUT_BYTES;  // staging buffer alternates with the accumulator
-            if constexpr (Epi::kAux) mbar_wait(&zfull_bar[acc], acc_phase);
+            if constexpr (Epi::kAux) mbar_wait(zfull_bar, zphase);
 #pragma unroll
             for (int ci = 0; ci < TC_EPI_CPW; ++ci) {
                 const int c = cq * TC_EPI_CPW + ci;
                 float v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(sub * 32) << 16) + (uint32_t)(acc * TC_BN + c * 32), v);
+                tc_acc_load32(sAcc, r, c, v);
                 const int col0 = n0 + c * 32;
                 const int nvalid = min(32, sh.N - col0);
                 if constexpr (Epi::kOut == 0) {
@@ -351,15 +345,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                     }
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty_bar[acc]);   // accumulator drained: the MMA warp may start the next-but-one tile
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+            if constexpr (Epi::kAux) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(zempty_bar);   // auxiliary tile read: the producer may load the next one
+                zphase ^= 1;
+            }
             if constexpr (Epi::kOut != 0) {
                 // Every epilogue warp owns rows 32*sub .. +31 of the 64-column (bf16) / 2 x 32-column (fp32) slab cq of the staging
                 // tile - a contiguous, swizzle-aligned 4 KB piece of each 128-row box - and stores it with its OWN bulk store (tensor-map
-                // box = 32 rows): no CTA-wide barrier per tile, the warps drift apart freely.  Buffer reuse is guarded per warp by
-                // `wait_group.read 1` at the top of the tile (the piece written two tiles ago has been read).
+                // box = 32 rows): no CTA-wide barrier per tile.  Buffer reuse is guarded per warp by `wait_group.read 0` at the top of
+                // the next tile.
                 fence_proxy_async();   // generic-proxy smem writes -> visible to the TMA (async proxy)
                 __syncwarp();
                 if (lane == 0 && m0 + sub * 32 < sh.M) {
@@ -380,12 +375,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             }
         }
         if (Epi::kOut != 0 && lane == 0) tma_store_wait_read();  // smem must outlive this warp's last bulk stores
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TC_TMEM_COLS);
     }
 }
 

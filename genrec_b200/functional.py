@@ -77,20 +77,10 @@ def cast_bf16(src: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Te
 _ZERO_TABLES = {}
 
 
-def attn_legacy(L: Optional[int] = None) -> bool:
-    """Which attention kernels will run (GRB_ATTN = tc | mma | auto, see csrc/api.cu attn_mode): True when the mma.sync kernels need
-    their [B, L, ld] bias-index matrix - always for GRB_ATTN=mma, and for seq_len <= 256 in the default auto mode."""
-    mode = os.environ.get("GRB_ATTN", "auto")
-    return mode == "mma" or (mode != "tc" and L is not None and L <= 256)
-
-
 class SeqMeta:
-    """Per-batch sequence metadata shared by all layers of one forward.
-
-    tcgen05 attention path (default): the pad flags, the raw timestamps and their per-sequence int32 rebasing
-    (``grb_hstu_seq_prepare``, one tiny launch per batch) - buckets and masks are derived inside the attention kernels.
-    The [B, L, ld] uint16 bias-index matrix of the mma.sync path is built lazily, only when that path will run
-    (non-uniform position buckets, or GRB_ATTN=mma)."""
+    """Per-batch sequence metadata shared by all layers of one forward: the pad flags, the raw timestamps and the
+    [B, L, ld] uint16 bias-index matrix the attention kernels read.  The per-sequence int32 rebasing of the timestamps
+    (``grb_hstu_seq_prepare``) is made on demand for the bucket test hook."""
 
     def __init__(self, pad_u8: torch.Tensor, timestamps: Optional[torch.Tensor], pos_bucket: torch.Tensor,
                  time_thr: torch.Tensor, num_time_buckets: int = 64, num_pos_buckets: int = 32, pos_uniform=None):
@@ -113,10 +103,7 @@ class SeqMeta:
         self.ld = (L + 7) // 8 * 8
         self.bias_index = None
         self.rel32 = self.wide = None
-        if self.pos_uniform and not attn_legacy(L):
-            self._ensure_rel()               # the tcgen05 kernels will run: they read the rebased timestamps
-        else:
-            self._build_bias_index()         # the mma.sync kernels will run: they read the index matrix
+        self._build_bias_index()
 
     def _ensure_rel(self):
         if self.timestamps is None or self.rel32 is not None:
@@ -145,20 +132,17 @@ class SeqMeta:
         check(_lib.load().grb_hstu_bias_index(ptr(self.timestamps), ptr(self.pad), ptr(self.time_thr), ptr(pb_arg), B, L,
                                               npos_arg, nt, ptr(self.bias_index), self.ld, stream_ptr(dev)))
 
-    def struct(self, tc: bool = False) -> HstuSeq:
-        """tc=True: the caller will run the tcgen05 kernels whatever the dispatch policy says (stand-alone attention entry points)."""
-        if tc or (self.pos_uniform and not attn_legacy(self.L)):
-            self._ensure_rel()
-        else:
-            self._build_bias_index()
+    def struct(self) -> HstuSeq:
         return HstuSeq(ptr(self.bias_index), self.ld, 1 if self.timestamps is not None else 0, 1 if self.pos_uniform else 0,
                        self.pos_bucket0, ptr(self.timestamps), ptr(self.pad), ptr(self.rel32), ptr(self.wide), ptr(self.time_thr))
 
     def bucket_bytes(self, num_time_buckets: Optional[int] = None) -> torch.Tensor:
-        """[B, L, L] uint8: the time bucket (or 64 = masked) the tcgen05 attention kernels derive for every cell (test hook)."""
+        """[B, L, L] uint8: the time bucket (or 64 = masked) of every cell as the in-kernel bucket routine derives it from the
+        rebased timestamps (test hook)."""
         nt = self.num_time_buckets if num_time_buckets is None else num_time_buckets
         out = torch.full((self.B, self.L, self.L), 255, dtype=torch.uint8, device=self.pad.device)
-        seq = self.struct(tc=True)
+        self._ensure_rel()
+        seq = self.struct()
         with torch.cuda.device(self.pad.device):
             check(_lib.load().grb_hstu_bucket_bytes_debug(C.byref(seq), self.B, self.L, nt if self.timestamps is not None else 0, ptr(out),
                                                           stream_ptr(self.pad.device)))
@@ -275,9 +259,11 @@ class EmbedFn(torch.autograd.Function):
         else:
             dtable = torch.zeros(tshape, dtype=torch.float32, device=dx.device)
             dpos = torch.zeros(pshape, dtype=torch.float32, device=dx.device) if pshape is not None else None
+        order = torch.sort(ids.reshape(-1), stable=True).indices   # tokens grouped by id, in token order
+        scratch = torch.empty(B * L, D, dtype=torch.float32, device=dx.device)
         with torch.cuda.device(dx.device):
-            check(lib.grb_embed_backward(ptr(ids), ptr(dx), ptr(dtable), ptr(dpos), B, L, D, float(scale), int(mask_pad_rows), float(p),
-                                         int(seed), ptr(seed_dev), stream_ptr(dx.device)))
+            check(lib.grb_embed_backward(ptr(ids), ptr(order), ptr(dx), ptr(dtable), ptr(dpos), B, L, D, float(scale), int(mask_pad_rows), float(p),
+                                         int(seed), ptr(seed_dev), ptr(scratch), stream_ptr(dx.device)))
         if ctx.sink is not None:
             return (None,) * 9
         return None, dtable, dpos, None, None, None, None, None, None
@@ -326,7 +312,7 @@ class HeadLossFn(torch.autograd.Function):
                                                      T, D, Cn, ptr(loss), ptr(dx), ptr(dtable), ptr(dg), ptr(db), ptr(ws),
                                                      stream_ptr(x.device)))
         if deferred:
-            _DEFER["keep"].append((ws, xc))                       # dlogits / xf are still read by the deferred dE GEMM
+            _DEFER["keep"].append((ws, xc, tg))                   # xf, the shifts and the targets are still read by the deferred dE pass
         ctx.grads = (dx, dg, db, dtable)
         return loss
 
@@ -381,7 +367,7 @@ def eval_rank_metrics(logits_last: torch.Tensor, targets: torch.Tensor, metrics:
 # ------------------------------------------------------------------------------------------------ attention core alone
 def hstu_attention_fwd(P: torch.Tensor, meta: SeqMeta, H: int, pos_table: torch.Tensor, time_table: Optional[torch.Tensor],
                        ntime: int = 64) -> torch.Tensor:
-    """P [B, L, 4D] bf16 = silu(x Wp^T + b) = [U | V | Q | K]  ->  O [B, L, D] bf16 (hstu.py:244-267); tcgen05 path."""
+    """P [B, L, 4D] bf16 = silu(x Wp^T + b) = [U | V | Q | K]  ->  O [B, L, D] bf16 (hstu.py:244-267)."""
     lib = _lib.load()
     require_cuda(P)
     B, L, D4 = P.shape
@@ -389,7 +375,7 @@ def hstu_attention_fwd(P: torch.Tensor, meta: SeqMeta, H: int, pos_table: torch.
     has_time = time_table is not None and meta.timestamps is not None
     dims = _dims(B, L, D, H, pos_table.shape[0], ntime if has_time else 0, 0.0, 0, None, 0)
     O = torch.empty(B, L, D, dtype=torch.bfloat16, device=P.device)
-    seq = meta.struct(tc=True)
+    seq = meta.struct()
     with torch.cuda.device(P.device):
         check(lib.grb_hstu_attention_forward(C.byref(dims), ptr(pos_table), ptr(time_table) if has_time else None, C.byref(seq), ptr(P), ptr(O),
                                              stream_ptr(P.device)))
@@ -407,7 +393,7 @@ def hstu_attention_bwd(P, zp, dO, meta: SeqMeta, H: int, pos_table, time_table, 
     dpos = torch.zeros_like(pos_table, dtype=torch.float32)
     dtime = torch.zeros_like(time_table, dtype=torch.float32) if has_time else None
     scratch = _u8(lib.grb_hstu_attention_scratch_bytes(C.byref(dims)), P.device)
-    seq = meta.struct(tc=True)
+    seq = meta.struct()
     with torch.cuda.device(P.device):
         check(lib.grb_hstu_attention_backward(C.byref(dims), ptr(pos_table), ptr(time_table) if has_time else None, C.byref(seq), ptr(P), ptr(zp),
                                               ptr(dO), ptr(dzp), ptr(dpos), ptr(dtime), ptr(scratch), stream_ptr(P.device)))
@@ -551,7 +537,7 @@ def split3(x: torch.Tensor, operand: int) -> torch.Tensor:
 
 
 def linear_f32x3(x_split: torch.Tensor, w_split: torch.Tensor, act: int = 0) -> torch.Tensor:
-    """y = act(x W^T) in fp32 accuracy on the tcgen05 path; x_split [T, 6K], w_split [N, 6K] from split3(); act 0 none, 1 silu."""
+    """y = act(x W^T) in fp32 accuracy on the tensor-core path; x_split [T, 6K], w_split [N, 6K] from split3(); act 0 none, 1 silu."""
     K6 = x_split.shape[-1]
     T, N = x_split.numel() // K6, w_split.shape[0]
     y = torch.empty(*x_split.shape[:-1], N, dtype=torch.float32, device=x_split.device)

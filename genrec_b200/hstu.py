@@ -1,4 +1,4 @@
-"""Drop-in mirror of ``genrec.models.hstu`` (reference: genrec/models/hstu.py) backed by the sm_100a C-ABI library.
+"""Drop-in mirror of ``genrec.models.hstu`` (reference: genrec/models/hstu.py) backed by the sm_90a C-ABI library.
 
 Same class names, constructor arguments, ``forward`` signatures, parameter names/shapes/init (SURVEY.md Appendix C),
 so the reference trainers, gin files and checkpoints work unchanged.  All arithmetic of the hot path runs in our CUDA

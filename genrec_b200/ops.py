@@ -25,8 +25,22 @@ from ._lib import HstuDims, HstuLayerGrads, HstuLayerParams, HstuSeq, check, ptr
 NS = "genrec_b200"
 
 
-def _seq(pad: Tensor, ts: Optional[Tensor], rel32: Optional[Tensor], wide: Optional[Tensor], thr: Tensor, pos_bucket0: int) -> HstuSeq:
-    return HstuSeq(None, 0, 1 if ts is not None else 0, 1, int(pos_bucket0), ptr(ts), ptr(pad), ptr(rel32), ptr(wide), ptr(thr))
+def _seq(pad: Tensor, ts: Optional[Tensor], rel32: Optional[Tensor], wide: Optional[Tensor], thr: Tensor, pos_bucket0: int,
+         ntime: int) -> HstuSeq:
+    """Sequence metadata with the [B, L, ld] bias-index matrix the attention kernels read (uniform position buckets: one
+    effective bucket).  The struct holds a reference to the index tensor, which lives as long as the struct."""
+    B, L = pad.shape
+    ld = (L + 7) // 8 * 8
+    index = torch.empty(B, L, ld, dtype=torch.int16, device=pad.device)
+    zero_pb = torch.zeros(L, dtype=torch.uint8, device=pad.device)
+    pad = pad.contiguous()
+    Fn._defer_for_call(False)   # built on the caller's stream: the kernels that read it and the tensor's lifetime follow that stream
+    with torch.cuda.device(pad.device):
+        check(_lib.load().grb_hstu_bias_index(ptr(ts), ptr(pad), ptr(thr), ptr(zero_pb), B, L, 1, ntime if ts is not None else 0, ptr(index), ld,
+                                              stream_ptr(pad.device)))
+    seq = HstuSeq(ptr(index), ld, 1 if ts is not None else 0, 1, int(pos_bucket0), ptr(ts), ptr(pad), ptr(rel32), ptr(wide), ptr(thr))
+    seq.index = index
+    return seq
 
 
 # ------------------------------------------------------------------------------------------------ sequence preparation
@@ -59,7 +73,7 @@ def hstu_attention(P: Tensor, pad: Tensor, timestamps: Optional[Tensor], rel32: 
     has_time = time_table is not None and timestamps is not None
     dims = HstuDims(B, L, D, num_heads, pos_table.shape[0], time_table.shape[0] if has_time else 0, 0.0, 0, None, 0)
     O = torch.empty(B, L, D, dtype=torch.bfloat16, device=P.device)
-    seq = _seq(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0)
+    seq = _seq(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0, dims.ntime)
     with torch.cuda.device(P.device):
         check(_lib.load().grb_hstu_attention_forward(C.byref(dims), ptr(pos_table), ptr(time_table) if has_time else None, C.byref(seq),
                                                      ptr(P.contiguous()), ptr(O), stream_ptr(P.device)))
@@ -86,7 +100,7 @@ def hstu_attention_backward(P: Tensor, zp: Tensor, dO: Tensor, pad: Tensor, time
     dpos = torch.zeros(pos_table.shape, dtype=torch.float32, device=P.device)
     dtime = torch.zeros(time_table.shape if time_table is not None else (0, num_heads), dtype=torch.float32, device=P.device)
     scratch = torch.empty(lib.grb_hstu_attention_scratch_bytes(C.byref(dims)), dtype=torch.uint8, device=P.device)
-    seq = _seq(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0)
+    seq = _seq(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0, dims.ntime)
     with torch.cuda.device(P.device):
         check(lib.grb_hstu_attention_backward(C.byref(dims), ptr(pos_table), ptr(time_table) if has_time else None, C.byref(seq),
                                               ptr(P.contiguous()), ptr(zp.contiguous()), ptr(dO.contiguous()), ptr(dzp), ptr(dpos),
@@ -113,7 +127,7 @@ def _layer_structs(x, pad, timestamps, rel32, wide, time_thr, params: List[Optio
     bw = dict(zip(("proj_w", "ffn1_w", "ffn2_w"), bf16w))
     ps = HstuLayerParams(*[ptr(bw[n]) if n in bw else (ptr(named[n]) if named[n] is not None and (n != "time_table" or has_time) else None)
                            for n in _PNAMES])
-    return dims, ps, _seq(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0), named, has_time
+    return dims, ps, _seq(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0, dims.ntime), named, has_time
 
 
 @custom_op(f"{NS}::hstu_layer", mutates_args=())

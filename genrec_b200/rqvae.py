@@ -2,7 +2,7 @@
 
 In scope (SURVEY.md section 8 rows a10/a11): ``Quantize.forward`` in eval mode (distance + first-min argmin + codebook
 gather + quantize loss, rqvae.py:185-199, :246-254) and the residual loop of ``RqVae.get_semantic_ids`` (:386-412), both
-executed by ONE launch of the sm_100a kernel ``rq_residual_argmin`` (csrc/rq_argmin.cuh) for all levels.
+executed by ONE launch of the sm_90a kernel ``rq_residual_argmin`` (csrc/rq_argmin.cuh) for all levels.
 Out of scope (raise): training-mode estimators (Gumbel / STE / rotation trick / Sinkhorn), k-means init, the decoder and
 the reconstruction losses.  The bias-free SiLU MLP encoder in front of the argmin (encoder.py:380-420, "next" row f3) runs
 on cuBLAS through ``torch.nn.functional.linear``.
@@ -72,7 +72,7 @@ class MLP(nn.Module):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         assert x.shape[-1] == self.input_dim, f"Invalid input dim: Expected {self.input_dim}, found {x.shape[-1]}"
         if x.is_cuda and not (torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters()))):
-            # inference (get_semantic_ids): every layer is one tcgen05 GEMM on three-term bf16 splits of both operands with the
+            # inference (get_semantic_ids): every layer is one wgmma GEMM on three-term bf16 splits of both operands with the
             # SiLU in its epilogue - fp32 accuracy (the semantic ids must not depend on a bf16 rounding of the latent)
             ws = self._split_weights()
             h = x.detach().float().contiguous()

@@ -1,8 +1,8 @@
-"""Drop-in mirror of ``genrec.models.sasrec`` (reference: genrec/models/sasrec.py) on the sm_100a C-ABI library.
+"""Drop-in mirror of ``genrec.models.sasrec`` (reference: genrec/models/sasrec.py) on the sm_90a C-ABI library.
 
 Same classes / constructor arguments / forward signatures / parameter names (SURVEY.md Appendix C).  The hot item of
 this model - the causal softmax attention core (sasrec.py:206-240) - runs in the flash-style CUDA kernels of
-csrc/attn_sasrec.cuh (forward + backward); the projections / FFN are the tcgen05 GEMMs with fused bias / ReLU / dropout /
+csrc/attn_sasrec.cuh (forward + backward); the projections / FFN are the wgmma GEMMs with fused bias / ReLU / dropout /
 residual / mask epilogues, LayerNorm and the embedding are our row kernels.  A handful of element-wise glue operations of
 the block's backward (mask multiply, one bf16+fp32 add) are plain torch ops on CUDA tensors.  CPU tensors raise.
 """

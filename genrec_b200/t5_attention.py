@@ -1,7 +1,7 @@
 """T5-style attention for TIGER (SURVEY.md section 8 row f4): drop-in mirror of ``genrec/modules/transformer.py:44-159``.
 
 Same constructor arguments, parameter names / shapes (``q``, ``kv`` | ``k`` + ``v``, ``o``, ``rel_bias``) and ``forward`` signature as
-the reference's ``T5Attention``; the q / k / v / o projections are the tcgen05 GEMMs of this library, the score / softmax / value core
+the reference's ``T5Attention``; the q / k / v / o projections are the wgmma GEMMs of this library, the score / softmax / value core
 is ``csrc/attn_t5.cuh`` (forward and backward), glued by one autograd function.  bf16 operands, fp32 accumulation, like the other
 modules of this package.  Supported masks: ``key_padding_mask`` [B, Lk] bool and ``attn_mask`` = None or the causal mask of
 ``nn.Transformer.generate_square_subsequent_mask`` (what genrec/models/tiger.py:203-206,306-309 passes); anything else raises.

@@ -1,4 +1,4 @@
-/* genrec_b200 - C ABI of the B200-native (sm_100a) hot path of phonism/genrec.
+/* genrec_b200 - C ABI of the H100-native (sm_90a) hot path of phonism/genrec.
  *
  * The reference is pure Python/PyTorch: it has no FFI of its own.  The interface each entry point below replaces is
  * therefore the body of the reference nn.Module method named in its comment (file:line under /root/reference); the
@@ -28,7 +28,7 @@ extern "C" {
 #define GRB_OK 0
 #define GRB_EINVAL (-1)   /* unsupported shape / null pointer / misaligned buffer */
 #define GRB_ECUDA (-2)    /* a CUDA launch or runtime call failed */
-#define GRB_ENODEV (-3)   /* no sm_100 device */
+#define GRB_ENODEV (-3)   /* no sm_90 device */
 
 const char* grb_last_error(void);
 int grb_version(void);
@@ -78,7 +78,7 @@ typedef struct {
     int pos_uniform;            /* 1 when every delta in [0, L) maps to the same position bucket (the reference's behaviour):
                                    a bias_index, if given, must then have been built with npos = 1 and an all-zero pos_bucket table */
     int pos_bucket0;            /* that bucket (row of the [npos, H] table that is live) */
-    /* tcgen05 attention path (the default): buckets and masks are derived inside the attention kernels from these */
+    /* per-sequence metadata: pad flags and timestamps (with their int32 rebasing for the bucket test hook) */
     const int64_t* timestamps;  /* [B, L] or NULL */
     const uint8_t* pad;         /* [B, L], 1 = input_ids == 0 */
     const int32_t* rel32;       /* [B, L] from grb_hstu_seq_prepare() (NULL when timestamps is NULL) */
@@ -87,11 +87,11 @@ typedef struct {
 } grb_hstu_seq;
 
 /* Per-sequence rebasing of the int64 timestamps (replaces nothing in the reference: it makes `ts[b,i] - ts[b,j]`
- * (hstu.py:400) a 32-bit subtraction inside the attention kernels): rel32[b,i] = ts[b,i] - min over non-padded positions;
+ * (hstu.py:400) a 32-bit subtraction in the in-kernel bucket routine): rel32[b,i] = ts[b,i] - min over non-padded positions;
  * wide[b] = 1 when the sequence spans >= 2^31 ticks, in which case the kernels use the int64 values themselves. */
 int grb_hstu_seq_prepare(const int64_t* timestamps, const uint8_t* pad, int B, int L, int32_t* rel32, uint8_t* wide, void* stream);
-/* Test hook: the time bucket / mask byte the tcgen05 attention kernels derive for every cell, [B, L, L] uint8
- * (bucket, or 64 when j > i or key j is padded), computed by the very device routine the kernels use. */
+/* Test hook: the time bucket / mask byte of every cell, [B, L, L] uint8 (bucket, or 64 when j > i or key j is padded), computed
+ * by the in-kernel bucket routine from the rebased timestamps. */
 int grb_hstu_bucket_bytes_debug(const grb_hstu_seq* s, int B, int L, int ntime, uint8_t* out, void* stream);
 /* The attention core alone (hstu.py:244-267) on the projection output P = [U | V | Q | K] ([T, 4D] bf16): O [T, D] bf16.
  * backward: dO [T, D] bf16, zp [T, 4D] the pre-activations of P -> dzp columns V, Q, K (gradients w.r.t. the pre-activations),
@@ -144,8 +144,10 @@ int grb_collate_jagged(const int64_t* items, const int64_t* stamps, const int64_
 int grb_embed_forward(const int64_t* ids, const float* table, const float* pos_table, float* x, uint8_t* pad,
                       int B, int L, int D, float scale, int mask_pad_rows, float dropout_p, uint64_t seed, const uint64_t* seed_dev,
                       void* stream);
-int grb_embed_backward(const int64_t* ids, const float* dx, float* dtable, float* dpos_table, int B, int L, int D,
-                       float scale, int mask_pad_rows, float dropout_p, uint64_t seed, const uint64_t* seed_dev,
+/* order: the B * L token indices sorted by id (stable); every table row is summed over its tokens in token order, in a fixed
+ * schedule (scratch: [B * L, D] fp32) - the gradient is the same from run to run */
+int grb_embed_backward(const int64_t* ids, const int64_t* order, const float* dx, float* dtable, float* dpos_table, int B, int L, int D,
+                       float scale, int mask_pad_rows, float dropout_p, uint64_t seed, const uint64_t* seed_dev, float* scratch,
                        void* stream);
 
 /* ------------------------------------------------------------------------------------------------ tied-embedding head
@@ -204,7 +206,7 @@ int grb_layernorm_backward(const float* dy, const float* x, const float* stats, 
 
 /* fp32-accurate linear layer on the bf16 tensor path (the RQ-VAE encoder MLP, genrec/modules/encoder.py:399-420: bias-free
  * Linear + SiLU).  Operands are split into three bf16 terms each and the six significant cross terms are laid out along K
- * (K' = 6 K), so one tcgen05 GEMM with fp32 accumulation reproduces the fp32 product to ~2^-22 relative.
+ * (K' = 6 K), so one wgmma GEMM with fp32 accumulation reproduces the fp32 product to ~2^-22 relative.
  *   grb_split3_f32_to_bf16: in [rows, K] fp32 -> out [rows, 6 K] bf16 ; operand 0 = activation (A) layout, 1 = weight (B) layout
  *   grb_linear_f32x3_forward: y [T, N] fp32 = act(x [T, K] @ W [N, K]^T), both operands pre-split ; act 0 none, 1 silu */
 int grb_split3_f32_to_bf16(const float* in, void* out_bf16, size_t rows, int K, int operand, void* stream);

@@ -72,12 +72,17 @@ def golden_hstu(name, V, D, H, blocks, B, L, seed, use_time=True, pass_ts=True):
     grads_ac = {n: (p.grad.clone() if p.grad is not None else torch.zeros_like(p)) for n, p in m.named_parameters()}
     m.eval()
     top = m.predict(ids, ts if pass_ts else None, top_k=10)
-    torch.save(dict(autocast=dict(loss=loss_ac.detach().float(), grads=grads_ac, logits_last=logits_ac.detach().float()[:, -1]),
-                    cfg=dict(num_items=V, embed_dim=D, num_heads=H, num_blocks=blocks, use_temporal_bias=use_time,
+    # the gradients and the autocast yardstick go to parts of their own (<stem>.grads.pt, <stem>.autocast.pt; tests/conftest.py
+    # merges them back) so that no fixture file exceeds 1 MB
+    stem = name[:-3]
+    torch.save(dict(loss=loss_ac.detach().float(), grads=grads_ac, logits_last=logits_ac.detach().float()[:, -1]),
+               os.path.join(OUT, stem + ".autocast.pt"))
+    torch.save(grads, os.path.join(OUT, stem + ".grads.pt"))
+    torch.save(dict(cfg=dict(num_items=V, embed_dim=D, num_heads=H, num_blocks=blocks, use_temporal_bias=use_time,
                              pass_ts=pass_ts),
                     state_dict={k: v.clone() for k, v in m.state_dict().items()},
                     input_ids=ids, timestamps=ts, targets=tg,
-                    logits=logits.detach(), loss=loss.detach(), grads=grads, top10=top),
+                    logits=logits.detach(), loss=loss.detach(), top10=top),
                os.path.join(OUT, name))
 
 
@@ -273,6 +278,21 @@ def golden_t5_attention(name, seed, D=64, H=2, B=3, Lq=37, Lk=21):
     torch.save(dict(cfg=dict(D=D, H=H), cases=cases), os.path.join(OUT, name))
 
 
+def golden_hstu_fp64(name):
+    """The unmodified reference model in fp64 (no dropout): inputs, parameters, logits and loss, for the oracle's fp64 check."""
+    R = ref_loader.ref_hstu()
+    torch.manual_seed(3)
+    m = R.HSTU(num_items=60, max_seq_len=40, embed_dim=64, num_heads=2, num_blocks=2, dropout=0.0).double()
+    B, L = 3, 37
+    ids = torch.randint(1, 61, (B, L)); ids[0, :11] = 0
+    ts = torch.cumsum(torch.randint(1, 10 ** 6, (B, L)), 1) + 1_300_000_000; ts[ids == 0] = 0
+    tg = torch.randint(1, 61, (B, L))
+    with torch.no_grad():
+        lo, ls = m(ids, ts, tg)
+    torch.save(dict(cfg=dict(num_heads=2, num_blocks=2), state_dict={k: v.detach().clone() for k, v in m.state_dict().items()},
+                    input_ids=ids, timestamps=ts, targets=tg, logits=lo.detach().clone(), loss=ls.detach().clone()), os.path.join(OUT, name))
+
+
 def main():
     assert ref_loader.available(), "reference tree not found"
     os.makedirs(OUT, exist_ok=True)
@@ -287,6 +307,7 @@ def main():
     golden_t5_attention("t5_attention.pt", seed=100)
     golden_tiger_decode("tiger_decode_trie.pt", seed=80)
     golden_tiger_decode("tiger_decode_notrie.pt", seed=90, use_trie=False)
+    golden_hstu_fp64("hstu_model_fp64.pt")
     for f in sorted(os.listdir(OUT)):
         print(f, os.path.getsize(os.path.join(OUT, f)))
 

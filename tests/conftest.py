@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (skipped on a machine without one)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -30,6 +30,12 @@ def golden():
     import torch
 
     def load(name):
-        return torch.load(os.path.join(GOLDEN, name), weights_only=False)
+        # a fixture may be stored in parts (every file stays under 1 MB): <stem>.<key>.pt holds entry <key> of <stem>.pt
+        g = torch.load(os.path.join(GOLDEN, name), weights_only=False)
+        stem = name[:-3]
+        for f in sorted(os.listdir(GOLDEN)):
+            if f.startswith(stem + ".") and f.endswith(".pt") and f != name:
+                g[f[len(stem) + 1:-3]] = torch.load(os.path.join(GOLDEN, f), weights_only=False)
+        return g
 
     return load

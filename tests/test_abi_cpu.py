@@ -44,7 +44,9 @@ def test_host_side_queries_and_errors(lib):
     bad = HstuDims(1, 8, 96, 3, 32, 64, 0.0, 0, None, 0)
     assert lib.grb_hstu_layer_saved_bytes(ctypes.byref(bad)) == 0
     assert b"unsupported" in lib.grb_last_error()
-    assert lib.grb_head_workspace_bytes(T, 128, 12102) >= T * 12104 * 2
+    # D = 256 stores the [T, C] logits (bf16 gradient + fp32 logits); D <= 128 runs the fused kernels, which never form them
+    assert lib.grb_head_workspace_bytes(T, 256, 12102) >= T * 12104 * (2 + 4)
+    assert 0 < lib.grb_head_workspace_bytes(T, 128, 12102) < T * 12104 * 2
 
 
 def test_product_never_imports_oracle():

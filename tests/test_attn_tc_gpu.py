@@ -1,6 +1,5 @@
-"""tcgen05 attention kernels (csrc/attn_tc.cuh) through the C ABI: bit-exact integer work (time buckets, masks) against the
-oracle, the attention core against a plain PyTorch fp32 restatement of the same op on the same bf16 operands, and against the
-first-generation mma.sync kernels."""
+"""HSTU attention through the C ABI: bit-exact integer work (time buckets, the bias-index matrix, masks) against the oracle, and
+the mma.sync attention core against a plain PyTorch fp32 restatement of the same op on the same bf16 operands."""
 import pytest
 import torch
 
@@ -150,42 +149,6 @@ def test_attention_core_vs_torch_fp32(B, L, D, H, with_ts):
     assert relerr(dpos[0], dpos_ref[0]) < 1e-2 and dpos[1:].abs().max() == 0, relerr(dpos[0], dpos_ref[0])
     if with_ts:
         assert relerr(dtime, dtime_ref) < 1e-2, relerr(dtime, dtime_ref)
-
-
-@pytest.mark.parametrize("B,L,D,H", [(3, 50, 64, 2), (4, 200, 128, 4), (2, 257, 256, 8), (2, 130, 128, 2)])
-def test_layer_tc_attention_matches_mma_attention(B, L, D, H, monkeypatch):
-    """The whole block forward + backward with the tcgen05 attention kernels vs the mma.sync ones (same operands, same math;
-    only the accumulation order differs)."""
-    from genrec_b200.hstu import HSTULayer
-    from tests.util import make_batch
-    dev = torch.device("cuda:0")
-    torch.manual_seed(L + D)
-    layer = HSTULayer(D, H, 0.0, 32, 64, 128, True).to(dev).train()
-    with torch.no_grad():
-        for n, p in layer.named_parameters():
-            if "attention_bias" in n:
-                p.normal_(0, 0.5)
-            elif n.endswith("bias"):
-                p.normal_(0, 0.1)
-            elif "norm" not in n:
-                p.normal_(0, 0.08)
-    ids, ts, _ = make_batch(max(B, 3), L, 50, seed=L)
-    ids, ts = ids[:B].to(dev), ts[:B].to(dev)
-    x = torch.randn(B, L, D, device=dev)
-    dy = torch.randn(B, L, D, device=dev)
-    res = []
-    for mode in ("tc", "mma"):
-        monkeypatch.setenv("GRB_ATTN", mode)      # (the default "auto" picks by sequence length)
-        layer.zero_grad(set_to_none=True)
-        xi = x.clone().requires_grad_(True)
-        y = layer(xi, None, ids == 0, ts)
-        y.backward(dy)
-        res.append((y.detach().clone(), xi.grad.clone(), {n: p.grad.clone() for n, p in layer.named_parameters()}))
-    (y0, dx0, g0), (y1, dx1, g1) = res
-    assert relerr(y0, y1) < 4e-3, relerr(y0, y1)
-    assert relerr(dx0, dx1) < 6e-3, relerr(dx0, dx1)
-    for n in g0:
-        assert relerr(g0[n], g1[n]) < 8e-3, (n, relerr(g0[n], g1[n]))
 
 
 def test_custom_op_block_equals_module_block():

@@ -1,9 +1,6 @@
 """Fused tied-embedding cross-entropy head (genrec/models/hstu.py:137-146) against a plain fp32 torch restatement of the same lines:
 loss, d loss / d x, the tied-table gradient and the final-LayerNorm gradients, over every D the kernels are compiled for, ragged token /
 class counts (partial tiles on both axes, a single class tile, class halves of unequal length) and ignored rows (target 0)."""
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -71,31 +68,9 @@ def test_head_all_rows_ignored_is_nan_like_the_reference():
     assert torch.isnan(got[0])                       # F.cross_entropy: 0 / 0 valid targets (hstu.py:141-146)
 
 
-def test_head_schedules_agree():
-    """GRB_CE=store keeps the G' tensor and the TN GEMM for dE (the only schedule at D = 256); GRB_CE=exact is the two-sweep kernel without
-    any [T, C] tensor; the default is the one-sweep kernel.  All three must agree at D = 128."""
-    code = (
-        "import torch, sys; sys.path.insert(0, %r)\n"
-        "from tests.test_head_gpu import _case, _ours\n"
-        "out = _ours(*_case(3, 90, 128, 2500, seed=9))\n"
-        "torch.save(out, sys.argv[1])\n" % os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    outs = []
-    for mode in ("store", "exact", ""):
-        path = f"/tmp/_head_{mode or 'default'}.pt"
-        env = dict(os.environ, GRB_CE=mode)
-        if not mode:
-            env.pop("GRB_CE")
-        subprocess.run([sys.executable, "-c", code, path], check=True, env=env, timeout=300)
-        outs.append(torch.load(path))
-    for other in outs[1:]:
-        assert abs(outs[0][0].item() - other[0].item()) < 1e-5
-        for a, b in zip(outs[0][1:], other[1:]):
-            assert relerr(a, b) < 1e-2, relerr(a, b)
-
-
 def test_head_wide_logit_range():
-    """Logits spread over +-60 nats, the target far from the row maximum for most rows: the one-sweep kernel's shift (probe tile / target
-    logit) sits well below the true maximum and the result must still be the exact softmax."""
+    """Logits spread over +-60 nats, the target far from the row maximum for most rows and the largest logits far from the first class
+    tiles: the online row maximum of the fused kernel must still give the exact softmax."""
     g = torch.Generator().manual_seed(4)
     x, ln_g, ln_b, table, tg = _case(3, 70, 128, 3000, seed=21)
     table = table * 3.0                                   # |logit| up to ~ 60
@@ -119,24 +94,10 @@ def _overflow_case():
     return x, ln_g, ln_b, table, tg
 
 
-def test_one_sweep_range_limit_is_loud_and_exact_mode_has_none():
-    """DESIGN 3.3: the one-sweep kernel's exponent shift is max(probe tile, target logit); a class beating both by more than ~98 nats
-    overflows that row - the loss comes out non-finite, never silently wrong - and GRB_CE=exact computes the same case exactly."""
-    code = (
-        "import torch, sys; sys.path.insert(0, %r)\n"
-        "from tests.test_head_gpu import _overflow_case, _ours\n"
-        "out = _ours(*_overflow_case())\n"
-        "torch.save(out, sys.argv[1])\n" % os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    res = {}
-    for mode in ("", "exact"):
-        path = f"/tmp/_head_overflow_{mode or 'default'}.pt"
-        env = dict(os.environ, GRB_CE=mode)
-        if not mode:
-            env.pop("GRB_CE")
-        subprocess.run([sys.executable, "-c", code, path], check=True, env=env, timeout=300)
-        res[mode] = torch.load(path)
-    assert not torch.isfinite(res[""][0])                            # loud
+def test_head_overflow_case_is_exact():
+    """A class beating the target and every other logit of its row by ~190 nats: the softmax is shifted by the exact row maximum,
+    so the loss and the gradients stay finite and match the reference."""
     ref = _reference(*_overflow_case())
-    got = res["exact"]
+    got = _ours(*_overflow_case())
     assert torch.isfinite(got[0]) and abs(got[0].item() - ref[0].item()) < 2e-3 * abs(ref[0].item())
     assert relerr(got[1], ref[1]) < 3e-2 and relerr(got[4], ref[4]) < 3e-2

@@ -92,7 +92,7 @@ def test_rq_kernel_generations_are_bit_identical(N, D, levels, monkeypatch):
 
 
 def test_rq_encoder_fp32_accurate_tensor_path(golden):
-    """RqVae.encode at inference = five tcgen05 GEMMs on three-term bf16 splits (SiLU in the epilogue): fp32 accuracy against the
+    """RqVae.encode at inference = five wgmma GEMMs on three-term bf16 splits (SiLU in the epilogue): fp32 accuracy against the
     oracle's fp32 MLP, and the semantic ids of the reference golden end to end."""
     from genrec_b200.rqvae import RqVae
     from oracle import rqvae as orq

@@ -1,4 +1,4 @@
-"""T5-style attention for TIGER (csrc/attn_t5.cuh + the tcgen05 projections) against the golden outputs / gradients of the UNMODIFIED
+"""T5-style attention for TIGER (csrc/attn_t5.cuh + the wgmma projections) against the golden outputs / gradients of the UNMODIFIED
 reference module (tests/golden/t5_attention.pt) and, for the attention core alone, against plain fp32 torch on the same bf16-rounded
 operands.  Tolerances: bf16 operand level for the module (the reference fixture is fp32), 4e-3 for the core's bf16 outputs, 2e-3 for
 its fp32 outputs."""

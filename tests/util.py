@@ -2,7 +2,7 @@ import torch
 
 
 def relerr(a: torch.Tensor, ref: torch.Tensor) -> float:
-    """max-norm relative error: |a - ref|_inf / |ref|_inf (SURVEY.md section 7 'autocast semantics')."""
+    """max-norm relative error: |a - ref|_inf / |ref|_inf (the reference's autocast semantics: SURVEY.md Appendix B)."""
     a, ref = a.detach().float().cpu(), ref.detach().float().cpu()
     d = ref.abs().max().item()
     return ((a - ref).abs().max().item() / d) if d > 0 else (a - ref).abs().max().item()
