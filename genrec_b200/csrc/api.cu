@@ -18,7 +18,6 @@
 #include "common.cuh"
 #include "dp_adam.cuh"
 #include "exact_f32.cuh"
-#include "gemm.cuh"
 #include "rowwise.cuh"
 #include "rq_argmin.cuh"
 #include "tc_gemm.cuh"
@@ -114,25 +113,9 @@ int det_finish(const float* part, int ngroups, int nmembers, int W, int gpo, int
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
-int splitk_for(int M, int N, int K) {
-    int tiles = ((M + GEMM_BM - 1) / GEMM_BM) * ((N + GEMM_BN - 1) / GEMM_BN);
-    int want = (2 * sm_count() + tiles - 1) / tiles;
-    int kt = (K + GEMM_BK - 1) / GEMM_BK;
-    int maxs = kt / 4 > 0 ? kt / 4 : 1;  // at least 4 k-tiles per split
-    return want < 1 ? 1 : (want > maxs ? maxs : want);
-}
 
-
-// ---- GEMM dispatch: wgmma/TMA path (default) or the first-generation mma.sync path (GRB_GEMM=mma, kept as an on-device
-//      cross-check).  Operand majors: *_MN = 0 -> K contiguous, 1 -> M/N contiguous (see tc_gemm.cuh / gemm.cuh).
-bool use_tc() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("GRB_GEMM");
-        v = (e && strcmp(e, "mma") == 0) ? 0 : 1;
-    }
-    return v == 1;
-}
+// ---- GEMMs: the wgmma/TMA kernel of tc_gemm.cuh with a fused epilogue.  Operand majors: *_MN = 0 -> K contiguous,
+//      1 -> M/N contiguous.
 int tn_splits(int M, int N, int K) {
     int tiles = ((M + TC_BM - 1) / TC_BM) * ((N + TC_BN - 1) / TC_BN);
     int want = (sm_count() + tiles - 1) / tiles;
@@ -143,50 +126,29 @@ int tn_splits(int M, int N, int K) {
 // z = x W^T + b ; act: 0 none, 1 silu, 2 relu   (NT)
 cudaError_t gemm_bias_act(int act, const bf16* x, const bf16* w, const float* bias, bf16* z, bf16* a, int M, int N, int K, const Dropout& drop,
                           cudaStream_t st) {
-    if (use_tc()) {
-        if (act == 0) return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasAct<0>{bias, N, drop}, z, nullptr, N, sm_count(), st);
-        if (act == 1) return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasAct<1>{bias, N, drop}, z, a, N, sm_count(), st);
-        return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasAct<2>{bias, N, drop}, z, a, N, sm_count(), st);
-    }
-    if (act == 0) return launch_gemm<0, 0>(x, w, M, N, K, K, K, 1, EpiBiasBf16{bias, z, N}, st);
-    if (act == 1) return launch_gemm<0, 0>(x, w, M, N, K, K, K, 1, EpiBiasSilu{bias, z, a, N, drop}, st);
-    return launch_gemm<0, 0>(x, w, M, N, K, K, K, 1, EpiBiasRelu{bias, z, a, N, drop}, st);
+    if (act == 0) return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasAct<0>{bias, N, drop}, z, nullptr, N, sm_count(), st);
+    if (act == 1) return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasAct<1>{bias, N, drop}, z, a, N, sm_count(), st);
+    return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasAct<2>{bias, N, drop}, z, a, N, sm_count(), st);
 }
 // y = res + drop(x W^T + b) (* row_scale)   (NT)
 cudaError_t gemm_bias_res(const bf16* x, const bf16* w, const float* bias, const float* res, const float* row_scale, float* y, int M, int N,
                           int K, const Dropout& drop, cudaStream_t st) {
-    if (use_tc()) return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasResidual{bias, res, row_scale, N, drop}, y, nullptr, N, sm_count(), st);
-    return launch_gemm<0, 0>(x, w, M, N, K, K, K, 1, EpiBiasResidual{bias, res, y, row_scale, N, drop}, st);
+    return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasResidual{bias, res, row_scale, N, drop}, y, nullptr, N, sm_count(), st);
 }
 // g[M,N] = dropmask(dy[M,K] W[K,N]) * act'(z)   (NN) ; act 1 silu, 2 relu
 cudaError_t gemm_dact(int act, const bf16* dy, const bf16* w, const bf16* z, bf16* g, int M, int N, int K, const Dropout& drop, cudaStream_t st) {
-    if (use_tc()) {
-        if (act == 1) return launch_tc_gemm<0, 1>(dy, w, M, N, K, K, N, 1, TcEpiDAct<1>{z, N, drop}, g, nullptr, N, sm_count(), st);
-        return launch_tc_gemm<0, 1>(dy, w, M, N, K, K, N, 1, TcEpiDAct<2>{z, N, drop}, g, nullptr, N, sm_count(), st);
-    }
-    if (act == 1) return launch_gemm<0, 1>(dy, w, M, N, K, K, N, 1, EpiDAct<0>{z, g, N, drop}, st);
-    return launch_gemm<0, 1>(dy, w, M, N, K, K, N, 1, EpiDAct<1>{z, g, N, drop}, st);
+    if (act == 1) return launch_tc_gemm<0, 1>(dy, w, M, N, K, K, N, 1, TcEpiDAct<1>{z, N, drop}, g, nullptr, N, sm_count(), st);
+    return launch_tc_gemm<0, 1>(dy, w, M, N, K, K, N, 1, TcEpiDAct<2>{z, N, drop}, g, nullptr, N, sm_count(), st);
 }
 // out[M,N] fp32 = scale * A[M,K] B[K,N] (+ res)   (NN)
 cudaError_t gemm_nn_f32(const bf16* A, const bf16* B, float* out, const float* res, float scale, int M, int N, int K, int lda, int ldb,
                         cudaStream_t st) {
-    if (use_tc()) return launch_tc_gemm<0, 1>(A, B, M, N, K, lda, ldb, 1, TcEpiF32{res, N, scale}, out, nullptr, N, sm_count(), st);
-    return launch_gemm<0, 1>(A, B, M, N, K, lda, ldb, 1, EpiF32{out, res, N, scale}, st);
+    return launch_tc_gemm<0, 1>(A, B, M, N, K, lda, ldb, 1, TcEpiF32{res, N, scale}, out, nullptr, N, sm_count(), st);
 }
-// out[M,N] fp32 += A^T B with A stored [K,M], B stored [K,N]   (TN, split-K, atomics)
+// out[M,N] fp32 += A^T B with A stored [K,M], B stored [K,N]   (TN, split-K, float atomics: the summation order varies from run to
+// run).  Only grb_linear_backward uses it, because its ABI has no workspace for the ordered split-K sum of launch_tc_tn_group.
 cudaError_t gemm_tn_atomic(const bf16* A, const bf16* B, float* out, int M, int N, int K, int lda, int ldb, cudaStream_t st) {
-    if (use_tc()) return launch_tc_gemm<1, 1>(A, B, M, N, K, lda, ldb, tn_splits(M, N, K), TcEpiAtomicF32{out, N, 1.f}, nullptr, nullptr, 0, sm_count(), st);
-    return launch_gemm<1, 1>(A, B, M, N, K, lda, ldb, splitk_for(M, N, K), EpiAtomicF32{out, N, 1.f}, st);
-}
-// out[M,N] fp32 (leading dim ldo, a multiple of 4) = A[M,K] B[N,K]^T   (NT)
-cudaError_t gemm_nt_f32(const bf16* A, const bf16* B, float* out, int ldo, int M, int N, int K, cudaStream_t st) {
-    if (use_tc()) return launch_tc_gemm<0, 0>(A, B, M, N, K, K, K, 1, TcEpiF32{nullptr, ldo, 1.f}, out, nullptr, ldo, sm_count(), st);
-    return launch_gemm<0, 0>(A, B, M, N, K, K, K, 1, EpiF32Scalar{out, ldo, N}, st);
-}
-// out[M,N] fp32 (leading dim N, any parity) = A B^T   (NT)
-cudaError_t gemm_nt_f32_plain(const bf16* A, const bf16* B, float* out, int M, int N, int K, cudaStream_t st) {
-    if (use_tc()) return launch_tc_gemm<0, 0>(A, B, M, N, K, K, K, 1, TcEpiF32Plain{out, N}, nullptr, nullptr, 0, sm_count(), st);
-    return launch_gemm<0, 0>(A, B, M, N, K, K, K, 1, EpiF32Scalar{out, N, N}, st);
+    return launch_tc_gemm<1, 1>(A, B, M, N, K, lda, ldb, tn_splits(M, N, K), TcEpiAtomicF32{out, N, 1.f}, nullptr, nullptr, 0, sm_count(), st);
 }
 
 // ---- carved layouts ------------------------------------------------------------------------------------------
@@ -280,25 +242,33 @@ int set_smem(Kern k, size_t bytes) {
     return 0;
 }
 
-HstuAttnArgs make_attn_args(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const LayerSaved& sv) {
+HstuBiasArgs make_attn_bias(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s) {
+    HstuBiasArgs b;
+    memset(&b, 0, sizeof(b));
+    // uniform position buckets (the reference's behaviour) collapse to ONE effective bucket: the index matrix was built with
+    // npos = 1, the tables shrink to 65 entries and the pointers are offset to the single live row of the [npos, H] table
+    b.wpos = pos_table + (s->pos_uniform ? (size_t)s->pos_bucket0 * d->H : 0);
+    const bool has_time = time_table != nullptr && s->has_time && d->ntime > 0;
+    b.wtime = has_time ? time_table : nullptr;
+    b.bias_index = s->bias_index;
+    b.ldix = s->ld_index;
+    b.pos_uniform = s->pos_uniform;
+    b.pos_bucket0 = 0;
+    b.npos = s->pos_uniform ? 1 : d->npos;
+    b.ntime = has_time ? d->ntime : 0;
+    return b;
+}
+// P: [T, 4D] bf16 U | V | Q | K ; O: [T, D] bf16 output, written by the forward only
+HstuAttnArgs make_attn_args(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s, const bf16* P,
+                            bf16* O) {
     HstuAttnArgs a;
     memset(&a, 0, sizeof(a));
     const int D = d->D;
-    a.q = sv.P + 2 * D; a.k = sv.P + 3 * D; a.v = sv.P + D;
+    a.q = P + 2 * D; a.k = P + 3 * D; a.v = P + D;
     a.ldq = a.ldk = a.ldv = 4 * D;
     a.B = d->B; a.L = d->L; a.H = d->H;
-    // uniform position buckets (the reference's behaviour) collapse to ONE effective bucket: the index matrix was built with
-    // npos = 1, the tables shrink to 65 entries and the pointers are offset to the single live row of the [npos, H] table
-    a.bias.wpos = p->pos_table + (s->pos_uniform ? (size_t)s->pos_bucket0 * d->H : 0);
-    const bool has_time = p->time_table != nullptr && s->has_time && d->ntime > 0;
-    a.bias.wtime = has_time ? p->time_table : nullptr;
-    a.bias.bias_index = s->bias_index;
-    a.bias.ldix = s->ld_index;
-    a.bias.pos_uniform = s->pos_uniform;
-    a.bias.pos_bucket0 = 0;
-    a.bias.npos = s->pos_uniform ? 1 : d->npos;
-    a.bias.ntime = has_time ? d->ntime : 0;
-    a.o = sv.O; a.ldo = D;
+    a.bias = make_attn_bias(d, pos_table, time_table, s);
+    a.o = O; a.ldo = D;
     return a;
 }
 
@@ -311,77 +281,63 @@ int launch_hstu_attn_fwd(const HstuAttnArgs& a, cudaStream_t st) {
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
-// Fork/join helper: dQ and dK/dV are independent, both latency-bound at low occupancy -> run them concurrently (the side
-// stream and the events are created on first use, i.e. during warm-up, never while a CUDA graph is being captured).
+// Fork/join helper: a non-blocking stream and its two events, created on first use, i.e. during warm-up, never while a CUDA graph
+// is being captured.  Event fork / join also pulls the side stream into a capture.
 struct SideStream {
     cudaStream_t s = nullptr;
     cudaEvent_t fork = nullptr, join = nullptr;
-    bool ok = false;
-    bool init() {
-        if (ok) return true;
-        if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) return false;
-        if (cudaEventCreateWithFlags(&fork, cudaEventDisableTiming) != cudaSuccess) return false;
-        if (cudaEventCreateWithFlags(&join, cudaEventDisableTiming) != cudaSuccess) return false;
-        ok = true;
-        return true;
+    bool ok = false, pending = false;
+    // run `launch(s)` after everything enqueued on `st` so far; returns 0 / error code
+    template <class F>
+    int run(cudaStream_t st, F&& launch) {
+        if (!ok) {
+            GRB_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+            GRB_CUDA(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
+            GRB_CUDA(cudaEventCreateWithFlags(&join, cudaEventDisableTiming));
+            ok = true;
+        }
+        GRB_CUDA(cudaEventRecord(fork, st));
+        GRB_CUDA(cudaStreamWaitEvent(s, fork, 0));
+        GRB_TRY(launch(s));
+        GRB_CUDA(cudaEventRecord(join, s));
+        pending = true;
+        return 0;
+    }
+    // make `st` wait for everything run() has enqueued since the last join
+    int join_into(cudaStream_t st) {
+        if (pending) {
+            GRB_CUDA(cudaStreamWaitEvent(st, join, 0));
+            pending = false;
+        }
+        return 0;
     }
 };
-SideStream& side_stream() {
-    static thread_local SideStream ss;   // the backward runs on the autograd thread: one side stream per calling thread
-    return ss;
+// dQ and dK/dV are independent, both latency-bound at low occupancy: dQ runs on this stream beside dK/dV.  Not the deferred
+// stream, where dQ would queue behind the weight-gradient GEMMs.  The backward runs on the autograd thread: one instance per
+// calling thread and device.
+SideStream& attn_side_stream() {
+    static thread_local SideStream ss[64];
+    return ss[current_device() & 63];
 }
 // ---- deferred weight gradients.  dW / dE GEMMs are not on the critical path of a training step: nothing reads them before the
 // optimizer.  With grb_set_defer_weight_grads(1) they go to a per-device side stream, forked where their operands are ready and
 // joined by grb_join_deferred() (FlatAdam.step calls it), so they fill the SM tails of the epilogue-bound GEMMs and run next to the
 // issue-bound attention kernels; the 620 MB dlogits stream of the head's dE GEMM overlaps the last block's backward.  The CALLER keeps
-// the operand buffers (layer workspace, saved blob, head workspace) alive until the join.  Works under CUDA-graph capture (event
-// fork / join pulls the side stream into the capture).
-struct DeferStream {
-    cudaStream_t s = nullptr;
-    cudaEvent_t fork = nullptr, join = nullptr;
-    bool ok = false, pending = false;
-};
+// the operand buffers (layer workspace, saved blob, head workspace) alive until the join.
 std::mutex g_defer_mu;
 bool g_defer_on = false;
-DeferStream& defer_stream() {
-    static DeferStream ds[64];
+SideStream& defer_stream() {
+    static SideStream ds[64];
     return ds[current_device() & 63];
 }
-// run `launch(side_stream)` after everything enqueued on `st` so far; returns 0 / error code
 template <class F>
 int defer_run(cudaStream_t st, F&& launch) {
     std::lock_guard<std::mutex> lock(g_defer_mu);
-    DeferStream& d = defer_stream();
-    if (!d.ok) {
-        GRB_CUDA(cudaStreamCreateWithFlags(&d.s, cudaStreamNonBlocking));
-        GRB_CUDA(cudaEventCreateWithFlags(&d.fork, cudaEventDisableTiming));
-        GRB_CUDA(cudaEventCreateWithFlags(&d.join, cudaEventDisableTiming));
-        d.ok = true;
-    }
-    GRB_CUDA(cudaEventRecord(d.fork, st));
-    GRB_CUDA(cudaStreamWaitEvent(d.s, d.fork, 0));
-    GRB_TRY(launch(d.s));
-    GRB_CUDA(cudaEventRecord(d.join, d.s));
-    d.pending = true;
-    return 0;
+    return defer_stream().run(st, launch);
 }
 int join_pending(cudaStream_t st) {
     std::lock_guard<std::mutex> lock(g_defer_mu);
-    DeferStream& d = defer_stream();
-    if (d.ok && d.pending) {
-        GRB_CUDA(cudaStreamWaitEvent(st, d.join, 0));
-        d.pending = false;
-    }
-    return 0;
-}
-bool use_side_stream() {
-    static int v = -1;
-    if (v < 0) {
-        // dQ and dK/dV side by side (the two backward kernels are independent); GRB_SIDE_STREAM=0 serialises them
-        const char* e = getenv("GRB_SIDE_STREAM");
-        v = (e && strcmp(e, "0") == 0) ? 0 : 1;
-    }
-    return v == 1;
+    return defer_stream().join_into(st);
 }
 
 template <int DH>
@@ -390,18 +346,12 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
     size_t posb = align_up((size_t)(a.bias.npos * 64 + 1) * 4, 16);  // combined bias table
     size_t smem_q = sizeof(AttSmem<DH>) + posb;
     GRB_TRY(set_smem(hstu_attn_bwd_dq_kernel<DH>, smem_q));
-    SideStream& ss = side_stream();
-    const bool forked = use_side_stream() && ss.init();
-    if (forked) {
-        GRB_CUDA(cudaEventRecord(ss.fork, st));
-        GRB_CUDA(cudaStreamWaitEvent(ss.s, ss.fork, 0));
-        launch_k(hstu_attn_bwd_dq_kernel<DH>, grid, ATT_THREADS, smem_q, ss.s, a);
+    SideStream& ss = attn_side_stream();
+    GRB_TRY(ss.run(st, [&](cudaStream_t side) -> int {
+        launch_k(hstu_attn_bwd_dq_kernel<DH>, grid, ATT_THREADS, smem_q, side, a);
         GRB_CUDA(cudaGetLastError());
-        GRB_CUDA(cudaEventRecord(ss.join, ss.s));
-    } else {
-        launch_k(hstu_attn_bwd_dq_kernel<DH>, grid, ATT_THREADS, smem_q, st, a);
-        GRB_CUDA(cudaGetLastError());
-    }
+        return 0;
+    }));
     size_t smem_k = sizeof(AttSmemKV<DH>) + posb + (size_t)4 * (a.bias.ntime + 1 + (a.bias.pos_uniform ? 0 : a.bias.npos + 1)) * 32 * sizeof(float);
     const bool has_time = a.bias.wtime != nullptr && a.bias.ntime > 0, pos_uni = a.bias.pos_uniform != 0;
     const int nmem = (int)(grid.x * grid.z), ngroups = has_time && a.dwtime ? 2 * a.H : a.H;
@@ -415,15 +365,13 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
     else if (has_time) GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, true, false>));
     else if (pos_uni) GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, false, true>));
     else GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, false, false>));
-    if (a.dw_part) {
-        // groups h < H: position buckets of head h ; H + h: time buckets of head h ; element = bucket
-        float* pos_out = a.dwpos + (pos_uni ? (size_t)a.bias.pos_bucket0 * a.H : 0);
-        const int pos_len = pos_uni ? a.H : a.bias.npos * a.H;
-        if (ngroups > a.H) GRB_TRY(det_finish(a.dw_part, ngroups, nmem, 64, a.H, 1, a.H, {{pos_out, pos_len}, {a.dwtime, a.bias.ntime * a.H}}, st));
-        else GRB_TRY(det_finish(a.dw_part, ngroups, nmem, 64, a.H, 1, a.H, {{pos_out, pos_len}}, st));
-    }
+    // groups h < H: position buckets of head h ; H + h: time buckets of head h ; element = bucket
+    float* pos_out = a.dwpos + (pos_uni ? (size_t)a.bias.pos_bucket0 * a.H : 0);
+    const int pos_len = pos_uni ? a.H : a.bias.npos * a.H;
+    if (ngroups > a.H) GRB_TRY(det_finish(a.dw_part, ngroups, nmem, 64, a.H, 1, a.H, {{pos_out, pos_len}, {a.dwtime, a.bias.ntime * a.H}}, st));
+    else GRB_TRY(det_finish(a.dw_part, ngroups, nmem, 64, a.H, 1, a.H, {{pos_out, pos_len}}, st));
     GRB_CUDA(cudaGetLastError());
-    if (forked) GRB_CUDA(cudaStreamWaitEvent(st, ss.join, 0));
+    GRB_TRY(ss.join_into(st));
     return 0;
 }
 
@@ -464,13 +412,13 @@ int cast_bf16(const float* in, bf16* out, size_t n, int D, const Dropout& drop, 
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
-// part (nullable): cast_colsum_grid(T, D).x * .y * 128 floats of scratch for the ordered sum; without it one atomic add per CTA
+// part: cast_colsum_grid(T, D).x * .y * 128 floats of scratch for the ordered sum
 int cast_colsum(const float* in, bf16* out, int T, int D, const Dropout& drop, float* colsum_out, float* part, cudaStream_t st) {
     GRB_REQUIRE(D > 0 && D % 4 == 0, "cast needs rows of a multiple-of-4 length D");
     const dim3 grid = cast_colsum_grid(T, D);
-    launch_k(cast_colsum_f32_bf16_kernel, grid, 256, 0, st, in, out, T, D, drop, colsum_out, part);
+    launch_k(cast_colsum_f32_bf16_kernel, grid, 256, 0, st, in, out, T, D, drop, part);
     GRB_CUDA(cudaGetLastError());
-    if (part) GRB_TRY(det_finish(part, grid.x, grid.y, 128, grid.x, 128, 1, {{colsum_out, D}}, st));
+    GRB_TRY(det_finish(part, grid.x, grid.y, 128, grid.x, 128, 1, {{colsum_out, D}}, st));
     return 0;
 }
 // part (nullable): colsum_grid(T, N).x * .y * 256 floats of scratch for the ordered sum; without it one atomic add per CTA
@@ -536,7 +484,7 @@ int grb_hstu_layer_forward(const grb_hstu_dims* d, const grb_hstu_layer_params* 
     // 3. O = silu(Q K^T + bias) V, causal + key padding                                      (hstu.py:244-267)
     GRB_TRY(join_pending(st));   // a bias-index matrix built on the side stream (deferred schedule) must be complete
     {
-        HstuAttnArgs a = make_attn_args(d, p, s, sv);
+        HstuAttnArgs a = make_attn_args(d, p->pos_table, p->time_table, s, sv.P, sv.O);
         if (D / d->H == 32) GRB_TRY(launch_hstu_attn_fwd<32>(a, st));
         else GRB_TRY(launch_hstu_attn_fwd<64>(a, st));
     }
@@ -578,22 +526,16 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
     // FFN second linear
     GRB_TRY(cast_colsum(dy, w.dyb, T, D, drop_out, g->ffn2_b, w.part_cast, st));   // dyb = bf16(dropmask(dy)) ; db2 += column sums
     {
-        if (!use_tc()) GRB_CUDA(gemm_tn_atomic(w.dyb, sv.hact, g->ffn2_w, D, 4 * D, T, D, 4 * D, st));  // dW2[D,4D] += dyb^T h
-    }
-    {
         GRB_CUDA(gemm_dact(1, w.dyb, (const bf16*)p->ffn2_w, sv.z1, w.dz1, T, 4 * D, D, drop_hid, st));  // dz1 = dropmask(dyb W2) * silu'(z1)
     }
     // FFN first linear
     // bias gradients are off the critical path too: with deferred weight gradients the column sums run beside the main chain
     auto colsum_maybe_deferred = [&](const bf16* in, float* out) -> int {
-        if (use_tc() && g_defer_on)
+        if (g_defer_on)
             return defer_run(st, [&](cudaStream_t side) -> int { return colsum(in, T, 4 * D, 4 * D, out, w.part_colsum, side); });
         return colsum(in, T, 4 * D, 4 * D, out, w.part_colsum, st);
     };
     GRB_TRY(colsum_maybe_deferred(w.dz1, g->ffn1_b));
-    {
-        if (!use_tc()) GRB_CUDA(gemm_tn_atomic(w.dz1, sv.xn, g->ffn1_w, 4 * D, D, T, 4 * D, D, st));  // dW1[4D,D] += dz1^T xn
-    }
     {
         GRB_CUDA(gemm_nn_f32(w.dz1, (const bf16*)p->ffn1_w, w.dxn, nullptr, 1.f, T, D, 4 * D, 4 * D, D, st));  // dxn = dz1 W1
     }
@@ -607,7 +549,7 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
     // attention backward -> gradients w.r.t. the V, Q, K pre-activations
     {
         GRB_REQUIRE(s->bias_index, "null sequence metadata: the attention kernels need bias_index");
-        HstuAttnArgs a = make_attn_args(d, p, s, sv);
+        HstuAttnArgs a = make_attn_args(d, p->pos_table, p->time_table, s, sv.P, sv.O);
         a.d_o = w.dO; a.lddo = D;
         a.zq = sv.zp + 2 * D; a.zk = sv.zp + 3 * D; a.zv = sv.zp + D; a.ldz = 4 * D;
         a.dq = w.dzp + 2 * D; a.dk = w.dzp + 3 * D; a.dv = w.dzp + D; a.lddq = 4 * D;
@@ -621,23 +563,18 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
     // projection
     GRB_TRY(colsum_maybe_deferred(w.dzp, g->proj_b));
     {
-        if (!use_tc()) GRB_CUDA(gemm_tn_atomic(w.dzp, sv.xb, g->proj_w, 4 * D, D, T, 4 * D, D, st));  // dWp[4D,D] += dzp^T xb
-    }
-    {
         GRB_CUDA(gemm_nn_f32(w.dzp, (const bf16*)p->proj_w, dx, w.dx1, 1.f, T, D, 4 * D, 4 * D, D, st));  // dx = dx1 + dzp Wp
     }
-    if (use_tc()) {
-        // the three weight gradients of the layer in ONE grouped launch: dW2 += dyb^T h, dW1 += dz1^T xn, dWp += dzp^T xb
-        TnSpec specs[3];
-        layer_tn_specs(specs, w.dyb, sv.hact, w.dz1, sv.xn, w.dzp, sv.xb, g->ffn2_w, g->ffn1_w, g->proj_w, T, D);
-        if (g_defer_on) {
-            GRB_TRY(defer_run(st, [&](cudaStream_t side) -> int {
-                GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, side));
-                return 0;
-            }));
-        } else {
-            GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, st));
-        }
+    // the three weight gradients of the layer in ONE grouped launch: dW2 += dyb^T h, dW1 += dz1^T xn, dWp += dzp^T xb
+    TnSpec specs[3];
+    layer_tn_specs(specs, w.dyb, sv.hact, w.dz1, sv.xn, w.dzp, sv.xb, g->ffn2_w, g->ffn1_w, g->proj_w, T, D);
+    if (g_defer_on) {
+        GRB_TRY(defer_run(st, [&](cudaStream_t side) -> int {
+            GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, side));
+            return 0;
+        }));
+    } else {
+        GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, st));
     }
     (void)nodrop;
     return 0;
@@ -700,18 +637,6 @@ size_t grb_hstu_attention_scratch_bytes(const grb_hstu_dims* d) {
     if (check_dims(d)) return 0;
     return align_up(attn_dw_part_floats(d->B, d->L, d->H) * sizeof(float));   // the bias-table gradient partials
 }
-namespace {
-HstuAttnArgs make_attn_args_p(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s, const bf16* P) {
-    grb_hstu_layer_params p;
-    memset(&p, 0, sizeof(p));
-    p.pos_table = pos_table;
-    p.time_table = time_table;
-    LayerSaved sv;
-    memset(&sv, 0, sizeof(sv));
-    sv.P = const_cast<bf16*>(P);
-    return make_attn_args(d, &p, s, sv);
-}
-}  // namespace
 
 int grb_hstu_attention_forward(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s,
                                const void* P_bf16, void* O_bf16, void* stream) {
@@ -720,8 +645,7 @@ int grb_hstu_attention_forward(const grb_hstu_dims* d, const float* pos_table, c
     GRB_REQUIRE(s->bias_index && s->ld_index >= d->L && s->ld_index % 8 == 0 && aligned16(s->bias_index),
                 "the attention kernels need bias_index (pitch a multiple of 8 and >= L)");
     GRB_REQUIRE(aligned16(P_bf16) && aligned16(O_bf16), "buffers must be 16-byte aligned");
-    HstuAttnArgs a = make_attn_args_p(d, pos_table, time_table, s, (const bf16*)P_bf16);
-    a.o = (bf16*)O_bf16;
+    HstuAttnArgs a = make_attn_args(d, pos_table, time_table, s, (const bf16*)P_bf16, (bf16*)O_bf16);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (d->D / d->H == 32) return launch_hstu_attn_fwd<32>(a, st);
     return launch_hstu_attn_fwd<64>(a, st);
@@ -735,7 +659,7 @@ int grb_hstu_attention_backward(const grb_hstu_dims* d, const float* pos_table, 
                 "the attention kernels need bias_index (pitch a multiple of 8 and >= L)");
     GRB_REQUIRE(aligned16(P_bf16) && aligned16(dO_bf16) && aligned16(dzp_bf16) && aligned16(scratch) && (zp_bf16 == nullptr || aligned16(zp_bf16)),
                 "buffers must be 16-byte aligned");
-    HstuAttnArgs a = make_attn_args_p(d, pos_table, time_table, s, (const bf16*)P_bf16);
+    HstuAttnArgs a = make_attn_args(d, pos_table, time_table, s, (const bf16*)P_bf16, nullptr);
     a.dw_part = static_cast<float*>(scratch);
     GRB_REQUIRE(a.bias.wtime == nullptr || dtime_table != nullptr, "time_table gradient pointer is null");
     const int D = d->D;
@@ -805,7 +729,7 @@ struct HeadWork {
     int ldl;
     size_t bytes;
 };
-bool head_fused(int D) { return use_tc() && (D == 64 || D == 128); }
+bool head_fused(int D) { return D <= 128; }
 HeadWork carve_head(void* base, size_t T, size_t D, size_t C) {
     HeadWork h;
     size_t off = 0;
@@ -816,7 +740,7 @@ HeadWork carve_head(void* base, size_t T, size_t D, size_t C) {
     h.stf = (float*)take(T * 2 * 4);
     h.dxf = (float*)take(T * D * 4);
     h.scal = (float*)take(64);
-    // D <= 128: the fused kernels (tc_ce.cuh) never form the [T, C] logits; D = 256 (and GRB_GEMM=mma) store them
+    // D <= 128: the fused kernels (tc_ce.cuh) never form the [T, C] logits; D = 256 stores them
     const bool fused = head_fused((int)D);
     h.logits = fused ? nullptr : (bf16*)take(T * (size_t)h.ldl * 2);
     h.logits32 = fused ? nullptr : (float*)take(T * (size_t)h.ldl * 4);
@@ -873,7 +797,9 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
         if (g_defer_on) GRB_TRY(defer_run(st, table_grad));
         else GRB_TRY(table_grad(st));
     } else {
-    GRB_CUDA(gemm_nt_f32(h.xf, (const bf16*)table_bf16, h.logits32, h.ldl, T, C, D, st));  // logits = xf E^T   (hstu.py:137)
+    // logits = xf E^T   (hstu.py:137)
+    GRB_CUDA((launch_tc_gemm<0, 0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, 1, TcEpiF32{nullptr, h.ldl, 1.f}, h.logits32, nullptr, h.ldl,
+                                   sm_count(), st)));
     if (h.ldl / 8 <= 256 * 8)
         launch_k(ce_fwd_bwd_vec_kernel<8>, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0,
                  (const float*)h.logits32);
@@ -886,18 +812,14 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
     if (!want_grad) return 0;
     GRB_CUDA(gemm_nn_f32(h.logits, (const bf16*)table_bf16, h.dxf, nullptr, 1.f, T, D, C, h.ldl, D, st));  // dxf = dlogits E
     // dE[C,D] += dlogits^T xf: a weight gradient, off the critical path with the deferred schedule
-    if (use_tc()) {
-        TnSpec spec{h.logits, h.xf, dtable, C, D, T, h.ldl, D, D};
-        if (g_defer_on) {
-            GRB_TRY(defer_run(st, [&](cudaStream_t side) -> int {
-                GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, side));
-                return 0;
-            }));
-        } else {
-            GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, st));
-        }
+    TnSpec spec{h.logits, h.xf, dtable, C, D, T, h.ldl, D, D};
+    if (g_defer_on) {
+        GRB_TRY(defer_run(st, [&](cudaStream_t side) -> int {
+            GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, side));
+            return 0;
+        }));
     } else {
-        GRB_CUDA(gemm_tn_atomic(h.logits, h.xf, dtable, C, D, T, h.ldl, D, st));
+        GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, st));
     }
     }
     {
@@ -918,7 +840,8 @@ int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float 
         LnFwdArgs a{x, ln_g, ln_b, h.xf, nullptr, h.stf, T, D, ln_eps};
         GRB_ROW_DISPATCH(D, ln_fwd_kernel, a, T, st);
     }
-    GRB_CUDA(gemm_nt_f32_plain(h.xf, (const bf16*)table_bf16, logits, T, C, D, st));
+    // logits [T, C] fp32, leading dimension C of any parity
+    GRB_CUDA((launch_tc_gemm<0, 0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, 1, TcEpiF32Plain{logits, C}, nullptr, nullptr, 0, sm_count(), st)));
     return 0;
 }
 
@@ -1156,14 +1079,7 @@ int grb_hstu_layer_forward_f32(const grb_hstu_dims* d, const grb_hstu_layer_para
     GRB_TRY(linear_f32x3(w.xs, (const bf16*)p->proj_w_split, p->proj_b, nullptr, T, 4 * D, D, 1, w.P, 4 * D, st));
     // O = silu(Q K^T + bias) V                                                                (hstu.py:244-267)
     {
-        HstuAttnF32Args a{w.P, 4 * D, d->B, d->L, d->H, {}, w.O};
-        // same conventions as make_attn_args(): uniform position buckets collapse to one effective bucket
-        a.bias.wpos = p->pos_table + (s->pos_uniform ? (size_t)s->pos_bucket0 * d->H : 0);
-        const bool has_time = p->time_table != nullptr && s->has_time && d->ntime > 0;
-        a.bias.wtime = has_time ? p->time_table : nullptr;
-        a.bias.bias_index = s->bias_index; a.bias.ldix = s->ld_index;
-        a.bias.npos = s->pos_uniform ? 1 : d->npos; a.bias.ntime = has_time ? d->ntime : 0;
-        a.bias.pos_uniform = s->pos_uniform; a.bias.pos_bucket0 = 0;
+        HstuAttnF32Args a{w.P, 4 * D, d->B, d->L, d->H, make_attn_bias(d, p->pos_table, p->time_table, s), w.O};
         int rc = DH == 32 ? launch_hstu_attn_f32<32>(a, st) : launch_hstu_attn_f32<64>(a, st);
         GRB_REQUIRE(rc == 0, "fp32 attention launch failed");
     }

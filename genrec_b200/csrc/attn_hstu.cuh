@@ -56,9 +56,9 @@ struct HstuAttnArgs {
     const bf16* d_o; int lddo;
     const bf16* zq; const bf16* zk; const bf16* zv; int ldz;    // pre-activations (nullable -> no silu' factor)
     bf16* dq; bf16* dk; bf16* dv; int lddq;                       // gradients w.r.t. pre-activations (or activations if z null)
-    float* dwpos;   // [npos, H]  accumulated (atomicAdd)
+    float* dwpos;   // [npos, H]  accumulated
     float* dwtime;  // [ntime, H] accumulated
-    float* dw_part; // nullable: [2H][B * key tiles][64] scratch for the ordered cross-CTA sum of dwpos / dwtime (det_finish_kernel)
+    float* dw_part; // [2H][B * key tiles][64] scratch for the ordered cross-CTA sum of dwpos / dwtime (det_finish_kernel)
 };
 
 GRB_DEVINL int time_bucket_dev(long long dt, const long long* thr, int ntime) {
@@ -583,7 +583,7 @@ __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 3 : 2) hstu_attn_bwd_d
         }
     }
 
-    // bias-table gradients: per-CTA sums, added across the CTAs of a head in (sequence, key tile) order when dw_part is given
+    // bias-table gradients: per-CTA sums, added across the CTAs of a head in (sequence, key tile) order by det_finish_kernel
     __shared__ float s_pos[ATT_THREADS / 32];
     if (pos_uniform) {
         pos_acc = warp_sum(pos_acc);
@@ -608,19 +608,9 @@ __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 3 : 2) hstu_attn_bwd_d
             for (int l = 0; l < 32; ++l) v += hist_t[(w * nt_bins + bk) * 32 + l];
         return v;
     };
-    if (a.dw_part) {
-        if (pos_uniform) det_store(a.dw_part, h, member, nmem, 64, 1, pos_sum);
-        else det_store(a.dw_part, h, member, nmem, 64, npos, pos_bin);
-        if (has_time && a.dwtime) det_store(a.dw_part, a.H + h, member, nmem, 64, ntime, time_bin);
-    } else {
-        if (pos_uniform) {
-            if (tid == 0) atomicAdd(a.dwpos + a.bias.pos_bucket0 * a.H + h, pos_sum(0));
-        } else {
-            for (int bk = tid; bk < npos; bk += ATT_THREADS) atomicAdd(a.dwpos + bk * a.H + h, pos_bin(bk));
-        }
-        if (has_time && a.dwtime)
-            for (int bk = tid; bk < ntime; bk += ATT_THREADS) atomicAdd(a.dwtime + bk * a.H + h, time_bin(bk));
-    }
+    if (pos_uniform) det_store(a.dw_part, h, member, nmem, 64, 1, pos_sum);
+    else det_store(a.dw_part, h, member, nmem, 64, npos, pos_bin);
+    if (has_time && a.dwtime) det_store(a.dw_part, a.H + h, member, nmem, 64, ntime, time_bin);
 }
 
 }  // namespace grb

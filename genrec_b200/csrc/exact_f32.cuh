@@ -19,7 +19,7 @@ struct HstuAttnF32Args {
     const float* P;   // [T, ld]  U | V | Q | K, each D wide, head h = columns h*DH .. (after SiLU)
     int ld;
     int B, L, H;
-    HstuBiasArgs bias;   // legacy [B, L, ldix] uint16 index matrix (built once per batch by hstu_bias_index_kernel)
+    HstuBiasArgs bias;   // [B, L, ldix] uint16 index matrix (built once per batch by hstu_bias_index_kernel)
     float* O;         // [T, D]
 };
 

@@ -102,7 +102,7 @@ struct LnGateBwdArgs {
     float *dg1, *db1, *dg2, *db2;  // accumulated
     int T, D;
     Dropout drop;
-    float* part;                   // nullable: [4][gridDim.x][D] scratch for the ordered cross-CTA sum (det_finish_kernel)
+    float* part;                   // [4][gridDim.x][D] scratch for the ordered cross-CTA sum (det_finish_kernel)
 };
 template <int NP>
 __global__ void __launch_bounds__(ROW_THREADS) ln_gate_bwd_kernel(LnGateBwdArgs a) {
@@ -198,7 +198,6 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_gate_bwd_kernel(LnGateBwdArgs 
             red[2][wib][c] = adg2[p][e]; red[3][wib][c] = adb2[p][e];
         }
     __syncthreads();
-    float* outs[4] = {a.dg1, a.db1, a.dg2, a.db2};
     for (int which = 0; which < 4; ++which) {
         auto colsum = [&](int c) {
             float s = 0.f;
@@ -206,8 +205,7 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_gate_bwd_kernel(LnGateBwdArgs 
             for (int w = 0; w < ROW_THREADS / 32; ++w) s += red[which][w][c];
             return s;
         };
-        if (a.part) det_store(a.part, which, blockIdx.x, gridDim.x, a.D, a.D, colsum);
-        else for (int c = threadIdx.x; c < a.D; c += ROW_THREADS) atomicAdd(outs[which] + c, colsum(c));
+        det_store(a.part, which, blockIdx.x, gridDim.x, a.D, a.D, colsum);
     }
 }
 
@@ -336,10 +334,11 @@ __global__ void cast_f32_bf16_kernel(const float* __restrict__ in, bf16* __restr
         if (cq >= D4) { cq -= D4; ++row; }
     }
 }
-// out_bf16[r, c] = bf16(dropmask(in[r, c]))  and  colsum[c] += sum_r out_bf16[r, c]   (the cast of dy and the bias gradient
-// of the layer's last linear in one pass).  grid (ceil(D / 128), chunks) ; block 256 = 8 row lanes x 32 threads of 4 columns.
+// out_bf16[r, c] = bf16(dropmask(in[r, c]))  and  the per-CTA column sums of out_bf16 -> part [ceil(D / 128)][chunks][128], which
+// det_finish_kernel adds to the bias gradient (the cast of dy and the bias gradient of the layer's last linear in one pass).
+// grid (ceil(D / 128), chunks) ; block 256 = 8 row lanes x 32 threads of 4 columns.
 __global__ void __launch_bounds__(256) cast_colsum_f32_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, int T, int D,
-                                                                  Dropout drop, float* __restrict__ colsum, float* __restrict__ part) {
+                                                                  Dropout drop, float* __restrict__ part) {
     pdl_wait();
     drop.resolve();
     __shared__ float red[8][128];
@@ -378,9 +377,7 @@ __global__ void __launch_bounds__(256) cast_colsum_f32_bf16_kernel(const float* 
         for (int w = 0; w < 8; ++w) t += red[w][i];
         return t;
     };
-    const int nc = min(128, D - (int)blockIdx.x * 128);
-    if (part) det_store(part, blockIdx.x, blockIdx.y, gridDim.y, 128, nc, sum8);
-    else if (threadIdx.x < nc) atomicAdd(colsum + blockIdx.x * 128 + threadIdx.x, sum8(threadIdx.x));
+    det_store(part, blockIdx.x, blockIdx.y, gridDim.y, 128, min(128, D - (int)blockIdx.x * 128), sum8);
 }
 // out[c] += sum_r in[r, c]   in: bf16 [T, ld] (ld % 8 == 0), columns [0, N) ; grid (ceil(N/256), chunks) ;
 // block 256 = 32 column groups of 8 (one 16-byte load each) x 8 row lanes, 4 rows in flight per thread

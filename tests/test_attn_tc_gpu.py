@@ -65,9 +65,8 @@ def test_bucket_bytes_bit_exact(L):
     assert torch.equal(got, _oracle_bytes(pad, None))
 
 
-def test_legacy_bias_index_bit_exact(monkeypatch):
-    """hstu_bias_index_kernel (the mma.sync path's [B, L, L] uint16 matrix): time bucket, position bucket and masks == oracle."""
-    monkeypatch.setenv("GRB_ATTN", "mma")
+def test_bias_index_bit_exact():
+    """hstu_bias_index_kernel (the attention kernels' [B, L, L] uint16 matrix): time bucket, position bucket and masks == oracle."""
     dev = torch.device("cuda:0")
     g = torch.Generator().manual_seed(3)
     B, L = 5, 70

@@ -282,3 +282,36 @@ def test_deferred_weight_gradients_equal_inline_ones():
     # mirror (seen in 3 of 40 repetitions, scripts/flake_deferred.py: 10 elements, 5e-5 of the largest gradient)
     torch.testing.assert_close(res[1][0][1], res[0][0][1], rtol=1e-3, atol=3e-4 * res[0][0][1].abs().max().item())
     assert ((res[1][1] - res[0][1]).abs() > 1e-4).float().mean().item() < 1e-3
+
+
+def test_training_steps_are_bit_identical_across_runs():
+    """Two training steps with the benchmark's optimizer settings (unit loss gradient, deferred weight gradients) and dropout, run
+    twice from the same seed: every cross-CTA sum of the step adds in a fixed order, so the gradients and the parameters of the two
+    runs are bit-identical."""
+    from genrec_b200.hstu import HSTU
+    from genrec_b200.optim import FlatAdam
+    import genrec_b200.functional as Fn
+    dev = torch.device("cuda:0")
+    ids, ts, tg = make_batch(8, 70, 1000, seed=4, pad=True, device=dev)
+    res = []
+    try:
+        for _ in range(2):
+            torch.manual_seed(0)
+            m = HSTU(1000, 70, 128, 4, 2, dropout=0.2).to(dev).train()
+            opt = FlatAdam(m, lr=1e-3, unit_loss_grad=True, defer_weight_grads=True)
+            gs = []
+            for _ in range(2):
+                _, loss = m(ids, ts, tg)
+                loss.backward()
+                opt.sync_grads()
+                gs.append(opt.grad.clone())
+                opt.step()
+            torch.cuda.synchronize()
+            res.append((gs, opt.flat.clone()))
+    finally:
+        Fn.set_defer_weight_grads(False)
+        Fn.join_deferred(dev)
+    for step, (a, b) in enumerate(zip(res[0][0], res[1][0])):
+        assert a.abs().max() > 0
+        assert torch.equal(a, b), (step, (a != b).sum().item())
+    assert torch.equal(res[0][1], res[1][1]), (res[0][1] != res[1][1]).sum().item()

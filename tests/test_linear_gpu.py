@@ -1,4 +1,4 @@
-"""GEMM building blocks through the C ABI (wgmma/TMA path by default; GRB_GEMM=mma selects the mma.sync path) vs torch."""
+"""GEMM building blocks through the C ABI (the wgmma/TMA kernels) vs torch."""
 import pytest
 import torch
 
