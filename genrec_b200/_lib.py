@@ -43,6 +43,11 @@ class HstuSeq(C.Structure):
                 ("timestamps", c_void_p), ("pad", c_void_p), ("rel32", c_void_p), ("wide", c_void_p), ("time_thr", c_void_p)]
 
 
+class HstuCache(C.Structure):
+    _fields_ = [("B", c_int), ("capacity", c_int), ("num_layers", c_int), ("kv", c_void_p), ("timestamps", c_void_p),
+                ("lengths", c_void_p), ("overflow", c_void_p)]
+
+
 class SasrecDims(C.Structure):
     _fields_ = [("B", c_int), ("L", c_int), ("D", c_int), ("H", c_int), ("dropout_p", c_float), ("seed", c_u64),
                 ("seed_dev", c_void_p), ("layer_index", c_int)]
@@ -69,6 +74,10 @@ SIGNATURES = {
     "grb_hstu_attention_forward": (c_int, [P(HstuDims), c_void_p, c_void_p, P(HstuSeq), c_void_p, c_void_p, c_void_p]),
     "grb_hstu_attention_backward": (c_int, [P(HstuDims), c_void_p, c_void_p, P(HstuSeq), c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_hstu_cache_append": (c_int, [P(HstuCache), c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "grb_hstu_layer_extend_workspace_bytes": (c_size_t, [P(HstuDims), c_int]),
+    "grb_hstu_layer_extend": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuCache), c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                      c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_collate_jagged": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_embed_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int,
                                   c_float, c_u64, c_void_p, c_void_p]),

@@ -11,6 +11,7 @@
 #include <utility>
 
 #include "attn_hstu.cuh"
+#include "attn_hstu_extend.cuh"
 #include "attn_sasrec.cuh"
 #include "attn_t5.cuh"
 #include "attn_buckets.cuh"
@@ -431,6 +432,58 @@ int colsum(const bf16* in, int T, int N, int ld, float* out, float* part, cudaSt
     return 0;
 }
 
+// ---- cached incremental inference (attn_hstu_extend.cuh)
+// keys per CTA of the chunk attention: enough key splits that B * H * query tiles * splits reaches about four CTAs per SM (one
+// new item per user must still fill the GPU), at least one 64-key tile each.  A function of the shapes and the capacity only, so
+// the grid is the same on every call and a captured graph stays valid while the lengths grow on the device.
+int extend_split(const grb_hstu_dims* d, int capacity) {
+    const long long base = (long long)d->B * d->H * ((d->L + ATT_BLK - 1) / ATT_BLK);
+    const long long want = (4LL * sm_count() + base - 1) / base;
+    const int per = (int)((capacity + want - 1) / want);
+    return (per + ATT_BLK - 1) / ATT_BLK * ATT_BLK;
+}
+int check_extend(const grb_hstu_dims* d, int capacity) {
+    GRB_TRY(check_dims(d));
+    GRB_REQUIRE(capacity >= 1 && capacity <= 16384, "cache capacity %d out of range [1, 16384]", capacity);
+    GRB_REQUIRE(d->dropout_p == 0.f, "the cached extend is inference only: dropout_p must be 0");
+    GRB_REQUIRE((long long)d->B * ((d->L + ATT_BLK - 1) / ATT_BLK) <= 65535, "B * ceil(n / 64) = %lld exceeds 65535",
+                (long long)d->B * ((d->L + ATT_BLK - 1) / ATT_BLK));
+    return 0;
+}
+// workspace: the forward's activation layout for the chunk's B * n rows, then the [splits, B * n, D] fp32 attention partials
+struct ExtendWork {
+    LayerSaved sv;
+    float* part;
+    size_t bytes;
+};
+ExtendWork carve_extend(void* base, const grb_hstu_dims* d, int capacity) {
+    const size_t T = (size_t)d->B * d->L;
+    ExtendWork w;
+    w.sv = carve_saved(base, T, d->D);
+    const int split = extend_split(d, capacity);
+    const size_t nsplit = (capacity + split - 1) / split;
+    w.part = base ? reinterpret_cast<float*>(static_cast<char*>(base) + w.sv.bytes) : nullptr;
+    w.bytes = w.sv.bytes + align_up(nsplit * T * d->D * 4);
+    return w;
+}
+template <int DH, bool UNIFORM, bool TIMED>
+int launch_attn_extend(const HstuExtendArgs& a, int nsplit, cudaStream_t st) {
+    const size_t smem = sizeof(ExtSmem<DH>) + align_up((size_t)(a.bias.npos * 64 + 1) * 4, 16);
+    GRB_TRY(set_smem(hstu_attn_extend_kernel<DH, UNIFORM, TIMED>, smem));
+    const dim3 grid(nsplit, a.H, a.B * ((a.n + ATT_BLK - 1) / ATT_BLK));
+    launch_k(hstu_attn_extend_kernel<DH, UNIFORM, TIMED>, grid, ATT_THREADS, smem, st, a);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+template <int DH>
+int dispatch_attn_extend(const HstuExtendArgs& a, int nsplit, cudaStream_t st) {
+    const bool uni = a.pos_bucket == nullptr, timed = a.bias.wtime != nullptr;
+    if (uni && timed) return launch_attn_extend<DH, true, true>(a, nsplit, st);
+    if (uni) return launch_attn_extend<DH, true, false>(a, nsplit, st);
+    if (timed) return launch_attn_extend<DH, false, true>(a, nsplit, st);
+    return launch_attn_extend<DH, false, false>(a, nsplit, st);
+}
+
 constexpr uint32_t SITE_GATE = 0, SITE_FFN_HID = 1, SITE_FFN_OUT = 2, SITE_EMBED = 250, SITE_ATTN = 3;
 inline uint32_t site_of(int layer, uint32_t which) { return (uint32_t)layer * 8u + which; }
 
@@ -577,6 +630,90 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
         GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, st));
     }
     (void)nodrop;
+    return 0;
+}
+
+int grb_hstu_cache_append(const grb_hstu_cache* c, const int64_t* input_ids, const int64_t* timestamps, int n, int32_t* positions,
+                          int32_t* last_row, void* stream) {
+    GRB_REQUIRE(c && input_ids && positions && last_row, "null argument");
+    GRB_REQUIRE(c->timestamps && c->lengths && c->overflow, "null cache pointer");
+    GRB_REQUIRE(c->B > 0 && n > 0, "bad shape B=%d n=%d", c->B, n);
+    GRB_REQUIRE(c->capacity >= 1 && c->capacity <= 16384, "cache capacity %d out of range [1, 16384]", c->capacity);
+    launch_k(hstu_cache_append_kernel, (unsigned)((c->B + 3) / 4), 128, 0, static_cast<cudaStream_t>(stream),
+             reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(timestamps), c->B, n, c->capacity,
+             reinterpret_cast<long long*>(c->timestamps), c->lengths, c->overflow, positions, last_row);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+size_t grb_hstu_layer_extend_workspace_bytes(const grb_hstu_dims* d, int capacity) {
+    if (check_extend(d, capacity)) return 0;
+    return carve_extend(nullptr, d, capacity).bytes;
+}
+
+// the steps of grb_hstu_layer_forward on the chunk's rows, with the attention against the cache in place of step 3
+int grb_hstu_layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_cache* c, int layer,
+                          const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr,
+                          const float* x, float* y, void* workspace, void* stream) {
+    GRB_REQUIRE(c != nullptr, "null cache");
+    GRB_TRY(check_extend(d, c->capacity));
+    GRB_REQUIRE(p && positions && x && y && workspace && c->kv && c->timestamps, "null argument");
+    GRB_REQUIRE(p->proj_w && p->proj_b && p->pos_table && p->ln1_g && p->ln1_b && p->ffn1_w && p->ffn1_b && p->ffn2_w &&
+                    p->ffn2_b && p->ln2_g && p->ln2_b, "null parameter pointer");
+    GRB_REQUIRE(c->B == d->B, "cache holds %d users, dims say B=%d", c->B, d->B);
+    GRB_REQUIRE(layer >= 0 && layer < c->num_layers, "layer %d out of range [0, %d)", layer, c->num_layers);
+    GRB_REQUIRE(pos_bucket != nullptr || (pos_bucket0 >= 0 && pos_bucket0 < d->npos), "pos_bucket0 %d out of range", pos_bucket0);
+    const bool timed = d->ntime > 0 && p->time_table != nullptr;
+    GRB_REQUIRE(!timed || time_thr != nullptr, "time_thr is null");
+    GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(workspace) && aligned16(c->kv) && aligned16(p->proj_w) && aligned16(p->ffn1_w) &&
+                    aligned16(p->ffn2_w), "buffers must be 16-byte aligned");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int T = d->B * d->L, D = d->D, cap = c->capacity;
+    ExtendWork w = carve_extend(workspace, d, cap);
+    LayerSaved& sv = w.sv;
+    const Dropout nodrop = make_dropout(0.f, 0, 0);
+    bf16* kv = static_cast<bf16*>(c->kv) + (size_t)layer * d->B * cap * 2 * D;
+
+    GRB_TRY(cast_bf16(x, sv.xb, (size_t)T * D, D, nodrop, nullptr, st));
+    GRB_CUDA(gemm_bias_act(1, sv.xb, (const bf16*)p->proj_w, p->proj_b, sv.zp, sv.P, T, 4 * D, D, nodrop, st));
+    {
+        const size_t pieces = (size_t)T * (2 * D / 8);
+        launch_k(hstu_kv_scatter_kernel, (unsigned)((pieces + 255) / 256), 256, 0, st, (const bf16*)sv.P, (const int*)positions, T, d->L, D,
+                 cap, kv);
+        GRB_CUDA(cudaGetLastError());
+    }
+    {
+        grb_hstu_seq s;
+        memset(&s, 0, sizeof(s));
+        s.has_time = timed;
+        s.pos_uniform = pos_bucket == nullptr;
+        s.pos_bucket0 = pos_bucket0;
+        HstuExtendArgs a;
+        memset(&a, 0, sizeof(a));
+        a.q = sv.P + 2 * D; a.ldq = 4 * D;
+        a.kv = kv;
+        a.ts = reinterpret_cast<const long long*>(c->timestamps);
+        a.pos = positions;
+        a.pos_bucket = pos_bucket;
+        a.thr = reinterpret_cast<const long long*>(time_thr);
+        a.bias = make_attn_bias(d, p->pos_table, timed ? p->time_table : nullptr, &s);
+        a.B = d->B; a.n = d->L; a.H = d->H; a.D = D; a.cap = cap;
+        a.split = extend_split(d, cap);
+        a.part = w.part;
+        const int nsplit = (cap + a.split - 1) / a.split;
+        if (D / d->H == 32) GRB_TRY(dispatch_attn_extend<32>(a, nsplit, st));
+        else GRB_TRY(dispatch_attn_extend<64>(a, nsplit, st));
+        const size_t quads = (size_t)T * D / 4;
+        launch_k(hstu_extend_combine_kernel, (unsigned)((quads + 255) / 256), 256, 0, st, (const float*)w.part, (const int*)positions, T, D,
+                 a.split, sv.O);
+        GRB_CUDA(cudaGetLastError());
+    }
+    {
+        LnGateFwdArgs a{sv.O, D, sv.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, sv.x1, sv.xn, sv.st1, sv.st2, T, D, 1e-5f, nodrop};
+        GRB_ROW_DISPATCH(D, ln_gate_fwd_kernel, a, T, st);
+    }
+    GRB_CUDA(gemm_bias_act(1, sv.xn, (const bf16*)p->ffn1_w, p->ffn1_b, sv.z1, sv.hact, T, 4 * D, D, nodrop, st));
+    GRB_CUDA(gemm_bias_res(sv.hact, (const bf16*)p->ffn2_w, p->ffn2_b, sv.x1, nullptr, y, T, D, 4 * D, nodrop, st));
     return 0;
 }
 

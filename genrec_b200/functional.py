@@ -400,6 +400,48 @@ def hstu_attention_bwd(P, zp, dO, meta: SeqMeta, H: int, pos_table, time_table, 
     return dzp, dpos, dtime
 
 
+# ------------------------------------------------------------------------------------------------ cached incremental inference
+def hstu_cache_append(cache: _lib.HstuCache, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor]):
+    """input_ids / timestamps [B, n] int64 -> (positions [B, n] int32, last_row [B] int32); advances the cache's lengths and stores
+    the chunk's timestamps (grb_hstu_cache_append)."""
+    require_cuda(input_ids, timestamps)
+    require_i64(input_ids, timestamps)
+    B, n = input_ids.shape
+    positions = torch.empty(B, n, dtype=torch.int32, device=input_ids.device)
+    last_row = torch.empty(B, dtype=torch.int32, device=input_ids.device)
+    with torch.cuda.device(input_ids.device):
+        check(_lib.load().grb_hstu_cache_append(C.byref(cache), ptr(input_ids.contiguous()),
+                                                ptr(timestamps.contiguous()) if timestamps is not None else None, n, ptr(positions),
+                                                ptr(last_row), stream_ptr(input_ids.device)))
+    return positions, last_row
+
+
+def hstu_layer_extend(x: torch.Tensor, cache: _lib.HstuCache, layer: int, positions: torch.Tensor, pos_bucket: Optional[torch.Tensor],
+                      pos_bucket0: int, time_thr: torch.Tensor, H: int, npos: int, ntime: int, bf16w: dict, params) -> torch.Tensor:
+    """One block on a chunk against the cache (grb_hstu_layer_extend): x [B, n, D] fp32 -> y [B, n, D] fp32.  ``params`` in
+    PARAM_ORDER (time_table None or ntime = 0: no temporal term), ``bf16w`` the three bf16 weight mirrors."""
+    lib = _lib.load()
+    require_cuda(x)
+    require_f32(x)
+    B, n, D = x.shape
+    xc = x.contiguous()
+    named = dict(zip(PARAM_ORDER, params))
+    has_time = named["time_table"] is not None and ntime > 0
+    dims = _dims(B, n, D, H, npos, ntime if has_time else 0, 0.0, 0, None, layer)
+    pstruct = HstuLayerParams(*[
+        ptr(bf16w[k]) if k in BF16_PARAMS else (ptr(named[k].detach()) if named[k] is not None and (k != "time_table" or has_time) else None)
+        for k in PARAM_ORDER])
+    nbytes = lib.grb_hstu_layer_extend_workspace_bytes(C.byref(dims), cache.capacity)
+    if nbytes == 0:
+        raise _lib.GrbError(lib.grb_last_error().decode())
+    ws = _u8(nbytes, x.device)
+    y = torch.empty_like(xc)
+    with torch.cuda.device(x.device):
+        check(lib.grb_hstu_layer_extend(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(positions), ptr(pos_bucket), int(pos_bucket0),
+                                        ptr(time_thr), ptr(xc), ptr(y), ptr(ws), stream_ptr(x.device)))
+    return y
+
+
 # ------------------------------------------------------------------------------------------------ SASRec pieces
 def layernorm_fwd(x, g, b, eps, want_bf16=True, want_f32=False):
     lib = _lib.load()

@@ -20,6 +20,7 @@ from typing import Optional, Tuple
 import torch
 import torch.nn as nn
 
+from . import _lib
 from . import functional as Fn
 from ._lib import ensure_device, require_cuda
 
@@ -232,6 +233,41 @@ class HSTULayer(nn.Module):
         return self._run(x, _meta, _seed, _seed_dev)
 
 
+class HSTUState:
+    """Cached history of a batch of users for incremental inference (``HSTU.new_state`` / ``HSTU.extend``).
+
+    Holds, per block, the K | V rows of every item seen so far (``kv`` [num_blocks, B, capacity, 2D] bf16), their timestamps,
+    the per-user item counts and overflow flags, and each user's last final-block output (``last_hidden`` [B, D] fp32).  A state
+    belongs to the parameters it was first written with: ``extend`` raises once any parameter's version counter has moved (a torch
+    optimizer step, ``load_state_dict``).  ``genrec_b200.optim.FlatAdam`` writes parameters through a raw pointer and is not caught,
+    so rebuild every state after any further training.  Items are never evicted: a user whose history outgrows ``capacity`` has
+    the excess dropped and is flagged in ``overflowed()``; start a new state for them.
+    """
+
+    def __init__(self, batch_size: int, capacity: int, num_layers: int, embed_dim: int, device):
+        if batch_size < 1:
+            raise ValueError(f"batch_size must be positive, got {batch_size}")
+        if not 1 <= capacity <= 16384:
+            raise ValueError(f"capacity must lie in [1, 16384], got {capacity}")
+        self.batch_size, self.capacity, self.num_layers = batch_size, capacity, num_layers
+        self.kv = torch.zeros(num_layers, batch_size, capacity, 2 * embed_dim, dtype=torch.bfloat16, device=device)
+        self.timestamps = torch.zeros(batch_size, capacity, dtype=torch.int64, device=device)
+        self.lengths = torch.zeros(batch_size, dtype=torch.int32, device=device)
+        self.overflow = torch.zeros(batch_size, dtype=torch.uint8, device=device)
+        self.last_hidden = torch.zeros(batch_size, embed_dim, dtype=torch.float32, device=device)
+        self.items_bound = 0      # host-side sum of the chunk widths extended so far: an upper bound of every user's length
+        self.has_time = None      # whether the temporal bias is in use, fixed by the first extend
+        self.param_versions = None
+
+    def overflowed(self) -> torch.Tensor:
+        """[B] bool on the device: users that had items dropped for lack of capacity.  Reading it on the host synchronises."""
+        return self.overflow != 0
+
+    def _struct(self) -> _lib.HstuCache:
+        return _lib.HstuCache(self.batch_size, self.capacity, self.num_layers, self.kv.data_ptr(), self.timestamps.data_ptr(),
+                              self.lengths.data_ptr(), self.overflow.data_ptr())
+
+
 class HSTU(nn.Module):
     """Mirror of genrec/models/hstu.py:19-157."""
 
@@ -372,6 +408,67 @@ class HSTU(nn.Module):
         if self.precision == "fp32":
             return self._head_logits_f32(x[:, -1:, :].contiguous())[:, 0, :]
         return Fn.head_logits(x[:, -1:, :].contiguous(), self.final_norm.weight, self.final_norm.bias, self.item_embedding.weight,
+                              self._table_mirror(), self.final_norm.eps)[:, 0, :]
+
+    def new_state(self, batch_size: int, capacity: int) -> HSTUState:
+        """An empty cache for ``batch_size`` users of up to ``capacity`` items each (<= 16384), on the model's device."""
+        return HSTUState(batch_size, capacity, len(self.layers), self.embed_dim, self.item_embedding.weight.device)
+
+    @torch.no_grad()
+    def extend(self, state: HSTUState, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Append the non-zero ids of each row of ``input_ids`` [B, n] (with ``timestamps`` [B, n] or None), in order, to that user's
+        history in ``state`` and return [B, V+1] fp32: the next-item logits of each user's latest item, as ``last_logits`` computes
+        them for the left-padded concatenation of everything extended so far.  Prefilling a history is ``extend`` on a new state.
+
+        Only the new items run through the blocks; the earlier ones are read from the cache.  Pads inside a chunk are compacted
+        (positions count items): with the reference's position bias, where every causal cell uses one bucket, any padding pattern
+        gives the full forward's result; with a non-uniform position-bucket table that holds for left-padded chunks only.  A user
+        whose row is all padding keeps their state and gets the same logits row as from the previous call; a user with no item yet
+        gets the head applied to a zero vector.  Inference only: bf16 precision, no dropout, no autograd.  CUDA-graph capturable
+        after one eager call; the host-side capacity check does not run on replay, where items that do not fit are dropped and
+        flagged (``state.overflowed()``)."""
+        if self.precision == "fp32":
+            raise RuntimeError("genrec_b200: extend runs the bf16 path only; set_precision('bf16') or use last_logits")
+        if self.training and any(isinstance(m, nn.Dropout) and m.p > 0 for m in self.modules()):
+            raise RuntimeError("genrec_b200: extend has no dropout; call model.eval()")
+        require_cuda(input_ids)
+        ensure_device(input_ids.device)
+        B, n = input_ids.shape
+        if B != state.batch_size or input_ids.device != state.lengths.device:
+            raise ValueError(f"the state holds {state.batch_size} users on {state.lengths.device}; got input_ids {tuple(input_ids.shape)} on "
+                             f"{input_ids.device}")
+        if state.items_bound + n > state.capacity:
+            raise ValueError(f"extending by {n} items could exceed the state's capacity ({state.items_bound} of {state.capacity} may be "
+                             "used); start a new state with a larger capacity")
+        use_time = timestamps is not None and self.use_temporal_bias
+        versions = tuple(p._version for p in self.parameters())
+        if state.param_versions is None:
+            state.param_versions, state.has_time = versions, use_time
+        elif state.param_versions != versions:
+            raise RuntimeError("genrec_b200: the model's parameters changed after this state was written; rebuild the state")
+        elif state.has_time != use_time:
+            raise ValueError("timestamps must be given on every extend of a state or on none")
+        dev = input_ids.device
+        ids = input_ids.contiguous()
+        cache = state._struct()
+        positions, last_row = Fn.hstu_cache_append(cache, ids, timestamps.contiguous() if timestamps is not None else None)
+        x, _ = Fn.EmbedFn.apply(ids, self.item_embedding.weight, None, 1.0, 0, 0.0, 0, None, None)
+        if len(self.layers):
+            rpb = self.layers[0].position_bias
+            uniform, bucket0 = rpb.uniform_of(state.capacity, dev)
+            pos_bucket = None if uniform else rpb.bucket_of_delta(state.capacity, dev)
+            ntime = self.layers[0].temporal_bias.num_buckets if use_time else 0
+            for i, layer in enumerate(self.layers):
+                layer._bf16_provider = self._bf16_provider
+                bf16w = {"proj_w": layer._mirror("proj_w", layer.projection.weight),
+                         "ffn1_w": layer._mirror("ffn1_w", layer.ffn[0].weight),
+                         "ffn2_w": layer._mirror("ffn2_w", layer.ffn[3].weight)}
+                x = Fn.hstu_layer_extend(x, cache, i, positions, pos_bucket, bucket0, _thresholds_on(dev), layer.num_heads, rpb.num_buckets,
+                                         ntime, bf16w, layer._params())
+        latest = x[torch.arange(B, device=dev), last_row.clamp(min=0).long()]
+        state.last_hidden.copy_(torch.where((last_row >= 0)[:, None], latest, state.last_hidden))
+        state.items_bound += n
+        return Fn.head_logits(state.last_hidden[:, None, :], self.final_norm.weight, self.final_norm.bias, self.item_embedding.weight,
                               self._table_mirror(), self.final_norm.eps)[:, 0, :]
 
     @torch.no_grad()

@@ -130,6 +130,34 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
                             const float* dy, const void* saved, float* dx, const grb_hstu_layer_grads* g,
                             void* workspace, void* stream);
 
+/* ------------------------------------------------------------------------------------------------ cached incremental inference
+ * Extends `predict` / evaluation (hstu.py:150-157, trainers/hstu_trainer.py:55-81), which rerun the whole history for every new
+ * item: a cache keeps, per layer, the K | V rows of every item seen so far for a batch of B users, and a chunk of n new slots per
+ * user runs through the blocks against it.  Causal attention and relative-only biases make a cached row exact: for a left-padded
+ * history the result equals the full forward's.  Inference only (no dropout, no backward).
+ * Positions count items, not slots: the pads of a chunk are compacted away. */
+typedef struct {
+    int B, capacity, num_layers; /* capacity <= 16384 items per user */
+    void* kv;                    /* bf16 [num_layers, B, capacity, 2D]: row p of user b = K | V of the user's p-th item */
+    int64_t* timestamps;         /* [B, capacity] */
+    int32_t* lengths;            /* [B] items cached per user */
+    uint8_t* overflow;           /* [B] set to 1 when an item did not fit in `capacity` (it is dropped, never written) */
+} grb_hstu_cache;
+/* One launch per chunk, before the layers: input_ids / timestamps [B, n] (timestamps may be NULL -> 0 is stored; ids == 0 are
+ * pads).  positions [B, n] int32 = the cache position of every valid row (-1 for a pad or a dropped item); the chunk's timestamps
+ * are stored, lengths advance (never past capacity) and last_row [B] int32 = the chunk row of each user's last valid item, or -1. */
+int grb_hstu_cache_append(const grb_hstu_cache* c, const int64_t* input_ids, const int64_t* timestamps, int n, int32_t* positions,
+                          int32_t* last_row, void* stream);
+/* One block on the chunk: d->L = n (dropout_p must be 0), x / y [B * n, D] fp32.  The K | V of the chunk's valid rows are written
+ * into layer `layer` of the cache, then every valid row attends to the cached keys [0, position] of its user.
+ * pos_bucket [capacity] uint8: position bucket of delta = p_i - p_j (the table RelativePositionBias.bucket_of_delta builds), or
+ * NULL when every delta maps to bucket pos_bucket0 (the reference's behaviour).  time_thr [65] as in grb_hstu_bias_index; the
+ * temporal term is used when d->ntime > 0 and p->time_table != NULL.  workspace: grb_hstu_layer_extend_workspace_bytes(d, capacity). */
+size_t grb_hstu_layer_extend_workspace_bytes(const grb_hstu_dims* d, int capacity);
+int grb_hstu_layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_cache* c, int layer,
+                          const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr,
+                          const float* x, float* y, void* workspace, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ input pipeline
  * Device-side hstu_collate_fn / sasrec_collate_fn (genrec/data/amazon_hstu.py:137-173, genrec/data/amazon_sasrec.py:125-161): a
  * jagged batch (items / stamps [N] in time order, offsets [B+1], one held-out target per user) -> the LEFT-padded [B, L]

@@ -1,5 +1,6 @@
-"""Stand-alone device timings of the secondary kernels (RQ-VAE residual argmin, SASRec attention, HSTU layer at cfg-3
-geometry) with CUDA events, against the relevant roofline.  Prints one JSON line per measurement."""
+"""Stand-alone device timings of the secondary kernels (RQ-VAE residual argmin, SASRec attention, HSTU layer at cfg-3 geometry,
+cached incremental HSTU inference next to full recompute) with CUDA events, against the relevant roofline.  Prints one JSON line per
+measurement."""
 import json
 import os
 import sys
@@ -46,6 +47,73 @@ def graph_timed(fn, reps=10, iters=10):
     return e0.elapsed_time(e1) / (reps * iters)
 
 
+def kernel_us(fn, name, iters=20):
+    """Mean device time (us) per launch of the kernels whose name contains `name`, from a torch.profiler run of its own."""
+    from torch.profiler import ProfilerActivity, profile
+    fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(iters):
+            fn()
+        torch.cuda.synchronize()
+    hits = [k for k in prof.key_averages() if name in k.key]
+    total, count = sum(k.device_time_total for k in hits), sum(k.count for k in hits)
+    return total / count if count else float("nan")
+
+
+def card():
+    import subprocess
+    q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                       text=True)
+    return dict(gpu=torch.cuda.get_device_name(0), power_limit_and_max_sm_clock=q.stdout.strip() or "unknown")
+
+
+def bench_extend(dev):
+    """Cached incremental inference (HSTU.extend) next to full recompute (HSTU.last_logits) on the same full sequences: one new
+    item per user on a history of L - 1, and the prefill of the whole history (extend on an empty state).  Both graph-captured.
+    The state is rewound on the device before every call (lengths.fill_, one small kernel inside the timed graph), so every call
+    appends at the same position.  The chunk-attention kernel's bytes are the cache K | V and timestamps it must read."""
+    from genrec_b200.hstu import HSTU
+    info = card()
+    HBM = 3.35e12   # H100 SXM data sheet, bytes/s
+    geoms = (("cfg2", dict(num_items=12101, embed_dim=128, num_heads=4, num_blocks=4), 200, (1, 128)),
+             ("cfg3", dict(num_items=12101, embed_dim=256, num_heads=8, num_blocks=8), 2048, (1, 32)))
+    g = torch.Generator().manual_seed(0)
+    for name, geo, L, batches in geoms:
+        torch.manual_seed(0)
+        m = HSTU(max_seq_len=L, dropout=0.0, **geo).to(dev).eval()
+        D, NB = geo["embed_dim"], geo["num_blocks"]
+        for B in batches:
+            ids = torch.randint(1, geo["num_items"] + 1, (B, L), generator=g).to(dev)
+            ts = (1_300_000_000 + torch.cumsum(torch.randint(1, 3 * 86400, (B, L), generator=g), 1)).to(dev)
+            st = m.new_state(B, L)
+            m.extend(st, ids[:, :-1], ts[:, :-1])
+
+            def one():
+                st.lengths.fill_(L - 1)
+                st.items_bound = L - 1
+                return m.extend(st, ids[:, -1:], ts[:, -1:])
+
+            def prefill():
+                st.lengths.zero_()
+                st.items_bound = 0
+                return m.extend(st, ids, ts)
+
+            full_ms = graph_timed(lambda: m.last_logits(ids, ts))
+            for work, fn, keys in (("extend_1", one, L), ("prefill", prefill, None)):
+                ms = graph_timed(fn)
+                row = dict(kernel="hstu_extend", geometry=name, workload=work, B=B, history=L - 1 if work == "extend_1" else 0,
+                           new_items=1 if work == "extend_1" else L, extend_us=ms * 1e3, last_logits_us=full_ms * 1e3,
+                           speedup_vs_last_logits=full_ms / ms, **info)
+                if keys is not None:
+                    attn_us = kernel_us(fn, "hstu_attn_extend_kernel")
+                    byt = B * keys * (2 * D * 2 + 8)            # per layer: K | V bf16 + int64 timestamp of every cached key
+                    row.update(attn_kernel_us=attn_us, attn_bytes_per_layer=byt, attn_hbm_gbs=byt / attn_us / 1e3,
+                               attn_frac_of_hbm_peak=byt / (attn_us * 1e-6) / HBM, blocks=NB)
+                print(json.dumps(row), flush=True)
+            assert torch.isfinite(one()).all()
+
+
 def main():
     dev = torch.device("cuda:0")
     peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) \
@@ -86,6 +154,7 @@ def main():
         print(json.dumps(dict(kernel="hstu_layer_fwd_bwd", B=B, L=L, D=D, H=H, ms=ms, seq_per_s=B / ms * 1e3,
                               algorithmic_tflops=flops / ms / 1e9, frac_of_bf16_peak=flops / ms / 1e9 / peak,
                               note="eager launches (not graph-captured): includes host launch gaps at L=200")))
+    bench_extend(dev)
 
 
 if __name__ == "__main__":
