@@ -48,6 +48,12 @@ class HstuCache(C.Structure):
                 ("lengths", c_void_p), ("overflow", c_void_p)]
 
 
+class HstuPool(C.Structure):
+    _fields_ = [("max_users", c_int), ("num_layers", c_int), ("page_size", c_int), ("num_pages", c_int), ("max_items", c_int),
+                ("kv", c_void_p), ("timestamps", c_void_p), ("page_table", c_void_p), ("lengths", c_void_p), ("overflow", c_void_p),
+                ("free_stack", c_void_p), ("free_top", c_void_p), ("errors", c_void_p), ("row_of", c_void_p)]
+
+
 class SasrecDims(C.Structure):
     _fields_ = [("B", c_int), ("L", c_int), ("D", c_int), ("H", c_int), ("dropout_p", c_float), ("seed", c_u64),
                 ("seed_dev", c_void_p), ("layer_index", c_int)]
@@ -78,6 +84,11 @@ SIGNATURES = {
     "grb_hstu_layer_extend_workspace_bytes": (c_size_t, [P(HstuDims), c_int]),
     "grb_hstu_layer_extend": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuCache), c_int, c_void_p, c_void_p, c_int, c_void_p,
                                       c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_hstu_pool_append": (c_int, [P(HstuPool), c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_hstu_pool_release": (c_int, [P(HstuPool), c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "grb_hstu_layer_extend_paged_workspace_bytes": (c_size_t, [P(HstuDims), P(HstuPool)]),
+    "grb_hstu_layer_extend_paged": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuPool), c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_collate_jagged": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_embed_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int,
                                   c_float, c_u64, c_void_p, c_void_p]),

@@ -484,6 +484,95 @@ int dispatch_attn_extend(const HstuExtendArgs& a, int nsplit, cudaStream_t st) {
     return launch_attn_extend<DH, false, false>(a, nsplit, st);
 }
 
+// Where one layer's cached K | V lives: the dense cache (users and page table null, page_size = capacity) or a pool.
+struct ExtendKv {
+    bf16* kv;                  // this layer's rows [pages * page_size, 2D]
+    const long long* ts;       // [pages * page_size]
+    const long long* users;    // [B] or null
+    KvPages pg;
+    int cap;                   // most items a user can hold
+};
+int check_pool(const grb_hstu_pool* p) {
+    GRB_REQUIRE(p != nullptr, "null pool");
+    GRB_REQUIRE(p->page_size >= ATT_BLK && p->page_size % ATT_BLK == 0, "page_size %d must be a positive multiple of %d", p->page_size, ATT_BLK);
+    GRB_REQUIRE(p->max_items >= 1 && p->max_items <= 16384, "pool max_items %d out of range [1, 16384]", p->max_items);
+    GRB_REQUIRE(p->max_users > 0 && p->num_pages > 0 && p->num_layers > 0, "bad pool shape max_users=%d num_pages=%d num_layers=%d",
+                p->max_users, p->num_pages, p->num_layers);
+    return 0;
+}
+inline int pool_pt_ld(const grb_hstu_pool* p) { return (p->max_items + p->page_size - 1) / p->page_size; }
+HstuPoolArgs pool_args(const grb_hstu_pool* p, const int64_t* users, int B) {
+    HstuPoolArgs a;
+    memset(&a, 0, sizeof(a));
+    a.users = reinterpret_cast<const long long*>(users); a.B = B;
+    a.max_users = p->max_users; a.max_items = p->max_items; a.num_pages = p->num_pages;
+    a.page_table = p->page_table; a.pt_ld = pool_pt_ld(p); a.page_size = p->page_size;
+    a.len = p->lengths; a.overflow = p->overflow; a.free_stack = p->free_stack; a.free_top = p->free_top;
+    a.errors = p->errors; a.row_of = p->row_of;
+    return a;
+}
+
+// the steps of grb_hstu_layer_forward on the chunk's rows, with the attention against the cache in place of step 3
+int layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const ExtendKv& c, const int32_t* positions,
+                 const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr, const float* x, float* y, void* workspace,
+                 cudaStream_t st) {
+    GRB_REQUIRE(p->proj_w && p->proj_b && p->pos_table && p->ln1_g && p->ln1_b && p->ffn1_w && p->ffn1_b && p->ffn2_w &&
+                    p->ffn2_b && p->ln2_g && p->ln2_b, "null parameter pointer");
+    GRB_REQUIRE(pos_bucket != nullptr || (pos_bucket0 >= 0 && pos_bucket0 < d->npos), "pos_bucket0 %d out of range", pos_bucket0);
+    const bool timed = d->ntime > 0 && p->time_table != nullptr;
+    GRB_REQUIRE(!timed || time_thr != nullptr, "time_thr is null");
+    GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(workspace) && aligned16(c.kv) && aligned16(p->proj_w) && aligned16(p->ffn1_w) &&
+                    aligned16(p->ffn2_w), "buffers must be 16-byte aligned");
+    const int T = d->B * d->L, D = d->D, cap = c.cap;
+    ExtendWork w = carve_extend(workspace, d, cap);
+    LayerSaved& sv = w.sv;
+    const Dropout nodrop = make_dropout(0.f, 0, 0);
+
+    GRB_TRY(cast_bf16(x, sv.xb, (size_t)T * D, D, nodrop, nullptr, st));
+    GRB_CUDA(gemm_bias_act(1, sv.xb, (const bf16*)p->proj_w, p->proj_b, sv.zp, sv.P, T, 4 * D, D, nodrop, st));
+    {
+        const size_t pieces = (size_t)T * (2 * D / 8);
+        launch_k(hstu_kv_scatter_kernel, (unsigned)((pieces + 255) / 256), 256, 0, st, (const bf16*)sv.P, (const int*)positions, c.users, T,
+                 d->L, D, c.pg, c.kv);
+        GRB_CUDA(cudaGetLastError());
+    }
+    {
+        grb_hstu_seq s;
+        memset(&s, 0, sizeof(s));
+        s.has_time = timed;
+        s.pos_uniform = pos_bucket == nullptr;
+        s.pos_bucket0 = pos_bucket0;
+        HstuExtendArgs a;
+        memset(&a, 0, sizeof(a));
+        a.q = sv.P + 2 * D; a.ldq = 4 * D;
+        a.kv = c.kv;
+        a.ts = c.ts;
+        a.users = c.users;
+        a.pg = c.pg;
+        a.pos = positions;
+        a.pos_bucket = pos_bucket;
+        a.thr = reinterpret_cast<const long long*>(time_thr);
+        a.bias = make_attn_bias(d, p->pos_table, timed ? p->time_table : nullptr, &s);
+        a.B = d->B; a.n = d->L; a.H = d->H; a.D = D; a.cap = cap;
+        a.split = extend_split(d, cap);
+        a.part = w.part;
+        const int nsplit = (cap + a.split - 1) / a.split;
+        if (D / d->H == 32) GRB_TRY(dispatch_attn_extend<32>(a, nsplit, st));
+        else GRB_TRY(dispatch_attn_extend<64>(a, nsplit, st));
+        const size_t quads = (size_t)T * D / 4;
+        launch_k(hstu_extend_combine_kernel, (unsigned)((quads + 255) / 256), 256, 0, st, (const float*)w.part, (const int*)positions, T, D,
+                 a.split, sv.O);
+        GRB_CUDA(cudaGetLastError());
+    }
+    {
+        LnGateFwdArgs a{sv.O, D, sv.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, sv.x1, sv.xn, sv.st1, sv.st2, T, D, 1e-5f, nodrop};
+        GRB_ROW_DISPATCH(D, ln_gate_fwd_kernel, a, T, st);
+    }
+    GRB_CUDA(gemm_bias_act(1, sv.xn, (const bf16*)p->ffn1_w, p->ffn1_b, sv.z1, sv.hact, T, 4 * D, D, nodrop, st));
+    GRB_CUDA(gemm_bias_res(sv.hact, (const bf16*)p->ffn2_w, p->ffn2_b, sv.x1, nullptr, y, T, D, 4 * D, nodrop, st));
+    return 0;
+}
+
 constexpr uint32_t SITE_GATE = 0, SITE_FFN_HID = 1, SITE_FFN_OUT = 2, SITE_EMBED = 250, SITE_ATTN = 3;
 inline uint32_t site_of(int layer, uint32_t which) { return (uint32_t)layer * 8u + which; }
 
@@ -640,8 +729,44 @@ int grb_hstu_cache_append(const grb_hstu_cache* c, const int64_t* input_ids, con
     GRB_REQUIRE(c->B > 0 && n > 0, "bad shape B=%d n=%d", c->B, n);
     GRB_REQUIRE(c->capacity >= 1 && c->capacity <= 16384, "cache capacity %d out of range [1, 16384]", c->capacity);
     launch_k(hstu_cache_append_kernel, (unsigned)((c->B + 3) / 4), 128, 0, static_cast<cudaStream_t>(stream),
-             reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(timestamps), c->B, n, c->capacity,
-             reinterpret_cast<long long*>(c->timestamps), c->lengths, c->overflow, positions, last_row);
+             reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(timestamps), (const long long*)nullptr,
+             (const int*)nullptr, c->B, n, c->capacity, KvPages{nullptr, 1, c->capacity}, reinterpret_cast<long long*>(c->timestamps),
+             c->lengths, c->overflow, positions, last_row);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int grb_hstu_pool_append(const grb_hstu_pool* pool, const int64_t* users, int B, const int64_t* input_ids, const int64_t* timestamps,
+                         int n, int32_t* positions, int32_t* last_row, int32_t* room, void* stream) {
+    GRB_TRY(check_pool(pool));
+    GRB_REQUIRE(users && input_ids && positions && last_row && room, "null argument");
+    GRB_REQUIRE(pool->timestamps && pool->page_table && pool->lengths && pool->overflow && pool->free_stack && pool->free_top &&
+                    pool->errors && pool->row_of, "null pool pointer");
+    GRB_REQUIRE(B > 0 && n > 0, "bad shape B=%d n=%d", B, n);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    HstuPoolArgs a = pool_args(pool, users, B);
+    a.ids = reinterpret_cast<const long long*>(input_ids); a.n = n;
+    a.room = room;
+    launch_k(hstu_pool_alloc_kernel, 1, POOL_THREADS, 0, st, a);
+    GRB_CUDA(cudaGetLastError());
+    launch_k(hstu_cache_append_kernel, (unsigned)((B + 3) / 4), 128, 0, st, reinterpret_cast<const long long*>(input_ids),
+             reinterpret_cast<const long long*>(timestamps), reinterpret_cast<const long long*>(users), (const int*)room, B, n,
+             pool->max_items, KvPages{pool->page_table, pool_pt_ld(pool), pool->page_size}, reinterpret_cast<long long*>(pool->timestamps),
+             pool->lengths, pool->overflow, positions, last_row);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int grb_hstu_pool_release(const grb_hstu_pool* pool, const int64_t* users, int B, float* last_hidden, int D, void* stream) {
+    GRB_TRY(check_pool(pool));
+    GRB_REQUIRE(users != nullptr, "null argument");
+    GRB_REQUIRE(pool->page_table && pool->lengths && pool->overflow && pool->free_stack && pool->free_top && pool->errors && pool->row_of,
+                "null pool pointer");
+    GRB_REQUIRE(B > 0, "bad shape B=%d", B);
+    GRB_REQUIRE(last_hidden == nullptr || D > 0, "last_hidden needs D > 0, got %d", D);
+    HstuPoolArgs a = pool_args(pool, users, B);
+    a.last_hidden = last_hidden; a.ld_hidden = D;
+    launch_k(hstu_pool_release_kernel, 1, POOL_THREADS, 0, static_cast<cudaStream_t>(stream), a);
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -651,70 +776,36 @@ size_t grb_hstu_layer_extend_workspace_bytes(const grb_hstu_dims* d, int capacit
     return carve_extend(nullptr, d, capacity).bytes;
 }
 
-// the steps of grb_hstu_layer_forward on the chunk's rows, with the attention against the cache in place of step 3
 int grb_hstu_layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_cache* c, int layer,
                           const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr,
                           const float* x, float* y, void* workspace, void* stream) {
     GRB_REQUIRE(c != nullptr, "null cache");
     GRB_TRY(check_extend(d, c->capacity));
     GRB_REQUIRE(p && positions && x && y && workspace && c->kv && c->timestamps, "null argument");
-    GRB_REQUIRE(p->proj_w && p->proj_b && p->pos_table && p->ln1_g && p->ln1_b && p->ffn1_w && p->ffn1_b && p->ffn2_w &&
-                    p->ffn2_b && p->ln2_g && p->ln2_b, "null parameter pointer");
     GRB_REQUIRE(c->B == d->B, "cache holds %d users, dims say B=%d", c->B, d->B);
     GRB_REQUIRE(layer >= 0 && layer < c->num_layers, "layer %d out of range [0, %d)", layer, c->num_layers);
-    GRB_REQUIRE(pos_bucket != nullptr || (pos_bucket0 >= 0 && pos_bucket0 < d->npos), "pos_bucket0 %d out of range", pos_bucket0);
-    const bool timed = d->ntime > 0 && p->time_table != nullptr;
-    GRB_REQUIRE(!timed || time_thr != nullptr, "time_thr is null");
-    GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(workspace) && aligned16(c->kv) && aligned16(p->proj_w) && aligned16(p->ffn1_w) &&
-                    aligned16(p->ffn2_w), "buffers must be 16-byte aligned");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int T = d->B * d->L, D = d->D, cap = c->capacity;
-    ExtendWork w = carve_extend(workspace, d, cap);
-    LayerSaved& sv = w.sv;
-    const Dropout nodrop = make_dropout(0.f, 0, 0);
-    bf16* kv = static_cast<bf16*>(c->kv) + (size_t)layer * d->B * cap * 2 * D;
+    const int cap = c->capacity;
+    ExtendKv kv{static_cast<bf16*>(c->kv) + (size_t)layer * d->B * cap * 2 * d->D, reinterpret_cast<const long long*>(c->timestamps),
+                nullptr, KvPages{nullptr, 1, cap}, cap};
+    return layer_extend(d, p, kv, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace, static_cast<cudaStream_t>(stream));
+}
 
-    GRB_TRY(cast_bf16(x, sv.xb, (size_t)T * D, D, nodrop, nullptr, st));
-    GRB_CUDA(gemm_bias_act(1, sv.xb, (const bf16*)p->proj_w, p->proj_b, sv.zp, sv.P, T, 4 * D, D, nodrop, st));
-    {
-        const size_t pieces = (size_t)T * (2 * D / 8);
-        launch_k(hstu_kv_scatter_kernel, (unsigned)((pieces + 255) / 256), 256, 0, st, (const bf16*)sv.P, (const int*)positions, T, d->L, D,
-                 cap, kv);
-        GRB_CUDA(cudaGetLastError());
-    }
-    {
-        grb_hstu_seq s;
-        memset(&s, 0, sizeof(s));
-        s.has_time = timed;
-        s.pos_uniform = pos_bucket == nullptr;
-        s.pos_bucket0 = pos_bucket0;
-        HstuExtendArgs a;
-        memset(&a, 0, sizeof(a));
-        a.q = sv.P + 2 * D; a.ldq = 4 * D;
-        a.kv = kv;
-        a.ts = reinterpret_cast<const long long*>(c->timestamps);
-        a.pos = positions;
-        a.pos_bucket = pos_bucket;
-        a.thr = reinterpret_cast<const long long*>(time_thr);
-        a.bias = make_attn_bias(d, p->pos_table, timed ? p->time_table : nullptr, &s);
-        a.B = d->B; a.n = d->L; a.H = d->H; a.D = D; a.cap = cap;
-        a.split = extend_split(d, cap);
-        a.part = w.part;
-        const int nsplit = (cap + a.split - 1) / a.split;
-        if (D / d->H == 32) GRB_TRY(dispatch_attn_extend<32>(a, nsplit, st));
-        else GRB_TRY(dispatch_attn_extend<64>(a, nsplit, st));
-        const size_t quads = (size_t)T * D / 4;
-        launch_k(hstu_extend_combine_kernel, (unsigned)((quads + 255) / 256), 256, 0, st, (const float*)w.part, (const int*)positions, T, D,
-                 a.split, sv.O);
-        GRB_CUDA(cudaGetLastError());
-    }
-    {
-        LnGateFwdArgs a{sv.O, D, sv.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, sv.x1, sv.xn, sv.st1, sv.st2, T, D, 1e-5f, nodrop};
-        GRB_ROW_DISPATCH(D, ln_gate_fwd_kernel, a, T, st);
-    }
-    GRB_CUDA(gemm_bias_act(1, sv.xn, (const bf16*)p->ffn1_w, p->ffn1_b, sv.z1, sv.hact, T, 4 * D, D, nodrop, st));
-    GRB_CUDA(gemm_bias_res(sv.hact, (const bf16*)p->ffn2_w, p->ffn2_b, sv.x1, nullptr, y, T, D, 4 * D, nodrop, st));
-    return 0;
+size_t grb_hstu_layer_extend_paged_workspace_bytes(const grb_hstu_dims* d, const grb_hstu_pool* pool) {
+    if (check_pool(pool) || check_extend(d, pool->max_items)) return 0;
+    return carve_extend(nullptr, d, pool->max_items).bytes;
+}
+
+int grb_hstu_layer_extend_paged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_pool* pool, int layer,
+                                const int64_t* users, const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0,
+                                const int64_t* time_thr, const float* x, float* y, void* workspace, void* stream) {
+    GRB_TRY(check_pool(pool));
+    GRB_TRY(check_extend(d, pool->max_items));
+    GRB_REQUIRE(p && users && positions && x && y && workspace && pool->kv && pool->timestamps && pool->page_table, "null argument");
+    GRB_REQUIRE(layer >= 0 && layer < pool->num_layers, "layer %d out of range [0, %d)", layer, pool->num_layers);
+    ExtendKv kv{static_cast<bf16*>(pool->kv) + (size_t)layer * pool->num_pages * pool->page_size * 2 * d->D,
+                reinterpret_cast<const long long*>(pool->timestamps), reinterpret_cast<const long long*>(users),
+                KvPages{pool->page_table, pool_pt_ld(pool), pool->page_size}, pool->max_items};
+    return layer_extend(d, p, kv, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace, static_cast<cudaStream_t>(stream));
 }
 
 int grb_hstu_bias_index(const int64_t* timestamps, const uint8_t* pad, const int64_t* time_thr, const uint8_t* pos_bucket, int B, int L,

@@ -14,22 +14,49 @@
 // Parallelism: keys are split across CTAs (grid.x) so that one new item per user still fills the GPU.  Without a softmax
 // the split partials combine by plain summation; each CTA stores its fp32 partial and hstu_extend_combine_kernel adds them
 // in split order, so the result is the same from run to run.
+//
+// Paged pool: the same kernels serve a pool of K | V pages shared by many users.  Row b of a call belongs to user users[b]
+// (any distinct subset of the pool's users), and item p of user u lives in page page_table[u, p / page_size] at row
+// p % page_size.  The dense cache above is the degenerate pool: page_size = cap, page b belongs to user b, users = 0 .. B-1,
+// which is what a null page table and a null user list stand for.  A page holds a whole number of 64-key tiles, so no key
+// tile of the attention straddles two pages.  hstu_pool_alloc_kernel hands out the pages a call needs (one CTA, in row order,
+// so the outcome of running out is deterministic) and hstu_pool_release_kernel gives a user's pages back.
 #pragma once
 #include "attn_hstu.cuh"
 
 namespace grb {
 
-// One warp per user.  pos[b, r] = len[b] + (valid rows of the chunk before r) for a valid row (id != 0), -1 for a pad
-// and for an item that does not fit in `cap` (dropped; overflow[b] = 1).  The chunk's timestamps are written into the
-// cache, len[b] becomes min(len[b] + valid, cap) and last_row[b] is the chunk row of the user's last valid item, or -1.
-__global__ void __launch_bounds__(128) hstu_cache_append_kernel(const long long* __restrict__ ids, const long long* __restrict__ ts, int B,
-                                                                int n, int cap, long long* __restrict__ cache_ts, int* __restrict__ len,
-                                                                uint8_t* __restrict__ overflow, int* __restrict__ pos,
+// Where item p of user u is stored: row pg.row(u, p) of the [pages * page_size] rows of K | V (and of timestamps).
+struct KvPages {
+    const int* page_table;   // [users, pt_ld] page of each page_size items ; null: the dense cache (page u, page_size = capacity)
+    int pt_ld, page_size;
+    GRB_DEVINL size_t row(int u, int p) const {
+        return page_table ? (size_t)page_table[(size_t)u * pt_ld + p / page_size] * page_size + p % page_size
+                          : (size_t)u * page_size + p;
+    }
+};
+
+// One warp per chunk row b of user u = users[b] (b without a user list).  pos[b, r] = len[u] + (valid rows of the chunk before
+// r) for a valid row (id != 0), -1 for a pad and for an item that does not fit in the user's room (dropped; overflow[u] = 1).
+// The room is room[b] (the pool: what the allocation left the user, -1 = a rejected row, treated as all padding) or `cap`
+// without a room list.  The chunk's timestamps are written into the cache, len[u] becomes min(len[u] + valid, room) and
+// last_row[b] is the chunk row of the user's last valid item, or -1.
+__global__ void __launch_bounds__(128) hstu_cache_append_kernel(const long long* __restrict__ ids, const long long* __restrict__ ts,
+                                                                const long long* __restrict__ users, const int* __restrict__ room, int B,
+                                                                int n, int cap, KvPages pg, long long* __restrict__ cache_ts,
+                                                                int* __restrict__ len, uint8_t* __restrict__ overflow, int* __restrict__ pos,
                                                                 int* __restrict__ last_row) {
     pdl_wait();
     const int b = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (b >= B) return;
-    const int base = len[b];
+    const int lim = room ? room[b] : cap;
+    if (lim < 0) {
+        for (int r = lane; r < n; r += 32) pos[(size_t)b * n + r] = -1;
+        if (lane == 0) last_row[b] = -1;
+        return;
+    }
+    const int u = users ? (int)users[b] : b;
+    const int base = len[u];
     int count = 0, last = -1;
     for (int r0 = 0; r0 < n; r0 += 32) {
         const int r = r0 + lane;
@@ -38,9 +65,9 @@ __global__ void __launch_bounds__(128) hstu_cache_append_kernel(const long long*
         const int q = base + count + __popc(m & ((1u << lane) - 1u));
         if (r < n) {
             int p = -1;
-            if (valid && q < cap) {
+            if (valid && q < lim) {
                 p = q;
-                cache_ts[(size_t)b * cap + q] = ts ? ts[(size_t)b * n + r] : 0;
+                cache_ts[pg.row(u, q)] = ts ? ts[(size_t)b * n + r] : 0;
             }
             pos[(size_t)b * n + r] = p;
         }
@@ -49,16 +76,17 @@ __global__ void __launch_bounds__(128) hstu_cache_append_kernel(const long long*
     }
     if (lane == 0) {
         const long long total = (long long)base + count;
-        len[b] = total > cap ? cap : (int)total;
-        if (total > cap) overflow[b] = 1;
+        len[u] = total > lim ? lim : (int)total;
+        if (total > lim) overflow[u] = 1;
         last_row[b] = last;
     }
 }
 
-// kv[b, pos, 0:D) = K row, kv[b, pos, D:2D) = V row of every chunk row with pos >= 0.  P = [U | V | Q | K] [B*n, 4D] bf16.
-// One thread per 16-byte piece.
-__global__ void __launch_bounds__(256) hstu_kv_scatter_kernel(const bf16* __restrict__ P, const int* __restrict__ pos, int T, int n, int D,
-                                                              int cap, bf16* __restrict__ kv) {
+// K | V row of every chunk row with pos >= 0 into the cache row of (users[b], pos): [0, D) = K, [D, 2D) = V.
+// P = [U | V | Q | K] [B*n, 4D] bf16.  One thread per 16-byte piece.
+__global__ void __launch_bounds__(256) hstu_kv_scatter_kernel(const bf16* __restrict__ P, const int* __restrict__ pos,
+                                                              const long long* __restrict__ users, int T, int n, int D, KvPages pg,
+                                                              bf16* __restrict__ kv) {
     pdl_wait();
     const int per_row = 2 * D / 8;
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -67,20 +95,22 @@ __global__ void __launch_bounds__(256) hstu_kv_scatter_kernel(const bf16* __rest
     const int p = pos[row];
     if (p < 0) return;
     const int b = row / n;
+    const int u = users ? (int)users[b] : b;
     const int src = c < D ? 3 * D + c : c;                                // K = P[:, 3D:4D) ; V = P[:, D:2D)
-    *reinterpret_cast<uint4*>(kv + ((size_t)b * cap + p) * 2 * D + c) =
-        *reinterpret_cast<const uint4*>(P + (size_t)row * 4 * D + src);
+    *reinterpret_cast<uint4*>(kv + pg.row(u, p) * 2 * D + c) = *reinterpret_cast<const uint4*>(P + (size_t)row * 4 * D + src);
 }
 
 struct HstuExtendArgs {
     const bf16* q; int ldq;            // chunk queries, [B * n] rows (P + 2D, ld 4D)
-    const bf16* kv;                    // this layer's cache [B, cap, 2D]: K | V
-    const long long* ts;               // [B, cap] cache timestamps
+    const bf16* kv;                    // this layer's K | V rows [pages * page_size, 2D]
+    const long long* ts;               // [pages * page_size] cache timestamps
+    const long long* users;            // [B] user of each chunk row ; null: row b is user b
+    KvPages pg;
     const int* pos;                    // [B * n] cache position of each chunk row, -1 = none
     const uint8_t* pos_bucket;         // [cap] bucket of delta = p_i - j ; null: every delta uses the single live row of bias.wpos
     const long long* thr;              // [65] time-bucket thresholds
     HstuBiasArgs bias;                 // wpos / wtime / npos / ntime (bias_index unused)
-    int B, n, H, D, cap;
+    int B, n, H, D, cap;               // cap: most items a user can hold
     int split;                         // keys per CTA, a multiple of ATT_BLK ; grid.x = ceil(cap / split)
     float* part;                       // [grid.x, B * n, D] fp32 partial outputs
 };
@@ -125,23 +155,24 @@ __global__ void __launch_bounds__(ATT_THREADS) hstu_attn_extend_kernel(HstuExten
     att_build_table(wcomb, a.bias, h, a.H, tid);
     if (TIMED)
         for (int i = tid; i <= ATT_MAX_BUCKETS; i += ATT_THREADS) sm.thr[i] = a.thr[i];
+    const int u = a.users ? (int)a.users[b] : b;              // read only for a row that has a position: a valid user
     const bf16* gq = a.q + row0 * a.ldq + h * DH;
-    const bf16* gk = a.kv + (size_t)b * a.cap * 2 * a.D + h * DH;
+    const bf16* gk = a.kv + h * DH;
     const bf16* gv = gk + a.D;
-    const long long* gts = a.ts + (size_t)b * a.cap;
     att_load_tile<DH>(sm.q, gq + (size_t)r0 * a.ldq, a.ldq, 0, 0, a.n - r0, 0, tid);
-    auto load_stream = [&](int k0, int buf) {
-        att_load_tile<DH>(sm.kv[buf][0], gk + (size_t)k0 * 2 * a.D, 2 * a.D, 0, 0, k_hi - k0, 0, tid);
-        att_load_tile<DH>(sm.kv[buf][1], gv + (size_t)k0 * 2 * a.D, 2 * a.D, 0, 0, k_hi - k0, 0, tid);
-        if (TIMED && tid < ATT_BLK) sm.ts[buf][tid] = k0 + tid < k_hi ? gts[k0 + tid] : 0;   // visible after the loop's barrier
+    auto load_stream = [&](int k0, int buf) {                 // the tile's 64 keys lie in one page
+        const size_t kr = a.pg.row(u, k0);
+        att_load_tile<DH>(sm.kv[buf][0], gk + kr * 2 * a.D, 2 * a.D, 0, 0, k_hi - k0, 0, tid);
+        att_load_tile<DH>(sm.kv[buf][1], gv + kr * 2 * a.D, 2 * a.D, 0, 0, k_hi - k0, 0, tid);
+        if (TIMED && tid < ATT_BLK) sm.ts[buf][tid] = k0 + tid < k_hi ? a.ts[kr + tid] : 0;   // visible after the loop's barrier
     };
     load_stream(k_lo, 0);
     cp_async_commit();
 
     long long tqa = 0, tqb = 0;
     if (TIMED) {
-        tqa = pa >= 0 ? gts[pa] : 0;
-        tqb = pb >= 0 ? gts[pb] : 0;
+        tqa = pa >= 0 ? a.ts[a.pg.row(u, pa)] : 0;
+        tqb = pb >= 0 ? a.ts[a.pg.row(u, pb)] : 0;
     }
     const int warp_pmax = wmax;
     uint32_t qf[DH / 16][4];
@@ -219,6 +250,154 @@ __global__ void __launch_bounds__(256) hstu_extend_combine_kernel(const float* _
     out.x = pack_bf16(acc.x, acc.y);
     out.y = pack_bf16(acc.z, acc.w);
     *reinterpret_cast<uint2*>(O + (size_t)row * D + c) = out;
+}
+
+// ---- page pool bookkeeping: one CTA per call, rows in order, so that which items find a page is a function of the call alone
+constexpr int POOL_THREADS = 1024;
+constexpr unsigned POOL_ERR_RANGE = 1u, POOL_ERR_REPEAT = 2u;   // bits of *errors
+
+struct HstuPoolArgs {
+    const long long* users; int B;     // [B] users of the call's rows
+    const long long* ids; int n;       // [B, n] chunk ids (allocation only)
+    int max_users, max_items, num_pages;
+    int* page_table; int pt_ld, page_size;
+    int* len; uint8_t* overflow;
+    int* free_stack; int* free_top;    // free pages are free_stack[0 .. *free_top), the next one handed out is the top
+    unsigned* errors;
+    int* row_of;                       // [max_users] scratch: INT_MAX between calls
+    int* room;                         // [B] out (allocation): items the row's user may now hold, -1 for a rejected row
+    float* last_hidden; int ld_hidden; // [max_users, ld_hidden] rows zeroed on release (nullable)
+};
+
+// exclusive prefix sum of v over the CTA's POOL_THREADS threads; *total = the CTA's sum.  ws: 32 ints of shared memory
+GRB_DEVINL int pool_scan(int v, int* ws, int* total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) ws[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        int w = ws[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, w, o);
+            if (lane >= o) w += y;
+        }
+        ws[lane] = w;
+    }
+    __syncthreads();
+    const int before = warp ? ws[warp - 1] : 0;
+    *total = ws[31];
+    __syncthreads();
+    return before + x - v;
+}
+
+// A row's user is accepted when it lies in [0, max_users) and no earlier row of the call names it; row_of[u] becomes the first
+// row naming u.  Rejections set bits of *errors.
+GRB_DEVINL void pool_mark_users(const HstuPoolArgs& a) {
+    for (int b = threadIdx.x; b < a.B; b += POOL_THREADS) {
+        const long long u = a.users[b];
+        if (u >= 0 && u < a.max_users) atomicMin(&a.row_of[u], b);
+        else atomicOr(a.errors, POOL_ERR_RANGE);
+    }
+    __syncthreads();
+}
+GRB_DEVINL int pool_user_of(const HstuPoolArgs& a, int b) {    // the row's user, or -1 for a rejected row
+    const long long u = a.users[b];
+    if (u < 0 || u >= a.max_users) return -1;
+    if (*reinterpret_cast<volatile int*>(&a.row_of[u]) != b) {
+        atomicOr(a.errors, POOL_ERR_REPEAT);
+        return -1;
+    }
+    return (int)u;
+}
+GRB_DEVINL void pool_unmark_users(const HstuPoolArgs& a) {
+    __syncthreads();
+    for (int b = threadIdx.x; b < a.B; b += POOL_THREADS) {
+        const long long u = a.users[b];
+        if (u >= 0 && u < a.max_users) a.row_of[u] = 0x7fffffff;
+    }
+}
+
+// Row b needs the pages that its user's items after this chunk (at most max_items) take beyond the ceil(len / page_size) the
+// user holds.  Pages are popped from the top of the free stack in row order; a row that finds the stack empty gets what is left
+// (possibly nothing) and its items beyond its pages are dropped by hstu_cache_append_kernel.
+__global__ void __launch_bounds__(POOL_THREADS) hstu_pool_alloc_kernel(HstuPoolArgs a) {
+    pdl_wait();
+    __shared__ int cnt[POOL_THREADS];
+    __shared__ int ws[32];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int avail = *a.free_top;
+    pool_mark_users(a);
+    int handed = 0;                                            // pages asked for by the rows before this chunk
+    for (int c0 = 0; c0 < a.B; c0 += POOL_THREADS) {
+        const int rows = min(POOL_THREADS, a.B - c0);
+        for (int r = warp; r < rows; r += 32) {                // valid items of each row: one warp per row
+            int c = 0;
+            for (int j = lane; j < a.n; j += 32) c += a.ids[(size_t)(c0 + r) * a.n + j] != 0;
+#pragma unroll
+            for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+            if (lane == 0) cnt[r] = c;
+        }
+        __syncthreads();
+        const int b = c0 + tid;
+        int u = -1, have = 0, need = 0;
+        if (tid < rows) {
+            u = pool_user_of(a, b);
+            if (u >= 0) {
+                const int l = a.len[u];
+                const int want = min(l + cnt[tid], a.max_items);
+                have = (l + a.page_size - 1) / a.page_size;
+                need = max(0, (want + a.page_size - 1) / a.page_size - have);
+            }
+        }
+        int total;
+        const int start = handed + pool_scan(need, ws, &total);
+        const int got = max(0, min(need, avail - start));
+        for (int k = 0; k < got; ++k) a.page_table[(size_t)u * a.pt_ld + have + k] = a.free_stack[avail - 1 - (start + k)];
+        if (tid < rows) a.room[b] = u >= 0 ? min(a.max_items, (have + got) * a.page_size) : -1;
+        handed += total;
+        __syncthreads();                                       // cnt is rewritten by the next chunk
+    }
+    pool_unmark_users(a);
+    if (tid == 0) *a.free_top = avail - min(handed, avail);
+}
+
+// Pushes each accepted row's pages back onto the free stack, in row order and then page order, and forgets the user: length,
+// overflow flag and last hidden row become 0.
+__global__ void __launch_bounds__(POOL_THREADS) hstu_pool_release_kernel(HstuPoolArgs a) {
+    pdl_wait();
+    __shared__ int ws[32];
+    const int tid = threadIdx.x;
+    const int top = *a.free_top;
+    pool_mark_users(a);
+    int pushed = 0;
+    for (int c0 = 0; c0 < a.B; c0 += POOL_THREADS) {
+        const int b = c0 + tid;
+        const int u = b < a.B ? pool_user_of(a, b) : -1;
+        const int pages = u >= 0 ? (a.len[u] + a.page_size - 1) / a.page_size : 0;
+        int total;
+        const int start = top + pushed + pool_scan(pages, ws, &total);
+        for (int k = 0; k < pages; ++k)
+            if (start + k < a.num_pages) a.free_stack[start + k] = a.page_table[(size_t)u * a.pt_ld + k];
+        if (u >= 0) {
+            a.len[u] = 0;
+            a.overflow[u] = 0;
+        }
+        pushed += total;
+    }
+    if (a.last_hidden) {
+        for (size_t i = tid; i < (size_t)a.B * a.ld_hidden; i += POOL_THREADS) {
+            const long long u = a.users[i / a.ld_hidden];
+            if (u >= 0 && u < a.max_users) a.last_hidden[(size_t)u * a.ld_hidden + i % a.ld_hidden] = 0.f;
+        }
+    }
+    pool_unmark_users(a);
+    if (tid == 0) *a.free_top = min(top + pushed, a.num_pages);
 }
 
 }  // namespace grb

@@ -416,9 +416,11 @@ def hstu_cache_append(cache: _lib.HstuCache, input_ids: torch.Tensor, timestamps
     return positions, last_row
 
 
-def hstu_layer_extend(x: torch.Tensor, cache: _lib.HstuCache, layer: int, positions: torch.Tensor, pos_bucket: Optional[torch.Tensor],
-                      pos_bucket0: int, time_thr: torch.Tensor, H: int, npos: int, ntime: int, bf16w: dict, params) -> torch.Tensor:
-    """One block on a chunk against the cache (grb_hstu_layer_extend): x [B, n, D] fp32 -> y [B, n, D] fp32.  ``params`` in
+def hstu_layer_extend(x: torch.Tensor, cache, layer: int, positions: torch.Tensor, pos_bucket: Optional[torch.Tensor],
+                      pos_bucket0: int, time_thr: torch.Tensor, H: int, npos: int, ntime: int, bf16w: dict, params,
+                      users: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """One block on a chunk against the cache: x [B, n, D] fp32 -> y [B, n, D] fp32.  ``cache`` is a dense ``HstuCache``
+    (grb_hstu_layer_extend) or an ``HstuPool`` with ``users`` [B] int64 on the device (grb_hstu_layer_extend_paged).  ``params`` in
     PARAM_ORDER (time_table None or ntime = 0: no temporal term), ``bf16w`` the three bf16 weight mirrors."""
     lib = _lib.load()
     require_cuda(x)
@@ -431,15 +433,51 @@ def hstu_layer_extend(x: torch.Tensor, cache: _lib.HstuCache, layer: int, positi
     pstruct = HstuLayerParams(*[
         ptr(bf16w[k]) if k in BF16_PARAMS else (ptr(named[k].detach()) if named[k] is not None and (k != "time_table" or has_time) else None)
         for k in PARAM_ORDER])
-    nbytes = lib.grb_hstu_layer_extend_workspace_bytes(C.byref(dims), cache.capacity)
+    paged = isinstance(cache, _lib.HstuPool)
+    if paged:
+        nbytes = lib.grb_hstu_layer_extend_paged_workspace_bytes(C.byref(dims), C.byref(cache))
+    else:
+        nbytes = lib.grb_hstu_layer_extend_workspace_bytes(C.byref(dims), cache.capacity)
     if nbytes == 0:
         raise _lib.GrbError(lib.grb_last_error().decode())
     ws = _u8(nbytes, x.device)
     y = torch.empty_like(xc)
     with torch.cuda.device(x.device):
-        check(lib.grb_hstu_layer_extend(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(positions), ptr(pos_bucket), int(pos_bucket0),
-                                        ptr(time_thr), ptr(xc), ptr(y), ptr(ws), stream_ptr(x.device)))
+        if paged:
+            check(lib.grb_hstu_layer_extend_paged(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(users), ptr(positions),
+                                                  ptr(pos_bucket), int(pos_bucket0), ptr(time_thr), ptr(xc), ptr(y), ptr(ws),
+                                                  stream_ptr(x.device)))
+        else:
+            check(lib.grb_hstu_layer_extend(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(positions), ptr(pos_bucket),
+                                            int(pos_bucket0), ptr(time_thr), ptr(xc), ptr(y), ptr(ws), stream_ptr(x.device)))
     return y
+
+
+def hstu_pool_append(pool: _lib.HstuPool, users: torch.Tensor, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor]):
+    """users [B] int64 and input_ids / timestamps [B, n] int64 on the device -> (positions [B, n] int32, last_row [B] int32, room [B]
+    int32); hands out the pages the chunk needs and stores its timestamps (grb_hstu_pool_append)."""
+    require_cuda(users, input_ids, timestamps)
+    require_i64(users, input_ids, timestamps)
+    B, n = input_ids.shape
+    dev = input_ids.device
+    positions = torch.empty(B, n, dtype=torch.int32, device=dev)
+    last_row = torch.empty(B, dtype=torch.int32, device=dev)
+    room = torch.empty(B, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().grb_hstu_pool_append(C.byref(pool), ptr(users.contiguous()), B, ptr(input_ids.contiguous()),
+                                               ptr(timestamps.contiguous()) if timestamps is not None else None, n, ptr(positions),
+                                               ptr(last_row), ptr(room), stream_ptr(dev)))
+    return positions, last_row, room
+
+
+def hstu_pool_release(pool: _lib.HstuPool, users: torch.Tensor, last_hidden: Optional[torch.Tensor]) -> None:
+    """Return the pages of users [B] int64 (device) to the pool and zero their lengths, flags and rows of last_hidden [*, D] fp32."""
+    require_cuda(users, last_hidden)
+    require_i64(users)
+    D = last_hidden.shape[1] if last_hidden is not None else 0
+    with torch.cuda.device(users.device):
+        check(_lib.load().grb_hstu_pool_release(C.byref(pool), ptr(users.contiguous()), users.numel(), ptr(last_hidden), D,
+                                                stream_ptr(users.device)))
 
 
 # ------------------------------------------------------------------------------------------------ SASRec pieces

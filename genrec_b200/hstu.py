@@ -268,6 +268,103 @@ class HSTUState:
                               self.lengths.data_ptr(), self.overflow.data_ptr())
 
 
+class HSTUPool:
+    """Paged history cache of many users for serving (``HSTU.new_pool`` / ``HSTU.extend_users`` / ``HSTUPool.release``).
+
+    Every block's K | V rows live in ``num_pages`` pages of ``page_size`` items shared by all users (``kv`` [num_blocks, num_pages,
+    page_size, 2D] bf16, ``timestamps`` [num_pages, page_size]); ``page_table`` [max_users, ceil(max_items / page_size)] maps a
+    user's item p to page ``page_table[u, p // page_size]``.  Pages are handed out on the device as a user's items arrive and come
+    back on ``release``, so memory follows the items actually cached.  A user holds at most ``max_items`` items; items beyond that,
+    or that find no free page, are dropped and flag the user in ``overflowed()``.  ``errors()`` has bit ``ERR_USER_RANGE`` set after
+    a call named a user outside [0, max_users) and ``ERR_USER_REPEAT`` after a call named a user twice (those rows count as padding).
+    Like ``HSTUState``, a pool belongs to the parameters it was first written with.
+
+    The host keeps a conservative bound of each user's items (the sum of the chunk widths since the user's last release) and of the
+    pages in use, and refuses an eager call with ``users`` on the CPU that could break a limit.  Calls with ``users`` on the device
+    (CUDA graphs) skip those checks and do not update the bounds; the device rules above decide instead.
+    """
+    ERR_USER_RANGE, ERR_USER_REPEAT = 1, 2
+
+    def __init__(self, max_users: int, num_pages: int, page_size: int, max_items: int, num_layers: int, embed_dim: int, device):
+        if max_users < 1 or num_pages < 1:
+            raise ValueError(f"max_users and num_pages must be positive, got {max_users}, {num_pages}")
+        if page_size < 64 or page_size % 64:
+            raise ValueError(f"page_size must be a positive multiple of 64 (the attention's key tile), got {page_size}")
+        if not 1 <= max_items <= 16384:
+            raise ValueError(f"max_items must lie in [1, 16384], got {max_items}")
+        self.max_users, self.num_pages, self.page_size, self.max_items = max_users, num_pages, page_size, max_items
+        self.num_layers = num_layers
+        self.kv = torch.zeros(num_layers, num_pages, page_size, 2 * embed_dim, dtype=torch.bfloat16, device=device)
+        self.timestamps = torch.zeros(num_pages, page_size, dtype=torch.int64, device=device)
+        self.page_table = torch.zeros(max_users, -(-max_items // page_size), dtype=torch.int32, device=device)
+        self.lengths = torch.zeros(max_users, dtype=torch.int32, device=device)
+        self.overflow = torch.zeros(max_users, dtype=torch.uint8, device=device)
+        self.free_stack = torch.arange(num_pages - 1, -1, -1, dtype=torch.int32, device=device)   # page 0 goes out first
+        self.free_top = torch.full((1,), num_pages, dtype=torch.int32, device=device)
+        self.error_bits = torch.zeros(1, dtype=torch.int32, device=device)
+        self.row_of = torch.full((max_users,), (1 << 31) - 1, dtype=torch.int32, device=device)
+        # each user's last final-block output; the extra last row stays zero and stands in for rejected rows
+        self.last_hidden = torch.zeros(max_users + 1, embed_dim, dtype=torch.float32, device=device)
+        self.items_bound = torch.zeros(max_users, dtype=torch.int64)   # host
+        self.pages_bound = 0
+        self.has_time = None
+        self.param_versions = None
+
+    def overflowed(self) -> torch.Tensor:
+        """[max_users] bool on the device: users that had items dropped.  Reading it on the host synchronises."""
+        return self.overflow != 0
+
+    def pages_free(self) -> torch.Tensor:
+        """0-dim int32 on the device: pages not held by any user."""
+        return self.free_top[0]
+
+    def errors(self) -> torch.Tensor:
+        """0-dim int32 on the device: ERR_USER_RANGE | ERR_USER_REPEAT bits of every call so far."""
+        return self.error_bits[0]
+
+    def _pages(self, items: torch.Tensor) -> torch.Tensor:
+        return (items + self.page_size - 1) // self.page_size
+
+    def _host_users(self, users: torch.Tensor) -> torch.Tensor:
+        if users.dim() != 1 or users.numel() == 0:
+            raise ValueError(f"users must be a non-empty 1-D tensor, got shape {tuple(users.shape)}")
+        u = users.long()
+        if bool(((u < 0) | (u >= self.max_users)).any()):
+            raise ValueError(f"users out of range [0, {self.max_users}): {u[(u < 0) | (u >= self.max_users)].tolist()[:8]}")
+        if torch.unique(u).numel() != u.numel():
+            raise ValueError("users must be distinct within a call")
+        return u
+
+    def _check_room(self, u: torch.Tensor, n: int):
+        """Host refusal of a chunk of width n for CPU users u; returns the bound update to apply once the call is launched."""
+        old = self.items_bound[u]
+        new = old + n
+        if bool((new > self.max_items).any()):
+            bad = u[new > self.max_items].tolist()[:8]
+            raise ValueError(f"extending by {n} items could exceed max_items ({self.max_items}) for users {bad}; release them first")
+        pages = self.pages_bound + int(self._pages(new).sum() - self._pages(old).sum())
+        if pages > self.num_pages:
+            raise ValueError(f"extending by {n} items could need {pages} pages of the pool's {self.num_pages}; release users first")
+        return new, pages
+
+    def release(self, users) -> None:
+        """Forget ``users`` (distinct, any subset): their pages return to the pool, their lengths, overflow flags and last outputs
+        become zero, and the next ``extend_users`` starts their histories afresh."""
+        users = torch.as_tensor(users, dtype=torch.int64) if not isinstance(users, torch.Tensor) else users
+        dev = self.lengths.device
+        if not users.is_cuda:
+            u = self._host_users(users)
+            self.pages_bound -= int(self._pages(self.items_bound[u]).sum())
+            self.items_bound[u] = 0
+            users = u.to(dev)
+        Fn.hstu_pool_release(self._struct(), users.long(), self.last_hidden)
+
+    def _struct(self) -> _lib.HstuPool:
+        return _lib.HstuPool(self.max_users, self.num_layers, self.page_size, self.num_pages, self.max_items, self.kv.data_ptr(),
+                             self.timestamps.data_ptr(), self.page_table.data_ptr(), self.lengths.data_ptr(), self.overflow.data_ptr(),
+                             self.free_stack.data_ptr(), self.free_top.data_ptr(), self.error_bits.data_ptr(), self.row_of.data_ptr())
+
+
 class HSTU(nn.Module):
     """Mirror of genrec/models/hstu.py:19-157."""
 
@@ -427,10 +524,7 @@ class HSTU(nn.Module):
         gets the head applied to a zero vector.  Inference only: bf16 precision, no dropout, no autograd.  CUDA-graph capturable
         after one eager call; the host-side capacity check does not run on replay, where items that do not fit are dropped and
         flagged (``state.overflowed()``)."""
-        if self.precision == "fp32":
-            raise RuntimeError("genrec_b200: extend runs the bf16 path only; set_precision('bf16') or use last_logits")
-        if self.training and any(isinstance(m, nn.Dropout) and m.p > 0 for m in self.modules()):
-            raise RuntimeError("genrec_b200: extend has no dropout; call model.eval()")
+        self._check_extend_mode("extend")
         require_cuda(input_ids)
         ensure_device(input_ids.device)
         B, n = input_ids.shape
@@ -440,23 +534,45 @@ class HSTU(nn.Module):
         if state.items_bound + n > state.capacity:
             raise ValueError(f"extending by {n} items could exceed the state's capacity ({state.items_bound} of {state.capacity} may be "
                              "used); start a new state with a larger capacity")
-        use_time = timestamps is not None and self.use_temporal_bias
-        versions = tuple(p._version for p in self.parameters())
-        if state.param_versions is None:
-            state.param_versions, state.has_time = versions, use_time
-        elif state.param_versions != versions:
-            raise RuntimeError("genrec_b200: the model's parameters changed after this state was written; rebuild the state")
-        elif state.has_time != use_time:
-            raise ValueError("timestamps must be given on every extend of a state or on none")
+        use_time = self._check_cache_owner(state, timestamps, "state")
         dev = input_ids.device
         ids = input_ids.contiguous()
         cache = state._struct()
         positions, last_row = Fn.hstu_cache_append(cache, ids, timestamps.contiguous() if timestamps is not None else None)
+        x = self._extend_blocks(ids, positions, cache, state.capacity, use_time)
+        latest = x[torch.arange(B, device=dev), last_row.clamp(min=0).long()]
+        state.last_hidden.copy_(torch.where((last_row >= 0)[:, None], latest, state.last_hidden))
+        state.items_bound += n
+        return self._hidden_logits(state.last_hidden)
+
+    def _check_extend_mode(self, what: str) -> None:
+        if self.precision == "fp32":
+            raise RuntimeError(f"genrec_b200: {what} runs the bf16 path only; set_precision('bf16') or use last_logits")
+        if self.training and any(isinstance(m, nn.Dropout) and m.p > 0 for m in self.modules()):
+            raise RuntimeError(f"genrec_b200: {what} has no dropout; call model.eval()")
+
+    def _check_cache_owner(self, cache, timestamps: Optional[torch.Tensor], what: str) -> bool:
+        """Ties a state / pool to the parameter versions and the timestamp mode of its first write; returns the timestamp mode."""
+        use_time = timestamps is not None and self.use_temporal_bias
+        versions = tuple(p._version for p in self.parameters())
+        if cache.param_versions is None:
+            cache.param_versions, cache.has_time = versions, use_time
+        elif cache.param_versions != versions:
+            raise RuntimeError(f"genrec_b200: the model's parameters changed after this {what} was written; rebuild the {what}")
+        elif cache.has_time != use_time:
+            raise ValueError(f"timestamps must be given on every extend of a {what} or on none")
+        return use_time
+
+    def _extend_blocks(self, ids: torch.Tensor, positions: torch.Tensor, cache, capacity: int, use_time: bool,
+                       users: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Embedding and every block of a chunk [B, n] against ``cache`` (a dense HstuCache, or an HstuPool with ``users``) -> the
+        final block's output [B, n, D] fp32."""
+        dev = ids.device
         x, _ = Fn.EmbedFn.apply(ids, self.item_embedding.weight, None, 1.0, 0, 0.0, 0, None, None)
         if len(self.layers):
             rpb = self.layers[0].position_bias
-            uniform, bucket0 = rpb.uniform_of(state.capacity, dev)
-            pos_bucket = None if uniform else rpb.bucket_of_delta(state.capacity, dev)
+            uniform, bucket0 = rpb.uniform_of(capacity, dev)
+            pos_bucket = None if uniform else rpb.bucket_of_delta(capacity, dev)
             ntime = self.layers[0].temporal_bias.num_buckets if use_time else 0
             for i, layer in enumerate(self.layers):
                 layer._bf16_provider = self._bf16_provider
@@ -464,12 +580,58 @@ class HSTU(nn.Module):
                          "ffn1_w": layer._mirror("ffn1_w", layer.ffn[0].weight),
                          "ffn2_w": layer._mirror("ffn2_w", layer.ffn[3].weight)}
                 x = Fn.hstu_layer_extend(x, cache, i, positions, pos_bucket, bucket0, _thresholds_on(dev), layer.num_heads, rpb.num_buckets,
-                                         ntime, bf16w, layer._params())
-        latest = x[torch.arange(B, device=dev), last_row.clamp(min=0).long()]
-        state.last_hidden.copy_(torch.where((last_row >= 0)[:, None], latest, state.last_hidden))
-        state.items_bound += n
-        return Fn.head_logits(state.last_hidden[:, None, :], self.final_norm.weight, self.final_norm.bias, self.item_embedding.weight,
+                                         ntime, bf16w, layer._params(), users=users)
+        return x
+
+    def _hidden_logits(self, hidden: torch.Tensor) -> torch.Tensor:
+        return Fn.head_logits(hidden[:, None, :], self.final_norm.weight, self.final_norm.bias, self.item_embedding.weight,
                               self._table_mirror(), self.final_norm.eps)[:, 0, :]
+
+    def new_pool(self, max_users: int, num_pages: int, page_size: int = 64, max_items: int = 2048) -> HSTUPool:
+        """An empty paged cache for serving: ``num_pages`` pages of ``page_size`` items (a multiple of 64) shared by users
+        0 .. max_users-1, each holding up to ``max_items`` (<= 16384) items, on the model's device."""
+        return HSTUPool(max_users, num_pages, page_size, max_items, len(self.layers), self.embed_dim, self.item_embedding.weight.device)
+
+    @torch.no_grad()
+    def extend_users(self, pool: HSTUPool, users, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``extend`` for the users named by ``users`` [B] (int64, distinct, any subset of the pool's users in any order): append the
+        non-zero ids of row b of ``input_ids`` [B, n] to the history of user ``users[b]`` in ``pool`` and return [B, V+1] fp32, row b
+        being that user's next-item logits - what ``extend`` returns for the same user, i.e. ``last_logits`` of the left-padded
+        concatenation of every item extended for them since their last ``pool.release``.  An all-pad row leaves its user untouched
+        and returns their previous logits.
+
+        With ``users`` on the CPU the call is refused before any launch if a user is out of range or repeated, or if the host
+        bounds say a user could exceed ``max_items`` or the pool could run out of pages.  With ``users`` on the device (CUDA graphs)
+        those checks are skipped: a row whose user is out of range or repeats an earlier row's counts as all padding (its logits are
+        the head of a zero vector) and sets ``pool.errors()``, and items beyond ``max_items`` or without a free page are dropped in
+        row order and flag their user in ``pool.overflowed()``."""
+        self._check_extend_mode("extend_users")
+        require_cuda(input_ids)
+        ensure_device(input_ids.device)
+        dev = input_ids.device
+        if input_ids.dim() != 2 or input_ids.device != pool.lengths.device:
+            raise ValueError(f"input_ids must be [B, n] on {pool.lengths.device}; got {tuple(input_ids.shape)} on {input_ids.device}")
+        B, n = input_ids.shape
+        users = torch.as_tensor(users, dtype=torch.int64) if not isinstance(users, torch.Tensor) else users
+        if users.shape != (B,):
+            raise ValueError(f"users must have one entry per row of input_ids ({B}), got shape {tuple(users.shape)}")
+        bound = None
+        if not users.is_cuda:
+            u_host = pool._host_users(users)
+            bound = pool._check_room(u_host, n)
+        use_time = self._check_cache_owner(pool, timestamps, "pool")
+        users = users.to(dev).long()
+        ids = input_ids.contiguous()
+        cache = pool._struct()
+        positions, last_row, room = Fn.hstu_pool_append(cache, users, ids, timestamps.contiguous() if timestamps is not None else None)
+        x = self._extend_blocks(ids, positions, cache, pool.max_items, use_time, users=users)
+        latest = x[torch.arange(B, device=dev), last_row.clamp(min=0).long()]
+        slot = torch.where(room >= 0, users, pool.max_users)     # rejected rows read and write the spare zero row
+        hidden = torch.where((last_row >= 0)[:, None], latest, pool.last_hidden[slot])
+        pool.last_hidden[slot] = hidden
+        if bound is not None:
+            pool.items_bound[u_host], pool.pages_bound = bound
+        return self._hidden_logits(hidden)
 
     @torch.no_grad()
     def evaluate_batch(self, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor], targets: torch.Tensor,

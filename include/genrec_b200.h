@@ -158,6 +158,46 @@ int grb_hstu_layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p
                           const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr,
                           const float* x, float* y, void* workspace, void* stream);
 
+/* Paged pool: the K | V rows of many users share one pool of pages, each user has a page table, and any set of distinct users
+ * can be extended in one call, so memory follows the items actually cached rather than a per-user capacity.  Item p of user u
+ * lives in page page_table[u, p / page_size] at row p % page_size.  The dense grb_hstu_cache is the pool with
+ * page_size = capacity whose page b belongs to user b; both run on the same kernels.
+ * Initial state: lengths, overflow and errors 0, free_stack = any permutation of 0 .. num_pages-1 (the next page handed out is
+ * free_stack[*free_top - 1]), *free_top = num_pages, row_of filled with INT32_MAX (the allocation kernels leave it so). */
+typedef struct {
+    int max_users, num_layers;
+    int page_size;               /* items per page: a positive multiple of 64 */
+    int num_pages;
+    int max_items;               /* most items one user can hold, <= 16384 */
+    void* kv;                    /* bf16 [num_layers, num_pages, page_size, 2D] */
+    int64_t* timestamps;         /* [num_pages, page_size] */
+    int32_t* page_table;         /* [max_users, ceil(max_items / page_size)] */
+    int32_t* lengths;            /* [max_users] items cached per user */
+    uint8_t* overflow;           /* [max_users] 1 when an item of the user was dropped (no room within max_items or no free page) */
+    int32_t* free_stack;         /* [num_pages] */
+    int32_t* free_top;           /* [1] number of free pages */
+    uint32_t* errors;            /* [1] bit 0: a row named a user outside [0, max_users); bit 1: a row repeated an earlier row's user */
+    int32_t* row_of;             /* [max_users] scratch of the allocation kernels */
+} grb_hstu_pool;
+/* One call per chunk, before the layers: users [B] int64, input_ids / timestamps [B, n] as in grb_hstu_cache_append.  One CTA
+ * validates the users (a row whose user is out of range or repeats an earlier row's is treated as all padding and sets a bit
+ * of *errors), then hands out the pages the rows' new items need from the free stack, in row order; items beyond max_items or
+ * without a page are dropped and flag their user in overflow.  Outputs as grb_hstu_cache_append, plus room [B] int32: the items
+ * the row's user may hold after the allocation, -1 for a rejected row. */
+int grb_hstu_pool_append(const grb_hstu_pool* pool, const int64_t* users, int B, const int64_t* input_ids, const int64_t* timestamps,
+                         int n, int32_t* positions, int32_t* last_row, int32_t* room, void* stream);
+/* Forgets users [B]: their pages go back onto the free stack (row order, then page order), their length and overflow flag become
+ * 0, and so do their rows of last_hidden [max_users, D] fp32 (nullable; a caller-side buffer of per-user state).  Rows are
+ * validated as in grb_hstu_pool_append. */
+int grb_hstu_pool_release(const grb_hstu_pool* pool, const int64_t* users, int B, float* last_hidden, int D, void* stream);
+/* grb_hstu_layer_extend on a pool: d->B = the call's rows, users [B] and positions [B, n] as given to / returned by
+ * grb_hstu_pool_append; pos_bucket [max_items] or NULL.  The key split is a function of d and max_items only, so a captured graph
+ * stays valid while lengths and page tables change on the device. */
+size_t grb_hstu_layer_extend_paged_workspace_bytes(const grb_hstu_dims* d, const grb_hstu_pool* pool);
+int grb_hstu_layer_extend_paged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_pool* pool, int layer,
+                                const int64_t* users, const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0,
+                                const int64_t* time_thr, const float* x, float* y, void* workspace, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ input pipeline
  * Device-side hstu_collate_fn / sasrec_collate_fn (genrec/data/amazon_hstu.py:137-173, genrec/data/amazon_sasrec.py:125-161): a
  * jagged batch (items / stamps [N] in time order, offsets [B+1], one held-out target per user) -> the LEFT-padded [B, L]

@@ -114,6 +114,75 @@ def bench_extend(dev):
             assert torch.isfinite(one()).all()
 
 
+def bench_pool(dev):
+    """Serving from the paged pool (HSTU.extend_users): a pool of many users with seeded history lengths, one new item for a random
+    subset of them, next to the dense HSTUState extend of the same users (cfg2) and last_logits on their left-padded histories.
+    Graph-captured with the users as a device tensor.  Every length is a non-multiple of the page size, so the timed item never
+    takes a page, and the lengths are rewound on the device before every call (one small kernel inside the timed graph).  The
+    allocation kernel and the chunk-attention kernel are timed on their own with torch.profiler."""
+    from genrec_b200.hstu import HSTU
+    info = card()
+    HBM = 3.35e12
+    geoms = (("cfg2", dict(num_items=12101, embed_dim=128, num_heads=4, num_blocks=4), 4096, 200, 128, True),
+             ("cfg3", dict(num_items=12101, embed_dim=256, num_heads=8, num_blocks=8), 512, 2048, 32, False))
+    for name, geo, nusers, cap, B, dense in geoms:
+        g = torch.Generator().manual_seed(1)
+        torch.manual_seed(0)
+        m = HSTU(max_seq_len=cap, dropout=0.0, **geo).to(dev).eval()
+        D, NB, ps = geo["embed_dim"], geo["num_blocks"], 64
+        lens = torch.randint(1, cap, (nusers,), generator=g)
+        lens[lens % ps == 0] -= 1                                  # the timed item stays inside the user's last page
+        pool = m.new_pool(max_users=nusers, num_pages=int(((lens + ps) // ps).sum()), page_size=ps, max_items=cap)
+        hist = torch.randint(1, geo["num_items"] + 1, (nusers, cap), generator=g)
+        hts = 1_300_000_000 + torch.cumsum(torch.randint(1, 3 * 86400, (nusers, cap), generator=g), 1)
+        pad = torch.arange(cap)[None, :] < (cap - 1 - lens)[:, None]   # user u: lens[u] items, then the timed one in column cap-1
+        hist[pad] = 0
+        hts[pad] = 0
+        chunk = 128 if name == "cfg2" else 16
+        for u0 in range(0, nusers, chunk):                         # device users: pages follow the real lengths, not the host bound
+            us = torch.arange(u0, min(u0 + chunk, nusers))
+            m.extend_users(pool, us.to(dev), hist[us, :-1].to(dev), hts[us, :-1].to(dev))
+        assert not pool.overflowed().any()
+        users = torch.randperm(nusers, generator=g)[:B]
+        users_dev = users.to(dev)
+        ulens = lens[users].to(dev, torch.int32)
+        ids1, ts1 = hist[users, -1:].to(dev), hts[users, -1:].to(dev)
+
+        def one():
+            pool.lengths.index_copy_(0, users_dev, ulens)
+            return m.extend_users(pool, users_dev, ids1, ts1)
+
+        ms = graph_timed(one)
+        hist_u, hts_u = hist[users].to(dev), hts[users].to(dev)
+        full_ms = graph_timed(lambda: m.last_logits(hist_u, hts_u))
+        attn_us = kernel_us(one, "hstu_attn_extend_kernel")
+        alloc_us = kernel_us(one, "hstu_pool_alloc_kernel")
+        item = NB * 2 * D * 2 + 8                                   # cached bytes per item: K | V of every block + timestamp
+        byt = int((lens[users] + 1).sum()) * (2 * D * 2 + 8)        # per layer: the keys the attention reads
+        pages = int(((lens[users] + ps) // ps).sum())
+        row = dict(kernel="hstu_pool_extend", geometry=name, workload="extend_1", pool_users=nusers, B=B, page_size=ps, max_items=cap,
+                   mean_history=float(lens[users].float().mean()), extend_users_us=ms * 1e3, last_logits_us=full_ms * 1e3,
+                   attn_kernel_us=attn_us, alloc_kernel_us=alloc_us, attn_bytes_per_layer=byt, attn_hbm_gbs=byt / attn_us / 1e3,
+                   attn_frac_of_hbm_peak=byt / (attn_us * 1e-6) / HBM, pool_bytes_of_users=pages * ps * item,
+                   dense_bytes_of_users=B * cap * item, blocks=NB, **info)
+        if dense:
+            st = m.new_state(B, cap)
+            m.extend(st, hist[users, :-1].to(dev), hts[users, :-1].to(dev))
+
+            def dense_one():
+                st.lengths.copy_(ulens)
+                st.items_bound = cap - 1
+                return m.extend(st, ids1, ts1)
+
+            dense_ms = graph_timed(dense_one)
+            assert torch.equal(one(), dense_one())                 # same users, same items: the same bits
+            row.update(dense_extend_us=dense_ms * 1e3, pool_over_dense=ms / dense_ms,
+                       dense_attn_kernel_us=kernel_us(dense_one, "hstu_attn_extend_kernel"))
+        print(json.dumps(row), flush=True)
+        del pool
+        torch.cuda.empty_cache()
+
+
 def main():
     dev = torch.device("cuda:0")
     peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) \
@@ -155,6 +224,7 @@ def main():
                               algorithmic_tflops=flops / ms / 1e9, frac_of_bf16_peak=flops / ms / 1e9 / peak,
                               note="eager launches (not graph-captured): includes host launch gaps at L=200")))
     bench_extend(dev)
+    bench_pool(dev)
 
 
 if __name__ == "__main__":
