@@ -254,9 +254,9 @@ HstuBiasArgs make_attn_bias(const grb_hstu_dims* d, const float* pos_table, cons
     b.bias_index = s->bias_index;
     b.ldix = s->ld_index;
     b.pos_uniform = s->pos_uniform;
-    b.pos_bucket0 = 0;
     b.npos = s->pos_uniform ? 1 : d->npos;
     b.ntime = has_time ? d->ntime : 0;
+    b.time_bins = att_time_bins(has_time, s->pos_uniform != 0, b.ntime);
     return b;
 }
 // P: [T, 4D] bf16 U | V | Q | K ; O: [T, D] bf16 output, written by the forward only
@@ -353,8 +353,9 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
         GRB_CUDA(cudaGetLastError());
         return 0;
     }));
-    size_t smem_k = sizeof(AttSmemKV<DH>) + posb + (size_t)4 * (a.bias.ntime + 1 + (a.bias.pos_uniform ? 0 : a.bias.npos + 1)) * 32 * sizeof(float);
     const bool has_time = a.bias.wtime != nullptr && a.bias.ntime > 0, pos_uni = a.bias.pos_uniform != 0;
+    size_t smem_k = sizeof(AttSmemKV<DH>) + posb +
+                    (size_t)4 * (att_time_bins(has_time, pos_uni, a.bias.ntime) + (pos_uni ? 0 : a.bias.npos + 1)) * 32 * sizeof(float);
     const int nmem = (int)(grid.x * grid.z), ngroups = has_time && a.dwtime ? 2 * a.H : a.H;
     GRB_REQUIRE((pos_uni || a.bias.npos <= 64) && a.bias.ntime <= 64, "attention backward: at most 64 position / time buckets");
     auto go = [&](auto kern) -> int {
@@ -366,8 +367,9 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
     else if (has_time) GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, true, false>));
     else if (pos_uni) GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, false, true>));
     else GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, false, false>));
-    // groups h < H: position buckets of head h ; H + h: time buckets of head h ; element = bucket
-    float* pos_out = a.dwpos + (pos_uni ? (size_t)a.bias.pos_bucket0 * a.H : 0);
+    // groups h < H: position buckets of head h ; H + h: time buckets of head h ; element = bucket.  With uniform positions
+    // the caller has already pointed dwpos at the single live row.
+    float* pos_out = a.dwpos;
     const int pos_len = pos_uni ? a.H : a.bias.npos * a.H;
     if (ngroups > a.H) GRB_TRY(det_finish(a.dw_part, ngroups, nmem, 64, a.H, 1, a.H, {{pos_out, pos_len}, {a.dwtime, a.bias.ntime * a.H}}, st));
     else GRB_TRY(det_finish(a.dw_part, ngroups, nmem, 64, a.H, 1, a.H, {{pos_out, pos_len}}, st));

@@ -41,8 +41,9 @@ struct HstuBiasArgs {
     const uint16_t* bias_index;  // [B, L, ldix]
     int ldix;                    // elements, multiple of 8
     int npos, ntime;
-    int pos_uniform;             // 1: every delta in [0, L) maps to pos bucket `pos_bucket0` (the reference's degenerate case)
-    int pos_bucket0;
+    int pos_uniform;             // 1: every delta in [0, L) maps to one position bucket (the reference's degenerate case); wpos
+                                 //    then points at that bucket's row and the index matrix is built with npos = 1
+    int time_bins;               // att_time_bins(): the dK/dV kernel's time-histogram bins per warp
 };
 
 struct HstuAttnArgs {
@@ -417,7 +418,7 @@ __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 4 : 2) hstu_attn_bwd_d
 // ============================================================================================ backward: dK, dV, bias tables
 // CTA owns 64 keys: fixed = {K, V} ; stream[buf] = {Q, dO}
 // K and V are only needed as register fragments, so they are staged through stream buffer 1 before the main loop.
-// dynamic smem tail: wcomb[npos*64+1] (padded to 16 B) then LANE-PRIVATE histograms hist_t[4][ntime+1][32], hist_p[4][npos+1][32]
+// dynamic smem tail: wcomb[npos*64+1] (padded to 16 B) then LANE-PRIVATE histograms hist_t[4][nt_bins][32], hist_p[4][npos+1][32]
 // (each lane owns one 4-byte column: plain read-modify-write, bank-conflict free, no atomics; hist_p only when the
 // position buckets are not uniform)
 template <int DH>
@@ -426,6 +427,14 @@ struct AttSmemKV {
     bf16 stream[2][2][ATT_BLK * LD];
     uint16_t ix[2][ATT_BLK * ATT_IX_LD];
 };
+// Time-histogram bins per warp: one past the largest bin a cell can index (masked cells carry dS == 0 but still index a bin).
+// Uniform positions: the bin is the whole index, a time bucket < ntime or the sentinel 1 * 64, so 65 bins whatever ntime is.
+// Per-bucket positions: the bin is (index & 63), a time bucket < ntime or 0 on a masked cell; ntime + 1 keeps a spare.
+// The host sizes the shared memory with it; the uniform kernels read it from HstuBiasArgs::time_bins (a compile-time 65 there
+// changes their register allocation and makes them spill).
+inline int att_time_bins(bool has_time, bool pos_uniform, int ntime) {
+    return has_time && pos_uniform ? ATT_MAX_BUCKETS + 1 : ntime + 1;
+}
 // HAS_TIME / POS_UNI are compile-time so that the per-cell histogram code carries no branches
 template <int DH, bool HAS_TIME, bool POS_UNI>
 __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 3 : 2) hstu_attn_bwd_dkdv_kernel(HstuAttnArgs a, int table_bytes) {
@@ -435,7 +444,7 @@ __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 3 : 2) hstu_attn_bwd_d
     float* wcomb = reinterpret_cast<float*>(att_smem_raw + sizeof(AttSmemKV<DH>));
     float* hist_t = reinterpret_cast<float*>(att_smem_raw + sizeof(AttSmemKV<DH>) + table_bytes);
     const int ntime = a.bias.ntime, npos = a.bias.npos;
-    const int nt_bins = ntime + 1;   // + one spare bin: masked cells of the uniform-position layout index it with an exact 0
+    const int nt_bins = POS_UNI ? a.bias.time_bins : ntime + 1;
     float* hist_p = hist_t + 4 * nt_bins * 32;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int kt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;

@@ -39,12 +39,13 @@ def time_bucket_thresholds() -> torch.Tensor:
 
     Derived by bisection on the reference fp32 expression itself (monotone), evaluated with torch on the CPU, so the
     kernel's integer compare ``|dt| >= thr[k]`` reproduces ``trunc(log_f32(float(|dt|)) / 0.693)`` bit-exactly,
-    including the places where 0.693 != ln 2 moves a boundary (|dt| = 1023 -> bucket 10).
+    including the places where 0.693 != ln 2 moves a boundary (|dt| = 1023 -> bucket 10).  The search runs up to INT64_MAX:
+    bucket 63 starts at |dt| ~ 9.14e18, above 2^62.
     """
     big = 1 << 20
     thr = [0] * 65
     for k in range(1, 64):
-        lo, hi = 1, 1 << 62
+        lo, hi = 1, INT64_MAX
         if int(_temporal_bucket_ref(torch.tensor([hi]), big)) < k:
             thr[k] = INT64_MAX
             continue

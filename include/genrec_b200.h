@@ -41,7 +41,7 @@ int grb_check_device(int ordinal);
  * Replaces HSTULayer.forward (genrec/models/hstu.py:222-280) incl. RelativePositionBias.forward (:330-349) and
  * TemporalBias.forward (:386-409), and their autograd backward. */
 typedef struct {
-    int B, L, D, H;          /* head_dim = D / H must be 32 (16 and 64 also compiled) ; D in {64,128,256} */
+    int B, L, D, H;          /* head_dim = D / H must be 32 or 64 ; D in {64,128,256} */
     int npos, ntime;         /* bucket counts of the two bias tables, each <= 64 ; ntime = 0 disables the temporal term */
     float dropout_p;         /* 0 in eval mode */
     uint64_t seed;           /* dropout stream ; the mask is a pure function of (seed, layer_index, site, element) */

@@ -166,7 +166,7 @@ def time_bucket_thresholds(num_buckets: int = 64) -> torch.Tensor:
     """
     thr = torch.empty(num_buckets, dtype=torch.int64)
     thr[0] = 0
-    hi_cap = (1 << 62)
+    hi_cap = torch.iinfo(torch.int64).max      # bucket 63 starts at |dt| ~ 9.14e18, above 2^62
     for k in range(1, num_buckets):
         lo, hi = 1, hi_cap
         if int(temporal_bucket(torch.tensor([hi]), 1 << 20)) < k:
