@@ -140,6 +140,9 @@ SIGNATURES = {
                                  c_void_p]),
     "grb_rq_residual_argmin": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
                                        c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_rq_sinkhorn_workspace_bytes": (c_size_t, [c_i64, c_int]),
+    "grb_rq_sinkhorn": (c_int, [c_void_p, c_i64, c_int, C.c_double, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_kmeans_update": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib: Optional[C.CDLL] = None

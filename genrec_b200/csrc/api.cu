@@ -21,6 +21,7 @@
 #include "exact_f32.cuh"
 #include "rowwise.cuh"
 #include "rq_argmin.cuh"
+#include "rq_sinkhorn.cuh"
 #include "tc_gemm.cuh"
 #include "tc_ce.cuh"
 #include "tc_tn_group.cuh"
@@ -1576,6 +1577,88 @@ int grb_rq_residual_argmin(const float* x, const float* codebooks, int64_t N, in
         GRB_TRY(set_smem(rq_residual_argmin_kernel<64, 1>, smem));
         launch_k(rq_residual_argmin_kernel<64, 1>, grid, RQ_THREADS, smem, st, a);
     }
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ RQ-VAE training: Sinkhorn, k-means
+namespace {
+size_t sk_workspace(int64_t B, int K) {
+    return align_up((size_t)B * sizeof(double)) + (sk_kmat_in_smem(B, K) ? 0 : align_up((size_t)B * K * sizeof(double)));
+}
+// once per device: both instantiations may use the full opt-in shared memory and the non-portable cluster size, and one cluster of
+// SK_CLUSTER such CTAs must fit the device
+int sk_prepare() {
+    static std::mutex mu;
+    static bool ready[64] = {false};
+    std::lock_guard<std::mutex> lock(mu);
+    const int dev = current_device() & 63;
+    if (ready[dev]) return 0;
+    for (auto kern : {rq_sinkhorn_kernel<true>, rq_sinkhorn_kernel<false>}) {
+        GRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+        GRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SK_SMEM_MAX));
+        cudaLaunchConfig_t cfg;
+        memset(&cfg, 0, sizeof(cfg));
+        cfg.gridDim = dim3(SK_CLUSTER);
+        cfg.blockDim = dim3(SK_THREADS);
+        cfg.dynamicSmemBytes = SK_SMEM_MAX;
+        cudaLaunchAttribute at;
+        at.id = cudaLaunchAttributeClusterDimension;
+        at.val.clusterDim.x = SK_CLUSTER;
+        at.val.clusterDim.y = 1;
+        at.val.clusterDim.z = 1;
+        cfg.attrs = &at;
+        cfg.numAttrs = 1;
+        int n = 0;
+        GRB_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
+        if (n < 1) return fail(GRB_ENODEV, "rq_sinkhorn: a cluster of %d CTAs x %d threads with %zu B of shared memory does not fit this device",
+                               SK_CLUSTER, SK_THREADS, SK_SMEM_MAX);
+    }
+    ready[dev] = true;
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+size_t grb_rq_sinkhorn_workspace_bytes(int64_t B, int K) {
+    if (B < 0 || K < 2 || K > SK_KMAX) {
+        fail(GRB_EINVAL, "rq_sinkhorn: B=%lld K=%d unsupported (B >= 0, 2 <= K <= %d)", (long long)B, K, SK_KMAX);
+        return 0;
+    }
+    return sk_workspace(B, K);
+}
+
+int grb_rq_sinkhorn(const float* dist, int64_t B, int K, double eps, int iters, int64_t* ids, double* u_out, double* v_out,
+                    void* workspace, void* stream) {
+    GRB_REQUIRE(B >= 0 && K >= 2 && K <= SK_KMAX, "rq_sinkhorn: B=%lld K=%d unsupported (B >= 0, 2 <= K <= %d)", (long long)B, K, SK_KMAX);
+    GRB_REQUIRE(iters >= 0 && eps > 0.0 && eps < INFINITY, "rq_sinkhorn: iters=%d eps=%g unsupported (iters >= 0, eps > 0 finite)", iters, eps);
+    if (B == 0) return 0;
+    GRB_REQUIRE(dist && ids && workspace, "rq_sinkhorn: null argument (dist, ids and workspace are required)");
+    GRB_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "rq_sinkhorn: workspace must be 8-byte aligned");
+    GRB_TRY(sk_prepare());
+    const bool in_smem = sk_kmat_in_smem(B, K);
+    const size_t rows = sk_rows_per_cta(B);
+    double* u = static_cast<double*>(workspace);
+    double* kmat = in_smem ? nullptr : reinterpret_cast<double*>(static_cast<char*>(workspace) + align_up((size_t)B * sizeof(double)));
+    SinkhornArgs a{dist, (long long)B, K, iters, (int)rows, eps, reinterpret_cast<long long*>(ids), u_out, v_out, u, kmat};
+    const size_t smem = SK_SMEM_FIXED + (in_smem ? rows * K * sizeof(double) : 0);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (in_smem) launch_kc(rq_sinkhorn_kernel<true>, SK_CLUSTER, SK_THREADS, SK_CLUSTER, smem, st, a);
+    else launch_kc(rq_sinkhorn_kernel<false>, SK_CLUSTER, SK_THREADS, SK_CLUSTER, smem, st, a);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int grb_kmeans_update(const float* x, const int64_t* assign, int64_t B, int D, int k, float* centroids, int32_t* counts, float* shift,
+                      void* stream) {
+    GRB_REQUIRE(B >= 0 && k >= 1 && k <= (1 << 20) && D >= 1 && D <= KM_THREADS,
+                "kmeans_update: B=%lld D=%d k=%d unsupported (B >= 0, 1 <= D <= %d, 1 <= k <= 2^20)", (long long)B, D, k, KM_THREADS);
+    GRB_REQUIRE(x && assign && centroids && counts && shift, "kmeans_update: null argument");
+    launch_k(kmeans_update_kernel, (unsigned)k, KM_THREADS, 0, static_cast<cudaStream_t>(stream), x, reinterpret_cast<const long long*>(assign),
+             (long long)B, D, centroids, counts, shift);
     GRB_CUDA(cudaGetLastError());
     return 0;
 }

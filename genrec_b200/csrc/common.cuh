@@ -40,22 +40,38 @@ inline unsigned long long& launch_counter() {
     static unsigned long long n = 0;
     return n;
 }
-// launch_k(kernel, grid, block, smem, st, args...) with the PDL attribute (GRB_PDL=0 turns it off).
+// launch_kc(kernel, grid, block, cluster, smem, st, args...) with the PDL attribute (GRB_PDL=0 turns it off) and, for cluster > 1, a
+// thread-block cluster of `cluster` CTAs along x; launch_k is the same without clusters.
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+inline cudaError_t launch_kc(void (*kern)(KArgs...), dim3 grid, dim3 block, unsigned cluster, size_t smem, cudaStream_t st, Args&&... args) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchAttribute at[2];
+    unsigned n = 0;
+    if (pdl_enabled()) {
+        at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        at[n].val.programmaticStreamSerializationAllowed = 1;
+        ++n;
+    }
+    if (cluster > 1) {
+        at[n].id = cudaLaunchAttributeClusterDimension;
+        at[n].val.clusterDim.x = cluster;
+        at[n].val.clusterDim.y = 1;
+        at[n].val.clusterDim.z = 1;
+        ++n;
+    }
     cfg.attrs = at;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = n;
     ++launch_counter();
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+}
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+    return launch_kc(kern, grid, block, 1u, smem, st, static_cast<Args&&>(args)...);
 }
 
 // ----------------------------------------------------------------------------- small math

@@ -603,6 +603,43 @@ def rq_residual_argmin(x: torch.Tensor, codebooks: torch.Tensor, commitment: flo
     return ids, emb, res, loss
 
 
+def rq_sinkhorn(dist: torch.Tensor, eps: float = 0.003, iters: int = 100):
+    """Sinkhorn-Knopp hard assignment of the SINKHORN estimator (csrc/rq_sinkhorn.cuh): dist [B, K] fp32, 2 <= K <= 256 ->
+    ids [B] int64, u [B] and v [K] fp64 (the final scalings; P = u K v)."""
+    lib = _lib.load()
+    require_cuda(dist)
+    require_f32(dist)
+    if dist.dim() != 2:
+        raise _lib.GrbError(f"genrec_b200 error -1: dist must be [B, K] (got {tuple(dist.shape)})")
+    dist = dist.detach().contiguous()
+    B, K = dist.shape
+    ids = torch.empty(B, dtype=torch.int64, device=dist.device)
+    u = torch.empty(B, dtype=torch.float64, device=dist.device)
+    v = torch.empty(K, dtype=torch.float64, device=dist.device)
+    ws = _u8(lib.grb_rq_sinkhorn_workspace_bytes(B, K), dist.device)
+    with torch.cuda.device(dist.device):
+        check(lib.grb_rq_sinkhorn(ptr(dist), B, K, float(eps), int(iters), ptr(ids), ptr(u), ptr(v), ptr(ws), stream_ptr(dist.device)))
+    return ids, u, v
+
+
+def kmeans_update(x: torch.Tensor, assign: torch.Tensor, centroids: torch.Tensor) -> torch.Tensor:
+    """One Lloyd update after the assignment (csrc/rq_sinkhorn.cuh kmeans_update_kernel): every non-empty cluster's centroid becomes
+    the mean of its rows, in place.  Returns [2, k] int32: row 0 the cluster sizes, row 1 the centroid shifts (fp32 bits)."""
+    require_cuda(x, assign, centroids)
+    require_f32(x, centroids)
+    require_i64(assign)
+    if not centroids.is_contiguous():
+        raise _lib.GrbError("genrec_b200 error -1: centroids must be contiguous (updated in place)")
+    x = x.detach().contiguous()
+    B, D = x.shape
+    k = centroids.shape[0]
+    stats = torch.empty(2, k, dtype=torch.int32, device=x.device)
+    with torch.cuda.device(x.device):
+        check(_lib.load().grb_kmeans_update(ptr(x), ptr(assign.contiguous()), B, D, k, ptr(centroids), ptr(stats[0]), ptr(stats[1]),
+                                            stream_ptr(x.device)))
+    return stats
+
+
 def split3(x: torch.Tensor, operand: int) -> torch.Tensor:
     """fp32 [rows, K] -> bf16 [rows, 6K]: the three-term bf16 split of every value, laid out along K for the fp32-accurate GEMM
     (operand 0 = activation layout, 1 = weight layout; csrc/rowwise.cuh split3_f32_bf16_kernel)."""

@@ -242,6 +242,18 @@ def _(x, codebooks, commitment):
             x.new_empty((N,), dtype=torch.float32))
 
 
+@custom_op(f"{NS}::rq_sinkhorn", mutates_args=())
+def rq_sinkhorn(dist: Tensor, eps: float, iters: int) -> Tuple[Tensor, Tensor, Tensor]:
+    """dist [B, K] fp32 -> Sinkhorn-Knopp hard ids [B] int64 and the final scalings u [B], v [K] fp64 (rqvae.py:85-110, :218-241)."""
+    return Fn.rq_sinkhorn(dist, eps, iters)
+
+
+@rq_sinkhorn.register_fake
+def _(dist, eps, iters):
+    B, K = dist.shape
+    return dist.new_empty((B,), dtype=torch.int64), dist.new_empty((B,), dtype=torch.float64), dist.new_empty((K,), dtype=torch.float64)
+
+
 @custom_op(f"{NS}::eval_rank_metrics", mutates_args=())
 def eval_rank_metrics(logits_last: Tensor, targets: Tensor) -> Tensor:
     """[B, C] fp32 logits of the last position, targets [B] -> [6] fp32: Recall@{1,5,10} hit counts, NDCG@{1,5,10} sums."""
@@ -298,4 +310,4 @@ torch.library.register_autograd(f"{NS}::sasrec_attention", _sas_backward, setup_
 
 
 OPS = ("hstu_seq_prepare", "hstu_attention", "hstu_attention_backward", "hstu_layer", "hstu_layer_backward", "rq_residual_argmin",
-       "eval_rank_metrics", "sasrec_attention", "sasrec_attention_backward")
+       "rq_sinkhorn", "eval_rank_metrics", "sasrec_attention", "sasrec_attention_backward")

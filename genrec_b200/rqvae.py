@@ -1,17 +1,23 @@
-"""Drop-in mirror of the RQ-VAE semantic-id path of ``genrec.models.rqvae`` (reference: genrec/models/rqvae.py).
+"""Drop-in mirror of ``genrec.models.rqvae`` (reference: genrec/models/rqvae.py): semantic ids and training.
 
-In scope (SURVEY.md section 8 rows a10/a11): ``Quantize.forward`` in eval mode (distance + first-min argmin + codebook
-gather + quantize loss, rqvae.py:185-199, :246-254) and the residual loop of ``RqVae.get_semantic_ids`` (:386-412), both
-executed by ONE launch of the sm_90a kernel ``rq_residual_argmin`` (csrc/rq_argmin.cuh) for all levels.
-Out of scope (raise): training-mode estimators (Gumbel / STE / rotation trick / Sinkhorn), k-means init, the decoder and
-the reconstruction losses.  The bias-free SiLU MLP encoder in front of the argmin (encoder.py:380-420, "next" row f3) runs
-on cuBLAS through ``torch.nn.functional.linear``.
+Semantic ids (SURVEY.md section 8 rows a10/a11): ``Quantize.forward`` in eval mode (distance + first-min argmin + codebook gather +
+quantize loss, rqvae.py:185-199, :246-254) and the residual loop of ``RqVae.get_semantic_ids`` (:386-412), both executed by ONE launch of
+the sm_90a kernel ``rq_residual_argmin`` (csrc/rq_argmin.cuh) for all levels.
+
+Training (row f3): ``RqVae.forward(batch, gumbel_t)`` returns the reference's ``RqVaeComputedLosses`` (rqvae.py:414-454) in train and
+eval mode.  The SINKHORN estimator's 100 fp64 Sinkhorn-Knopp iterations and its hard assignment are one launch of ``rq_sinkhorn``
+(csrc/rq_sinkhorn.cuh); the k-means codebook initialisation (modules/kmeans.py) runs on the device, with the Lloyd update in
+``kmeans_update_kernel`` and the assignment in ``rq_residual_argmin``.  STE, ROTATION_TRICK and GUMBEL_SOFTMAX keep the reference's
+element-wise formulas around the kernel's nearest-code search, and the bias-free SiLU MLP encoder / decoder (encoder.py:380-420) train on
+torch's fp32 cuBLAS GEMMs.
+Out of scope (raise): fusing the GUMBEL_SOFTMAX estimator, cosine distance, ``sim_vq`` and ``codebook_normalize``.
 """
 from __future__ import annotations
 
 from enum import Enum
 from typing import List, NamedTuple
 
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -45,20 +51,40 @@ class RqVaeOutput(NamedTuple):
     quantize_loss: torch.Tensor
 
 
+class RqVaeComputedLosses(NamedTuple):
+    loss: torch.Tensor
+    reconstruction_loss: torch.Tensor
+    rqvae_loss: torch.Tensor
+    embs_norm: torch.Tensor
+    p_unique_ids: torch.Tensor
+
+
+class L2Norm(nn.Module):
+    """genrec/modules/normalize.py:10-33: F.normalize(x, p=2, dim, eps); no parameters."""
+
+    def __init__(self, dim: int = -1, eps: float = 1e-12) -> None:
+        super().__init__()
+        self.dim, self.eps = dim, eps
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return F.normalize(x, p=2, dim=self.dim, eps=self.eps)
+
+
 class MLP(nn.Module):
-    """Mirror of genrec/modules/encoder.py:380-420 (bias-free Linear + SiLU stack; keys ``mlp.{0,2,4,...}.weight``)."""
+    """Mirror of genrec/modules/encoder.py:380-420 (bias-free Linear + SiLU stack, then L2Norm or Identity; keys
+    ``mlp.{0,2,4,...}.weight``)."""
 
     def __init__(self, input_dim: int, hidden_dims: List[int], out_dim: int, dropout: float = 0.0, normalize: bool = False):
         super().__init__()
-        assert dropout == 0.0 and not normalize, "only the configuration shipped by the reference configs is mirrored"
-        self.input_dim, self.hidden_dims, self.out_dim = input_dim, hidden_dims, out_dim
+        assert dropout == 0.0, "only the configuration shipped by the reference configs is mirrored"
+        self.input_dim, self.hidden_dims, self.out_dim, self.normalize = input_dim, hidden_dims, out_dim, normalize
         dims = [input_dim] + list(hidden_dims) + [out_dim]
         self.mlp = nn.Sequential()
         for i, (a, b) in enumerate(zip(dims[:-1], dims[1:])):
             self.mlp.append(nn.Linear(a, b, bias=False))
             if i != len(dims) - 2:
                 self.mlp.append(nn.SiLU())
-        self.mlp.append(nn.Identity())
+        self.mlp.append(L2Norm() if normalize else nn.Identity())
 
     def _split_weights(self):
         """bf16 three-term splits of the layer weights (weight layout of the fp32-accurate GEMM), cached per parameter version."""
@@ -78,8 +104,61 @@ class MLP(nn.Module):
             h = x.detach().float().contiguous()
             for i, w in enumerate(ws):
                 h = Fn.linear_f32x3(Fn.split3(h, 0), w, act=1 if i != len(ws) - 1 else 0)
-            return h
+            return F.normalize(h, p=2, dim=-1, eps=1e-12) if self.normalize else h
         return self.mlp(x)     # training of the encoder (autograd) stays on the library GEMM: out of scope of the hot path
+
+
+SINKHORN_EPS, SINKHORN_ITERS = 0.003, 100        # rqvae.py:229-235
+KMEANS_STOP, KMEANS_MAX_ITERS = 1e-10, 10_000
+
+
+@torch.no_grad()
+def kmeans_init_(weight: torch.Tensor, x: torch.Tensor, stop_threshold: float = KMEANS_STOP, max_iters: int = KMEANS_MAX_ITERS) -> int:
+    """Lloyd's k-means of genrec/modules/kmeans.py:11-99 on the device; writes the centroids into ``weight`` [k, D] and returns the
+    index of the converging iteration.  The same RNG use as the reference: the initial rows from ``np.random.choice(B, k,
+    replace=False)``, and one ``torch.randint(0, B, (1,))`` draw of the CPU generator per empty cluster, in ascending cluster order.
+    Each iteration is the nearest-centroid search (``rq_residual_argmin``, first index on ties), the centroid update
+    (``kmeans_update_kernel``) and one host read of the cluster sizes and shifts.  It stops when the largest centroid shift falls
+    below ``stop_threshold``.  The reference has no cap, and on inputs with fewer than k distinct rows an empty cluster is reseeded
+    at random forever: this raises after ``max_iters`` iterations instead."""
+    require_cuda(x)
+    ensure_device(x.device)
+    k = weight.shape[0]
+    x = x.detach().float().contiguous()
+    B = x.shape[0]
+    if B < k:
+        raise ValueError(f"k-means needs at least k = {k} rows to draw its initial centroids from, got {B}")
+    c = x[torch.from_numpy(np.random.choice(B, k, replace=False)).to(x.device)].contiguous()     # kmeans.py:52-56
+    for it in range(max_iters):
+        assign = Fn.rq_residual_argmin(x, c.unsqueeze(0), want_aux=False)[0][:, 0]                 # kmeans.py:59-62
+        stats = Fn.kmeans_update(x, assign, c).cpu()                                              # kmeans.py:67-75
+        counts, shift = stats[0], stats[1].view(torch.float32)
+        full = counts > 0
+        moved = float(shift[full].max()) if bool(full.any()) else 0.0
+        empty = torch.nonzero(~full).flatten()
+        if len(empty):                                                                            # kmeans.py:69-73
+            rows = torch.cat([torch.randint(0, B, (1,)) for _ in range(len(empty))]).to(x.device)
+            empty = empty.to(x.device)
+            if moved < stop_threshold:       # only then can the reseeded clusters decide whether this was the last iteration
+                moved = max(moved, float(torch.linalg.vector_norm(x[rows] - c[empty], dim=1).max()))
+            c[empty] = x[rows]
+        if moved < stop_threshold:                                                                # kmeans.py:92-93
+            weight.data.copy_(c)
+            return it
+    raise RuntimeError(f"k-means did not converge in {max_iters} iterations (B = {B}, k = {k}): with fewer than k distinct rows some "
+                       "cluster stays empty and is reseeded at random every iteration")
+
+
+def p_unique_ids(sem_ids: torch.Tensor, codebook_size: int) -> torch.Tensor:
+    """Fraction of rows whose semantic id differs from every later row's, i.e. distinct ids / B (rqvae.py:443-446), without the
+    [B, B, levels] comparison and without a host synchronisation: the ids of a row are packed into one int64 key and sorted."""
+    B, levels = sem_ids.shape
+    bits = max(1, (codebook_size - 1).bit_length())
+    if levels * bits > 63:
+        raise NotImplementedError(f"p_unique_ids packs {levels} levels x {bits} bits into an int64 key; at most 63 bits are supported")
+    key = (sem_ids << (torch.arange(levels, device=sem_ids.device) * bits)).sum(-1)
+    key = key.sort().values
+    return (1 + (key[1:] != key[:-1]).sum()) / B
 
 
 def _rotation_trick(u: torch.Tensor, q: torch.Tensor, e: torch.Tensor) -> torch.Tensor:
@@ -91,7 +170,8 @@ def _rotation_trick(u: torch.Tensor, q: torch.Tensor, e: torch.Tensor) -> torch.
 
 
 class Quantize(nn.Module):
-    """Mirror of genrec/models/rqvae.py:115-254 (eval-mode L2 path)."""
+    """Mirror of genrec/models/rqvae.py:115-254 (L2 distance, out_proj = Identity).  The k-means initialisation runs in
+    ``RqVae.forward``; every reference caller of a standalone Quantize builds it without."""
 
     def __init__(self, embed_dim: int, n_embed: int, do_kmeans_init: bool = True, codebook_normalize: bool = False,
                  sim_vq: bool = False, commitment_weight: float = 0.25,
@@ -126,31 +206,36 @@ class Quantize(nn.Module):
         if not self.training:
             ids, emb, _res, loss = Fn.rq_residual_argmin(x, self.embedding.weight.unsqueeze(0), self.commitment_weight)
             return QuantizeOutput(embeddings=emb[:, :, 0], ids=ids[:, 0], loss=loss)
-        # training (rqvae.py:201-245): the nearest-code search is the CUDA kernel (ids are not differentiated, `dist.detach()`
-        # at rqvae.py:199); the estimator around it is the reference's element-wise formula on [N, D] tensors
-        ids = Fn.rq_residual_argmin(x, self.embedding.weight.unsqueeze(0), self.commitment_weight, want_aux=False)[0][:, 0]
+        # training (rqvae.py:201-245): the nearest-code search (STE, rotation trick) or the Sinkhorn assignment is a CUDA kernel (ids
+        # are not differentiated, `dist.detach()` at rqvae.py:199); the estimator around it is the reference's element-wise formula
         codebook = self.embedding.weight
-        if self.forward_mode == QuantizeForwardMode.STE:                                     # rqvae.py:207-209
+        if self.forward_mode == QuantizeForwardMode.SINKHORN:                                # rqvae.py:218-241
+            with torch.no_grad():
+                dist = (x ** 2).sum(1, keepdim=True) + (codebook.T ** 2).sum(0, keepdim=True) - 2 * x @ codebook.T
+            ids = Fn.rq_sinkhorn(dist, SINKHORN_EPS, SINKHORN_ITERS)[0]
             emb = self.get_item_embeddings(ids)
             emb_out = x + (emb - x).detach()
-        elif self.forward_mode == QuantizeForwardMode.ROTATION_TRICK:                        # rqvae.py:210-216
-            emb = self.get_item_embeddings(ids)
-            emb_out = _rotation_trick(x / (x.norm(dim=-1, keepdim=True) + 1e-8), emb / (emb.norm(dim=-1, keepdim=True) + 1e-8), x)
         elif self.forward_mode == QuantizeForwardMode.GUMBEL_SOFTMAX:                        # rqvae.py:201-206
+            ids = Fn.rq_residual_argmin(x, codebook.unsqueeze(0), self.commitment_weight, want_aux=False)[0][:, 0]
             dist = (x ** 2).sum(1, keepdim=True) + (codebook.T ** 2).sum(0, keepdim=True) - 2 * x @ codebook.T
             u = torch.rand(dist.shape, device=x.device)
             y = -dist + -torch.log(-torch.log(u + 1e-20) + 1e-20)                            # modules/gumbel.py:10-46
             emb = F.softmax(y / temperature, dim=-1) @ codebook
             emb_out = emb
         else:
-            raise NotImplementedError("the Sinkhorn estimator (fp64, 100 iterations) is out of scope (SURVEY.md section 8, row f3)")
+            ids = Fn.rq_residual_argmin(x, codebook.unsqueeze(0), self.commitment_weight, want_aux=False)[0][:, 0]
+            emb = self.get_item_embeddings(ids)
+            if self.forward_mode == QuantizeForwardMode.STE:                                 # rqvae.py:207-209
+                emb_out = x + (emb - x).detach()
+            else:                                                                            # rqvae.py:210-216
+                emb_out = _rotation_trick(x / (x.norm(dim=-1, keepdim=True) + 1e-8), emb / (emb.norm(dim=-1, keepdim=True) + 1e-8), x)
         emb_loss = ((x.detach() - emb) ** 2).sum(-1)                                          # modules/loss.py:75-77
         query_loss = ((x - emb.detach()) ** 2).sum(-1)
         return QuantizeOutput(embeddings=emb_out, ids=ids, loss=emb_loss + self.commitment_weight * query_loss)
 
 
 class RqVae(nn.Module):
-    """Mirror of genrec/models/rqvae.py:277-412 restricted to the semantic-id path."""
+    """Mirror of genrec/models/rqvae.py:277-454."""
 
     def __init__(self, input_dim: int, embed_dim: int, hidden_dims: List[int], codebook_size: int,
                  codebook_kmeans_init: bool = True, codebook_normalize: bool = False, codebook_sim_vq: bool = False,
@@ -158,6 +243,10 @@ class RqVae(nn.Module):
                  codebook_last_layer_mode: QuantizeForwardMode = QuantizeForwardMode.GUMBEL_SOFTMAX, n_layers: int = 3,
                  commitment_weight: float = 0.25, n_cat_features: int = 18) -> None:
         super().__init__()
+        self._config = dict(input_dim=input_dim, embed_dim=embed_dim, hidden_dims=hidden_dims, codebook_size=codebook_size,
+                            codebook_kmeans_init=codebook_kmeans_init, codebook_normalize=codebook_normalize,
+                            codebook_sim_vq=codebook_sim_vq, codebook_mode=codebook_mode, codebook_last_layer_mode=codebook_last_layer_mode,
+                            n_layers=n_layers, commitment_weight=commitment_weight, n_cat_features=n_cat_features)
         self.input_dim, self.embed_dim, self.hidden_dims = input_dim, embed_dim, hidden_dims
         self.n_layers, self.codebook_size, self.commitment_weight = n_layers, codebook_size, commitment_weight
         self.n_cat_feats = n_cat_features
@@ -167,8 +256,12 @@ class RqVae(nn.Module):
                      do_kmeans_init=codebook_kmeans_init, codebook_normalize=(i == 0 and codebook_normalize),
                      sim_vq=codebook_sim_vq, commitment_weight=commitment_weight) for i in range(n_layers)])
         self.encoder = MLP(input_dim=input_dim, hidden_dims=hidden_dims, out_dim=embed_dim)
-        # the decoder exists only so that reference checkpoints load with strict=True; it is never run here
-        self.decoder = MLP(input_dim=embed_dim, hidden_dims=hidden_dims[-1::-1], out_dim=input_dim)
+        self.decoder = MLP(input_dim=embed_dim, hidden_dims=hidden_dims[-1::-1], out_dim=input_dim, normalize=True)
+
+    @property
+    def config(self) -> dict:
+        """The constructor arguments (saved by the reference trainer as ``model_config``)."""
+        return dict(self._config)
 
     @property
     def device(self) -> torch.device:
@@ -180,6 +273,9 @@ class RqVae(nn.Module):
 
     def encode(self, x: torch.Tensor) -> torch.Tensor:
         return self.encoder(x)
+
+    def decode(self, x: torch.Tensor) -> torch.Tensor:
+        return self.decoder(x)
 
     def codebooks(self) -> torch.Tensor:
         return torch.stack([l.embedding.weight for l in self.layers])     # [levels, K, D]
@@ -193,5 +289,36 @@ class RqVae(nn.Module):
         ids, emb, residuals, loss = Fn.rq_residual_argmin(res, self.codebooks(), self.commitment_weight)
         return RqVaeOutput(embeddings=emb, residuals=residuals, sem_ids=ids, quantize_loss=loss)
 
-    def forward(self, batch, gumbel_t):
-        raise NotImplementedError("RQ-VAE training (reconstruction + estimators) is out of scope; see SURVEY.md section 8")
+    def forward(self, batch: torch.Tensor, gumbel_t: float) -> RqVaeComputedLosses:
+        """rqvae.py:414-454 in train or eval mode.  On the first call every level with ``do_kmeans_init`` set initialises its codebook
+        by k-means on its input residual before it quantises (rqvae.py:182-183)."""
+        require_cuda(batch)
+        ensure_device(batch.device)
+        x = batch
+        res = self.encode(x)
+        quantize_loss = 0
+        embs, sem_ids = [], []
+        for layer in self.layers:
+            if layer.do_kmeans_init and not layer.kmeans_initted:
+                kmeans_init_(layer.embedding.weight, res)
+                layer.kmeans_initted = True
+            q = layer(res, temperature=gumbel_t)
+            quantize_loss = quantize_loss + q.loss
+            res = res - q.embeddings
+            embs.append(q.embeddings)
+            sem_ids.append(q.ids)
+        embs = torch.stack(embs, -1)                                   # [B, D, levels]
+        x_hat = self.decode(embs.sum(-1))
+        n = self.n_cat_feats
+        if n > 0:                                                      # modules/loss.py:26-54
+            x_hat = torch.cat([F.normalize(x_hat[..., :-n], p=2, dim=-1, eps=1e-12), x_hat[..., -n:]], dim=-1)
+            rec = ((x_hat[:, :-n] - x[:, :-n]) ** 2).sum(-1)
+            rec = rec + F.binary_cross_entropy_with_logits(x_hat[:, -n:], x[:, -n:], reduction="none").sum(-1)
+        else:                                                          # modules/loss.py:8-23
+            x_hat = F.normalize(x_hat, p=2, dim=-1, eps=1e-12)
+            rec = ((x_hat - x) ** 2).sum(-1)
+        with torch.no_grad():
+            embs_norm = embs.norm(dim=1)
+            p_unique = p_unique_ids(torch.stack(sem_ids, -1), self.codebook_size)
+        return RqVaeComputedLosses(loss=(rec + quantize_loss).mean(), reconstruction_loss=rec.mean(), rqvae_loss=quantize_loss.mean(),
+                                   embs_norm=embs_norm, p_unique_ids=p_unique)

@@ -370,6 +370,25 @@ int grb_rq_residual_argmin(const float* x, const float* codebooks, int64_t N, in
                            float commitment, int64_t* ids, float* emb, float* res, float* loss, float* res_out,
                            void* stream);
 
+/* ------------------------------------------------------------------------------------------------ RQ-VAE training
+ * Sinkhorn-Knopp hard assignment of the SINKHORN estimator (genrec/models/rqvae.py:85-110, :218-241) in one launch of one
+ * thread-block cluster.  dist [B, K] fp32 distances of the level; 1 <= B, 2 <= K <= 256 (B = 0 returns 0).  In fp32:
+ * mid = (max + min) / 2, amp = (max - mid) + 1e-5, dn = (dist - mid) / amp; then fp64: K = exp(-dn / eps), v = 1,
+ * `iters` x { u = r / (K v + 1e-8); v = c / (K^T u + 1e-8) } with r = (float)(1/B), c = (float)(1/K);
+ * ids[i] = argmax_j (u_i K_ij) v_j (first index on ties).  u_out [B] / v_out [K] (nullable) receive the final u and v.
+ * Deterministic (fixed-order sums), graph-capturable; the workspace holds u and, when a CTA's rows of K do not fit shared memory,
+ * K itself.  GRB_ENODEV when one cluster of 16 CTAs does not fit the device. */
+size_t grb_rq_sinkhorn_workspace_bytes(int64_t B, int K);
+int grb_rq_sinkhorn(const float* dist, int64_t B, int K, double eps, int iters, int64_t* ids, double* u_out, double* v_out,
+                    void* workspace, void* stream);
+
+/* One Lloyd step of the k-means codebook initialisation (genrec/modules/kmeans.py:58-76) after the assignment: for every cluster c
+ * of the k, counts[c] = rows with assign == c; a non-empty cluster's centroid [c, :] becomes the mean of its rows (fixed-order fp64
+ * sum, rounded to fp32) and shift[c] = |new - old|; an empty one is left as it was (shift[c] = 0) for the caller to reseed.
+ * x [B, D] fp32, 1 <= D <= 256, assign [B] int64 in [0, k), centroids [k, D] fp32 updated in place. */
+int grb_kmeans_update(const float* x, const int64_t* assign, int64_t B, int D, int k, float* centroids, int32_t* counts, float* shift,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,6 +1,7 @@
 """Stand-alone device timings of the secondary kernels (RQ-VAE residual argmin, SASRec attention, HSTU layer at cfg-3 geometry,
-cached incremental HSTU inference next to full recompute) with CUDA events, against the relevant roofline.  Prints one JSON line per
-measurement."""
+cached incremental HSTU inference next to full recompute, RQ-VAE Sinkhorn and k-means init) with CUDA events, against the relevant
+roofline or the torch code they replace.  Prints one JSON line per measurement; `bench_kernels.py rqvae_train` runs only the RQ-VAE
+training rows."""
 import json
 import os
 import sys
@@ -183,8 +184,48 @@ def bench_pool(dev):
         torch.cuda.empty_cache()
 
 
+def bench_rqvae_train(dev):
+    """The RQ-VAE training kernels next to the torch code they replace, on the same GPU: rq_sinkhorn (one launch, 100 fp64
+    iterations) against the reference's Sinkhorn restated in torch fp64, eager and graph-captured, at the training batch and the
+    k-means warm-start batch; the device k-means initialisation against the reference's Lloyd loop restated in torch."""
+    import time
+    import numpy as np
+    from genrec_b200.rqvae import kmeans_init_
+    from tests import rqvae_train_oracle as O
+    info = card()
+    g = torch.Generator().manual_seed(3)
+    for B in (1024, 20480):
+        x, cb = torch.randn(B, 32, generator=g).to(dev) * 0.3, torch.randn(256, 32, generator=g).to(dev) * 0.3
+        dist = O.l2_dist(x, cb)
+        ours = timed(lambda: Fn.rq_sinkhorn(dist), iters=20, warm=3)
+        ours_g = graph_timed(lambda: Fn.rq_sinkhorn(dist), reps=5, iters=4)
+        eager = timed(lambda: O.sinkhorn(dist), iters=5, warm=2)
+        graph = graph_timed(lambda: O.sinkhorn(dist), reps=2, iters=3)
+        kern = kernel_us(lambda: Fn.rq_sinkhorn(dist), "rq_sinkhorn_kernel", iters=10)
+        print(json.dumps(dict(kernel="rq_sinkhorn", B=B, K=256, iters=100, kernel_us=kern, us=ours * 1e3, graph_us=ours_g * 1e3,
+                              torch_fp64_eager_us=eager * 1e3, torch_fp64_graph_us=graph * 1e3, speedup_vs_torch_graph=graph / ours_g,
+                              kernel_us_per_iteration=kern / 100, **info)), flush=True)
+    x = (torch.randn(256, 32, generator=g)[torch.arange(20480) % 256] + 0.1 * torch.randn(20480, 32, generator=g)).to(dev)
+    w = torch.empty(256, 32, device=dev)
+    for name, fn in (("ours", lambda: kmeans_init_(w, x)), ("torch_reference_loop", lambda: O.kmeans(x, 256))):
+        fn()
+        np.random.seed(0)
+        torch.manual_seed(0)
+        torch.cuda.synchronize()
+        t = time.perf_counter()
+        r = fn()
+        torch.cuda.synchronize()
+        ms = (time.perf_counter() - t) * 1e3
+        it = r if name == "ours" else r[1]
+        print(json.dumps(dict(kernel="kmeans_init", impl=name, B=20480, D=32, k=256, iterations=it, ms=ms, ms_per_iteration=ms / (it + 1),
+                              **info)), flush=True)
+
+
 def main():
     dev = torch.device("cuda:0")
+    if sys.argv[1:] == ["rqvae_train"]:
+        bench_rqvae_train(dev)
+        return
     peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) \
         if os.path.exists("MEASURED_PEAKS.json") else {}
     g = torch.Generator().manual_seed(0)
@@ -225,6 +266,7 @@ def main():
                               note="eager launches (not graph-captured): includes host launch gaps at L=200")))
     bench_extend(dev)
     bench_pool(dev)
+    bench_rqvae_train(dev)
 
 
 if __name__ == "__main__":
