@@ -8,6 +8,7 @@
 #include <initializer_list>
 #include <map>
 #include <mutex>
+#include <type_traits>
 #include <utility>
 
 #include "attn_hstu.cuh"
@@ -73,6 +74,38 @@ int sm_count() {     // per device ordinal: a process may drive several GPUs
         n[dev] = v > 0 ? v : 132;
     }
     return n[dev];
+}
+// 256-thread CTAs for n items, at most per_sm CTAs per SM (the grid-stride kernels loop over the rest)
+unsigned capped_blocks(size_t n, int per_sm = 16) {
+    const size_t need = (n + 255) / 256, cap = (size_t)sm_count() * per_sm;
+    return (unsigned)(need < 1 ? 1 : (need < cap ? need : cap));
+}
+// bump allocator of the carved layouts: every buffer starts on a 256-byte boundary; with a null base only the size is counted
+struct Carver {
+    char* base;
+    size_t off = 0;
+    template <class T>
+    T* take(size_t bytes) {
+        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+        off += align_up(bytes);
+        return p;
+    }
+};
+// head-dim dispatch of the attention kernels: f(integral_constant DH) for DH = 32 or 64 (check_dims admits nothing else)
+template <class F>
+int with_head_dim(int dh, F&& f) {
+    if (dh == 32) return f(std::integral_constant<int, 32>{});
+    return f(std::integral_constant<int, 64>{});
+}
+// the row kernels are instantiated per D: f(integral_constant D) launches one for D = 64, 128 or 256
+template <class F>
+int with_row_dim(int D, F&& f) {
+    if (D == 64) f(std::integral_constant<int, 64>{});
+    else if (D == 128) f(std::integral_constant<int, 128>{});
+    else if (D == 256) f(std::integral_constant<int, 256>{});
+    else return fail(GRB_EINVAL, "row kernels support D in {64,128,256}, got %d", D);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
 }
 int row_grid(int T) {
     int need = (T + ROW_THREADS / 32 - 1) / (ROW_THREADS / 32);
@@ -161,20 +194,18 @@ struct LayerSaved {
 };
 LayerSaved carve_saved(void* base, size_t T, size_t D) {
     LayerSaved s;
-    size_t off = 0;
-    char* b = static_cast<char*>(base);
-    auto take = [&](size_t n) { char* p = b ? b + off : nullptr; off += align_up(n); return p; };
-    s.xb = (bf16*)take(T * D * 2);
-    s.zp = (bf16*)take(T * 4 * D * 2);
-    s.P = (bf16*)take(T * 4 * D * 2);
-    s.O = (bf16*)take(T * D * 2);
-    s.st1 = (float*)take(T * 2 * 4);
-    s.x1 = (float*)take(T * D * 4);
-    s.xn = (bf16*)take(T * D * 2);
-    s.st2 = (float*)take(T * 2 * 4);
-    s.z1 = (bf16*)take(T * 4 * D * 2);
-    s.hact = (bf16*)take(T * 4 * D * 2);
-    s.bytes = off;
+    Carver c{static_cast<char*>(base)};
+    s.xb = c.take<bf16>(T * D * 2);
+    s.zp = c.take<bf16>(T * 4 * D * 2);
+    s.P = c.take<bf16>(T * 4 * D * 2);
+    s.O = c.take<bf16>(T * D * 2);
+    s.st1 = c.take<float>(T * 2 * 4);
+    s.x1 = c.take<float>(T * D * 4);
+    s.xn = c.take<bf16>(T * D * 2);
+    s.st2 = c.take<float>(T * 2 * 4);
+    s.z1 = c.take<bf16>(T * 4 * D * 2);
+    s.hact = c.take<bf16>(T * 4 * D * 2);
+    s.bytes = c.off;
     return s;
 }
 struct LayerWork {
@@ -193,24 +224,22 @@ void layer_tn_specs(TnSpec (&specs)[3], const bf16* dyb, const bf16* hact, const
 LayerWork carve_work(void* base, const grb_hstu_dims* d) {
     const size_t T = (size_t)d->B * d->L, D = d->D;
     LayerWork w;
-    size_t off = 0;
-    char* b = static_cast<char*>(base);
-    auto take = [&](size_t n) { char* p = b ? b + off : nullptr; off += align_up(n); return p; };
-    w.dyb = (bf16*)take(T * D * 2);
-    w.dz1 = (bf16*)take(T * 4 * D * 2);
-    w.dxn = (float*)take(T * D * 4);
-    w.dx1 = (float*)take(T * D * 4);
-    w.dO = (bf16*)take(T * D * 2);
-    w.dzp = (bf16*)take(T * 4 * D * 2);
+    Carver c{static_cast<char*>(base)};
+    w.dyb = c.take<bf16>(T * D * 2);
+    w.dz1 = c.take<bf16>(T * 4 * D * 2);
+    w.dxn = c.take<float>(T * D * 4);
+    w.dx1 = c.take<float>(T * D * 4);
+    w.dO = c.take<bf16>(T * D * 2);
+    w.dzp = c.take<bf16>(T * 4 * D * 2);
     TnSpec specs[3];
     layer_tn_specs(specs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, (int)T, (int)D);
-    w.part_tn = (float*)take(tn_part_floats(specs, 3, sm_count()) * 4);
+    w.part_tn = c.take<float>(tn_part_floats(specs, 3, sm_count()) * 4);
     const dim3 cg = colsum_grid((int)T, 4 * (int)D), kg = cast_colsum_grid((int)T, (int)D);
-    w.part_colsum = (float*)take((size_t)cg.x * cg.y * 256 * 4);
-    w.part_cast = (float*)take((size_t)kg.x * kg.y * 128 * 4);
-    w.part_ln = (float*)take((size_t)4 * row_grid((int)T) * D * 4);
-    w.part_attn = (float*)take(attn_dw_part_floats(d->B, d->L, d->H) * 4);
-    w.bytes = off;
+    w.part_colsum = c.take<float>((size_t)cg.x * cg.y * 256 * 4);
+    w.part_cast = c.take<float>((size_t)kg.x * kg.y * 128 * 4);
+    w.part_ln = c.take<float>((size_t)4 * row_grid((int)T) * D * 4);
+    w.part_attn = c.take<float>(attn_dw_part_floats(d->B, d->L, d->H) * 4);
+    w.bytes = c.off;
     return w;
 }
 
@@ -225,6 +254,19 @@ int check_dims(const grb_hstu_dims* d) {
     GRB_REQUIRE(d->ntime >= 0 && d->ntime <= ATT_MAX_BUCKETS, "num_time_buckets %d out of range [0,64]", d->ntime);
     GRB_REQUIRE(d->L <= 16384, "seq_len %d too long", d->L);
     GRB_REQUIRE(d->dropout_p >= 0.f && d->dropout_p < 1.f, "dropout_p out of range");
+    return 0;
+}
+int check_layer_params(const grb_hstu_layer_params* p) {
+    GRB_REQUIRE(p != nullptr, "null argument");
+    GRB_REQUIRE(p->proj_w && p->proj_b && p->pos_table && p->ln1_g && p->ln1_b && p->ffn1_w && p->ffn1_b && p->ffn2_w &&
+                    p->ffn2_b && p->ln2_g && p->ln2_b, "null parameter pointer");
+    GRB_REQUIRE(aligned16(p->proj_w) && aligned16(p->ffn1_w) && aligned16(p->ffn2_w), "weights must be 16-byte aligned");
+    return 0;
+}
+int check_seq(const grb_hstu_dims* d, const grb_hstu_seq* s) {
+    GRB_REQUIRE(s != nullptr && s->bias_index, "null sequence metadata: the attention kernels need bias_index");
+    GRB_REQUIRE(s->ld_index >= d->L && s->ld_index % 8 == 0 && aligned16(s->bias_index),
+                "bias_index must be 16-byte aligned with a pitch that is a multiple of 8 and >= L");
     return 0;
 }
 
@@ -244,20 +286,26 @@ int set_smem(Kern k, size_t bytes) {
     return 0;
 }
 
-HstuBiasArgs make_attn_bias(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s) {
+// the bias tables without the index matrix (bias_index null, ldix 0)
+HstuBiasArgs make_attn_bias(const grb_hstu_dims* d, const float* pos_table, const float* time_table, int has_time, int pos_uniform,
+                            int pos_bucket0) {
     HstuBiasArgs b;
     memset(&b, 0, sizeof(b));
     // uniform position buckets (the reference's behaviour) collapse to ONE effective bucket: the index matrix was built with
     // npos = 1, the tables shrink to 65 entries and the pointers are offset to the single live row of the [npos, H] table
-    b.wpos = pos_table + (s->pos_uniform ? (size_t)s->pos_bucket0 * d->H : 0);
-    const bool has_time = time_table != nullptr && s->has_time && d->ntime > 0;
-    b.wtime = has_time ? time_table : nullptr;
+    b.wpos = pos_table + (pos_uniform ? (size_t)pos_bucket0 * d->H : 0);
+    const bool timed = time_table != nullptr && has_time && d->ntime > 0;
+    b.wtime = timed ? time_table : nullptr;
+    b.pos_uniform = pos_uniform;
+    b.npos = pos_uniform ? 1 : d->npos;
+    b.ntime = timed ? d->ntime : 0;
+    b.time_bins = att_time_bins(timed, pos_uniform != 0, b.ntime);
+    return b;
+}
+HstuBiasArgs make_attn_bias(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s) {
+    HstuBiasArgs b = make_attn_bias(d, pos_table, time_table, s->has_time, s->pos_uniform, s->pos_bucket0);
     b.bias_index = s->bias_index;
     b.ldix = s->ld_index;
-    b.pos_uniform = s->pos_uniform;
-    b.npos = s->pos_uniform ? 1 : d->npos;
-    b.ntime = has_time ? d->ntime : 0;
-    b.time_bins = att_time_bins(has_time, s->pos_uniform != 0, b.ntime);
     return b;
 }
 // P: [T, 4D] bf16 U | V | Q | K ; O: [T, D] bf16 output, written by the forward only
@@ -272,6 +320,20 @@ HstuAttnArgs make_attn_args(const grb_hstu_dims* d, const float* pos_table, cons
     a.bias = make_attn_bias(d, pos_table, time_table, s);
     a.o = O; a.ldo = D;
     return a;
+}
+// the backward's side of the attention arguments.  zp (nullable) and dzp are [T, 4D] bf16 in U | V | Q | K order: the
+// pre-activations and their gradients.  With uniform position buckets dpos is pointed at the single live row of the table.
+int set_attn_bwd_args(HstuAttnArgs& a, const grb_hstu_dims* d, const grb_hstu_seq* s, const bf16* dO, const bf16* zp, bf16* dzp,
+                      float* dpos, float* dtime, float* part) {
+    GRB_REQUIRE(a.bias.wtime == nullptr || dtime != nullptr, "time_table gradient pointer is null");
+    const int D = d->D;
+    a.d_o = dO; a.lddo = D;
+    a.zq = zp ? zp + 2 * D : nullptr; a.zk = zp ? zp + 3 * D : nullptr; a.zv = zp ? zp + D : nullptr; a.ldz = 4 * D;
+    a.dq = dzp + 2 * D; a.dk = dzp + 3 * D; a.dv = dzp + D; a.lddq = 4 * D;
+    a.dwpos = dpos + (s->pos_uniform ? (size_t)s->pos_bucket0 * d->H : 0);
+    a.dwtime = dtime;
+    a.dw_part = part;
+    return 0;
 }
 
 template <int DH>
@@ -341,6 +403,12 @@ int join_pending(cudaStream_t st) {
     std::lock_guard<std::mutex> lock(g_defer_mu);
     return defer_stream().join_into(st);
 }
+// launch(side stream) with the deferred schedule on, launch(st) without it
+template <class F>
+int run_maybe_deferred(cudaStream_t st, F&& launch) {
+    if (g_defer_on) return defer_run(st, launch);
+    return launch(st);
+}
 
 template <int DH>
 int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
@@ -379,40 +447,9 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
     return 0;
 }
 
-template <int NP, class Args, class Kern>
-int launch_row(Kern k, const Args& a, int T, cudaStream_t st) {
-    launch_k(k, row_grid(T), ROW_THREADS, 0, st, a);
-    GRB_CUDA(cudaGetLastError());
-    return 0;
-}
-template <int NP, class Args, class Kern>
-int launch_row_bwd(Kern k, const Args& a, int T, cudaStream_t st) {
-    launch_k(k, row_bwd_grid(T), ROW_THREADS, 0, st, a);
-    GRB_CUDA(cudaGetLastError());
-    return 0;
-}
-#define GRB_ROW_BWD_DISPATCH(D, KERN, ARGS, T, ST)                                        \
-    do {                                                                                  \
-        if ((D) == 64) GRB_TRY((launch_row_bwd<1>(KERN<1>, ARGS, T, ST)));                \
-        else if ((D) == 128) GRB_TRY((launch_row_bwd<2>(KERN<2>, ARGS, T, ST)));          \
-        else if ((D) == 256) GRB_TRY((launch_row_bwd<4>(KERN<4>, ARGS, T, ST)));          \
-        else return fail(GRB_EINVAL, "row kernels support D in {64,128,256}, got %d", (D)); \
-    } while (0)
-#define GRB_ROW_DISPATCH(D, KERN, ARGS, T, ST)                                            \
-    do {                                                                                  \
-        if ((D) == 64) GRB_TRY((launch_row<1>(KERN<1>, ARGS, T, ST)));                    \
-        else if ((D) == 128) GRB_TRY((launch_row<2>(KERN<2>, ARGS, T, ST)));              \
-        else if ((D) == 256) GRB_TRY((launch_row<4>(KERN<4>, ARGS, T, ST)));              \
-        else return fail(GRB_EINVAL, "row kernels support D in {64,128,256}, got %d", (D)); \
-    } while (0)
-
 int cast_bf16(const float* in, bf16* out, size_t n, int D, const Dropout& drop, const float* row_scale, cudaStream_t st) {
     GRB_REQUIRE(D > 0 && D % 4 == 0 && n % (size_t)D == 0, "cast needs rows of a multiple-of-4 length D");
-    int threads = 256;
-    size_t blocks = (n / 4 + threads - 1) / threads;
-    if (blocks > (size_t)sm_count() * 16) blocks = (size_t)sm_count() * 16;
-    if (blocks < 1) blocks = 1;
-    launch_k(cast_f32_bf16_kernel, (unsigned)blocks, threads, 0, st, in, out, n, D, drop, row_scale);
+    launch_k(cast_f32_bf16_kernel, capped_blocks(n / 4), 256, 0, st, in, out, n, D, drop, row_scale);
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -515,24 +552,41 @@ HstuPoolArgs pool_args(const grb_hstu_pool* p, const int64_t* users, int B) {
     return a;
 }
 
+// steps 1-2 of the block: xb = bf16(x) (GEMM operand; also the dWp operand in backward) ; P = silu(x Wp^T + bp) -> [U | V | Q | K]
+//                                                                                            (hstu.py:234-235)
+int block_steps_in(const grb_hstu_layer_params* p, const float* x, const LayerSaved& sv, int T, int D, cudaStream_t st) {
+    const Dropout nodrop = make_dropout(0.f, 0, 0);
+    GRB_TRY(cast_bf16(x, sv.xb, (size_t)T * D, D, nodrop, nullptr, st));
+    GRB_CUDA(gemm_bias_act(1, sv.xb, (const bf16*)p->proj_w, p->proj_b, sv.zp, sv.P, T, 4 * D, D, nodrop, st));
+    return 0;
+}
+// steps 4-6 of the block, after the attention has written O
+int block_steps_out(const grb_hstu_layer_params* p, const float* x, float* y, const LayerSaved& sv, int T, int D, const Dropout& drop_gate,
+                    const Dropout& drop_hid, const Dropout& drop_out, cudaStream_t st) {
+    // 4. x1 = x + drop(LN1(O) * U) ; xn = LN2(x1)                                            (hstu.py:271-278)
+    LnGateFwdArgs a{sv.O, D, sv.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, sv.x1, sv.xn, sv.st1, sv.st2, T, D, 1e-5f, drop_gate};
+    GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_gate_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
+    // 5. h = drop(silu(xn W1^T + b1))                                                        (hstu.py:210-212)
+    GRB_CUDA(gemm_bias_act(1, sv.xn, (const bf16*)p->ffn1_w, p->ffn1_b, sv.z1, sv.hact, T, 4 * D, D, drop_hid, st));
+    // 6. y = x1 + drop(h W2^T + b2)                                                          (hstu.py:213-214, :278)
+    GRB_CUDA(gemm_bias_res(sv.hact, (const bf16*)p->ffn2_w, p->ffn2_b, sv.x1, nullptr, y, T, D, 4 * D, drop_out, st));
+    return 0;
+}
+
 // the steps of grb_hstu_layer_forward on the chunk's rows, with the attention against the cache in place of step 3
 int layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const ExtendKv& c, const int32_t* positions,
                  const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr, const float* x, float* y, void* workspace,
                  cudaStream_t st) {
-    GRB_REQUIRE(p->proj_w && p->proj_b && p->pos_table && p->ln1_g && p->ln1_b && p->ffn1_w && p->ffn1_b && p->ffn2_w &&
-                    p->ffn2_b && p->ln2_g && p->ln2_b, "null parameter pointer");
+    GRB_TRY(check_layer_params(p));
     GRB_REQUIRE(pos_bucket != nullptr || (pos_bucket0 >= 0 && pos_bucket0 < d->npos), "pos_bucket0 %d out of range", pos_bucket0);
     const bool timed = d->ntime > 0 && p->time_table != nullptr;
     GRB_REQUIRE(!timed || time_thr != nullptr, "time_thr is null");
-    GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(workspace) && aligned16(c.kv) && aligned16(p->proj_w) && aligned16(p->ffn1_w) &&
-                    aligned16(p->ffn2_w), "buffers must be 16-byte aligned");
+    GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(workspace) && aligned16(c.kv), "buffers must be 16-byte aligned");
     const int T = d->B * d->L, D = d->D, cap = c.cap;
     ExtendWork w = carve_extend(workspace, d, cap);
     LayerSaved& sv = w.sv;
-    const Dropout nodrop = make_dropout(0.f, 0, 0);
 
-    GRB_TRY(cast_bf16(x, sv.xb, (size_t)T * D, D, nodrop, nullptr, st));
-    GRB_CUDA(gemm_bias_act(1, sv.xb, (const bf16*)p->proj_w, p->proj_b, sv.zp, sv.P, T, 4 * D, D, nodrop, st));
+    GRB_TRY(block_steps_in(p, x, sv, T, D, st));
     {
         const size_t pieces = (size_t)T * (2 * D / 8);
         launch_k(hstu_kv_scatter_kernel, (unsigned)((pieces + 255) / 256), 256, 0, st, (const bf16*)sv.P, (const int*)positions, c.users, T,
@@ -540,11 +594,6 @@ int layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const E
         GRB_CUDA(cudaGetLastError());
     }
     {
-        grb_hstu_seq s;
-        memset(&s, 0, sizeof(s));
-        s.has_time = timed;
-        s.pos_uniform = pos_bucket == nullptr;
-        s.pos_bucket0 = pos_bucket0;
         HstuExtendArgs a;
         memset(&a, 0, sizeof(a));
         a.q = sv.P + 2 * D; a.ldq = 4 * D;
@@ -555,25 +604,19 @@ int layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const E
         a.pos = positions;
         a.pos_bucket = pos_bucket;
         a.thr = reinterpret_cast<const long long*>(time_thr);
-        a.bias = make_attn_bias(d, p->pos_table, timed ? p->time_table : nullptr, &s);
+        a.bias = make_attn_bias(d, p->pos_table, p->time_table, timed, pos_bucket == nullptr, pos_bucket0);
         a.B = d->B; a.n = d->L; a.H = d->H; a.D = D; a.cap = cap;
         a.split = extend_split(d, cap);
         a.part = w.part;
         const int nsplit = (cap + a.split - 1) / a.split;
-        if (D / d->H == 32) GRB_TRY(dispatch_attn_extend<32>(a, nsplit, st));
-        else GRB_TRY(dispatch_attn_extend<64>(a, nsplit, st));
+        GRB_TRY(with_head_dim(D / d->H, [&](auto DH) { return dispatch_attn_extend<DH>(a, nsplit, st); }));
         const size_t quads = (size_t)T * D / 4;
         launch_k(hstu_extend_combine_kernel, (unsigned)((quads + 255) / 256), 256, 0, st, (const float*)w.part, (const int*)positions, T, D,
                  a.split, sv.O);
         GRB_CUDA(cudaGetLastError());
     }
-    {
-        LnGateFwdArgs a{sv.O, D, sv.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, sv.x1, sv.xn, sv.st1, sv.st2, T, D, 1e-5f, nodrop};
-        GRB_ROW_DISPATCH(D, ln_gate_fwd_kernel, a, T, st);
-    }
-    GRB_CUDA(gemm_bias_act(1, sv.xn, (const bf16*)p->ffn1_w, p->ffn1_b, sv.z1, sv.hact, T, 4 * D, D, nodrop, st));
-    GRB_CUDA(gemm_bias_res(sv.hact, (const bf16*)p->ffn2_w, p->ffn2_b, sv.x1, nullptr, y, T, D, 4 * D, nodrop, st));
-    return 0;
+    const Dropout nodrop = make_dropout(0.f, 0, 0);
+    return block_steps_out(p, x, y, sv, T, D, nodrop, nodrop, nodrop, st);
 }
 
 constexpr uint32_t SITE_GATE = 0, SITE_FFN_HID = 1, SITE_FFN_OUT = 2, SITE_EMBED = 250, SITE_ATTN = 3;
@@ -607,55 +650,29 @@ size_t grb_hstu_layer_workspace_bytes(const grb_hstu_dims* d) {
 int grb_hstu_layer_forward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const float* x,
                            float* y, void* saved, void* stream) {
     GRB_TRY(check_dims(d));
-    GRB_REQUIRE(p && s && x && y && saved, "null argument");
-    GRB_REQUIRE(p->proj_w && p->proj_b && p->pos_table && p->ln1_g && p->ln1_b && p->ffn1_w && p->ffn1_b && p->ffn2_w &&
-                    p->ffn2_b && p->ln2_g && p->ln2_b, "null parameter pointer");
-    GRB_REQUIRE(s->bias_index, "null sequence metadata: the attention kernels need bias_index");
-    GRB_REQUIRE((s->ld_index >= d->L && s->ld_index % 8 == 0 && aligned16(s->bias_index)),
-                "bias_index pitch must be a multiple of 8 and >= L");
-    GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(saved) && aligned16(p->proj_w) && aligned16(p->ffn1_w) && aligned16(p->ffn2_w),
-                "buffers must be 16-byte aligned");
+    GRB_REQUIRE(x && y && saved, "null argument");
+    GRB_TRY(check_layer_params(p));
+    GRB_TRY(check_seq(d, s));
+    GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(saved), "buffers must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int T = d->B * d->L, D = d->D;
     LayerSaved sv = carve_saved(saved, T, D);
-    const Dropout nodrop = make_dropout(0.f, 0, 0);
 
-    // 1. bf16 copy of the block input (GEMM operand; also the dWp operand in backward)
-    GRB_TRY(cast_bf16(x, sv.xb, (size_t)T * D, D, nodrop, nullptr, st));
-    // 2. P = silu(x Wp^T + bp) -> [U | V | Q | K]                                            (hstu.py:234-235)
-    {
-        GRB_CUDA(gemm_bias_act(1, sv.xb, (const bf16*)p->proj_w, p->proj_b, sv.zp, sv.P, T, 4 * D, D, nodrop, st));
-    }
+    GRB_TRY(block_steps_in(p, x, sv, T, D, st));
     // 3. O = silu(Q K^T + bias) V, causal + key padding                                      (hstu.py:244-267)
     GRB_TRY(join_pending(st));   // a bias-index matrix built on the side stream (deferred schedule) must be complete
-    {
-        HstuAttnArgs a = make_attn_args(d, p->pos_table, p->time_table, s, sv.P, sv.O);
-        if (D / d->H == 32) GRB_TRY(launch_hstu_attn_fwd<32>(a, st));
-        else GRB_TRY(launch_hstu_attn_fwd<64>(a, st));
-    }
-    // 4. x1 = x + drop(LN1(O) * U) ; xn = LN2(x1)                                            (hstu.py:271-278)
-    {
-        LnGateFwdArgs a{sv.O, D, sv.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, sv.x1, sv.xn, sv.st1, sv.st2, T, D, 1e-5f,
-                        make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_GATE), d->seed_dev)};
-        GRB_ROW_DISPATCH(D, ln_gate_fwd_kernel, a, T, st);
-    }
-    // 5. h = drop(silu(xn W1^T + b1))                                                        (hstu.py:210-212)
-    {
-        GRB_CUDA(gemm_bias_act(1, sv.xn, (const bf16*)p->ffn1_w, p->ffn1_b, sv.z1, sv.hact, T, 4 * D, D,
-                               make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_HID), d->seed_dev), st));
-    }
-    // 6. y = x1 + drop(h W2^T + b2)                                                          (hstu.py:213-214, :278)
-    {
-        GRB_CUDA(gemm_bias_res(sv.hact, (const bf16*)p->ffn2_w, p->ffn2_b, sv.x1, nullptr, y, T, D, 4 * D,
-                               make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_OUT), d->seed_dev), st));
-    }
-    return 0;
+    HstuAttnArgs a = make_attn_args(d, p->pos_table, p->time_table, s, sv.P, sv.O);
+    GRB_TRY(with_head_dim(D / d->H, [&](auto DH) { return launch_hstu_attn_fwd<DH>(a, st); }));
+    return block_steps_out(p, x, y, sv, T, D, make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_GATE), d->seed_dev),
+                           make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_HID), d->seed_dev),
+                           make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_OUT), d->seed_dev), st);
 }
 
 int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const float* dy,
                             const void* saved, float* dx, const grb_hstu_layer_grads* g, void* workspace, void* stream) {
     GRB_TRY(check_dims(d));
-    GRB_REQUIRE(p && s && dy && saved && dx && g && workspace, "null argument");
+    GRB_REQUIRE(p && dy && saved && dx && g && workspace, "null argument");
+    GRB_TRY(check_seq(d, s));
     GRB_REQUIRE(g->proj_w && g->proj_b && g->pos_table && g->ln1_g && g->ln1_b && g->ffn1_w && g->ffn1_b && g->ffn2_w && g->ffn2_b &&
                     g->ln2_g && g->ln2_b, "null gradient pointer");
     GRB_REQUIRE(aligned16(dy) && aligned16(dx) && aligned16(saved) && aligned16(workspace), "buffers must be 16-byte aligned");
@@ -663,66 +680,43 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
     const int T = d->B * d->L, D = d->D;
     LayerSaved sv = carve_saved(const_cast<void*>(saved), T, D);
     LayerWork w = carve_work(workspace, d);
-    const Dropout nodrop = make_dropout(0.f, 0, 0);
     const Dropout drop_out = make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_OUT), d->seed_dev);
     const Dropout drop_hid = make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_HID), d->seed_dev);
     const Dropout drop_gate = make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_GATE), d->seed_dev);
 
     // FFN second linear
     GRB_TRY(cast_colsum(dy, w.dyb, T, D, drop_out, g->ffn2_b, w.part_cast, st));   // dyb = bf16(dropmask(dy)) ; db2 += column sums
-    {
-        GRB_CUDA(gemm_dact(1, w.dyb, (const bf16*)p->ffn2_w, sv.z1, w.dz1, T, 4 * D, D, drop_hid, st));  // dz1 = dropmask(dyb W2) * silu'(z1)
-    }
+    GRB_CUDA(gemm_dact(1, w.dyb, (const bf16*)p->ffn2_w, sv.z1, w.dz1, T, 4 * D, D, drop_hid, st));  // dz1 = dropmask(dyb W2) * silu'(z1)
     // FFN first linear
     // bias gradients are off the critical path too: with deferred weight gradients the column sums run beside the main chain
-    auto colsum_maybe_deferred = [&](const bf16* in, float* out) -> int {
-        if (g_defer_on)
-            return defer_run(st, [&](cudaStream_t side) -> int { return colsum(in, T, 4 * D, 4 * D, out, w.part_colsum, side); });
-        return colsum(in, T, 4 * D, 4 * D, out, w.part_colsum, st);
+    auto colsum_4d = [&](const bf16* in, float* out) {
+        return run_maybe_deferred(st, [&](cudaStream_t s_) -> int { return colsum(in, T, 4 * D, 4 * D, out, w.part_colsum, s_); });
     };
-    GRB_TRY(colsum_maybe_deferred(w.dz1, g->ffn1_b));
-    {
-        GRB_CUDA(gemm_nn_f32(w.dz1, (const bf16*)p->ffn1_w, w.dxn, nullptr, 1.f, T, D, 4 * D, 4 * D, D, st));  // dxn = dz1 W1
-    }
+    GRB_TRY(colsum_4d(w.dz1, g->ffn1_b));
+    GRB_CUDA(gemm_nn_f32(w.dz1, (const bf16*)p->ffn1_w, w.dxn, nullptr, 1.f, T, D, 4 * D, 4 * D, D, st));  // dxn = dz1 W1
     // LN2 + residual + gate + LN1
     {
         LnGateBwdArgs a{dy, w.dxn, sv.x1, sv.st1, sv.st2, sv.O, D, sv.P, 4 * D, sv.zp, 4 * D, p->ln1_g, p->ln1_b, p->ln2_g,
                         w.dx1, w.dO, D, w.dzp, 4 * D, g->ln1_g, g->ln1_b, g->ln2_g, g->ln2_b, T, D, drop_gate, w.part_ln};
-        GRB_ROW_DISPATCH(D, ln_gate_bwd_kernel, a, T, st);
+        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_gate_bwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
         GRB_TRY(det_finish(w.part_ln, 4, row_grid(T), D, 1, 0, 1, {{a.dg1, D}, {a.db1, D}, {a.dg2, D}, {a.db2, D}}, st));
     }
     // attention backward -> gradients w.r.t. the V, Q, K pre-activations
     {
-        GRB_REQUIRE(s->bias_index, "null sequence metadata: the attention kernels need bias_index");
         HstuAttnArgs a = make_attn_args(d, p->pos_table, p->time_table, s, sv.P, sv.O);
-        a.d_o = w.dO; a.lddo = D;
-        a.zq = sv.zp + 2 * D; a.zk = sv.zp + 3 * D; a.zv = sv.zp + D; a.ldz = 4 * D;
-        a.dq = w.dzp + 2 * D; a.dk = w.dzp + 3 * D; a.dv = w.dzp + D; a.lddq = 4 * D;
-        a.dwpos = g->pos_table + (s->pos_uniform ? (size_t)s->pos_bucket0 * d->H : 0);
-        a.dwtime = g->time_table;
-        a.dw_part = w.part_attn;
-        GRB_REQUIRE(a.bias.wtime == nullptr || g->time_table != nullptr, "time_table gradient pointer is null");
-        if (D / d->H == 32) GRB_TRY(launch_hstu_attn_bwd<32>(a, st));
-        else GRB_TRY(launch_hstu_attn_bwd<64>(a, st));
+        GRB_TRY(set_attn_bwd_args(a, d, s, w.dO, sv.zp, w.dzp, g->pos_table, g->time_table, w.part_attn));
+        GRB_TRY(with_head_dim(D / d->H, [&](auto DH) { return launch_hstu_attn_bwd<DH>(a, st); }));
     }
     // projection
-    GRB_TRY(colsum_maybe_deferred(w.dzp, g->proj_b));
-    {
-        GRB_CUDA(gemm_nn_f32(w.dzp, (const bf16*)p->proj_w, dx, w.dx1, 1.f, T, D, 4 * D, 4 * D, D, st));  // dx = dx1 + dzp Wp
-    }
+    GRB_TRY(colsum_4d(w.dzp, g->proj_b));
+    GRB_CUDA(gemm_nn_f32(w.dzp, (const bf16*)p->proj_w, dx, w.dx1, 1.f, T, D, 4 * D, 4 * D, D, st));  // dx = dx1 + dzp Wp
     // the three weight gradients of the layer in ONE grouped launch: dW2 += dyb^T h, dW1 += dz1^T xn, dWp += dzp^T xb
     TnSpec specs[3];
     layer_tn_specs(specs, w.dyb, sv.hact, w.dz1, sv.xn, w.dzp, sv.xb, g->ffn2_w, g->ffn1_w, g->proj_w, T, D);
-    if (g_defer_on) {
-        GRB_TRY(defer_run(st, [&](cudaStream_t side) -> int {
-            GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, side));
-            return 0;
-        }));
-    } else {
-        GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, st));
-    }
-    (void)nodrop;
-    return 0;
+    return run_maybe_deferred(st, [&](cudaStream_t s_) -> int {
+        GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, s_));
+        return 0;
+    });
 }
 
 int grb_hstu_cache_append(const grb_hstu_cache* c, const int64_t* input_ids, const int64_t* timestamps, int n, int32_t* positions,
@@ -826,8 +820,7 @@ int grb_hstu_bias_index(const int64_t* timestamps, const uint8_t* pad, const int
     };
     // the index matrix is first needed by the attention kernel of the first block: with the deferred schedule it is built beside
     // that block's cast + projection GEMM (grb_hstu_layer_forward joins before its attention launch)
-    if (g_defer_on) return defer_run(static_cast<cudaStream_t>(stream), go);
-    return go(static_cast<cudaStream_t>(stream));
+    return run_maybe_deferred(static_cast<cudaStream_t>(stream), go);
 }
 
 int grb_set_defer_weight_grads(int on) {
@@ -872,38 +865,24 @@ size_t grb_hstu_attention_scratch_bytes(const grb_hstu_dims* d) {
 int grb_hstu_attention_forward(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s,
                                const void* P_bf16, void* O_bf16, void* stream) {
     GRB_TRY(check_dims(d));
-    GRB_REQUIRE(pos_table && s && P_bf16 && O_bf16, "null argument");
-    GRB_REQUIRE(s->bias_index && s->ld_index >= d->L && s->ld_index % 8 == 0 && aligned16(s->bias_index),
-                "the attention kernels need bias_index (pitch a multiple of 8 and >= L)");
+    GRB_REQUIRE(pos_table && P_bf16 && O_bf16, "null argument");
+    GRB_TRY(check_seq(d, s));
     GRB_REQUIRE(aligned16(P_bf16) && aligned16(O_bf16), "buffers must be 16-byte aligned");
     HstuAttnArgs a = make_attn_args(d, pos_table, time_table, s, (const bf16*)P_bf16, (bf16*)O_bf16);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (d->D / d->H == 32) return launch_hstu_attn_fwd<32>(a, st);
-    return launch_hstu_attn_fwd<64>(a, st);
+    return with_head_dim(d->D / d->H, [&](auto DH) { return launch_hstu_attn_fwd<DH>(a, static_cast<cudaStream_t>(stream)); });
 }
 int grb_hstu_attention_backward(const grb_hstu_dims* d, const float* pos_table, const float* time_table, const grb_hstu_seq* s,
                                 const void* P_bf16, const void* zp_bf16, const void* dO_bf16, void* dzp_bf16, float* dpos_table,
                                 float* dtime_table, void* scratch, void* stream) {
     GRB_TRY(check_dims(d));
-    GRB_REQUIRE(pos_table && s && P_bf16 && dO_bf16 && dzp_bf16 && dpos_table && scratch, "null argument");
-    GRB_REQUIRE(s->bias_index && s->ld_index >= d->L && s->ld_index % 8 == 0 && aligned16(s->bias_index),
-                "the attention kernels need bias_index (pitch a multiple of 8 and >= L)");
+    GRB_REQUIRE(pos_table && P_bf16 && dO_bf16 && dzp_bf16 && dpos_table && scratch, "null argument");
+    GRB_TRY(check_seq(d, s));
     GRB_REQUIRE(aligned16(P_bf16) && aligned16(dO_bf16) && aligned16(dzp_bf16) && aligned16(scratch) && (zp_bf16 == nullptr || aligned16(zp_bf16)),
                 "buffers must be 16-byte aligned");
     HstuAttnArgs a = make_attn_args(d, pos_table, time_table, s, (const bf16*)P_bf16, nullptr);
-    a.dw_part = static_cast<float*>(scratch);
-    GRB_REQUIRE(a.bias.wtime == nullptr || dtime_table != nullptr, "time_table gradient pointer is null");
-    const int D = d->D;
-    const bf16* zp = (const bf16*)zp_bf16;
-    bf16* dzp = (bf16*)dzp_bf16;
-    a.d_o = (const bf16*)dO_bf16; a.lddo = D;
-    a.zq = zp ? zp + 2 * D : nullptr; a.zk = zp ? zp + 3 * D : nullptr; a.zv = zp ? zp + D : nullptr; a.ldz = 4 * D;
-    a.dq = dzp + 2 * D; a.dk = dzp + 3 * D; a.dv = dzp + D; a.lddq = 4 * D;
-    a.dwpos = dpos_table + (s->pos_uniform ? (size_t)s->pos_bucket0 * d->H : 0);
-    a.dwtime = dtime_table;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (D / d->H == 32) return launch_hstu_attn_bwd<32>(a, st);
-    return launch_hstu_attn_bwd<64>(a, st);
+    GRB_TRY(set_attn_bwd_args(a, d, s, (const bf16*)dO_bf16, (const bf16*)zp_bf16, (bf16*)dzp_bf16, dpos_table, dtime_table,
+                              static_cast<float*>(scratch)));
+    return with_head_dim(d->D / d->H, [&](auto DH) { return launch_hstu_attn_bwd<DH>(a, static_cast<cudaStream_t>(stream)); });
 }
 
 int grb_collate_jagged(const int64_t* items, const int64_t* stamps, const int64_t* offsets, const int64_t* targets, int B, int L,
@@ -963,24 +942,22 @@ struct HeadWork {
 bool head_fused(int D) { return D <= 128; }
 HeadWork carve_head(void* base, size_t T, size_t D, size_t C) {
     HeadWork h;
-    size_t off = 0;
-    char* b = static_cast<char*>(base);
-    auto take = [&](size_t n) { char* p = b ? b + off : nullptr; off += align_up(n); return p; };
+    Carver c{static_cast<char*>(base)};
     h.ldl = (int)((C + 7) / 8 * 8);
-    h.xf = (bf16*)take(T * D * 2);
-    h.stf = (float*)take(T * 2 * 4);
-    h.dxf = (float*)take(T * D * 4);
-    h.scal = (float*)take(64);
+    h.xf = c.take<bf16>(T * D * 2);
+    h.stf = c.take<float>(T * 2 * 4);
+    h.dxf = c.take<float>(T * D * 4);
+    h.scal = c.take<float>(64);
     // D <= 128: the fused kernels (tc_ce.cuh) never form the [T, C] logits; D = 256 stores them
     const bool fused = head_fused((int)D);
-    h.logits = fused ? nullptr : (bf16*)take(T * (size_t)h.ldl * 2);
-    h.logits32 = fused ? nullptr : (float*)take(T * (size_t)h.ldl * 4);
-    h.row_loss = (float*)take(T * 4);
-    h.shift = (float*)take(T * 4);
-    h.part_ln = (float*)take((size_t)2 * row_bwd_grid((int)T) * D * 4);
+    h.logits = fused ? nullptr : c.take<bf16>(T * (size_t)h.ldl * 2);
+    h.logits32 = fused ? nullptr : c.take<float>(T * (size_t)h.ldl * 4);
+    h.row_loss = c.take<float>(T * 4);
+    h.shift = c.take<float>(T * 4);
+    h.part_ln = c.take<float>((size_t)2 * row_bwd_grid((int)T) * D * 4);
     const TnSpec spec{nullptr, nullptr, nullptr, (int)C, (int)D, (int)T, h.ldl, (int)D, (int)D};
-    h.part_tn = fused ? nullptr : (float*)take(tn_part_floats(&spec, 1, sm_count()) * 4);
-    h.bytes = off;
+    h.part_tn = fused ? nullptr : c.take<float>(tn_part_floats(&spec, 1, sm_count()) * 4);
+    h.bytes = c.off;
     return h;
 }
 }  // namespace
@@ -1007,7 +984,7 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
     if (count_aside) GRB_TRY(defer_run(st, count));
     {
         LnFwdArgs a{x, ln_g, ln_b, h.xf, nullptr, h.stf, T, D, ln_eps};
-        GRB_ROW_DISPATCH(D, ln_fwd_kernel, a, T, st);
+        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
     }
     if (count_aside) GRB_TRY(join_pending(st));
     else GRB_TRY(count(st));
@@ -1020,13 +997,11 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
         launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
         GRB_CUDA(cudaGetLastError());
         if (!want_grad) return 0;
-        auto table_grad = [&](cudaStream_t s_) -> int {
+        GRB_TRY(run_maybe_deferred(st, [&](cudaStream_t s_) -> int {
             if (D == 64) GRB_CUDA(launch_ce_table<64>(h.xf, (const bf16*)table_bf16, ca, s_));
             else GRB_CUDA(launch_ce_table<128>(h.xf, (const bf16*)table_bf16, ca, s_));
             return 0;
-        };
-        if (g_defer_on) GRB_TRY(defer_run(st, table_grad));
-        else GRB_TRY(table_grad(st));
+        }));
     } else {
     // logits = xf E^T   (hstu.py:137)
     GRB_CUDA((launch_tc_gemm<0, 0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, 1, TcEpiF32{nullptr, h.ldl, 1.f}, h.logits32, nullptr, h.ldl,
@@ -1044,18 +1019,14 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
     GRB_CUDA(gemm_nn_f32(h.logits, (const bf16*)table_bf16, h.dxf, nullptr, 1.f, T, D, C, h.ldl, D, st));  // dxf = dlogits E
     // dE[C,D] += dlogits^T xf: a weight gradient, off the critical path with the deferred schedule
     TnSpec spec{h.logits, h.xf, dtable, C, D, T, h.ldl, D, D};
-    if (g_defer_on) {
-        GRB_TRY(defer_run(st, [&](cudaStream_t side) -> int {
-            GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, side));
-            return 0;
-        }));
-    } else {
-        GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, st));
-    }
+    GRB_TRY(run_maybe_deferred(st, [&](cudaStream_t s_) -> int {
+        GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, s_));
+        return 0;
+    }));
     }
     {
         LnBwdArgs a{h.dxf, x, h.stf, ln_g, nullptr, dx, dln_g, dln_b, T, D, h.part_ln};
-        GRB_ROW_BWD_DISPATCH(D, ln_bwd_kernel, a, T, st);
+        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_bwd_kernel<DC / 64>, row_bwd_grid(T), ROW_THREADS, 0, st, a); }));
         GRB_TRY(det_finish(h.part_ln, 2, row_bwd_grid(T), D, 1, 0, 1, {{a.dg, D}, {a.db, D}}, st));
     }
     return 0;
@@ -1069,7 +1040,7 @@ int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float 
     HeadWork h = carve_head(workspace, T, D, C);
     {
         LnFwdArgs a{x, ln_g, ln_b, h.xf, nullptr, h.stf, T, D, ln_eps};
-        GRB_ROW_DISPATCH(D, ln_fwd_kernel, a, T, st);
+        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
     }
     // logits [T, C] fp32, leading dimension C of any parity
     GRB_CUDA((launch_tc_gemm<0, 0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, 1, TcEpiF32Plain{logits, C}, nullptr, nullptr, 0, sm_count(), st)));
@@ -1108,13 +1079,11 @@ int grb_sasrec_attention_forward(const grb_sasrec_dims* d, const void* q, const 
     a.q = (const bf16*)q; a.k = (const bf16*)k; a.v = (const bf16*)v; a.pad = pad; a.out = (bf16*)out; a.lse = lse;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     dim3 grid((a.L + ATT_BLK - 1) / ATT_BLK, a.H, a.B);
-    if (d->D / d->H == 32) {
-        GRB_TRY(set_smem(sas_attn_fwd_kernel<32>, sizeof(SasSmem<32>)));
-        launch_k(sas_attn_fwd_kernel<32>, grid, ATT_THREADS, sizeof(SasSmem<32>), st, a);
-    } else {
-        GRB_TRY(set_smem(sas_attn_fwd_kernel<64>, sizeof(SasSmem<64>)));
-        launch_k(sas_attn_fwd_kernel<64>, grid, ATT_THREADS, sizeof(SasSmem<64>), st, a);
-    }
+    GRB_TRY(with_head_dim(d->D / d->H, [&](auto DH) -> int {
+        GRB_TRY(set_smem(sas_attn_fwd_kernel<DH>, sizeof(SasSmem<DH>)));
+        launch_k(sas_attn_fwd_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
+        return 0;
+    }));
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1129,17 +1098,13 @@ int grb_sasrec_attention_backward(const grb_sasrec_dims* d, const void* q, const
     a.dq = (bf16*)dq; a.dk = (bf16*)dk; a.dv = (bf16*)dv;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     dim3 grid((a.L + ATT_BLK - 1) / ATT_BLK, a.H, a.B);
-    if (d->D / d->H == 32) {
-        GRB_TRY(set_smem(sas_attn_bwd_dq_kernel<32>, sizeof(SasSmem<32>)));
-        GRB_TRY(set_smem(sas_attn_bwd_dkdv_kernel<32>, sizeof(SasSmem<32>)));
-        launch_k(sas_attn_bwd_dq_kernel<32>, grid, ATT_THREADS, sizeof(SasSmem<32>), st, a);
-        launch_k(sas_attn_bwd_dkdv_kernel<32>, grid, ATT_THREADS, sizeof(SasSmem<32>), st, a);
-    } else {
-        GRB_TRY(set_smem(sas_attn_bwd_dq_kernel<64>, sizeof(SasSmem<64>)));
-        GRB_TRY(set_smem(sas_attn_bwd_dkdv_kernel<64>, sizeof(SasSmem<64>)));
-        launch_k(sas_attn_bwd_dq_kernel<64>, grid, ATT_THREADS, sizeof(SasSmem<64>), st, a);
-        launch_k(sas_attn_bwd_dkdv_kernel<64>, grid, ATT_THREADS, sizeof(SasSmem<64>), st, a);
-    }
+    GRB_TRY(with_head_dim(d->D / d->H, [&](auto DH) -> int {
+        GRB_TRY(set_smem(sas_attn_bwd_dq_kernel<DH>, sizeof(SasSmem<DH>)));
+        GRB_TRY(set_smem(sas_attn_bwd_dkdv_kernel<DH>, sizeof(SasSmem<DH>)));
+        launch_k(sas_attn_bwd_dq_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
+        launch_k(sas_attn_bwd_dkdv_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
+        return 0;
+    }));
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1197,9 +1162,7 @@ __global__ void dact_kernel(bf16* g, const bf16* z, size_t n, int act) {
 }  // namespace
 int grb_dact(const void* g_bf16_in_out, const void* z_bf16, size_t n, int act, void* stream) {
     GRB_REQUIRE(g_bf16_in_out && z_bf16 && n % 2 == 0 && (act == 1 || act == 2), "bad argument");
-    size_t blocks = (n / 2 + 255) / 256;
-    if (blocks > (size_t)sm_count() * 16) blocks = (size_t)sm_count() * 16;
-    launch_k(dact_kernel, (unsigned)(blocks ? blocks : 1), 256, 0, static_cast<cudaStream_t>(stream), (bf16*)const_cast<void*>(g_bf16_in_out), (const bf16*)z_bf16, n, act);
+    launch_k(dact_kernel, capped_blocks(n / 2), 256, 0, static_cast<cudaStream_t>(stream), (bf16*)const_cast<void*>(g_bf16_in_out), (const bf16*)z_bf16, n, act);
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1224,24 +1187,21 @@ int grb_layernorm_forward(const float* x, const float* g, const float* b, float 
     GRB_REQUIRE(x && g && b && (y_bf16 || y_f32), "null argument");
     LnFwdArgs a{x, g, b, (bf16*)y_bf16, y_f32, stats, T, D, eps};
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    GRB_ROW_DISPATCH(D, ln_fwd_kernel, a, T, st);
-    return 0;
+    return with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); });
 }
 int grb_layernorm_backward(const float* dy, const float* x, const float* stats, const float* g, const float* residual, int T, int D,
                            float* dx, float* dg, float* db, void* stream) {
     GRB_REQUIRE(dy && x && stats && g && dx && dg && db, "null argument");
     LnBwdArgs a{dy, x, stats, g, residual, dx, dg, db, T, D};
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    GRB_ROW_DISPATCH(D, ln_bwd_kernel, a, T, st);
-    return 0;
+    return with_row_dim(D, [&](auto DC) { launch_k(ln_bwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); });
 }
 
 int grb_split3_f32_to_bf16(const float* in, void* out_bf16, size_t rows, int K, int operand, void* stream) {
     GRB_REQUIRE(in && out_bf16 && K > 0 && (operand == 0 || operand == 1), "bad argument");
     if (rows == 0) return 0;
-    size_t blocks = (rows * (size_t)K + 255) / 256;
-    if (blocks > (size_t)sm_count() * 16) blocks = (size_t)sm_count() * 16;
-    launch_k(split3_f32_bf16_kernel, (unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream), in, (bf16*)out_bf16, rows, K, operand);
+    launch_k(split3_f32_bf16_kernel, capped_blocks(rows * (size_t)K), 256, 0, static_cast<cudaStream_t>(stream), in, (bf16*)out_bf16, rows, K,
+             operand);
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1277,16 +1237,15 @@ struct LayerF32Work {
 };
 static LayerF32Work carve_f32(void* base, size_t T, size_t D) {
     LayerF32Work w;
-    size_t off = 0;
-    auto take = [&](size_t n) { void* p = base ? (char*)base + off : nullptr; off += (n + 255) & ~size_t(255); return p; };
-    w.xs = (bf16*)take(T * 6 * D * 2);
-    w.P = (float*)take(T * 4 * D * 4);
-    w.O = (float*)take(T * D * 4);
-    w.x1 = (float*)take(T * D * 4);
-    w.xn = (float*)take(T * D * 4);
-    w.h = (float*)take(T * 4 * D * 4);
-    w.hs = (bf16*)take(T * 24 * D * 2);
-    w.bytes = off;
+    Carver c{static_cast<char*>(base)};
+    w.xs = c.take<bf16>(T * 6 * D * 2);
+    w.P = c.take<float>(T * 4 * D * 4);
+    w.O = c.take<float>(T * D * 4);
+    w.x1 = c.take<float>(T * D * 4);
+    w.xn = c.take<float>(T * D * 4);
+    w.h = c.take<float>(T * 4 * D * 4);
+    w.hs = c.take<bf16>(T * 24 * D * 2);
+    w.bytes = c.off;
     return w;
 }
 size_t grb_hstu_layer_f32_workspace_bytes(const grb_hstu_dims* d) {
@@ -1299,10 +1258,10 @@ int grb_hstu_layer_forward_f32(const grb_hstu_dims* d, const grb_hstu_layer_para
     GRB_REQUIRE(p && s && x && y && workspace, "null argument");
     GRB_REQUIRE(p->proj_w_split && p->proj_b && p->pos_table && p->ln1_g && p->ln1_b && p->ffn1_w_split && p->ffn1_b && p->ffn2_w_split &&
                     p->ffn2_b && p->ln2_g && p->ln2_b, "null parameter pointer");
-    GRB_REQUIRE(s->bias_index && s->ld_index >= d->L && s->ld_index % 8 == 0, "the fp32 path reads the [B, L, ld] bias index matrix");
+    GRB_TRY(check_seq(d, s));
     GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(workspace), "buffers must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int T = d->B * d->L, D = d->D, DH = D / d->H;
+    const int T = d->B * d->L, D = d->D;
     LayerF32Work w = carve_f32(workspace, T, D);
     GRB_TRY(join_pending(st));
     // P = silu(x Wp^T + bp)                                                                   (hstu.py:234-235)
@@ -1311,17 +1270,12 @@ int grb_hstu_layer_forward_f32(const grb_hstu_dims* d, const grb_hstu_layer_para
     // O = silu(Q K^T + bias) V                                                                (hstu.py:244-267)
     {
         HstuAttnF32Args a{w.P, 4 * D, d->B, d->L, d->H, make_attn_bias(d, p->pos_table, p->time_table, s), w.O};
-        int rc = DH == 32 ? launch_hstu_attn_f32<32>(a, st) : launch_hstu_attn_f32<64>(a, st);
-        GRB_REQUIRE(rc == 0, "fp32 attention launch failed");
+        GRB_REQUIRE(with_head_dim(D / d->H, [&](auto DH) { return launch_hstu_attn_f32<DH>(a, st); }) == 0, "fp32 attention launch failed");
     }
     // x1 = x + LN1(O) * U ; xn = LN2(x1)                                                      (hstu.py:271-278)
     {
         LnGateF32Args a{w.O, w.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, w.x1, w.xn, T, 1e-5f};
-        const int grid = row_grid(T);
-        if (D == 64) launch_k(ln_gate_f32_kernel<2>, grid, 256, 0, st, a);
-        else if (D == 128) launch_k(ln_gate_f32_kernel<4>, grid, 256, 0, st, a);
-        else launch_k(ln_gate_f32_kernel<8>, grid, 256, 0, st, a);
-        GRB_CUDA(cudaGetLastError());
+        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_gate_f32_kernel<DC / 32>, row_grid(T), 256, 0, st, a); }));
     }
     // y = x1 + (silu(xn W1^T + b1) W2^T + b2)                                                 (hstu.py:210-214, :278)
     GRB_TRY(grb_split3_f32_to_bf16(w.xn, w.xs, T, D, 0, stream));
@@ -1333,12 +1287,7 @@ int grb_hstu_layer_forward_f32(const grb_hstu_dims* d, const grb_hstu_layer_para
 int grb_layernorm_f32_forward(const float* x, const float* g, const float* b, float eps, int T, int D, float* y, void* stream) {
     GRB_REQUIRE(x && g && b && y && T > 0 && (D == 64 || D == 128 || D == 256), "bad argument T=%d D=%d", T, D);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int grid = row_grid(T);
-    if (D == 64) launch_k(ln_f32_kernel<2>, grid, 256, 0, st, x, g, b, y, T, eps);
-    else if (D == 128) launch_k(ln_f32_kernel<4>, grid, 256, 0, st, x, g, b, y, T, eps);
-    else launch_k(ln_f32_kernel<8>, grid, 256, 0, st, x, g, b, y, T, eps);
-    GRB_CUDA(cudaGetLastError());
-    return 0;
+    return with_row_dim(D, [&](auto DC) { launch_k(ln_f32_kernel<DC / 32>, row_grid(T), 256, 0, st, x, g, b, y, T, eps); });
 }
 
 // ------------------------------------------------------------------------------------------------ T5-style attention core (TIGER)
@@ -1366,15 +1315,12 @@ int grb_t5_attention_forward(const void* q, const void* k, const void* v, int B,
     a.out = (bf16*)out; a.ldo = ldo; a.lse = lse;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     dim3 grid((Lq + T5_ROWS - 1) / T5_ROWS, B * H);
-    if (head_dim == 32) {
-        const size_t smem = t5_fwd_smem<32>(a.nb);
-        GRB_TRY(set_smem(t5_attn_fwd_kernel<32>, smem));
-        launch_k(t5_attn_fwd_kernel<32>, grid, T5_THREADS, smem, st, a);
-    } else {
-        const size_t smem = t5_fwd_smem<64>(a.nb);
-        GRB_TRY(set_smem(t5_attn_fwd_kernel<64>, smem));
-        launch_k(t5_attn_fwd_kernel<64>, grid, T5_THREADS, smem, st, a);
-    }
+    GRB_TRY(with_head_dim(head_dim, [&](auto DH) -> int {
+        const size_t smem = t5_fwd_smem<DH>(a.nb);
+        GRB_TRY(set_smem(t5_attn_fwd_kernel<DH>, smem));
+        launch_k(t5_attn_fwd_kernel<DH>, grid, T5_THREADS, smem, st, a);
+        return 0;
+    }));
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1393,15 +1339,12 @@ int grb_t5_attention_backward(const void* q, const void* k, const void* v, int B
     GRB_CUDA(cudaMemsetAsync(dk, 0, (size_t)B * Lk * H * head_dim * sizeof(float), st));
     GRB_CUDA(cudaMemsetAsync(dv, 0, (size_t)B * Lk * H * head_dim * sizeof(float), st));
     dim3 grid((Lq + T5_ROWS - 1) / T5_ROWS, B * H);
-    if (head_dim == 32) {
-        const size_t smem = t5_bwd_smem<32>(a.nb);
-        GRB_TRY(set_smem(t5_attn_bwd_kernel<32>, smem));
-        launch_k(t5_attn_bwd_kernel<32>, grid, T5_THREADS, smem, st, a);
-    } else {
-        const size_t smem = t5_bwd_smem<64>(a.nb);
-        GRB_TRY(set_smem(t5_attn_bwd_kernel<64>, smem));
-        launch_k(t5_attn_bwd_kernel<64>, grid, T5_THREADS, smem, st, a);
-    }
+    GRB_TRY(with_head_dim(head_dim, [&](auto DH) -> int {
+        const size_t smem = t5_bwd_smem<DH>(a.nb);
+        GRB_TRY(set_smem(t5_attn_bwd_kernel<DH>, smem));
+        launch_k(t5_attn_bwd_kernel<DH>, grid, T5_THREADS, smem, st, a);
+        return 0;
+    }));
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1439,9 +1382,7 @@ int grb_beam_select(const int64_t* beam_seqs, const float* beam_logps, const int
 int grb_cast_f32_to_bf16(const float* in, void* out_bf16, size_t n, void* stream) {
     GRB_REQUIRE(in && out_bf16, "null argument");
     if (n == 0) return 0;
-    size_t blocks = (n + 255) / 256;
-    if (blocks > (size_t)sm_count() * 16) blocks = (size_t)sm_count() * 16;
-    launch_k(cast_flat_f32_bf16_kernel, (unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream), in, (bf16*)out_bf16, n);
+    launch_k(cast_flat_f32_bf16_kernel, capped_blocks(n), 256, 0, static_cast<cudaStream_t>(stream), in, (bf16*)out_bf16, n);
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1453,9 +1394,7 @@ int grb_adam_step(float* p, float* g, float* m, float* v, void* p_bf16, size_t n
     GRB_CUDA(cudaGetLastError());
     if (n == 0) return 0;
     AdamArgs a{p, g, m, v, (bf16*)p_bf16, n, state, lr, beta1, beta2, eps, weight_decay, grad_scale, zero_grad};
-    size_t blocks = (n + 255) / 256;
-    if (blocks > (size_t)sm_count() * 16) blocks = (size_t)sm_count() * 16;
-    launch_k(adam_step_kernel, (unsigned)blocks, 256, 0, st, a);
+    launch_k(adam_step_kernel, capped_blocks(n), 256, 0, st, a);
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1478,11 +1417,9 @@ int grb_dp_adam_step(float* p, float* g, float* m, float* v, void* p_bf16, const
     DpAdamArgs a{p, g, m, v, (bf16*)p_bf16, (const float*)mc_g, (float*)mc_p, (bf16*)mc_p_bf16,
                  reinterpret_cast<const float* const*>(peer_g), reinterpret_cast<float* const*>(peer_p), reinterpret_cast<bf16* const*>(peer_p_bf16),
                  n, rank, world, state, lr, beta1, beta2, eps, weight_decay, grad_scale};
-    size_t blocks = (n / world / 8 + 255) / 256;
-    if (blocks > (size_t)sm_count() * 4) blocks = (size_t)sm_count() * 4;
-    if (blocks < 1) blocks = 1;
-    if (mc) launch_k(dp_adam_kernel<true>, (unsigned)blocks, 256, 0, st, a);
-    else launch_k(dp_adam_kernel<false>, (unsigned)blocks, 256, 0, st, a);
+    const unsigned blocks = capped_blocks(n / world / 8, 4);
+    if (mc) launch_k(dp_adam_kernel<true>, blocks, 256, 0, st, a);
+    else launch_k(dp_adam_kernel<false>, blocks, 256, 0, st, a);
     GRB_CUDA(cudaGetLastError());
     launch_k(dp_barrier_kernel, 1, 32, 0, st, reinterpret_cast<unsigned* const*>(peer_sig), reinterpret_cast<unsigned*>(sig),
              reinterpret_cast<unsigned*>(epoch), rank, world, 1);

@@ -82,8 +82,11 @@ class SeqMeta:
     [B, L, ld] uint16 bias-index matrix the attention kernels read.  The per-sequence int32 rebasing of the timestamps
     (``grb_hstu_seq_prepare``) is made on demand for the bucket test hook."""
 
-    def __init__(self, pad_u8: torch.Tensor, timestamps: Optional[torch.Tensor], pos_bucket: torch.Tensor,
-                 time_thr: torch.Tensor, num_time_buckets: int = 64, num_pos_buckets: int = 32, pos_uniform=None):
+    def __init__(self, pad_u8: torch.Tensor, timestamps: Optional[torch.Tensor], pos_bucket: Optional[torch.Tensor],
+                 time_thr: torch.Tensor, num_time_buckets: int = 64, num_pos_buckets: int = 32, pos_uniform=None,
+                 may_defer: bool = True):
+        # may_defer=False builds the index on the caller's stream even under the deferred schedule (the custom ops, whose
+        # callers order and free everything by that stream); pos_bucket may be None when pos_uniform is given
         require_cuda(pad_u8)
         B, L = pad_u8.shape
         self.B, self.L = B, L
@@ -101,9 +104,8 @@ class SeqMeta:
             pos_uniform = (bool((pb == pb[0]).all()), int(pb[0]))
         self.pos_uniform, self.pos_bucket0 = pos_uniform
         self.ld = (L + 7) // 8 * 8
-        self.bias_index = None
         self.rel32 = self.wide = None
-        self._build_bias_index()
+        self._build_bias_index(may_defer)
 
     def _ensure_rel(self):
         if self.timestamps is None or self.rel32 is not None:
@@ -115,9 +117,7 @@ class SeqMeta:
             check(_lib.load().grb_hstu_seq_prepare(ptr(self.timestamps), ptr(self.pad), self.B, self.L, ptr(self.rel32), ptr(self.wide),
                                                    stream_ptr(dev)))
 
-    def _build_bias_index(self):
-        if self.bias_index is not None:
-            return
+    def _build_bias_index(self, may_defer: bool):
         B, L, dev = self.B, self.L, self.pad.device
         self.bias_index = torch.empty(B, L, self.ld, dtype=torch.int16, device=dev)
         nt = self.num_time_buckets if self.timestamps is not None else 0
@@ -128,9 +128,11 @@ class SeqMeta:
             pb_arg, npos_arg = _ZERO_TABLES[key], 1
         else:
             pb_arg, npos_arg = self.pos_bucket, self.num_pos_buckets
-        _defer_for_call(_DEFER["on"])        # deferred schedule: built on the side stream, joined before the first attention launch
-        check(_lib.load().grb_hstu_bias_index(ptr(self.timestamps), ptr(self.pad), ptr(self.time_thr), ptr(pb_arg), B, L,
-                                              npos_arg, nt, ptr(self.bias_index), self.ld, stream_ptr(dev)))
+        # deferred schedule: built on the side stream, joined before the first attention launch
+        _defer_for_call(_DEFER["on"] and may_defer)
+        with torch.cuda.device(dev):
+            check(_lib.load().grb_hstu_bias_index(ptr(self.timestamps), ptr(self.pad), ptr(self.time_thr), ptr(pb_arg), B, L,
+                                                  npos_arg, nt, ptr(self.bias_index), self.ld, stream_ptr(dev)))
 
     def struct(self) -> HstuSeq:
         return HstuSeq(ptr(self.bias_index), self.ld, 1 if self.timestamps is not None else 0, 1 if self.pos_uniform else 0,
@@ -153,73 +155,86 @@ def _dims(B, L, D, H, npos, ntime, p, seed, seed_dev, layer) -> HstuDims:
     return HstuDims(B, L, D, H, npos, ntime, float(p), int(seed) & (2 ** 64 - 1), ptr(seed_dev), layer)
 
 
+def _layer_param_struct(params, bf16w: dict, has_time: bool) -> HstuLayerParams:
+    """``params`` in PARAM_ORDER (fp32 masters; time_table may be None), ``bf16w`` the bf16 mirrors of BF16_PARAMS.  The
+    time table is passed only when the block uses the temporal term."""
+    named = dict(zip(PARAM_ORDER, params))
+    return HstuLayerParams(*[
+        ptr(bf16w[n]) if n in BF16_PARAMS else (ptr(named[n].detach()) if named[n] is not None and (n != "time_table" or has_time) else None)
+        for n in PARAM_ORDER])
+
+
+def layer_saved_bytes(dims: HstuDims) -> int:
+    """Size of the block's saved-for-backward blob (a host-side query: no device needed)."""
+    lib = _lib.load()
+    nbytes = lib.grb_hstu_layer_saved_bytes(C.byref(dims))
+    if nbytes == 0:
+        raise _lib.GrbError(lib.grb_last_error().decode())
+    return nbytes
+
+
+def hstu_block_forward(dims: HstuDims, params, bf16w: dict, has_time: bool, meta: SeqMeta, x: torch.Tensor):
+    """One HSTU block (grb_hstu_layer_forward): x [B, L, D] fp32 contiguous -> (y, saved-for-backward blob)."""
+    saved = _u8(layer_saved_bytes(dims), x.device)
+    y = torch.empty_like(x)
+    pstruct, seq = _layer_param_struct(params, bf16w, has_time), meta.struct()
+    with torch.cuda.device(x.device):
+        check(_lib.load().grb_hstu_layer_forward(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(x), ptr(y), ptr(saved),
+                                                 stream_ptr(x.device)))
+    return y, saved
+
+
+def hstu_block_backward(dims: HstuDims, params, bf16w: dict, has_time: bool, meta: SeqMeta, dy: torch.Tensor, saved: torch.Tensor,
+                        sink: Optional[dict] = None):
+    """grb_hstu_layer_backward -> (dx, parameter gradients in PARAM_ORDER, None where a parameter is absent).  With a ``sink``
+    (name -> view of the flat gradient buffer of genrec_b200.optim.FlatAdam) the gradients accumulate there, and the weight
+    gradients follow the deferred schedule when it is on."""
+    lib = _lib.load()
+    if sink is not None:
+        grads = [sink[n] if q is not None else None for n, q in zip(PARAM_ORDER, params)]
+    else:
+        grads = [torch.zeros(q.shape, dtype=torch.float32, device=dy.device) if q is not None else None for q in params]
+    pstruct, gstruct, seq = _layer_param_struct(params, bf16w, has_time), HstuLayerGrads(*[ptr(g) for g in grads]), meta.struct()
+    dyc = dy.contiguous().float()
+    dx = torch.empty_like(dyc)
+    ws = _u8(lib.grb_hstu_layer_workspace_bytes(C.byref(dims)), dy.device)
+    deferred = _defer_for_call(_DEFER["on"] and sink is not None)
+    with torch.cuda.device(dy.device):
+        check(lib.grb_hstu_layer_backward(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(dyc), ptr(saved), ptr(dx), C.byref(gstruct),
+                                          ptr(ws), stream_ptr(dy.device)))
+    if deferred:
+        _DEFER["keep"].append((ws, saved, dyc))     # still read by the deferred dW GEMM
+    return dx, grads
+
+
 class HstuLayerFn(torch.autograd.Function):
     """One HSTU block.  forward = grb_hstu_layer_forward, backward = grb_hstu_layer_backward."""
 
     @staticmethod
     def forward(ctx, x, meta: SeqMeta, cfg: dict, bf16w: dict, *params):
         # params in PARAM_ORDER (fp32 masters; time_table may be None)
-        lib = _lib.load()
         require_cuda(x)
         B, L, D = x.shape
-        xc = x.detach().contiguous().float()
-        named = dict(zip(PARAM_ORDER, params))
         require_f32(*[q for q in params if q is not None])
-        has_time = named["time_table"] is not None and meta.timestamps is not None
+        has_time = params[PARAM_ORDER.index("time_table")] is not None and meta.timestamps is not None
         dims = _dims(B, L, D, cfg["H"], cfg["npos"], cfg["ntime"] if has_time else 0, cfg["p"], cfg["seed"], cfg["seed_dev"],
                      cfg["layer"])
-        pstruct = HstuLayerParams(*[
-            ptr(bf16w[n]) if n in BF16_PARAMS else (ptr(named[n].detach()) if named[n] is not None and (n != "time_table" or has_time) else None)
-            for n in PARAM_ORDER])
-        nbytes = lib.grb_hstu_layer_saved_bytes(C.byref(dims))
-        if nbytes == 0:
-            raise _lib.GrbError(lib.grb_last_error().decode())
-        saved = _u8(nbytes, x.device)
-        y = torch.empty_like(xc)
-        seq = meta.struct()
-        with torch.cuda.device(x.device):
-            check(lib.grb_hstu_layer_forward(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(xc), ptr(y), ptr(saved),
-                                             stream_ptr(x.device)))
-        ctx.meta, ctx.cfg, ctx.bf16w, ctx.has_time = meta, cfg, bf16w, has_time
-        ctx.saved_blob = saved
-        ctx.shape = (B, L, D)
+        y, ctx.saved_blob = hstu_block_forward(dims, params, bf16w, has_time, meta, x.detach().contiguous().float())
+        ctx.meta, ctx.cfg, ctx.bf16w, ctx.has_time, ctx.dims = meta, cfg, bf16w, has_time, dims
         ctx.save_for_backward(*[p for p in params if p is not None])
         ctx.param_present = [p is not None for p in params]
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        lib = _lib.load()
-        B, L, D = ctx.shape
-        cfg, meta, has_time = ctx.cfg, ctx.meta, ctx.has_time
         it = iter(ctx.saved_tensors)
         params = [next(it) if present else None for present in ctx.param_present]
-        named = dict(zip(PARAM_ORDER, params))
-        dims = _dims(B, L, D, cfg["H"], cfg["npos"], cfg["ntime"] if has_time else 0, cfg["p"], cfg["seed"], cfg["seed_dev"],
-                     cfg["layer"])
-        pstruct = HstuLayerParams(*[
-            ptr(ctx.bf16w[n]) if n in BF16_PARAMS else (ptr(named[n].detach()) if named[n] is not None and (n != "time_table" or has_time) else None)
-            for n in PARAM_ORDER])
-        sink = cfg.get("grad_sink")
-        if sink is not None:      # accumulate straight into the flat gradient buffer (genrec_b200.optim.FlatAdam)
-            grads = {n: (sink[n] if named[n] is not None else None) for n in PARAM_ORDER}
-        else:
-            grads = {n: (torch.zeros_like(named[n], dtype=torch.float32) if named[n] is not None else None) for n in PARAM_ORDER}
-        gstruct = HstuLayerGrads(*[ptr(grads[n]) for n in PARAM_ORDER])
-        dyc = dy.contiguous().float()
-        dx = torch.empty_like(dyc)
-        ws = _u8(lib.grb_hstu_layer_workspace_bytes(C.byref(dims)), dy.device)
-        seq = meta.struct()
-        deferred = _defer_for_call(_DEFER["on"] and sink is not None)
-        with torch.cuda.device(dy.device):
-            check(lib.grb_hstu_layer_backward(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(dyc), ptr(ctx.saved_blob), ptr(dx),
-                                              C.byref(gstruct), ptr(ws), stream_ptr(dy.device)))
-        if deferred:
-            _DEFER["keep"].append((ws, ctx.saved_blob, dyc))     # still read by the deferred dW GEMM
+        sink = ctx.cfg.get("grad_sink")     # accumulate straight into the flat gradient buffer (genrec_b200.optim.FlatAdam)
+        dx, grads = hstu_block_backward(ctx.dims, params, ctx.bf16w, ctx.has_time, ctx.meta, dy, ctx.saved_blob, sink)
         ctx.saved_blob = None
         if sink is not None:
             return (dx, None, None, None, *([None] * len(PARAM_ORDER)))
-        return (dx, None, None, None, *[grads[n] for n in PARAM_ORDER])
+        return (dx, None, None, None, *grads)
 
 
 class EmbedFn(torch.autograd.Function):
@@ -427,12 +442,9 @@ def hstu_layer_extend(x: torch.Tensor, cache, layer: int, positions: torch.Tenso
     require_f32(x)
     B, n, D = x.shape
     xc = x.contiguous()
-    named = dict(zip(PARAM_ORDER, params))
-    has_time = named["time_table"] is not None and ntime > 0
+    has_time = params[PARAM_ORDER.index("time_table")] is not None and ntime > 0
     dims = _dims(B, n, D, H, npos, ntime if has_time else 0, 0.0, 0, None, layer)
-    pstruct = HstuLayerParams(*[
-        ptr(bf16w[k]) if k in BF16_PARAMS else (ptr(named[k].detach()) if named[k] is not None and (k != "time_table" or has_time) else None)
-        for k in PARAM_ORDER])
+    pstruct = _layer_param_struct(params, bf16w, has_time)
     paged = isinstance(cache, _lib.HstuPool)
     if paged:
         nbytes = lib.grb_hstu_layer_extend_paged_workspace_bytes(C.byref(dims), C.byref(cache))
@@ -698,10 +710,8 @@ def hstu_layer_forward_f32(x: torch.Tensor, meta: SeqMeta, H: int, npos: int, nt
     B, L, D = x.shape
     xc = x.detach().contiguous()
     (_, proj_b, pos_t, time_t, ln1_g, ln1_b, _, ffn1_b, _, ffn2_b, ln2_g, ln2_b) = params
-    meta._build_bias_index()
     join_deferred(x.device)
-    seq = HstuSeq(ptr(meta.bias_index), meta.ld, 1 if meta.timestamps is not None else 0, 1 if meta.pos_uniform else 0, meta.pos_bucket0,
-                  ptr(meta.timestamps), ptr(meta.pad), None, None, ptr(meta.time_thr))
+    seq = meta.struct()
     d = _dims(B, L, D, H, npos, ntime, 0.0, 0, None, 0)
     p = _lib.HstuLayerParamsF32(ptr(split_w["proj_w"]), ptr(proj_b.detach()), ptr(pos_t.detach()), ptr(time_t.detach()) if time_t is not None else None,
                                 ptr(ln1_g.detach()), ptr(ln1_b.detach()), ptr(split_w["ffn1_w"]), ptr(ffn1_b.detach()), ptr(split_w["ffn2_w"]),

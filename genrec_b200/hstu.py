@@ -72,6 +72,21 @@ def _thresholds_on(device) -> torch.Tensor:
     return _THR_CACHE[key]
 
 
+def _cached(cache: dict, key, param: torch.Tensor, make, remake: bool = False) -> torch.Tensor:
+    """cache[key]: ``make(param, out)`` of the parameter's current version, remade when the version or the device changes or
+    when ``remake`` is set; ``out`` is the previous result on the same device (or None), for makers that can write in place."""
+    ent = cache.get(key)
+    out = ent[1] if ent is not None and ent[1].device == param.device else None
+    if remake or out is None or ent[0] != param._version:
+        ent = (param._version, make(param, out))
+        cache[key] = ent
+    return ent[1]
+
+
+def _split3_weight(param: torch.Tensor, _out) -> torch.Tensor:
+    return Fn.split3(param, 1)
+
+
 class RelativePositionBias(nn.Module):
     """Mirror of genrec/models/hstu.py:284-349."""
 
@@ -165,12 +180,9 @@ class HSTULayer(nn.Module):
         self.precision = "bf16"     # "fp32": the fp32-exact forward path (HSTU.set_precision)
         self._split = {}            # name -> (version, tensor): three-term bf16 splits of the weight matrices (fp32 path)
 
-    def _split_weight(self, name: str, param: torch.Tensor) -> torch.Tensor:
-        ent = self._split.get(name)
-        if ent is None or ent[0] != param._version or ent[1].device != param.device:
-            ent = (param._version, Fn.split3(param, 1))
-            self._split[name] = ent
-        return ent[1]
+    def _weights(self) -> dict:
+        """The three weight matrices, by their names in Fn.BF16_PARAMS."""
+        return {"proj_w": self.projection.weight, "ffn1_w": self.ffn[0].weight, "ffn2_w": self.ffn[3].weight}
 
     def _run_f32(self, x: torch.Tensor, meta: Fn.SeqMeta) -> torch.Tensor:
         """fp32-exact forward (what the reference computes without autocast; 1e-5 parity target).  Forward only."""
@@ -179,24 +191,26 @@ class HSTULayer(nn.Module):
                                "wrap the call in torch.no_grad() or train with precision='bf16'")
         if self.training and self.dropout.p > 0:
             raise RuntimeError("genrec_b200: precision='fp32' has no dropout; call model.eval()")
-        sw = {"proj_w": self._split_weight("proj_w", self.projection.weight),
-              "ffn1_w": self._split_weight("ffn1_w", self.ffn[0].weight),
-              "ffn2_w": self._split_weight("ffn2_w", self.ffn[3].weight)}
+        sw = {n: _cached(self._split, n, w, _split3_weight) for n, w in self._weights().items()}
         return Fn.hstu_layer_forward_f32(x, meta, self.num_heads, self.position_bias.num_buckets,
                                          self.temporal_bias.num_buckets if self.use_temporal_bias else 0, sw, self._params())
 
-    # -- bf16 operand mirrors of the three weight matrices
     def _mirror(self, name: str, param: torch.Tensor) -> torch.Tensor:
         if self._bf16_provider is not None:
             return self._bf16_provider(param)
-        ent = self._bf16.get(name)
-        fresh = ent is not None and ent[0] == param._version and ent[1].device == param.device
-        if self.training and torch.is_grad_enabled():
-            fresh = False  # always re-cast while training: an optimizer step (possibly inside a CUDA graph) may have run
-        if not fresh:
-            ent = (param._version, Fn.cast_bf16(param, ent[1] if ent is not None and ent[1].device == param.device else None))
-            self._bf16[name] = ent
-        return ent[1]
+        # always re-cast while training: an optimizer step (possibly inside a CUDA graph) may have run
+        return _cached(self._bf16, name, param, Fn.cast_bf16, remake=self.training and torch.is_grad_enabled())
+
+    def _bf16_weights(self) -> dict:
+        """bf16 operand mirrors of the three weight matrices."""
+        return {n: self._mirror(n, w) for n, w in self._weights().items()}
+
+    def _seq_meta(self, pad_u8: torch.Tensor, timestamps: Optional[torch.Tensor], L: int, device) -> Fn.SeqMeta:
+        """Sequence metadata of a batch for this block's bias configuration (every block of an HSTU shares it)."""
+        ts = timestamps.contiguous() if (timestamps is not None and self.use_temporal_bias) else None
+        return Fn.SeqMeta(pad_u8, ts, self.position_bias.bucket_of_delta(L, device), _thresholds_on(device),
+                          self.temporal_bias.num_buckets if self.use_temporal_bias else 0, self.position_bias.num_buckets,
+                          self.position_bias.uniform_of(L, device))
 
     def _params(self):
         tb = self.temporal_bias.temporal_attention_bias.weight if self.use_temporal_bias else None
@@ -207,9 +221,7 @@ class HSTULayer(nn.Module):
     def _run(self, x: torch.Tensor, meta: Fn.SeqMeta, seed: int, seed_dev) -> torch.Tensor:
         if self.precision == "fp32":
             return self._run_f32(x, meta)
-        bf16w = {"proj_w": self._mirror("proj_w", self.projection.weight),
-                 "ffn1_w": self._mirror("ffn1_w", self.ffn[0].weight),
-                 "ffn2_w": self._mirror("ffn2_w", self.ffn[3].weight)}
+        bf16w = self._bf16_weights()
         cfg = dict(H=self.num_heads, npos=self.position_bias.num_buckets,
                    ntime=self.temporal_bias.num_buckets if self.use_temporal_bias else 0,
                    p=self.dropout.p if self.training else 0.0, seed=seed, seed_dev=seed_dev, layer=self.layer_index)
@@ -225,12 +237,7 @@ class HSTULayer(nn.Module):
         require_cuda(x)
         ensure_device(x.device)
         if _meta is None:
-            B, L, _ = x.shape
-            ts = timestamps.contiguous() if (timestamps is not None and self.use_temporal_bias) else None
-            _meta = Fn.SeqMeta(padding_mask.to(torch.uint8).contiguous(), ts,
-                               self.position_bias.bucket_of_delta(L, x.device), _thresholds_on(x.device),
-                               self.temporal_bias.num_buckets if self.use_temporal_bias else 0,
-                               self.position_bias.num_buckets, self.position_bias.uniform_of(L, x.device))
+            _meta = self._seq_meta(padding_mask.to(torch.uint8).contiguous(), timestamps, x.shape[1], x.device)
         return self._run(x, _meta, _seed, _seed_dev)
 
 
@@ -384,8 +391,7 @@ class HSTU(nn.Module):
             l.layer_index = i
         self.final_norm = nn.LayerNorm(embed_dim)
         self.return_train_logits = False
-        self._table_bf16 = None
-        self._table_split = None
+        self._table_casts = {}     # "bf16" / "split" -> (version, tensor): the embedding table's operand copies
         self.precision = "bf16"
         self._bf16_provider = None
         self._grad_sink = None
@@ -421,26 +427,15 @@ class HSTU(nn.Module):
         return self
 
     def _head_logits_f32(self, x: torch.Tensor) -> torch.Tensor:
-        w = self.item_embedding.weight
-        ent = self._table_split
-        if ent is None or ent[0] != w._version or ent[1].device != w.device:
-            ent = (w._version, Fn.split3(w, 1))
-            self._table_split = ent
+        split = _cached(self._table_casts, "split", self.item_embedding.weight, _split3_weight)
         xf = Fn.layernorm_f32(x, self.final_norm.weight, self.final_norm.bias, self.final_norm.eps)
-        return Fn.linear_f32x3_bias(Fn.split3(xf, 0), ent[1], None, None, 0)
+        return Fn.linear_f32x3_bias(Fn.split3(xf, 0), split, None, None, 0)
 
     def _table_mirror(self) -> torch.Tensor:
         w = self.item_embedding.weight
         if self._bf16_provider is not None:
             return self._bf16_provider(w)
-        ent = self._table_bf16
-        fresh = ent is not None and ent[0] == w._version and ent[1].device == w.device
-        if self.training and torch.is_grad_enabled():
-            fresh = False
-        if not fresh:
-            ent = (w._version, Fn.cast_bf16(w, ent[1] if ent is not None and ent[1].device == w.device else None))
-            self._table_bf16 = ent
-        return ent[1]
+        return _cached(self._table_casts, "bf16", w, Fn.cast_bf16, remake=self.training and torch.is_grad_enabled())
 
     def _seeds(self, device):
         if not (self.training and self.emb_dropout.p > 0):
@@ -465,12 +460,7 @@ class HSTU(nn.Module):
             esink = (self._grad_sink(self.item_embedding.weight), None)
         x, pad = Fn.EmbedFn.apply(input_ids, self.item_embedding.weight, None, 1.0, 0, p, seed, seed_dev, esink)
         if len(self.layers):
-            ts = timestamps.contiguous() if (timestamps is not None and self.use_temporal_bias) else None
-            meta = Fn.SeqMeta(pad, ts, self.layers[0].position_bias.bucket_of_delta(L, input_ids.device),
-                              _thresholds_on(input_ids.device),
-                              self.layers[0].temporal_bias.num_buckets if self.use_temporal_bias else 0,
-                              self.layers[0].position_bias.num_buckets,
-                              self.layers[0].position_bias.uniform_of(L, input_ids.device))
+            meta = self.layers[0]._seq_meta(pad, timestamps, L, input_ids.device)
             for layer in self.layers:
                 layer._bf16_provider = self._bf16_provider
                 x = layer(x, None, None, timestamps, _meta=meta, _seed=seed, _seed_dev=seed_dev)
@@ -577,11 +567,8 @@ class HSTU(nn.Module):
             ntime = self.layers[0].temporal_bias.num_buckets if use_time else 0
             for i, layer in enumerate(self.layers):
                 layer._bf16_provider = self._bf16_provider
-                bf16w = {"proj_w": layer._mirror("proj_w", layer.projection.weight),
-                         "ffn1_w": layer._mirror("ffn1_w", layer.ffn[0].weight),
-                         "ffn2_w": layer._mirror("ffn2_w", layer.ffn[3].weight)}
                 x = Fn.hstu_layer_extend(x, cache, i, positions, pos_bucket, bucket0, _thresholds_on(dev), layer.num_heads, rpb.num_buckets,
-                                         ntime, bf16w, layer._params(), users=users)
+                                         ntime, layer._bf16_weights(), layer._params(), users=users)
         return x
 
     def _hidden_logits(self, hidden: torch.Tensor) -> torch.Tensor:

@@ -11,7 +11,6 @@ rqvae.py) call the same C entry points; the grad-sink fast path of FlatAdam muta
 ``autograd.Function`` (functional.py)."""
 from __future__ import annotations
 
-import ctypes as C
 from typing import List, Optional, Tuple
 
 import torch
@@ -20,27 +19,18 @@ from torch.library import custom_op
 
 from . import _lib
 from . import functional as Fn
-from ._lib import HstuDims, HstuLayerGrads, HstuLayerParams, HstuSeq, check, ptr, require_cuda, stream_ptr
+from ._lib import HstuDims, check, ptr, require_cuda, stream_ptr
 
 NS = "genrec_b200"
 
 
-def _seq(pad: Tensor, ts: Optional[Tensor], rel32: Optional[Tensor], wide: Optional[Tensor], thr: Tensor, pos_bucket0: int,
-         ntime: int) -> HstuSeq:
-    """Sequence metadata with the [B, L, ld] bias-index matrix the attention kernels read (uniform position buckets: one
-    effective bucket).  The struct holds a reference to the index tensor, which lives as long as the struct."""
-    B, L = pad.shape
-    ld = (L + 7) // 8 * 8
-    index = torch.empty(B, L, ld, dtype=torch.int16, device=pad.device)
-    zero_pb = torch.zeros(L, dtype=torch.uint8, device=pad.device)
-    pad = pad.contiguous()
-    Fn._defer_for_call(False)   # built on the caller's stream: the kernels that read it and the tensor's lifetime follow that stream
-    with torch.cuda.device(pad.device):
-        check(_lib.load().grb_hstu_bias_index(ptr(ts), ptr(pad), ptr(thr), ptr(zero_pb), B, L, 1, ntime if ts is not None else 0, ptr(index), ld,
-                                              stream_ptr(pad.device)))
-    seq = HstuSeq(ptr(index), ld, 1 if ts is not None else 0, 1, int(pos_bucket0), ptr(ts), ptr(pad), ptr(rel32), ptr(wide), ptr(thr))
-    seq.index = index
-    return seq
+def _meta(pad: Tensor, ts: Optional[Tensor], rel32: Optional[Tensor], wide: Optional[Tensor], thr: Tensor, pos_bucket0: int,
+          ntime: int) -> Fn.SeqMeta:
+    """Sequence metadata of one op call: uniform position buckets (bucket pos_bucket0), and the bias-index matrix built on the
+    caller's stream even under the deferred schedule - the kernels that read it and the tensor's lifetime follow that stream."""
+    meta = Fn.SeqMeta(pad, ts, None, thr, ntime, 1, (True, int(pos_bucket0)), may_defer=False)
+    meta.rel32, meta.wide = rel32, wide
+    return meta
 
 
 # ------------------------------------------------------------------------------------------------ sequence preparation
@@ -68,16 +58,9 @@ def hstu_attention(P: Tensor, pad: Tensor, timestamps: Optional[Tensor], rel32: 
                    pos_table: Tensor, time_table: Optional[Tensor], num_heads: int, pos_bucket0: int) -> Tensor:
     """P [B, L, 4D] bf16 = [U | V | Q | K] -> O [B, L, D] bf16 = silu(Q K^T + bias) V, causal + key padding (hstu.py:244-267)."""
     require_cuda(P)
-    B, L, D4 = P.shape
-    D = D4 // 4
-    has_time = time_table is not None and timestamps is not None
-    dims = HstuDims(B, L, D, num_heads, pos_table.shape[0], time_table.shape[0] if has_time else 0, 0.0, 0, None, 0)
-    O = torch.empty(B, L, D, dtype=torch.bfloat16, device=P.device)
-    seq = _seq(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0, dims.ntime)
-    with torch.cuda.device(P.device):
-        check(_lib.load().grb_hstu_attention_forward(C.byref(dims), ptr(pos_table), ptr(time_table) if has_time else None, C.byref(seq),
-                                                     ptr(P.contiguous()), ptr(O), stream_ptr(P.device)))
-    return O
+    ntime = time_table.shape[0] if time_table is not None else 0
+    meta = _meta(pad, timestamps if time_table is not None else None, rel32, wide, time_thr, pos_bucket0, ntime)
+    return Fn.hstu_attention_fwd(P.contiguous(), meta, num_heads, pos_table, time_table, ntime)
 
 
 @hstu_attention.register_fake
@@ -91,20 +74,11 @@ def hstu_attention_backward(P: Tensor, zp: Tensor, dO: Tensor, pad: Tensor, time
                             wide: Optional[Tensor], time_thr: Tensor, pos_table: Tensor, time_table: Optional[Tensor], num_heads: int,
                             pos_bucket0: int) -> Tuple[Tensor, Tensor, Tensor]:
     """-> dzp [B, L, 4D] bf16 (gradient w.r.t. the PRE-activations zp, columns V, Q, K; U = 0), dpos_table, dtime_table (fp32)."""
-    B, L, D4 = P.shape
-    D = D4 // 4
-    has_time = time_table is not None and timestamps is not None
-    dims = HstuDims(B, L, D, num_heads, pos_table.shape[0], time_table.shape[0] if has_time else 0, 0.0, 0, None, 0)
-    lib = _lib.load()
-    dzp = torch.zeros(B, L, D4, dtype=torch.bfloat16, device=P.device)
-    dpos = torch.zeros(pos_table.shape, dtype=torch.float32, device=P.device)
-    dtime = torch.zeros(time_table.shape if time_table is not None else (0, num_heads), dtype=torch.float32, device=P.device)
-    scratch = torch.empty(lib.grb_hstu_attention_scratch_bytes(C.byref(dims)), dtype=torch.uint8, device=P.device)
-    seq = _seq(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0, dims.ntime)
-    with torch.cuda.device(P.device):
-        check(lib.grb_hstu_attention_backward(C.byref(dims), ptr(pos_table), ptr(time_table) if has_time else None, C.byref(seq),
-                                              ptr(P.contiguous()), ptr(zp.contiguous()), ptr(dO.contiguous()), ptr(dzp), ptr(dpos),
-                                              ptr(dtime) if has_time else None, ptr(scratch), stream_ptr(P.device)))
+    ntime = time_table.shape[0] if time_table is not None else 0
+    meta = _meta(pad, timestamps if time_table is not None else None, rel32, wide, time_thr, pos_bucket0, ntime)
+    dzp, dpos, dtime = Fn.hstu_attention_bwd(P.contiguous(), zp.contiguous(), dO.contiguous(), meta, num_heads, pos_table, time_table, ntime)
+    if dtime is None:       # no temporal term: an all-zero gradient of the table, or [0, H] without one
+        dtime = torch.zeros(time_table.shape if time_table is not None else (0, num_heads), dtype=torch.float32, device=P.device)
     return dzp, dpos, dtime
 
 
@@ -115,19 +89,15 @@ def _(P, zp, dO, pad, timestamps, rel32, wide, time_thr, pos_table, time_table, 
 
 
 # ------------------------------------------------------------------------------------------------ the whole block
-_PNAMES = ("proj_w", "proj_b", "pos_table", "time_table", "ln1_g", "ln1_b", "ffn1_w", "ffn1_b", "ffn2_w", "ffn2_b", "ln2_g", "ln2_b")
-
-
-def _layer_structs(x, pad, timestamps, rel32, wide, time_thr, params: List[Optional[Tensor]], bf16w: List[Tensor], H, ntime, pos_bucket0, p, seed,
-                   seed_dev, layer):
-    B, L, D = x.shape
-    named = dict(zip(_PNAMES, params))
+def _layer_call(shape, pad, timestamps, rel32, wide, time_thr, params: List[Optional[Tensor]], H, ntime, pos_bucket0, p, seed, seed_dev,
+                layer):
+    """-> (dims, bf16 weight mirrors, has_time, meta) of one block op; params in Fn.PARAM_ORDER."""
+    B, L, D = shape
+    named = dict(zip(Fn.PARAM_ORDER, params))
+    bf16w = {n: Fn.cast_bf16(named[n]) for n in Fn.BF16_PARAMS}
     has_time = named["time_table"] is not None and timestamps is not None
-    dims = HstuDims(B, L, D, H, named["pos_table"].shape[0], ntime if has_time else 0, float(p), int(seed) & (2 ** 64 - 1), ptr(seed_dev), layer)
-    bw = dict(zip(("proj_w", "ffn1_w", "ffn2_w"), bf16w))
-    ps = HstuLayerParams(*[ptr(bw[n]) if n in bw else (ptr(named[n]) if named[n] is not None and (n != "time_table" or has_time) else None)
-                           for n in _PNAMES])
-    return dims, ps, _seq(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0, dims.ntime), named, has_time
+    dims = Fn._dims(B, L, D, H, named["pos_table"].shape[0], ntime if has_time else 0, p, seed, seed_dev, layer)
+    return dims, bf16w, has_time, _meta(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0, dims.ntime)
 
 
 @custom_op(f"{NS}::hstu_layer", mutates_args=())
@@ -138,33 +108,18 @@ def hstu_layer(x: Tensor, pad: Tensor, timestamps: Optional[Tensor], rel32: Opti
     """One HSTU block (hstu.py:222-280): x [B, L, D] fp32 -> (y [B, L, D] fp32, saved-for-backward blob uint8).  fp32 master
     weights in; the bf16 operand copies are made inside (one cast kernel each)."""
     require_cuda(x)
-    lib = _lib.load()
     params = [proj_w, proj_b, pos_table, time_table, ln1_g, ln1_b, ffn1_w, ffn1_b, ffn2_w, ffn2_b, ln2_g, ln2_b]
-    bf16w = [Fn.cast_bf16(w) for w in (proj_w, ffn1_w, ffn2_w)]
-    xc = x.contiguous().float()
-    dims, ps, seq, _, _ = _layer_structs(xc, pad, timestamps, rel32, wide, time_thr, params, bf16w, num_heads, ntime, pos_bucket0, dropout_p, seed,
-                                         seed_dev, layer_index)
-    nbytes = lib.grb_hstu_layer_saved_bytes(C.byref(dims))
-    if nbytes == 0:
-        raise _lib.GrbError(lib.grb_last_error().decode())
-    saved = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
-    y = torch.empty_like(xc)
-    with torch.cuda.device(x.device):
-        check(lib.grb_hstu_layer_forward(C.byref(dims), C.byref(ps), C.byref(seq), ptr(xc), ptr(y), ptr(saved), stream_ptr(x.device)))
-    return y, saved
-
-
-def _saved_bytes(B, L, D):
-    T = B * L
-    al = lambda n: (n + 255) // 256 * 256
-    return sum(al(n) for n in (T * D * 2, T * 4 * D * 2, T * 4 * D * 2, T * D * 2, T * 8, T * D * 4, T * D * 2, T * 8, T * 4 * D * 2, T * 4 * D * 2))
+    dims, bf16w, has_time, meta = _layer_call(x.shape, pad, timestamps, rel32, wide, time_thr, params, num_heads, ntime, pos_bucket0,
+                                              dropout_p, seed, seed_dev, layer_index)
+    return Fn.hstu_block_forward(dims, params, bf16w, has_time, meta, x.contiguous().float())
 
 
 @hstu_layer.register_fake
 def _(x, pad, timestamps, rel32, wide, time_thr, proj_w, proj_b, pos_table, time_table, ln1_g, ln1_b, ffn1_w, ffn1_b, ffn2_w, ffn2_b, ln2_g, ln2_b,
       num_heads, ntime, pos_bucket0, dropout_p, seed, seed_dev, layer_index):
     B, L, D = x.shape
-    return x.new_empty(x.shape, dtype=torch.float32), x.new_empty((_saved_bytes(B, L, D),), dtype=torch.uint8)
+    nbytes = Fn.layer_saved_bytes(HstuDims(B, L, D, num_heads, pos_table.shape[0], 0, 0.0, 0, None, 0))   # depends on B, L, D only
+    return x.new_empty(x.shape, dtype=torch.float32), x.new_empty((nbytes,), dtype=torch.uint8)
 
 
 @custom_op(f"{NS}::hstu_layer_backward", mutates_args=())
@@ -175,23 +130,11 @@ def hstu_layer_backward(dy: Tensor, saved: Tensor, pad: Tensor, timestamps: Opti
                         layer_index: int) -> List[Tensor]:
     """-> [dx, d proj_w, d proj_b, d pos_table, d time_table, d ln1_g, d ln1_b, d ffn1_w, d ffn1_b, d ffn2_w, d ffn2_b, d ln2_g, d ln2_b]
     (fp32; d time_table is an empty [0, H] tensor when the block has no temporal bias)."""
-    lib = _lib.load()
     params = [proj_w, proj_b, pos_table, time_table, ln1_g, ln1_b, ffn1_w, ffn1_b, ffn2_w, ffn2_b, ln2_g, ln2_b]
-    bf16w = [Fn.cast_bf16(w) for w in (proj_w, ffn1_w, ffn2_w)]
-    dyc = dy.contiguous().float()
-    dims, ps, seq, named, has_time = _layer_structs(dyc, pad, timestamps, rel32, wide, time_thr, params, bf16w, num_heads, ntime, pos_bucket0,
-                                                    dropout_p, seed, seed_dev, layer_index)
-    grads = {n: (torch.zeros(named[n].shape, dtype=torch.float32, device=dy.device) if named[n] is not None else None) for n in _PNAMES}
-    gs = HstuLayerGrads(*[ptr(grads[n]) for n in _PNAMES])
-    dx = torch.empty_like(dyc)
-    ws = torch.empty(lib.grb_hstu_layer_workspace_bytes(C.byref(dims)), dtype=torch.uint8, device=dy.device)
-    with torch.cuda.device(dy.device):
-        check(lib.grb_hstu_layer_backward(C.byref(dims), C.byref(ps), C.byref(seq), ptr(dyc), ptr(saved), ptr(dx), C.byref(gs), ptr(ws),
-                                          stream_ptr(dy.device)))
-    out = [dx]
-    for n in _PNAMES:
-        out.append(grads[n] if grads[n] is not None else torch.zeros(0, num_heads, dtype=torch.float32, device=dy.device))
-    return out
+    dims, bf16w, has_time, meta = _layer_call(dy.shape, pad, timestamps, rel32, wide, time_thr, params, num_heads, ntime, pos_bucket0,
+                                              dropout_p, seed, seed_dev, layer_index)
+    dx, grads = Fn.hstu_block_backward(dims, params, bf16w, has_time, meta, dy, saved)
+    return [dx] + [g if g is not None else torch.zeros(0, num_heads, dtype=torch.float32, device=dy.device) for g in grads]
 
 
 @hstu_layer_backward.register_fake

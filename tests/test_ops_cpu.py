@@ -1,6 +1,30 @@
 """torch.ops.genrec_b200.*: schemas are registered and the FakeTensor implementations + autograd wiring trace without a GPU."""
+import ctypes
+
+import pytest
 import torch
 from torch._subclasses.fake_tensor import FakeTensorMode
+
+
+@pytest.fixture(scope="module", autouse=True)
+def lib():
+    """The fake implementation of hstu_layer sizes its blob with the library's host-side query."""
+    from genrec_b200 import build
+    build.build()
+    from genrec_b200 import _lib
+    return _lib.load()
+
+
+@pytest.mark.parametrize("D", [64, 128, 256])
+def test_fake_saved_blob_matches_the_library(lib, D):
+    import genrec_b200.ops  # noqa: F401
+    from genrec_b200._lib import HstuDims
+    B, L, H = 3, 77, D // 64
+    with FakeTensorMode():
+        a = _layer_args(B, L, D, H, "cuda")
+        _, saved = torch.ops.genrec_b200.hstu_layer(a["x"], a["pad"], a["ts"], a["rel"], a["wide"], a["thr"], *a["params"], H, 64, 0, 0.1, 7,
+                                                    None, 0)
+    assert saved.shape == (lib.grb_hstu_layer_saved_bytes(ctypes.byref(HstuDims(B, L, D, H, 32, 64, 0.1, 7, None, 0))),)
 
 
 def test_ops_are_registered_with_schemas():
