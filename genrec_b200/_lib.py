@@ -108,16 +108,17 @@ SIGNATURES = {
                                    c_u64, c_void_p, c_u32, c_void_p]),
     "grb_linear_residual_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
                                             c_float, c_u64, c_void_p, c_u32, c_void_p]),
+    "grb_linear_backward_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "grb_linear_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
-                                    c_void_p, c_void_p]),
-    "grb_dact": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
+                                    c_void_p, c_void_p, c_void_p]),
     "grb_linear_dact_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_u64, c_void_p, c_u32,
                                          c_void_p, c_void_p]),
     "grb_cast_rows_f32_to_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_float, c_u64, c_void_p, c_u32, c_void_p]),
     "grb_layernorm_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                       c_void_p]),
+    "grb_layernorm_backward_workspace_bytes": (c_size_t, [c_int, c_int]),
     "grb_layernorm_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
-                                       c_void_p, c_void_p]),
+                                       c_void_p, c_void_p, c_void_p]),
     "grb_split3_f32_to_bf16": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p]),
     "grb_linear_f32x3_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "grb_linear_f32x3_bias_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),

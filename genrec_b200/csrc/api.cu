@@ -149,41 +149,29 @@ int det_finish(const float* part, int ngroups, int nmembers, int W, int gpo, int
     return 0;
 }
 
-// ---- GEMMs: the wgmma/TMA kernel of tc_gemm.cuh with a fused epilogue.  Operand majors: *_MN = 0 -> K contiguous,
-//      1 -> M/N contiguous.
-int tn_splits(int M, int N, int K) {
-    int tiles = ((M + TC_BM - 1) / TC_BM) * ((N + TC_BN - 1) / TC_BN);
-    int want = (sm_count() + tiles - 1) / tiles;
-    int kb = (K + TC_BK - 1) / TC_BK;
-    int maxs = kb / 2 > 0 ? kb / 2 : 1;
-    return want < 1 ? 1 : (want > maxs ? maxs : want);
-}
+// ---- GEMMs: the wgmma/TMA kernel of tc_gemm.cuh with a fused epilogue.  A is K contiguous; B_MN = 0 -> B K contiguous,
+//      1 -> N contiguous.
 // z = x W^T + b ; act: 0 none, 1 silu, 2 relu   (NT)
 cudaError_t gemm_bias_act(int act, const bf16* x, const bf16* w, const float* bias, bf16* z, bf16* a, int M, int N, int K, const Dropout& drop,
                           cudaStream_t st) {
-    if (act == 0) return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasAct<0>{bias, N, drop}, z, nullptr, N, sm_count(), st);
-    if (act == 1) return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasAct<1>{bias, N, drop}, z, a, N, sm_count(), st);
-    return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasAct<2>{bias, N, drop}, z, a, N, sm_count(), st);
+    if (act == 0) return launch_tc_gemm<0>(x, w, M, N, K, K, K, TcEpiBiasAct<0>{bias, N, drop}, z, nullptr, N, sm_count(), st);
+    if (act == 1) return launch_tc_gemm<0>(x, w, M, N, K, K, K, TcEpiBiasAct<1>{bias, N, drop}, z, a, N, sm_count(), st);
+    return launch_tc_gemm<0>(x, w, M, N, K, K, K, TcEpiBiasAct<2>{bias, N, drop}, z, a, N, sm_count(), st);
 }
 // y = res + drop(x W^T + b) (* row_scale)   (NT)
 cudaError_t gemm_bias_res(const bf16* x, const bf16* w, const float* bias, const float* res, const float* row_scale, float* y, int M, int N,
                           int K, const Dropout& drop, cudaStream_t st) {
-    return launch_tc_gemm<0, 0>(x, w, M, N, K, K, K, 1, TcEpiBiasResidual{bias, res, row_scale, N, drop}, y, nullptr, N, sm_count(), st);
+    return launch_tc_gemm<0>(x, w, M, N, K, K, K, TcEpiBiasResidual{bias, res, row_scale, N, drop}, y, nullptr, N, sm_count(), st);
 }
 // g[M,N] = dropmask(dy[M,K] W[K,N]) * act'(z)   (NN) ; act 1 silu, 2 relu
 cudaError_t gemm_dact(int act, const bf16* dy, const bf16* w, const bf16* z, bf16* g, int M, int N, int K, const Dropout& drop, cudaStream_t st) {
-    if (act == 1) return launch_tc_gemm<0, 1>(dy, w, M, N, K, K, N, 1, TcEpiDAct<1>{z, N, drop}, g, nullptr, N, sm_count(), st);
-    return launch_tc_gemm<0, 1>(dy, w, M, N, K, K, N, 1, TcEpiDAct<2>{z, N, drop}, g, nullptr, N, sm_count(), st);
+    if (act == 1) return launch_tc_gemm<1>(dy, w, M, N, K, K, N, TcEpiDAct<1>{z, N, drop}, g, nullptr, N, sm_count(), st);
+    return launch_tc_gemm<1>(dy, w, M, N, K, K, N, TcEpiDAct<2>{z, N, drop}, g, nullptr, N, sm_count(), st);
 }
 // out[M,N] fp32 = scale * A[M,K] B[K,N] (+ res)   (NN)
 cudaError_t gemm_nn_f32(const bf16* A, const bf16* B, float* out, const float* res, float scale, int M, int N, int K, int lda, int ldb,
                         cudaStream_t st) {
-    return launch_tc_gemm<0, 1>(A, B, M, N, K, lda, ldb, 1, TcEpiF32{res, N, scale}, out, nullptr, N, sm_count(), st);
-}
-// out[M,N] fp32 += A^T B with A stored [K,M], B stored [K,N]   (TN, split-K, float atomics: the summation order varies from run to
-// run).  Only grb_linear_backward uses it, because its ABI has no workspace for the ordered split-K sum of launch_tc_tn_group.
-cudaError_t gemm_tn_atomic(const bf16* A, const bf16* B, float* out, int M, int N, int K, int lda, int ldb, cudaStream_t st) {
-    return launch_tc_gemm<1, 1>(A, B, M, N, K, lda, ldb, tn_splits(M, N, K), TcEpiAtomicF32{out, N, 1.f}, nullptr, nullptr, 0, sm_count(), st);
+    return launch_tc_gemm<1>(A, B, M, N, K, lda, ldb, TcEpiF32{res, N, scale}, out, nullptr, N, sm_count(), st);
 }
 
 // ---- carved layouts ------------------------------------------------------------------------------------------
@@ -462,14 +450,19 @@ int cast_colsum(const float* in, bf16* out, int T, int D, const Dropout& drop, f
     GRB_TRY(det_finish(part, grid.x, grid.y, 128, grid.x, 128, 1, {{colsum_out, D}}, st));
     return 0;
 }
-// part (nullable): colsum_grid(T, N).x * .y * 256 floats of scratch for the ordered sum; without it one atomic add per CTA
+// part: colsum_grid(T, N).x * .y * 256 floats of scratch for the ordered sum
 int colsum(const bf16* in, int T, int N, int ld, float* out, float* part, cudaStream_t st) {
     if (N % 8 != 0 || ld % 8 != 0) return fail(GRB_EINVAL, "colsum needs N and ld to be multiples of 8");
     const dim3 grid = colsum_grid(T, N);
-    launch_k(colsum_bf16_kernel, grid, 256, 0, st, in, T, N, ld, out, part);
+    launch_k(colsum_bf16_kernel, grid, 256, 0, st, in, T, N, ld, part);
     GRB_CUDA(cudaGetLastError());
-    if (part) GRB_TRY(det_finish(part, grid.x, grid.y, 256, grid.x, 256, 1, {{out, N}}, st));
+    GRB_TRY(det_finish(part, grid.x, grid.y, 256, grid.x, 256, 1, {{out, N}}, st));
     return 0;
+}
+// dx = (res ? res : 0) + LNbwd(dy) ; dg += , db += in a fixed order.  a.part: 2 * row_bwd_grid(T) * D floats of scratch
+int ln_backward(const LnBwdArgs& a, cudaStream_t st) {
+    GRB_TRY(with_row_dim(a.D, [&](auto DC) { launch_k(ln_bwd_kernel<DC / 64>, row_bwd_grid(a.T), ROW_THREADS, 0, st, a); }));
+    return det_finish(a.part, 2, row_bwd_grid(a.T), a.D, 1, 0, 1, {{a.dg, a.D}, {a.db, a.D}}, st);
 }
 
 // ---- cached incremental inference (attn_hstu_extend.cuh)
@@ -1004,8 +997,8 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
         }));
     } else {
     // logits = xf E^T   (hstu.py:137)
-    GRB_CUDA((launch_tc_gemm<0, 0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, 1, TcEpiF32{nullptr, h.ldl, 1.f}, h.logits32, nullptr, h.ldl,
-                                   sm_count(), st)));
+    GRB_CUDA((launch_tc_gemm<0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, TcEpiF32{nullptr, h.ldl, 1.f}, h.logits32, nullptr, h.ldl,
+                                sm_count(), st)));
     if (h.ldl / 8 <= 256 * 8)
         launch_k(ce_fwd_bwd_vec_kernel<8>, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0,
                  (const float*)h.logits32);
@@ -1024,12 +1017,7 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
         return 0;
     }));
     }
-    {
-        LnBwdArgs a{h.dxf, x, h.stf, ln_g, nullptr, dx, dln_g, dln_b, T, D, h.part_ln};
-        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_bwd_kernel<DC / 64>, row_bwd_grid(T), ROW_THREADS, 0, st, a); }));
-        GRB_TRY(det_finish(h.part_ln, 2, row_bwd_grid(T), D, 1, 0, 1, {{a.dg, D}, {a.db, D}}, st));
-    }
-    return 0;
+    return ln_backward(LnBwdArgs{h.dxf, x, h.stf, ln_g, nullptr, dx, dln_g, dln_b, T, D, h.part_ln}, st);
 }
 
 int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int T, int D, int C,
@@ -1043,7 +1031,7 @@ int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float 
         GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
     }
     // logits [T, C] fp32, leading dimension C of any parity
-    GRB_CUDA((launch_tc_gemm<0, 0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, 1, TcEpiF32Plain{logits, C}, nullptr, nullptr, 0, sm_count(), st)));
+    GRB_CUDA((launch_tc_gemm<0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, TcEpiF32Plain{logits, C}, nullptr, nullptr, 0, sm_count(), st)));
     return 0;
 }
 
@@ -1130,40 +1118,47 @@ int grb_linear_residual_forward(const void* x_bf16, const void* w_bf16, const fl
                            make_dropout(dropout_p, seed, site, seed_dev), static_cast<cudaStream_t>(stream)));
     return 0;
 }
+namespace {
+struct LinearBwdWork {
+    float *part_colsum, *part_tn;
+    size_t bytes;
+};
+// dW [N, K] += dy^T x: one problem of the grouped weight-gradient GEMM, dy [T, N] and x [T, K] stored token-major
+TnSpec linear_dw_spec(const void* dy_bf16, const void* x_bf16, float* dw, int T, int N, int K) {
+    return TnSpec{(const bf16*)dy_bf16, (const bf16*)x_bf16, dw, N, K, T, N, K, K};
+}
+LinearBwdWork carve_linear_bwd(void* base, int T, int N, int K) {
+    LinearBwdWork w;
+    Carver c{static_cast<char*>(base)};
+    const dim3 cg = colsum_grid(T, N);
+    w.part_colsum = c.take<float>((size_t)cg.x * cg.y * 256 * 4);
+    const TnSpec spec = linear_dw_spec(nullptr, nullptr, nullptr, T, N, K);
+    w.part_tn = c.take<float>(tn_part_floats(&spec, 1, sm_count()) * 4);
+    w.bytes = c.off;
+    return w;
+}
+}  // namespace
+
+size_t grb_linear_backward_workspace_bytes(int T, int N, int K) {
+    if (T <= 0 || N <= 0 || K <= 0) return 0;
+    return carve_linear_bwd(nullptr, T, N, K).bytes;
+}
 int grb_linear_backward(const void* dy_bf16, const void* w_bf16, const void* x_bf16, int T, int N, int K, float* dx_f32,
-                        const float* dx_residual, float* dw, float* db, void* stream) {
+                        const float* dx_residual, float* dw, float* db, void* workspace, void* stream) {
     GRB_REQUIRE(dy_bf16 && w_bf16, "null argument");
     GRB_REQUIRE(T > 0 && N % 8 == 0 && K % 8 == 0, "N and K must be multiples of 8");
+    GRB_REQUIRE(workspace || (!dw && !db), "workspace is null");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (db) GRB_TRY(colsum((const bf16*)dy_bf16, T, N, N, db, nullptr, st));
+    const LinearBwdWork w = carve_linear_bwd(workspace, T, N, K);
+    if (db) GRB_TRY(colsum((const bf16*)dy_bf16, T, N, N, db, w.part_colsum, st));
     if (dw) {
         GRB_REQUIRE(x_bf16, "x is null");
-        GRB_CUDA(gemm_tn_atomic((const bf16*)dy_bf16, (const bf16*)x_bf16, dw, N, K, T, N, K, st));
+        const TnSpec spec = linear_dw_spec(dy_bf16, x_bf16, dw, T, N, K);
+        GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), w.part_tn, st));
     }
     if (dx_f32) {
         GRB_CUDA(gemm_nn_f32((const bf16*)dy_bf16, (const bf16*)w_bf16, dx_f32, dx_residual, 1.f, T, K, N, N, K, st));
     }
-    return 0;
-}
-
-namespace {
-__global__ void dact_kernel(bf16* g, const bf16* z, size_t n, int act) {
-    pdl_wait();
-    size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 2;
-    size_t stride = (size_t)gridDim.x * blockDim.x * 2;
-    for (; i < n; i += stride) {
-        float2 gv = unpack_bf16(*reinterpret_cast<const uint32_t*>(g + i));
-        float2 zv = unpack_bf16(*reinterpret_cast<const uint32_t*>(z + i));
-        float d0 = act == 1 ? dsiluf(zv.x) : (zv.x > 0.f ? 1.f : 0.f);
-        float d1 = act == 1 ? dsiluf(zv.y) : (zv.y > 0.f ? 1.f : 0.f);
-        *reinterpret_cast<uint32_t*>(g + i) = pack_bf16(gv.x * d0, gv.y * d1);
-    }
-}
-}  // namespace
-int grb_dact(const void* g_bf16_in_out, const void* z_bf16, size_t n, int act, void* stream) {
-    GRB_REQUIRE(g_bf16_in_out && z_bf16 && n % 2 == 0 && (act == 1 || act == 2), "bad argument");
-    launch_k(dact_kernel, capped_blocks(n / 2), 256, 0, static_cast<cudaStream_t>(stream), (bf16*)const_cast<void*>(g_bf16_in_out), (const bf16*)z_bf16, n, act);
-    GRB_CUDA(cudaGetLastError());
     return 0;
 }
 
@@ -1189,12 +1184,14 @@ int grb_layernorm_forward(const float* x, const float* g, const float* b, float 
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     return with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); });
 }
+size_t grb_layernorm_backward_workspace_bytes(int T, int D) {
+    if (T <= 0 || D <= 0) return 0;
+    return (size_t)2 * row_bwd_grid(T) * D * 4;
+}
 int grb_layernorm_backward(const float* dy, const float* x, const float* stats, const float* g, const float* residual, int T, int D,
-                           float* dx, float* dg, float* db, void* stream) {
-    GRB_REQUIRE(dy && x && stats && g && dx && dg && db, "null argument");
-    LnBwdArgs a{dy, x, stats, g, residual, dx, dg, db, T, D};
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    return with_row_dim(D, [&](auto DC) { launch_k(ln_bwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); });
+                           float* dx, float* dg, float* db, void* workspace, void* stream) {
+    GRB_REQUIRE(dy && x && stats && g && dx && dg && db && workspace, "null argument");
+    return ln_backward(LnBwdArgs{dy, x, stats, g, residual, dx, dg, db, T, D, static_cast<float*>(workspace)}, static_cast<cudaStream_t>(stream));
 }
 
 int grb_split3_f32_to_bf16(const float* in, void* out_bf16, size_t rows, int K, int operand, void* stream) {
@@ -1212,9 +1209,9 @@ static int linear_f32x3(const bf16* xs, const bf16* ws, const float* bias, const
     // the running sum per step: 288 steps over the six-term K (K = 768) measured 2e-5.  The five small cross terms (<= 2^-8 of
     // the result) are therefore summed on their own (their truncation is 2^-8 smaller), and the hi*hi term, K/16 steps, is
     // added to that sum in the epilogue of a second pass together with bias, activation and residual.  y doubles as the scratch of pass 1.
-    GRB_CUDA((launch_tc_gemm<0, 0>(xs + K, ws + K, T, N, 5 * K, K6, K6, 1, TcEpiF32{nullptr, ldy, 1.f}, y, nullptr, ldy, sm_count(), st)));
-    if (act == 1) GRB_CUDA((launch_tc_gemm<0, 0>(xs, ws, T, N, K, K6, K6, 1, TcEpiActResF32<1>{y, ldy, bias, res2}, y, nullptr, ldy, sm_count(), st)));
-    else GRB_CUDA((launch_tc_gemm<0, 0>(xs, ws, T, N, K, K6, K6, 1, TcEpiActResF32<0>{y, ldy, bias, res2}, y, nullptr, ldy, sm_count(), st)));
+    GRB_CUDA((launch_tc_gemm<0>(xs + K, ws + K, T, N, 5 * K, K6, K6, TcEpiF32{nullptr, ldy, 1.f}, y, nullptr, ldy, sm_count(), st)));
+    if (act == 1) GRB_CUDA((launch_tc_gemm<0>(xs, ws, T, N, K, K6, K6, TcEpiActResF32<1>{y, ldy, bias, res2}, y, nullptr, ldy, sm_count(), st)));
+    else GRB_CUDA((launch_tc_gemm<0>(xs, ws, T, N, K, K6, K6, TcEpiActResF32<0>{y, ldy, bias, res2}, y, nullptr, ldy, sm_count(), st)));
     return 0;
 }
 int grb_linear_f32x3_forward(const void* x_split_bf16, const void* w_split_bf16, int T, int N, int K, int act, float* y, void* stream) {

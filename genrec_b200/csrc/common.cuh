@@ -242,9 +242,7 @@ GRB_DEVINL int lane_b_col(int lane) { return ((lane >> 3) & 1) * 8; }
 // Float atomics from many CTAs add in whatever order the CTAs finish, so the last bits of a gradient (and through Adam the
 // parameters) would change from run to run.  The cross-CTA reductions of the training step are split in two instead: each CTA
 // stores its partials to scratch from the caller's workspace (det_store, layout [group][member][W]), and det_finish_kernel,
-// launched right after on the same stream, sums them in a fixed order and adds the result once.  Two kernels also keep one
-// atomic add per CTA for the entry points whose ABI has no workspace: ln_bwd_kernel for grb_layernorm_backward and
-// colsum_bf16_kernel for grb_linear_backward.
+// launched right after on the same stream, sums them in a fixed order and adds the result once.
 template <class F>
 GRB_DEVINL void det_store(float* part, int group, int member, int nmembers, int W, int n, F vals) {
     float* dst = part + ((size_t)group * nmembers + member) * W;

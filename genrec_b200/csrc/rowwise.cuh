@@ -247,7 +247,7 @@ struct LnBwdArgs {
     const float* res;  // nullable, added to dx
     float* dx; float *dg, *db;
     int T, D;
-    float* part;       // nullable: [2][gridDim.x][D] scratch for the ordered cross-CTA sum (det_finish_kernel)
+    float* part;       // [2][gridDim.x][D] scratch for the ordered cross-CTA sum (det_finish_kernel adds it to dg, db)
 };
 template <int NP>
 __global__ void __launch_bounds__(ROW_THREADS) ln_bwd_kernel(LnBwdArgs a) {
@@ -302,8 +302,7 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_bwd_kernel(LnBwdArgs a) {
             for (int w = 0; w < ROW_THREADS / 32; ++w) s += red[which][w][c];
             return s;
         };
-        if (a.part) det_store(a.part, which, blockIdx.x, gridDim.x, a.D, a.D, colsum);
-        else for (int c = threadIdx.x; c < a.D; c += ROW_THREADS) atomicAdd((which ? a.db : a.dg) + c, colsum(c));
+        det_store(a.part, which, blockIdx.x, gridDim.x, a.D, a.D, colsum);
     }
 }
 
@@ -379,10 +378,10 @@ __global__ void __launch_bounds__(256) cast_colsum_f32_bf16_kernel(const float* 
     };
     det_store(part, blockIdx.x, blockIdx.y, gridDim.y, 128, min(128, D - (int)blockIdx.x * 128), sum8);
 }
-// out[c] += sum_r in[r, c]   in: bf16 [T, ld] (ld % 8 == 0), columns [0, N) ; grid (ceil(N/256), chunks) ;
+// the per-CTA column sums of in: bf16 [T, ld] (ld % 8 == 0), columns [0, N) -> part [ceil(N / 256)][chunks][256], which
+// det_finish_kernel adds to the output ; grid (ceil(N/256), chunks) ;
 // block 256 = 32 column groups of 8 (one 16-byte load each) x 8 row lanes, 4 rows in flight per thread
-__global__ void __launch_bounds__(256) colsum_bf16_kernel(const bf16* __restrict__ in, int T, int N, int ld, float* __restrict__ out,
-                                                         float* __restrict__ part) {
+__global__ void __launch_bounds__(256) colsum_bf16_kernel(const bf16* __restrict__ in, int T, int N, int ld, float* __restrict__ part) {
     pdl_wait();
     __shared__ float red[8][256];
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
@@ -428,8 +427,7 @@ __global__ void __launch_bounds__(256) colsum_bf16_kernel(const bf16* __restrict
         return t;
     };
     const int nc = min(256, N - (int)blockIdx.x * 256);
-    if (part) det_store(part, blockIdx.x, blockIdx.y, gridDim.y, 256, nc, sum8);
-    else if ((int)threadIdx.x < nc) atomicAdd(out + blockIdx.x * 256 + threadIdx.x, sum8(threadIdx.x));
+    det_store(part, blockIdx.x, blockIdx.y, gridDim.y, 256, nc, sum8);
 }
 
 // ------------------------------------------------------------------------------------------------ embedding

@@ -1,11 +1,12 @@
 // genrec_b200 - Hopper GEMM: TMA (cp.async.bulk.tensor, 128B swizzle) -> shared-memory ring (mbarrier pipeline) -> wgmma
 // (fp32 accumulators in registers) -> shared-memory accumulator tile -> fused element-wise epilogue -> TMA stores.
 //
-//   C[M,N] (+)= opA(A) * opB(B)          bf16 operands, fp32 accumulate
-//     A_MN = 0 : A stored [M][K] (K contiguous)        A_MN = 1 : A stored [K][M] (M contiguous)
+//   C[M,N] (+)= A * opB(B)               bf16 operands, fp32 accumulate
+//     A stored [M][K] (K contiguous)
 //     B_MN = 0 : B stored [N][K] (K contiguous)        B_MN = 1 : B stored [K][N] (N contiguous)
 //   Both majors map straight onto wgmma shared-memory descriptors (K-major / MN-major canonical SWIZZLE_128B layouts, the
-//   MN-major ones through the instruction's transpose bits), so no operand is ever transposed in memory.
+//   MN-major ones through the instruction's transpose bits), so no operand is ever transposed in memory.  tc_mainloop also takes
+//   an MN-major A, which the grouped weight-gradient GEMM (tc_tn_group.cuh) uses.
 //
 // Persistent kernel, one CTA per SM, 384 threads:
 //   warp 0        : TMA producer (one elected lane)      - ring of TC_STAGES x (A 16 KB + B 16 KB)
@@ -13,7 +14,7 @@
 //   warpgroups 1-2: consumers; warpgroup g issues m64n128k16 wgmma for rows 64*g .. 64*g+63 of the 128 x 128 tile, parks the
 //                   accumulators in shared memory and runs the epilogue on them: its warp w owns 32 rows and one 64-column
 //                   half of the tile (the same row / column split for every epilogue functor below)
-// Work item = (m tile, n tile, k split).  Split-K partial sums go out through an atomic epilogue.
+// Work item = one 128 x 128 output tile over the whole K.
 #pragma once
 #include <cuda.h>
 
@@ -164,17 +165,17 @@ GRB_DEVINL void tc_acc_load32(const float* sAcc, int r, int c, float (&v)[32]) {
 
 struct TcGemmShape {
     int M, N, K;
-    int num_m, num_n, splits;
-    int kblocks_total, kblocks_per_split;
+    int num_m, num_n;
+    int kblocks_total;
 };
 
 // Epilogue concept:
-//   static constexpr int kOut;   0: the functor stores by itself (atomics / odd strides)      signature (row, col0, v, nvalid)
+//   static constexpr int kOut;   0: the functor stores by itself (odd strides)                signature (row, col0, v, nvalid)
 //                                1: one bf16 output tile   2: two bf16 output tiles   3: one fp32 output tile
 //                                   -> signature (row, col0, v /*in: acc, out: primary*/, w /*out: secondary*/, nvalid); the kernel
 //                                      stages the tile in shared memory (128B swizzle) and writes it with TMA stores (tmC0 / tmC1).
 //   void prepare();
-template <int A_MN, int B_MN, class Epi>
+template <int B_MN, class Epi>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC0,
                    const __grid_constant__ CUtensorMap tmC1, TcGemmShape sh, Epi epi) {
@@ -208,7 +209,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     __syncthreads();
     pdl_wait();  // prologue above overlaps the previous kernel's tail
 
-    const int num_work = sh.num_m * sh.num_n * sh.splits;
+    const int num_work = sh.num_m * sh.num_n;
 
     if (warp < 4) {
         // ===================================================================== TMA producer
@@ -216,23 +217,14 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             int stage = 0;
             uint32_t phase = 0, zphase = 0;
             for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-                const int split = w % sh.splits;
-                const int tile = w / sh.splits;
-                const int m0 = (tile / sh.num_n) * TC_BM, n0 = (tile % sh.num_n) * TC_BN;
-                const int kb0 = split * sh.kblocks_per_split;
-                const int kb1 = min(sh.kblocks_total, kb0 + sh.kblocks_per_split);
-                for (int kb = kb0; kb < kb1; ++kb) {
+                const int m0 = (w / sh.num_n) * TC_BM, n0 = (w % sh.num_n) * TC_BN;
+                for (int kb = 0; kb < sh.kblocks_total; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     mbar_expect_tx(&full_bar[stage], 2 * TC_TILE_BYTES);
                     unsigned char* a_dst = sA + stage * TC_TILE_BYTES;
                     unsigned char* b_dst = sB + stage * TC_TILE_BYTES;
                     const int k0 = kb * TC_BK;
-                    if (A_MN == 0) {
-                        tma_load_2d(a_dst, &tmA, k0, m0, &full_bar[stage]);            // box {64 k, 128 rows}
-                    } else {
-                        tma_load_2d(a_dst, &tmA, m0, k0, &full_bar[stage]);            // box {64 m, 64 k-rows}
-                        tma_load_2d(a_dst + TC_TILE_BYTES / 2, &tmA, m0 + 64, k0, &full_bar[stage]);
-                    }
+                    tma_load_2d(a_dst, &tmA, k0, m0, &full_bar[stage]);                // box {64 k, 128 rows}
                     if (B_MN == 0) {
                         tma_load_2d(b_dst, &tmB, k0, n0, &full_bar[stage]);
                     } else {
@@ -263,12 +255,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         uint32_t phase = 0, zphase = 0;
         float acc[64];
         for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-            const int split = w % sh.splits;
-            const int tile = w / sh.splits;
-            const int m0 = (tile / sh.num_n) * TC_BM, n0 = (tile % sh.num_n) * TC_BN;
-            const int kb0 = split * sh.kblocks_per_split;
-            const int kb1 = min(sh.kblocks_total, kb0 + sh.kblocks_per_split);
-            tc_mainloop<A_MN, B_MN, TC_STAGES>(acc, sA, sB, full_bar, empty_bar, kb0, kb1, g, stage, phase);
+            const int m0 = (w / sh.num_n) * TC_BM, n0 = (w % sh.num_n) * TC_BN;
+            tc_mainloop<0, B_MN, TC_STAGES>(acc, sA, sB, full_bar, empty_bar, 0, sh.kblocks_total, g, stage, phase);
             wg_bar_sync(g);                        // the previous tile's epilogue of this warpgroup has read sAcc
             tc_acc_store(sAcc, acc, g);
             wg_bar_sync(g);
@@ -563,22 +551,6 @@ struct TcEpiActResF32 {
         }
     }
 };
-// out += scale * acc (split-K partial sums of grb_linear_backward's weight gradient)
-struct TcEpiAtomicF32 {
-    static constexpr int kOut = 0;
-    static constexpr bool kPre = false;
-    static constexpr bool kAux = false;
-    float* out;
-    int ld;
-    float scale;
-    GRB_DEVINL void prepare() {}
-    GRB_DEVINL void operator()(int row, int col0, const float (&v)[32], int nvalid) const {
-        float* dst = out + (size_t)row * ld + col0;
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-            if (i < nvalid) atomicAdd(dst + i, v[i] * scale);
-    }
-};
 // plain fp32 store, arbitrary leading dimension
 struct TcEpiF32Plain {
     static constexpr int kOut = 0;
@@ -626,13 +598,13 @@ inline bool make_tmap_bf16(CUtensorMap* m, const void* base, uint64_t rows, uint
     return make_tmap(m, base, false, rows, cols, ld, box_cols, box_rows);
 }
 
-// A: A_MN == 0 -> [M][K] ld=lda ; A_MN == 1 -> [K][M] ld=lda.   Same for B with N.
+// A: [M][K] ld=lda.   B: B_MN == 0 -> [N][K] ld=ldb ; B_MN == 1 -> [K][N] ld=ldb.
 // out0 / out1: output tensors [M][N] with leading dimension ldo (bf16 for kOut 1/2, fp32 for kOut 3); unused for kOut 0.
-template <int A_MN, int B_MN, class Epi>
-inline cudaError_t launch_tc_gemm(const bf16* A, const bf16* B, int M, int N, int K, int lda, int ldb, int splits, const Epi& epi,
-                                  void* out0, void* out1, int ldo, int num_sms, cudaStream_t st) {
+template <int B_MN, class Epi>
+inline cudaError_t launch_tc_gemm(const bf16* A, const bf16* B, int M, int N, int K, int lda, int ldb, const Epi& epi, void* out0, void* out1,
+                                  int ldo, int num_sms, cudaStream_t st) {
     CUtensorMap tmA, tmB, tmC0, tmC1;
-    bool ok = A_MN == 0 ? make_tmap_bf16(&tmA, A, M, K, lda, TC_BK, TC_BM) : make_tmap_bf16(&tmA, A, K, M, lda, 64, TC_BK);
+    bool ok = make_tmap_bf16(&tmA, A, M, K, lda, TC_BK, TC_BM);
     ok = ok && (B_MN == 0 ? make_tmap_bf16(&tmB, B, N, K, ldb, TC_BK, TC_BN) : make_tmap_bf16(&tmB, B, K, N, ldb, 64, TC_BK));
     if (Epi::kOut == 0) {
         tmC0 = tmA; tmC1 = tmA;
@@ -654,11 +626,7 @@ inline cudaError_t launch_tc_gemm(const bf16* A, const bf16* B, int M, int N, in
     sh.num_m = (M + TC_BM - 1) / TC_BM;
     sh.num_n = (N + TC_BN - 1) / TC_BN;
     sh.kblocks_total = (K + TC_BK - 1) / TC_BK;
-    if (splits < 1) splits = 1;
-    if (splits > sh.kblocks_total) splits = sh.kblocks_total;
-    sh.kblocks_per_split = (sh.kblocks_total + splits - 1) / splits;
-    sh.splits = (sh.kblocks_total + sh.kblocks_per_split - 1) / sh.kblocks_per_split;
-    auto kern = tc_gemm_kernel<A_MN, B_MN, Epi>;
+    auto kern = tc_gemm_kernel<B_MN, Epi>;
     static bool attr_set_dev[64] = {false};
     int attr_dev = 0;
     cudaGetDevice(&attr_dev);
@@ -668,7 +636,7 @@ inline cudaError_t launch_tc_gemm(const bf16* A, const bf16* B, int M, int N, in
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    int work = sh.num_m * sh.num_n * sh.splits;
+    int work = sh.num_m * sh.num_n;
     int grid = work < num_sms ? work : num_sms;
     launch_k(kern, grid, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, tmC0, tmC1, sh, epi);
     return cudaGetLastError();

@@ -509,7 +509,9 @@ def layernorm_bwd(dy, x, st, g, residual=None):
     dx = torch.empty_like(x)
     dg = torch.zeros_like(g)
     db = torch.zeros_like(g)
-    check(lib.grb_layernorm_backward(ptr(dy), ptr(x), ptr(st), ptr(g), ptr(residual), T, D, ptr(dx), ptr(dg), ptr(db), stream_ptr(x.device)))
+    ws = _u8(lib.grb_layernorm_backward_workspace_bytes(T, D), x.device)
+    check(lib.grb_layernorm_backward(ptr(dy), ptr(x), ptr(st), ptr(g), ptr(residual), T, D, ptr(dx), ptr(dg), ptr(db), ptr(ws),
+                                     stream_ptr(x.device)))
     return dx, dg, db
 
 
@@ -543,7 +545,9 @@ def linear_bwd(dyb, wb, xb, need_dx=True, dx_residual=None, need_dw=True):
     dx = torch.empty(*dyb.shape[:-1], K, dtype=torch.float32, device=dyb.device) if need_dx else None
     dw = torch.zeros(N, K, dtype=torch.float32, device=dyb.device) if need_dw else None
     db = torch.zeros(N, dtype=torch.float32, device=dyb.device) if need_dw else None
-    check(lib.grb_linear_backward(ptr(dyb), ptr(wb), ptr(xb), T, N, K, ptr(dx), ptr(dx_residual), ptr(dw), ptr(db), stream_ptr(dyb.device)))
+    ws = _u8(lib.grb_linear_backward_workspace_bytes(T, N, K), dyb.device) if need_dw else None
+    check(lib.grb_linear_backward(ptr(dyb), ptr(wb), ptr(xb), T, N, K, ptr(dx), ptr(dx_residual), ptr(dw), ptr(db), ptr(ws),
+                                  stream_ptr(dyb.device)))
     return dx, dw, db
 
 
@@ -585,11 +589,6 @@ def cast_rows_bf16(x, row_scale=None, p=0.0, seed=0, seed_dev=None, site=0):
     check(_lib.load().grb_cast_rows_f32_to_bf16(ptr(x), ptr(out), T, D, ptr(row_scale), float(p), int(seed), ptr(seed_dev), site,
                                                 stream_ptr(x.device)))
     return out
-
-
-def dact_(g_bf16, z_bf16, act):
-    check(_lib.load().grb_dact(ptr(g_bf16), ptr(z_bf16), g_bf16.numel(), act, stream_ptr(g_bf16.device)))
-    return g_bf16
 
 
 # ------------------------------------------------------------------------------------------------ RQ-VAE

@@ -257,10 +257,11 @@ int grb_linear_forward(const void* x_bf16, const void* w_bf16, const float* bias
 int grb_linear_residual_forward(const void* x_bf16, const void* w_bf16, const float* bias, const float* residual,
                                 const float* row_scale, int T, int N, int K, float* y, float dropout_p, uint64_t seed,
                                 const uint64_t* seed_dev, uint32_t site, void* stream);
-/* dx[T,K] (+res) = dy[T,N] @ W[N,K] ; dW[N,K] += dy^T x ; db[N] += colsum(dy) */
+/* dx[T,K] (+res) = dy[T,N] @ W[N,K] ; dW[N,K] += dy^T x ; db[N] += colsum(dy).  dW and db are summed in a fixed order, so they
+ * are the same from run to run.  workspace: grb_linear_backward_workspace_bytes(T, N, K) bytes, required when dw or db is non-NULL. */
+size_t grb_linear_backward_workspace_bytes(int T, int N, int K);
 int grb_linear_backward(const void* dy_bf16, const void* w_bf16, const void* x_bf16, int T, int N, int K,
-                        float* dx_f32, const float* dx_residual, float* dw, float* db, void* stream);
-int grb_dact(const void* g_bf16_in_out, const void* z_bf16, size_t n, int act, void* stream);
+                        float* dx_f32, const float* dx_residual, float* dw, float* db, void* workspace, void* stream);
 /* g[T,K] bf16 = dropmask(dy[T,N] @ W[N,K]) * act'(z[T,K])   (backward through `act(dropout)` of a hidden layer) ; act 1 silu, 2 relu */
 int grb_linear_dact_backward(const void* dy_bf16, const void* w_bf16, const void* z_bf16, int T, int N, int K, int act,
                              float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t site, void* g_bf16, void* stream);
@@ -269,8 +270,10 @@ int grb_cast_rows_f32_to_bf16(const float* in, void* out_bf16, int T, int D, con
                               const uint64_t* seed_dev, uint32_t site, void* stream);
 int grb_layernorm_forward(const float* x, const float* g, const float* b, float eps, int T, int D, void* y_bf16,
                           float* y_f32, float* stats, void* stream);
+/* dx = LayerNorm backward of dy (+ residual) ; dg, db += in a fixed order.  workspace: grb_layernorm_backward_workspace_bytes(T, D). */
+size_t grb_layernorm_backward_workspace_bytes(int T, int D);
 int grb_layernorm_backward(const float* dy, const float* x, const float* stats, const float* g, const float* residual,
-                           int T, int D, float* dx, float* dg, float* db, void* stream);
+                           int T, int D, float* dx, float* dg, float* db, void* workspace, void* stream);
 
 /* fp32-accurate linear layer on the bf16 tensor path (the RQ-VAE encoder MLP, genrec/modules/encoder.py:399-420: bias-free
  * Linear + SiLU).  Operands are split into three bf16 terms each and the six significant cross terms are laid out along K

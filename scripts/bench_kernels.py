@@ -1,7 +1,7 @@
 """Stand-alone device timings of the secondary kernels (RQ-VAE residual argmin, SASRec attention, HSTU layer at cfg-3 geometry,
 cached incremental HSTU inference next to full recompute, RQ-VAE Sinkhorn and k-means init) with CUDA events, against the relevant
 roofline or the torch code they replace.  Prints one JSON line per measurement; `bench_kernels.py rqvae_train` runs only the RQ-VAE
-training rows."""
+training rows, `bench_kernels.py linear_bwd` only the linear-backward and SASRec training-step rows."""
 import json
 import os
 import sys
@@ -221,10 +221,49 @@ def bench_rqvae_train(dev):
                               **info)), flush=True)
 
 
+def bench_linear_bwd(dev):
+    """Fn.linear_bwd (dx, dW and db) at the SASRec shapes (configs[0]: B = 128, L = 50, d = 64, FFN 256) and at the T5 projection
+    shapes of TIGER (d_model 384, kv projection 768; batch 256, 61 encoder and 4 decoder tokens per sequence), then one SASRec
+    training step (forward + backward) at configs[0] geometry.  Graph-captured device time.  Only the Python API is used, so the
+    script times any tree that has it."""
+    from genrec_b200.sasrec import SASRec
+    info = card()
+    g = torch.Generator().manual_seed(0)
+    shapes = [("sasrec", 6400, 64, 64), ("sasrec", 6400, 256, 64), ("sasrec", 6400, 64, 256),
+              ("tiger_encoder", 256 * 61, 384, 384), ("tiger_encoder", 256 * 61, 768, 384),
+              ("tiger_decoder", 256 * 4, 384, 384), ("tiger_decoder", 256 * 4, 768, 384)]
+    for geo, T, N, K in shapes:
+        dy = (torch.randn(T, N, generator=g) * 0.1).to(dev).bfloat16()
+        w = (torch.randn(N, K, generator=g) * 0.1).to(dev).bfloat16()
+        x = torch.randn(T, K, generator=g).to(dev).bfloat16()
+        ms = graph_timed(lambda: Fn.linear_bwd(dy, w, x))
+        print(json.dumps(dict(kernel="linear_bwd", geometry=geo, T=T, N=N, K=K, us=ms * 1e3, **info)), flush=True)
+    B, L, V = 128, 50, 1000
+    torch.manual_seed(0)
+    m = SASRec(V, L, 64, 2, 2, 256, dropout=0.2).to(dev).train()
+    ids = torch.randint(1, V + 1, (B, L), generator=g)
+    ids[torch.arange(L)[None, :] < torch.randint(0, L - 1, (B, 1), generator=g)] = 0      # left padding
+    tg = torch.roll(ids, -1, 1)
+    ids, tg = ids.to(dev), tg.to(dev)
+    for p in m.parameters():
+        p.grad = torch.zeros_like(p)
+
+    def step():
+        for p in m.parameters():
+            p.grad.zero_()
+        m(ids, tg)[1].backward()
+
+    ms = graph_timed(step)
+    print(json.dumps(dict(kernel="sasrec_train_step", B=B, L=L, D=64, blocks=2, num_items=V, dropout=0.2, ms=ms, **info)), flush=True)
+
+
 def main():
     dev = torch.device("cuda:0")
     if sys.argv[1:] == ["rqvae_train"]:
         bench_rqvae_train(dev)
+        return
+    if sys.argv[1:] == ["linear_bwd"]:
+        bench_linear_bwd(dev)
         return
     peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) \
         if os.path.exists("MEASURED_PEAKS.json") else {}

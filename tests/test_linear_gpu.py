@@ -46,6 +46,41 @@ def test_linear_backward(T, N, K):
     assert ((db - ref_db).abs().max() / ref_db.abs().max()).item() < 2e-3
 
 
+@pytest.mark.parametrize("T,N,K", [(25600, 512, 128), (6400, 64, 64)])
+def test_linear_backward_is_reproducible(T, N, K):
+    """dW and db are split over many CTAs and summed in a fixed order: two calls on the same inputs give the same bits."""
+    import genrec_b200.functional as Fn
+    dev = torch.device("cuda:0")
+    g = torch.Generator(device="cpu").manual_seed(T + N + K + 2)
+    dy = (torch.randn(T, N, generator=g) * 0.1).to(dev).bfloat16()
+    x = torch.randn(T, K, generator=g).to(dev).bfloat16()
+    w = (torch.randn(N, K, generator=g) * 0.1).to(dev).bfloat16()
+    _, dw0, db0 = Fn.linear_bwd(dy, w, x, need_dx=False)
+    _, dw1, db1 = Fn.linear_bwd(dy, w, x, need_dx=False)
+    assert torch.equal(dw0, dw1) and torch.equal(db0, db1)
+    assert ((dw0 - dy.float().T @ x.float()).abs().max() / dw0.abs().max()).item() < 2e-3
+
+
+def test_layernorm_backward_is_reproducible():
+    """The LayerNorm parameter gradients are summed over the CTAs in a fixed order: two calls give the same bits."""
+    import genrec_b200.functional as Fn
+    dev = torch.device("cuda:0")
+    g = torch.Generator(device="cpu").manual_seed(7)
+    T, D = 6400, 64
+    x = torch.randn(T, D, generator=g).to(dev)
+    gamma, beta = (1 + 0.1 * torch.randn(D, generator=g)).to(dev), (0.1 * torch.randn(D, generator=g)).to(dev)
+    dy = torch.randn(T, D, generator=g).to(dev)
+    _, _, st = Fn.layernorm_fwd(x, gamma, beta, 1e-8)
+    dx0, dg0, db0 = Fn.layernorm_bwd(dy, x, st, gamma)
+    dx1, dg1, db1 = Fn.layernorm_bwd(dy, x, st, gamma)
+    assert torch.equal(dx0, dx1) and torch.equal(dg0, dg1) and torch.equal(db0, db1)
+    xr = x.clone().requires_grad_(True)
+    gr, br = gamma.clone().requires_grad_(True), beta.clone().requires_grad_(True)
+    torch.nn.functional.layer_norm(xr, (D,), gr, br, 1e-8).backward(dy)
+    torch.testing.assert_close(dg0, gr.grad, rtol=1e-4, atol=1e-3)
+    torch.testing.assert_close(db0, br.grad, rtol=1e-4, atol=1e-3)
+
+
 def test_linear_residual_and_rowscale():
     import genrec_b200.functional as Fn
     dev = torch.device("cuda:0")

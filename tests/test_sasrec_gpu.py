@@ -110,6 +110,31 @@ def test_cfg1_shape_vs_oracle(B, L, D, H):
         assert gm <= 1.0, gm
 
 
+def test_block_backward_is_reproducible():
+    """One SASRecBlock forward + backward at configs[0] geometry (B=128, L=50, d=64), run twice: x.grad and every parameter
+    gradient are the same bits (the linear and LayerNorm backward sum their cross-CTA partials in a fixed order)."""
+    from genrec_b200.sasrec import SASRecBlock
+    dev = torch.device("cuda:0")
+    torch.manual_seed(4)
+    B, L, D = 128, 50, 64
+    blk = SASRecBlock(D, 2, 4 * D, 0.0).to(dev).train()
+    g = torch.Generator().manual_seed(4)
+    x = torch.randn(B, L, D, generator=g).to(dev)
+    dy = torch.randn(B, L, D, generator=g).to(dev)
+    mask = (torch.arange(L)[None, :] >= torch.randint(0, L - 1, (B, 1), generator=g)).float().unsqueeze(-1).to(dev)   # left padding
+
+    def run():
+        blk.zero_grad(set_to_none=True)
+        xg = x.clone().requires_grad_(True)
+        blk(xg, mask).backward(dy)
+        return {"x": xg.grad, **{n: p.grad for n, p in blk.named_parameters()}}
+
+    first, second = run(), run()
+    assert len(first) == 15
+    for n in first:
+        assert torch.equal(first[n], second[n]), n
+
+
 def test_pointwise_feed_forward_standalone():
     """PointWiseFeedForward.forward(x, residual) on its own (sasrec.py:258-266) against torch fp32, forward and backward."""
     from genrec_b200.sasrec import PointWiseFeedForward
