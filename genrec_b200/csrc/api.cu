@@ -20,6 +20,7 @@
 #include "common.cuh"
 #include "dp_adam.cuh"
 #include "exact_f32.cuh"
+#include "head_topk.cuh"
 #include "rowwise.cuh"
 #include "rq_argmin.cuh"
 #include "rq_sinkhorn.cuh"
@@ -1032,6 +1033,79 @@ int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float 
     }
     // logits [T, C] fp32, leading dimension C of any parity
     GRB_CUDA((launch_tc_gemm<0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, TcEpiF32Plain{logits, C}, nullptr, nullptr, 0, sm_count(), st)));
+    return 0;
+}
+
+namespace {
+struct TopkWork {
+    bf16* xf;                  // [R, D] LN(x), the GEMM operand grb_head_logits builds
+    int* excl;                 // [R, E] sorted exclusion lists
+    float* cand_s; int* cand_i;  // [R, splits, k] per-range lists
+    int splits;
+    size_t bytes;
+};
+// item ranges per row tile: enough CTAs to cover the SMs once, never more ranges than item tiles
+int topk_splits(int R, int C) {
+    const int num_m = (R + TC_BM - 1) / TC_BM, num_n = (C + TC_BN - 1) / TC_BN;
+    int s = sm_count() / num_m;
+    s = s < num_n ? s : num_n;
+    s = s < TOPK_MAX_SPLITS ? s : TOPK_MAX_SPLITS;
+    return s < 1 ? 1 : s;
+}
+TopkWork carve_topk(void* base, int R, int D, int C, int k, int E) {
+    TopkWork w;
+    Carver c{static_cast<char*>(base)};
+    w.splits = topk_splits(R, C);
+    w.xf = c.take<bf16>((size_t)R * D * 2);
+    w.excl = E > 0 ? c.take<int>((size_t)R * E * 4) : nullptr;
+    w.cand_s = c.take<float>((size_t)R * w.splits * k * 4);
+    w.cand_i = c.take<int>((size_t)R * w.splits * k * 4);
+    w.bytes = c.off;
+    return w;
+}
+int topk_check(int R, int D, int C, int k, int E) {
+    GRB_REQUIRE(R > 0 && C > 1 && (D == 64 || D == 128 || D == 256), "bad shape R=%d D=%d C=%d (R >= 1, D in {64,128,256}, C >= 2)", R, D, C);
+    GRB_REQUIRE(k >= 1 && k <= TOPK_MAX_K, "k must lie in [1, %d], got %d", TOPK_MAX_K, k);
+    GRB_REQUIRE(E >= 0 && E <= TOPK_MAX_EXCLUDE, "exclusion lists hold at most %d ids per row, got E=%d", TOPK_MAX_EXCLUDE, E);
+    return 0;
+}
+}  // namespace
+
+size_t grb_head_topk_workspace_bytes(int R, int D, int C, int k, int E) {
+    if (topk_check(R, D, C, k, E)) return 0;
+    return carve_topk(nullptr, R, D, C, k, E).bytes;
+}
+
+int grb_head_topk(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D, int C, int k,
+                  const int64_t* exclude, int E, float* scores, int64_t* items, void* workspace, void* stream) {
+    GRB_REQUIRE(x && ln_g && ln_b && table_bf16 && scores && items && workspace, "null argument");
+    GRB_TRY(topk_check(R, D, C, k, E));
+    GRB_REQUIRE(E == 0 || exclude, "exclude is null with E=%d", E);
+    GRB_REQUIRE(aligned16(table_bf16) && aligned16(workspace), "table and workspace must be 16-byte aligned");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const TopkWork w = carve_topk(workspace, R, D, C, k, E);
+    CUtensorMap tmA, tmB;
+    GRB_REQUIRE(make_tmap_bf16(&tmA, w.xf, R, D, D, TC_BK, TC_BM) && make_tmap_bf16(&tmB, table_bf16, C, D, D, TC_BK, TC_BN),
+                "cannot encode the TMA descriptors (driver entry point missing)");
+    {
+        LnFwdArgs a{x, ln_g, ln_b, w.xf, nullptr, nullptr, R, D, ln_eps};
+        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(R), ROW_THREADS, 0, st, a); }));
+    }
+    if (E > 0) {
+        int P = 1;
+        while (P < E) P <<= 1;
+        GRB_TRY(set_smem(topk_sort_exclude_kernel, (size_t)P * 4));
+        launch_k(topk_sort_exclude_kernel, R, TOPK_SORT_THREADS, (size_t)P * 4, st, reinterpret_cast<const long long*>(exclude), E, P, C, w.excl);
+        GRB_CUDA(cudaGetLastError());
+    }
+    HeadTopkArgs a{R, C, k, E, w.splits, (C + TC_BN - 1) / TC_BN, D / TC_BK, w.excl, w.cand_s, w.cand_i};
+    GRB_TRY(set_smem(head_topk_kernel, TC_SMEM_BYTES));
+    const int num_m = (R + TC_BM - 1) / TC_BM;
+    launch_k(head_topk_kernel, num_m * w.splits, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, a);
+    GRB_CUDA(cudaGetLastError());
+    launch_k(topk_merge_kernel, (R + TOPK_MERGE_ROWS - 1) / TOPK_MERGE_ROWS, 32 * TOPK_MERGE_ROWS, 0, st, (const float*)w.cand_s,
+             (const int*)w.cand_i, R, w.splits, k, scores, reinterpret_cast<long long*>(items));
+    GRB_CUDA(cudaGetLastError());
     return 0;
 }
 

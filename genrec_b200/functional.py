@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import List, Optional, Tuple
+from typing import List, NamedTuple, Optional, Tuple
 
 import torch
 
@@ -361,6 +361,59 @@ def head_logits(x, ln_g, ln_b, table, table_bf16, eps) -> torch.Tensor:
         check(lib.grb_head_logits(ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), T, D, Cn, ptr(logits), ptr(ws),
                                   stream_ptr(x.device)))
     return logits
+
+
+class TopItems(NamedTuple):
+    """The k best items per row, best first: ``scores`` [R, k] fp32 and ``items`` [R, k] int64 (slots without an eligible item hold
+    score -inf and item 0)."""
+    scores: torch.Tensor
+    items: torch.Tensor
+
+
+TOPK_MAX_K, TOPK_MAX_EXCLUDE = 64, 16384
+
+
+def check_topk_args(k: int, exclude: Optional[torch.Tensor], rows: int, device) -> None:
+    """ValueError unless 1 <= k <= 64 and ``exclude`` is None or an int64 [rows, E <= 16384] tensor on ``device``."""
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= TOPK_MAX_K:
+        raise ValueError(f"top_k must be an int in [1, {TOPK_MAX_K}], got {k!r}")
+    if exclude is None:
+        return
+    if not isinstance(exclude, torch.Tensor) or exclude.dim() != 2 or exclude.shape[0] != rows:
+        raise ValueError(f"exclude must be a [{rows}, E] tensor (one row per input row), got "
+                         f"{tuple(exclude.shape) if isinstance(exclude, torch.Tensor) else type(exclude).__name__}")
+    if exclude.dtype != torch.int64:
+        raise ValueError(f"exclude must be int64, got {exclude.dtype}")
+    if exclude.device != torch.device(device):
+        raise ValueError(f"exclude must be on {device}, got {exclude.device}")
+    if exclude.shape[1] > TOPK_MAX_EXCLUDE:
+        raise ValueError(f"exclude holds at most {TOPK_MAX_EXCLUDE} ids per row, got {exclude.shape[1]}")
+
+
+def head_topk(x, ln_g, ln_b, table_bf16, eps, k: int, exclude: Optional[torch.Tensor] = None) -> TopItems:
+    """The ``k`` best items of every row of ``x`` [R, D] under the tied head, without forming the logits (grb_head_topk): scores are
+    bit-identical to ``head_logits`` of the same rows; item 0 and the row's ``exclude`` ids ([R, E] int64, any order) never appear;
+    ties go to the lower item id.  Inference only (no autograd)."""
+    lib = _lib.load()
+    require_cuda(x, table_bf16)
+    if x.dim() != 2:
+        raise ValueError(f"x must be [R, D], got {tuple(x.shape)}")
+    R, D = x.shape
+    Cn = table_bf16.shape[0]
+    check_topk_args(k, exclude, R, x.device)
+    xc = x.detach().contiguous().float()
+    ex = exclude.contiguous() if exclude is not None and exclude.shape[1] > 0 else None
+    E = ex.shape[1] if ex is not None else 0
+    nbytes = lib.grb_head_topk_workspace_bytes(R, D, Cn, k, E)
+    if nbytes == 0:
+        raise _lib.GrbError(lib.grb_last_error().decode())
+    ws = _u8(nbytes, x.device)
+    scores = torch.empty(R, k, dtype=torch.float32, device=x.device)
+    items = torch.empty(R, k, dtype=torch.int64, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.grb_head_topk(ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), R, D, Cn, k, ptr(ex), E,
+                                ptr(scores), ptr(items), ptr(ws), stream_ptr(x.device)))
+    return TopItems(scores, items)
 
 
 def eval_rank_metrics(logits_last: torch.Tensor, targets: torch.Tensor, metrics: Optional[torch.Tensor] = None,

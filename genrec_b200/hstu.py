@@ -498,15 +498,47 @@ class HSTU(nn.Module):
         return Fn.head_logits(x[:, -1:, :].contiguous(), self.final_norm.weight, self.final_norm.bias, self.item_embedding.weight,
                               self._table_mirror(), self.final_norm.eps)[:, 0, :]
 
+    @torch.no_grad()
+    def recommend(self, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None, top_k: int = 10,
+                  exclude: Optional[torch.Tensor] = None) -> Fn.TopItems:
+        """The ``top_k`` (1..64) best next items of each row, best first, as ``TopItems(scores [B, top_k] fp32, items [B, top_k]
+        int64)``, without forming the [B, V+1] logits: the head runs on the last position only and keeps each row's best items as it
+        scores the table.  The scores are bit-identical to ``last_logits``; item 0 and the ids of the row's ``exclude`` ([B, E]
+        int64 on the model's device, any order, E <= 16384) never appear; equal scores go to the lower item id; slots without an
+        eligible item hold (-inf, 0).  bf16 precision only."""
+        self._check_topk("recommend", top_k, exclude, input_ids.shape[0], input_ids.device)
+        x = self.encode(input_ids, timestamps)
+        return self._hidden_topk(x[:, -1, :], top_k, exclude)
+
+    def _check_topk(self, what: str, top_k: int, exclude: Optional[torch.Tensor], rows: int, device) -> None:
+        if self.precision == "fp32":
+            raise RuntimeError(f"genrec_b200: {what} runs the bf16 path only; set_precision('bf16') or use last_logits")
+        Fn.check_topk_args(top_k, exclude, rows, device)
+
+    def _check_serving_topk(self, what: str, top_k: Optional[int], exclude: Optional[torch.Tensor], rows: int, device) -> None:
+        """Argument check of the top_k / exclude keywords of extend and extend_users (before any launch)."""
+        if top_k is None:
+            if exclude is not None:
+                raise ValueError(f"{what}: exclude needs top_k")
+            return
+        self._check_topk(what, top_k, exclude, rows, device)
+
+    def _hidden_topk(self, hidden: torch.Tensor, top_k: int, exclude: Optional[torch.Tensor]) -> Fn.TopItems:
+        return Fn.head_topk(hidden, self.final_norm.weight, self.final_norm.bias, self._table_mirror(), self.final_norm.eps, top_k,
+                            exclude)
+
     def new_state(self, batch_size: int, capacity: int) -> HSTUState:
         """An empty cache for ``batch_size`` users of up to ``capacity`` items each (<= 16384), on the model's device."""
         return HSTUState(batch_size, capacity, len(self.layers), self.embed_dim, self.item_embedding.weight.device)
 
     @torch.no_grad()
-    def extend(self, state: HSTUState, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def extend(self, state: HSTUState, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None, *, top_k: Optional[int] = None,
+               exclude: Optional[torch.Tensor] = None):
         """Append the non-zero ids of each row of ``input_ids`` [B, n] (with ``timestamps`` [B, n] or None), in order, to that user's
         history in ``state`` and return [B, V+1] fp32: the next-item logits of each user's latest item, as ``last_logits`` computes
         them for the left-padded concatenation of everything extended so far.  Prefilling a history is ``extend`` on a new state.
+        With ``top_k`` (1..64) it returns ``TopItems`` of the same rows instead, as ``recommend`` selects them from those logits
+        (``exclude`` [B, E] int64: ids left out per row), and the logits are never formed.
 
         Only the new items run through the blocks; the earlier ones are read from the cache.  Pads inside a chunk are compacted
         (positions count items): with the reference's position bias, where every causal cell uses one bucket, any padding pattern
@@ -522,6 +554,7 @@ class HSTU(nn.Module):
         if B != state.batch_size or input_ids.device != state.lengths.device:
             raise ValueError(f"the state holds {state.batch_size} users on {state.lengths.device}; got input_ids {tuple(input_ids.shape)} on "
                              f"{input_ids.device}")
+        self._check_serving_topk("extend", top_k, exclude, B, input_ids.device)
         if state.items_bound + n > state.capacity:
             raise ValueError(f"extending by {n} items could exceed the state's capacity ({state.items_bound} of {state.capacity} may be "
                              "used); start a new state with a larger capacity")
@@ -534,6 +567,8 @@ class HSTU(nn.Module):
         latest = x[torch.arange(B, device=dev), last_row.clamp(min=0).long()]
         state.last_hidden.copy_(torch.where((last_row >= 0)[:, None], latest, state.last_hidden))
         state.items_bound += n
+        if top_k is not None:
+            return self._hidden_topk(state.last_hidden, top_k, exclude)
         return self._hidden_logits(state.last_hidden)
 
     def _check_extend_mode(self, what: str) -> None:
@@ -581,12 +616,14 @@ class HSTU(nn.Module):
         return HSTUPool(max_users, num_pages, page_size, max_items, len(self.layers), self.embed_dim, self.item_embedding.weight.device)
 
     @torch.no_grad()
-    def extend_users(self, pool: HSTUPool, users, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def extend_users(self, pool: HSTUPool, users, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None, *,
+                     top_k: Optional[int] = None, exclude: Optional[torch.Tensor] = None):
         """``extend`` for the users named by ``users`` [B] (int64, distinct, any subset of the pool's users in any order): append the
         non-zero ids of row b of ``input_ids`` [B, n] to the history of user ``users[b]`` in ``pool`` and return [B, V+1] fp32, row b
         being that user's next-item logits - what ``extend`` returns for the same user, i.e. ``last_logits`` of the left-padded
         concatenation of every item extended for them since their last ``pool.release``.  An all-pad row leaves its user untouched
-        and returns their previous logits.
+        and returns their previous logits.  With ``top_k`` (1..64) it returns ``TopItems`` of the same rows instead (``exclude`` [B, E]
+        int64: ids left out per row), selected without forming the logits.
 
         With ``users`` on the CPU the call is refused before any launch if a user is out of range or repeated, or if the host
         bounds say a user could exceed ``max_items`` or the pool could run out of pages.  With ``users`` on the device (CUDA graphs)
@@ -603,6 +640,7 @@ class HSTU(nn.Module):
         users = torch.as_tensor(users, dtype=torch.int64) if not isinstance(users, torch.Tensor) else users
         if users.shape != (B,):
             raise ValueError(f"users must have one entry per row of input_ids ({B}), got shape {tuple(users.shape)}")
+        self._check_serving_topk("extend_users", top_k, exclude, B, dev)
         bound = None
         if not users.is_cuda:
             u_host = pool._host_users(users)
@@ -619,6 +657,8 @@ class HSTU(nn.Module):
         pool.last_hidden[slot] = hidden
         if bound is not None:
             pool.items_bound[u_host], pool.pages_bound = bound
+        if top_k is not None:
+            return self._hidden_topk(hidden, top_k, exclude)
         return self._hidden_logits(hidden)
 
     @torch.no_grad()

@@ -208,6 +208,19 @@ def _(logits_last, targets):
     return logits_last.new_empty((6,), dtype=torch.float32)
 
 
+@custom_op(f"{NS}::head_topk", mutates_args=())
+def head_topk(x: Tensor, ln_g: Tensor, ln_b: Tensor, table_bf16: Tensor, eps: float, k: int, exclude: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
+    """x [R, D] fp32 -> (scores [R, k] fp32, items [R, k] int64): the k best items of LN(x) E^T without the logits, item 0 and the
+    row's exclude ids [R, E] int64 left out, ties to the lower id (hstu.py:150-157 for serving).  Inference only."""
+    return tuple(Fn.head_topk(x, ln_g, ln_b, table_bf16, eps, k, exclude))
+
+
+@head_topk.register_fake
+def _(x, ln_g, ln_b, table_bf16, eps, k, exclude):
+    R = x.shape[0]
+    return x.new_empty((R, k), dtype=torch.float32), x.new_empty((R, k), dtype=torch.int64)
+
+
 # ------------------------------------------------------------------------------------------------ SASRec attention core
 @custom_op(f"{NS}::sasrec_attention", mutates_args=())
 def sasrec_attention(q: Tensor, k: Tensor, v: Tensor, pad: Tensor, num_heads: int, dropout_p: float, seed: int, seed_dev: Optional[Tensor],
@@ -253,4 +266,4 @@ torch.library.register_autograd(f"{NS}::sasrec_attention", _sas_backward, setup_
 
 
 OPS = ("hstu_seq_prepare", "hstu_attention", "hstu_attention_backward", "hstu_layer", "hstu_layer_backward", "rq_residual_argmin",
-       "rq_sinkhorn", "eval_rank_metrics", "sasrec_attention", "sasrec_attention_backward")
+       "rq_sinkhorn", "eval_rank_metrics", "head_topk", "sasrec_attention", "sasrec_attention_backward")

@@ -239,9 +239,8 @@ class SASRec(nn.Module):
         # per-forward snapshot: the backward re-derives the masks from the value THIS forward saw
         return self._step_seed, self._seed_dev.clone()
 
-    def forward(self, input_ids: torch.Tensor, targets: Optional[torch.Tensor] = None
-                ) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
-        """sasrec.py:79-130.  Returns (logits [B,L,V+1] fp32 | None when training with targets, loss | None)."""
+    def encode(self, input_ids: torch.Tensor) -> torch.Tensor:
+        """Embedding + all blocks (everything before final_norm).  sasrec.py:100-116."""
         require_cuda(input_ids)
         ensure_device(input_ids.device)
         B, L = input_ids.shape
@@ -253,6 +252,12 @@ class SASRec(nn.Module):
         mask = (pad == 0).float().unsqueeze(-1)
         for blk in self.blocks:
             x = blk(x, mask, _apply_mask=True, _seed=seed, _seed_dev=sd)                         # :114-116
+        return x
+
+    def forward(self, input_ids: torch.Tensor, targets: Optional[torch.Tensor] = None
+                ) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """sasrec.py:79-130.  Returns (logits [B,L,V+1] fp32 | None when training with targets, loss | None)."""
+        x = self.encode(input_ids)
         table = self.item_embedding.weight
         table_bf16 = Fn.cast_bf16(table)
         logits = loss = None
@@ -270,3 +275,13 @@ class SASRec(nn.Module):
         last_logits[:, 0] = float("-inf")
         _, top_k_items = torch.topk(last_logits, top_k, dim=-1)
         return top_k_items
+
+    @torch.no_grad()
+    def recommend(self, input_ids: torch.Tensor, top_k: int = 10, exclude: Optional[torch.Tensor] = None) -> Fn.TopItems:
+        """The ``top_k`` (1..64) best next items of each row as ``TopItems(scores, items)``, without forming the logits: the scores
+        are bit-identical to the last row of ``forward``'s logits; item 0 and the row's ``exclude`` ids ([B, E] int64) never appear;
+        equal scores go to the lower item id (see ``HSTU.recommend``)."""
+        Fn.check_topk_args(top_k, exclude, input_ids.shape[0], input_ids.device)
+        x = self.encode(input_ids)
+        return Fn.head_topk(x[:, -1, :], self.final_norm.weight, self.final_norm.bias, Fn.cast_bf16(self.item_embedding.weight),
+                            self.final_norm.eps, top_k, exclude)

@@ -229,6 +229,16 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
 /* inference / API parity: logits fp32 [T, C] (contiguous), optional loss. */
 int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int T,
                     int D, int C, float* logits, void* workspace, void* stream);
+/* Serving: the k best items of each of R rows without forming the logits (replaces `logits[:, 0] = -inf; topk` of predict,
+ * hstu.py:150-157, sasrec.py:132-138).  scores [R, k] fp32 / items [R, k] int64, best first in the total order (score desc,
+ * item id asc); every score is bit-identical to what grb_head_logits writes for that row and item.  Item 0 and the ids of the
+ * row's exclusion list (exclude [R, E] int64, any order, duplicates allowed, entries outside 1..C-1 ignored; NULL when E = 0)
+ * never appear; a row with fewer than k eligible items has (-inf, 0) in the remaining slots.  D in {64,128,256}, C >= 2,
+ * 1 <= k <= 64, 0 <= E <= 16384.  Deterministic.  workspace: grb_head_topk_workspace_bytes(), which grows with R * k and R * E,
+ * not with C (0 for unsupported arguments). */
+size_t grb_head_topk_workspace_bytes(int R, int D, int C, int k, int E);
+int grb_head_topk(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D, int C,
+                  int k, const int64_t* exclude, int E, float* scores, int64_t* items, void* workspace, void* stream);
 
 /* Leave-one-out evaluation without host round trips (replaces the per-sample loop of genrec/trainers/hstu_trainer.py:55-81):
  * logits [B, C] fp32 of the LAST position, targets [B] (0 = skip).  The rank of the target among classes 1..C-1 (class 0 is

@@ -1,7 +1,8 @@
 """Stand-alone device timings of the secondary kernels (RQ-VAE residual argmin, SASRec attention, HSTU layer at cfg-3 geometry,
 cached incremental HSTU inference next to full recompute, RQ-VAE Sinkhorn and k-means init) with CUDA events, against the relevant
 roofline or the torch code they replace.  Prints one JSON line per measurement; `bench_kernels.py rqvae_train` runs only the RQ-VAE
-training rows, `bench_kernels.py linear_bwd` only the linear-backward and SASRec training-step rows."""
+training rows, `bench_kernels.py linear_bwd` only the linear-backward and SASRec training-step rows, `bench_kernels.py head_topk` only
+the fused top-k head rows."""
 import json
 import os
 import sys
@@ -115,44 +116,106 @@ def bench_extend(dev):
             assert torch.isfinite(one()).all()
 
 
+POOL_GEOMS = (("cfg2", dict(num_items=12101, embed_dim=128, num_heads=4, num_blocks=4), 4096, 200, 128, True),
+              ("cfg3", dict(num_items=12101, embed_dim=256, num_heads=8, num_blocks=8), 512, 2048, 32, False))
+
+
+def _pool_workload(dev, name, geo, nusers, cap, B):
+    """A pool of `nusers` users with seeded history lengths (none a multiple of the page size) and B random users to extend by one
+    item -> (model, pool, lens, hist, hts, users, one(**kw)); one() rewinds the users' lengths on the device and calls
+    extend_users(..., **kw)."""
+    from genrec_b200.hstu import HSTU
+    g = torch.Generator().manual_seed(1)
+    torch.manual_seed(0)
+    m = HSTU(max_seq_len=cap, dropout=0.0, **geo).to(dev).eval()
+    ps = 64
+    lens = torch.randint(1, cap, (nusers,), generator=g)
+    lens[lens % ps == 0] -= 1                                  # the timed item stays inside the user's last page
+    pool = m.new_pool(max_users=nusers, num_pages=int(((lens + ps) // ps).sum()), page_size=ps, max_items=cap)
+    hist = torch.randint(1, geo["num_items"] + 1, (nusers, cap), generator=g)
+    hts = 1_300_000_000 + torch.cumsum(torch.randint(1, 3 * 86400, (nusers, cap), generator=g), 1)
+    pad = torch.arange(cap)[None, :] < (cap - 1 - lens)[:, None]   # user u: lens[u] items, then the timed one in column cap-1
+    hist[pad] = 0
+    hts[pad] = 0
+    chunk = 128 if name == "cfg2" else 16
+    for u0 in range(0, nusers, chunk):                         # device users: pages follow the real lengths, not the host bound
+        us = torch.arange(u0, min(u0 + chunk, nusers))
+        m.extend_users(pool, us.to(dev), hist[us, :-1].to(dev), hts[us, :-1].to(dev))
+    assert not pool.overflowed().any()
+    users = torch.randperm(nusers, generator=g)[:B]
+    users_dev = users.to(dev)
+    ulens = lens[users].to(dev, torch.int32)
+    ids1, ts1 = hist[users, -1:].to(dev), hts[users, -1:].to(dev)
+
+    def one(**kw):
+        pool.lengths.index_copy_(0, users_dev, ulens)
+        return m.extend_users(pool, users_dev, ids1, ts1, **kw)
+
+    return m, pool, lens, hist, hts, users, one
+
+
+def bench_head_topk(dev):
+    """The fused top-k head (Fn.head_topk: LayerNorm, wgmma scoring with per-row lists, merge) against the logits path it replaces
+    for serving (Fn.head_logits, column 0 set to -inf, torch.topk), both graph-captured, k = 10 and 64: the head alone at the project's
+    catalog (cfg2: D = 128, C = 12,102) and at a 1,000,000-item catalog, then extend_users(top_k=10) against extend_users + the same
+    top-k on the cfg2 pool workload.  The scoring kernel's time (torch.profiler) is set against its bound, the larger of the table
+    read (C D 2 bytes at 3.35 TB/s) and the GEMM (2 R C D FLOP at 989 TFLOP/s), both H100 SXM data-sheet figures."""
+    info = card()
+    HBM, BF16 = 3.35e12, 989e12
+    g = torch.Generator().manual_seed(0)
+    D, eps = 128, 1e-5
+    for C, batches in ((12102, (1, 128)), (1000001, (1, 128, 1024))):
+        tb = (0.05 * torch.randn(C, D, generator=g)).to(torch.bfloat16).to(dev)
+        ln_g, ln_b = (1 + 0.1 * torch.randn(D, generator=g)).to(dev), (0.1 * torch.randn(D, generator=g)).to(dev)
+        for B in batches:
+            x = torch.randn(B, D, generator=g).to(dev)
+            for k in (10, 64):
+                def fused():
+                    return Fn.head_topk(x, ln_g, ln_b, tb, eps, k)
+
+                def logits_topk():
+                    lo = Fn.head_logits(x[:, None, :], ln_g, ln_b, tb, tb, eps)[:, 0, :]
+                    lo[:, 0] = float("-inf")
+                    return torch.topk(lo, k, dim=1)
+
+                assert torch.equal(fused().scores, logits_topk().values)
+                f_ms, b_ms = graph_timed(fused), graph_timed(logits_topk)
+                kern = kernel_us(fused, "head_topk_kernel")
+                t_bytes, t_flop = C * D * 2 / HBM * 1e6, 2 * B * C * D / BF16 * 1e6
+                bound = max(t_bytes, t_flop)
+                print(json.dumps(dict(kernel="head_topk", workload="head", D=D, C=C, B=B, k=k, fused_us=f_ms * 1e3,
+                                      logits_topk_us=b_ms * 1e3, speedup_vs_logits_topk=b_ms / f_ms, scoring_kernel_us=kern,
+                                      bound_us=bound, bound_by="table read" if t_bytes >= t_flop else "bf16 GEMM",
+                                      fused_over_bound=f_ms * 1e3 / bound, scoring_kernel_over_bound=kern / bound, **info)), flush=True)
+        del tb
+        torch.cuda.empty_cache()
+    name, geo, nusers, cap, B, _ = POOL_GEOMS[0]
+    m, pool, lens, hist, hts, users, one = _pool_workload(dev, name, geo, nusers, cap, B)
+
+    def one_topk():
+        lo = one()
+        lo[:, 0] = float("-inf")
+        return torch.topk(lo, 10, dim=1)
+
+    assert torch.equal(one(top_k=10).scores, one_topk().values)
+    f_ms, b_ms = graph_timed(lambda: one(top_k=10)), graph_timed(one_topk)
+    print(json.dumps(dict(kernel="head_topk", workload="extend_users", geometry=name, pool_users=nusers, B=B, k=10, max_items=cap,
+                          fused_us=f_ms * 1e3, logits_topk_us=b_ms * 1e3, speedup_vs_logits_topk=b_ms / f_ms, **info)), flush=True)
+
+
 def bench_pool(dev):
     """Serving from the paged pool (HSTU.extend_users): a pool of many users with seeded history lengths, one new item for a random
     subset of them, next to the dense HSTUState extend of the same users (cfg2) and last_logits on their left-padded histories.
     Graph-captured with the users as a device tensor.  Every length is a non-multiple of the page size, so the timed item never
     takes a page, and the lengths are rewound on the device before every call (one small kernel inside the timed graph).  The
     allocation kernel and the chunk-attention kernel are timed on their own with torch.profiler."""
-    from genrec_b200.hstu import HSTU
     info = card()
     HBM = 3.35e12
-    geoms = (("cfg2", dict(num_items=12101, embed_dim=128, num_heads=4, num_blocks=4), 4096, 200, 128, True),
-             ("cfg3", dict(num_items=12101, embed_dim=256, num_heads=8, num_blocks=8), 512, 2048, 32, False))
-    for name, geo, nusers, cap, B, dense in geoms:
-        g = torch.Generator().manual_seed(1)
-        torch.manual_seed(0)
-        m = HSTU(max_seq_len=cap, dropout=0.0, **geo).to(dev).eval()
-        D, NB, ps = geo["embed_dim"], geo["num_blocks"], 64
-        lens = torch.randint(1, cap, (nusers,), generator=g)
-        lens[lens % ps == 0] -= 1                                  # the timed item stays inside the user's last page
-        pool = m.new_pool(max_users=nusers, num_pages=int(((lens + ps) // ps).sum()), page_size=ps, max_items=cap)
-        hist = torch.randint(1, geo["num_items"] + 1, (nusers, cap), generator=g)
-        hts = 1_300_000_000 + torch.cumsum(torch.randint(1, 3 * 86400, (nusers, cap), generator=g), 1)
-        pad = torch.arange(cap)[None, :] < (cap - 1 - lens)[:, None]   # user u: lens[u] items, then the timed one in column cap-1
-        hist[pad] = 0
-        hts[pad] = 0
-        chunk = 128 if name == "cfg2" else 16
-        for u0 in range(0, nusers, chunk):                         # device users: pages follow the real lengths, not the host bound
-            us = torch.arange(u0, min(u0 + chunk, nusers))
-            m.extend_users(pool, us.to(dev), hist[us, :-1].to(dev), hts[us, :-1].to(dev))
-        assert not pool.overflowed().any()
-        users = torch.randperm(nusers, generator=g)[:B]
-        users_dev = users.to(dev)
+    for name, geo, nusers, cap, B, dense in POOL_GEOMS:
+        m, pool, lens, hist, hts, users, one = _pool_workload(dev, name, geo, nusers, cap, B)
+        D, NB, ps = geo["embed_dim"], geo["num_blocks"], pool.page_size
         ulens = lens[users].to(dev, torch.int32)
         ids1, ts1 = hist[users, -1:].to(dev), hts[users, -1:].to(dev)
-
-        def one():
-            pool.lengths.index_copy_(0, users_dev, ulens)
-            return m.extend_users(pool, users_dev, ids1, ts1)
-
         ms = graph_timed(one)
         hist_u, hts_u = hist[users].to(dev), hts[users].to(dev)
         full_ms = graph_timed(lambda: m.last_logits(hist_u, hts_u))
@@ -264,6 +327,9 @@ def main():
         return
     if sys.argv[1:] == ["linear_bwd"]:
         bench_linear_bwd(dev)
+        return
+    if sys.argv[1:] == ["head_topk"]:
+        bench_head_topk(dev)
         return
     peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) \
         if os.path.exists("MEASURED_PEAKS.json") else {}
