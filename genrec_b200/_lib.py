@@ -39,8 +39,7 @@ class HstuLayerGrads(C.Structure):
 
 
 class HstuSeq(C.Structure):
-    _fields_ = [("bias_index", c_void_p), ("ld_index", c_int), ("has_time", c_int), ("pos_uniform", c_int), ("pos_bucket0", c_int),
-                ("timestamps", c_void_p), ("pad", c_void_p), ("rel32", c_void_p), ("wide", c_void_p), ("time_thr", c_void_p)]
+    _fields_ = [("bias_index", c_void_p), ("ld_index", c_int), ("has_time", c_int), ("pos_uniform", c_int), ("pos_bucket0", c_int)]
 
 
 class HstuCache(C.Structure):
@@ -74,8 +73,6 @@ SIGNATURES = {
     "grb_hstu_layer_backward": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuSeq), c_void_p, c_void_p, c_void_p,
                                         P(HstuLayerGrads), c_void_p, c_void_p]),
     "grb_hstu_bias_index": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
-    "grb_hstu_seq_prepare": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
-    "grb_hstu_bucket_bytes_debug": (c_int, [P(HstuSeq), c_int, c_int, c_int, c_void_p, c_void_p]),
     "grb_hstu_attention_scratch_bytes": (c_size_t, [P(HstuDims)]),
     "grb_hstu_attention_forward": (c_int, [P(HstuDims), c_void_p, c_void_p, P(HstuSeq), c_void_p, c_void_p, c_void_p]),
     "grb_hstu_attention_backward": (c_int, [P(HstuDims), c_void_p, c_void_p, P(HstuSeq), c_void_p, c_void_p, c_void_p, c_void_p,

@@ -15,7 +15,6 @@
 #include "attn_hstu_extend.cuh"
 #include "attn_sasrec.cuh"
 #include "attn_t5.cuh"
-#include "attn_buckets.cuh"
 #include "beam.cuh"
 #include "common.cuh"
 #include "dp_adam.cuh"
@@ -823,33 +822,6 @@ int grb_set_defer_weight_grads(int on) {
     return 0;
 }
 int grb_join_deferred(void* stream) { return join_pending(static_cast<cudaStream_t>(stream)); }
-
-int grb_hstu_seq_prepare(const int64_t* timestamps, const uint8_t* pad, int B, int L, int32_t* rel32, uint8_t* wide, void* stream) {
-    GRB_REQUIRE(timestamps && pad && rel32 && wide, "null argument");
-    GRB_REQUIRE(B > 0 && L > 0, "bad shape B=%d L=%d", B, L);
-    launch_k(hstu_seq_prep_kernel, (unsigned)B, 256, 0, static_cast<cudaStream_t>(stream), reinterpret_cast<const long long*>(timestamps), pad, L,
-             reinterpret_cast<int*>(rel32), wide);
-    GRB_CUDA(cudaGetLastError());
-    return 0;
-}
-
-int grb_hstu_bucket_bytes_debug(const grb_hstu_seq* s, int B, int L, int ntime, uint8_t* out, void* stream) {
-    GRB_REQUIRE(s && out && s->pad && s->time_thr, "null argument");
-    GRB_REQUIRE(B > 0 && L > 0 && B <= 65535 && ntime >= 0 && ntime <= 64, "bad shape");
-    HstuBucketArgs a;
-    memset(&a, 0, sizeof(a));
-    const bool has_time = s->timestamps != nullptr && s->has_time && ntime > 0;
-    GRB_REQUIRE(!has_time || (s->rel32 && s->wide), "rel32 / wide missing: call grb_hstu_seq_prepare first");
-    a.ts = has_time ? reinterpret_cast<const long long*>(s->timestamps) : nullptr;
-    a.rel32 = s->rel32; a.wide = s->wide; a.pad = s->pad;
-    a.thr64 = reinterpret_cast<const long long*>(s->time_thr);
-    a.ntime = has_time ? ntime : 0;
-    a.B = B; a.L = L;
-    dim3 grid((L + 31) / 32, (L + 127) / 128, B);
-    launch_k(hstu_bucket_bytes_debug_kernel, grid, 128, 0, static_cast<cudaStream_t>(stream), a, out);
-    GRB_CUDA(cudaGetLastError());
-    return 0;
-}
 
 size_t grb_hstu_attention_scratch_bytes(const grb_hstu_dims* d) {
     if (check_dims(d)) return 0;

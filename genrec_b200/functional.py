@@ -79,8 +79,7 @@ _ZERO_TABLES = {}
 
 class SeqMeta:
     """Per-batch sequence metadata shared by all layers of one forward: the pad flags, the raw timestamps and the
-    [B, L, ld] uint16 bias-index matrix the attention kernels read.  The per-sequence int32 rebasing of the timestamps
-    (``grb_hstu_seq_prepare``) is made on demand for the bucket test hook."""
+    [B, L, ld] uint16 bias-index matrix the attention kernels read."""
 
     def __init__(self, pad_u8: torch.Tensor, timestamps: Optional[torch.Tensor], pos_bucket: Optional[torch.Tensor],
                  time_thr: torch.Tensor, num_time_buckets: int = 64, num_pos_buckets: int = 32, pos_uniform=None,
@@ -104,18 +103,7 @@ class SeqMeta:
             pos_uniform = (bool((pb == pb[0]).all()), int(pb[0]))
         self.pos_uniform, self.pos_bucket0 = pos_uniform
         self.ld = (L + 7) // 8 * 8
-        self.rel32 = self.wide = None
         self._build_bias_index(may_defer)
-
-    def _ensure_rel(self):
-        if self.timestamps is None or self.rel32 is not None:
-            return
-        dev = self.pad.device
-        self.rel32 = torch.empty(self.B, self.L, dtype=torch.int32, device=dev)
-        self.wide = torch.empty(self.B, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            check(_lib.load().grb_hstu_seq_prepare(ptr(self.timestamps), ptr(self.pad), self.B, self.L, ptr(self.rel32), ptr(self.wide),
-                                                   stream_ptr(dev)))
 
     def _build_bias_index(self, may_defer: bool):
         B, L, dev = self.B, self.L, self.pad.device
@@ -136,19 +124,7 @@ class SeqMeta:
 
     def struct(self) -> HstuSeq:
         return HstuSeq(ptr(self.bias_index), self.ld, 1 if self.timestamps is not None else 0, 1 if self.pos_uniform else 0,
-                       self.pos_bucket0, ptr(self.timestamps), ptr(self.pad), ptr(self.rel32), ptr(self.wide), ptr(self.time_thr))
-
-    def bucket_bytes(self, num_time_buckets: Optional[int] = None) -> torch.Tensor:
-        """[B, L, L] uint8: the time bucket (or 64 = masked) of every cell as the in-kernel bucket routine derives it from the
-        rebased timestamps (test hook)."""
-        nt = self.num_time_buckets if num_time_buckets is None else num_time_buckets
-        out = torch.full((self.B, self.L, self.L), 255, dtype=torch.uint8, device=self.pad.device)
-        self._ensure_rel()
-        seq = self.struct()
-        with torch.cuda.device(self.pad.device):
-            check(_lib.load().grb_hstu_bucket_bytes_debug(C.byref(seq), self.B, self.L, nt if self.timestamps is not None else 0, ptr(out),
-                                                          stream_ptr(self.pad.device)))
-        return out
+                       self.pos_bucket0)
 
 
 def _dims(B, L, D, H, npos, ntime, p, seed, seed_dev, layer) -> HstuDims:

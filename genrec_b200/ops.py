@@ -17,65 +17,41 @@ import torch
 from torch import Tensor
 from torch.library import custom_op
 
-from . import _lib
 from . import functional as Fn
-from ._lib import HstuDims, check, ptr, require_cuda, stream_ptr
+from ._lib import HstuDims, require_cuda
 
 NS = "genrec_b200"
 
 
-def _meta(pad: Tensor, ts: Optional[Tensor], rel32: Optional[Tensor], wide: Optional[Tensor], thr: Tensor, pos_bucket0: int,
-          ntime: int) -> Fn.SeqMeta:
+def _meta(pad: Tensor, ts: Optional[Tensor], thr: Tensor, pos_bucket0: int, ntime: int) -> Fn.SeqMeta:
     """Sequence metadata of one op call: uniform position buckets (bucket pos_bucket0), and the bias-index matrix built on the
     caller's stream even under the deferred schedule - the kernels that read it and the tensor's lifetime follow that stream."""
-    meta = Fn.SeqMeta(pad, ts, None, thr, ntime, 1, (True, int(pos_bucket0)), may_defer=False)
-    meta.rel32, meta.wide = rel32, wide
-    return meta
-
-
-# ------------------------------------------------------------------------------------------------ sequence preparation
-@custom_op(f"{NS}::hstu_seq_prepare", mutates_args=())
-def hstu_seq_prepare(timestamps: Tensor, pad: Tensor) -> Tuple[Tensor, Tensor]:
-    """timestamps [B, L] int64, pad [B, L] uint8 -> rel32 [B, L] int32, wide [B] uint8 (grb_hstu_seq_prepare)."""
-    require_cuda(timestamps, pad)
-    B, L = timestamps.shape
-    rel = torch.empty(B, L, dtype=torch.int32, device=pad.device)
-    wide = torch.empty(B, dtype=torch.uint8, device=pad.device)
-    with torch.cuda.device(pad.device):
-        check(_lib.load().grb_hstu_seq_prepare(ptr(timestamps.contiguous()), ptr(pad.contiguous()), B, L, ptr(rel), ptr(wide), stream_ptr(pad.device)))
-    return rel, wide
-
-
-@hstu_seq_prepare.register_fake
-def _(timestamps, pad):
-    B, L = timestamps.shape
-    return timestamps.new_empty((B, L), dtype=torch.int32), timestamps.new_empty((B,), dtype=torch.uint8)
+    return Fn.SeqMeta(pad, ts, None, thr, ntime, 1, (True, int(pos_bucket0)), may_defer=False)
 
 
 # ------------------------------------------------------------------------------------------------ attention core
 @custom_op(f"{NS}::hstu_attention", mutates_args=())
-def hstu_attention(P: Tensor, pad: Tensor, timestamps: Optional[Tensor], rel32: Optional[Tensor], wide: Optional[Tensor], time_thr: Tensor,
-                   pos_table: Tensor, time_table: Optional[Tensor], num_heads: int, pos_bucket0: int) -> Tensor:
+def hstu_attention(P: Tensor, pad: Tensor, timestamps: Optional[Tensor], time_thr: Tensor, pos_table: Tensor, time_table: Optional[Tensor],
+                   num_heads: int, pos_bucket0: int) -> Tensor:
     """P [B, L, 4D] bf16 = [U | V | Q | K] -> O [B, L, D] bf16 = silu(Q K^T + bias) V, causal + key padding (hstu.py:244-267)."""
     require_cuda(P)
     ntime = time_table.shape[0] if time_table is not None else 0
-    meta = _meta(pad, timestamps if time_table is not None else None, rel32, wide, time_thr, pos_bucket0, ntime)
+    meta = _meta(pad, timestamps if time_table is not None else None, time_thr, pos_bucket0, ntime)
     return Fn.hstu_attention_fwd(P.contiguous(), meta, num_heads, pos_table, time_table, ntime)
 
 
 @hstu_attention.register_fake
-def _(P, pad, timestamps, rel32, wide, time_thr, pos_table, time_table, num_heads, pos_bucket0):
+def _(P, pad, timestamps, time_thr, pos_table, time_table, num_heads, pos_bucket0):
     B, L, D4 = P.shape
     return P.new_empty((B, L, D4 // 4))
 
 
 @custom_op(f"{NS}::hstu_attention_backward", mutates_args=())
-def hstu_attention_backward(P: Tensor, zp: Tensor, dO: Tensor, pad: Tensor, timestamps: Optional[Tensor], rel32: Optional[Tensor],
-                            wide: Optional[Tensor], time_thr: Tensor, pos_table: Tensor, time_table: Optional[Tensor], num_heads: int,
-                            pos_bucket0: int) -> Tuple[Tensor, Tensor, Tensor]:
+def hstu_attention_backward(P: Tensor, zp: Tensor, dO: Tensor, pad: Tensor, timestamps: Optional[Tensor], time_thr: Tensor,
+                            pos_table: Tensor, time_table: Optional[Tensor], num_heads: int, pos_bucket0: int) -> Tuple[Tensor, Tensor, Tensor]:
     """-> dzp [B, L, 4D] bf16 (gradient w.r.t. the PRE-activations zp, columns V, Q, K; U = 0), dpos_table, dtime_table (fp32)."""
     ntime = time_table.shape[0] if time_table is not None else 0
-    meta = _meta(pad, timestamps if time_table is not None else None, rel32, wide, time_thr, pos_bucket0, ntime)
+    meta = _meta(pad, timestamps if time_table is not None else None, time_thr, pos_bucket0, ntime)
     dzp, dpos, dtime = Fn.hstu_attention_bwd(P.contiguous(), zp.contiguous(), dO.contiguous(), meta, num_heads, pos_table, time_table, ntime)
     if dtime is None:       # no temporal term: an all-zero gradient of the table, or [0, H] without one
         dtime = torch.zeros(time_table.shape if time_table is not None else (0, num_heads), dtype=torch.float32, device=P.device)
@@ -83,39 +59,38 @@ def hstu_attention_backward(P: Tensor, zp: Tensor, dO: Tensor, pad: Tensor, time
 
 
 @hstu_attention_backward.register_fake
-def _(P, zp, dO, pad, timestamps, rel32, wide, time_thr, pos_table, time_table, num_heads, pos_bucket0):
+def _(P, zp, dO, pad, timestamps, time_thr, pos_table, time_table, num_heads, pos_bucket0):
     tshape = time_table.shape if time_table is not None else (0, num_heads)
     return P.new_empty(P.shape), pos_table.new_empty(pos_table.shape, dtype=torch.float32), pos_table.new_empty(tshape, dtype=torch.float32)
 
 
 # ------------------------------------------------------------------------------------------------ the whole block
-def _layer_call(shape, pad, timestamps, rel32, wide, time_thr, params: List[Optional[Tensor]], H, ntime, pos_bucket0, p, seed, seed_dev,
-                layer):
+def _layer_call(shape, pad, timestamps, time_thr, params: List[Optional[Tensor]], H, ntime, pos_bucket0, p, seed, seed_dev, layer):
     """-> (dims, bf16 weight mirrors, has_time, meta) of one block op; params in Fn.PARAM_ORDER."""
     B, L, D = shape
     named = dict(zip(Fn.PARAM_ORDER, params))
     bf16w = {n: Fn.cast_bf16(named[n]) for n in Fn.BF16_PARAMS}
     has_time = named["time_table"] is not None and timestamps is not None
     dims = Fn._dims(B, L, D, H, named["pos_table"].shape[0], ntime if has_time else 0, p, seed, seed_dev, layer)
-    return dims, bf16w, has_time, _meta(pad, timestamps if has_time else None, rel32, wide, time_thr, pos_bucket0, dims.ntime)
+    return dims, bf16w, has_time, _meta(pad, timestamps if has_time else None, time_thr, pos_bucket0, dims.ntime)
 
 
 @custom_op(f"{NS}::hstu_layer", mutates_args=())
-def hstu_layer(x: Tensor, pad: Tensor, timestamps: Optional[Tensor], rel32: Optional[Tensor], wide: Optional[Tensor], time_thr: Tensor,
-               proj_w: Tensor, proj_b: Tensor, pos_table: Tensor, time_table: Optional[Tensor], ln1_g: Tensor, ln1_b: Tensor, ffn1_w: Tensor,
-               ffn1_b: Tensor, ffn2_w: Tensor, ffn2_b: Tensor, ln2_g: Tensor, ln2_b: Tensor, num_heads: int, ntime: int, pos_bucket0: int,
-               dropout_p: float, seed: int, seed_dev: Optional[Tensor], layer_index: int) -> Tuple[Tensor, Tensor]:
+def hstu_layer(x: Tensor, pad: Tensor, timestamps: Optional[Tensor], time_thr: Tensor, proj_w: Tensor, proj_b: Tensor, pos_table: Tensor,
+               time_table: Optional[Tensor], ln1_g: Tensor, ln1_b: Tensor, ffn1_w: Tensor, ffn1_b: Tensor, ffn2_w: Tensor, ffn2_b: Tensor,
+               ln2_g: Tensor, ln2_b: Tensor, num_heads: int, ntime: int, pos_bucket0: int, dropout_p: float, seed: int,
+               seed_dev: Optional[Tensor], layer_index: int) -> Tuple[Tensor, Tensor]:
     """One HSTU block (hstu.py:222-280): x [B, L, D] fp32 -> (y [B, L, D] fp32, saved-for-backward blob uint8).  fp32 master
     weights in; the bf16 operand copies are made inside (one cast kernel each)."""
     require_cuda(x)
     params = [proj_w, proj_b, pos_table, time_table, ln1_g, ln1_b, ffn1_w, ffn1_b, ffn2_w, ffn2_b, ln2_g, ln2_b]
-    dims, bf16w, has_time, meta = _layer_call(x.shape, pad, timestamps, rel32, wide, time_thr, params, num_heads, ntime, pos_bucket0,
-                                              dropout_p, seed, seed_dev, layer_index)
+    dims, bf16w, has_time, meta = _layer_call(x.shape, pad, timestamps, time_thr, params, num_heads, ntime, pos_bucket0, dropout_p, seed,
+                                              seed_dev, layer_index)
     return Fn.hstu_block_forward(dims, params, bf16w, has_time, meta, x.contiguous().float())
 
 
 @hstu_layer.register_fake
-def _(x, pad, timestamps, rel32, wide, time_thr, proj_w, proj_b, pos_table, time_table, ln1_g, ln1_b, ffn1_w, ffn1_b, ffn2_w, ffn2_b, ln2_g, ln2_b,
+def _(x, pad, timestamps, time_thr, proj_w, proj_b, pos_table, time_table, ln1_g, ln1_b, ffn1_w, ffn1_b, ffn2_w, ffn2_b, ln2_g, ln2_b,
       num_heads, ntime, pos_bucket0, dropout_p, seed, seed_dev, layer_index):
     B, L, D = x.shape
     nbytes = Fn.layer_saved_bytes(HstuDims(B, L, D, num_heads, pos_table.shape[0], 0, 0.0, 0, None, 0))   # depends on B, L, D only
@@ -123,47 +98,46 @@ def _(x, pad, timestamps, rel32, wide, time_thr, proj_w, proj_b, pos_table, time
 
 
 @custom_op(f"{NS}::hstu_layer_backward", mutates_args=())
-def hstu_layer_backward(dy: Tensor, saved: Tensor, pad: Tensor, timestamps: Optional[Tensor], rel32: Optional[Tensor], wide: Optional[Tensor],
-                        time_thr: Tensor, proj_w: Tensor, proj_b: Tensor, pos_table: Tensor, time_table: Optional[Tensor], ln1_g: Tensor,
-                        ln1_b: Tensor, ffn1_w: Tensor, ffn1_b: Tensor, ffn2_w: Tensor, ffn2_b: Tensor, ln2_g: Tensor, ln2_b: Tensor,
-                        num_heads: int, ntime: int, pos_bucket0: int, dropout_p: float, seed: int, seed_dev: Optional[Tensor],
-                        layer_index: int) -> List[Tensor]:
+def hstu_layer_backward(dy: Tensor, saved: Tensor, pad: Tensor, timestamps: Optional[Tensor], time_thr: Tensor, proj_w: Tensor,
+                        proj_b: Tensor, pos_table: Tensor, time_table: Optional[Tensor], ln1_g: Tensor, ln1_b: Tensor, ffn1_w: Tensor,
+                        ffn1_b: Tensor, ffn2_w: Tensor, ffn2_b: Tensor, ln2_g: Tensor, ln2_b: Tensor, num_heads: int, ntime: int,
+                        pos_bucket0: int, dropout_p: float, seed: int, seed_dev: Optional[Tensor], layer_index: int) -> List[Tensor]:
     """-> [dx, d proj_w, d proj_b, d pos_table, d time_table, d ln1_g, d ln1_b, d ffn1_w, d ffn1_b, d ffn2_w, d ffn2_b, d ln2_g, d ln2_b]
     (fp32; d time_table is an empty [0, H] tensor when the block has no temporal bias)."""
     params = [proj_w, proj_b, pos_table, time_table, ln1_g, ln1_b, ffn1_w, ffn1_b, ffn2_w, ffn2_b, ln2_g, ln2_b]
-    dims, bf16w, has_time, meta = _layer_call(dy.shape, pad, timestamps, rel32, wide, time_thr, params, num_heads, ntime, pos_bucket0,
-                                              dropout_p, seed, seed_dev, layer_index)
+    dims, bf16w, has_time, meta = _layer_call(dy.shape, pad, timestamps, time_thr, params, num_heads, ntime, pos_bucket0, dropout_p, seed,
+                                              seed_dev, layer_index)
     dx, grads = Fn.hstu_block_backward(dims, params, bf16w, has_time, meta, dy, saved)
     return [dx] + [g if g is not None else torch.zeros(0, num_heads, dtype=torch.float32, device=dy.device) for g in grads]
 
 
 @hstu_layer_backward.register_fake
-def _(dy, saved, pad, timestamps, rel32, wide, time_thr, proj_w, proj_b, pos_table, time_table, ln1_g, ln1_b, ffn1_w, ffn1_b, ffn2_w, ffn2_b, ln2_g,
-      ln2_b, num_heads, ntime, pos_bucket0, dropout_p, seed, seed_dev, layer_index):
+def _(dy, saved, pad, timestamps, time_thr, proj_w, proj_b, pos_table, time_table, ln1_g, ln1_b, ffn1_w, ffn1_b, ffn2_w, ffn2_b, ln2_g, ln2_b,
+      num_heads, ntime, pos_bucket0, dropout_p, seed, seed_dev, layer_index):
     ps = [proj_w, proj_b, pos_table, time_table, ln1_g, ln1_b, ffn1_w, ffn1_b, ffn2_w, ffn2_b, ln2_g, ln2_b]
     return [dy.new_empty(dy.shape, dtype=torch.float32)] + [
         (dy.new_empty(q.shape, dtype=torch.float32) if q is not None else dy.new_empty((0, num_heads), dtype=torch.float32)) for q in ps]
 
 
 def _layer_setup(ctx, inputs, output):
-    (x, pad, ts, rel32, wide, thr, *params, H, ntime, pb0, p, seed, seed_dev, layer) = inputs
-    ctx.save_for_backward(output[1], pad, ts, rel32, wide, thr, *[q for q in params if q is not None], *([seed_dev] if seed_dev is not None else []))
+    (x, pad, ts, thr, *params, H, ntime, pb0, p, seed, seed_dev, layer) = inputs
+    ctx.save_for_backward(output[1], pad, ts, thr, *[q for q in params if q is not None], *([seed_dev] if seed_dev is not None else []))
     ctx.present = [q is not None for q in params]
-    ctx.has = (ts is not None, rel32 is not None, wide is not None, seed_dev is not None)
+    ctx.has_sd = seed_dev is not None
     ctx.scalars = (H, ntime, pb0, p, seed, layer)
 
 
 def _layer_backward(ctx, dy, _dsaved):
     it = iter(ctx.saved_tensors)
     saved, pad = next(it), next(it)
-    ts, rel32, wide = next(it), next(it), next(it)       # saved as None when absent
+    ts = next(it)       # saved as None when absent
     thr = next(it)
     params = [next(it) if pr else None for pr in ctx.present]
-    seed_dev = next(it) if ctx.has[3] else None
+    seed_dev = next(it) if ctx.has_sd else None
     H, ntime, pb0, p, seed, layer = ctx.scalars
-    g = torch.ops.genrec_b200.hstu_layer_backward(dy, saved, pad, ts, rel32, wide, thr, *params, H, ntime, pb0, p, seed, seed_dev, layer)
+    g = torch.ops.genrec_b200.hstu_layer_backward(dy, saved, pad, ts, thr, *params, H, ntime, pb0, p, seed, seed_dev, layer)
     pg = [g[1 + i] if pr else None for i, pr in enumerate(ctx.present)]
-    return (g[0], None, None, None, None, None, *pg, None, None, None, None, None, None, None)
+    return (g[0], None, None, None, *pg, None, None, None, None, None, None, None)
 
 
 torch.library.register_autograd(f"{NS}::hstu_layer", _layer_backward, setup_context=_layer_setup)
@@ -265,5 +239,5 @@ def _sas_backward(ctx, dout, _dlse):
 torch.library.register_autograd(f"{NS}::sasrec_attention", _sas_backward, setup_context=_sas_setup)
 
 
-OPS = ("hstu_seq_prepare", "hstu_attention", "hstu_attention_backward", "hstu_layer", "hstu_layer_backward", "rq_residual_argmin",
-       "rq_sinkhorn", "eval_rank_metrics", "head_topk", "sasrec_attention", "sasrec_attention_backward")
+OPS = ("hstu_attention", "hstu_attention_backward", "hstu_layer", "hstu_layer_backward", "rq_residual_argmin", "rq_sinkhorn",
+       "eval_rank_metrics", "head_topk", "sasrec_attention", "sasrec_attention_backward")

@@ -71,28 +71,15 @@ typedef struct {             /* fp32, same shapes as the parameters, accumulated
 } grb_hstu_layer_grads;
 
 typedef struct {
-    const uint16_t* bias_index; /* LEGACY (mma.sync) attention path only, NULL otherwise: [B, L, ld_index] from grb_hstu_bias_index():
+    const uint16_t* bias_index; /* required: [B, L, ld_index] from grb_hstu_bias_index():
                                    pos_bucket(i-j)*64 + time_bucket(|ts_i-ts_j|), or npos*64 for a masked cell (j > i, padded key) */
     int ld_index;               /* row pitch in ELEMENTS: a multiple of 8, >= L */
     int has_time;               /* 0: timestamps were None -> the temporal term is dropped (hstu.py:251) */
     int pos_uniform;            /* 1 when every delta in [0, L) maps to the same position bucket (the reference's behaviour):
-                                   a bias_index, if given, must then have been built with npos = 1 and an all-zero pos_bucket table */
+                                   bias_index must then have been built with npos = 1 and an all-zero pos_bucket table */
     int pos_bucket0;            /* that bucket (row of the [npos, H] table that is live) */
-    /* per-sequence metadata: pad flags and timestamps (with their int32 rebasing for the bucket test hook) */
-    const int64_t* timestamps;  /* [B, L] or NULL */
-    const uint8_t* pad;         /* [B, L], 1 = input_ids == 0 */
-    const int32_t* rel32;       /* [B, L] from grb_hstu_seq_prepare() (NULL when timestamps is NULL) */
-    const uint8_t* wide;        /* [B]    from grb_hstu_seq_prepare() */
-    const int64_t* time_thr;    /* [65] integer thresholds of the reference's fp32 log/0.693 bucket expression (see below) */
 } grb_hstu_seq;
 
-/* Per-sequence rebasing of the int64 timestamps (replaces nothing in the reference: it makes `ts[b,i] - ts[b,j]`
- * (hstu.py:400) a 32-bit subtraction in the in-kernel bucket routine): rel32[b,i] = ts[b,i] - min over non-padded positions;
- * wide[b] = 1 when the sequence spans >= 2^31 ticks, in which case the kernels use the int64 values themselves. */
-int grb_hstu_seq_prepare(const int64_t* timestamps, const uint8_t* pad, int B, int L, int32_t* rel32, uint8_t* wide, void* stream);
-/* Test hook: the time bucket / mask byte of every cell, [B, L, L] uint8 (bucket, or 64 when j > i or key j is padded), computed
- * by the in-kernel bucket routine from the rebased timestamps. */
-int grb_hstu_bucket_bytes_debug(const grb_hstu_seq* s, int B, int L, int ntime, uint8_t* out, void* stream);
 /* The attention core alone (hstu.py:244-267) on the projection output P = [U | V | Q | K] ([T, 4D] bf16): O [T, D] bf16.
  * backward: dO [T, D] bf16, zp [T, 4D] the pre-activations of P -> dzp columns V, Q, K (gradients w.r.t. the pre-activations),
  * bias-table gradients accumulated.  scratch: grb_hstu_attention_scratch_bytes(). */

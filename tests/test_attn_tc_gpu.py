@@ -34,20 +34,23 @@ BOUNDARY = [0, 1, 2, 3, 4, 1022, 1023, 1024, 2044, 2045, 2046, 522823, 522824, 5
             2 ** 31 - 1, 2 ** 31, 2 ** 31 + 129, 2 ** 40, 2 ** 62]
 
 
+@pytest.mark.parametrize("ntime", [64, 20, None], ids=["t64", "t20", "no_ts"])
 @pytest.mark.parametrize("L", [1, 33, 130, 200])
-def test_bucket_bytes_bit_exact(L):
+def test_bias_index_time_buckets_bit_exact(L, ntime):
+    """The bias-index matrix for the timestamp rows below at several lengths, with 64 / 20 time buckets and without timestamps:
+    every cell's time bucket and mask == oracle."""
     dev = torch.device("cuda:0")
     g = torch.Generator().manual_seed(L)
     B = 6
     gaps = torch.randint(0, 3 * 86400, (B, L), generator=g)
     gaps[:, ::7] = torch.randint(0, 3, (B, (L + 6) // 7), generator=g)
     ts = 1_300_000_000 + torch.cumsum(gaps, 1)
-    # row 1: boundary differences against the first event, in order (narrow where they fit in 31 bits ...)
+    # row 1: the boundary differences below 2^31 - 1 against the first event, in order
     narrow = [d for d in BOUNDARY if d < 2 ** 31 - 1]
     for k, d in enumerate(narrow[: max(0, L - 1)]):
         ts[1, k + 1] = ts[1, 0] + d
     ts[1, len(narrow) + 1:] = ts[1, 0] + 2 ** 30
-    # row 2: unsorted timestamps (negative differences) ; row 3: the wide path (span >= 2^31 incl. 2^40, 2^62)
+    # row 2: unsorted timestamps (negative differences) ; row 3: every boundary difference (spans >= 2^31 incl. 2^40, 2^62)
     ts[2] = ts[2][torch.randperm(L, generator=g)]
     for k, d in enumerate(BOUNDARY[: max(0, L - 1)]):
         ts[3, k + 1] = ts[3, 0] + d
@@ -57,12 +60,12 @@ def test_bucket_bytes_bit_exact(L):
     pad[5, :] = True; ts[5, :] = 0
     if L > 5:
         pad[0, 3] = True
-    for nt in (64, 20):
-        got = _meta(pad, ts, dev, nt).bucket_bytes().cpu()
-        want = _oracle_bytes(pad, ts, nt)
-        assert torch.equal(got, want), (nt, (got != want).nonzero()[:5], got[got != want][:5], want[got != want][:5])
-    got = _meta(pad, None, dev).bucket_bytes().cpu()
-    assert torch.equal(got, _oracle_bytes(pad, None))
+    if ntime is None:
+        ts = None
+    got = (_meta(pad, ts, dev, ntime or 64).bias_index.cpu().to(torch.int32) & 0xFFFF)[:, :, :L]
+    want = _oracle_bytes(pad, ts, ntime or 64).to(torch.int32)      # uniform position buckets: index = time bucket, 64 = masked
+    bad = got != want
+    assert not bad.any(), (bad.nonzero()[:5], got[bad][:5], want[bad][:5])
 
 
 def test_bias_index_bit_exact():
@@ -173,9 +176,8 @@ def test_custom_op_block_equals_module_block():
     ref = (y.detach().clone(), xi.grad.clone(), [p.grad.clone() for p in layer._params()])
     layer.zero_grad(set_to_none=True)
     pad = (ids == 0).to(torch.uint8)
-    rel, wide = torch.ops.genrec_b200.hstu_seq_prepare(ts, pad)
     xj = x.clone().requires_grad_(True)
-    y2, _saved = torch.ops.genrec_b200.hstu_layer(xj, pad, ts, rel, wide, _thresholds_on(dev), *layer._params(), H, 64, 0, 0.0, 0, None, 0)
+    y2, _saved = torch.ops.genrec_b200.hstu_layer(xj, pad, ts, _thresholds_on(dev), *layer._params(), H, 64, 0, 0.0, 0, None, 0)
     y2.backward(dy)
     torch.testing.assert_close(y2, ref[0], rtol=1e-5, atol=1e-5)
     torch.testing.assert_close(xj.grad, ref[1], rtol=1e-4, atol=1e-5)

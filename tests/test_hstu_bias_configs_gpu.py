@@ -430,10 +430,8 @@ def test_custom_op_block_equals_module_block_20_time_buckets():
     ref = (y.detach().clone(), xi.grad.clone(), [p.grad.clone() for p in layer._params()])
     layer.zero_grad(set_to_none=True)
     pad8 = pad.to(torch.uint8)
-    rel, wide = torch.ops.genrec_b200.hstu_seq_prepare(ts, pad8)
     xj = x.clone().requires_grad_(True)
-    y2, _saved = torch.ops.genrec_b200.hstu_layer(xj, pad8, ts, rel, wide, _thresholds_on(dev), *layer._params(), c["H"], 20, 0, 0.0, 0,
-                                                  None, 0)
+    y2, _saved = torch.ops.genrec_b200.hstu_layer(xj, pad8, ts, _thresholds_on(dev), *layer._params(), c["H"], 20, 0, 0.0, 0, None, 0)
     y2.backward(dy)
     torch.testing.assert_close(y2, ref[0], rtol=1e-5, atol=1e-5)
     torch.testing.assert_close(xj.grad, ref[1], rtol=1e-4, atol=1e-5)

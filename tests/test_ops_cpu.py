@@ -22,8 +22,7 @@ def test_fake_saved_blob_matches_the_library(lib, D):
     B, L, H = 3, 77, D // 64
     with FakeTensorMode():
         a = _layer_args(B, L, D, H, "cuda")
-        _, saved = torch.ops.genrec_b200.hstu_layer(a["x"], a["pad"], a["ts"], a["rel"], a["wide"], a["thr"], *a["params"], H, 64, 0, 0.1, 7,
-                                                    None, 0)
+        _, saved = torch.ops.genrec_b200.hstu_layer(a["x"], a["pad"], a["ts"], a["thr"], *a["params"], H, 64, 0, 0.1, 7, None, 0)
     assert saved.shape == (lib.grb_hstu_layer_saved_bytes(ctypes.byref(HstuDims(B, L, D, H, 32, 64, 0.1, 7, None, 0))),)
 
 
@@ -37,8 +36,7 @@ def test_ops_are_registered_with_schemas():
 def _layer_args(B, L, D, H, dev):
     f = lambda *s: torch.empty(*s, device=dev)
     return dict(x=f(B, L, D).requires_grad_(True), pad=torch.empty(B, L, dtype=torch.uint8, device=dev),
-                ts=torch.empty(B, L, dtype=torch.int64, device=dev), rel=torch.empty(B, L, dtype=torch.int32, device=dev),
-                wide=torch.empty(B, dtype=torch.uint8, device=dev), thr=torch.empty(65, dtype=torch.int64, device=dev),
+                ts=torch.empty(B, L, dtype=torch.int64, device=dev), thr=torch.empty(65, dtype=torch.int64, device=dev),
                 params=[f(4 * D, D).requires_grad_(True), f(4 * D).requires_grad_(True), f(32, H).requires_grad_(True),
                         f(64, H).requires_grad_(True), f(D).requires_grad_(True), f(D).requires_grad_(True),
                         f(4 * D, D).requires_grad_(True), f(4 * D).requires_grad_(True), f(D, 4 * D).requires_grad_(True),
@@ -50,8 +48,7 @@ def test_fake_tensor_forward_of_the_block():
     B, L, D, H = 3, 50, 128, 4
     with FakeTensorMode():
         a = _layer_args(B, L, D, H, "cuda")
-        y, saved = torch.ops.genrec_b200.hstu_layer(a["x"], a["pad"], a["ts"], a["rel"], a["wide"], a["thr"], *a["params"], H, 64, 0, 0.1, 7,
-                                                    None, 0)
+        y, saved = torch.ops.genrec_b200.hstu_layer(a["x"], a["pad"], a["ts"], a["thr"], *a["params"], H, 64, 0, 0.1, 7, None, 0)
         assert y.shape == (B, L, D) and y.device.type == "cuda" and saved.dtype == torch.uint8 and y.requires_grad
 
 
@@ -62,8 +59,7 @@ def test_meta_forward_and_backward_of_the_block():
     B, L, D, H = 3, 50, 128, 4
     if True:
         a = _layer_args(B, L, D, H, "meta")
-        y, saved = torch.ops.genrec_b200.hstu_layer(a["x"], a["pad"], a["ts"], a["rel"], a["wide"], a["thr"], *a["params"], H, 64, 0, 0.1, 7,
-                                                    None, 0)
+        y, saved = torch.ops.genrec_b200.hstu_layer(a["x"], a["pad"], a["ts"], a["thr"], *a["params"], H, 64, 0, 0.1, 7, None, 0)
         assert y.shape == (B, L, D) and y.dtype == torch.float32 and saved.dtype == torch.uint8
         y.sum().backward()
         assert a["x"].grad.shape == (B, L, D)
@@ -72,7 +68,7 @@ def test_meta_forward_and_backward_of_the_block():
         # without the temporal term
         a = _layer_args(B, L, D, H, "meta")
         a["params"][3] = None
-        y, _ = torch.ops.genrec_b200.hstu_layer(a["x"], a["pad"], None, None, None, a["thr"], *a["params"], H, 0, 0, 0.0, 0, None, 1)
+        y, _ = torch.ops.genrec_b200.hstu_layer(a["x"], a["pad"], None, a["thr"], *a["params"], H, 0, 0, 0.0, 0, None, 1)
         y.sum().backward()
         assert a["params"][2].grad.shape == (32, H)
 
@@ -83,13 +79,11 @@ def test_fake_tensor_other_ops():
         P = torch.empty(2, 40, 512, dtype=torch.bfloat16, device="cuda")
         pad = torch.empty(2, 40, dtype=torch.uint8, device="cuda")
         ts = torch.empty(2, 40, dtype=torch.int64, device="cuda")
-        rel, wide = torch.ops.genrec_b200.hstu_seq_prepare(ts, pad)
-        assert rel.shape == (2, 40) and rel.dtype == torch.int32 and wide.shape == (2,)
         thr = torch.empty(65, dtype=torch.int64, device="cuda")
         wp, wt = torch.empty(32, 4, device="cuda"), torch.empty(64, 4, device="cuda")
-        O = torch.ops.genrec_b200.hstu_attention(P, pad, ts, rel, wide, thr, wp, wt, 4, 0)
+        O = torch.ops.genrec_b200.hstu_attention(P, pad, ts, thr, wp, wt, 4, 0)
         assert O.shape == (2, 40, 128) and O.dtype == torch.bfloat16
-        dzp, dpos, dtime = torch.ops.genrec_b200.hstu_attention_backward(P, P, O, pad, ts, rel, wide, thr, wp, wt, 4, 0)
+        dzp, dpos, dtime = torch.ops.genrec_b200.hstu_attention_backward(P, P, O, pad, ts, thr, wp, wt, 4, 0)
         assert dzp.shape == P.shape and dpos.shape == (32, 4) and dtime.shape == (64, 4)
         ids, emb, res, loss = torch.ops.genrec_b200.rq_residual_argmin(torch.empty(100, 32, device="cuda"), torch.empty(3, 256, 32, device="cuda"), 0.25)
         assert ids.shape == (100, 3) and ids.dtype == torch.int64 and emb.shape == (100, 32, 3) and loss.shape == (100,)
