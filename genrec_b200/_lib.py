@@ -119,7 +119,11 @@ SIGNATURES = {
     "grb_layernorm_backward_workspace_bytes": (c_size_t, [c_int, c_int]),
     "grb_layernorm_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                        c_void_p, c_void_p, c_void_p]),
-    "grb_split3_f32_to_bf16": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p]),
+    "grb_rmsnorm_forward": (c_int, [c_void_p, c_void_p, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_rmsnorm_backward_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "grb_rmsnorm_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                     c_void_p]),
+    "grb_split3_f32_to_bf16":(c_int, [c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p]),
     "grb_linear_f32x3_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "grb_linear_f32x3_bias_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "grb_hstu_layer_f32_workspace_bytes": (c_size_t, [P(HstuDims)]),

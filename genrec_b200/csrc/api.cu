@@ -107,6 +107,18 @@ int with_row_dim(int D, F&& f) {
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
+// the RMS norm kernels add TIGER's attn_dim, 384 (its embedding_dim is 128).  The LayerNorm / HSTU row kernels are not
+// instantiated at 384: nothing calls them there.
+template <class F>
+int with_rms_dim(int D, F&& f) {
+    if (D == 64) f(std::integral_constant<int, 64>{});
+    else if (D == 128) f(std::integral_constant<int, 128>{});
+    else if (D == 256) f(std::integral_constant<int, 256>{});
+    else if (D == 384) f(std::integral_constant<int, 384>{});
+    else return fail(GRB_EINVAL, "rms norm supports D in {64,128,256,384}, got %d", D);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
 int row_grid(int T) {
     int need = (T + ROW_THREADS / 32 - 1) / (ROW_THREADS / 32);
     int cap = sm_count() * 8;
@@ -1238,6 +1250,25 @@ int grb_layernorm_backward(const float* dy, const float* x, const float* stats, 
                            float* dx, float* dg, float* db, void* workspace, void* stream) {
     GRB_REQUIRE(dy && x && stats && g && dx && dg && db && workspace, "null argument");
     return ln_backward(LnBwdArgs{dy, x, stats, g, residual, dx, dg, db, T, D, static_cast<float*>(workspace)}, static_cast<cudaStream_t>(stream));
+}
+
+int grb_rmsnorm_forward(const float* x, const float* w, float eps, int T, int D, void* y_bf16, float* y_f32, float* rstd, void* stream) {
+    GRB_REQUIRE(x && w && (y_bf16 || y_f32) && T > 0, "bad argument");
+    RmsFwdArgs a{x, w, (bf16*)y_bf16, y_f32, rstd, T, D, eps};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return with_rms_dim(D, [&](auto DC) { launch_k(rms_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); });
+}
+size_t grb_rmsnorm_backward_workspace_bytes(int T, int D) {
+    if (T <= 0 || D <= 0) return 0;
+    return (size_t)row_bwd_grid(T) * D * 4;
+}
+int grb_rmsnorm_backward(const float* dy, const float* x, const float* rstd, const float* w, const float* residual, int T, int D, float* dx,
+                         float* dw, void* workspace, void* stream) {
+    GRB_REQUIRE(dy && x && rstd && w && dx && dw && workspace && T > 0, "bad argument");
+    RmsBwdArgs a{dy, x, rstd, w, residual, dx, dw, T, D, static_cast<float*>(workspace)};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GRB_TRY(with_rms_dim(D, [&](auto DC) { launch_k(rms_bwd_kernel<DC / 64>, row_bwd_grid(T), ROW_THREADS, 0, st, a); }));
+    return det_finish(a.part, 1, row_bwd_grid(T), D, 1, 0, 1, {{dw, D}}, st);
 }
 
 int grb_split3_f32_to_bf16(const float* in, void* out_bf16, size_t rows, int K, int operand, void* stream) {

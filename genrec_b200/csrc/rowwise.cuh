@@ -306,6 +306,97 @@ __global__ void __launch_bounds__(ROW_THREADS) ln_bwd_kernel(LnBwdArgs a) {
     }
 }
 
+// ------------------------------------------------------------------------------------------------ T5 RMS norm fwd / bwd
+// y = w * (x * r), r = rsqrt(mean(x^2) + eps)   (genrec/modules/normalize.py:38-55 and :73-96: no mean, no bias)
+struct RmsFwdArgs {
+    const float* x; const float* w;
+    bf16* y_bf16; float* y_f32;  // either nullable
+    float* rstd;                 // nullable [T]
+    int T, D; float eps;
+};
+template <int NP>
+__global__ void __launch_bounds__(ROW_THREADS) rms_fwd_kernel(RmsFwdArgs a) {
+    pdl_wait();
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const int nw = gridDim.x * (ROW_THREADS / 32);
+    for (int row = blockIdx.x * (ROW_THREADS / 32) + wib; row < a.T; row += nw) {
+        float xv[NP][2];
+        float q = 0.f;
+#pragma unroll
+        for (int p = 0; p < NP; ++p) {
+            float2 f = *reinterpret_cast<const float2*>(a.x + (size_t)row * a.D + 2 * lane + 64 * p);
+            xv[p][0] = f.x; xv[p][1] = f.y;
+            q += f.x * f.x + f.y * f.y;
+        }
+        const float r = rsqrtf(warp_sum(q) / (float)a.D + a.eps);
+#pragma unroll
+        for (int p = 0; p < NP; ++p) {
+            int c = 2 * lane + 64 * p;
+            float y0 = a.w[c] * (xv[p][0] * r), y1 = a.w[c + 1] * (xv[p][1] * r);
+            if (a.y_bf16) *reinterpret_cast<uint32_t*>(a.y_bf16 + (size_t)row * a.D + c) = pack_bf16(y0, y1);
+            if (a.y_f32) *reinterpret_cast<float2*>(a.y_f32 + (size_t)row * a.D + c) = make_float2(y0, y1);
+        }
+        if (lane == 0 && a.rstd) a.rstd[row] = r;
+    }
+}
+// dx = (res ? res : 0) + r * (g - xh * mean(g * xh)), g = dy * w, xh = x * r ; dw += sum over rows of dy * xh
+struct RmsBwdArgs {
+    const float* dy; const float* x; const float* rstd; const float* w;
+    const float* res;  // nullable, added to dx
+    float* dx; float* dw;
+    int T, D;
+    float* part;       // [gridDim.x][D] scratch for the ordered cross-CTA sum (det_finish_kernel adds it to dw)
+};
+template <int NP>
+__global__ void __launch_bounds__(ROW_THREADS) rms_bwd_kernel(RmsBwdArgs a) {
+    pdl_wait();
+    __shared__ float red[ROW_THREADS / 32][64 * NP];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const int nw = gridDim.x * (ROW_THREADS / 32);
+    float adw[NP][2];
+#pragma unroll
+    for (int p = 0; p < NP; ++p) adw[p][0] = adw[p][1] = 0.f;
+    const float invD = 1.f / (float)a.D;
+    for (int row = blockIdx.x * (ROW_THREADS / 32) + wib; row < a.T; row += nw) {
+        const float r = a.rstd[row];
+        float xh[NP][2], gg[NP][2];
+        float sb = 0.f;
+#pragma unroll
+        for (int p = 0; p < NP; ++p) {
+            int c = 2 * lane + 64 * p;
+            float2 xv = *reinterpret_cast<const float2*>(a.x + (size_t)row * a.D + c);
+            float2 dv = *reinterpret_cast<const float2*>(a.dy + (size_t)row * a.D + c);
+            xh[p][0] = xv.x * r; xh[p][1] = xv.y * r;
+            adw[p][0] += dv.x * xh[p][0]; adw[p][1] += dv.y * xh[p][1];
+            gg[p][0] = dv.x * a.w[c]; gg[p][1] = dv.y * a.w[c + 1];
+            sb += gg[p][0] * xh[p][0] + gg[p][1] * xh[p][1];
+        }
+        sb = warp_sum(sb) * invD;
+#pragma unroll
+        for (int p = 0; p < NP; ++p) {
+            int c = 2 * lane + 64 * p;
+            float d0 = r * (gg[p][0] - xh[p][0] * sb), d1 = r * (gg[p][1] - xh[p][1] * sb);
+            if (a.res) {
+                float2 rv = *reinterpret_cast<const float2*>(a.res + (size_t)row * a.D + c);
+                d0 += rv.x; d1 += rv.y;
+            }
+            *reinterpret_cast<float2*>(a.dx + (size_t)row * a.D + c) = make_float2(d0, d1);
+        }
+    }
+#pragma unroll
+    for (int p = 0; p < NP; ++p)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) red[wib][2 * lane + 64 * p + e] = adw[p][e];
+    __syncthreads();
+    auto colsum = [&](int c) {
+        float s = 0.f;
+#pragma unroll
+        for (int w = 0; w < ROW_THREADS / 32; ++w) s += red[w][c];
+        return s;
+    };
+    det_store(a.part, 0, blockIdx.x, gridDim.x, a.D, a.D, colsum);
+}
+
 // ------------------------------------------------------------------------------------------------ casts / column sums
 // out_bf16[i] = bf16(dropmask(in[i]) * row_scale[row])       (n = T*D elements, D = row length)
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, size_t n, int D, Dropout drop,

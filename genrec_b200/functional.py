@@ -544,6 +544,27 @@ def layernorm_bwd(dy, x, st, g, residual=None):
     return dx, dg, db
 
 
+def rmsnorm_fwd(x, w, eps, want_bf16=True, want_f32=False):
+    """T5 RMS norm of x [..., D] fp32 contiguous -> (y bf16 | None, y fp32 | None, rstd fp32 [T])"""
+    T, D = x.numel() // x.shape[-1], x.shape[-1]
+    yb = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if want_bf16 else None
+    yf = torch.empty(x.shape, dtype=torch.float32, device=x.device) if want_f32 else None
+    rstd = torch.empty(T, dtype=torch.float32, device=x.device)
+    check(_lib.load().grb_rmsnorm_forward(ptr(x), ptr(w), float(eps), T, D, ptr(yb), ptr(yf), ptr(rstd), stream_ptr(x.device)))
+    return yb, yf, rstd
+
+
+def rmsnorm_bwd(dy, x, rstd, w, residual=None):
+    """-> (dx fp32 (+ residual), dw fp32), dw summed in a fixed order"""
+    lib = _lib.load()
+    T, D = x.numel() // x.shape[-1], x.shape[-1]
+    dx = torch.empty_like(x)
+    dw = torch.zeros_like(w)
+    ws = _u8(lib.grb_rmsnorm_backward_workspace_bytes(T, D), x.device)
+    check(lib.grb_rmsnorm_backward(ptr(dy), ptr(x), ptr(rstd), ptr(w), ptr(residual), T, D, ptr(dx), ptr(dw), ptr(ws), stream_ptr(x.device)))
+    return dx, dw
+
+
 def linear_fwd(xb, wb, bias, act, p=0.0, seed=0, seed_dev=None, site=0):
     """z = xb @ wb^T + bias (bf16) ; act: 0 none, 1 silu, 2 relu -> returns (z, act(z) with dropout)"""
     lib = _lib.load()

@@ -1,0 +1,366 @@
+"""TIGER (SURVEY.md section 8 row f4): drop-in mirror of ``genrec/models/tiger.py:88-452``.
+
+Same constructor arguments, parameter names / shapes (a reference checkpoint loads with ``strict=True``), ``forward``,
+``_encode_context``, ``_decode_step`` and ``generate`` as the reference's ``Tiger``.  Bind it with
+
+    import genrec.models.tiger, genrec_b200.tiger
+    genrec.models.tiger.Tiger = genrec_b200.tiger.Tiger
+
+The norms are the T5 RMS norm kernels, the projections and the ReLU FFN the wgmma GEMMs of this library (ReLU and the hidden dropout
+in the GEMM epilogue), attention the T5 attention core (``t5_attention._T5AttnFn``).  bf16 operands, fp32 accumulation.  The
+embedding gathers, the residual adds, the dropouts on the block inputs / residual branches and the 769-class cross-entropy stay in
+torch.
+
+``generate`` projects the encoder memory's cross-attention K and V once per user (not once per beam, as the reference's expanded
+memory does), runs step 0 on one row per user, and otherwise computes row for row what ``tiger_decode.generate`` on this module
+computes: the same kernels on the same rows, so the beams and log-probabilities are the same bits.
+"""
+from __future__ import annotations
+
+import math
+from typing import NamedTuple, Optional
+
+import torch
+import torch.nn.functional as F
+from torch import nn
+
+from . import _lib
+from . import functional as Fn
+from . import tiger_decode as td
+from .t5_attention import T5Attention, _T5AttnFn, _bucket_map, _zero_bias, attention_core_fwd
+from .tiger_decode import TigerGenerationOutput
+
+__all__ = ["Tiger", "TigerOutput", "TigerGenerationOutput"]
+
+RMS_EPS = 1e-6                      # RMSNorm / RootMeanSquareLayerNorm default (normalize.py:42, :77)
+RMS_DIMS = (64, 128, 256, 384)      # widths of the RMS norm kernels
+FFN_DIM = 1024                      # tiger.py:140
+_SITES = {"n": 1 << 30}             # dropout sites of the FFN epilogues (the attention core numbers its own from 1)
+
+
+class TigerOutput(NamedTuple):      # (tiger.py:73-78)
+    logits: torch.Tensor
+    loss: torch.Tensor
+
+
+def _seed(p: float) -> int:
+    return torch.initial_seed() & 0x7FFFFFFFFFFFFFFF if p > 0 else 0
+
+
+class _RmsNormFn(torch.autograd.Function):
+    """y = w * x * rsqrt(mean(x^2) + eps) on fp32 rows."""
+
+    @staticmethod
+    def forward(ctx, x, w):
+        xc = x.detach().contiguous().float()
+        _, y, rstd = Fn.rmsnorm_fwd(xc, w.detach(), RMS_EPS, want_bf16=False, want_f32=True)
+        ctx.save_for_backward(xc, rstd, w)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xc, rstd, w = ctx.saved_tensors
+        dx, dw = Fn.rmsnorm_bwd(dy.contiguous().float(), xc, rstd, w.detach())
+        return dx, dw
+
+
+class _LinearFn(torch.autograd.Function):
+    """Bias-free nn.Linear: fp32 rows -> bf16 operand -> fp32 result (in_proj / in_proj_context)."""
+
+    @staticmethod
+    def forward(ctx, x, w):
+        xb = Fn.cast_rows_bf16(x.detach().contiguous().float())
+        wb = Fn.cast_bf16(w)
+        y, _ = Fn.linear_fwd(xb, wb, _zero_bias(w.shape[0], x.device), 0)
+        ctx.save_for_backward(xb, wb)
+        return y.float()
+
+    @staticmethod
+    def backward(ctx, dy):
+        xb, wb = ctx.saved_tensors
+        dx, dw, _ = Fn.linear_bwd(Fn.cast_rows_bf16(dy.contiguous().float()), wb, xb)
+        return dx, dw
+
+
+class _FfnFn(torch.autograd.Function):
+    """x + drop(wo(drop(relu(wi(norm2(x)))))) - the FFN half of a block (transformer.py:181-189, :323): the norm writes the bf16
+    operand, ReLU and the hidden dropout run in the first GEMM's epilogue, the output dropout and the residual in the second's."""
+
+    @staticmethod
+    def forward(ctx, x, nw, wi, wo, p):
+        xc = x.detach().contiguous().float()
+        dev, D = xc.device, xc.shape[-1]
+        xnb, _, rstd = Fn.rmsnorm_fwd(xc, nw.detach(), RMS_EPS)
+        wib, wob = Fn.cast_bf16(wi), Fn.cast_bf16(wo)
+        seed = _seed(p)
+        _SITES["n"] += 2
+        site = _SITES["n"]
+        z, h = Fn.linear_fwd(xnb, wib, _zero_bias(wi.shape[0], dev), 2, p, seed, None, site)
+        y = Fn.linear_residual_fwd(h, wob, _zero_bias(D, dev), xc, None, p, seed, None, site + 1)
+        ctx.save_for_backward(xc, rstd, xnb, z, h, wib, wob, nw)
+        ctx.cfg = (p, seed, site)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xc, rstd, xnb, z, h, wib, wob, nw = ctx.saved_tensors
+        p, seed, site = ctx.cfg
+        dyc = dy.contiguous().float()
+        dyb = Fn.cast_rows_bf16(dyc, None, p, seed, None, site + 1)
+        _, dwo, _ = Fn.linear_bwd(dyb, wob, h, need_dx=False)
+        dz = Fn.linear_dact_bwd(dyb, wob, z, 2, p, seed, None, site)
+        dxn, dwi, _ = Fn.linear_bwd(dz, wib, xnb)
+        dx, dnw = Fn.rmsnorm_bwd(dxn, xc, rstd, nw.detach(), residual=dyc)
+        return dx, dnw, dwi, dwo, None
+
+
+def _head_mirrors(w: torch.Tensor):
+    """bf16 copies of output_head.weight [V, D] padded with zero rows to a multiple of 8: [Vp, D] and its transpose [D, Vp]."""
+    V, D = w.shape
+    Vp = (V + 7) // 8 * 8
+    wp = torch.zeros(Vp, D, dtype=torch.bfloat16, device=w.device)
+    Fn.cast_bf16(w, wp[:V])
+    return wp, wp.t().contiguous()
+
+
+def _head_logits(xb: torch.Tensor, wpt: torch.Tensor, V: int) -> torch.Tensor:
+    """fp32 logits [R, V] = x W^T: the linear backward's dx GEMM (fp32 output) with W^T [D, Vp] as its weight operand."""
+    y, _, _ = Fn.linear_bwd(xb, wpt, None, need_dw=False)
+    return y[..., :V]
+
+
+class _HeadFn(torch.autograd.Function):
+    """output_head (tiger.py:147, :207): fp32 logits [..., V] of fp32 rows."""
+
+    @staticmethod
+    def forward(ctx, x, w):
+        xb = Fn.cast_rows_bf16(x.detach().contiguous().float())
+        wp, wpt = _head_mirrors(w)
+        ctx.save_for_backward(xb, wp)
+        ctx.V = w.shape[0]
+        return _head_logits(xb, wpt, ctx.V)
+
+    @staticmethod
+    def backward(ctx, dy):
+        xb, wp = ctx.saved_tensors
+        dpad = torch.zeros(*dy.shape[:-1], wp.shape[0], dtype=torch.float32, device=dy.device)
+        dpad[..., :ctx.V] = dy
+        dx, dw, _ = Fn.linear_bwd(Fn.cast_rows_bf16(dpad), wp, xb)
+        return dx, dw[:ctx.V]
+
+
+# ---- modules with the reference's parameter names (embedding.py, normalize.py, transformer.py)
+class _Norm(nn.Module):
+    def __init__(self, dim: int) -> None:
+        super().__init__()
+        self.weight = nn.Parameter(torch.ones(dim))
+
+    def forward(self, x):
+        return _RmsNormFn.apply(x, self.weight)
+
+
+class _Emb(nn.Module):
+    def __init__(self, n: int, dim: int, padding_idx: Optional[int] = None) -> None:
+        super().__init__()
+        self.emb = nn.Embedding(n, dim, padding_idx=padding_idx)
+
+
+class _MHA(nn.Module):
+    def __init__(self, dim: int, heads: int, dropout: float, cross: bool) -> None:
+        super().__init__()
+        self.attn = T5Attention(dim, heads, dropout, is_cross_attention=cross)
+
+
+class _FF(nn.Module):
+    def __init__(self, dim: int, hidden: int) -> None:
+        super().__init__()
+        self.wi = nn.Linear(dim, hidden, bias=False)
+        self.wo = nn.Linear(hidden, dim, bias=False)
+
+
+class _Block(nn.Module):
+    def __init__(self, dim: int, heads: int, dropout: float, cross: bool) -> None:
+        super().__init__()
+        self.self_attn = _MHA(dim, heads, dropout, False)
+        self.norm1 = _Norm(dim)
+        if cross:
+            self.cross_attn = _MHA(dim, heads, dropout, True)
+            self.norm_cross = _Norm(dim)
+        self.ff = _FF(dim, FFN_DIM)
+        self.norm2 = _Norm(dim)
+
+
+class _Stack(nn.Module):
+    def __init__(self, dim: int, depth: int, heads: int, dropout: float, cross: bool) -> None:
+        super().__init__()
+        self.layers = nn.ModuleList([_Block(dim, heads, dropout, cross) for _ in range(depth)])
+
+
+class _EncDec(nn.Module):
+    def __init__(self, dim: int, heads: int, n_enc: int, n_dec: int, dropout: float) -> None:
+        super().__init__()
+        self.encoder = _Stack(dim, n_enc, heads, dropout, False)
+        self.decoder = _Stack(dim, n_dec, heads, dropout, True)
+
+
+class Tiger(nn.Module):
+    """Mirror of genrec/models/tiger.py:88-452."""
+
+    def __init__(self, embedding_dim: int, attn_dim: int, dropout: float, num_heads: int, n_layers: int, num_item_embeddings: int,
+                 num_user_embeddings: int, sem_id_dim: int, max_pos: int = 2048) -> None:
+        super().__init__()
+        if attn_dim % num_heads or attn_dim // num_heads not in (32, 64):
+            raise _lib.GrbError(f"genrec_b200 error -1: head_dim {attn_dim / num_heads:g} unsupported (32, 64)")
+        for name, d in (("embedding_dim", embedding_dim), ("attn_dim", attn_dim)):
+            if d % 8 or d not in RMS_DIMS:
+                raise _lib.GrbError(f"genrec_b200 error -1: {name} {d} unsupported {RMS_DIMS}")
+        self.embedding_dim, self.attn_dim, self.dropout, self.num_heads, self.n_layers = embedding_dim, attn_dim, dropout, num_heads, n_layers
+        self.num_item_embeddings, self.num_user_embeddings, self.sem_id_dim, self.max_pos = (num_item_embeddings, num_user_embeddings,
+                                                                                            sem_id_dim, max_pos)
+        self.bos_embedding = nn.Parameter(torch.randn(embedding_dim))
+        self.norm = _Norm(embedding_dim)
+        self.norm_context = _Norm(embedding_dim)
+        self.drop = nn.Dropout(p=dropout)
+        self.sem_id_embedding = _Emb(num_item_embeddings * sem_id_dim + 1, embedding_dim, padding_idx=num_item_embeddings * sem_id_dim)
+        self.user_id_embedding = _Emb(num_user_embeddings, embedding_dim)
+        self.pos_embedding = nn.Embedding(max_pos, embedding_dim)                 # unused by the reference's forward, kept for checkpoints
+        self.decoder_pos_embedding = nn.Embedding(sem_id_dim, embedding_dim)
+        self.in_proj = nn.Linear(embedding_dim, attn_dim, bias=False)
+        self.in_proj_context = nn.Linear(embedding_dim, attn_dim, bias=False)
+        self.transformer = _EncDec(attn_dim, num_heads, n_layers // 2, n_layers // 2, dropout)
+        self.out_proj = nn.Linear(attn_dim, embedding_dim, bias=False)
+        self.vocab_size = num_item_embeddings * sem_id_dim + 1
+        self.output_head = nn.Linear(attn_dim, self.vocab_size, bias=False)
+
+    # ---- pieces
+    def _p(self) -> float:
+        return self.dropout if self.training else 0.0
+
+    def _sem_emb(self, ids, types):
+        return self.sem_id_embedding.emb(types * self.num_item_embeddings + ids)          # embedding.py:42-43
+
+    def _context_input(self, user_input_ids, item_input_ids, token_type_ids, seq_mask):
+        """-> (encoder input [B, 1+N, attn_dim] fp32, key padding [B, 1+N] bool)"""
+        user_emb = self.user_id_embedding.emb(user_input_ids % self.num_user_embeddings)   # embedding.py:73-74
+        x = torch.cat([user_emb, self._sem_emb(item_input_ids, token_type_ids)], dim=1)
+        pad = torch.cat([torch.zeros(seq_mask.size(0), 1, dtype=torch.bool, device=seq_mask.device), seq_mask == 0], dim=1)
+        x = _LinearFn.apply(F.dropout(self.norm_context(x), self._p(), self.training), self.in_proj_context.weight)
+        return x, pad
+
+    def _decoder_input(self, B: int, tgt_ids, tgt_type):
+        bos = self.bos_embedding.view(1, 1, -1).expand(B, 1, -1)
+        x = bos if tgt_ids is None else torch.cat([bos, self._sem_emb(tgt_ids, tgt_type)], dim=1)
+        return _LinearFn.apply(F.dropout(self.norm(x), self._p(), self.training), self.in_proj.weight)
+
+    def _self_attn(self, blk, x, pad, causal):
+        a = blk.self_attn.attn
+        L = x.shape[1]
+        bucket = _bucket_map(L, L, a.num_relative_buckets, a.max_distance, x.device)
+        kp = pad.to(torch.uint8).contiguous() if pad is not None else None
+        out = _T5AttnFn.apply(blk.norm1(x), None, None, kp, causal, a.n_heads, self._p(), bucket, a.q.weight, a.kv.weight, None,
+                              a.o.weight, a.rel_bias.weight, True)
+        return x + F.dropout(out, self._p(), self.training)
+
+    def _ffn(self, blk, x):
+        return _FfnFn.apply(x, blk.norm2.weight, blk.ff.wi.weight, blk.ff.wo.weight, self._p())
+
+    def _encoder(self, x, pad):
+        for blk in self.transformer.encoder.layers:                                      # transformer.py:363-365, :303-324
+            x = self._ffn(blk, self._self_attn(blk, x, pad, False))
+        return x
+
+    def _cross(self, blk, x, memory, memory_pad):
+        a = blk.cross_attn.attn
+        kp = memory_pad.to(torch.uint8).contiguous()
+        out = _T5AttnFn.apply(blk.norm_cross(x), memory, memory, kp, False, a.n_heads, self._p(), None, a.q.weight, a.k.weight, a.v.weight,
+                              a.o.weight, None, False)
+        return x + F.dropout(out, self._p(), self.training)
+
+    def _decoder(self, x, cross):
+        for i, blk in enumerate(self.transformer.decoder.layers):                        # transformer.py:406-414, :303-324
+            x = self._self_attn(blk, x, None, True)
+            x = cross(i, blk, x)
+            x = self._ffn(blk, x)
+        return x
+
+    # ---- the reference's interface
+    def forward(self, user_input_ids, item_input_ids, token_type_ids, target_input_ids, target_token_type_ids, seq_mask) -> TigerOutput:
+        if seq_mask is None:
+            seq_mask = torch.ones_like(item_input_ids, dtype=torch.long, device=item_input_ids.device)
+        B = item_input_ids.size(0)
+        src, pad = self._context_input(user_input_ids, item_input_ids, token_type_ids, seq_mask)
+        tgt = self._decoder_input(B, target_input_ids, target_token_type_ids)
+        memory = self._encoder(src, pad)
+        out = self._decoder(tgt, lambda i, blk, x: self._cross(blk, x, memory, pad))
+        logits = _HeadFn.apply(out, self.output_head.weight)
+        loss = None
+        if target_input_ids is not None and target_input_ids.shape[1] == self.sem_id_dim:   # tiger.py:232-242
+            target_vocab_ids = target_token_type_ids * self.num_item_embeddings + target_input_ids
+            loss_logits = logits[:, :-1, :]
+            loss = F.cross_entropy(loss_logits.reshape(-1, loss_logits.size(-1)), target_vocab_ids.reshape(-1),
+                                   reduction="none").reshape(B, -1).sum(dim=1).mean()
+        return TigerOutput(logits=logits, loss=loss)
+
+    def _encode_context(self, user_input_ids, item_input_ids, token_type_ids, seq_mask=None):
+        if seq_mask is None:
+            seq_mask = torch.ones_like(item_input_ids, dtype=torch.long, device=item_input_ids.device)
+        src, pad = self._context_input(user_input_ids, item_input_ids, token_type_ids, seq_mask)
+        return self._encoder(src, pad), pad
+
+    def _decode_step(self, memory, memory_mask, tgt_ids, tgt_type):
+        x = self._decoder_input(memory.size(0), tgt_ids, tgt_type)
+        out = self._decoder(x, lambda i, blk, h: self._cross(blk, h, memory, memory_mask))
+        return _HeadFn.apply(out[:, -1], self.output_head.weight)
+
+    @torch.no_grad()
+    def generate(self, user_input_ids, item_input_ids, token_type_ids, seq_mask=None, temperature: float = 0.2, n_top_k_candidates: int = 10,
+                 valid_item_ids=None, use_trie: bool = True, generator: Optional[torch.Generator] = None) -> TigerGenerationOutput:
+        """Trie-constrained beam search (tiger.py:312-452) with the memory's cross-attention K / V projected once per user.  No host
+        synchronisation once the trie is built (first call), so a warmed-up call can be captured in a CUDA graph."""
+        B, K = user_input_ids.size(0), n_top_k_candidates
+        dev = user_input_ids.device
+        trie = None
+        if use_trie:
+            trie = getattr(self, "_grb_trie", None)
+            if trie is None:
+                trie = td.TrieCSR.build(valid_item_ids).to(dev)
+                self._grb_trie = trie
+        memory, memory_pad = self._encode_context(user_input_ids, item_input_ids, token_type_ids, seq_mask)
+        kp = memory_pad.to(torch.uint8).contiguous()
+        xm = Fn.cast_rows_bf16(memory.contiguous())
+        D, Lm = self.attn_dim, memory.size(1)
+        mem_kv = []                                                  # per decoder block: K, V [B, 1+N, D] bf16
+        for blk in self.transformer.decoder.layers:
+            a = blk.cross_attn.attn
+            Km, _ = Fn.linear_fwd(xm, Fn.cast_bf16(a.k.weight), _zero_bias(D, dev), 0)
+            Vm, _ = Fn.linear_fwd(xm, Fn.cast_bf16(a.v.weight), _zero_bias(D, dev), 0)
+            mem_kv.append((Km, Vm))
+        wcache = [(Fn.cast_bf16(b.cross_attn.attn.q.weight), Fn.cast_bf16(b.cross_attn.attn.o.weight)) for b in self.transformer.decoder.layers]
+        H = self.num_heads
+        scale = 1.0 / math.sqrt(D // H)
+
+        def cross(i, blk, x):
+            # the queries of a user's beams against that user's memory: [B*R, S, D] viewed as [B, R*S, D]
+            R, S = x.size(0) // B, x.size(1)
+            wq, wo = wcache[i]
+            Q, _ = Fn.linear_fwd(Fn.cast_rows_bf16(blk.norm_cross(x).contiguous()), wq, _zero_bias(D, dev), 0)
+            A, _ = attention_core_fwd(Q.view(B, R * S, D), mem_kv[i][0], mem_kv[i][1], H, None, None, kp, False, scale)
+            out, _ = Fn.linear_fwd(A.view(B * R, S, D), wo, _zero_bias(D, dev), 0)
+            return x + out.float()
+
+        wp, wpt = _head_mirrors(self.output_head.weight)
+        V = self.vocab_size
+
+        def decode_step(tgt):
+            if tgt.size(1) == 0:                                     # every beam is [bos]: one row per user, logits broadcast
+                x = self._decoder_input(B, None, None)
+                rows = B
+            else:
+                types = torch.arange(tgt.size(1), device=dev).unsqueeze(0).expand(tgt.size(0), -1)
+                x = self._decoder_input(tgt.size(0), tgt, types)
+                rows = tgt.size(0)
+            out = self._decoder(x, cross)
+            logits = _head_logits(Fn.cast_rows_bf16(out[:, -1].contiguous()), wpt, V)
+            return logits if rows == B * K else logits.unsqueeze(1).expand(B, K, V).reshape(B * K, V)
+
+        return td.beam_search(decode_step, B, K, self.sem_id_dim, self.num_item_embeddings, dev, temperature, trie, generator)

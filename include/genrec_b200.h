@@ -271,6 +271,14 @@ int grb_layernorm_forward(const float* x, const float* g, const float* b, float 
 size_t grb_layernorm_backward_workspace_bytes(int T, int D);
 int grb_layernorm_backward(const float* dy, const float* x, const float* stats, const float* g, const float* residual,
                            int T, int D, float* dx, float* dg, float* db, void* workspace, void* stream);
+/* T5 RMS norm (TIGER's RMSNorm and RootMeanSquareLayerNorm): y = w * x * rsqrt(mean(x^2) + eps), no mean, no bias.
+ * x [T, D] fp32, D in {64, 128, 256, 384}.  Forward writes y as bf16 and / or fp32 (either may be NULL) and rstd [T] (may be NULL).
+ * Backward: dx = RMS norm backward of dy (+ residual, may be NULL) ; dw += in a fixed order, so two calls give the same bits.
+ * workspace: grb_rmsnorm_backward_workspace_bytes(T, D). */
+int grb_rmsnorm_forward(const float* x, const float* w, float eps, int T, int D, void* y_bf16, float* y_f32, float* rstd, void* stream);
+size_t grb_rmsnorm_backward_workspace_bytes(int T, int D);
+int grb_rmsnorm_backward(const float* dy, const float* x, const float* rstd, const float* w, const float* residual, int T, int D,
+                         float* dx, float* dw, void* workspace, void* stream);
 
 /* fp32-accurate linear layer on the bf16 tensor path (the RQ-VAE encoder MLP, genrec/modules/encoder.py:399-420: bias-free
  * Linear + SiLU).  Operands are split into three bf16 terms each and the six significant cross terms are laid out along K

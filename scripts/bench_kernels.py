@@ -2,7 +2,7 @@
 cached incremental HSTU inference next to full recompute, RQ-VAE Sinkhorn and k-means init) with CUDA events, against the relevant
 roofline or the torch code they replace.  Prints one JSON line per measurement; `bench_kernels.py rqvae_train` runs only the RQ-VAE
 training rows, `bench_kernels.py linear_bwd` only the linear-backward and SASRec training-step rows, `bench_kernels.py head_topk` only
-the fused top-k head rows."""
+the fused top-k head rows, `bench_kernels.py tiger` only the TIGER rows (training step, generate eager / graph / uncached loop)."""
 import json
 import os
 import sys
@@ -320,6 +320,58 @@ def bench_linear_bwd(dev):
     print(json.dumps(dict(kernel="sasrec_train_step", B=B, L=L, D=64, blocks=2, num_items=V, dropout=0.2, ms=ms, **info)), flush=True)
 
 
+def bench_tiger(dev):
+    """TIGER at config/tiger/amazon/tiger.gin shape: one training step (forward, backward, AdamW) at B = 256, and generate at B = 256,
+    K = 10 with a 12,000-item trie - eager, replayed from a CUDA graph, and the uncached tiger_decode.generate loop (the reference's
+    schedule: memory expanded to every beam) on the same module, the three alternated in rounds."""
+    from genrec_b200 import tiger_decode as td
+    from genrec_b200.tiger import Tiger
+    from tests import tiger_params as tp
+    info = card()
+    cfg = dict(tp.PUBLISHED, dropout=0.1)
+    B, K = 256, 10
+    m = Tiger(**cfg)
+    m.load_state_dict(tp.tiger_params([(k, v.shape) for k, v in m.state_dict().items()], 3))
+    m = m.to(dev)
+    b = {k: v.to(dev) for k, v in tp.batch(cfg, B, 20, 5).items()}
+    opt = torch.optim.AdamW(m.parameters(), lr=1e-4, weight_decay=0.035, fused=True)
+
+    def step():
+        opt.zero_grad(set_to_none=False)
+        m(**b).loss.backward()
+        opt.step()
+
+    m.train()
+    ms = timed(step, iters=20, warm=5)
+    print(json.dumps(dict(kernel="tiger_train_step", B=B, history_items=20, dropout=0.1, optimizer="AdamW (torch fused)", ms=ms, **info)),
+          flush=True)
+    m.eval()
+    valid = torch.randint(0, 256, (12000, 3), generator=torch.Generator().manual_seed(1))
+    m._grb_trie = td.TrieCSR.build(valid).to(dev)
+    args = (b["user_input_ids"], b["item_input_ids"], b["token_type_ids"], b["seq_mask"])
+    eager = lambda: m.generate(*args, n_top_k_candidates=K)                 # noqa: E731
+    uncached = lambda: td.generate(m, *args, n_top_k_candidates=K)          # noqa: E731
+    for _ in range(2):
+        eager(), uncached()
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        eager()
+    torch.cuda.current_stream().wait_stream(s)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        eager()
+    rows = {"eager": [], "graph": [], "uncached": []}
+    for _ in range(3):
+        rows["eager"].append(timed(eager, iters=10, warm=1))
+        rows["graph"].append(timed(graph.replay, iters=10, warm=1))
+        rows["uncached"].append(timed(uncached, iters=10, warm=1))
+    for name, v in rows.items():
+        print(json.dumps(dict(kernel="tiger_generate_" + name, B=B, K=K, trie_items=12000, ms_per_round=v, ms=min(v), **info)), flush=True)
+    print(json.dumps(dict(kernel="tiger_generate_speedup", eager_vs_uncached=min(rows["uncached"]) / min(rows["eager"]),
+                          graph_vs_uncached=min(rows["uncached"]) / min(rows["graph"]))), flush=True)
+
+
 def main():
     dev = torch.device("cuda:0")
     if sys.argv[1:] == ["rqvae_train"]:
@@ -330,6 +382,9 @@ def main():
         return
     if sys.argv[1:] == ["head_topk"]:
         bench_head_topk(dev)
+        return
+    if sys.argv[1:] == ["tiger"]:
+        bench_tiger(dev)
         return
     peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) \
         if os.path.exists("MEASURED_PEAKS.json") else {}
