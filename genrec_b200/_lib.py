@@ -131,9 +131,10 @@ SIGNATURES = {
     "grb_layernorm_f32_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_void_p, c_void_p]),
     "grb_t5_attention_forward": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 8 + [c_void_p, c_void_p, c_int, c_void_p, c_int, c_float, c_float,
                                          c_u64, c_void_p, C.c_uint32, c_void_p, c_int, c_void_p, c_void_p]),
+    "grb_t5_attention_backward_workspace_bytes": (c_size_t, [c_int] * 6),
     "grb_t5_attention_backward": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 8 + [c_void_p, c_void_p, c_int, c_void_p, c_int, c_float, c_float,
                                           c_u64, c_void_p, C.c_uint32, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
-                                          c_void_p, c_void_p, c_void_p]),
+                                          c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_trie_log_softmax": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                      c_void_p, c_void_p]),
     "grb_beam_select": (c_int, [c_void_p] * 8 + [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -1398,28 +1398,61 @@ int grb_t5_attention_forward(const void* q, const void* k, const void* v, int B,
     GRB_CUDA(cudaGetLastError());
     return 0;
 }
+namespace {
+struct T5BwdWork {
+    float *db_part, *dkv_part;   // null when not needed
+    size_t bytes;
+};
+// the backward's scratch: the bias bins of every CTA when there is a bias table, and the per-query-tile dK / dV partials when
+// there are more than two query tiles (with one or two, the atomics onto zero are exact in either order)
+T5BwdWork carve_t5_bwd(void* base, int B, int Lq, int Lk, int H, int head_dim, int nb) {
+    T5BwdWork w{nullptr, nullptr, 0};
+    Carver c{static_cast<char*>(base)};
+    const int nqt = (Lq + T5_ROWS - 1) / T5_ROWS;
+    if (nb > 0) w.db_part = c.take<float>((size_t)H * B * nqt * nb * 4);
+    if (nqt > 2) w.dkv_part = c.take<float>((size_t)2 * nqt * B * Lk * H * head_dim * 4);
+    w.bytes = c.off;
+    return w;
+}
+}  // namespace
+
+size_t grb_t5_attention_backward_workspace_bytes(int B, int Lq, int Lk, int H, int head_dim, int num_buckets) {
+    if (B <= 0 || Lq <= 0 || Lk <= 0 || H <= 0 || head_dim <= 0 || num_buckets < 0) return 0;
+    return carve_t5_bwd(nullptr, B, Lq, Lk, H, head_dim, num_buckets).bytes;
+}
 int grb_t5_attention_backward(const void* q, const void* k, const void* v, int B, int Lq, int Lk, int H, int head_dim, int ldq, int ldk, int ldv,
                               const float* bias, const int32_t* bucket, int num_buckets, const uint8_t* key_pad, int causal, float scale,
                               float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t site, const void* out, int ldo,
                               const float* lse, const void* dout, int lddo, void* dq, int lddq, float* dk, float* dv, float* dbias,
-                              void* stream) {
+                              void* workspace, void* stream) {
     T5AttnArgs a;
     GRB_TRY(t5_args(a, q, k, v, B, Lq, Lk, H, head_dim, ldq, ldk, ldv, bias, bucket, num_buckets, key_pad, causal, scale, dropout_p, seed, seed_dev, site));
     GRB_REQUIRE(out && lse && dout && dq && dk && dv && ldo % 8 == 0 && lddo % 8 == 0 && lddq % 8 == 0, "bad argument");
-    GRB_REQUIRE(aligned16(out) && aligned16(dout) && aligned16(dq), "rows must be 16-byte aligned");
+    GRB_REQUIRE(aligned16(out) && aligned16(dout) && aligned16(dq) && aligned16(dk) && aligned16(dv), "rows must be 16-byte aligned");
     a.out = (bf16*)const_cast<void*>(out); a.ldo = ldo; a.lse = const_cast<float*>(lse); a.dout = (const bf16*)dout; a.lddo = lddo;
     a.dq = (bf16*)dq; a.lddq = lddq; a.dk = dk; a.dv = dv; a.dbias = bias ? dbias : nullptr;
+    const T5BwdWork w = carve_t5_bwd(workspace, B, Lq, Lk, H, head_dim, a.nb);
+    GRB_REQUIRE(workspace || w.bytes == 0, "workspace is null");
+    GRB_REQUIRE(!workspace || aligned16(workspace), "workspace must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    GRB_CUDA(cudaMemsetAsync(dk, 0, (size_t)B * Lk * H * head_dim * sizeof(float), st));
-    GRB_CUDA(cudaMemsetAsync(dv, 0, (size_t)B * Lk * H * head_dim * sizeof(float), st));
+    const size_t n = (size_t)B * Lk * H * head_dim;
+    if (!w.dkv_part) {
+        GRB_CUDA(cudaMemsetAsync(dk, 0, n * sizeof(float), st));
+        GRB_CUDA(cudaMemsetAsync(dv, 0, n * sizeof(float), st));
+    }
     dim3 grid((Lq + T5_ROWS - 1) / T5_ROWS, B * H);
     GRB_TRY(with_head_dim(head_dim, [&](auto DH) -> int {
         const size_t smem = t5_bwd_smem<DH>(a.nb);
         GRB_TRY(set_smem(t5_attn_bwd_kernel<DH>, smem));
-        launch_k(t5_attn_bwd_kernel<DH>, grid, T5_THREADS, smem, st, a);
+        launch_k(t5_attn_bwd_kernel<DH>, grid, T5_THREADS, smem, st, a, w.dkv_part, w.db_part);
         return 0;
     }));
     GRB_CUDA(cudaGetLastError());
+    if (w.dkv_part) {
+        launch_k(t5_dkdv_sum_kernel, capped_blocks(2 * n / 4), 256, 0, st, (const float*)w.dkv_part, (int)grid.x, n, dk, dv);
+        GRB_CUDA(cudaGetLastError());
+    }
+    if (a.dbias) GRB_TRY(det_finish(w.db_part, H, B * (int)grid.x, a.nb, H, a.nb, 1, {{a.dbias, H * a.nb}}, st));
     return 0;
 }
 

@@ -10,8 +10,11 @@
 // tile with its own online-softmax state; the four states of a row are merged with shuffles.  Rectangular (cross-attention) and
 // non-causal (encoder) shapes are the general case; the relative-position bucket of every delta = j - i is a host-made table.
 // Backward: one pass per query tile recomputes the probabilities from the saved log-sum-exp; dQ stays in registers, the dK / dV
-// contributions of the tile are reduced over its 32 query rows in shared memory and leave as one fp32 atomic per (key, d); the
-// bias-table gradient is accumulated per CTA in shared memory bins.
+// contributions of the tile are reduced over its 32 query rows in shared memory.  With one or two query tiles they leave as one
+// fp32 atomic per (key, d) onto zero, which commutes exactly; with more, each tile stores its partials and t5_dkdv_sum_kernel adds
+// them in tile order.  The bias-table gradient is accumulated per CTA in shared-memory bins in a fixed order (each diagonal
+// delta = j - i of a key tile in row order, then the diagonals of a bucket in delta order) and the CTAs' bins are added by
+// det_finish, so two calls give the same bits.
 #pragma once
 #include "common.cuh"
 #include "tc_gemm.cuh"   // exp_accurate
@@ -147,8 +150,12 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_fwd_kernel(T5AttnArgs a) {
     }
 }
 
+constexpr int T5_DIAGS = T5_ROWS + T5_KEYS - 1;   // diagonals delta = j - i of a 32 x 64 tile
+
+// dkv_part: [2][gridDim.x][B * Lk * H * DH] per-query-tile dK / dV partials when the grid has more than two query tiles, else null
+// (atomics).  db_part: [H][B * gridDim.x][nb] the bias bins of each CTA, non-null iff a.dbias is.
 template <int DH>
-__global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a) {
+__global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a, float* dkv_part, float* db_part) {
     pdl_wait();
     a.drop.resolve();
     extern __shared__ float t5_smem[];
@@ -156,9 +163,11 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a) {
     float* Vs = Ks + T5_KEYS * (DH + 1);
     float* Qs = Vs + T5_KEYS * (DH + 1);                  // [32][DH + 1]
     float* dOs = Qs + T5_ROWS * (DH + 1);                 // [32][DH + 1]
-    float* dSs = dOs + T5_ROWS * (DH + 1);                // [32][64 + 1]  dS * scale (0 where not differentiable)
+    float* dSs = dOs + T5_ROWS * (DH + 1);                // [32][64 + 1]  dS (0 where not differentiable)
     float* Pds = dSs + T5_ROWS * (T5_KEYS + 1);           // [32][64 + 1]  dropped probabilities
-    float* sbias = Pds + T5_ROWS * (T5_KEYS + 1);         // [nb]
+    float* sdiag = Pds + T5_ROWS * (T5_KEYS + 1);         // [95] the tile's diagonal sums of dS
+    int* sbk = reinterpret_cast<int*>(sdiag + T5_DIAGS);  // [95] their buckets (-1: outside the bucket map)
+    float* sbias = sdiag + 2 * T5_DIAGS;                  // [nb]
     float* sdb = sbias + a.nb;                            // [nb] gradient bins of this CTA
     const int tid = threadIdx.x, r = tid >> 2, kq = tid & 3;
     const int b = blockIdx.y / a.H, h = blockIdx.y % a.H;
@@ -204,16 +213,35 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a) {
                 const float ds = p * (dp - Dsum);
                 Pds[r * (T5_KEYS + 1) + jj] = pd;
                 if (diff) {
-                    if (a.dbias) atomicAdd(&sdb[a.bucket[j0 + jj - i + a.Lq - 1]], ds);
+                    dSs[r * (T5_KEYS + 1) + jj] = ds;
                     const float dss = ds * a.scale;
-                    dSs[r * (T5_KEYS + 1) + jj] = dss;
 #pragma unroll
                     for (int d = 0; d < DH; ++d) dq[d] = fmaf(dss, kr[d], dq[d]);
                 }
             }
         }
         __syncthreads();
-        // dK_j += sum_r dS_rj q_r ; dV_j += sum_r Pd_rj dO_r : thread (key jj, half of the head dims), one atomic per (key, d)
+        // bias bins: thread t sums diagonal t (jj - r = t - 31) over the tile's rows in order, then each bin adds its diagonals in order
+        if (a.dbias) {
+            if (tid < T5_DIAGS) {
+                float s = 0.f;
+                for (int rr = 0; rr < T5_ROWS; ++rr) {
+                    const int jj = tid - (T5_ROWS - 1) + rr;
+                    if (jj >= 0 && jj < T5_KEYS) s += dSs[rr * (T5_KEYS + 1) + jj];
+                }
+                sdiag[tid] = s;
+                const int idx = j0 + tid - (T5_ROWS - 1) - i0 + a.Lq - 1;   // delta + Lq - 1
+                sbk[tid] = idx >= 0 && idx < a.Lq + a.Lk - 1 ? a.bucket[idx] : -1;
+            }
+            __syncthreads();
+            for (int e = tid; e < a.nb; e += T5_THREADS) {
+                float acc = sdb[e];
+                for (int t = 0; t < T5_DIAGS; ++t)
+                    if (sbk[t] == e) acc += sdiag[t];
+                sdb[e] = acc;
+            }
+        }
+        // dK_j += sum_r dS_rj scale q_r ; dV_j += sum_r Pd_rj dO_r : thread (key jj, half of the head dims)
         {
             const int jj = tid >> 1, half = tid & 1;
             if (j0 + jj < a.Lk) {
@@ -221,16 +249,26 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a) {
 #pragma unroll
                 for (int d = 0; d < DH / 2; ++d) { gk[d] = 0.f; gv[d] = 0.f; }
                 for (int rr = 0; rr < T5_ROWS; ++rr) {
-                    const float ds = dSs[rr * (T5_KEYS + 1) + jj], pd = Pds[rr * (T5_KEYS + 1) + jj];
+                    const float ds = dSs[rr * (T5_KEYS + 1) + jj] * a.scale, pd = Pds[rr * (T5_KEYS + 1) + jj];
                     const float* qr = Qs + rr * (DH + 1) + half * (DH / 2);
                     const float* gr = dOs + rr * (DH + 1) + half * (DH / 2);
 #pragma unroll
                     for (int d = 0; d < DH / 2; ++d) { gk[d] = fmaf(ds, qr[d], gk[d]); gv[d] = fmaf(pd, gr[d], gv[d]); }
                 }
-                float* dkp = a.dk + ((size_t)b * a.Lk + j0 + jj) * D + h * DH + half * (DH / 2);
-                float* dvp = a.dv + ((size_t)b * a.Lk + j0 + jj) * D + h * DH + half * (DH / 2);
+                const size_t at = ((size_t)b * a.Lk + j0 + jj) * D + h * DH + half * (DH / 2);
+                if (dkv_part) {                           // this query tile's slot of the partials
+                    const size_t n = (size_t)a.B * a.Lk * D;
+                    float4* dkp = reinterpret_cast<float4*>(dkv_part + blockIdx.x * n + at);
+                    float4* dvp = reinterpret_cast<float4*>(dkv_part + (gridDim.x + blockIdx.x) * n + at);
 #pragma unroll
-                for (int d = 0; d < DH / 2; ++d) { atomicAdd(dkp + d, gk[d]); atomicAdd(dvp + d, gv[d]); }
+                    for (int d = 0; d < DH / 8; ++d) {
+                        dkp[d] = make_float4(gk[4 * d], gk[4 * d + 1], gk[4 * d + 2], gk[4 * d + 3]);
+                        dvp[d] = make_float4(gv[4 * d], gv[4 * d + 1], gv[4 * d + 2], gv[4 * d + 3]);
+                    }
+                } else {                                  // at most two adds onto zero per element: exact in either order
+#pragma unroll
+                    for (int d = 0; d < DH / 2; ++d) { atomicAdd(a.dk + at + d, gk[d]); atomicAdd(a.dv + at + d, gv[d]); }
+                }
             }
         }
     }
@@ -247,8 +285,24 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a) {
     }
     if (a.dbias) {
         __syncthreads();
-        for (int e = tid; e < a.nb; e += T5_THREADS)
-            if (sdb[e] != 0.f) atomicAdd(a.dbias + h * a.nb + e, sdb[e]);
+        det_store(db_part, h, b * gridDim.x + blockIdx.x, a.B * gridDim.x, a.nb, a.nb, [&](int e) { return sdb[e]; });
+    }
+}
+
+// dk / dv [n] = the dkv_part partials of t5_attn_bwd_kernel summed over its ntiles query tiles in tile order (n % 4 == 0)
+__global__ void __launch_bounds__(256) t5_dkdv_sum_kernel(const float* part, int ntiles, size_t n, float* dk, float* dv) {
+    pdl_wait();
+    const size_t n4 = n / 4;
+    for (size_t e = (size_t)blockIdx.x * 256 + threadIdx.x; e < 2 * n4; e += (size_t)gridDim.x * 256) {
+        const int w = e >= n4;
+        const size_t c = e - w * n4;
+        const float4* p = reinterpret_cast<const float4*>(part + (size_t)w * ntiles * n) + c;
+        float4 s = p[0];
+        for (int t = 1; t < ntiles; ++t) {
+            const float4 x = p[(size_t)t * n4];
+            s.x += x.x; s.y += x.y; s.z += x.z; s.w += x.w;
+        }
+        reinterpret_cast<float4*>(w ? dv : dk)[c] = s;
     }
 }
 
@@ -256,7 +310,7 @@ template <int DH>
 inline size_t t5_fwd_smem(int nb) { return (size_t)(2 * T5_KEYS * (DH + 1) + nb) * sizeof(float); }
 template <int DH>
 inline size_t t5_bwd_smem(int nb) {
-    return (size_t)(2 * T5_KEYS * (DH + 1) + 2 * T5_ROWS * (DH + 1) + 2 * T5_ROWS * (T5_KEYS + 1) + 2 * nb) * sizeof(float);
+    return (size_t)(2 * T5_KEYS * (DH + 1) + 2 * T5_ROWS * (DH + 1) + 2 * T5_ROWS * (T5_KEYS + 1) + 2 * T5_DIAGS + 2 * nb) * sizeof(float);
 }
 
 }  // namespace grb

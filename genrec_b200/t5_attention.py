@@ -90,11 +90,13 @@ def attention_core_bwd(Q, K, V, H, bias, bucket, key_pad, causal, scale, out, ls
     dv = torch.empty(B, Lk, D, dtype=torch.float32, device=Q.device)
     dbias = torch.zeros_like(bias) if bias is not None else None
     nb = bias.shape[1] if bias is not None else 0
+    lib = _lib.load()
+    ws = torch.empty(lib.grb_t5_attention_backward_workspace_bytes(B, Lq, Lk, H, D // H, nb), dtype=torch.uint8, device=Q.device)
     with torch.cuda.device(Q.device):
-        check(_lib.load().grb_t5_attention_backward(ptr(Q), ptr(K), ptr(V), B, Lq, Lk, H, D // H, Q.stride(1), K.stride(1), V.stride(1), ptr(bias),
-                                                    ptr(bucket), nb, ptr(key_pad), 1 if causal else 0, float(scale), float(p), int(seed), None,
-                                                    int(site) & 0xFFFFFFFF, ptr(out), D, ptr(lse), ptr(dout), D, ptr(dq), D, ptr(dk), ptr(dv),
-                                                    ptr(dbias), stream_ptr(Q.device)))
+        check(lib.grb_t5_attention_backward(ptr(Q), ptr(K), ptr(V), B, Lq, Lk, H, D // H, Q.stride(1), K.stride(1), V.stride(1), ptr(bias),
+                                            ptr(bucket), nb, ptr(key_pad), 1 if causal else 0, float(scale), float(p), int(seed), None,
+                                            int(site) & 0xFFFFFFFF, ptr(out), D, ptr(lse), ptr(dout), D, ptr(dq), D, ptr(dk), ptr(dv),
+                                            ptr(dbias), ptr(ws) if ws.numel() else None, stream_ptr(Q.device)))
     return dq, dk, dv, dbias
 
 

@@ -318,16 +318,19 @@ int grb_layernorm_f32_forward(const float* x, const float* g, const float* b, fl
  * the weights, times v.  q [B, Lq, ldq], k / v [B, Lk, ld] and out are bf16 with head h in columns h*head_dim .. ; bias [H,
  * num_buckets] fp32 with bucket [Lq + Lk - 1] int32 = the bucket of delta = j - i at index delta + Lq - 1 (both NULL for
  * cross-attention); key_pad [B, Lk] 1 = padded (NULL: none); lse [B, H, Lq, 2] = {row max, sum of exp(s - max)} is saved for the backward.
- * Backward: dq bf16 [B, Lq, lddq]; dk, dv fp32 [B, Lk, H * head_dim] (zero-filled here, then accumulated); dbias [H, num_buckets] +=. */
+ * Backward: dq bf16 [B, Lq, lddq]; dk, dv fp32 [B, Lk, H * head_dim] (overwritten); dbias [H, num_buckets] +=.  Every sum runs in a
+ * fixed order, so two calls give the same bits.  workspace: grb_t5_attention_backward_workspace_bytes(B, Lq, Lk, H, head_dim,
+ * num_buckets), 16-byte aligned; num_buckets = 0 without a bias table.  It may be 0 bytes (workspace NULL then allowed). */
 int grb_t5_attention_forward(const void* q, const void* k, const void* v, int B, int Lq, int Lk, int H, int head_dim, int ldq, int ldk, int ldv,
                              const float* bias, const int32_t* bucket, int num_buckets, const uint8_t* key_pad, int causal, float scale,
                              float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t site, void* out, int ldo, float* lse,
                              void* stream);
+size_t grb_t5_attention_backward_workspace_bytes(int B, int Lq, int Lk, int H, int head_dim, int num_buckets);
 int grb_t5_attention_backward(const void* q, const void* k, const void* v, int B, int Lq, int Lk, int H, int head_dim, int ldq, int ldk, int ldv,
                               const float* bias, const int32_t* bucket, int num_buckets, const uint8_t* key_pad, int causal, float scale,
                               float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t site, const void* out, int ldo,
                               const float* lse, const void* dout, int lddo, void* dq, int lddq, float* dk, float* dv, float* dbias,
-                              void* stream);
+                              void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ TIGER constrained beam step
  * The per-step post-processing of Tiger.generate (genrec/models/tiger.py:364-441), host-bound Python loops in the reference.

@@ -61,7 +61,7 @@ def test_model_vs_reference_golden(golden):
         assert frob_relerr(got, ref) < 6e-2 and close(got, ref, 0.3), (n, frob_relerr(got, ref), relerr(got, ref))
 
 
-@pytest.mark.parametrize("B,L,D,H", [(128, 50, 64, 2), (3, 130, 128, 4), (2, 1, 64, 2)])
+@pytest.mark.parametrize("B,L,D,H", [(128, 50, 64, 2), (3, 130, 128, 4), (2, 1, 64, 2), (64, 50, 128, 2)])
 def test_cfg1_shape_vs_oracle(B, L, D, H):
     """BASELINE configs[0] (SASRec 2 blocks, d=64, L=50, 1k items) on the GPU against the CPU oracle."""
     from genrec_b200.sasrec import SASRec
@@ -108,6 +108,40 @@ def test_cfg1_shape_vs_oracle(B, L, D, H):
         gm = math.exp(sum(math.log(max(r[1] / max(r[2], 1e-12), 1e-6)) for r in rows) / len(rows))
         print(f"geometric mean of ours / reference-autocast: {gm:.3f}")
         assert gm <= 1.0, gm
+
+
+@pytest.mark.parametrize("D,H", [(64, 2), (128, 2)])
+def test_attention_module_standalone_vs_oracle(D, H):
+    """MultiHeadAttention on its own (sasrec.py:168-246) against the fp32 oracle, forward and backward, at head_dim 32 and 64, with
+    left padding, a hole and a fully padded sequence."""
+    from genrec_b200.sasrec import MultiHeadAttention
+    from oracle import sasrec as osr
+    dev = torch.device("cuda:0")
+    torch.manual_seed(D + H)
+    attn = MultiHeadAttention(D, H, 0.0)
+    B, L = 4, 70
+    g = torch.Generator().manual_seed(D)
+    q, kv, dy = torch.randn(B, L, D, generator=g), torch.randn(B, L, D, generator=g), torch.randn(B, L, D, generator=g)
+    mask = torch.ones(B, L, 1)
+    mask[0, :20] = 0
+    mask[1, 30:37] = 0
+    mask[2] = 0
+    sd = {"a." + k: v.detach().clone().requires_grad_(True) for k, v in attn.state_dict().items()}
+    qr, kvr = q.clone().requires_grad_(True), kv.clone().requires_grad_(True)
+    ref = osr.sasrec_attention_forward(qr, kvr, mask, sd, "a.", H)
+    ref.backward(dy)
+    attn = attn.to(dev).train()
+    qg, kvg = q.to(dev).requires_grad_(True), kv.to(dev).requires_grad_(True)
+    out = attn(qg, kvg, mask.to(dev))
+    out.backward(dy.to(dev))
+    assert relerr(out, ref) < 1.5e-2, relerr(out, ref)
+    assert relerr(qg.grad, qr.grad) < 2e-2 and relerr(kvg.grad, kvr.grad) < 2e-2, (relerr(qg.grad, qr.grad), relerr(kvg.grad, kvr.grad))
+    for n, p in attn.named_parameters():
+        if n.endswith(ZERO_GRAD):
+            continue
+        assert close(p.grad, sd["a." + n].grad, 2e-2), (n, relerr(p.grad, sd["a." + n].grad))
+    padq = mask.squeeze(-1) == 0
+    assert torch.equal(out.detach().cpu()[padq], q[padq])
 
 
 def test_block_backward_is_reproducible():
