@@ -900,7 +900,7 @@ int grb_embed_backward(const int64_t* ids, const int64_t* order, const float* dx
     launch_k(embed_bwd_run_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), pa);
     GRB_CUDA(cudaGetLastError());
     if (dpos_table) {
-        launch_k(embed_bwd_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
+        launch_k(embed_bwd_pos_kernel, L < 8 * sm_count() ? L : 8 * sm_count(), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
         GRB_CUDA(cudaGetLastError());
     }
     return 0;

@@ -558,28 +558,61 @@ __global__ void __launch_bounds__(ROW_THREADS) embed_fwd_kernel(EmbedArgs a) {
         }
     }
 }
-// dpos[t % L,:] += dropmask(dx[t,:])   (the table rows: embed_bwd_piece_kernel + embed_bwd_run_kernel)
 struct EmbedBwdArgs {
     const long long* ids; const float* dx; float* dE; float* dpos;
     int T, L, D; float scale; int mask_pad_rows;
     Dropout drop;
     const long long* order;   // token indices sorted by id (stable)
 };
-__global__ void __launch_bounds__(ROW_THREADS) embed_bwd_kernel(EmbedBwdArgs a) {
+// dpos[l,:] += sum over b = 0 .. B-1, in ascending b, of dropmask(dx[b L + l,:]) in fp32 (with mask_pad_rows, the tokens with id 0
+// are left out), then one add of that sum per element: one CTA owns position row l and thread q its float4 column q, so the
+// result does not depend on timing.  The CTA stages EMB_POS_STAGE float4 of the row's tokens at a time in shared memory (all of
+// a chunk's loads in flight at once, 8 per thread), and the column owners add them in b order.
+constexpr int EMB_POS_STAGE = 8 * ROW_THREADS;
+__global__ void __launch_bounds__(ROW_THREADS) embed_bwd_pos_kernel(EmbedBwdArgs a) {
+    __shared__ float4 stage[EMB_POS_STAGE];
+    __shared__ uint8_t live[EMB_POS_STAGE];
     pdl_wait();
     a.drop.resolve();
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const int nw = gridDim.x * (ROW_THREADS / 32);
-    for (int row = blockIdx.x * (ROW_THREADS / 32) + wib; row < a.T; row += nw) {
-        const long long id = a.ids[row];
-        if (a.mask_pad_rows && id == 0) continue;
-        // four columns per lane and one 16-byte vector reduction per destination (D % 4 == 0, rows 16-byte aligned)
-        for (int c = 4 * lane; c < a.D; c += 128) {
-            float4 v = *reinterpret_cast<const float4*>(a.dx + (size_t)row * a.D + c);
-            a.drop.apply2(v.x, v.y, row, c);
-            a.drop.apply2(v.z, v.w, row, c + 2);
-            red_add_v4(a.dpos + (size_t)(row % a.L) * a.D + c, v.x, v.y, v.z, v.w);
+    const int nq = a.D / 4, B = a.T / a.L, chunk = EMB_POS_STAGE / nq;   // D <= 256: chunk >= 32 tokens
+    const int q = threadIdx.x;
+    for (int l = blockIdx.x; l < a.L; l += gridDim.x) {
+        float4* d = reinterpret_cast<float4*>(a.dpos + (size_t)l * a.D + 4 * q);
+        const float4 o = q < nq ? *d : make_float4(0.f, 0.f, 0.f, 0.f);   // requested before the row's loads, added after its sum
+        float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int b0 = 0; b0 < B; b0 += chunk) {
+            const int nb = min(chunk, B - b0);
+            float4 v[EMB_POS_STAGE / ROW_THREADS];
+            bool pad[EMB_POS_STAGE / ROW_THREADS];
+#pragma unroll
+            for (int i = 0; i < EMB_POS_STAGE / ROW_THREADS; ++i) {
+                const int e = threadIdx.x + i * ROW_THREADS, u = e / nq, c = 4 * (e - u * nq);
+                const size_t row = (size_t)(b0 + u) * a.L + l;
+                if (u < nb) v[i] = *reinterpret_cast<const float4*>(a.dx + row * a.D + c);
+                pad[i] = u < nb && c == 0 && a.mask_pad_rows && a.ids[row] == 0;
+            }
+#pragma unroll
+            for (int i = 0; i < EMB_POS_STAGE / ROW_THREADS; ++i) {
+                const int e = threadIdx.x + i * ROW_THREADS, u = e / nq, c = 4 * (e - u * nq);
+                if (u >= nb) continue;
+                const int row = (b0 + u) * a.L + l;
+                a.drop.apply2(v[i].x, v[i].y, row, c);
+                a.drop.apply2(v[i].z, v[i].w, row, c + 2);
+                stage[e] = v[i];
+                if (c == 0) live[u] = !pad[i];
+            }
+            __syncthreads();
+            if (q < nq) {
+#pragma unroll 8
+                for (int u = 0; u < nb; ++u) {
+                    if (!live[u]) continue;
+                    const float4 t = stage[u * nq + q];
+                    s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
+                }
+            }
+            __syncthreads();
         }
+        if (q < nq) *d = make_float4(o.x + s.x, o.y + s.y, o.z + s.z, o.w + s.w);
     }
 }
 
