@@ -92,6 +92,7 @@ SIGNATURES = {
     "grb_embed_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int, c_float,
                                    c_u64, c_void_p, c_void_p, c_void_p]),
     "grb_head_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "grb_head_splits": (c_int, [c_int, c_int, c_int, c_int]),
     "grb_head_loss_forward_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_int, c_int, c_int,
                                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_head_logits": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,

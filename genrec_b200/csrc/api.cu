@@ -914,6 +914,9 @@ struct HeadWork {
     float* row_loss;                                               // per-token loss, summed in a fixed order
     float* shift;                                                  // fused schedule: per-token log2-domain softmax shift
     float *part_ln, *part_tn;                                      // scratch of the ordered cross-CTA sums (LayerNorm, stored-schedule dE)
+    int *ce_rsched, *ce_tsched;                                    // fused schedule: unit counters and finished segments per tile
+    float *ce_rcarry, *ce_tcarry;                                  // fused schedule: running sums handed from segment to segment
+    int rseg, tseg;                                                // fused schedule: segments of a row tile's / a class tile's sweep
     int ldl;
     size_t bytes;
 };
@@ -921,13 +924,15 @@ bool head_fused(int D) { return D <= 128; }
 HeadWork carve_head(void* base, size_t T, size_t D, size_t C) {
     HeadWork h;
     Carver c{static_cast<char*>(base)};
+    // D <= 128: the fused kernels (tc_ce.cuh) never form the [T, C] logits; D = 256 stores them
+    const bool fused = head_fused((int)D);
+    h.rseg = fused ? ce_row_segments((int)T, (int)C, sm_count()) : 1;
+    h.tseg = fused ? ce_table_segments((int)T, (int)C, sm_count()) : 1;
     h.ldl = (int)((C + 7) / 8 * 8);
     h.xf = c.take<bf16>(T * D * 2);
     h.stf = c.take<float>(T * 2 * 4);
     h.dxf = c.take<float>(T * D * 4);
     h.scal = c.take<float>(64);
-    // D <= 128: the fused kernels (tc_ce.cuh) never form the [T, C] logits; D = 256 stores them
-    const bool fused = head_fused((int)D);
     h.logits = fused ? nullptr : c.take<bf16>(T * (size_t)h.ldl * 2);
     h.logits32 = fused ? nullptr : c.take<float>(T * (size_t)h.ldl * 4);
     h.row_loss = c.take<float>(T * 4);
@@ -935,12 +940,20 @@ HeadWork carve_head(void* base, size_t T, size_t D, size_t C) {
     h.part_ln = c.take<float>((size_t)2 * row_bwd_grid((int)T) * D * 4);
     const TnSpec spec{nullptr, nullptr, nullptr, (int)C, (int)D, (int)T, h.ldl, (int)D, (int)D};
     h.part_tn = fused ? nullptr : c.take<float>(tn_part_floats(&spec, 1, sm_count()) * 4);
+    h.ce_rsched = fused ? c.take<int>((1 + 2 * ((T + 127) / 128)) * 4) : nullptr;
+    h.ce_tsched = fused ? c.take<int>((1 + (C + 63) / 64) * 4) : nullptr;
+    h.ce_rcarry = fused && h.rseg > 1 ? c.take<float>(3 * T * 4 * 4) : nullptr;
+    h.ce_tcarry = fused && h.tseg > 1 ? c.take<float>((C + 63) / 64 * 128 * D * 4) : nullptr;
     h.bytes = c.off;
     return h;
 }
 }  // namespace
 
 size_t grb_head_workspace_bytes(int T, int D, int C) { return carve_head(nullptr, T, D, C).bytes; }
+int grb_head_splits(int T, int D, int C, int table) {
+    const HeadWork h = carve_head(nullptr, T, D, C);
+    return table ? h.tseg : h.rseg;
+}
 
 int grb_head_loss_forward_backward(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16,
                                    const int64_t* targets, int T, int D, int C, float* loss, float* dx, float* dtable, float* dln_g,
@@ -969,15 +982,16 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
     if (head_fused(D)) {
         // loss, dxf and the per-token shifts in one row-stationary pass; dE in a class-stationary pass (a weight gradient: off the
         // critical path with the deferred schedule)                                                      (hstu.py:137-146)
-        CeArgs ca{reinterpret_cast<const long long*>(targets), h.scal, T, C, want_grad ? h.dxf : nullptr, h.shift, h.row_loss, dtable};
-        if (D == 64) GRB_CUDA(launch_tc_ce<64>(h.xf, (const bf16*)table_bf16, ca, st));
-        else GRB_CUDA(launch_tc_ce<128>(h.xf, (const bf16*)table_bf16, ca, st));
+        CeArgs ca{reinterpret_cast<const long long*>(targets), h.scal, T, C, want_grad ? h.dxf : nullptr, h.shift, h.row_loss, dtable,
+                  h.rseg, h.tseg, h.ce_rsched, h.ce_tsched, h.ce_rcarry, h.ce_tcarry};
+        if (D == 64) GRB_CUDA(launch_tc_ce<64>(h.xf, (const bf16*)table_bf16, ca, sm_count(), st));
+        else GRB_CUDA(launch_tc_ce<128>(h.xf, (const bf16*)table_bf16, ca, sm_count(), st));
         launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
         GRB_CUDA(cudaGetLastError());
         if (!want_grad) return 0;
         GRB_TRY(run_maybe_deferred(st, [&](cudaStream_t s_) -> int {
-            if (D == 64) GRB_CUDA(launch_ce_table<64>(h.xf, (const bf16*)table_bf16, ca, s_));
-            else GRB_CUDA(launch_ce_table<128>(h.xf, (const bf16*)table_bf16, ca, s_));
+            if (D == 64) GRB_CUDA(launch_ce_table<64>(h.xf, (const bf16*)table_bf16, ca, sm_count(), s_));
+            else GRB_CUDA(launch_ce_table<128>(h.xf, (const bf16*)table_bf16, ca, sm_count(), s_));
             return 0;
         }));
     } else {

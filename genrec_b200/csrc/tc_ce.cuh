@@ -1,15 +1,21 @@
 // genrec_b200 - fused tied-embedding logits + cross-entropy on wgmma: loss, d(loss)/d(x) and d(loss)/d(table) without ever
 // writing a [tokens, classes] tensor.  D = 64 or 128 (the table rows fit one shared-memory tile).
 //
-//   ce_rows_kernel   (row-stationary, one CTA per 128 token rows): the token tile X [128 x D] stays in shared memory while the
+//   ce_rows_kernel   (row-stationary, 128 token rows per unit): the token tile X [128 x D] stays in shared memory while the
 //                    table streams through a TMA ring in 64-class tiles.  Sweep 1: S = X E^T (wgmma, register accumulators),
 //                    online row maximum / exponent sum and the target logit -> per-row loss and the row's log2-domain shift.
 //                    Sweep 2: S again, G = (softmax - onehot) / count in registers, converted in place to the bf16 A operand of
-//                    dX += G E (wgmma with A from registers, the same table tile read MN-major) -> dX [T, D] fp32, written once.
-//   ce_table_kernel  (class-stationary, one CTA per 64 classes): the table tile stays resident while the token tiles stream;
+//                    dX += G E (wgmma with A from registers, the same table tile read MN-major) -> dX [T, D] fp32.
+//   ce_table_kernel  (class-stationary, 64 classes per unit): the table tile stays resident while the token tiles stream;
 //                    S^T = E X^T, G^T from the saved row shifts, dE += G^T X, the two consumer warpgroups take alternate token
 //                    tiles and their sums are added in a fixed order -> dE [C, D] += once per element.
-// Every sum runs in a fixed order, so the results do not depend on timing.
+// Load balance without reordering a sum: each sweep is cut into segments (contiguous class tiles of a row tile, token tiles of a
+// class tile), and a segment continues from the running sums (row maximum, exponent sums, target logit, the dX or dE
+// accumulators) the segment before it left in global memory, so every row and class sees the same operations in the same order
+// as one uninterrupted sweep, and the results are the same bits whatever the segment count.  Both kernels are persistent: one CTA
+// per SM takes (segment, tile) units from a counter, segment-major, and waits only for the previous segment of its chain.  At
+// 128 x 200 tokens and 12,102 classes on 132 SMs, 200 row tiles x 2 sweeps on whole-sweep units need 4 rounds where 3.03 would
+// do, 190 class tiles 2 where 1.44 would do; ce_segments picks the counts from the shapes and the SM count only.
 #pragma once
 #include "tc_gemm.cuh"
 
@@ -61,16 +67,39 @@ GRB_DEVINL void wgmma_rs_d(float (&d)[D / 2], const uint32_t (&a)[4], uint64_t b
 constexpr int CE_THREADS = 384;           // producer warpgroup + 2 consumer warpgroups
 constexpr int CE_STAGES = 4;
 constexpr float CE_L2E = 1.4426950408889634f;
+constexpr int CE_MAX_SEGMENTS = 8;
 
 struct CeArgs {
     const long long* tg;        // [T] targets (0 = ignored)
     const float* inv_count;     // device scalar: 1 / #(targets != 0)
     int T, C;
-    float* dx;                  // [T, D] fp32 out (nullable: loss only)
+    float* dx;                  // [T, D] fp32 out (nullable: loss only); between the segments of a row tile it holds the running sum
     float* shift;               // [T] out of ce_rows_kernel, in of ce_table_kernel: log2(sum_c 2^(S_c log2e)) (the log2-domain lse)
     float* row_loss;            // [T] out
     float* dtable;              // [C, D] += (ce_table_kernel)
+    int rseg, tseg;             // segments of a row tile's class sweep, of a class tile's token sweep
+    int* rsched;                // [1 + 2 * row tiles]: unit counter, then statistics / dX segments finished per row tile
+    int* tsched;                // [1 + class tiles]: unit counter, then segments finished per class tile (both zeroed per launch)
+    float* rcarry;              // [3][T][4] running row maximum, exponent sum and target logit of each lane (rseg > 1)
+    float* tcarry;              // [class tiles][2][D / 2][128] running dE sums of the two consumer warpgroups (tseg > 1)
 };
+
+// The smallest segment count s <= min(CE_MAX_SEGMENTS, span) for which items * s units, one CTA per SM on `sms` SMs, leave at most
+// 1/16 of their rounds' slots idle; when none does, the count with the fullest rounds (the smallest on a tie).
+inline int ce_segments(int items, int span, int sms) {
+    const int cap = span < CE_MAX_SEGMENTS ? span : CE_MAX_SEGMENTS;
+    int best = 1;
+    long long best_n = 0, best_slots = 1;
+    for (int s = 1; s <= cap; ++s) {
+        const long long n = (long long)items * s, slots = (n + sms - 1) / sms * sms;
+        if (16 * n >= 15 * slots) return s;
+        if (n * best_slots > best_n * slots) { best = s; best_n = n; best_slots = slots; }
+    }
+    return best;
+}
+// the row pass sweeps every row tile twice (statistics, then dX); the table pass sweeps every class tile once
+inline int ce_row_segments(int T, int C, int sms) { return ce_segments(2 * ((T + 127) / 128), (C + 63) / 64, sms); }
+inline int ce_table_segments(int T, int C, int sms) { return ce_segments((C + 63) / 64, (T + 63) / 64, sms); }
 
 template <int D>
 struct CeSmem {
@@ -80,6 +109,25 @@ struct CeSmem {
     static constexpr int ROWS_BYTES = ROW_TILE + CE_STAGES * CLS_TILE + 1024 + 256;
     static constexpr int TABLE_BYTES = CLS_TILE + CE_STAGES * CLS_TILE + 1024 + 256;
 };
+
+// Both kernels are persistent: every CTA takes units from a counter, so a unit only ever waits for units taken before it, whose
+// CTAs are running.  Barrier 1: the producer warp and both consumer warpgroups between units; barrier 2: the consumers.
+GRB_DEVINL void ce_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// the consumers wait until `need` segments of their chain have finished
+GRB_DEVINL void ce_wait_chain(const int* flag, int need) {
+    if (threadIdx.x == 128) {
+        int v;
+        do asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
+        while (v < need);
+    }
+    ce_bar(2, 256);
+}
+// the consumers' stores of this segment are visible: count it finished
+GRB_DEVINL void ce_finish_segment(int* flag) {
+    __threadfence();
+    ce_bar(2, 256);
+    if (threadIdx.x == 128) atomicAdd(flag, 1);
+}
 
 // S[64 x 64] = A (64 rows of a K-major tile, D wide) * B^T (64 rows of a K-major tile); box b of A at a_addr + b * a_box
 template <int D>
@@ -110,11 +158,14 @@ GRB_DEVINL void ce_accumulate(float (&acc)[D / 2], const float (&G)[32], uint32_
     wgmma_wait<0>();
 }
 
+// Unit u: sweep u / (rseg R) (0: statistics, 1: dX), segment k = u / R % rseg, row tile u % R: the class tiles
+// [k ntile / rseg, (k + 1) ntile / rseg) of that row tile, continuing from the running sums segment k - 1 left in global memory.
 template <int D>
 __global__ void __launch_bounds__(CE_THREADS, 1)
     ce_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmE, CeArgs a) {
     using SM = CeSmem<D>;
     extern __shared__ unsigned char ce_smem_raw[];
+    __shared__ int unit_slot[2];
     unsigned char* base = ce_smem_raw + ((1024u - (smem_u32(ce_smem_raw) & 1023u)) & 1023u);
     unsigned char* sX = base;
     unsigned char* sE = base + SM::ROW_TILE;
@@ -123,7 +174,6 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     uint64_t* empty = bars + CE_STAGES;
     uint64_t* xfull = bars + 2 * CE_STAGES;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int row0 = blockIdx.x * 128;
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmX);
         tma_prefetch_desc(&tmE);
@@ -133,124 +183,173 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     }
     __syncthreads();
     pdl_wait();
-    const int ntile = (a.C + 63) / 64;
-    const int sweeps = a.dx ? 2 : 1;
-
-    if (warp < 4) {
-        if (warp == 0 && lane == 0) {
-            mbar_expect_tx(xfull, SM::ROW_TILE);
-            for (int b = 0; b < SM::XB; ++b) tma_load_2d(sX + b * 16384, &tmX, b * 64, row0, xfull);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int sw = 0; sw < sweeps; ++sw)
-                for (int j = 0; j < ntile; ++j) {
+    if (warp >= 1 && warp < 4) return;            // warp 0 produces (lane 0 issues the loads), warps 4..11 consume
+    const int ntile = (a.C + 63) / 64, R = (a.T + 127) / 128, K = a.rseg;
+    const int units = (a.dx ? 2 : 1) * K * R;
+    // consumer warpgroup g: tile rows 64 g .. 64 g + 63 ; this thread: rows r[0], r[1] = r[0] + 8, columns 8 j + 2 q + {0, 1}
+    const int g = (warp >> 2) - 1, w = warp & 3, q = lane & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    int stage = 0;                                 // the table ring runs on across units
+    uint32_t phase = 0;
+    for (int n = 0;; ++n) {
+        if (threadIdx.x == 0) unit_slot[n & 1] = atomicAdd(a.rsched, 1);
+        ce_bar(1, 288);
+        const int u = unit_slot[n & 1];
+        if (u >= units) break;
+        const bool dxp = u >= K * R;
+        const int k = u / R % K, rt = u % R, row0 = rt * 128;
+        const int j0 = k * ntile / K, j1 = (k + 1) * ntile / K;
+        int* sdone = a.rsched + 1 + rt;            // statistics segments finished for this row tile
+        int* xdone = a.rsched + 1 + R + rt;        // dX segments finished
+        if (warp == 0) {
+            if (lane == 0) {
+                mbar_expect_tx(xfull, SM::ROW_TILE);
+                for (int b = 0; b < SM::XB; ++b) tma_load_2d(sX + b * 16384, &tmX, b * 64, row0, xfull);
+                for (int j = j0; j < j1; ++j) {
                     mbar_wait(&empty[stage], phase ^ 1);
                     mbar_expect_tx(&full[stage], SM::CLS_TILE);
                     for (int b = 0; b < SM::XB; ++b) tma_load_2d(sE + stage * SM::CLS_TILE + b * 8192, &tmE, b * 64, j * 64, &full[stage]);
                     if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
                 }
+            }
+            __syncwarp();
+            continue;
         }
-        return;
-    }
-    // consumer warpgroup g: tile rows 64 g .. 64 g + 63 ; this thread: rows r[0], r[1] = r[0] + 8, columns 8 j + 2 q + {0, 1}
-    const int g = (warp >> 2) - 1, w = warp & 3, q = lane & 3;
-    const bool leader = (threadIdx.x & 127) == 0;
-    int row[2], tgt[2];
-    float ic[2];
-    const float inv = *a.inv_count;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        row[i] = row0 + 64 * g + 16 * w + (lane >> 2) + 8 * i;
-        tgt[i] = row[i] < a.T ? (int)a.tg[row[i]] : 0;
-        ic[i] = tgt[i] != 0 ? inv : 0.f;
-    }
-    mbar_wait(xfull, 0);
-    const uint32_t xa = smem_u32(sX) + g * 8192;
-    int stage = 0;
-    uint32_t phase = 0;
-    float m[2] = {-INFINITY, -INFINITY}, s[2] = {0.f, 0.f}, tl[2] = {0.f, 0.f};
-    for (int j = 0; j < ntile; ++j) {
-        mbar_wait(&full[stage], phase);
-        float S[32];
-        ce_scores<D>(S, xa, 16384, smem_u32(sE + stage * SM::CLS_TILE));
-        if (leader) mbar_arrive(&empty[stage]);
-        if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
+        int row[2], tgt[2];
+        float ic[2];
+        const float inv = *a.inv_count;
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-            float mx = -INFINITY;
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    const int col = j * 64 + 8 * jj + 2 * q + c;
-                    float& v = S[jj * 4 + i * 2 + c];
-                    if (col >= a.C) v = -INFINITY;
-                    if (col == tgt[i]) tl[i] = v;
-                    mx = fmaxf(mx, v);
-                }
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-            const float mn = fmaxf(m[i], mx);
-            float acc = s[i] * ex2_fast((m[i] - mn) * CE_L2E);
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-                for (int c = 0; c < 2; ++c) acc += ex2_fast((S[jj * 4 + i * 2 + c] - mn) * CE_L2E);
-            s[i] = acc;
-            m[i] = mn;
+            row[i] = row0 + 64 * g + 16 * w + (lane >> 2) + 8 * i;
+            tgt[i] = row[i] < a.T ? (int)a.tg[row[i]] : 0;
+            ic[i] = tgt[i] != 0 ? inv : 0.f;
         }
-    }
-    float shift[2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        s[i] += __shfl_xor_sync(0xffffffffu, s[i], 1);
-        s[i] += __shfl_xor_sync(0xffffffffu, s[i], 2);
-        tl[i] += __shfl_xor_sync(0xffffffffu, tl[i], 1);
-        tl[i] += __shfl_xor_sync(0xffffffffu, tl[i], 2);
-        shift[i] = m[i] * CE_L2E + __log2f(s[i]);
-        if (q == 0 && row[i] < a.T) {
-            a.row_loss[row[i]] = tgt[i] != 0 ? (m[i] + __logf(s[i]) - tl[i]) * ic[i] : 0.f;
-            a.shift[row[i]] = shift[i];
-        }
-    }
-    if (!a.dx) return;
-    float dx[D / 2];
-#pragma unroll
-    for (int k = 0; k < D / 2; ++k) dx[k] = 0.f;
-    for (int j = 0; j < ntile; ++j) {
-        mbar_wait(&full[stage], phase);
-        float S[32];
-        const uint32_t e_addr = smem_u32(sE + stage * SM::CLS_TILE);
-        ce_scores<D>(S, xa, 16384, e_addr);
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
+        mbar_wait(xfull, n & 1);
+        const uint32_t xa = smem_u32(sX) + g * 8192;
+        if (!dxp) {
+            if (k > 0) ce_wait_chain(sdone, k);
+            float m[2] = {-INFINITY, -INFINITY}, s[2] = {0.f, 0.f}, tl[2] = {0.f, 0.f};
+            const size_t plane = (size_t)a.T * 4;
 #pragma unroll
             for (int i = 0; i < 2; ++i)
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    const int col = j * 64 + 8 * jj + 2 * q + c;
-                    float& v = S[jj * 4 + i * 2 + c];
-                    float gv = col < a.C ? ex2_fast(v * CE_L2E - shift[i]) * ic[i] : 0.f;
-                    if (col == tgt[i]) gv -= ic[i];
-                    v = gv;
+                if (k > 0 && row[i] < a.T) {
+                    const size_t at = (size_t)row[i] * 4 + q;
+                    m[i] = __ldcg(a.rcarry + at);
+                    s[i] = __ldcg(a.rcarry + plane + at);
+                    tl[i] = __ldcg(a.rcarry + 2 * plane + at);
                 }
-        ce_accumulate<D>(dx, S, e_addr);
-        if (leader) mbar_arrive(&empty[stage]);
-        if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
+            for (int j = j0; j < j1; ++j) {
+                mbar_wait(&full[stage], phase);
+                float S[32];
+                ce_scores<D>(S, xa, 16384, smem_u32(sE + stage * SM::CLS_TILE));
+                if (leader) mbar_arrive(&empty[stage]);
+                if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    float mx = -INFINITY;
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                        for (int c = 0; c < 2; ++c) {
+                            const int col = j * 64 + 8 * jj + 2 * q + c;
+                            float& v = S[jj * 4 + i * 2 + c];
+                            if (col >= a.C) v = -INFINITY;
+                            if (col == tgt[i]) tl[i] = v;
+                            mx = fmaxf(mx, v);
+                        }
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                    const float mn = fmaxf(m[i], mx);
+                    float acc = s[i] * ex2_fast((m[i] - mn) * CE_L2E);
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                        for (int c = 0; c < 2; ++c) acc += ex2_fast((S[jj * 4 + i * 2 + c] - mn) * CE_L2E);
+                    s[i] = acc;
+                    m[i] = mn;
+                }
+            }
+            if (k + 1 < K) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+                    if (row[i] < a.T) {
+                        const size_t at = (size_t)row[i] * 4 + q;
+                        a.rcarry[at] = m[i];
+                        a.rcarry[plane + at] = s[i];
+                        a.rcarry[2 * plane + at] = tl[i];
+                    }
+            } else {
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    s[i] += __shfl_xor_sync(0xffffffffu, s[i], 1);
+                    s[i] += __shfl_xor_sync(0xffffffffu, s[i], 2);
+                    tl[i] += __shfl_xor_sync(0xffffffffu, tl[i], 1);
+                    tl[i] += __shfl_xor_sync(0xffffffffu, tl[i], 2);
+                    const float shift = m[i] * CE_L2E + __log2f(s[i]);
+                    if (q == 0 && row[i] < a.T) {
+                        a.row_loss[row[i]] = tgt[i] != 0 ? (m[i] + __logf(s[i]) - tl[i]) * ic[i] : 0.f;
+                        a.shift[row[i]] = shift;
+                    }
+                }
+            }
+            ce_finish_segment(sdone);
+        } else {
+            // rows past T: zero X rows and zero weights, so their G is 0 whatever the shift
+            if (k > 0) ce_wait_chain(xdone, k);
+            else ce_wait_chain(sdone, K);
+            float shift[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) shift[i] = row[i] < a.T ? __ldcg(a.shift + row[i]) : 0.f;
+            float dx[D / 2];
+#pragma unroll
+            for (int jj = 0; jj < D / 8; ++jj)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    float2 v = make_float2(0.f, 0.f);
+                    if (k > 0 && row[i] < a.T) v = __ldcg(reinterpret_cast<const float2*>(a.dx + (size_t)row[i] * D + 8 * jj + 2 * q));
+                    dx[jj * 4 + i * 2] = v.x;
+                    dx[jj * 4 + i * 2 + 1] = v.y;
+                }
+            for (int j = j0; j < j1; ++j) {
+                mbar_wait(&full[stage], phase);
+                float S[32];
+                const uint32_t e_addr = smem_u32(sE + stage * SM::CLS_TILE);
+                ce_scores<D>(S, xa, 16384, e_addr);
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+#pragma unroll
+                        for (int c = 0; c < 2; ++c) {
+                            const int col = j * 64 + 8 * jj + 2 * q + c;
+                            float& v = S[jj * 4 + i * 2 + c];
+                            float gv = col < a.C ? ex2_fast(v * CE_L2E - shift[i]) * ic[i] : 0.f;
+                            if (col == tgt[i]) gv -= ic[i];
+                            v = gv;
+                        }
+                ce_accumulate<D>(dx, S, e_addr);
+                if (leader) mbar_arrive(&empty[stage]);
+                if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
+            }
+#pragma unroll
+            for (int jj = 0; jj < D / 8; ++jj)
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+                    if (row[i] < a.T)
+                        *reinterpret_cast<float2*>(a.dx + (size_t)row[i] * D + 8 * jj + 2 * q) = make_float2(dx[jj * 4 + i * 2], dx[jj * 4 + i * 2 + 1]);
+            ce_finish_segment(xdone);
+        }
     }
-#pragma unroll
-    for (int jj = 0; jj < D / 8; ++jj)
-#pragma unroll
-        for (int i = 0; i < 2; ++i)
-            if (row[i] < a.T)
-                *reinterpret_cast<float2*>(a.dx + (size_t)row[i] * D + 8 * jj + 2 * q) = make_float2(dx[jj * 4 + i * 2], dx[jj * 4 + i * 2 + 1]);
 }
 
+// Unit u: segment k = u / NC of class tile u % NC: the token tiles [k ntt / tseg, (k + 1) ntt / tseg), continuing from the sums
+// segment k - 1 left.  Consumer warpgroup g takes the token tiles tt = g (mod 2) of every segment.
 template <int D>
 __global__ void __launch_bounds__(CE_THREADS, 1)
     ce_table_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmE, CeArgs a) {
     using SM = CeSmem<D>;
     extern __shared__ unsigned char ce_smem_raw[];
+    __shared__ int unit_slot[2];
     unsigned char* base = ce_smem_raw + ((1024u - (smem_u32(ce_smem_raw) & 1023u)) & 1023u);
     unsigned char* sE = base;
     unsigned char* sX = base + SM::CLS_TILE;
@@ -259,7 +358,6 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     uint64_t* empty = bars + CE_STAGES;
     uint64_t* efull = bars + 2 * CE_STAGES;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int cls0 = blockIdx.x * 64;
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmX);
         tma_prefetch_desc(&tmE);
@@ -269,33 +367,50 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     }
     __syncthreads();
     pdl_wait();
-    const int ntt = (a.T + 63) / 64;
+    if (warp >= 1 && warp < 4) return;
+    const int ntt = (a.T + 63) / 64, NC = (a.C + 63) / 64, K = a.tseg;
     const int g = (warp >> 2) - 1, w = warp & 3, q = lane & 3;
-    float acc[D / 2];
-    if (warp < 4) {
-        if (warp == 0 && lane == 0) {
-            mbar_expect_tx(efull, SM::CLS_TILE);
-            for (int b = 0; b < SM::XB; ++b) tma_load_2d(sE + b * 8192, &tmE, b * 64, cls0, efull);
-            // token tile tt -> stage tt % CE_STAGES; consumer warpgroup tt % 2 owns it (CE_STAGES is even)
-            for (int tt = 0; tt < ntt; ++tt) {
-                const int stage = tt % CE_STAGES;
-                mbar_wait(&empty[stage], ((tt / CE_STAGES) & 1) ^ 1);
-                mbar_expect_tx(&full[stage], SM::CLS_TILE);
-                for (int b = 0; b < SM::XB; ++b) tma_load_2d(sX + stage * SM::CLS_TILE + b * 8192, &tmX, b * 64, tt * 64, &full[stage]);
+    const bool leader = (threadIdx.x & 127) == 0;
+    uint32_t pos = 0;                              // token tiles this CTA has streamed: the ring position of the unit's first tile
+    for (int n = 0;; ++n) {
+        if (threadIdx.x == 0) unit_slot[n & 1] = atomicAdd(a.tsched, 1);
+        ce_bar(1, 288);
+        const int u = unit_slot[n & 1];
+        if (u >= K * NC) break;
+        const int k = u / NC, ct = u % NC, cls0 = ct * 64;
+        const int t0 = k * ntt / K, t1 = (k + 1) * ntt / K;
+        int* done = a.tsched + 1 + ct;
+        if (warp == 0) {
+            if (lane == 0) {
+                mbar_expect_tx(efull, SM::CLS_TILE);
+                for (int b = 0; b < SM::XB; ++b) tma_load_2d(sE + b * 8192, &tmE, b * 64, cls0, efull);
+                // ring position p -> stage p % CE_STAGES
+                for (int tt = t0; tt < t1; ++tt) {
+                    const uint32_t p = pos + (tt - t0);
+                    const int stage = p % CE_STAGES;
+                    mbar_wait(&empty[stage], ((p / CE_STAGES) & 1) ^ 1);
+                    mbar_expect_tx(&full[stage], SM::CLS_TILE);
+                    for (int b = 0; b < SM::XB; ++b) tma_load_2d(sX + stage * SM::CLS_TILE + b * 8192, &tmX, b * 64, tt * 64, &full[stage]);
+                }
             }
+            __syncwarp();
+            pos += t1 - t0;
+            continue;
         }
-    } else {
-        const bool leader = (threadIdx.x & 127) == 0;
         int cls[2];
 #pragma unroll
         for (int i = 0; i < 2; ++i) cls[i] = cls0 + 16 * w + (lane >> 2) + 8 * i;
         const float inv = *a.inv_count;
+        float acc[D / 2];
+        float* carry = a.tcarry + ((size_t)ct * 2 + g) * (D / 2) * 128 + (threadIdx.x & 127);
+        if (k > 0) ce_wait_chain(done, k);
 #pragma unroll
-        for (int k = 0; k < D / 2; ++k) acc[k] = 0.f;
-        mbar_wait(efull, 0);
-        const uint32_t ea = smem_u32(sE) + 0;
-        for (int tt = g; tt < ntt; tt += 2) {
-            const int stage = tt % CE_STAGES;
+        for (int kk = 0; kk < D / 2; ++kk) acc[kk] = k > 0 ? __ldcg(carry + (size_t)kk * 128) : 0.f;
+        mbar_wait(efull, n & 1);
+        const uint32_t ea = smem_u32(sE);
+        for (int tt = t0 + ((t0 ^ g) & 1); tt < t1; tt += 2) {
+            const uint32_t p = pos + (tt - t0);
+            const int stage = p % CE_STAGES;
             // this thread's 16 token columns: shift, target, 1 / count
             float sh[16], icc[16];
             int tg[16];
@@ -309,10 +424,10 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
                     sh[jj * 2 + c] = ok ? a.shift[t] : 0.f;
                     icc[jj * 2 + c] = tg[jj * 2 + c] != 0 ? inv : 0.f;
                 }
-            mbar_wait(&full[stage], (tt / CE_STAGES) & 1);
+            mbar_wait(&full[stage], (p / CE_STAGES) & 1);
             const uint32_t x_addr = smem_u32(sX + stage * SM::CLS_TILE);
             float S[32];
-            ce_scores<D>(S, ea + 0, 8192, x_addr);   // S^T: rows = this warpgroup's... all 64 classes, columns = 64 tokens
+            ce_scores<D>(S, ea, 8192, x_addr);     // S^T: rows = the 64 classes, columns = 64 tokens
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
@@ -320,38 +435,45 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
 #pragma unroll
                     for (int c = 0; c < 2; ++c) {
                         float& v = S[jj * 4 + i * 2 + c];
-                        const int k = jj * 2 + c;
-                        float gv = ex2_fast(v * CE_L2E - sh[k]) * icc[k];
-                        if (cls[i] == tg[k]) gv -= icc[k];
+                        const int kq = jj * 2 + c;
+                        float gv = ex2_fast(v * CE_L2E - sh[kq]) * icc[kq];
+                        if (cls[i] == tg[kq]) gv -= icc[kq];
                         v = gv;
                     }
             ce_accumulate<D>(acc, S, x_addr);
             if (leader) mbar_arrive(&empty[stage]);
         }
-    }
-    // warpgroup 2 hands its sum to warpgroup 1 through shared memory (the X ring is free by now); fixed order: wg1 + wg2
-    float* red = reinterpret_cast<float*>(sX);
-    asm volatile("bar.sync 1, 384;" ::: "memory");
-    if (g == 1) {
+        pos += t1 - t0;
+        if (k + 1 < K) {
 #pragma unroll
-        for (int k = 0; k < D / 2; ++k) red[(size_t)k * 128 + (threadIdx.x & 127)] = acc[k];
-    }
-    asm volatile("bar.sync 1, 384;" ::: "memory");
-    if (g == 0) {
+            for (int kk = 0; kk < D / 2; ++kk) carry[(size_t)kk * 128] = acc[kk];
+            ce_finish_segment(done);
+            continue;
+        }
+        // warpgroup 2 hands its sum to warpgroup 1 through shared memory (the X ring is free by now); fixed order: wg1 + wg2
+        float* red = reinterpret_cast<float*>(sX);
+        ce_bar(2, 256);                            // both warpgroups are done with the ring
+        if (g == 1) {
 #pragma unroll
-        for (int jj = 0; jj < D / 8; ++jj)
+            for (int kk = 0; kk < D / 2; ++kk) red[(size_t)kk * 128 + (threadIdx.x & 127)] = acc[kk];
+        }
+        ce_bar(2, 256);
+        if (g == 0) {
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const int c = cls0 + 16 * w + (lane >> 2) + 8 * i;
-                const int k = jj * 4 + i * 2;
-                const float v0 = acc[k] + red[(size_t)k * 128 + (threadIdx.x & 127)];
-                const float v1 = acc[k + 1] + red[(size_t)(k + 1) * 128 + (threadIdx.x & 127)];
-                if (c < a.C) {
-                    float* dst = a.dtable + (size_t)c * D + 8 * jj + 2 * q;
-                    atomicAdd(dst, v0);          // one add per element and launch
-                    atomicAdd(dst + 1, v1);
+            for (int jj = 0; jj < D / 8; ++jj)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int c = cls0 + 16 * w + (lane >> 2) + 8 * i;
+                    const int kk = jj * 4 + i * 2;
+                    const float v0 = acc[kk] + red[(size_t)kk * 128 + (threadIdx.x & 127)];
+                    const float v1 = acc[kk + 1] + red[(size_t)(kk + 1) * 128 + (threadIdx.x & 127)];
+                    if (c < a.C) {
+                        float* dst = a.dtable + (size_t)c * D + 8 * jj + 2 * q;
+                        atomicAdd(dst, v0);          // one add per element and launch
+                        atomicAdd(dst + 1, v1);
+                    }
                 }
-            }
+        }
     }
 }
 
@@ -366,24 +488,30 @@ inline cudaError_t ce_set_smem() {
     if (e == cudaSuccess) attr_set[dev & 63] = true;
     return e;
 }
-// loss per row, shift per row and (a.dx != null) d loss / d xf
+// loss per row, shift per row and (a.dx != null) d loss / d xf, on at most `ctas` CTAs
 template <int D>
-inline cudaError_t launch_tc_ce(const bf16* xf, const bf16* table, const CeArgs& a, cudaStream_t st) {
+inline cudaError_t launch_tc_ce(const bf16* xf, const bf16* table, const CeArgs& a, int ctas, cudaStream_t st) {
     CUtensorMap tmX, tmE;
     if (!make_tmap_bf16(&tmX, xf, a.T, D, D, 64, 128) || !make_tmap_bf16(&tmE, table, a.C, D, D, 64, 64)) return cudaErrorInvalidValue;
     cudaError_t e = ce_set_smem<D>();
     if (e != cudaSuccess) return e;
-    launch_k(ce_rows_kernel<D>, (a.T + 127) / 128, CE_THREADS, CeSmem<D>::ROWS_BYTES, st, tmX, tmE, a);
+    const int R = (a.T + 127) / 128, units = (a.dx ? 2 : 1) * a.rseg * R;
+    e = cudaMemsetAsync(a.rsched, 0, (size_t)(1 + 2 * R) * sizeof(int), st);
+    if (e != cudaSuccess) return e;
+    launch_k(ce_rows_kernel<D>, units < ctas ? units : ctas, CE_THREADS, CeSmem<D>::ROWS_BYTES, st, tmX, tmE, a);
     return cudaGetLastError();
 }
-// a.dtable += d loss / d table, from the shifts launch_tc_ce left
+// a.dtable += d loss / d table, from the shifts launch_tc_ce left, on at most `ctas` CTAs
 template <int D>
-inline cudaError_t launch_ce_table(const bf16* xf, const bf16* table, const CeArgs& a, cudaStream_t st) {
+inline cudaError_t launch_ce_table(const bf16* xf, const bf16* table, const CeArgs& a, int ctas, cudaStream_t st) {
     CUtensorMap tmX, tmE;
     if (!make_tmap_bf16(&tmX, xf, a.T, D, D, 64, 64) || !make_tmap_bf16(&tmE, table, a.C, D, D, 64, 64)) return cudaErrorInvalidValue;
     cudaError_t e = ce_set_smem<D>();
     if (e != cudaSuccess) return e;
-    launch_k(ce_table_kernel<D>, (a.C + 63) / 64, CE_THREADS, CeSmem<D>::TABLE_BYTES, st, tmX, tmE, a);
+    const int NC = (a.C + 63) / 64, units = a.tseg * NC;
+    e = cudaMemsetAsync(a.tsched, 0, (size_t)(1 + NC) * sizeof(int), st);
+    if (e != cudaSuccess) return e;
+    launch_k(ce_table_kernel<D>, units < ctas ? units : ctas, CE_THREADS, CeSmem<D>::TABLE_BYTES, st, tmX, tmE, a);
     return cudaGetLastError();
 }
 

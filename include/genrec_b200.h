@@ -209,6 +209,9 @@ int grb_embed_backward(const int64_t* ids, const int64_t* order, const float* dx
  * Replaces final_norm + `x @ item_embedding.weight.T` + cross_entropy(ignore_index=0) (hstu.py:134-146,
  * sasrec.py:118-128) and their backward.  C = num_items + 1 classes. */
 size_t grb_head_workspace_bytes(int T, int D, int C);
+/* D <= 128: how many segments each row tile's class sweep (table = 0) or each class tile's token sweep (table = 1) is cut
+ * into on the current device; 1 for D = 256.  A function of T, D, C and the SM count only; the results do not depend on it. */
+int grb_head_splits(int T, int D, int C, int table);
 /* training: loss (scalar, mean over targets != 0), dx [T,D], and the three parameter gradients (accumulated). */
 int grb_head_loss_forward_backward(const float* x, const float* ln_g, const float* ln_b, float ln_eps,
                                    const void* table_bf16, const int64_t* targets, int T, int D, int C, float* loss,
