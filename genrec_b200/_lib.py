@@ -95,6 +95,10 @@ SIGNATURES = {
     "grb_head_splits": (c_int, [c_int, c_int, c_int, c_int]),
     "grb_head_loss_forward_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_int, c_int, c_int,
                                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_head_sampled_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "grb_head_sampled_loss_forward_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                       c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                       c_void_p, c_void_p]),
     "grb_head_logits": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                 c_void_p]),
     "grb_head_topk_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),

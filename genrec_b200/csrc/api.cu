@@ -25,6 +25,7 @@
 #include "rq_sinkhorn.cuh"
 #include "tc_gemm.cuh"
 #include "tc_ce.cuh"
+#include "tc_sampled_ce.cuh"
 #include "tc_tn_group.cuh"
 #include <cstdlib>
 
@@ -1016,6 +1017,79 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
         return 0;
     }));
     }
+    return ln_backward(LnBwdArgs{h.dxf, x, h.stf, ln_g, nullptr, dx, dln_g, dln_b, T, D, h.part_ln}, st);
+}
+
+// ---- sampled-softmax head (tc_sampled_ce.cuh)
+namespace {
+struct SampledWork {
+    bf16* xf; float* stf; float* dxf; float* scal;      // as HeadWork
+    bf16* Es; float* bias; int* sid;                     // the gathered negatives
+    float *ztgt, *shift, *row_loss, *gtgt;               // per token
+    float* part; int ks;                                 // token-range partial sums of the sub-table gradient
+    float* part_ln;
+    int Npad;
+    size_t bytes;
+};
+SampledWork carve_sampled(void* base, size_t T, size_t D, size_t N) {
+    SampledWork h;
+    Carver c{static_cast<char*>(base)};
+    h.Npad = (int)((N + 63) / 64 * 64);
+    h.ks = sce_table_splits((int)T, h.Npad, sm_count());
+    h.xf = c.take<bf16>(T * D * 2);
+    h.stf = c.take<float>(T * 2 * 4);
+    h.dxf = c.take<float>(T * D * 4);
+    h.scal = c.take<float>(64);
+    h.Es = c.take<bf16>((size_t)h.Npad * D * 2);
+    h.bias = c.take<float>((size_t)h.Npad * 4);
+    h.sid = c.take<int>((size_t)h.Npad * 4);
+    h.ztgt = c.take<float>(T * 4);
+    h.shift = c.take<float>(T * 4);
+    h.row_loss = c.take<float>(T * 4);
+    h.gtgt = c.take<float>(T * 4);
+    h.part = c.take<float>((size_t)h.ks * h.Npad * D * 4);
+    h.part_ln = c.take<float>((size_t)2 * row_bwd_grid((int)T) * D * 4);
+    h.bytes = c.off;
+    return h;
+}
+int check_sampled_shape(int T, int D, int N) {
+    GRB_REQUIRE(T >= 1, "sampled head: T=%d must be >= 1", T);
+    GRB_REQUIRE(D == 64 || D == 128, "sampled head: D=%d is not supported (D must be 64 or 128; D = 256 is served by the full head only)", D);
+    GRB_REQUIRE(N >= 1 && N <= SCE_MAX_N, "sampled head: N=%d negatives, must be 1 .. %d", N, SCE_MAX_N);
+    return 0;
+}
+}  // namespace
+
+size_t grb_head_sampled_workspace_bytes(int T, int D, int N) {
+    if (check_sampled_shape(T, D, N) != 0) return 0;
+    return carve_sampled(nullptr, T, D, N).bytes;
+}
+
+int grb_head_sampled_loss_forward_backward(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16,
+                                           const int64_t* targets, const int64_t* negatives, const float* log_q, int T, int D, int C, int N,
+                                           float* loss, float* dx, float* dtable, float* dln_g, float* dln_b, void* workspace, void* stream) {
+    GRB_REQUIRE(x && ln_g && ln_b && table_bf16 && targets && negatives && loss && workspace, "null argument");
+    GRB_TRY(check_sampled_shape(T, D, N));
+    GRB_REQUIRE(C >= 2, "sampled head: C=%d classes, must be >= 2", C);
+    const bool want_grad = dx != nullptr;
+    GRB_REQUIRE(!want_grad || (dtable && dln_g && dln_b), "null gradient pointer");
+    GRB_REQUIRE(aligned16(table_bf16) && aligned16(workspace) && (!want_grad || aligned16(dtable)), "table_bf16, dtable and workspace must be 16-byte aligned");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    SampledWork h = carve_sampled(workspace, T, D, N);
+    launch_k(ce_count_kernel, 1, 1024, 0, st, reinterpret_cast<const long long*>(targets), T, h.scal, loss);
+    GRB_CUDA(cudaGetLastError());
+    {
+        LnFwdArgs a{x, ln_g, ln_b, h.xf, nullptr, h.stf, T, D, ln_eps};
+        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
+    }
+    SceArgs sa{reinterpret_cast<const long long*>(targets), reinterpret_cast<const long long*>(negatives), log_q, (const bf16*)table_bf16, h.xf,
+               h.scal, T, C, N, h.Npad, D, h.Es, h.bias, h.sid, h.ztgt, h.shift, h.row_loss, h.gtgt, want_grad ? h.dxf : nullptr, h.part, h.ks,
+               dtable};
+    if (D == 64) GRB_CUDA(launch_sampled_ce<64>(sa, sm_count(), st));
+    else GRB_CUDA(launch_sampled_ce<128>(sa, sm_count(), st));
+    launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
+    GRB_CUDA(cudaGetLastError());
+    if (!want_grad) return 0;
     return ln_backward(LnBwdArgs{h.dxf, x, h.stf, ln_g, nullptr, dx, dln_g, dln_b, T, D, h.part_ln}, st);
 }
 

@@ -1,9 +1,10 @@
 """Input contract of the hot path: collate functions (mirrors of genrec/data/amazon_hstu.py:137-200 and
 genrec/data/amazon_sasrec.py:125-181), synthetic generators (SURVEY.md section 8d) and data-parallel batch sharding.
-Host-side, pure Python/torch-CPU; nothing here computes model arithmetic."""
+Host-side, pure Python/torch-CPU; nothing here computes model arithmetic.  ``sample_negatives`` draws the shared negatives of the
+sampled-softmax head on whichever device its inputs live on."""
 from __future__ import annotations
 
-from typing import Dict, List
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -107,3 +108,25 @@ def collate_jagged(items: torch.Tensor, offsets: torch.Tensor, targets: torch.Te
     if tss is not None:
         out["timestamps"] = tss
     return out
+
+
+def sample_negatives(num_items: int, n: int, *, probs: Optional[torch.Tensor] = None, generator: Optional[torch.Generator] = None,
+                     device=None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """The shared negatives of one sampled-softmax step: ``(negatives [n] int64 in 1..num_items, log_q [num_items + 1] fp32 | None)``,
+    drawn with replacement, on the device and without a host synchronisation (so a captured step can redraw them).
+
+    Without ``probs`` the draw is uniform and ``log_q`` is None (a constant correction changes nothing).  ``probs`` [num_items + 1]
+    are non-negative item frequencies or probabilities (entry 0, the padding id, is never drawn): the draw is
+    ``torch.multinomial(probs[1:], n, replacement=True)`` and ``log_q = log(probs / probs[1:].sum())`` (``-inf`` for never-drawn
+    items; such an item only ever appears as a target, where a finite correction is needed, so pass smoothed frequencies)."""
+    if num_items < 1 or n < 1:
+        raise ValueError(f"sample_negatives needs num_items >= 1 and n >= 1 (got {num_items}, {n})")
+    if probs is None:
+        dev = device if device is not None else (generator.device if generator is not None else "cpu")
+        return torch.randint(1, num_items + 1, (n,), dtype=torch.int64, device=dev, generator=generator), None
+    if tuple(probs.shape) != (num_items + 1,):
+        raise ValueError(f"probs must be [{num_items + 1}] (one entry per id 0..num_items), got {tuple(probs.shape)}")
+    w = probs.detach().float()
+    negatives = torch.multinomial(w[1:], n, replacement=True, generator=generator) + 1
+    log_q = torch.log(w / w[1:].sum())
+    return negatives, log_q

@@ -324,6 +324,82 @@ class HeadLossFn(torch.autograd.Function):
         return dx * dloss, dg * dloss, db * dloss, dtable * dloss, None, None, None, None, None
 
 
+def head_sampled_loss_raw(x, ln_g, ln_b, table_bf16, targets, negatives, log_q, eps, grads=None):
+    """grb_head_sampled_loss_forward_backward on x [T, D]: -> loss (0-dim fp32).  ``grads = (dx, dtable, dln_g, dln_b)``: dx is
+    written, the other three are accumulated into; ``None``: loss only."""
+    lib = _lib.load()
+    require_cuda(x, table_bf16, targets, negatives, log_q)
+    require_i64(targets, negatives)
+    require_f32(x, ln_g, ln_b, log_q)
+    T, D = x.shape
+    Cn, N = table_bf16.shape[0], negatives.numel()
+    if negatives.dim() != 1:
+        raise _lib.GrbError(f"genrec_b200 error -1: negatives must be one [N] vector shared by every token (got shape {tuple(negatives.shape)})")
+    if log_q is not None and tuple(log_q.shape) != (Cn,):
+        raise _lib.GrbError(f"genrec_b200 error -1: log_q must be [{Cn}] (one entry per table row), got {tuple(log_q.shape)}")
+    for t in (negatives, log_q):
+        if t is not None and t.device != x.device:
+            raise _lib.GrbError(f"genrec_b200 error -1: negatives / log_q must live on the model's device {x.device} (got {t.device})")
+    neg = negatives.contiguous()
+    lq = log_q.detach().contiguous() if log_q is not None else None
+    loss = torch.empty((), dtype=torch.float32, device=x.device)   # zeroed on the device by the target-count kernel
+    with torch.cuda.device(x.device):
+        nbytes = lib.grb_head_sampled_workspace_bytes(T, D, N)
+        if nbytes == 0:
+            check(-1)
+        ws = _u8(nbytes, x.device)
+        dx, dtable, dg, db = grads if grads is not None else (None,) * 4
+        check(lib.grb_head_sampled_loss_forward_backward(ptr(x), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), ptr(targets),
+                                                         ptr(neg), ptr(lq), T, D, Cn, N, ptr(loss), ptr(dx), ptr(dtable), ptr(dg), ptr(db), ptr(ws),
+                                                         stream_ptr(x.device)))
+    return loss
+
+
+class SampledHeadLossFn(torch.autograd.Function):
+    """loss = sampled softmax of LN(x) against E[targets] and the shared ``negatives`` [N], scores corrected by ``-log_q`` (see
+    grb_head_sampled_loss_forward_backward).  ``sink`` / ``unit_loss_grad`` behave as in ``HeadLossFn``."""
+
+    @staticmethod
+    def forward(ctx, x, ln_g, ln_b, table, table_bf16, targets, negatives, log_q, eps, sink=None, unit_loss_grad=False):
+        require_f32(table)
+        B, L, D = x.shape
+        xc = x.detach().contiguous().float().view(B * L, D)
+        tg = targets.contiguous().view(-1)
+        need_grad = any(ctx.needs_input_grad[:4])
+        direct = need_grad and sink is not None and unit_loss_grad
+        ctx.sink, ctx.direct, ctx.xshape = sink, direct, x.shape
+        if direct:
+            dx = torch.empty_like(xc)
+            dg, db, dtable = sink
+        elif need_grad:
+            dx = torch.empty_like(xc)
+            dtable = torch.zeros(table.shape, dtype=torch.float32, device=x.device)
+            dg = torch.zeros_like(ln_g, dtype=torch.float32)
+            db = torch.zeros_like(ln_b, dtype=torch.float32)
+        else:
+            dx = dtable = dg = db = None
+        loss = head_sampled_loss_raw(xc, ln_g, ln_b, table_bf16, tg, negatives, log_q, eps, (dx, dtable, dg, db) if need_grad else None)
+        ctx.grads = (dx, dg, db, dtable)
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        dx, dg, db, dtable = ctx.grads
+        ctx.grads = None
+        if dx is None:
+            return (None,) * 11
+        dx = dx.view(ctx.xshape)
+        if ctx.direct:
+            with torch.cuda.device(dx.device):
+                check(_lib.load().grb_assert_unit_scalar(ptr(dloss.detach().float().contiguous()), stream_ptr(dx.device)))
+            return (dx,) + (None,) * 10
+        if ctx.sink is not None:
+            sg, sb, st = ctx.sink
+            sg.add_(dg * dloss); sb.add_(db * dloss); st.addcmul_(dtable, dloss)
+            return (dx * dloss,) + (None,) * 10
+        return (dx * dloss, dg * dloss, db * dloss, dtable * dloss) + (None,) * 7
+
+
 def head_logits(x, ln_g, ln_b, table, table_bf16, eps) -> torch.Tensor:
     """fp32 logits [B, L, C] (no autograd - inference / API parity path)."""
     lib = _lib.load()

@@ -466,9 +466,18 @@ class HSTU(nn.Module):
                 x = layer(x, None, None, timestamps, _meta=meta, _seed=seed, _seed_dev=seed_dev)
         return x
 
-    def forward(self, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None,
-                targets: Optional[torch.Tensor] = None) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
-        """hstu.py:99-148.  Returns (logits [B,L,V+1] fp32 | None, loss | None)."""
+    def forward(self, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None, targets: Optional[torch.Tensor] = None, *,
+                negatives: Optional[torch.Tensor] = None, log_q: Optional[torch.Tensor] = None
+                ) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """hstu.py:99-148.  Returns (logits [B,L,V+1] fp32 | None, loss | None).
+
+        ``negatives`` ([N] int64 on the model's device, shared by every token; ``data.sample_negatives``) switches the loss to the
+        sampled softmax with the logQ correction ``log_q`` ([V+1] fp32 or None): its cost does not depend on the catalog size.  It
+        needs ``targets`` and returns ``(None, loss)``; evaluation and serving always score the full catalog."""
+        if negatives is None and log_q is not None:
+            raise ValueError("log_q corrects the sampled softmax: pass negatives with it")
+        if negatives is not None and targets is None:
+            raise ValueError("negatives select the sampled-softmax loss, which needs targets")
         x = self.encode(input_ids, timestamps)
         if self.precision == "fp32":
             if targets is not None:
@@ -482,6 +491,10 @@ class HSTU(nn.Module):
             hsink = None
             if self._grad_sink is not None and torch.is_grad_enabled():
                 hsink = (self._grad_sink(self.final_norm.weight), self._grad_sink(self.final_norm.bias), self._grad_sink(table))
+            if negatives is not None:
+                loss = Fn.SampledHeadLossFn.apply(x, self.final_norm.weight, self.final_norm.bias, table, table_bf16, targets, negatives,
+                                                  log_q, self.final_norm.eps, hsink, self._unit_loss_grad)
+                return None, loss
             loss = Fn.HeadLossFn.apply(x, self.final_norm.weight, self.final_norm.bias, table, table_bf16, targets,
                                        self.final_norm.eps, hsink, self._unit_loss_grad)
         if targets is None or not self.training or self.return_train_logits:

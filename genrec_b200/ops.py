@@ -195,6 +195,42 @@ def _(x, ln_g, ln_b, table_bf16, eps, k, exclude):
     return x.new_empty((R, k), dtype=torch.float32), x.new_empty((R, k), dtype=torch.int64)
 
 
+# ------------------------------------------------------------------------------------------------ sampled-softmax head
+@custom_op(f"{NS}::head_sampled_loss", mutates_args=())
+def head_sampled_loss(x: Tensor, ln_g: Tensor, ln_b: Tensor, table: Tensor, targets: Tensor, negatives: Tensor, log_q: Optional[Tensor],
+                      eps: float) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """x [T, D] fp32, table [C, D] fp32, targets [T] (0 = ignored), negatives [N] shared by every token, log_q [C] or None ->
+    (loss, dx [T, D], dln_g [D], dln_b [D], dtable [C, D]): the sampled softmax with logQ correction and, from the same pass, its
+    gradients for a unit gradient of the loss (the autograd formula scales them)."""
+    require_cuda(x)
+    xc = x.contiguous().float()
+    dx = torch.empty_like(xc)
+    dtable = torch.zeros(table.shape, dtype=torch.float32, device=x.device)
+    dg = torch.zeros(ln_g.shape, dtype=torch.float32, device=x.device)
+    db = torch.zeros(ln_b.shape, dtype=torch.float32, device=x.device)
+    loss = Fn.head_sampled_loss_raw(xc, ln_g, ln_b, Fn.cast_bf16(table), targets.contiguous(), negatives, log_q, eps, (dx, dtable, dg, db))
+    return loss, dx, dg, db, dtable
+
+
+@head_sampled_loss.register_fake
+def _(x, ln_g, ln_b, table, targets, negatives, log_q, eps):
+    f32 = dict(dtype=torch.float32)
+    return (x.new_empty((), **f32), x.new_empty(x.shape, **f32), x.new_empty(ln_g.shape, **f32), x.new_empty(ln_b.shape, **f32),
+            x.new_empty(table.shape, **f32))
+
+
+def _sampled_setup(ctx, inputs, output):
+    ctx.save_for_backward(*output[1:])
+
+
+def _sampled_backward(ctx, dloss, *_):
+    dx, dg, db, dtable = ctx.saved_tensors
+    return dx * dloss, dg * dloss, db * dloss, dtable * dloss, None, None, None, None
+
+
+torch.library.register_autograd(f"{NS}::head_sampled_loss", _sampled_backward, setup_context=_sampled_setup)
+
+
 # ------------------------------------------------------------------------------------------------ SASRec attention core
 @custom_op(f"{NS}::sasrec_attention", mutates_args=())
 def sasrec_attention(q: Tensor, k: Tensor, v: Tensor, pad: Tensor, num_heads: int, dropout_p: float, seed: int, seed_dev: Optional[Tensor],
@@ -240,4 +276,4 @@ torch.library.register_autograd(f"{NS}::sasrec_attention", _sas_backward, setup_
 
 
 OPS = ("hstu_attention", "hstu_attention_backward", "hstu_layer", "hstu_layer_backward", "rq_residual_argmin", "rq_sinkhorn",
-       "eval_rank_metrics", "head_topk", "sasrec_attention", "sasrec_attention_backward")
+       "eval_rank_metrics", "head_topk", "head_sampled_loss", "sasrec_attention", "sasrec_attention_backward")

@@ -254,13 +254,22 @@ class SASRec(nn.Module):
             x = blk(x, mask, _apply_mask=True, _seed=seed, _seed_dev=sd)                         # :114-116
         return x
 
-    def forward(self, input_ids: torch.Tensor, targets: Optional[torch.Tensor] = None
-                ) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
-        """sasrec.py:79-130.  Returns (logits [B,L,V+1] fp32 | None when training with targets, loss | None)."""
+    def forward(self, input_ids: torch.Tensor, targets: Optional[torch.Tensor] = None, *, negatives: Optional[torch.Tensor] = None,
+                log_q: Optional[torch.Tensor] = None) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """sasrec.py:79-130.  Returns (logits [B,L,V+1] fp32 | None when training with targets, loss | None).  With ``negatives``
+        ([N] int64, shared by every token) and optionally ``log_q`` ([V+1] fp32) the loss is the sampled softmax with logQ correction
+        (see ``HSTU.forward``) and the result is ``(None, loss)``."""
+        if negatives is None and log_q is not None:
+            raise ValueError("log_q corrects the sampled softmax: pass negatives with it")
+        if negatives is not None and targets is None:
+            raise ValueError("negatives select the sampled-softmax loss, which needs targets")
         x = self.encode(input_ids)
         table = self.item_embedding.weight
         table_bf16 = Fn.cast_bf16(table)
         logits = loss = None
+        if negatives is not None:
+            return None, Fn.SampledHeadLossFn.apply(x, self.final_norm.weight, self.final_norm.bias, table, table_bf16, targets, negatives,
+                                                    log_q, self.final_norm.eps)
         if targets is not None:
             loss = Fn.HeadLossFn.apply(x, self.final_norm.weight, self.final_norm.bias, table, table_bf16, targets, self.final_norm.eps)
         if targets is None or not self.training or self.return_train_logits:

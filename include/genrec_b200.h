@@ -216,6 +216,20 @@ int grb_head_splits(int T, int D, int C, int table);
 int grb_head_loss_forward_backward(const float* x, const float* ln_g, const float* ln_b, float ln_eps,
                                    const void* table_bf16, const int64_t* targets, int T, int D, int C, float* loss,
                                    float* dx, float* dtable, float* dln_g, float* dln_b, void* workspace, void* stream);
+/* Sampled softmax for catalogs too large for the full head: every token is scored against its target and against N negatives
+ * shared by all tokens of the call (negatives [N] int64, sampled with replacement: a repeated id is two classes), each score
+ * corrected by -log_q[id] (log_q [C] fp32: log of the proposal probability or expected count; NULL = no correction).  A negative
+ * equal to the token's target (an accidental hit) or outside 1 .. C-1 is left out of that token's softmax; validity is decided on
+ * the device.  loss = mean over targets != 0 of logsumexp(z_tgt, z_0 .. z_{N-1}) - z_tgt; targets lie in 0 .. C-1 as above.
+ * Outputs and conventions as grb_head_loss_forward_backward (dx NULL: loss only; parameter gradients accumulated; no target
+ * != 0: NaN loss, zero gradients).  Every sum has a fixed order: two calls with the same arguments give the same bits.
+ * D in {64, 128}, 1 <= N <= 8192, C >= 2, T >= 1.  The cost is 6 T D (N + 1) FLOP and the workspace
+ * (grb_head_sampled_workspace_bytes; 0 for unsupported arguments) grows with T and N, not with C. */
+size_t grb_head_sampled_workspace_bytes(int T, int D, int N);
+int grb_head_sampled_loss_forward_backward(const float* x, const float* ln_g, const float* ln_b, float ln_eps,
+                                           const void* table_bf16, const int64_t* targets, const int64_t* negatives,
+                                           const float* log_q, int T, int D, int C, int N, float* loss, float* dx, float* dtable,
+                                           float* dln_g, float* dln_b, void* workspace, void* stream);
 /* inference / API parity: logits fp32 [T, C] (contiguous), optional loss. */
 int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int T,
                     int D, int C, float* logits, void* workspace, void* stream);

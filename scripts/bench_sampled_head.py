@@ -1,0 +1,190 @@
+"""Measure the sampled-softmax head on the GPU: python scripts/bench_sampled_head.py [--out result.json]
+
+  1. head alone at T = 128 x 200 tokens, D = 128 and 64: the full head at C = 12,102 next to the sampled head at N = 128, 1,024 and
+     4,096, alternated in one session, each call replayed from a CUDA graph and timed with CUDA events; the sampled head again at
+     C = 1,000,001 (its time must not depend on C);
+  2. the time of each kernel of the sampled head (torch.profiler, a run of its own), and for the row pass the least time the
+     hardware could take: the larger of 6 T D (N + 1) FLOP at 989 TFLOP/s and the bytes it must move at 3.35 TB/s (data-sheet
+     figures of the H100 SXM at 700 W);
+  3. one training step of HSTU at the cfg2 geometry with V = 1,000,000 items and N = 1,024 under FlatAdam, and the part of it the
+     optimizer's pass over the flat buffer (the dense table is nearly all of it) takes.
+A GPU is required; there is no fallback.  The card's name and power limit are read in the same run and printed with the numbers."""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+PEAK_FLOPS, PEAK_BYTES = 989e12, 3.35e12
+EPS = 1e-5
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+    return q.stdout.strip() or torch.cuda.get_device_name(0)
+
+
+def graph_time(fn, iters=20, rounds=5):
+    """median over `rounds` of the mean time (ms) of `iters` replays of fn captured in a CUDA graph"""
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        for _ in range(3):
+            fn()
+    torch.cuda.current_stream().wait_stream(s)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        fn()
+    g.replay()
+    torch.cuda.synchronize()
+    out = []
+    for _ in range(rounds):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        for _ in range(iters):
+            g.replay()
+        b.record()
+        torch.cuda.synchronize()
+        out.append(a.elapsed_time(b) / iters)
+    return statistics.median(out)
+
+
+class Head:
+    """operands of one head call at (T, D, C) and closures that run the full / the sampled head through the C ABI"""
+
+    def __init__(self, T, D, C, dev):
+        from genrec_b200 import functional as Fn
+        g = torch.Generator(device=dev).manual_seed(T + D + C)
+        self.T, self.D, self.C, self.dev = T, D, C, dev
+        self.x = torch.randn(T, D, device=dev, generator=g)
+        self.ln_g, self.ln_b = torch.ones(D, device=dev), torch.zeros(D, device=dev)
+        self.tb = Fn.cast_bf16(0.05 * torch.randn(C, D, device=dev, generator=g))
+        self.tg = torch.randint(1, C, (T,), device=dev, generator=g)
+        self.log_q = torch.log_softmax(torch.randn(C, device=dev, generator=g), 0)
+        self.dx, self.dE = torch.empty_like(self.x), torch.zeros(C, D, device=dev)
+        self.dg, self.db = torch.zeros(D, device=dev), torch.zeros(D, device=dev)
+        self.loss = torch.empty((), device=dev)
+        self.gen = g
+
+    def full(self):
+        from genrec_b200 import _lib
+        from genrec_b200._lib import check, ptr, stream_ptr
+        lib = _lib.load()
+        ws = torch.empty(lib.grb_head_workspace_bytes(self.T, self.D, self.C), dtype=torch.uint8, device=self.dev)
+        return lambda: check(lib.grb_head_loss_forward_backward(ptr(self.x), ptr(self.ln_g), ptr(self.ln_b), EPS, ptr(self.tb), ptr(self.tg), self.T,
+                                                                self.D, self.C, ptr(self.loss), ptr(self.dx), ptr(self.dE), ptr(self.dg), ptr(self.db),
+                                                                ptr(ws), stream_ptr(self.dev)))
+
+    def sampled(self, N):
+        from genrec_b200 import _lib
+        from genrec_b200._lib import check, ptr, stream_ptr
+        lib = _lib.load()
+        neg = torch.randint(1, self.C, (N,), device=self.dev, generator=self.gen)
+        ws = torch.empty(lib.grb_head_sampled_workspace_bytes(self.T, self.D, N), dtype=torch.uint8, device=self.dev)
+        return lambda: check(lib.grb_head_sampled_loss_forward_backward(ptr(self.x), ptr(self.ln_g), ptr(self.ln_b), EPS, ptr(self.tb), ptr(self.tg),
+                                                                        ptr(neg), ptr(self.log_q), self.T, self.D, self.C, N, ptr(self.loss),
+                                                                        ptr(self.dx), ptr(self.dE), ptr(self.dg), ptr(self.db), ptr(ws),
+                                                                        stream_ptr(self.dev)))
+
+
+def head_alone(dev, T, res):
+    for D in (128, 64):
+        small, big = Head(T, D, 12102, dev), Head(T, D, 1_000_001, dev)
+        runs = [("full head C=12102", small.full())]
+        for N in (128, 1024, 4096):
+            runs.append((f"sampled N={N} C=12102", small.sampled(N)))
+        runs.append(("sampled N=1024 C=1000001", big.sampled(1024)))
+        times = {k: [] for k, _ in runs}
+        for _ in range(3):                               # alternate the variants: drift of the card hits all of them alike
+            for k, fn in runs:
+                times[k].append(graph_time(fn, rounds=3))
+        for k, v in times.items():
+            res[f"head D={D} T={T} {k} ms"] = round(statistics.median(v), 4)
+        del small, big
+        torch.cuda.empty_cache()
+
+
+def per_kernel(dev, T, res):
+    from torch.profiler import ProfilerActivity, profile
+    D = 128
+    h = Head(T, D, 12102, dev)
+    for N in (1024, 4096):
+        fn = h.sampled(N)
+        for _ in range(3):
+            fn()
+        torch.cuda.synchronize()
+        reps = 20
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                fn()
+            torch.cuda.synchronize()
+        for ev in prof.key_averages():
+            name = ev.key
+            for short in ("sce_gather_kernel", "sce_target_kernel", "sce_rows_kernel", "sce_table_kernel", "sce_scatter_kernel", "ln_fwd_kernel",
+                          "ln_bwd_kernel"):
+                if short in name:
+                    t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0.0)
+                    res[f"kernel D={D} T={T} N={N} {short} us"] = round(t / reps, 2)
+        Npad = (N + 63) // 64 * 64
+        flop_t = 6.0 * T * D * (N + 1) / PEAK_FLOPS
+        bytes_t = (T * D * 2 + T * D * 4 + Npad * D * 2 + T * 8 * 4) / PEAK_BYTES      # H in, dH out, Es once, the per-token vectors
+        res[f"row pass bound D={D} T={T} N={N} us"] = round(max(flop_t, bytes_t) * 1e6, 2)
+        res[f"row pass bound D={D} T={T} N={N} binds"] = "FLOP at 989 TFLOP/s" if flop_t >= bytes_t else "bytes at 3.35 TB/s"
+
+
+def full_step(dev, res):
+    from genrec_b200.data import sample_negatives
+    from genrec_b200.hstu import HSTU
+    from genrec_b200.optim import FlatAdam
+    V, B, L, N = 1_000_000, 128, 200, 1024
+    torch.manual_seed(0)
+    model = HSTU(num_items=V, max_seq_len=L, embed_dim=128, num_heads=4, num_blocks=4, dropout=0.2).to(dev).train()
+    opt = FlatAdam(model, lr=1e-3, betas=(0.9, 0.98), unit_loss_grad=True)
+    g = torch.Generator(device=dev).manual_seed(1)
+    ids = torch.randint(1, V + 1, (B, L), device=dev, generator=g)
+    tg = torch.randint(1, V + 1, (B, L), device=dev, generator=g)
+    ts = 1_300_000_000 + torch.cumsum(torch.randint(1, 86400, (B, L), device=dev, generator=g), 1)
+    neg = torch.empty(N, dtype=torch.int64, device=dev)
+
+    def step():
+        neg.copy_(sample_negatives(V, N, device=dev)[0])       # redrawn on the device inside the captured step
+        _, loss = model(ids, ts, tg, negatives=neg)
+        loss.backward()
+        opt.step()
+
+    res[f"cfg2 geometry V={V} N={N} training step ms"] = round(graph_time(step, iters=5, rounds=3), 3)
+    res[f"cfg2 geometry V={V} FlatAdam step alone ms"] = round(graph_time(opt.step, iters=5, rounds=3), 3)
+    table = model.item_embedding.weight.numel()
+    res["table share of the parameters"] = round(table / sum(p.numel() for p in model.parameters()), 4)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default=None)
+    ap.add_argument("--skip-step", action="store_true")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_sampled_head.py needs a CUDA GPU (sm_90a); there is no fallback")
+    from genrec_b200 import _lib
+    dev = torch.device("cuda:0")
+    _lib.ensure_device(dev)
+    res = {"card": card()}
+    T = 128 * 200
+    head_alone(dev, T, res)
+    per_kernel(dev, T, res)
+    if not args.skip_step:
+        full_step(dev, res)
+    print(json.dumps(res, indent=1))
+    if args.out:
+        with open(args.out, "w") as f:
+            json.dump(res, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
