@@ -605,21 +605,30 @@ __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 3 : 2) hstu_attn_bwd_d
         for (int w = 0; w < ATT_THREADS / 32; ++w) v += s_pos[w];
         return v;
     };
-    auto pos_bin = [&](int bk) {
-        float v = 0.f;
-        for (int w = 0; w < 4; ++w)
-            for (int l = 0; l < 32; ++l) v += hist_p[(w * (npos + 1) + bk) * 32 + l];
-        return v;
-    };
-    auto time_bin = [&](int bk) {
-        float v = 0.f;
-        for (int w = 0; w < 4; ++w)
-            for (int l = 0; l < 32; ++l) v += hist_t[(w * nt_bins + bk) * 32 + l];
-        return v;
+    // Bin bk of a histogram is the sum over (warp w, lane l) in that order.  Read in place, the threads of one warp (consecutive
+    // bins) would hit one bank 32 times per load, so the first n bins are first transposed into the free stream / index buffers as
+    // tr[(w * 32 + l) * ld + bk] with an odd ld: the copy (lanes = l) and the sums (lanes = bk) are both conflict-free, and each
+    // bin keeps its order of addition.
+    float* tr = reinterpret_cast<float*>(att_smem_raw);
+    static_assert(sizeof(AttSmemKV<DH>) >= 4 * 32 * (ATT_MAX_BUCKETS + 1) * sizeof(float), "transposed histogram does not fit");
+    auto binned = [&](const float* hist, int stride, int n, int group) {
+        const int ld = n | 1;
+        for (int r = warp; r < 4 * n; r += ATT_THREADS / 32) {
+            const int w = r / n, bk = r - w * n;
+            tr[(w * 32 + lane) * ld + bk] = hist[(w * stride + bk) * 32 + lane];
+        }
+        __syncthreads();
+        det_store(a.dw_part, group, member, nmem, 64, n, [&](int bk) {
+            float v = 0.f;
+            for (int w = 0; w < 4; ++w)
+                for (int l = 0; l < 32; ++l) v += tr[(w * 32 + l) * ld + bk];
+            return v;
+        });
+        __syncthreads();   // tr is reused by the next histogram
     };
     if (pos_uniform) det_store(a.dw_part, h, member, nmem, 64, 1, pos_sum);
-    else det_store(a.dw_part, h, member, nmem, 64, npos, pos_bin);
-    if (has_time && a.dwtime) det_store(a.dw_part, a.H + h, member, nmem, 64, ntime, time_bin);
+    else binned(hist_p, npos + 1, npos, h);
+    if (has_time && a.dwtime) binned(hist_t, nt_bins, ntime, a.H + h);
 }
 
 }  // namespace grb

@@ -2,7 +2,8 @@
 cached incremental HSTU inference next to full recompute, RQ-VAE Sinkhorn and k-means init) with CUDA events, against the relevant
 roofline or the torch code they replace.  Prints one JSON line per measurement; `bench_kernels.py rqvae_train` runs only the RQ-VAE
 training rows, `bench_kernels.py linear_bwd` only the linear-backward and SASRec training-step rows, `bench_kernels.py head_topk` only
-the fused top-k head rows, `bench_kernels.py tiger` only the TIGER rows (training step, generate eager / graph / uncached loop)."""
+the fused top-k head rows, `bench_kernels.py tiger` only the TIGER rows (training step, generate eager / graph / uncached loop),
+`bench_kernels.py hstu_attn` only the HSTU attention backward rows."""
 import json
 import os
 import sys
@@ -372,8 +373,48 @@ def bench_tiger(dev):
                           graph_vs_uncached=min(rows["uncached"]) / min(rows["graph"]))), flush=True)
 
 
+def bench_hstu_attn(dev):
+    """Fn.hstu_attention_bwd alone, replayed from a CUDA graph, at the benchmark's two geometries (cfg2: B = 128, L = 200, D = 128,
+    H = 4; cfg3: B = 32, L = 2048, D = 256, H = 8), uniform position buckets, with and without the 64-bucket time table.  The call
+    also clears its dzp output.  The attention kernels' device time per call comes from a torch.profiler run of its own."""
+    from genrec_b200.hstu import _thresholds_on
+    from torch.profiler import ProfilerActivity, profile
+    info = card()
+    for name, B, L, D, H in (("cfg2", 128, 200, 128, 4), ("cfg3", 32, 2048, 256, 8)):
+        g = torch.Generator().manual_seed(0)
+        zp = (0.7 * torch.randn(B, L, 4 * D, generator=g)).bfloat16().to(dev)
+        P = torch.nn.functional.silu(zp.float()).bfloat16()
+        dO = (torch.randn(B, L, D, generator=g) / L ** 0.5).bfloat16().to(dev)
+        ts = (1_300_000_000 + torch.cumsum(torch.randint(1, 3 * 86400, (B, L), generator=g), 1)).to(dev)
+        pad = torch.zeros(B, L, dtype=torch.uint8, device=dev)
+        pb = torch.zeros(L, dtype=torch.uint8, device=dev)
+        wpos, wtime = (0.3 * torch.randn(32, H, generator=g)).to(dev), (0.5 * torch.randn(64, H, generator=g)).to(dev)
+        for time_table in (True, False):
+            meta = Fn.SeqMeta(pad, ts if time_table else None, pb, _thresholds_on(dev), 64, 32, (True, 0))
+            wt = wtime if time_table else None
+
+            def call():
+                return Fn.hstu_attention_bwd(P, zp, dO, meta, H, wpos, wt, 64)
+
+            ms = graph_timed(call)
+            call()
+            torch.cuda.synchronize()
+            iters = 20
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(iters):
+                    call()
+                torch.cuda.synchronize()
+            kern = {k.key.split("<")[0].replace("void ", "").replace("grb::", ""): round(k.device_time_total / iters, 2)
+                    for k in prof.key_averages() if "hstu_attn_bwd" in k.key or "det_finish" in k.key}
+            print(json.dumps(dict(kernel="hstu_attention_bwd", geometry=name, B=B, L=L, D=D, H=H, time_table=time_table,
+                                  us=ms * 1e3, kernel_us_per_call=kern, **info)), flush=True)
+
+
 def main():
     dev = torch.device("cuda:0")
+    if sys.argv[1:] == ["hstu_attn"]:
+        bench_hstu_attn(dev)
+        return
     if sys.argv[1:] == ["rqvae_train"]:
         bench_rqvae_train(dev)
         return
