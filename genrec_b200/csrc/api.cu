@@ -6,7 +6,6 @@
 #include <cstdio>
 #include <cstring>
 #include <initializer_list>
-#include <map>
 #include <mutex>
 #include <type_traits>
 #include <utility>
@@ -107,6 +106,13 @@ int with_row_dim(int D, F&& f) {
     else return fail(GRB_EINVAL, "row kernels support D in {64,128,256}, got %d", D);
     GRB_CUDA(cudaGetLastError());
     return 0;
+}
+// the fused loss heads (tc_ce.cuh, tc_sampled_ce.cuh) are instantiated for D = 64 and 128: f(integral_constant D) (head_fused and
+// check_sampled_shape admit nothing else)
+template <class F>
+auto with_ce_dim(int D, F&& f) {
+    if (D == 64) return f(std::integral_constant<int, 64>{});
+    return f(std::integral_constant<int, 128>{});
 }
 // the RMS norm kernels add TIGER's attn_dim, 384 (its embedding_dim is 128).  The LayerNorm / HSTU row kernels are not
 // instantiated at 384: nothing calls them there.
@@ -271,19 +277,10 @@ int check_seq(const grb_hstu_dims* d, const grb_hstu_seq* s) {
     return 0;
 }
 
-// opt in to > 48 KB dynamic shared memory once per (kernel, high-water mark): no runtime call on the steady-state path,
-// in particular none while a CUDA graph is being captured after warm-up.
+// set_max_smem (common.cuh) with the library's error reporting
 template <class Kern>
 int set_smem(Kern k, size_t bytes) {
-    static std::mutex mu;
-    static std::map<std::pair<int, const void*>, size_t> high_water;  // keyed by (device, kernel address): the attribute is per device
-    std::lock_guard<std::mutex> lock(mu);
-    size_t& hw = high_water[std::make_pair(current_device(), reinterpret_cast<const void*>(k))];
-    if (hw < 48 * 1024) hw = 48 * 1024;
-    if (bytes > hw) {
-        GRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-        hw = bytes;
-    }
+    GRB_CUDA(set_max_smem(k, bytes));
     return 0;
 }
 
@@ -909,12 +906,26 @@ int grb_embed_backward(const int64_t* ids, const int64_t* order, const float* dx
 
 // ------------------------------------------------------------------------------------------------ head
 namespace {
-struct HeadWork {
-    bf16* xf; float* stf; bf16* logits; float* dxf; float* scal;  // scal[0] = inv_count
-    float* logits32;                                               // stored schedule: fp32 logits (the CE reads them, the bf16 buffer takes the gradient)
+// what the full and the sampled loss head both keep in their workspace
+struct HeadCommon {
+    bf16* xf; float* stf; float* dxf; float* scal;                 // LN(x) and its statistics, d loss / d LN(x), scal[0] = inv_count
     float* row_loss;                                               // per-token loss, summed in a fixed order
-    float* shift;                                                  // fused schedule: per-token log2-domain softmax shift
-    float *part_ln, *part_tn;                                      // scratch of the ordered cross-CTA sums (LayerNorm, stored-schedule dE)
+    float* shift;                                                  // fused kernels: per-token log2-domain softmax shift
+    float* part_ln;                                                // scratch of the LayerNorm backward's ordered cross-CTA sums
+};
+void carve_head_common(Carver& c, HeadCommon& h, size_t T, size_t D) {
+    h.xf = c.take<bf16>(T * D * 2);
+    h.stf = c.take<float>(T * 2 * 4);
+    h.dxf = c.take<float>(T * D * 4);
+    h.scal = c.take<float>(64);
+    h.row_loss = c.take<float>(T * 4);
+    h.shift = c.take<float>(T * 4);
+    h.part_ln = c.take<float>((size_t)2 * row_bwd_grid((int)T) * D * 4);
+}
+struct HeadWork : HeadCommon {
+    bf16* logits;                                                  // stored schedule: takes the gradient
+    float* logits32;                                               // stored schedule: fp32 logits (the CE reads them, the bf16 buffer takes the gradient)
+    float* part_tn;                                                // stored schedule: scratch of dE's ordered cross-CTA sums
     int *ce_rsched, *ce_tsched;                                    // fused schedule: unit counters and finished segments per tile
     float *ce_rcarry, *ce_tcarry;                                  // fused schedule: running sums handed from segment to segment
     int rseg, tseg;                                                // fused schedule: segments of a row tile's / a class tile's sweep
@@ -930,15 +941,9 @@ HeadWork carve_head(void* base, size_t T, size_t D, size_t C) {
     h.rseg = fused ? ce_row_segments((int)T, (int)C, sm_count()) : 1;
     h.tseg = fused ? ce_table_segments((int)T, (int)C, sm_count()) : 1;
     h.ldl = (int)((C + 7) / 8 * 8);
-    h.xf = c.take<bf16>(T * D * 2);
-    h.stf = c.take<float>(T * 2 * 4);
-    h.dxf = c.take<float>(T * D * 4);
-    h.scal = c.take<float>(64);
+    carve_head_common(c, h, T, D);
     h.logits = fused ? nullptr : c.take<bf16>(T * (size_t)h.ldl * 2);
     h.logits32 = fused ? nullptr : c.take<float>(T * (size_t)h.ldl * 4);
-    h.row_loss = c.take<float>(T * 4);
-    h.shift = c.take<float>(T * 4);
-    h.part_ln = c.take<float>((size_t)2 * row_bwd_grid((int)T) * D * 4);
     const TnSpec spec{nullptr, nullptr, nullptr, (int)C, (int)D, (int)T, h.ldl, (int)D, (int)D};
     h.part_tn = fused ? nullptr : c.take<float>(tn_part_floats(&spec, 1, sm_count()) * 4);
     h.ce_rsched = fused ? c.take<int>((1 + 2 * ((T + 127) / 128)) * 4) : nullptr;
@@ -947,6 +952,15 @@ HeadWork carve_head(void* base, size_t T, size_t D, size_t C) {
     h.ce_tcarry = fused && h.tseg > 1 ? c.take<float>((C + 63) / 64 * 128 * D * 4) : nullptr;
     h.bytes = c.off;
     return h;
+}
+// the prologue of every head entry point: xf = bf16(LayerNorm(x)), stf = the rows' statistics (nullable)
+int head_ln_forward(const float* x, const float* g, const float* b, float eps, bf16* xf, float* stf, int T, int D, cudaStream_t st) {
+    LnFwdArgs a{x, g, b, xf, nullptr, stf, T, D, eps};
+    return with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); });
+}
+// the epilogue of both loss heads: d loss / d LN(x) in h.dxf -> dx, dln_g +=, dln_b +=
+int head_ln_backward(const HeadCommon& h, const float* x, const float* ln_g, float* dx, float* dln_g, float* dln_b, int T, int D, cudaStream_t st) {
+    return ln_backward(LnBwdArgs{h.dxf, x, h.stf, ln_g, nullptr, dx, dln_g, dln_b, T, D, h.part_ln}, st);
 }
 }  // namespace
 
@@ -974,10 +988,7 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
         return 0;
     };
     if (count_aside) GRB_TRY(defer_run(st, count));
-    {
-        LnFwdArgs a{x, ln_g, ln_b, h.xf, nullptr, h.stf, T, D, ln_eps};
-        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
-    }
+    GRB_TRY(head_ln_forward(x, ln_g, ln_b, ln_eps, h.xf, h.stf, T, D, st));
     if (count_aside) GRB_TRY(join_pending(st));
     else GRB_TRY(count(st));
     if (head_fused(D)) {
@@ -985,49 +996,45 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
         // critical path with the deferred schedule)                                                      (hstu.py:137-146)
         CeArgs ca{reinterpret_cast<const long long*>(targets), h.scal, T, C, want_grad ? h.dxf : nullptr, h.shift, h.row_loss, dtable,
                   h.rseg, h.tseg, h.ce_rsched, h.ce_tsched, h.ce_rcarry, h.ce_tcarry};
-        if (D == 64) GRB_CUDA(launch_tc_ce<64>(h.xf, (const bf16*)table_bf16, ca, sm_count(), st));
-        else GRB_CUDA(launch_tc_ce<128>(h.xf, (const bf16*)table_bf16, ca, sm_count(), st));
+        GRB_CUDA(with_ce_dim(D, [&](auto DC) { return launch_tc_ce<DC>(h.xf, (const bf16*)table_bf16, ca, sm_count(), st); }));
         launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
         GRB_CUDA(cudaGetLastError());
         if (!want_grad) return 0;
         GRB_TRY(run_maybe_deferred(st, [&](cudaStream_t s_) -> int {
-            if (D == 64) GRB_CUDA(launch_ce_table<64>(h.xf, (const bf16*)table_bf16, ca, sm_count(), s_));
-            else GRB_CUDA(launch_ce_table<128>(h.xf, (const bf16*)table_bf16, ca, sm_count(), s_));
+            GRB_CUDA(with_ce_dim(D, [&](auto DC) { return launch_ce_table<DC>(h.xf, (const bf16*)table_bf16, ca, sm_count(), s_); }));
             return 0;
         }));
     } else {
-    // logits = xf E^T   (hstu.py:137)
-    GRB_CUDA((launch_tc_gemm<0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, TcEpiF32{nullptr, h.ldl, 1.f}, h.logits32, nullptr, h.ldl,
-                                sm_count(), st)));
-    if (h.ldl / 8 <= 256 * 8)
-        launch_k(ce_fwd_bwd_vec_kernel<8>, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0,
-                 (const float*)h.logits32);
-    else
-        launch_k(ce_fwd_bwd_kernel, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0,
-                 (const float*)h.logits32);
-    GRB_CUDA(cudaGetLastError());
-    launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
-    GRB_CUDA(cudaGetLastError());
-    if (!want_grad) return 0;
-    GRB_CUDA(gemm_nn_f32(h.logits, (const bf16*)table_bf16, h.dxf, nullptr, 1.f, T, D, C, h.ldl, D, st));  // dxf = dlogits E
-    // dE[C,D] += dlogits^T xf: a weight gradient, off the critical path with the deferred schedule
-    TnSpec spec{h.logits, h.xf, dtable, C, D, T, h.ldl, D, D};
-    GRB_TRY(run_maybe_deferred(st, [&](cudaStream_t s_) -> int {
-        GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, s_));
-        return 0;
-    }));
+        // logits = xf E^T   (hstu.py:137)
+        GRB_CUDA((launch_tc_gemm<0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, TcEpiF32{nullptr, h.ldl, 1.f}, h.logits32, nullptr, h.ldl,
+                                    sm_count(), st)));
+        if (h.ldl / 8 <= 256 * 8)
+            launch_k(ce_fwd_bwd_vec_kernel<8>, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0,
+                     (const float*)h.logits32);
+        else
+            launch_k(ce_fwd_bwd_kernel, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0,
+                     (const float*)h.logits32);
+        GRB_CUDA(cudaGetLastError());
+        launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
+        GRB_CUDA(cudaGetLastError());
+        if (!want_grad) return 0;
+        GRB_CUDA(gemm_nn_f32(h.logits, (const bf16*)table_bf16, h.dxf, nullptr, 1.f, T, D, C, h.ldl, D, st));  // dxf = dlogits E
+        // dE[C,D] += dlogits^T xf: a weight gradient, off the critical path with the deferred schedule
+        TnSpec spec{h.logits, h.xf, dtable, C, D, T, h.ldl, D, D};
+        GRB_TRY(run_maybe_deferred(st, [&](cudaStream_t s_) -> int {
+            GRB_CUDA(launch_tc_tn_group(&spec, 1, sm_count(), h.part_tn, s_));
+            return 0;
+        }));
     }
-    return ln_backward(LnBwdArgs{h.dxf, x, h.stf, ln_g, nullptr, dx, dln_g, dln_b, T, D, h.part_ln}, st);
+    return head_ln_backward(h, x, ln_g, dx, dln_g, dln_b, T, D, st);
 }
 
 // ---- sampled-softmax head (tc_sampled_ce.cuh)
 namespace {
-struct SampledWork {
-    bf16* xf; float* stf; float* dxf; float* scal;      // as HeadWork
+struct SampledWork : HeadCommon {
     bf16* Es; float* bias; int* sid;                     // the gathered negatives
-    float *ztgt, *shift, *row_loss, *gtgt;               // per token
+    float *ztgt, *gtgt;                                  // per token
     float* part; int ks;                                 // token-range partial sums of the sub-table gradient
-    float* part_ln;
     int Npad;
     size_t bytes;
 };
@@ -1036,19 +1043,13 @@ SampledWork carve_sampled(void* base, size_t T, size_t D, size_t N) {
     Carver c{static_cast<char*>(base)};
     h.Npad = (int)((N + 63) / 64 * 64);
     h.ks = sce_table_splits((int)T, h.Npad, sm_count());
-    h.xf = c.take<bf16>(T * D * 2);
-    h.stf = c.take<float>(T * 2 * 4);
-    h.dxf = c.take<float>(T * D * 4);
-    h.scal = c.take<float>(64);
+    carve_head_common(c, h, T, D);
     h.Es = c.take<bf16>((size_t)h.Npad * D * 2);
     h.bias = c.take<float>((size_t)h.Npad * 4);
     h.sid = c.take<int>((size_t)h.Npad * 4);
     h.ztgt = c.take<float>(T * 4);
-    h.shift = c.take<float>(T * 4);
-    h.row_loss = c.take<float>(T * 4);
     h.gtgt = c.take<float>(T * 4);
     h.part = c.take<float>((size_t)h.ks * h.Npad * D * 4);
-    h.part_ln = c.take<float>((size_t)2 * row_bwd_grid((int)T) * D * 4);
     h.bytes = c.off;
     return h;
 }
@@ -1078,19 +1079,15 @@ int grb_head_sampled_loss_forward_backward(const float* x, const float* ln_g, co
     SampledWork h = carve_sampled(workspace, T, D, N);
     launch_k(ce_count_kernel, 1, 1024, 0, st, reinterpret_cast<const long long*>(targets), T, h.scal, loss);
     GRB_CUDA(cudaGetLastError());
-    {
-        LnFwdArgs a{x, ln_g, ln_b, h.xf, nullptr, h.stf, T, D, ln_eps};
-        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
-    }
+    GRB_TRY(head_ln_forward(x, ln_g, ln_b, ln_eps, h.xf, h.stf, T, D, st));
     SceArgs sa{reinterpret_cast<const long long*>(targets), reinterpret_cast<const long long*>(negatives), log_q, (const bf16*)table_bf16, h.xf,
                h.scal, T, C, N, h.Npad, D, h.Es, h.bias, h.sid, h.ztgt, h.shift, h.row_loss, h.gtgt, want_grad ? h.dxf : nullptr, h.part, h.ks,
                dtable};
-    if (D == 64) GRB_CUDA(launch_sampled_ce<64>(sa, sm_count(), st));
-    else GRB_CUDA(launch_sampled_ce<128>(sa, sm_count(), st));
+    GRB_CUDA(with_ce_dim(D, [&](auto DC) { return launch_sampled_ce<DC>(sa, sm_count(), st); }));
     launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
     GRB_CUDA(cudaGetLastError());
     if (!want_grad) return 0;
-    return ln_backward(LnBwdArgs{h.dxf, x, h.stf, ln_g, nullptr, dx, dln_g, dln_b, T, D, h.part_ln}, st);
+    return head_ln_backward(h, x, ln_g, dx, dln_g, dln_b, T, D, st);
 }
 
 int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int T, int D, int C,
@@ -1099,10 +1096,7 @@ int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float 
     GRB_REQUIRE(T > 0 && C > 1 && (D == 64 || D == 128 || D == 256), "bad shape T=%d D=%d C=%d", T, D, C);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     HeadWork h = carve_head(workspace, T, D, C);
-    {
-        LnFwdArgs a{x, ln_g, ln_b, h.xf, nullptr, h.stf, T, D, ln_eps};
-        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
-    }
+    GRB_TRY(head_ln_forward(x, ln_g, ln_b, ln_eps, h.xf, h.stf, T, D, st));
     // logits [T, C] fp32, leading dimension C of any parity
     GRB_CUDA((launch_tc_gemm<0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, TcEpiF32Plain{logits, C}, nullptr, nullptr, 0, sm_count(), st)));
     return 0;
@@ -1159,10 +1153,7 @@ int grb_head_topk(const float* x, const float* ln_g, const float* ln_b, float ln
     CUtensorMap tmA, tmB;
     GRB_REQUIRE(make_tmap_bf16(&tmA, w.xf, R, D, D, TC_BK, TC_BM) && make_tmap_bf16(&tmB, table_bf16, C, D, D, TC_BK, TC_BN),
                 "cannot encode the TMA descriptors (driver entry point missing)");
-    {
-        LnFwdArgs a{x, ln_g, ln_b, w.xf, nullptr, nullptr, R, D, ln_eps};
-        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(R), ROW_THREADS, 0, st, a); }));
-    }
+    GRB_TRY(head_ln_forward(x, ln_g, ln_b, ln_eps, w.xf, nullptr, R, D, st));
     if (E > 0) {
         int P = 1;
         while (P < E) P <<= 1;

@@ -6,6 +6,10 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <map>
+#include <mutex>
+#include <utility>
+
 namespace grb {
 
 typedef __nv_bfloat16 bf16;
@@ -72,6 +76,26 @@ inline cudaError_t launch_kc(void (*kern)(KArgs...), dim3 grid, dim3 block, unsi
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
     return launch_kc(kern, grid, block, 1u, smem, st, static_cast<Args&&>(args)...);
+}
+
+// opt in to > 48 KB dynamic shared memory once per (kernel, high-water mark): no runtime call on the steady-state path,
+// in particular none while a CUDA graph is being captured after warm-up.
+template <class Kern>
+inline cudaError_t set_max_smem(Kern k, size_t bytes) {
+    static std::mutex mu;
+    // keyed by (device, kernel address): the attribute is per device.  One map per instantiation, that is per kernel signature.
+    static std::map<std::pair<int, const void*>, size_t> high_water;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& hw = high_water[std::make_pair(dev, reinterpret_cast<const void*>(k))];
+    if (hw < 48 * 1024) hw = 48 * 1024;
+    if (bytes > hw) {
+        cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+        if (e != cudaSuccess) return e;
+        hw = bytes;
+    }
+    return cudaSuccess;
 }
 
 // ----------------------------------------------------------------------------- small math

@@ -16,6 +16,8 @@
 // per SM takes (segment, tile) units from a counter, segment-major, and waits only for the previous segment of its chain.  At
 // 128 x 200 tokens and 12,102 classes on 132 SMs, 200 row tiles x 2 sweeps on whole-sweep units need 4 rounds where 3.03 would
 // do, 190 class tiles 2 where 1.44 would do; ce_segments picks the counts from the shapes and the SM count only.
+// The steps of a tile (shared-memory set-up, producer loads, lane coordinates, online-softmax step, row finish, the table pass's
+// column metadata, warpgroup hand-over) are functions of their own below: the sampled-softmax head (tc_sampled_ce.cuh) is built from the same ones.
 #pragma once
 #include "tc_gemm.cuh"
 
@@ -158,6 +160,124 @@ GRB_DEVINL void ce_accumulate(float (&acc)[D / 2], const float (&G)[32], uint32_
     wgmma_wait<0>();
 }
 
+// A CTA's dynamic shared memory: the stationary tile (128 token rows in a row pass, 64 classes in a table pass), the ring of
+// CE_STAGES streamed 64-row tiles, and their barriers.
+struct CeCta {
+    unsigned char* stat;        // the stationary tile, 1024-byte aligned
+    unsigned char* ring;        // CE_STAGES tiles of CeSmem<D>::CLS_TILE bytes
+    uint64_t *full, *empty;     // per ring stage: the tile has landed / its readers are done with it
+    uint64_t* sfull;            // the stationary tile has landed
+    unsigned char* tail;        // the first byte after the 256 bytes kept for the barriers
+};
+// Every thread of the CTA: carve the shared memory, let thread 0 prefetch the descriptors and initialise the barriers, and wait for
+// the kernel before.  A stage is released by `empty_arrivals` consumer warpgroups: 2 in a row pass, where both read every
+// streamed tile, 1 in a table pass, where they take alternate tiles.
+template <int D>
+GRB_DEVINL CeCta ce_cta_init(unsigned char* raw, int stat_bytes, int empty_arrivals, const CUtensorMap* tmX, const CUtensorMap* tmE) {
+    CeCta cta;
+    cta.stat = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
+    cta.ring = cta.stat + stat_bytes;
+    cta.full = reinterpret_cast<uint64_t*>(cta.ring + CE_STAGES * CeSmem<D>::CLS_TILE);
+    cta.empty = cta.full + CE_STAGES;
+    cta.sfull = cta.full + 2 * CE_STAGES;
+    cta.tail = cta.ring + CE_STAGES * CeSmem<D>::CLS_TILE + 256;
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(tmX);
+        tma_prefetch_desc(tmE);
+        for (int s = 0; s < CE_STAGES; ++s) { mbar_init(&cta.full[s], 1); mbar_init(&cta.empty[s], empty_arrivals); }
+        mbar_init(cta.sfull, 1);
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_wait();
+    return cta;
+}
+// producer: rows row0 .. row0 + ROWS - 1 of tm into the stationary tile
+template <int D, int ROWS>
+GRB_DEVINL void ce_tile_load(const CeCta& cta, const CUtensorMap* tm, int row0) {
+    mbar_expect_tx(cta.sfull, D / 64 * ROWS * 128);
+    for (int b = 0; b < D / 64; ++b) tma_load_2d(cta.stat + b * ROWS * 128, tm, b * 64, row0, cta.sfull);
+}
+// producer: rows row0 .. row0 + 63 of tm into ring stage `stage`, once its readers have released it (`empty_parity`)
+template <int D>
+GRB_DEVINL void ce_ring_load(const CeCta& cta, const CUtensorMap* tm, int row0, int stage, uint32_t empty_parity) {
+    mbar_wait(&cta.empty[stage], empty_parity);
+    mbar_expect_tx(&cta.full[stage], CeSmem<D>::CLS_TILE);
+    for (int b = 0; b < D / 64; ++b) tma_load_2d(cta.ring + stage * CeSmem<D>::CLS_TILE + b * 8192, tm, b * 64, row0, &cta.full[stage]);
+}
+
+// A consumer thread's place in the 64 x 64 accumulator of its warpgroup g (0, 1): S[4 j + 2 i + c] is tile row row(0, i),
+// i = 0, 1, column 8 j + 2 q + c, j = 0 .. 7, c = 0, 1.
+struct CeLane {
+    int g, w, q, lane;
+    bool leader;                // arrives on the ring's `empty` barriers for its warpgroup
+    GRB_DEVINL int row(int base, int i) const { return base + 16 * w + (lane >> 2) + 8 * i; }
+};
+GRB_DEVINL CeLane ce_lane() {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    return CeLane{(warp >> 2) - 1, warp & 3, lane & 3, lane, (threadIdx.x & 127) == 0};
+}
+
+// One 64-column tile of the online softmax of this thread's row i (0, 1): the running maximum m is shared by the quad that holds
+// the row, the exponent sum s is this lane's part.  S is final: masked columns hold -inf.
+GRB_DEVINL void ce_softmax_step(const float (&S)[32], int i, float& m, float& s) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) mx = fmaxf(mx, S[jj * 4 + i * 2 + c]);
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const float mn = fmaxf(m, mx);
+    float acc = s * ex2_fast((m - mn) * CE_L2E);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) acc += ex2_fast((S[jj * 4 + i * 2 + c] - mn) * CE_L2E);
+    s = acc;
+    m = mn;
+}
+// The end of a row's sweep: the quad's exponent sums are added; returns the row's log2-domain shift, lse = log sum_c exp(S_c)
+GRB_DEVINL float ce_row_finish(float m, float s, float& lse) {
+    s += __shfl_xor_sync(0xffffffffu, s, 1);
+    s += __shfl_xor_sync(0xffffffffu, s, 2);
+    lse = m + __logf(s);
+    return m * CE_L2E + __log2f(s);
+}
+
+// A table pass thread's 16 token columns of token tile tt (column kq = 2 j + c is token 64 tt + 8 j + 2 q + c): target, the
+// row's shift and 1 / count.  target(t) reads the target of token t < T; tokens past T and ignored tokens get weight 0.
+struct CeCols {
+    int tg[16];
+    float sh[16], icc[16];
+};
+template <class Target>
+GRB_DEVINL void ce_table_cols(CeCols& k, const CeLane& l, int tt, int T, const float* shift, float inv, Target target) {
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+            const int t = tt * 64 + 8 * jj + 2 * l.q + c;
+            const bool ok = t < T;
+            k.tg[jj * 2 + c] = ok ? target(t) : 0;
+            k.sh[jj * 2 + c] = ok ? shift[t] : 0.f;
+            k.icc[jj * 2 + c] = k.tg[jj * 2 + c] != 0 ? inv : 0.f;
+        }
+}
+// The end of a table pass: warpgroup 2 hands its sums to warpgroup 1 through shared memory (the ring is free by now).  After
+// ce_wg_handover, warpgroup 1 stores acc[kk] + ce_wg_peer(cta, kk): always wg1 + wg2, a fixed order.
+template <int D>
+GRB_DEVINL void ce_wg_handover(const CeCta& cta, const CeLane& l, const float (&acc)[D / 2]) {
+    float* red = reinterpret_cast<float*>(cta.ring);
+    ce_bar(2, 256);                                // both warpgroups are done with the ring
+    if (l.g == 1) {
+#pragma unroll
+        for (int kk = 0; kk < D / 2; ++kk) red[(size_t)kk * 128 + (threadIdx.x & 127)] = acc[kk];
+    }
+    ce_bar(2, 256);
+}
+GRB_DEVINL float ce_wg_peer(const CeCta& cta, int kk) { return reinterpret_cast<const float*>(cta.ring)[(size_t)kk * 128 + (threadIdx.x & 127)]; }
+
 // Unit u: sweep u / (rseg R) (0: statistics, 1: dX), segment k = u / R % rseg, row tile u % R: the class tiles
 // [k ntile / rseg, (k + 1) ntile / rseg) of that row tile, continuing from the running sums segment k - 1 left in global memory.
 template <int D>
@@ -166,29 +286,13 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     using SM = CeSmem<D>;
     extern __shared__ unsigned char ce_smem_raw[];
     __shared__ int unit_slot[2];
-    unsigned char* base = ce_smem_raw + ((1024u - (smem_u32(ce_smem_raw) & 1023u)) & 1023u);
-    unsigned char* sX = base;
-    unsigned char* sE = base + SM::ROW_TILE;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sE + CE_STAGES * SM::CLS_TILE);
-    uint64_t* full = bars;
-    uint64_t* empty = bars + CE_STAGES;
-    uint64_t* xfull = bars + 2 * CE_STAGES;
+    const CeCta cta = ce_cta_init<D>(ce_smem_raw, SM::ROW_TILE, 2, &tmX, &tmE);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmX);
-        tma_prefetch_desc(&tmE);
-        for (int s = 0; s < CE_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-        mbar_init(xfull, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
-    pdl_wait();
     if (warp >= 1 && warp < 4) return;            // warp 0 produces (lane 0 issues the loads), warps 4..11 consume
     const int ntile = (a.C + 63) / 64, R = (a.T + 127) / 128, K = a.rseg;
     const int units = (a.dx ? 2 : 1) * K * R;
-    // consumer warpgroup g: tile rows 64 g .. 64 g + 63 ; this thread: rows r[0], r[1] = r[0] + 8, columns 8 j + 2 q + {0, 1}
-    const int g = (warp >> 2) - 1, w = warp & 3, q = lane & 3;
-    const bool leader = (threadIdx.x & 127) == 0;
+    const CeLane l = ce_lane();                    // consumer warpgroup g: tile rows 64 g .. 64 g + 63
+    const int q = l.q;
     int stage = 0;                                 // the table ring runs on across units
     uint32_t phase = 0;
     for (int n = 0;; ++n) {
@@ -203,12 +307,9 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
         int* xdone = a.rsched + 1 + R + rt;        // dX segments finished
         if (warp == 0) {
             if (lane == 0) {
-                mbar_expect_tx(xfull, SM::ROW_TILE);
-                for (int b = 0; b < SM::XB; ++b) tma_load_2d(sX + b * 16384, &tmX, b * 64, row0, xfull);
+                ce_tile_load<D, 128>(cta, &tmX, row0);
                 for (int j = j0; j < j1; ++j) {
-                    mbar_wait(&empty[stage], phase ^ 1);
-                    mbar_expect_tx(&full[stage], SM::CLS_TILE);
-                    for (int b = 0; b < SM::XB; ++b) tma_load_2d(sE + stage * SM::CLS_TILE + b * 8192, &tmE, b * 64, j * 64, &full[stage]);
+                    ce_ring_load<D>(cta, &tmE, j * 64, stage, phase ^ 1);
                     if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
                 }
             }
@@ -220,12 +321,12 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
         const float inv = *a.inv_count;
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-            row[i] = row0 + 64 * g + 16 * w + (lane >> 2) + 8 * i;
+            row[i] = l.row(row0 + 64 * l.g, i);
             tgt[i] = row[i] < a.T ? (int)a.tg[row[i]] : 0;
             ic[i] = tgt[i] != 0 ? inv : 0.f;
         }
-        mbar_wait(xfull, n & 1);
-        const uint32_t xa = smem_u32(sX) + g * 8192;
+        mbar_wait(cta.sfull, n & 1);
+        const uint32_t xa = smem_u32(cta.stat) + l.g * 8192;
         if (!dxp) {
             if (k > 0) ce_wait_chain(sdone, k);
             float m[2] = {-INFINITY, -INFINITY}, s[2] = {0.f, 0.f}, tl[2] = {0.f, 0.f};
@@ -239,14 +340,14 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
                     tl[i] = __ldcg(a.rcarry + 2 * plane + at);
                 }
             for (int j = j0; j < j1; ++j) {
-                mbar_wait(&full[stage], phase);
+                mbar_wait(&cta.full[stage], phase);
                 float S[32];
-                ce_scores<D>(S, xa, 16384, smem_u32(sE + stage * SM::CLS_TILE));
-                if (leader) mbar_arrive(&empty[stage]);
+                ce_scores<D>(S, xa, 16384, smem_u32(cta.ring + stage * SM::CLS_TILE));
+                if (l.leader) mbar_arrive(&cta.empty[stage]);
                 if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
+                // classes past C leave the softmax; the target's logit is kept
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
-                    float mx = -INFINITY;
 #pragma unroll
                     for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
@@ -255,18 +356,8 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
                             float& v = S[jj * 4 + i * 2 + c];
                             if (col >= a.C) v = -INFINITY;
                             if (col == tgt[i]) tl[i] = v;
-                            mx = fmaxf(mx, v);
                         }
-                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-                    const float mn = fmaxf(m[i], mx);
-                    float acc = s[i] * ex2_fast((m[i] - mn) * CE_L2E);
-#pragma unroll
-                    for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-                        for (int c = 0; c < 2; ++c) acc += ex2_fast((S[jj * 4 + i * 2 + c] - mn) * CE_L2E);
-                    s[i] = acc;
-                    m[i] = mn;
+                    ce_softmax_step(S, i, m[i], s[i]);
                 }
             }
             if (k + 1 < K) {
@@ -281,13 +372,12 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
             } else {
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
-                    s[i] += __shfl_xor_sync(0xffffffffu, s[i], 1);
-                    s[i] += __shfl_xor_sync(0xffffffffu, s[i], 2);
+                    float lse;
+                    const float shift = ce_row_finish(m[i], s[i], lse);
                     tl[i] += __shfl_xor_sync(0xffffffffu, tl[i], 1);
                     tl[i] += __shfl_xor_sync(0xffffffffu, tl[i], 2);
-                    const float shift = m[i] * CE_L2E + __log2f(s[i]);
                     if (q == 0 && row[i] < a.T) {
-                        a.row_loss[row[i]] = tgt[i] != 0 ? (m[i] + __logf(s[i]) - tl[i]) * ic[i] : 0.f;
+                        a.row_loss[row[i]] = tgt[i] != 0 ? (lse - tl[i]) * ic[i] : 0.f;
                         a.shift[row[i]] = shift;
                     }
                 }
@@ -311,9 +401,9 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
                     dx[jj * 4 + i * 2 + 1] = v.y;
                 }
             for (int j = j0; j < j1; ++j) {
-                mbar_wait(&full[stage], phase);
+                mbar_wait(&cta.full[stage], phase);
                 float S[32];
-                const uint32_t e_addr = smem_u32(sE + stage * SM::CLS_TILE);
+                const uint32_t e_addr = smem_u32(cta.ring + stage * SM::CLS_TILE);
                 ce_scores<D>(S, xa, 16384, e_addr);
 #pragma unroll
                 for (int jj = 0; jj < 8; ++jj)
@@ -328,7 +418,7 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
                             v = gv;
                         }
                 ce_accumulate<D>(dx, S, e_addr);
-                if (leader) mbar_arrive(&empty[stage]);
+                if (l.leader) mbar_arrive(&cta.empty[stage]);
                 if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
             }
 #pragma unroll
@@ -350,27 +440,12 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     using SM = CeSmem<D>;
     extern __shared__ unsigned char ce_smem_raw[];
     __shared__ int unit_slot[2];
-    unsigned char* base = ce_smem_raw + ((1024u - (smem_u32(ce_smem_raw) & 1023u)) & 1023u);
-    unsigned char* sE = base;
-    unsigned char* sX = base + SM::CLS_TILE;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sX + CE_STAGES * SM::CLS_TILE);
-    uint64_t* full = bars;
-    uint64_t* empty = bars + CE_STAGES;
-    uint64_t* efull = bars + 2 * CE_STAGES;
+    const CeCta cta = ce_cta_init<D>(ce_smem_raw, SM::CLS_TILE, 1, &tmX, &tmE);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmX);
-        tma_prefetch_desc(&tmE);
-        for (int s = 0; s < CE_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(efull, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
-    pdl_wait();
     if (warp >= 1 && warp < 4) return;
     const int ntt = (a.T + 63) / 64, NC = (a.C + 63) / 64, K = a.tseg;
-    const int g = (warp >> 2) - 1, w = warp & 3, q = lane & 3;
-    const bool leader = (threadIdx.x & 127) == 0;
+    const CeLane l = ce_lane();
+    const int g = l.g, q = l.q;
     uint32_t pos = 0;                              // token tiles this CTA has streamed: the ring position of the unit's first tile
     for (int n = 0;; ++n) {
         if (threadIdx.x == 0) unit_slot[n & 1] = atomicAdd(a.tsched, 1);
@@ -382,50 +457,33 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
         int* done = a.tsched + 1 + ct;
         if (warp == 0) {
             if (lane == 0) {
-                mbar_expect_tx(efull, SM::CLS_TILE);
-                for (int b = 0; b < SM::XB; ++b) tma_load_2d(sE + b * 8192, &tmE, b * 64, cls0, efull);
+                ce_tile_load<D, 64>(cta, &tmE, cls0);
                 // ring position p -> stage p % CE_STAGES
                 for (int tt = t0; tt < t1; ++tt) {
                     const uint32_t p = pos + (tt - t0);
-                    const int stage = p % CE_STAGES;
-                    mbar_wait(&empty[stage], ((p / CE_STAGES) & 1) ^ 1);
-                    mbar_expect_tx(&full[stage], SM::CLS_TILE);
-                    for (int b = 0; b < SM::XB; ++b) tma_load_2d(sX + stage * SM::CLS_TILE + b * 8192, &tmX, b * 64, tt * 64, &full[stage]);
+                    ce_ring_load<D>(cta, &tmX, tt * 64, p % CE_STAGES, ((p / CE_STAGES) & 1) ^ 1);
                 }
             }
             __syncwarp();
             pos += t1 - t0;
             continue;
         }
-        int cls[2];
-#pragma unroll
-        for (int i = 0; i < 2; ++i) cls[i] = cls0 + 16 * w + (lane >> 2) + 8 * i;
+        const int cls[2] = {l.row(cls0, 0), l.row(cls0, 1)};
         const float inv = *a.inv_count;
         float acc[D / 2];
         float* carry = a.tcarry + ((size_t)ct * 2 + g) * (D / 2) * 128 + (threadIdx.x & 127);
         if (k > 0) ce_wait_chain(done, k);
 #pragma unroll
         for (int kk = 0; kk < D / 2; ++kk) acc[kk] = k > 0 ? __ldcg(carry + (size_t)kk * 128) : 0.f;
-        mbar_wait(efull, n & 1);
-        const uint32_t ea = smem_u32(sE);
+        mbar_wait(cta.sfull, n & 1);
+        const uint32_t ea = smem_u32(cta.stat);
         for (int tt = t0 + ((t0 ^ g) & 1); tt < t1; tt += 2) {
             const uint32_t p = pos + (tt - t0);
             const int stage = p % CE_STAGES;
-            // this thread's 16 token columns: shift, target, 1 / count
-            float sh[16], icc[16];
-            int tg[16];
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    const int t = tt * 64 + 8 * jj + 2 * q + c;
-                    const bool ok = t < a.T;
-                    tg[jj * 2 + c] = ok ? (int)a.tg[t] : 0;
-                    sh[jj * 2 + c] = ok ? a.shift[t] : 0.f;
-                    icc[jj * 2 + c] = tg[jj * 2 + c] != 0 ? inv : 0.f;
-                }
-            mbar_wait(&full[stage], (p / CE_STAGES) & 1);
-            const uint32_t x_addr = smem_u32(sX + stage * SM::CLS_TILE);
+            CeCols col;
+            ce_table_cols(col, l, tt, a.T, a.shift, inv, [&](int t) { return (int)a.tg[t]; });
+            mbar_wait(&cta.full[stage], (p / CE_STAGES) & 1);
+            const uint32_t x_addr = smem_u32(cta.ring + stage * SM::CLS_TILE);
             float S[32];
             ce_scores<D>(S, ea, 8192, x_addr);     // S^T: rows = the 64 classes, columns = 64 tokens
 #pragma unroll
@@ -436,12 +494,12 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
                     for (int c = 0; c < 2; ++c) {
                         float& v = S[jj * 4 + i * 2 + c];
                         const int kq = jj * 2 + c;
-                        float gv = ex2_fast(v * CE_L2E - sh[kq]) * icc[kq];
-                        if (cls[i] == tg[kq]) gv -= icc[kq];
+                        float gv = ex2_fast(v * CE_L2E - col.sh[kq]) * col.icc[kq];
+                        if (cls[i] == col.tg[kq]) gv -= col.icc[kq];
                         v = gv;
                     }
             ce_accumulate<D>(acc, S, x_addr);
-            if (leader) mbar_arrive(&empty[stage]);
+            if (l.leader) mbar_arrive(&cta.empty[stage]);
         }
         pos += t1 - t0;
         if (k + 1 < K) {
@@ -450,23 +508,15 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
             ce_finish_segment(done);
             continue;
         }
-        // warpgroup 2 hands its sum to warpgroup 1 through shared memory (the X ring is free by now); fixed order: wg1 + wg2
-        float* red = reinterpret_cast<float*>(sX);
-        ce_bar(2, 256);                            // both warpgroups are done with the ring
-        if (g == 1) {
-#pragma unroll
-            for (int kk = 0; kk < D / 2; ++kk) red[(size_t)kk * 128 + (threadIdx.x & 127)] = acc[kk];
-        }
-        ce_bar(2, 256);
+        ce_wg_handover<D>(cta, l, acc);
         if (g == 0) {
 #pragma unroll
             for (int jj = 0; jj < D / 8; ++jj)
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
-                    const int c = cls0 + 16 * w + (lane >> 2) + 8 * i;
+                    const int c = l.row(cls0, i);
                     const int kk = jj * 4 + i * 2;
-                    const float v0 = acc[kk] + red[(size_t)kk * 128 + (threadIdx.x & 127)];
-                    const float v1 = acc[kk + 1] + red[(size_t)(kk + 1) * 128 + (threadIdx.x & 127)];
+                    const float v0 = acc[kk] + ce_wg_peer(cta, kk), v1 = acc[kk + 1] + ce_wg_peer(cta, kk + 1);
                     if (c < a.C) {
                         float* dst = a.dtable + (size_t)c * D + 8 * jj + 2 * q;
                         atomicAdd(dst, v0);          // one add per element and launch
@@ -477,23 +527,12 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     }
 }
 
-template <int D>
-inline cudaError_t ce_set_smem() {
-    static bool attr_set[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (attr_set[dev & 63]) return cudaSuccess;
-    cudaError_t e = cudaFuncSetAttribute(ce_rows_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, CeSmem<D>::ROWS_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(ce_table_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, CeSmem<D>::TABLE_BYTES);
-    if (e == cudaSuccess) attr_set[dev & 63] = true;
-    return e;
-}
 // loss per row, shift per row and (a.dx != null) d loss / d xf, on at most `ctas` CTAs
 template <int D>
 inline cudaError_t launch_tc_ce(const bf16* xf, const bf16* table, const CeArgs& a, int ctas, cudaStream_t st) {
     CUtensorMap tmX, tmE;
     if (!make_tmap_bf16(&tmX, xf, a.T, D, D, 64, 128) || !make_tmap_bf16(&tmE, table, a.C, D, D, 64, 64)) return cudaErrorInvalidValue;
-    cudaError_t e = ce_set_smem<D>();
+    cudaError_t e = set_max_smem(ce_rows_kernel<D>, CeSmem<D>::ROWS_BYTES);
     if (e != cudaSuccess) return e;
     const int R = (a.T + 127) / 128, units = (a.dx ? 2 : 1) * a.rseg * R;
     e = cudaMemsetAsync(a.rsched, 0, (size_t)(1 + 2 * R) * sizeof(int), st);
@@ -506,7 +545,7 @@ template <int D>
 inline cudaError_t launch_ce_table(const bf16* xf, const bf16* table, const CeArgs& a, int ctas, cudaStream_t st) {
     CUtensorMap tmX, tmE;
     if (!make_tmap_bf16(&tmX, xf, a.T, D, D, 64, 64) || !make_tmap_bf16(&tmE, table, a.C, D, D, 64, 64)) return cudaErrorInvalidValue;
-    cudaError_t e = ce_set_smem<D>();
+    cudaError_t e = set_max_smem(ce_table_kernel<D>, CeSmem<D>::TABLE_BYTES);
     if (e != cudaSuccess) return e;
     const int NC = (a.C + 63) / 64, units = a.tseg * NC;
     e = cudaMemsetAsync(a.tsched, 0, (size_t)(1 + NC) * sizeof(int), st);

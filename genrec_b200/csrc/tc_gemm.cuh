@@ -627,15 +627,8 @@ inline cudaError_t launch_tc_gemm(const bf16* A, const bf16* B, int M, int N, in
     sh.num_n = (N + TC_BN - 1) / TC_BN;
     sh.kblocks_total = (K + TC_BK - 1) / TC_BK;
     auto kern = tc_gemm_kernel<B_MN, Epi>;
-    static bool attr_set_dev[64] = {false};
-    int attr_dev = 0;
-    cudaGetDevice(&attr_dev);
-    bool& attr_set = attr_set_dev[attr_dev & 63];   // the attribute is per device
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES);
-        if (e != cudaSuccess) return e;
-        attr_set = true;
-    }
+    cudaError_t e = set_max_smem(kern, TC_SMEM_BYTES);
+    if (e != cudaSuccess) return e;
     int work = sh.num_m * sh.num_n;
     int grid = work < num_sms ? work : num_sms;
     launch_k(kern, grid, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, tmC0, tmC1, sh, epi);

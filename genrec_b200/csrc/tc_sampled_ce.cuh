@@ -5,18 +5,20 @@
 //   sce_gather_kernel   Es [Npad, D] bf16 = the table rows of the negatives (Npad = N rounded up to the 64-class tile), the
 //                       per-class bias -log_q[s_j] (-inf for padding classes and ids outside 1 .. C-1) and the checked ids.
 //   sce_target_kernel   z_tgt[t] = h_t . E[y_t] - log_q[y_t]: one warp per token, a gather-dot.
-//   sce_rows_kernel     row-stationary, one CTA per 128-token tile (the shape of ce_rows_kernel): the token tile stays in shared
+//   sce_rows_kernel     row-stationary, one CTA per 128-token tile: the token tile stays in shared
 //                       memory and Es streams through a TMA ring twice.  Sweep 1: S = H Es^T + bias, accidental hits (s_j == y_t)
 //                       masked, online maximum / exponent sum starting from the target column -> per-row loss and log2-domain
 //                       shift.  Sweep 2: S again, G in registers -> bf16 A operand of dH += G Es; the target's own term
 //                       g_tgt E[y_t] is added in the epilogue.  N is small, so a row tile's sweep is not cut into segments: one
 //                       unit per row tile, 200 units on 132 SMs at 128 x 200 tokens (two rounds where 1.52 would do).
-//   sce_table_kernel    class-stationary (the shape of ce_table_kernel): CTA (class tile, token range k) sums G^T H over its
+//   sce_table_kernel    class-stationary: CTA (class tile, token range k) sums G^T H over its
 //                       token range into part[k][Npad][D]; the ranges are added in index order by the scatter.
 //   sce_scatter_kernel  dtable[id] += for the negatives and the targets.  CTA p owns the table rows id % P == p: it walks the
 //                       negatives, then the tokens, in index order, keeps the ones it owns, and the first occurrence of an id sums
 //                       all its occurrences in that order.  One writer per table row, no sort, no order-dependent atomics.
-// G is rounded to bf16 for the two wgmma products exactly as in tc_ce.cuh; g_tgt stays fp32.
+// The row and table kernels are built from the tile steps of tc_ce.cuh (ce_cta_init, ce_tile_load / ce_ring_load, ce_lane,
+// ce_softmax_step, ce_row_finish, ce_table_cols, ce_wg_handover), so the ring, the barriers, the softmax arithmetic and the bf16
+// rounding of G for the two wgmma products are the full head's by construction; g_tgt stays fp32.
 #pragma once
 #include "tc_ce.cuh"
 
@@ -96,25 +98,10 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     sce_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmE, SceArgs a) {
     using SM = CeSmem<D>;
     extern __shared__ unsigned char ce_smem_raw[];
-    unsigned char* base = ce_smem_raw + ((1024u - (smem_u32(ce_smem_raw) & 1023u)) & 1023u);
-    unsigned char* sX = base;
-    unsigned char* sE = base + SM::ROW_TILE;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sE + CE_STAGES * SM::CLS_TILE);
-    uint64_t* full = bars;
-    uint64_t* empty = bars + CE_STAGES;
-    uint64_t* xfull = bars + 2 * CE_STAGES;
-    float* sBias = reinterpret_cast<float*>(sE + CE_STAGES * SM::CLS_TILE + 256);
+    const CeCta cta = ce_cta_init<D>(ce_smem_raw, SM::ROW_TILE, 2, &tmX, &tmE);
+    float* sBias = reinterpret_cast<float*>(cta.tail);
     int* sSid = reinterpret_cast<int*>(sBias + a.Npad);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmX);
-        tma_prefetch_desc(&tmE);
-        for (int s = 0; s < CE_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-        mbar_init(xfull, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
-    pdl_wait();
     if (warp >= 1 && warp < 4) return;            // warp 0 produces (lane 0 issues the loads), warps 4..11 consume
     const int ntile = a.Npad / 64, row0 = blockIdx.x * 128;
     const int sweeps = a.dxf ? 2 : 1;
@@ -122,21 +109,16 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     uint32_t phase = 0;
     if (warp == 0) {
         if (lane == 0) {
-            mbar_expect_tx(xfull, SM::ROW_TILE);
-            for (int b = 0; b < SM::XB; ++b) tma_load_2d(sX + b * 16384, &tmX, b * 64, row0, xfull);
+            ce_tile_load<D, 128>(cta, &tmX, row0);
             for (int n = 0; n < sweeps * ntile; ++n) {
-                const int j = n % ntile;
-                mbar_wait(&empty[stage], phase ^ 1);
-                mbar_expect_tx(&full[stage], SM::CLS_TILE);
-                for (int b = 0; b < SM::XB; ++b) tma_load_2d(sE + stage * SM::CLS_TILE + b * 8192, &tmE, b * 64, j * 64, &full[stage]);
+                ce_ring_load<D>(cta, &tmE, n % ntile * 64, stage, phase ^ 1);
                 if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
             }
         }
         return;
     }
-    // consumer warpgroup g: tile rows 64 g .. 64 g + 63 ; this thread: rows r[0], r[1] = r[0] + 8, columns 8 j + 2 q + {0, 1}
-    const int g = (warp >> 2) - 1, w = warp & 3, q = lane & 3;
-    const bool leader = (threadIdx.x & 127) == 0;
+    const CeLane l = ce_lane();                    // consumer warpgroup g: tile rows 64 g .. 64 g + 63
+    const int q = l.q;
     for (int i = threadIdx.x - 128; i < a.Npad; i += 256) {
         sBias[i] = a.bias[i];
         sSid[i] = a.sid[i];
@@ -146,21 +128,21 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     const float inv = *a.inv_count;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-        row[i] = row0 + 64 * g + 16 * w + (lane >> 2) + 8 * i;
+        row[i] = l.row(row0 + 64 * l.g, i);
         tgt[i] = sce_target(a.tg, row[i], a.T, a.C);
         ic[i] = tgt[i] != 0 ? inv : 0.f;
         zt[i] = tgt[i] != 0 ? a.ztgt[row[i]] : 0.f;
     }
     ce_bar(2, 256);
-    mbar_wait(xfull, 0);
-    const uint32_t xa = smem_u32(sX) + g * 8192;
+    mbar_wait(cta.sfull, 0);
+    const uint32_t xa = smem_u32(cta.stat) + l.g * 8192;
     // the softmax starts from the target column (the quad's lane 0 carries its exponent); an accidental hit never enters it
     float m[2] = {zt[0], zt[1]}, s[2] = {q == 0 ? 1.f : 0.f, q == 0 ? 1.f : 0.f};
     for (int j = 0; j < ntile; ++j) {
-        mbar_wait(&full[stage], phase);
+        mbar_wait(&cta.full[stage], phase);
         float S[32];
-        ce_scores<D>(S, xa, 16384, smem_u32(sE + stage * SM::CLS_TILE));
-        if (leader) mbar_arrive(&empty[stage]);
+        ce_scores<D>(S, xa, 16384, smem_u32(cta.ring + stage * SM::CLS_TILE));
+        if (l.leader) mbar_arrive(&cta.empty[stage]);
         if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
@@ -174,32 +156,15 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
             }
         }
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            float mx = -INFINITY;
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-                for (int c = 0; c < 2; ++c) mx = fmaxf(mx, S[jj * 4 + i * 2 + c]);
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-            const float mn = fmaxf(m[i], mx);
-            float acc = s[i] * ex2_fast((m[i] - mn) * CE_L2E);
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-                for (int c = 0; c < 2; ++c) acc += ex2_fast((S[jj * 4 + i * 2 + c] - mn) * CE_L2E);
-            s[i] = acc;
-            m[i] = mn;
-        }
+        for (int i = 0; i < 2; ++i) ce_softmax_step(S, i, m[i], s[i]);
     }
     float shift[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-        s[i] += __shfl_xor_sync(0xffffffffu, s[i], 1);
-        s[i] += __shfl_xor_sync(0xffffffffu, s[i], 2);
-        shift[i] = m[i] * CE_L2E + __log2f(s[i]);
+        float lse;
+        shift[i] = ce_row_finish(m[i], s[i], lse);
         if (q == 0 && row[i] < a.T) {
-            a.row_loss[row[i]] = tgt[i] != 0 ? (m[i] + __logf(s[i]) - zt[i]) * ic[i] : 0.f;
+            a.row_loss[row[i]] = tgt[i] != 0 ? (lse - zt[i]) * ic[i] : 0.f;
             a.shift[row[i]] = shift[i];
         }
     }
@@ -210,9 +175,9 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     for (int kk = 0; kk < D / 2; ++kk) dx[kk] = 0.f;
     float gsum[2] = {0.f, 0.f};                    // sum_j G of the row: g_tgt = (p_tgt - 1) / count = -gsum, without the cancellation
     for (int j = 0; j < ntile; ++j) {
-        mbar_wait(&full[stage], phase);
+        mbar_wait(&cta.full[stage], phase);
         float S[32];
-        const uint32_t e_addr = smem_u32(sE + stage * SM::CLS_TILE);
+        const uint32_t e_addr = smem_u32(cta.ring + stage * SM::CLS_TILE);
         ce_scores<D>(S, xa, 16384, e_addr);
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
@@ -229,7 +194,7 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
             }
         }
         ce_accumulate<D>(dx, S, e_addr);
-        if (leader) mbar_arrive(&empty[stage]);
+        if (l.leader) mbar_arrive(&cta.empty[stage]);
         if (++stage == CE_STAGES) { stage = 0; phase ^= 1; }
     }
 #pragma unroll
@@ -255,71 +220,43 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
     sce_table_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmE, SceArgs a) {
     using SM = CeSmem<D>;
     extern __shared__ unsigned char ce_smem_raw[];
-    unsigned char* base = ce_smem_raw + ((1024u - (smem_u32(ce_smem_raw) & 1023u)) & 1023u);
-    unsigned char* sE = base;
-    unsigned char* sX = base + SM::CLS_TILE;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sX + CE_STAGES * SM::CLS_TILE);
-    uint64_t* full = bars;
-    uint64_t* empty = bars + CE_STAGES;
-    uint64_t* efull = bars + 2 * CE_STAGES;
+    const CeCta cta = ce_cta_init<D>(ce_smem_raw, SM::CLS_TILE, 1, &tmX, &tmE);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmX);
-        tma_prefetch_desc(&tmE);
-        for (int s = 0; s < CE_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(efull, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
-    pdl_wait();
     if (warp >= 1 && warp < 4) return;
     const int ntt = (a.T + 63) / 64, ct = blockIdx.x, k = blockIdx.y, cls0 = ct * 64;
     const int t0 = (int)((long long)k * ntt / a.ks), t1 = (int)((long long)(k + 1) * ntt / a.ks);
     if (warp == 0) {
         if (lane == 0) {
-            mbar_expect_tx(efull, SM::CLS_TILE);
-            for (int b = 0; b < SM::XB; ++b) tma_load_2d(sE + b * 8192, &tmE, b * 64, cls0, efull);
+            ce_tile_load<D, 64>(cta, &tmE, cls0);
             for (int tt = t0; tt < t1; ++tt) {
-                const int p = tt - t0, stage = p % CE_STAGES;
-                mbar_wait(&empty[stage], ((p / CE_STAGES) & 1) ^ 1);
-                mbar_expect_tx(&full[stage], SM::CLS_TILE);
-                for (int b = 0; b < SM::XB; ++b) tma_load_2d(sX + stage * SM::CLS_TILE + b * 8192, &tmX, b * 64, tt * 64, &full[stage]);
+                const int p = tt - t0;
+                ce_ring_load<D>(cta, &tmX, tt * 64, p % CE_STAGES, ((p / CE_STAGES) & 1) ^ 1);
             }
         }
         return;
     }
-    const int g = (warp >> 2) - 1, w = warp & 3, q = lane & 3;
-    const bool leader = (threadIdx.x & 127) == 0;
+    const CeLane l = ce_lane();
+    const int q = l.q;
     int cid[2];
     float cb[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-        const int c = cls0 + 16 * w + (lane >> 2) + 8 * i;
-        cid[i] = a.sid[c];
-        cb[i] = a.bias[c];
+        cid[i] = a.sid[l.row(cls0, i)];
+        cb[i] = a.bias[l.row(cls0, i)];
     }
     const float inv = *a.inv_count;
     float acc[D / 2];
 #pragma unroll
     for (int kk = 0; kk < D / 2; ++kk) acc[kk] = 0.f;
-    mbar_wait(efull, 0);
-    const uint32_t ea = smem_u32(sE);
-    for (int tt = t0 + ((t0 ^ g) & 1); tt < t1; tt += 2) {
-        const int p = tt - t0, stage = p % CE_STAGES;
-        // this thread's 16 token columns: shift, target, 1 / count
-        float sh[16], icc[16];
-        int tg[16];
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                const int t = tt * 64 + 8 * jj + 2 * q + c;
-                tg[jj * 2 + c] = sce_target(a.tg, t, a.T, a.C);
-                sh[jj * 2 + c] = t < a.T ? a.shift[t] : 0.f;
-                icc[jj * 2 + c] = tg[jj * 2 + c] != 0 ? inv : 0.f;
-            }
-        mbar_wait(&full[stage], (p / CE_STAGES) & 1);
-        const uint32_t x_addr = smem_u32(sX + stage * SM::CLS_TILE);
+    mbar_wait(cta.sfull, 0);
+    const uint32_t ea = smem_u32(cta.stat);
+    for (int tt = t0 + ((t0 ^ l.g) & 1); tt < t1; tt += 2) {
+        const int p = tt - t0;
+        const int stage = p % CE_STAGES;
+        CeCols col;
+        ce_table_cols(col, l, tt, a.T, a.shift, inv, [&](int t) { return sce_target(a.tg, t, a.T, a.C); });
+        mbar_wait(&cta.full[stage], (p / CE_STAGES) & 1);
+        const uint32_t x_addr = smem_u32(cta.ring + stage * SM::CLS_TILE);
         float S[32];
         ce_scores<D>(S, ea, 8192, x_addr);     // S^T: rows = the 64 classes, columns = 64 tokens
 #pragma unroll
@@ -330,28 +267,20 @@ __global__ void __launch_bounds__(CE_THREADS, 1)
                 for (int c = 0; c < 2; ++c) {
                     float& v = S[jj * 4 + i * 2 + c];
                     const int kq = jj * 2 + c;
-                    v = cid[i] == tg[kq] ? 0.f : ex2_fast((v + cb[i]) * CE_L2E - sh[kq]) * icc[kq];
+                    v = cid[i] == col.tg[kq] ? 0.f : ex2_fast((v + cb[i]) * CE_L2E - col.sh[kq]) * col.icc[kq];
                 }
         ce_accumulate<D>(acc, S, x_addr);
-        if (leader) mbar_arrive(&empty[stage]);
+        if (l.leader) mbar_arrive(&cta.empty[stage]);
     }
-    // warpgroup 2 hands its sum to warpgroup 1 through shared memory (the X ring is free by now); fixed order: wg1 + wg2
-    float* red = reinterpret_cast<float*>(sX);
-    ce_bar(2, 256);
-    if (g == 1) {
-#pragma unroll
-        for (int kk = 0; kk < D / 2; ++kk) red[(size_t)kk * 128 + (threadIdx.x & 127)] = acc[kk];
-    }
-    ce_bar(2, 256);
-    if (g == 0) {
+    ce_wg_handover<D>(cta, l, acc);
+    if (l.g == 0) {
 #pragma unroll
         for (int jj = 0; jj < D / 8; ++jj)
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
-                const int c = cls0 + 16 * w + (lane >> 2) + 8 * i;
                 const int kk = jj * 4 + i * 2;
-                *reinterpret_cast<float2*>(a.part + ((size_t)k * a.Npad + c) * D + 8 * jj + 2 * q) =
-                    make_float2(acc[kk] + red[(size_t)kk * 128 + (threadIdx.x & 127)], acc[kk + 1] + red[(size_t)(kk + 1) * 128 + (threadIdx.x & 127)]);
+                *reinterpret_cast<float2*>(a.part + ((size_t)k * a.Npad + l.row(cls0, i)) * D + 8 * jj + 2 * q) =
+                    make_float2(acc[kk] + ce_wg_peer(cta, kk), acc[kk + 1] + ce_wg_peer(cta, kk + 1));
             }
     }
 }
@@ -440,18 +369,6 @@ inline int sce_table_splits(int T, int Npad, int sms) {
     return ks < 1 ? 1 : ks;
 }
 
-template <int D>
-inline cudaError_t sce_set_smem() {
-    static bool attr_set[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (attr_set[dev & 63]) return cudaSuccess;
-    cudaError_t e = cudaFuncSetAttribute(sce_rows_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, sce_rows_smem<D>(SCE_MAX_N));
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(sce_table_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, CeSmem<D>::TABLE_BYTES);
-    if (e == cudaSuccess) attr_set[dev & 63] = true;
-    return e;
-}
-
 // the whole sampled head after the LayerNorm forward and the target count: loss per row, dxf, dtable +=
 template <int D>
 inline cudaError_t launch_sampled_ce(const SceArgs& a, int sms, cudaStream_t st) {
@@ -459,7 +376,9 @@ inline cudaError_t launch_sampled_ce(const SceArgs& a, int sms, cudaStream_t st)
     if (!make_tmap_bf16(&tmX128, a.xf, a.T, D, D, 64, 128) || !make_tmap_bf16(&tmX64, a.xf, a.T, D, D, 64, 64) ||
         !make_tmap_bf16(&tmE, a.Es, a.Npad, D, D, 64, 64))
         return cudaErrorInvalidValue;
-    cudaError_t e = sce_set_smem<D>();
+    // the row kernel asks for its largest size once, so no later call with more negatives has to raise the attribute
+    cudaError_t e = set_max_smem(sce_rows_kernel<D>, sce_rows_smem<D>(SCE_MAX_N));
+    if (e == cudaSuccess) e = set_max_smem(sce_table_kernel<D>, CeSmem<D>::TABLE_BYTES);
     if (e != cudaSuccess) return e;
     launch_k(sce_gather_kernel, (a.Npad + 7) / 8, 256, 0, st, a);
     launch_k(sce_target_kernel, (a.T + 7) / 8, 256, 0, st, a);

@@ -230,18 +230,11 @@ inline cudaError_t launch_tc_tn_group(const TnSpec* specs, int n, int num_sms, f
             return cudaErrorInvalidValue;
     }
     const int work = P.total_work;
-    static bool attr_set_dev[64] = {false};
-    int attr_dev = 0;
-    cudaGetDevice(&attr_dev);
-    bool& attr_set = attr_set_dev[attr_dev & 63];   // the attribute is per device
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(tc_tn_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TN_SMEM_BYTES);
-        if (e != cudaSuccess) return e;
-        attr_set = true;
-    }
+    cudaError_t e = set_max_smem(tc_tn_group_kernel, TN_SMEM_BYTES);
+    if (e != cudaSuccess) return e;
     int grid = work < num_sms ? work : num_sms;
     launch_k(tc_tn_group_kernel, grid, TC_THREADS, TN_SMEM_BYTES, st, P);
-    cudaError_t e = cudaGetLastError();
+    e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     int tiles = 0;
     for (int i = 0; i < n; ++i)

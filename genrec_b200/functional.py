@@ -260,6 +260,37 @@ class EmbedFn(torch.autograd.Function):
         return None, dtable, dpos, None, None, None, None, None, None
 
 
+def _head_grad_buffers(ctx, xc, ln_g, ln_b, table, sink, unit_loss_grad):
+    """-> (dx, dg, db, dtable, direct) for a loss head's forward: the sink's views when the kernels may add straight into it
+    (``direct``), fresh zeroed tensors when gradients are needed otherwise, ``None``s for a loss-only call."""
+    need_grad = any(ctx.needs_input_grad[:4])
+    direct = need_grad and sink is not None and unit_loss_grad
+    ctx.sink, ctx.direct = sink, direct
+    if direct:
+        return (torch.empty_like(xc), *sink, True)
+    if not need_grad:
+        return None, None, None, None, False
+    return (torch.empty_like(xc), torch.zeros_like(ln_g, dtype=torch.float32), torch.zeros_like(ln_b, dtype=torch.float32),
+            torch.zeros(table.shape, dtype=torch.float32, device=xc.device), False)
+
+
+def _head_loss_backward(ctx, dloss, n_inputs):
+    """backward of both loss heads: ``ctx.grads`` scaled by ``dloss`` (see ``HeadLossFn``), ``None`` for the other inputs."""
+    dx, dg, db, dtable = ctx.grads
+    ctx.grads = None
+    if dx is None:
+        return (None,) * n_inputs
+    if ctx.direct:
+        with torch.cuda.device(dx.device):
+            check(_lib.load().grb_assert_unit_scalar(ptr(dloss.detach().float().contiguous()), stream_ptr(dx.device)))
+        return (dx,) + (None,) * (n_inputs - 1)
+    if ctx.sink is not None:
+        sg, sb, st = ctx.sink
+        sg.add_(dg * dloss); sb.add_(db * dloss); st.addcmul_(dtable, dloss)
+        return (dx * dloss,) + (None,) * (n_inputs - 1)
+    return (dx * dloss, dg * dloss, db * dloss, dtable * dloss) + (None,) * (n_inputs - 4)
+
+
 class HeadLossFn(torch.autograd.Function):
     """loss = CE(LN(x) @ E^T, targets, ignore_index=0).  The fused kernel produces the gradients in the same pass as the loss;
     ``backward`` scales them by the incoming gradient of the loss.
@@ -282,21 +313,9 @@ class HeadLossFn(torch.autograd.Function):
         T, Cn = B * L, table.shape[0]
         xc = x.detach().contiguous().float()
         tg = targets.contiguous()
-        need_grad = any(ctx.needs_input_grad[:4])
-        direct = need_grad and sink is not None and unit_loss_grad
-        ctx.sink, ctx.direct = sink, direct
+        dx, dg, db, dtable, direct = _head_grad_buffers(ctx, xc, ln_g, ln_b, table, sink, unit_loss_grad)
         loss = torch.empty((), dtype=torch.float32, device=x.device)   # zeroed on the device by the target-count kernel
         ws = _u8(lib.grb_head_workspace_bytes(T, D, Cn), x.device)
-        if direct:
-            dx = torch.empty_like(xc)
-            dg, db, dtable = sink
-        elif need_grad:
-            dx = torch.empty_like(xc)
-            dtable = torch.zeros(table.shape, dtype=torch.float32, device=x.device)
-            dg = torch.zeros_like(ln_g, dtype=torch.float32)
-            db = torch.zeros_like(ln_b, dtype=torch.float32)
-        else:
-            dx = dtable = dg = db = None
         deferred = _defer_for_call(_DEFER["on"] and direct)
         with torch.cuda.device(x.device):
             check(lib.grb_head_loss_forward_backward(ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), ptr(tg),
@@ -309,19 +328,7 @@ class HeadLossFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dloss):
-        dx, dg, db, dtable = ctx.grads
-        ctx.grads = None
-        if dx is None:
-            return (None,) * 9
-        if ctx.direct:
-            with torch.cuda.device(dx.device):
-                check(_lib.load().grb_assert_unit_scalar(ptr(dloss.detach().float().contiguous()), stream_ptr(dx.device)))
-            return dx, None, None, None, None, None, None, None, None
-        if ctx.sink is not None:
-            sg, sb, st = ctx.sink
-            sg.add_(dg * dloss); sb.add_(db * dloss); st.addcmul_(dtable, dloss)
-            return dx * dloss, None, None, None, None, None, None, None, None
-        return dx * dloss, dg * dloss, db * dloss, dtable * dloss, None, None, None, None, None
+        return _head_loss_backward(ctx, dloss, 9)
 
 
 def head_sampled_loss_raw(x, ln_g, ln_b, table_bf16, targets, negatives, log_q, eps, grads=None):
@@ -363,41 +370,17 @@ class SampledHeadLossFn(torch.autograd.Function):
     def forward(ctx, x, ln_g, ln_b, table, table_bf16, targets, negatives, log_q, eps, sink=None, unit_loss_grad=False):
         require_f32(table)
         B, L, D = x.shape
-        xc = x.detach().contiguous().float().view(B * L, D)
+        xc = x.detach().contiguous().float()
         tg = targets.contiguous().view(-1)
-        need_grad = any(ctx.needs_input_grad[:4])
-        direct = need_grad and sink is not None and unit_loss_grad
-        ctx.sink, ctx.direct, ctx.xshape = sink, direct, x.shape
-        if direct:
-            dx = torch.empty_like(xc)
-            dg, db, dtable = sink
-        elif need_grad:
-            dx = torch.empty_like(xc)
-            dtable = torch.zeros(table.shape, dtype=torch.float32, device=x.device)
-            dg = torch.zeros_like(ln_g, dtype=torch.float32)
-            db = torch.zeros_like(ln_b, dtype=torch.float32)
-        else:
-            dx = dtable = dg = db = None
-        loss = head_sampled_loss_raw(xc, ln_g, ln_b, table_bf16, tg, negatives, log_q, eps, (dx, dtable, dg, db) if need_grad else None)
+        dx, dg, db, dtable, _ = _head_grad_buffers(ctx, xc, ln_g, ln_b, table, sink, unit_loss_grad)
+        loss = head_sampled_loss_raw(xc.view(B * L, D), ln_g, ln_b, table_bf16, tg, negatives, log_q, eps,
+                                     (dx.view(B * L, D), dtable, dg, db) if dx is not None else None)
         ctx.grads = (dx, dg, db, dtable)
         return loss
 
     @staticmethod
     def backward(ctx, dloss):
-        dx, dg, db, dtable = ctx.grads
-        ctx.grads = None
-        if dx is None:
-            return (None,) * 11
-        dx = dx.view(ctx.xshape)
-        if ctx.direct:
-            with torch.cuda.device(dx.device):
-                check(_lib.load().grb_assert_unit_scalar(ptr(dloss.detach().float().contiguous()), stream_ptr(dx.device)))
-            return (dx,) + (None,) * 10
-        if ctx.sink is not None:
-            sg, sb, st = ctx.sink
-            sg.add_(dg * dloss); sb.add_(db * dloss); st.addcmul_(dtable, dloss)
-            return (dx * dloss,) + (None,) * 10
-        return (dx * dloss, dg * dloss, db * dloss, dtable * dloss) + (None,) * 7
+        return _head_loss_backward(ctx, dloss, 11)
 
 
 def head_logits(x, ln_g, ln_b, table, table_bf16, eps) -> torch.Tensor:
