@@ -146,6 +146,9 @@ SIGNATURES = {
     "grb_cast_f32_to_bf16": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
     "grb_adam_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_float, c_float,
                               c_float, c_float, c_float, c_float, c_int, c_void_p]),
+    "grb_rowset_mark": (c_int, [c_void_p, c_size_t, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_rowset_mark_all": (c_int, [c_void_p, c_void_p]),
+    "grb_adam_step_lazy_table": (c_int, [c_void_p] * 5 + [c_size_t, c_size_t, c_int, c_int] + [c_void_p] * 5 + [c_float] * 6 + [c_void_p]),
     "grb_assert_unit_scalar": (c_int, [c_void_p, c_void_p]),
     "grb_dp_adam_step": (c_int, [c_void_p] * 14 + [c_size_t, c_int, c_int, c_void_p, c_float, c_float, c_float, c_float, c_float, c_float,
                                  c_void_p]),

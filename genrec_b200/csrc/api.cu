@@ -19,6 +19,7 @@
 #include "dp_adam.cuh"
 #include "exact_f32.cuh"
 #include "head_topk.cuh"
+#include "lazy_adam.cuh"
 #include "rowwise.cuh"
 #include "rq_argmin.cuh"
 #include "rq_sinkhorn.cuh"
@@ -1581,6 +1582,56 @@ int grb_adam_step(float* p, float* g, float* m, float* v, void* p_bf16, size_t n
     if (n == 0) return 0;
     AdamArgs a{p, g, m, v, (bf16*)p_bf16, n, state, lr, beta1, beta2, eps, weight_decay, grad_scale, zero_grad};
     launch_k(adam_step_kernel, capped_blocks(n), 256, 0, st, a);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int grb_rowset_mark(const int64_t* ids, size_t n, int C, int32_t* flag, int32_t* rows, int32_t* count, void* stream) {
+    GRB_REQUIRE((ids || n == 0) && flag && rows && count, "null argument");
+    GRB_REQUIRE(C >= 2, "bad table size C=%d (C >= 2)", C);
+    if (n == 0) return 0;
+    launch_k(rowset_mark_kernel, capped_blocks(n), 256, 0, static_cast<cudaStream_t>(stream), reinterpret_cast<const long long*>(ids), n, C,
+             flag, rows, count);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+int grb_rowset_mark_all(int32_t* all_word, void* stream) {
+    GRB_REQUIRE(all_word, "null argument");
+    launch_k(rowset_mark_all_kernel, 1, 1, 0, static_cast<cudaStream_t>(stream), all_word);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+int grb_adam_step_lazy_table(float* p, float* g, float* m, float* v, void* p_bf16, size_t n, size_t table_off, int C, int D, int32_t* flag,
+                             const int32_t* rows, int32_t* count, int32_t* all_word, float* state, float lr, float beta1, float beta2, float eps,
+                             float weight_decay, float grad_scale, void* stream) {
+    GRB_REQUIRE(p && g && m && v && p_bf16 && flag && rows && count && all_word && state, "null argument");
+    GRB_REQUIRE(C >= 2, "bad table size C=%d (C >= 2)", C);
+    GRB_REQUIRE(D == 64 || D == 128 || D == 256, "table width D=%d unsupported (64, 128, 256)", D);
+    const size_t hi = table_off + (size_t)C * D;
+    GRB_REQUIRE(hi <= n, "table slot [%zu, %zu) lies outside the flat buffer [0, %zu)", table_off, hi, n);
+    GRB_REQUIRE(aligned16(p + table_off) && aligned16(g + table_off) && aligned16(m + table_off) && aligned16(v + table_off) &&
+                    (reinterpret_cast<uintptr_t>(static_cast<bf16*>(p_bf16) + table_off) & 7) == 0,
+                "the table slot must start 16-byte aligned (8 bytes in the bf16 mirror)");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    launch_k(adam_tick_kernel, 1, 1, 0, st, state, beta1, beta2);
+    GRB_CUDA(cudaGetLastError());
+    // every parameter outside the table: the dense kernel, as grb_adam_step runs it, over [0, table_off) and [hi, n)
+    bf16* pb = static_cast<bf16*>(p_bf16);
+    for (const size_t lo : {(size_t)0, hi}) {
+        const size_t len = lo == 0 ? table_off : n - hi;
+        if (len == 0) continue;
+        AdamArgs a{p + lo, g + lo, m + lo, v + lo, pb + lo, len, state, lr, beta1, beta2, eps, weight_decay, grad_scale, 1};
+        launch_k(adam_step_kernel, capped_blocks(len), 256, 0, st, a);
+        GRB_CUDA(cudaGetLastError());
+    }
+    const size_t o = table_off;
+    LazyTableArgs a{p + o, g + o, m + o, v + o, pb + o, C, flag, rows, count, all_word, state, lr, beta1, beta2, eps, weight_decay, grad_scale};
+    const unsigned blocks = (unsigned)sm_count() * 8;     // fixed: the row count is only known on the device
+    if (D == 64) launch_k(lazy_table_step_kernel<16>, blocks, 256, 0, st, a);
+    else if (D == 128) launch_k(lazy_table_step_kernel<32>, blocks, 256, 0, st, a);
+    else launch_k(lazy_table_step_kernel<64>, blocks, 256, 0, st, a);
+    GRB_CUDA(cudaGetLastError());
+    launch_k(rowset_reset_kernel, 1, 1, 0, st, count, all_word);
     GRB_CUDA(cudaGetLastError());
     return 0;
 }

@@ -935,6 +935,17 @@ struct AdamArgs {
     float lr, beta1, beta2, eps, weight_decay, grad_scale;
     int zero_grad;
 };
+// One element of the step: p, and m / v in place, from the raw gradient g.  adam_step_kernel and the lazy table step
+// (lazy_adam.cuh) both call it, so an element gets the same bits from either.
+GRB_DEVINL float adam_update(float p, float g, float& m, float& v, float grad_scale, float beta1, float beta2, float eps,
+                             float weight_decay, float step_size, float inv_sqrt_bc2) {
+    g *= grad_scale;
+    if (weight_decay != 0.f) g += weight_decay * p;
+    m = beta1 * m + (1.f - beta1) * g;
+    v = beta2 * v + (1.f - beta2) * g * g;
+    float denom = sqrtf(v) * inv_sqrt_bc2 + eps;
+    return p - step_size * (m / denom);
+}
 __global__ void adam_step_kernel(AdamArgs a) {
     pdl_wait();
     const float bc1 = a.state[1], bc2 = a.state[2];
@@ -943,14 +954,10 @@ __global__ void adam_step_kernel(AdamArgs a) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     size_t stride = (size_t)gridDim.x * blockDim.x;
     for (; i < a.n; i += stride) {
-        float p = a.p[i], g = a.g[i] * a.grad_scale;
-        if (a.weight_decay != 0.f) g += a.weight_decay * p;
-        float m = a.beta1 * a.m[i] + (1.f - a.beta1) * g;
-        float v = a.beta2 * a.v[i] + (1.f - a.beta2) * g * g;
+        float m = a.m[i], v = a.v[i];
+        const float p = adam_update(a.p[i], a.g[i], m, v, a.grad_scale, a.beta1, a.beta2, a.eps, a.weight_decay, step_size, inv_sqrt_bc2);
         a.m[i] = m;
         a.v[i] = v;
-        float denom = sqrtf(v) * inv_sqrt_bc2 + a.eps;
-        p -= step_size * (m / denom);
         a.p[i] = p;
         if (a.p_bf16) a.p_bf16[i] = __float2bfloat16(p);
         if (a.zero_grad) a.g[i] = 0.f;

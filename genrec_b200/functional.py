@@ -835,3 +835,26 @@ def adam_step(p, g, m, v, p_bf16, state, lr, beta1, beta2, eps, weight_decay, gr
     with torch.cuda.device(p.device):
         check(_lib.load().grb_adam_step(ptr(p), ptr(g), ptr(m), ptr(v), ptr(p_bf16), p.numel(), ptr(state), lr, beta1, beta2, eps, weight_decay,
                                         grad_scale, int(zero_grad), stream_ptr(p.device)))
+
+
+def rowset_mark(ids, C, flag, rows, count):
+    """Add the ids in 1 .. C-1 of ``ids`` (int64, any shape, on the device) to the row set ``(flag, rows, count)`` (csrc/lazy_adam.cuh)."""
+    require_cuda(ids)
+    require_i64(ids)
+    ids = ids.contiguous()
+    with torch.cuda.device(ids.device):
+        check(_lib.load().grb_rowset_mark(ptr(ids), ids.numel(), C, ptr(flag), ptr(rows), ptr(count), stream_ptr(ids.device)))
+
+
+def rowset_mark_all(all_word):
+    with torch.cuda.device(all_word.device):
+        check(_lib.load().grb_rowset_mark_all(ptr(all_word), stream_ptr(all_word.device)))
+
+
+def adam_step_lazy_table(p, g, m, v, p_bf16, table_off, C, D, flag, rows, count, all_word, state, lr, beta1, beta2, eps, weight_decay,
+                         grad_scale=1.0):
+    """``adam_step`` with the table slot [table_off, table_off + C * D) updated on the rows of the row set only; empties the set."""
+    with torch.cuda.device(p.device):
+        check(_lib.load().grb_adam_step_lazy_table(ptr(p), ptr(g), ptr(m), ptr(v), ptr(p_bf16), p.numel(), table_off, C, D, ptr(flag), ptr(rows),
+                                                   ptr(count), ptr(all_word), ptr(state), lr, beta1, beta2, eps, weight_decay, grad_scale,
+                                                   stream_ptr(p.device)))

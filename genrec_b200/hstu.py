@@ -396,6 +396,7 @@ class HSTU(nn.Module):
         self._bf16_provider = None
         self._grad_sink = None
         self._unit_loss_grad = False   # FlatAdam(unit_loss_grad=True): head gradients go straight into the flat buffer (see HeadLossFn)
+        self._row_marker = None        # set by FlatAdam(lazy_table=True): training forwards mark the item-table rows they touch
         self._step_seed = 0
         self._seed_dev = None  # device uint64 counter, bumped once per training forward (CUDA-graph-safe dropout reseeding)
         self._init_weights()
@@ -448,6 +449,10 @@ class HSTU(nn.Module):
         # training-mode forward has bumped the counter in between
         return self._step_seed, self._seed_dev.clone()
 
+    def _marks_rows(self) -> bool:
+        """A training forward under FlatAdam(lazy_table=True): the gradient sink is set and grad is enabled (as for esink / hsink)."""
+        return self._row_marker is not None and self._grad_sink is not None and torch.is_grad_enabled()
+
     def encode(self, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor]) -> torch.Tensor:
         """Embedding + all blocks (everything before final_norm).  hstu.py:117-132."""
         require_cuda(input_ids)
@@ -459,6 +464,8 @@ class HSTU(nn.Module):
         if self._grad_sink is not None and torch.is_grad_enabled():
             esink = (self._grad_sink(self.item_embedding.weight), None)
         x, pad = Fn.EmbedFn.apply(input_ids, self.item_embedding.weight, None, 1.0, 0, p, seed, seed_dev, esink)
+        if self._marks_rows():
+            self._row_marker._mark(input_ids)
         if len(self.layers):
             meta = self.layers[0]._seq_meta(pad, timestamps, L, input_ids.device)
             for layer in self.layers:
@@ -494,9 +501,14 @@ class HSTU(nn.Module):
             if negatives is not None:
                 loss = Fn.SampledHeadLossFn.apply(x, self.final_norm.weight, self.final_norm.bias, table, table_bf16, targets, negatives,
                                                   log_q, self.final_norm.eps, hsink, self._unit_loss_grad)
+                if self._marks_rows():
+                    self._row_marker._mark(targets)
+                    self._row_marker._mark(negatives)
                 return None, loss
             loss = Fn.HeadLossFn.apply(x, self.final_norm.weight, self.final_norm.bias, table, table_bf16, targets,
                                        self.final_norm.eps, hsink, self._unit_loss_grad)
+            if self._marks_rows():
+                self._row_marker._mark_all()       # the full softmax writes a gradient into every row, 0 included
         if targets is None or not self.training or self.return_train_logits:
             logits = Fn.head_logits(x, self.final_norm.weight, self.final_norm.bias, table, table_bf16, self.final_norm.eps)
         return logits, loss

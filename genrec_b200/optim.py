@@ -113,14 +113,26 @@ class PeerMemory:
 class FlatAdam:
     def __init__(self, model: torch.nn.Module, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, process_group=None, grad_sink: bool = True, unit_loss_grad: bool = False,
-                 peer_memory: Optional[bool] = None, defer_weight_grads: bool = False):
-        """``unit_loss_grad=True`` promises that every training forward is followed by exactly one ``loss.backward()`` with
+                 peer_memory: Optional[bool] = None, defer_weight_grads: bool = False, lazy_table: bool = False):
+        """``lazy_table=True`` updates only the rows of the HSTU item table that the step touched (lazy Adam); every other
+        parameter follows the dense rule.  The touched rows of a step are the union, over every training forward since the last
+        ``step()`` (grad enabled), of the input ids, the targets and the negatives that lie in 1 .. C-1: exactly the rows the
+        embedding backward and the sampled head can write a gradient into.  A forward with the full head (no ``negatives``)
+        touches every row 0 .. C-1.  A touched row gets this optimizer's per-element rule bit for bit (global step count and bias
+        corrections included); an untouched row keeps its parameters, moments and mirror.  The marks accumulate over several
+        forward / backward passes, and a training forward that is never back-propagated still marks its rows, which then step with
+        a zero gradient.  Unlike ``torch.optim.SparseAdam`` / LazyAdam (``lr sqrt(bc2) / bc1 * m / (sqrt(v) + eps)``) the update
+        is ``lr / bc1 * m / (sqrt(v) / sqrt(bc2) + eps)``, the dense rule; the two agree at eps = 0.  The table gradient stays a
+        dense slot of the flat buffer (zero after every step); the step's work over it follows the touched rows.  Needs exactly
+        one HSTU in ``model``, one process and the gradient sink; checkpoints are interchangeable with the dense optimizer's.
+        ``unit_loss_grad=True`` promises that every training forward is followed by exactly one ``loss.backward()`` with
         gradient 1 (no loss scaling, no gradient accumulation through a scaled loss): the fused head then accumulates its
         parameter gradients into the flat buffer in the same pass that computes the loss.  The promise is checked on the
         device (``grb_assert_unit_scalar``).  Default False: fully general, a few microseconds slower per step.
         ``defer_weight_grads=True`` moves the dW / dE GEMMs of the backward pass to a side stream that ``step()`` joins (they are not
         on the critical path); anything else that reads ``.grad`` / the flat gradient before ``step()`` must call
         ``sync_grads()`` first.  Process-wide switch (``grb_set_defer_weight_grads``)."""
+        lazy_owner = self._lazy_table_owner(model, process_group, grad_sink) if lazy_table else None
         dev0 = next(p for p in model.parameters() if p.requires_grad).device
         assert dev0.type == "cuda", "FlatAdam drives CUDA kernels; move the model to the GPU first"
         # data-parallel step: one pass over NVLink peer memory (multimem reduce + Adam + multicast parameter store, csrc/dp_adam.cuh)
@@ -167,6 +179,39 @@ class FlatAdam:
         if defer_weight_grads:
             assert grad_sink, "deferred weight gradients need the gradient sink (nothing but this optimizer consumes them)"
             Fn.set_defer_weight_grads(True)
+        self.lazy_table = lazy_owner is not None
+        if self.lazy_table:
+            table = lazy_owner.item_embedding.weight
+            self._table_rows, self._table_dim = table.shape
+            self._table_off = self.buffers.offsets[next(i for i, p in enumerate(self.params) if p is table)]
+            # the row set of the next step (csrc/lazy_adam.cuh): flags, the list of flagged rows, its length and the "every row" word
+            self._row_flag = torch.zeros(self._table_rows, dtype=torch.int32, device=dev)
+            self._row_list = torch.zeros(self._table_rows, dtype=torch.int32, device=dev)
+            self._row_count = torch.zeros(2, dtype=torch.int32, device=dev)    # [0] = count, [1] = all
+            lazy_owner._row_marker = self
+
+    @staticmethod
+    def _lazy_table_owner(model: torch.nn.Module, process_group, grad_sink: bool):
+        """The one HSTU whose item table FlatAdam(lazy_table=True) updates lazily; ValueError for the cases it does not cover."""
+        from .hstu import HSTU
+        owners = [mod for mod in model.modules() if isinstance(mod, HSTU)]
+        if len(owners) != 1:
+            raise ValueError(f"lazy_table=True needs exactly one HSTU in the model, found {len(owners)}")
+        if world_size(process_group) > 1:
+            raise ValueError("lazy_table=True runs in one process; data-parallel lazy updates are not supported")
+        if not grad_sink:
+            raise ValueError("lazy_table=True needs grad_sink=True: the table gradient must land in the flat buffer")
+        if not owners[0].item_embedding.weight.requires_grad:
+            raise ValueError("lazy_table=True: the HSTU item table is frozen (requires_grad=False)")
+        return owners[0]
+
+    def _mark(self, ids: torch.Tensor) -> None:
+        """Add the table rows named by ``ids`` (ids outside 1 .. C-1 are ignored) to the next step's row set."""
+        Fn.rowset_mark(ids, self._table_rows, self._row_flag, self._row_list, self._row_count[0:1])
+
+    def _mark_all(self) -> None:
+        """Make the next step update every table row."""
+        Fn.rowset_mark_all(self._row_count[1:2])
 
     def mirror_of(self, p: torch.Tensor) -> torch.Tensor:
         return self.buffers.mirror_of(p)
@@ -205,6 +250,11 @@ class FlatAdam:
                     self._mc[2] or None, ptr(pg), ptr(pp), ptr(pmir), ptr(psig), ptr(self._sig), ptr(self._epoch), self.n, self.peer.rank,
                     self.peer.world, ptr(self.state), self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay,
                     1.0 / self.peer.world, stream_ptr(self.flat.device)))
+            return
+        if self.lazy_table:
+            Fn.adam_step_lazy_table(self.flat, self.grad, self.m, self.v, self.mirror, self._table_off, self._table_rows, self._table_dim,
+                                    self._row_flag, self._row_list, self._row_count[0:1], self._row_count[1:2], self.state, self.lr,
+                                    self.betas[0], self.betas[1], self.eps, self.weight_decay)
             return
         scale = allreduce_gradients(self.buffers, self.group)
         Fn.adam_step(self.flat, self.grad, self.m, self.v, self.mirror, self.state, self.lr, self.betas[0], self.betas[1],

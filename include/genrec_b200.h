@@ -372,6 +372,21 @@ int grb_cast_f32_to_bf16(const float* in, void* out_bf16, size_t n, void* stream
 int grb_adam_step(float* p, float* g, float* m, float* v, void* p_bf16, size_t n, float* state, float lr, float beta1,
                   float beta2, float eps, float weight_decay, float grad_scale, int zero_grad, void* stream);
 
+/* Lazy Adam over the rows of one table a step touched.  A row set is flag [C] int32 (zeroed once), rows [C] int32, count (1 int32,
+ * zeroed once) and all_word (1 int32, zeroed once); all are read and reset on the device, so the calls can be captured.
+ *   grb_rowset_mark:     add every id in 1 .. C-1 of ids [n] (int64) to the set: flag[id] = 1, newly flagged ids appended to rows
+ *                        (in an order that depends on timing), count = their number.  Other ids are ignored.
+ *   grb_rowset_mark_all: make the next step update every row 0 .. C-1.
+ *   grb_adam_step_lazy_table: tick state once, grb_adam_step's update (zero_grad = 1) over [0, table_off) and
+ *                        [table_off + C*D, n), then the same per-element update, bf16 mirror and gradient zeroing on the rows of the
+ *                        set only, inside the table slot [table_off, table_off + C*D) of p, g, m, v, p_bf16 (row-major [C, D],
+ *                        D = 64 / 128 / 256, 16-byte aligned).  The other rows keep p, m, v and mirror bits.  Empties the set. */
+int grb_rowset_mark(const int64_t* ids, size_t n, int C, int32_t* flag, int32_t* rows, int32_t* count, void* stream);
+int grb_rowset_mark_all(int32_t* all_word, void* stream);
+int grb_adam_step_lazy_table(float* p, float* g, float* m, float* v, void* p_bf16, size_t n, size_t table_off, int C, int D, int32_t* flag,
+                             const int32_t* rows, int32_t* count, int32_t* all_word, float* state, float lr, float beta1, float beta2, float eps,
+                             float weight_decay, float grad_scale, void* stream);
+
 /* Device-side contract check: traps (asynchronous CUDA error at the next synchronisation) unless *value == 1.0f.  Used by the
  * opt-in "unit loss gradient" fast path, where parameter gradients are accumulated into the flat buffer before the incoming
  * gradient of the loss is known. */

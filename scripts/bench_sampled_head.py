@@ -6,8 +6,10 @@
   2. the time of each kernel of the sampled head (torch.profiler, a run of its own), and for the row pass the least time the
      hardware could take: the larger of 6 T D (N + 1) FLOP at 989 TFLOP/s and the bytes it must move at 3.35 TB/s (data-sheet
      figures of the H100 SXM at 700 W);
-  3. one training step of HSTU at the cfg2 geometry with V = 1,000,000 items and N = 1,024 under FlatAdam, and the part of it the
-     optimizer's pass over the flat buffer (the dense table is nearly all of it) takes.
+  3. one training step of HSTU at the cfg2 geometry with V = 1,000,000 and 10,000,000 items and N = 1,024 under FlatAdam, dense and
+     with lazy_table=True alternated, and the optimizer's part of it (the dense table is nearly all the parameters); the lazy
+     kernels' times under torch.profiler and the lazy table pass against its byte bound (34 B per touched element at 3.35 TB/s).
+     --skip-head runs this part only.
 A GPU is required; there is no fallback.  The card's name and power limit are read in the same run and printed with the numbers."""
 import argparse
 import json
@@ -138,14 +140,43 @@ def per_kernel(dev, T, res):
         res[f"row pass bound D={D} T={T} N={N} binds"] = "FLOP at 989 TFLOP/s" if flop_t >= bytes_t else "bytes at 3.35 TB/s"
 
 
-def full_step(dev, res):
+class _DenseMode:
+    """Run `opt` (built with lazy_table=True) as the dense FlatAdam while a graph is captured: the step takes the dense path and the
+    forwards mark no rows.  Both variants then share one model and one set of flat buffers (23 GB at V = 10,000,000)."""
+
+    def __init__(self, model, opt, on):
+        self.model, self.opt, self.on = model, opt, on
+
+    def __enter__(self):
+        if self.on:
+            self.opt.lazy_table, self.model._row_marker = False, None
+
+    def __exit__(self, *exc):
+        if self.on:
+            self.opt.lazy_table, self.model._row_marker = True, self.opt
+
+
+def graph_time_alternating(variants, iters=5, rounds=3, alternations=3):
+    """{name: (fn, dense?)} -> {name: median ms}, the variants alternated `alternations` times in one session"""
+    times = {k: [] for k in variants}
+    for _ in range(alternations):
+        for k, (fn, ctx) in variants.items():
+            with ctx:
+                times[k].append(graph_time(fn, iters=iters, rounds=rounds))
+    return {k: statistics.median(v) for k, v in times.items()}
+
+
+def full_step(dev, res, V):
+    """One cfg2-geometry HSTU training step with N = 1,024 sampled negatives, and FlatAdam's part of it (the marks of the step's ids
+    and the optimizer step), dense against lazy_table=True, alternated; then the lazy kernels under torch.profiler."""
     from genrec_b200.data import sample_negatives
     from genrec_b200.hstu import HSTU
     from genrec_b200.optim import FlatAdam
-    V, B, L, N = 1_000_000, 128, 200, 1024
+    B, L, N, D = 128, 200, 1024, 128
     torch.manual_seed(0)
-    model = HSTU(num_items=V, max_seq_len=L, embed_dim=128, num_heads=4, num_blocks=4, dropout=0.2).to(dev).train()
-    opt = FlatAdam(model, lr=1e-3, betas=(0.9, 0.98), unit_loss_grad=True)
+    with torch.device(dev):          # a 10 M-row table is initialised on the GPU, not on the CPU
+        model = HSTU(num_items=V, max_seq_len=L, embed_dim=D, num_heads=4, num_blocks=4, dropout=0.2).train()
+    opt = FlatAdam(model, lr=1e-3, betas=(0.9, 0.98), unit_loss_grad=True, lazy_table=True)
     g = torch.Generator(device=dev).manual_seed(1)
     ids = torch.randint(1, V + 1, (B, L), device=dev, generator=g)
     tg = torch.randint(1, V + 1, (B, L), device=dev, generator=g)
@@ -158,16 +189,51 @@ def full_step(dev, res):
         loss.backward()
         opt.step()
 
-    res[f"cfg2 geometry V={V} N={N} training step ms"] = round(graph_time(step, iters=5, rounds=3), 3)
-    res[f"cfg2 geometry V={V} FlatAdam step alone ms"] = round(graph_time(opt.step, iters=5, rounds=3), 3)
+    def optimizer_part():
+        if opt.lazy_table:           # what the forwards add to the optimizer's work: the marks of the step's ids
+            opt._mark(ids); opt._mark(tg); opt._mark(neg)
+        opt.step()
+
+    t = graph_time_alternating({"dense step": (step, _DenseMode(model, opt, True)), "lazy step": (step, _DenseMode(model, opt, False)),
+                                "dense opt": (optimizer_part, _DenseMode(model, opt, True)),
+                                "lazy opt": (optimizer_part, _DenseMode(model, opt, False))})
+    res[f"cfg2 geometry V={V} N={N} training step ms, dense FlatAdam"] = round(t["dense step"], 3)
+    res[f"cfg2 geometry V={V} N={N} training step ms, lazy_table=True"] = round(t["lazy step"], 3)
+    res[f"cfg2 geometry V={V} FlatAdam step alone ms, dense"] = round(t["dense opt"], 3)
+    res[f"cfg2 geometry V={V} FlatAdam marks + step ms, lazy_table=True"] = round(t["lazy opt"], 3)
     table = model.item_embedding.weight.numel()
-    res["table share of the parameters"] = round(table / sum(p.numel() for p in model.parameters()), 4)
+    res[f"V={V} table share of the parameters"] = round(table / sum(p.numel() for p in model.parameters()), 4)
+
+    from torch.profiler import ProfilerActivity, profile
+    reps, touched = 5, []
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            opt._mark(ids); opt._mark(tg); opt._mark(neg)
+            touched.append(opt._row_count[0].clone())
+            opt.step()
+        torch.cuda.synchronize()
+    rows = int(touched[0])
+    res[f"V={V} touched rows per step"] = rows
+    for ev in prof.key_averages():
+        for short in ("rowset_mark_kernel", "lazy_table_step_kernel", "adam_step_kernel", "rowset_reset_kernel", "adam_tick_kernel"):
+            if short in ev.key:
+                t_us = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0.0)
+                res[f"V={V} kernel {short} us per step"] = round(t_us / reps, 2)
+    bound_us = 34.0 * rows * D / PEAK_BYTES * 1e6
+    res[f"V={V} lazy table pass byte bound us (34 B per touched element at 3.35 TB/s)"] = round(bound_us, 2)
+    k = res.get(f"V={V} kernel lazy_table_step_kernel us per step")
+    if k:
+        res[f"V={V} lazy table pass share of its byte bound"] = round(bound_us / k, 3)
+    del model, opt
+    torch.cuda.empty_cache()
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--skip-step", action="store_true")
+    ap.add_argument("--skip-head", action="store_true")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_sampled_head.py needs a CUDA GPU (sm_90a); there is no fallback")
@@ -176,10 +242,12 @@ def main():
     _lib.ensure_device(dev)
     res = {"card": card()}
     T = 128 * 200
-    head_alone(dev, T, res)
-    per_kernel(dev, T, res)
+    if not args.skip_head:
+        head_alone(dev, T, res)
+        per_kernel(dev, T, res)
     if not args.skip_step:
-        full_step(dev, res)
+        for V in (1_000_000, 10_000_000):
+            full_step(dev, res, V)
     print(json.dumps(res, indent=1))
     if args.out:
         with open(args.out, "w") as f:
