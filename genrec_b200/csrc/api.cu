@@ -18,6 +18,7 @@
 #include "common.cuh"
 #include "dp_adam.cuh"
 #include "exact_f32.cuh"
+#include "head_rank.cuh"
 #include "head_topk.cuh"
 #include "lazy_adam.cuh"
 #include "rowwise.cuh"
@@ -1169,6 +1170,87 @@ int grb_head_topk(const float* x, const float* ln_g, const float* ln_b, float ln
     GRB_CUDA(cudaGetLastError());
     launch_k(topk_merge_kernel, (R + TOPK_MERGE_ROWS - 1) / TOPK_MERGE_ROWS, 32 * TOPK_MERGE_ROWS, 0, st, (const float*)w.cand_s,
              (const int*)w.cand_i, R, w.splits, k, scores, reinterpret_cast<long long*>(items));
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+namespace {
+struct RankWork {
+    bf16* xf;                  // [R, D] LN(x), the GEMM operand grb_head_logits builds
+    bf16* G;                   // [R, D] the targets' table rows
+    int *tid, *cnt;            // [R]
+    float* tscore;             // [R]
+    int* excl;                 // [R, E] sorted exclusion lists
+    size_t bytes;
+};
+RankWork carve_rank(void* base, int R, int D, int E) {
+    RankWork w;
+    Carver c{static_cast<char*>(base)};
+    w.xf = c.take<bf16>((size_t)R * D * 2);
+    w.G = c.take<bf16>((size_t)R * D * 2);
+    w.tid = c.take<int>((size_t)R * 4);
+    w.cnt = c.take<int>((size_t)R * 4);
+    w.tscore = c.take<float>((size_t)R * 4);
+    w.excl = E > 0 ? c.take<int>((size_t)R * E * 4) : nullptr;
+    w.bytes = c.off;
+    return w;
+}
+int rank_check(int R, int D, int C, int E) {
+    GRB_REQUIRE(D == 64 || D == 128 || D == 256, "head_rank: D=%d is not supported (64, 128 or 256)", D);
+    GRB_REQUIRE(C >= 2, "head_rank: C=%d classes, must be >= 2", C);
+    GRB_REQUIRE(R >= 1, "head_rank: R=%d rows, must be >= 1", R);
+    GRB_REQUIRE(E >= 0 && E <= TOPK_MAX_EXCLUDE, "head_rank: E=%d exclusion ids per row, must be 0 .. %d", E, TOPK_MAX_EXCLUDE);
+    return 0;
+}
+}  // namespace
+
+size_t grb_head_rank_workspace_bytes(int R, int D, int C, int E) {
+    if (rank_check(R, D, C, E)) return 0;
+    return carve_rank(nullptr, R, D, E).bytes;
+}
+
+int grb_head_rank(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D, int C,
+                  const int64_t* targets, const int64_t* exclude, int E, float* metrics, int32_t* ranks, void* workspace, void* stream) {
+    GRB_TRY(rank_check(R, D, C, E));
+    GRB_REQUIRE(x, "head_rank: x is null");
+    GRB_REQUIRE(table_bf16, "head_rank: table_bf16 is null");
+    GRB_REQUIRE(targets, "head_rank: targets is null");
+    GRB_REQUIRE(ln_g && ln_b, "head_rank: ln_g / ln_b is null");
+    GRB_REQUIRE(workspace, "head_rank: workspace is null");
+    GRB_REQUIRE(E == 0 || exclude, "head_rank: exclude is null with E=%d", E);
+    GRB_REQUIRE(metrics || ranks, "head_rank: metrics and ranks are both null (nothing to write)");
+    GRB_REQUIRE(aligned16(table_bf16) && aligned16(workspace), "head_rank: table_bf16 and workspace must be 16-byte aligned");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const RankWork w = carve_rank(workspace, R, D, E);
+    CUtensorMap tmA, tmG, tmB;
+    GRB_REQUIRE(make_tmap_bf16(&tmA, w.xf, R, D, D, TC_BK, TC_BM) && make_tmap_bf16(&tmG, w.G, R, D, D, TC_BK, TC_BN) &&
+                    make_tmap_bf16(&tmB, table_bf16, C, D, D, TC_BK, TC_BN),
+                "cannot encode the TMA descriptors (driver entry point missing)");
+    const int num_m = (R + TC_BM - 1) / TC_BM, num_n = (C + TC_BN - 1) / TC_BN;
+    // item ranges per row tile: enough CTAs to cover the SMs once, never more ranges than item tiles
+    int splits = sm_count() / num_m;
+    splits = splits < num_n ? splits : num_n;
+    splits = splits < 1 ? 1 : splits;
+    HeadRankArgs a{R, C, E, splits, num_n, D / TC_BK, reinterpret_cast<const long long*>(targets), w.excl, w.tid, w.tscore, w.cnt,
+                   metrics, reinterpret_cast<int*>(ranks)};
+    GRB_TRY(head_ln_forward(x, ln_g, ln_b, ln_eps, w.xf, nullptr, R, D, st));
+    if (E > 0) {
+        int P = 1;
+        while (P < E) P <<= 1;
+        GRB_TRY(set_smem(topk_sort_exclude_kernel, (size_t)P * 4));
+        launch_k(topk_sort_exclude_kernel, R, TOPK_SORT_THREADS, (size_t)P * 4, st, reinterpret_cast<const long long*>(exclude), E, P, C, w.excl);
+        GRB_CUDA(cudaGetLastError());
+    }
+    launch_k(head_rank_gather_kernel, (R + 7) / 8, 256, 0, st, (const bf16*)table_bf16, D, a, w.G);
+    GRB_CUDA(cudaGetLastError());
+    GRB_TRY(set_smem(head_rank_target_kernel, RANK_SMEM_BYTES));
+    launch_k(head_rank_target_kernel, num_m, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmG, a);
+    GRB_CUDA(cudaGetLastError());
+    auto sweep = E > 0 ? head_rank_kernel<true> : head_rank_kernel<false>;
+    GRB_TRY(set_smem(sweep, RANK_SMEM_BYTES));
+    launch_k(sweep, num_m * splits, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmB, a);
+    GRB_CUDA(cudaGetLastError());
+    launch_k(head_rank_finish_kernel, (R + 255) / 256, 256, 0, st, a);
     GRB_CUDA(cudaGetLastError());
     return 0;
 }

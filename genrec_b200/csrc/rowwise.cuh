@@ -1001,6 +1001,13 @@ __global__ void __launch_bounds__(256) split3_f32_bf16_kernel(const float* __res
 // (logit_j == logit_t and j < t)} (torch.topk's order on ties: lower index first) - and Recall@k / NDCG@k for k in {1, 5, 10}
 // are ACCUMULATED on the device:  out[0..2] += hit@{1,5,10}, out[3..5] += ndcg@{1,5,10}.  One CTA per sample; targets of 0
 // (padding) contribute nothing.  ranks (nullable) receives the per-sample rank (0 for skipped samples).
+// One ranked sample's share of the sums; the fused head (head_rank.cuh) adds its samples with the same expressions.
+GRB_DEVINL void rank_metrics_add(float* out, int rank) {
+    const float nd = 1.f / log2f((float)rank + 1.f);
+    if (rank <= 1) { atomicAdd(out + 0, 1.f); atomicAdd(out + 3, nd); }
+    if (rank <= 5) { atomicAdd(out + 1, 1.f); atomicAdd(out + 4, nd); }
+    if (rank <= 10) { atomicAdd(out + 2, 1.f); atomicAdd(out + 5, nd); }
+}
 __global__ void __launch_bounds__(256) eval_rank_kernel(const float* __restrict__ logits, int C, const long long* __restrict__ targets,
                                                        float* __restrict__ out, int* __restrict__ ranks) {
     pdl_wait();
@@ -1025,10 +1032,7 @@ __global__ void __launch_bounds__(256) eval_rank_kernel(const float* __restrict_
         int rank = 1;
         for (int w = 0; w < 8; ++w) rank += red[w];
         if (ranks) ranks[b] = rank;
-        const float nd = 1.f / log2f((float)rank + 1.f);
-        if (rank <= 1) { atomicAdd(out + 0, 1.f); atomicAdd(out + 3, nd); }
-        if (rank <= 5) { atomicAdd(out + 1, 1.f); atomicAdd(out + 4, nd); }
-        if (rank <= 10) { atomicAdd(out + 2, 1.f); atomicAdd(out + 5, nd); }
+        rank_metrics_add(out, rank);
     }
 }
 

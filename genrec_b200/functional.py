@@ -412,6 +412,11 @@ def check_topk_args(k: int, exclude: Optional[torch.Tensor], rows: int, device) 
     """ValueError unless 1 <= k <= 64 and ``exclude`` is None or an int64 [rows, E <= 16384] tensor on ``device``."""
     if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= TOPK_MAX_K:
         raise ValueError(f"top_k must be an int in [1, {TOPK_MAX_K}], got {k!r}")
+    check_exclude_arg(exclude, rows, device)
+
+
+def check_exclude_arg(exclude: Optional[torch.Tensor], rows: int, device) -> None:
+    """ValueError unless ``exclude`` is None or an int64 [rows, E <= 16384] tensor on ``device``."""
     if exclude is None:
         return
     if not isinstance(exclude, torch.Tensor) or exclude.dim() != 2 or exclude.shape[0] != rows:
@@ -464,6 +469,40 @@ def eval_rank_metrics(logits_last: torch.Tensor, targets: torch.Tensor, metrics:
     ranks = torch.empty(B, dtype=torch.int32, device=lg.device) if want_ranks else None
     with torch.cuda.device(lg.device):
         check(_lib.load().grb_eval_rank_metrics(ptr(lg), ptr(targets.contiguous()), B, Cn, ptr(metrics), ptr(ranks), stream_ptr(lg.device)))
+    return (metrics, ranks) if want_ranks else metrics
+
+
+def head_rank_metrics(x, ln_g, ln_b, table_bf16, eps, targets: torch.Tensor, metrics: Optional[torch.Tensor] = None,
+                      exclude: Optional[torch.Tensor] = None, want_ranks: bool = False):
+    """``eval_rank_metrics(head_logits(x))`` without the [R, C] logits (grb_head_rank): x [R, D] fp32, targets [R] int64 ->
+    metrics [6] fp32 accumulated on the device (Recall@{1,5,10} hit counts, NDCG@{1,5,10} sums), and with ``want_ranks`` the
+    int32 ranks [R] too.  The target's rank is counted while the head scores the table, with scores bit-identical to
+    ``head_logits``, so the ranks equal ``eval_rank_metrics``' exactly.  ``exclude`` ([R, E] int64, any order, E <= 16384) removes
+    ids from the count; a row whose target is 0, out of 1..C-1 or excluded gets rank 0 and adds nothing.  Memory grows with R and
+    R * E, not with the catalog.  Inference only (no autograd)."""
+    lib = _lib.load()
+    require_cuda(x, table_bf16, targets)
+    require_i64(targets)
+    if x.dim() != 2:
+        raise ValueError(f"x must be [R, D], got {tuple(x.shape)}")
+    R, D = x.shape
+    if targets.shape != (R,):
+        raise ValueError(f"targets must be [{R}] (one per row of x), got {tuple(targets.shape)}")
+    check_exclude_arg(exclude, R, x.device)
+    Cn = table_bf16.shape[0]
+    xc = x.detach().contiguous().float()
+    ex = exclude.contiguous() if exclude is not None and exclude.shape[1] > 0 else None
+    E = ex.shape[1] if ex is not None else 0
+    nbytes = lib.grb_head_rank_workspace_bytes(R, D, Cn, E)
+    if nbytes == 0:
+        raise _lib.GrbError(lib.grb_last_error().decode())
+    ws = _u8(nbytes, x.device)
+    if metrics is None:
+        metrics = torch.zeros(6, dtype=torch.float32, device=x.device)
+    ranks = torch.empty(R, dtype=torch.int32, device=x.device) if want_ranks else None
+    with torch.cuda.device(x.device):
+        check(lib.grb_head_rank(ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), R, D, Cn,
+                                ptr(targets.contiguous()), ptr(ex), E, ptr(metrics), ptr(ranks), ptr(ws), stream_ptr(x.device)))
     return (metrics, ranks) if want_ranks else metrics
 
 

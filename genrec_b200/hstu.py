@@ -688,11 +688,23 @@ class HSTU(nn.Module):
 
     @torch.no_grad()
     def evaluate_batch(self, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor], targets: torch.Tensor,
-                       metrics: Optional[torch.Tensor] = None) -> torch.Tensor:
+                       metrics: Optional[torch.Tensor] = None, *, exclude: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Leave-one-out metrics of one evaluation batch, accumulated ON THE DEVICE into ``metrics`` ([6] fp32: Recall@{1,5,10} hit
         counts, NDCG@{1,5,10} sums) - the loop of genrec/trainers/hstu_trainer.py:55-81 without per-sample ``.item()`` calls.
-        Divide by the number of samples (and all-reduce across ranks) once at the end of the evaluation."""
-        return Fn.eval_rank_metrics(self.last_logits(input_ids, timestamps), targets, metrics)
+        Divide by the number of samples (and all-reduce across ranks) once at the end of the evaluation.
+
+        At bf16 precision the target's rank is counted while the head scores the table (``Fn.head_rank_metrics``), so no
+        [B, V+1] logits are formed and memory does not grow with the catalog; the ranks equal those of ``last_logits`` exactly.
+        ``exclude`` ([B, E] int64, E <= 16384) leaves ids out of each row's ranking; a row whose target is excluded is not counted.
+        At fp32 precision the metrics come from ``last_logits`` and ``exclude`` is refused."""
+        if self.precision == "fp32":
+            if exclude is not None:
+                raise RuntimeError("genrec_b200: evaluate_batch with exclude runs the bf16 path only; set_precision('bf16')")
+            return Fn.eval_rank_metrics(self.last_logits(input_ids, timestamps), targets, metrics)
+        Fn.check_exclude_arg(exclude, input_ids.shape[0], input_ids.device)
+        x = self.encode(input_ids, timestamps)
+        return Fn.head_rank_metrics(x[:, -1, :], self.final_norm.weight, self.final_norm.bias, self._table_mirror(), self.final_norm.eps,
+                                    targets, metrics, exclude)
 
     @torch.no_grad()
     def predict(self, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None, top_k: int = 10) -> torch.Tensor:

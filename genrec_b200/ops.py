@@ -195,6 +195,19 @@ def _(x, ln_g, ln_b, table_bf16, eps, k, exclude):
     return x.new_empty((R, k), dtype=torch.float32), x.new_empty((R, k), dtype=torch.int64)
 
 
+@custom_op(f"{NS}::head_rank_metrics", mutates_args=())
+def head_rank_metrics(x: Tensor, ln_g: Tensor, ln_b: Tensor, table_bf16: Tensor, eps: float, targets: Tensor,
+                      exclude: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
+    """x [R, D] fp32, targets [R] int64 -> (metrics [6] fp32, ranks [R] int32): eval_rank_metrics of the head's logits, counted
+    without forming them; the row's exclude ids [R, E] int64 are left out of the count.  Inference only."""
+    return tuple(Fn.head_rank_metrics(x, ln_g, ln_b, table_bf16, eps, targets, exclude=exclude, want_ranks=True))
+
+
+@head_rank_metrics.register_fake
+def _(x, ln_g, ln_b, table_bf16, eps, targets, exclude):
+    return x.new_empty((6,), dtype=torch.float32), x.new_empty((x.shape[0],), dtype=torch.int32)
+
+
 # ------------------------------------------------------------------------------------------------ sampled-softmax head
 @custom_op(f"{NS}::head_sampled_loss", mutates_args=())
 def head_sampled_loss(x: Tensor, ln_g: Tensor, ln_b: Tensor, table: Tensor, targets: Tensor, negatives: Tensor, log_q: Optional[Tensor],
@@ -276,4 +289,4 @@ torch.library.register_autograd(f"{NS}::sasrec_attention", _sas_backward, setup_
 
 
 OPS = ("hstu_attention", "hstu_attention_backward", "hstu_layer", "hstu_layer_backward", "rq_residual_argmin", "rq_sinkhorn",
-       "eval_rank_metrics", "head_topk", "head_sampled_loss", "sasrec_attention", "sasrec_attention_backward")
+       "eval_rank_metrics", "head_topk", "head_rank_metrics", "head_sampled_loss", "sasrec_attention", "sasrec_attention_backward")

@@ -294,3 +294,16 @@ class SASRec(nn.Module):
         x = self.encode(input_ids)
         return Fn.head_topk(x[:, -1, :], self.final_norm.weight, self.final_norm.bias, Fn.cast_bf16(self.item_embedding.weight),
                             self.final_norm.eps, top_k, exclude)
+
+    @torch.no_grad()
+    def evaluate_batch(self, input_ids: torch.Tensor, targets: torch.Tensor, metrics: Optional[torch.Tensor] = None, *,
+                       exclude: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Leave-one-out metrics of one evaluation batch, accumulated on the device into ``metrics`` ([6] fp32: Recall@{1,5,10} hit
+        counts, NDCG@{1,5,10} sums): the loop of genrec/trainers/sasrec_trainer.py:39-82 without the logits or per-sample
+        ``.item()`` calls.  Ranks are those of the last row of ``forward``'s logits with item 0 left out, ties to the lower id;
+        ``exclude`` ([B, E] int64) and rows whose target is 0 behave as in ``HSTU.evaluate_batch``.  Divide by the number of samples
+        once at the end of the evaluation."""
+        Fn.check_exclude_arg(exclude, input_ids.shape[0], input_ids.device)
+        x = self.encode(input_ids)
+        return Fn.head_rank_metrics(x[:, -1, :], self.final_norm.weight, self.final_norm.bias, Fn.cast_bf16(self.item_embedding.weight),
+                                    self.final_norm.eps, targets, metrics, exclude)

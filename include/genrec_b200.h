@@ -249,6 +249,17 @@ int grb_head_topk(const float* x, const float* ln_g, const float* ln_b, float ln
  * excluded as the trainer's `logits[:, 0] = -inf` does) is counted on the device and the metric sums are ACCUMULATED:
  * metrics[0..2] += Recall@{1,5,10} hits, metrics[3..5] += NDCG@{1,5,10}.  ranks [B] int32 is optional. */
 int grb_eval_rank_metrics(const float* logits, const int64_t* targets, int B, int C, float* metrics, int32_t* ranks, void* stream);
+/* Evaluation without logits: the same ranks and metric sums as grb_head_logits followed by grb_eval_rank_metrics, counted while
+ * the head sweeps the table.  rank = 1 + #{j in 1..C-1, not excluded : s_j > s_t or (s_j == s_t and j < t)}, where every score
+ * is bit-identical to grb_head_logits' for that row and item (the target's included).  exclude [R, E] int64 (any order,
+ * duplicates allowed, entries outside 1..C-1 ignored; NULL when E = 0) removes ids from the count; a row whose target is 0, out
+ * of 1..C-1 or excluded is not ranked: ranks[r] = 0 and nothing is added to the metrics.  metrics [6] (nullable) is
+ * ACCUMULATED as by grb_eval_rank_metrics; ranks [R] int32 (nullable, not both).  D in {64,128,256}, C >= 2, R >= 1,
+ * 0 <= E <= 16384.  Deterministic ranks.  workspace: grb_head_rank_workspace_bytes(), which grows with R and R * E, never with
+ * C (0 for unsupported arguments). */
+size_t grb_head_rank_workspace_bytes(int R, int D, int C, int E);
+int grb_head_rank(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D, int C,
+                  const int64_t* targets, const int64_t* exclude, int E, float* metrics, int32_t* ranks, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ SASRec attention
  * Replaces MultiHeadAttention.forward (genrec/models/sasrec.py:192-246) after the three projections:

@@ -3,7 +3,8 @@ cached incremental HSTU inference next to full recompute, RQ-VAE Sinkhorn and k-
 roofline or the torch code they replace.  Prints one JSON line per measurement; `bench_kernels.py rqvae_train` runs only the RQ-VAE
 training rows, `bench_kernels.py linear_bwd` only the linear-backward and SASRec training-step rows, `bench_kernels.py head_topk` only
 the fused top-k head rows, `bench_kernels.py tiger` only the TIGER rows (training step, generate eager / graph / uncached loop),
-`bench_kernels.py hstu_attn` only the HSTU attention backward rows."""
+`bench_kernels.py hstu_attn` only the HSTU attention backward rows, `bench_kernels.py head_rank` only the rows of evaluation without
+logits."""
 import json
 import os
 import sys
@@ -202,6 +203,86 @@ def bench_head_topk(dev):
     f_ms, b_ms = graph_timed(lambda: one(top_k=10)), graph_timed(one_topk)
     print(json.dumps(dict(kernel="head_topk", workload="extend_users", geometry=name, pool_users=nusers, B=B, k=10, max_items=cap,
                           fused_us=f_ms * 1e3, logits_topk_us=b_ms * 1e3, speedup_vs_logits_topk=b_ms / f_ms, **info)), flush=True)
+
+
+LOGITS_CAP_GB = 16
+
+
+def bench_head_rank(dev):
+    """Leave-one-out evaluation without logits (Fn.head_rank_metrics: LayerNorm, target gather and score, wgmma sweep counting the
+    target's rank, finish) against the logits path it replaces (Fn.head_logits on the last rows + Fn.eval_rank_metrics), both
+    graph-captured, at D = 128.  The logits path runs only where its [B, C] fp32 logits fit under LOGITS_CAP_GB.  The sweep kernel's
+    time (torch.profiler) is set against its bound, the larger of the table read (C D 2 bytes at 3.35 TB/s) and the GEMM (2 B C D
+    FLOP at 989 TFLOP/s), both H100 SXM data-sheet figures.  Peak memory is torch.cuda.max_memory_allocated above the inputs.  Last,
+    HSTU.evaluate_batch at the cfg2 geometry, B = 128, against eval_rank_metrics(last_logits(...)), alternated three times."""
+    from genrec_b200.hstu import HSTU
+    info = card()
+    HBM, BF16 = 3.35e12, 989e12
+    D, eps = 128, 1e-5
+    gd = torch.Generator(device=dev).manual_seed(0)
+
+    def peak_mb(fn):
+        fn()
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        base = torch.cuda.memory_allocated()
+        fn()
+        torch.cuda.synchronize()
+        return (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+
+    for C in (12102, 1000001, 10000001):
+        tb = (0.05 * torch.randn(C, D, device=dev, generator=gd)).to(torch.bfloat16)
+        ln_g, ln_b = 1 + 0.1 * torch.randn(D, device=dev, generator=gd), 0.1 * torch.randn(D, device=dev, generator=gd)
+        for B in (128, 1024):
+            x = torch.randn(B, D, device=dev, generator=gd)
+            tg = torch.randint(1, C, (B,), device=dev, generator=gd)
+            met = torch.zeros(6, device=dev)
+
+            def fused():
+                return Fn.head_rank_metrics(x, ln_g, ln_b, tb, eps, tg, met)
+
+            def logits_path():
+                return Fn.eval_rank_metrics(Fn.head_logits(x[:, None, :], ln_g, ln_b, tb, tb, eps)[:, 0, :], tg, met)
+
+            logits_gb = B * C * 4 / 1e9
+            t_bytes, t_flop = C * D * 2 / HBM * 1e6, 2 * B * C * D / BF16 * 1e6
+            bound = max(t_bytes, t_flop)
+            f_ms = graph_timed(fused)
+            kern = kernel_us(fused, "head_rank_kernel")
+            row = dict(kernel="head_rank", D=D, C=C, B=B, fused_us=f_ms * 1e3, kernel_us=kern, bound_us=bound,
+                       bound_by="table read" if t_bytes >= t_flop else "bf16 GEMM", kernel_over_bound=kern / bound,
+                       fused_peak_mb=peak_mb(fused), logits_gb=logits_gb)
+            if logits_gb <= LOGITS_CAP_GB:
+                r_f = Fn.head_rank_metrics(x, ln_g, ln_b, tb, eps, tg, want_ranks=True)[1]
+                r_l = Fn.eval_rank_metrics(Fn.head_logits(x[:, None, :], ln_g, ln_b, tb, tb, eps)[:, 0, :], tg, want_ranks=True)[1]
+                assert torch.equal(r_f, r_l)
+                b_ms = graph_timed(logits_path, reps=2, iters=5)
+                row.update(logits_path_us=b_ms * 1e3, speedup_vs_logits=b_ms / f_ms, logits_peak_mb=peak_mb(logits_path))
+            else:
+                row.update(logits_path=f"not run ({logits_gb:.1f} GB of logits, cap {LOGITS_CAP_GB} GB)")
+            print(json.dumps(dict(**row, **info)), flush=True)
+            del x
+            torch.cuda.empty_cache()
+        del tb
+        torch.cuda.empty_cache()
+    # whole evaluate_batch at cfg2 (num_items = 12,101, D = 128, 4 heads, 4 blocks, L = 200), B = 128
+    torch.manual_seed(0)
+    V, L, B = 12101, 200, 128
+    m = HSTU(V, L, 128, 4, 4, dropout=0.0).to(dev).eval()
+    g = torch.Generator().manual_seed(1)
+    ids = torch.randint(1, V + 1, (B, L), generator=g).to(dev)
+    ts = (1_300_000_000 + torch.cumsum(torch.randint(1, 3 * 86400, (B, L), generator=g), 1)).to(dev)
+    tg = torch.randint(1, V + 1, (B,), generator=g).to(dev)
+    met = torch.zeros(6, device=dev)
+    new = lambda: m.evaluate_batch(ids, ts, tg, met)                                     # noqa: E731
+    old = lambda: Fn.eval_rank_metrics(m.last_logits(ids, ts), tg, met)                   # noqa: E731
+    assert torch.equal(Fn.eval_rank_metrics(m.last_logits(ids, ts), tg)[:3], m.evaluate_batch(ids, ts, tg)[:3])
+    runs = {"evaluate_batch": [], "last_logits_eval_rank": []}
+    for _ in range(3):
+        runs["evaluate_batch"].append(graph_timed(new) * 1e3)
+        runs["last_logits_eval_rank"].append(graph_timed(old) * 1e3)
+    print(json.dumps(dict(kernel="head_rank", workload="HSTU.evaluate_batch", geometry="cfg2", B=B, L=L, C=V + 1, us=runs,
+                          peak_mb=dict(evaluate_batch=peak_mb(new), last_logits_eval_rank=peak_mb(old)), **info)), flush=True)
 
 
 def bench_pool(dev):
@@ -426,6 +507,9 @@ def main():
         return
     if sys.argv[1:] == ["tiger"]:
         bench_tiger(dev)
+        return
+    if sys.argv[1:] == ["head_rank"]:
+        bench_head_rank(dev)
         return
     peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) \
         if os.path.exists("MEASURED_PEAKS.json") else {}
