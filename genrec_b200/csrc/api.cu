@@ -1105,36 +1105,68 @@ int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float 
 }
 
 namespace {
-struct TopkWork {
+// what the top-k and the rank head share: LN(x), the sorted exclusion lists, the split of the items into ranges (head_sweep.cuh)
+struct SweepWork {
     bf16* xf;                  // [R, D] LN(x), the GEMM operand grb_head_logits builds
-    int* excl;                 // [R, E] sorted exclusion lists
+    int* excl;                 // [R, E] sorted exclusion lists, or null
+    int num_m, num_n, splits;  // row tiles, item tiles, item ranges per row tile
+};
+void carve_sweep(Carver& c, SweepWork& w, int R, int D, int C, int E) {
+    w.xf = c.take<bf16>((size_t)R * D * 2);
+    w.excl = E > 0 ? c.take<int>((size_t)R * E * 4) : nullptr;
+    w.num_m = (R + TC_BM - 1) / TC_BM;
+    w.num_n = (C + TC_BN - 1) / TC_BN;
+    // enough CTAs to cover the SMs once, never more ranges than item tiles or than topk_merge_kernel merges
+    int s = sm_count() / w.num_m;
+    s = s < w.num_n ? s : w.num_n;
+    s = s < TOPK_MAX_SPLITS ? s : TOPK_MAX_SPLITS;
+    w.splits = s < 1 ? 1 : s;
+}
+int sweep_check(int R, int D, int C, int E) {
+    GRB_REQUIRE(R > 0 && C > 1 && (D == 64 || D == 128 || D == 256), "bad shape R=%d D=%d C=%d (R >= 1, D in {64,128,256}, C >= 2)", R, D, C);
+    GRB_REQUIRE(E >= 0 && E <= SWEEP_MAX_EXCLUDE, "exclusion lists hold at most %d ids per row, got E=%d", SWEEP_MAX_EXCLUDE, E);
+    return 0;
+}
+// checks the arguments both heads take and encodes the TMA descriptors of LN(x) (tmA) and of the table (tmB), then puts LN(x) and
+// the sorted exclusion lists on the stream.  The caller has checked the shape with sweep_check.
+int sweep_prologue(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D, int C,
+                   const int64_t* exclude, int E, const void* workspace, const SweepWork& w, CUtensorMap* tmA, CUtensorMap* tmB,
+                   cudaStream_t st) {
+    GRB_REQUIRE(x, "x is null");
+    GRB_REQUIRE(table_bf16, "table_bf16 is null");
+    GRB_REQUIRE(ln_g && ln_b, "ln_g / ln_b is null");
+    GRB_REQUIRE(workspace, "workspace is null");
+    GRB_REQUIRE(E == 0 || exclude, "exclude is null with E=%d", E);
+    GRB_REQUIRE(aligned16(table_bf16) && aligned16(workspace), "table_bf16 and workspace must be 16-byte aligned");
+    GRB_REQUIRE(make_tmap_bf16(tmA, w.xf, R, D, D, TC_BK, TC_BM) && make_tmap_bf16(tmB, table_bf16, C, D, D, TC_BK, TC_BN),
+                "cannot encode the TMA descriptors (driver entry point missing)");
+    GRB_TRY(head_ln_forward(x, ln_g, ln_b, ln_eps, w.xf, nullptr, R, D, st));
+    if (E > 0) {
+        int P = 1;
+        while (P < E) P <<= 1;
+        GRB_TRY(set_smem(sweep_sort_exclude_kernel, (size_t)P * 4));
+        launch_k(sweep_sort_exclude_kernel, R, SWEEP_SORT_THREADS, (size_t)P * 4, st, reinterpret_cast<const long long*>(exclude), E, P, C, w.excl);
+        GRB_CUDA(cudaGetLastError());
+    }
+    return 0;
+}
+
+struct TopkWork : SweepWork {
     float* cand_s; int* cand_i;  // [R, splits, k] per-range lists
-    int splits;
     size_t bytes;
 };
-// item ranges per row tile: enough CTAs to cover the SMs once, never more ranges than item tiles
-int topk_splits(int R, int C) {
-    const int num_m = (R + TC_BM - 1) / TC_BM, num_n = (C + TC_BN - 1) / TC_BN;
-    int s = sm_count() / num_m;
-    s = s < num_n ? s : num_n;
-    s = s < TOPK_MAX_SPLITS ? s : TOPK_MAX_SPLITS;
-    return s < 1 ? 1 : s;
-}
 TopkWork carve_topk(void* base, int R, int D, int C, int k, int E) {
     TopkWork w;
     Carver c{static_cast<char*>(base)};
-    w.splits = topk_splits(R, C);
-    w.xf = c.take<bf16>((size_t)R * D * 2);
-    w.excl = E > 0 ? c.take<int>((size_t)R * E * 4) : nullptr;
+    carve_sweep(c, w, R, D, C, E);
     w.cand_s = c.take<float>((size_t)R * w.splits * k * 4);
     w.cand_i = c.take<int>((size_t)R * w.splits * k * 4);
     w.bytes = c.off;
     return w;
 }
 int topk_check(int R, int D, int C, int k, int E) {
-    GRB_REQUIRE(R > 0 && C > 1 && (D == 64 || D == 128 || D == 256), "bad shape R=%d D=%d C=%d (R >= 1, D in {64,128,256}, C >= 2)", R, D, C);
+    GRB_TRY(sweep_check(R, D, C, E));
     GRB_REQUIRE(k >= 1 && k <= TOPK_MAX_K, "k must lie in [1, %d], got %d", TOPK_MAX_K, k);
-    GRB_REQUIRE(E >= 0 && E <= TOPK_MAX_EXCLUDE, "exclusion lists hold at most %d ids per row, got E=%d", TOPK_MAX_EXCLUDE, E);
     return 0;
 }
 }  // namespace
@@ -1146,27 +1178,15 @@ size_t grb_head_topk_workspace_bytes(int R, int D, int C, int k, int E) {
 
 int grb_head_topk(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D, int C, int k,
                   const int64_t* exclude, int E, float* scores, int64_t* items, void* workspace, void* stream) {
-    GRB_REQUIRE(x && ln_g && ln_b && table_bf16 && scores && items && workspace, "null argument");
+    GRB_REQUIRE(scores && items, "null argument: scores / items");
     GRB_TRY(topk_check(R, D, C, k, E));
-    GRB_REQUIRE(E == 0 || exclude, "exclude is null with E=%d", E);
-    GRB_REQUIRE(aligned16(table_bf16) && aligned16(workspace), "table and workspace must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const TopkWork w = carve_topk(workspace, R, D, C, k, E);
     CUtensorMap tmA, tmB;
-    GRB_REQUIRE(make_tmap_bf16(&tmA, w.xf, R, D, D, TC_BK, TC_BM) && make_tmap_bf16(&tmB, table_bf16, C, D, D, TC_BK, TC_BN),
-                "cannot encode the TMA descriptors (driver entry point missing)");
-    GRB_TRY(head_ln_forward(x, ln_g, ln_b, ln_eps, w.xf, nullptr, R, D, st));
-    if (E > 0) {
-        int P = 1;
-        while (P < E) P <<= 1;
-        GRB_TRY(set_smem(topk_sort_exclude_kernel, (size_t)P * 4));
-        launch_k(topk_sort_exclude_kernel, R, TOPK_SORT_THREADS, (size_t)P * 4, st, reinterpret_cast<const long long*>(exclude), E, P, C, w.excl);
-        GRB_CUDA(cudaGetLastError());
-    }
-    HeadTopkArgs a{R, C, k, E, w.splits, (C + TC_BN - 1) / TC_BN, D / TC_BK, w.excl, w.cand_s, w.cand_i};
+    GRB_TRY(sweep_prologue(x, ln_g, ln_b, ln_eps, table_bf16, R, D, C, exclude, E, workspace, w, &tmA, &tmB, st));
+    HeadTopkArgs a{R, C, k, E, w.splits, w.num_n, D / TC_BK, w.excl, w.cand_s, w.cand_i};
     GRB_TRY(set_smem(head_topk_kernel, TC_SMEM_BYTES));
-    const int num_m = (R + TC_BM - 1) / TC_BM;
-    launch_k(head_topk_kernel, num_m * w.splits, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, a);
+    launch_k(head_topk_kernel, w.num_m * w.splits, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, a);
     GRB_CUDA(cudaGetLastError());
     launch_k(topk_merge_kernel, (R + TOPK_MERGE_ROWS - 1) / TOPK_MERGE_ROWS, 32 * TOPK_MERGE_ROWS, 0, st, (const float*)w.cand_s,
              (const int*)w.cand_i, R, w.splits, k, scores, reinterpret_cast<long long*>(items));
@@ -1175,80 +1195,50 @@ int grb_head_topk(const float* x, const float* ln_g, const float* ln_b, float ln
 }
 
 namespace {
-struct RankWork {
-    bf16* xf;                  // [R, D] LN(x), the GEMM operand grb_head_logits builds
+struct RankWork : SweepWork {
     bf16* G;                   // [R, D] the targets' table rows
     int *tid, *cnt;            // [R]
     float* tscore;             // [R]
-    int* excl;                 // [R, E] sorted exclusion lists
     size_t bytes;
 };
-RankWork carve_rank(void* base, int R, int D, int E) {
+RankWork carve_rank(void* base, int R, int D, int C, int E) {
     RankWork w;
     Carver c{static_cast<char*>(base)};
-    w.xf = c.take<bf16>((size_t)R * D * 2);
+    carve_sweep(c, w, R, D, C, E);
     w.G = c.take<bf16>((size_t)R * D * 2);
     w.tid = c.take<int>((size_t)R * 4);
     w.cnt = c.take<int>((size_t)R * 4);
     w.tscore = c.take<float>((size_t)R * 4);
-    w.excl = E > 0 ? c.take<int>((size_t)R * E * 4) : nullptr;
     w.bytes = c.off;
     return w;
-}
-int rank_check(int R, int D, int C, int E) {
-    GRB_REQUIRE(D == 64 || D == 128 || D == 256, "head_rank: D=%d is not supported (64, 128 or 256)", D);
-    GRB_REQUIRE(C >= 2, "head_rank: C=%d classes, must be >= 2", C);
-    GRB_REQUIRE(R >= 1, "head_rank: R=%d rows, must be >= 1", R);
-    GRB_REQUIRE(E >= 0 && E <= TOPK_MAX_EXCLUDE, "head_rank: E=%d exclusion ids per row, must be 0 .. %d", E, TOPK_MAX_EXCLUDE);
-    return 0;
 }
 }  // namespace
 
 size_t grb_head_rank_workspace_bytes(int R, int D, int C, int E) {
-    if (rank_check(R, D, C, E)) return 0;
-    return carve_rank(nullptr, R, D, E).bytes;
+    if (sweep_check(R, D, C, E)) return 0;
+    return carve_rank(nullptr, R, D, C, E).bytes;
 }
 
 int grb_head_rank(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D, int C,
                   const int64_t* targets, const int64_t* exclude, int E, float* metrics, int32_t* ranks, void* workspace, void* stream) {
-    GRB_TRY(rank_check(R, D, C, E));
-    GRB_REQUIRE(x, "head_rank: x is null");
-    GRB_REQUIRE(table_bf16, "head_rank: table_bf16 is null");
-    GRB_REQUIRE(targets, "head_rank: targets is null");
-    GRB_REQUIRE(ln_g && ln_b, "head_rank: ln_g / ln_b is null");
-    GRB_REQUIRE(workspace, "head_rank: workspace is null");
-    GRB_REQUIRE(E == 0 || exclude, "head_rank: exclude is null with E=%d", E);
-    GRB_REQUIRE(metrics || ranks, "head_rank: metrics and ranks are both null (nothing to write)");
-    GRB_REQUIRE(aligned16(table_bf16) && aligned16(workspace), "head_rank: table_bf16 and workspace must be 16-byte aligned");
+    GRB_TRY(sweep_check(R, D, C, E));
+    GRB_REQUIRE(targets, "targets is null");
+    GRB_REQUIRE(metrics || ranks, "metrics and ranks are both null (nothing to write)");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const RankWork w = carve_rank(workspace, R, D, E);
-    CUtensorMap tmA, tmG, tmB;
-    GRB_REQUIRE(make_tmap_bf16(&tmA, w.xf, R, D, D, TC_BK, TC_BM) && make_tmap_bf16(&tmG, w.G, R, D, D, TC_BK, TC_BN) &&
-                    make_tmap_bf16(&tmB, table_bf16, C, D, D, TC_BK, TC_BN),
-                "cannot encode the TMA descriptors (driver entry point missing)");
-    const int num_m = (R + TC_BM - 1) / TC_BM, num_n = (C + TC_BN - 1) / TC_BN;
-    // item ranges per row tile: enough CTAs to cover the SMs once, never more ranges than item tiles
-    int splits = sm_count() / num_m;
-    splits = splits < num_n ? splits : num_n;
-    splits = splits < 1 ? 1 : splits;
-    HeadRankArgs a{R, C, E, splits, num_n, D / TC_BK, reinterpret_cast<const long long*>(targets), w.excl, w.tid, w.tscore, w.cnt,
+    const RankWork w = carve_rank(workspace, R, D, C, E);
+    CUtensorMap tmA, tmB, tmG;
+    GRB_TRY(sweep_prologue(x, ln_g, ln_b, ln_eps, table_bf16, R, D, C, exclude, E, workspace, w, &tmA, &tmB, st));
+    GRB_REQUIRE(make_tmap_bf16(&tmG, w.G, R, D, D, TC_BK, TC_BN), "cannot encode the TMA descriptor of G");
+    HeadRankArgs a{R, C, E, w.splits, w.num_n, D / TC_BK, reinterpret_cast<const long long*>(targets), w.excl, w.tid, w.tscore, w.cnt,
                    metrics, reinterpret_cast<int*>(ranks)};
-    GRB_TRY(head_ln_forward(x, ln_g, ln_b, ln_eps, w.xf, nullptr, R, D, st));
-    if (E > 0) {
-        int P = 1;
-        while (P < E) P <<= 1;
-        GRB_TRY(set_smem(topk_sort_exclude_kernel, (size_t)P * 4));
-        launch_k(topk_sort_exclude_kernel, R, TOPK_SORT_THREADS, (size_t)P * 4, st, reinterpret_cast<const long long*>(exclude), E, P, C, w.excl);
-        GRB_CUDA(cudaGetLastError());
-    }
     launch_k(head_rank_gather_kernel, (R + 7) / 8, 256, 0, st, (const bf16*)table_bf16, D, a, w.G);
     GRB_CUDA(cudaGetLastError());
     GRB_TRY(set_smem(head_rank_target_kernel, RANK_SMEM_BYTES));
-    launch_k(head_rank_target_kernel, num_m, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmG, a);
+    launch_k(head_rank_target_kernel, w.num_m, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmG, a);
     GRB_CUDA(cudaGetLastError());
     auto sweep = E > 0 ? head_rank_kernel<true> : head_rank_kernel<false>;
     GRB_TRY(set_smem(sweep, RANK_SMEM_BYTES));
-    launch_k(sweep, num_m * splits, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmB, a);
+    launch_k(sweep, w.num_m * w.splits, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmB, a);
     GRB_CUDA(cudaGetLastError());
     launch_k(head_rank_finish_kernel, (R + 255) / 256, 256, 0, st, a);
     GRB_CUDA(cudaGetLastError());

@@ -3,21 +3,21 @@
 //   rank[r] = 1 + #{ j in 1..C-1, j not excluded : s_j > s_t  or  (s_j == s_t and j < t) },   s = LN(x[r]) . E^T,  t = targets[r]
 //
 // the rule eval_rank_kernel (rowwise.cuh) applies to stored logits.  Rows whose target is 0, out of 1..C-1 or in the row's
-// exclusion list are not ranked (rank 0).  Launches after the LayerNorm (ln_fwd_kernel, the operand grb_head_logits builds) and
-// the exclusion sort (topk_sort_exclude_kernel, head_topk.cuh):
+// exclusion list are not ranked (rank 0).  Launches after the LayerNorm and the exclusion sort (head_sweep.cuh):
 //   head_rank_gather_kernel    one warp per row: the target's bf16 table row -> G [R, D]; which rows are ranked; counts = 0
-//   head_rank_target_kernel    one CTA per row tile: the same wgmma sequence as the sweep, row tile mt of LN(x) against
-//                              tile mt of G, and keeps the diagonal.  The same A row, the same B column and the same k-sequence
-//                              of wgmma give the fp32 bits the sweep computes for column t, so the target never counts itself
-//                              and ties are ordered exactly.
-//   head_rank_kernel           TMA + mbarrier + wgmma, one CTA per (row tile, item range), blockIdx.x = split * num_m + row tile
-//                              (the CTAs of one item range run side by side, so a table tile comes from HBM once).  Each consumer
-//                              thread compares its 64 accumulators straight from the registers against the target scores of
-//                              its two rows; at the end of the range 4 lanes per row add up and one atomicAdd per (row, CTA)
-//                              adds the range's count.  Integer sums: the result does not depend on the split.
+//   head_rank_target_kernel    one CTA per row tile: the sweep's steps on one tile, row tile mt of LN(x) against tile mt of G,
+//                              keeping the diagonal.  The same A row, the same B column and the same tc_mainloop give the fp32
+//                              bits the sweep computes for column t, so the target never counts itself and ties are ordered
+//                              exactly.
+//   head_rank_kernel           TMA + mbarrier + wgmma (tc_mainloop with A resident, K = D), one CTA per (row tile, item range)
+//                              as sweep_range (head_sweep.cuh) assigns them.  tc_mainloop is the wgmma sequence grb_head_logits
+//                              runs, so every score has the bits of its logit.  Each consumer thread compares its 64
+//                              accumulators straight from the registers against the target scores of its two rows; at the end
+//                              of the range 4 lanes per row add up and one atomicAdd per (row, CTA) adds the range's count.
+//                              Integer sums: the result does not depend on the split.
 //   head_rank_finish_kernel    rank = 1 + count -> ranks; Recall / NDCG @{1,5,10} with rank_metrics_add, as eval_rank_kernel
 #pragma once
-#include "head_topk.cuh"
+#include "head_sweep.cuh"
 #include "rowwise.cuh"
 
 namespace grb {
@@ -47,7 +47,7 @@ __global__ void __launch_bounds__(256) head_rank_gather_kernel(const bf16* __res
     if (r >= a.R) return;
     const long long t = a.targets[r];
     bool ok = t >= 1 && t < a.C;
-    if (ok && a.excl) ok = !topk_excluded(a.excl + (size_t)r * a.E, a.E, (int)t);
+    if (ok && a.excl) ok = !sweep_excluded(a.excl + (size_t)r * a.E, a.E, (int)t);
     const uint4* src = reinterpret_cast<const uint4*>(table + (size_t)(ok ? t : 0) * D);
     uint4* dst = reinterpret_cast<uint4*>(G + (size_t)r * D);
     for (int c = lane; c < D / 8; c += 32) dst[c] = ok ? src[c] : make_uint4(0u, 0u, 0u, 0u);
@@ -57,7 +57,7 @@ __global__ void __launch_bounds__(256) head_rank_gather_kernel(const bf16* __res
     }
 }
 
-// ------------------------------------------------------------------------------------------------ shared CTA steps
+// ------------------------------------------------------------------------------------------------ CTA steps
 struct RankSmem {
     unsigned char *sA, *sB;                      // sA: [kblocks] resident A tiles ; sB: [RANK_STAGES] ring of B tiles
     uint64_t *full_bar, *empty_bar, *a_bar;
@@ -100,31 +100,6 @@ GRB_DEVINL void rank_produce(const CUtensorMap* tmA, const CUtensorMap* tmB, con
         }
     }
 }
-// One consumer warpgroup's 64 x 128 scores of one B tile: tc_mainloop<0, 0, ...> of tc_gemm.cuh with the A k-block read from the
-// resident tiles instead of the ring.  The wgmma instructions, their descriptors' layout, their operands and their order are
-// those of tc_mainloop, so every fp32 accumulator has the bits grb_head_logits stores for that (row, item).
-GRB_DEVINL void rank_mainloop(float (&acc)[64], const RankSmem& s, int kblocks, int g, int& stage, uint32_t& phase) {
-    const bool leader = (threadIdx.x & 127) == 0;
-    int prev = -1;
-#pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-    for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(&s.full_bar[stage], phase);
-        const uint32_t a_addr = smem_u32(s.sA + kb * TC_TILE_BYTES) + g * (TC_TILE_BYTES / 2);
-        const uint32_t b_addr = smem_u32(s.sB + stage * TC_TILE_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k)
-            wgmma_m64n128k16<0, 0>(acc, wgmma_desc(a_addr + k * 32, 16, 1024), wgmma_desc(b_addr + k * 32, 16, 1024), (kb > 0 || k > 0) ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (prev >= 0 && leader) mbar_arrive(&s.empty_bar[prev]);
-        prev = stage;
-        if (++stage == RANK_STAGES) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    if (prev >= 0 && leader) mbar_arrive(&s.empty_bar[prev]);
-}
 // tile row of accumulator row i (0, 1) of this consumer thread: wgmma D fragment rows lane / 4 and lane / 4 + 8 of the warp's 16
 GRB_DEVINL int rank_frag_row(int g, int i) { return g * 64 + ((threadIdx.x >> 5) & 3) * 16 + ((threadIdx.x & 31) >> 2) + 8 * i; }
 
@@ -144,7 +119,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     uint32_t phase = 0;
     float acc[64];
     mbar_wait(s.a_bar, 0);
-    rank_mainloop(acc, s, a.kblocks, g, stage, phase);
+    tc_mainloop<0, 0, RANK_STAGES, true>(acc, s.sA, s.sB, s.full_bar, s.empty_bar, 0, a.kblocks, g, stage, phase);
     // tile row rr meets G column rr.  The thread holds columns 8 j + 2 (lane % 4) + e and rr % 8 = lane / 4, so the diagonal lies
     // with the lanes where lane % 4 = lane / 8, at e = (lane / 4) % 2 and j = rr / 8.
     if ((lane & 3) != (lane >> 3)) return;
@@ -178,7 +153,7 @@ GRB_DEVINL void rank_count_tile(const float (&acc)[64], const float (&st)[2], co
                 const float v = acc[4 * j + 2 * i + e];
                 bool h = v > st[i] || (v == st[i] && k < tl);
                 if (EDGE) h = h && k >= lo && k < hi;
-                if (EXCL && h) h = !topk_excluded(ex[i], E, n0 + cb + k);
+                if (EXCL && h) h = !sweep_excluded(ex[i], E, n0 + cb + k);
                 c += h;
             }
         }
@@ -192,12 +167,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     extern __shared__ unsigned char rank_smem_raw[];
     const RankSmem s = rank_cta_init(rank_smem_raw, &tmA, &tmB);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int num_m = (a.R + TC_BM - 1) / TC_BM;
-    const int mt = blockIdx.x % num_m, split = blockIdx.x / num_m;
-    const int m0 = mt * TC_BM;
-    const int n_begin = (int)((long long)split * a.num_n / a.splits), n_end = (int)((long long)(split + 1) * a.num_n / a.splits);
+    const SweepRange t = sweep_range(a.R, a.num_n, a.splits);
+    const int m0 = t.m0;
     if (warp < 4) {
-        if (warp == 0 && lane == 0) rank_produce(&tmA, &tmB, s, m0, n_begin * TC_BN, n_end - n_begin, a.kblocks);
+        if (warp == 0 && lane == 0) rank_produce(&tmA, &tmB, s, m0, t.n_begin * TC_BN, t.n_end - t.n_begin, a.kblocks);
         return;
     }
     const int g = (warp >> 2) - 1;
@@ -216,8 +189,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     uint32_t phase = 0;
     float acc[64];
     mbar_wait(s.a_bar, 0);
-    for (int nt = n_begin; nt < n_end; ++nt) {
-        rank_mainloop(acc, s, a.kblocks, g, stage, phase);
+    for (int nt = t.n_begin; nt < t.n_end; ++nt) {
+        tc_mainloop<0, 0, RANK_STAGES, true>(acc, s.sA, s.sB, s.full_bar, s.empty_bar, 0, a.kblocks, g, stage, phase);
         const int n0 = nt * TC_BN;
         if (n0 > 0 && n0 + TC_BN <= a.C) rank_count_tile<false, EXCL>(acc, st, tgt, ex, a.E, n0, cb, a.C, cnt);
         else rank_count_tile<true, EXCL>(acc, st, tgt, ex, a.E, n0, cb, a.C, cnt);

@@ -3,29 +3,25 @@
 //   scores[r, :], items[r, :] = the k best items of LN(x[r]) . E^T, best first, in the total order (score desc, item id asc);
 //   item 0 (padding) and the ids of the row's exclusion list never appear; missing slots hold (-inf, 0).
 //
-// Three launches after the LayerNorm (ln_fwd_kernel, the bf16 operand grb_head_logits builds):
-//   topk_sort_exclude_kernel   one CTA per row: the row's exclusion list -> int32, ids outside 1..C-1 -> INT_MAX, bitonic sort
-//   head_topk_kernel           TMA + mbarrier + wgmma (tc_mainloop of tc_gemm.cuh, K = D), one CTA per (row tile, item range):
-//                              the CTA walks its contiguous range of 128-item tiles, and for each row of its tile keeps a sorted
-//                              list of k (score, id) in the shared memory tc_gemm_kernel uses for output staging.  The list's k-th
-//                              score is the row's threshold, so a score that cannot enter costs one compare; the few that pass are
-//                              merged into the list by one warp at once.  Ids are visited in increasing order, so "pass when
-//                              strictly greater than the k-th score" is the tie rule exactly.
+// Launches after the LayerNorm and the exclusion sort (head_sweep.cuh):
+//   head_topk_kernel           TMA + mbarrier + wgmma (tc_mainloop of tc_gemm.cuh, K = D), one CTA per (row tile, item range) as
+//                              sweep_range (head_sweep.cuh) assigns them: the CTA walks its contiguous range of 128-item tiles,
+//                              and for each row of its tile keeps a sorted list of k (score, id) in the shared memory
+//                              tc_gemm_kernel uses for output staging.  The list's k-th score is the row's threshold, so a score
+//                              that cannot enter costs one compare; the few that pass are merged into the list by one warp at
+//                              once.  Ids are visited in increasing order, so "pass when strictly greater than the k-th score"
+//                              is the tie rule exactly.
 //   topk_merge_kernel          one warp per row: k-way merge of the per-range lists under the same total order
 // Every score is the fp32 accumulator of the same wgmma sequence grb_head_logits runs for that (row, item), so the scores are
 // bit-identical to its logits, and the total order makes the result independent of how the items are split across CTAs.
 #pragma once
-#include <climits>
-
-#include "tc_gemm.cuh"
+#include "head_sweep.cuh"
 
 namespace grb {
 
 constexpr int TOPK_MAX_K = 64;
-constexpr int TOPK_MAX_EXCLUDE = 16384;
 constexpr int TOPK_MAX_SPLITS = 256;            // item ranges per row tile (the merge keeps one cursor per range in shared memory)
 constexpr int TOPK_MERGE_ROWS = 4;              // rows (warps) per merge CTA
-constexpr int TOPK_SORT_THREADS = 1024;
 static_assert(TOPK_MAX_K * TC_BM * 8 <= TC_STAGE_OUT_BYTES, "the per-row lists live in the output staging buffer");
 
 struct HeadTopkArgs {
@@ -35,42 +31,6 @@ struct HeadTopkArgs {
     float* cand_s;              // [R, splits, k]
     int* cand_i;                // [R, splits, k]
 };
-
-// ------------------------------------------------------------------------------------------------ exclusion lists
-__global__ void __launch_bounds__(TOPK_SORT_THREADS) topk_sort_exclude_kernel(const long long* ex, int E, int P, int C, int* out) {
-    pdl_wait();
-    extern __shared__ int sort_buf[];           // [P], P = the power of two >= E
-    const long long* src = ex + (size_t)blockIdx.x * E;
-    for (int i = threadIdx.x; i < P; i += blockDim.x) {
-        const long long v = i < E ? src[i] : 0;
-        sort_buf[i] = (v >= 1 && v < C) ? (int)v : INT_MAX;
-    }
-    __syncthreads();
-    for (int size = 2; size <= P; size <<= 1) {
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int t = threadIdx.x; t < P / 2; t += blockDim.x) {
-                const int i = 2 * t - (t & (stride - 1));          // lower index of the pair, j = i + stride
-                const int j = i + stride;
-                const bool up = (i & size) == 0;
-                const int a = sort_buf[i], b = sort_buf[j];
-                if ((a > b) == up) { sort_buf[i] = b; sort_buf[j] = a; }
-            }
-            __syncthreads();
-        }
-    }
-    int* dst = out + (size_t)blockIdx.x * E;
-    for (int i = threadIdx.x; i < E; i += blockDim.x) dst[i] = sort_buf[i];
-}
-
-GRB_DEVINL bool topk_excluded(const int* ex, int E, int id) {
-    int lo = 0, hi = E;
-    while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(ex + mid) < id) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo < E && __ldg(ex + lo) == id;
-}
 
 // total order of every list: the higher score first, then the lower id
 GRB_DEVINL bool topk_better(float s, int id, float s2, int id2) { return s > s2 || (s == s2 && id < id2); }
@@ -136,9 +96,8 @@ GRB_DEVINL void topk_merge_row(float* ls, int* li, int k, const float (&v)[4], c
 }
 
 // ------------------------------------------------------------------------------------------------ scoring + per-range lists
-// blockIdx.x = split * num_m + row tile: the CTAs that read the same item range for different row tiles run side by side, so a
-// table tile comes from HBM once.  Warp roles as tc_gemm_kernel; in the selection step warp w of consumer warpgroup g owns rows
-// 64 g + 16 w .. +15 of the tile (among the rows its warpgroup's wgmma produced) and their lists.
+// Warp roles as tc_gemm_kernel; in the selection step warp w of consumer warpgroup g owns rows 64 g + 16 w .. +15 of the tile
+// (among the rows its warpgroup's wgmma produced) and their lists.
 __global__ void __launch_bounds__(TC_THREADS, 1)
     head_topk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, HeadTopkArgs a) {
     extern __shared__ unsigned char topk_smem_raw[];
@@ -153,10 +112,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     uint64_t* empty_bar = bars + TC_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int num_m = (a.R + TC_BM - 1) / TC_BM;
-    const int mt = blockIdx.x % num_m, split = blockIdx.x / num_m;
-    const int m0 = mt * TC_BM;
-    const int n_begin = (int)((long long)split * a.num_n / a.splits), n_end = (int)((long long)(split + 1) * a.num_n / a.splits);
+    const SweepRange t = sweep_range(a.R, a.num_n, a.splits);
+    const int m0 = t.m0;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmA);
@@ -175,7 +132,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         if (warp == 0 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            for (int nt = n_begin; nt < n_end; ++nt) {
+            for (int nt = t.n_begin; nt < t.n_end; ++nt) {
                 for (int kb = 0; kb < a.kblocks; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     mbar_expect_tx(&full_bar[stage], 2 * TC_TILE_BYTES);
@@ -199,7 +156,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     int stage = 0;
     uint32_t phase = 0;
     float acc[64];
-    for (int nt = n_begin; nt < n_end; ++nt) {
+    for (int nt = t.n_begin; nt < t.n_end; ++nt) {
         tc_mainloop<0, 0, TC_STAGES>(acc, sA, sB, full_bar, empty_bar, 0, a.kblocks, g, stage, phase);
         wg_bar_sync(g);                          // this warpgroup's selection of the previous tile has read sAcc
         tc_acc_store(sAcc, acc, g);
@@ -228,7 +185,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                 any = 0;
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {
-                    if (ok[q] && topk_excluded(ex, a.E, id[q])) ok[q] = false;
+                    if (ok[q] && sweep_excluded(ex, a.E, id[q])) ok[q] = false;
                     any |= __ballot_sync(0xffffffffu, ok[q]);
                 }
                 if (!any) continue;
@@ -239,8 +196,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     for (int j = lane; j < 16 * k; j += 32) {
         const int i = j / k, s = j - i * k, row = m0 + r0 + i;
         if (row < a.R) {
-            a.cand_s[((size_t)row * a.splits + split) * k + s] = lsc[(r0 + i) * TOPK_MAX_K + s];
-            a.cand_i[((size_t)row * a.splits + split) * k + s] = lid[(r0 + i) * TOPK_MAX_K + s];
+            a.cand_s[((size_t)row * a.splits + t.split) * k + s] = lsc[(r0 + i) * TOPK_MAX_K + s];
+            a.cand_i[((size_t)row * a.splits + t.split) * k + s] = lid[(r0 + i) * TOPK_MAX_K + s];
         }
     }
 }

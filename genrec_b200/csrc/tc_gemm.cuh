@@ -110,7 +110,8 @@ GRB_DEVINL uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t 
 
 // One consumer warpgroup's share of a work item: rows 64*g .. +63 of the 128 x 128 tile over k-blocks kb0 .. kb1-1 of the ring.
 // Each stage is released to the producer once the wgmma reading it has retired (one MMA batch stays in flight).
-template <int A_MN, int B_MN, int STAGES>
+// A_RES: A stays resident (k-block kb at sA + kb * TC_TILE_BYTES, loaded before the call) and the ring carries B only.
+template <int A_MN, int B_MN, int STAGES, bool A_RES = false>
 GRB_DEVINL void tc_mainloop(float (&acc)[64], const unsigned char* sA, const unsigned char* sB, uint64_t* full_bar, uint64_t* empty_bar,
                             int kb0, int kb1, int g, int& stage, uint32_t& phase) {
     const bool leader = (threadIdx.x & 127) == 0;
@@ -119,7 +120,7 @@ GRB_DEVINL void tc_mainloop(float (&acc)[64], const unsigned char* sA, const uns
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;   // the first wgmma overwrites them; this only ends their live range at the previous epilogue
     for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        const uint32_t a_addr = smem_u32(sA + stage * TC_TILE_BYTES) + g * (TC_TILE_BYTES / 2);  // 64 rows (K-major) or one 64-wide M box
+        const uint32_t a_addr = smem_u32(sA + (A_RES ? kb : stage) * TC_TILE_BYTES) + g * (TC_TILE_BYTES / 2);  // 64 rows (K-major) or one 64-wide M box
         const uint32_t b_addr = smem_u32(sB + stage * TC_TILE_BYTES);
         wgmma_fence();
 #pragma unroll

@@ -430,24 +430,31 @@ def check_exclude_arg(exclude: Optional[torch.Tensor], rows: int, device) -> Non
         raise ValueError(f"exclude holds at most {TOPK_MAX_EXCLUDE} ids per row, got {exclude.shape[1]}")
 
 
+def _sweep_inputs(x, table_bf16, exclude, check_rows, workspace_bytes):
+    """What head_topk and head_rank_metrics share: x must be [R, D], and ``check_rows(R)`` runs the head's own argument checks.
+    -> (x as contiguous fp32, exclude or None when it holds no ids, E, a workspace of ``workspace_bytes(R, D, C, E)`` bytes)"""
+    if x.dim() != 2:
+        raise ValueError(f"x must be [R, D], got {tuple(x.shape)}")
+    R, D = x.shape
+    check_rows(R)
+    ex = exclude.contiguous() if exclude is not None and exclude.shape[1] > 0 else None
+    E = ex.shape[1] if ex is not None else 0
+    nbytes = workspace_bytes(R, D, table_bf16.shape[0], E)
+    if nbytes == 0:
+        raise _lib.GrbError(_lib.load().grb_last_error().decode())
+    return x.detach().contiguous().float(), ex, E, _u8(nbytes, x.device)
+
+
 def head_topk(x, ln_g, ln_b, table_bf16, eps, k: int, exclude: Optional[torch.Tensor] = None) -> TopItems:
     """The ``k`` best items of every row of ``x`` [R, D] under the tied head, without forming the logits (grb_head_topk): scores are
     bit-identical to ``head_logits`` of the same rows; item 0 and the row's ``exclude`` ids ([R, E] int64, any order) never appear;
     ties go to the lower item id.  Inference only (no autograd)."""
     lib = _lib.load()
     require_cuda(x, table_bf16)
-    if x.dim() != 2:
-        raise ValueError(f"x must be [R, D], got {tuple(x.shape)}")
+    xc, ex, E, ws = _sweep_inputs(x, table_bf16, exclude, lambda R: check_topk_args(k, exclude, R, x.device),
+                                  lambda R, D, Cn, E: lib.grb_head_topk_workspace_bytes(R, D, Cn, k, E))
     R, D = x.shape
     Cn = table_bf16.shape[0]
-    check_topk_args(k, exclude, R, x.device)
-    xc = x.detach().contiguous().float()
-    ex = exclude.contiguous() if exclude is not None and exclude.shape[1] > 0 else None
-    E = ex.shape[1] if ex is not None else 0
-    nbytes = lib.grb_head_topk_workspace_bytes(R, D, Cn, k, E)
-    if nbytes == 0:
-        raise _lib.GrbError(lib.grb_last_error().decode())
-    ws = _u8(nbytes, x.device)
     scores = torch.empty(R, k, dtype=torch.float32, device=x.device)
     items = torch.empty(R, k, dtype=torch.int64, device=x.device)
     with torch.cuda.device(x.device):
@@ -483,20 +490,15 @@ def head_rank_metrics(x, ln_g, ln_b, table_bf16, eps, targets: torch.Tensor, met
     lib = _lib.load()
     require_cuda(x, table_bf16, targets)
     require_i64(targets)
-    if x.dim() != 2:
-        raise ValueError(f"x must be [R, D], got {tuple(x.shape)}")
+
+    def check_rows(R):
+        if targets.shape != (R,):
+            raise ValueError(f"targets must be [{R}] (one per row of x), got {tuple(targets.shape)}")
+        check_exclude_arg(exclude, R, x.device)
+
+    xc, ex, E, ws = _sweep_inputs(x, table_bf16, exclude, check_rows, lib.grb_head_rank_workspace_bytes)
     R, D = x.shape
-    if targets.shape != (R,):
-        raise ValueError(f"targets must be [{R}] (one per row of x), got {tuple(targets.shape)}")
-    check_exclude_arg(exclude, R, x.device)
     Cn = table_bf16.shape[0]
-    xc = x.detach().contiguous().float()
-    ex = exclude.contiguous() if exclude is not None and exclude.shape[1] > 0 else None
-    E = ex.shape[1] if ex is not None else 0
-    nbytes = lib.grb_head_rank_workspace_bytes(R, D, Cn, E)
-    if nbytes == 0:
-        raise _lib.GrbError(lib.grb_last_error().decode())
-    ws = _u8(nbytes, x.device)
     if metrics is None:
         metrics = torch.zeros(6, dtype=torch.float32, device=x.device)
     ranks = torch.empty(R, dtype=torch.int32, device=x.device) if want_ranks else None

@@ -85,7 +85,7 @@ def test_fewer_eligible_items_than_k():
 
 
 def _split_edges(R, C):
-    """first item of every per-CTA item range of the kernel (the split rule of topk_splits in api.cu)"""
+    """first item of every per-CTA item range of the kernel (the split rule of carve_sweep in api.cu)"""
     num_m, num_n = -(-R // 128), -(-C // 128)
     splits = max(1, min(torch.cuda.get_device_properties(0).multi_processor_count // num_m, num_n, 256))
     return sorted({s * num_n // splits * 128 for s in range(1, splits)})
