@@ -104,6 +104,9 @@ SIGNATURES = {
     "grb_head_topk_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "grb_head_topk": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
                               c_void_p, c_void_p, c_void_p]),
+    "grb_head_candidates_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "grb_head_candidates": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                                    c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_eval_rank_metrics": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "grb_head_rank_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "grb_head_rank": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,

@@ -18,6 +18,7 @@
 #include "common.cuh"
 #include "dp_adam.cuh"
 #include "exact_f32.cuh"
+#include "head_candidates.cuh"
 #include "head_rank.cuh"
 #include "head_topk.cuh"
 #include "lazy_adam.cuh"
@@ -1169,6 +1170,21 @@ int topk_check(int R, int D, int C, int k, int E) {
     GRB_REQUIRE(k >= 1 && k <= TOPK_MAX_K, "k must lie in [1, %d], got %d", TOPK_MAX_K, k);
     return 0;
 }
+// the top-k head for k <= TOPK_MAX_K (grb_head_topk, and grb_head_candidates at such k); the caller has checked the arguments
+int topk_run(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D, int C, int k,
+             const int64_t* exclude, int E, float* scores, int64_t* items, void* workspace, cudaStream_t st) {
+    const TopkWork w = carve_topk(workspace, R, D, C, k, E);
+    CUtensorMap tmA, tmB;
+    GRB_TRY(sweep_prologue(x, ln_g, ln_b, ln_eps, table_bf16, R, D, C, exclude, E, workspace, w, &tmA, &tmB, st));
+    HeadTopkArgs a{R, C, k, E, w.splits, w.num_n, D / TC_BK, w.excl, w.cand_s, w.cand_i};
+    GRB_TRY(set_smem(head_topk_kernel, TC_SMEM_BYTES));
+    launch_k(head_topk_kernel, w.num_m * w.splits, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, a);
+    GRB_CUDA(cudaGetLastError());
+    launch_k(topk_merge_kernel, (R + TOPK_MERGE_ROWS - 1) / TOPK_MERGE_ROWS, 32 * TOPK_MERGE_ROWS, 0, st, (const float*)w.cand_s,
+             (const int*)w.cand_i, R, w.splits, k, scores, reinterpret_cast<long long*>(items));
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
 }  // namespace
 
 size_t grb_head_topk_workspace_bytes(int R, int D, int C, int k, int E) {
@@ -1180,16 +1196,93 @@ int grb_head_topk(const float* x, const float* ln_g, const float* ln_b, float ln
                   const int64_t* exclude, int E, float* scores, int64_t* items, void* workspace, void* stream) {
     GRB_REQUIRE(scores && items, "null argument: scores / items");
     GRB_TRY(topk_check(R, D, C, k, E));
+    return topk_run(x, ln_g, ln_b, ln_eps, table_bf16, R, D, C, k, exclude, E, scores, items, workspace, static_cast<cudaStream_t>(stream));
+}
+
+namespace {
+// grb_head_candidates for k > TOPK_MAX_K (head_candidates.cuh)
+struct CandWork : SweepWork {
+    unsigned long long *lists, *tau, *prefix;  // [R, splits, 4, CAND_M], [R], [R]
+    int *krem, *cnt, *redo, *hist;             // [R], [R], [R], [R, 256]
+    float* buf_s; int* buf_i;                  // [R, cap]
+    int cap;
+    size_t bytes;
+};
+CandWork carve_cand(void* base, int R, int D, int C, int k, int E) {
+    CandWork w;
+    Carver c{static_cast<char*>(base)};
+    carve_sweep(c, w, R, D, C, E);
+    // the bound sweep lists 4 CAND_M pairs per (row, range): take enough ranges that a row lists at least 2 k of them, even when
+    // that is more CTAs than one wave (B = 1,024 has 16 ranges per row tile on an H100).  With only k listed, the k-th would be the
+    // worst of them and collect far more than the buffer holds.
+    const int need = (CAND_LIST_PER_K * k + 4 * CAND_M - 1) / (4 * CAND_M);
+    if (w.splits < need) w.splits = need < w.num_n ? need : w.num_n;
+    w.cap = CAND_CAP_PER_K * k;
+    w.lists = c.take<unsigned long long>((size_t)R * w.splits * 4 * CAND_M * 8);
+    w.tau = c.take<unsigned long long>((size_t)R * 8);
+    w.prefix = c.take<unsigned long long>((size_t)R * 8);
+    w.krem = c.take<int>((size_t)R * 4);
+    w.cnt = c.take<int>((size_t)R * 4);
+    w.redo = c.take<int>((size_t)R * 4);
+    w.hist = c.take<int>((size_t)R * 256 * 4);
+    w.buf_s = c.take<float>((size_t)R * w.cap * 4);
+    w.buf_i = c.take<int>((size_t)R * w.cap * 4);
+    w.bytes = c.off;
+    return w;
+}
+int cand_check(int R, int D, int C, int k, int E) {
+    GRB_TRY(sweep_check(R, D, C, E));
+    GRB_REQUIRE(k >= 1 && k <= CAND_MAX_K, "k must lie in [1, %d], got %d", CAND_MAX_K, k);
+    return 0;
+}
+using CandSweep = void (*)(const CUtensorMap, const CUtensorMap, HeadCandArgs, int);
+int cand_sweep(CandSweep kern, const CUtensorMap& tmA, const CUtensorMap& tmB, const HeadCandArgs& a, unsigned grid, int pass,
+               cudaStream_t st) {
+    GRB_TRY(set_smem(kern, RANK_SMEM_BYTES));
+    launch_k(kern, grid, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmB, a, pass);
+    GRB_CUDA(cudaGetLastError());
+    return 0;
+}
+int cand_sweeps(const CUtensorMap& tmA, const CUtensorMap& tmB, const HeadCandArgs& a, unsigned grid, cudaStream_t st) {
+    const bool ex = a.E > 0;
+    GRB_TRY(cand_sweep(ex ? head_cand_sweep_kernel<CAND_BOUND, true> : head_cand_sweep_kernel<CAND_BOUND, false>, tmA, tmB, a, grid, 0, st));
+    launch_k(head_cand_threshold_kernel, a.R, 256, 0, st, a);
+    GRB_CUDA(cudaGetLastError());
+    GRB_TRY(cand_sweep(ex ? head_cand_sweep_kernel<CAND_COLLECT, true> : head_cand_sweep_kernel<CAND_COLLECT, false>, tmA, tmB, a, grid, 0, st));
+    // refinement of the rows whose buffer overflowed: always launched, so the launch sequence does not depend on the data
+    for (int p = 0; p < CAND_RADIX_PASSES; ++p) {
+        GRB_TRY(cand_sweep(ex ? head_cand_sweep_kernel<CAND_HIST, true> : head_cand_sweep_kernel<CAND_HIST, false>, tmA, tmB, a, grid, p, st));
+        launch_k(head_cand_digit_kernel, (a.R + CAND_DIGIT_THREADS / 32 - 1) / (CAND_DIGIT_THREADS / 32), CAND_DIGIT_THREADS, 0, st, a, p);
+        GRB_CUDA(cudaGetLastError());
+    }
+    return cand_sweep(ex ? head_cand_sweep_kernel<CAND_RECOLLECT, true> : head_cand_sweep_kernel<CAND_RECOLLECT, false>, tmA, tmB, a, grid,
+                      0, st);
+}
+}  // namespace
+
+size_t grb_head_candidates_workspace_bytes(int R, int D, int C, int k, int E) {
+    if (cand_check(R, D, C, k, E)) return 0;
+    return k <= TOPK_MAX_K ? carve_topk(nullptr, R, D, C, k, E).bytes : carve_cand(nullptr, R, D, C, k, E).bytes;
+}
+
+int grb_head_candidates(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D, int C,
+                        int k, const int64_t* exclude, int E, float* scores, int64_t* items, void* workspace, void* stream) {
+    GRB_REQUIRE(scores && items, "null argument: scores / items");
+    GRB_TRY(cand_check(R, D, C, k, E));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const TopkWork w = carve_topk(workspace, R, D, C, k, E);
+    if (k <= TOPK_MAX_K) return topk_run(x, ln_g, ln_b, ln_eps, table_bf16, R, D, C, k, exclude, E, scores, items, workspace, st);
+    const CandWork w = carve_cand(workspace, R, D, C, k, E);
     CUtensorMap tmA, tmB;
     GRB_TRY(sweep_prologue(x, ln_g, ln_b, ln_eps, table_bf16, R, D, C, exclude, E, workspace, w, &tmA, &tmB, st));
-    HeadTopkArgs a{R, C, k, E, w.splits, w.num_n, D / TC_BK, w.excl, w.cand_s, w.cand_i};
-    GRB_TRY(set_smem(head_topk_kernel, TC_SMEM_BYTES));
-    launch_k(head_topk_kernel, w.num_m * w.splits, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, a);
-    GRB_CUDA(cudaGetLastError());
-    launch_k(topk_merge_kernel, (R + TOPK_MERGE_ROWS - 1) / TOPK_MERGE_ROWS, 32 * TOPK_MERGE_ROWS, 0, st, (const float*)w.cand_s,
-             (const int*)w.cand_i, R, w.splits, k, scores, reinterpret_cast<long long*>(items));
+    const HeadCandArgs a{R, C, k, E, w.cap, w.splits, w.num_n, D / TC_BK, w.excl, w.lists, w.tau, w.prefix, w.krem, w.cnt, w.redo,
+                         w.hist, w.buf_s, w.buf_i};
+    const unsigned grid = (unsigned)(w.num_m * w.splits);
+    GRB_TRY(cand_sweeps(tmA, tmB, a, grid, st));
+    int P = 1;
+    while (P < w.cap) P <<= 1;
+    const size_t sort_bytes = (size_t)P * 12;   // keys and scores
+    GRB_TRY(set_smem(head_cand_select_kernel, sort_bytes));
+    launch_k(head_cand_select_kernel, R, CAND_SELECT_THREADS, sort_bytes, st, a, scores, reinterpret_cast<long long*>(items));
     GRB_CUDA(cudaGetLastError());
     return 0;
 }

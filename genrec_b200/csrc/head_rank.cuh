@@ -22,12 +22,6 @@
 
 namespace grb {
 
-// A CTA keeps one row tile: its LN(x) operand (up to D / 64 = 4 k-blocks of 16 KB) is loaded once and stays in shared memory, and
-// the ring carries table tiles only, 8 stages of 16 KB.
-constexpr int RANK_STAGES = 8;
-constexpr int RANK_MAX_KBLOCKS = 4;
-constexpr int RANK_SMEM_BYTES = (RANK_MAX_KBLOCKS + RANK_STAGES) * TC_TILE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-
 struct HeadRankArgs {
     int R, C, E;
     int splits, num_n, kblocks;
@@ -56,52 +50,6 @@ __global__ void __launch_bounds__(256) head_rank_gather_kernel(const bf16* __res
         a.cnt[r] = 0;
     }
 }
-
-// ------------------------------------------------------------------------------------------------ CTA steps
-struct RankSmem {
-    unsigned char *sA, *sB;                      // sA: [kblocks] resident A tiles ; sB: [RANK_STAGES] ring of B tiles
-    uint64_t *full_bar, *empty_bar, *a_bar;
-};
-// carve the shared memory, initialise the barriers and wait for the previous kernel
-GRB_DEVINL RankSmem rank_cta_init(unsigned char* raw, const CUtensorMap* tmA, const CUtensorMap* tmB) {
-    unsigned char* base = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
-    RankSmem s;
-    s.sA = base;
-    s.sB = base + RANK_MAX_KBLOCKS * TC_TILE_BYTES;
-    s.full_bar = reinterpret_cast<uint64_t*>(base + (RANK_MAX_KBLOCKS + RANK_STAGES) * TC_TILE_BYTES);
-    s.empty_bar = s.full_bar + RANK_STAGES;
-    s.a_bar = s.empty_bar + RANK_STAGES;
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(tmA);
-        tma_prefetch_desc(tmB);
-        for (int i = 0; i < RANK_STAGES; ++i) {
-            mbar_init(&s.full_bar[i], 1);
-            mbar_init(&s.empty_bar[i], 2);
-        }
-        mbar_init(s.a_bar, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
-    pdl_wait();
-    return s;
-}
-// TMA producer (one lane): row tile m0 of A once, then the B tiles starting at rows b0, b0 + 128, ... (ntiles of them)
-GRB_DEVINL void rank_produce(const CUtensorMap* tmA, const CUtensorMap* tmB, const RankSmem& s, int m0, int b0, int ntiles, int kblocks) {
-    mbar_expect_tx(s.a_bar, kblocks * TC_TILE_BYTES);
-    for (int kb = 0; kb < kblocks; ++kb) tma_load_2d(s.sA + kb * TC_TILE_BYTES, tmA, kb * TC_BK, m0, s.a_bar);
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int n = 0; n < ntiles; ++n) {
-        for (int kb = 0; kb < kblocks; ++kb) {
-            mbar_wait(&s.empty_bar[stage], phase ^ 1);
-            mbar_expect_tx(&s.full_bar[stage], TC_TILE_BYTES);
-            tma_load_2d(s.sB + stage * TC_TILE_BYTES, tmB, kb * TC_BK, b0 + n * TC_BN, &s.full_bar[stage]);
-            if (++stage == RANK_STAGES) { stage = 0; phase ^= 1; }
-        }
-    }
-}
-// tile row of accumulator row i (0, 1) of this consumer thread: wgmma D fragment rows lane / 4 and lane / 4 + 8 of the warp's 16
-GRB_DEVINL int rank_frag_row(int g, int i) { return g * 64 + ((threadIdx.x >> 5) & 3) * 16 + ((threadIdx.x & 31) >> 2) + 8 * i; }
 
 // ------------------------------------------------------------------------------------------------ target scores
 __global__ void __launch_bounds__(TC_THREADS, 1)

@@ -32,16 +32,6 @@ struct HeadTopkArgs {
     int* cand_i;                // [R, splits, k]
 };
 
-// total order of every list: the higher score first, then the lower id
-GRB_DEVINL bool topk_better(float s, int id, float s2, int id2) { return s > s2 || (s == s2 && id < id2); }
-
-// order-preserving unsigned key of a float score (-0 and +0 compare equal, so they share a key)
-GRB_DEVINL unsigned topk_key(float s) {
-    unsigned b = __float_as_uint(s);
-    if ((b << 1) == 0u) b = 0u;
-    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-
 // One warp merges the candidates ok[q] (score v[q], item id[q]; lane holds 4) into the row's sorted list ls / li [k] in shared
 // memory.  When more than k candidates pass, those with at least k others of strictly higher score cannot enter and are dropped
 // first (the k-th largest key, found bit by bit with ballots).  Then every entry's new slot is its rank in the union, i.e. the

@@ -463,6 +463,35 @@ def head_topk(x, ln_g, ln_b, table_bf16, eps, k: int, exclude: Optional[torch.Te
     return TopItems(scores, items)
 
 
+CANDIDATES_MAX_K = 2048
+
+
+def check_candidates_args(k: int, exclude: Optional[torch.Tensor], rows: int, device) -> None:
+    """ValueError unless 1 <= k <= 2048 and ``exclude`` is None or an int64 [rows, E <= 16384] tensor on ``device``."""
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= CANDIDATES_MAX_K:
+        raise ValueError(f"num_candidates must be an int in [1, {CANDIDATES_MAX_K}], got {k!r}")
+    check_exclude_arg(exclude, rows, device)
+
+
+def head_candidates(x, ln_g, ln_b, table_bf16, eps, k: int, exclude: Optional[torch.Tensor] = None) -> TopItems:
+    """``head_topk`` for up to 2048 items per row (grb_head_candidates): the ``k`` best items of every row of ``x`` [R, D] under
+    the tied head, best first, without forming the logits.  Same rules: scores bit-identical to ``head_logits``, item 0 and the
+    row's ``exclude`` ids never appear, ties go to the lower item id, (-inf, 0) where no eligible item is left.  Memory grows with
+    R * k and R * E, not with the catalog.  Inference only (no autograd)."""
+    lib = _lib.load()
+    require_cuda(x, table_bf16)
+    xc, ex, E, ws = _sweep_inputs(x, table_bf16, exclude, lambda R: check_candidates_args(k, exclude, R, x.device),
+                                  lambda R, D, Cn, E: lib.grb_head_candidates_workspace_bytes(R, D, Cn, k, E))
+    R, D = x.shape
+    Cn = table_bf16.shape[0]
+    scores = torch.empty(R, k, dtype=torch.float32, device=x.device)
+    items = torch.empty(R, k, dtype=torch.int64, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib.grb_head_candidates(ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), R, D, Cn, k, ptr(ex),
+                                      E, ptr(scores), ptr(items), ptr(ws), stream_ptr(x.device)))
+    return TopItems(scores, items)
+
+
 def eval_rank_metrics(logits_last: torch.Tensor, targets: torch.Tensor, metrics: Optional[torch.Tensor] = None,
                       want_ranks: bool = False):
     """logits_last [B, C] fp32, targets [B] int64 -> metrics [6] fp32 accumulated on the device:

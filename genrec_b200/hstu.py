@@ -535,16 +535,38 @@ class HSTU(nn.Module):
         x = self.encode(input_ids, timestamps)
         return self._hidden_topk(x[:, -1, :], top_k, exclude)
 
+    @torch.no_grad()
+    def retrieve(self, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None, num_candidates: int = 500,
+                 exclude: Optional[torch.Tensor] = None) -> Fn.TopItems:
+        """The retrieval stage of serving: ``recommend`` for up to 2048 items per row.  The ``num_candidates`` (1..2048) best next
+        items of each row, best first, as ``TopItems(scores [B, num_candidates] fp32, items [B, num_candidates] int64)``, without
+        forming the [B, V+1] logits, under ``recommend``'s rules (scores bit-identical to ``last_logits``, item 0 and ``exclude``
+        ids left out, ties to the lower id, (-inf, 0) where no eligible item is left).  bf16 precision only."""
+        self._check_candidates("retrieve", num_candidates, exclude, input_ids.shape[0], input_ids.device)
+        x = self.encode(input_ids, timestamps)
+        return self._hidden_select(x[:, -1, :], None, num_candidates, exclude)
+
     def _check_topk(self, what: str, top_k: int, exclude: Optional[torch.Tensor], rows: int, device) -> None:
         if self.precision == "fp32":
             raise RuntimeError(f"genrec_b200: {what} runs the bf16 path only; set_precision('bf16') or use last_logits")
         Fn.check_topk_args(top_k, exclude, rows, device)
 
-    def _check_serving_topk(self, what: str, top_k: Optional[int], exclude: Optional[torch.Tensor], rows: int, device) -> None:
-        """Argument check of the top_k / exclude keywords of extend and extend_users (before any launch)."""
+    def _check_candidates(self, what: str, num_candidates: int, exclude: Optional[torch.Tensor], rows: int, device) -> None:
+        if self.precision == "fp32":
+            raise RuntimeError(f"genrec_b200: {what} runs the bf16 path only; set_precision('bf16') or use last_logits")
+        Fn.check_candidates_args(num_candidates, exclude, rows, device)
+
+    def _check_serving_topk(self, what: str, top_k: Optional[int], num_candidates: Optional[int], exclude: Optional[torch.Tensor],
+                            rows: int, device) -> None:
+        """Argument check of the top_k / num_candidates / exclude keywords of extend and extend_users (before any launch)."""
+        if top_k is not None and num_candidates is not None:
+            raise ValueError(f"{what}: give top_k or num_candidates, not both")
+        if num_candidates is not None:
+            self._check_candidates(what, num_candidates, exclude, rows, device)
+            return
         if top_k is None:
             if exclude is not None:
-                raise ValueError(f"{what}: exclude needs top_k")
+                raise ValueError(f"{what}: exclude needs top_k or num_candidates")
             return
         self._check_topk(what, top_k, exclude, rows, device)
 
@@ -552,18 +574,29 @@ class HSTU(nn.Module):
         return Fn.head_topk(hidden, self.final_norm.weight, self.final_norm.bias, self._table_mirror(), self.final_norm.eps, top_k,
                             exclude)
 
+    def _hidden_select(self, hidden: torch.Tensor, top_k: Optional[int], num_candidates: Optional[int],
+                       exclude: Optional[torch.Tensor]):
+        """TopItems of ``hidden`` for top_k or num_candidates, or the logits when neither is given."""
+        if top_k is not None:
+            return self._hidden_topk(hidden, top_k, exclude)
+        if num_candidates is not None:
+            return Fn.head_candidates(hidden, self.final_norm.weight, self.final_norm.bias, self._table_mirror(), self.final_norm.eps,
+                                      num_candidates, exclude)
+        return self._hidden_logits(hidden)
+
     def new_state(self, batch_size: int, capacity: int) -> HSTUState:
         """An empty cache for ``batch_size`` users of up to ``capacity`` items each (<= 16384), on the model's device."""
         return HSTUState(batch_size, capacity, len(self.layers), self.embed_dim, self.item_embedding.weight.device)
 
     @torch.no_grad()
     def extend(self, state: HSTUState, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None, *, top_k: Optional[int] = None,
-               exclude: Optional[torch.Tensor] = None):
+               num_candidates: Optional[int] = None, exclude: Optional[torch.Tensor] = None):
         """Append the non-zero ids of each row of ``input_ids`` [B, n] (with ``timestamps`` [B, n] or None), in order, to that user's
         history in ``state`` and return [B, V+1] fp32: the next-item logits of each user's latest item, as ``last_logits`` computes
         them for the left-padded concatenation of everything extended so far.  Prefilling a history is ``extend`` on a new state.
         With ``top_k`` (1..64) it returns ``TopItems`` of the same rows instead, as ``recommend`` selects them from those logits
-        (``exclude`` [B, E] int64: ids left out per row), and the logits are never formed.
+        (``exclude`` [B, E] int64: ids left out per row), and the logits are never formed; ``num_candidates`` (1..2048, not together
+        with ``top_k``) does the same for up to 2048 items, as ``retrieve`` selects them.
 
         Only the new items run through the blocks; the earlier ones are read from the cache.  Pads inside a chunk are compacted
         (positions count items): with the reference's position bias, where every causal cell uses one bucket, any padding pattern
@@ -579,7 +612,7 @@ class HSTU(nn.Module):
         if B != state.batch_size or input_ids.device != state.lengths.device:
             raise ValueError(f"the state holds {state.batch_size} users on {state.lengths.device}; got input_ids {tuple(input_ids.shape)} on "
                              f"{input_ids.device}")
-        self._check_serving_topk("extend", top_k, exclude, B, input_ids.device)
+        self._check_serving_topk("extend", top_k, num_candidates, exclude, B, input_ids.device)
         if state.items_bound + n > state.capacity:
             raise ValueError(f"extending by {n} items could exceed the state's capacity ({state.items_bound} of {state.capacity} may be "
                              "used); start a new state with a larger capacity")
@@ -592,9 +625,7 @@ class HSTU(nn.Module):
         latest = x[torch.arange(B, device=dev), last_row.clamp(min=0).long()]
         state.last_hidden.copy_(torch.where((last_row >= 0)[:, None], latest, state.last_hidden))
         state.items_bound += n
-        if top_k is not None:
-            return self._hidden_topk(state.last_hidden, top_k, exclude)
-        return self._hidden_logits(state.last_hidden)
+        return self._hidden_select(state.last_hidden, top_k, num_candidates, exclude)
 
     def _check_extend_mode(self, what: str) -> None:
         if self.precision == "fp32":
@@ -642,13 +673,14 @@ class HSTU(nn.Module):
 
     @torch.no_grad()
     def extend_users(self, pool: HSTUPool, users, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None, *,
-                     top_k: Optional[int] = None, exclude: Optional[torch.Tensor] = None):
+                     top_k: Optional[int] = None, num_candidates: Optional[int] = None, exclude: Optional[torch.Tensor] = None):
         """``extend`` for the users named by ``users`` [B] (int64, distinct, any subset of the pool's users in any order): append the
         non-zero ids of row b of ``input_ids`` [B, n] to the history of user ``users[b]`` in ``pool`` and return [B, V+1] fp32, row b
         being that user's next-item logits - what ``extend`` returns for the same user, i.e. ``last_logits`` of the left-padded
         concatenation of every item extended for them since their last ``pool.release``.  An all-pad row leaves its user untouched
         and returns their previous logits.  With ``top_k`` (1..64) it returns ``TopItems`` of the same rows instead (``exclude`` [B, E]
-        int64: ids left out per row), selected without forming the logits.
+        int64: ids left out per row), selected without forming the logits; ``num_candidates`` (1..2048, not together with ``top_k``)
+        returns up to 2048 of them, as ``retrieve`` does.
 
         With ``users`` on the CPU the call is refused before any launch if a user is out of range or repeated, or if the host
         bounds say a user could exceed ``max_items`` or the pool could run out of pages.  With ``users`` on the device (CUDA graphs)
@@ -665,7 +697,7 @@ class HSTU(nn.Module):
         users = torch.as_tensor(users, dtype=torch.int64) if not isinstance(users, torch.Tensor) else users
         if users.shape != (B,):
             raise ValueError(f"users must have one entry per row of input_ids ({B}), got shape {tuple(users.shape)}")
-        self._check_serving_topk("extend_users", top_k, exclude, B, dev)
+        self._check_serving_topk("extend_users", top_k, num_candidates, exclude, B, dev)
         bound = None
         if not users.is_cuda:
             u_host = pool._host_users(users)
@@ -682,9 +714,7 @@ class HSTU(nn.Module):
         pool.last_hidden[slot] = hidden
         if bound is not None:
             pool.items_bound[u_host], pool.pages_bound = bound
-        if top_k is not None:
-            return self._hidden_topk(hidden, top_k, exclude)
-        return self._hidden_logits(hidden)
+        return self._hidden_select(hidden, top_k, num_candidates, exclude)
 
     @torch.no_grad()
     def evaluate_batch(self, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor], targets: torch.Tensor,

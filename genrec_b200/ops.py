@@ -195,6 +195,20 @@ def _(x, ln_g, ln_b, table_bf16, eps, k, exclude):
     return x.new_empty((R, k), dtype=torch.float32), x.new_empty((R, k), dtype=torch.int64)
 
 
+@custom_op(f"{NS}::head_candidates", mutates_args=())
+def head_candidates(x: Tensor, ln_g: Tensor, ln_b: Tensor, table_bf16: Tensor, eps: float, k: int,
+                    exclude: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
+    """head_topk for up to 2048 items per row: x [R, D] fp32 -> (scores [R, k] fp32, items [R, k] int64), 1 <= k <= 2048, the
+    same selection rules, without the logits.  Inference only."""
+    return tuple(Fn.head_candidates(x, ln_g, ln_b, table_bf16, eps, k, exclude))
+
+
+@head_candidates.register_fake
+def _(x, ln_g, ln_b, table_bf16, eps, k, exclude):
+    R = x.shape[0]
+    return x.new_empty((R, k), dtype=torch.float32), x.new_empty((R, k), dtype=torch.int64)
+
+
 @custom_op(f"{NS}::head_rank_metrics", mutates_args=())
 def head_rank_metrics(x: Tensor, ln_g: Tensor, ln_b: Tensor, table_bf16: Tensor, eps: float, targets: Tensor,
                       exclude: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
@@ -289,4 +303,5 @@ torch.library.register_autograd(f"{NS}::sasrec_attention", _sas_backward, setup_
 
 
 OPS = ("hstu_attention", "hstu_attention_backward", "hstu_layer", "hstu_layer_backward", "rq_residual_argmin", "rq_sinkhorn",
-       "eval_rank_metrics", "head_topk", "head_rank_metrics", "head_sampled_loss", "sasrec_attention", "sasrec_attention_backward")
+       "eval_rank_metrics", "head_topk", "head_candidates", "head_rank_metrics", "head_sampled_loss", "sasrec_attention",
+       "sasrec_attention_backward")

@@ -296,6 +296,15 @@ class SASRec(nn.Module):
                             self.final_norm.eps, top_k, exclude)
 
     @torch.no_grad()
+    def retrieve(self, input_ids: torch.Tensor, num_candidates: int = 500, exclude: Optional[torch.Tensor] = None) -> Fn.TopItems:
+        """``recommend`` for up to 2048 items per row: the ``num_candidates`` (1..2048) best next items of each row as
+        ``TopItems(scores, items)``, under the same rules, without forming the logits (see ``HSTU.retrieve``)."""
+        Fn.check_candidates_args(num_candidates, exclude, input_ids.shape[0], input_ids.device)
+        x = self.encode(input_ids)
+        return Fn.head_candidates(x[:, -1, :], self.final_norm.weight, self.final_norm.bias, Fn.cast_bf16(self.item_embedding.weight),
+                                  self.final_norm.eps, num_candidates, exclude)
+
+    @torch.no_grad()
     def evaluate_batch(self, input_ids: torch.Tensor, targets: torch.Tensor, metrics: Optional[torch.Tensor] = None, *,
                        exclude: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Leave-one-out metrics of one evaluation batch, accumulated on the device into ``metrics`` ([6] fp32: Recall@{1,5,10} hit

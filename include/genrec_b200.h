@@ -243,6 +243,17 @@ int grb_head_logits(const float* x, const float* ln_g, const float* ln_b, float 
 size_t grb_head_topk_workspace_bytes(int R, int D, int C, int k, int E);
 int grb_head_topk(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D, int C,
                   int k, const int64_t* exclude, int E, float* scores, int64_t* items, void* workspace, void* stream);
+/* Retrieval: grb_head_topk for up to 2048 candidates per row.  The same contract (best first in the total order, scores
+ * bit-identical to grb_head_logits, item 0 and the row's exclude ids never appear, (-inf, 0) in the slots without an eligible
+ * item), with 1 <= k <= 2048.  k <= 64 runs grb_head_topk's kernels; larger k sweeps the table twice (a bound on each row's
+ * k-th score, then a collect of the items at or above it) and sorts what it collected; a row whose collect buffer (4 k pairs)
+ * overflows, such as one of a flat table, is resolved exactly by up to 8 more radix sweeps that skip every other row.
+ * Deterministic; no host synchronisation and a launch sequence that does not depend on the data (CUDA-graph capturable).
+ * workspace: grb_head_candidates_workspace_bytes(), which grows with R * k, R * E and R * (item ranges), not with C (0 for
+ * unsupported arguments). */
+size_t grb_head_candidates_workspace_bytes(int R, int D, int C, int k, int E);
+int grb_head_candidates(const float* x, const float* ln_g, const float* ln_b, float ln_eps, const void* table_bf16, int R, int D,
+                        int C, int k, const int64_t* exclude, int E, float* scores, int64_t* items, void* workspace, void* stream);
 
 /* Leave-one-out evaluation without host round trips (replaces the per-sample loop of genrec/trainers/hstu_trainer.py:55-81):
  * logits [B, C] fp32 of the LAST position, targets [B] (0 = skip).  The rank of the target among classes 1..C-1 (class 0 is

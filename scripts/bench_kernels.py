@@ -4,7 +4,7 @@ roofline or the torch code they replace.  Prints one JSON line per measurement; 
 training rows, `bench_kernels.py linear_bwd` only the linear-backward and SASRec training-step rows, `bench_kernels.py head_topk` only
 the fused top-k head rows, `bench_kernels.py tiger` only the TIGER rows (training step, generate eager / graph / uncached loop),
 `bench_kernels.py hstu_attn` only the HSTU attention backward rows, `bench_kernels.py head_rank` only the rows of evaluation without
-logits."""
+logits, `bench_kernels.py head_candidates` only the rows of retrieval without logits."""
 import json
 import os
 import sys
@@ -203,6 +203,104 @@ def bench_head_topk(dev):
     f_ms, b_ms = graph_timed(lambda: one(top_k=10)), graph_timed(one_topk)
     print(json.dumps(dict(kernel="head_topk", workload="extend_users", geometry=name, pool_users=nusers, B=B, k=10, max_items=cap,
                           fused_us=f_ms * 1e3, logits_topk_us=b_ms * 1e3, speedup_vs_logits_topk=b_ms / f_ms, **info)), flush=True)
+
+
+def kernels_us(fn, prefix, iters=20):
+    """Mean device time (us) per call of every kernel whose name contains `prefix`, from a torch.profiler run of its own."""
+    from torch.profiler import ProfilerActivity, profile
+    fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(iters):
+            fn()
+        torch.cuda.synchronize()
+    return {k.key.split("(")[0][:80]: k.device_time_total / iters for k in prof.key_averages() if prefix in k.key}
+
+
+def bench_head_candidates(dev):
+    """Retrieval without logits (Fn.head_candidates: LayerNorm, bound sweep, threshold, collect sweep, overflow passes, sort)
+    against the logits path (Fn.head_logits, column 0 set to -inf, torch.topk), both graph-captured, at D = 128: C = 12,102 and
+    1,000,001, B = 1, 128 and 1,024, k = 64 (the top-k head), 256, 1,024 and 2,048.  Then a clustered table whose best 3,000 items
+    sit in one item range for every row, the per-kernel times (torch.profiler, a run of their own) and extend_users(num_candidates=
+    500) on the cfg2 pool workload against extend_users + torch.topk.  The one-sweep bound is the larger of the table read (C D 2
+    bytes at 3.35 TB/s) and the GEMM (2 B C D FLOP at 989 TFLOP/s), H100 SXM data-sheet figures; peak memory is
+    torch.cuda.max_memory_allocated above the inputs."""
+    info = card()
+    HBM, BF16 = 3.35e12, 989e12
+    D, eps = 128, 1e-5
+    gd = torch.Generator(device=dev).manual_seed(0)
+
+    def peak_mb(fn):
+        fn()
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        base = torch.cuda.memory_allocated()
+        fn()
+        torch.cuda.synchronize()
+        return (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+
+    def measure(workload, x, ln_g, ln_b, tb, k, profile_kernels):
+        B, C = x.shape[0], tb.shape[0]
+
+        def fused():
+            return Fn.head_candidates(x, ln_g, ln_b, tb, eps, k)
+
+        def logits_topk():
+            lo = Fn.head_logits(x[:, None, :], ln_g, ln_b, tb, tb, eps)[:, 0, :]
+            lo[:, 0] = float("-inf")
+            return torch.topk(lo, k, dim=1)
+
+        assert torch.equal(fused().scores, logits_topk().values)
+        f_ms = graph_timed(fused)
+        b_ms = graph_timed(logits_topk, reps=2, iters=5)
+        t_bytes, t_flop = C * D * 2 / HBM * 1e6, 2 * B * C * D / BF16 * 1e6
+        bound = max(t_bytes, t_flop)
+        row = dict(kernel="head_candidates", workload=workload, D=D, C=C, B=B, k=k, fused_us=f_ms * 1e3, logits_topk_us=b_ms * 1e3,
+                   speedup_vs_logits_topk=b_ms / f_ms, bound_us=bound, bound_by="table read" if t_bytes >= t_flop else "bf16 GEMM",
+                   fused_over_bound=f_ms * 1e3 / bound, fused_peak_mb=peak_mb(fused), logits_topk_peak_mb=peak_mb(logits_topk))
+        if profile_kernels:
+            row.update(kernels_us=kernels_us(fused, "head_" if k <= 64 else "head_cand"))
+        print(json.dumps(dict(**row, **info)), flush=True)
+
+    for C in (12102, 1000001):
+        tb = (0.05 * torch.randn(C, D, device=dev, generator=gd)).to(torch.bfloat16)
+        ln_g, ln_b = 1 + 0.1 * torch.randn(D, device=dev, generator=gd), 0.1 * torch.randn(D, device=dev, generator=gd)
+        for B in (1, 128, 1024):
+            x = torch.randn(B, D, device=dev, generator=gd)
+            for k in (64, 256, 1024, 2048):
+                measure("head", x, ln_g, ln_b, tb, k, profile_kernels=k in (64, 1024))
+            del x
+            torch.cuda.empty_cache()
+        del tb
+        torch.cuda.empty_cache()
+    # clustered: rows lo .. lo + 2,999 of the table score above every other item for every row of x
+    C, B, n = 1000001, 128, 3000
+    b = torch.randn(D, device=dev, generator=gd)
+    ln_g, ln_b = torch.full((D,), 0.1, device=dev), b
+    tb = 0.05 * torch.randn(C, D, device=dev, generator=gd)
+    lo = 128 * 70
+    tb[lo:lo + n] += 0.05 * b
+    tb = tb.to(torch.bfloat16)
+    x = torch.randn(B, D, device=dev, generator=gd)
+    for k in (500, 1024, 2048):
+        measure("clustered", x, ln_g, ln_b, tb, k, profile_kernels=True)
+    del tb
+    torch.cuda.empty_cache()
+    name, geo, nusers, cap, B, _ = POOL_GEOMS[0]
+    m, pool, lens, hist, hts, users, one = _pool_workload(dev, name, geo, nusers, cap, B)
+
+    def one_topk():
+        lo = one()
+        lo[:, 0] = float("-inf")
+        return torch.topk(lo, 500, dim=1)
+
+    assert torch.equal(one(num_candidates=500).scores, one_topk().values)
+    runs = {"num_candidates": [], "logits_topk": []}
+    for _ in range(3):
+        runs["num_candidates"].append(graph_timed(lambda: one(num_candidates=500)) * 1e3)
+        runs["logits_topk"].append(graph_timed(one_topk) * 1e3)
+    print(json.dumps(dict(kernel="head_candidates", workload="extend_users", geometry=name, pool_users=nusers, B=B, k=500, max_items=cap,
+                          us=runs, **info)), flush=True)
 
 
 LOGITS_CAP_GB = 16
@@ -510,6 +608,9 @@ def main():
         return
     if sys.argv[1:] == ["head_rank"]:
         bench_head_rank(dev)
+        return
+    if sys.argv[1:] == ["head_candidates"]:
+        bench_head_candidates(dev)
         return
     peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) \
         if os.path.exists("MEASURED_PEAKS.json") else {}
