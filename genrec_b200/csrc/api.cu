@@ -50,6 +50,13 @@ int fail(int code, const char* fmt, ...) {
         cudaError_t _e = (expr);                                                                        \
         if (_e != cudaSuccess) return fail(GRB_ECUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); \
     } while (0)
+// launch_k (common.cuh) that returns GRB_ECUDA, naming the kernel, when this launch fails.  A kernel whose template arguments hold a
+// comma goes in parentheses.
+#define GRB_LAUNCH(kern, ...)                                                                                         \
+    do {                                                                                                              \
+        cudaError_t _e = launch_k(kern, __VA_ARGS__);                                                                 \
+        if (_e != cudaSuccess) return fail(GRB_ECUDA, "%s:%d %s: %s", __FILE__, __LINE__, #kern, cudaGetErrorString(_e)); \
+    } while (0)
 #define GRB_REQUIRE(cond, ...)                            \
     do {                                                  \
         if (!(cond)) return fail(GRB_EINVAL, __VA_ARGS__); \
@@ -100,15 +107,13 @@ int with_head_dim(int dh, F&& f) {
     if (dh == 32) return f(std::integral_constant<int, 32>{});
     return f(std::integral_constant<int, 64>{});
 }
-// the row kernels are instantiated per D: f(integral_constant D) launches one for D = 64, 128 or 256
+// the row kernels are instantiated per D: f(integral_constant D) launches one for D = 64, 128 or 256 and returns 0 / error code
 template <class F>
 int with_row_dim(int D, F&& f) {
-    if (D == 64) f(std::integral_constant<int, 64>{});
-    else if (D == 128) f(std::integral_constant<int, 128>{});
-    else if (D == 256) f(std::integral_constant<int, 256>{});
-    else return fail(GRB_EINVAL, "row kernels support D in {64,128,256}, got %d", D);
-    GRB_CUDA(cudaGetLastError());
-    return 0;
+    if (D == 64) return f(std::integral_constant<int, 64>{});
+    if (D == 128) return f(std::integral_constant<int, 128>{});
+    if (D == 256) return f(std::integral_constant<int, 256>{});
+    return fail(GRB_EINVAL, "row kernels support D in {64,128,256}, got %d", D);
 }
 // the fused loss heads (tc_ce.cuh, tc_sampled_ce.cuh) are instantiated for D = 64 and 128: f(integral_constant D) (head_fused and
 // check_sampled_shape admit nothing else)
@@ -121,13 +126,11 @@ auto with_ce_dim(int D, F&& f) {
 // instantiated at 384: nothing calls them there.
 template <class F>
 int with_rms_dim(int D, F&& f) {
-    if (D == 64) f(std::integral_constant<int, 64>{});
-    else if (D == 128) f(std::integral_constant<int, 128>{});
-    else if (D == 256) f(std::integral_constant<int, 256>{});
-    else if (D == 384) f(std::integral_constant<int, 384>{});
-    else return fail(GRB_EINVAL, "rms norm supports D in {64,128,256,384}, got %d", D);
-    GRB_CUDA(cudaGetLastError());
-    return 0;
+    if (D == 64) return f(std::integral_constant<int, 64>{});
+    if (D == 128) return f(std::integral_constant<int, 128>{});
+    if (D == 256) return f(std::integral_constant<int, 256>{});
+    if (D == 384) return f(std::integral_constant<int, 384>{});
+    return fail(GRB_EINVAL, "rms norm supports D in {64,128,256,384}, got %d", D);
 }
 int row_grid(int T) {
     int need = (T + ROW_THREADS / 32 - 1) / (ROW_THREADS / 32);
@@ -166,8 +169,7 @@ int det_finish(const float* part, int ngroups, int nmembers, int W, int gpo, int
     int k = 0;
     for (const DetOut& o : outs) { f.out[k] = o.out; f.len[k] = o.len; ++k; }
     const unsigned blocks = (unsigned)(((size_t)ngroups * W * 32 + 255) / 256);
-    launch_k(det_finish_kernel, blocks, 256, 0, st, f);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(det_finish_kernel, blocks, 256, 0, st, f);
     return 0;
 }
 
@@ -280,13 +282,6 @@ int check_seq(const grb_hstu_dims* d, const grb_hstu_seq* s) {
     return 0;
 }
 
-// set_max_smem (common.cuh) with the library's error reporting
-template <class Kern>
-int set_smem(Kern k, size_t bytes) {
-    GRB_CUDA(set_max_smem(k, bytes));
-    return 0;
-}
-
 // the bias tables without the index matrix (bias_index null, ldix 0)
 HstuBiasArgs make_attn_bias(const grb_hstu_dims* d, const float* pos_table, const float* time_table, int has_time, int pos_uniform,
                             int pos_bucket0) {
@@ -340,10 +335,8 @@ int set_attn_bwd_args(HstuAttnArgs& a, const grb_hstu_dims* d, const grb_hstu_se
 template <int DH>
 int launch_hstu_attn_fwd(const HstuAttnArgs& a, cudaStream_t st) {
     size_t smem = sizeof(AttSmem<DH, 1>) + align_up((size_t)(a.bias.npos * 64 + 1) * 4, 16);
-    GRB_TRY(set_smem(hstu_attn_fwd_kernel<DH>, smem));
     dim3 grid((a.L + ATT_BLK - 1) / ATT_BLK, a.H, a.B);
-    launch_k(hstu_attn_fwd_kernel<DH>, grid, ATT_THREADS, smem, st, a);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(hstu_attn_fwd_kernel<DH>, grid, ATT_THREADS, smem, st, a);
     return 0;
 }
 // Fork/join helper: a non-blocking stream and its two events, created on first use, i.e. during warm-up, never while a CUDA graph
@@ -416,11 +409,9 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
     dim3 grid((a.L + ATT_BLK - 1) / ATT_BLK, a.H, a.B);
     size_t posb = align_up((size_t)(a.bias.npos * 64 + 1) * 4, 16);  // combined bias table
     size_t smem_q = sizeof(AttSmem<DH>) + posb;
-    GRB_TRY(set_smem(hstu_attn_bwd_dq_kernel<DH>, smem_q));
     SideStream& ss = attn_side_stream();
     GRB_TRY(ss.run(st, [&](cudaStream_t side) -> int {
-        launch_k(hstu_attn_bwd_dq_kernel<DH>, grid, ATT_THREADS, smem_q, side, a);
-        GRB_CUDA(cudaGetLastError());
+        GRB_LAUNCH(hstu_attn_bwd_dq_kernel<DH>, grid, ATT_THREADS, smem_q, side, a);
         return 0;
     }));
     const bool has_time = a.bias.wtime != nullptr && a.bias.ntime > 0, pos_uni = a.bias.pos_uniform != 0;
@@ -428,38 +419,29 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
                     (size_t)4 * (att_time_bins(has_time, pos_uni, a.bias.ntime) + (pos_uni ? 0 : a.bias.npos + 1)) * 32 * sizeof(float);
     const int nmem = (int)(grid.x * grid.z), ngroups = has_time && a.dwtime ? 2 * a.H : a.H;
     GRB_REQUIRE((pos_uni || a.bias.npos <= 64) && a.bias.ntime <= 64, "attention backward: at most 64 position / time buckets");
-    auto go = [&](auto kern) -> int {
-        GRB_TRY(set_smem(kern, smem_k));
-        launch_k(kern, grid, ATT_THREADS, smem_k, st, a, (int)posb);
-        return 0;
-    };
-    if (has_time && pos_uni) GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, true, true>));
-    else if (has_time) GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, true, false>));
-    else if (pos_uni) GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, false, true>));
-    else GRB_TRY(go(hstu_attn_bwd_dkdv_kernel<DH, false, false>));
+    auto dkdv_kernel = has_time ? (pos_uni ? hstu_attn_bwd_dkdv_kernel<DH, true, true> : hstu_attn_bwd_dkdv_kernel<DH, true, false>)
+                                : (pos_uni ? hstu_attn_bwd_dkdv_kernel<DH, false, true> : hstu_attn_bwd_dkdv_kernel<DH, false, false>);
+    GRB_LAUNCH(dkdv_kernel, grid, ATT_THREADS, smem_k, st, a, (int)posb);
     // groups h < H: position buckets of head h ; H + h: time buckets of head h ; element = bucket.  With uniform positions
     // the caller has already pointed dwpos at the single live row.
     float* pos_out = a.dwpos;
     const int pos_len = pos_uni ? a.H : a.bias.npos * a.H;
     if (ngroups > a.H) GRB_TRY(det_finish(a.dw_part, ngroups, nmem, 64, a.H, 1, a.H, {{pos_out, pos_len}, {a.dwtime, a.bias.ntime * a.H}}, st));
     else GRB_TRY(det_finish(a.dw_part, ngroups, nmem, 64, a.H, 1, a.H, {{pos_out, pos_len}}, st));
-    GRB_CUDA(cudaGetLastError());
     GRB_TRY(ss.join_into(st));
     return 0;
 }
 
 int cast_bf16(const float* in, bf16* out, size_t n, int D, const Dropout& drop, const float* row_scale, cudaStream_t st) {
     GRB_REQUIRE(D > 0 && D % 4 == 0 && n % (size_t)D == 0, "cast needs rows of a multiple-of-4 length D");
-    launch_k(cast_f32_bf16_kernel, capped_blocks(n / 4), 256, 0, st, in, out, n, D, drop, row_scale);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(cast_f32_bf16_kernel, capped_blocks(n / 4), 256, 0, st, in, out, n, D, drop, row_scale);
     return 0;
 }
 // part: cast_colsum_grid(T, D).x * .y * 128 floats of scratch for the ordered sum
 int cast_colsum(const float* in, bf16* out, int T, int D, const Dropout& drop, float* colsum_out, float* part, cudaStream_t st) {
     GRB_REQUIRE(D > 0 && D % 4 == 0, "cast needs rows of a multiple-of-4 length D");
     const dim3 grid = cast_colsum_grid(T, D);
-    launch_k(cast_colsum_f32_bf16_kernel, grid, 256, 0, st, in, out, T, D, drop, part);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(cast_colsum_f32_bf16_kernel, grid, 256, 0, st, in, out, T, D, drop, part);
     GRB_TRY(det_finish(part, grid.x, grid.y, 128, grid.x, 128, 1, {{colsum_out, D}}, st));
     return 0;
 }
@@ -467,14 +449,13 @@ int cast_colsum(const float* in, bf16* out, int T, int D, const Dropout& drop, f
 int colsum(const bf16* in, int T, int N, int ld, float* out, float* part, cudaStream_t st) {
     if (N % 8 != 0 || ld % 8 != 0) return fail(GRB_EINVAL, "colsum needs N and ld to be multiples of 8");
     const dim3 grid = colsum_grid(T, N);
-    launch_k(colsum_bf16_kernel, grid, 256, 0, st, in, T, N, ld, part);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(colsum_bf16_kernel, grid, 256, 0, st, in, T, N, ld, part);
     GRB_TRY(det_finish(part, grid.x, grid.y, 256, grid.x, 256, 1, {{out, N}}, st));
     return 0;
 }
 // dx = (res ? res : 0) + LNbwd(dy) ; dg += , db += in a fixed order.  a.part: 2 * row_bwd_grid(T) * D floats of scratch
 int ln_backward(const LnBwdArgs& a, cudaStream_t st) {
-    GRB_TRY(with_row_dim(a.D, [&](auto DC) { launch_k(ln_bwd_kernel<DC / 64>, row_bwd_grid(a.T), ROW_THREADS, 0, st, a); }));
+    GRB_TRY(with_row_dim(a.D, [&](auto DC) -> int { GRB_LAUNCH(ln_bwd_kernel<DC / 64>, row_bwd_grid(a.T), ROW_THREADS, 0, st, a); return 0; }));
     return det_finish(a.part, 2, row_bwd_grid(a.T), a.D, 1, 0, 1, {{a.dg, a.D}, {a.db, a.D}}, st);
 }
 
@@ -515,10 +496,8 @@ ExtendWork carve_extend(void* base, const grb_hstu_dims* d, int capacity) {
 template <int DH, bool UNIFORM, bool TIMED>
 int launch_attn_extend(const HstuExtendArgs& a, int nsplit, cudaStream_t st) {
     const size_t smem = sizeof(ExtSmem<DH>) + align_up((size_t)(a.bias.npos * 64 + 1) * 4, 16);
-    GRB_TRY(set_smem(hstu_attn_extend_kernel<DH, UNIFORM, TIMED>, smem));
     const dim3 grid(nsplit, a.H, a.B * ((a.n + ATT_BLK - 1) / ATT_BLK));
-    launch_k(hstu_attn_extend_kernel<DH, UNIFORM, TIMED>, grid, ATT_THREADS, smem, st, a);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH((hstu_attn_extend_kernel<DH, UNIFORM, TIMED>), grid, ATT_THREADS, smem, st, a);
     return 0;
 }
 template <int DH>
@@ -571,7 +550,7 @@ int block_steps_out(const grb_hstu_layer_params* p, const float* x, float* y, co
                     const Dropout& drop_hid, const Dropout& drop_out, cudaStream_t st) {
     // 4. x1 = x + drop(LN1(O) * U) ; xn = LN2(x1)                                            (hstu.py:271-278)
     LnGateFwdArgs a{sv.O, D, sv.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, sv.x1, sv.xn, sv.st1, sv.st2, T, D, 1e-5f, drop_gate};
-    GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_gate_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
+    GRB_TRY(with_row_dim(D, [&](auto DC) -> int { GRB_LAUNCH(ln_gate_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); return 0; }));
     // 5. h = drop(silu(xn W1^T + b1))                                                        (hstu.py:210-212)
     GRB_CUDA(gemm_bias_act(1, sv.xn, (const bf16*)p->ffn1_w, p->ffn1_b, sv.z1, sv.hact, T, 4 * D, D, drop_hid, st));
     // 6. y = x1 + drop(h W2^T + b2)                                                          (hstu.py:213-214, :278)
@@ -595,9 +574,8 @@ int layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const E
     GRB_TRY(block_steps_in(p, x, sv, T, D, st));
     {
         const size_t pieces = (size_t)T * (2 * D / 8);
-        launch_k(hstu_kv_scatter_kernel, (unsigned)((pieces + 255) / 256), 256, 0, st, (const bf16*)sv.P, (const int*)positions, c.users, T,
-                 d->L, D, c.pg, c.kv);
-        GRB_CUDA(cudaGetLastError());
+        GRB_LAUNCH(hstu_kv_scatter_kernel, (unsigned)((pieces + 255) / 256), 256, 0, st, (const bf16*)sv.P, (const int*)positions, c.users, T,
+                   d->L, D, c.pg, c.kv);
     }
     {
         HstuExtendArgs a;
@@ -617,9 +595,8 @@ int layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const E
         const int nsplit = (cap + a.split - 1) / a.split;
         GRB_TRY(with_head_dim(D / d->H, [&](auto DH) { return dispatch_attn_extend<DH>(a, nsplit, st); }));
         const size_t quads = (size_t)T * D / 4;
-        launch_k(hstu_extend_combine_kernel, (unsigned)((quads + 255) / 256), 256, 0, st, (const float*)w.part, (const int*)positions, T, D,
-                 a.split, sv.O);
-        GRB_CUDA(cudaGetLastError());
+        GRB_LAUNCH(hstu_extend_combine_kernel, (unsigned)((quads + 255) / 256), 256, 0, st, (const float*)w.part, (const int*)positions, T, D,
+                   a.split, sv.O);
     }
     const Dropout nodrop = make_dropout(0.f, 0, 0);
     return block_steps_out(p, x, y, sv, T, D, nodrop, nodrop, nodrop, st);
@@ -704,7 +681,7 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
     {
         LnGateBwdArgs a{dy, w.dxn, sv.x1, sv.st1, sv.st2, sv.O, D, sv.P, 4 * D, sv.zp, 4 * D, p->ln1_g, p->ln1_b, p->ln2_g,
                         w.dx1, w.dO, D, w.dzp, 4 * D, g->ln1_g, g->ln1_b, g->ln2_g, g->ln2_b, T, D, drop_gate, w.part_ln};
-        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_gate_bwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); }));
+        GRB_TRY(with_row_dim(D, [&](auto DC) -> int { GRB_LAUNCH(ln_gate_bwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); return 0; }));
         GRB_TRY(det_finish(w.part_ln, 4, row_grid(T), D, 1, 0, 1, {{a.dg1, D}, {a.db1, D}, {a.dg2, D}, {a.db2, D}}, st));
     }
     // attention backward -> gradients w.r.t. the V, Q, K pre-activations
@@ -731,11 +708,10 @@ int grb_hstu_cache_append(const grb_hstu_cache* c, const int64_t* input_ids, con
     GRB_REQUIRE(c->timestamps && c->lengths && c->overflow, "null cache pointer");
     GRB_REQUIRE(c->B > 0 && n > 0, "bad shape B=%d n=%d", c->B, n);
     GRB_REQUIRE(c->capacity >= 1 && c->capacity <= 16384, "cache capacity %d out of range [1, 16384]", c->capacity);
-    launch_k(hstu_cache_append_kernel, (unsigned)((c->B + 3) / 4), 128, 0, static_cast<cudaStream_t>(stream),
-             reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(timestamps), (const long long*)nullptr,
-             (const int*)nullptr, c->B, n, c->capacity, KvPages{nullptr, 1, c->capacity}, reinterpret_cast<long long*>(c->timestamps),
-             c->lengths, c->overflow, positions, last_row);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(hstu_cache_append_kernel, (unsigned)((c->B + 3) / 4), 128, 0, static_cast<cudaStream_t>(stream),
+               reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(timestamps), (const long long*)nullptr,
+               (const int*)nullptr, c->B, n, c->capacity, KvPages{nullptr, 1, c->capacity}, reinterpret_cast<long long*>(c->timestamps),
+               c->lengths, c->overflow, positions, last_row);
     return 0;
 }
 
@@ -750,13 +726,11 @@ int grb_hstu_pool_append(const grb_hstu_pool* pool, const int64_t* users, int B,
     HstuPoolArgs a = pool_args(pool, users, B);
     a.ids = reinterpret_cast<const long long*>(input_ids); a.n = n;
     a.room = room;
-    launch_k(hstu_pool_alloc_kernel, 1, POOL_THREADS, 0, st, a);
-    GRB_CUDA(cudaGetLastError());
-    launch_k(hstu_cache_append_kernel, (unsigned)((B + 3) / 4), 128, 0, st, reinterpret_cast<const long long*>(input_ids),
-             reinterpret_cast<const long long*>(timestamps), reinterpret_cast<const long long*>(users), (const int*)room, B, n,
-             pool->max_items, KvPages{pool->page_table, pool_pt_ld(pool), pool->page_size}, reinterpret_cast<long long*>(pool->timestamps),
-             pool->lengths, pool->overflow, positions, last_row);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(hstu_pool_alloc_kernel, 1, POOL_THREADS, 0, st, a);
+    GRB_LAUNCH(hstu_cache_append_kernel, (unsigned)((B + 3) / 4), 128, 0, st, reinterpret_cast<const long long*>(input_ids),
+               reinterpret_cast<const long long*>(timestamps), reinterpret_cast<const long long*>(users), (const int*)room, B, n,
+               pool->max_items, KvPages{pool->page_table, pool_pt_ld(pool), pool->page_size}, reinterpret_cast<long long*>(pool->timestamps),
+               pool->lengths, pool->overflow, positions, last_row);
     return 0;
 }
 
@@ -769,8 +743,7 @@ int grb_hstu_pool_release(const grb_hstu_pool* pool, const int64_t* users, int B
     GRB_REQUIRE(last_hidden == nullptr || D > 0, "last_hidden needs D > 0, got %d", D);
     HstuPoolArgs a = pool_args(pool, users, B);
     a.last_hidden = last_hidden; a.ld_hidden = D;
-    launch_k(hstu_pool_release_kernel, 1, POOL_THREADS, 0, static_cast<cudaStream_t>(stream), a);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(hstu_pool_release_kernel, 1, POOL_THREADS, 0, static_cast<cudaStream_t>(stream), a);
     return 0;
 }
 
@@ -819,9 +792,8 @@ int grb_hstu_bias_index(const int64_t* timestamps, const uint8_t* pad, const int
     GRB_REQUIRE(ntime >= 0 && ntime <= ATT_MAX_BUCKETS && npos >= 1 && npos <= ATT_MAX_BUCKETS, "bucket counts out of range");
     dim3 grid((ld_index + 255) / 256, (L + 7) / 8, B);
     auto go = [&](cudaStream_t s_) -> int {
-        launch_k(hstu_bias_index_kernel, grid, 256, 0, s_, reinterpret_cast<const long long*>(timestamps), pad,
-                 reinterpret_cast<const long long*>(time_thr), pos_bucket, L, ld_index, npos, ntime, out);
-        GRB_CUDA(cudaGetLastError());
+        GRB_LAUNCH(hstu_bias_index_kernel, grid, 256, 0, s_, reinterpret_cast<const long long*>(timestamps), pad,
+                   reinterpret_cast<const long long*>(time_thr), pos_bucket, L, ld_index, npos, ntime, out);
         return 0;
     };
     // the index matrix is first needed by the attention kernel of the first block: with the deferred schedule it is built beside
@@ -869,10 +841,9 @@ int grb_collate_jagged(const int64_t* items, const int64_t* stamps, const int64_
     GRB_REQUIRE(items && offsets && targets && out_input_ids && out_targets, "null argument");
     GRB_REQUIRE(B > 0 && L > 0, "bad shape B=%d L=%d", B, L);
     const size_t n = (size_t)B * L;
-    launch_k(collate_jagged_kernel, (unsigned)((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream), reinterpret_cast<const long long*>(items),
-             reinterpret_cast<const long long*>(stamps), reinterpret_cast<const long long*>(offsets), reinterpret_cast<const long long*>(targets), B, L,
-             reinterpret_cast<long long*>(out_input_ids), reinterpret_cast<long long*>(out_targets), reinterpret_cast<long long*>(out_timestamps));
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(collate_jagged_kernel, (unsigned)((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream), reinterpret_cast<const long long*>(items),
+               reinterpret_cast<const long long*>(stamps), reinterpret_cast<const long long*>(offsets), reinterpret_cast<const long long*>(targets), B, L,
+               reinterpret_cast<long long*>(out_input_ids), reinterpret_cast<long long*>(out_targets), reinterpret_cast<long long*>(out_timestamps));
     return 0;
 }
 
@@ -883,8 +854,7 @@ int grb_embed_forward(const int64_t* ids, const float* table, const float* pos_t
     GRB_REQUIRE(B > 0 && L > 0 && D > 0 && D % 4 == 0, "bad shape");
     EmbedArgs a{reinterpret_cast<const long long*>(ids), table, pos_table, x, pad, B * L, L, D, scale, mask_pad_rows,
                 make_dropout(dropout_p, seed, SITE_EMBED, seed_dev)};
-    launch_k(embed_fwd_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(embed_fwd_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
     return 0;
 }
 int grb_embed_backward(const int64_t* ids, const int64_t* order, const float* dx, float* dtable, float* dpos_table, int B, int L, int D,
@@ -896,14 +866,9 @@ int grb_embed_backward(const int64_t* ids, const int64_t* order, const float* dx
     EmbedBwdArgs a{reinterpret_cast<const long long*>(ids), dx, dtable, dpos_table, B * L, L, D, scale, mask_pad_rows,
                    make_dropout(dropout_p, seed, SITE_EMBED, seed_dev), reinterpret_cast<const long long*>(order)};
     const EmbedPieceArgs pa{a, scratch};
-    launch_k(embed_bwd_piece_kernel, row_grid((B * L + 31) / 32), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), pa);
-    GRB_CUDA(cudaGetLastError());
-    launch_k(embed_bwd_run_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), pa);
-    GRB_CUDA(cudaGetLastError());
-    if (dpos_table) {
-        launch_k(embed_bwd_pos_kernel, L < 8 * sm_count() ? L : 8 * sm_count(), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
-        GRB_CUDA(cudaGetLastError());
-    }
+    GRB_LAUNCH(embed_bwd_piece_kernel, row_grid((B * L + 31) / 32), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), pa);
+    GRB_LAUNCH(embed_bwd_run_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), pa);
+    if (dpos_table) GRB_LAUNCH(embed_bwd_pos_kernel, L < 8 * sm_count() ? L : 8 * sm_count(), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
     return 0;
 }
 
@@ -959,7 +924,7 @@ HeadWork carve_head(void* base, size_t T, size_t D, size_t C) {
 // the prologue of every head entry point: xf = bf16(LayerNorm(x)), stf = the rows' statistics (nullable)
 int head_ln_forward(const float* x, const float* g, const float* b, float eps, bf16* xf, float* stf, int T, int D, cudaStream_t st) {
     LnFwdArgs a{x, g, b, xf, nullptr, stf, T, D, eps};
-    return with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); });
+    return with_row_dim(D, [&](auto DC) -> int { GRB_LAUNCH(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); return 0; });
 }
 // the epilogue of both loss heads: d loss / d LN(x) in h.dxf -> dx, dln_g +=, dln_b +=
 int head_ln_backward(const HeadCommon& h, const float* x, const float* ln_g, float* dx, float* dln_g, float* dln_b, int T, int D, cudaStream_t st) {
@@ -986,8 +951,7 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
     // LayerNorm and is joined before the CE kernel
     const bool count_aside = g_defer_on;
     auto count = [&](cudaStream_t s_) -> int {
-        launch_k(ce_count_kernel, 1, 1024, 0, s_, reinterpret_cast<const long long*>(targets), T, h.scal, loss);
-        GRB_CUDA(cudaGetLastError());
+        GRB_LAUNCH(ce_count_kernel, 1, 1024, 0, s_, reinterpret_cast<const long long*>(targets), T, h.scal, loss);
         return 0;
     };
     if (count_aside) GRB_TRY(defer_run(st, count));
@@ -1000,8 +964,7 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
         CeArgs ca{reinterpret_cast<const long long*>(targets), h.scal, T, C, want_grad ? h.dxf : nullptr, h.shift, h.row_loss, dtable,
                   h.rseg, h.tseg, h.ce_rsched, h.ce_tsched, h.ce_rcarry, h.ce_tcarry};
         GRB_CUDA(with_ce_dim(D, [&](auto DC) { return launch_tc_ce<DC>(h.xf, (const bf16*)table_bf16, ca, sm_count(), st); }));
-        launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
-        GRB_CUDA(cudaGetLastError());
+        GRB_LAUNCH(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
         if (!want_grad) return 0;
         GRB_TRY(run_maybe_deferred(st, [&](cudaStream_t s_) -> int {
             GRB_CUDA(with_ce_dim(D, [&](auto DC) { return launch_ce_table<DC>(h.xf, (const bf16*)table_bf16, ca, sm_count(), s_); }));
@@ -1011,15 +974,9 @@ int grb_head_loss_forward_backward(const float* x, const float* ln_g, const floa
         // logits = xf E^T   (hstu.py:137)
         GRB_CUDA((launch_tc_gemm<0>(h.xf, (const bf16*)table_bf16, T, C, D, D, D, TcEpiF32{nullptr, h.ldl, 1.f}, h.logits32, nullptr, h.ldl,
                                     sm_count(), st)));
-        if (h.ldl / 8 <= 256 * 8)
-            launch_k(ce_fwd_bwd_vec_kernel<8>, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0,
-                     (const float*)h.logits32);
-        else
-            launch_k(ce_fwd_bwd_kernel, T, 256, 0, st, h.logits, h.ldl, C, reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0,
-                     (const float*)h.logits32);
-        GRB_CUDA(cudaGetLastError());
-        launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
-        GRB_CUDA(cudaGetLastError());
+        GRB_LAUNCH(h.ldl / 8 <= 256 * 8 ? ce_fwd_bwd_vec_kernel<8> : ce_fwd_bwd_kernel, T, 256, 0, st, h.logits, h.ldl, C,
+                   reinterpret_cast<const long long*>(targets), h.scal, h.row_loss, want_grad ? 1 : 0, (const float*)h.logits32);
+        GRB_LAUNCH(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
         if (!want_grad) return 0;
         GRB_CUDA(gemm_nn_f32(h.logits, (const bf16*)table_bf16, h.dxf, nullptr, 1.f, T, D, C, h.ldl, D, st));  // dxf = dlogits E
         // dE[C,D] += dlogits^T xf: a weight gradient, off the critical path with the deferred schedule
@@ -1080,15 +1037,13 @@ int grb_head_sampled_loss_forward_backward(const float* x, const float* ln_g, co
     GRB_REQUIRE(aligned16(table_bf16) && aligned16(workspace) && (!want_grad || aligned16(dtable)), "table_bf16, dtable and workspace must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     SampledWork h = carve_sampled(workspace, T, D, N);
-    launch_k(ce_count_kernel, 1, 1024, 0, st, reinterpret_cast<const long long*>(targets), T, h.scal, loss);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(ce_count_kernel, 1, 1024, 0, st, reinterpret_cast<const long long*>(targets), T, h.scal, loss);
     GRB_TRY(head_ln_forward(x, ln_g, ln_b, ln_eps, h.xf, h.stf, T, D, st));
     SceArgs sa{reinterpret_cast<const long long*>(targets), reinterpret_cast<const long long*>(negatives), log_q, (const bf16*)table_bf16, h.xf,
                h.scal, T, C, N, h.Npad, D, h.Es, h.bias, h.sid, h.ztgt, h.shift, h.row_loss, h.gtgt, want_grad ? h.dxf : nullptr, h.part, h.ks,
                dtable};
     GRB_CUDA(with_ce_dim(D, [&](auto DC) { return launch_sampled_ce<DC>(sa, sm_count(), st); }));
-    launch_k(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(ce_loss_sum_kernel, 1, 1024, 0, st, (const float*)h.row_loss, T, loss);
     if (!want_grad) return 0;
     return head_ln_backward(h, x, ln_g, dx, dln_g, dln_b, T, D, st);
 }
@@ -1145,9 +1100,7 @@ int sweep_prologue(const float* x, const float* ln_g, const float* ln_b, float l
     if (E > 0) {
         int P = 1;
         while (P < E) P <<= 1;
-        GRB_TRY(set_smem(sweep_sort_exclude_kernel, (size_t)P * 4));
-        launch_k(sweep_sort_exclude_kernel, R, SWEEP_SORT_THREADS, (size_t)P * 4, st, reinterpret_cast<const long long*>(exclude), E, P, C, w.excl);
-        GRB_CUDA(cudaGetLastError());
+        GRB_LAUNCH(sweep_sort_exclude_kernel, R, SWEEP_SORT_THREADS, (size_t)P * 4, st, reinterpret_cast<const long long*>(exclude), E, P, C, w.excl);
     }
     return 0;
 }
@@ -1177,12 +1130,9 @@ int topk_run(const float* x, const float* ln_g, const float* ln_b, float ln_eps,
     CUtensorMap tmA, tmB;
     GRB_TRY(sweep_prologue(x, ln_g, ln_b, ln_eps, table_bf16, R, D, C, exclude, E, workspace, w, &tmA, &tmB, st));
     HeadTopkArgs a{R, C, k, E, w.splits, w.num_n, D / TC_BK, w.excl, w.cand_s, w.cand_i};
-    GRB_TRY(set_smem(head_topk_kernel, TC_SMEM_BYTES));
-    launch_k(head_topk_kernel, w.num_m * w.splits, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, a);
-    GRB_CUDA(cudaGetLastError());
-    launch_k(topk_merge_kernel, (R + TOPK_MERGE_ROWS - 1) / TOPK_MERGE_ROWS, 32 * TOPK_MERGE_ROWS, 0, st, (const float*)w.cand_s,
-             (const int*)w.cand_i, R, w.splits, k, scores, reinterpret_cast<long long*>(items));
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(head_topk_kernel, w.num_m * w.splits, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, a);
+    GRB_LAUNCH(topk_merge_kernel, (R + TOPK_MERGE_ROWS - 1) / TOPK_MERGE_ROWS, 32 * TOPK_MERGE_ROWS, 0, st, (const float*)w.cand_s,
+               (const int*)w.cand_i, R, w.splits, k, scores, reinterpret_cast<long long*>(items));
     return 0;
 }
 }  // namespace
@@ -1238,22 +1188,18 @@ int cand_check(int R, int D, int C, int k, int E) {
 using CandSweep = void (*)(const CUtensorMap, const CUtensorMap, HeadCandArgs, int);
 int cand_sweep(CandSweep kern, const CUtensorMap& tmA, const CUtensorMap& tmB, const HeadCandArgs& a, unsigned grid, int pass,
                cudaStream_t st) {
-    GRB_TRY(set_smem(kern, RANK_SMEM_BYTES));
-    launch_k(kern, grid, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmB, a, pass);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(kern, grid, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmB, a, pass);
     return 0;
 }
 int cand_sweeps(const CUtensorMap& tmA, const CUtensorMap& tmB, const HeadCandArgs& a, unsigned grid, cudaStream_t st) {
     const bool ex = a.E > 0;
     GRB_TRY(cand_sweep(ex ? head_cand_sweep_kernel<CAND_BOUND, true> : head_cand_sweep_kernel<CAND_BOUND, false>, tmA, tmB, a, grid, 0, st));
-    launch_k(head_cand_threshold_kernel, a.R, 256, 0, st, a);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(head_cand_threshold_kernel, a.R, 256, 0, st, a);
     GRB_TRY(cand_sweep(ex ? head_cand_sweep_kernel<CAND_COLLECT, true> : head_cand_sweep_kernel<CAND_COLLECT, false>, tmA, tmB, a, grid, 0, st));
     // refinement of the rows whose buffer overflowed: always launched, so the launch sequence does not depend on the data
     for (int p = 0; p < CAND_RADIX_PASSES; ++p) {
         GRB_TRY(cand_sweep(ex ? head_cand_sweep_kernel<CAND_HIST, true> : head_cand_sweep_kernel<CAND_HIST, false>, tmA, tmB, a, grid, p, st));
-        launch_k(head_cand_digit_kernel, (a.R + CAND_DIGIT_THREADS / 32 - 1) / (CAND_DIGIT_THREADS / 32), CAND_DIGIT_THREADS, 0, st, a, p);
-        GRB_CUDA(cudaGetLastError());
+        GRB_LAUNCH(head_cand_digit_kernel, (a.R + CAND_DIGIT_THREADS / 32 - 1) / (CAND_DIGIT_THREADS / 32), CAND_DIGIT_THREADS, 0, st, a, p);
     }
     return cand_sweep(ex ? head_cand_sweep_kernel<CAND_RECOLLECT, true> : head_cand_sweep_kernel<CAND_RECOLLECT, false>, tmA, tmB, a, grid,
                       0, st);
@@ -1281,9 +1227,7 @@ int grb_head_candidates(const float* x, const float* ln_g, const float* ln_b, fl
     int P = 1;
     while (P < w.cap) P <<= 1;
     const size_t sort_bytes = (size_t)P * 12;   // keys and scores
-    GRB_TRY(set_smem(head_cand_select_kernel, sort_bytes));
-    launch_k(head_cand_select_kernel, R, CAND_SELECT_THREADS, sort_bytes, st, a, scores, reinterpret_cast<long long*>(items));
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(head_cand_select_kernel, R, CAND_SELECT_THREADS, sort_bytes, st, a, scores, reinterpret_cast<long long*>(items));
     return 0;
 }
 
@@ -1324,26 +1268,18 @@ int grb_head_rank(const float* x, const float* ln_g, const float* ln_b, float ln
     GRB_REQUIRE(make_tmap_bf16(&tmG, w.G, R, D, D, TC_BK, TC_BN), "cannot encode the TMA descriptor of G");
     HeadRankArgs a{R, C, E, w.splits, w.num_n, D / TC_BK, reinterpret_cast<const long long*>(targets), w.excl, w.tid, w.tscore, w.cnt,
                    metrics, reinterpret_cast<int*>(ranks)};
-    launch_k(head_rank_gather_kernel, (R + 7) / 8, 256, 0, st, (const bf16*)table_bf16, D, a, w.G);
-    GRB_CUDA(cudaGetLastError());
-    GRB_TRY(set_smem(head_rank_target_kernel, RANK_SMEM_BYTES));
-    launch_k(head_rank_target_kernel, w.num_m, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmG, a);
-    GRB_CUDA(cudaGetLastError());
-    auto sweep = E > 0 ? head_rank_kernel<true> : head_rank_kernel<false>;
-    GRB_TRY(set_smem(sweep, RANK_SMEM_BYTES));
-    launch_k(sweep, w.num_m * w.splits, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmB, a);
-    GRB_CUDA(cudaGetLastError());
-    launch_k(head_rank_finish_kernel, (R + 255) / 256, 256, 0, st, a);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(head_rank_gather_kernel, (R + 7) / 8, 256, 0, st, (const bf16*)table_bf16, D, a, w.G);
+    GRB_LAUNCH(head_rank_target_kernel, w.num_m, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmG, a);
+    GRB_LAUNCH(E > 0 ? head_rank_kernel<true> : head_rank_kernel<false>, w.num_m * w.splits, TC_THREADS, RANK_SMEM_BYTES, st, tmA, tmB, a);
+    GRB_LAUNCH(head_rank_finish_kernel, (R + 255) / 256, 256, 0, st, a);
     return 0;
 }
 
 int grb_eval_rank_metrics(const float* logits, const int64_t* targets, int B, int C, float* metrics, int32_t* ranks, void* stream) {
     GRB_REQUIRE(logits && targets && metrics, "null argument");
     GRB_REQUIRE(B > 0 && C > 1, "bad shape B=%d C=%d", B, C);
-    launch_k(eval_rank_kernel, (unsigned)B, 256, 0, static_cast<cudaStream_t>(stream), logits, C, reinterpret_cast<const long long*>(targets), metrics,
-             reinterpret_cast<int*>(ranks));
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(eval_rank_kernel, (unsigned)B, 256, 0, static_cast<cudaStream_t>(stream), logits, C, reinterpret_cast<const long long*>(targets), metrics,
+               reinterpret_cast<int*>(ranks));
     return 0;
 }
 
@@ -1370,13 +1306,10 @@ int grb_sasrec_attention_forward(const grb_sasrec_dims* d, const void* q, const 
     a.q = (const bf16*)q; a.k = (const bf16*)k; a.v = (const bf16*)v; a.pad = pad; a.out = (bf16*)out; a.lse = lse;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     dim3 grid((a.L + ATT_BLK - 1) / ATT_BLK, a.H, a.B);
-    GRB_TRY(with_head_dim(d->D / d->H, [&](auto DH) -> int {
-        GRB_TRY(set_smem(sas_attn_fwd_kernel<DH>, sizeof(SasSmem<DH>)));
-        launch_k(sas_attn_fwd_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
+    return with_head_dim(d->D / d->H, [&](auto DH) -> int {
+        GRB_LAUNCH(sas_attn_fwd_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
         return 0;
-    }));
-    GRB_CUDA(cudaGetLastError());
-    return 0;
+    });
 }
 
 int grb_sasrec_attention_backward(const grb_sasrec_dims* d, const void* q, const void* k, const void* v, const uint8_t* pad,
@@ -1389,15 +1322,11 @@ int grb_sasrec_attention_backward(const grb_sasrec_dims* d, const void* q, const
     a.dq = (bf16*)dq; a.dk = (bf16*)dk; a.dv = (bf16*)dv;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     dim3 grid((a.L + ATT_BLK - 1) / ATT_BLK, a.H, a.B);
-    GRB_TRY(with_head_dim(d->D / d->H, [&](auto DH) -> int {
-        GRB_TRY(set_smem(sas_attn_bwd_dq_kernel<DH>, sizeof(SasSmem<DH>)));
-        GRB_TRY(set_smem(sas_attn_bwd_dkdv_kernel<DH>, sizeof(SasSmem<DH>)));
-        launch_k(sas_attn_bwd_dq_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
-        launch_k(sas_attn_bwd_dkdv_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
+    return with_head_dim(d->D / d->H, [&](auto DH) -> int {
+        GRB_LAUNCH(sas_attn_bwd_dq_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
+        GRB_LAUNCH(sas_attn_bwd_dkdv_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
         return 0;
-    }));
-    GRB_CUDA(cudaGetLastError());
-    return 0;
+    });
 }
 
 // ------------------------------------------------------------------------------------------------ generic fused linear pieces
@@ -1485,7 +1414,7 @@ int grb_layernorm_forward(const float* x, const float* g, const float* b, float 
     GRB_REQUIRE(x && g && b && (y_bf16 || y_f32), "null argument");
     LnFwdArgs a{x, g, b, (bf16*)y_bf16, y_f32, stats, T, D, eps};
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    return with_row_dim(D, [&](auto DC) { launch_k(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); });
+    return with_row_dim(D, [&](auto DC) -> int { GRB_LAUNCH(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); return 0; });
 }
 size_t grb_layernorm_backward_workspace_bytes(int T, int D) {
     if (T <= 0 || D <= 0) return 0;
@@ -1501,7 +1430,7 @@ int grb_rmsnorm_forward(const float* x, const float* w, float eps, int T, int D,
     GRB_REQUIRE(x && w && (y_bf16 || y_f32) && T > 0, "bad argument");
     RmsFwdArgs a{x, w, (bf16*)y_bf16, y_f32, rstd, T, D, eps};
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    return with_rms_dim(D, [&](auto DC) { launch_k(rms_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); });
+    return with_rms_dim(D, [&](auto DC) -> int { GRB_LAUNCH(rms_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); return 0; });
 }
 size_t grb_rmsnorm_backward_workspace_bytes(int T, int D) {
     if (T <= 0 || D <= 0) return 0;
@@ -1512,16 +1441,15 @@ int grb_rmsnorm_backward(const float* dy, const float* x, const float* rstd, con
     GRB_REQUIRE(dy && x && rstd && w && dx && dw && workspace && T > 0, "bad argument");
     RmsBwdArgs a{dy, x, rstd, w, residual, dx, dw, T, D, static_cast<float*>(workspace)};
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    GRB_TRY(with_rms_dim(D, [&](auto DC) { launch_k(rms_bwd_kernel<DC / 64>, row_bwd_grid(T), ROW_THREADS, 0, st, a); }));
+    GRB_TRY(with_rms_dim(D, [&](auto DC) -> int { GRB_LAUNCH(rms_bwd_kernel<DC / 64>, row_bwd_grid(T), ROW_THREADS, 0, st, a); return 0; }));
     return det_finish(a.part, 1, row_bwd_grid(T), D, 1, 0, 1, {{dw, D}}, st);
 }
 
 int grb_split3_f32_to_bf16(const float* in, void* out_bf16, size_t rows, int K, int operand, void* stream) {
     GRB_REQUIRE(in && out_bf16 && K > 0 && (operand == 0 || operand == 1), "bad argument");
     if (rows == 0) return 0;
-    launch_k(split3_f32_bf16_kernel, capped_blocks(rows * (size_t)K), 256, 0, static_cast<cudaStream_t>(stream), in, (bf16*)out_bf16, rows, K,
-             operand);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(split3_f32_bf16_kernel, capped_blocks(rows * (size_t)K), 256, 0, static_cast<cudaStream_t>(stream), in, (bf16*)out_bf16, rows, K,
+               operand);
     return 0;
 }
 static int linear_f32x3(const bf16* xs, const bf16* ws, const float* bias, const float* res2, int T, int N, int K, int act, float* y, int ldy,
@@ -1589,12 +1517,12 @@ int grb_hstu_layer_forward_f32(const grb_hstu_dims* d, const grb_hstu_layer_para
     // O = silu(Q K^T + bias) V                                                                (hstu.py:244-267)
     {
         HstuAttnF32Args a{w.P, 4 * D, d->B, d->L, d->H, make_attn_bias(d, p->pos_table, p->time_table, s), w.O};
-        GRB_REQUIRE(with_head_dim(D / d->H, [&](auto DH) { return launch_hstu_attn_f32<DH>(a, st); }) == 0, "fp32 attention launch failed");
+        GRB_TRY(with_head_dim(D / d->H, [&](auto DH) -> int { GRB_CUDA(launch_hstu_attn_f32<DH>(a, st)); return 0; }));
     }
     // x1 = x + LN1(O) * U ; xn = LN2(x1)                                                      (hstu.py:271-278)
     {
         LnGateF32Args a{w.O, w.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, w.x1, w.xn, T, 1e-5f};
-        GRB_TRY(with_row_dim(D, [&](auto DC) { launch_k(ln_gate_f32_kernel<DC / 32>, row_grid(T), 256, 0, st, a); }));
+        GRB_TRY(with_row_dim(D, [&](auto DC) -> int { GRB_LAUNCH(ln_gate_f32_kernel<DC / 32>, row_grid(T), 256, 0, st, a); return 0; }));
     }
     // y = x1 + (silu(xn W1^T + b1) W2^T + b2)                                                 (hstu.py:210-214, :278)
     GRB_TRY(grb_split3_f32_to_bf16(w.xn, w.xs, T, D, 0, stream));
@@ -1606,7 +1534,7 @@ int grb_hstu_layer_forward_f32(const grb_hstu_dims* d, const grb_hstu_layer_para
 int grb_layernorm_f32_forward(const float* x, const float* g, const float* b, float eps, int T, int D, float* y, void* stream) {
     GRB_REQUIRE(x && g && b && y && T > 0 && (D == 64 || D == 128 || D == 256), "bad argument T=%d D=%d", T, D);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    return with_row_dim(D, [&](auto DC) { launch_k(ln_f32_kernel<DC / 32>, row_grid(T), 256, 0, st, x, g, b, y, T, eps); });
+    return with_row_dim(D, [&](auto DC) -> int { GRB_LAUNCH(ln_f32_kernel<DC / 32>, row_grid(T), 256, 0, st, x, g, b, y, T, eps); return 0; });
 }
 
 // ------------------------------------------------------------------------------------------------ T5-style attention core (TIGER)
@@ -1634,14 +1562,10 @@ int grb_t5_attention_forward(const void* q, const void* k, const void* v, int B,
     a.out = (bf16*)out; a.ldo = ldo; a.lse = lse;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     dim3 grid((Lq + T5_ROWS - 1) / T5_ROWS, B * H);
-    GRB_TRY(with_head_dim(head_dim, [&](auto DH) -> int {
-        const size_t smem = t5_fwd_smem<DH>(a.nb);
-        GRB_TRY(set_smem(t5_attn_fwd_kernel<DH>, smem));
-        launch_k(t5_attn_fwd_kernel<DH>, grid, T5_THREADS, smem, st, a);
+    return with_head_dim(head_dim, [&](auto DH) -> int {
+        GRB_LAUNCH(t5_attn_fwd_kernel<DH>, grid, T5_THREADS, t5_fwd_smem<DH>(a.nb), st, a);
         return 0;
-    }));
-    GRB_CUDA(cudaGetLastError());
-    return 0;
+    });
 }
 namespace {
 struct T5BwdWork {
@@ -1687,16 +1611,10 @@ int grb_t5_attention_backward(const void* q, const void* k, const void* v, int B
     }
     dim3 grid((Lq + T5_ROWS - 1) / T5_ROWS, B * H);
     GRB_TRY(with_head_dim(head_dim, [&](auto DH) -> int {
-        const size_t smem = t5_bwd_smem<DH>(a.nb);
-        GRB_TRY(set_smem(t5_attn_bwd_kernel<DH>, smem));
-        launch_k(t5_attn_bwd_kernel<DH>, grid, T5_THREADS, smem, st, a, w.dkv_part, w.db_part);
+        GRB_LAUNCH(t5_attn_bwd_kernel<DH>, grid, T5_THREADS, t5_bwd_smem<DH>(a.nb), st, a, w.dkv_part, w.db_part);
         return 0;
     }));
-    GRB_CUDA(cudaGetLastError());
-    if (w.dkv_part) {
-        launch_k(t5_dkdv_sum_kernel, capped_blocks(2 * n / 4), 256, 0, st, (const float*)w.dkv_part, (int)grid.x, n, dk, dv);
-        GRB_CUDA(cudaGetLastError());
-    }
+    if (w.dkv_part) GRB_LAUNCH(t5_dkdv_sum_kernel, capped_blocks(2 * n / 4), 256, 0, st, (const float*)w.dkv_part, (int)grid.x, n, dk, dv);
     if (a.dbias) GRB_TRY(det_finish(w.db_part, H, B * (int)grid.x, a.nb, H, a.nb, 1, {{a.dbias, H * a.nb}}, st));
     return 0;
 }
@@ -1711,9 +1629,8 @@ int grb_trie_log_softmax(const float* logits, int rows, int V, const int32_t* no
     if (rows == 0) return 0;
     TrieCsr t{child_off, child_tok, nullptr, n_nodes};
     const size_t smem = (size_t)((V + 31) / 32) * 4;
-    launch_k(trie_log_softmax_kernel, rows, 256, smem, static_cast<cudaStream_t>(stream), logits, V, node, t, use_trie, vocab_offset,
-             num_embeddings, temperature, probs, logp);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(trie_log_softmax_kernel, rows, 256, smem, static_cast<cudaStream_t>(stream), logits, V, node, t, use_trie, vocab_offset,
+               num_embeddings, temperature, probs, logp);
     return 0;
 }
 int grb_beam_select(const int64_t* beam_seqs, const float* beam_logps, const int64_t* cand_tok, const float* cand_logp, const int32_t* nodes,
@@ -1725,8 +1642,7 @@ int grb_beam_select(const int64_t* beam_seqs, const float* beam_logps, const int
     if (B == 0) return 0;
     BeamSelectArgs a{reinterpret_cast<const long long*>(beam_seqs), beam_logps, reinterpret_cast<const long long*>(cand_tok), cand_logp, nodes,
                      TrieCsr{child_off, child_tok, child_node, n_nodes}, K, KK, S, reinterpret_cast<long long*>(new_seqs), new_logps, new_nodes};
-    launch_k(beam_select_kernel, B, BEAM_MAX_CAND, 0, static_cast<cudaStream_t>(stream), a);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(beam_select_kernel, B, BEAM_MAX_CAND, 0, static_cast<cudaStream_t>(stream), a);
     return 0;
 }
 
@@ -1734,20 +1650,17 @@ int grb_beam_select(const int64_t* beam_seqs, const float* beam_logps, const int
 int grb_cast_f32_to_bf16(const float* in, void* out_bf16, size_t n, void* stream) {
     GRB_REQUIRE(in && out_bf16, "null argument");
     if (n == 0) return 0;
-    launch_k(cast_flat_f32_bf16_kernel, capped_blocks(n), 256, 0, static_cast<cudaStream_t>(stream), in, (bf16*)out_bf16, n);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(cast_flat_f32_bf16_kernel, capped_blocks(n), 256, 0, static_cast<cudaStream_t>(stream), in, (bf16*)out_bf16, n);
     return 0;
 }
 int grb_adam_step(float* p, float* g, float* m, float* v, void* p_bf16, size_t n, float* state, float lr, float beta1, float beta2,
                   float eps, float weight_decay, float grad_scale, int zero_grad, void* stream) {
     GRB_REQUIRE(p && g && m && v && state, "null argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    launch_k(adam_tick_kernel, 1, 1, 0, st, state, beta1, beta2);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(adam_tick_kernel, 1, 1, 0, st, state, beta1, beta2);
     if (n == 0) return 0;
     AdamArgs a{p, g, m, v, (bf16*)p_bf16, n, state, lr, beta1, beta2, eps, weight_decay, grad_scale, zero_grad};
-    launch_k(adam_step_kernel, capped_blocks(n), 256, 0, st, a);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(adam_step_kernel, capped_blocks(n), 256, 0, st, a);
     return 0;
 }
 
@@ -1755,15 +1668,13 @@ int grb_rowset_mark(const int64_t* ids, size_t n, int C, int32_t* flag, int32_t*
     GRB_REQUIRE((ids || n == 0) && flag && rows && count, "null argument");
     GRB_REQUIRE(C >= 2, "bad table size C=%d (C >= 2)", C);
     if (n == 0) return 0;
-    launch_k(rowset_mark_kernel, capped_blocks(n), 256, 0, static_cast<cudaStream_t>(stream), reinterpret_cast<const long long*>(ids), n, C,
-             flag, rows, count);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(rowset_mark_kernel, capped_blocks(n), 256, 0, static_cast<cudaStream_t>(stream), reinterpret_cast<const long long*>(ids), n, C,
+               flag, rows, count);
     return 0;
 }
 int grb_rowset_mark_all(int32_t* all_word, void* stream) {
     GRB_REQUIRE(all_word, "null argument");
-    launch_k(rowset_mark_all_kernel, 1, 1, 0, static_cast<cudaStream_t>(stream), all_word);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(rowset_mark_all_kernel, 1, 1, 0, static_cast<cudaStream_t>(stream), all_word);
     return 0;
 }
 int grb_adam_step_lazy_table(float* p, float* g, float* m, float* v, void* p_bf16, size_t n, size_t table_off, int C, int D, int32_t* flag,
@@ -1778,26 +1689,22 @@ int grb_adam_step_lazy_table(float* p, float* g, float* m, float* v, void* p_bf1
                     (reinterpret_cast<uintptr_t>(static_cast<bf16*>(p_bf16) + table_off) & 7) == 0,
                 "the table slot must start 16-byte aligned (8 bytes in the bf16 mirror)");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    launch_k(adam_tick_kernel, 1, 1, 0, st, state, beta1, beta2);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(adam_tick_kernel, 1, 1, 0, st, state, beta1, beta2);
     // every parameter outside the table: the dense kernel, as grb_adam_step runs it, over [0, table_off) and [hi, n)
     bf16* pb = static_cast<bf16*>(p_bf16);
     for (const size_t lo : {(size_t)0, hi}) {
         const size_t len = lo == 0 ? table_off : n - hi;
         if (len == 0) continue;
         AdamArgs a{p + lo, g + lo, m + lo, v + lo, pb + lo, len, state, lr, beta1, beta2, eps, weight_decay, grad_scale, 1};
-        launch_k(adam_step_kernel, capped_blocks(len), 256, 0, st, a);
-        GRB_CUDA(cudaGetLastError());
+        GRB_LAUNCH(adam_step_kernel, capped_blocks(len), 256, 0, st, a);
     }
     const size_t o = table_off;
     LazyTableArgs a{p + o, g + o, m + o, v + o, pb + o, C, flag, rows, count, all_word, state, lr, beta1, beta2, eps, weight_decay, grad_scale};
     const unsigned blocks = (unsigned)sm_count() * 8;     // fixed: the row count is only known on the device
-    if (D == 64) launch_k(lazy_table_step_kernel<16>, blocks, 256, 0, st, a);
-    else if (D == 128) launch_k(lazy_table_step_kernel<32>, blocks, 256, 0, st, a);
-    else launch_k(lazy_table_step_kernel<64>, blocks, 256, 0, st, a);
-    GRB_CUDA(cudaGetLastError());
-    launch_k(rowset_reset_kernel, 1, 1, 0, st, count, all_word);
-    GRB_CUDA(cudaGetLastError());
+    if (D == 64) GRB_LAUNCH(lazy_table_step_kernel<16>, blocks, 256, 0, st, a);
+    else if (D == 128) GRB_LAUNCH(lazy_table_step_kernel<32>, blocks, 256, 0, st, a);
+    else GRB_LAUNCH(lazy_table_step_kernel<64>, blocks, 256, 0, st, a);
+    GRB_LAUNCH(rowset_reset_kernel, 1, 1, 0, st, count, all_word);
     return 0;
 }
 
@@ -1811,21 +1718,16 @@ int grb_dp_adam_step(float* p, float* g, float* m, float* v, void* p_bf16, const
     const bool mc = mc_g != nullptr && mc_p != nullptr && mc_p_bf16 != nullptr;
     GRB_REQUIRE(mc || (peer_g && peer_p && peer_p_bf16), "neither multicast addresses nor peer pointer arrays given");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    launch_k(adam_tick_kernel, 1, 1, 0, st, state, beta1, beta2);
-    GRB_CUDA(cudaGetLastError());
-    launch_k(dp_barrier_kernel, 1, 32, 0, st, reinterpret_cast<unsigned* const*>(peer_sig), reinterpret_cast<unsigned*>(sig),
-             reinterpret_cast<unsigned*>(epoch), rank, world, 0);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(adam_tick_kernel, 1, 1, 0, st, state, beta1, beta2);
+    GRB_LAUNCH(dp_barrier_kernel, 1, 32, 0, st, reinterpret_cast<unsigned* const*>(peer_sig), reinterpret_cast<unsigned*>(sig),
+               reinterpret_cast<unsigned*>(epoch), rank, world, 0);
     DpAdamArgs a{p, g, m, v, (bf16*)p_bf16, (const float*)mc_g, (float*)mc_p, (bf16*)mc_p_bf16,
                  reinterpret_cast<const float* const*>(peer_g), reinterpret_cast<float* const*>(peer_p), reinterpret_cast<bf16* const*>(peer_p_bf16),
                  n, rank, world, state, lr, beta1, beta2, eps, weight_decay, grad_scale};
     const unsigned blocks = capped_blocks(n / world / 8, 4);
-    if (mc) launch_k(dp_adam_kernel<true>, blocks, 256, 0, st, a);
-    else launch_k(dp_adam_kernel<false>, blocks, 256, 0, st, a);
-    GRB_CUDA(cudaGetLastError());
-    launch_k(dp_barrier_kernel, 1, 32, 0, st, reinterpret_cast<unsigned* const*>(peer_sig), reinterpret_cast<unsigned*>(sig),
-             reinterpret_cast<unsigned*>(epoch), rank, world, 1);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(mc ? dp_adam_kernel<true> : dp_adam_kernel<false>, blocks, 256, 0, st, a);
+    GRB_LAUNCH(dp_barrier_kernel, 1, 32, 0, st, reinterpret_cast<unsigned* const*>(peer_sig), reinterpret_cast<unsigned*>(sig),
+               reinterpret_cast<unsigned*>(epoch), rank, world, 1);
     GRB_CUDA(cudaMemsetAsync(g, 0, n * sizeof(float), st));
     return 0;
 }
@@ -1841,8 +1743,7 @@ __global__ void assert_unit_scalar_kernel(const float* v) {
 }  // namespace
 int grb_assert_unit_scalar(const float* value, void* stream) {
     GRB_REQUIRE(value, "null argument");
-    launch_k(assert_unit_scalar_kernel, 1, 1, 0, static_cast<cudaStream_t>(stream), value);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(assert_unit_scalar_kernel, 1, 1, 0, static_cast<cudaStream_t>(stream), value);
     return 0;
 }
 
@@ -1869,10 +1770,8 @@ int grb_rq_residual_argmin(const float* x, const float* codebooks, int64_t N, in
         const bool stage = emb != nullptr || res != nullptr;
         const size_t smem = rq_tile_smem_bytes(D, K, levels, stage);
         if (!force_thread && !force_split && D == 32 && K % 256 == 0 && smem <= 220 * 1024) {
-            GRB_TRY(set_smem(rq_residual_argmin_tile_kernel<32>, smem));
             const unsigned grid = (unsigned)((N + RQT_ROWS - 1) / RQT_ROWS);
-            launch_k(rq_residual_argmin_tile_kernel<32>, grid, RQT_THREADS, smem, st, a);
-            GRB_CUDA(cudaGetLastError());
+            GRB_LAUNCH(rq_residual_argmin_tile_kernel<32>, grid, RQT_THREADS, smem, st, a);
             return 0;
         }
     }
@@ -1885,18 +1784,10 @@ int grb_rq_residual_argmin(const float* x, const float* codebooks, int64_t N, in
         const bool staged = stage > 0 && base + stage <= 200 * 1024;
         const size_t smem = base + (staged ? stage : 0);
         const unsigned grid = (unsigned)((N + (int64_t)RQ_ROWS_PER_CTA * rows - 1) / ((int64_t)RQ_ROWS_PER_CTA * rows));
-        auto go = [&](auto kern) -> int {
-            GRB_TRY(set_smem(kern, smem));
-            launch_k(kern, grid, RQ_THREADS, smem, st, a);
-            return 0;
-        };
-        if (D == 32) {
-            if (rows == 2) GRB_TRY(staged ? go(rq_residual_argmin_split_kernel<32, 2, true>) : go(rq_residual_argmin_split_kernel<32, 2, false>));
-            else GRB_TRY(staged ? go(rq_residual_argmin_split_kernel<32, 1, true>) : go(rq_residual_argmin_split_kernel<32, 1, false>));
-        } else {
-            GRB_TRY(staged ? go(rq_residual_argmin_split_kernel<64, 1, true>) : go(rq_residual_argmin_split_kernel<64, 1, false>));
-        }
-        GRB_CUDA(cudaGetLastError());
+        auto split_kernel = D != 32    ? (staged ? rq_residual_argmin_split_kernel<64, 1, true> : rq_residual_argmin_split_kernel<64, 1, false>)
+                            : rows == 2 ? (staged ? rq_residual_argmin_split_kernel<32, 2, true> : rq_residual_argmin_split_kernel<32, 2, false>)
+                                        : (staged ? rq_residual_argmin_split_kernel<32, 1, true> : rq_residual_argmin_split_kernel<32, 1, false>);
+        GRB_LAUNCH(split_kernel, grid, RQ_THREADS, smem, st, a);
         return 0;
     }
     size_t smem = (size_t)K * (D + 1) * sizeof(float);
@@ -1904,19 +1795,15 @@ int grb_rq_residual_argmin(const float* x, const float* codebooks, int64_t N, in
         // two rows per thread once there is more than a wave of work; one row per thread for small N (more CTAs)
         if (N > (int64_t)sm_count() * RQ_THREADS * 2) {
             unsigned grid = (unsigned)((N + 2 * RQ_THREADS - 1) / (2 * RQ_THREADS));
-            GRB_TRY(set_smem(rq_residual_argmin_kernel<32, 2>, smem));
-            launch_k(rq_residual_argmin_kernel<32, 2>, grid, RQ_THREADS, smem, st, a);
+            GRB_LAUNCH((rq_residual_argmin_kernel<32, 2>), grid, RQ_THREADS, smem, st, a);
         } else {
             unsigned grid = (unsigned)((N + RQ_THREADS - 1) / RQ_THREADS);
-            GRB_TRY(set_smem(rq_residual_argmin_kernel<32, 1>, smem));
-            launch_k(rq_residual_argmin_kernel<32, 1>, grid, RQ_THREADS, smem, st, a);
+            GRB_LAUNCH((rq_residual_argmin_kernel<32, 1>), grid, RQ_THREADS, smem, st, a);
         }
     } else {
         unsigned grid = (unsigned)((N + RQ_THREADS - 1) / RQ_THREADS);
-        GRB_TRY(set_smem(rq_residual_argmin_kernel<64, 1>, smem));
-        launch_k(rq_residual_argmin_kernel<64, 1>, grid, RQ_THREADS, smem, st, a);
+        GRB_LAUNCH((rq_residual_argmin_kernel<64, 1>), grid, RQ_THREADS, smem, st, a);
     }
-    GRB_CUDA(cudaGetLastError());
     return 0;
 }
 
@@ -1937,7 +1824,7 @@ int sk_prepare() {
     if (ready[dev]) return 0;
     for (auto kern : {rq_sinkhorn_kernel<true>, rq_sinkhorn_kernel<false>}) {
         GRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        GRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SK_SMEM_MAX));
+        GRB_CUDA(set_max_smem(kern, SK_SMEM_MAX));
         cudaLaunchConfig_t cfg;
         memset(&cfg, 0, sizeof(cfg));
         cfg.gridDim = dim3(SK_CLUSTER);
@@ -1985,9 +1872,7 @@ int grb_rq_sinkhorn(const float* dist, int64_t B, int K, double eps, int iters, 
     SinkhornArgs a{dist, (long long)B, K, iters, (int)rows, eps, reinterpret_cast<long long*>(ids), u_out, v_out, u, kmat};
     const size_t smem = SK_SMEM_FIXED + (in_smem ? rows * K * sizeof(double) : 0);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (in_smem) launch_kc(rq_sinkhorn_kernel<true>, SK_CLUSTER, SK_THREADS, SK_CLUSTER, smem, st, a);
-    else launch_kc(rq_sinkhorn_kernel<false>, SK_CLUSTER, SK_THREADS, SK_CLUSTER, smem, st, a);
-    GRB_CUDA(cudaGetLastError());
+    GRB_CUDA(launch_kc(in_smem ? rq_sinkhorn_kernel<true> : rq_sinkhorn_kernel<false>, SK_CLUSTER, SK_THREADS, SK_CLUSTER, smem, st, a));
     return 0;
 }
 
@@ -1996,9 +1881,8 @@ int grb_kmeans_update(const float* x, const int64_t* assign, int64_t B, int D, i
     GRB_REQUIRE(B >= 0 && k >= 1 && k <= (1 << 20) && D >= 1 && D <= KM_THREADS,
                 "kmeans_update: B=%lld D=%d k=%d unsupported (B >= 0, 1 <= D <= %d, 1 <= k <= 2^20)", (long long)B, D, k, KM_THREADS);
     GRB_REQUIRE(x && assign && centroids && counts && shift, "kmeans_update: null argument");
-    launch_k(kmeans_update_kernel, (unsigned)k, KM_THREADS, 0, static_cast<cudaStream_t>(stream), x, reinterpret_cast<const long long*>(assign),
-             (long long)B, D, centroids, counts, shift);
-    GRB_CUDA(cudaGetLastError());
+    GRB_LAUNCH(kmeans_update_kernel, (unsigned)k, KM_THREADS, 0, static_cast<cudaStream_t>(stream), x, reinterpret_cast<const long long*>(assign),
+               (long long)B, D, centroids, counts, shift);
     return 0;
 }
 

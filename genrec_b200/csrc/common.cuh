@@ -39,15 +39,41 @@ inline bool pdl_enabled() {
     return v != 0;
 }
 
-// every kernel launch of the library goes through launch_k, which also counts them (grb_launch_count in the C ABI)
+// opt in to > 48 KB dynamic shared memory once per (kernel, high-water mark): no runtime call on the steady-state path,
+// in particular none while a CUDA graph is being captured after warm-up.
+template <class Kern>
+inline cudaError_t set_max_smem(Kern k, size_t bytes) {
+    static std::mutex mu;
+    // keyed by (device, kernel address): the attribute is per device.  One map per instantiation, that is per kernel signature.
+    static std::map<std::pair<int, const void*>, size_t> high_water;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& hw = high_water[std::make_pair(dev, reinterpret_cast<const void*>(k))];
+    if (hw < 48 * 1024) hw = 48 * 1024;
+    if (bytes > hw) {
+        cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+        if (e != cudaSuccess) return e;
+        hw = bytes;
+    }
+    return cudaSuccess;
+}
+
+// Every kernel launch of the library goes through launch_kc, which also counts them (grb_launch_count in the C ABI).
 inline unsigned long long& launch_counter() {
     static unsigned long long n = 0;
     return n;
 }
 // launch_kc(kernel, grid, block, cluster, smem, st, args...) with the PDL attribute (GRB_PDL=0 turns it off) and, for cluster > 1, a
-// thread-block cluster of `cluster` CTAs along x; launch_k is the same without clusters.
+// thread-block cluster of `cluster` CTAs along x; launch_k is the same without clusters.  A launch with more than 48 KB of dynamic
+// shared memory first raises the kernel's limit through set_max_smem.  The result is this launch's own error: the opt-in's, or
+// cudaLaunchKernelEx's, never one an earlier runtime call left behind.
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_kc(void (*kern)(KArgs...), dim3 grid, dim3 block, unsigned cluster, size_t smem, cudaStream_t st, Args&&... args) {
+    if (smem > 48 * 1024) {
+        const cudaError_t e = set_max_smem(kern, smem);
+        if (e != cudaSuccess) return e;
+    }
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = grid;
@@ -76,26 +102,6 @@ inline cudaError_t launch_kc(void (*kern)(KArgs...), dim3 grid, dim3 block, unsi
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
     return launch_kc(kern, grid, block, 1u, smem, st, static_cast<Args&&>(args)...);
-}
-
-// opt in to > 48 KB dynamic shared memory once per (kernel, high-water mark): no runtime call on the steady-state path,
-// in particular none while a CUDA graph is being captured after warm-up.
-template <class Kern>
-inline cudaError_t set_max_smem(Kern k, size_t bytes) {
-    static std::mutex mu;
-    // keyed by (device, kernel address): the attribute is per device.  One map per instantiation, that is per kernel signature.
-    static std::map<std::pair<int, const void*>, size_t> high_water;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    std::lock_guard<std::mutex> lock(mu);
-    size_t& hw = high_water[std::make_pair(dev, reinterpret_cast<const void*>(k))];
-    if (hw < 48 * 1024) hw = 48 * 1024;
-    if (bytes > hw) {
-        cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-        if (e != cudaSuccess) return e;
-        hw = bytes;
-    }
-    return cudaSuccess;
 }
 
 // ----------------------------------------------------------------------------- small math

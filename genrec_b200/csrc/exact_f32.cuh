@@ -103,19 +103,10 @@ __global__ void __launch_bounds__(AF_THREADS) hstu_attn_f32_fwd_kernel(HstuAttnF
 }
 
 template <int DH>
-inline int launch_hstu_attn_f32(const HstuAttnF32Args& a, cudaStream_t st) {
+inline cudaError_t launch_hstu_attn_f32(const HstuAttnF32Args& a, cudaStream_t st) {
     const size_t smem = (size_t)(2 * AF_KEYS * DH + a.bias.npos * 64 + 1) * sizeof(float);
-    static bool attr_dev[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (!attr_dev[dev & 63]) {
-        if (cudaFuncSetAttribute(hstu_attn_f32_fwd_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024) != cudaSuccess) return 1;
-        attr_dev[dev & 63] = true;
-    }
-    if (smem > 96 * 1024) return 1;
     dim3 grid((a.L + AF_ROWS - 1) / AF_ROWS, a.B * a.H);
-    launch_k(hstu_attn_f32_fwd_kernel<DH>, grid, AF_THREADS, smem, st, a);
-    return cudaGetLastError() == cudaSuccess ? 0 : 1;
+    return launch_k(hstu_attn_f32_fwd_kernel<DH>, grid, AF_THREADS, smem, st, a);
 }
 
 // ------------------------------------------------------------------------------------------------ fp32 row kernels (one warp per row)

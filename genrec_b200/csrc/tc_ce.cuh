@@ -532,26 +532,20 @@ template <int D>
 inline cudaError_t launch_tc_ce(const bf16* xf, const bf16* table, const CeArgs& a, int ctas, cudaStream_t st) {
     CUtensorMap tmX, tmE;
     if (!make_tmap_bf16(&tmX, xf, a.T, D, D, 64, 128) || !make_tmap_bf16(&tmE, table, a.C, D, D, 64, 64)) return cudaErrorInvalidValue;
-    cudaError_t e = set_max_smem(ce_rows_kernel<D>, CeSmem<D>::ROWS_BYTES);
-    if (e != cudaSuccess) return e;
     const int R = (a.T + 127) / 128, units = (a.dx ? 2 : 1) * a.rseg * R;
-    e = cudaMemsetAsync(a.rsched, 0, (size_t)(1 + 2 * R) * sizeof(int), st);
+    const cudaError_t e = cudaMemsetAsync(a.rsched, 0, (size_t)(1 + 2 * R) * sizeof(int), st);
     if (e != cudaSuccess) return e;
-    launch_k(ce_rows_kernel<D>, units < ctas ? units : ctas, CE_THREADS, CeSmem<D>::ROWS_BYTES, st, tmX, tmE, a);
-    return cudaGetLastError();
+    return launch_k(ce_rows_kernel<D>, units < ctas ? units : ctas, CE_THREADS, CeSmem<D>::ROWS_BYTES, st, tmX, tmE, a);
 }
 // a.dtable += d loss / d table, from the shifts launch_tc_ce left, on at most `ctas` CTAs
 template <int D>
 inline cudaError_t launch_ce_table(const bf16* xf, const bf16* table, const CeArgs& a, int ctas, cudaStream_t st) {
     CUtensorMap tmX, tmE;
     if (!make_tmap_bf16(&tmX, xf, a.T, D, D, 64, 64) || !make_tmap_bf16(&tmE, table, a.C, D, D, 64, 64)) return cudaErrorInvalidValue;
-    cudaError_t e = set_max_smem(ce_table_kernel<D>, CeSmem<D>::TABLE_BYTES);
-    if (e != cudaSuccess) return e;
     const int NC = (a.C + 63) / 64, units = a.tseg * NC;
-    e = cudaMemsetAsync(a.tsched, 0, (size_t)(1 + NC) * sizeof(int), st);
+    const cudaError_t e = cudaMemsetAsync(a.tsched, 0, (size_t)(1 + NC) * sizeof(int), st);
     if (e != cudaSuccess) return e;
-    launch_k(ce_table_kernel<D>, units < ctas ? units : ctas, CE_THREADS, CeSmem<D>::TABLE_BYTES, st, tmX, tmE, a);
-    return cudaGetLastError();
+    return launch_k(ce_table_kernel<D>, units < ctas ? units : ctas, CE_THREADS, CeSmem<D>::TABLE_BYTES, st, tmX, tmE, a);
 }
 
 }  // namespace grb

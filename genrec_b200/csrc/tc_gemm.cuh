@@ -627,13 +627,9 @@ inline cudaError_t launch_tc_gemm(const bf16* A, const bf16* B, int M, int N, in
     sh.num_m = (M + TC_BM - 1) / TC_BM;
     sh.num_n = (N + TC_BN - 1) / TC_BN;
     sh.kblocks_total = (K + TC_BK - 1) / TC_BK;
-    auto kern = tc_gemm_kernel<B_MN, Epi>;
-    cudaError_t e = set_max_smem(kern, TC_SMEM_BYTES);
-    if (e != cudaSuccess) return e;
     int work = sh.num_m * sh.num_n;
     int grid = work < num_sms ? work : num_sms;
-    launch_k(kern, grid, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, tmC0, tmC1, sh, epi);
-    return cudaGetLastError();
+    return launch_k(tc_gemm_kernel<B_MN, Epi>, grid, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, tmC0, tmC1, sh, epi);
 }
 
 }  // namespace grb

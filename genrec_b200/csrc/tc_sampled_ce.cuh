@@ -378,16 +378,13 @@ inline cudaError_t launch_sampled_ce(const SceArgs& a, int sms, cudaStream_t st)
         return cudaErrorInvalidValue;
     // the row kernel asks for its largest size once, so no later call with more negatives has to raise the attribute
     cudaError_t e = set_max_smem(sce_rows_kernel<D>, sce_rows_smem<D>(SCE_MAX_N));
-    if (e == cudaSuccess) e = set_max_smem(sce_table_kernel<D>, CeSmem<D>::TABLE_BYTES);
-    if (e != cudaSuccess) return e;
-    launch_k(sce_gather_kernel, (a.Npad + 7) / 8, 256, 0, st, a);
-    launch_k(sce_target_kernel, (a.T + 7) / 8, 256, 0, st, a);
-    launch_k(sce_rows_kernel<D>, (a.T + 127) / 128, CE_THREADS, sce_rows_smem<D>(a.Npad), st, tmX128, tmE, a);
-    if (a.dxf) {
-        launch_k(sce_table_kernel<D>, dim3(a.Npad / 64, a.ks), CE_THREADS, CeSmem<D>::TABLE_BYTES, st, tmX64, tmE, a);
-        launch_k(sce_scatter_kernel, 2 * sms, SCE_SCATTER_THREADS, 0, st, a);
-    }
-    return cudaGetLastError();
+    if (e == cudaSuccess) e = launch_k(sce_gather_kernel, (a.Npad + 7) / 8, 256, 0, st, a);
+    if (e == cudaSuccess) e = launch_k(sce_target_kernel, (a.T + 7) / 8, 256, 0, st, a);
+    if (e == cudaSuccess) e = launch_k(sce_rows_kernel<D>, (a.T + 127) / 128, CE_THREADS, sce_rows_smem<D>(a.Npad), st, tmX128, tmE, a);
+    if (e != cudaSuccess || !a.dxf) return e;
+    e = launch_k(sce_table_kernel<D>, dim3(a.Npad / 64, a.ks), CE_THREADS, CeSmem<D>::TABLE_BYTES, st, tmX64, tmE, a);
+    if (e == cudaSuccess) e = launch_k(sce_scatter_kernel, 2 * sms, SCE_SCATTER_THREADS, 0, st, a);
+    return e;
 }
 
 }  // namespace grb

@@ -230,18 +230,14 @@ inline cudaError_t launch_tc_tn_group(const TnSpec* specs, int n, int num_sms, f
             return cudaErrorInvalidValue;
     }
     const int work = P.total_work;
-    cudaError_t e = set_max_smem(tc_tn_group_kernel, TN_SMEM_BYTES);
-    if (e != cudaSuccess) return e;
     int grid = work < num_sms ? work : num_sms;
-    launch_k(tc_tn_group_kernel, grid, TC_THREADS, TN_SMEM_BYTES, st, P);
-    e = cudaGetLastError();
+    const cudaError_t e = launch_k(tc_tn_group_kernel, grid, TC_THREADS, TN_SMEM_BYTES, st, P);
     if (e != cudaSuccess) return e;
     int tiles = 0;
     for (int i = 0; i < n; ++i)
         if (P.p[i].splits > 1) tiles += P.p[i].num_m * P.p[i].num_n;
     if (tiles == 0) return cudaSuccess;
-    launch_k(tn_finish_kernel, tiles * TN_FINISH_SLABS, 256, 0, st, P);
-    return cudaGetLastError();
+    return launch_k(tn_finish_kernel, tiles * TN_FINISH_SLABS, 256, 0, st, P);
 }
 
 }  // namespace grb
