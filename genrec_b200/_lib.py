@@ -149,6 +149,8 @@ SIGNATURES = {
     "grb_trie_log_softmax": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                      c_void_p, c_void_p]),
     "grb_beam_select": (c_int, [c_void_p] * 8 + [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_beam_select_wide_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "grb_beam_select_wide": (c_int, [c_void_p] * 8 + [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_cast_f32_to_bf16": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
     "grb_adam_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_float, c_float,
                               c_float, c_float, c_float, c_float, c_int, c_void_p]),

@@ -2,6 +2,7 @@
 // Nothing here allocates or synchronises; every kernel goes onto the caller's stream.
 #include "../../include/genrec_b200.h"
 
+#include <climits>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -1561,9 +1562,16 @@ int grb_t5_attention_forward(const void* q, const void* k, const void* v, int B,
     GRB_REQUIRE(out && lse && ldo % 8 == 0 && aligned16(out), "bad output");
     a.out = (bf16*)out; a.ldo = ldo; a.lse = lse;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    dim3 grid((Lq + T5_ROWS - 1) / T5_ROWS, B * H);
+    const long long bh = (long long)B * H;
+    GRB_REQUIRE(bh <= INT_MAX, "B * H = %lld too large (at most 2^31 - 1)", bh);
+    const unsigned nx = (Lq + T5_ROWS - 1) / T5_ROWS;
     return with_head_dim(head_dim, [&](auto DH) -> int {
-        GRB_LAUNCH(t5_attn_fwd_kernel<DH>, grid, T5_THREADS, t5_fwd_smem<DH>(a.nb), st, a);
+        if (bh <= 65535) {
+            GRB_LAUNCH((t5_attn_fwd_kernel<DH, false>), dim3(nx, (unsigned)bh), T5_THREADS, t5_fwd_smem<DH>(a.nb), st, a);
+        } else {
+            GRB_LAUNCH((t5_attn_fwd_kernel<DH, true>), dim3(nx, 65535u, (unsigned)((bh + 65534) / 65535)), T5_THREADS, t5_fwd_smem<DH>(a.nb),
+                       st, a);
+        }
         return 0;
     });
 }
@@ -1643,6 +1651,59 @@ int grb_beam_select(const int64_t* beam_seqs, const float* beam_logps, const int
     BeamSelectArgs a{reinterpret_cast<const long long*>(beam_seqs), beam_logps, reinterpret_cast<const long long*>(cand_tok), cand_logp, nodes,
                      TrieCsr{child_off, child_tok, child_node, n_nodes}, K, KK, S, reinterpret_cast<long long*>(new_seqs), new_logps, new_nodes};
     GRB_LAUNCH(beam_select_kernel, B, BEAM_MAX_CAND, 0, static_cast<cudaStream_t>(stream), a);
+    return 0;
+}
+
+namespace {
+struct BeamWideWork {
+    int* cls;
+    unsigned long long* table;
+    unsigned* mono;
+    int cap_log2;
+    size_t table_bytes, bytes;
+};
+BeamWideWork carve_beam_wide(void* base, int B, int K, int KK) {
+    BeamWideWork w{};
+    const size_t n = (size_t)K * KK;
+    while (((size_t)1 << w.cap_log2) < 2 * n) ++w.cap_log2;
+    Carver c{static_cast<char*>(base)};
+    w.table_bytes = ((size_t)B << w.cap_log2) * sizeof(unsigned long long);
+    w.table = c.take<unsigned long long>(w.table_bytes);
+    w.cls = c.take<int>((size_t)B * K * sizeof(int));
+    w.mono = c.take<unsigned>((size_t)B * n * sizeof(unsigned));
+    w.bytes = c.off;
+    return w;
+}
+bool beam_wide_shape_ok(int B, int K, int KK, int S) {
+    return B >= 0 && K >= 1 && K <= BEAM_WIDE_MAX_K && KK >= 1 && (long long)K * KK <= BEAM_WIDE_MAX_CAND && S >= 0;
+}
+}  // namespace
+
+size_t grb_beam_select_wide_workspace_bytes(int B, int K, int KK) {
+    if (!beam_wide_shape_ok(B, K, KK, 0)) return 0;
+    return carve_beam_wide(nullptr, B, K, KK).bytes;
+}
+int grb_beam_select_wide(const int64_t* beam_seqs, const float* beam_logps, const int64_t* cand_tok, const float* cand_logp, const int32_t* nodes,
+                         const int32_t* child_off, const int32_t* child_tok, const int32_t* child_node, int n_nodes, int B, int K, int KK, int S,
+                         int64_t* new_seqs, float* new_logps, int32_t* new_nodes, void* workspace, void* stream) {
+    GRB_REQUIRE(beam_logps && cand_tok && cand_logp && new_seqs && new_logps && (S == 0 || beam_seqs), "null argument");
+    GRB_REQUIRE(beam_wide_shape_ok(B, K, KK, S), "bad shape B=%d K=%d KK=%d S=%d (1 <= K <= %d, K*KK <= %d)", B, K, KK, S, BEAM_WIDE_MAX_K,
+                BEAM_WIDE_MAX_CAND);
+    GRB_REQUIRE(!new_nodes || (nodes && child_off && child_tok && child_node && n_nodes > 0), "trie arrays missing");
+    GRB_REQUIRE(workspace && aligned16(workspace), "workspace must be non-null and 16-byte aligned");
+    if (B == 0) return 0;
+    const BeamWideWork ws = carve_beam_wide(workspace, B, K, KK);
+    BeamWideArgs w{BeamSelectArgs{reinterpret_cast<const long long*>(beam_seqs), beam_logps, reinterpret_cast<const long long*>(cand_tok),
+                                  cand_logp, nodes, TrieCsr{child_off, child_tok, child_node, n_nodes}, K, KK, S,
+                                  reinterpret_cast<long long*>(new_seqs), new_logps, new_nodes},
+                   B, ws.cap_log2, ws.cls, ws.table, ws.mono};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t total = (size_t)B * K * KK;
+    GRB_CUDA(cudaMemsetAsync(ws.table, 0, ws.table_bytes, st));
+    GRB_LAUNCH(beam_class_kernel, B, BEAM_WIDE_THREADS, 0, st, w);
+    GRB_LAUNCH(beam_dedup_insert_kernel, capped_blocks(total), 256, 0, st, w);
+    GRB_LAUNCH(beam_dedup_mark_kernel, capped_blocks(total), 256, 0, st, w);
+    GRB_LAUNCH(beam_wide_select_kernel, B, BEAM_WIDE_THREADS, 0, st, w);
     return 0;
 }
 

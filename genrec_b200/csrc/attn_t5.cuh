@@ -84,7 +84,8 @@ GRB_DEVINL bool t5_score(const T5AttnArgs& a, const float* sbias, int b, int i, 
     return true;
 }
 
-template <int DH>
+// SPLIT_BH: (b, h) = blockIdx.z * gridDim.y + blockIdx.y, for B * H past the 65,535 CTAs gridDim.y allows; otherwise blockIdx.y
+template <int DH, bool SPLIT_BH>
 __global__ void __launch_bounds__(T5_THREADS) t5_attn_fwd_kernel(T5AttnArgs a) {
     pdl_wait();
     a.drop.resolve();
@@ -93,7 +94,9 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_fwd_kernel(T5AttnArgs a) {
     float* Vs = Ks + T5_KEYS * (DH + 1);
     float* sbias = a.bias ? Vs + T5_KEYS * (DH + 1) : nullptr;   // [nb] this head's row of the table
     const int tid = threadIdx.x, r = tid >> 2, kq = tid & 3;
-    const int b = blockIdx.y / a.H, h = blockIdx.y % a.H;
+    const int bh = SPLIT_BH ? (int)(blockIdx.z * gridDim.y + blockIdx.y) : (int)blockIdx.y;
+    if (SPLIT_BH && bh >= a.B * a.H) return;
+    const int b = bh / a.H, h = bh % a.H;
     const int i = blockIdx.x * T5_ROWS + r;
     if (sbias) for (int e = tid; e < a.nb; e += T5_THREADS) sbias[e] = a.bias[h * a.nb + e];
     float q[DH], o[DH];

@@ -316,13 +316,35 @@ class Tiger(nn.Module):
     def generate(self, user_input_ids, item_input_ids, token_type_ids, seq_mask=None, temperature: float = 0.2, n_top_k_candidates: int = 10,
                  valid_item_ids=None, use_trie: bool = True, generator: Optional[torch.Generator] = None) -> TigerGenerationOutput:
         """Trie-constrained beam search (tiger.py:312-452) with the memory's cross-attention K / V projected once per user.  No host
-        synchronisation once the trie is built (first call), so a warmed-up call can be captured in a CUDA graph."""
-        B, K = user_input_ids.size(0), n_top_k_candidates
+        synchronisation once the trie is built (first call), so a warmed-up call can be captured in a CUDA graph.  1 <= K <= 1024
+        beams per user with K * min(6 K, num_item_embeddings) <= 262,144 (ValueError before anything runs otherwise)."""
+        out, _, _ = self._generate(user_input_ids, item_input_ids, token_type_ids, seq_mask, temperature, n_top_k_candidates, valid_item_ids,
+                                   use_trie, generator)
+        return out
+
+    @torch.no_grad()
+    def retrieve(self, user_input_ids, item_input_ids, token_type_ids, seq_mask=None, num_candidates: int = 500, valid_item_ids=None,
+                 temperature: float = 0.2, generator: Optional[torch.Generator] = None):
+        """Candidates for a ranker: ``generate`` with the trie, plus the catalog row of each beam's item.  Returns (items [B, K] int64,
+        sem_ids [B, K, sem_id_dim], log_probas [B, K]); items are rows of ``valid_item_ids`` (the smallest row holding the beam's
+        tuple), -1 for filler beams and for beams whose sequence left the trie.  The beams are ``generate``'s under the same generator
+        state."""
+        out, nodes, trie = self._generate(user_input_ids, item_input_ids, token_type_ids, seq_mask, temperature, num_candidates,
+                                          valid_item_ids, True, generator, want_nodes=True)
+        return trie.rows(nodes), out.sem_ids, out.log_probas
+
+    def _generate(self, user_input_ids, item_input_ids, token_type_ids, seq_mask, temperature, K, valid_item_ids, use_trie, generator,
+                  want_nodes=False):
+        """-> (beams, final trie nodes if want_nodes else None, trie); the arguments are checked before anything runs."""
+        td.check_width(K, td.candidates_per_beam(K, self.num_item_embeddings))
+        B = user_input_ids.size(0)
         dev = user_input_ids.device
         trie = None
         if use_trie:
             trie = getattr(self, "_grb_trie", None)
             if trie is None:
+                if valid_item_ids is None:
+                    raise ValueError("the trie is built from valid_item_ids on the first call")
                 trie = td.TrieCSR.build(valid_item_ids).to(dev)
                 self._grb_trie = trie
         memory, memory_pad = self._encode_context(user_input_ids, item_input_ids, token_type_ids, seq_mask)
@@ -363,4 +385,8 @@ class Tiger(nn.Module):
             logits = _head_logits(Fn.cast_rows_bf16(out[:, -1].contiguous()), wpt, V)
             return logits if rows == B * K else logits.unsqueeze(1).expand(B, K, V).reshape(B * K, V)
 
-        return td.beam_search(decode_step, B, K, self.sem_id_dim, self.num_item_embeddings, dev, temperature, trie, generator)
+        run = (B, K, self.sem_id_dim, self.num_item_embeddings, dev, temperature, trie, generator)
+        if want_nodes:
+            out, nodes = td.beam_search(decode_step, *run, return_nodes=True)
+            return out, nodes, trie
+        return td.beam_search(decode_step, *run), None, trie

@@ -30,8 +30,9 @@ class TrieCSR:
     """The reference's dict trie (tiger.py:40-69) as three int32 arrays.  Node 0 is the root; the nodes of level l are the distinct
     prefixes of length l + 1 in lexicographic order, so the children of a node are contiguous and sorted by token."""
 
-    def __init__(self, child_off: torch.Tensor, child_tok: torch.Tensor, child_node: torch.Tensor, depth: int):
+    def __init__(self, child_off: torch.Tensor, child_tok: torch.Tensor, child_node: torch.Tensor, depth: int, leaf_row: torch.Tensor):
         self.child_off, self.child_tok, self.child_node, self.depth = child_off, child_tok, child_node, depth
+        self.leaf_row = leaf_row      # [n_nodes] int64: the smallest row of valid_item_ids holding a leaf's tuple, -1 for other nodes
 
     @property
     def n_nodes(self) -> int:
@@ -48,7 +49,7 @@ class TrieCSR:
         n, depth = v.shape
         parents, toks = [], []
         base_prev, inv_prev = 0, torch.zeros(n, dtype=torch.int64)          # level -1: everything hangs off the root
-        base = 1
+        base, rep = 1, torch.zeros(0, dtype=torch.int64)
         for lvl in range(depth):
             uniq, inv = torch.unique(v[:, :lvl + 1], dim=0, return_inverse=True)
             rep = torch.full((uniq.size(0),), n, dtype=torch.int64).scatter_reduce_(0, inv, torch.arange(n), "amin")   # a row per node
@@ -57,6 +58,8 @@ class TrieCSR:
             base_prev, inv_prev = base, inv
             base += uniq.size(0)
         n_nodes = base
+        leaf_row = torch.full((n_nodes,), -1, dtype=torch.int64)
+        leaf_row[n_nodes - rep.numel():] = rep                             # the last level's nodes are the leaves
         parent = torch.cat(parents) if parents else torch.zeros(0, dtype=torch.int64)
         tok = torch.cat(toks) if toks else torch.zeros(0, dtype=torch.int64)
         child = torch.arange(1, n_nodes, dtype=torch.int64)
@@ -65,10 +68,15 @@ class TrieCSR:
         off = torch.zeros(n_nodes + 1, dtype=torch.int64)
         off[1:] = torch.cumsum(counts, 0)
         order = torch.argsort(parent * (int(tok.max().item()) + 1 if tok.numel() else 1) + tok, stable=True)
-        return TrieCSR(off.to(torch.int32), tok[order].to(torch.int32), child[order].to(torch.int32), depth)
+        return TrieCSR(off.to(torch.int32), tok[order].to(torch.int32), child[order].to(torch.int32), depth, leaf_row)
 
     def to(self, device) -> "TrieCSR":
-        return TrieCSR(self.child_off.to(device), self.child_tok.to(device), self.child_node.to(device), self.depth)
+        return TrieCSR(self.child_off.to(device), self.child_tok.to(device), self.child_node.to(device), self.depth,
+                       self.leaf_row.to(device))
+
+    def rows(self, nodes: torch.Tensor) -> torch.Tensor:
+        """Catalog row of the leaf each node id stands for (int64), -1 for dead (-1) and non-leaf nodes."""
+        return torch.where(nodes >= 0, self.leaf_row[nodes.long().clamp(min=0)], -1)
 
 
 def trie_log_softmax(logits: torch.Tensor, nodes: Optional[torch.Tensor], trie: Optional[TrieCSR], vocab_offset: int, num_embeddings: int,
@@ -89,12 +97,30 @@ def trie_log_softmax(logits: torch.Tensor, nodes: Optional[torch.Tensor], trie: 
     return probs, logp
 
 
+MAX_BEAMS = 1024                   # K: beams per user
+MAX_CANDIDATES = 262144            # K * KK: candidates per user and step
+
+
+def candidates_per_beam(K: int, num_item_embeddings: int) -> int:
+    return min(K * 6, num_item_embeddings)                                       # (tiger.py:349-350)
+
+
+def check_width(K: int, KK: int) -> None:
+    """Refuse a beam step the kernels cannot run, before anything is launched."""
+    if not 1 <= K <= MAX_BEAMS:
+        raise ValueError(f"n_top_k_candidates = {K} is outside 1 .. {MAX_BEAMS} (beams per user)")
+    if KK < 1 or K * KK > MAX_CANDIDATES:
+        raise ValueError(f"K * KK = {K} * {KK} = {K * KK} candidates per user and step; the limit is {MAX_CANDIDATES} "
+                         f"(KK = min(6 K, num_item_embeddings))")
+
+
 def beam_select(beam_seqs: torch.Tensor, beam_logps: torch.Tensor, cand_tok: torch.Tensor, cand_logp: torch.Tensor,
                 nodes: Optional[torch.Tensor], trie: Optional[TrieCSR]):
     """One beam update (tiger.py:386-441): beam_seqs [B, K, S] int64, beam_logps [B, K], cand_tok / cand_logp [B, K, KK] ->
     (new_seqs [B, K, S+1], new_logps [B, K], new_nodes [B, K] int32 | None)."""
-    require_cuda(beam_logps, cand_tok, cand_logp)
     B, K, KK = cand_tok.shape
+    check_width(K, KK)
+    require_cuda(beam_logps, cand_tok, cand_logp)
     S = beam_seqs.size(2)
     dev = beam_logps.device
     seqs = beam_seqs.to(torch.int64).contiguous()
@@ -103,22 +129,27 @@ def beam_select(beam_seqs: torch.Tensor, beam_logps: torch.Tensor, cand_tok: tor
     use = trie is not None
     new_nodes = torch.empty(B, K, dtype=torch.int32, device=dev) if use else None
     nodes_c = nodes.to(torch.int32).contiguous() if use else None
+    lib = _lib.load()
+    args = (ptr(seqs) if S > 0 else None, ptr(beam_logps.float().contiguous()), ptr(cand_tok.to(torch.int64).contiguous()),
+            ptr(cand_logp.float().contiguous()), ptr(nodes_c), ptr(trie.child_off) if use else None, ptr(trie.child_tok) if use else None,
+            ptr(trie.child_node) if use else None, trie.n_nodes if use else 0, B, K, KK, S, ptr(new_seqs), ptr(new_logps), ptr(new_nodes))
     with torch.cuda.device(dev):
-        check(_lib.load().grb_beam_select(ptr(seqs) if S > 0 else None, ptr(beam_logps.float().contiguous()), ptr(cand_tok.to(torch.int64).contiguous()),
-                                          ptr(cand_logp.float().contiguous()), ptr(nodes_c), ptr(trie.child_off) if use else None,
-                                          ptr(trie.child_tok) if use else None, ptr(trie.child_node) if use else None,
-                                          trie.n_nodes if use else 0, B, K, KK, S, ptr(new_seqs), ptr(new_logps), ptr(new_nodes),
-                                          stream_ptr(dev)))
+        if K <= 32 and K * KK <= 1024:                                           # one CTA sorts a row's candidates
+            check(lib.grb_beam_select(*args, stream_ptr(dev)))
+        else:
+            ws = torch.empty(lib.grb_beam_select_wide_workspace_bytes(B, K, KK), dtype=torch.uint8, device=dev)
+            check(lib.grb_beam_select_wide(*args, ptr(ws), stream_ptr(dev)))
     return new_seqs, new_logps, new_nodes
 
 
 @torch.no_grad()
 def beam_search(decode_step, B: int, K: int, sem_id_dim: int, num_item_embeddings: int, device, temperature: float = 0.2,
-                trie: Optional[TrieCSR] = None, generator: Optional[torch.Generator] = None, draws=None) -> TigerGenerationOutput:
+                trie: Optional[TrieCSR] = None, generator: Optional[torch.Generator] = None, draws=None, return_nodes: bool = False):
     """The loop of Tiger.generate (tiger.py:352-452).  ``decode_step(beam_seqs [B*K, S] int64) -> logits [B*K, V]`` is the caller's
-    decoder; ``draws`` (test hook) replaces torch.multinomial by recorded candidate indices, one [B*K, KK] tensor per step."""
-    R = 6
-    KK = min(K * R, num_item_embeddings)                                         # (tiger.py:349-350)
+    decoder; ``draws`` (test hook) replaces torch.multinomial by recorded candidate indices, one [B*K, KK] tensor per step.
+    ``return_nodes``: also return the trie node each final beam reached ([B, K] int32, None without a trie)."""
+    KK = candidates_per_beam(K, num_item_embeddings)
+    check_width(K, KK)
     beam_seqs = torch.empty(B, K, 0, dtype=torch.long, device=device)
     beam_logps = torch.zeros(B, K, device=device)
     nodes = torch.zeros(B, K, dtype=torch.int32, device=device) if trie is not None else None
@@ -131,7 +162,8 @@ def beam_search(decode_step, B: int, K: int, sem_id_dim: int, num_item_embedding
         cand_logp = torch.gather(logp, 1, cand)
         beam_seqs, beam_logps, nodes = beam_select(beam_seqs, beam_logps, (cand - vocab_offset).view(B, K, KK), cand_logp.view(B, K, KK),
                                                    nodes, trie)
-    return TigerGenerationOutput(sem_ids=beam_seqs, log_probas=beam_logps)
+    out = TigerGenerationOutput(sem_ids=beam_seqs, log_probas=beam_logps)
+    return (out, nodes) if return_nodes else out
 
 
 @torch.no_grad()
@@ -142,6 +174,7 @@ def generate(model, user_input_ids: torch.Tensor, item_input_ids: torch.Tensor, 
     """Same arguments and result as ``Tiger.generate`` (tiger.py:312-323) for any module with the reference's ``_encode_context`` /
     ``_decode_step`` / ``sem_id_dim`` / ``num_item_embeddings``; ``trie`` (a TrieCSR already on the device) avoids rebuilding it."""
     B, K = user_input_ids.size(0), n_top_k_candidates
+    check_width(K, candidates_per_beam(K, model.num_item_embeddings))
     device = user_input_ids.device
     memory, memory_mask = model._encode_context(user_input_ids, item_input_ids, token_type_ids, seq_mask)
     memory = memory.unsqueeze(1).expand(-1, K, -1, -1).reshape(B * K, memory.size(1), -1)

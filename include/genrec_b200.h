@@ -359,7 +359,8 @@ int grb_layernorm_f32_forward(const float* x, const float* g, const float* b, fl
  * cross-attention); key_pad [B, Lk] 1 = padded (NULL: none); lse [B, H, Lq, 2] = {row max, sum of exp(s - max)} is saved for the backward.
  * Backward: dq bf16 [B, Lq, lddq]; dk, dv fp32 [B, Lk, H * head_dim] (overwritten); dbias [H, num_buckets] +=.  Every sum runs in a
  * fixed order, so two calls give the same bits.  workspace: grb_t5_attention_backward_workspace_bytes(B, Lq, Lk, H, head_dim,
- * num_buckets), 16-byte aligned; num_buckets = 0 without a bias table.  It may be 0 bytes (workspace NULL then allowed). */
+ * num_buckets), 16-byte aligned; num_buckets = 0 without a bias table.  It may be 0 bytes (workspace NULL then allowed).  The
+ * forward runs at any B * H up to 2^31 - 1; the backward needs B * H <= 65,535. */
 int grb_t5_attention_forward(const void* q, const void* k, const void* v, int B, int Lq, int Lk, int H, int head_dim, int ldq, int ldk, int ldv,
                              const float* bias, const int32_t* bucket, int num_buckets, const uint8_t* key_pad, int causal, float scale,
                              float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t site, void* out, int ldo, float* lse,
@@ -387,6 +388,16 @@ int grb_trie_log_softmax(const float* logits, int rows, int V, const int32_t* no
 int grb_beam_select(const int64_t* beam_seqs, const float* beam_logps, const int64_t* cand_tok, const float* cand_logp, const int32_t* nodes,
                     const int32_t* child_off, const int32_t* child_tok, const int32_t* child_node, int n_nodes, int B, int K, int KK, int S,
                     int64_t* new_seqs, float* new_logps, int32_t* new_nodes, void* stream);
+/* grb_beam_select for retrieval-sized beams: the same contract with 1 <= K <= 1024 and K * KK <= 262,144 (GRB_EINVAL otherwise,
+ * before any launch).  cand_tok may hold any int64, negative ones included; totals may be -inf or any finite value.  Every
+ * duplicate (class, token) - class = the smallest parent with the same token sequence - is removed as the greedy scan removes it,
+ * whole classes of identical parents included.  Deterministic, no host synchronisation.  grb_beam_select is faster where it
+ * applies (K <= 32, K * KK <= 1024).  workspace: grb_beam_select_wide_workspace_bytes(B, K, KK) bytes, 16-byte aligned (0 for
+ * unsupported arguments); it grows with B * K * KK. */
+size_t grb_beam_select_wide_workspace_bytes(int B, int K, int KK);
+int grb_beam_select_wide(const int64_t* beam_seqs, const float* beam_logps, const int64_t* cand_tok, const float* cand_logp, const int32_t* nodes,
+                         const int32_t* child_off, const int32_t* child_tok, const int32_t* child_node, int n_nodes, int B, int K, int KK, int S,
+                         int64_t* new_seqs, float* new_logps, int32_t* new_nodes, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ optimizer / casts */
 int grb_cast_f32_to_bf16(const float* in, void* out_bf16, size_t n, void* stream);

@@ -2,7 +2,7 @@
 cached incremental HSTU inference next to full recompute, RQ-VAE Sinkhorn and k-means init) with CUDA events, against the relevant
 roofline or the torch code they replace.  Prints one JSON line per measurement; `bench_kernels.py rqvae_train` runs only the RQ-VAE
 training rows, `bench_kernels.py linear_bwd` only the linear-backward and SASRec training-step rows, `bench_kernels.py head_topk` only
-the fused top-k head rows, `bench_kernels.py tiger` only the TIGER rows (training step, generate eager / graph / uncached loop),
+the fused top-k head rows, `bench_kernels.py tiger` only the TIGER rows (training step, generate eager / graph / uncached loop, wide beams),
 `bench_kernels.py hstu_attn` only the HSTU attention backward rows, `bench_kernels.py head_rank` only the rows of evaluation without
 logits, `bench_kernels.py head_candidates` only the rows of retrieval without logits."""
 import json
@@ -550,6 +550,102 @@ def bench_tiger(dev):
         print(json.dumps(dict(kernel="tiger_generate_" + name, B=B, K=K, trie_items=12000, ms_per_round=v, ms=min(v), **info)), flush=True)
     print(json.dumps(dict(kernel="tiger_generate_speedup", eager_vs_uncached=min(rows["uncached"]) / min(rows["eager"]),
                           graph_vs_uncached=min(rows["uncached"]) / min(rows["graph"]))), flush=True)
+    del graph
+    bench_tiger_wide(dev, m, args, info)
+
+
+def bench_tiger_wide(dev, m, args, info):
+    """Retrieval-sized beams at B = 256 on the published model and a 12,000-item trie: Tiger.generate at K = 64, 256, 1024 (eager and
+    replayed from a CUDA graph, alternated in rounds) with its peak memory; per decode step, the device time of the beam-select
+    launches next to that step's torch.multinomial (torch.profiler, a run of its own); and the beam step alone at K = 10, where
+    both the one-CTA kernel and the wide path apply."""
+    from torch.profiler import ProfilerActivity, profile, record_function
+    from genrec_b200 import _lib
+    from genrec_b200 import tiger_decode as td
+    from genrec_b200._lib import ptr, stream_ptr
+    B = 256
+    for K in (10, 64, 256, 1024):
+        gen = lambda: m.generate(*args, n_top_k_candidates=K)                  # noqa: E731
+        gen()
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        base = torch.cuda.memory_allocated()
+        gen()
+        torch.cuda.synchronize()
+        peak = torch.cuda.max_memory_allocated() - base
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            gen()
+        torch.cuda.current_stream().wait_stream(s)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            gen()
+        rows = {"eager": [], "graph": []}
+        iters = 10 if K <= 64 else 3
+        for _ in range(3):
+            rows["eager"].append(timed(gen, iters=iters, warm=1))
+            rows["graph"].append(timed(graph.replay, iters=iters, warm=1))
+        del graph
+        torch.cuda.empty_cache()
+        if K > 10:
+            for name, v in rows.items():
+                print(json.dumps(dict(kernel="tiger_generate_" + name, B=B, K=K, trie_items=12000, ms_per_round=v, ms=min(v),
+                                      peak_extra_bytes=peak, **info)), flush=True)
+        # per-step device time: the beam step's launches (a record_function range around tiger_decode.beam_select) and the
+        # step's torch.multinomial, over 3 generate calls of 3 steps each
+        orig = td.beam_select
+
+        def traced(*a, **k):
+            with record_function("grb_beam_step"):
+                return orig(*a, **k)
+
+        td.beam_select = traced
+        try:
+            with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+                for _ in range(3):
+                    gen()
+                torch.cuda.synchronize()
+        finally:
+            td.beam_select = orig
+        steps = 3 * m.sem_id_dim
+        ev = {e.key: e.device_time_total / steps for e in prof.key_averages()}
+        kern = {k.split("(")[0].replace("void ", "").replace("grb::", ""): round(v, 1) for k, v in ev.items() if "beam_" in k}
+        print(json.dumps(dict(kernel="tiger_beam_step_vs_multinomial", B=B, K=K, KK=min(6 * K, 256), us_beam_step=round(ev.get("grb_beam_step", 0), 1),
+                              us_multinomial=round(ev.get("aten::multinomial", 0), 1), kernels_us_per_step=kern,
+                              us_trie_log_softmax=round(sum(v for k, v in ev.items() if "trie_log_softmax_kernel" in k), 1), **info)), flush=True)
+    # the beam step alone at K = 10 (KK = 60, second step): the one-CTA kernel against the wide path, alternated
+    lib = _lib.load()
+    g = torch.Generator().manual_seed(4)
+    K, KK, S = 10, 60, 1
+    valid = torch.randint(0, 256, (12000, 3), generator=g)
+    trie = td.TrieCSR.build(valid).to(dev)
+    seqs = valid[torch.randint(0, 12000, (B, K), generator=g)][:, :, :S].contiguous().to(dev)
+    off, toks, kids = trie.child_off.tolist(), trie.child_tok.tolist(), trie.child_node.tolist()
+    root = dict(zip(toks[off[0]:off[1]], kids[off[0]:off[1]]))
+    nodes = torch.tensor([[root.get(t, -1) for t in r] for r in seqs[..., 0].tolist()], dtype=torch.int32, device=dev)
+    logps = (-torch.rand(B, K, generator=g) * 3).to(dev)
+    tok = torch.stack([torch.randperm(256, generator=g)[:KK] for _ in range(B * K)]).view(B, K, KK).to(dev)
+    clogp = (-torch.rand(B, K, KK, generator=g) * 5).to(dev)
+    out_s, out_l = torch.empty(B, K, S + 1, dtype=torch.long, device=dev), torch.empty(B, K, device=dev)
+    out_n = torch.empty(B, K, dtype=torch.int32, device=dev)
+    ws = torch.empty(lib.grb_beam_select_wide_workspace_bytes(B, K, KK), dtype=torch.uint8, device=dev)
+    a = (ptr(seqs), ptr(logps), ptr(tok), ptr(clogp), ptr(nodes), ptr(trie.child_off), ptr(trie.child_tok), ptr(trie.child_node), trie.n_nodes,
+         B, K, KK, S, ptr(out_s), ptr(out_l), ptr(out_n))
+    calls = {"one_cta": lambda: lib.grb_beam_select(*a, stream_ptr(dev)), "wide": lambda: lib.grb_beam_select_wide(*a, ptr(ws), stream_ptr(dev))}
+    res = {}
+    for name, fn in calls.items():
+        assert fn() == 0
+        torch.cuda.synchronize()
+        res[name] = (out_s.clone(), out_l.clone(), out_n.clone())
+    same = all(torch.equal(x, y) for x, y in zip(res["one_cta"], res["wide"]))
+    rows = {n: [] for n in calls}
+    for _ in range(5):
+        for n, fn in calls.items():
+            rows[n].append(graph_timed(fn) * 1e3)
+    for n, v in rows.items():
+        print(json.dumps(dict(kernel="tiger_beam_step_k10_" + n, B=B, K=K, KK=KK, S=S, us_per_round=v, us=min(v), same_beams=same, **info)),
+              flush=True)
 
 
 def bench_hstu_attn(dev):
