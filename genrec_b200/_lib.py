@@ -73,6 +73,13 @@ SIGNATURES = {
     "grb_hstu_layer_backward": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuSeq), c_void_p, c_void_p, c_void_p,
                                         P(HstuLayerGrads), c_void_p, c_void_p]),
     "grb_hstu_bias_index": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "grb_hstu_bias_index_jagged": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p, c_int, c_void_p]),
+    "grb_hstu_layer_saved_bytes_jagged": (c_size_t, [P(HstuDims), c_int]),
+    "grb_hstu_layer_workspace_bytes_jagged": (c_size_t, [P(HstuDims), c_int]),
+    "grb_hstu_layer_forward_jagged": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuSeq), c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                              c_void_p]),
+    "grb_hstu_layer_backward_jagged": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuSeq), c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                               P(HstuLayerGrads), c_void_p, c_void_p]),
     "grb_hstu_attention_scratch_bytes": (c_size_t, [P(HstuDims)]),
     "grb_hstu_attention_forward": (c_int, [P(HstuDims), c_void_p, c_void_p, P(HstuSeq), c_void_p, c_void_p, c_void_p]),
     "grb_hstu_attention_backward": (c_int, [P(HstuDims), c_void_p, c_void_p, P(HstuSeq), c_void_p, c_void_p, c_void_p, c_void_p,
@@ -87,6 +94,7 @@ SIGNATURES = {
     "grb_hstu_layer_extend_paged": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuPool), c_int, c_void_p, c_void_p, c_void_p, c_int,
                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_collate_jagged": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_pack_jagged": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p] * 6),
     "grb_embed_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int,
                                   c_float, c_u64, c_void_p, c_void_p]),
     "grb_embed_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int, c_float,

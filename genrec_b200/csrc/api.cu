@@ -234,8 +234,9 @@ void layer_tn_specs(TnSpec (&specs)[3], const bf16* dyb, const bf16* hact, const
     specs[1] = {dz1, xn, dw1, 4 * D, D, T, 4 * D, D, D};         // dW1 += dz1^T xn
     specs[2] = {dzp, xb, dwp, 4 * D, D, T, 4 * D, D, D};         // dWp += dzp^T xb
 }
-LayerWork carve_work(void* base, const grb_hstu_dims* d) {
-    const size_t T = (size_t)d->B * d->L, D = d->D;
+// T token rows: B * L for a padded batch, the packed row count for a jagged one (the attention partials follow B * L either way)
+LayerWork carve_work(void* base, const grb_hstu_dims* d, size_t T) {
+    const size_t D = d->D;
     LayerWork w;
     Carver c{static_cast<char*>(base)};
     w.dyb = c.take<bf16>(T * D * 2);
@@ -282,6 +283,13 @@ int check_seq(const grb_hstu_dims* d, const grb_hstu_seq* s) {
                 "bias_index must be 16-byte aligned with a pitch that is a multiple of 8 and >= L");
     return 0;
 }
+// a packed batch: B sequences of at most L = max_len rows in T token rows (offsets on the device, never read here)
+int check_jagged(const grb_hstu_dims* d, const int64_t* offsets, int T) {
+    GRB_REQUIRE(offsets != nullptr, "offsets is null");
+    GRB_REQUIRE(T >= 1 && (long long)T * 4 * d->D <= INT32_MAX, "token rows T=%d out of range [1, 2^31 / (4 D)]", T);
+    GRB_REQUIRE(d->B <= 65535, "B=%d exceeds 65535 sequences", d->B);
+    return 0;
+}
 
 // the bias tables without the index matrix (bias_index null, ldix 0)
 HstuBiasArgs make_attn_bias(const grb_hstu_dims* d, const float* pos_table, const float* time_table, int has_time, int pos_uniform,
@@ -314,6 +322,7 @@ HstuAttnArgs make_attn_args(const grb_hstu_dims* d, const float* pos_table, cons
     a.q = P + 2 * D; a.k = P + 3 * D; a.v = P + D;
     a.ldq = a.ldk = a.ldv = 4 * D;
     a.B = d->B; a.L = d->L; a.H = d->H;
+    a.T = d->B * d->L;   // offsets stay null: a padded batch
     a.bias = make_attn_bias(d, pos_table, time_table, s);
     a.o = O; a.ldo = D;
     return a;
@@ -337,7 +346,8 @@ template <int DH>
 int launch_hstu_attn_fwd(const HstuAttnArgs& a, cudaStream_t st) {
     size_t smem = sizeof(AttSmem<DH, 1>) + align_up((size_t)(a.bias.npos * 64 + 1) * 4, 16);
     dim3 grid((a.L + ATT_BLK - 1) / ATT_BLK, a.H, a.B);
-    GRB_LAUNCH(hstu_attn_fwd_kernel<DH>, grid, ATT_THREADS, smem, st, a);
+    if (a.offsets) GRB_LAUNCH((hstu_attn_fwd_kernel<DH, true>), grid, ATT_THREADS, smem, st, a);
+    else GRB_LAUNCH((hstu_attn_fwd_kernel<DH, false>), grid, ATT_THREADS, smem, st, a);
     return 0;
 }
 // Fork/join helper: a non-blocking stream and its two events, created on first use, i.e. during warm-up, never while a CUDA graph
@@ -412,7 +422,8 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
     size_t smem_q = sizeof(AttSmem<DH>) + posb;
     SideStream& ss = attn_side_stream();
     GRB_TRY(ss.run(st, [&](cudaStream_t side) -> int {
-        GRB_LAUNCH(hstu_attn_bwd_dq_kernel<DH>, grid, ATT_THREADS, smem_q, side, a);
+        if (a.offsets) GRB_LAUNCH((hstu_attn_bwd_dq_kernel<DH, true>), grid, ATT_THREADS, smem_q, side, a);
+        else GRB_LAUNCH((hstu_attn_bwd_dq_kernel<DH, false>), grid, ATT_THREADS, smem_q, side, a);
         return 0;
     }));
     const bool has_time = a.bias.wtime != nullptr && a.bias.ntime > 0, pos_uni = a.bias.pos_uniform != 0;
@@ -420,8 +431,12 @@ int launch_hstu_attn_bwd(const HstuAttnArgs& a, cudaStream_t st) {
                     (size_t)4 * (att_time_bins(has_time, pos_uni, a.bias.ntime) + (pos_uni ? 0 : a.bias.npos + 1)) * 32 * sizeof(float);
     const int nmem = (int)(grid.x * grid.z), ngroups = has_time && a.dwtime ? 2 * a.H : a.H;
     GRB_REQUIRE((pos_uni || a.bias.npos <= 64) && a.bias.ntime <= 64, "attention backward: at most 64 position / time buckets");
-    auto dkdv_kernel = has_time ? (pos_uni ? hstu_attn_bwd_dkdv_kernel<DH, true, true> : hstu_attn_bwd_dkdv_kernel<DH, true, false>)
-                                : (pos_uni ? hstu_attn_bwd_dkdv_kernel<DH, false, true> : hstu_attn_bwd_dkdv_kernel<DH, false, false>);
+    auto pick = [&](auto jagged) {
+        constexpr bool J = decltype(jagged)::value;
+        return has_time ? (pos_uni ? hstu_attn_bwd_dkdv_kernel<DH, true, true, J> : hstu_attn_bwd_dkdv_kernel<DH, true, false, J>)
+                        : (pos_uni ? hstu_attn_bwd_dkdv_kernel<DH, false, true, J> : hstu_attn_bwd_dkdv_kernel<DH, false, false, J>);
+    };
+    auto dkdv_kernel = a.offsets ? pick(std::true_type{}) : pick(std::false_type{});
     GRB_LAUNCH(dkdv_kernel, grid, ATT_THREADS, smem_k, st, a, (int)posb);
     // groups h < H: position buckets of head h ; H + h: time buckets of head h ; element = bucket.  With uniform positions
     // the caller has already pointed dwpos at the single live row.
@@ -628,42 +643,60 @@ size_t grb_hstu_layer_saved_bytes(const grb_hstu_dims* d) {
 }
 size_t grb_hstu_layer_workspace_bytes(const grb_hstu_dims* d) {
     if (check_dims(d)) return 0;
-    return carve_work(nullptr, d).bytes;
+    return carve_work(nullptr, d, (size_t)d->B * d->L).bytes;
+}
+size_t grb_hstu_layer_saved_bytes_jagged(const grb_hstu_dims* d, int T) {
+    if (check_dims(d) || T < 1) return 0;
+    return carve_saved(nullptr, (size_t)T, d->D).bytes;
+}
+size_t grb_hstu_layer_workspace_bytes_jagged(const grb_hstu_dims* d, int T) {
+    if (check_dims(d) || T < 1) return 0;
+    return carve_work(nullptr, d, (size_t)T).bytes;
 }
 
-int grb_hstu_layer_forward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const float* x,
-                           float* y, void* saved, void* stream) {
-    GRB_TRY(check_dims(d));
+}  // extern "C"
+
+namespace {
+
+// hstu_idle_rows_zero_kernel on a grid that does not depend on the data (CUDA-graph replays change the offsets)
+int zero_idle_rows(const int64_t* offsets, int B, int T, bf16* base, int ld, int ncols, cudaStream_t st) {
+    GRB_LAUNCH(hstu_idle_rows_zero_kernel, (unsigned)(2 * sm_count()), 256, 0, st, reinterpret_cast<const long long*>(offsets), B, T, base,
+               ld, ncols);
+    return 0;
+}
+
+// One block on T token rows.  offsets null: a padded batch (T = B * L); otherwise the packed batch of check_jagged.
+int layer_forward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const int64_t* offsets, int T,
+                  const float* x, float* y, void* saved, cudaStream_t st) {
     GRB_REQUIRE(x && y && saved, "null argument");
     GRB_TRY(check_layer_params(p));
     GRB_TRY(check_seq(d, s));
     GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(saved), "buffers must be 16-byte aligned");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int T = d->B * d->L, D = d->D;
+    const int D = d->D;
     LayerSaved sv = carve_saved(saved, T, D);
 
     GRB_TRY(block_steps_in(p, x, sv, T, D, st));
     // 3. O = silu(Q K^T + bias) V, causal + key padding                                      (hstu.py:244-267)
     GRB_TRY(join_pending(st));   // a bias-index matrix built on the side stream (deferred schedule) must be complete
     HstuAttnArgs a = make_attn_args(d, p->pos_table, p->time_table, s, sv.P, sv.O);
+    a.offsets = reinterpret_cast<const long long*>(offsets); a.T = T;
     GRB_TRY(with_head_dim(D / d->H, [&](auto DH) { return launch_hstu_attn_fwd<DH>(a, st); }));
+    if (offsets) GRB_TRY(zero_idle_rows(offsets, d->B, T, sv.O, D, D, st));
     return block_steps_out(p, x, y, sv, T, D, make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_GATE), d->seed_dev),
                            make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_HID), d->seed_dev),
                            make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_OUT), d->seed_dev), st);
 }
 
-int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const float* dy,
-                            const void* saved, float* dx, const grb_hstu_layer_grads* g, void* workspace, void* stream) {
-    GRB_TRY(check_dims(d));
+int layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const int64_t* offsets, int T,
+                   const float* dy, const void* saved, float* dx, const grb_hstu_layer_grads* g, void* workspace, cudaStream_t st) {
     GRB_REQUIRE(p && dy && saved && dx && g && workspace, "null argument");
     GRB_TRY(check_seq(d, s));
     GRB_REQUIRE(g->proj_w && g->proj_b && g->pos_table && g->ln1_g && g->ln1_b && g->ffn1_w && g->ffn1_b && g->ffn2_w && g->ffn2_b &&
                     g->ln2_g && g->ln2_b, "null gradient pointer");
     GRB_REQUIRE(aligned16(dy) && aligned16(dx) && aligned16(saved) && aligned16(workspace), "buffers must be 16-byte aligned");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const int T = d->B * d->L, D = d->D;
+    const int D = d->D;
     LayerSaved sv = carve_saved(const_cast<void*>(saved), T, D);
-    LayerWork w = carve_work(workspace, d);
+    LayerWork w = carve_work(workspace, d, T);
     const Dropout drop_out = make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_OUT), d->seed_dev);
     const Dropout drop_hid = make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_FFN_HID), d->seed_dev);
     const Dropout drop_gate = make_dropout(d->dropout_p, d->seed, site_of(d->layer_index, SITE_GATE), d->seed_dev);
@@ -689,7 +722,9 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
     {
         HstuAttnArgs a = make_attn_args(d, p->pos_table, p->time_table, s, sv.P, sv.O);
         GRB_TRY(set_attn_bwd_args(a, d, s, w.dO, sv.zp, w.dzp, g->pos_table, g->time_table, w.part_attn));
+        a.offsets = reinterpret_cast<const long long*>(offsets); a.T = T;
         GRB_TRY(with_head_dim(D / d->H, [&](auto DH) { return launch_hstu_attn_bwd<DH>(a, st); }));
+        if (offsets) GRB_TRY(zero_idle_rows(offsets, d->B, T, w.dzp + D, 4 * D, 3 * D, st));   // the V | Q | K columns
     }
     // projection
     GRB_TRY(colsum_4d(w.dzp, g->proj_b));
@@ -701,6 +736,34 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
         GRB_CUDA(launch_tc_tn_group(specs, 3, sm_count(), w.part_tn, s_));
         return 0;
     });
+}
+
+}  // namespace
+
+extern "C" {
+
+int grb_hstu_layer_forward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const float* x,
+                           float* y, void* saved, void* stream) {
+    GRB_TRY(check_dims(d));
+    return layer_forward(d, p, s, nullptr, d->B * d->L, x, y, saved, static_cast<cudaStream_t>(stream));
+}
+int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const float* dy,
+                            const void* saved, float* dx, const grb_hstu_layer_grads* g, void* workspace, void* stream) {
+    GRB_TRY(check_dims(d));
+    return layer_backward(d, p, s, nullptr, d->B * d->L, dy, saved, dx, g, workspace, static_cast<cudaStream_t>(stream));
+}
+int grb_hstu_layer_forward_jagged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const int64_t* offsets,
+                                  int T, const float* x, float* y, void* saved, void* stream) {
+    GRB_TRY(check_dims(d));
+    GRB_TRY(check_jagged(d, offsets, T));
+    return layer_forward(d, p, s, offsets, T, x, y, saved, static_cast<cudaStream_t>(stream));
+}
+int grb_hstu_layer_backward_jagged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const int64_t* offsets,
+                                   int T, const float* dy, const void* saved, float* dx, const grb_hstu_layer_grads* g, void* workspace,
+                                   void* stream) {
+    GRB_TRY(check_dims(d));
+    GRB_TRY(check_jagged(d, offsets, T));
+    return layer_backward(d, p, s, offsets, T, dy, saved, dx, g, workspace, static_cast<cudaStream_t>(stream));
 }
 
 int grb_hstu_cache_append(const grb_hstu_cache* c, const int64_t* input_ids, const int64_t* timestamps, int n, int32_t* positions,
@@ -785,8 +848,12 @@ int grb_hstu_layer_extend_paged(const grb_hstu_dims* d, const grb_hstu_layer_par
     return layer_extend(d, p, kv, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace, static_cast<cudaStream_t>(stream));
 }
 
-int grb_hstu_bias_index(const int64_t* timestamps, const uint8_t* pad, const int64_t* time_thr, const uint8_t* pos_bucket, int B, int L,
-                        int npos, int ntime, uint16_t* out, int ld_index, void* stream) {
+}  // extern "C"
+
+namespace {
+
+int bias_index(const int64_t* timestamps, const uint8_t* pad, const int64_t* offsets, const int64_t* time_thr, const uint8_t* pos_bucket,
+               int B, int T, int L, int npos, int ntime, uint16_t* out, int ld_index, cudaStream_t st) {
     GRB_REQUIRE(pad && time_thr && pos_bucket && out, "null argument");
     GRB_REQUIRE(B > 0 && L > 0 && B <= 65535 && L <= 65535, "bad shape B=%d L=%d", B, L);
     GRB_REQUIRE(ld_index >= L && ld_index % 8 == 0, "ld_index must be a multiple of 8 and >= L");
@@ -794,12 +861,32 @@ int grb_hstu_bias_index(const int64_t* timestamps, const uint8_t* pad, const int
     dim3 grid((ld_index + 255) / 256, (L + 7) / 8, B);
     auto go = [&](cudaStream_t s_) -> int {
         GRB_LAUNCH(hstu_bias_index_kernel, grid, 256, 0, s_, reinterpret_cast<const long long*>(timestamps), pad,
-                   reinterpret_cast<const long long*>(time_thr), pos_bucket, L, ld_index, npos, ntime, out);
+                   reinterpret_cast<const long long*>(time_thr), pos_bucket, L, ld_index, npos, ntime, out,
+                   reinterpret_cast<const long long*>(offsets), T);
         return 0;
     };
     // the index matrix is first needed by the attention kernel of the first block: with the deferred schedule it is built beside
     // that block's cast + projection GEMM (grb_hstu_layer_forward joins before its attention launch)
-    return run_maybe_deferred(static_cast<cudaStream_t>(stream), go);
+    return run_maybe_deferred(st, go);
+}
+
+}  // namespace
+
+extern "C" {
+
+int grb_hstu_bias_index(const int64_t* timestamps, const uint8_t* pad, const int64_t* time_thr, const uint8_t* pos_bucket, int B, int L,
+                        int npos, int ntime, uint16_t* out, int ld_index, void* stream) {
+    return bias_index(timestamps, pad, nullptr, time_thr, pos_bucket, B, 0, L, npos, ntime, out, ld_index,   // T unused without offsets
+                      static_cast<cudaStream_t>(stream));
+}
+int grb_hstu_bias_index_jagged(const int64_t* timestamps, const uint8_t* pad, const int64_t* offsets, const int64_t* time_thr,
+                               const uint8_t* pos_bucket, int B, int T, int max_len, int npos, int ntime, uint16_t* out, int ld_index,
+                               void* stream) {
+    GRB_REQUIRE(offsets != nullptr, "offsets is null");
+    GRB_REQUIRE(T >= 1, "token rows T=%d must be positive", T);
+    GRB_REQUIRE(max_len <= 16384, "max_len %d exceeds 16384", max_len);
+    return bias_index(timestamps, pad, offsets, time_thr, pos_bucket, B, T, max_len, npos, ntime, out, ld_index,
+                      static_cast<cudaStream_t>(stream));
 }
 
 int grb_set_defer_weight_grads(int on) {
@@ -845,6 +932,21 @@ int grb_collate_jagged(const int64_t* items, const int64_t* stamps, const int64_
     GRB_LAUNCH(collate_jagged_kernel, (unsigned)((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream), reinterpret_cast<const long long*>(items),
                reinterpret_cast<const long long*>(stamps), reinterpret_cast<const long long*>(offsets), reinterpret_cast<const long long*>(targets), B, L,
                reinterpret_cast<long long*>(out_input_ids), reinterpret_cast<long long*>(out_targets), reinterpret_cast<long long*>(out_timestamps));
+    return 0;
+}
+
+int grb_pack_jagged(const int64_t* items, const int64_t* stamps, const int64_t* offsets, const int64_t* targets, int B, int max_seq_len,
+                    int T, int64_t* out_input_ids, int64_t* out_targets, int64_t* out_timestamps, int64_t* out_offsets, int64_t* info,
+                    void* stream) {
+    GRB_REQUIRE(items && offsets && targets && out_input_ids && out_targets && out_offsets && info, "null argument");
+    GRB_REQUIRE(B > 0 && max_seq_len > 0 && T > 0, "bad shape B=%d max_seq_len=%d T=%d", B, max_seq_len, T);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GRB_LAUNCH(pack_jagged_offsets_kernel, 1, 1024, 0, st, reinterpret_cast<const long long*>(offsets), B, max_seq_len, T,
+               reinterpret_cast<long long*>(out_offsets), reinterpret_cast<long long*>(info));
+    GRB_LAUNCH(pack_jagged_kernel, (unsigned)(((size_t)T + 255) / 256), 256, 0, st, reinterpret_cast<const long long*>(items),
+               reinterpret_cast<const long long*>(stamps), reinterpret_cast<const long long*>(offsets), reinterpret_cast<const long long*>(targets),
+               reinterpret_cast<const long long*>(out_offsets), B, T, reinterpret_cast<long long*>(out_input_ids),
+               reinterpret_cast<long long*>(out_targets), reinterpret_cast<long long*>(out_timestamps));
     return 0;
 }
 

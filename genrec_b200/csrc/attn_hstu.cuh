@@ -13,7 +13,8 @@
 // The per-element work is then: one 16-bit index load, one table load, one add, the SiLU.
 // The 10 MB index matrix (cfg-2) stays L2-resident and is shared by every head of every layer, forward and backward.
 //
-// Layout: Q/K/V/dO/O are row-major [T = B*L, ld] bf16 with head h at columns h*DH .. h*DH+DH-1.
+// Layout: Q/K/V/dO/O are row-major [T = B*L, ld] bf16 with head h at columns h*DH .. h*DH+DH-1; in a packed batch
+// (HstuAttnArgs::offsets) sequence b is rows offsets[b] .. offsets[b+1]-1 of T, with no pad rows between sequences.
 // One CTA = 4 warps = 64 query rows (fwd, dQ) or 64 key rows (dK/dV); the other operand streams through shared memory
 // in double-buffered 64-row tiles (cp.async).  Warps whose rows lie beyond L and 8-wide blocks above the causal diagonal
 // are skipped (warp-uniform branches).
@@ -60,7 +61,28 @@ struct HstuAttnArgs {
     float* dwpos;   // [npos, H]  accumulated
     float* dwtime;  // [ntime, H] accumulated
     float* dw_part; // [2H][B * key tiles][64] scratch for the ordered cross-CTA sum of dwpos / dwtime (det_finish_kernel)
+    // packed (jagged) batch: null -> sequence b is rows b*L .. b*L+L-1.  Otherwise sequence b is rows offsets[b] .. offsets[b+1]-1
+    // of T token rows, L is the longest length the grid covers, and each sequence is clamped to [0, T) and to L.
+    const long long* offsets;
+    int T;
 };
+
+// First row and length of sequence b.  A malformed device `offsets` yields wrong numbers but never a row outside [0, T).
+// The attention kernels take JAGGED as a template parameter, so that their padded instantiations keep the registers (and the
+// code) they had before packed batches existed.
+template <bool JAGGED = true>
+GRB_DEVINL void seq_span(const long long* offsets, int T, int L, int b, long long& tok0, int& len) {
+    if (!JAGGED || offsets == nullptr) {
+        tok0 = (long long)b * L;
+        len = L;
+        return;
+    }
+    long long lo = offsets[b], hi = offsets[b + 1];
+    lo = lo < 0 ? 0 : (lo > T ? T : lo);
+    hi = hi < lo ? lo : (hi > T ? T : hi);
+    tok0 = lo;
+    len = (int)(hi - lo < L ? hi - lo : L);
+}
 
 GRB_DEVINL int time_bucket_dev(long long dt, const long long* thr, int ntime) {
     long long d = dt < 0 ? -dt : dt;
@@ -72,17 +94,22 @@ GRB_DEVINL int time_bucket_dev(long long dt, const long long* thr, int ntime) {
 
 // out[b, i, j] = (j <= i && !pad[b, j]) ? pos_bucket[i - j] * 64 + bucket(|ts[b,i] - ts[b,j]|) : npos * 64
 // grid (ceil(ld / 256), ceil(L / 8), B), block 256 = 8 query rows x 32 threads ; a thread produces 8 neighbouring key
-// columns and writes them with one 16-byte store (ld % 8 == 0).
+// columns and writes them with one 16-byte store (ld % 8 == 0).  With `offsets` (a packed batch of T rows, L = the longest
+// length) sequence b starts at row offsets[b] and the row of out is the query token: out [T, ld] (seq_span).
 __global__ void __launch_bounds__(256) hstu_bias_index_kernel(const long long* __restrict__ ts, const uint8_t* __restrict__ pad,
                                                              const long long* __restrict__ thr_g, const uint8_t* __restrict__ pos_bucket,
-                                                             int L, int ld, int npos, int ntime, uint16_t* __restrict__ out) {
+                                                             int L, int ld, int npos, int ntime, uint16_t* __restrict__ out,
+                                                             const long long* __restrict__ offsets, int T) {
     pdl_wait();
     __shared__ long long thr[ATT_MAX_BUCKETS + 1];
     for (int i = threadIdx.x; i <= ATT_MAX_BUCKETS; i += 256) thr[i] = thr_g[i];
     __syncthreads();
     const int b = blockIdx.z, i = blockIdx.y * 8 + (threadIdx.x >> 5), j0 = (blockIdx.x * 32 + (threadIdx.x & 31)) * 8;
-    if (i >= L || j0 >= ld) return;
-    const size_t row = (size_t)b * L;
+    long long tok0;
+    int len;
+    seq_span(offsets, T, L, b, tok0, len);
+    if (i >= len || j0 >= ld) return;
+    const size_t row = (size_t)tok0;
     const unsigned masked = (unsigned)npos * 64u;
     const bool timed = ts != nullptr && ntime > 0;
     const long long ti = timed ? ts[row + i] : 0;
@@ -99,6 +126,23 @@ __global__ void __launch_bounds__(256) hstu_bias_index_kernel(const long long* _
     uint4 o;
     o.x = v[0] | (v[1] << 16); o.y = v[2] | (v[3] << 16); o.z = v[4] | (v[5] << 16); o.w = v[6] | (v[7] << 16);
     *reinterpret_cast<uint4*>(out + (row + i) * ld + j0) = o;
+}
+
+// Zero columns [0, ncols) (a multiple of 8) of the rows of a packed batch that lie in no sequence: [0, offsets[0]) and
+// [offsets[B], T), clamped to [0, T).  The attention kernels write only sequence rows; the idle rows of O (forward) and of
+// dQ | dK | dV (backward) must still hold finite zeros, because the GEMMs and column sums of the block run on all T rows.
+__global__ void __launch_bounds__(256) hstu_idle_rows_zero_kernel(const long long* __restrict__ offsets, int B, int T, bf16* __restrict__ base,
+                                                                 int ld, int ncols) {
+    pdl_wait();
+    long long lo = offsets[0], hi = offsets[B];
+    lo = lo < 0 ? 0 : (lo > T ? T : lo);
+    hi = hi < lo ? lo : (hi > T ? T : hi);
+    const int ch = ncols / 8;
+    const long long n = (lo + (T - hi)) * ch;
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (long long)gridDim.x * blockDim.x) {
+        const long long r = k / ch, row = r < lo ? r : hi + (r - lo);
+        *reinterpret_cast<uint4*>(base + row * ld + (k % ch) * 8) = make_uint4(0u, 0u, 0u, 0u);
+    }
 }
 
 template <int DH, int NFIXED = 2>
@@ -223,7 +267,7 @@ GRB_DEVINL void att_pack_p(uint32_t (&pf)[4][4], const float (&s)[8][4]) {
 
 // ============================================================================================ forward
 // fixed[0] = Q ; stream[buf] = {K, V}
-template <int DH>
+template <int DH, bool JAGGED>
 __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 5 : 3) hstu_attn_fwd_kernel(HstuAttnArgs a) {
     pdl_wait();
     extern __shared__ __align__(16) unsigned char att_smem_raw[];
@@ -231,8 +275,11 @@ __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 5 : 3) hstu_attn_fwd_k
     float* wcomb = reinterpret_cast<float*>(att_smem_raw + sizeof(AttSmem<DH, 1>));
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int L = a.L, q0 = qt * ATT_BLK;
-    const long long tok0 = (long long)b * L;
+    const int q0 = qt * ATT_BLK;
+    long long tok0;
+    int L;
+    seq_span<JAGGED>(a.offsets, a.T, a.L, b, tok0, L);
+    if (JAGGED && q0 >= L) return;   // query tile past the end of a packed sequence
     const unsigned sentinel = (unsigned)a.bias.npos * 64u;
 
     att_build_table(wcomb, a.bias, h, a.H, tid);
@@ -311,7 +358,7 @@ __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 5 : 3) hstu_attn_fwd_k
 
 // ============================================================================================ backward: dQ
 // fixed = {Q, dO} ; stream[buf] = {K, V}
-template <int DH>
+template <int DH, bool JAGGED>
 __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 4 : 2) hstu_attn_bwd_dq_kernel(HstuAttnArgs a) {
     pdl_wait();
     extern __shared__ __align__(16) unsigned char att_smem_raw[];
@@ -319,8 +366,11 @@ __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 4 : 2) hstu_attn_bwd_d
     float* wcomb = reinterpret_cast<float*>(att_smem_raw + sizeof(AttSmem<DH>));
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int L = a.L, q0 = qt * ATT_BLK;
-    const long long tok0 = (long long)b * L;
+    const int q0 = qt * ATT_BLK;
+    long long tok0;
+    int L;
+    seq_span<JAGGED>(a.offsets, a.T, a.L, b, tok0, L);
+    if (JAGGED && q0 >= L) return;   // query tile past the end of a packed sequence
     const unsigned sentinel = (unsigned)a.bias.npos * 64u;
 
     att_build_table(wcomb, a.bias, h, a.H, tid);
@@ -436,7 +486,7 @@ inline int att_time_bins(bool has_time, bool pos_uniform, int ntime) {
     return has_time && pos_uniform ? ATT_MAX_BUCKETS + 1 : ntime + 1;
 }
 // HAS_TIME / POS_UNI are compile-time so that the per-cell histogram code carries no branches
-template <int DH, bool HAS_TIME, bool POS_UNI>
+template <int DH, bool HAS_TIME, bool POS_UNI, bool JAGGED>
 __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 3 : 2) hstu_attn_bwd_dkdv_kernel(HstuAttnArgs a, int table_bytes) {
     pdl_wait();
     extern __shared__ __align__(16) unsigned char att_smem_raw[];
@@ -448,8 +498,10 @@ __global__ void __launch_bounds__(ATT_THREADS, DH == 32 ? 3 : 2) hstu_attn_bwd_d
     float* hist_p = hist_t + 4 * nt_bins * 32;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int kt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int L = a.L, k0 = kt * ATT_BLK;
-    const long long tok0 = (long long)b * L;
+    const int k0 = kt * ATT_BLK;
+    long long tok0;
+    int L;   // a key tile past the end of a packed sequence runs no query tile but still stores its (zero) table partials
+    seq_span<JAGGED>(a.offsets, a.T, a.L, b, tok0, L);
     constexpr bool has_time = HAS_TIME, pos_uniform = POS_UNI;
     const int nqt = (L + ATT_BLK - 1) / ATT_BLK;
     const unsigned sentinel = (unsigned)npos * 64u;

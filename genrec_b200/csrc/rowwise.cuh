@@ -1061,5 +1061,82 @@ __global__ void __launch_bounds__(256) collate_jagged_kernel(const long long* __
     if (out_ts != nullptr) out_ts[e] = (p < pad || stamps == nullptr) ? 0 : stamps[(hi - n) + (p - pad)];
 }
 
+// ------------------------------------------------------------------------------------------------ jagged -> packed batch
+// The rows of collate_jagged_kernel without their pads: sequence b keeps n_b = min(len_b, max_seq_len) rows (its LAST n_b events),
+// packed one after another from row 0.  out_off [B+1] = the running sum of n_b, clamped to T; info[0] = the unclamped total (> T:
+// the batch did not fit and its tail was cut), info[1] = the longest n_b.  One CTA.
+__global__ void __launch_bounds__(1024) pack_jagged_offsets_kernel(const long long* __restrict__ offsets, int B, int max_seq_len, int T,
+                                                                  long long* __restrict__ out_off, long long* __restrict__ info) {
+    pdl_wait();
+    __shared__ long long warp_sum[32];
+    __shared__ long long s_carry;
+    __shared__ int warp_max[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) { s_carry = 0; out_off[0] = 0; }
+    int mx = 0;
+    for (int base = 0; base < B; base += 1024) {
+        __syncthreads();                                   // s_carry of the previous chunk is visible, warp_sum free
+        const long long carry = s_carry;
+        const int b = base + threadIdx.x;
+        long long n = 0;
+        if (b < B) {
+            n = offsets[b + 1] - offsets[b];
+            n = n < 0 ? 0 : (n > max_seq_len ? max_seq_len : n);
+        }
+        mx = max(mx, (int)n);
+        long long v = n;                                   // inclusive scan: lanes, then warps
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const long long u = __shfl_up_sync(0xffffffffu, v, o);
+            if (lane >= o) v += u;
+        }
+        if (lane == 31) warp_sum[warp] = v;
+        __syncthreads();
+        long long before = 0;
+        for (int w = 0; w < warp; ++w) before += warp_sum[w];
+        const long long incl = carry + before + v;
+        if (b < B) out_off[b + 1] = incl < T ? incl : T;
+        __syncthreads();                                   // every thread has read s_carry and warp_sum
+        if (threadIdx.x == 1023) s_carry = incl;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (lane == 0) warp_max[warp] = mx;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int m = 0;
+        for (int w = 0; w < 32; ++w) m = max(m, warp_max[w]);
+        info[0] = s_carry;
+        info[1] = m;
+    }
+}
+// Row t < out_off[B] of sequence b (out_off[b] <= t < out_off[b+1]), p = t - out_off[b], n = its packed length:
+//   input_ids[t] = hist[p]    timestamps[t] = ts[p]    targets[t] = p + 1 < n ? hist[p + 1] : target_b
+// with hist / ts the last n events of user b; rows t >= out_off[B] are idle (id 0, target 0, timestamp 0).
+__global__ void __launch_bounds__(256) pack_jagged_kernel(const long long* __restrict__ items, const long long* __restrict__ stamps,
+                                                         const long long* __restrict__ offsets, const long long* __restrict__ targets,
+                                                         const long long* __restrict__ out_off, int B, int T, long long* __restrict__ out_ids,
+                                                         long long* __restrict__ out_tg, long long* __restrict__ out_ts) {
+    pdl_wait();
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= T) return;
+    long long id = 0, tg = 0, ts = 0;
+    if (t < out_off[B]) {
+        int lo = 0, hi = B - 1;                            // the first b with out_off[b + 1] > t
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (out_off[mid + 1] > t) hi = mid; else lo = mid + 1;
+        }
+        const long long p = t - out_off[lo], n = out_off[lo + 1] - out_off[lo];
+        const long long src = offsets[lo + 1] - n + p;
+        id = items[src];
+        tg = p + 1 < n ? items[src + 1] : targets[lo];
+        ts = stamps != nullptr ? stamps[src] : 0;
+    }
+    out_ids[t] = id;
+    out_tg[t] = tg;
+    if (out_ts != nullptr) out_ts[t] = ts;
+}
+
 
 }  // namespace grb

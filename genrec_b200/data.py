@@ -110,6 +110,51 @@ def collate_jagged(items: torch.Tensor, offsets: torch.Tensor, targets: torch.Te
     return out
 
 
+def pack_jagged(items: torch.Tensor, offsets: torch.Tensor, targets: torch.Tensor, max_seq_len: int = 50,
+                timestamps: "torch.Tensor | None" = None, num_tokens: "int | None" = None) -> Dict[str, torch.Tensor]:
+    """``collate_jagged`` without the pads, for ``HSTU.forward_jagged``: the same jagged batch on the device (items / timestamps [N]
+    int64 in time order, offsets [B+1], one held-out target per user) -> a packed batch.  Sequence b is hstu_collate_fn's row b
+    with its pads removed: the last min(len_b, max_seq_len) items, the targets shifted by one with the held-out item last.
+    Returns input_ids, targets (and timestamps) [T], offsets [B+1] (sequence b = rows offsets[b] .. offsets[b+1]-1), the host int
+    max_len and overflow (a 0-dim bool on the device).
+
+    Without ``num_tokens`` T is the packed total and max_len the longest packed length, read from the device in one
+    synchronisation.  With ``num_tokens`` T = num_tokens and max_len = max_seq_len, with no synchronisation (a captured step keeps
+    fixed shapes): rows past the packed total are idle (id 0, target 0, timestamp 0), and a batch that does not fit sets
+    ``overflow``, is cut at T and writes nothing past it - do not train on it."""
+    from . import _lib
+    from ._lib import check, ptr, require_cuda, stream_ptr
+    require_cuda(items, offsets, targets)
+    for t in (items, offsets, targets, timestamps):
+        if t is not None and t.dtype != torch.int64:
+            raise _lib.GrbError(f"genrec_b200 error -1: jagged batches are int64 (got {t.dtype})")
+    B = offsets.numel() - 1
+    if B < 1 or int(max_seq_len) < 1:
+        raise ValueError(f"pack_jagged needs B >= 1 and max_seq_len >= 1 (got {B}, {max_seq_len})")
+    if num_tokens is None:
+        lens = (offsets[1:] - offsets[:-1]).clamp(0, int(max_seq_len))
+        total, longest = torch.stack([lens.sum(), lens.max()]).tolist()
+        T, max_len = max(1, int(total)), max(1, int(longest))
+    else:
+        if int(num_tokens) < 1:
+            raise ValueError(f"num_tokens must be positive, got {num_tokens}")
+        T, max_len = int(num_tokens), int(max_seq_len)
+    dev = items.device
+    ids = torch.empty(T, dtype=torch.int64, device=dev)
+    tgs = torch.empty(T, dtype=torch.int64, device=dev)
+    tss = torch.empty(T, dtype=torch.int64, device=dev) if timestamps is not None else None
+    out_off = torch.empty(B + 1, dtype=torch.int64, device=dev)
+    info = torch.empty(2, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().grb_pack_jagged(ptr(items.contiguous()), ptr(timestamps.contiguous()) if timestamps is not None else None,
+                                          ptr(offsets.contiguous()), ptr(targets.contiguous()), B, int(max_seq_len), T, ptr(ids), ptr(tgs),
+                                          ptr(tss), ptr(out_off), ptr(info), stream_ptr(dev)))
+    out = {"input_ids": ids, "targets": tgs, "offsets": out_off, "max_len": max_len, "overflow": info[0] > T}
+    if tss is not None:
+        out["timestamps"] = tss
+    return out
+
+
 def sample_negatives(num_items: int, n: int, *, probs: Optional[torch.Tensor] = None, generator: Optional[torch.Generator] = None,
                      device=None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """The shared negatives of one sampled-softmax step: ``(negatives [n] int64 in 1..num_items, log_q [num_items + 1] fp32 | None)``,

@@ -79,15 +79,22 @@ _ZERO_TABLES = {}
 
 class SeqMeta:
     """Per-batch sequence metadata shared by all layers of one forward: the pad flags, the raw timestamps and the
-    [B, L, ld] uint16 bias-index matrix the attention kernels read."""
+    [B, L, ld] uint16 bias-index matrix the attention kernels read.  With ``offsets`` ([B+1] int64 on the device) and
+    ``max_len`` the batch is packed: pad_u8 / timestamps are [T] and the index matrix is [T, ld] (grb_hstu_bias_index_jagged)."""
 
     def __init__(self, pad_u8: torch.Tensor, timestamps: Optional[torch.Tensor], pos_bucket: Optional[torch.Tensor],
                  time_thr: torch.Tensor, num_time_buckets: int = 64, num_pos_buckets: int = 32, pos_uniform=None,
-                 may_defer: bool = True):
+                 may_defer: bool = True, offsets: Optional[torch.Tensor] = None, max_len: Optional[int] = None):
         # may_defer=False builds the index on the caller's stream even under the deferred schedule (the custom ops, whose
         # callers order and free everything by that stream); pos_bucket may be None when pos_uniform is given
-        require_cuda(pad_u8)
-        B, L = pad_u8.shape
+        require_cuda(pad_u8, offsets)
+        self.offsets = offsets
+        if offsets is None:
+            B, L = pad_u8.shape
+            self.T = B * L
+        else:
+            B, L = offsets.numel() - 1, int(max_len)
+            self.T = pad_u8.numel()
         self.B, self.L = B, L
         self.pad = pad_u8.contiguous()
         if self.pad.dtype != torch.uint8:
@@ -107,7 +114,8 @@ class SeqMeta:
 
     def _build_bias_index(self, may_defer: bool):
         B, L, dev = self.B, self.L, self.pad.device
-        self.bias_index = torch.empty(B, L, self.ld, dtype=torch.int16, device=dev)
+        rows = (B, L) if self.offsets is None else (self.T,)
+        self.bias_index = torch.empty(*rows, self.ld, dtype=torch.int16, device=dev)
         nt = self.num_time_buckets if self.timestamps is not None else 0
         if self.pos_uniform:      # collapse to one effective position bucket (see grb_hstu_seq.pos_uniform)
             key = (L, str(dev))
@@ -119,8 +127,13 @@ class SeqMeta:
         # deferred schedule: built on the side stream, joined before the first attention launch
         _defer_for_call(_DEFER["on"] and may_defer)
         with torch.cuda.device(dev):
-            check(_lib.load().grb_hstu_bias_index(ptr(self.timestamps), ptr(self.pad), ptr(self.time_thr), ptr(pb_arg), B, L,
-                                                  npos_arg, nt, ptr(self.bias_index), self.ld, stream_ptr(dev)))
+            if self.offsets is None:
+                check(_lib.load().grb_hstu_bias_index(ptr(self.timestamps), ptr(self.pad), ptr(self.time_thr), ptr(pb_arg), B, L,
+                                                      npos_arg, nt, ptr(self.bias_index), self.ld, stream_ptr(dev)))
+            else:
+                check(_lib.load().grb_hstu_bias_index_jagged(ptr(self.timestamps), ptr(self.pad), ptr(self.offsets), ptr(self.time_thr),
+                                                             ptr(pb_arg), B, self.T, L, npos_arg, nt, ptr(self.bias_index), self.ld,
+                                                             stream_ptr(dev)))
 
     def struct(self) -> HstuSeq:
         return HstuSeq(ptr(self.bias_index), self.ld, 1 if self.timestamps is not None else 0, 1 if self.pos_uniform else 0,
@@ -150,13 +163,24 @@ def layer_saved_bytes(dims: HstuDims) -> int:
 
 
 def hstu_block_forward(dims: HstuDims, params, bf16w: dict, has_time: bool, meta: SeqMeta, x: torch.Tensor):
-    """One HSTU block (grb_hstu_layer_forward): x [B, L, D] fp32 contiguous -> (y, saved-for-backward blob)."""
-    saved = _u8(layer_saved_bytes(dims), x.device)
+    """One HSTU block (grb_hstu_layer_forward): x [B, L, D] fp32 contiguous -> (y, saved-for-backward blob).  A packed ``meta``
+    (offsets set) takes x [T, D] and runs grb_hstu_layer_forward_jagged."""
+    lib = _lib.load()
+    if meta.offsets is None:
+        nbytes = layer_saved_bytes(dims)
+    else:
+        nbytes = lib.grb_hstu_layer_saved_bytes_jagged(C.byref(dims), meta.T)
+        if nbytes == 0:
+            raise _lib.GrbError(lib.grb_last_error().decode())
+    saved = _u8(nbytes, x.device)
     y = torch.empty_like(x)
     pstruct, seq = _layer_param_struct(params, bf16w, has_time), meta.struct()
     with torch.cuda.device(x.device):
-        check(_lib.load().grb_hstu_layer_forward(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(x), ptr(y), ptr(saved),
-                                                 stream_ptr(x.device)))
+        if meta.offsets is None:
+            check(lib.grb_hstu_layer_forward(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(x), ptr(y), ptr(saved), stream_ptr(x.device)))
+        else:
+            check(lib.grb_hstu_layer_forward_jagged(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(meta.offsets), meta.T, ptr(x), ptr(y),
+                                                    ptr(saved), stream_ptr(x.device)))
     return y, saved
 
 
@@ -173,24 +197,35 @@ def hstu_block_backward(dims: HstuDims, params, bf16w: dict, has_time: bool, met
     pstruct, gstruct, seq = _layer_param_struct(params, bf16w, has_time), HstuLayerGrads(*[ptr(g) for g in grads]), meta.struct()
     dyc = dy.contiguous().float()
     dx = torch.empty_like(dyc)
-    ws = _u8(lib.grb_hstu_layer_workspace_bytes(C.byref(dims)), dy.device)
+    if meta.offsets is None:
+        ws = _u8(lib.grb_hstu_layer_workspace_bytes(C.byref(dims)), dy.device)
+    else:
+        ws = _u8(lib.grb_hstu_layer_workspace_bytes_jagged(C.byref(dims), meta.T), dy.device)
     deferred = _defer_for_call(_DEFER["on"] and sink is not None)
     with torch.cuda.device(dy.device):
-        check(lib.grb_hstu_layer_backward(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(dyc), ptr(saved), ptr(dx), C.byref(gstruct),
-                                          ptr(ws), stream_ptr(dy.device)))
+        if meta.offsets is None:
+            check(lib.grb_hstu_layer_backward(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(dyc), ptr(saved), ptr(dx), C.byref(gstruct),
+                                              ptr(ws), stream_ptr(dy.device)))
+        else:
+            check(lib.grb_hstu_layer_backward_jagged(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(meta.offsets), meta.T, ptr(dyc),
+                                                     ptr(saved), ptr(dx), C.byref(gstruct), ptr(ws), stream_ptr(dy.device)))
     if deferred:
         _DEFER["keep"].append((ws, saved, dyc))     # still read by the deferred dW GEMM
     return dx, grads
 
 
 class HstuLayerFn(torch.autograd.Function):
-    """One HSTU block.  forward = grb_hstu_layer_forward, backward = grb_hstu_layer_backward."""
+    """One HSTU block.  forward = grb_hstu_layer_forward, backward = grb_hstu_layer_backward; on a packed ``meta`` (x [T, D]) their
+    _jagged forms, with B = the sequence count and L = max_len."""
 
     @staticmethod
     def forward(ctx, x, meta: SeqMeta, cfg: dict, bf16w: dict, *params):
         # params in PARAM_ORDER (fp32 masters; time_table may be None)
         require_cuda(x)
-        B, L, D = x.shape
+        if meta.offsets is None:
+            B, L, D = x.shape
+        else:
+            B, L, D = meta.B, meta.L, x.shape[-1]
         require_f32(*[q for q in params if q is not None])
         has_time = params[PARAM_ORDER.index("time_table")] is not None and meta.timestamps is not None
         dims = _dims(B, L, D, cfg["H"], cfg["npos"], cfg["ntime"] if has_time else 0, cfg["p"], cfg["seed"], cfg["seed_dev"],

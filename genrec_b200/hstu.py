@@ -212,6 +212,14 @@ class HSTULayer(nn.Module):
                           self.temporal_bias.num_buckets if self.use_temporal_bias else 0, self.position_bias.num_buckets,
                           self.position_bias.uniform_of(L, device))
 
+    def _seq_meta_jagged(self, pad_u8: torch.Tensor, timestamps: Optional[torch.Tensor], offsets: torch.Tensor, max_len: int,
+                         device) -> Fn.SeqMeta:
+        """``_seq_meta`` of a packed batch: pad_u8 / timestamps [T], offsets [B+1] on the device, the index matrix [T, ld]."""
+        ts = timestamps.contiguous() if (timestamps is not None and self.use_temporal_bias) else None
+        return Fn.SeqMeta(pad_u8, ts, self.position_bias.bucket_of_delta(max_len, device), _thresholds_on(device),
+                          self.temporal_bias.num_buckets if self.use_temporal_bias else 0, self.position_bias.num_buckets,
+                          self.position_bias.uniform_of(max_len, device), offsets=offsets, max_len=max_len)
+
     def _params(self):
         tb = self.temporal_bias.temporal_attention_bias.weight if self.use_temporal_bias else None
         return (self.projection.weight, self.projection.bias, self.position_bias.relative_attention_bias.weight, tb,
@@ -490,6 +498,11 @@ class HSTU(nn.Module):
             if targets is not None:
                 raise RuntimeError("genrec_b200: precision='fp32' computes logits only (no loss / training)")
             return self._head_logits_f32(x), None
+        return self._head(x, targets, negatives, log_q)
+
+    def _head(self, x: torch.Tensor, targets: Optional[torch.Tensor], negatives: Optional[torch.Tensor], log_q: Optional[torch.Tensor]
+              ) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """The bf16 head of ``forward`` on x [B, L, D]: (logits [B, L, V+1] | None, loss | None) under forward's rules."""
         table = self.item_embedding.weight
         table_bf16 = self._table_mirror()
         loss = None
@@ -512,6 +525,104 @@ class HSTU(nn.Module):
         if targets is None or not self.training or self.return_train_logits:
             logits = Fn.head_logits(x, self.final_norm.weight, self.final_norm.bias, table, table_bf16, self.final_norm.eps)
         return logits, loss
+
+    def _check_jagged(self, what: str, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int,
+                      timestamps: Optional[torch.Tensor]) -> torch.Tensor:
+        """Argument check of a packed batch (before any launch) -> offsets on the model's device.  CPU offsets are refused with
+        ValueError unless offsets[0] == 0, they never decrease, no length exceeds max_len and offsets[B] <= T; device offsets are
+        not read on the host (CUDA graphs), and the kernels keep a malformed one inside the T rows."""
+        if self.precision == "fp32":
+            raise RuntimeError(f"genrec_b200: {what} runs the bf16 path only; set_precision('bf16')")
+        if input_ids.dim() != 1 or input_ids.numel() == 0 or input_ids.dtype != torch.int64:
+            raise ValueError(f"{what}: input_ids must be a non-empty [T] int64 tensor, got {tuple(input_ids.shape)} {input_ids.dtype}")
+        T = input_ids.numel()
+        if not isinstance(offsets, torch.Tensor) or offsets.dim() != 1 or offsets.numel() < 2 or offsets.dtype != torch.int64:
+            raise ValueError(f"{what}: offsets must be a [B+1] int64 tensor with B >= 1")
+        if isinstance(max_len, bool) or not isinstance(max_len, int) or not 1 <= max_len <= 16384:
+            raise ValueError(f"{what}: max_len must be an int in [1, 16384], got {max_len!r}")
+        if timestamps is not None and tuple(timestamps.shape) != (T,):
+            raise ValueError(f"{what}: timestamps must be [{T}] like input_ids, got {tuple(timestamps.shape)}")
+        if not offsets.is_cuda:
+            o = offsets
+            if int(o[0]) != 0:
+                raise ValueError(f"{what}: offsets[0] must be 0, got {int(o[0])}")
+            lens = o[1:] - o[:-1]
+            if bool((lens < 0).any()):
+                raise ValueError(f"{what}: offsets must be non-decreasing")
+            if int(lens.max()) > max_len:
+                raise ValueError(f"{what}: a sequence of length {int(lens.max())} exceeds max_len {max_len}")
+            if int(o[-1]) > T:
+                raise ValueError(f"{what}: offsets[B] = {int(o[-1])} exceeds the {T} token rows")
+        elif offsets.device != input_ids.device:
+            raise ValueError(f"{what}: offsets must be on the CPU or on {input_ids.device}, got {offsets.device}")
+        require_cuda(input_ids)
+        ensure_device(input_ids.device)
+        return offsets.to(input_ids.device)
+
+    def encode_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, timestamps: Optional[torch.Tensor] = None
+                      ) -> torch.Tensor:
+        """``encode`` of a packed batch: input_ids / timestamps [T], offsets [B+1] int64 on the device (sequence b = rows
+        offsets[b] .. offsets[b+1]-1), max_len >= every length -> [T, D] fp32.  No pads are computed: the blocks run on T rows."""
+        T = input_ids.numel()
+        seed, seed_dev = self._seeds(input_ids.device)
+        p = self.emb_dropout.p if self.training else 0.0
+        esink = None
+        if self._grad_sink is not None and torch.is_grad_enabled():
+            esink = (self._grad_sink(self.item_embedding.weight), None)
+        # HSTU has no position table, so the embedding of a packed batch is that of one [1, T] row
+        x, pad = Fn.EmbedFn.apply(input_ids.view(1, T), self.item_embedding.weight, None, 1.0, 0, p, seed, seed_dev, esink)
+        if self._marks_rows():
+            self._row_marker._mark(input_ids)
+        x = x.view(T, self.embed_dim)
+        if len(self.layers):
+            meta = self.layers[0]._seq_meta_jagged(pad.view(T), timestamps, offsets, max_len, input_ids.device)
+            for layer in self.layers:
+                layer._bf16_provider = self._bf16_provider
+                x = layer(x, None, None, timestamps, _meta=meta, _seed=seed, _seed_dev=seed_dev)
+        return x
+
+    def forward_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, timestamps: Optional[torch.Tensor] = None,
+                       targets: Optional[torch.Tensor] = None, *, negatives: Optional[torch.Tensor] = None,
+                       log_q: Optional[torch.Tensor] = None) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """``forward`` on a packed batch (``data.pack_jagged``): input_ids / timestamps / targets [T] int64, offsets [B+1] int64
+        (sequence b = rows offsets[b] .. offsets[b+1]-1; rows from offsets[B] to T are idle, id 0 and target 0), max_len >= every
+        length (<= 16384).  Returns (logits [T, V+1] fp32 | None, loss | None) under ``forward``'s rules (dropout, sampled head,
+        FlatAdam's gradient sinks, unit_loss_grad, lazy_table row marks).  Every stage runs on the T rows, none on padding.
+
+        HSTU has no absolute position embedding, so each token computes what it computes in the left-padded batch of the same users;
+        only dropout differs: its masks are keyed by token row, so a packed batch draws other masks than the padded one.  With
+        offsets on the CPU the batch is checked before any launch (ValueError); offsets on the device are not read on the host, so a
+        step with fixed (B, T, max_len) can be captured in a CUDA graph and replayed with new offsets, ids and targets.  bf16 only."""
+        if negatives is None and log_q is not None:
+            raise ValueError("log_q corrects the sampled softmax: pass negatives with it")
+        if negatives is not None and targets is None:
+            raise ValueError("negatives select the sampled-softmax loss, which needs targets")
+        T = input_ids.numel()
+        if targets is not None and tuple(targets.shape) != (T,):
+            raise ValueError(f"forward_jagged: targets must be [{T}] like input_ids, got {tuple(targets.shape)}")
+        offsets = self._check_jagged("forward_jagged", input_ids, offsets, max_len, timestamps)
+        x = self.encode_jagged(input_ids, offsets, max_len, timestamps)
+        logits, loss = self._head(x.view(1, T, self.embed_dim), targets, negatives, log_q)
+        return (logits.view(T, -1) if logits is not None else None), loss
+
+    @torch.no_grad()
+    def evaluate_batch_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, timestamps: Optional[torch.Tensor],
+                              targets: torch.Tensor, metrics: Optional[torch.Tensor] = None, *, exclude: Optional[torch.Tensor] = None,
+                              want_ranks: bool = False):
+        """``evaluate_batch`` on a packed batch (input_ids / timestamps [T], offsets [B+1], max_len as in ``forward_jagged``; targets
+        [B] the held-out item of each sequence): each sequence is ranked from its last row, offsets[b+1] - 1, and the metrics are
+        accumulated into ``metrics`` on the device.  A sequence of length 0 is not ranked (rank 0, adds nothing).  With
+        ``want_ranks`` it returns (metrics, ranks [B] int32)."""
+        B, T = offsets.numel() - 1, input_ids.numel()
+        if tuple(targets.shape) != (B,):
+            raise ValueError(f"evaluate_batch_jagged: targets must be [{B}] (one per sequence), got {tuple(targets.shape)}")
+        offsets = self._check_jagged("evaluate_batch_jagged", input_ids, offsets, max_len, timestamps)
+        Fn.check_exclude_arg(exclude, B, input_ids.device)
+        x = self.encode_jagged(input_ids, offsets, max_len, timestamps)
+        last = (offsets[1:] - 1).clamp(0, T - 1)
+        ranked = torch.where(offsets[1:] > offsets[:-1], targets, torch.zeros_like(targets))
+        return Fn.head_rank_metrics(x.index_select(0, last), self.final_norm.weight, self.final_norm.bias, self._table_mirror(),
+                                    self.final_norm.eps, ranked, metrics, exclude, want_ranks)
 
     @torch.no_grad()
     def last_logits(self, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor] = None) -> torch.Tensor:

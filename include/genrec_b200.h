@@ -117,6 +117,29 @@ int grb_hstu_layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params*
                             const float* dy, const void* saved, float* dx, const grb_hstu_layer_grads* g,
                             void* workspace, void* stream);
 
+/* ------------------------------------------------------------------------------------------------ packed (jagged) HSTU batches
+ * A packed batch holds B sequences without padding: token rows [T, D], offsets [B+1] int64 on the DEVICE (sequence b is rows
+ * offsets[b] .. offsets[b+1]-1), a host max_len >= every length (<= 16384) and a host T >= offsets[B]; rows offsets[B] .. T-1 are
+ * idle (id 0, target 0).  Nothing reads the lengths on the host, so a step with fixed (B, T, max_len) can be captured in a CUDA
+ * graph and replayed with new offsets and ids.  HSTU has no absolute position embedding, so every real token computes what it
+ * computes in the left-padded batch of the same users.  A malformed device offsets gives wrong numbers, never an access outside
+ * the T rows: each sequence is clamped to [0, T) and to max_len.
+ *   grb_hstu_bias_index_jagged: out [T, ld_index] (ld_index >= max_len, a multiple of 8): row = the query token, column = the key's
+ *       position in that token's sequence, cells as grb_hstu_bias_index.  timestamps (nullable) / pad [T].
+ *   grb_hstu_layer_*_jagged: grb_hstu_layer_* on the packed rows, with d->B = the sequence count and d->L = max_len; x, y, dy, dx are
+ *       [T, D] and s->bias_index comes from grb_hstu_bias_index_jagged.  Dropout masks are keyed by token row, so under dropout a
+ *       packed batch draws different masks than the padded batch of the same users. */
+int grb_hstu_bias_index_jagged(const int64_t* timestamps, const uint8_t* pad, const int64_t* offsets, const int64_t* time_thr,
+                               const uint8_t* pos_bucket, int B, int T, int max_len, int npos, int ntime, uint16_t* out, int ld_index,
+                               void* stream);
+size_t grb_hstu_layer_saved_bytes_jagged(const grb_hstu_dims* d, int T);
+size_t grb_hstu_layer_workspace_bytes_jagged(const grb_hstu_dims* d, int T);
+int grb_hstu_layer_forward_jagged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const int64_t* offsets,
+                                  int T, const float* x, float* y, void* saved, void* stream);
+int grb_hstu_layer_backward_jagged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_seq* s, const int64_t* offsets,
+                                   int T, const float* dy, const void* saved, float* dx, const grb_hstu_layer_grads* g, void* workspace,
+                                   void* stream);
+
 /* ------------------------------------------------------------------------------------------------ cached incremental inference
  * Extends `predict` / evaluation (hstu.py:150-157, trainers/hstu_trainer.py:55-81), which rerun the whole history for every new
  * item: a cache keeps, per layer, the K | V rows of every item seen so far for a batch of B users, and a chunk of n new slots per
@@ -192,6 +215,14 @@ int grb_hstu_layer_extend_paged(const grb_hstu_dims* d, const grb_hstu_layer_par
  * is chosen by the caller, who knows the lengths when it forms the batch.  stamps / out_timestamps may be NULL. */
 int grb_collate_jagged(const int64_t* items, const int64_t* stamps, const int64_t* offsets, const int64_t* targets, int B, int L,
                        int64_t* out_input_ids, int64_t* out_targets, int64_t* out_timestamps, void* stream);
+/* The same batch packed instead of padded: each sequence is collate's row without its pads (the last min(len, max_seq_len) events,
+ * targets shifted by one, the held-out target last), sequences back to back from row 0, into T rows.  out_offsets [B+1] = the running
+ * sum of the packed lengths, clamped to T; rows past out_offsets[B] are idle (id 0, target 0, timestamp 0).  info [2] int64:
+ * info[0] = the packed total (> T: the batch did not fit, its tail was cut and nothing was written past T), info[1] = the longest
+ * packed length.  No host synchronisation. */
+int grb_pack_jagged(const int64_t* items, const int64_t* stamps, const int64_t* offsets, const int64_t* targets, int B, int max_seq_len,
+                    int T, int64_t* out_input_ids, int64_t* out_targets, int64_t* out_timestamps, int64_t* out_offsets, int64_t* info,
+                    void* stream);
 
 /* ------------------------------------------------------------------------------------------------ embedding gather
  * Replaces item_embedding + emb_dropout (hstu.py:124-128) / the scaled item+position embedding of SASRec
