@@ -528,7 +528,8 @@ class HSTU(nn.Module):
 
     def _check_jagged(self, what: str, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int,
                       timestamps: Optional[torch.Tensor]) -> torch.Tensor:
-        """Argument check of a packed batch (before any launch) -> offsets on the model's device.  CPU offsets are refused with
+        """Argument check of a packed batch (before any launch) -> offsets on the model's device.  More than 65535 sequences are
+        refused with ValueError wherever the offsets live.  CPU offsets are refused with
         ValueError unless offsets[0] == 0, they never decrease, no length exceeds max_len and offsets[B] <= T; device offsets are
         not read on the host (CUDA graphs), and the kernels keep a malformed one inside the T rows."""
         if self.precision == "fp32":
@@ -538,6 +539,8 @@ class HSTU(nn.Module):
         T = input_ids.numel()
         if not isinstance(offsets, torch.Tensor) or offsets.dim() != 1 or offsets.numel() < 2 or offsets.dtype != torch.int64:
             raise ValueError(f"{what}: offsets must be a [B+1] int64 tensor with B >= 1")
+        if offsets.numel() - 1 > 65535:
+            raise ValueError(f"{what}: B = {offsets.numel() - 1} sequences exceeds 65535 (the attention grid's z dimension)")
         if isinstance(max_len, bool) or not isinstance(max_len, int) or not 1 <= max_len <= 16384:
             raise ValueError(f"{what}: max_len must be an int in [1, 16384], got {max_len!r}")
         if timestamps is not None and tuple(timestamps.shape) != (T,):

@@ -177,6 +177,59 @@ def linear_dact_backward(dyb, w, z, p=0.0, seed=0, site_=0):
     return {"g": g, "a_g": a}
 
 
+# ------------------------------------------------------------------------------------------------ the row-wise stages of one block
+def block_stage_items(r, seq=None):
+    """Every stage of one block but the attention, each on the kernel's own inputs to it: projection, gate forward and backward, FFN,
+    the cast of dy with its column sums, projection backward.  r: the inputs, intermediates and gradients of one forward + backward
+    (x, y, dy, dx, grads, prm, p, layer, seed = the effective dropout seed, and the saved / workspace regions by name).  Asserts the
+    bit-for-bit stages and the drop masks (x1 - x == 0 where the gate drops, hact == 0 where drop_hid drops).
+
+    seq: None, or a bool [T] that is False on the idle rows of a packed batch (dy == 0 there).  The reference then takes the
+    backward's intermediates dxn, dx1, dz1 and dzp as zero on the idle rows: the gradients of those rows are held to 0 and the column
+    sums and weight gradients are the sums over the sequence rows alone.  -> [(name, got, ref, allowance)]"""
+    p, layer, seed = r["p"], r["layer"], r["seed"]
+    prm, gr, D = r["prm"], r["grads"], r["x"].shape[1]
+    s_gate, s_hid, s_out = (site(layer, w) for w in (SITE_GATE, SITE_FFN_HID, SITE_FFN_OUT))
+    live = (lambda t: t) if seq is None else (lambda t: torch.where(seq[:, None], t, torch.zeros((), dtype=t.dtype, device=t.device)))
+    for n in ("xb", "zp", "P", "O", "st1", "x1", "xn", "st2", "z1", "hact", "dyb", "dz1", "dxn", "dx1", "dO", "dzp"):
+        assert bool(torch.isfinite(r[n].float()).all()), f"{n} has an unwritten or non-finite element"
+    assert torch.equal(r["xb"], r["x"].bfloat16()), "xb != RNE(x)"
+    pj = linear_forward(r["xb"], prm["proj_w"], prm["proj_b"], 1, r["zp"])
+    items = [("zp", r["zp"], pj["z"], pj["a_z"]), ("P", r["P"], pj["a"], pj["a_a"])]
+    # gate forward
+    Uc = r["P"][:, :D]
+    gf = gate_forward(r["O"], Uc, r["x"], r["x1"], prm["ln1_g"], prm["ln1_b"], prm["ln2_g"], prm["ln2_b"], p, seed, s_gate)
+    assert not bool((r["x1"] - r["x"])[gf["drop"]].any()), "x1 - x != 0 where the gate drops"
+    items += [("x1", r["x1"], gf["x1"], gf["a_x1"]), ("xn", r["xn"], gf["xn"], gf["a_xn"]),
+              ("st1 mean", r["st1"][:, 0], gf["mean1"], gf["a_mean1"]), ("st1 rstd", r["st1"][:, 1], gf["rstd1"], gf["a_rstd1"]),
+              ("st2 mean", r["st2"][:, 0], gf["mean2"], gf["a_mean2"]), ("st2 rstd", r["st2"][:, 1], gf["rstd2"], gf["a_rstd2"])]
+    # FFN forward
+    f1 = linear_forward(r["xn"], prm["ffn1_w"], prm["ffn1_b"], 1, r["z1"], p, seed, s_hid)
+    assert not bool(r["hact"][f1["a"] == 0].any()), "hact != 0 where drop_hid drops"
+    f2 = linear_residual(r["hact"], prm["ffn2_w"], prm["ffn2_b"], r["x1"], None, p, seed, s_out)
+    items += [("z1", r["z1"], f1["z"], f1["a_z"]), ("hact", r["hact"], f1["a"], f1["a_a"]), ("y", r["y"], f2["y"], f2["a_y"])]
+    # backward: cast of dy, FFN, gate
+    cc = cast_colsum(r["dy"], p, seed, s_out)
+    assert torch.equal(r["dyb"], cc["dyb_exact"]), "dyb != RNE(fp32(dy keep))"
+    if p in (0.0, 0.5):
+        assert torch.equal(gr["ffn2_b"].double(), cc["db"]), "db2 is not the exact column sum of dyb"
+    items.append(("dffn2_b", gr["ffn2_b"], cc["db"], cc["a_db"]))
+    dz = linear_dact_backward(r["dyb"], prm["ffn2_w"], r["z1"], p, seed, s_hid)
+    b1 = linear_backward(live(r["dz1"]), prm["ffn1_w"], r["xn"])
+    b2 = linear_backward(r["dyb"], prm["ffn2_w"], r["hact"])
+    items += [("dz1", r["dz1"], dz["g"], dz["a_g"]), ("dxn", r["dxn"], b1["dx"], b1["a_dx"]), ("dW1", gr["ffn1_w"], b1["dw"], b1["a_dw"]),
+              ("dffn1_b", gr["ffn1_b"], b1["db"], b1["a_db"]), ("dW2", gr["ffn2_w"], b2["dw"], b2["a_dw"])]
+    gb = gate_backward(r["dy"], live(r["dxn"]), r["x1"], r["st1"], r["st2"], r["O"], Uc, r["zp"][:, :D], live(r["dx1"]), prm["ln1_g"],
+                       prm["ln1_b"], prm["ln2_g"], p, seed, s_gate)
+    items += [("dx1", r["dx1"], gb["dx1"], gb["a_dx1"]), ("dzu", r["dzp"][:, :D], gb["dzu"], gb["a_dzu"]), ("dO", r["dO"], gb["dO"], gb["a_dO"]),
+              ("dln1_g", gr["ln1_g"], gb["dg1"], gb["a_dg1"]), ("dln1_b", gr["ln1_b"], gb["db1"], gb["a_db1"]),
+              ("dln2_g", gr["ln2_g"], gb["dg2"], gb["a_dg2"]), ("dln2_b", gr["ln2_b"], gb["db2"], gb["a_db2"])]
+    # projection backward
+    bp = linear_backward(live(r["dzp"]), prm["proj_w"], r["xb"], res=live(r["dx1"]))
+    items += [("dx", r["dx"], bp["dx"], bp["a_dx"]), ("dWp", gr["proj_w"], bp["dw"], bp["a_dw"]), ("dproj_b", gr["proj_b"], bp["db"], bp["a_db"])]
+    return items
+
+
 # ------------------------------------------------------------------------------------------------ attention
 def cell_bias(bias_index, wpos, wtime, npos_index, H):
     """Decode the [B, L, ld] index matrix the attention kernels read (pb * 64 + tb, sentinel npos_index * 64) into the fp32 table sum

@@ -59,6 +59,30 @@ def _oracle_run(ids, ts, tg, sd, autocast):
     return float(lo), grads, grabbed["x_last"].grad.float()
 
 
+def autocast_yardstick(rows, small):
+    """rows: (name, ours Frobenius, reference-autocast Frobenius, ours max-norm, reference-autocast max-norm) relative errors against
+    the fp32 oracle; small: the names of tensors of < 4096 elements.  Prints the table (pytest -s) and asserts the yardstick."""
+    lines = ["| tensor | ours, Frobenius | reference autocast, Frobenius | ratio | ours, max-norm | reference autocast, max-norm | ratio |",
+             "|---|---|---|---|---|---|---|"]
+    lines += [f"| {n} | {a:.2e} | {b:.2e} | {a / max(b, 1e-12):.2f} | {c:.2e} | {d:.2e} | {c / max(d, 1e-12):.2f} |" for n, a, b, c, d in rows]
+    print("\n".join(lines))
+    # Yardstick.  Both columns are one realisation of bf16 rounding noise, so the ratio of the two scatters from tensor to tensor
+    # (and, for ours, from build to build: +-10 % on the matrices, a factor ~2 on a 399-entry bias table whose every entry is a
+    # cancelling sum of ~10^5 noisy terms).
+    #   weight matrices / embedding table / dX (>= 4096 elements): Frobenius error <= 1.1 x the reference algorithm's own
+    #       bf16-autocast error, and the geometric mean of the ratio over all of them <= 1.0;
+    #   vectors of < 4096 elements (bias tables, norm parameters): <= 3 x each, geometric mean <= 1.25;
+    #   the max-norm (one worst element out of up to 1.5 M) is reported and held within 3 x.
+    import math
+    big_r = [a / b for n, a, b, c, d in rows if n not in small and n != "loss" and b > 0]
+    small_r = [a / b for n, a, b, c, d in rows if n in small and b > 0]
+    gm = lambda v: math.exp(sum(math.log(max(x, 1e-6)) for x in v) / max(len(v), 1))
+    print(f"geometric mean of ours / reference-autocast: matrices {gm(big_r):.3f} ({len(big_r)}), small vectors {gm(small_r):.3f} ({len(small_r)})")
+    bad = [(n, a, b, c, d) for n, a, b, c, d in rows if a > (3.0 if n in small else 1.1) * b + 5e-4 or c > 3.0 * d + 1e-3]
+    assert not bad, bad
+    assert gm(big_r) <= 1.0 and gm(small_r) <= 1.25, (gm(big_r), gm(small_r))
+
+
 def test_cfg2_full_model_vs_oracle():
     """Headline configuration, whole model: loss, the gradient entering the last block, the tied embedding-table gradient (through
     the fused V=12,101 CE head with its 95 class tiles and half-block items) and every other parameter gradient, against the fp32
@@ -102,25 +126,7 @@ def test_cfg2_full_model_vs_oracle():
         rows.append((n + ".grad", frob_relerr(g, ref), frob_relerr(gac[n], ref), relerr(g, ref), relerr(gac[n], ref)))
         if ref.numel() < 4096:
             small.add(n + ".grad")
-    lines = ["| tensor | ours, Frobenius | reference autocast, Frobenius | ratio | ours, max-norm | reference autocast, max-norm | ratio |",
-             "|---|---|---|---|---|---|---|"]
-    lines += [f"| {n} | {a:.2e} | {b:.2e} | {a / max(b, 1e-12):.2f} | {c:.2e} | {d:.2e} | {c / max(d, 1e-12):.2f} |" for n, a, b, c, d in rows]
-    print("\n".join(lines))
-    # Yardstick.  Both columns are one realisation of bf16 rounding noise, so the ratio of the two scatters from tensor to tensor
-    # (and, for ours, from build to build: +-10 % on the matrices, a factor ~2 on a 399-entry bias table whose every entry is a
-    # cancelling sum of ~10^5 noisy terms).
-    #   weight matrices / embedding table / dX (>= 4096 elements): Frobenius error <= 1.1 x the reference algorithm's own
-    #       bf16-autocast error, and the geometric mean of the ratio over all of them <= 1.0;
-    #   vectors of < 4096 elements (bias tables, norm parameters): <= 3 x each, geometric mean <= 1.25;
-    #   the max-norm (one worst element out of up to 1.5 M) is reported and held within 3 x.
-    import math
-    big_r = [a / b for n, a, b, c, d in rows if n not in small and n != "loss" and b > 0]
-    small_r = [a / b for n, a, b, c, d in rows if n in small and b > 0]
-    gm = lambda v: math.exp(sum(math.log(max(x, 1e-6)) for x in v) / max(len(v), 1))
-    print(f"geometric mean of ours / reference-autocast: matrices {gm(big_r):.3f} ({len(big_r)}), small vectors {gm(small_r):.3f} ({len(small_r)})")
-    bad = [(n, a, b, c, d) for n, a, b, c, d in rows if a > (3.0 if n in small else 1.1) * b + 5e-4 or c > 3.0 * d + 1e-3]
-    assert not bad, bad
-    assert gm(big_r) <= 1.0 and gm(small_r) <= 1.25, (gm(big_r), gm(small_r))
+    autocast_yardstick(rows, small)
     assert torch.isfinite(m.item_embedding.weight.grad).all()
 
 

@@ -140,15 +140,9 @@ def run_block(B, L, D, H, p, layer, seed_dev, pos, time, seed=1, defer=False):
 
 
 def check_block(r, case):
-    T, D, H, p, layer, seed = r["T"], r["D"], r["H"], r["p"], r["layer"], r["seed"]
+    D, H = r["D"], r["H"]
     prm, gr = r["prm"], r["grads"]
-    s_gate, s_hid, s_out = (hr.site(layer, w) for w in (hr.SITE_GATE, hr.SITE_FFN_HID, hr.SITE_FFN_OUT))
-    for n in ("xb", "zp", "P", "O", "st1", "x1", "xn", "st2", "z1", "hact", "dyb", "dz1", "dxn", "dx1", "dO", "dzp"):
-        assert bool(torch.isfinite(r[n].float()).all()), f"{n} has an unwritten or non-finite element"
-    # inputs and projection
-    assert torch.equal(r["xb"], r["x"].bfloat16()), "xb != RNE(x)"
-    pj = dr.linear_forward(r["xb"], prm["proj_w"], prm["proj_b"], 1, r["zp"])
-    items = [("zp", r["zp"], pj["z"], pj["a_z"]), ("P", r["P"], pj["a"], pj["a_a"])]
+    items = hr.block_stage_items(r)
     # attention forward / backward on the kernel's P, zp and dO
     B, L = r["B"], r["L"]
     wpos = prm["pos_table"][r["pb0"]:r["pb0"] + 1] if r["uniform"] else prm["pos_table"]
@@ -176,37 +170,6 @@ def check_block(r, case):
         if n not in _WORST or v > _WORST[n][0]:
             _WORST[n] = (v, case)
     assert max(ex.values()) <= 1.0, (case, ex)
-    # gate forward
-    Uc = r["P"][:, :D]
-    gf = hr.gate_forward(r["O"], Uc, r["x"], r["x1"], prm["ln1_g"], prm["ln1_b"], prm["ln2_g"], prm["ln2_b"], p, seed, s_gate)
-    assert not bool((r["x1"] - r["x"])[gf["drop"]].any()), "x1 - x != 0 where the gate drops"
-    items += [("x1", r["x1"], gf["x1"], gf["a_x1"]), ("xn", r["xn"], gf["xn"], gf["a_xn"]),
-              ("st1 mean", r["st1"][:, 0], gf["mean1"], gf["a_mean1"]), ("st1 rstd", r["st1"][:, 1], gf["rstd1"], gf["a_rstd1"]),
-              ("st2 mean", r["st2"][:, 0], gf["mean2"], gf["a_mean2"]), ("st2 rstd", r["st2"][:, 1], gf["rstd2"], gf["a_rstd2"])]
-    # FFN forward
-    f1 = dr.linear_forward(r["xn"], prm["ffn1_w"], prm["ffn1_b"], 1, r["z1"], p, seed, s_hid)
-    assert not bool(r["hact"][f1["a"] == 0].any()), "hact != 0 where drop_hid drops"
-    f2 = dr.linear_residual(r["hact"], prm["ffn2_w"], prm["ffn2_b"], r["x1"], None, p, seed, s_out)
-    items += [("z1", r["z1"], f1["z"], f1["a_z"]), ("hact", r["hact"], f1["a"], f1["a_a"]), ("y", r["y"], f2["y"], f2["a_y"])]
-    # backward: cast of dy, FFN, gate
-    cc = hr.cast_colsum(r["dy"], p, seed, s_out)
-    assert torch.equal(r["dyb"], cc["dyb_exact"]), "dyb != RNE(fp32(dy keep))"
-    if p in (0.0, 0.5):
-        assert torch.equal(gr["ffn2_b"].double(), cc["db"]), "db2 is not the exact column sum of dyb"
-    items.append(("dffn2_b", gr["ffn2_b"], cc["db"], cc["a_db"]))
-    dz = hr.linear_dact_backward(r["dyb"], prm["ffn2_w"], r["z1"], p, seed, s_hid)
-    b1 = dr.linear_backward(r["dz1"], prm["ffn1_w"], r["xn"])
-    b2 = dr.linear_backward(r["dyb"], prm["ffn2_w"], r["hact"])
-    items += [("dz1", r["dz1"], dz["g"], dz["a_g"]), ("dxn", r["dxn"], b1["dx"], b1["a_dx"]), ("dW1", gr["ffn1_w"], b1["dw"], b1["a_dw"]),
-              ("dffn1_b", gr["ffn1_b"], b1["db"], b1["a_db"]), ("dW2", gr["ffn2_w"], b2["dw"], b2["a_dw"])]
-    gb = hr.gate_backward(r["dy"], r["dxn"], r["x1"], r["st1"], r["st2"], r["O"], Uc, r["zp"][:, :D], r["dx1"], prm["ln1_g"],
-                          prm["ln1_b"], prm["ln2_g"], p, seed, s_gate)
-    items += [("dx1", r["dx1"], gb["dx1"], gb["a_dx1"]), ("dzu", r["dzp"][:, :D], gb["dzu"], gb["a_dzu"]), ("dO", r["dO"], gb["dO"], gb["a_dO"]),
-              ("dln1_g", gr["ln1_g"], gb["dg1"], gb["a_dg1"]), ("dln1_b", gr["ln1_b"], gb["db1"], gb["a_db1"]),
-              ("dln2_g", gr["ln2_g"], gb["dg2"], gb["a_dg2"]), ("dln2_b", gr["ln2_b"], gb["db2"], gb["a_db2"])]
-    # projection backward
-    bp = dr.linear_backward(r["dzp"], prm["proj_w"], r["xb"], res=r["dx1"])
-    items += [("dx", r["dx"], bp["dx"], bp["a_dx"]), ("dWp", gr["proj_w"], bp["dw"], bp["a_dw"]), ("dproj_b", gr["proj_b"], bp["db"], bp["a_db"])]
     _check(case, items)
 
 

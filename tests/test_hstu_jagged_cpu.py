@@ -56,6 +56,18 @@ def test_forward_jagged_refuses_bad_shapes(bad):
         m.forward_jagged(ids, off, max_len, ts, tg)
 
 
+def test_forward_jagged_refuses_more_than_65535_sequences():
+    """B = 65,536 sequences of length 1 is a well-formed batch, but the attention grid holds at most 65,535 sequences: the refusal
+    comes before the embedding launches."""
+    m = _model()
+    B = 65536
+    off = torch.arange(B + 1, dtype=torch.int64)
+    with pytest.raises(ValueError, match="65535"):
+        m.forward_jagged(_ids(B), off, 1)
+    with pytest.raises(ValueError, match="65535"):
+        m.evaluate_batch_jagged(_ids(B), off, 1, None, torch.ones(B, dtype=torch.int64))
+
+
 def test_jagged_paths_refuse_fp32_precision():
     m = _model().set_precision("fp32")
     off = torch.tensor([0, 2, 6])

@@ -101,9 +101,13 @@ def test_jagged_bias_index_equals_the_padded_rows(pos, timed):
 
 
 # ---------------------------------------------------------------------------------------------------- one block, fp64 references
-def run_block_jagged(lengths, D, H, pos, time, idle=5, seed=1):
+def run_block_jagged(lengths, D, H, pos, time, idle=5, seed=1, *, p=0.0, layer=0, seed_dev=None, max_len=None, offsets=None, lead=0, canary=0):
     """Forward and backward of one block through grb_hstu_layer_forward_jagged / _backward_jagged with a NaN-filled saved blob and
-    workspace.  pos: ("uni", bucket) or ("fix", npos, max_distance); time: buckets or "nots".  -> the kernel's intermediates."""
+    workspace (its scratch for the ordered sums included).  pos: ("uni", bucket) or ("fix", npos, max_distance); time: buckets or "nots".  T = sum(lengths) + idle token rows;
+    max_len defaults to the longest length.  lead: idle rows put in front of the batch (offsets[0] = lead, out of contract), the
+    other rows' inputs unchanged.  offsets (a list of B + 1) replaces the device offsets (the kernels clamp it to [0, T)).  Rows
+    outside [offsets[0], offsets[B]) are idle: pad, and dy = 0 there as the head gives it.  canary: rows of x, dy, y and dx past T
+    in the same allocations, y / dx filled with 7.0.  -> the kernel's intermediates and gradients."""
     import genrec_b200.functional as Fn
     from genrec_b200 import _lib
     from genrec_b200._lib import HstuDims, HstuLayerGrads, HstuLayerParams, check, ptr, stream_ptr
@@ -111,12 +115,20 @@ def run_block_jagged(lengths, D, H, pos, time, idle=5, seed=1):
     lib = _lib.load()
     g = torch.Generator().manual_seed(seed)
     n_real = sum(lengths)
-    T, B, max_len = n_real + idle, len(lengths), max(max(lengths), 1)
+    Tm, B = n_real + idle, len(lengths)
+    T = Tm + lead
+    max_len = max_len or max(max(lengths), 1)
     off = torch.zeros(B + 1, dtype=torch.int64)
     off[1:] = torch.cumsum(torch.tensor(lengths), 0)
-    ts = 1_300_000_000 + torch.cumsum(torch.randint(1, 3 * 86400, (T,), generator=g), 0)
-    pad = torch.zeros(T, dtype=torch.uint8)
-    pad[n_real:] = 1
+    off += lead
+    if offsets is not None:
+        off = torch.tensor(offsets, dtype=torch.int64)
+    lo, hi = min(max(int(off[0]), 0), T), min(max(int(off[-1]), 0), T)
+    seq = torch.zeros(T, dtype=torch.bool)
+    seq[lo:hi] = True
+    ts = 1_300_000_000 + torch.cumsum(torch.randint(1, 3 * 86400, (Tm,), generator=g), 0)
+    ts = torch.cat([torch.full((lead,), 1_300_000_000), ts])
+    pad = (~seq).to(torch.uint8)
     uniform = pos[0] == "uni"
     npos = 8 if uniform else pos[1]
     pb = torch.full((max_len,), pos[1]) if uniform else pos_fixed(torch.arange(max_len), pos[1], pos[2])
@@ -126,73 +138,93 @@ def run_block_jagged(lengths, D, H, pos, time, idle=5, seed=1):
     meta = Fn.SeqMeta(pad.to(DEV), ts.to(DEV) if has_time else None, pb.to(torch.uint8).to(DEV), _thresholds_on(DEV), ntime or 64, npos,
                       (uniform, int(pb[0])), offsets=offd, max_len=max_len)
     prm = _params(D, H, npos, ntime, seed + 7)
-    x = torch.randn(T, D, generator=g).to(DEV)
-    dy = (torch.randint(-64, 65, (T, D), generator=g).float() / 64)
-    dy[n_real:] = 0
-    dy = dy.to(DEV)
-    dims = HstuDims(B, max_len, D, H, npos, ntime, 0.0, 0, None, 0)
+    xa = torch.randn(Tm + canary, D, generator=g)
+    xa[:Tm:3] += 1000.0 * torch.where(torch.arange(0, Tm, 3) % 2 == 0, 1.0, -1.0)[:, None]   # LayerNorm's large-offset rows
+    dya = torch.randint(-64, 65, (Tm + canary, D), generator=g).float() / 64
+    xa = torch.cat([torch.randn(lead, D, generator=g), xa])
+    dya = torch.cat([torch.zeros(lead, D), dya])
+    dya[:T][~seq] = 0
+    xa, dya = xa.to(DEV), dya.to(DEV)
+    x, dy = xa[:T], dya[:T]
+    sdev = None if seed_dev is None else torch.tensor([seed_dev], dtype=torch.int64, device=DEV)
+    dseed = 0x1234_5678_9ABC_DEF0 + layer
+    dims = HstuDims(B, max_len, D, H, npos, ntime, float(p), dseed, ptr(sdev), layer)
     names = ("proj_w", "proj_b", "pos_table", "time_table", "ln1_g", "ln1_b", "ffn1_w", "ffn1_b", "ffn2_w", "ffn2_b", "ln2_g", "ln2_b")
     pstruct = HstuLayerParams(*[ptr(prm[n]) if (n != "time_table" or has_time) else None for n in names])
     grads = {n: torch.zeros(prm[n].shape, dtype=torch.float32, device=DEV) for n in names}
     gstruct = HstuLayerGrads(*[ptr(grads[n]) for n in names])
-    seq = meta.struct()
+    st_ = meta.struct()
     sl, wl = hr.saved_layout(T, D), hr.work_layout(T, D)
     nsaved, nwork = lib.grb_hstu_layer_saved_bytes_jagged(C.byref(dims), T), lib.grb_hstu_layer_workspace_bytes_jagged(C.byref(dims), T)
     assert nsaved == sl["bytes"] and wl["bytes"] <= nwork
     saved = torch.full((nsaved,), 0xFF, dtype=torch.uint8, device=DEV)        # NaN in bf16 and fp32
-    ws = torch.zeros(nwork, dtype=torch.uint8, device=DEV)
-    ws[:wl["bytes"]] = 0xFF
-    y, dx = torch.empty_like(x), torch.empty_like(x)
+    ws = torch.full((nwork,), 0xFF, dtype=torch.uint8, device=DEV)   # the ordered sums' scratch too: a partial never stored shows
+    ya, dxa = torch.full_like(xa, 7.0), torch.full_like(xa, 7.0)
     st = stream_ptr(DEV)
-    check(lib.grb_hstu_layer_forward_jagged(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(offd), T, ptr(x), ptr(y), ptr(saved), st))
-    check(lib.grb_hstu_layer_backward_jagged(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(offd), T, ptr(dy), ptr(saved), ptr(dx),
+    check(lib.grb_hstu_layer_forward_jagged(C.byref(dims), C.byref(pstruct), C.byref(st_), ptr(offd), T, ptr(x), ptr(ya), ptr(saved), st))
+    check(lib.grb_hstu_layer_backward_jagged(C.byref(dims), C.byref(pstruct), C.byref(st_), ptr(offd), T, ptr(dy), ptr(saved), ptr(dxa),
                                              C.byref(gstruct), ptr(ws), st))
     torch.cuda.synchronize()
     out = {n: hr.view(saved, sl, n) for n in sl if n != "bytes"}
     out.update({n: hr.view(ws, wl, n) for n in wl if n != "bytes"})
-    out.update(grads=grads, prm=prm, meta=meta, off=off.tolist(), D=D, H=H, n_real=n_real, y=y, dx=dx, uniform=uniform, npos=npos,
-               pb0=int(pb[0]), has_time=has_time, ntime=ntime)
+    out.update(grads=grads, prm=prm, meta=meta, off=[min(max(int(v), lo), hi) for v in off], D=D, H=H, n_real=n_real, T=T, x=x, dy=dy,
+               y=ya[:T], dx=dxa[:T], y_canary=ya[T:], dx_canary=dxa[T:], seq=seq.to(DEV), uniform=uniform, npos=npos, pb0=int(pb[0]),
+               has_time=has_time, ntime=ntime, p=p, layer=layer, seed=hr.effective_seed(dseed, p, seed_dev), max_len=max_len)
     return out
 
 
-def check_attention_jagged(r):
+def attention_errors_jagged(r):
+    """The attention of a packed block against hr.attention per sequence (the sequences of one length batched; on the GPU, in fp64),
+    on the kernel's P, zp and dO.  Idle rows must hold O = 0 and dQ | dK | dV = 0.  -> ({O, dV, dQ, dK: worst error / allowance},
+    {dpos, dtime: table_excess})"""
     D, H, prm, gr = r["D"], r["H"], r["prm"], r["grads"]
     for n in ("P", "O", "dO", "dzp", "y", "dx"):
         assert bool(torch.isfinite(r[n].float()).all()), f"{n} has an unwritten or non-finite element"
-    n_real = r["n_real"]
-    assert not bool(r["O"][n_real:].any()) and not bool(r["dzp"][n_real:, D:].any()), "idle rows of O / dQ dK dV are not zero"
+    seq = r["seq"]
+    assert not bool(r["O"][~seq].any()) and not bool(r["dzp"][~seq][:, D:].any()), "idle rows of O / dQ dK dV are not zero"
     wpos = prm["pos_table"][r["pb0"]:r["pb0"] + 1] if r["uniform"] else prm["pos_table"]
     wtime = prm["time_table"][:r["ntime"]] if r["has_time"] else None
     nrows = 1 if r["uniform"] else r["npos"]
     acc = {"pos": None, "time": None}
-    worst = {}
+    worst = {k: 0.0 for k in ("O", "dV", "dQ", "dK")}
+    by_len = {}
     for b in range(len(r["off"]) - 1):
-        lo, hi = r["off"][b], r["off"][b + 1]
-        n = hi - lo
-        if n == 0:
-            continue
-        w, masked, pbc, tbc = hr.cell_bias(r["meta"].bias_index[lo:hi][None], wpos, wtime, nrows, H)
-        valid = hr.causal_valid(torch.zeros(1, n, dtype=torch.bool, device=DEV))
-        assert torch.equal(masked, ~valid), b
-        at = hr.attention(r["P"][lo:hi][None], w, valid, H, r["zp"][lo:hi][None], r["dO"][lo:hi][None])
-        dzp = r["dzp"][lo:hi][None]
-        for name, got, ref, allow in [("O", r["O"][lo:hi][None], at["O"], at["a_O"]), ("dV", dzp[..., D:2 * D], at["dV"], at["a_dV"]),
-                                      ("dQ", dzp[..., 2 * D:3 * D], at["dQ"], at["a_dQ"]), ("dK", dzp[..., 3 * D:], at["dK"], at["a_dK"])]:
-            worst[name] = max(worst.get(name, 0.0), dr.worst(got, ref, allow))
-        rows = torch.full_like(pbc, r["pb0"]) if r["uniform"] else pbc
-        parts = {"pos": hr.table_sums(at["dS"], valid, rows[:, None], r["npos"])}
-        if r["has_time"]:
-            parts["time"] = hr.table_sums(at["dS"], valid, tbc[:, None], r["ntime"])
-        for k, v in parts.items():
-            acc[k] = v if acc[k] is None else tuple(a + c for a, c in zip(acc[k], v))
+        lo, n = r["off"][b], min(r["off"][b + 1] - r["off"][b], r["max_len"])
+        if n > 0:
+            by_len.setdefault(n, []).append(lo)
+    for n, starts in sorted(by_len.items()):
+        step = max(1, (1 << 24) // (H * n * n))           # fp64 [seqs, H, n, n] tensors of at most 128 MB
+        for c in range(0, len(starts), step):
+            rows = (torch.tensor(starts[c:c + step])[:, None] + torch.arange(n)[None]).to(DEV)
+            w, masked, pbc, tbc = hr.cell_bias(r["meta"].bias_index[rows], wpos, wtime, nrows, H)
+            valid = hr.causal_valid(torch.zeros(rows.shape, dtype=torch.bool, device=DEV))
+            assert torch.equal(masked, ~valid.expand_as(masked)), n
+            at = hr.attention(r["P"][rows], w, valid, H, r["zp"][rows], r["dO"][rows])
+            dzp = r["dzp"][rows]
+            for name, got, ref, allow in [("O", r["O"][rows], at["O"], at["a_O"]), ("dV", dzp[..., D:2 * D], at["dV"], at["a_dV"]),
+                                          ("dQ", dzp[..., 2 * D:3 * D], at["dQ"], at["a_dQ"]), ("dK", dzp[..., 3 * D:], at["dK"], at["a_dK"])]:
+                worst[name] = max(worst[name], dr.worst(got, ref, allow))
+            bucket = torch.full_like(pbc, r["pb0"]) if r["uniform"] else pbc
+            parts = {"pos": hr.table_sums(at["dS"], valid, bucket[:, None], r["npos"])}
+            if r["has_time"]:
+                parts["time"] = hr.table_sums(at["dS"], valid, tbc[:, None], r["ntime"])
+            for k, v in parts.items():
+                acc[k] = v if acc[k] is None else tuple(a + e for a, e in zip(acc[k], v))
+            del at, w, masked, valid
+    excess = {}
+    for k, name, table in (("pos", "dpos", "pos_table"), ("time", "dtime", "time_table")):
+        if acc[k] is not None:
+            ref, mass, count = acc[k]
+            excess[name] = table_excess(gr[table], ref, mass.cpu(), count.cpu())
+        else:                                             # no time term, or no sequence at all
+            assert not bool(gr[table].any()), f"{table} gradient without a live cell"
+    return worst, excess
+
+
+def check_attention_jagged(r):
+    worst, excess = attention_errors_jagged(r)
     assert max(worst.values()) <= dr.TOL, worst
-    ref, mass, count = acc["pos"]
-    assert table_excess(gr["pos_table"], ref, mass.cpu(), count.cpu()) <= 1.0
-    if r["has_time"]:
-        ref, mass, count = acc["time"]
-        assert table_excess(gr["time_table"], ref, mass.cpu(), count.cpu()) <= 1.0
-    else:
-        assert not bool(gr["time_table"].any())
+    assert all(v <= 1.0 for v in excess.values()), excess
 
 
 BLOCK_CASES = [
