@@ -99,6 +99,8 @@ SIGNATURES = {
                                   c_float, c_u64, c_void_p, c_void_p]),
     "grb_embed_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int, c_float,
                                    c_u64, c_void_p, c_void_p, c_void_p]),
+    "grb_embed_forward_jagged": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_float, c_int, c_float, c_u64] + [c_void_p] * 5),
+    "grb_embed_backward_jagged": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_float, c_int, c_float, c_u64] + [c_void_p] * 3),
     "grb_head_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "grb_head_splits": (c_int, [c_int, c_int, c_int, c_int]),
     "grb_head_loss_forward_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_int, c_int, c_int,
@@ -123,6 +125,8 @@ SIGNATURES = {
                                              c_void_p]),
     "grb_sasrec_attention_backward": (c_int, [P(SasrecDims), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_sasrec_attention_forward_jagged": (c_int, [P(SasrecDims), c_void_p, c_int] + [c_void_p] * 7),
+    "grb_sasrec_attention_backward_jagged": (c_int, [P(SasrecDims), c_void_p, c_int] + [c_void_p] * 11),
     "grb_linear_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float,
                                    c_u64, c_void_p, c_u32, c_void_p]),
     "grb_linear_residual_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,

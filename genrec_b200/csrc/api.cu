@@ -957,7 +957,7 @@ int grb_embed_forward(const int64_t* ids, const float* table, const float* pos_t
     GRB_REQUIRE(B > 0 && L > 0 && D > 0 && D % 4 == 0, "bad shape");
     EmbedArgs a{reinterpret_cast<const long long*>(ids), table, pos_table, x, pad, B * L, L, D, scale, mask_pad_rows,
                 make_dropout(dropout_p, seed, SITE_EMBED, seed_dev)};
-    GRB_LAUNCH(embed_fwd_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
+    GRB_LAUNCH(embed_fwd_kernel<false>, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
     return 0;
 }
 int grb_embed_backward(const int64_t* ids, const int64_t* order, const float* dx, float* dtable, float* dpos_table, int B, int L, int D,
@@ -972,6 +972,48 @@ int grb_embed_backward(const int64_t* ids, const int64_t* order, const float* dx
     GRB_LAUNCH(embed_bwd_piece_kernel, row_grid((B * L + 31) / 32), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), pa);
     GRB_LAUNCH(embed_bwd_run_kernel, row_grid(B * L), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), pa);
     if (dpos_table) GRB_LAUNCH(embed_bwd_pos_kernel, L < 8 * sm_count() ? L : 8 * sm_count(), ROW_THREADS, 0, static_cast<cudaStream_t>(stream), a);
+    return 0;
+}
+
+namespace {
+int check_embed_jagged(const int64_t* offsets, int B, int T, int max_len, int D) {
+    GRB_REQUIRE(offsets != nullptr, "offsets is null");
+    GRB_REQUIRE(B >= 1 && B <= 65535, "B=%d sequences out of range [1, 65535]", B);
+    GRB_REQUIRE(T >= 1 && max_len >= 1 && (long long)T * D <= INT32_MAX, "bad shape T=%d max_len=%d D=%d", T, max_len, D);
+    return 0;
+}
+}  // namespace
+
+int grb_embed_forward_jagged(const int64_t* ids, const float* table, const float* pos_table, const int64_t* offsets, int B, int T,
+                             int max_len, int D, float scale, int mask_pad_rows, float dropout_p, uint64_t seed, const uint64_t* seed_dev,
+                             float* x, uint8_t* pad, int32_t* positions, void* stream) {
+    GRB_REQUIRE(ids && table && pos_table && x && positions, "null argument");
+    GRB_REQUIRE(D > 0 && D % 4 == 0, "bad shape");
+    GRB_TRY(check_embed_jagged(offsets, B, T, max_len, D));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GRB_LAUNCH(sas_positions_kernel, 1, 1024, 0, st, reinterpret_cast<const long long*>(offsets), B, T, max_len, positions);
+    EmbedArgs a{reinterpret_cast<const long long*>(ids), table, pos_table, x, pad, T, max_len, D, scale, mask_pad_rows,
+                make_dropout(dropout_p, seed, SITE_EMBED, seed_dev), positions};
+    GRB_LAUNCH(embed_fwd_kernel<true>, row_grid(T), ROW_THREADS, 0, st, a);
+    return 0;
+}
+int grb_embed_backward_jagged(const int64_t* ids, const int64_t* order, const float* dx, float* dtable, float* dpos_table,
+                              const int64_t* offsets, int B, int T, int max_len, int D, float scale, int mask_pad_rows, float dropout_p,
+                              uint64_t seed, const uint64_t* seed_dev, float* scratch, void* stream) {
+    GRB_REQUIRE(ids && order && dx && dtable && scratch, "null argument");
+    GRB_REQUIRE(D <= 128 * EMB_MAX_CH, "embedding backward supports D <= %d", 128 * EMB_MAX_CH);
+    GRB_REQUIRE(D % 4 == 0 && aligned16(dx) && aligned16(dtable) && aligned16(scratch) && (dpos_table == nullptr || aligned16(dpos_table)),
+                "embedding backward needs D %% 4 == 0 and 16-byte aligned buffers");
+    GRB_TRY(check_embed_jagged(offsets, B, T, max_len, D));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    EmbedBwdArgs a{reinterpret_cast<const long long*>(ids), dx, dtable, dpos_table, T, max_len, D, scale, mask_pad_rows,
+                   make_dropout(dropout_p, seed, SITE_EMBED, seed_dev), reinterpret_cast<const long long*>(order)};
+    const EmbedPieceArgs pa{a, scratch};
+    GRB_LAUNCH(embed_bwd_piece_kernel, row_grid((T + 31) / 32), ROW_THREADS, 0, st, pa);
+    GRB_LAUNCH(embed_bwd_run_kernel, row_grid(T), ROW_THREADS, 0, st, pa);
+    if (dpos_table)
+        GRB_LAUNCH(embed_bwd_pos_jagged_kernel, max_len < 8 * sm_count() ? max_len : 8 * sm_count(), ROW_THREADS, 0, st, a,
+                   reinterpret_cast<const long long*>(offsets), B);
     return 0;
 }
 
@@ -1401,35 +1443,77 @@ int sas_args(const grb_sasrec_dims* d, SasAttnArgs& a) {
 }
 }  // namespace
 
-int grb_sasrec_attention_forward(const grb_sasrec_dims* d, const void* q, const void* k, const void* v, const uint8_t* pad, void* out,
-                                 float* lse, void* stream) {
+}  // extern "C"
+
+namespace {
+// the SASRec attention on a padded batch (offsets null, T = B * L) or on a packed one; the packed form zeroes the idle rows
+template <bool JAGGED>
+int sas_forward(const grb_sasrec_dims* d, const int64_t* offsets, int T, const void* q, const void* k, const void* v, const uint8_t* pad,
+                void* out, float* lse, cudaStream_t st) {
     SasAttnArgs a;
     GRB_TRY(sas_args(d, a));
     GRB_REQUIRE(q && k && v && pad && out && lse, "null argument");
     a.q = (const bf16*)q; a.k = (const bf16*)k; a.v = (const bf16*)v; a.pad = pad; a.out = (bf16*)out; a.lse = lse;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    a.offsets = reinterpret_cast<const long long*>(offsets); a.T = T;
     dim3 grid((a.L + ATT_BLK - 1) / ATT_BLK, a.H, a.B);
-    return with_head_dim(d->D / d->H, [&](auto DH) -> int {
-        GRB_LAUNCH(sas_attn_fwd_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
+    GRB_TRY(with_head_dim(d->D / d->H, [&](auto DH) -> int {
+        GRB_LAUNCH((sas_attn_fwd_kernel<DH, JAGGED>), grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
         return 0;
-    });
+    }));
+    if (JAGGED) GRB_TRY(zero_idle_rows(offsets, d->B, T, (bf16*)out, d->D, d->D, st));
+    return 0;
 }
-
-int grb_sasrec_attention_backward(const grb_sasrec_dims* d, const void* q, const void* k, const void* v, const uint8_t* pad,
-                                  const void* out, const float* lse, const void* dout, void* dq, void* dk, void* dv, void* stream) {
+template <bool JAGGED>
+int sas_backward(const grb_sasrec_dims* d, const int64_t* offsets, int T, const void* q, const void* k, const void* v, const uint8_t* pad,
+                 const void* out, const float* lse, const void* dout, void* dq, void* dk, void* dv, cudaStream_t st) {
     SasAttnArgs a;
     GRB_TRY(sas_args(d, a));
     GRB_REQUIRE(q && k && v && pad && out && lse && dout && dq && dk && dv, "null argument");
     a.q = (const bf16*)q; a.k = (const bf16*)k; a.v = (const bf16*)v; a.pad = pad;
     a.out = (bf16*)const_cast<void*>(out); a.lse = const_cast<float*>(lse); a.d_out = (const bf16*)dout;
     a.dq = (bf16*)dq; a.dk = (bf16*)dk; a.dv = (bf16*)dv;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    a.offsets = reinterpret_cast<const long long*>(offsets); a.T = T;
     dim3 grid((a.L + ATT_BLK - 1) / ATT_BLK, a.H, a.B);
-    return with_head_dim(d->D / d->H, [&](auto DH) -> int {
-        GRB_LAUNCH(sas_attn_bwd_dq_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
-        GRB_LAUNCH(sas_attn_bwd_dkdv_kernel<DH>, grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
+    GRB_TRY(with_head_dim(d->D / d->H, [&](auto DH) -> int {
+        GRB_LAUNCH((sas_attn_bwd_dq_kernel<DH, JAGGED>), grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
+        GRB_LAUNCH((sas_attn_bwd_dkdv_kernel<DH, JAGGED>), grid, ATT_THREADS, sizeof(SasSmem<DH>), st, a);
         return 0;
-    });
+    }));
+    if (JAGGED)
+        for (void* g : {dq, dk, dv}) GRB_TRY(zero_idle_rows(offsets, d->B, T, (bf16*)g, d->D, d->D, st));
+    return 0;
+}
+// a packed SASRec batch: B sequences of at most L = max_len rows in T token rows (offsets on the device, never read here)
+int check_sas_jagged(const grb_sasrec_dims* d, const int64_t* offsets, int T) {
+    GRB_REQUIRE(d != nullptr && offsets != nullptr, "null argument");
+    GRB_REQUIRE(T >= 1 && (long long)T * d->H < INT32_MAX && (long long)T * d->D <= INT32_MAX, "token rows T=%d out of range", T);
+    GRB_REQUIRE(d->B <= 65535, "B=%d exceeds 65535 sequences", d->B);
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int grb_sasrec_attention_forward(const grb_sasrec_dims* d, const void* q, const void* k, const void* v, const uint8_t* pad, void* out,
+                                 float* lse, void* stream) {
+    return sas_forward<false>(d, nullptr, 0, q, k, v, pad, out, lse, static_cast<cudaStream_t>(stream));
+}
+int grb_sasrec_attention_backward(const grb_sasrec_dims* d, const void* q, const void* k, const void* v, const uint8_t* pad,
+                                  const void* out, const float* lse, const void* dout, void* dq, void* dk, void* dv, void* stream) {
+    return sas_backward<false>(d, nullptr, 0, q, k, v, pad, out, lse, dout, dq, dk, dv, static_cast<cudaStream_t>(stream));
+}
+int grb_sasrec_attention_forward_jagged(const grb_sasrec_dims* d, const int64_t* offsets, int T, const void* q, const void* k,
+                                        const void* v, const uint8_t* pad, void* out, float* lse, void* stream) {
+    GRB_TRY(check_sas_jagged(d, offsets, T));
+    GRB_REQUIRE(aligned16(out), "out must be 16-byte aligned");
+    return sas_forward<true>(d, offsets, T, q, k, v, pad, out, lse, static_cast<cudaStream_t>(stream));
+}
+int grb_sasrec_attention_backward_jagged(const grb_sasrec_dims* d, const int64_t* offsets, int T, const void* q, const void* k,
+                                         const void* v, const uint8_t* pad, const void* out, const float* lse, const void* dout,
+                                         void* dq, void* dk, void* dv, void* stream) {
+    GRB_TRY(check_sas_jagged(d, offsets, T));
+    GRB_REQUIRE(aligned16(dq) && aligned16(dk) && aligned16(dv), "dq, dk and dv must be 16-byte aligned");
+    return sas_backward<true>(d, offsets, T, q, k, v, pad, out, lse, dout, dq, dk, dv, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------------ generic fused linear pieces

@@ -67,23 +67,6 @@ struct HstuAttnArgs {
     int T;
 };
 
-// First row and length of sequence b.  A malformed device `offsets` yields wrong numbers but never a row outside [0, T).
-// The attention kernels take JAGGED as a template parameter, so that their padded instantiations keep the registers (and the
-// code) they had before packed batches existed.
-template <bool JAGGED = true>
-GRB_DEVINL void seq_span(const long long* offsets, int T, int L, int b, long long& tok0, int& len) {
-    if (!JAGGED || offsets == nullptr) {
-        tok0 = (long long)b * L;
-        len = L;
-        return;
-    }
-    long long lo = offsets[b], hi = offsets[b + 1];
-    lo = lo < 0 ? 0 : (lo > T ? T : lo);
-    hi = hi < lo ? lo : (hi > T ? T : hi);
-    tok0 = lo;
-    len = (int)(hi - lo < L ? hi - lo : L);
-}
-
 GRB_DEVINL int time_bucket_dev(long long dt, const long long* thr, int ntime) {
     long long d = dt < 0 ? -dt : dt;
     d = d < 1 ? 1 : d;

@@ -4,6 +4,13 @@
 // A padded query row has qmask = 0, so its output is exactly 0 (the reference's "uniform softmax over -1e9" never
 // survives the post-softmax query mask, sasrec.py:232-233); a non-padded query always sees its own key.
 // Shares tile/fragment helpers with attn_hstu.cuh.
+//
+// Packed (jagged) batches: with SasAttnArgs::offsets set, sequence b is token rows offsets[b] .. offsets[b+1]-1 of T, clamped to
+// [0, T) and to L = the longest length the grid covers (seq_span).  A query tile past a sequence's end exits at once.  lse is then
+// per token, [H, T].  Under dropout the mask of a packed batch is keyed by the query's TOKEN ROW and the head, and by the key's
+// index within its sequence: row key (tok0 + i) * H + h, column j; the padded layout keeps row key (b H + h) L + i, column j.
+// The kernels write only sequence rows: the caller zeroes the idle rows [0, offsets[0]) and [offsets[B], T) of O and dQ | dK | dV.
+// JAGGED is a template parameter, so the padded instantiations compile to the code they had before packed batches existed.
 #pragma once
 #include "attn_hstu.cuh"
 
@@ -11,14 +18,26 @@ namespace grb {
 
 struct SasAttnArgs {
     const bf16* q; const bf16* k; const bf16* v; int ld;  // [T, D] each
-    const uint8_t* pad;                                   // [B, L] 1 = padding (mask == 0)
+    const uint8_t* pad;                                   // [B, L] (packed: [T]) 1 = padding (mask == 0)
     int B, L, H;
     float scale;
     Dropout drop;
     bf16* out; float* lse;                                // out [T, D] ; lse [B, H, L]
     const bf16* d_out;                                    // [T, D]
     bf16* dq; bf16* dk; bf16* dv;                         // [T, D]
+    const long long* offsets;                             // packed batch: [B+1] (null: sequence b is rows b*L .. b*L+L-1)
+    int T;                                                // packed batch: token rows
 };
+
+// lse slot and dropout row key of query i of sequence b (first row tok0, L rows), head h
+template <bool JAGGED>
+GRB_DEVINL size_t sas_lse_at(const SasAttnArgs& a, int b, int h, long long tok0, int L, int i) {
+    return JAGGED ? (size_t)h * a.T + (size_t)(tok0 + i) : ((size_t)b * a.H + h) * L + i;
+}
+template <bool JAGGED>
+GRB_DEVINL uint32_t sas_drop_row(const SasAttnArgs& a, int b, int h, long long tok0, int L, int i) {
+    return JAGGED ? ((uint32_t)tok0 + (uint32_t)i) * (uint32_t)a.H + (uint32_t)h : (uint32_t)((b * a.H + h) * L + i);
+}
 
 template <int DH>
 struct SasSmem {
@@ -39,7 +58,7 @@ GRB_DEVINL float quad_sum(float v) {
 }
 
 // tile roles: 0 = Q, 1 = K, 2 = V
-template <int DH>
+template <int DH, bool JAGGED>
 __global__ void __launch_bounds__(ATT_THREADS) sas_attn_fwd_kernel(SasAttnArgs a) {
     pdl_wait();
     a.drop.resolve();
@@ -47,8 +66,11 @@ __global__ void __launch_bounds__(ATT_THREADS) sas_attn_fwd_kernel(SasAttnArgs a
     SasSmem<DH>& sm = *reinterpret_cast<SasSmem<DH>*>(att_smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int L = a.L, q0 = qt * ATT_BLK;
-    const long long tok0 = (long long)b * L;
+    const int q0 = qt * ATT_BLK;
+    long long tok0;
+    int L;
+    seq_span<JAGGED>(a.offsets, a.T, a.L, b, tok0, L);
+    if (JAGGED && q0 >= L) return;   // query tile past the end of a packed sequence
 
     att_load_tile<DH>(sm.tile[0], a.q + (size_t)tok0 * a.ld + h * DH, a.ld, 0, q0, L, 0, tid);
     cp_async_commit();
@@ -108,7 +130,7 @@ __global__ void __launch_bounds__(ATT_THREADS) sas_attn_fwd_kernel(SasAttnArgs a
                 if (a.drop.thresh) {
                     const int jl = n * 8 + 2 * t + (r & 1);
                     const int i = (r < 2) ? i0 : i1;
-                    p = a.drop.apply(p, (uint32_t)((b * a.H + h) * L + i), (uint32_t)(k0 + jl));
+                    p = a.drop.apply(p, sas_drop_row<JAGGED>(a, b, h, tok0, L, i), (uint32_t)(k0 + jl));
                 }
                 s[n][r] = p;
             }
@@ -131,8 +153,8 @@ __global__ void __launch_bounds__(ATT_THREADS) sas_attn_fwd_kernel(SasAttnArgs a
         if (i1 < L) *reinterpret_cast<uint32_t*>(a.out + (size_t)(tok0 + i1) * a.ld + col) = pack_bf16(o[n][2] * inv1, o[n][3] * inv1);
     }
     if (t == 0) {
-        if (i0 < L) a.lse[((size_t)b * a.H + h) * L + i0] = l0 > 0.f ? m0 + logf(l0) : 0.f;
-        if (i1 < L) a.lse[((size_t)b * a.H + h) * L + i1] = l1 > 0.f ? m1 + logf(l1) : 0.f;
+        if (i0 < L) a.lse[sas_lse_at<JAGGED>(a, b, h, tok0, L, i0)] = l0 > 0.f ? m0 + logf(l0) : 0.f;
+        if (i1 < L) a.lse[sas_lse_at<JAGGED>(a, b, h, tok0, L, i1)] = l1 > 0.f ? m1 + logf(l1) : 0.f;
     }
 }
 
@@ -152,7 +174,7 @@ GRB_DEVINL void sas_rowdot(float* dsum, const bf16* tdo, const bf16* to, int tid
 }
 
 // backward dQ: tile roles 0 = Q, 1 = K, 2 = V, 3 = dO, 4 = O
-template <int DH>
+template <int DH, bool JAGGED>
 __global__ void __launch_bounds__(ATT_THREADS) sas_attn_bwd_dq_kernel(SasAttnArgs a) {
     pdl_wait();
     a.drop.resolve();
@@ -160,8 +182,11 @@ __global__ void __launch_bounds__(ATT_THREADS) sas_attn_bwd_dq_kernel(SasAttnArg
     SasSmem<DH>& sm = *reinterpret_cast<SasSmem<DH>*>(att_smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int L = a.L, q0 = qt * ATT_BLK;
-    const long long tok0 = (long long)b * L;
+    const int q0 = qt * ATT_BLK;
+    long long tok0;
+    int L;
+    seq_span<JAGGED>(a.offsets, a.T, a.L, b, tok0, L);
+    if (JAGGED && q0 >= L) return;   // query tile past the end of a packed sequence
 
     att_load_tile<DH>(sm.tile[0], a.q + (size_t)tok0 * a.ld + h * DH, a.ld, 0, q0, L, 0, tid);
     att_load_tile<DH>(sm.tile[3], a.d_out + (size_t)tok0 * a.ld + h * DH, a.ld, 0, q0, L, 0, tid);
@@ -170,7 +195,7 @@ __global__ void __launch_bounds__(ATT_THREADS) sas_attn_bwd_dq_kernel(SasAttnArg
     cp_async_wait<0>();
     __syncthreads();
     sas_rowdot<DH>(sm.dsum_tile, sm.tile[3], sm.tile[4], tid);
-    if (tid < ATT_BLK) sm.lse_tile[tid] = (q0 + tid < L) ? a.lse[((size_t)b * a.H + h) * L + q0 + tid] : 0.f;
+    if (tid < ATT_BLK) sm.lse_tile[tid] = (q0 + tid < L) ? (JAGGED ? a.lse[(size_t)h * a.T + (size_t)(tok0 + q0 + tid)] : a.lse[((size_t)b * a.H + h) * L + q0 + tid]) : 0.f;
     __syncthreads();
     uint32_t qf[DH / 16][4], dof[DH / 16][4];
     att_load_afrag<DH>(qf, sm.tile[0], warp * 16, lane);
@@ -211,7 +236,7 @@ __global__ void __launch_bounds__(ATT_THREADS) sas_attn_bwd_dq_kernel(SasAttnArg
                 float dsv = 0.f;
                 if (valid) {
                     float p = __expf(s[n][r] * a.scale - ((r < 2) ? lse0 : lse1));
-                    float dA = a.drop.apply(da[n][r], (uint32_t)((b * a.H + h) * L + i), (uint32_t)j);
+                    float dA = a.drop.apply(da[n][r], sas_drop_row<JAGGED>(a, b, h, tok0, L, i), (uint32_t)j);
                     dsv = p * (dA - ((r < 2) ? ds0 : ds1)) * a.scale;
                 }
                 s[n][r] = dsv;
@@ -229,7 +254,7 @@ __global__ void __launch_bounds__(ATT_THREADS) sas_attn_bwd_dq_kernel(SasAttnArg
 }
 
 // backward dK/dV: CTA owns 64 keys ; tile roles 0 = K, 1 = V, 2 = Q, 3 = dO, 4 = O (streamed)
-template <int DH>
+template <int DH, bool JAGGED>
 __global__ void __launch_bounds__(ATT_THREADS) sas_attn_bwd_dkdv_kernel(SasAttnArgs a) {
     pdl_wait();
     a.drop.resolve();
@@ -237,8 +262,11 @@ __global__ void __launch_bounds__(ATT_THREADS) sas_attn_bwd_dkdv_kernel(SasAttnA
     SasSmem<DH>& sm = *reinterpret_cast<SasSmem<DH>*>(att_smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int kt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int L = a.L, k0 = kt * ATT_BLK;
-    const long long tok0 = (long long)b * L;
+    const int k0 = kt * ATT_BLK;
+    long long tok0;
+    int L;
+    seq_span<JAGGED>(a.offsets, a.T, a.L, b, tok0, L);
+    if (JAGGED && k0 >= L) return;   // key tile past the end of a packed sequence
     const int nqt = (L + ATT_BLK - 1) / ATT_BLK;
 
     att_load_tile<DH>(sm.tile[0], a.k + (size_t)tok0 * a.ld + h * DH, a.ld, 0, k0, L, 0, tid);
@@ -266,7 +294,7 @@ __global__ void __launch_bounds__(ATT_THREADS) sas_attn_bwd_dkdv_kernel(SasAttnA
         cp_async_commit();
         if (tid < ATT_BLK) {
             int i = q0 + tid;
-            sm.lse_tile[tid] = (i < L) ? a.lse[((size_t)b * a.H + h) * L + i] : 0.f;
+            sm.lse_tile[tid] = (i < L) ? a.lse[sas_lse_at<JAGGED>(a, b, h, tok0, L, i)] : 0.f;
             sm.pad_tile[tid] = (i < L) ? a.pad[tok0 + i] : 1;  // QUERY padding here
         }
         cp_async_wait<0>();
@@ -291,7 +319,7 @@ __global__ void __launch_bounds__(ATT_THREADS) sas_attn_bwd_dkdv_kernel(SasAttnA
                 float pd = 0.f, dsv = 0.f;
                 if (valid) {
                     float p = __expf(st[n][r] * a.scale - sm.lse_tile[il]);
-                    const uint32_t drow = (uint32_t)((b * a.H + h) * L + i);
+                    const uint32_t drow = sas_drop_row<JAGGED>(a, b, h, tok0, L, i);
                     pd = a.drop.apply(p, drow, (uint32_t)j);
                     float dA = a.drop.apply(dat[n][r], drow, (uint32_t)j);
                     dsv = p * (dA - sm.dsum_tile[il]) * a.scale;

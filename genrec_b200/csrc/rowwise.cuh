@@ -523,12 +523,16 @@ __global__ void __launch_bounds__(256) colsum_bf16_kernel(const bf16* __restrict
 
 // ------------------------------------------------------------------------------------------------ embedding
 // x[t,:] = drop(E[ids[t],:] * scale (+ pos[t % L,:]))  -> fp32 ; pad[t] = ids[t]==0   (hstu.py:124-128 ; sasrec.py:100-111)
+// JAGGED (a packed SASRec batch): the position row of token t is tokpos[t] (sas_positions_kernel) instead of t % L, and a row
+// outside every sequence (tokpos[t] < 0) gets x = 0 and pad = 1 whatever its id.
 struct EmbedArgs {
     const long long* ids; const float* E; const float* pos;  // pos nullable [>=L, D]
     float* x; uint8_t* pad;
     int T, L, D; float scale; int mask_pad_rows;  // sasrec: x *= (id != 0)
     Dropout drop;
+    const int* tokpos;   // JAGGED: [T] position row of each token, -1 = idle
 };
+template <bool JAGGED = false>
 __global__ void __launch_bounds__(ROW_THREADS) embed_fwd_kernel(EmbedArgs a) {
     pdl_wait();
     a.drop.resolve();
@@ -536,9 +540,16 @@ __global__ void __launch_bounds__(ROW_THREADS) embed_fwd_kernel(EmbedArgs a) {
     const int nw = gridDim.x * (ROW_THREADS / 32);
     for (int row = blockIdx.x * (ROW_THREADS / 32) + wib; row < a.T; row += nw) {
         long long id = a.ids[row];
+        if constexpr (JAGGED) {
+            if (a.tokpos[row] < 0) {
+                if (lane == 0 && a.pad) a.pad[row] = 1;
+                for (int c = lane * 4; c < a.D; c += 128) *reinterpret_cast<float4*>(a.x + (size_t)row * a.D + c) = make_float4(0.f, 0.f, 0.f, 0.f);
+                continue;
+            }
+        }
         if (lane == 0 && a.pad) a.pad[row] = id == 0;
         const float* src = a.E + (size_t)id * a.D;
-        const float* ps = a.pos ? a.pos + (size_t)(row % a.L) * a.D : nullptr;
+        const float* ps = a.pos ? a.pos + (size_t)(JAGGED ? a.tokpos[row] : row % a.L) * a.D : nullptr;
         const float keep = (a.mask_pad_rows && id == 0) ? 0.f : 1.f;
         for (int c = lane * 4; c < a.D; c += 128) {
             float4 v = *reinterpret_cast<const float4*>(src + c);
@@ -556,6 +567,42 @@ __global__ void __launch_bounds__(ROW_THREADS) embed_fwd_kernel(EmbedArgs a) {
             }
             *reinterpret_cast<float4*>(a.x + o) = make_float4(e[0], e[1], e[2], e[3]);
         }
+    }
+}
+// The longest sequence P of a packed batch, each sequence clamped to [0, T) and to L (seq_span), over one CTA's threads.
+GRB_DEVINL int jagged_longest(const long long* offsets, int B, int T, int L, int* red) {
+    int m = 0;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        long long tok0;
+        int len;
+        seq_span(offsets, T, L, b, tok0, len);
+        m = max(m, len);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+    __syncthreads();
+    int P = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) P = max(P, red[w]);
+    __syncthreads();
+    return P;
+}
+// SASRec's position rule on a packed batch (one CTA): sasrec_collate_fn left-pads every sequence to P = the longest of the batch,
+// so item i of a sequence of packed length n sits at position P - n + i.  tokpos[t] = that position for each sequence row and -1
+// for every other row.  Every value is -1 or in [0, L), whatever the device offsets hold (overlapping sequences: one wins).
+__global__ void __launch_bounds__(1024) sas_positions_kernel(const long long* __restrict__ offsets, int B, int T, int L,
+                                                            int* __restrict__ tokpos) {
+    pdl_wait();
+    __shared__ int red[32];
+    const int P = jagged_longest(offsets, B, T, L, red);
+    for (int t = threadIdx.x; t < T; t += blockDim.x) tokpos[t] = -1;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    for (int b = threadIdx.x >> 5; b < B; b += blockDim.x >> 5) {
+        long long tok0;
+        int len;
+        seq_span(offsets, T, L, b, tok0, len);
+        for (int i = lane; i < len; i += 32) tokpos[tok0 + i] = P - len + i;
     }
 }
 struct EmbedBwdArgs {
@@ -599,6 +646,70 @@ __global__ void __launch_bounds__(ROW_THREADS) embed_bwd_pos_kernel(EmbedBwdArgs
                 a.drop.apply2(v[i].x, v[i].y, row, c);
                 a.drop.apply2(v[i].z, v[i].w, row, c + 2);
                 stage[e] = v[i];
+                if (c == 0) live[u] = !pad[i];
+            }
+            __syncthreads();
+            if (q < nq) {
+#pragma unroll 8
+                for (int u = 0; u < nb; ++u) {
+                    if (!live[u]) continue;
+                    const float4 t = stage[u * nq + q];
+                    s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
+                }
+            }
+            __syncthreads();
+        }
+        if (q < nq) *d = make_float4(o.x + s.x, o.y + s.y, o.z + s.z, o.w + s.w);
+    }
+}
+
+// embed_bwd_pos_kernel on a packed batch (a.T token rows, a.L = max_len): position row l < P (the longest sequence, jagged_longest)
+// sums, in ascending b, dropmask(dx) of the token at position l of every sequence that reaches it (n_b >= P - l: row
+// tok0_b + n_b - (P - l)), leaving out id-0 tokens with mask_pad_rows, then adds that sum once per element.  These are the
+// terms, in the order, that embed_bwd_pos_kernel sums on the left-padded batch of the same sequences (whose other tokens at
+// position l are pads), so the two give the same bits.  Rows l >= P are not written.
+__global__ void __launch_bounds__(ROW_THREADS) embed_bwd_pos_jagged_kernel(EmbedBwdArgs a, const long long* __restrict__ offsets, int B) {
+    __shared__ float4 stage[EMB_POS_STAGE];
+    __shared__ uint8_t live[EMB_POS_STAGE];
+    __shared__ int srow[EMB_POS_STAGE];
+    __shared__ int red[ROW_THREADS / 32];
+    pdl_wait();
+    a.drop.resolve();
+    const int nq = a.D / 4, chunk = EMB_POS_STAGE / nq;
+    const int q = threadIdx.x;
+    const int P = jagged_longest(offsets, B, a.T, a.L, red);
+    for (int l = blockIdx.x; l < P; l += gridDim.x) {
+        float4* d = reinterpret_cast<float4*>(a.dpos + (size_t)l * a.D + 4 * q);
+        const float4 o = q < nq ? *d : make_float4(0.f, 0.f, 0.f, 0.f);
+        float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int b0 = 0; b0 < B; b0 += chunk) {
+            const int nb = min(chunk, B - b0);
+            for (int u = threadIdx.x; u < nb; u += ROW_THREADS) {   // the token of sequence b0 + u at position l, or -1
+                long long tok0;
+                int len;
+                seq_span(offsets, a.T, a.L, b0 + u, tok0, len);
+                srow[u] = len >= P - l ? (int)(tok0 + len - (P - l)) : -1;
+            }
+            __syncthreads();
+            float4 v[EMB_POS_STAGE / ROW_THREADS];
+            bool pad[EMB_POS_STAGE / ROW_THREADS];
+#pragma unroll
+            for (int i = 0; i < EMB_POS_STAGE / ROW_THREADS; ++i) {
+                const int e = threadIdx.x + i * ROW_THREADS, u = e / nq, c = 4 * (e - u * nq);
+                const int row = u < nb ? srow[u] : -1;
+                if (row >= 0) v[i] = *reinterpret_cast<const float4*>(a.dx + (size_t)row * a.D + c);
+                pad[i] = u < nb && c == 0 && (row < 0 || (a.mask_pad_rows && a.ids[row] == 0));
+            }
+#pragma unroll
+            for (int i = 0; i < EMB_POS_STAGE / ROW_THREADS; ++i) {
+                const int e = threadIdx.x + i * ROW_THREADS, u = e / nq, c = 4 * (e - u * nq);
+                if (u >= nb) continue;
+                const int row = srow[u];
+                if (row >= 0) {
+                    a.drop.apply2(v[i].x, v[i].y, row, c);
+                    a.drop.apply2(v[i].z, v[i].w, row, c + 2);
+                    stage[e] = v[i];
+                }
                 if (c == 0) live[u] = !pad[i];
             }
             __syncthreads();

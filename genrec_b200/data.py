@@ -112,9 +112,11 @@ def collate_jagged(items: torch.Tensor, offsets: torch.Tensor, targets: torch.Te
 
 def pack_jagged(items: torch.Tensor, offsets: torch.Tensor, targets: torch.Tensor, max_seq_len: int = 50,
                 timestamps: "torch.Tensor | None" = None, num_tokens: "int | None" = None) -> Dict[str, torch.Tensor]:
-    """``collate_jagged`` without the pads, for ``HSTU.forward_jagged``: the same jagged batch on the device (items / timestamps [N]
-    int64 in time order, offsets [B+1], one held-out target per user) -> a packed batch.  Sequence b is hstu_collate_fn's row b
-    with its pads removed: the last min(len_b, max_seq_len) items, the targets shifted by one with the held-out item last.
+    """``collate_jagged`` without the pads, for ``HSTU.forward_jagged`` and ``SASRec.forward_jagged``: the same jagged batch on the
+    device (items / timestamps [N] int64 in time order, offsets [B+1], one held-out target per user) -> a packed batch.  Sequence b
+    is hstu_collate_fn's row b with its pads removed: the last min(len_b, max_seq_len) items, the targets shifted by one with the
+    held-out item last.  With ``timestamps=None`` that is sasrec_collate_fn's row b without its pads, SASRec's packed batch; its
+    ``input_ids`` with the held-out targets [B] also serve ``evaluate_batch_jagged``.
     Returns input_ids, targets (and timestamps) [T], offsets [B+1] (sequence b = rows offsets[b] .. offsets[b+1]-1), the host int
     max_len and overflow (a 0-dim bool on the device).
 

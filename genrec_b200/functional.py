@@ -12,7 +12,7 @@ from typing import List, NamedTuple, Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import HstuDims, HstuLayerGrads, HstuLayerParams, HstuSeq, SasrecDims, check, ptr, require_cuda, stream_ptr
+from ._lib import HstuDims, HstuLayerGrads, HstuLayerParams, HstuSeq, SasrecDims, check, ensure_device, ptr, require_cuda, stream_ptr
 
 PARAM_ORDER = ("proj_w", "proj_b", "pos_table", "time_table", "ln1_g", "ln1_b", "ffn1_w", "ffn1_b", "ffn2_w", "ffn2_b",
                "ln2_g", "ln2_b")
@@ -248,25 +248,74 @@ class HstuLayerFn(torch.autograd.Function):
         return (dx, None, None, None, *grads)
 
 
+def check_jagged_batch(what: str, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, max_len_limit: int) -> torch.Tensor:
+    """Argument check of a packed batch before any launch (HSTU and SASRec) -> offsets on input_ids' device.  input_ids must be a
+    non-empty [T] int64 tensor, offsets a [B+1] int64 tensor with 1 <= B <= 65535 (the attention grid's z dimension), max_len an int
+    in [1, max_len_limit].  CPU offsets are refused with ValueError unless offsets[0] == 0, they never decrease, no length exceeds
+    max_len and offsets[B] <= T; device offsets are not read on the host (CUDA graphs), and the kernels keep a malformed one inside
+    the T rows."""
+    if input_ids.dim() != 1 or input_ids.numel() == 0 or input_ids.dtype != torch.int64:
+        raise ValueError(f"{what}: input_ids must be a non-empty [T] int64 tensor, got {tuple(input_ids.shape)} {input_ids.dtype}")
+    T = input_ids.numel()
+    if not isinstance(offsets, torch.Tensor) or offsets.dim() != 1 or offsets.numel() < 2 or offsets.dtype != torch.int64:
+        raise ValueError(f"{what}: offsets must be a [B+1] int64 tensor with B >= 1")
+    if offsets.numel() - 1 > 65535:
+        raise ValueError(f"{what}: B = {offsets.numel() - 1} sequences exceeds 65535 (the attention grid's z dimension)")
+    if isinstance(max_len, bool) or not isinstance(max_len, int) or not 1 <= max_len <= max_len_limit:
+        raise ValueError(f"{what}: max_len must be an int in [1, {max_len_limit}], got {max_len!r}")
+    if not offsets.is_cuda:
+        o = offsets
+        if int(o[0]) != 0:
+            raise ValueError(f"{what}: offsets[0] must be 0, got {int(o[0])}")
+        lens = o[1:] - o[:-1]
+        if bool((lens < 0).any()):
+            raise ValueError(f"{what}: offsets must be non-decreasing")
+        if int(lens.max()) > max_len:
+            raise ValueError(f"{what}: a sequence of length {int(lens.max())} exceeds max_len {max_len}")
+        if int(o[-1]) > T:
+            raise ValueError(f"{what}: offsets[B] = {int(o[-1])} exceeds the {T} token rows")
+    elif offsets.device != input_ids.device:
+        raise ValueError(f"{what}: offsets must be on the CPU or on {input_ids.device}, got {offsets.device}")
+    require_cuda(input_ids)
+    ensure_device(input_ids.device)
+    return offsets.to(input_ids.device)
+
+
 class EmbedFn(torch.autograd.Function):
-    """x = dropout(E[ids] * scale (+ pos)) ; also emits the uint8 pad flags."""
+    """x = dropout(E[ids] * scale (+ pos)) ; also emits the uint8 pad flags.  With ``offsets`` ([B+1] int64 on the device) and
+    ``max_len`` the batch is packed (ids [T] -> x [T, D], pad [T]) and each token takes SASRec's position row P - n_b + i, P the
+    longest sequence, derived on the device (grb_embed_forward_jagged); rows outside every sequence get x = 0 and pad = 1."""
 
     @staticmethod
-    def forward(ctx, ids, table, pos_table, scale, mask_pad_rows, p, seed, seed_dev, sink=None):
+    def forward(ctx, ids, table, pos_table, scale, mask_pad_rows, p, seed, seed_dev, sink=None, offsets=None, max_len=None):
         lib = _lib.load()
         require_cuda(ids, table)
         require_i64(ids)
         require_f32(table, pos_table)
         ctx.sink = sink
-        B, L = ids.shape
+        ctx.jagged = None
         D = table.shape[1]
         ids = ids.contiguous()
-        x = torch.empty(B, L, D, dtype=torch.float32, device=ids.device)
-        pad = torch.empty(B, L, dtype=torch.uint8, device=ids.device)
-        with torch.cuda.device(ids.device):
-            check(lib.grb_embed_forward(ptr(ids), ptr(table.detach()), ptr(pos_table.detach()) if pos_table is not None else None,
-                                        ptr(x), ptr(pad), B, L, D, float(scale), int(mask_pad_rows), float(p), int(seed), ptr(seed_dev),
-                                        stream_ptr(ids.device)))
+        if offsets is not None:
+            T = ids.numel()
+            B = offsets.numel() - 1
+            x = torch.empty(T, D, dtype=torch.float32, device=ids.device)
+            pad = torch.empty(T, dtype=torch.uint8, device=ids.device)
+            positions = torch.empty(T, dtype=torch.int32, device=ids.device)
+            with torch.cuda.device(ids.device):
+                check(lib.grb_embed_forward_jagged(ptr(ids), ptr(table.detach()), ptr(pos_table.detach()), ptr(offsets), B, T, int(max_len), D,
+                                                   float(scale), int(mask_pad_rows), float(p), int(seed), ptr(seed_dev), ptr(x), ptr(pad),
+                                                   ptr(positions), stream_ptr(ids.device)))
+            ids = torch.where(positions >= 0, ids, 0)   # the idle rows' x does not depend on the table
+            ctx.jagged = (offsets, B, T, int(max_len))
+        else:
+            B, L = ids.shape
+            x = torch.empty(B, L, D, dtype=torch.float32, device=ids.device)
+            pad = torch.empty(B, L, dtype=torch.uint8, device=ids.device)
+            with torch.cuda.device(ids.device):
+                check(lib.grb_embed_forward(ptr(ids), ptr(table.detach()), ptr(pos_table.detach()) if pos_table is not None else None,
+                                            ptr(x), ptr(pad), B, L, D, float(scale), int(mask_pad_rows), float(p), int(seed), ptr(seed_dev),
+                                            stream_ptr(ids.device)))
         ctx.save_for_backward(ids)
         ctx.args = (table.shape, None if pos_table is None else pos_table.shape, scale, mask_pad_rows, p, seed, seed_dev)
         ctx.mark_non_differentiable(pad)
@@ -277,7 +326,6 @@ class EmbedFn(torch.autograd.Function):
         lib = _lib.load()
         (ids,) = ctx.saved_tensors
         tshape, pshape, scale, mask_pad_rows, p, seed, seed_dev = ctx.args
-        B, L = ids.shape
         D = tshape[1]
         dx = dx.contiguous().float()
         if ctx.sink is not None:
@@ -286,13 +334,20 @@ class EmbedFn(torch.autograd.Function):
             dtable = torch.zeros(tshape, dtype=torch.float32, device=dx.device)
             dpos = torch.zeros(pshape, dtype=torch.float32, device=dx.device) if pshape is not None else None
         order = torch.sort(ids.reshape(-1), stable=True).indices   # tokens grouped by id, in token order
-        scratch = torch.empty(B * L, D, dtype=torch.float32, device=dx.device)
+        scratch = torch.empty(ids.numel(), D, dtype=torch.float32, device=dx.device)
         with torch.cuda.device(dx.device):
-            check(lib.grb_embed_backward(ptr(ids), ptr(order), ptr(dx), ptr(dtable), ptr(dpos), B, L, D, float(scale), int(mask_pad_rows), float(p),
-                                         int(seed), ptr(seed_dev), ptr(scratch), stream_ptr(dx.device)))
+            if ctx.jagged is not None:
+                offsets, B, T, max_len = ctx.jagged
+                check(lib.grb_embed_backward_jagged(ptr(ids), ptr(order), ptr(dx), ptr(dtable), ptr(dpos), ptr(offsets), B, T, max_len, D,
+                                                    float(scale), int(mask_pad_rows), float(p), int(seed), ptr(seed_dev), ptr(scratch),
+                                                    stream_ptr(dx.device)))
+            else:
+                B, L = ids.shape
+                check(lib.grb_embed_backward(ptr(ids), ptr(order), ptr(dx), ptr(dtable), ptr(dpos), B, L, D, float(scale), int(mask_pad_rows),
+                                             float(p), int(seed), ptr(seed_dev), ptr(scratch), stream_ptr(dx.device)))
         if ctx.sink is not None:
-            return (None,) * 9
-        return None, dtable, dpos, None, None, None, None, None, None
+            return (None,) * 11
+        return None, dtable, dpos, None, None, None, None, None, None, None, None
 
 
 def _head_grad_buffers(ctx, xc, ln_g, ln_b, table, sink, unit_loss_grad):
@@ -765,23 +820,42 @@ def linear_bwd(dyb, wb, xb, need_dx=True, dx_residual=None, need_dw=True):
     return dx, dw, db
 
 
-def sasrec_attention_fwd(q, k, v, pad, H, p=0.0, seed=0, seed_dev=None, layer=0):
+def _sasrec_dims(q, H, p, seed, seed_dev, layer, offsets, max_len):
+    if offsets is None:
+        B, L, D = q.shape
+        return SasrecDims(B, L, D, H, float(p), int(seed), ptr(seed_dev), layer)
+    return SasrecDims(offsets.numel() - 1, int(max_len), q.shape[-1], H, float(p), int(seed), ptr(seed_dev), layer)
+
+
+def sasrec_attention_fwd(q, k, v, pad, H, p=0.0, seed=0, seed_dev=None, layer=0, offsets=None, max_len=None):
+    """q, k, v [B, L, D] bf16, pad [B, L] -> (out [B, L, D] bf16, lse [B, H, L]).  With ``offsets`` ([B+1] int64 on the device) and
+    ``max_len`` the batch is packed (grb_sasrec_attention_forward_jagged): q, k, v, out [T, D], pad [T], lse [H, T]."""
     lib = _lib.load()
-    B, L, D = q.shape
-    dims = SasrecDims(B, L, D, H, float(p), int(seed), ptr(seed_dev), layer)
+    dims = _sasrec_dims(q, H, p, seed, seed_dev, layer, offsets, max_len)
     out = torch.empty_like(q)
-    lse = torch.empty(B, H, L, dtype=torch.float32, device=q.device)
-    check(lib.grb_sasrec_attention_forward(C.byref(dims), ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out), ptr(lse), stream_ptr(q.device)))
+    if offsets is None:
+        B, L, D = q.shape
+        lse = torch.empty(B, H, L, dtype=torch.float32, device=q.device)
+        check(lib.grb_sasrec_attention_forward(C.byref(dims), ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out), ptr(lse), stream_ptr(q.device)))
+    else:
+        T = q.shape[0]
+        lse = torch.empty(H, T, dtype=torch.float32, device=q.device)
+        check(lib.grb_sasrec_attention_forward_jagged(C.byref(dims), ptr(offsets), T, ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out), ptr(lse),
+                                                      stream_ptr(q.device)))
     return out, lse
 
 
-def sasrec_attention_bwd(q, k, v, pad, out, lse, dout, H, p=0.0, seed=0, seed_dev=None, layer=0):
+def sasrec_attention_bwd(q, k, v, pad, out, lse, dout, H, p=0.0, seed=0, seed_dev=None, layer=0, offsets=None, max_len=None):
+    """The backward of ``sasrec_attention_fwd`` -> (dq, dk, dv) shaped like q; packed with ``offsets`` and ``max_len``."""
     lib = _lib.load()
-    B, L, D = q.shape
-    dims = SasrecDims(B, L, D, H, float(p), int(seed), ptr(seed_dev), layer)
+    dims = _sasrec_dims(q, H, p, seed, seed_dev, layer, offsets, max_len)
     dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
-    check(lib.grb_sasrec_attention_backward(C.byref(dims), ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out), ptr(lse), ptr(dout), ptr(dq), ptr(dk),
-                                            ptr(dv), stream_ptr(q.device)))
+    if offsets is None:
+        check(lib.grb_sasrec_attention_backward(C.byref(dims), ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out), ptr(lse), ptr(dout), ptr(dq),
+                                                ptr(dk), ptr(dv), stream_ptr(q.device)))
+    else:
+        check(lib.grb_sasrec_attention_backward_jagged(C.byref(dims), ptr(offsets), q.shape[0], ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out),
+                                                       ptr(lse), ptr(dout), ptr(dq), ptr(dk), ptr(dv), stream_ptr(q.device)))
     return dq, dk, dv
 
 

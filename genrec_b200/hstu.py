@@ -534,33 +534,9 @@ class HSTU(nn.Module):
         not read on the host (CUDA graphs), and the kernels keep a malformed one inside the T rows."""
         if self.precision == "fp32":
             raise RuntimeError(f"genrec_b200: {what} runs the bf16 path only; set_precision('bf16')")
-        if input_ids.dim() != 1 or input_ids.numel() == 0 or input_ids.dtype != torch.int64:
-            raise ValueError(f"{what}: input_ids must be a non-empty [T] int64 tensor, got {tuple(input_ids.shape)} {input_ids.dtype}")
-        T = input_ids.numel()
-        if not isinstance(offsets, torch.Tensor) or offsets.dim() != 1 or offsets.numel() < 2 or offsets.dtype != torch.int64:
-            raise ValueError(f"{what}: offsets must be a [B+1] int64 tensor with B >= 1")
-        if offsets.numel() - 1 > 65535:
-            raise ValueError(f"{what}: B = {offsets.numel() - 1} sequences exceeds 65535 (the attention grid's z dimension)")
-        if isinstance(max_len, bool) or not isinstance(max_len, int) or not 1 <= max_len <= 16384:
-            raise ValueError(f"{what}: max_len must be an int in [1, 16384], got {max_len!r}")
-        if timestamps is not None and tuple(timestamps.shape) != (T,):
-            raise ValueError(f"{what}: timestamps must be [{T}] like input_ids, got {tuple(timestamps.shape)}")
-        if not offsets.is_cuda:
-            o = offsets
-            if int(o[0]) != 0:
-                raise ValueError(f"{what}: offsets[0] must be 0, got {int(o[0])}")
-            lens = o[1:] - o[:-1]
-            if bool((lens < 0).any()):
-                raise ValueError(f"{what}: offsets must be non-decreasing")
-            if int(lens.max()) > max_len:
-                raise ValueError(f"{what}: a sequence of length {int(lens.max())} exceeds max_len {max_len}")
-            if int(o[-1]) > T:
-                raise ValueError(f"{what}: offsets[B] = {int(o[-1])} exceeds the {T} token rows")
-        elif offsets.device != input_ids.device:
-            raise ValueError(f"{what}: offsets must be on the CPU or on {input_ids.device}, got {offsets.device}")
-        require_cuda(input_ids)
-        ensure_device(input_ids.device)
-        return offsets.to(input_ids.device)
+        if timestamps is not None and tuple(timestamps.shape) != (input_ids.numel(),):
+            raise ValueError(f"{what}: timestamps must be [{input_ids.numel()}] like input_ids, got {tuple(timestamps.shape)}")
+        return Fn.check_jagged_batch(what, input_ids, offsets, max_len, 16384)
 
     def encode_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, timestamps: Optional[torch.Tensor] = None
                       ) -> torch.Tensor:

@@ -20,7 +20,8 @@ SITE_ATT, SITE_HID, SITE_OUT = 3, 1, 2   # dropout sites inside one block (layer
 
 
 class _BlockFn(torch.autograd.Function):
-    """One SASRecBlock (sasrec.py:152-165) + the optional trailing `x * mask` of SASRec.forward (:116)."""
+    """One SASRecBlock (sasrec.py:152-165) + the optional trailing `x * mask` of SASRec.forward (:116).  x [B, L, D] with pad [B, L],
+    or a packed batch: x [T, D], rowmask / pad [T], and cfg["offsets"] ([B+1] on the device) with cfg["max_len"]."""
 
     @staticmethod
     def forward(ctx, x, rowmask, pad, cfg, bf16w, *params):
@@ -32,7 +33,7 @@ class _BlockFn(torch.autograd.Function):
         Q, _ = Fn.linear_fwd(qb, bf16w["wq"], bq.detach(), 0)                                                    # :201-203
         K, _ = Fn.linear_fwd(xb, bf16w["wk"], bk.detach(), 0)
         V, _ = Fn.linear_fwd(xb, bf16w["wv"], bv.detach(), 0)
-        att, lse = Fn.sasrec_attention_fwd(Q, K, V, pad, H, p, seed, sd, layer)                                   # :206-240
+        att, lse = Fn.sasrec_attention_fwd(Q, K, V, pad, H, p, seed, sd, layer, cfg["offsets"], cfg["max_len"])   # :206-240
         h = att.float() + qf                                                                                      # :244 residual = normalised query
         hnb, _, st2 = Fn.layernorm_fwd(h, g2.detach(), b2.detach(), 1e-8)                                        # :163 norm2
         z1, a1 = Fn.linear_fwd(hnb, bf16w["w1"], bb1.detach(), 2, p, seed, sd, layer * 8 + SITE_HID)              # fc1 + relu + dropout
@@ -56,7 +57,7 @@ class _BlockFn(torch.autograd.Function):
         dhn, dw1, db1 = Fn.linear_bwd(dz1, w["w1"], hnb)
         dh, dg2, dbt2 = Fn.layernorm_bwd(dhn, h, st2, g2, residual=dy)
         datt = Fn.cast_rows_bf16(dh)
-        dQ, dK, dV = Fn.sasrec_attention_bwd(Q, K, V, pad, att, lse, datt, H, p, seed, sd, layer)
+        dQ, dK, dV = Fn.sasrec_attention_bwd(Q, K, V, pad, att, lse, datt, H, p, seed, sd, layer, cfg["offsets"], cfg["max_len"])
         dq, dwq, dbq = Fn.linear_bwd(dQ, w["wq"], qb, dx_residual=dh)          # + residual path through the normalised query
         dxk, dwk, dbk = Fn.linear_bwd(dK, w["wk"], xb)
         dxkv, dwv, dbv = Fn.linear_bwd(dV, w["wv"], xb, dx_residual=dxk)
@@ -187,11 +188,14 @@ class SASRecBlock(nn.Module):
         B, L, _ = x.shape
         rowmask = mask.reshape(B * L).float().contiguous()
         pad = (rowmask == 0).to(torch.uint8).view(B, L).contiguous()
+        return self._run(x, rowmask, pad, _apply_mask, _seed, _seed_dev)
+
+    def _run(self, x, rowmask, pad, apply_mask, seed, seed_dev, offsets=None, max_len=None):
         a, f = self.attention, self.ffn
         bf16w = dict(wq=Fn.cast_bf16(a.q_proj.weight), wk=Fn.cast_bf16(a.k_proj.weight), wv=Fn.cast_bf16(a.v_proj.weight),
                      w1=Fn.cast_bf16(f.fc1.weight), w2=Fn.cast_bf16(f.fc2.weight))
-        cfg = dict(H=a.num_heads, layer=self.layer_index, p=self.p if self.training else 0.0, seed=_seed, seed_dev=_seed_dev,
-                   apply_mask=_apply_mask)
+        cfg = dict(H=a.num_heads, layer=self.layer_index, p=self.p if self.training else 0.0, seed=seed, seed_dev=seed_dev,
+                   apply_mask=apply_mask, offsets=offsets, max_len=max_len)
         return _BlockFn.apply(x, rowmask, pad, cfg, bf16w, *self._params())
 
 
@@ -263,7 +267,11 @@ class SASRec(nn.Module):
             raise ValueError("log_q corrects the sampled softmax: pass negatives with it")
         if negatives is not None and targets is None:
             raise ValueError("negatives select the sampled-softmax loss, which needs targets")
-        x = self.encode(input_ids)
+        return self._head(self.encode(input_ids), targets, negatives, log_q)
+
+    def _head(self, x: torch.Tensor, targets: Optional[torch.Tensor], negatives: Optional[torch.Tensor], log_q: Optional[torch.Tensor]
+              ) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """The head of ``forward`` on x [B, L, D]: (logits [B, L, V+1] | None, loss | None) under forward's rules."""
         table = self.item_embedding.weight
         table_bf16 = Fn.cast_bf16(table)
         logits = loss = None
@@ -275,6 +283,45 @@ class SASRec(nn.Module):
         if targets is None or not self.training or self.return_train_logits:
             logits = Fn.head_logits(x, self.final_norm.weight, self.final_norm.bias, table, table_bf16, self.final_norm.eps)
         return logits, loss
+
+    def encode_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int) -> torch.Tensor:
+        """``encode`` of a packed batch: input_ids [T], offsets [B+1] int64 on the device (sequence b = rows offsets[b] ..
+        offsets[b+1]-1), max_len >= every length (<= max_seq_len) -> [T, D] fp32.  Item i of a sequence of length n takes position
+        P - n + i, P the batch's longest sequence (derived on the device), as in sasrec_collate_fn's left-padded batch."""
+        T = input_ids.numel()
+        seed, sd = self._seeds(input_ids.device)
+        p = self.emb_dropout.p if self.training else 0.0
+        x, pad = Fn.EmbedFn.apply(input_ids, self.item_embedding.weight, self.position_embedding.weight, self.embed_dim ** 0.5, 1, p,
+                                  seed, sd, None, offsets, max_len)
+        rowmask = (pad == 0).float()
+        for blk in self.blocks:
+            x = blk._run(x, rowmask, pad, True, seed, sd, offsets, max_len)
+        return x.view(T, self.embed_dim)
+
+    def forward_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, targets: Optional[torch.Tensor] = None, *,
+                       negatives: Optional[torch.Tensor] = None, log_q: Optional[torch.Tensor] = None
+                       ) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """``forward`` on a packed batch (``data.pack_jagged``): input_ids / targets [T] int64, offsets [B+1] int64 (sequence b =
+        rows offsets[b] .. offsets[b+1]-1; rows from offsets[B] to T are idle, id 0 and target 0), max_len >= every length and
+        <= max_seq_len.  Returns (logits [T, V+1] fp32 | None, loss | None) under ``forward``'s rules (dropout, the sampled head,
+        ``return_train_logits``).  Every stage runs on the T rows, none on padding.
+
+        Position rule: item i of a sequence of length n sits at position P - n + i, P the longest sequence of the batch, as in the
+        left-padded batch of sasrec_collate_fn; P is derived on the device, so every real token computes what it computes there
+        (to fp32 summation order).  Dropout masks are keyed by token row, so under dropout a packed batch draws other masks.  With
+        offsets on the CPU the batch is checked before any launch (ValueError); offsets on the device are not read on the host, so
+        a step with fixed (B, T, max_len) can be captured in a CUDA graph and replayed with new offsets, ids and targets."""
+        if negatives is None and log_q is not None:
+            raise ValueError("log_q corrects the sampled softmax: pass negatives with it")
+        if negatives is not None and targets is None:
+            raise ValueError("negatives select the sampled-softmax loss, which needs targets")
+        T = input_ids.numel()
+        if targets is not None and tuple(targets.shape) != (T,):
+            raise ValueError(f"forward_jagged: targets must be [{T}] like input_ids, got {tuple(targets.shape)}")
+        offsets = Fn.check_jagged_batch("forward_jagged", input_ids, offsets, max_len, self.max_seq_len)   # the position table's rows
+        x = self.encode_jagged(input_ids, offsets, max_len)
+        logits, loss = self._head(x.view(1, T, self.embed_dim), targets.view(1, T) if targets is not None else None, negatives, log_q)
+        return (logits.view(T, -1) if logits is not None else None), loss
 
     @torch.no_grad()
     def predict(self, input_ids: torch.Tensor, top_k: int = 10) -> torch.Tensor:
@@ -316,3 +363,21 @@ class SASRec(nn.Module):
         x = self.encode(input_ids)
         return Fn.head_rank_metrics(x[:, -1, :], self.final_norm.weight, self.final_norm.bias, Fn.cast_bf16(self.item_embedding.weight),
                                     self.final_norm.eps, targets, metrics, exclude)
+
+    @torch.no_grad()
+    def evaluate_batch_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, targets: torch.Tensor,
+                              metrics: Optional[torch.Tensor] = None, *, exclude: Optional[torch.Tensor] = None, want_ranks: bool = False):
+        """``evaluate_batch`` on a packed batch (input_ids [T], offsets [B+1], max_len as in ``forward_jagged``; targets [B] the
+        held-out item of each sequence): each sequence is ranked from its last row, offsets[b+1] - 1, and the metrics are accumulated
+        into ``metrics`` on the device.  A sequence of length 0 is not ranked (rank 0, adds nothing).  With ``want_ranks`` it returns
+        (metrics, ranks [B] int32)."""
+        B, T = offsets.numel() - 1, input_ids.numel()
+        if tuple(targets.shape) != (B,):
+            raise ValueError(f"evaluate_batch_jagged: targets must be [{B}] (one per sequence), got {tuple(targets.shape)}")
+        offsets = Fn.check_jagged_batch("evaluate_batch_jagged", input_ids, offsets, max_len, self.max_seq_len)
+        Fn.check_exclude_arg(exclude, B, input_ids.device)
+        x = self.encode_jagged(input_ids, offsets, max_len)
+        last = (offsets[1:] - 1).clamp(0, T - 1)
+        ranked = torch.where(offsets[1:] > offsets[:-1], targets, torch.zeros_like(targets))
+        return Fn.head_rank_metrics(x.index_select(0, last), self.final_norm.weight, self.final_norm.bias,
+                                    Fn.cast_bf16(self.item_embedding.weight), self.final_norm.eps, ranked, metrics, exclude, want_ranks)

@@ -140,6 +140,34 @@ int grb_hstu_layer_backward_jagged(const grb_hstu_dims* d, const grb_hstu_layer_
                                    int T, const float* dy, const void* saved, float* dx, const grb_hstu_layer_grads* g, void* workspace,
                                    void* stream);
 
+/* ------------------------------------------------------------------------------------------------ packed (jagged) SASRec batches
+ * The packed layout above (token rows [T, D], device offsets [B+1], host max_len and T, idle rows offsets[B] .. T-1), for SASRec.
+ * Position rule: sasrec_collate_fn left-pads every sequence of a batch to P = its longest history, and SASRec adds
+ * position_embedding(arange(P)), so item i (0-based) of a sequence of packed length n sits at position P - n + i.  P is a property
+ * of the whole batch: here it is the longest sequence of the packed batch after each one is clamped to [0, T) and to max_len,
+ * derived on the device from offsets (never from the host max_len), so a captured step replayed with new offsets takes the new P.
+ * With this rule every real token computes what it computes in the padded batch of the same users, to fp32 summation order;
+ * only dropout differs (its masks are keyed by token row).  A malformed device offsets gives wrong numbers, never an access
+ * outside the T rows (or outside the max_len rows of the position table).  B <= 65535.
+ *   grb_embed_forward_jagged: x [T, D] = drop(E[id] * scale + pos[P - n_b + i]) * (mask_pad_rows ? id != 0 : 1) on the rows of
+ *       sequence b; rows outside every sequence get x = 0 and pad = 1 whatever their id.  pos_table has >= max_len rows.  pad [T]
+ *       (nullable) as grb_embed_forward; positions [T] int32 (out) = each token's position row, -1 on the idle rows.
+ *   grb_embed_backward_jagged: dtable as grb_embed_backward on [1, T] rows (order: the T token indices sorted by id, stable; give the
+ *       idle rows id 0, as pack_jagged does, since their x does not depend on the table); dpos_table (nullable) row l < P gets, in
+ *       ascending sequence order, the dropped dx of the token at position l of every sequence that reaches it, id-0 tokens left out,
+ *       then one add per element: the terms and the order of grb_embed_backward on the padded batch, so equal dx give equal bits.
+ *       scratch [T, D] fp32.
+ *   grb_sasrec_attention_*_jagged: grb_sasrec_attention_* on the packed rows, with d->B = the sequence count and d->L = max_len;
+ *       q, k, v, out, dout, dq, dk, dv [T, D], pad [T], lse [H, T] (per token).  Under dropout the mask is keyed by the query's
+ *       token row, the head and the key's index j within its sequence: row key (row * H + h), column j.  The idle rows of out and
+ *       of dq | dk | dv are written as exact zeros. */
+int grb_embed_forward_jagged(const int64_t* ids, const float* table, const float* pos_table, const int64_t* offsets, int B, int T,
+                             int max_len, int D, float scale, int mask_pad_rows, float dropout_p, uint64_t seed, const uint64_t* seed_dev,
+                             float* x, uint8_t* pad, int32_t* positions, void* stream);
+int grb_embed_backward_jagged(const int64_t* ids, const int64_t* order, const float* dx, float* dtable, float* dpos_table,
+                              const int64_t* offsets, int B, int T, int max_len, int D, float scale, int mask_pad_rows, float dropout_p,
+                              uint64_t seed, const uint64_t* seed_dev, float* scratch, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ cached incremental inference
  * Extends `predict` / evaluation (hstu.py:150-157, trainers/hstu_trainer.py:55-81), which rerun the whole history for every new
  * item: a cache keeps, per layer, the K | V rows of every item seen so far for a batch of B users, and a chunk of n new slots per
@@ -315,6 +343,12 @@ int grb_sasrec_attention_forward(const grb_sasrec_dims* d, const void* q, const 
 int grb_sasrec_attention_backward(const grb_sasrec_dims* d, const void* q, const void* k, const void* v,
                                   const uint8_t* pad, const void* out, const float* lse, const void* dout, void* dq,
                                   void* dk, void* dv, void* stream);
+/* packed batches: see "packed (jagged) SASRec batches" above */
+int grb_sasrec_attention_forward_jagged(const grb_sasrec_dims* d, const int64_t* offsets, int T, const void* q, const void* k,
+                                        const void* v, const uint8_t* pad, void* out, float* lse, void* stream);
+int grb_sasrec_attention_backward_jagged(const grb_sasrec_dims* d, const int64_t* offsets, int T, const void* q, const void* k,
+                                         const void* v, const uint8_t* pad, const void* out, const float* lse, const void* dout,
+                                         void* dq, void* dk, void* dv, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ generic fused linear pieces
  * (used by the SASRec block and by tests)   act: 0 none, 1 silu, 2 relu */
