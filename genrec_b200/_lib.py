@@ -93,6 +93,14 @@ SIGNATURES = {
     "grb_hstu_layer_extend_paged_workspace_bytes": (c_size_t, [P(HstuDims), P(HstuPool)]),
     "grb_hstu_layer_extend_paged": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuPool), c_int, c_void_p, c_void_p, c_void_p, c_int,
                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_hstu_cache_append_jagged": (c_int, [P(HstuCache)] + [c_void_p] * 3 + [c_int] * 3 + [c_void_p] * 3),
+    "grb_hstu_pool_append_jagged": (c_int, [P(HstuPool), c_void_p, c_int] + [c_void_p] * 3 + [c_int, c_int] + [c_void_p] * 4),
+    "grb_hstu_layer_extend_workspace_bytes_jagged": (c_size_t, [P(HstuDims), c_int, c_int]),
+    "grb_hstu_layer_extend_jagged": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuCache), c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                             c_int] + [c_void_p] * 5),
+    "grb_hstu_layer_extend_paged_workspace_bytes_jagged": (c_size_t, [P(HstuDims), P(HstuPool), c_int]),
+    "grb_hstu_layer_extend_paged_jagged": (c_int, [P(HstuDims), P(HstuLayerParams), P(HstuPool), c_int, c_void_p, c_void_p, c_int,
+                                                   c_void_p, c_void_p, c_int] + [c_void_p] * 5),
     "grb_collate_jagged": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_pack_jagged": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p] * 6),
     "grb_embed_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int,

@@ -493,14 +493,13 @@ int check_extend(const grb_hstu_dims* d, int capacity) {
                 (long long)d->B * ((d->L + ATT_BLK - 1) / ATT_BLK));
     return 0;
 }
-// workspace: the forward's activation layout for the chunk's B * n rows, then the [splits, B * n, D] fp32 attention partials
+// workspace: the forward's activation layout for the chunk's T rows (B * n padded), then the [splits, T, D] fp32 attention partials
 struct ExtendWork {
     LayerSaved sv;
     float* part;
     size_t bytes;
 };
-ExtendWork carve_extend(void* base, const grb_hstu_dims* d, int capacity) {
-    const size_t T = (size_t)d->B * d->L;
+ExtendWork carve_extend(void* base, const grb_hstu_dims* d, int capacity, size_t T) {
     ExtendWork w;
     w.sv = carve_saved(base, T, d->D);
     const int split = extend_split(d, capacity);
@@ -509,20 +508,20 @@ ExtendWork carve_extend(void* base, const grb_hstu_dims* d, int capacity) {
     w.bytes = w.sv.bytes + align_up(nsplit * T * d->D * 4);
     return w;
 }
-template <int DH, bool UNIFORM, bool TIMED>
+template <int DH, bool UNIFORM, bool TIMED, bool JAGGED>
 int launch_attn_extend(const HstuExtendArgs& a, int nsplit, cudaStream_t st) {
-    const size_t smem = sizeof(ExtSmem<DH>) + align_up((size_t)(a.bias.npos * 64 + 1) * 4, 16);
+    const size_t smem = sizeof(ExtSmem<DH>) + ext_table_bytes(a.bias.npos) + (JAGGED ? sizeof(long long) : 0);
     const dim3 grid(nsplit, a.H, a.B * ((a.n + ATT_BLK - 1) / ATT_BLK));
-    GRB_LAUNCH((hstu_attn_extend_kernel<DH, UNIFORM, TIMED>), grid, ATT_THREADS, smem, st, a);
+    GRB_LAUNCH((hstu_attn_extend_kernel<DH, UNIFORM, TIMED, JAGGED>), grid, ATT_THREADS, smem, st, a);
     return 0;
 }
-template <int DH>
+template <int DH, bool JAGGED>
 int dispatch_attn_extend(const HstuExtendArgs& a, int nsplit, cudaStream_t st) {
     const bool uni = a.pos_bucket == nullptr, timed = a.bias.wtime != nullptr;
-    if (uni && timed) return launch_attn_extend<DH, true, true>(a, nsplit, st);
-    if (uni) return launch_attn_extend<DH, true, false>(a, nsplit, st);
-    if (timed) return launch_attn_extend<DH, false, true>(a, nsplit, st);
-    return launch_attn_extend<DH, false, false>(a, nsplit, st);
+    if (uni && timed) return launch_attn_extend<DH, true, true, JAGGED>(a, nsplit, st);
+    if (uni) return launch_attn_extend<DH, true, false, JAGGED>(a, nsplit, st);
+    if (timed) return launch_attn_extend<DH, false, true, JAGGED>(a, nsplit, st);
+    return launch_attn_extend<DH, false, false, JAGGED>(a, nsplit, st);
 }
 
 // Where one layer's cached K | V lives: the dense cache (users and page table null, page_size = capacity) or a pool.
@@ -574,24 +573,30 @@ int block_steps_out(const grb_hstu_layer_params* p, const float* x, float* y, co
     return 0;
 }
 
-// the steps of grb_hstu_layer_forward on the chunk's rows, with the attention against the cache in place of step 3
-int layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const ExtendKv& c, const int32_t* positions,
-                 const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr, const float* x, float* y, void* workspace,
-                 cudaStream_t st) {
+// the steps of grb_hstu_layer_forward on the chunk's T rows, with the attention against the cache in place of step 3.  offsets
+// null: a padded [B, L] chunk (T = B * L); otherwise the packed chunk of check_jagged (L = max_len).
+int layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const ExtendKv& c, const int64_t* offsets, int T,
+                 const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr, const float* x, float* y,
+                 void* workspace, cudaStream_t st) {
     GRB_TRY(check_layer_params(p));
     GRB_REQUIRE(pos_bucket != nullptr || (pos_bucket0 >= 0 && pos_bucket0 < d->npos), "pos_bucket0 %d out of range", pos_bucket0);
     const bool timed = d->ntime > 0 && p->time_table != nullptr;
     GRB_REQUIRE(!timed || time_thr != nullptr, "time_thr is null");
     GRB_REQUIRE(aligned16(x) && aligned16(y) && aligned16(workspace) && aligned16(c.kv), "buffers must be 16-byte aligned");
-    const int T = d->B * d->L, D = d->D, cap = c.cap;
-    ExtendWork w = carve_extend(workspace, d, cap);
+    const int D = d->D, cap = c.cap;
+    const long long* offs = reinterpret_cast<const long long*>(offsets);
+    ExtendWork w = carve_extend(workspace, d, cap, (size_t)T);
     LayerSaved& sv = w.sv;
 
     GRB_TRY(block_steps_in(p, x, sv, T, D, st));
     {
-        const size_t pieces = (size_t)T * (2 * D / 8);
-        GRB_LAUNCH(hstu_kv_scatter_kernel, (unsigned)((pieces + 255) / 256), 256, 0, st, (const bf16*)sv.P, (const int*)positions, c.users, T,
-                   d->L, D, c.pg, c.kv);
+        const unsigned grid = (unsigned)(((size_t)T * (2 * D / 8) + 255) / 256);
+        if (offsets)
+            GRB_LAUNCH(hstu_kv_scatter_kernel<true>, grid, 256, 0, st, (const bf16*)sv.P, (const int*)positions, c.users, T, d->L, D, c.pg,
+                       c.kv, offs, d->B);
+        else
+            GRB_LAUNCH(hstu_kv_scatter_kernel<false>, grid, 256, 0, st, (const bf16*)sv.P, (const int*)positions, c.users, T, d->L, D, c.pg,
+                       c.kv, offs, 0);
     }
     {
         HstuExtendArgs a;
@@ -608,8 +613,11 @@ int layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const E
         a.B = d->B; a.n = d->L; a.H = d->H; a.D = D; a.cap = cap;
         a.split = extend_split(d, cap);
         a.part = w.part;
+        a.offsets = offs; a.T = T;
         const int nsplit = (cap + a.split - 1) / a.split;
-        GRB_TRY(with_head_dim(D / d->H, [&](auto DH) { return dispatch_attn_extend<DH>(a, nsplit, st); }));
+        GRB_TRY(with_head_dim(D / d->H, [&](auto DH) {
+            return offsets ? dispatch_attn_extend<DH, true>(a, nsplit, st) : dispatch_attn_extend<DH, false>(a, nsplit, st);
+        }));
         const size_t quads = (size_t)T * D / 4;
         GRB_LAUNCH(hstu_extend_combine_kernel, (unsigned)((quads + 255) / 256), 256, 0, st, (const float*)w.part, (const int*)positions, T, D,
                    a.split, sv.O);
@@ -738,6 +746,74 @@ int layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const
     });
 }
 
+// hstu_cache_append_kernel on a padded [B, n] chunk (offsets null) or on a packed chunk of T token rows (n = max_len), whose
+// rows in no sequence keep position -1
+int cache_append(const int64_t* ids, const int64_t* ts, const int64_t* users, const int32_t* room, int B, int n, int cap, KvPages pg,
+                 int64_t* cache_ts, int32_t* lengths, uint8_t* overflow, int32_t* positions, int32_t* last_row, const int64_t* offsets, int T,
+                 cudaStream_t st) {
+    const long long *i = reinterpret_cast<const long long*>(ids), *t = reinterpret_cast<const long long*>(ts),
+                    *u = reinterpret_cast<const long long*>(users), *o = reinterpret_cast<const long long*>(offsets);
+    long long* cts = reinterpret_cast<long long*>(cache_ts);
+    if (offsets) {
+        GRB_CUDA(cudaMemsetAsync(positions, 0xff, (size_t)T * sizeof(int32_t), st));
+        GRB_LAUNCH(hstu_cache_append_kernel<true>, (unsigned)((B + 3) / 4), 128, 0, st, i, t, u, (const int*)room, B, n, cap, pg, cts,
+                   lengths, overflow, positions, last_row, o, T);
+    } else {
+        GRB_LAUNCH(hstu_cache_append_kernel<false>, (unsigned)((B + 3) / 4), 128, 0, st, i, t, u, (const int*)room, B, n, cap, pg, cts,
+                   lengths, overflow, positions, last_row, o, 0);
+    }
+    return 0;
+}
+// the pages a chunk needs, then its positions: grb_hstu_pool_append (offsets null) or grb_hstu_pool_append_jagged
+int pool_append(const grb_hstu_pool* pool, const int64_t* users, int B, const int64_t* input_ids, const int64_t* timestamps,
+                const int64_t* offsets, int T, int n, int32_t* positions, int32_t* last_row, int32_t* room, cudaStream_t st) {
+    GRB_TRY(check_pool(pool));
+    GRB_REQUIRE(users && input_ids && positions && last_row && room, "null argument");
+    GRB_REQUIRE(pool->timestamps && pool->page_table && pool->lengths && pool->overflow && pool->free_stack && pool->free_top &&
+                    pool->errors && pool->row_of, "null pool pointer");
+    GRB_REQUIRE(B > 0 && n > 0, "bad shape B=%d n=%d", B, n);
+    HstuPoolArgs a = pool_args(pool, users, B);
+    a.ids = reinterpret_cast<const long long*>(input_ids); a.n = n;
+    a.room = room;
+    const long long* offs = reinterpret_cast<const long long*>(offsets);
+    if (offsets) GRB_LAUNCH(hstu_pool_alloc_kernel<true>, 1, POOL_THREADS, 0, st, a, offs, T);
+    else GRB_LAUNCH(hstu_pool_alloc_kernel<false>, 1, POOL_THREADS, 0, st, a, offs, 0);
+    return cache_append(input_ids, timestamps, users, room, B, n, pool->max_items, KvPages{pool->page_table, pool_pt_ld(pool), pool->page_size},
+                        pool->timestamps, pool->lengths, pool->overflow, positions, last_row, offsets, T, st);
+}
+int check_jagged_chunk(int B, const int64_t* offsets, int T, int max_len) {
+    GRB_REQUIRE(offsets != nullptr, "offsets is null");
+    GRB_REQUIRE(B >= 1 && B <= 65535 && T >= 1 && max_len >= 1, "bad packed chunk B=%d T=%d max_len=%d", B, T, max_len);
+    return 0;
+}
+int dense_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_cache* c, int layer, const int64_t* offsets, int T,
+                 const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr, const float* x, float* y,
+                 void* workspace, cudaStream_t st) {
+    GRB_REQUIRE(c != nullptr, "null cache");
+    GRB_TRY(check_extend(d, c->capacity));
+    GRB_REQUIRE(p && positions && x && y && workspace && c->kv && c->timestamps, "null argument");
+    GRB_REQUIRE(c->B == d->B, "cache holds %d users, dims say B=%d", c->B, d->B);
+    GRB_REQUIRE(layer >= 0 && layer < c->num_layers, "layer %d out of range [0, %d)", layer, c->num_layers);
+    if (offsets) GRB_TRY(check_jagged(d, offsets, T));
+    const int cap = c->capacity;
+    ExtendKv kv{static_cast<bf16*>(c->kv) + (size_t)layer * d->B * cap * 2 * d->D, reinterpret_cast<const long long*>(c->timestamps),
+                nullptr, KvPages{nullptr, 1, cap}, cap};
+    return layer_extend(d, p, kv, offsets, T, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace, st);
+}
+int paged_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_pool* pool, int layer, const int64_t* users,
+                 const int64_t* offsets, int T, const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr,
+                 const float* x, float* y, void* workspace, cudaStream_t st) {
+    GRB_TRY(check_pool(pool));
+    GRB_TRY(check_extend(d, pool->max_items));
+    GRB_REQUIRE(p && users && positions && x && y && workspace && pool->kv && pool->timestamps && pool->page_table, "null argument");
+    GRB_REQUIRE(layer >= 0 && layer < pool->num_layers, "layer %d out of range [0, %d)", layer, pool->num_layers);
+    if (offsets) GRB_TRY(check_jagged(d, offsets, T));
+    ExtendKv kv{static_cast<bf16*>(pool->kv) + (size_t)layer * pool->num_pages * pool->page_size * 2 * d->D,
+                reinterpret_cast<const long long*>(pool->timestamps), reinterpret_cast<const long long*>(users),
+                KvPages{pool->page_table, pool_pt_ld(pool), pool->page_size}, pool->max_items};
+    return layer_extend(d, p, kv, offsets, T, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace, st);
+}
+
 }  // namespace
 
 extern "C" {
@@ -772,30 +848,30 @@ int grb_hstu_cache_append(const grb_hstu_cache* c, const int64_t* input_ids, con
     GRB_REQUIRE(c->timestamps && c->lengths && c->overflow, "null cache pointer");
     GRB_REQUIRE(c->B > 0 && n > 0, "bad shape B=%d n=%d", c->B, n);
     GRB_REQUIRE(c->capacity >= 1 && c->capacity <= 16384, "cache capacity %d out of range [1, 16384]", c->capacity);
-    GRB_LAUNCH(hstu_cache_append_kernel, (unsigned)((c->B + 3) / 4), 128, 0, static_cast<cudaStream_t>(stream),
-               reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(timestamps), (const long long*)nullptr,
-               (const int*)nullptr, c->B, n, c->capacity, KvPages{nullptr, 1, c->capacity}, reinterpret_cast<long long*>(c->timestamps),
-               c->lengths, c->overflow, positions, last_row);
-    return 0;
+    return cache_append(input_ids, timestamps, nullptr, nullptr, c->B, n, c->capacity, KvPages{nullptr, 1, c->capacity}, c->timestamps,
+                        c->lengths, c->overflow, positions, last_row, nullptr, 0, static_cast<cudaStream_t>(stream));
+}
+int grb_hstu_cache_append_jagged(const grb_hstu_cache* c, const int64_t* input_ids, const int64_t* timestamps, const int64_t* offsets,
+                                 int B, int T, int max_len, int32_t* positions, int32_t* last_row, void* stream) {
+    GRB_REQUIRE(c && input_ids && positions && last_row, "null argument");
+    GRB_REQUIRE(c->timestamps && c->lengths && c->overflow, "null cache pointer");
+    GRB_TRY(check_jagged_chunk(B, offsets, T, max_len));
+    GRB_REQUIRE(c->B == B, "cache holds %d users, the chunk has B=%d sequences", c->B, B);
+    GRB_REQUIRE(c->capacity >= 1 && c->capacity <= 16384, "cache capacity %d out of range [1, 16384]", c->capacity);
+    return cache_append(input_ids, timestamps, nullptr, nullptr, B, max_len, c->capacity, KvPages{nullptr, 1, c->capacity}, c->timestamps,
+                        c->lengths, c->overflow, positions, last_row, offsets, T, static_cast<cudaStream_t>(stream));
 }
 
 int grb_hstu_pool_append(const grb_hstu_pool* pool, const int64_t* users, int B, const int64_t* input_ids, const int64_t* timestamps,
                          int n, int32_t* positions, int32_t* last_row, int32_t* room, void* stream) {
-    GRB_TRY(check_pool(pool));
-    GRB_REQUIRE(users && input_ids && positions && last_row && room, "null argument");
-    GRB_REQUIRE(pool->timestamps && pool->page_table && pool->lengths && pool->overflow && pool->free_stack && pool->free_top &&
-                    pool->errors && pool->row_of, "null pool pointer");
-    GRB_REQUIRE(B > 0 && n > 0, "bad shape B=%d n=%d", B, n);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    HstuPoolArgs a = pool_args(pool, users, B);
-    a.ids = reinterpret_cast<const long long*>(input_ids); a.n = n;
-    a.room = room;
-    GRB_LAUNCH(hstu_pool_alloc_kernel, 1, POOL_THREADS, 0, st, a);
-    GRB_LAUNCH(hstu_cache_append_kernel, (unsigned)((B + 3) / 4), 128, 0, st, reinterpret_cast<const long long*>(input_ids),
-               reinterpret_cast<const long long*>(timestamps), reinterpret_cast<const long long*>(users), (const int*)room, B, n,
-               pool->max_items, KvPages{pool->page_table, pool_pt_ld(pool), pool->page_size}, reinterpret_cast<long long*>(pool->timestamps),
-               pool->lengths, pool->overflow, positions, last_row);
-    return 0;
+    return pool_append(pool, users, B, input_ids, timestamps, nullptr, 0, n, positions, last_row, room, static_cast<cudaStream_t>(stream));
+}
+int grb_hstu_pool_append_jagged(const grb_hstu_pool* pool, const int64_t* users, int B, const int64_t* input_ids, const int64_t* timestamps,
+                                const int64_t* offsets, int T, int max_len, int32_t* positions, int32_t* last_row, int32_t* room,
+                                void* stream) {
+    GRB_TRY(check_jagged_chunk(B, offsets, T, max_len));
+    return pool_append(pool, users, B, input_ids, timestamps, offsets, T, max_len, positions, last_row, room,
+                       static_cast<cudaStream_t>(stream));
 }
 
 int grb_hstu_pool_release(const grb_hstu_pool* pool, const int64_t* users, int B, float* last_hidden, int D, void* stream) {
@@ -813,39 +889,48 @@ int grb_hstu_pool_release(const grb_hstu_pool* pool, const int64_t* users, int B
 
 size_t grb_hstu_layer_extend_workspace_bytes(const grb_hstu_dims* d, int capacity) {
     if (check_extend(d, capacity)) return 0;
-    return carve_extend(nullptr, d, capacity).bytes;
+    return carve_extend(nullptr, d, capacity, (size_t)d->B * d->L).bytes;
+}
+size_t grb_hstu_layer_extend_workspace_bytes_jagged(const grb_hstu_dims* d, int capacity, int T) {
+    if (check_extend(d, capacity) || T < 1) return 0;
+    return carve_extend(nullptr, d, capacity, (size_t)T).bytes;
 }
 
 int grb_hstu_layer_extend(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_cache* c, int layer,
                           const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0, const int64_t* time_thr,
                           const float* x, float* y, void* workspace, void* stream) {
-    GRB_REQUIRE(c != nullptr, "null cache");
-    GRB_TRY(check_extend(d, c->capacity));
-    GRB_REQUIRE(p && positions && x && y && workspace && c->kv && c->timestamps, "null argument");
-    GRB_REQUIRE(c->B == d->B, "cache holds %d users, dims say B=%d", c->B, d->B);
-    GRB_REQUIRE(layer >= 0 && layer < c->num_layers, "layer %d out of range [0, %d)", layer, c->num_layers);
-    const int cap = c->capacity;
-    ExtendKv kv{static_cast<bf16*>(c->kv) + (size_t)layer * d->B * cap * 2 * d->D, reinterpret_cast<const long long*>(c->timestamps),
-                nullptr, KvPages{nullptr, 1, cap}, cap};
-    return layer_extend(d, p, kv, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace, static_cast<cudaStream_t>(stream));
+    return dense_extend(d, p, c, layer, nullptr, d ? d->B * d->L : 0, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace,
+                        static_cast<cudaStream_t>(stream));
+}
+int grb_hstu_layer_extend_jagged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_cache* c, int layer,
+                                 const int64_t* offsets, int T, const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0,
+                                 const int64_t* time_thr, const float* x, float* y, void* workspace, void* stream) {
+    GRB_REQUIRE(offsets != nullptr, "offsets is null");
+    return dense_extend(d, p, c, layer, offsets, T, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace,
+                        static_cast<cudaStream_t>(stream));
 }
 
 size_t grb_hstu_layer_extend_paged_workspace_bytes(const grb_hstu_dims* d, const grb_hstu_pool* pool) {
     if (check_pool(pool) || check_extend(d, pool->max_items)) return 0;
-    return carve_extend(nullptr, d, pool->max_items).bytes;
+    return carve_extend(nullptr, d, pool->max_items, (size_t)d->B * d->L).bytes;
+}
+size_t grb_hstu_layer_extend_paged_workspace_bytes_jagged(const grb_hstu_dims* d, const grb_hstu_pool* pool, int T) {
+    if (check_pool(pool) || check_extend(d, pool->max_items) || T < 1) return 0;
+    return carve_extend(nullptr, d, pool->max_items, (size_t)T).bytes;
 }
 
 int grb_hstu_layer_extend_paged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_pool* pool, int layer,
                                 const int64_t* users, const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0,
                                 const int64_t* time_thr, const float* x, float* y, void* workspace, void* stream) {
-    GRB_TRY(check_pool(pool));
-    GRB_TRY(check_extend(d, pool->max_items));
-    GRB_REQUIRE(p && users && positions && x && y && workspace && pool->kv && pool->timestamps && pool->page_table, "null argument");
-    GRB_REQUIRE(layer >= 0 && layer < pool->num_layers, "layer %d out of range [0, %d)", layer, pool->num_layers);
-    ExtendKv kv{static_cast<bf16*>(pool->kv) + (size_t)layer * pool->num_pages * pool->page_size * 2 * d->D,
-                reinterpret_cast<const long long*>(pool->timestamps), reinterpret_cast<const long long*>(users),
-                KvPages{pool->page_table, pool_pt_ld(pool), pool->page_size}, pool->max_items};
-    return layer_extend(d, p, kv, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace, static_cast<cudaStream_t>(stream));
+    return paged_extend(d, p, pool, layer, users, nullptr, d ? d->B * d->L : 0, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace,
+                        static_cast<cudaStream_t>(stream));
+}
+int grb_hstu_layer_extend_paged_jagged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_pool* pool, int layer,
+                                       const int64_t* users, const int64_t* offsets, int T, const int32_t* positions, const uint8_t* pos_bucket,
+                                       int pos_bucket0, const int64_t* time_thr, const float* x, float* y, void* workspace, void* stream) {
+    GRB_REQUIRE(offsets != nullptr, "offsets is null");
+    return paged_extend(d, p, pool, layer, users, offsets, T, positions, pos_bucket, pos_bucket0, time_thr, x, y, workspace,
+                        static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -41,35 +41,43 @@ struct KvPages {
 // The room is room[b] (the pool: what the allocation left the user, -1 = a rejected row, treated as all padding) or `cap`
 // without a room list.  The chunk's timestamps are written into the cache, len[u] becomes min(len[u] + valid, room) and
 // last_row[b] is the chunk row of the user's last valid item, or -1.
+// JAGGED (a packed chunk of T token rows, n = max_len): sequence b is the token rows of seq_span(offsets, T, n, b), ids / ts / pos
+// are [T], and last_row[b] is the token row of the user's last valid item.  The caller sets pos to -1 beforehand: rows in no
+// sequence (idle rows) are not visited.
+template <bool JAGGED>
 __global__ void __launch_bounds__(128) hstu_cache_append_kernel(const long long* __restrict__ ids, const long long* __restrict__ ts,
                                                                 const long long* __restrict__ users, const int* __restrict__ room, int B,
                                                                 int n, int cap, KvPages pg, long long* __restrict__ cache_ts,
                                                                 int* __restrict__ len, uint8_t* __restrict__ overflow, int* __restrict__ pos,
-                                                                int* __restrict__ last_row) {
+                                                                int* __restrict__ last_row, const long long* __restrict__ offsets, int T) {
     pdl_wait();
     const int b = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (b >= B) return;
+    long long tok0 = 0;
+    int rows = n;
+    if constexpr (JAGGED) seq_span(offsets, T, n, b, tok0, rows);
+    auto at = [&](int r) { return JAGGED ? (size_t)tok0 + r : (size_t)b * n + r; };   // the token row of row r of the sequence
     const int lim = room ? room[b] : cap;
     if (lim < 0) {
-        for (int r = lane; r < n; r += 32) pos[(size_t)b * n + r] = -1;
+        for (int r = lane; r < rows; r += 32) pos[at(r)] = -1;
         if (lane == 0) last_row[b] = -1;
         return;
     }
     const int u = users ? (int)users[b] : b;
     const int base = len[u];
     int count = 0, last = -1;
-    for (int r0 = 0; r0 < n; r0 += 32) {
+    for (int r0 = 0; r0 < rows; r0 += 32) {
         const int r = r0 + lane;
-        const bool valid = r < n && ids[(size_t)b * n + r] != 0;
+        const bool valid = r < rows && ids[at(r)] != 0;
         const unsigned m = __ballot_sync(0xffffffffu, valid);
         const int q = base + count + __popc(m & ((1u << lane) - 1u));
-        if (r < n) {
+        if (r < rows) {
             int p = -1;
             if (valid && q < lim) {
                 p = q;
-                cache_ts[pg.row(u, q)] = ts ? ts[(size_t)b * n + r] : 0;
+                cache_ts[pg.row(u, q)] = ts ? ts[at(r)] : 0;
             }
-            pos[(size_t)b * n + r] = p;
+            pos[at(r)] = p;
         }
         if (m) last = r0 + 31 - __clz((int)m);
         count += __popc(m);
@@ -78,15 +86,33 @@ __global__ void __launch_bounds__(128) hstu_cache_append_kernel(const long long*
         const long long total = (long long)base + count;
         len[u] = total > lim ? lim : (int)total;
         if (total > lim) overflow[u] = 1;
-        last_row[b] = last;
+        last_row[b] = JAGGED && last >= 0 ? (int)tok0 + last : last;
     }
 }
 
+// The sequence b of a packed batch whose rows seq_span(offsets, T, L, b) hold token row `row`, or -1 for an idle row: a binary
+// search for the last b with offsets[b] <= row, then a check against that sequence's clamped span (a malformed device offsets
+// gives some sequence or -1, never a row outside the span).
+GRB_DEVINL int jagged_seq_of(const long long* offsets, int B, int T, int L, int row) {
+    int lo = 0, hi = B - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (offsets[mid] <= row) lo = mid;
+        else hi = mid - 1;
+    }
+    long long tok0;
+    int len;
+    seq_span(offsets, T, L, lo, tok0, len);
+    return row >= tok0 && row < tok0 + len ? lo : -1;
+}
+
 // K | V row of every chunk row with pos >= 0 into the cache row of (users[b], pos): [0, D) = K, [D, 2D) = V.
-// P = [U | V | Q | K] [B*n, 4D] bf16.  One thread per 16-byte piece.
+// P = [U | V | Q | K] [B*n, 4D] bf16.  One thread per 16-byte piece.  JAGGED (P [T, 4D] of B sequences, n = max_len): the row's
+// sequence comes from jagged_seq_of, searched only for rows that have a position.
+template <bool JAGGED>
 __global__ void __launch_bounds__(256) hstu_kv_scatter_kernel(const bf16* __restrict__ P, const int* __restrict__ pos,
                                                               const long long* __restrict__ users, int T, int n, int D, KvPages pg,
-                                                              bf16* __restrict__ kv) {
+                                                              bf16* __restrict__ kv, const long long* __restrict__ offsets, int B) {
     pdl_wait();
     const int per_row = 2 * D / 8;
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -94,7 +120,8 @@ __global__ void __launch_bounds__(256) hstu_kv_scatter_kernel(const bf16* __rest
     const int row = (int)(idx / per_row), c = (int)(idx % per_row) * 8;   // column of the cache row
     const int p = pos[row];
     if (p < 0) return;
-    const int b = row / n;
+    const int b = JAGGED ? jagged_seq_of(offsets, B, T, n, row) : row / n;
+    if (JAGGED && b < 0) return;
     const int u = users ? (int)users[b] : b;
     const int src = c < D ? 3 * D + c : c;                                // K = P[:, 3D:4D) ; V = P[:, D:2D)
     *reinterpret_cast<uint4*>(kv + pg.row(u, p) * 2 * D + c) = *reinterpret_cast<const uint4*>(P + (size_t)row * 4 * D + src);
@@ -112,7 +139,9 @@ struct HstuExtendArgs {
     HstuBiasArgs bias;                 // wpos / wtime / npos / ntime (bias_index unused)
     int B, n, H, D, cap;               // cap: most items a user can hold
     int split;                         // keys per CTA, a multiple of ATT_BLK ; grid.x = ceil(cap / split)
-    float* part;                       // [grid.x, B * n, D] fp32 partial outputs
+    float* part;                       // [grid.x, B * n, D] fp32 partial outputs ; a packed chunk: [grid.x, T, D]
+    const long long* offsets;          // null: a padded [B, n] chunk ; else sequence b is token rows seq_span(offsets, T, n, b)
+    int T;                             // token rows of a packed chunk (n = max_len)
 };
 
 template <int DH>
@@ -124,12 +153,23 @@ struct ExtSmem {
     long long thr[ATT_MAX_BUCKETS + 1];
     int pmax;
 };
-// dynamic tail: float wcomb[npos * 64 + 1] (att_build_table)
+// dynamic tail: float wcomb[npos * 64 + 1] (att_build_table) ; JAGGED: then, 16-byte aligned, the sequence's first token row
+__host__ __device__ inline size_t ext_table_bytes(int npos) { return ((size_t)(npos * 64 + 1) * 4 + 15) / 16 * 16; }
 
 // grid (ceil(cap / split), H, B * ceil(n / 64)), 128 threads: 64 chunk rows of one user and head against the keys
-// [split * x, split * (x + 1)) of the user's cache.  Tiles that lie beyond every row's position are skipped.
+// [split * x, split * (x + 1)) of the user's cache.  Tiles that lie beyond every row's position are skipped.  JAGGED: the
+// tile's rows are those of sequence b from its first token row, and a tile past the sequence's end exits.
+// CTAs per SM of the padded instantiation (ptxas -v registers, 128 threads), which the packed one is held to: its sequence's
+// first row and length come from a load, not from the launch, and ptxas otherwise spends more registers on them and loses an
+// SM slot.  0 (no floor) where the floor would spill: the packed kernel has the padded kernel's occupancy without it at dh 32,
+// and loses one CTA per SM at dh 64 (130 registers against 128).
 template <int DH, bool UNIFORM, bool TIMED>
-__global__ void __launch_bounds__(ATT_THREADS) hstu_attn_extend_kernel(HstuExtendArgs a) {
+constexpr int ext_jagged_min_blocks() {
+    return DH == 32 ? (UNIFORM ? (TIMED ? 5 : 0) : (TIMED ? 3 : 4)) : (UNIFORM ? (TIMED ? 0 : 4) : 3);
+}
+template <int DH, bool UNIFORM, bool TIMED, bool JAGGED>
+__global__ void __launch_bounds__(ATT_THREADS, JAGGED ? ext_jagged_min_blocks<DH, UNIFORM, TIMED>() : 0)
+    hstu_attn_extend_kernel(HstuExtendArgs a) {
     pdl_wait();
     extern __shared__ __align__(16) unsigned char ext_smem_raw[];
     ExtSmem<DH>& sm = *reinterpret_cast<ExtSmem<DH>*>(ext_smem_raw);
@@ -138,12 +178,21 @@ __global__ void __launch_bounds__(ATT_THREADS) hstu_attn_extend_kernel(HstuExten
     const int qtiles = (a.n + ATT_BLK - 1) / ATT_BLK;
     const int h = blockIdx.y, b = blockIdx.z / qtiles, r0 = (blockIdx.z % qtiles) * ATT_BLK;
     const int k_lo = blockIdx.x * a.split;
+    long long tok0 = 0;                                        // JAGGED: the sequence's first token row and its rows
+    int rows = a.n;
+    if constexpr (JAGGED) {
+        seq_span(a.offsets, a.T, a.n, b, tok0, rows);
+        if (r0 >= rows) return;                                // query tile past the end of a packed sequence
+    }
 
     // positions of this thread's two rows (mma fragment rows g and g + 8 of the warp's 16)
     const int ra = r0 + warp * 16 + g, rb = ra + 8;
-    const size_t row0 = (size_t)b * a.n;
-    const int pa = ra < a.n ? a.pos[row0 + ra] : -1, pb = rb < a.n ? a.pos[row0 + rb] : -1;
+    const size_t row0 = JAGGED ? (size_t)tok0 : (size_t)b * a.n;
+    const int pa = ra < rows ? a.pos[row0 + ra] : -1, pb = rb < rows ? a.pos[row0 + rb] : -1;
     if (tid == 0) sm.pmax = -1;
+    // the partials' stores read the first row back from shared memory: no register holds it (or its address) across the key loop
+    auto first_row = [&]() { return reinterpret_cast<long long*>(ext_smem_raw + sizeof(ExtSmem<DH>) + ext_table_bytes(a.bias.npos)); };
+    if (JAGGED && tid == 0) *first_row() = tok0;
     __syncthreads();
     const int wmax = __reduce_max_sync(0xffffffffu, max(pa, pb));
     if (lane == 0) atomicMax(&sm.pmax, wmax);
@@ -159,7 +208,7 @@ __global__ void __launch_bounds__(ATT_THREADS) hstu_attn_extend_kernel(HstuExten
     const bf16* gq = a.q + row0 * a.ldq + h * DH;
     const bf16* gk = a.kv + h * DH;
     const bf16* gv = gk + a.D;
-    att_load_tile<DH>(sm.q, gq + (size_t)r0 * a.ldq, a.ldq, 0, 0, a.n - r0, 0, tid);
+    att_load_tile<DH>(sm.q, gq + (size_t)r0 * a.ldq, a.ldq, 0, 0, rows - r0, 0, tid);
     auto load_stream = [&](int k0, int buf) {                 // the tile's 64 keys lie in one page
         const size_t kr = a.pg.row(u, k0);
         att_load_tile<DH>(sm.kv[buf][0], gk + kr * 2 * a.D, 2 * a.D, 0, 0, k_hi - k0, 0, tid);
@@ -220,7 +269,9 @@ __global__ void __launch_bounds__(ATT_THREADS) hstu_attn_extend_kernel(HstuExten
     }
 
     // partial of this split for every row that reaches it (the combine reads splits 0 .. p / split of a row at position p)
-    float* dst = a.part + ((size_t)blockIdx.x * a.B * a.n + row0) * a.D + h * DH;
+    const size_t split0 = JAGGED ? (size_t)blockIdx.x * a.T : (size_t)blockIdx.x * a.B * a.n;   // the split's first partial row
+    const size_t out0 = JAGGED ? (size_t)*first_row() : row0;
+    float* dst = a.part + (split0 + out0) * a.D + h * DH;
 #pragma unroll
     for (int i = 0; i < DH / 8; ++i) {
         const int col = i * 8 + 2 * t;
@@ -325,8 +376,10 @@ GRB_DEVINL void pool_unmark_users(const HstuPoolArgs& a) {
 
 // Row b needs the pages that its user's items after this chunk (at most max_items) take beyond the ceil(len / page_size) the
 // user holds.  Pages are popped from the top of the free stack in row order; a row that finds the stack empty gets what is left
-// (possibly nothing) and its items beyond its pages are dropped by hstu_cache_append_kernel.
-__global__ void __launch_bounds__(POOL_THREADS) hstu_pool_alloc_kernel(HstuPoolArgs a) {
+// (possibly nothing) and its items beyond its pages are dropped by hstu_cache_append_kernel.  JAGGED: ids [T] of a packed chunk
+// (a.n = max_len), and a row's valid items are counted over its sequence's token rows, seq_span(offsets, T, a.n, b).
+template <bool JAGGED>
+__global__ void __launch_bounds__(POOL_THREADS) hstu_pool_alloc_kernel(HstuPoolArgs a, const long long* __restrict__ offsets, int T) {
     pdl_wait();
     __shared__ int cnt[POOL_THREADS];
     __shared__ int ws[32];
@@ -338,7 +391,14 @@ __global__ void __launch_bounds__(POOL_THREADS) hstu_pool_alloc_kernel(HstuPoolA
         const int rows = min(POOL_THREADS, a.B - c0);
         for (int r = warp; r < rows; r += 32) {                // valid items of each row: one warp per row
             int c = 0;
-            for (int j = lane; j < a.n; j += 32) c += a.ids[(size_t)(c0 + r) * a.n + j] != 0;
+            if constexpr (JAGGED) {
+                long long tok0;
+                int len;
+                seq_span(offsets, T, a.n, c0 + r, tok0, len);
+                for (int j = lane; j < len; j += 32) c += a.ids[tok0 + j] != 0;
+            } else {
+                for (int j = lane; j < a.n; j += 32) c += a.ids[(size_t)(c0 + r) * a.n + j] != 0;
+            }
 #pragma unroll
             for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
             if (lane == 0) cnt[r] = c;

@@ -281,6 +281,12 @@ def check_jagged_batch(what: str, input_ids: torch.Tensor, offsets: torch.Tensor
     return offsets.to(input_ids.device)
 
 
+def last_rows_jagged(x: torch.Tensor, offsets: torch.Tensor) -> torch.Tensor:
+    """x [T, D] of a packed batch -> [B, D]: the last row of each sequence, offsets[b+1] - 1, and zeros for a sequence of length 0."""
+    last = (offsets[1:] - 1).clamp(0, x.shape[0] - 1)
+    return torch.where((offsets[1:] > offsets[:-1])[:, None], x.index_select(0, last), torch.zeros((), dtype=x.dtype, device=x.device))
+
+
 class EmbedFn(torch.autograd.Function):
     """x = dropout(E[ids] * scale (+ pos)) ; also emits the uint8 pad flags.  With ``offsets`` ([B+1] int64 on the device) and
     ``max_len`` the batch is packed (ids [T] -> x [T, D], pad [T]) and each token takes SASRec's position row P - n_b + i, P the
@@ -664,37 +670,58 @@ def hstu_attention_bwd(P, zp, dO, meta: SeqMeta, H: int, pos_table, time_table, 
 
 
 # ------------------------------------------------------------------------------------------------ cached incremental inference
-def hstu_cache_append(cache: _lib.HstuCache, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor]):
+def hstu_cache_append(cache: _lib.HstuCache, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor],
+                      offsets: Optional[torch.Tensor] = None, max_len: Optional[int] = None):
     """input_ids / timestamps [B, n] int64 -> (positions [B, n] int32, last_row [B] int32); advances the cache's lengths and stores
-    the chunk's timestamps (grb_hstu_cache_append)."""
-    require_cuda(input_ids, timestamps)
-    require_i64(input_ids, timestamps)
+    the chunk's timestamps (grb_hstu_cache_append).  With ``offsets`` ([B+1] int64 on the device) and ``max_len`` the chunk is
+    packed: input_ids / timestamps [T] -> positions [T], last_row [B] holding token rows (grb_hstu_cache_append_jagged)."""
+    require_cuda(input_ids, timestamps, offsets)
+    require_i64(input_ids, timestamps, offsets)
+    dev = input_ids.device
+    ids = input_ids.contiguous()
+    ts = timestamps.contiguous() if timestamps is not None else None
+    lib = _lib.load()
+    if offsets is not None:
+        B, T = offsets.numel() - 1, ids.numel()
+        positions = torch.empty(T, dtype=torch.int32, device=dev)
+        last_row = torch.empty(B, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            check(lib.grb_hstu_cache_append_jagged(C.byref(cache), ptr(ids), ptr(ts), ptr(offsets.contiguous()), B, T, int(max_len),
+                                                   ptr(positions), ptr(last_row), stream_ptr(dev)))
+        return positions, last_row
     B, n = input_ids.shape
-    positions = torch.empty(B, n, dtype=torch.int32, device=input_ids.device)
-    last_row = torch.empty(B, dtype=torch.int32, device=input_ids.device)
-    with torch.cuda.device(input_ids.device):
-        check(_lib.load().grb_hstu_cache_append(C.byref(cache), ptr(input_ids.contiguous()),
-                                                ptr(timestamps.contiguous()) if timestamps is not None else None, n, ptr(positions),
-                                                ptr(last_row), stream_ptr(input_ids.device)))
+    positions = torch.empty(B, n, dtype=torch.int32, device=dev)
+    last_row = torch.empty(B, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.grb_hstu_cache_append(C.byref(cache), ptr(ids), ptr(ts), n, ptr(positions), ptr(last_row), stream_ptr(dev)))
     return positions, last_row
 
 
 def hstu_layer_extend(x: torch.Tensor, cache, layer: int, positions: torch.Tensor, pos_bucket: Optional[torch.Tensor],
                       pos_bucket0: int, time_thr: torch.Tensor, H: int, npos: int, ntime: int, bf16w: dict, params,
-                      users: Optional[torch.Tensor] = None) -> torch.Tensor:
+                      users: Optional[torch.Tensor] = None, offsets: Optional[torch.Tensor] = None,
+                      max_len: Optional[int] = None) -> torch.Tensor:
     """One block on a chunk against the cache: x [B, n, D] fp32 -> y [B, n, D] fp32.  ``cache`` is a dense ``HstuCache``
     (grb_hstu_layer_extend) or an ``HstuPool`` with ``users`` [B] int64 on the device (grb_hstu_layer_extend_paged).  ``params`` in
-    PARAM_ORDER (time_table None or ntime = 0: no temporal term), ``bf16w`` the three bf16 weight mirrors."""
+    PARAM_ORDER (time_table None or ntime = 0: no temporal term), ``bf16w`` the three bf16 weight mirrors.  With ``offsets``
+    ([B+1] int64 on the device) and ``max_len`` the chunk is packed: x [T, D] -> y [T, D] (the ``_jagged`` entry points)."""
     lib = _lib.load()
     require_cuda(x)
     require_f32(x)
-    B, n, D = x.shape
     xc = x.contiguous()
+    D = x.shape[-1]
+    if offsets is not None:
+        B, n, T = offsets.numel() - 1, int(max_len), x.numel() // D
+    else:
+        B, n, D = x.shape
     has_time = params[PARAM_ORDER.index("time_table")] is not None and ntime > 0
     dims = _dims(B, n, D, H, npos, ntime if has_time else 0, 0.0, 0, None, layer)
     pstruct = _layer_param_struct(params, bf16w, has_time)
     paged = isinstance(cache, _lib.HstuPool)
-    if paged:
+    if offsets is not None:
+        nbytes = (lib.grb_hstu_layer_extend_paged_workspace_bytes_jagged(C.byref(dims), C.byref(cache), T) if paged else
+                  lib.grb_hstu_layer_extend_workspace_bytes_jagged(C.byref(dims), cache.capacity, T))
+    elif paged:
         nbytes = lib.grb_hstu_layer_extend_paged_workspace_bytes(C.byref(dims), C.byref(cache))
     else:
         nbytes = lib.grb_hstu_layer_extend_workspace_bytes(C.byref(dims), cache.capacity)
@@ -702,31 +729,43 @@ def hstu_layer_extend(x: torch.Tensor, cache, layer: int, positions: torch.Tenso
         raise _lib.GrbError(lib.grb_last_error().decode())
     ws = _u8(nbytes, x.device)
     y = torch.empty_like(xc)
+    tail = (ptr(positions), ptr(pos_bucket), int(pos_bucket0), ptr(time_thr), ptr(xc), ptr(y), ptr(ws), stream_ptr(x.device))
     with torch.cuda.device(x.device):
-        if paged:
-            check(lib.grb_hstu_layer_extend_paged(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(users), ptr(positions),
-                                                  ptr(pos_bucket), int(pos_bucket0), ptr(time_thr), ptr(xc), ptr(y), ptr(ws),
-                                                  stream_ptr(x.device)))
+        if offsets is not None and paged:
+            check(lib.grb_hstu_layer_extend_paged_jagged(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(users), ptr(offsets),
+                                                         T, *tail))
+        elif offsets is not None:
+            check(lib.grb_hstu_layer_extend_jagged(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(offsets), T, *tail))
+        elif paged:
+            check(lib.grb_hstu_layer_extend_paged(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(users), *tail))
         else:
-            check(lib.grb_hstu_layer_extend(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(positions), ptr(pos_bucket),
-                                            int(pos_bucket0), ptr(time_thr), ptr(xc), ptr(y), ptr(ws), stream_ptr(x.device)))
+            check(lib.grb_hstu_layer_extend(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, *tail))
     return y
 
 
-def hstu_pool_append(pool: _lib.HstuPool, users: torch.Tensor, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor]):
+def hstu_pool_append(pool: _lib.HstuPool, users: torch.Tensor, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor],
+                     offsets: Optional[torch.Tensor] = None, max_len: Optional[int] = None):
     """users [B] int64 and input_ids / timestamps [B, n] int64 on the device -> (positions [B, n] int32, last_row [B] int32, room [B]
-    int32); hands out the pages the chunk needs and stores its timestamps (grb_hstu_pool_append)."""
-    require_cuda(users, input_ids, timestamps)
-    require_i64(users, input_ids, timestamps)
-    B, n = input_ids.shape
+    int32); hands out the pages the chunk needs and stores its timestamps (grb_hstu_pool_append).  With ``offsets`` ([B+1] int64 on
+    the device) and ``max_len`` the chunk is packed: input_ids / timestamps [T] -> positions [T], last_row [B] holding token rows
+    (grb_hstu_pool_append_jagged)."""
+    require_cuda(users, input_ids, timestamps, offsets)
+    require_i64(users, input_ids, timestamps, offsets)
     dev = input_ids.device
-    positions = torch.empty(B, n, dtype=torch.int32, device=dev)
+    B = users.numel() if offsets is not None else input_ids.shape[0]
+    ids = input_ids.contiguous()
+    ts = timestamps.contiguous() if timestamps is not None else None
+    positions = torch.empty(ids.shape, dtype=torch.int32, device=dev)
     last_row = torch.empty(B, dtype=torch.int32, device=dev)
     room = torch.empty(B, dtype=torch.int32, device=dev)
+    lib = _lib.load()
     with torch.cuda.device(dev):
-        check(_lib.load().grb_hstu_pool_append(C.byref(pool), ptr(users.contiguous()), B, ptr(input_ids.contiguous()),
-                                               ptr(timestamps.contiguous()) if timestamps is not None else None, n, ptr(positions),
-                                               ptr(last_row), ptr(room), stream_ptr(dev)))
+        if offsets is not None:
+            check(lib.grb_hstu_pool_append_jagged(C.byref(pool), ptr(users.contiguous()), B, ptr(ids), ptr(ts), ptr(offsets.contiguous()),
+                                                  ids.numel(), int(max_len), ptr(positions), ptr(last_row), ptr(room), stream_ptr(dev)))
+        else:
+            check(lib.grb_hstu_pool_append(C.byref(pool), ptr(users.contiguous()), B, ptr(ids), ptr(ts), ids.shape[1], ptr(positions),
+                                           ptr(last_row), ptr(room), stream_ptr(dev)))
     return positions, last_row, room
 
 

@@ -636,6 +636,26 @@ class HSTU(nn.Module):
         x = self.encode(input_ids, timestamps)
         return self._hidden_select(x[:, -1, :], None, num_candidates, exclude)
 
+    @torch.no_grad()
+    def recommend_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, timestamps: Optional[torch.Tensor] = None,
+                         top_k: int = 10, exclude: Optional[torch.Tensor] = None) -> Fn.TopItems:
+        """``recommend`` on a packed batch (input_ids / timestamps [T], offsets [B+1], max_len as in ``forward_jagged``): one row of
+        ``TopItems`` per sequence, selected from the head of its last row, offsets[b+1] - 1.  A sequence of length 0 gets the head
+        of a zero vector, as ``extend`` gives a user with no items.  The uncached counterpart of a packed prefill."""
+        offsets = self._check_jagged("recommend_jagged", input_ids, offsets, max_len, timestamps)
+        self._check_topk("recommend_jagged", top_k, exclude, offsets.numel() - 1, input_ids.device)
+        x = self.encode_jagged(input_ids, offsets, max_len, timestamps)
+        return self._hidden_topk(Fn.last_rows_jagged(x, offsets), top_k, exclude)
+
+    @torch.no_grad()
+    def retrieve_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, timestamps: Optional[torch.Tensor] = None,
+                        num_candidates: int = 500, exclude: Optional[torch.Tensor] = None) -> Fn.TopItems:
+        """``retrieve`` on a packed batch, under ``recommend_jagged``'s rules: up to 2048 items per sequence."""
+        offsets = self._check_jagged("retrieve_jagged", input_ids, offsets, max_len, timestamps)
+        self._check_candidates("retrieve_jagged", num_candidates, exclude, offsets.numel() - 1, input_ids.device)
+        x = self.encode_jagged(input_ids, offsets, max_len, timestamps)
+        return self._hidden_select(Fn.last_rows_jagged(x, offsets), None, num_candidates, exclude)
+
     def _check_topk(self, what: str, top_k: int, exclude: Optional[torch.Tensor], rows: int, device) -> None:
         if self.precision == "fp32":
             raise RuntimeError(f"genrec_b200: {what} runs the bf16 path only; set_precision('bf16') or use last_logits")
@@ -703,19 +723,69 @@ class HSTU(nn.Module):
             raise ValueError(f"the state holds {state.batch_size} users on {state.lengths.device}; got input_ids {tuple(input_ids.shape)} on "
                              f"{input_ids.device}")
         self._check_serving_topk("extend", top_k, num_candidates, exclude, B, input_ids.device)
-        if state.items_bound + n > state.capacity:
-            raise ValueError(f"extending by {n} items could exceed the state's capacity ({state.items_bound} of {state.capacity} may be "
+        return self._extend_state(state, input_ids, timestamps, None, n, n, top_k, num_candidates, exclude)
+
+    @torch.no_grad()
+    def extend_jagged(self, state: HSTUState, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int,
+                      timestamps: Optional[torch.Tensor] = None, *, top_k: Optional[int] = None, num_candidates: Optional[int] = None,
+                      exclude: Optional[torch.Tensor] = None):
+        """``extend`` on a packed chunk: input_ids / timestamps [T] int64, offsets [B+1] int64 with B = ``state.batch_size``
+        (sequence b = rows offsets[b] .. offsets[b+1]-1 appends to user b; rows from offsets[B] to T are idle), max_len >= every
+        length and <= the state's capacity.  Returns what ``extend`` returns for the padded [B, max_len] chunk holding the same
+        items per user, bit for bit, and leaves the state as that call does; only the T rows run through the blocks, none of them
+        padding.  An empty sequence leaves its user untouched.  Ids equal to 0 inside a sequence still count as pads.  A packed chunk
+        has no pads ahead of a user's items, so prefilling packed histories gives ``last_logits`` of the left-padded batch for
+        every position-bucket table.
+
+        With offsets on the CPU the chunk is checked before any launch (ValueError) and the host's capacity bound advances by the
+        longest sequence; offsets on the device are not read on the host (the bound advances by max_len), so a call with fixed
+        (B, T, max_len) is CUDA-graph capturable after one eager call and can be replayed with new ids, timestamps and offsets."""
+        self._check_extend_mode("extend_jagged")
+        B = state.batch_size
+        offsets, grow = self._check_jagged_chunk("extend_jagged", input_ids, offsets, max_len, timestamps, B, state.capacity,
+                                                 "the state's capacity", top_k, num_candidates, exclude)
+        if input_ids.device != state.lengths.device:
+            raise ValueError(f"the state lives on {state.lengths.device}; got input_ids on {input_ids.device}")
+        grow = int(grow.max()) if isinstance(grow, torch.Tensor) else grow
+        return self._extend_state(state, input_ids, timestamps, offsets, max_len, grow, top_k, num_candidates, exclude)
+
+    def _check_jagged_chunk(self, what: str, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int,
+                            timestamps: Optional[torch.Tensor], B: int, limit: int, limit_name: str, top_k: Optional[int],
+                            num_candidates: Optional[int], exclude: Optional[torch.Tensor]):
+        """Argument check of a packed chunk of B sequences, all of it before the device is touched -> (offsets on the device, how
+        far each sequence can grow its user: the lengths [B] for CPU offsets, max_len for device offsets)."""
+        if isinstance(offsets, torch.Tensor) and offsets.dim() == 1 and offsets.numel() != B + 1:
+            raise ValueError(f"{what}: offsets must be [{B + 1}] (one sequence per user of the call), got [{offsets.numel()}]")
+        if isinstance(max_len, int) and max_len > limit:
+            raise ValueError(f"{what}: max_len {max_len} exceeds {limit_name} ({limit})")
+        self._check_serving_topk(what, top_k, num_candidates, exclude, B, input_ids.device)
+        dev_offsets = self._check_jagged(what, input_ids, offsets, max_len, timestamps)
+        return dev_offsets, (max_len if offsets.is_cuda else offsets[1:] - offsets[:-1])
+
+    def _extend_state(self, state: HSTUState, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor], offsets: Optional[torch.Tensor],
+                      max_len: int, grow: int, top_k: Optional[int], num_candidates: Optional[int], exclude: Optional[torch.Tensor]):
+        """The body of ``extend`` (offsets None: a padded [B, max_len] chunk) and ``extend_jagged``, after their argument checks;
+        ``grow`` advances the host's bound of every user's length."""
+        if state.items_bound + grow > state.capacity:
+            raise ValueError(f"extending by {grow} items could exceed the state's capacity ({state.items_bound} of {state.capacity} may be "
                              "used); start a new state with a larger capacity")
         use_time = self._check_cache_owner(state, timestamps, "state")
-        dev = input_ids.device
         ids = input_ids.contiguous()
         cache = state._struct()
-        positions, last_row = Fn.hstu_cache_append(cache, ids, timestamps.contiguous() if timestamps is not None else None)
-        x = self._extend_blocks(ids, positions, cache, state.capacity, use_time)
-        latest = x[torch.arange(B, device=dev), last_row.clamp(min=0).long()]
+        positions, last_row = Fn.hstu_cache_append(cache, ids, timestamps.contiguous() if timestamps is not None else None, offsets,
+                                                   max_len)
+        x = self._extend_blocks(ids, positions, cache, state.capacity, use_time, offsets=offsets, max_len=max_len)
+        latest = x[self._last_tokens(last_row, offsets, max_len)]
         state.last_hidden.copy_(torch.where((last_row >= 0)[:, None], latest, state.last_hidden))
-        state.items_bound += n
+        state.items_bound += grow
         return self._hidden_select(state.last_hidden, top_k, num_candidates, exclude)
+
+    @staticmethod
+    def _last_tokens(last_row: torch.Tensor, offsets: Optional[torch.Tensor], n: int) -> torch.Tensor:
+        """The token row of each user's last item (row 0 where the chunk had none): a packed chunk's append returns token rows, a
+        padded one the row within the user's n slots."""
+        tok = last_row.clamp(min=0).long()
+        return tok if offsets is not None else tok + torch.arange(tok.numel(), device=tok.device) * n
 
     def _check_extend_mode(self, what: str) -> None:
         if self.precision == "fp32":
@@ -736,11 +806,15 @@ class HSTU(nn.Module):
         return use_time
 
     def _extend_blocks(self, ids: torch.Tensor, positions: torch.Tensor, cache, capacity: int, use_time: bool,
-                       users: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Embedding and every block of a chunk [B, n] against ``cache`` (a dense HstuCache, or an HstuPool with ``users``) -> the
-        final block's output [B, n, D] fp32."""
+                       users: Optional[torch.Tensor] = None, offsets: Optional[torch.Tensor] = None,
+                       max_len: Optional[int] = None) -> torch.Tensor:
+        """Embedding and every block of a chunk [B, n] (or, with ``offsets`` and ``max_len``, a packed chunk [T]) against ``cache`` (a
+        dense HstuCache, or an HstuPool with ``users``) -> the final block's output [B * n or T, D] fp32, one row per token."""
         dev = ids.device
-        x, _ = Fn.EmbedFn.apply(ids, self.item_embedding.weight, None, 1.0, 0, 0.0, 0, None, None)
+        # HSTU has no position table, so the embedding of a packed chunk is that of one [1, T] row
+        x, _ = Fn.EmbedFn.apply(ids if offsets is None else ids.view(1, -1), self.item_embedding.weight, None, 1.0, 0, 0.0, 0, None, None)
+        if offsets is not None:
+            x = x.view(-1, self.embed_dim)
         if len(self.layers):
             rpb = self.layers[0].position_bias
             uniform, bucket0 = rpb.uniform_of(capacity, dev)
@@ -749,8 +823,8 @@ class HSTU(nn.Module):
             for i, layer in enumerate(self.layers):
                 layer._bf16_provider = self._bf16_provider
                 x = Fn.hstu_layer_extend(x, cache, i, positions, pos_bucket, bucket0, _thresholds_on(dev), layer.num_heads, rpb.num_buckets,
-                                         ntime, layer._bf16_weights(), layer._params(), users=users)
-        return x
+                                         ntime, layer._bf16_weights(), layer._params(), users=users, offsets=offsets, max_len=max_len)
+        return x.view(-1, self.embed_dim)
 
     def _hidden_logits(self, hidden: torch.Tensor) -> torch.Tensor:
         return Fn.head_logits(hidden[:, None, :], self.final_norm.weight, self.final_norm.bias, self.item_embedding.weight,
@@ -780,25 +854,56 @@ class HSTU(nn.Module):
         self._check_extend_mode("extend_users")
         require_cuda(input_ids)
         ensure_device(input_ids.device)
-        dev = input_ids.device
         if input_ids.dim() != 2 or input_ids.device != pool.lengths.device:
             raise ValueError(f"input_ids must be [B, n] on {pool.lengths.device}; got {tuple(input_ids.shape)} on {input_ids.device}")
         B, n = input_ids.shape
         users = torch.as_tensor(users, dtype=torch.int64) if not isinstance(users, torch.Tensor) else users
         if users.shape != (B,):
             raise ValueError(f"users must have one entry per row of input_ids ({B}), got shape {tuple(users.shape)}")
-        self._check_serving_topk("extend_users", top_k, num_candidates, exclude, B, dev)
+        self._check_serving_topk("extend_users", top_k, num_candidates, exclude, B, input_ids.device)
+        return self._extend_pool(pool, users, input_ids, timestamps, None, n, n, top_k, num_candidates, exclude)
+
+    @torch.no_grad()
+    def extend_users_jagged(self, pool: HSTUPool, users, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int,
+                            timestamps: Optional[torch.Tensor] = None, *, top_k: Optional[int] = None,
+                            num_candidates: Optional[int] = None, exclude: Optional[torch.Tensor] = None):
+        """``extend_users`` on a packed chunk: sequence b (rows offsets[b] .. offsets[b+1]-1 of input_ids / timestamps [T], as in
+        ``extend_jagged``) appends to user ``users[b]``, max_len <= the pool's max_items.  Returns what ``extend_users`` returns for
+        the padded [B, max_len] chunk holding the same items per user, bit for bit, and leaves the pool (page tables, free pages,
+        errors) as that call does, under the same device rules.
+
+        With ``users`` on the CPU the call is refused before any launch as ``extend_users`` refuses it; the host's bound of each
+        user advances by their exact length when the offsets are on the CPU too, and by max_len when the offsets are on the device
+        (not read on the host).  With ``users`` on the device those checks are skipped.  A call with fixed (B, T, max_len) and
+        device ``users`` / ``offsets`` is CUDA-graph capturable after one eager call."""
+        self._check_extend_mode("extend_users_jagged")
+        users = torch.as_tensor(users, dtype=torch.int64) if not isinstance(users, torch.Tensor) else users
+        if users.dim() != 1:
+            raise ValueError(f"users must be a 1-D tensor with one entry per sequence, got shape {tuple(users.shape)}")
+        offsets, grow = self._check_jagged_chunk("extend_users_jagged", input_ids, offsets, max_len, timestamps, users.shape[0],
+                                                 pool.max_items, "the pool's max_items", top_k, num_candidates, exclude)
+        if input_ids.device != pool.lengths.device:
+            raise ValueError(f"input_ids must be on {pool.lengths.device}; got {input_ids.device}")
+        return self._extend_pool(pool, users, input_ids, timestamps, offsets, max_len, grow, top_k, num_candidates, exclude)
+
+    def _extend_pool(self, pool: HSTUPool, users: torch.Tensor, input_ids: torch.Tensor, timestamps: Optional[torch.Tensor],
+                     offsets: Optional[torch.Tensor], max_len: int, grow, top_k: Optional[int], num_candidates: Optional[int],
+                     exclude: Optional[torch.Tensor]):
+        """The body of ``extend_users`` (offsets None: a padded [B, max_len] chunk) and ``extend_users_jagged``, after their argument
+        checks; ``grow`` (an int or a [B] tensor) advances the host's bound of each CPU user's length."""
+        dev = input_ids.device
         bound = None
         if not users.is_cuda:
             u_host = pool._host_users(users)
-            bound = pool._check_room(u_host, n)
+            bound = pool._check_room(u_host, grow)
         use_time = self._check_cache_owner(pool, timestamps, "pool")
         users = users.to(dev).long()
         ids = input_ids.contiguous()
         cache = pool._struct()
-        positions, last_row, room = Fn.hstu_pool_append(cache, users, ids, timestamps.contiguous() if timestamps is not None else None)
-        x = self._extend_blocks(ids, positions, cache, pool.max_items, use_time, users=users)
-        latest = x[torch.arange(B, device=dev), last_row.clamp(min=0).long()]
+        positions, last_row, room = Fn.hstu_pool_append(cache, users, ids, timestamps.contiguous() if timestamps is not None else None,
+                                                        offsets, max_len)
+        x = self._extend_blocks(ids, positions, cache, pool.max_items, use_time, users=users, offsets=offsets, max_len=max_len)
+        latest = x[self._last_tokens(last_row, offsets, max_len)]
         slot = torch.where(room >= 0, users, pool.max_users)     # rejected rows read and write the spare zero row
         hidden = torch.where((last_row >= 0)[:, None], latest, pool.last_hidden[slot])
         pool.last_hidden[slot] = hidden

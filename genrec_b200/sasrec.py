@@ -352,6 +352,28 @@ class SASRec(nn.Module):
                                   self.final_norm.eps, num_candidates, exclude)
 
     @torch.no_grad()
+    def recommend_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, top_k: int = 10,
+                         exclude: Optional[torch.Tensor] = None) -> Fn.TopItems:
+        """``recommend`` on a packed batch (input_ids [T], offsets [B+1], max_len as in ``forward_jagged``, positions by its batch-wide
+        rule): one row of ``TopItems`` per sequence, selected from the head of its last row, offsets[b+1] - 1.  A sequence of length
+        0 gets the head of a zero vector."""
+        offsets = Fn.check_jagged_batch("recommend_jagged", input_ids, offsets, max_len, self.max_seq_len)
+        Fn.check_topk_args(top_k, exclude, offsets.numel() - 1, input_ids.device)
+        x = Fn.last_rows_jagged(self.encode_jagged(input_ids, offsets, max_len), offsets)
+        return Fn.head_topk(x, self.final_norm.weight, self.final_norm.bias, Fn.cast_bf16(self.item_embedding.weight), self.final_norm.eps,
+                            top_k, exclude)
+
+    @torch.no_grad()
+    def retrieve_jagged(self, input_ids: torch.Tensor, offsets: torch.Tensor, max_len: int, num_candidates: int = 500,
+                        exclude: Optional[torch.Tensor] = None) -> Fn.TopItems:
+        """``retrieve`` on a packed batch, under ``recommend_jagged``'s rules: up to 2048 items per sequence."""
+        offsets = Fn.check_jagged_batch("retrieve_jagged", input_ids, offsets, max_len, self.max_seq_len)
+        Fn.check_candidates_args(num_candidates, exclude, offsets.numel() - 1, input_ids.device)
+        x = Fn.last_rows_jagged(self.encode_jagged(input_ids, offsets, max_len), offsets)
+        return Fn.head_candidates(x, self.final_norm.weight, self.final_norm.bias, Fn.cast_bf16(self.item_embedding.weight),
+                                  self.final_norm.eps, num_candidates, exclude)
+
+    @torch.no_grad()
     def evaluate_batch(self, input_ids: torch.Tensor, targets: torch.Tensor, metrics: Optional[torch.Tensor] = None, *,
                        exclude: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Leave-one-out metrics of one evaluation batch, accumulated on the device into ``metrics`` ([6] fp32: Recall@{1,5,10} hit

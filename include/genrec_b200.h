@@ -236,6 +236,33 @@ int grb_hstu_layer_extend_paged(const grb_hstu_dims* d, const grb_hstu_layer_par
                                 const int64_t* users, const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0,
                                 const int64_t* time_thr, const float* x, float* y, void* workspace, void* stream);
 
+/* Packed chunks: the entry points above on B sequences packed into T token rows with no pads between them.  Sequence b is the
+ * token rows offsets[b] .. offsets[b+1]-1 (offsets [B+1] int64 on the device, never read on the host; a malformed one is kept
+ * inside [0, T) and each sequence is clamped to max_len), and rows in no sequence (offsets[B] .. T-1) are idle.  Ids == 0 inside a
+ * sequence still count as pads.  Each sequence's items are handled as the same items in a padded [B, max_len] chunk row: equal
+ * positions, lengths, overflow flags, page hand-out, room, errors and cache bytes, and, in the layers, bit-identical outputs on
+ * the sequence rows (the key split is the padded call's, with n = max_len).
+ *   grb_hstu_cache_append_jagged: input_ids / timestamps [T] (timestamps may be NULL), B == c->B (sequence b appends to user b),
+ *       positions [T] int32 (-1 for a pad, a dropped item or an idle row), last_row [B] int32 = the token row of the user's last
+ *       valid item, or -1.
+ *   grb_hstu_pool_append_jagged: users [B], sequence b appends to user users[b]; outputs as grb_hstu_cache_append_jagged plus room.
+ *   grb_hstu_layer_extend_jagged / grb_hstu_layer_extend_paged_jagged: d->B = the sequence count, d->L = max_len, x / y [T, D]
+ *       fp32, positions [T] as returned by the append; B * ceil(max_len / 64) <= 65535.  y of an idle row is that of a row with
+ *       no position.  workspace: the _workspace_bytes_jagged of the same d and T. */
+int grb_hstu_cache_append_jagged(const grb_hstu_cache* c, const int64_t* input_ids, const int64_t* timestamps, const int64_t* offsets,
+                                 int B, int T, int max_len, int32_t* positions, int32_t* last_row, void* stream);
+int grb_hstu_pool_append_jagged(const grb_hstu_pool* pool, const int64_t* users, int B, const int64_t* input_ids, const int64_t* timestamps,
+                                const int64_t* offsets, int T, int max_len, int32_t* positions, int32_t* last_row, int32_t* room,
+                                void* stream);
+size_t grb_hstu_layer_extend_workspace_bytes_jagged(const grb_hstu_dims* d, int capacity, int T);
+int grb_hstu_layer_extend_jagged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_cache* c, int layer,
+                                 const int64_t* offsets, int T, const int32_t* positions, const uint8_t* pos_bucket, int pos_bucket0,
+                                 const int64_t* time_thr, const float* x, float* y, void* workspace, void* stream);
+size_t grb_hstu_layer_extend_paged_workspace_bytes_jagged(const grb_hstu_dims* d, const grb_hstu_pool* pool, int T);
+int grb_hstu_layer_extend_paged_jagged(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const grb_hstu_pool* pool, int layer,
+                                       const int64_t* users, const int64_t* offsets, int T, const int32_t* positions, const uint8_t* pos_bucket,
+                                       int pos_bucket0, const int64_t* time_thr, const float* x, float* y, void* workspace, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ input pipeline
  * Device-side hstu_collate_fn / sasrec_collate_fn (genrec/data/amazon_hstu.py:137-173, genrec/data/amazon_sasrec.py:125-161): a
  * jagged batch (items / stamps [N] in time order, offsets [B+1], one held-out target per user) -> the LEFT-padded [B, L]
