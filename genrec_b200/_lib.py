@@ -163,6 +163,12 @@ SIGNATURES = {
     "grb_t5_attention_forward": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 8 + [c_void_p, c_void_p, c_int, c_void_p, c_int, c_float, c_float,
                                          c_u64, c_void_p, C.c_uint32, c_void_p, c_int, c_void_p, c_void_p]),
     "grb_t5_attention_backward_workspace_bytes": (c_size_t, [c_int] * 6),
+    "grb_t5_attention_forward_jagged": (c_int, [c_void_p] * 4 + [c_int] * 9 + [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_u64,
+                                                                             c_void_p, C.c_uint32, c_void_p, c_int, c_void_p, c_void_p]),
+    "grb_t5_attention_backward_workspace_bytes_jagged": (c_size_t, [c_int] * 7),
+    "grb_t5_attention_backward_jagged": (c_int, [c_void_p] * 4 + [c_int] * 9 + [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_u64,
+                                                                              c_void_p, C.c_uint32, c_void_p, c_int, c_void_p, c_void_p, c_int,
+                                                                              c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_t5_attention_backward": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 8 + [c_void_p, c_void_p, c_int, c_void_p, c_int, c_float, c_float,
                                           c_u64, c_void_p, C.c_uint32, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
                                           c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -1824,6 +1824,42 @@ static int t5_args(T5AttnArgs& a, const void* q, const void* k, const void* v, i
     a.scale = scale; a.drop = make_dropout(p, seed, site, seed_dev);
     return 0;
 }
+// packed batches: Lq = 0 for self-attention (queries = the packed rows), else the dense query count of cross-attention
+}  // extern "C"
+
+namespace {
+int t5_args_jagged(T5AttnArgs& a, const void* q, const void* k, const void* v, const int64_t* offsets, int B, int T, int max_len, int Lq,
+                   int H, int DH, int ldq, int ldk, int ldv, const float* bias, const int32_t* bucket, int bucket_len, int nb, int causal,
+                   float scale, float p, uint64_t seed, const uint64_t* seed_dev, uint32_t site) {
+    GRB_REQUIRE(offsets != nullptr, "offsets is null");
+    GRB_REQUIRE(B >= 1 && B <= 65535, "B=%d out of range [1, 65535]", B);
+    GRB_REQUIRE(T >= 1 && max_len >= 1 && Lq >= 0, "bad shape T=%d max_len=%d Lq=%d", T, max_len, Lq);
+    const int lq = Lq > 0 ? Lq : max_len;
+    GRB_TRY(t5_args(a, q, k, v, B, lq, max_len, H, DH, ldq, ldk, ldv, bias, bucket, nb, nullptr, causal, scale, p, seed, seed_dev, site));
+    GRB_REQUIRE((long long)T * ldk <= INT32_MAX && (long long)T * ldv <= INT32_MAX && (long long)T * H <= INT32_MAX &&
+                    (Lq > 0 || (long long)T * ldq <= INT32_MAX), "token rows T=%d out of range", T);
+    GRB_REQUIRE(!bias || bucket_len >= lq + max_len - 1, "bucket map of %d entries, %d needed (Lq + max_len - 1)", bucket_len,
+                lq + max_len - 1);
+    return 0;
+}
+template <int PACK>
+int t5_launch_fwd(const T5AttnArgs& a, const T5Packed& pk, int head_dim, cudaStream_t st) {
+    const long long bh = (long long)a.B * a.H;
+    GRB_REQUIRE(bh <= INT_MAX, "B * H = %lld too large (at most 2^31 - 1)", bh);
+    const unsigned nx = (a.Lq + T5_ROWS - 1) / T5_ROWS;
+    return with_head_dim(head_dim, [&](auto DH) -> int {
+        if (bh <= 65535) {
+            GRB_LAUNCH((t5_attn_fwd_kernel<DH, false, PACK>), dim3(nx, (unsigned)bh), T5_THREADS, t5_fwd_smem<DH>(a.nb), st, a, pk);
+        } else {
+            GRB_LAUNCH((t5_attn_fwd_kernel<DH, true, PACK>), dim3(nx, 65535u, (unsigned)((bh + 65534) / 65535)), T5_THREADS,
+                       t5_fwd_smem<DH>(a.nb), st, a, pk);
+        }
+        return 0;
+    });
+}
+}  // namespace
+
+extern "C" {
 int grb_t5_attention_forward(const void* q, const void* k, const void* v, int B, int Lq, int Lk, int H, int head_dim, int ldq, int ldk, int ldv,
                              const float* bias, const int32_t* bucket, int num_buckets, const uint8_t* key_pad, int causal, float scale,
                              float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t site, void* out, int ldo, float* lse,
@@ -1832,19 +1868,7 @@ int grb_t5_attention_forward(const void* q, const void* k, const void* v, int B,
     GRB_TRY(t5_args(a, q, k, v, B, Lq, Lk, H, head_dim, ldq, ldk, ldv, bias, bucket, num_buckets, key_pad, causal, scale, dropout_p, seed, seed_dev, site));
     GRB_REQUIRE(out && lse && ldo % 8 == 0 && aligned16(out), "bad output");
     a.out = (bf16*)out; a.ldo = ldo; a.lse = lse;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const long long bh = (long long)B * H;
-    GRB_REQUIRE(bh <= INT_MAX, "B * H = %lld too large (at most 2^31 - 1)", bh);
-    const unsigned nx = (Lq + T5_ROWS - 1) / T5_ROWS;
-    return with_head_dim(head_dim, [&](auto DH) -> int {
-        if (bh <= 65535) {
-            GRB_LAUNCH((t5_attn_fwd_kernel<DH, false>), dim3(nx, (unsigned)bh), T5_THREADS, t5_fwd_smem<DH>(a.nb), st, a);
-        } else {
-            GRB_LAUNCH((t5_attn_fwd_kernel<DH, true>), dim3(nx, 65535u, (unsigned)((bh + 65534) / 65535)), T5_THREADS, t5_fwd_smem<DH>(a.nb),
-                       st, a);
-        }
-        return 0;
-    });
+    return t5_launch_fwd<T5_PADDED>(a, T5Packed{nullptr, 0}, head_dim, static_cast<cudaStream_t>(stream));
 }
 namespace {
 struct T5BwdWork {
@@ -1853,12 +1877,12 @@ struct T5BwdWork {
 };
 // the backward's scratch: the bias bins of every CTA when there is a bias table, and the per-query-tile dK / dV partials when
 // there are more than two query tiles (with one or two, the atomics onto zero are exact in either order)
-T5BwdWork carve_t5_bwd(void* base, int B, int Lq, int Lk, int H, int head_dim, int nb) {
+// (nqt query tiles per batch entry, key_rows = B * Lk, or T when packed)
+T5BwdWork carve_t5_bwd(void* base, int B, int nqt, size_t key_rows, int H, int head_dim, int nb) {
     T5BwdWork w{nullptr, nullptr, 0};
     Carver c{static_cast<char*>(base)};
-    const int nqt = (Lq + T5_ROWS - 1) / T5_ROWS;
     if (nb > 0) w.db_part = c.take<float>((size_t)H * B * nqt * nb * 4);
-    if (nqt > 2) w.dkv_part = c.take<float>((size_t)2 * nqt * B * Lk * H * head_dim * 4);
+    if (nqt > 2) w.dkv_part = c.take<float>((size_t)2 * nqt * key_rows * H * head_dim * 4);
     w.bytes = c.off;
     return w;
 }
@@ -1866,7 +1890,7 @@ T5BwdWork carve_t5_bwd(void* base, int B, int Lq, int Lk, int H, int head_dim, i
 
 size_t grb_t5_attention_backward_workspace_bytes(int B, int Lq, int Lk, int H, int head_dim, int num_buckets) {
     if (B <= 0 || Lq <= 0 || Lk <= 0 || H <= 0 || head_dim <= 0 || num_buckets < 0) return 0;
-    return carve_t5_bwd(nullptr, B, Lq, Lk, H, head_dim, num_buckets).bytes;
+    return carve_t5_bwd(nullptr, B, (Lq + T5_ROWS - 1) / T5_ROWS, (size_t)B * Lk, H, head_dim, num_buckets).bytes;
 }
 int grb_t5_attention_backward(const void* q, const void* k, const void* v, int B, int Lq, int Lk, int H, int head_dim, int ldq, int ldk, int ldv,
                               const float* bias, const int32_t* bucket, int num_buckets, const uint8_t* key_pad, int causal, float scale,
@@ -1879,7 +1903,7 @@ int grb_t5_attention_backward(const void* q, const void* k, const void* v, int B
     GRB_REQUIRE(aligned16(out) && aligned16(dout) && aligned16(dq) && aligned16(dk) && aligned16(dv), "rows must be 16-byte aligned");
     a.out = (bf16*)const_cast<void*>(out); a.ldo = ldo; a.lse = const_cast<float*>(lse); a.dout = (const bf16*)dout; a.lddo = lddo;
     a.dq = (bf16*)dq; a.lddq = lddq; a.dk = dk; a.dv = dv; a.dbias = bias ? dbias : nullptr;
-    const T5BwdWork w = carve_t5_bwd(workspace, B, Lq, Lk, H, head_dim, a.nb);
+    const T5BwdWork w = carve_t5_bwd(workspace, B, (Lq + T5_ROWS - 1) / T5_ROWS, (size_t)B * Lk, H, head_dim, a.nb);
     GRB_REQUIRE(workspace || w.bytes == 0, "workspace is null");
     GRB_REQUIRE(!workspace || aligned16(workspace), "workspace must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1890,10 +1914,69 @@ int grb_t5_attention_backward(const void* q, const void* k, const void* v, int B
     }
     dim3 grid((Lq + T5_ROWS - 1) / T5_ROWS, B * H);
     GRB_TRY(with_head_dim(head_dim, [&](auto DH) -> int {
-        GRB_LAUNCH(t5_attn_bwd_kernel<DH>, grid, T5_THREADS, t5_bwd_smem<DH>(a.nb), st, a, w.dkv_part, w.db_part);
+        GRB_LAUNCH(t5_attn_bwd_kernel<DH>, grid, T5_THREADS, t5_bwd_smem<DH>(a.nb), st, a, w.dkv_part, w.db_part, T5Packed{nullptr, 0});
         return 0;
     }));
     if (w.dkv_part) GRB_LAUNCH(t5_dkdv_sum_kernel, capped_blocks(2 * n / 4), 256, 0, st, (const float*)w.dkv_part, (int)grid.x, n, dk, dv);
+    if (a.dbias) GRB_TRY(det_finish(w.db_part, H, B * (int)grid.x, a.nb, H, a.nb, 1, {{a.dbias, H * a.nb}}, st));
+    return 0;
+}
+
+
+size_t grb_t5_attention_backward_workspace_bytes_jagged(int B, int T, int max_len, int Lq, int H, int head_dim, int num_buckets) {
+    if (B <= 0 || T <= 0 || max_len <= 0 || Lq < 0 || H <= 0 || head_dim <= 0 || num_buckets < 0) return 0;
+    return carve_t5_bwd(nullptr, B, ((Lq > 0 ? Lq : max_len) + T5_ROWS - 1) / T5_ROWS, (size_t)T, H, head_dim, num_buckets).bytes;
+}
+int grb_t5_attention_forward_jagged(const void* q, const void* k, const void* v, const int64_t* offsets, int B, int T, int max_len, int Lq,
+                                    int H, int head_dim, int ldq, int ldk, int ldv, const float* bias, const int32_t* bucket,
+                                    int bucket_len, int num_buckets, int causal, float scale, float dropout_p, uint64_t seed,
+                                    const uint64_t* seed_dev, uint32_t site, void* out, int ldo, float* lse, void* stream) {
+    T5AttnArgs a;
+    GRB_TRY(t5_args_jagged(a, q, k, v, offsets, B, T, max_len, Lq, H, head_dim, ldq, ldk, ldv, bias, bucket, bucket_len, num_buckets,
+                           causal, scale, dropout_p, seed, seed_dev, site));
+    GRB_REQUIRE(out && lse && ldo % 8 == 0 && aligned16(out), "bad output");
+    a.out = (bf16*)out; a.ldo = ldo; a.lse = lse;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const T5Packed pk{reinterpret_cast<const long long*>(offsets), T};
+    if (Lq > 0) return t5_launch_fwd<T5_PACKED_CROSS>(a, pk, head_dim, st);
+    GRB_TRY(t5_launch_fwd<T5_PACKED_SELF>(a, pk, head_dim, st));
+    return zero_idle_rows(offsets, B, T, (bf16*)out, ldo, H * head_dim, st);
+}
+int grb_t5_attention_backward_jagged(const void* q, const void* k, const void* v, const int64_t* offsets, int B, int T, int max_len, int Lq,
+                                     int H, int head_dim, int ldq, int ldk, int ldv, const float* bias, const int32_t* bucket,
+                                     int bucket_len, int num_buckets, int causal, float scale, float dropout_p, uint64_t seed,
+                                     const uint64_t* seed_dev, uint32_t site, const void* out, int ldo, const float* lse, const void* dout,
+                                     int lddo, void* dq, int lddq, float* dk, float* dv, float* dbias, void* workspace, void* stream) {
+    T5AttnArgs a;
+    GRB_TRY(t5_args_jagged(a, q, k, v, offsets, B, T, max_len, Lq, H, head_dim, ldq, ldk, ldv, bias, bucket, bucket_len, num_buckets,
+                           causal, scale, dropout_p, seed, seed_dev, site));
+    GRB_REQUIRE(out && lse && dout && dq && dk && dv && ldo % 8 == 0 && lddo % 8 == 0 && lddq % 8 == 0, "bad argument");
+    GRB_REQUIRE(aligned16(out) && aligned16(dout) && aligned16(dq) && aligned16(dk) && aligned16(dv), "rows must be 16-byte aligned");
+    GRB_REQUIRE((long long)B * H <= 65535, "B * H = %lld exceeds 65535", (long long)B * H);
+    a.out = (bf16*)const_cast<void*>(out); a.ldo = ldo; a.lse = const_cast<float*>(lse); a.dout = (const bf16*)dout; a.lddo = lddo;
+    a.dq = (bf16*)dq; a.lddq = lddq; a.dk = dk; a.dv = dv; a.dbias = bias ? dbias : nullptr;
+    const int D = H * head_dim;
+    dim3 grid((a.Lq + T5_ROWS - 1) / T5_ROWS, B * H);
+    const T5BwdWork w = carve_t5_bwd(workspace, B, (int)grid.x, (size_t)T, H, head_dim, a.nb);
+    GRB_REQUIRE(workspace || w.bytes == 0, "workspace is null");
+    GRB_REQUIRE(!workspace || aligned16(workspace), "workspace must be 16-byte aligned");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t n = (size_t)T * D;
+    if (!w.dkv_part) {                          // the atomics add onto zero; rows outside every sequence keep it
+        GRB_CUDA(cudaMemsetAsync(dk, 0, n * sizeof(float), st));
+        GRB_CUDA(cudaMemsetAsync(dv, 0, n * sizeof(float), st));
+    }
+    const T5Packed pk{reinterpret_cast<const long long*>(offsets), T};
+    GRB_TRY(with_head_dim(head_dim, [&](auto DH) -> int {
+        if (Lq > 0) GRB_LAUNCH((t5_attn_bwd_kernel<DH, T5_PACKED_CROSS>), grid, T5_THREADS, t5_bwd_smem<DH>(a.nb), st, a, w.dkv_part, w.db_part, pk);
+        else GRB_LAUNCH((t5_attn_bwd_kernel<DH, T5_PACKED_SELF>), grid, T5_THREADS, t5_bwd_smem<DH>(a.nb), st, a, w.dkv_part, w.db_part, pk);
+        return 0;
+    }));
+    if (w.dkv_part) {                           // the idle rows' partials were never written: their sums are overwritten with zeros
+        GRB_LAUNCH(t5_dkdv_sum_kernel, capped_blocks(2 * n / 4), 256, 0, st, (const float*)w.dkv_part, (int)grid.x, n, dk, dv);
+        for (float* g : {dk, dv}) GRB_TRY(zero_idle_rows(offsets, B, T, reinterpret_cast<bf16*>(g), 2 * D, 2 * D, st));   // fp32 rows as bf16 pairs
+    }
+    if (Lq == 0) GRB_TRY(zero_idle_rows(offsets, B, T, (bf16*)dq, lddq, D, st));
     if (a.dbias) GRB_TRY(det_finish(w.db_part, H, B * (int)grid.x, a.nb, H, a.nb, 1, {{a.dbias, H * a.nb}}, st));
     return 0;
 }

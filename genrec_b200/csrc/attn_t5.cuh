@@ -15,6 +15,18 @@
 // them in tile order.  The bias-table gradient is accumulated per CTA in shared-memory bins in a fixed order (each diagonal
 // delta = j - i of a key tile in row order, then the diagonals of a bucket in delta order) and the CTAs' bins are added by
 // det_finish, so two calls give the same bits.
+//
+// Packed (jagged) batches: sequence b is rows offsets[b] .. offsets[b+1]-1 of T, clamped to [0, T) and to Lk = max_len (seq_span).
+//   T5_PACKED_SELF  (encoder self-attention): queries and keys are the rows of one sequence; i and j count from its first row, so the
+//                   bucket of j - i is the padded one when the pads follow the items.  Query tiles past a sequence's end exit at once
+//                   (forward) or only store their zero bias bins / dK | dV partials (backward).  lse is per token, [H, T, 2], and the
+//                   dropout row key is the query's token row: (row * H + h), column j.
+//   T5_PACKED_CROSS (decoder cross-attention): queries stay dense [B, Lq]; the keys of b are its packed rows.  lse and the dropout
+//                   keys are the padded ones, so the masks equal those of the padded batch whose pads follow the keys.
+// No key padding in either.  The kernels write only sequence rows: the caller zeroes the idle rows of out (self), dq (self) and dk / dv.
+// PACK is a template parameter, so the padded instantiations compile to the code they had before packed batches existed (up to
+// the order of two independent register initialisations in the forward).  Loop bounds are written out inline below: behind a
+// helper call the compiler rotates the padded key loops differently.
 #pragma once
 #include "common.cuh"
 #include "tc_gemm.cuh"   // exp_accurate
@@ -42,19 +54,62 @@ struct T5AttnArgs {
     float* dk; float* dv;            // [B, Lk, H * DH] fp32, accumulated (zero before the launch)
     float* dbias;                    // [H, nb] accumulated, or null
 };
+// packed batches: offsets [B+1] on the device and T packed rows, with T5AttnArgs::Lk = max_len (and Lq = max_len for self-attention).
+// A trailing kernel parameter, so that the padded kernels keep their parameter layout.
+struct T5Packed {
+    const long long* offsets;
+    int T;
+};
+
+enum { T5_PADDED = 0, T5_PACKED_SELF = 1, T5_PACKED_CROSS = 2 };
+
+// The rows of batch entry b.  Packed: queries q0 .. q0 + nq - 1 of q / out / dout / dq (self) and keys k0 .. k0 + nk - 1 of
+// k / v / dk / dv.  The helpers below give the padded instantiations the very expressions they had before packed layouts existed.
+struct T5Span {
+    size_t q0, k0;
+    int nq, nk;
+};
+template <int PACK>
+GRB_DEVINL T5Span t5_span(const T5AttnArgs& a, const T5Packed& pk, int b) {
+    T5Span sp{0, 0, 0, 0};
+    if constexpr (PACK != T5_PADDED) {
+        long long tok0;
+        seq_span<true>(pk.offsets, pk.T, a.Lk, b, tok0, sp.nk);
+        sp.k0 = (size_t)tok0;
+        sp.q0 = PACK == T5_PACKED_SELF ? sp.k0 : (size_t)b * a.Lq;
+        sp.nq = PACK == T5_PACKED_SELF ? sp.nk : a.Lq;
+    }
+    return sp;
+}
+template <int PACK> GRB_DEVINL size_t t5_qrow(const T5AttnArgs& a, const T5Span& sp, int b, int i) {
+    if constexpr (PACK != T5_PADDED) return sp.q0 + i; else return (size_t)b * a.Lq + i;
+}
+template <int PACK> GRB_DEVINL size_t t5_krow(const T5AttnArgs& a, const T5Span& sp, int b, int j0, int jj) {
+    if constexpr (PACK != T5_PADDED) return sp.k0 + j0 + jj; else return (size_t)b * a.Lk + j0 + jj;
+}
+// lse slot and dropout row key of query i
+template <int PACK>
+GRB_DEVINL size_t t5_lse_at(const T5AttnArgs& a, const T5Packed& pk, const T5Span& sp, int b, int h, int i) {
+    if constexpr (PACK == T5_PACKED_SELF) return (size_t)h * pk.T + sp.q0 + i; else return ((size_t)b * a.H + h) * a.Lq + i;
+}
+template <int PACK>
+GRB_DEVINL uint32_t t5_drop_row(const T5AttnArgs& a, const T5Span& sp, int b, int h, int i) {
+    if constexpr (PACK == T5_PACKED_SELF) return ((uint32_t)sp.q0 + (uint32_t)i) * (uint32_t)a.H + (uint32_t)h;
+    else return (uint32_t)(((size_t)b * a.H + h) * a.Lq + i);
+}
 
 constexpr int T5_ROWS = 32, T5_KEYS = 64, T5_THREADS = 128;
 
-template <int DH>
-GRB_DEVINL void t5_load_tile(float* Ks, float* Vs, const T5AttnArgs& a, int b, int h, int j0, int tid) {
+template <int DH, int PACK>
+GRB_DEVINL void t5_load_tile(float* Ks, float* Vs, const T5AttnArgs& a, const T5Span& sp, int b, int h, int j0, int tid) {
     for (int e = tid; e < T5_KEYS * (DH / 8); e += T5_THREADS) {
         const int jj = e / (DH / 8), c = e % (DH / 8);
         float kf[8], vf[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) kf[i] = vf[i] = 0.f;
-        if (j0 + jj < a.Lk) {
-            const uint4 ku = *reinterpret_cast<const uint4*>(a.k + ((size_t)b * a.Lk + j0 + jj) * a.ldk + h * DH + c * 8);
-            const uint4 vu = *reinterpret_cast<const uint4*>(a.v + ((size_t)b * a.Lk + j0 + jj) * a.ldv + h * DH + c * 8);
+        if (j0 + jj < (PACK != T5_PADDED ? sp.nk : a.Lk)) {
+            const uint4 ku = *reinterpret_cast<const uint4*>(a.k + t5_krow<PACK>(a, sp, b, j0, jj) * a.ldk + h * DH + c * 8);
+            const uint4 vu = *reinterpret_cast<const uint4*>(a.v + t5_krow<PACK>(a, sp, b, j0, jj) * a.ldv + h * DH + c * 8);
             const float2 k0 = unpack_bf16(ku.x), k1 = unpack_bf16(ku.y), k2 = unpack_bf16(ku.z), k3 = unpack_bf16(ku.w);
             const float2 v0 = unpack_bf16(vu.x), v1 = unpack_bf16(vu.y), v2 = unpack_bf16(vu.z), v3 = unpack_bf16(vu.w);
             kf[0] = k0.x; kf[1] = k0.y; kf[2] = k1.x; kf[3] = k1.y; kf[4] = k2.x; kf[5] = k2.y; kf[6] = k3.x; kf[7] = k3.y;
@@ -85,8 +140,8 @@ GRB_DEVINL bool t5_score(const T5AttnArgs& a, const float* sbias, int b, int i, 
 }
 
 // SPLIT_BH: (b, h) = blockIdx.z * gridDim.y + blockIdx.y, for B * H past the 65,535 CTAs gridDim.y allows; otherwise blockIdx.y
-template <int DH, bool SPLIT_BH>
-__global__ void __launch_bounds__(T5_THREADS) t5_attn_fwd_kernel(T5AttnArgs a) {
+template <int DH, bool SPLIT_BH, int PACK = T5_PADDED>
+__global__ void __launch_bounds__(T5_THREADS) t5_attn_fwd_kernel(T5AttnArgs a, T5Packed pk) {
     pdl_wait();
     a.drop.resolve();
     extern __shared__ float t5_smem[];
@@ -97,20 +152,23 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_fwd_kernel(T5AttnArgs a) {
     const int bh = SPLIT_BH ? (int)(blockIdx.z * gridDim.y + blockIdx.y) : (int)blockIdx.y;
     if (SPLIT_BH && bh >= a.B * a.H) return;
     const int b = bh / a.H, h = bh % a.H;
+    const T5Span sp = t5_span<PACK>(a, pk, b);
+    if constexpr (PACK == T5_PACKED_SELF)
+        if ((int)blockIdx.x * T5_ROWS >= sp.nq) return;   // query tile past the end of its sequence
     const int i = blockIdx.x * T5_ROWS + r;
     if (sbias) for (int e = tid; e < a.nb; e += T5_THREADS) sbias[e] = a.bias[h * a.nb + e];
     float q[DH], o[DH];
 #pragma unroll
     for (int d = 0; d < DH; ++d) { q[d] = 0.f; o[d] = 0.f; }
-    if (i < a.Lq) t5_load_row<DH>(q, a.q + ((size_t)b * a.Lq + i) * a.ldq + h * DH);
+    if (i < (PACK != T5_PADDED ? sp.nq : a.Lq)) t5_load_row<DH>(q, a.q + t5_qrow<PACK>(a, sp, b, i) * a.ldq + h * DH);
     float m = -INFINITY, l = 0.f;
-    const uint32_t drow = (uint32_t)(((size_t)b * a.H + h) * a.Lq + i);
-    for (int j0 = 0; j0 < a.Lk; j0 += T5_KEYS) {
+    const uint32_t drow = t5_drop_row<PACK>(a, sp, b, h, i);
+    for (int j0 = 0; j0 < (PACK != T5_PADDED ? sp.nk : a.Lk); j0 += T5_KEYS) {
         __syncthreads();
-        t5_load_tile<DH>(Ks, Vs, a, b, h, j0, tid);
+        t5_load_tile<DH, PACK>(Ks, Vs, a, sp, b, h, j0, tid);
         __syncthreads();
-        if (i >= a.Lq) continue;
-        for (int jj = kq; jj < T5_KEYS && j0 + jj < a.Lk; jj += 4) {
+        if (i >= (PACK != T5_PADDED ? sp.nq : a.Lq)) continue;
+        for (int jj = kq; jj < T5_KEYS && j0 + jj < (PACK != T5_PADDED ? sp.nk : a.Lk); jj += 4) {
             const float* kr = Ks + jj * (DH + 1);
             float qk = 0.f;
 #pragma unroll
@@ -143,22 +201,22 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_fwd_kernel(T5AttnArgs a) {
         for (int d = 0; d < DH; ++d) o[d] = o[d] * c1 + __shfl_xor_sync(0xffffffffu, o[d], sh) * c2;
         m = M;
     }
-    if (i < a.Lq) {
+    if (i < (PACK != T5_PADDED ? sp.nq : a.Lq)) {
         const float inv = l > 0.f ? __fdiv_rn(1.f, l) : 0.f;
-        bf16* dst = a.out + ((size_t)b * a.Lq + i) * a.ldo + h * DH;
+        bf16* dst = a.out + t5_qrow<PACK>(a, sp, b, i) * a.ldo + h * DH;
 #pragma unroll
         for (int d = 0; d < DH; d += 2)
             if (((d >> 1) & 3) == kq) *reinterpret_cast<uint32_t*>(dst + d) = pack_bf16(o[d] * inv, o[d + 1] * inv);
-        if (kq == 0) reinterpret_cast<float2*>(a.lse)[((size_t)b * a.H + h) * a.Lq + i] = make_float2(m, l);
+        if (kq == 0) reinterpret_cast<float2*>(a.lse)[t5_lse_at<PACK>(a, pk, sp, b, h, i)] = make_float2(m, l);
     }
 }
 
 constexpr int T5_DIAGS = T5_ROWS + T5_KEYS - 1;   // diagonals delta = j - i of a 32 x 64 tile
 
-// dkv_part: [2][gridDim.x][B * Lk * H * DH] per-query-tile dK / dV partials when the grid has more than two query tiles, else null
-// (atomics).  db_part: [H][B * gridDim.x][nb] the bias bins of each CTA, non-null iff a.dbias is.
-template <int DH>
-__global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a, float* dkv_part, float* db_part) {
+// dkv_part: [2][gridDim.x][K * H * DH] per-query-tile dK / dV partials when the grid has more than two query tiles, else null
+// (atomics); K = B * Lk key rows, or T when packed.  db_part: [H][B * gridDim.x][nb] the bias bins of each CTA, non-null iff a.dbias is.
+template <int DH, int PACK = T5_PADDED>
+__global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a, float* dkv_part, float* db_part, T5Packed pk) {
     pdl_wait();
     a.drop.resolve();
     extern __shared__ float t5_smem[];
@@ -176,33 +234,37 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a, f
     const int b = blockIdx.y / a.H, h = blockIdx.y % a.H;
     const int i0 = blockIdx.x * T5_ROWS, i = i0 + r;
     const int D = a.H * DH;
+    T5Span sp = t5_span<PACK>(a, pk, b);
+    // a query tile past the end of its sequence adds nothing: it skips the keys, unless its zero partials must be stored
+    if constexpr (PACK == T5_PACKED_SELF)
+        if (i0 >= sp.nq && !dkv_part) sp.nk = 0;
     if (a.bias) for (int e = tid; e < a.nb; e += T5_THREADS) { sbias[e] = a.bias[h * a.nb + e]; sdb[e] = 0.f; }
     float q[DH], dO[DH], dq[DH];
 #pragma unroll
     for (int d = 0; d < DH; ++d) { q[d] = 0.f; dO[d] = 0.f; dq[d] = 0.f; }
     float rmax = 0.f, rinv = 0.f, Dsum = 0.f;
-    if (i < a.Lq) {
-        t5_load_row<DH>(q, a.q + ((size_t)b * a.Lq + i) * a.ldq + h * DH);
-        t5_load_row<DH>(dO, a.dout + ((size_t)b * a.Lq + i) * a.lddo + h * DH);
+    if (i < (PACK != T5_PADDED ? sp.nq : a.Lq)) {
+        t5_load_row<DH>(q, a.q + t5_qrow<PACK>(a, sp, b, i) * a.ldq + h * DH);
+        t5_load_row<DH>(dO, a.dout + t5_qrow<PACK>(a, sp, b, i) * a.lddo + h * DH);
         float o[DH];
-        t5_load_row<DH>(o, a.out + ((size_t)b * a.Lq + i) * a.ldo + h * DH);
+        t5_load_row<DH>(o, a.out + t5_qrow<PACK>(a, sp, b, i) * a.ldo + h * DH);
 #pragma unroll
         for (int d = 0; d < DH; ++d) Dsum = fmaf(dO[d], o[d], Dsum);   // rowsum(dO * O) = sum_j P_ij dP_ij
-        const float2 ml = reinterpret_cast<const float2*>(a.lse)[((size_t)b * a.H + h) * a.Lq + i];
+        const float2 ml = reinterpret_cast<const float2*>(a.lse)[t5_lse_at<PACK>(a, pk, sp, b, h, i)];
         rmax = ml.x; rinv = ml.y > 0.f ? __fdiv_rn(1.f, ml.y) : 0.f;
     }
     if (kq == 0) {
 #pragma unroll
         for (int d = 0; d < DH; ++d) { Qs[r * (DH + 1) + d] = q[d]; dOs[r * (DH + 1) + d] = dO[d]; }
     }
-    const uint32_t drow = (uint32_t)(((size_t)b * a.H + h) * a.Lq + i);
-    for (int j0 = 0; j0 < a.Lk; j0 += T5_KEYS) {
+    const uint32_t drow = t5_drop_row<PACK>(a, sp, b, h, i);
+    for (int j0 = 0; j0 < (PACK != T5_PADDED ? sp.nk : a.Lk); j0 += T5_KEYS) {
         __syncthreads();
-        t5_load_tile<DH>(Ks, Vs, a, b, h, j0, tid);
+        t5_load_tile<DH, PACK>(Ks, Vs, a, sp, b, h, j0, tid);
         for (int e = tid; e < T5_ROWS * (T5_KEYS + 1); e += T5_THREADS) { dSs[e] = 0.f; Pds[e] = 0.f; }
         __syncthreads();
-        if (i < a.Lq) {
-            for (int jj = kq; jj < T5_KEYS && j0 + jj < a.Lk; jj += 4) {
+        if (i < (PACK != T5_PADDED ? sp.nq : a.Lq)) {
+            for (int jj = kq; jj < T5_KEYS && j0 + jj < (PACK != T5_PADDED ? sp.nk : a.Lk); jj += 4) {
                 const float* kr = Ks + jj * (DH + 1);
                 const float* vr = Vs + jj * (DH + 1);
                 float qk = 0.f, dov = 0.f;
@@ -247,7 +309,7 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a, f
         // dK_j += sum_r dS_rj scale q_r ; dV_j += sum_r Pd_rj dO_r : thread (key jj, half of the head dims)
         {
             const int jj = tid >> 1, half = tid & 1;
-            if (j0 + jj < a.Lk) {
+            if (j0 + jj < (PACK != T5_PADDED ? sp.nk : a.Lk)) {
                 float gk[DH / 2], gv[DH / 2];
 #pragma unroll
                 for (int d = 0; d < DH / 2; ++d) { gk[d] = 0.f; gv[d] = 0.f; }
@@ -258,9 +320,10 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a, f
 #pragma unroll
                     for (int d = 0; d < DH / 2; ++d) { gk[d] = fmaf(ds, qr[d], gk[d]); gv[d] = fmaf(pd, gr[d], gv[d]); }
                 }
-                const size_t at = ((size_t)b * a.Lk + j0 + jj) * D + h * DH + half * (DH / 2);
+                const size_t at = t5_krow<PACK>(a, sp, b, j0, jj) * D + h * DH + half * (DH / 2);
                 if (dkv_part) {                           // this query tile's slot of the partials
-                    const size_t n = (size_t)a.B * a.Lk * D;
+                    size_t n;
+                    if constexpr (PACK != T5_PADDED) n = (size_t)pk.T * D; else n = (size_t)a.B * a.Lk * D;
                     float4* dkp = reinterpret_cast<float4*>(dkv_part + blockIdx.x * n + at);
                     float4* dvp = reinterpret_cast<float4*>(dkv_part + (gridDim.x + blockIdx.x) * n + at);
 #pragma unroll
@@ -280,8 +343,8 @@ __global__ void __launch_bounds__(T5_THREADS) t5_attn_bwd_kernel(T5AttnArgs a, f
         dq[d] += __shfl_xor_sync(0xffffffffu, dq[d], 1);
         dq[d] += __shfl_xor_sync(0xffffffffu, dq[d], 2);
     }
-    if (i < a.Lq) {
-        bf16* dst = a.dq + ((size_t)b * a.Lq + i) * a.lddq + h * DH;
+    if (i < (PACK != T5_PADDED ? sp.nq : a.Lq)) {
+        bf16* dst = a.dq + t5_qrow<PACK>(a, sp, b, i) * a.lddq + h * DH;
 #pragma unroll
         for (int d = 0; d < DH; d += 2)
             if (((d >> 1) & 3) == kq) *reinterpret_cast<uint32_t*>(dst + d) = pack_bf16(dq[d], dq[d + 1]);

@@ -157,6 +157,60 @@ def pack_jagged(items: torch.Tensor, offsets: torch.Tensor, targets: torch.Tenso
     return out
 
 
+def pack_tiger(user_ids: torch.Tensor, item_tokens: torch.Tensor, token_offsets: torch.Tensor, target_ids: torch.Tensor, max_items: int = 20,
+               num_tokens: "int | None" = None) -> Dict[str, torch.Tensor]:
+    """TIGER's ``pad_collate`` (genrec/trainers/tiger_trainer.py:27-80) without the pads, for ``Tiger.forward_jagged`` and
+    ``generate_jagged``: user b's semantic-id tokens are item_tokens[token_offsets[b] : token_offsets[b+1]] (three per item, in the
+    reference's order; int64), user_ids [B], target_ids [B, S].  Sequence b of the packed encoder memory is its user row followed by
+    its last min(n_b, 3 max_items) item tokens: pad_collate's row b (with the user token in front, as Tiger.forward puts it) without
+    its pads.  Returns user_input_ids [B], item_input_ids and token_type_ids [T] (types arange(n) % 3; the user row holds id 0, type
+    0, and forward_jagged puts the user embedding there), mem_offsets [B+1], the host int max_len, target_input_ids and
+    target_token_type_ids [B, S] (types arange(S)), and overflow (a 0-dim bool).  Every tensor lives on item_tokens' device.
+
+    Without ``num_tokens`` T is the packed total and max_len the longest sequence, read in one synchronisation.  With ``num_tokens``
+    T = num_tokens and max_len = 1 + 3 max_items, with no synchronisation (a captured call keeps fixed shapes): rows past the packed
+    total are idle, and a batch that does not fit sets ``overflow`` and is cut at T - do not use it."""
+    dev = item_tokens.device
+    for t in (user_ids, item_tokens, token_offsets, target_ids):
+        if t.dtype != torch.int64:
+            raise ValueError(f"pack_tiger: every input is int64 (got {t.dtype})")
+    if token_offsets.dim() != 1 or token_offsets.numel() < 2 or user_ids.numel() != token_offsets.numel() - 1:
+        raise ValueError("pack_tiger: token_offsets must be [B+1] with B >= 1 and user_ids [B]")
+    if target_ids.dim() != 2 or target_ids.shape[0] != user_ids.numel():
+        raise ValueError(f"pack_tiger: target_ids must be [B, S], got {tuple(target_ids.shape)}")
+    if int(max_items) < 1:
+        raise ValueError(f"pack_tiger: max_items must be positive, got {max_items}")
+    off = token_offsets.to(dev)
+    B, cap = off.numel() - 1, 3 * int(max_items)
+    lens = (off[1:] - off[:-1]).clamp(0, cap)
+    start = off[1:] - lens                                     # the last min(n_b, cap) tokens
+    mem_off = torch.zeros(B + 1, dtype=torch.int64, device=dev)
+    mem_off[1:] = torch.cumsum(lens + 1, 0)
+    if num_tokens is None:
+        total, longest = torch.stack([mem_off[-1], lens.max() + 1]).tolist()
+        T, max_len = int(total), int(longest)
+    else:
+        if int(num_tokens) < 1:
+            raise ValueError(f"num_tokens must be positive, got {num_tokens}")
+        T, max_len = int(num_tokens), 1 + cap
+    rows = torch.arange(T, dtype=torch.int64, device=dev)
+    b = torch.searchsorted(mem_off[1:], rows, right=True)      # sequence of each row; B for idle rows
+    bc = b.clamp(max=B - 1)
+    k = rows - mem_off[bc]                                     # 0 = the user row
+    item = (b < B) & (k > 0)
+    if item_tokens.numel():
+        tok = (start[bc] + k - 1).clamp(0, item_tokens.numel() - 1)
+        ids = torch.where(item, item_tokens[tok], torch.zeros_like(rows))
+    else:
+        ids = torch.zeros_like(rows)
+    types = torch.where(item, (k - 1) % 3, torch.zeros_like(rows))
+    S = target_ids.shape[1]
+    return {"user_input_ids": user_ids.reshape(-1).to(dev), "item_input_ids": ids, "token_type_ids": types,
+            "mem_offsets": mem_off.clamp(max=T), "max_len": max_len, "target_input_ids": target_ids.to(dev),
+            "target_token_type_ids": torch.arange(S, dtype=torch.int64, device=dev).unsqueeze(0).expand(B, S).contiguous(),
+            "overflow": mem_off[-1] > T}
+
+
 def sample_negatives(num_items: int, n: int, *, probs: Optional[torch.Tensor] = None, generator: Optional[torch.Generator] = None,
                      device=None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """The shared negatives of one sampled-softmax step: ``(negatives [n] int64 in 1..num_items, log_q [num_items + 1] fp32 | None)``,

@@ -100,11 +100,58 @@ def attention_core_bwd(Q, K, V, H, bias, bucket, key_pad, causal, scale, out, ls
     return dq, dk, dv, dbias
 
 
+def _jagged_shape(Q, K, max_len):
+    """(B, T, Lq) of a packed call: Q [T, D] (self-attention, Lq = 0: the queries are the packed rows) or [B, Lq, D] (cross-attention,
+    the keys K [T, D] are packed)."""
+    return (None, Q.shape[0], 0) if Q.dim() == 2 else (Q.shape[0], K.shape[0], Q.shape[1])
+
+
+def attention_core_fwd_jagged(Q, K, V, H, bias, bucket, offsets, max_len, causal, scale, p=0.0, seed=0, site=0):
+    """``attention_core_fwd`` on a packed batch (``grb_t5_attention_forward_jagged``): sequence b is rows offsets[b] .. offsets[b+1]-1
+    of the packed K / V [T, *] (and of Q [T, *] in self-attention; Q [B, Lq, *] stays dense in cross-attention).  bucket is
+    ``relative_position_buckets(Lq or max_len, max_len)``.  -> (out like Q, softmax statistics [H, T, 2] or [B, H, Lq, 2])."""
+    _, T, Lq = _jagged_shape(Q, K, max_len)
+    B = offsets.numel() - 1
+    D = Q.shape[-1]
+    out = torch.empty(*Q.shape[:-1], D, dtype=torch.bfloat16, device=Q.device)
+    lse = torch.empty(*((H, T) if Lq == 0 else (B, H, Lq)), 2, dtype=torch.float32, device=Q.device)
+    nb = bias.shape[1] if bias is not None else 0
+    with torch.cuda.device(Q.device):
+        check(_lib.load().grb_t5_attention_forward_jagged(
+            ptr(Q), ptr(K), ptr(V), ptr(offsets), B, T, int(max_len), Lq, H, D // H, Q.stride(-2), K.stride(-2), V.stride(-2), ptr(bias),
+            ptr(bucket), bucket.numel() if bucket is not None else 0, nb, 1 if causal else 0, float(scale), float(p), int(seed), None,
+            int(site) & 0xFFFFFFFF, ptr(out), D, ptr(lse), stream_ptr(Q.device)))
+    return out, lse
+
+
+def attention_core_bwd_jagged(Q, K, V, H, bias, bucket, offsets, max_len, causal, scale, out, lse, dout, p=0.0, seed=0, site=0):
+    """``attention_core_bwd`` on a packed batch: -> (dq like Q bf16, dk, dv [T, D] fp32, dbias)."""
+    _, T, Lq = _jagged_shape(Q, K, max_len)
+    B = offsets.numel() - 1
+    D = Q.shape[-1]
+    dq = torch.empty(*Q.shape[:-1], D, dtype=torch.bfloat16, device=Q.device)
+    dk = torch.empty(T, D, dtype=torch.float32, device=Q.device)
+    dv = torch.empty(T, D, dtype=torch.float32, device=Q.device)
+    dbias = torch.zeros_like(bias) if bias is not None else None
+    nb = bias.shape[1] if bias is not None else 0
+    lib = _lib.load()
+    ws = torch.empty(lib.grb_t5_attention_backward_workspace_bytes_jagged(B, T, int(max_len), Lq, H, D // H, nb), dtype=torch.uint8,
+                     device=Q.device)
+    with torch.cuda.device(Q.device):
+        check(lib.grb_t5_attention_backward_jagged(
+            ptr(Q), ptr(K), ptr(V), ptr(offsets), B, T, int(max_len), Lq, H, D // H, Q.stride(-2), K.stride(-2), V.stride(-2), ptr(bias),
+            ptr(bucket), bucket.numel() if bucket is not None else 0, nb, 1 if causal else 0, float(scale), float(p), int(seed), None,
+            int(site) & 0xFFFFFFFF, ptr(out), D, ptr(lse), ptr(dout), D, ptr(dq), D, ptr(dk), ptr(dv), ptr(dbias),
+            ptr(ws) if ws.numel() else None, stream_ptr(Q.device)))
+    return dq, dk, dv, dbias
+
+
 class _T5AttnFn(torch.autograd.Function):
-    """T5Attention.forward as a unit: projections, attention core, output projection."""
+    """T5Attention.forward as a unit: projections, attention core, output projection.  With ``offsets`` [B+1] (device) and
+    ``max_len`` the batch is packed: the query rows [T, D] in self-attention, the key / value rows [T, D] in cross-attention."""
 
     @staticmethod
-    def forward(ctx, query, key, value, key_pad, causal, H, p, bucket, wq, wk, wv, wo, rel_w, fused_kv):
+    def forward(ctx, query, key, value, key_pad, causal, H, p, bucket, wq, wk, wv, wo, rel_w, fused_kv, offsets=None, max_len=0):
         require_cuda(query)
         ensure_device(query.device)
         dev = query.device
@@ -129,23 +176,34 @@ class _T5AttnFn(torch.autograd.Function):
         _CALLS["n"] += 1
         site = _CALLS["n"]
         scale = 1.0 / math.sqrt(D // H)
-        A, lse = attention_core_fwd(Q, K, V, H, bias, bucket, key_pad, causal, scale, p, seed, site)
+        if offsets is None:
+            A, lse = attention_core_fwd(Q, K, V, H, bias, bucket, key_pad, causal, scale, p, seed, site)
+        else:
+            A, lse = attention_core_fwd_jagged(Q, K, V, H, bias, bucket, offsets, max_len, causal, scale, p, seed, site)
         out, _ = Fn.linear_fwd(A, wob, _zero_bias(D, dev), 0)
         ctx.save_for_backward(xq, xk, xv, Q, K, V, A, lse, wqb, wkb, wvb if wvb is not None else wqb, wob, bias if bias is not None else lse,
-                              bucket if bucket is not None else lse, key_pad if key_pad is not None else lse)
+                              bucket if bucket is not None else lse, key_pad if key_pad is not None else lse,
+                              offsets if offsets is not None else lse)
         ctx.cfg = (H, p, seed, site, scale, causal, fused_kv, bias is not None, key_pad is not None, value is key)
+        ctx.jagged = (offsets is not None, max_len)
         return out.float()
 
     @staticmethod
     def backward(ctx, dout):
-        xq, xk, xv, Q, K, V, A, lse, wqb, wkb, wvb, wob, bias, bucket, key_pad = ctx.saved_tensors
+        xq, xk, xv, Q, K, V, A, lse, wqb, wkb, wvb, wob, bias, bucket, key_pad, offsets = ctx.saved_tensors
         H, p, seed, site, scale, causal, fused_kv, has_bias, has_pad, same_kv = ctx.cfg
+        jagged, max_len = ctx.jagged
         bias = bias if has_bias else None
         bucket = bucket if has_bias else None
         key_pad = key_pad if has_pad else None
         dyb = Fn.cast_rows_bf16(dout.contiguous().float())
         dA, dwo, _ = Fn.linear_bwd(dyb, wob, A)
-        dQ, dK32, dV32, dbias = attention_core_bwd(Q, K, V, H, bias, bucket, key_pad, causal, scale, A, lse, Fn.cast_rows_bf16(dA), p, seed, site)
+        if jagged:
+            dQ, dK32, dV32, dbias = attention_core_bwd_jagged(Q, K, V, H, bias, bucket, offsets, max_len, causal, scale, A, lse,
+                                                              Fn.cast_rows_bf16(dA), p, seed, site)
+        else:
+            dQ, dK32, dV32, dbias = attention_core_bwd(Q, K, V, H, bias, bucket, key_pad, causal, scale, A, lse, Fn.cast_rows_bf16(dA), p,
+                                                       seed, site)
         if fused_kv:
             dKV = Fn.cast_rows_bf16(torch.cat([dK32, dV32], dim=-1))
             dx_kv, dwkv, _ = Fn.linear_bwd(dKV, wkb, xq)
@@ -157,7 +215,7 @@ class _T5AttnFn(torch.autograd.Function):
             dkey, dwk, _ = Fn.linear_bwd(Fn.cast_rows_bf16(dK32), wkb, xk)
             dvalue, dwv, _ = Fn.linear_bwd(Fn.cast_rows_bf16(dV32), wvb, xv)
         drel = dbias.reshape(-1, 1) if has_bias else None
-        return dquery, dkey, dvalue, None, None, None, None, None, dwq, dwk, dwv, dwo, drel, None
+        return dquery, dkey, dvalue, None, None, None, None, None, dwq, dwk, dwv, dwo, drel, None, None, None
 
 
 class T5Attention(nn.Module):

@@ -14,6 +14,9 @@ torch.
 ``generate`` projects the encoder memory's cross-attention K and V once per user (not once per beam, as the reference's expanded
 memory does), runs step 0 on one row per user, and otherwise computes row for row what ``tiger_decode.generate`` on this module
 computes: the same kernels on the same rows, so the beams and log-probabilities are the same bits.
+
+``forward_jagged`` / ``generate_jagged`` / ``retrieve_jagged`` take the encoder memory packed (``data.pack_tiger``): each user's
+rows without the pads of the batch's longest history, through the packed T5 attention core (INTEGRATION.md).
 """
 from __future__ import annotations
 
@@ -27,7 +30,7 @@ from torch import nn
 from . import _lib
 from . import functional as Fn
 from . import tiger_decode as td
-from .t5_attention import T5Attention, _T5AttnFn, _bucket_map, _zero_bias, attention_core_fwd
+from .t5_attention import T5Attention, _T5AttnFn, _bucket_map, _zero_bias, attention_core_fwd, attention_core_fwd_jagged
 from .tiger_decode import TigerGenerationOutput
 
 __all__ = ["Tiger", "TigerOutput", "TigerGenerationOutput"]
@@ -252,28 +255,30 @@ class Tiger(nn.Module):
         x = bos if tgt_ids is None else torch.cat([bos, self._sem_emb(tgt_ids, tgt_type)], dim=1)
         return _LinearFn.apply(F.dropout(self.norm(x), self._p(), self.training), self.in_proj.weight)
 
-    def _self_attn(self, blk, x, pad, causal):
+    def _self_attn(self, blk, x, pad, causal, jagged=None):
+        """jagged = (offsets, max_len): x [T, D] holds the packed sequences (no key padding)"""
         a = blk.self_attn.attn
-        L = x.shape[1]
+        L = x.shape[1] if jagged is None else jagged[1]
         bucket = _bucket_map(L, L, a.num_relative_buckets, a.max_distance, x.device)
         kp = pad.to(torch.uint8).contiguous() if pad is not None else None
         out = _T5AttnFn.apply(blk.norm1(x), None, None, kp, causal, a.n_heads, self._p(), bucket, a.q.weight, a.kv.weight, None,
-                              a.o.weight, a.rel_bias.weight, True)
+                              a.o.weight, a.rel_bias.weight, True, *(jagged or ()))
         return x + F.dropout(out, self._p(), self.training)
 
     def _ffn(self, blk, x):
         return _FfnFn.apply(x, blk.norm2.weight, blk.ff.wi.weight, blk.ff.wo.weight, self._p())
 
-    def _encoder(self, x, pad):
+    def _encoder(self, x, pad, jagged=None):
         for blk in self.transformer.encoder.layers:                                      # transformer.py:363-365, :303-324
-            x = self._ffn(blk, self._self_attn(blk, x, pad, False))
+            x = self._ffn(blk, self._self_attn(blk, x, pad, False, jagged))
         return x
 
-    def _cross(self, blk, x, memory, memory_pad):
+    def _cross(self, blk, x, memory, memory_pad, jagged=None):
+        """jagged = (offsets, max_len): memory [T, D] holds the packed sequences, memory_pad is None"""
         a = blk.cross_attn.attn
-        kp = memory_pad.to(torch.uint8).contiguous()
+        kp = memory_pad.to(torch.uint8).contiguous() if memory_pad is not None else None
         out = _T5AttnFn.apply(blk.norm_cross(x), memory, memory, kp, False, a.n_heads, self._p(), None, a.q.weight, a.k.weight, a.v.weight,
-                              a.o.weight, None, False)
+                              a.o.weight, None, False, *(jagged or ()))
         return x + F.dropout(out, self._p(), self.training)
 
     def _decoder(self, x, cross):
@@ -282,6 +287,75 @@ class Tiger(nn.Module):
             x = cross(i, blk, x)
             x = self._ffn(blk, x)
         return x
+
+    # ---- packed (jagged) encoder memory
+    def _check_jagged(self, what, user_input_ids, item_input_ids, token_type_ids, mem_offsets, max_len):
+        """ValueError before anything runs -> (user ids [B], offsets on the device)"""
+        if not isinstance(token_type_ids, torch.Tensor) or token_type_ids.shape != item_input_ids.shape:
+            raise ValueError(f"{what}: token_type_ids must be [T] like item_input_ids, got "
+                             f"{tuple(token_type_ids.shape) if isinstance(token_type_ids, torch.Tensor) else token_type_ids!r}")
+        users = user_input_ids.reshape(-1)
+        if isinstance(mem_offsets, torch.Tensor) and mem_offsets.dim() == 1:
+            if users.numel() != mem_offsets.numel() - 1:
+                raise ValueError(f"{what}: {users.numel()} user ids for {mem_offsets.numel() - 1} sequences")
+            if not mem_offsets.is_cuda and bool(((mem_offsets[1:] - mem_offsets[:-1]) == 0).any()):
+                raise ValueError(f"{what}: every sequence starts with its user row (length >= 1)")
+        return users, Fn.check_jagged_batch(what, item_input_ids, mem_offsets, max_len, self.max_pos)
+
+    def _encode_context_jagged(self, users, item_input_ids, token_type_ids, offsets, max_len):
+        """-> encoder memory [T, attn_dim] fp32: row offsets[b] is user b's token (its item_input_ids / token_type_ids are ignored),
+        the rows behind it its item tokens - Tiger.forward's [user, items] without the pads."""
+        x = self._sem_emb(item_input_ids, token_type_ids)
+        user_emb = self.user_id_embedding.emb(users % self.num_user_embeddings)
+        x = x.index_put((offsets[:-1].clamp(max=x.size(0) - 1),), user_emb)
+        x = _LinearFn.apply(F.dropout(self.norm_context(x), self._p(), self.training), self.in_proj_context.weight)
+        return self._encoder(x, None, (offsets, max_len))
+
+    def forward_jagged(self, user_input_ids, item_input_ids, token_type_ids, mem_offsets, max_len: int, target_input_ids,
+                       target_token_type_ids) -> TigerOutput:
+        """``forward`` on a packed encoder memory (``data.pack_tiger``): user b's memory is rows mem_offsets[b] .. mem_offsets[b+1]-1
+        of item_input_ids / token_type_ids [T] (its user row first), at most max_len rows; user_input_ids [B] (or [B, 1]); the
+        decoder input stays [B, S].  Returns logits [B, S+1, V] and the reference's loss (sum over positions, mean over users): on the
+        same users the values of ``forward`` on pad_collate's batch, without computing the pads.  Rows past mem_offsets[B] are idle.
+        Dropout draws its encoder self-attention masks by token row, so under dropout a packed batch draws other masks than the
+        padded one.  Refusals are ValueError before anything runs; device offsets are not read on the host."""
+        users, offsets = self._check_jagged("Tiger.forward_jagged", user_input_ids, item_input_ids, token_type_ids, mem_offsets, max_len)
+        B = users.numel()
+        memory = self._encode_context_jagged(users, item_input_ids, token_type_ids, offsets, max_len)
+        tgt = self._decoder_input(B, target_input_ids, target_token_type_ids)
+        out = self._decoder(tgt, lambda i, blk, x: self._cross(blk, x, memory, None, (offsets, max_len)))
+        return self._output(B, out, target_input_ids, target_token_type_ids)
+
+    @torch.no_grad()
+    def generate_jagged(self, user_input_ids, item_input_ids, token_type_ids, mem_offsets, max_len: int, temperature: float = 0.2,
+                        n_top_k_candidates: int = 10, valid_item_ids=None, use_trie: bool = True,
+                        generator: Optional[torch.Generator] = None) -> TigerGenerationOutput:
+        """``generate`` on a packed encoder memory (the layout of ``forward_jagged``): the same beams and log-probabilities as
+        ``generate`` on the padded batch of the same users.  No host synchronisation once the trie is built, so with device offsets a
+        warmed-up call can be captured in a CUDA graph and replayed with other ids and offsets of the same T and max_len."""
+        users, offsets = self._check_jagged("Tiger.generate_jagged", user_input_ids, item_input_ids, token_type_ids, mem_offsets, max_len)
+        out, _, _ = self._generate(users, item_input_ids, token_type_ids, None, temperature, n_top_k_candidates, valid_item_ids, use_trie,
+                                   generator, jagged=(offsets, max_len))
+        return out
+
+    @torch.no_grad()
+    def retrieve_jagged(self, user_input_ids, item_input_ids, token_type_ids, mem_offsets, max_len: int, num_candidates: int = 500,
+                        valid_item_ids=None, temperature: float = 0.2, generator: Optional[torch.Generator] = None):
+        """``retrieve`` on a packed encoder memory: (items [B, K], sem_ids [B, K, sem_id_dim], log_probas [B, K])."""
+        users, offsets = self._check_jagged("Tiger.retrieve_jagged", user_input_ids, item_input_ids, token_type_ids, mem_offsets, max_len)
+        out, nodes, trie = self._generate(users, item_input_ids, token_type_ids, None, temperature, num_candidates, valid_item_ids, True,
+                                          generator, want_nodes=True, jagged=(offsets, max_len))
+        return trie.rows(nodes), out.sem_ids, out.log_probas
+
+    def _output(self, B, out, target_input_ids, target_token_type_ids) -> TigerOutput:
+        logits = _HeadFn.apply(out, self.output_head.weight)
+        loss = None
+        if target_input_ids is not None and target_input_ids.shape[1] == self.sem_id_dim:   # tiger.py:232-242
+            target_vocab_ids = target_token_type_ids * self.num_item_embeddings + target_input_ids
+            loss_logits = logits[:, :-1, :]
+            loss = F.cross_entropy(loss_logits.reshape(-1, loss_logits.size(-1)), target_vocab_ids.reshape(-1),
+                                   reduction="none").reshape(B, -1).sum(dim=1).mean()
+        return TigerOutput(logits=logits, loss=loss)
 
     # ---- the reference's interface
     def forward(self, user_input_ids, item_input_ids, token_type_ids, target_input_ids, target_token_type_ids, seq_mask) -> TigerOutput:
@@ -292,14 +366,7 @@ class Tiger(nn.Module):
         tgt = self._decoder_input(B, target_input_ids, target_token_type_ids)
         memory = self._encoder(src, pad)
         out = self._decoder(tgt, lambda i, blk, x: self._cross(blk, x, memory, pad))
-        logits = _HeadFn.apply(out, self.output_head.weight)
-        loss = None
-        if target_input_ids is not None and target_input_ids.shape[1] == self.sem_id_dim:   # tiger.py:232-242
-            target_vocab_ids = target_token_type_ids * self.num_item_embeddings + target_input_ids
-            loss_logits = logits[:, :-1, :]
-            loss = F.cross_entropy(loss_logits.reshape(-1, loss_logits.size(-1)), target_vocab_ids.reshape(-1),
-                                   reduction="none").reshape(B, -1).sum(dim=1).mean()
-        return TigerOutput(logits=logits, loss=loss)
+        return self._output(B, out, target_input_ids, target_token_type_ids)
 
     def _encode_context(self, user_input_ids, item_input_ids, token_type_ids, seq_mask=None):
         if seq_mask is None:
@@ -334,8 +401,9 @@ class Tiger(nn.Module):
         return trie.rows(nodes), out.sem_ids, out.log_probas
 
     def _generate(self, user_input_ids, item_input_ids, token_type_ids, seq_mask, temperature, K, valid_item_ids, use_trie, generator,
-                  want_nodes=False):
-        """-> (beams, final trie nodes if want_nodes else None, trie); the arguments are checked before anything runs."""
+                  want_nodes=False, jagged=None):
+        """-> (beams, final trie nodes if want_nodes else None, trie); the arguments are checked before anything runs.  jagged =
+        (offsets, max_len): the memory is packed (``generate_jagged``)."""
         td.check_width(K, td.candidates_per_beam(K, self.num_item_embeddings))
         B = user_input_ids.size(0)
         dev = user_input_ids.device
@@ -347,11 +415,14 @@ class Tiger(nn.Module):
                     raise ValueError("the trie is built from valid_item_ids on the first call")
                 trie = td.TrieCSR.build(valid_item_ids).to(dev)
                 self._grb_trie = trie
-        memory, memory_pad = self._encode_context(user_input_ids, item_input_ids, token_type_ids, seq_mask)
-        kp = memory_pad.to(torch.uint8).contiguous()
+        if jagged is None:
+            memory, memory_pad = self._encode_context(user_input_ids, item_input_ids, token_type_ids, seq_mask)
+            kp = memory_pad.to(torch.uint8).contiguous()
+        else:
+            memory = self._encode_context_jagged(user_input_ids, item_input_ids, token_type_ids, *jagged)
         xm = Fn.cast_rows_bf16(memory.contiguous())
-        D, Lm = self.attn_dim, memory.size(1)
-        mem_kv = []                                                  # per decoder block: K, V [B, 1+N, D] bf16
+        D = self.attn_dim
+        mem_kv = []                                                  # per decoder block: K, V [B, 1+N, D] (packed: [T, D]) bf16
         for blk in self.transformer.decoder.layers:
             a = blk.cross_attn.attn
             Km, _ = Fn.linear_fwd(xm, Fn.cast_bf16(a.k.weight), _zero_bias(D, dev), 0)
@@ -366,7 +437,10 @@ class Tiger(nn.Module):
             R, S = x.size(0) // B, x.size(1)
             wq, wo = wcache[i]
             Q, _ = Fn.linear_fwd(Fn.cast_rows_bf16(blk.norm_cross(x).contiguous()), wq, _zero_bias(D, dev), 0)
-            A, _ = attention_core_fwd(Q.view(B, R * S, D), mem_kv[i][0], mem_kv[i][1], H, None, None, kp, False, scale)
+            if jagged is None:
+                A, _ = attention_core_fwd(Q.view(B, R * S, D), mem_kv[i][0], mem_kv[i][1], H, None, None, kp, False, scale)
+            else:
+                A, _ = attention_core_fwd_jagged(Q.view(B, R * S, D), mem_kv[i][0], mem_kv[i][1], H, None, None, *jagged, False, scale)
             out, _ = Fn.linear_fwd(A.view(B * R, S, D), wo, _zero_bias(D, dev), 0)
             return x + out.float()
 

@@ -463,6 +463,30 @@ int grb_t5_attention_backward(const void* q, const void* k, const void* v, int B
                               float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t site, const void* out, int ldo,
                               const float* lse, const void* dout, int lddo, void* dq, int lddq, float* dk, float* dv, float* dbias,
                               void* workspace, void* stream);
+/* The same core on a packed (jagged) batch: sequence b is rows offsets[b] .. offsets[b+1]-1 of T packed rows (offsets [B+1] int64
+ * on the device, never read on the host; a malformed one is clamped to [0, T) and to max_len rows, giving wrong numbers but no
+ * access outside the rows).  No key padding: every row of a sequence is a key.
+ *   Lq = 0, self-attention (TIGER's encoder): q / k / v / out [T, ld]; queries and keys are the rows of one sequence, i and j count
+ *       from its first row, and bucket [bucket_len >= 2 max_len - 1] holds the bucket of delta = j - i at index delta + max_len - 1
+ *       (relative_position_buckets(max_len, max_len)), so a sequence gets the padded batch's bias when the pads follow the items.
+ *       lse [H, T, 2].  Dropout is keyed by the query's token row: an equal batch draws other masks than the padded one.
+ *   Lq > 0, cross-attention (TIGER's decoder): q / out [B, Lq, ld] dense, k / v [T, ld] the packed keys of each user;
+ *       lse [B, H, Lq, 2]; a bias table, if any, needs bucket_len >= Lq + max_len - 1.  The dropout masks equal the padded ones.
+ * Backward: dq like q; dk, dv fp32 [T, H * head_dim] (overwritten); dbias [H, num_buckets] +=; the sums run in the padded order, so
+ * two calls give the same bits.  Rows outside every sequence ([0, offsets[0]) and [offsets[B], T)) are zeros in out (Lq = 0),
+ * dq (Lq = 0), dk and dv.  workspace: grb_t5_attention_backward_workspace_bytes_jagged(B, T, max_len, Lq, H, head_dim, num_buckets).
+ * GRB_EINVAL before any launch: a null pointer, B outside [1, 65,535] (the backward: B * H > 65,535), head_dim not 32 or 64, a
+ * bucket map shorter than stated. */
+int grb_t5_attention_forward_jagged(const void* q, const void* k, const void* v, const int64_t* offsets, int B, int T, int max_len, int Lq,
+                                    int H, int head_dim, int ldq, int ldk, int ldv, const float* bias, const int32_t* bucket,
+                                    int bucket_len, int num_buckets, int causal, float scale, float dropout_p, uint64_t seed,
+                                    const uint64_t* seed_dev, uint32_t site, void* out, int ldo, float* lse, void* stream);
+size_t grb_t5_attention_backward_workspace_bytes_jagged(int B, int T, int max_len, int Lq, int H, int head_dim, int num_buckets);
+int grb_t5_attention_backward_jagged(const void* q, const void* k, const void* v, const int64_t* offsets, int B, int T, int max_len, int Lq,
+                                     int H, int head_dim, int ldq, int ldk, int ldv, const float* bias, const int32_t* bucket,
+                                     int bucket_len, int num_buckets, int causal, float scale, float dropout_p, uint64_t seed,
+                                     const uint64_t* seed_dev, uint32_t site, const void* out, int ldo, const float* lse, const void* dout,
+                                     int lddo, void* dq, int lddq, float* dk, float* dv, float* dbias, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ TIGER constrained beam step
  * The per-step post-processing of Tiger.generate (genrec/models/tiger.py:364-441), host-bound Python loops in the reference.
