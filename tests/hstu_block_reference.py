@@ -165,15 +165,17 @@ def cast_colsum(dy, p=0.0, seed=0, site_=0):
     return {"dyb_exact": dyb, "db": dyb.double().sum(0), "a_db": T * ACC * dyb.double().abs().sum(0), "drop": drop}
 
 
-def linear_dact_backward(dyb, w, z, p=0.0, seed=0, site_=0):
-    """g = bf16(dropmask(dyb w) silu'(z)) (TcEpiDAct<1>): dyb [T, K] bf16, w [K, N] bf16, z [T, N] bf16.  -> "g", "a_g"."""
+def linear_dact_backward(dyb, w, z, p=0.0, seed=0, site_=0, act=1):
+    """g = bf16(dropmask(dyb w) act'(z)) (TcEpiDAct<act>: 1 SiLU, 2 ReLU): dyb [T, K] bf16, w [K, N] bf16, z [T, N] bf16.
+    -> "g", "a_g"."""
     DY, W, Z = dyb.double(), w.double(), z.double()
     T, K = DY.shape
     acc = DY @ W
-    d = dsilu(Z)
+    d = dsilu(Z) if act == 1 else (Z > 0).double()
     km = keep(range(T), W.shape[1], p, seed, site_, DY.device)
     g = acc * d * km
-    a = U * g.abs() + (K * ACC * (DY.abs() @ W.abs()) * d.abs() + SILU_SLACK * acc.abs() * (1 + Z.abs())) * km
+    slack = SILU_SLACK * acc.abs() * (1 + Z.abs()) if act == 1 else 0.0
+    a = U * g.abs() + (K * ACC * (DY.abs() @ W.abs()) * d.abs() + slack) * km
     return {"g": g, "a_g": a}
 
 

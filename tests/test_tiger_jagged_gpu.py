@@ -146,8 +146,9 @@ def _model(cfg, seed=7):
     return m.to(DEV)
 
 
-def _padded_and_packed(cfg, B, n_items, seed, lengths=None):
-    """tp.batch's padded batch (or one with the given item counts) and the same users packed by data.pack_tiger"""
+def _padded_and_packed(cfg, B, n_items, seed, lengths=None, num_tokens=None):
+    """tp.batch's padded batch (or one with the given item counts) and the same users packed by data.pack_tiger (into num_tokens
+    rows, the rest idle, when given)"""
     from genrec_b200.data import pack_tiger
     from tests import tiger_params as tp
     b = tp.batch(cfg, B, n_items, seed)
@@ -164,7 +165,8 @@ def _padded_and_packed(cfg, B, n_items, seed, lengths=None):
     toks = torch.cat([b["item_input_ids"][i, :int(lens[i])] for i in range(B)])
     off = torch.zeros(B + 1, dtype=torch.int64)
     off[1:] = lens.cumsum(0)
-    pk = pack_tiger(b["user_input_ids"].view(-1).to(DEV), toks.to(DEV), off.to(DEV), b["target_input_ids"].to(DEV), max_items=n_items)
+    pk = pack_tiger(b["user_input_ids"].view(-1).to(DEV), toks.to(DEV), off.to(DEV), b["target_input_ids"].to(DEV), max_items=n_items,
+                    num_tokens=num_tokens)
     # the padded batch at the width of its longest history, as pad_collate makes it
     width = int(lens.max())
     padded = {k: v.to(DEV) for k, v in b.items()}
