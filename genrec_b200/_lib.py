@@ -166,6 +166,17 @@ SIGNATURES = {
     "grb_t5_attention_forward_jagged": (c_int, [c_void_p] * 4 + [c_int] * 9 + [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_u64,
                                                                              c_void_p, C.c_uint32, c_void_p, c_int, c_void_p, c_void_p]),
     "grb_t5_attention_backward_workspace_bytes_jagged": (c_size_t, [c_int] * 7),
+    "grb_post_layernorm_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "grb_post_layernorm_backward": (c_int, [c_void_p] * 4 + [c_int, c_int] + [c_void_p] * 5),
+    "grb_cobra_pack_texts": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_cobra_text_rows": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_seg_layernorm_mean_forward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_float, c_int, c_void_p, c_void_p, c_void_p]),
+    "grb_seg_layernorm_mean_backward_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "grb_seg_layernorm_mean_backward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                                c_void_p, c_void_p]),
+    "grb_l2norm_forward": (c_int, [c_void_p, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),
+    "grb_l2norm_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p]),
+    "grb_infonce_forward_backward": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_t5_attention_backward_jagged": (c_int, [c_void_p] * 4 + [c_int] * 9 + [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_u64,
                                                                               c_void_p, C.c_uint32, c_void_p, c_int, c_void_p, c_void_p, c_int,
                                                                               c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -1,0 +1,481 @@
+"""COBRA (SURVEY.md section 8): drop-in mirror of ``genrec/models/cobra.py:47-529`` for training, with its ``LightT5Encoder``
+(``genrec/modules/encoder.py:15-105``).
+
+Same constructor arguments, parameter and buffer names / shapes (a reference checkpoint loads with ``strict=True``), ``forward``
+-> ``CobraOutput`` and ``generate_itemvec`` as the reference's ``Cobra``; ``encode_items`` adds the catalog vectors BeamFusion needs.
+Bind it with
+
+    import genrec.models.cobra, genrec_b200.cobra
+    genrec.models.cobra.Cobra = genrec_b200.cobra.Cobra
+
+Item-text encoder: the texts are packed into token rows on the device (``functional.cobra_pack_texts``): a text is its leading
+non-zero tokens and the texts of pad items have none, so neither text pads nor pad items are encoded (the reference's key mask and
+pooling keep both out of every output).  A text where a non-zero token follows a zero is refused with ValueError.  The projections
+and the ReLU FFN are the wgmma GEMMs of this library (ReLU and the hidden dropout in the GEMM epilogue, the output dropout and the
+residual in the second GEMM's), attention is the packed T5 core at head dim 96 (no bias, not causal), the post-LN residual norms
+the LayerNorm row kernels, the final LayerNorm and the mean over each text one segmented kernel, then the ``proj`` GEMM and an L2
+normalisation kernel.
+
+Decoder: the interleaved [sparse ids of item t, dense vector of item t] sequence (torch gathers), self-attention on the padded T5
+core (causal, key padding, no bias), the cross-attention over the empty memory as the bias add it reduces to (its projection
+weights get zero gradients, as in the reference), post-LN and the ReLU FFN as in the encoder.
+
+Heads: three 384 -> 256 GEMMs on their gathered rows with a cross-entropy in torch (ignore_index = pad_id); the in-batch InfoNCE
+is a GEMM for the scores, one row kernel for the loss and dS, and a GEMM for dpred.  bf16 operands, fp32 accumulation.  The
+embedding gathers, the residual adds, the dropouts on the residual branches and the metrics stay in torch.  Dropout seeds come
+from torch's CPU generator, so ``torch.manual_seed`` makes a step reproducible bit for bit.
+
+``generate`` and ``beam_fusion`` are not implemented here (NotImplementedError).
+"""
+from __future__ import annotations
+
+import math
+from typing import NamedTuple, Optional
+
+import torch
+import torch.nn.functional as F
+from torch import nn
+
+from . import _lib
+from . import functional as Fn
+from ._lib import ensure_device, require_cuda
+from .t5_attention import attention_core_bwd, attention_core_bwd_jagged, attention_core_fwd, attention_core_fwd_jagged
+
+__all__ = ["Cobra", "CobraOutput"]
+
+LN_DIMS = (64, 128, 192, 256, 384, 768)           # widths of the LayerNorm row kernels
+POOL_DIMS = (128, 192, 256, 384, 768)             # widths of the pooled LayerNorm kernel
+ENC_HEAD_DIMS = (32, 64, 96)
+DEC_HEAD_DIMS = (32, 64)
+MAX_ATTN_ROWS = 65535                             # texts x heads (or users x heads) of one attention backward
+
+
+class CobraOutput(NamedTuple):      # (cobra.py:12-26)
+    loss: torch.Tensor
+    loss_sparse: torch.Tensor
+    loss_dense: torch.Tensor
+    acc_correct: torch.Tensor
+    acc_total: torch.Tensor
+    recall_correct: torch.Tensor
+    recall_total: torch.Tensor
+    vec_cos_sim: torch.Tensor
+    codebook_entropy: torch.Tensor
+
+
+def _bad(msg: str) -> _lib.GrbError:
+    return _lib.GrbError(f"genrec_b200 error -1: {msg}")
+
+
+# ---- autograd pieces
+class _LayerNormFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, g, b, eps):
+        xc = x.detach().contiguous().float()
+        y, st = Fn.post_layernorm_fwd(xc, g.detach().contiguous(), b.detach().contiguous(), eps)
+        ctx.save_for_backward(xc, st, g)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xc, st, g = ctx.saved_tensors
+        dx, dg, db = Fn.post_layernorm_bwd(dy.contiguous().float(), xc, st, g.detach().contiguous())
+        return dx, dg, db, None
+
+
+class _LinearF32Fn(torch.autograd.Function):
+    """nn.Linear with an fp32 result: y = x W^T + b (the GEMM writes fp32, the bias is added in fp32)."""
+
+    @staticmethod
+    def forward(ctx, x, w, b):
+        ctx.empty = x.numel() == 0                    # no rows (no user has a second item): nothing to launch
+        if ctx.empty:
+            ctx.shapes = (x.shape, w.shape)
+            return x.new_zeros(*x.shape[:-1], w.shape[0], dtype=torch.float32)
+        xb = Fn.cast_rows_bf16(x.detach().contiguous().float())
+        wb = Fn.cast_bf16(w)
+        y, _, _ = Fn.linear_bwd(xb, wb.t().contiguous(), None, need_dw=False)
+        ctx.save_for_backward(xb, wb)
+        return y + b.detach()
+
+    @staticmethod
+    def backward(ctx, dy):
+        if ctx.empty:
+            xs, ws = ctx.shapes
+            return dy.new_zeros(xs), dy.new_zeros(ws), dy.new_zeros(ws[0])
+        xb, wb = ctx.saved_tensors
+        dyc = dy.contiguous().float()
+        dx, dw, _ = Fn.linear_bwd(Fn.cast_rows_bf16(dyc), wb, xb)
+        return dx, dw, dyc.reshape(-1, dyc.shape[-1]).sum(0)
+
+
+class _MhaFn(torch.autograd.Function):
+    """nn.MultiheadAttention self-attention (in_proj with bias, out_proj with bias) on the T5 core without a bias table.  Padded:
+    x [B, L, D] with key_pad [B, L] uint8 and causal; packed: x [T, D] with offsets [N+1] and max_len (no key padding)."""
+
+    @staticmethod
+    def forward(ctx, x, w_in, b_in, w_out, b_out, H, p, seed, site, key_pad, causal, offsets, max_len):
+        D = x.shape[-1]
+        xb = Fn.cast_rows_bf16(x.detach().contiguous().float())
+        wib, wob = Fn.cast_bf16(w_in), Fn.cast_bf16(w_out)
+        QKV, _ = Fn.linear_fwd(xb, wib, b_in.detach().contiguous(), 0)
+        Q, K, V = QKV[..., :D], QKV[..., D:2 * D], QKV[..., 2 * D:]
+        scale = 1.0 / math.sqrt(D // H)
+        if offsets is None:
+            A, lse = attention_core_fwd(Q, K, V, H, None, None, key_pad, causal, scale, p, seed, site)
+        else:
+            A, lse = attention_core_fwd_jagged(Q, K, V, H, None, None, offsets, max_len, causal, scale, p, seed, site)
+        out, _ = Fn.linear_fwd(A, wob, b_out.detach().contiguous(), 0)
+        ctx.save_for_backward(xb, QKV, A, lse, wib, wob, key_pad if key_pad is not None else lse, offsets if offsets is not None else lse)
+        ctx.cfg = (H, p, seed, site, scale, causal, key_pad is not None, offsets is not None, max_len)
+        return out.float()
+
+    @staticmethod
+    def backward(ctx, dout):
+        xb, QKV, A, lse, wib, wob, key_pad, offsets = ctx.saved_tensors
+        H, p, seed, site, scale, causal, has_pad, packed, max_len = ctx.cfg
+        D = A.shape[-1]
+        Q, K, V = QKV[..., :D], QKV[..., D:2 * D], QKV[..., 2 * D:]
+        dA, dwo, _ = Fn.linear_bwd(Fn.cast_rows_bf16(dout.contiguous().float()), wob, A)
+        dAb = Fn.cast_rows_bf16(dA)
+        if packed:
+            dQ, dK, dV, _ = attention_core_bwd_jagged(Q, K, V, H, None, None, offsets, max_len, causal, scale, A, lse, dAb, p, seed, site)
+        else:
+            dQ, dK, dV, _ = attention_core_bwd(Q, K, V, H, None, None, key_pad if has_pad else None, causal, scale, A, lse, dAb, p, seed,
+                                               site)
+        dqkv = torch.cat([dQ.float(), dK, dV], dim=-1)
+        dx, dwi, _ = Fn.linear_bwd(Fn.cast_rows_bf16(dqkv), wib, xb)
+        dyc = dout.contiguous().float()
+        return (dx, dwi, dqkv.reshape(-1, 3 * D).sum(0), dwo, dyc.reshape(-1, D).sum(0), None, None, None, None, None, None, None, None)
+
+
+class _FfnFn(torch.autograd.Function):
+    """x + drop(linear2(drop(relu(linear1(x))))) with biases: ReLU and the hidden dropout in the first GEMM's epilogue, the output
+    dropout and the residual in the second's."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, w2, b2, p_in, p_out, seed, site):
+        xc = x.detach().contiguous().float()
+        xb = Fn.cast_rows_bf16(xc)
+        w1b, w2b = Fn.cast_bf16(w1), Fn.cast_bf16(w2)
+        z, h = Fn.linear_fwd(xb, w1b, b1.detach().contiguous(), 2, p_in, seed, None, site)
+        y = Fn.linear_residual_fwd(h, w2b, b2.detach().contiguous(), xc, None, p_out, seed, None, site + 1)
+        ctx.save_for_backward(xb, z, h, w1b, w2b)
+        ctx.cfg = (p_in, p_out, seed, site)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xb, z, h, w1b, w2b = ctx.saved_tensors
+        p_in, p_out, seed, site = ctx.cfg
+        dyc = dy.contiguous().float()
+        dyb = Fn.cast_rows_bf16(dyc, None, p_out, seed, None, site + 1)
+        _, dw2, db2 = Fn.linear_bwd(dyb, w2b, h, need_dx=False)
+        dz = Fn.linear_dact_bwd(dyb, w2b, z, 2, p_in, seed, None, site)
+        dx, dw1, db1 = Fn.linear_bwd(dz, w1b, xb, dx_residual=dyc)
+        return dx, dw1, db1, dw2, db2, None, None, None, None
+
+
+class _SegLnMeanFn(torch.autograd.Function):
+    """pooled [N, D] = mean over the rows of each text of LayerNorm(x) (encoder.py:88-96 on packed rows)"""
+
+    @staticmethod
+    def forward(ctx, x, g, b, offsets, eps):
+        xc = x.detach().contiguous().float()
+        pooled, st = Fn.seg_layernorm_mean_fwd(offsets, xc, g.detach().contiguous(), b.detach().contiguous(), eps)
+        ctx.save_for_backward(xc, st, g, offsets)
+        return pooled
+
+    @staticmethod
+    def backward(ctx, dpooled):
+        xc, st, g, offsets = ctx.saved_tensors
+        dx, dg, db = Fn.seg_layernorm_mean_bwd(offsets, xc, st, g.detach().contiguous(), dpooled.contiguous().float())
+        return dx, dg, db, None, None
+
+
+class _L2NormFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        y, n = Fn.l2norm_fwd(x.detach().contiguous().float())
+        ctx.save_for_backward(y, n)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        y, n = ctx.saved_tensors
+        return Fn.l2norm_bwd(dy.contiguous().float(), y, n)
+
+
+class _InfoNceFn(torch.autograd.Function):
+    """mean over the Q rows of the in-batch InfoNCE of unit rows pred, gt [Q, d] (cobra.py:484-493); no gradient into gt"""
+
+    @staticmethod
+    def forward(ctx, pred, gt, lo, hi, inv_tau):
+        Q, d = pred.shape
+        Qp = (Q + 127) // 128 * 128                  # dS is the K operand of the dpred GEMM: at least two 64-wide K tiles
+        pb = Fn.cast_rows_bf16(pred.detach().contiguous())
+        gpad = torch.zeros(Qp, d, dtype=torch.bfloat16, device=pred.device)
+        gpad[:Q] = Fn.cast_rows_bf16(gt.detach().contiguous())
+        S, _, _ = Fn.linear_bwd(pb, gpad.t().contiguous(), None, need_dw=False)      # [Q, Qp] fp32 = pred gt^T
+        loss, dS = Fn.infonce_fwd_bwd(S, lo, hi, inv_tau)
+        ctx.save_for_backward(dS, gpad)
+        return (loss / Q).reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        dS, gpad = ctx.saved_tensors
+        dpred, _, _ = Fn.linear_bwd(dS, gpad, None, need_dw=False)
+        return dpred * g, None, None, None, None
+
+
+class _ZeroGrads(torch.autograd.Function):
+    """t unchanged; the other inputs get zero-tensor gradients (the cross-attention weights that an empty memory never reaches, and
+    the encoder when no text has a token: the reference's autograd gives them zero tensors, not None, which AdamW's weight decay
+    tells apart)."""
+
+    @staticmethod
+    def forward(ctx, t, *others):
+        ctx.shapes = [(o.shape, o.dtype, o.device) for o in others]
+        return t.view_as(t)
+
+    @staticmethod
+    def backward(ctx, g):
+        return (g, *[torch.zeros(s, dtype=dt, device=dev) for s, dt, dev in ctx.shapes])
+
+
+# ---- modules with the reference's parameter names (encoder.py:15-60, cobra.py:47-224)
+class _LightT5Encoder(nn.Module):
+    def __init__(self, n_layers, hidden_dim, output_dim, num_heads, ff_dim=2048, vocab_size=32128, max_seq_len=512, dropout=0.1):
+        super().__init__()
+        self.embedding = nn.Embedding(vocab_size, hidden_dim)
+        self.pos_embedding = nn.Embedding(max_seq_len, hidden_dim)
+        layer = nn.TransformerEncoderLayer(d_model=hidden_dim, nhead=num_heads, dim_feedforward=ff_dim, dropout=dropout, batch_first=True)
+        self.encoder = nn.TransformerEncoder(layer, num_layers=n_layers, enable_nested_tensor=False)
+        self.proj = nn.Linear(hidden_dim, output_dim)
+        self.layer_norm = nn.LayerNorm(hidden_dim)
+
+
+class _CobraEmbedding(nn.Module):
+    def __init__(self, id_vocab_size, n_codebooks=3, d_model=768, max_len=1024, pad_id=0):
+        super().__init__()
+        self.C, self.pad_id, self.id_vocab_size = n_codebooks, pad_id, id_vocab_size
+        self.id_embed = nn.Embedding(id_vocab_size * n_codebooks + 1, d_model, padding_idx=id_vocab_size * n_codebooks)
+        self.type_embed = nn.Embedding(2, d_model)
+        self.pos_embed = nn.Embedding(max_len, d_model)
+
+
+class _CobraDecoder(nn.Module):
+    def __init__(self, hidden_dim, n_layers, n_heads, ff_dim=2048, dropout=0.1):
+        super().__init__()
+        layer = nn.TransformerDecoderLayer(d_model=hidden_dim, nhead=n_heads, dim_feedforward=ff_dim, dropout=dropout, batch_first=True)
+        self.decoder = nn.TransformerDecoder(layer, num_layers=n_layers)
+
+
+class Cobra(nn.Module):
+    """Mirror of genrec/models/cobra.py:227-529 (training and item vectors)."""
+
+    def __init__(self, encoder_n_layers: int = 1, encoder_hidden_dim: int = 768, encoder_num_heads: int = 8, encoder_vocab_size: int = 32128,
+                 id_vocab_size: int = 512, n_codebooks: int = 3, d_model: int = 768, max_len: int = 1024, temperature=0.2, queue_size=1024,
+                 decoder_n_layers: int = 8, decoder_num_heads: int = 6, decoder_dropout: float = 0.1, encoder_type: str = "light",
+                 encoder_model_name: str = "./models_hub/sentence-t5-base") -> None:
+        super().__init__()
+        if encoder_type != "light":
+            raise NotImplementedError("genrec_b200.Cobra: only the light (randomly initialised) item-text encoder is native")
+        if encoder_hidden_dim not in POOL_DIMS or encoder_hidden_dim % encoder_num_heads or \
+                encoder_hidden_dim // encoder_num_heads not in ENC_HEAD_DIMS:
+            raise _bad(f"encoder_hidden_dim {encoder_hidden_dim} with {encoder_num_heads} heads unsupported (widths {POOL_DIMS}, "
+                       f"head dims {ENC_HEAD_DIMS})")
+        if d_model not in LN_DIMS or d_model % decoder_num_heads or d_model // decoder_num_heads not in DEC_HEAD_DIMS:
+            raise _bad(f"d_model {d_model} with {decoder_num_heads} heads unsupported (widths {LN_DIMS}, head dims {DEC_HEAD_DIMS})")
+        self.C = n_codebooks
+        self.d_model = d_model
+        self.pad_id = id_vocab_size * self.C
+        self.max_len = max_len
+        self.encoder = _LightT5Encoder(n_layers=encoder_n_layers, hidden_dim=encoder_hidden_dim, output_dim=d_model,
+                                       num_heads=encoder_num_heads, vocab_size=encoder_vocab_size)
+        self.cobra_emb = _CobraEmbedding(id_vocab_size=id_vocab_size, d_model=d_model, max_len=max_len, pad_id=self.pad_id)
+        self.decoder = _CobraDecoder(d_model, n_layers=decoder_n_layers, n_heads=decoder_num_heads, dropout=decoder_dropout)
+        self.sparse_head = nn.ModuleList([nn.Linear(d_model, id_vocab_size) for _ in range(n_codebooks)])
+        self.temperature = temperature
+        self.register_buffer("feat_queue", torch.randn(queue_size, d_model))
+        self.register_buffer("queue_ptr", torch.zeros(1, dtype=torch.long))
+        self.queue_size = queue_size
+        self.feat_queue = F.normalize(self.feat_queue, dim=-1)
+
+    # ---- dropout
+    def _p(self, p: float) -> float:
+        return p if self.training else 0.0
+
+    def _drop(self, x, p):
+        return F.dropout(x, p, self.training) if self.training and p > 0 else x
+
+    def _seed(self) -> int:
+        """one dropout seed per step from torch's CPU generator (reproducible under torch.manual_seed, new every step)"""
+        return int(torch.randint(1, 1 << 62, (1,)).item()) if self.training else 0
+
+    # ---- item-text encoder
+    def _encode(self, tokens: torch.Tensor, keep: Optional[torch.Tensor]) -> torch.Tensor:
+        """tokens [N, L] -> normalised item vectors [N, d_model] fp32 (encoder.py:61-103 on packed rows)"""
+        require_cuda(tokens)
+        ensure_device(tokens.device)
+        enc = self.encoder
+        N, L = tokens.shape
+        if L > enc.pos_embedding.num_embeddings:
+            raise _bad(f"text length {L} exceeds the position table ({enc.pos_embedding.num_embeddings})")
+        tokens = tokens.contiguous().long()
+        offsets, info = Fn.cobra_pack_texts(tokens, keep)
+        rows, longest, bad = info.tolist()
+        if bad:
+            raise ValueError(f"Cobra: text {bad - 1} has a non-zero token after a zero; item texts must be right-padded with 0")
+        H = enc.encoder.layers[0].self_attn.num_heads
+        if torch.is_grad_enabled() and N * H > MAX_ATTN_ROWS:
+            raise _bad(f"{N} texts x {H} heads exceed {MAX_ATTN_ROWS} for the attention backward")
+        hid = enc.embedding.embedding_dim
+        if rows == 0:
+            # no text has a token: every pooled vector is zero.  The reference still runs the encoder, whose parameters (all but
+            # proj) get zero-tensor gradients through the masked pooling; they get the same here, so AdamW decays them alike.
+            skipped = [p for n, p in enc.named_parameters() if not n.startswith("proj.")]
+            pooled = _ZeroGrads.apply(torch.zeros(N, hid, dtype=torch.float32, device=tokens.device), *skipped)
+        else:
+            tok, pos = Fn.cobra_text_rows(tokens, offsets, rows)
+            x = F.embedding(tok, enc.embedding.weight) + F.embedding(pos, enc.pos_embedding.weight)
+            seed = self._seed()
+            for i, layer in enumerate(enc.encoder.layers):
+                sa = layer.self_attn
+                a = _MhaFn.apply(x, sa.in_proj_weight, sa.in_proj_bias, sa.out_proj.weight, sa.out_proj.bias, sa.num_heads,
+                                 self._p(sa.dropout), seed, 16 * i + 1, None, False, offsets, longest)
+                x = _LayerNormFn.apply(x + self._drop(a, layer.dropout1.p), layer.norm1.weight, layer.norm1.bias, layer.norm1.eps)
+                f = _FfnFn.apply(x, layer.linear1.weight, layer.linear1.bias, layer.linear2.weight, layer.linear2.bias,
+                                 self._p(layer.dropout.p), self._p(layer.dropout2.p), seed, 16 * i + 2)
+                x = _LayerNormFn.apply(f, layer.norm2.weight, layer.norm2.bias, layer.norm2.eps)
+            pooled = _SegLnMeanFn.apply(x, enc.layer_norm.weight, enc.layer_norm.bias, offsets, enc.layer_norm.eps)
+        return _L2NormFn.apply(_LinearF32Fn.apply(pooled, enc.proj.weight, enc.proj.bias))
+
+    def encode_items(self, tokens: torch.Tensor) -> torch.Tensor:
+        """Catalog vectors for BeamFusion (the reference's compute_item_dense_vecs): tokens [N, L] -> [N, d_model], each the
+        normalised encoder vector of its text (what generate_itemvec gives for the same texts)."""
+        return _L2NormFn.apply(self._encode(tokens, None))
+
+    def generate_itemvec(self, encoder_input_ids: torch.Tensor):
+        """cobra.py:667-677"""
+        if encoder_input_ids.dim() == 3:
+            B, T, L = encoder_input_ids.shape
+            return self.encode_items(encoder_input_ids.reshape(B * T, L)).view(B, T, -1)
+        if encoder_input_ids.dim() != 2:
+            raise ValueError(f"Expected 2D or 3D input, got {encoder_input_ids.dim()}D")
+        return self.encode_items(encoder_input_ids)
+
+    # ---- decoder
+    def _interleave(self, input_ids, vecs, mask_items):
+        """CobraEmbedding.forward (cobra.py:75-147) for complete items: -> (h [B, T(C+1), d] fp32, mask [B, T(C+1)] bool)"""
+        e = self.cobra_emb
+        B, L = input_ids.shape
+        C, T = self.C, L // self.C
+        dev = input_ids.device
+        ct = torch.arange(L, device=dev) % C
+        ids = torch.where(input_ids != self.pad_id, input_ids + ct * e.id_vocab_size, input_ids)
+        tok = F.embedding(ids, e.id_embed.weight, padding_idx=e.id_embed.padding_idx)
+        h = torch.cat([tok.view(B, T, C, -1), vecs.view(B, T, 1, -1)], dim=2).reshape(B, T * (C + 1), -1)
+        mask = torch.cat([mask_items, mask_items[:, :, C - 1:]], dim=2).reshape(B, T * (C + 1))
+        Li = T * (C + 1)
+        types = torch.arange(Li, device=dev) % (C + 1) == C
+        m = mask.unsqueeze(-1).float()
+        h = h * m + e.pos_embed.weight[:Li].unsqueeze(0) * m + F.embedding(types.long(), e.type_embed.weight).unsqueeze(0) * m
+        return h, mask
+
+    def _decode(self, x, mask):
+        key_pad = (~mask).to(torch.uint8).contiguous()
+        seed = self._seed()
+        for i, layer in enumerate(self.decoder.decoder.layers):
+            sa, ca = layer.self_attn, layer.multihead_attn
+            a = _MhaFn.apply(x, sa.in_proj_weight, sa.in_proj_bias, sa.out_proj.weight, sa.out_proj.bias, sa.num_heads, self._p(sa.dropout),
+                             seed, 16 * i + 1, key_pad, True, None, 0)
+            x = _LayerNormFn.apply(x + self._drop(a, layer.dropout1.p), layer.norm1.weight, layer.norm1.bias, layer.norm1.eps)
+            # attention over a zero-length memory is the out_proj bias (cobra.py:209-223)
+            cross = _ZeroGrads.apply(ca.out_proj.bias, ca.in_proj_weight, ca.in_proj_bias, ca.out_proj.weight).expand_as(x)
+            x = _LayerNormFn.apply(x + self._drop(cross, layer.dropout2.p), layer.norm2.weight, layer.norm2.bias, layer.norm2.eps)
+            f = _FfnFn.apply(x, layer.linear1.weight, layer.linear1.bias, layer.linear2.weight, layer.linear2.bias, self._p(layer.dropout.p),
+                             self._p(layer.dropout3.p), seed, 16 * i + 2)
+            x = _LayerNormFn.apply(f, layer.norm3.weight, layer.norm3.bias, layer.norm3.eps)
+        return x
+
+    # ---- the reference's interface
+    def forward(self, input_ids: torch.Tensor, encoder_input_ids: torch.Tensor, mask=None) -> CobraOutput:
+        """cobra.py:379-529.  input_ids [B, T*C], encoder_input_ids [B, T, L] (right-padded with 0)."""
+        require_cuda(input_ids, encoder_input_ids)
+        B, TC = input_ids.shape
+        C = self.C
+        if TC % C or encoder_input_ids.dim() != 3 or encoder_input_ids.shape[:2] != (B, TC // C):
+            raise ValueError(f"Cobra.forward: input_ids [B, T*C] and encoder_input_ids [B, T, L] expected, got {tuple(input_ids.shape)} "
+                             f"and {tuple(encoder_input_ids.shape)}")
+        T = TC // C
+        if T * (C + 1) > self.max_len:
+            raise _bad(f"interleaved length {T * (C + 1)} exceeds max_len {self.max_len}")
+        H = self.decoder.decoder.layers[0].self_attn.num_heads
+        if torch.is_grad_enabled() and B * H > MAX_ATTN_ROWS:
+            raise _bad(f"{B} users x {H} heads exceed {MAX_ATTN_ROWS} for the attention backward")
+        L = encoder_input_ids.shape[2]
+        mask_items = (input_ids != self.pad_id).view(B, T, C)
+        keep = mask_items[:, :, C - 1].reshape(-1).to(torch.uint8).contiguous()      # pad items: no rows
+        vecs = self._encode(encoder_input_ids.reshape(B * T, L), keep).view(B, T, -1)
+        emb, seq_mask = self._interleave(input_ids, vecs, mask_items)
+        h = self._decode(emb, seq_mask)
+        dev = h.device
+
+        loss_sparse = 0.0
+        total_correct = total_tokens = 0
+        all_item_correct = torch.ones(B, T - 1, dtype=torch.bool, device=dev)
+        all_valid_mask = None
+        for c in range(C):                                                         # cobra.py:417-457
+            if c == 0:
+                pos_c = torch.arange(0, T - 1, device=dev) * (C + 1) + C
+                target = input_ids[:, torch.arange(1, T, device=dev) * C]
+            else:
+                pos_c = torch.arange(1, T, device=dev) * (C + 1) + (c - 1)
+                target = input_ids[:, torch.arange(1, T, device=dev) * C + c]
+            head = self.sparse_head[c]
+            logits = _LinearF32Fn.apply(h[:, pos_c, :], head.weight, head.bias)
+            loss_c = F.cross_entropy(logits.reshape(-1, logits.size(-1)), target.reshape(-1), ignore_index=self.pad_id, reduction="sum")
+            loss_sparse = loss_sparse + loss_c / (target != self.pad_id).sum().clamp(min=1)
+            with torch.no_grad():
+                valid_mask = target != self.pad_id
+                if all_valid_mask is None:
+                    all_valid_mask = valid_mask
+                pred_top1 = logits.argmax(-1)
+                total_correct = total_correct + ((pred_top1 == target) & valid_mask).sum()
+                total_tokens = total_tokens + valid_mask.sum()
+                all_item_correct &= (pred_top1 == target) | ~valid_mask
+        loss_sparse = loss_sparse / C
+        item_correct_masked = all_item_correct & all_valid_mask
+
+        # dense InfoNCE (cobra.py:466-493): rows grouped by user, each user's other items left out
+        vec_pos = torch.arange(1, T, device=dev) * (C + 1) + (C - 1)
+        valid = seq_mask[:, (C + 1)::(C + 1)]                                       # [B, T-1]
+        vec_pred = h[:, vec_pos, :self.d_model][valid]
+        vec_gt = Fn.l2norm_fwd(vecs[:, 1:].detach()[valid].contiguous())[0] if vec_pred.shape[0] else vec_pred.detach()
+        Q = vec_pred.shape[0]
+        if Q == 0:
+            loss_dense = vec_cos_sim = torch.full((), float("nan"), device=dev)     # an empty cross-entropy's mean
+        else:
+            vec_pred = _L2NormFn.apply(vec_pred)
+            counts = valid.sum(1)
+            ends = counts.cumsum(0)
+            user = torch.arange(B, device=dev).repeat_interleave(counts, output_size=Q)
+            hi = ends[user]
+            lo = hi - counts[user]
+            loss_dense = _InfoNceFn.apply(vec_pred, vec_gt, lo.contiguous(), hi.contiguous(), 1.0 / self.temperature)
+            with torch.no_grad():
+                vec_cos_sim = F.cosine_similarity(vec_pred, vec_gt).mean()
+        with torch.no_grad():                                                      # cobra.py:514-517, stride 3 as written
+            usage = torch.stack([F.one_hot(input_ids[:, c::3], self.pad_id + 1).sum((0, 1)).float() for c in range(C)])
+            prob = usage / usage.sum(1, keepdim=True)
+            codebook_entropy = -(prob * (prob.add(1e-12).log())).sum(1).mean()
+        return CobraOutput(loss=loss_sparse + loss_dense, loss_sparse=loss_sparse, loss_dense=loss_dense, acc_correct=total_correct,
+                           acc_total=total_tokens, recall_correct=item_correct_masked.sum(), recall_total=all_valid_mask.sum(),
+                           vec_cos_sim=vec_cos_sim, codebook_entropy=codebook_entropy)
+
+    def generate(self, *args, **kwargs):
+        raise NotImplementedError("genrec_b200.Cobra.generate: prefix-cached COBRA generation is a separate follow-up (its ragged-batch "
+                                  "semantics are not settled)")
+
+    def beam_fusion(self, *args, **kwargs):
+        raise NotImplementedError("genrec_b200.Cobra.beam_fusion: BeamFusion follows native COBRA generation, a separate follow-up")

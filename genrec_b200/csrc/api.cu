@@ -16,6 +16,7 @@
 #include "attn_sasrec.cuh"
 #include "attn_t5.cuh"
 #include "beam.cuh"
+#include "cobra.cuh"
 #include "common.cuh"
 #include "dp_adam.cuh"
 #include "exact_f32.cuh"
@@ -122,6 +123,16 @@ template <class F>
 auto with_ce_dim(int D, F&& f) {
     if (D == 64) return f(std::integral_constant<int, 64>{});
     return f(std::integral_constant<int, 128>{});
+}
+// COBRA's post-LN LayerNorms (grb_post_layernorm_*) run the plain LayerNorm kernels at its widths too: 192 and 768 (the item-text
+// encoder's hidden sizes) and 384 (its d_model)
+template <class F>
+int with_post_ln_dim(int D, F&& f) {
+    if (D == 192) return f(std::integral_constant<int, 192>{});
+    if (D == 384) return f(std::integral_constant<int, 384>{});
+    if (D == 768) return f(std::integral_constant<int, 768>{});
+    if (D == 64 || D == 128 || D == 256) return with_row_dim(D, f);
+    return fail(GRB_EINVAL, "post-LN layernorm supports D in {64,128,192,256,384,768}, got %d", D);
 }
 // the RMS norm kernels add TIGER's attn_dim, 384 (its embedding_dim is 128).  The LayerNorm / HSTU row kernels are not
 // instantiated at 384: nothing calls them there.
@@ -1812,9 +1823,10 @@ int grb_layernorm_f32_forward(const float* x, const float* g, const float* b, fl
 // ------------------------------------------------------------------------------------------------ T5-style attention core (TIGER)
 static int t5_args(T5AttnArgs& a, const void* q, const void* k, const void* v, int B, int Lq, int Lk, int H, int DH, int ldq, int ldk, int ldv,
                    const float* bias, const int32_t* bucket, int nb, const uint8_t* key_pad, int causal, float scale, float p, uint64_t seed,
-                   const uint64_t* seed_dev, uint32_t site) {
+                   const uint64_t* seed_dev, uint32_t site, bool allow96 = false) {
     GRB_REQUIRE(q && k && v, "null argument");
-    GRB_REQUIRE(B > 0 && Lq > 0 && Lk > 0 && H > 0 && (DH == 32 || DH == 64), "bad shape B=%d Lq=%d Lk=%d H=%d head_dim=%d", B, Lq, Lk, H, DH);
+    GRB_REQUIRE(B > 0 && Lq > 0 && Lk > 0 && H > 0 && (DH == 32 || DH == 64 || (DH == 96 && allow96)),
+                "bad shape B=%d Lq=%d Lk=%d H=%d head_dim=%d", B, Lq, Lk, H, DH);
     GRB_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && aligned16(q) && aligned16(k) && aligned16(v), "rows must be 16-byte aligned");
     GRB_REQUIRE((bias == nullptr) == (bucket == nullptr) && (!bias || (nb > 0 && nb <= 1024)), "bias table and bucket map go together");
     GRB_REQUIRE(p >= 0.f && p < 1.f, "dropout_p out of range");
@@ -1835,19 +1847,28 @@ int t5_args_jagged(T5AttnArgs& a, const void* q, const void* k, const void* v, c
     GRB_REQUIRE(B >= 1 && B <= 65535, "B=%d out of range [1, 65535]", B);
     GRB_REQUIRE(T >= 1 && max_len >= 1 && Lq >= 0, "bad shape T=%d max_len=%d Lq=%d", T, max_len, Lq);
     const int lq = Lq > 0 ? Lq : max_len;
-    GRB_TRY(t5_args(a, q, k, v, B, lq, max_len, H, DH, ldq, ldk, ldv, bias, bucket, nb, nullptr, causal, scale, p, seed, seed_dev, site));
+    GRB_TRY(t5_args(a, q, k, v, B, lq, max_len, H, DH, ldq, ldk, ldv, bias, bucket, nb, nullptr, causal, scale, p, seed, seed_dev, site,
+                    Lq == 0));
     GRB_REQUIRE((long long)T * ldk <= INT32_MAX && (long long)T * ldv <= INT32_MAX && (long long)T * H <= INT32_MAX &&
                     (Lq > 0 || (long long)T * ldq <= INT32_MAX), "token rows T=%d out of range", T);
     GRB_REQUIRE(!bias || bucket_len >= lq + max_len - 1, "bucket map of %d entries, %d needed (Lq + max_len - 1)", bucket_len,
                 lq + max_len - 1);
     return 0;
 }
+// head dims of the T5 core: 32 and 64 everywhere, and 96 (COBRA's item-text encoder) in packed self-attention only, so that the
+// other layouts instantiate nothing new
+template <int PACK, class F>
+int with_t5_head_dim(int dh, F&& f) {
+    if constexpr (PACK == T5_PACKED_SELF)
+        if (dh == 96) return f(std::integral_constant<int, 96>{});
+    return with_head_dim(dh, f);
+}
 template <int PACK>
 int t5_launch_fwd(const T5AttnArgs& a, const T5Packed& pk, int head_dim, cudaStream_t st) {
     const long long bh = (long long)a.B * a.H;
     GRB_REQUIRE(bh <= INT_MAX, "B * H = %lld too large (at most 2^31 - 1)", bh);
     const unsigned nx = (a.Lq + T5_ROWS - 1) / T5_ROWS;
-    return with_head_dim(head_dim, [&](auto DH) -> int {
+    return with_t5_head_dim<PACK>(head_dim, [&](auto DH) -> int {
         if (bh <= 65535) {
             GRB_LAUNCH((t5_attn_fwd_kernel<DH, false, PACK>), dim3(nx, (unsigned)bh), T5_THREADS, t5_fwd_smem<DH>(a.nb), st, a, pk);
         } else {
@@ -1967,17 +1988,118 @@ int grb_t5_attention_backward_jagged(const void* q, const void* k, const void* v
         GRB_CUDA(cudaMemsetAsync(dv, 0, n * sizeof(float), st));
     }
     const T5Packed pk{reinterpret_cast<const long long*>(offsets), T};
-    GRB_TRY(with_head_dim(head_dim, [&](auto DH) -> int {
-        if (Lq > 0) GRB_LAUNCH((t5_attn_bwd_kernel<DH, T5_PACKED_CROSS>), grid, T5_THREADS, t5_bwd_smem<DH>(a.nb), st, a, w.dkv_part, w.db_part, pk);
-        else GRB_LAUNCH((t5_attn_bwd_kernel<DH, T5_PACKED_SELF>), grid, T5_THREADS, t5_bwd_smem<DH>(a.nb), st, a, w.dkv_part, w.db_part, pk);
-        return 0;
-    }));
+    if (Lq > 0) {
+        GRB_TRY(with_head_dim(head_dim, [&](auto DH) -> int {
+            GRB_LAUNCH((t5_attn_bwd_kernel<DH, T5_PACKED_CROSS>), grid, T5_THREADS, t5_bwd_smem<DH>(a.nb), st, a, w.dkv_part, w.db_part, pk);
+            return 0;
+        }));
+    } else {
+        GRB_TRY(with_t5_head_dim<T5_PACKED_SELF>(head_dim, [&](auto DH) -> int {
+            GRB_LAUNCH((t5_attn_bwd_kernel<DH, T5_PACKED_SELF>), grid, T5_THREADS, t5_bwd_smem<DH>(a.nb), st, a, w.dkv_part, w.db_part, pk);
+            return 0;
+        }));
+    }
     if (w.dkv_part) {                           // the idle rows' partials were never written: their sums are overwritten with zeros
         GRB_LAUNCH(t5_dkdv_sum_kernel, capped_blocks(2 * n / 4), 256, 0, st, (const float*)w.dkv_part, (int)grid.x, n, dk, dv);
         for (float* g : {dk, dv}) GRB_TRY(zero_idle_rows(offsets, B, T, reinterpret_cast<bf16*>(g), 2 * D, 2 * D, st));   // fp32 rows as bf16 pairs
     }
     if (Lq == 0) GRB_TRY(zero_idle_rows(offsets, B, T, (bf16*)dq, lddq, D, st));
     if (a.dbias) GRB_TRY(det_finish(w.db_part, H, B * (int)grid.x, a.nb, H, a.nb, 1, {{a.dbias, H * a.nb}}, st));
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ COBRA item-text encoder and dense loss
+int grb_post_layernorm_forward(const float* x, const float* g, const float* b, float eps, int T, int D, float* y, float* stats, void* stream) {
+    GRB_REQUIRE(x && g && b && y && stats && T >= 1, "bad argument");
+    LnFwdArgs a{x, g, b, nullptr, y, stats, T, D, eps};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return with_post_ln_dim(D, [&](auto DC) -> int { GRB_LAUNCH(ln_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); return 0; });
+}
+int grb_post_layernorm_backward(const float* dy, const float* x, const float* stats, const float* g, int T, int D, float* dx, float* dg,
+                                float* db, void* workspace, void* stream) {
+    GRB_REQUIRE(dy && x && stats && g && dx && dg && db && workspace && T >= 1, "bad argument");
+    const LnBwdArgs a{dy, x, stats, g, nullptr, dx, dg, db, T, D, static_cast<float*>(workspace)};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GRB_TRY(with_post_ln_dim(D, [&](auto DC) -> int { GRB_LAUNCH(ln_bwd_kernel<DC / 64>, row_bwd_grid(T), ROW_THREADS, 0, st, a); return 0; }));
+    return det_finish(a.part, 2, row_bwd_grid(T), D, 1, 0, 1, {{dg, D}, {db, D}}, st);
+}
+int grb_cobra_pack_texts(const int64_t* tokens, int N, int L, const uint8_t* keep, int32_t* lens, int64_t* offsets, int64_t* info,
+                         void* stream) {
+    GRB_REQUIRE(tokens && lens && offsets && info, "null argument");
+    GRB_REQUIRE(N >= 1 && L >= 1, "bad shape N=%d L=%d", N, L);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GRB_LAUNCH(cobra_text_lens_kernel, capped_blocks((size_t)N * 32), 256, 0, st, reinterpret_cast<const long long*>(tokens), N, L,
+               keep, lens);
+    GRB_LAUNCH(cobra_text_offsets_kernel, 1, COBRA_SCAN_THREADS, 0, st, lens, N, reinterpret_cast<long long*>(offsets),
+               reinterpret_cast<long long*>(info));
+    return 0;
+}
+int grb_cobra_text_rows(const int64_t* tokens, int N, int L, const int64_t* offsets, int64_t* tok, int64_t* pos, void* stream) {
+    GRB_REQUIRE(tokens && offsets && tok && pos, "null argument");
+    GRB_REQUIRE(N >= 1 && L >= 1, "bad shape N=%d L=%d", N, L);
+    GRB_LAUNCH(cobra_text_rows_kernel, capped_blocks((size_t)N * 32), 256, 0, static_cast<cudaStream_t>(stream),
+               reinterpret_cast<const long long*>(tokens), N, L, reinterpret_cast<const long long*>(offsets),
+               reinterpret_cast<long long*>(tok), reinterpret_cast<long long*>(pos));
+    return 0;
+}
+}  // extern "C"
+namespace {
+// the pooling kernels keep a row in registers: D = 64 NP for COBRA's encoder widths
+template <class F>
+int with_seg_dim(int D, F&& f) {
+    if (D == 128) return f(std::integral_constant<int, 2>{});
+    if (D == 192) return f(std::integral_constant<int, 3>{});
+    if (D == 256) return f(std::integral_constant<int, 4>{});
+    if (D == 384) return f(std::integral_constant<int, 6>{});
+    if (D == 768) return f(std::integral_constant<int, 12>{});
+    return fail(GRB_EINVAL, "the pooled LayerNorm supports D in {128,192,256,384,768}, got %d", D);
+}
+}  // namespace
+extern "C" {
+int grb_seg_layernorm_mean_forward(const int64_t* offsets, int N, const float* x, const float* g, const float* b, float eps, int D,
+                                   float* stats, float* pooled, void* stream) {
+    GRB_REQUIRE(offsets && g && b && stats && pooled && N >= 1, "bad argument");
+    SegLnArgs a;
+    memset(&a, 0, sizeof(a));
+    a.offsets = reinterpret_cast<const long long*>(offsets); a.N = N; a.D = D; a.eps = eps; a.x = x; a.g = g; a.b = b; a.st = stats;
+    a.pooled = pooled;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return with_seg_dim(D, [&](auto NP) -> int { GRB_LAUNCH(seg_ln_mean_fwd_kernel<NP>, (unsigned)N, ROW_THREADS, 0, st, a); return 0; });
+}
+size_t grb_seg_layernorm_mean_backward_workspace_bytes(int N, int D) {
+    if (N <= 0 || D <= 0) return 0;
+    return (size_t)2 * N * D * sizeof(float);
+}
+int grb_seg_layernorm_mean_backward(const int64_t* offsets, int N, const float* x, const float* stats, const float* g, const float* dpooled,
+                                    int D, float* dx, float* dg, float* db, void* workspace, void* stream) {
+    GRB_REQUIRE(offsets && stats && g && dpooled && dg && db && workspace && N >= 1, "bad argument");
+    SegLnArgs a;
+    memset(&a, 0, sizeof(a));
+    a.offsets = reinterpret_cast<const long long*>(offsets); a.N = N; a.D = D; a.x = x; a.g = g; a.st = const_cast<float*>(stats);
+    a.dpooled = dpooled; a.dx = dx; a.part = static_cast<float*>(workspace);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GRB_TRY(with_seg_dim(D, [&](auto NP) -> int { GRB_LAUNCH(seg_ln_mean_bwd_kernel<NP>, (unsigned)N, ROW_THREADS, 0, st, a); return 0; }));
+    return det_finish(a.part, 2, N, D, 1, 0, 1, {{dg, D}, {db, D}}, st);
+}
+int grb_l2norm_forward(const float* x, int T, int D, float eps, float* y, float* norms, void* stream) {
+    GRB_REQUIRE(x && y && T >= 1 && D >= 1 && D <= 4096, "bad argument T=%d D=%d", T, D);
+    GRB_LAUNCH(l2norm_fwd_kernel, capped_blocks((size_t)T * 32), 256, 0, static_cast<cudaStream_t>(stream), x, T, D, eps, y, norms);
+    return 0;
+}
+int grb_l2norm_backward(const float* dy, const float* y, const float* norms, int T, int D, float eps, float* dx, void* stream) {
+    GRB_REQUIRE(dy && y && norms && dx && T >= 1 && D >= 1 && D <= 4096, "bad argument T=%d D=%d", T, D);
+    GRB_LAUNCH(l2norm_bwd_kernel, capped_blocks((size_t)T * 32), 256, 0, static_cast<cudaStream_t>(stream), dy, y, norms, T, D, eps, dx);
+    return 0;
+}
+int grb_infonce_forward_backward(const float* scores, int Q, int ld, const int64_t* lo, const int64_t* hi, float inv_tau, float* row_loss,
+                                 float* loss, void* dscores, void* stream) {
+    GRB_REQUIRE(scores && lo && hi && row_loss && loss && dscores, "null argument");
+    GRB_REQUIRE(Q >= 1 && ld >= Q, "bad shape Q=%d ld=%d", Q, ld);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GRB_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), st));
+    GRB_LAUNCH(infonce_rows_kernel, (unsigned)Q, 256, 0, st, scores, Q, ld, reinterpret_cast<const long long*>(lo),
+               reinterpret_cast<const long long*>(hi), inv_tau, row_loss, static_cast<bf16*>(dscores));
+    GRB_LAUNCH(ce_loss_sum_kernel, 1, 1024, 0, st, row_loss, Q, loss);
     return 0;
 }
 

@@ -591,9 +591,17 @@ inline bool make_tmap(CUtensorMap* m, const void* base, bool fp32, uint64_t rows
     cuuint64_t strides[1] = {ld * esz};
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    return enc(m, fp32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    auto encode = [&] {
+        return enc(m, fp32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box,
+                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    };
+    if (encode()) return true;
+    // The encoder is a driver call and needs a current context.  A thread whose first CUDA call this is (an autograd worker whose
+    // backward starts with a GEMM) has none yet: bind the current device's primary context and try once more.
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaSetDevice(dev) != cudaSuccess) return false;
+    return encode();
 }
 inline bool make_tmap_bf16(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_cols, uint32_t box_rows) {
     return make_tmap(m, base, false, rows, cols, ld, box_cols, box_rows);

@@ -1076,3 +1076,94 @@ def adam_step_lazy_table(p, g, m, v, p_bf16, table_off, C, D, flag, rows, count,
         check(_lib.load().grb_adam_step_lazy_table(ptr(p), ptr(g), ptr(m), ptr(v), ptr(p_bf16), p.numel(), table_off, C, D, ptr(flag), ptr(rows),
                                                    ptr(count), ptr(all_word), ptr(state), lr, beta1, beta2, eps, weight_decay, grad_scale,
                                                    stream_ptr(p.device)))
+
+
+# ------------------------------------------------------------------------------------------------ COBRA
+def post_layernorm_fwd(x, g, b, eps):
+    """LayerNorm of fp32 rows x [..., D] at COBRA's widths -> (y fp32, stats [T, 2])"""
+    T, D = x.numel() // x.shape[-1], x.shape[-1]
+    y = torch.empty_like(x)
+    st = torch.empty(T, 2, dtype=torch.float32, device=x.device)
+    check(_lib.load().grb_post_layernorm_forward(ptr(x), ptr(g), ptr(b), float(eps), T, D, ptr(y), ptr(st), stream_ptr(x.device)))
+    return y, st
+
+
+def post_layernorm_bwd(dy, x, st, g):
+    """-> (dx, dg, db), dg / db summed in a fixed order"""
+    lib = _lib.load()
+    T, D = x.numel() // x.shape[-1], x.shape[-1]
+    dx = torch.empty_like(x)
+    dg, db = torch.zeros_like(g), torch.zeros_like(g)
+    ws = _u8(lib.grb_layernorm_backward_workspace_bytes(T, D), x.device)
+    check(lib.grb_post_layernorm_backward(ptr(dy), ptr(x), ptr(st), ptr(g), T, D, ptr(dx), ptr(dg), ptr(db), ptr(ws), stream_ptr(x.device)))
+    return dx, dg, db
+
+
+def cobra_pack_texts(tokens: torch.Tensor, keep: Optional[torch.Tensor] = None):
+    """tokens [N, L] int64 (CUDA), keep [N] uint8 or None -> (offsets [N+1] int64, info [3] int64 on the device): text n is its
+    leading non-zero tokens (none where keep is 0); info = {rows, longest text, first refused text + 1 or 0}."""
+    N, L = tokens.shape
+    dev = tokens.device
+    lens = torch.empty(N, dtype=torch.int32, device=dev)
+    offsets = torch.empty(N + 1, dtype=torch.int64, device=dev)
+    info = torch.empty(3, dtype=torch.int64, device=dev)
+    check(_lib.load().grb_cobra_pack_texts(ptr(tokens), N, L, ptr(keep), ptr(lens), ptr(offsets), ptr(info), stream_ptr(dev)))
+    return offsets, info
+
+
+def cobra_text_rows(tokens: torch.Tensor, offsets: torch.Tensor, rows: int):
+    """-> (token id [rows], position in its text [rows]) int64 of the packed rows"""
+    N, L = tokens.shape
+    tok = torch.empty(rows, dtype=torch.int64, device=tokens.device)
+    pos = torch.empty(rows, dtype=torch.int64, device=tokens.device)
+    check(_lib.load().grb_cobra_text_rows(ptr(tokens), N, L, ptr(offsets), ptr(tok), ptr(pos), stream_ptr(tokens.device)))
+    return tok, pos
+
+
+def seg_layernorm_mean_fwd(offsets, x, g, b, eps):
+    """x [rows, D] fp32 -> (pooled [N, D] = mean of LayerNorm(x) over each text's rows, stats [rows, 2])"""
+    N, D = offsets.numel() - 1, g.numel()
+    pooled = torch.empty(N, D, dtype=torch.float32, device=g.device)
+    st = torch.empty(max(x.shape[0], 1), 2, dtype=torch.float32, device=g.device)
+    check(_lib.load().grb_seg_layernorm_mean_forward(ptr(offsets), N, ptr(x), ptr(g), ptr(b), float(eps), D, ptr(st), ptr(pooled),
+                                                     stream_ptr(g.device)))
+    return pooled, st
+
+
+def seg_layernorm_mean_bwd(offsets, x, st, g, dpooled):
+    """-> (dx [rows, D], dg, db [D]), dg / db summed in a fixed order"""
+    lib = _lib.load()
+    N, D = offsets.numel() - 1, g.numel()
+    dx = torch.empty_like(x)
+    dg, db = torch.zeros_like(g), torch.zeros_like(g)
+    ws = _u8(lib.grb_seg_layernorm_mean_backward_workspace_bytes(N, D), g.device)
+    check(lib.grb_seg_layernorm_mean_backward(ptr(offsets), N, ptr(x), ptr(st), ptr(g), ptr(dpooled), D, ptr(dx), ptr(dg), ptr(db), ptr(ws),
+                                              stream_ptr(g.device)))
+    return dx, dg, db
+
+
+def l2norm_fwd(x, eps=1e-12):
+    """F.normalize(x, dim=-1) of fp32 rows -> (y, norms [T])"""
+    T, D = x.numel() // x.shape[-1], x.shape[-1]
+    y = torch.empty_like(x)
+    n = torch.empty(T, dtype=torch.float32, device=x.device)
+    check(_lib.load().grb_l2norm_forward(ptr(x), T, D, float(eps), ptr(y), ptr(n), stream_ptr(x.device)))
+    return y, n
+
+
+def l2norm_bwd(dy, y, norms, eps=1e-12):
+    T, D = y.numel() // y.shape[-1], y.shape[-1]
+    dx = torch.empty_like(y)
+    check(_lib.load().grb_l2norm_backward(ptr(dy), ptr(y), ptr(norms), T, D, float(eps), ptr(dx), stream_ptr(y.device)))
+    return dx
+
+
+def infonce_fwd_bwd(scores, lo, hi, inv_tau: float):
+    """scores [Q, ld] fp32, lo / hi [Q] int64 -> (sum of the row losses [1], dscores [Q, ld] bf16 of the mean loss)"""
+    Q, ld = scores.shape
+    row = torch.empty(Q, dtype=torch.float32, device=scores.device)
+    loss = torch.empty(1, dtype=torch.float32, device=scores.device)
+    ds = torch.empty(Q, ld, dtype=torch.bfloat16, device=scores.device)
+    check(_lib.load().grb_infonce_forward_backward(ptr(scores), Q, ld, ptr(lo), ptr(hi), float(inv_tau), ptr(row), ptr(loss), ptr(ds),
+                                                   stream_ptr(scores.device)))
+    return loss, ds

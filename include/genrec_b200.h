@@ -475,8 +475,8 @@ int grb_t5_attention_backward(const void* q, const void* k, const void* v, int B
  * Backward: dq like q; dk, dv fp32 [T, H * head_dim] (overwritten); dbias [H, num_buckets] +=; the sums run in the padded order, so
  * two calls give the same bits.  Rows outside every sequence ([0, offsets[0]) and [offsets[B], T)) are zeros in out (Lq = 0),
  * dq (Lq = 0), dk and dv.  workspace: grb_t5_attention_backward_workspace_bytes_jagged(B, T, max_len, Lq, H, head_dim, num_buckets).
- * GRB_EINVAL before any launch: a null pointer, B outside [1, 65,535] (the backward: B * H > 65,535), head_dim not 32 or 64, a
- * bucket map shorter than stated. */
+ * GRB_EINVAL before any launch: a null pointer, B outside [1, 65,535] (the backward: B * H > 65,535), head_dim not 32 or 64 (or
+ * 96 in self-attention, Lq = 0: COBRA's item-text encoder), a bucket map shorter than stated. */
 int grb_t5_attention_forward_jagged(const void* q, const void* k, const void* v, const int64_t* offsets, int B, int T, int max_len, int Lq,
                                     int H, int head_dim, int ldq, int ldk, int ldv, const float* bias, const int32_t* bucket,
                                     int bucket_len, int num_buckets, int causal, float scale, float dropout_p, uint64_t seed,
@@ -580,6 +580,40 @@ int grb_rq_sinkhorn(const float* dist, int64_t B, int K, double eps, int iters, 
  * x [B, D] fp32, 1 <= D <= 256, assign [B] int64 in [0, k), centroids [k, D] fp32 updated in place. */
 int grb_kmeans_update(const float* x, const int64_t* assign, int64_t B, int D, int k, float* centroids, int32_t* counts, float* shift,
                       void* stream);
+
+/* ------------------------------------------------------------------------------------------------ COBRA
+ * Post-LN LayerNorm of COBRA's transformer layers: grb_layernorm_forward / _backward (fp32 y, no residual) at D in
+ * {64, 128, 192, 256, 384, 768}.  workspace: grb_layernorm_backward_workspace_bytes(T, D).
+ *
+ * Item texts on packed token rows (genrec/modules/encoder.py:15-105 as genrec/models/cobra.py:394 runs it).  Text n is
+ * tokens[n, 0 .. L) (int64 [N, L]); its length is its count of leading non-zero tokens, 0 when keep[n] == 0 (keep [N] uint8,
+ * nullable: the texts of pad items).  grb_cobra_pack_texts writes lens [N] int32 (scratch), offsets [N + 1] int64 (text n is rows
+ * offsets[n] .. offsets[n+1]-1) and info [3] int64 = {rows, longest text, first refused text + 1 or 0}.  A text where a non-zero
+ * token follows a zero is refused (its packed rows would not be the reference's key mask): the caller reads info[2] and raises.
+ * grb_cobra_text_rows then writes tok / pos [rows] int64: each row's token id and its position in its text. */
+int grb_post_layernorm_forward(const float* x, const float* g, const float* b, float eps, int T, int D, float* y, float* stats, void* stream);
+int grb_post_layernorm_backward(const float* dy, const float* x, const float* stats, const float* g, int T, int D, float* dx, float* dg,
+                                float* db, void* workspace, void* stream);
+int grb_cobra_pack_texts(const int64_t* tokens, int N, int L, const uint8_t* keep, int32_t* lens, int64_t* offsets, int64_t* info,
+                         void* stream);
+int grb_cobra_text_rows(const int64_t* tokens, int N, int L, const int64_t* offsets, int64_t* tok, int64_t* pos, void* stream);
+/* pooled [N, D] = mean over the rows of text n of LayerNorm(x) (zero for a text without rows); stats [rows, 2] {mean, rstd}.
+ * Backward: dx [rows, D] of dpooled; dg, db [D] += in a fixed order.  D in {128, 192, 256, 384, 768}.
+ * workspace: grb_seg_layernorm_mean_backward_workspace_bytes(N, D). */
+int grb_seg_layernorm_mean_forward(const int64_t* offsets, int N, const float* x, const float* g, const float* b, float eps, int D,
+                                   float* stats, float* pooled, void* stream);
+size_t grb_seg_layernorm_mean_backward_workspace_bytes(int N, int D);
+int grb_seg_layernorm_mean_backward(const int64_t* offsets, int N, const float* x, const float* stats, const float* g, const float* dpooled,
+                                    int D, float* dx, float* dg, float* db, void* workspace, void* stream);
+/* y = x / max(|x|, eps) row by row (F.normalize), norms [T] = |x| (nullable); backward dx of dy. */
+int grb_l2norm_forward(const float* x, int T, int D, float eps, float* y, float* norms, void* stream);
+int grb_l2norm_backward(const float* dy, const float* y, const float* norms, int T, int D, float eps, float* dx, void* stream);
+/* In-batch InfoNCE rows (genrec/models/cobra.py:484-493).  scores [Q, ld] fp32 = pred . gt (columns Q .. ld-1 ignored); row i leaves
+ * out the columns lo[i] .. hi[i]-1 except i (its own sequence's other items).  row_loss [Q] = logsumexp(scores / tau) - scores_ii / tau
+ * over the kept columns; *loss = their sum (fixed order); dscores [Q, ld] bf16 = d(mean loss) / d scores, zero in the left-out and
+ * padding columns. */
+int grb_infonce_forward_backward(const float* scores, int Q, int ld, const int64_t* lo, const int64_t* hi, float inv_tau, float* row_loss,
+                                 float* loss, void* dscores, void* stream);
 
 #ifdef __cplusplus
 }
