@@ -258,9 +258,12 @@ __global__ void __launch_bounds__(256) infonce_rows_kernel(const float* __restri
     const float* s = S + (size_t)i * ld;
     const long long l0 = lo[i], l1 = hi[i];
     auto keep = [&](int j) { return j == i || j < l0 || j >= l1; };
+    // every use of a logit rounds it once, the same way (no product fused into the subtraction that follows): the row's own logit
+    // minus the max is then exactly 0 where the row keeps only itself, whose loss is exactly 0
+    auto logit = [&](int j) { return __fmul_rn(s[j], inv_tau); };
     float m = -INFINITY;
     for (int j = tid; j < Q; j += 256)
-        if (keep(j)) m = fmaxf(m, s[j] * inv_tau);
+        if (keep(j)) m = fmaxf(m, logit(j));
     m = warp_max(m);
     if (lane == 0) red[w] = m;
     __syncthreads();
@@ -273,7 +276,7 @@ __global__ void __launch_bounds__(256) infonce_rows_kernel(const float* __restri
     m = bcast;
     float z = 0.f;
     for (int j = tid; j < Q; j += 256)
-        if (keep(j)) z += exp_accurate(s[j] * inv_tau - m);
+        if (keep(j)) z += exp_accurate(logit(j) - m);
     z = warp_sum(z);
     __syncthreads();
     if (lane == 0) red[w] = z;
@@ -282,14 +285,14 @@ __global__ void __launch_bounds__(256) infonce_rows_kernel(const float* __restri
         float v = 0.f;
         for (int k = 0; k < 8; ++k) v += red[k];
         bcast = v;
-        row_loss[i] = logf(v) + m - s[i] * inv_tau;
+        row_loss[i] = logf(v) + (m - logit(i));
     }
     __syncthreads();
     const float inv_z = __fdiv_rn(1.f, bcast), gscale = __fdiv_rn(inv_tau, (float)Q);
     bf16* d = dS + (size_t)i * ld;
     for (int j = tid; j < ld; j += 256) {
         float g = 0.f;
-        if (j < Q && keep(j)) g = (exp_accurate(s[j] * inv_tau - m) * inv_z - (j == i ? 1.f : 0.f)) * gscale;
+        if (j < Q && keep(j)) g = (exp_accurate(logit(j) - m) * inv_z - (j == i ? 1.f : 0.f)) * gscale;
         d[j] = __float2bfloat16_rn(g);
     }
 }

@@ -45,6 +45,44 @@ def test_restatement_matches_the_reference_fixture(golden, name):
     assert set(g["vec_grads"]) | set(g["sampled_grads"]) == set(grads)
 
 
+def test_restatement_equals_the_reference_under_dropout(golden):
+    """cobra_small_dropout.pt: the reference's step in fp64 at p = 0.3 everywhere on pre-drawn masks; the masked restatement on the
+    same masks matches it to 1e-10"""
+    g = golden("cobra_small_dropout.pt")
+    cfg = g["cfg"]
+    ids, text = cp.batch(cfg, seed=g["batch_seed"])
+    masks = cr.fixture_masks(g["shapes"], g["mask_seed"], g["p"])
+    assert len(masks) == 4 + 5 * cfg["decoder_n_layers"] and all(bool((k == 0).any()) for k in masks)
+    out, grads = cr.step(cp.cobra_params(cp.shapes(cfg), g["param_seed"]), cfg, ids, text, masks=masks)
+    for k, v in g["fields"].items():
+        if v.is_floating_point():
+            # codebook_entropy: the reference counts the ids' usage in fp32 whatever the model's dtype
+            assert _rel(out[k], v) <= (FP32_TOL if k == "codebook_entropy" else 1e-10), k
+        else:
+            assert out[k].item() == v.item(), k
+    for n, v in g["vec_grads"].items():
+        assert _rel(grads[n], v) <= 1e-10, n
+    for n, s in g["sampled_grads"].items():
+        a = grads[n].reshape(-1)[s["pos"].long()]
+        assert (a - s["values"]).abs().max().item() <= 1e-10 * s["frob"], n
+        assert abs(grads[n].norm().item() - s["frob"]) <= 1e-10 * s["frob"], n
+    for bad in (masks[:-1], masks + masks[-1:]):                 # one mask short, one too many
+        with pytest.raises(ValueError, match="masks than"):
+            cr.step(cp.cobra_params(cp.shapes(cfg), g["param_seed"]), cfg, ids, text, masks=bad)
+
+
+@pytest.mark.skipif(not cobra_ref.available(), reason="the reference tree is not present")
+def test_the_dropout_fixture_regenerates_byte_for_byte(tmp_path):
+    import importlib.util
+    spec = importlib.util.spec_from_file_location("make_golden_cobra_dropout", os.path.join(ROOT, "scripts", "make_golden_cobra_dropout.py"))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    out = tmp_path / "cobra_small_dropout.pt"
+    mod.main(str(out))
+    with open(os.path.join(ROOT, "tests", "golden", "cobra_small_dropout.pt"), "rb") as f:
+        assert out.read_bytes() == f.read()
+
+
 @pytest.mark.skipif(not cobra_ref.available(), reason="the reference tree is not present")
 @pytest.mark.parametrize("cfg", [cp.SMALL, cp.TRAINER], ids=["small", "trainer"])
 def test_state_dict_round_trips_strictly(cfg):

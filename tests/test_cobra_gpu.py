@@ -256,17 +256,41 @@ def _text(L, n, gap_at=None):
     return t
 
 
-@pytest.mark.parametrize("refuse", [False, True])
-def test_packing_kernels_follow_the_host_rule(refuse):
+def _many_texts(N, L, refuse):
+    """N texts of seeded lengths 0 .. 40.  The longest text (L tokens) and, with refuse, two refused texts sit at the end of the
+    batch (N - 2, N - 3 and N - 1), in a chunk after the first of the offsets scan's 1,024-text chunks once N > 1,027; a text that is
+    not right-padded but belongs to a pad item (never read) sits at N // 2"""
+    g = torch.Generator().manual_seed(N)
+    lens = torch.randint(0, 41, (N,), generator=g).tolist()
+    texts = [_text(L, n) for n in lens]
+    keep = [1] * N
+    texts[N - 2] = _text(L, L)
+    texts[N // 2] = _text(L, 3, gap_at=70)
+    keep[N // 2] = 0
+    if refuse:
+        texts[N - 3] = _text(L, 35, gap_at=80)
+        texts[N - 1] = _text(L, 5, gap_at=9)
+    return texts, keep
+
+
+PACK_CASES = [(False, None), (True, None)] + [(r, n) for n in (1023, 1024, 1025, 5000, 20000) for r in (False, True)]
+
+
+@pytest.mark.parametrize("refuse,n_texts", PACK_CASES, ids=[str(r) if n is None else f"N{n}-{r}" for r, n in PACK_CASES])
+def test_packing_kernels_follow_the_host_rule(refuse, n_texts):
     """lengths 0, 1, 31, 32, 33, 64 and L; keep = 0 over a text that is not right-padded (not refused: a pad item is never read);
-    with refuse, texts whose stray token lies in the first 32-token chunk and past it"""
+    with refuse, texts whose stray token lies in the first 32-token chunk and past it.  With n_texts, that many texts: the offsets
+    scan carries its total over chunks of 1,024 texts, and the length / row kernels loop past their grid at 20,000"""
     from genrec_b200 import functional as Fn
     L = 100
-    texts = [_text(L, n) for n in (0, 1, 31, 32, 33, 64, L)] + [_text(L, 3, gap_at=70), _text(L, 40, gap_at=90)]
-    keep = [1] * 7 + [0, 0]
-    if refuse:
-        texts += [_text(L, 5, gap_at=9), _text(L, 35, gap_at=80), _text(L, 64, gap_at=65)]
-        keep += [1, 1, 1]
+    if n_texts is None:
+        texts = [_text(L, n) for n in (0, 1, 31, 32, 33, 64, L)] + [_text(L, 3, gap_at=70), _text(L, 40, gap_at=90)]
+        keep = [1] * 7 + [0, 0]
+        if refuse:
+            texts += [_text(L, 5, gap_at=9), _text(L, 35, gap_at=80), _text(L, 64, gap_at=65)]
+            keep += [1, 1, 1]
+    else:
+        texts, keep = _many_texts(n_texts, L, refuse)
     tokens = torch.tensor(texts, dtype=torch.long)
     lens, first_bad = _pack_rule(tokens, keep)
     offsets, info = Fn.cobra_pack_texts(tokens.to(DEV), torch.tensor(keep, dtype=torch.uint8, device=DEV))
