@@ -23,6 +23,7 @@
 #include "head_candidates.cuh"
 #include "head_rank.cuh"
 #include "head_topk.cuh"
+#include "hstu_ffn.cuh"
 #include "lazy_adam.cuh"
 #include "rowwise.cuh"
 #include "rq_argmin.cuh"
@@ -143,6 +144,16 @@ int with_rms_dim(int D, F&& f) {
     if (D == 256) return f(std::integral_constant<int, 256>{});
     if (D == 384) return f(std::integral_constant<int, 384>{});
     return fail(GRB_EINVAL, "rms norm supports D in {64,128,256,384}, got %d", D);
+}
+// The fused feed-forward (hstu_ffn.cuh) keeps two [64 x 128] fp32 accumulators per consumer thread: 128 of the 232 registers a
+// consumer thread holds, and ptxas reports no spills at D = 128.  At D = 256 the second one is [64 x 256], 64 + 128 accumulator
+// registers before the epilogue's 32 preloaded values and its addressing, past 232; so D = 256 keeps the four tc_gemm_kernel
+// launches.
+constexpr int FFN_FUSED_MAX_D = 128;
+template <class F>
+cudaError_t with_ffn_dim(int D, F&& f) {
+    if (D == 64) return f(std::integral_constant<int, 64>{});
+    return f(std::integral_constant<int, 128>{});
 }
 int row_grid(int T) {
     int need = (T + ROW_THREADS / 32 - 1) / (ROW_THREADS / 32);
@@ -578,8 +589,15 @@ int block_steps_out(const grb_hstu_layer_params* p, const float* x, float* y, co
     LnGateFwdArgs a{sv.O, D, sv.P, 4 * D, x, p->ln1_g, p->ln1_b, p->ln2_g, p->ln2_b, sv.x1, sv.xn, sv.st1, sv.st2, T, D, 1e-5f, drop_gate};
     GRB_TRY(with_row_dim(D, [&](auto DC) -> int { GRB_LAUNCH(ln_gate_fwd_kernel<DC / 64>, row_grid(T), ROW_THREADS, 0, st, a); return 0; }));
     // 5. h = drop(silu(xn W1^T + b1))                                                        (hstu.py:210-212)
-    GRB_CUDA(gemm_bias_act(1, sv.xn, (const bf16*)p->ffn1_w, p->ffn1_b, sv.z1, sv.hact, T, 4 * D, D, drop_hid, st));
     // 6. y = x1 + drop(h W2^T + b2)                                                          (hstu.py:213-214, :278)
+    if (D <= FFN_FUSED_MAX_D) {   // one kernel: h goes to the saved blob but is not read back (hstu_ffn.cuh)
+        GRB_CUDA(with_ffn_dim(D, [&](auto DC) {
+            return launch_ffn_fwd<DC>(sv.xn, (const bf16*)p->ffn1_w, p->ffn1_b, (const bf16*)p->ffn2_w, p->ffn2_b, sv.x1, sv.z1, sv.hact, y, T,
+                                      drop_hid, drop_out, sm_count(), st);
+        }));
+        return 0;
+    }
+    GRB_CUDA(gemm_bias_act(1, sv.xn, (const bf16*)p->ffn1_w, p->ffn1_b, sv.z1, sv.hact, T, 4 * D, D, drop_hid, st));
     GRB_CUDA(gemm_bias_res(sv.hact, (const bf16*)p->ffn2_w, p->ffn2_b, sv.x1, nullptr, y, T, D, 4 * D, drop_out, st));
     return 0;
 }
@@ -722,14 +740,21 @@ int layer_backward(const grb_hstu_dims* d, const grb_hstu_layer_params* p, const
 
     // FFN second linear
     GRB_TRY(cast_colsum(dy, w.dyb, T, D, drop_out, g->ffn2_b, w.part_cast, st));   // dyb = bf16(dropmask(dy)) ; db2 += column sums
-    GRB_CUDA(gemm_dact(1, w.dyb, (const bf16*)p->ffn2_w, sv.z1, w.dz1, T, 4 * D, D, drop_hid, st));  // dz1 = dropmask(dyb W2) * silu'(z1)
-    // FFN first linear
     // bias gradients are off the critical path too: with deferred weight gradients the column sums run beside the main chain
     auto colsum_4d = [&](const bf16* in, float* out) {
         return run_maybe_deferred(st, [&](cudaStream_t s_) -> int { return colsum(in, T, 4 * D, 4 * D, out, w.part_colsum, s_); });
     };
-    GRB_TRY(colsum_4d(w.dz1, g->ffn1_b));
-    GRB_CUDA(gemm_nn_f32(w.dz1, (const bf16*)p->ffn1_w, w.dxn, nullptr, 1.f, T, D, 4 * D, 4 * D, D, st));  // dxn = dz1 W1
+    // dz1 = dropmask(dyb W2) * silu'(z1) ; dxn = dz1 W1
+    if (D <= FFN_FUSED_MAX_D) {   // one kernel: dz1 goes to the workspace but is not read back (hstu_ffn.cuh)
+        GRB_CUDA(with_ffn_dim(D, [&](auto DC) {
+            return launch_ffn_bwd<DC>(w.dyb, (const bf16*)p->ffn2_w, (const bf16*)p->ffn1_w, sv.z1, w.dz1, w.dxn, T, drop_hid, sm_count(), st);
+        }));
+        GRB_TRY(colsum_4d(w.dz1, g->ffn1_b));
+    } else {
+        GRB_CUDA(gemm_dact(1, w.dyb, (const bf16*)p->ffn2_w, sv.z1, w.dz1, T, 4 * D, D, drop_hid, st));
+        GRB_TRY(colsum_4d(w.dz1, g->ffn1_b));
+        GRB_CUDA(gemm_nn_f32(w.dz1, (const bf16*)p->ffn1_w, w.dxn, nullptr, 1.f, T, D, 4 * D, 4 * D, D, st));
+    }
     // LN2 + residual + gate + LN1
     {
         LnGateBwdArgs a{dy, w.dxn, sv.x1, sv.st1, sv.st2, sv.O, D, sv.P, 4 * D, sv.zp, 4 * D, p->ln1_g, p->ln1_b, p->ln2_g,
