@@ -183,6 +183,13 @@ SIGNATURES = {
     "grb_t5_attention_backward": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 8 + [c_void_p, c_void_p, c_int, c_void_p, c_int, c_float, c_float,
                                           c_u64, c_void_p, C.c_uint32, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p,
                                           c_void_p, c_void_p, c_void_p, c_void_p]),
+    "grb_cobra_beam_attention_workspace_bytes": (c_size_t, [c_int] * 5),
+    "grb_cobra_beam_attention": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_void_p]
+                                 + [c_int] * 5 + [c_void_p, c_int, c_void_p, c_void_p]),
+    "grb_cobra_beam_topk_workspace_bytes": (c_size_t, [c_int] * 4),
+    "grb_cobra_beam_topk": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int] + [c_void_p] * 6),
+    "grb_cobra_dense_match_workspace_bytes": (c_size_t, [c_int] * 3),
+    "grb_cobra_dense_match": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int] + [c_void_p] * 4),
     "grb_trie_log_softmax": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                      c_void_p, c_void_p]),
     "grb_beam_select": (c_int, [c_void_p] * 8 + [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),

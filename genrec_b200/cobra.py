@@ -25,7 +25,16 @@ is a GEMM for the scores, one row kernel for the loss and dS, and a GEMM for dpr
 embedding gathers, the residual adds, the dropouts on the residual branches and the metrics stay in torch.  Dropout seeds come
 from torch's CPU generator, so ``torch.manual_seed`` makes a step reproducible bit for bit.
 
-``generate`` and ``beam_fusion`` are not implemented here (NotImplementedError).
+Generation (``generate``, cobra.py:531-665) decodes each user's history once: the encoder and the decoder run over the B padded
+histories (``_decode``, which keeps every layer's QKV), and each later codebook is one new token per beam.  Its layer runs the QKV
+GEMM into a per-step buffer, ``grb_cobra_beam_attention`` (the history's K | V read in place from the prefill's QKV, the beam's own
+earlier tokens through an ancestry table), and then the same layer body as training (``_layer_tail``).  ``grb_cobra_beam_topk``
+adds log_softmax(logits / temperature) to the parents' scores and keeps the K best per user, writing the next ancestry table, so
+beam selection never moves K | V.  Each user gets the beams the reference gives that user alone (INTEGRATION.md), bit for bit
+whatever the batch around it.  ``beam_fusion`` (cobra.py:679-760) finds each beam's best catalog row with ``grb_cobra_dense_match``,
+one wgmma sweep of the bf16 catalog, without the [B, n_beam, N] similarity; the B x n_beam fusion tail stays in torch.  Both run
+without gradients and without dropout, and read two values to the host: the item-layout flag of ``_check_generate`` and the
+encoder's packing info.
 """
 from __future__ import annotations
 
@@ -41,13 +50,37 @@ from . import functional as Fn
 from ._lib import ensure_device, require_cuda
 from .t5_attention import attention_core_bwd, attention_core_bwd_jagged, attention_core_fwd, attention_core_fwd_jagged
 
-__all__ = ["Cobra", "CobraOutput"]
+__all__ = ["Cobra", "CobraOutput", "CobraGenerationOutput", "BeamFusionOutput"]
 
 LN_DIMS = (64, 128, 192, 256, 384, 768)           # widths of the LayerNorm row kernels
 POOL_DIMS = (128, 192, 256, 384, 768)             # widths of the pooled LayerNorm kernel
 ENC_HEAD_DIMS = (32, 64, 96)
 DEC_HEAD_DIMS = (32, 64)
 MAX_ATTN_ROWS = 65535                             # texts x heads (or users x heads) of one attention backward
+_MAX_BEAMS = 1024                                 # beams per user of generate (grb_cobra_beam_topk, grb_cobra_beam_attention)
+_MAX_CANDIDATES = 262144                          # beams x id_vocab_size of one beam step
+_CATALOG_CHUNK = 65536                            # catalog rows normalised at a time by beam_fusion
+
+
+class CobraGenerationOutput(NamedTuple):     # (cobra.py:29-35)
+    sem_ids: torch.Tensor           # [B, K, C]
+    dense_vecs: torch.Tensor        # [B, K, d_model]
+    scores: torch.Tensor            # [B, K]
+
+
+class BeamFusionOutput(NamedTuple):          # (cobra.py:38-44)
+    item_ids: torch.Tensor          # [B, K]
+    sem_ids: torch.Tensor           # [B, K, C]
+    scores: torch.Tensor            # [B, K]
+
+
+class _MissingArguments(TypeError, NotImplementedError):
+    """a generation call without its history inputs: a TypeError naming them, as Python's own, and a NotImplementedError, which a
+    call without arguments raised before generation was native"""
+
+    def __init__(self, fn: str, names):
+        super().__init__(f"{fn}() missing {len(names)} required argument{'s' if len(names) > 1 else ''}: "
+                         + ", ".join(repr(n) for n in names))
 
 
 class CobraOutput(NamedTuple):      # (cobra.py:12-26)
@@ -113,11 +146,13 @@ class _MhaFn(torch.autograd.Function):
     x [B, L, D] with key_pad [B, L] uint8 and causal; packed: x [T, D] with offsets [N+1] and max_len (no key padding)."""
 
     @staticmethod
-    def forward(ctx, x, w_in, b_in, w_out, b_out, H, p, seed, site, key_pad, causal, offsets, max_len):
+    def forward(ctx, x, w_in, b_in, w_out, b_out, H, p, seed, site, key_pad, causal, offsets, max_len, keep_qkv=None):
         D = x.shape[-1]
         xb = Fn.cast_rows_bf16(x.detach().contiguous().float())
         wib, wob = Fn.cast_bf16(w_in), Fn.cast_bf16(w_out)
         QKV, _ = Fn.linear_fwd(xb, wib, b_in.detach().contiguous(), 0)
+        if keep_qkv is not None:                      # generation's prefill keeps every layer's K | V
+            keep_qkv.append(QKV)
         Q, K, V = QKV[..., :D], QKV[..., D:2 * D], QKV[..., 2 * D:]
         scale = 1.0 / math.sqrt(D // H)
         if offsets is None:
@@ -145,7 +180,8 @@ class _MhaFn(torch.autograd.Function):
         dqkv = torch.cat([dQ.float(), dK, dV], dim=-1)
         dx, dwi, _ = Fn.linear_bwd(Fn.cast_rows_bf16(dqkv), wib, xb)
         dyc = dout.contiguous().float()
-        return (dx, dwi, dqkv.reshape(-1, 3 * D).sum(0), dwo, dyc.reshape(-1, D).sum(0), None, None, None, None, None, None, None, None)
+        return (dx, dwi, dqkv.reshape(-1, 3 * D).sum(0), dwo, dyc.reshape(-1, D).sum(0), None, None, None, None, None, None, None, None,
+                None)
 
 
 class _FfnFn(torch.autograd.Function):
@@ -382,21 +418,27 @@ class Cobra(nn.Module):
         h = h * m + e.pos_embed.weight[:Li].unsqueeze(0) * m + F.embedding(types.long(), e.type_embed.weight).unsqueeze(0) * m
         return h, mask
 
-    def _decode(self, x, mask):
+    def _decode(self, x, mask, keep_qkv=None):
+        """keep_qkv: a list that receives each layer's self-attention QKV [B, Li, 3D] bf16 (generation's prefill), or None"""
         key_pad = (~mask).to(torch.uint8).contiguous()
         seed = self._seed()
         for i, layer in enumerate(self.decoder.decoder.layers):
-            sa, ca = layer.self_attn, layer.multihead_attn
+            sa = layer.self_attn
             a = _MhaFn.apply(x, sa.in_proj_weight, sa.in_proj_bias, sa.out_proj.weight, sa.out_proj.bias, sa.num_heads, self._p(sa.dropout),
-                             seed, 16 * i + 1, key_pad, True, None, 0)
-            x = _LayerNormFn.apply(x + self._drop(a, layer.dropout1.p), layer.norm1.weight, layer.norm1.bias, layer.norm1.eps)
-            # attention over a zero-length memory is the out_proj bias (cobra.py:209-223)
-            cross = _ZeroGrads.apply(ca.out_proj.bias, ca.in_proj_weight, ca.in_proj_bias, ca.out_proj.weight).expand_as(x)
-            x = _LayerNormFn.apply(x + self._drop(cross, layer.dropout2.p), layer.norm2.weight, layer.norm2.bias, layer.norm2.eps)
-            f = _FfnFn.apply(x, layer.linear1.weight, layer.linear1.bias, layer.linear2.weight, layer.linear2.bias, self._p(layer.dropout.p),
-                             self._p(layer.dropout3.p), seed, 16 * i + 2)
-            x = _LayerNormFn.apply(f, layer.norm3.weight, layer.norm3.bias, layer.norm3.eps)
+                             seed, 16 * i + 1, key_pad, True, None, 0, keep_qkv)
+            x = self._layer_tail(i, layer, x, a, seed)
         return x
+
+    def _layer_tail(self, i, layer, x, a, seed):
+        """a decoder layer after its self-attention output a: the residual and norm1, the cross-attention and norm2, the FFN and norm3"""
+        ca = layer.multihead_attn
+        x = _LayerNormFn.apply(x + self._drop(a, layer.dropout1.p), layer.norm1.weight, layer.norm1.bias, layer.norm1.eps)
+        # attention over a zero-length memory is the out_proj bias (cobra.py:209-223)
+        cross = _ZeroGrads.apply(ca.out_proj.bias, ca.in_proj_weight, ca.in_proj_bias, ca.out_proj.weight).expand_as(x)
+        x = _LayerNormFn.apply(x + self._drop(cross, layer.dropout2.p), layer.norm2.weight, layer.norm2.bias, layer.norm2.eps)
+        f = _FfnFn.apply(x, layer.linear1.weight, layer.linear1.bias, layer.linear2.weight, layer.linear2.bias, self._p(layer.dropout.p),
+                         self._p(layer.dropout3.p), seed, 16 * i + 2)
+        return _LayerNormFn.apply(f, layer.norm3.weight, layer.norm3.bias, layer.norm3.eps)
 
     # ---- the reference's interface
     def forward(self, input_ids: torch.Tensor, encoder_input_ids: torch.Tensor, mask=None) -> CobraOutput:
@@ -473,9 +515,130 @@ class Cobra(nn.Module):
                            acc_total=total_tokens, recall_correct=item_correct_masked.sum(), recall_total=all_valid_mask.sum(),
                            vec_cos_sim=vec_cos_sim, codebook_entropy=codebook_entropy)
 
-    def generate(self, *args, **kwargs):
-        raise NotImplementedError("genrec_b200.Cobra.generate: prefix-cached COBRA generation is a separate follow-up (its ragged-batch "
-                                  "semantics are not settled)")
+    # ---- generation (cobra.py:531-760)
+    def generate(self, input_ids: Optional[torch.Tensor] = None, encoder_input_ids: Optional[torch.Tensor] = None, n_candidates: int = 10,
+                 temperature: float = 1.0) -> CobraGenerationOutput:
+        """cobra.py:531-665 with per-user semantics: each user gets the beams the reference gives that user alone (its generated token j
+        at position n_b (C+1) + j, attending to its own n_b (C+1) history rows), whatever the batch around it.  input_ids [B, T*C] with
+        pad items after the real ones, encoder_input_ids [B, T, L] right-padded with 0.  -> sem_ids [B, K, C], dense_vecs [B, K, d_model]
+        (unit rows of h at the last input position of the final step), scores [B, K] (summed log-softmax of logits / temperature), best
+        first, equal totals by the lower beam * V + token.  Runs without gradients and without dropout."""
+        missing = [n for n, v in (("input_ids", input_ids), ("encoder_input_ids", encoder_input_ids)) if v is None]
+        if missing:
+            raise _MissingArguments("Cobra.generate", missing)
+        self._check_generate(input_ids, encoder_input_ids, n_candidates, temperature, "n_candidates")
+        with torch.no_grad():
+            return self._generate(input_ids, encoder_input_ids, n_candidates, temperature)
 
-    def beam_fusion(self, *args, **kwargs):
-        raise NotImplementedError("genrec_b200.Cobra.beam_fusion: BeamFusion follows native COBRA generation, a separate follow-up")
+    def beam_fusion(self, input_ids: Optional[torch.Tensor] = None, encoder_input_ids: Optional[torch.Tensor] = None,
+                    item_dense_vecs: Optional[torch.Tensor] = None, item_sem_ids: Optional[torch.Tensor] = None, n_candidates: int = 10,
+                    n_beam: int = 50, temperature: float = 1.0, alpha: float = 0.5) -> BeamFusionOutput:
+        """cobra.py:679-760 on native generate(n_beam): each beam's best catalog row (item_dense_vecs [N, d_model], re-normalised as
+        the reference does) and its similarity come from one sweep of the catalog, without the [B, n_beam, N] similarity; then
+        alpha softmax(scores) + (1 - alpha) (max_sim + 1) / 2 and its top n_candidates (equal fused scores: the lower beam first).
+        Equal similarities: the lower catalog row.  -> item_ids [B, n_candidates], sem_ids [B, n_candidates, C] (item_sem_ids [N, C]
+        gathered), scores."""
+        missing = [n for n, v in (("input_ids", input_ids), ("encoder_input_ids", encoder_input_ids), ("item_dense_vecs", item_dense_vecs),
+                                  ("item_sem_ids", item_sem_ids)) if v is None]
+        if missing:
+            raise _MissingArguments("Cobra.beam_fusion", missing)
+        if not 1 <= n_candidates <= n_beam:
+            raise ValueError(f"Cobra.beam_fusion: n_candidates {n_candidates} must lie in 1 .. n_beam ({n_beam})")
+        if item_dense_vecs.dim() != 2 or item_dense_vecs.shape[1] != self.d_model or item_dense_vecs.shape[0] < 1:
+            raise ValueError(f"Cobra.beam_fusion: item_dense_vecs must be [N >= 1, {self.d_model}], got {tuple(item_dense_vecs.shape)}")
+        N = item_dense_vecs.shape[0]
+        if tuple(item_sem_ids.shape) != (N, self.C):
+            raise ValueError(f"Cobra.beam_fusion: item_sem_ids must be [{N}, {self.C}], got {tuple(item_sem_ids.shape)}")
+        self._check_generate(input_ids, encoder_input_ids, n_beam, temperature, "n_beam")
+        require_cuda(item_dense_vecs, item_sem_ids)
+        with torch.no_grad():
+            gen = self._generate(input_ids, encoder_input_ids, n_beam, temperature)
+            B = input_ids.shape[0]
+            table = torch.empty(N, self.d_model, dtype=torch.bfloat16, device=input_ids.device)
+            for s in range(0, N, _CATALOG_CHUNK):                   # F.normalize(item_dense_vecs), bf16, a chunk of rows at a time
+                chunk = item_dense_vecs[s:s + _CATALOG_CHUNK].to(device=input_ids.device, dtype=torch.float32).contiguous()
+                table[s:s + _CATALOG_CHUNK] = Fn.cast_rows_bf16(Fn.l2norm_fwd(chunk)[0])
+            best, item = Fn.cobra_dense_match(Fn.cast_rows_bf16(gen.dense_vecs.reshape(-1, self.d_model).contiguous()), table)
+            max_sim, best_item = best.view(B, n_beam), item.view(B, n_beam)
+            fused = alpha * torch.softmax(gen.scores, dim=-1) + (1 - alpha) * ((max_sim + 1) / 2)
+            top, idx = torch.sort(fused, dim=-1, descending=True, stable=True)
+            item_ids = best_item.gather(1, idx[:, :n_candidates])
+            return BeamFusionOutput(item_ids=item_ids, sem_ids=item_sem_ids[item_ids], scores=top[:, :n_candidates].contiguous())
+
+    def _check_generate(self, input_ids, encoder_input_ids, K, temperature, k_name):
+        """the refusals of generate / beam_fusion, before any launch; the item checks read one flag to the host"""
+        C, V = self.C, self.sparse_head[0].out_features
+        if input_ids.dim() != 2 or input_ids.shape[1] % C or encoder_input_ids.dim() != 3 or \
+                tuple(encoder_input_ids.shape[:2]) != (input_ids.shape[0], input_ids.shape[1] // C) or input_ids.shape[0] < 1:
+            raise ValueError(f"Cobra: input_ids [B, T*C] and encoder_input_ids [B, T, L] expected, got {tuple(input_ids.shape)} and "
+                             f"{tuple(encoder_input_ids.shape)}")
+        if not 1 <= K <= min(V, _MAX_BEAMS) or K * V > _MAX_CANDIDATES:
+            raise ValueError(f"Cobra: {k_name} {K} must lie in 1 .. min(id_vocab_size, {_MAX_BEAMS}) = {min(V, _MAX_BEAMS)} with "
+                             f"{k_name} * id_vocab_size <= {_MAX_CANDIDATES}")
+        if not temperature > 0:
+            raise ValueError(f"Cobra: temperature must be positive, got {temperature}")
+        T = input_ids.shape[1] // C
+        if T * (C + 1) + C - 1 >= self.max_len:
+            raise ValueError(f"Cobra: {T} items leave no positions for the generated tokens: T*(C+1) + C - 1 = {T * (C + 1) + C - 1} must "
+                             f"be below max_len {self.max_len}")
+        real = (input_ids != self.pad_id).view(-1, T, C)[:, :, C - 1]
+        flag = int(((~real.any(1)).any().long() + 2 * (real[:, 1:] & ~real[:, :-1]).any().long()).item())
+        if flag & 1:
+            raise ValueError("Cobra: a user has no item")
+        if flag & 2:
+            raise ValueError("Cobra: a real item follows a pad item; pad items must come after a user's real ones")
+
+    def _generate(self, input_ids, encoder_input_ids, K, temperature) -> CobraGenerationOutput:
+        require_cuda(input_ids, encoder_input_ids)
+        ensure_device(input_ids.device)
+        training = self.training
+        self.train(False)                             # no dropout; restored below
+        try:
+            return self._beam_search(input_ids, encoder_input_ids, K, temperature)
+        finally:
+            self.train(training)
+
+    def _beam_search(self, input_ids, encoder_input_ids, K, temperature):
+        e = self.cobra_emb
+        B, TC = input_ids.shape
+        C, D, V = self.C, self.d_model, self.sparse_head[0].out_features
+        T, L = TC // C, encoder_input_ids.shape[2]
+        dev = input_ids.device
+        # prefill: the histories once, each layer's QKV kept
+        mask_items = (input_ids != self.pad_id).view(B, T, C)
+        keep = mask_items[:, :, C - 1].reshape(-1).to(torch.uint8).contiguous()
+        vecs = self._encode(encoder_input_ids.reshape(B * T, L), keep).view(B, T, -1)
+        emb, seq_mask = self._interleave(input_ids, vecs, mask_items)
+        hist_qkv = []
+        h = self._decode(emb, seq_mask, hist_qkv)
+        hist_len = (mask_items[:, :, C - 1].sum(1) * (C + 1)).to(torch.int32)
+        h = h[torch.arange(B, device=dev), hist_len.long() - 1]                       # the last dense position: codebook 0
+        head = self.sparse_head[0]
+        tokens, scores, _, _ = Fn.cobra_beam_topk(_LinearF32Fn.apply(h, head.weight, head.bias).contiguous(), None, B, K, temperature)
+        seqs = tokens.unsqueeze(-1)
+        h_last = h.unsqueeze(1).expand(B, K, D) if C == 1 else None
+        # extension: one new token per beam and codebook, attending to its user's history and its own earlier tokens
+        layers = self.decoder.decoder.layers
+        R = B * K
+        suf = [torch.empty(C - 1, R, 3 * D, dtype=torch.bfloat16, device=dev) for _ in layers] if C > 1 else []
+        w = [(Fn.cast_bf16(l.self_attn.in_proj_weight), Fn.cast_bf16(l.self_attn.out_proj.weight)) for l in layers] if C > 1 else []
+        pos = hist_len.long().repeat_interleave(K)
+        anc = None
+        for c in range(1, C):
+            tok = tokens.reshape(-1) + (c - 1) * e.id_vocab_size
+            x = e.id_embed.weight[tok] + e.pos_embed.weight[pos + (c - 1)] + e.type_embed.weight[0]
+            for i, layer in enumerate(layers):
+                sa = layer.self_attn
+                qkv = suf[i][c - 1]
+                Fn.linear_fwd(Fn.cast_rows_bf16(x.contiguous()), w[i][0], sa.in_proj_bias.detach().contiguous(), 0, out=qkv)
+                A = Fn.cobra_beam_attention(qkv[:, :D], hist_qkv[i], hist_len, suf[i], anc, c, sa.num_heads)
+                a, _ = Fn.linear_fwd(A, w[i][1], sa.out_proj.bias.detach().contiguous(), 0)
+                x = self._layer_tail(i, layer, x, a.float(), 0)
+            head = self.sparse_head[c]
+            logits = _LinearF32Fn.apply(x, head.weight, head.bias).contiguous()
+            tokens, scores, parents, anc = Fn.cobra_beam_topk(logits, scores, B, K, temperature, anc)
+            seqs = torch.cat([seqs.gather(1, parents.unsqueeze(-1).expand(-1, -1, c)), tokens.unsqueeze(-1)], dim=-1)
+            if c == C - 1:
+                h_last = x.view(B, K, D).gather(1, parents.unsqueeze(-1).expand(-1, -1, D))
+        dense = Fn.l2norm_fwd(h_last.contiguous())[0]
+        return CobraGenerationOutput(sem_ids=seqs, dense_vecs=dense, scores=scores)

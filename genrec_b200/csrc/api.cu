@@ -17,6 +17,7 @@
 #include "attn_t5.cuh"
 #include "beam.cuh"
 #include "cobra.cuh"
+#include "cobra_generate.cuh"
 #include "common.cuh"
 #include "dp_adam.cuh"
 #include "exact_f32.cuh"
@@ -2125,6 +2126,124 @@ int grb_infonce_forward_backward(const float* scores, int Q, int ld, const int64
     GRB_LAUNCH(infonce_rows_kernel, (unsigned)Q, 256, 0, st, scores, Q, ld, reinterpret_cast<const long long*>(lo),
                reinterpret_cast<const long long*>(hi), inv_tau, row_loss, static_cast<bf16*>(dscores));
     GRB_LAUNCH(ce_loss_sum_kernel, 1, 1024, 0, st, row_loss, Q, loss);
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ COBRA generation
+namespace {
+int cobra_attn_check(int B, int K, int H, int head_dim, int hist_rows) {
+    GRB_REQUIRE(B >= 1 && H >= 1 && (head_dim == 32 || head_dim == 64), "bad shape B=%d H=%d head_dim=%d (head_dim 32 or 64)", B, H,
+                head_dim);
+    GRB_REQUIRE(K >= 1 && K <= CBA_MAX_K, "K=%d beams per user, must lie in [1, %d]", K, CBA_MAX_K);
+    GRB_REQUIRE(hist_rows >= 1 && hist_rows <= CBA_MAX_HIST, "hist_rows=%d, must lie in [1, %d]", hist_rows, CBA_MAX_HIST);
+    return 0;
+}
+int cobra_attn_splits(int hist_rows) { return (hist_rows + CBA_CHUNK - 1) / CBA_CHUNK; }
+}  // namespace
+
+size_t grb_cobra_beam_attention_workspace_bytes(int B, int K, int H, int head_dim, int hist_rows) {
+    if (cobra_attn_check(B, K, H, head_dim, hist_rows)) return 0;
+    return (size_t)B * H * cobra_attn_splits(hist_rows) * K * (head_dim + 2) * 4;
+}
+
+int grb_cobra_beam_attention(const void* q, int ldq, const void* hist_k, const void* hist_v, int ld_hist, int hist_rows,
+                             const int32_t* hist_len, const void* suf_k, const void* suf_v, int ld_suf, int64_t suf_step_stride,
+                             const int32_t* anc, int S, int B, int K, int H, int head_dim, void* out, int ldo, void* workspace,
+                             void* stream) {
+    GRB_TRY(cobra_attn_check(B, K, H, head_dim, hist_rows));
+    GRB_REQUIRE(q && hist_k && hist_v && hist_len && out && workspace, "null argument");
+    GRB_REQUIRE(S >= 1 && suf_k && suf_v && (S == 1 || anc), "S=%d suffix keys need suf_k, suf_v (and anc for S > 1)", S);
+    const int D = H * head_dim;
+    GRB_REQUIRE(ldq >= D && ld_hist >= D && ld_suf >= D && ldo >= D && suf_step_stride >= (int64_t)B * K * ld_suf,
+                "leading dimensions below H * head_dim = %d, or suffix steps overlap", D);
+    GRB_REQUIRE(ldq % 2 == 0 && ld_hist % 2 == 0 && aligned16(hist_k) && aligned16(hist_v) && aligned16(workspace),
+                "hist_k / hist_v / workspace must be 16-byte aligned and ldq, ld_hist even");
+    CobraBeamAttnArgs a{(const bf16*)q, ldq, (const bf16*)hist_k, (const bf16*)hist_v, ld_hist, hist_rows, hist_len, (const bf16*)suf_k,
+                        (const bf16*)suf_v, ld_suf, (long long)suf_step_stride, anc, S, B, K, H, cobra_attn_splits(hist_rows),
+                        1.f / sqrtf((float)head_dim), static_cast<float*>(workspace), static_cast<bf16*>(out), ldo};
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const unsigned merge_blocks = (unsigned)(((long long)B * K * H + CBA_THREADS / 32 - 1) / (CBA_THREADS / 32));
+    return with_head_dim(head_dim, [&](auto DH) {
+        GRB_LAUNCH(cobra_attn_part_kernel<DH>, (unsigned)(B * H * a.splits), CBA_THREADS, 0, st, a);
+        GRB_LAUNCH(cobra_attn_merge_kernel<DH>, merge_blocks, CBA_THREADS, 0, st, a);
+        return 0;
+    });
+}
+
+namespace {
+int cobra_topk_check(int B, int K_in, int V, int K, int S_in) {
+    GRB_REQUIRE(B >= 1 && K_in >= 1 && K_in <= CBA_MAX_K && V >= 1 && S_in >= 0, "bad shape B=%d K_in=%d V=%d S_in=%d", B, K_in, V, S_in);
+    GRB_REQUIRE(K >= 1 && K <= BEAM_WIDE_MAX_K, "K=%d beams, must lie in [1, %d]", K, BEAM_WIDE_MAX_K);
+    GRB_REQUIRE((long long)K_in * V <= CBT_MAX_CAND && (long long)K * V <= CBT_MAX_CAND, "K * V and K_in * V must be <= %d (K=%d K_in=%d V=%d)",
+                CBT_MAX_CAND, K, K_in, V);
+    GRB_REQUIRE(K <= K_in * V, "K=%d beams from %d candidates", K, K_in * V);
+    return 0;
+}
+}  // namespace
+
+size_t grb_cobra_beam_topk_workspace_bytes(int B, int K_in, int V, int K) {
+    if (cobra_topk_check(B, K_in, V, K, 0)) return 0;
+    return (size_t)B * K_in * V * 4;
+}
+
+int grb_cobra_beam_topk(const float* logits, const float* scores_in, int B, int K_in, int V, int K, float temperature, const int32_t* anc_in,
+                        int S_in, int64_t* tokens, float* scores, int32_t* parents, int32_t* anc_out, void* workspace, void* stream) {
+    GRB_TRY(cobra_topk_check(B, K_in, V, K, S_in));
+    GRB_REQUIRE(logits && tokens && scores && parents && workspace, "null argument");
+    GRB_REQUIRE(S_in == 0 || (anc_in && anc_out), "anc_in / anc_out missing with S_in=%d", S_in);
+    GRB_REQUIRE(temperature > 0.f, "temperature must be positive");
+    CobraTopkArgs a{logits, scores_in, anc_in, B, K_in, V, K, S_in, temperature, static_cast<unsigned*>(workspace),
+                    reinterpret_cast<long long*>(tokens), scores, parents, anc_out};
+    GRB_LAUNCH(cobra_beam_topk_kernel, (unsigned)B, BEAM_WIDE_THREADS, 0, static_cast<cudaStream_t>(stream), a);
+    return 0;
+}
+
+namespace {
+struct DenseMatchWork {
+    float* cand_s; int* cand_i;
+    int num_m, num_n, splits;
+    size_t bytes;
+};
+DenseMatchWork carve_dense_match(void* base, int R, int N) {
+    DenseMatchWork w;
+    Carver c{static_cast<char*>(base)};
+    w.num_m = (R + TC_BM - 1) / TC_BM;
+    w.num_n = (N + TC_BN - 1) / TC_BN;
+    int s = sm_count() / w.num_m;               // enough CTAs to cover the SMs once, never more ranges than item tiles
+    s = s < w.num_n ? s : w.num_n;
+    s = s < DMATCH_MAX_SPLITS ? s : DMATCH_MAX_SPLITS;
+    w.splits = s < 1 ? 1 : s;
+    w.cand_s = c.take<float>((size_t)R * w.splits * 4);
+    w.cand_i = c.take<int>((size_t)R * w.splits * 4);
+    w.bytes = c.off;
+    return w;
+}
+int dense_match_check(int R, int D, int N) {
+    GRB_REQUIRE(R >= 1 && N >= 1 && (D == 64 || D == 128 || D == 192 || D == 256 || D == 384 || D == 768),
+                "bad shape R=%d D=%d N=%d (R, N >= 1, D in {64,128,192,256,384,768})", R, D, N);
+    return 0;
+}
+}  // namespace
+
+size_t grb_cobra_dense_match_workspace_bytes(int R, int D, int N) {
+    if (dense_match_check(R, D, N)) return 0;
+    return carve_dense_match(nullptr, R, N).bytes;
+}
+
+int grb_cobra_dense_match(const void* x_bf16, const void* table_bf16, int R, int D, int N, float* best, int64_t* item, void* workspace,
+                          void* stream) {
+    GRB_TRY(dense_match_check(R, D, N));
+    GRB_REQUIRE(x_bf16 && table_bf16 && best && item && workspace, "null argument");
+    GRB_REQUIRE(aligned16(x_bf16) && aligned16(table_bf16) && aligned16(workspace), "x, table and workspace must be 16-byte aligned");
+    const DenseMatchWork w = carve_dense_match(workspace, R, N);
+    CUtensorMap tmA, tmB;
+    GRB_REQUIRE(make_tmap_bf16(&tmA, x_bf16, R, D, D, TC_BK, TC_BM) && make_tmap_bf16(&tmB, table_bf16, N, D, D, TC_BK, TC_BN),
+                "cannot encode the TMA descriptors (driver entry point missing)");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DenseMatchArgs a{R, N, w.splits, w.num_n, D / TC_BK, w.cand_s, w.cand_i};
+    GRB_LAUNCH(cobra_dense_match_kernel, w.num_m * w.splits, TC_THREADS, TC_SMEM_BYTES, st, tmA, tmB, a);
+    GRB_LAUNCH(cobra_dense_merge_kernel, (unsigned)((R + 255) / 256), 256, 0, st, (const float*)w.cand_s, (const int*)w.cand_i, R, w.splits,
+               best, reinterpret_cast<long long*>(item));
     return 0;
 }
 

@@ -204,8 +204,8 @@ __global__ void __launch_bounds__(BEAM_MAX_CAND) beam_select_kernel(BeamSelectAr
 //   beam_class_kernel         class of every parent = the smallest parent with the same token sequence           (one CTA per row)
 //   beam_dedup_insert_kernel  hash table per row: (class, token) -> the largest key among its candidates        (grid-stride)
 //   beam_dedup_mark_kernel    mono[i] = the monotone total of candidate i if it holds its group's slot, else 0    (grid-stride)
-//   beam_wide_select_kernel   radix select of the K-th largest mono, index-ordered ties, a sort of the K picks,
-//                             and the output of beam_emit / beam_fill                                          (one CTA per row)
+//   beam_wide_select_kernel   beam_radix_topk (radix select of the K-th largest mono, index-ordered ties, a sort of the K picks;
+//                             COBRA's beam step shares it), then the output of beam_emit / beam_fill            (one CTA per row)
 // key = monotone total << 32 | (2^32 - 1 - flat index): unique per candidate, larger = earlier in the order; 0 never occurs (the
 // flat index is < 2^18), so 0 marks an empty slot.  The selected set and its order do not depend on which CTA inserts first.
 constexpr int BEAM_WIDE_MAX_K = 1024;
@@ -304,99 +304,112 @@ __global__ void __launch_bounds__(256) beam_dedup_mark_kernel(BeamWideArgs w) {
     }
 }
 
-__global__ void __launch_bounds__(BEAM_WIDE_THREADS) beam_wide_select_kernel(BeamWideArgs w) {
-    pdl_wait();
-    __shared__ unsigned hist[256];
-    __shared__ unsigned long long s_key[BEAM_WIDE_MAX_K];
-    __shared__ int s_warp[BEAM_WIDE_THREADS / 32];
-    __shared__ unsigned s_prefix;
-    __shared__ int s_need, s_cnt, s_all;
-    const BeamSelectArgs& a = w.s;
-    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int n = a.K * a.KK;
-    const unsigned* mono = w.mono + (size_t)b * n;
-    if (tid == 0) { s_prefix = 0u; s_need = a.K; s_cnt = 0; s_all = 0; }
-    // radix select, 8 bits at a time from the top, of the K-th largest nonzero mono (the threshold T = s_prefix); s_need ends as
-    // the number of first occurrences equal to T that are picked.  With at most K first occurrences, every one is picked.
+// Shared memory of beam_radix_topk.
+struct BeamRadixSmem {
+    unsigned hist[256];
+    unsigned long long key[BEAM_WIDE_MAX_K];
+    int warp[BEAM_WIDE_THREADS / 32];
+    unsigned prefix;
+    int need, cnt, all;
+};
+
+// The K largest nonzero entries of mono [n] (n < 2^31), by all BEAM_WIDE_THREADS threads of the CTA: radix select of the K-th
+// largest value, index-ordered ties, then a sort of the picks.  Returns the number of picks (min(K, nonzero entries)); s.key[0 ..]
+// holds their beam_key, largest first (equal values: the lower index first).
+GRB_DEVINL int beam_radix_topk(const unsigned* mono, int n, int K, BeamRadixSmem& s) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) { s.prefix = 0u; s.need = K; s.cnt = 0; s.all = 0; }
+    // radix select, 8 bits at a time from the top, of the K-th largest nonzero mono (the threshold T = s.prefix); s.need ends as
+    // the number of entries equal to T that are picked.  With at most K nonzero entries, every one is picked.
     unsigned pmask = 0u;
     for (int shift = 24; shift >= 0; shift -= 8) {
-        if (tid < 256) hist[tid] = 0u;
+        if (tid < 256) s.hist[tid] = 0u;
         __syncthreads();
-        const unsigned prefix = s_prefix;
+        const unsigned prefix = s.prefix;
         for (int i = tid; i < n; i += BEAM_WIDE_THREADS) {
             const unsigned v = mono[i];
-            if (v != 0u && (v & pmask) == prefix) atomicAdd(&hist[(v >> shift) & 255u], 1u);
+            if (v != 0u && (v & pmask) == prefix) atomicAdd(&s.hist[(v >> shift) & 255u], 1u);
         }
         __syncthreads();
         if (warp == 0) {                                  // lane l holds bins 255 - 8 l ... 248 - 8 l, largest digit first
             unsigned c[8], sum = 0u;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) { c[j] = hist[255 - 8 * lane - j]; sum += c[j]; }
+            for (int j = 0; j < 8; ++j) { c[j] = s.hist[255 - 8 * lane - j]; sum += c[j]; }
             unsigned incl = sum;
             for (int o = 1; o < 32; o <<= 1) {
                 const unsigned u = __shfl_up_sync(0xffffffffu, incl, o);
                 if (lane >= o) incl += u;
             }
-            const unsigned need = (unsigned)s_need;
+            const unsigned need = (unsigned)s.need;
             const unsigned all = __shfl_sync(0xffffffffu, incl, 31);
             if (shift == 24 && all <= need) {
-                if (lane == 0) s_all = 1;
+                if (lane == 0) s.all = 1;
             } else {
                 const unsigned hit = __ballot_sync(0xffffffffu, incl >= need);
                 if (lane == __ffs(hit) - 1) {
                     unsigned above = incl - sum;
                     int j = 0;
                     while (above + c[j] < need) above += c[j++];
-                    s_prefix = prefix | ((unsigned)(255 - 8 * lane - j) << shift);
-                    s_need = (int)(need - above);
+                    s.prefix = prefix | ((unsigned)(255 - 8 * lane - j) << shift);
+                    s.need = (int)(need - above);
                 }
             }
         }
         __syncthreads();
-        if (s_all) break;
+        if (s.all) break;
         pmask |= 255u << shift;
     }
-    const bool all = s_all != 0;
-    const unsigned T = all ? 0u : s_prefix;
-    const int need = all ? 0 : s_need;
-    // collect the picks: every first occurrence above T, and the `need` ones equal to T with the lowest flat index
+    const bool all = s.all != 0;
+    const unsigned T = all ? 0u : s.prefix;
+    const int need = all ? 0 : s.need;
+    // collect the picks: every entry above T, and the `need` ones equal to T with the lowest index
     int tie_base = 0;
     for (int base = 0; base < n; base += BEAM_WIDE_THREADS) {
         const int i = base + tid;
         const unsigned v = i < n ? mono[i] : 0u;
         const bool tie = need > 0 && v == T;
         const unsigned bal = __ballot_sync(0xffffffffu, tie);
-        if (lane == 0) s_warp[warp] = __popc(bal);
+        if (lane == 0) s.warp[warp] = __popc(bal);
         __syncthreads();
         int rank = tie_base + __popc(bal & ((1u << lane) - 1u)), tile = 0;
         for (int q = 0; q < BEAM_WIDE_THREADS / 32; ++q) {
-            const int cq = s_warp[q];
+            const int cq = s.warp[q];
             if (q < warp) rank += cq;
             tile += cq;
         }
-        if (v > T || (tie && rank < need)) s_key[atomicAdd(&s_cnt, 1)] = beam_key(v, i);
+        if (v > T || (tie && rank < need)) s.key[atomicAdd(&s.cnt, 1)] = beam_key(v, i);
         tie_base += tile;
         __syncthreads();
     }
-    const int npick = s_cnt;
+    const int npick = s.cnt;
     int P = 1;
-    while (P < a.K) P <<= 1;
-    if (tid < P && tid >= npick) s_key[tid] = 0ull;
+    while (P < K) P <<= 1;
+    if (tid < P && tid >= npick) s.key[tid] = 0ull;
     __syncthreads();
     // bitonic sort of the picks, largest key first
     for (int k = 2; k <= P; k <<= 1) {
         for (int j = k >> 1; j > 0; j >>= 1) {
             const int o = tid ^ j;
             if (tid < P && o > tid) {
-                const unsigned long long ka = s_key[tid], kb = s_key[o];
-                if (((tid & k) == 0) ? ka < kb : ka > kb) { s_key[tid] = kb; s_key[o] = ka; }
+                const unsigned long long ka = s.key[tid], kb = s.key[o];
+                if (((tid & k) == 0) ? ka < kb : ka > kb) { s.key[tid] = kb; s.key[o] = ka; }
             }
             __syncthreads();
         }
     }
+    return npick;
+}
+
+__global__ void __launch_bounds__(BEAM_WIDE_THREADS) beam_wide_select_kernel(BeamWideArgs w) {
+    pdl_wait();
+    __shared__ BeamRadixSmem s;
+    const BeamSelectArgs& a = w.s;
+    const int b = blockIdx.x, tid = threadIdx.x;
+    const int n = a.K * a.KK;
+    const int npick = beam_radix_topk(w.mono + (size_t)b * n, n, a.K, s);
     if (tid < a.K) {
         if (tid < npick) {
-            const int f = beam_key_flat(s_key[tid]), p = f / a.KK;
+            const int f = beam_key_flat(s.key[tid]), p = f / a.KK;
             const size_t e = (size_t)b * n + f;
             beam_emit(a, b, tid, p, a.cand_tok[e], a.beam_logps[(size_t)b * a.K + p] + a.cand_logp[e]);
         } else {

@@ -823,12 +823,13 @@ def rmsnorm_bwd(dy, x, rstd, w, residual=None):
     return dx, dw
 
 
-def linear_fwd(xb, wb, bias, act, p=0.0, seed=0, seed_dev=None, site=0):
-    """z = xb @ wb^T + bias (bf16) ; act: 0 none, 1 silu, 2 relu -> returns (z, act(z) with dropout)"""
+def linear_fwd(xb, wb, bias, act, p=0.0, seed=0, seed_dev=None, site=0, out=None):
+    """z = xb @ wb^T + bias (bf16) ; act: 0 none, 1 silu, 2 relu -> returns (z, act(z) with dropout); out: a contiguous bf16 tensor of
+    z's shape that receives z"""
     lib = _lib.load()
     T, K = xb.numel() // xb.shape[-1], xb.shape[-1]
     N = wb.shape[0]
-    z = torch.empty(*xb.shape[:-1], N, dtype=torch.bfloat16, device=xb.device)
+    z = torch.empty(*xb.shape[:-1], N, dtype=torch.bfloat16, device=xb.device) if out is None else out
     a = torch.empty_like(z) if act else None
     check(lib.grb_linear_forward(ptr(xb), ptr(wb), ptr(bias), T, N, K, act, ptr(z), ptr(a), float(p), int(seed), ptr(seed_dev), site,
                                  stream_ptr(xb.device)))
@@ -1167,3 +1168,56 @@ def infonce_fwd_bwd(scores, lo, hi, inv_tau: float):
     check(_lib.load().grb_infonce_forward_backward(ptr(scores), Q, ld, ptr(lo), ptr(hi), float(inv_tau), ptr(row), ptr(loss), ptr(ds),
                                                    stream_ptr(scores.device)))
     return loss, ds
+
+
+# ------------------------------------------------------------------------------------------------ COBRA generation
+def cobra_beam_attention(q, hist_qkv, hist_len, suf_qkv, anc, S: int, H: int) -> torch.Tensor:
+    """One decoder layer's self-attention of one new token per beam (grb_cobra_beam_attention).  q [B K, D] bf16 (a column view of the
+    step's QKV); hist_qkv [B, Li, 3D] bf16, the prefill's QKV, whose K | V are read in place, user b's keys its first hist_len[b]
+    (int32 [B]) rows; suf_qkv [steps, B K, 3D] bf16, the new tokens' QKV per step; anc [B K, S - 1] int32 (None for S = 1): the row of
+    step s < S - 1 a beam descends from (step S - 1 is its own row).  -> [B K, D] bf16."""
+    lib = _lib.load()
+    B, Li, D3 = hist_qkv.shape
+    D = D3 // 3
+    R = q.shape[0]
+    K = R // B
+    out = torch.empty(R, D, dtype=torch.bfloat16, device=q.device)
+    ws = _u8(lib.grb_cobra_beam_attention_workspace_bytes(B, K, H, D // H, Li), q.device)
+    check(lib.grb_cobra_beam_attention(ptr(q), q.stride(0), ptr(hist_qkv[..., D:]), ptr(hist_qkv[..., 2 * D:]), D3, Li, ptr(hist_len),
+                                       ptr(suf_qkv[..., D:]), ptr(suf_qkv[..., 2 * D:]), D3, suf_qkv.stride(0), ptr(anc), S, B, K, H, D // H,
+                                       ptr(out), D, ptr(ws), stream_ptr(q.device)))
+    return out
+
+
+def cobra_beam_topk(logits, scores_in, B: int, K: int, temperature: float, anc_in=None):
+    """One beam step (grb_cobra_beam_topk): logits [B K_in, V] fp32, scores_in [B, K_in] or None (zero) -> (tokens [B, K] int64,
+    scores [B, K], parents [B, K] int64, anc_out [B K, S_in + 1] int32: the parent's ancestry row and the parent's own row)."""
+    lib = _lib.load()
+    V = logits.shape[-1]
+    K_in = logits.shape[0] // B
+    S_in = 0 if anc_in is None else anc_in.shape[1]
+    dev = logits.device
+    tokens = torch.empty(B, K, dtype=torch.int64, device=dev)
+    scores = torch.empty(B, K, dtype=torch.float32, device=dev)
+    parents = torch.empty(B, K, dtype=torch.int32, device=dev)
+    anc_out = torch.empty(B * K, S_in + 1, dtype=torch.int32, device=dev)
+    ws = _u8(lib.grb_cobra_beam_topk_workspace_bytes(B, K_in, V, K), dev)
+    check(lib.grb_cobra_beam_topk(ptr(logits), ptr(scores_in), B, K_in, V, K, float(temperature), ptr(anc_in), S_in, ptr(tokens), ptr(scores),
+                                  ptr(parents), ptr(anc_out), ptr(ws), stream_ptr(dev)))
+    return tokens, scores, parents.long(), anc_out
+
+
+def cobra_dense_match(x_bf16, table_bf16):
+    """x [R, D], table [N, D] bf16 -> (best [R] fp32, item [R] int64): each row's highest x . table_n, the lowest n among equal
+    scores, without the [R, N] scores (grb_cobra_dense_match)."""
+    lib = _lib.load()
+    R, D = x_bf16.shape
+    N = table_bf16.shape[0]
+    best = torch.empty(R, dtype=torch.float32, device=x_bf16.device)
+    item = torch.empty(R, dtype=torch.int64, device=x_bf16.device)
+    nbytes = lib.grb_cobra_dense_match_workspace_bytes(R, D, N)
+    if nbytes == 0:
+        raise _lib.GrbError(lib.grb_last_error().decode())
+    ws = _u8(nbytes, x_bf16.device)
+    check(lib.grb_cobra_dense_match(ptr(x_bf16), ptr(table_bf16), R, D, N, ptr(best), ptr(item), ptr(ws), stream_ptr(x_bf16.device)))
+    return best, item

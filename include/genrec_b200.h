@@ -615,6 +615,37 @@ int grb_l2norm_backward(const float* dy, const float* y, const float* norms, int
 int grb_infonce_forward_backward(const float* scores, int Q, int ld, const int64_t* lo, const int64_t* hi, float inv_tau, float* row_loss,
                                  float* loss, void* dscores, void* stream);
 
+/* COBRA generation and BeamFusion (genrec/models/cobra.py:531-760) on a prefix cache.
+ *
+ * grb_cobra_beam_attention: one decoder layer's causal self-attention for one new token per beam, softmax(q k^T / sqrt(head_dim)) v
+ * without bias, fp32 softmax and sums, bf16 in and out.  Beam row r = b K + k: its query q[r, h head_dim ..] (leading dimension ldq),
+ * its keys the rows 0 .. hist_len[b]-1 of user b's history (key j of head h at hist_k[(b hist_rows + j) ld_hist + h head_dim], the same
+ * for hist_v: the prefill's QKV read in place) and then S suffix keys: for s < S-1 the row anc[r (S-1) + s] of suffix step s, and its
+ * own row r of step S-1 (step s, row i at suf_k / suf_v + s suf_step_stride + i ld_suf).  1 <= hist_len[b] <= hist_rows <= 8192,
+ * 1 <= K <= 1024, head_dim 32 or 64.  Deterministic, no atomics; a beam's output does not depend on the other users of the batch.
+ * workspace: grb_cobra_beam_attention_workspace_bytes() (0 for unsupported arguments), 16-byte aligned. */
+size_t grb_cobra_beam_attention_workspace_bytes(int B, int K, int H, int head_dim, int hist_rows);
+int grb_cobra_beam_attention(const void* q, int ldq, const void* hist_k, const void* hist_v, int ld_hist, int hist_rows,
+                             const int32_t* hist_len, const void* suf_k, const void* suf_v, int ld_suf, int64_t suf_step_stride,
+                             const int32_t* anc, int S, int B, int K, int H, int head_dim, void* out, int ldo, void* workspace,
+                             void* stream);
+/* grb_cobra_beam_topk: one beam step.  Per row of logits [B K_in, V] fp32: log_softmax(logits / temperature), plus the parent's score
+ * scores_in [B, K_in] (NULL: 0); then the K best of user b's K_in V totals, best first, equal totals by the lower flat index
+ * parent V + token (NaN above every number).  Writes tokens [B, K] int64, scores [B, K], parents [B, K] int32 (the
+ * parent's index in 0 .. K_in-1) and, when S_in > 0 or anc_out is given, anc_out [B K, S_in + 1]: the parent's row of anc_in
+ * [B K_in, S_in] followed by the parent's row b K_in + parent.  1 <= K, K_in <= 1024, K <= K_in V, K V and K_in V <= 262144.
+ * workspace: grb_cobra_beam_topk_workspace_bytes() bytes (0 for unsupported arguments). */
+size_t grb_cobra_beam_topk_workspace_bytes(int B, int K_in, int V, int K);
+int grb_cobra_beam_topk(const float* logits, const float* scores_in, int B, int K_in, int V, int K, float temperature, const int32_t* anc_in,
+                        int S_in, int64_t* tokens, float* scores, int32_t* parents, int32_t* anc_out, void* workspace, void* stream);
+/* grb_cobra_dense_match: best [R] fp32 and item [R] int64 = each row's highest x . table_n over the N catalog rows (x [R, D] and
+ * table [N, D] bf16, fp32 accumulation), the lowest n among equal scores, without forming the [R, N] scores.  No normalisation.
+ * D in {64,128,192,256,384,768}, R, N >= 1.  The result does not depend on how the catalog is split across CTAs.  workspace:
+ * grb_cobra_dense_match_workspace_bytes() (0 for unsupported arguments), 16-byte aligned; it grows with R, not with N. */
+size_t grb_cobra_dense_match_workspace_bytes(int R, int D, int N);
+int grb_cobra_dense_match(const void* x_bf16, const void* table_bf16, int R, int D, int N, float* best, int64_t* item, void* workspace,
+                          void* stream);
+
 #ifdef __cplusplus
 }
 #endif
