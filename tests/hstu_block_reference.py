@@ -1,7 +1,7 @@
 """fp64 references of the HSTU block's kernels - the gate (ln_gate_fwd_kernel / ln_gate_bwd_kernel), the cast of dy with the
 FFN output bias gradient (cast_colsum_f32_bf16_kernel), the HSTU attention (csrc/attn_hstu.cuh) - of the wiring of the block's
 linear layers (grb_hstu_layer_forward / _backward in csrc/api.cu) and of the fused Adam step (adam_tick_kernel + adam_step_kernel),
-that know where the kernels round.
+that know where the kernels round; and the fp64 rule of FlatAdam's lazy item-table step (lazy_adam_reference).
 
 Each reference takes the kernel's own inputs to its stage (the bf16 P, zp, O, xn, hact and the saved LayerNorm statistics of the
 forward's saved blob; dO, dxn, dx1, dyb, dz1 of the backward's workspace), so an error in one stage is not charged to the next and
@@ -360,3 +360,18 @@ def adam(p0, g0, m0, v0, t, lr, beta1, beta2, eps, weight_decay=0.0, grad_scale=
     r["p"] = P0 - upd
     r["a_p"] = e_upd + C * r["p"].abs()
     return r
+
+
+def lazy_adam_reference(p, g, m, v, rows, step, lr, betas, eps, weight_decay, grad_scale=1.0, bias_corrections=None):
+    """One lazy step in fp64: FlatAdam's per-element rule (torch.optim.Adam with L2 weight decay, bias corrections of the global
+    step count `step`, already ticked) on the rows `rows` of the [C, D] tensors; every other row is copied.  -> (p, m, v).
+    ``bias_corrections`` = (1 - beta1^step, 1 - beta2^step) as the optimizer's state holds them, when given."""
+    p, g, m, v = (t.double().clone() for t in (p, g, m, v))
+    r = torch.as_tensor(sorted(set(int(i) for i in rows)), dtype=torch.long)
+    b1, b2 = betas
+    bc1, bc2 = bias_corrections if bias_corrections is not None else (1 - b1 ** step, 1 - b2 ** step)
+    gr = g[r] * grad_scale + weight_decay * p[r]
+    m[r] = b1 * m[r] + (1 - b1) * gr
+    v[r] = b2 * v[r] + (1 - b2) * gr * gr
+    p[r] = p[r] - lr / bc1 * (m[r] / (v[r].sqrt() / bc2 ** 0.5 + eps))
+    return p, m, v

@@ -221,9 +221,32 @@ def test_t5_mutant_fails(defect):
     assert any(fails), defect
 
 
+def _np_drop_mask(T, D, p, seed, site):
+    """numpy restatement of genrec_b200/csrc/common.cuh Dropout (row keys + pair hash); True = dropped."""
+    import numpy as np
+    u = np.uint32
+    k0 = u((seed & 0xffffffff) ^ ((site * 0x9E3779B1) & 0xffffffff))
+    k1 = u(((seed >> 32) + 0x7F4A7C15) & 0xffffffff)
+    row = np.arange(T, dtype=np.uint32)[:, None]
+    cp = np.arange(D // 2, dtype=np.uint32)[None, :]
+    with np.errstate(over="ignore"):
+        ka = (row ^ k1) * u(0x9E3779B1)
+        ka = ka ^ (ka >> u(16))
+        b = ka * u(0x846CA68B)
+        kb = k0 ^ (b ^ (b >> u(15)))
+        x = (cp ^ kb) * u(0x7FEB352D)
+        x = x ^ (x >> u(15))
+        x = (x ^ ka) * u(0x846CA68B)
+        x = x ^ (x >> u(16))
+    t = u(int(p * 65536.0 + 0.5))
+    m = np.empty((T, D), dtype=bool)
+    m[:, 0::2] = (x & u(0xffff)) < t
+    m[:, 1::2] = (x >> u(16)) < t
+    return m
+
+
 def test_drop_mask_matches_the_paired_column_form():
-    """drop_mask on rows 0 .. T - 1 is the [T, D] mask the row-cast kernel's test restates (tests/test_linear_gpu.py)."""
-    from tests.test_linear_gpu import _np_drop_mask
+    """drop_mask on rows 0 .. T - 1 is _np_drop_mask's [T, D] mask, restated in the paired-column form of csrc/common.cuh."""
     for T, D, p, seed, site in [(77, 136, 0.2, 1234567, 6), (5, 9, 0.5, (3 << 40) + 5, 11)]:
         m = ar.drop_mask(range(T), D, p, seed, site)
         if D % 2 == 0:

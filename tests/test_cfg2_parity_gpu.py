@@ -4,83 +4,11 @@ interleaved forwards, optimizer state)."""
 import pytest
 import torch
 
+from tests.exact_check import autocast_yardstick
+from tests.hstu_cases import CFG2_H as H, CFG2_L as L, CFG2_NB as NB, CFG2_V as V, _cfg2_model, _oracle_run
 from tests.util import frob_relerr, make_batch, relerr
 
 pytestmark = pytest.mark.gpu
-
-V, L, D, H, NB = 12101, 200, 128, 4, 4
-
-
-def _cfg2_model(seed=0, dropout=0.0):
-    from genrec_b200.hstu import HSTU
-    torch.manual_seed(seed)
-    m = HSTU(V, L, D, H, NB, dropout=dropout)
-    g = torch.Generator().manual_seed(seed + 1)
-    with torch.no_grad():                      # leave the reference init but make every term matter
-        for n, p in m.named_parameters():
-            if "attention_bias" in n:
-                p.copy_(0.3 * torch.randn(p.shape, generator=g))
-            elif n.endswith("bias") and p.dim() == 1:
-                p.copy_(0.05 * torch.randn(p.shape, generator=g))
-            elif "norm" in n and n.endswith("weight"):
-                p.add_(0.1 * torch.randn(p.shape, generator=g))
-            elif "item_embedding" in n:
-                p.mul_(10.0)
-                p[0].zero_()
-            elif p.dim() == 2:
-                p.mul_(3.0)
-    return m
-
-
-def _oracle_run(ids, ts, tg, sd, autocast):
-    """Oracle forward + backward on the host cores; returns loss, parameter grads and the gradient entering the last block."""
-    from oracle import hstu as oh
-    p = {k: v.clone().requires_grad_(True) for k, v in sd.items()}
-    grabbed = {}
-    orig = oh.hstu_layer_forward
-
-    def spy(x, *a, **kw):
-        if a[3] == f"layers.{NB - 1}.":
-            x.retain_grad(); grabbed["x_last"] = x
-        return orig(x, *a, **kw)
-
-    oh.hstu_layer_forward = spy
-    try:
-        if autocast:
-            with torch.autocast("cpu", dtype=torch.bfloat16):
-                _, lo = oh.hstu_forward(ids, ts, tg, p, H, NB)
-            lo.float().backward()
-        else:
-            _, lo = oh.hstu_forward(ids, ts, tg, p, H, NB)
-            lo.backward()
-    finally:
-        oh.hstu_layer_forward = orig
-    grads = {k: (v.grad if v.grad is not None else torch.zeros_like(v)) for k, v in p.items()}
-    return float(lo), grads, grabbed["x_last"].grad.float()
-
-
-def autocast_yardstick(rows, small):
-    """rows: (name, ours Frobenius, reference-autocast Frobenius, ours max-norm, reference-autocast max-norm) relative errors against
-    the fp32 oracle; small: the names of tensors of < 4096 elements.  Prints the table (pytest -s) and asserts the yardstick."""
-    lines = ["| tensor | ours, Frobenius | reference autocast, Frobenius | ratio | ours, max-norm | reference autocast, max-norm | ratio |",
-             "|---|---|---|---|---|---|---|"]
-    lines += [f"| {n} | {a:.2e} | {b:.2e} | {a / max(b, 1e-12):.2f} | {c:.2e} | {d:.2e} | {c / max(d, 1e-12):.2f} |" for n, a, b, c, d in rows]
-    print("\n".join(lines))
-    # Yardstick.  Both columns are one realisation of bf16 rounding noise, so the ratio of the two scatters from tensor to tensor
-    # (and, for ours, from build to build: +-10 % on the matrices, a factor ~2 on a 399-entry bias table whose every entry is a
-    # cancelling sum of ~10^5 noisy terms).
-    #   weight matrices / embedding table / dX (>= 4096 elements): Frobenius error <= 1.1 x the reference algorithm's own
-    #       bf16-autocast error, and the geometric mean of the ratio over all of them <= 1.0;
-    #   vectors of < 4096 elements (bias tables, norm parameters): <= 3 x each, geometric mean <= 1.25;
-    #   the max-norm (one worst element out of up to 1.5 M) is reported and held within 3 x.
-    import math
-    big_r = [a / b for n, a, b, c, d in rows if n not in small and n != "loss" and b > 0]
-    small_r = [a / b for n, a, b, c, d in rows if n in small and b > 0]
-    gm = lambda v: math.exp(sum(math.log(max(x, 1e-6)) for x in v) / max(len(v), 1))
-    print(f"geometric mean of ours / reference-autocast: matrices {gm(big_r):.3f} ({len(big_r)}), small vectors {gm(small_r):.3f} ({len(small_r)})")
-    bad = [(n, a, b, c, d) for n, a, b, c, d in rows if a > (3.0 if n in small else 1.1) * b + 5e-4 or c > 3.0 * d + 1e-3]
-    assert not bad, bad
-    assert gm(big_r) <= 1.0 and gm(small_r) <= 1.25, (gm(big_r), gm(small_r))
 
 
 def test_cfg2_full_model_vs_oracle():

@@ -23,89 +23,26 @@ from tests import cobra_reference as cr
 from tests import cobra_stage_reference as sr
 from tests import dense_reference as dr
 from tests import hstu_block_reference as hr
-from tests.test_tiger_exact_gpu import FTZ, _packed_core_ref
+from tests.exact_check import (FTZ, Ledger, Spy, _TorchDropout, _cid, _dy, _packed_core_ref, _seeded, _sms,
+                                autocast_yardstick)
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
 PS = [0.0, 0.1, 0.3]
 EPS = 1e-5                                            # nn.LayerNorm
 SEED = 0x2F6B_1D3C_5A79_4E81                          # a 62-bit dropout seed, as Cobra._seed draws
-_WORST = {}
+LEDGER = Ledger("worst error / allowance per quantity of the COBRA stages (dense tolerance 1, attention core: attention_reference.TOL):",
+                width=18, floor=FTZ)
+_error_table = LEDGER.fixture()
+_check = LEDGER.check
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _error_table():
-    yield
-    if _WORST:
-        print("\nworst error / allowance per quantity of the COBRA stages (dense tolerance 1, attention core: attention_reference.TOL):")
-        for name, (w, case) in sorted(_WORST.items()):
-            print(f"  {name:18s} {w:8.4f}   {case}")
-
-
-def _record(case, name, w, tol=dr.TOL):
-    if name not in _WORST or w > _WORST[name][0]:
-        _WORST[name] = (w, case)
-    return None if w <= tol else f"{name} {w:.3g}"
-
-
-def _check(case, items):
-    """items: (name, got, ref, allowance)"""
-    bad = [_record(case, n, dr.worst(g, r, a + FTZ)) for n, g, r, a in items]
-    bad = [b for b in bad if b]
-    assert not bad, (case, bad)
-
-
-def _check_core(case, err):
-    for n, (w, f) in err.items():
-        tw, tf = ar.tolerance("t5", n)
-        _record(case, "core " + n, w / tw, 1.0)
-        _record(case, "core " + n + " frob", f / tf, 1.0)
-    bad = ar.violations(err, "t5")
-    assert not bad, (case, bad)
-
-
-class _Spy:
-    """records the outputs of the functional calls made while it is active, by name, in call order"""
-
-    def __init__(self, monkeypatch):
-        from genrec_b200 import cobra
-        from genrec_b200 import functional as Fn
-        self.calls = []
-        for mod, names in ((Fn, ("cast_rows_bf16", "linear_bwd", "linear_dact_bwd", "infonce_fwd_bwd")),
-                           (cobra, ("attention_core_bwd", "attention_core_bwd_jagged"))):
-            for n in names:
-                monkeypatch.setattr(mod, n, self._wrap(n, getattr(mod, n)))
-
-    def _wrap(self, name, fn):
-        def spy(*a, **k):
-            out = fn(*a, **k)
-            self.calls.append((name, out))
-            return out
-        return spy
-
-    def take(self, *names):
-        assert [n for n, _ in self.calls] == list(names), [n for n, _ in self.calls]
-        got = [out for _, out in self.calls]
-        self.calls.clear()
-        return got
-
-
-def _dy(shape, seed):
-    """small integers / 64: every masked bf16 cast of it is exact"""
-    g = torch.Generator().manual_seed(seed)
-    return (torch.randint(-64, 65, shape, generator=g).float() / 64).to(DEV)
-
-
-def _seeded(shape, seed, scale=1.0, shift=0.0):
-    return (scale * torch.randn(shape, generator=torch.Generator().manual_seed(seed)) + shift).to(DEV)
-
-
-def _sms():
-    return torch.cuda.get_device_properties(DEV).multi_processor_count
-
-
-def _cid(c):
-    return "-".join(str(v) for v in c)
+def _spy(monkeypatch):
+    """the functional calls made while it is active"""
+    from genrec_b200 import cobra
+    from genrec_b200 import functional as Fn
+    return Spy(monkeypatch, {Fn: ("cast_rows_bf16", "linear_bwd", "linear_dact_bwd", "infonce_fwd_bwd"),
+                             cobra: ("attention_core_bwd", "attention_core_bwd_jagged")})
 
 
 def _offsets(lens):
@@ -241,7 +178,7 @@ def test_infonce_stage(case, monkeypatch):
     lo = hi - cnt[user]
     pred = torch.nn.functional.normalize(_seeded((Q, d), Q + 11), dim=-1).requires_grad_(True)
     gt = torch.nn.functional.normalize(_seeded((Q, d), Q + 12), dim=-1)
-    spy = _Spy(monkeypatch)
+    spy = _spy(monkeypatch)
     loss = _InfoNceFn.apply(pred, gt, lo.contiguous(), hi.contiguous(), 1 / 0.2)
     pb, gb, (S, _, _), (lsum, dS) = spy.take("cast_rows_bf16", "cast_rows_bf16", "linear_bwd", "infonce_fwd_bwd")
     dS_saved, gpad = loss.grad_fn.saved_tensors
@@ -270,7 +207,7 @@ def test_linear_f32_stage(case, monkeypatch):
     x = _seeded((R, K), K + R, 2.0).requires_grad_(True)
     w = _seeded((N, K), N, K ** -0.5).requires_grad_(True)
     b = _seeded((N,), N + 1, 0.5).requires_grad_(True)
-    spy = _Spy(monkeypatch)
+    spy = _spy(monkeypatch)
     y = _LinearF32Fn.apply(x, w, b)
     assert y.dtype == torch.float32 and y.shape == (R, N)
     dy = _dy((R, N), R + 2)
@@ -313,7 +250,7 @@ def test_ffn_stage(case, monkeypatch):
     xb, z, h, w1b, w2b = y.grad_fn.saved_tensors
     assert y.grad_fn.cfg == (p, p, SEED, site)
     dy = _dy((R, D), R + 1)
-    spy = _Spy(monkeypatch)
+    spy = _spy(monkeypatch)
     y.backward(dy)
     dyb, (_, dw2, db2), dz, (dx, dw1, db1) = spy.take("cast_rows_bf16", "linear_bwd", "linear_dact_bwd", "linear_bwd")
     xc = x.detach()
@@ -386,7 +323,7 @@ def test_mha_stage(case, monkeypatch):
     Hc, pc, seed, sc, scale, *_ = out.grad_fn.cfg
     assert (Hc, pc, seed, sc) == (H, p, SEED, site)
     dy = _dy(tuple(out.shape), D + H)
-    spy = _Spy(monkeypatch)
+    spy = _spy(monkeypatch)
     out.backward(dy)
     core = "attention_core_bwd_jagged" if packed else "attention_core_bwd"
     dyb, (dA, dwo, _), dAb, (dQ, dK, dV, _), dqkvb, (dx, dwi, _) = spy.take(
@@ -406,7 +343,8 @@ def test_mha_stage(case, monkeypatch):
         got = {"out": A, "dq": dQ, "dk": dK, "dv": dV}
         assert not ar.t5_exact(got, ref, key_pad)
     names = ("out", "dq", "dk", "dv")
-    _check_core(case_id, ar.errors({k: flat(got[k]) for k in names}, {k: flat(ref[k]) for n in names for k in (n, "a_" + n)}, names))
+    LEDGER.check_core(case_id, ar.errors({k: flat(got[k]) for k in names}, {k: flat(ref[k]) for n in names for k in (n, "a_" + n)}, names),
+                      "t5")
     dqkv = torch.cat([dQ.float(), dK, dV], dim=-1)
     assert torch.equal(dqkvb, dqkv.bfloat16())
     bo = dr.linear_backward(flat(dyb), wob, flat(A))
@@ -467,11 +405,9 @@ STEPS = [("small", 0.1), ("small", 0.3), ("small B=256", 0.1), ("small B=256", 0
 def test_training_step_vs_fp64(case, monkeypatch):
     """Cobra.forward + backward with every dropout at p against the fp64 restatement on the same masks: torch's F.dropout masks
     recorded by a shim, the kernels' restated from the step's two seeds (cobra_reference.kernel_step_masks).  The yardstick is the
-    restatement under bf16 autocast (test_cfg2_parity_gpu.autocast_yardstick); the integer metrics match to within the counted
+    restatement under bf16 autocast (exact_check.autocast_yardstick); the integer metrics match to within the counted
     positions whose top-1 lead is below cobra_reference.MARGIN."""
     from genrec_b200 import cobra
-    from tests.test_cfg2_parity_gpu import autocast_yardstick
-    from tests.test_tiger_exact_gpu import _TorchDropout
     from tests.util import frob_relerr, relerr
     shape, p = case
     trainer = shape.startswith("trainer")

@@ -5,7 +5,7 @@ import pytest
 import torch
 
 import genrec_b200.functional as Fn
-from tests.test_head_topk_gpu import EPS, NEG, _assert_same, _head, _select
+from tests.head_cases import EPS, NEG, _assert_same, _head, _select
 
 pytestmark = pytest.mark.gpu
 
@@ -166,8 +166,8 @@ def test_memory_does_not_grow_with_the_catalog():
 
 # ------------------------------------------------------------------------------------------------ models
 def _hstu(D=64, H=2, use_time=True, seed=0):
-    from tests.test_hstu_extend_gpu import _model
-    return _model(D, H, use_time=use_time, seed=seed)
+    from tests.hstu_cases import _serve_model
+    return _serve_model(D, H, use_time=use_time, seed=seed)
 
 
 @pytest.mark.parametrize("timestamps", [True, False])
@@ -200,7 +200,7 @@ def test_sasrec_retrieve_matches_forward():
 
 
 def test_extend_with_num_candidates_matches_twin_state():
-    from tests.test_hstu_extend_gpu import _absolute_ts, _chunks
+    from tests.hstu_cases import _absolute_ts, _chunks
     m = _hstu(128, 4)
     B = 3
     chunks = _absolute_ts(_chunks(B, [40, 1, 1, 3, 1], seed=4))
@@ -238,7 +238,7 @@ def test_extend_users_with_num_candidates_matches_twin_pool():
 
 
 def test_extend_users_num_candidates_cuda_graph_replay():
-    from tests.test_hstu_pool_gpu import _fill
+    from tests.hstu_cases import _fill
     m = _hstu(128, 4)
     V = m.num_items
     eager = m.new_pool(max_users=6, num_pages=16, page_size=64, max_items=192)

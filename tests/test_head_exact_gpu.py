@@ -9,11 +9,11 @@ import math
 import pytest
 import torch
 
-from tests.head_reference import LOSS_FLOOR, TOL, format_table, head_errors, make_case, reference, violations
+from tests.head_cases import EPS, _call, _dev, _reference, _to_dev
+from tests.head_reference import LOSS_FLOOR, TOL, format_table, head_errors, make_case, violations
 
 pytestmark = pytest.mark.gpu
 
-EPS = 1e-5
 TOKENS = (1, 63, 64, 65, 127, 128, 129, 385)
 # logits of grb_head_logits: |error| <= TOL_LOGITS * (|xf| |E|^T), fp32 accumulation of exact bf16 products.  Measured 1.9e-7 on an
 # H100 80GB HBM3 (700 W power limit).
@@ -34,47 +34,6 @@ def _error_table():
     if _LOGITS:
         print(f"grb_head_logits, {len(_LOGITS)} cases: max |error| / (|xf| |E|^T) = {max(e for e, _ in _LOGITS):.2e}, "
               f"loss of these logits vs the fused loss = {max(e for _, e in _LOGITS):.2e}")
-
-
-def _dev():
-    return torch.device("cuda:0")
-
-
-def _to_dev(case):
-    dev = _dev()
-    from genrec_b200 import functional as Fn
-    c = {k: v.to(dev).contiguous() for k, v in case.items()}
-    c["tb"] = Fn.cast_bf16(c["table"])
-    return c
-
-
-def _call(c, *, dx=None, dtable=None, dg=None, db=None, ws=None, loss_only=False, tg=None):
-    """grb_head_loss_forward_backward through the C ABI; zeroed gradient buffers and workspace unless given."""
-    from genrec_b200 import _lib
-    from genrec_b200._lib import check, ptr, stream_ptr
-    lib = _lib.load()
-    x, tb = c["x"], c["tb"]
-    T, D = x.shape
-    C = tb.shape[0]
-    dev = x.device
-    if ws is None:
-        ws = torch.zeros(lib.grb_head_workspace_bytes(T, D, C), dtype=torch.uint8, device=dev)
-    if not loss_only:
-        dx = torch.empty_like(x) if dx is None else dx
-        dtable = torch.zeros(C, D, device=dev) if dtable is None else dtable
-        dg = torch.zeros(D, device=dev) if dg is None else dg
-        db = torch.zeros(D, device=dev) if db is None else db
-    loss = torch.empty((), dtype=torch.float32, device=dev)
-    check(lib.grb_head_loss_forward_backward(ptr(x), ptr(c["ln_g"]), ptr(c["ln_b"]), EPS, ptr(tb), ptr(c["tg"] if tg is None else tg), T, D, C,
-                                             ptr(loss), ptr(dx), ptr(dtable), ptr(dg), ptr(db), ptr(ws), stream_ptr(dev)))
-    torch.cuda.synchronize()
-    return {"loss": loss.item(), "dx": dx, "dg": dg, "db": db, "dE": dtable}
-
-
-def _reference(c, chunk=2048):
-    from genrec_b200 import functional as Fn
-    xf, _, st = Fn.layernorm_fwd(c["x"], c["ln_g"], c["ln_b"], EPS)     # ln_fwd_kernel, as the head launches it: the same bits
-    return reference(c["x"], st, xf, c["ln_g"], c["tb"], c["tg"], chunk=chunk)
 
 
 def _check(name, T, D, C, kind="plain", seed=None):

@@ -143,8 +143,8 @@ def test_agrees_with_recommend_under_exclusions(R, D, C, E):
 
 # ------------------------------------------------------------------------------------------------ 4. models
 def _hstu(D=64, H=2, use_time=True, seed=0):
-    from tests.test_hstu_extend_gpu import _model
-    return _model(D, H, use_time=use_time, seed=seed)
+    from tests.hstu_cases import _serve_model
+    return _serve_model(D, H, use_time=use_time, seed=seed)
 
 
 @pytest.mark.parametrize("timestamps", [True, False])

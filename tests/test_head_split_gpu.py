@@ -6,7 +6,7 @@ import pytest
 import torch
 
 from tests.head_reference import make_case, violations, head_errors
-from tests.test_head_exact_gpu import _call, _dev, _reference, _to_dev
+from tests.head_cases import _call, _dev, _reference, _to_dev
 
 pytestmark = pytest.mark.gpu
 

@@ -5,45 +5,14 @@ import pytest
 import torch
 
 import genrec_b200.functional as Fn
+from tests.head_cases import EPS, NEG, _assert_same, _head, _select
 
 pytestmark = pytest.mark.gpu
-
-EPS = 1e-5
-NEG = float("-inf")
 
 
 def _reference(x, ln_g, ln_b, tb, eps, k, exclude=None):
     logits = Fn.head_logits(x[:, None, :], ln_g, ln_b, tb, tb, eps)[:, 0, :]
     return _select(logits, k, exclude)
-
-
-def _select(logits, k, exclude=None):
-    logits = logits.clone()
-    C = logits.shape[1]
-    logits[:, 0] = NEG
-    if exclude is not None and exclude.shape[1]:
-        logits.scatter_(1, torch.where((exclude >= 1) & (exclude < C), exclude, 0), NEG)
-    if C < k:                                   # fewer items than slots: the rest is (-inf, 0)
-        logits = torch.cat([logits, logits.new_full((logits.shape[0], k - C), NEG)], 1)
-    s, i = torch.sort(logits, dim=1, descending=True, stable=True)
-    s, i = s[:, :k], i[:, :k]
-    return s, torch.where(s == NEG, torch.zeros_like(i), i)
-
-
-def _assert_same(got, ref):
-    s, i = got
-    rs, ri = ref
-    assert torch.equal(s, rs), (s - rs).abs().max()
-    assert torch.equal(i, ri), (i != ri).nonzero()[:8]
-
-
-def _head(R, D, C, seed):
-    g = torch.Generator().manual_seed(seed)
-    x = torch.randn(R, D, generator=g).cuda()
-    ln_g = (1 + 0.1 * torch.randn(D, generator=g)).cuda()
-    ln_b = (0.1 * torch.randn(D, generator=g)).cuda()
-    tb = (0.05 * torch.randn(C, D, generator=g)).to(torch.bfloat16).cuda()
-    return x, ln_g, ln_b, tb
 
 
 def _exclusions(x, ln_g, ln_b, tb, E, seed):
@@ -142,8 +111,8 @@ def test_memory_does_not_grow_with_the_catalog():
 
 # ------------------------------------------------------------------------------------------------ models
 def _hstu(D=64, H=2, use_time=True, seed=0):
-    from tests.test_hstu_extend_gpu import _model
-    return _model(D, H, use_time=use_time, seed=seed)
+    from tests.hstu_cases import _serve_model
+    return _serve_model(D, H, use_time=use_time, seed=seed)
 
 
 @pytest.mark.parametrize("timestamps", [True, False])
@@ -188,7 +157,7 @@ def test_sasrec_recommend_matches_forward():
 
 
 def test_extend_with_top_k_matches_twin_state():
-    from tests.test_hstu_extend_gpu import _absolute_ts, _chunks
+    from tests.hstu_cases import _absolute_ts, _chunks
     m = _hstu(128, 4)
     B = 3
     chunks = _absolute_ts(_chunks(B, [40, 1, 1, 3, 1], seed=4))
@@ -238,7 +207,7 @@ def test_extend_users_with_top_k_matches_twin_pool():
 
 
 def test_extend_users_top_k_cuda_graph_replay():
-    from tests.test_hstu_pool_gpu import _fill
+    from tests.hstu_cases import _fill
     m = _hstu(128, 4)
     V = m.num_items
     eager = m.new_pool(max_users=6, num_pages=16, page_size=64, max_items=192)

@@ -5,9 +5,12 @@ row 0, a left-padded row 1 and a fully padded row 2."""
 import pytest
 import torch
 
-from tests.test_hstu_block_exact_gpu import DEV, _attn_case
+from tests.exact_check import DEV, Ledger
+from tests.hstu_cases import _attn_case, core_case, pos_fixed
 
 pytestmark = pytest.mark.gpu
+LEDGER = Ledger("worst error / allowance per quantity of the attention backward (tolerance 1):")
+_error_table = LEDGER.fixture()
 
 # (pos, time) of the four kernel instantiations <HAS_TIME, POS_UNI>: "ref" buckets are uniform (bucket 0 on every causal cell)
 BIAS = [(("fix", 32, 100), 64), (("ref", 32, 128), 64), (("fix", 64, 80), "notable"), (("ref", 32, 128), "nots")]
@@ -17,13 +20,12 @@ CASES = [(L, D, H, pos, time) for L in (63, 64, 65, 192, 193, 255, 256, 257) for
 @pytest.mark.parametrize("case", CASES, ids=lambda c: f"L{c[0]}-dh{c[1] // c[2]}-{c[3][0]}{c[3][1]}-t{c[4]}")
 def test_attention_backward_vs_fp64(case):
     L, D, H, pos, time = case
-    _attn_case(L, D, H, pos, time, seed=L * 5 + D + H)
+    _attn_case(L, D, H, pos, time, seed=L * 5 + D + H, ledger=LEDGER)
 
 
 def _operands(L, D, H, seed):
     import genrec_b200.functional as Fn
     from genrec_b200.hstu import _thresholds_on
-    from tests.test_hstu_bias_configs_gpu import core_case, pos_fixed
     c = core_case(L, D, H, ("fix", 32, 100), 64, seed)
     pb = pos_fixed(torch.arange(L), 32, 100)
     meta = Fn.SeqMeta(c["pad"].to(torch.uint8).to(DEV), c["ts"].to(DEV), pb.to(torch.uint8).to(DEV), _thresholds_on(DEV), 64, 32,

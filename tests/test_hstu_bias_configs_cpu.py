@@ -4,7 +4,7 @@ import pytest
 import torch
 
 from oracle import hstu as oh
-from tests import test_hstu_bias_configs_gpu as G
+from tests import hstu_cases as G
 
 MARGIN = 3.0
 POS_TABLE = "position_bias.relative_attention_bias.weight"

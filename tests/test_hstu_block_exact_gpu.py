@@ -11,22 +11,15 @@ import ctypes as C
 import pytest
 import torch
 
-from tests import dense_reference as dr
 from tests import hstu_block_reference as hr
-from tests.test_hstu_bias_configs_gpu import CORE_CASES, batch, core_case, pos_fixed, table_excess
+from tests.exact_check import Ledger, _sms, row_pass
+from tests.hstu_cases import CORE_CASES, _attn_case, _params, batch, pos_fixed, table_excess
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
-_WORST = {}
-
-
-def _sms():
-    return torch.cuda.get_device_properties(DEV).multi_processor_count
-
-
-def row_pass():
-    """rows one pass of the gate kernels' grid covers: row_grid caps at 8 CTAs per SM, of 8 rows each"""
-    return 8 * _sms() * 8
+LEDGER = Ledger("worst error / allowance per quantity (tolerance 1):")
+_error_table = LEDGER.fixture()
+_check = LEDGER.check
 
 
 def adam_pass():
@@ -34,49 +27,14 @@ def adam_pass():
     return 16 * _sms() * 256
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _error_table():
-    yield
-    if _WORST:
-        print("\nworst error / allowance per quantity (tolerance 1):")
-        for name, (w, case) in sorted(_WORST.items()):
-            print(f"  {name:12s} {w:8.4f}   {case}")
-
-
-def _check(case, items):
-    """items: (name, got, ref, allowance).  Records each worst ratio and fails on any above dense_reference.TOL."""
-    bad = []
-    for name, got, ref, allow in items:
-        w = dr.worst(got, ref, allow)
-        if name not in _WORST or w > _WORST[name][0]:
-            _WORST[name] = (w, case)
-        if not w <= dr.TOL:
-            bad.append(f"{name} {w:.3g}")
-    assert not bad, (case, bad)
-
-
 # ------------------------------------------------------------------------------------------------ one block through the C ABI
 def _batch(B, L, seed):
-    """ids-free pad / ts of B rows: row b follows row b % 4 of test_hstu_bias_configs_gpu.batch (a pad in the middle, a left-padded
+    """ids-free pad / ts of B rows: row b follows row b % 4 of hstu_cases.batch (a pad in the middle, a left-padded
     row, a fully padded row, timestamps spanning more than 2^62)."""
     rows = [batch(L, seed + k) for k in range((B + 3) // 4)]
     ts = torch.cat([r[1] for r in rows])[:B]
     pad = torch.cat([r[2] for r in rows])[:B]
     return ts, pad
-
-
-def _params(D, H, npos, ntime, seed):
-    g = torch.Generator().manual_seed(seed)
-    r = lambda *s: torch.randn(*s, generator=g)                            # noqa: E731
-    wp = 0.08 * r(4 * D, D)
-    wp -= wp.mean(1, keepdim=True)          # rows summing to ~0: the +-1000 row offsets of x stay out of the projection
-    p = dict(proj_w=wp, proj_b=0.1 * r(4 * D), pos_table=0.3 * r(npos, H), time_table=0.5 * r(max(ntime, 1), H),
-             ln1_g=1 + 0.1 * r(D), ln1_b=0.1 * r(D), ffn1_w=0.08 * r(4 * D, D), ffn1_b=0.1 * r(4 * D), ffn2_w=0.08 * r(D, 4 * D),
-             ffn2_b=0.1 * r(D), ln2_g=1 + 0.1 * r(D), ln2_b=0.1 * r(D))
-    p = {k: v.to(DEV) for k, v in p.items()}
-    for k in ("proj_w", "ffn1_w", "ffn2_w"):
-        p[k] = p[k].bfloat16()
-    return p
 
 
 def run_block(B, L, D, H, p, layer, seed_dev, pos, time, seed=1, defer=False):
@@ -167,8 +125,7 @@ def check_block(r, case):
         assert not bool(gr["time_table"].any()), "time table gradient without a time term"
     del at, w, masked, pbc, tbc, valid
     for n, v in ex.items():
-        if n not in _WORST or v > _WORST[n][0]:
-            _WORST[n] = (v, case)
+        LEDGER.record(case, n, v)
     assert max(ex.values()) <= 1.0, (case, ex)
     _check(case, items)
 
@@ -237,40 +194,7 @@ def test_edges_are_reached():
 
 
 # ------------------------------------------------------------------------------------------------ attention, element by element
-def _attn_case(L, D, H, pos, time, seed):
-    import genrec_b200.functional as Fn
-    from genrec_b200.hstu import _thresholds_on
-    c = core_case(L, D, H, pos, time, seed)
-    kind, npos, md = pos
-    pb = pos_fixed(torch.arange(L), npos, md) if kind == "fix" else pos_fixed(-torch.arange(L), npos, md)
-    uniform = bool((pb == pb[0]).all())
-    ntime = time if isinstance(time, int) else 64
-    meta = Fn.SeqMeta(c["pad"].to(torch.uint8).to(DEV), c["ts"].to(DEV) if c["ts"] is not None else None, pb.to(torch.uint8).to(DEV),
-                      _thresholds_on(DEV), ntime, npos, (uniform, int(pb[0])))
-    P, zp, dO = c["P"].to(DEV), c["zp"].to(DEV), c["dO"].to(DEV)
-    wpos = c["wpos"].to(DEV)
-    wtime = c["wtime"].to(DEV) if c["wtime"] is not None else None
-    O = Fn.hstu_attention_fwd(P, meta, H, wpos, wtime, ntime)
-    dzp, dpos, dtime = Fn.hstu_attention_bwd(P, zp, dO, meta, H, wpos, wtime, ntime)
-    timed = wtime is not None and c["ts"] is not None
-    w, masked, pbc, tbc = hr.cell_bias(meta.bias_index, wpos[int(pb[0]):int(pb[0]) + 1] if uniform else wpos, wtime if timed else None,
-                                       1 if uniform else npos, H)
-    valid = hr.causal_valid(c["pad"].to(DEV))
-    assert torch.equal(masked, ~valid)
-    at = hr.attention(P, w, valid, H, zp, dO)
-    case = f"attn L{L}-D{D}-dh{D // H}-{kind}{npos}-t{time}"
-    assert not bool(dzp[..., :D].any()), "the attention backward wrote the U columns"
-    _check(case, [("attn O", O, at["O"], at["a_O"]), ("attn dV", dzp[..., D:2 * D], at["dV"], at["a_dV"]),
-                  ("attn dQ", dzp[..., 2 * D:3 * D], at["dQ"], at["a_dQ"]), ("attn dK", dzp[..., 3 * D:], at["dK"], at["a_dK"])])
-    rows = torch.full_like(pbc, int(pb[0])) if uniform else pbc
-    ref, mass, count = hr.table_sums(at["dS"], valid, rows[:, None], npos)
-    assert table_excess(dpos, ref, mass.cpu(), count.cpu()) <= 1.0
-    if timed:
-        ref, mass, count = hr.table_sums(at["dS"], valid, tbc[:, None], wtime.shape[0])
-        assert table_excess(dtime, ref, mass.cpu(), count.cpu()) <= 1.0
-
-
-# CORE_CASES of test_hstu_bias_configs_gpu, the shapes of test_attn_tc_gpu (the reference's uniform buckets), and L = 63, 128, 129
+# hstu_cases.CORE_CASES, the shapes of test_attn_tc_gpu (the reference's uniform buckets), and L = 63, 128, 129
 ATTN_CASES = list(CORE_CASES) + [(L, D, H, ("ref", 32, 128), t) for L, D, H, t in
                                  [(1, 64, 2, 64), (7, 128, 4, 64), (64, 128, 4, 64), (128, 128, 4, "nots"), (130, 256, 8, 64),
                                   (200, 128, 4, 64), (257, 64, 2, 64), (300, 128, 2, 64), (520, 128, 4, 64)]] + \
@@ -280,7 +204,7 @@ ATTN_CASES = list(CORE_CASES) + [(L, D, H, ("ref", 32, 128), t) for L, D, H, t i
 @pytest.mark.parametrize("case", ATTN_CASES, ids=lambda c: f"L{c[0]}-dh{c[1] // c[2]}-{c[3][0]}{c[3][1]}-t{c[4]}")
 def test_attention_elementwise_vs_fp64(case):
     L, D, H, pos, time = case
-    _attn_case(L, D, H, pos, time, seed=L * 7 + D + H)
+    _attn_case(L, D, H, pos, time, seed=L * 7 + D + H, ledger=LEDGER)
 
 
 # ------------------------------------------------------------------------------------------------ Adam

@@ -15,23 +15,16 @@ import torch
 
 from tests import extend_reference as er
 from tests import hstu_block_reference as hr
-from tests.test_hstu_bias_configs_gpu import batch, pos_fixed
-from tests.test_hstu_block_exact_gpu import _WORST, _check, _params, _sms
+from tests.exact_check import Ledger, _sms
+from tests.hstu_cases import _params, batch, pos_fixed
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
 NPOS, MAXD, NTIME = 32, 100, 64
 INT_MAX = (1 << 31) - 1
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _error_table():
-    yield
-    mine = {k: v for k, v in _WORST.items() if k.startswith("extend")}
-    if mine:
-        print("\nworst error / allowance per quantity (tolerance 1):")
-        for name, (w, case) in sorted(mine.items()):
-            print(f"  {name:12s} {w:8.4f}   {case}")
+LEDGER = Ledger("worst error / allowance per quantity (tolerance 1):")
+_error_table = LEDGER.fixture()
+_check = LEDGER.check
 
 
 # ------------------------------------------------------------------------------------------------ caches the test owns
@@ -494,9 +487,8 @@ def test_page_size_invariance():
 def test_model_extend_users_equals_extend_at_132_users():
     """HSTU.extend_users on a pool of 128-item pages (free stack scrambled by other users) against HSTU.extend on the dense state,
     at B = 132: logits bit for bit"""
-    from tests.test_hstu_extend_gpu import _absolute_ts, _chunks, _model
-    from tests.test_hstu_pool_gpu import _fill
-    m = _model(128, 4, use_time=True, seed=2)
+    from tests.hstu_cases import _absolute_ts, _chunks, _fill, _serve_model
+    m = _serve_model(128, 4, use_time=True, seed=2)
     B, cap = 132, 1000
     st = m.new_state(B, cap)
     pool = m.new_pool(max_users=150, num_pages=500, page_size=128, max_items=cap)

@@ -3,49 +3,10 @@ import pytest
 import torch
 
 from tests.sign_fixed_buckets import use_sign_fixed_oracle
-from tests.util import budget, make_batch, relerr
+from tests.hstu_cases import SERVE_V as V, _absolute_ts, _check_extend as _check, _chunks, _concat, _serve_model as _model, _sign_fixed
+from tests.util import make_batch
 
 pytestmark = pytest.mark.gpu
-
-V, NB = 500, 2
-
-
-def _model(D, H, use_time=True, seed=0, dropout=0.0):
-    from genrec_b200.hstu import HSTU
-    torch.manual_seed(seed)
-    m = HSTU(V, 64, D, H, NB, dropout=dropout, use_temporal_bias=use_time)
-    g = torch.Generator().manual_seed(seed + 100)
-    with torch.no_grad():
-        for n, p in m.named_parameters():
-            if "attention_bias" in n:
-                p.copy_(torch.randn(p.shape, generator=g) * 0.3)
-    return m.to("cuda").eval()
-
-
-def _oracle_last(m, ids, ts):
-    from oracle import hstu as oh
-    sd = {k: v.detach().double().cpu() for k, v in m.state_dict().items()}
-    logits, _ = oh.hstu_forward(ids.cpu(), ts.cpu() if ts is not None else None, None, sd, m.layers[0].num_heads, len(m.layers),
-                                use_temporal_bias=m.use_temporal_bias)
-    return logits[:, -1]
-
-
-def _check(ext, m, ids, ts, rows):
-    """extend's logits of `rows` are as close to the fp64 oracle as last_logits on the same left-padded batch."""
-    ref = _oracle_last(m, ids, ts)
-    full = m.last_logits(ids, ts)
-    e, b = relerr(ext[rows], ref[rows]), budget(full[rows], ref[rows])
-    assert e <= b, (e, b)
-    return full
-
-
-def _sign_fixed(m):
-    """Set the sign-fixed (non-uniform) position-bucket table through bucket_of_delta: bucket(i - j) instead of bucket(j - i)."""
-    for layer in m.layers:
-        rpb = layer.position_bias
-        rpb._relative_position_bucket = (lambda f: (lambda rel: f(-rel)))(rpb._relative_position_bucket)
-        rpb._table_cache.clear()
-        rpb._uniform_cache.clear()
 
 
 @pytest.mark.parametrize("D,H", [(64, 2), (128, 4), (128, 2), (256, 8)])
@@ -61,54 +22,6 @@ def test_prefill_matches_full_forward(D, H, time_mode):
     assert ext.shape == (4, V + 1) and torch.isfinite(ext).all()
     _check(ext, m, ids, ts, [0, 1, 3])                  # row 2 is all padding
     assert st.lengths.tolist() == [50, 50 - 50 // 3, 0, 50]
-
-
-def _chunks(B, widths, seed, max_pad=3):
-    """Per chunk of width w, user b's row holds min(b * max_pad, w - 1) left pads and then its next items."""
-    g = torch.Generator().manual_seed(seed)
-    chunks = []
-    for w in widths:
-        ids = torch.randint(1, V + 1, (B, w), generator=g)
-        ts = torch.randint(1, 3 * 86400, (B, w), generator=g)
-        ts[:, ::3] = torch.randint(0, 30, (B, (w + 2) // 3), generator=g)
-        for b in range(B):
-            p = min(b * max_pad, w - 1)
-            ids[b, :p] = 0
-        chunks.append((ids, ts))
-    return chunks
-
-
-def _concat(chunks, upto):
-    """left-padded [B, Lmax] batch of each user's items in the first `upto` chunks (timestamps made increasing per user)."""
-    B = chunks[0][0].shape[0]
-    rows_i, rows_t = [], []
-    for b in range(B):
-        items = torch.cat([c[0][b] for c in chunks[:upto]])
-        gaps = torch.cat([c[1][b] for c in chunks[:upto]])
-        keep = items != 0
-        rows_i.append(items[keep])
-        rows_t.append(gaps[keep])
-    Lm = max(len(r) for r in rows_i)
-    ids = torch.zeros(B, Lm, dtype=torch.int64)
-    ts = torch.zeros(B, Lm, dtype=torch.int64)
-    for b in range(B):
-        n = len(rows_i[b])
-        ids[b, Lm - n:] = rows_i[b]
-        ts[b, Lm - n:] = rows_t[b]
-    return ids, ts
-
-
-def _absolute_ts(chunks):
-    """turn the per-slot gaps into increasing timestamps per user, identically in chunk and concatenated form"""
-    B = chunks[0][0].shape[0]
-    last = torch.full((B,), 1_300_000_000, dtype=torch.int64)
-    out = []
-    for ids, gaps in chunks:
-        ts = last[:, None] + torch.cumsum(gaps * (ids != 0), 1)
-        ts[ids == 0] = 0
-        last = torch.where((ids != 0).any(1), ts.max(1).values, last)
-        out.append((ids, ts))
-    return out
 
 
 def _run_chunked(m, B, widths, seed):

@@ -9,7 +9,7 @@ from tests import dense_reference as dr
 from tests import extend_jagged_reference as jr
 from tests import extend_reference as er
 from tests.sign_fixed_buckets import use_sign_fixed_oracle
-from tests.test_hstu_extend_gpu import V, _check, _model, _sign_fixed
+from tests.hstu_cases import SERVE_V as V, _check_extend as _check, _serve_model as _model, _sign_fixed
 from tests.util import relerr
 
 pytestmark = pytest.mark.gpu

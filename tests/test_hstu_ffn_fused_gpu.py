@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from tests.hstu_block_reference import site
-from tests.test_hstu_jagged_gpu import run_block_jagged
+from tests.hstu_cases import run_block_jagged
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")

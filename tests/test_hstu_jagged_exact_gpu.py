@@ -8,7 +8,7 @@
   O = 0, dQ | dK | dV = 0 and dx = 0, and the weight gradients are the sums over the sequence rows alone.  `pytest -s` prints the
   worst error / allowance of every quantity.
 - Device offsets out of contract (offsets[B] past T, offsets[0] > 0): no write past T, and the bits of the clamped batch.
-- The model against the oracle on the left-padded batch of the same users, with test_cfg2_parity_gpu's autocast yardstick.
+- The model against the oracle on the left-padded batch of the same users, with exact_check's autocast yardstick.
 - Bit identity: a full-length packed batch is the padded batch (loss, gradients, one FlatAdam step, under dropout), and a user's
   hidden rows and evaluation rank do not depend on the other users of the batch.
 - The sampled-softmax head through forward_jagged against tests/sampled_head_reference.py."""
@@ -19,27 +19,14 @@ import torch
 
 from tests import dense_reference as dr
 from tests import hstu_block_reference as hr
-from tests.test_hstu_block_exact_gpu import row_pass
-from tests.test_hstu_jagged_gpu import EDGE_LENGTHS, _users, attention_errors_jagged, run_block_jagged
+from tests.exact_check import Ledger, row_pass
+from tests.hstu_cases import EDGE_LENGTHS, _users, attention_errors_jagged, run_block_jagged
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
-_WORST = {}
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _error_table():
-    yield
-    if _WORST:
-        print("\nworst error / allowance per quantity of the packed block (tolerance 1):")
-        for name, (w, case) in sorted(_WORST.items()):
-            print(f"  {name:12s} {w:8.4f}   {case}")
-
-
-def _record(case, name, w, tol=dr.TOL):
-    if name not in _WORST or w > _WORST[name][0]:
-        _WORST[name] = (w, case)
-    return None if w <= tol else f"{name} {w:.3g}"
+LEDGER = Ledger("worst error / allowance per quantity of the packed block (tolerance 1):")
+_error_table = LEDGER.fixture()
+_record = LEDGER.record
 
 
 def check_block_jagged(r, case):
@@ -164,7 +151,8 @@ def test_model_vs_oracle_within_the_autocast_yardstick():
     test_cfg2_full_model_vs_oracle's yardstick: the reference algorithm's own bf16-autocast error.  The batch has an empty history,
     a history of 1, a full one and 23 idle rows."""
     from genrec_b200.data import collate_jagged, pack_jagged
-    from tests.test_cfg2_parity_gpu import L, V, _cfg2_model, _oracle_run, autocast_yardstick
+    from tests.exact_check import autocast_yardstick
+    from tests.hstu_cases import CFG2_L as L, CFG2_V as V, _cfg2_model, _oracle_run
     from tests.util import frob_relerr, relerr
     lengths = [57, 0, 200, 1, 130, 199, 64, 2]
     m = _cfg2_model()
@@ -234,11 +222,11 @@ def test_a_users_rows_and_rank_do_not_depend_on_the_batch():
     users, and with idle rows behind.  The forward GEMMs and LayerNorm are row-independent and the attention's tiles start at each
     sequence's first row, so a rank never depends on the batch it is served in."""
     from genrec_b200.data import pack_jagged
-    from tests.test_hstu_jagged_gpu import _model
+    from tests.hstu_cases import _jagged_model
     V, n = 300, 77
     others = [130, 5, 200, 0]
     items, ts, off, tgt, _ = _users(others + [n], V, 21)
-    m = _model(V).eval()
+    m = _jagged_model(V).eval()
     o = off.tolist()
     u_items, u_ts = items[o[-2]:], ts[o[-2]:]
 
@@ -270,12 +258,12 @@ def test_forward_jagged_with_negatives_matches_the_reference_on_its_hidden_state
     from genrec_b200.data import pack_jagged, sample_negatives
     from tests.head_reference import TOL
     from tests.sampled_head_reference import reference
-    from tests.test_hstu_jagged_gpu import _model
+    from tests.hstu_cases import _jagged_model
     V = 500
     items, ts, off, tgt, _ = _users(EDGE_LENGTHS, V, 31)
     pk = pack_jagged(items, off, tgt, 200, timestamps=ts, num_tokens=sum(EDGE_LENGTHS) + 19)
     args = (pk["input_ids"], pk["offsets"], pk["max_len"], pk["timestamps"])
-    m = _model(V)
+    m = _jagged_model(V)
     probs = torch.rand(V + 1, device=DEV) + 0.1
     neg, log_q = sample_negatives(V, 100, probs=probs)
     logits, loss = m.forward_jagged(*args, pk["targets"], negatives=neg, log_q=log_q)

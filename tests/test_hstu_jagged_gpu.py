@@ -3,36 +3,19 @@ the padded one, one block's packed attention (forward, dQ, dK/dV, bias-table gra
 tests/hstu_block_reference.py, the whole model against the padded batch of the same users, bit-identical repeats, the evaluation
 ranks, and a FlatAdam step captured in a CUDA graph and replayed with new offsets, ids and targets."""
 import copy
-import ctypes as C
 
 import pytest
 import torch
 
 from tests import dense_reference as dr
-from tests import hstu_block_reference as hr
-from tests.test_hstu_bias_configs_gpu import pos_fixed, sign_fix, table_excess
-from tests.test_hstu_block_exact_gpu import _params
+from tests.hstu_cases import EDGE_LENGTHS, _jagged_model as _model, _users, attention_errors_jagged, run_block_jagged, sign_fix
 from tests.util import relerr
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
-EDGE_LENGTHS = [0, 1, 63, 64, 65, 127, 128, 129, 200]
 # forward_jagged against forward on the padded batch: the same bf16 operands, the fp32 sums taken over other tile boundaries
 MODEL_LOSS_TOL = 2e-3
 MODEL_GRAD_TOL = 2e-2
-
-
-def _users(lengths, V, seed):
-    """per-user histories (time order), timestamps and held-out targets -> the jagged device batch and hstu_collate_fn's input"""
-    g = torch.Generator().manual_seed(seed)
-    hist = [torch.randint(1, V + 1, (n,), generator=g) for n in lengths]
-    stamps = [1_300_000_000 + torch.cumsum(torch.randint(1, 10 ** 6, (n,), generator=g), 0) for n in lengths]
-    tgt = torch.randint(1, V + 1, (len(lengths),), generator=g)
-    offsets = torch.zeros(len(lengths) + 1, dtype=torch.int64)
-    offsets[1:] = torch.cumsum(torch.tensor(lengths, dtype=torch.int64), 0)
-    items, ts = torch.cat(hist).long(), torch.cat(stamps).long()
-    rows = [dict(history=h.tolist(), timestamps=s.tolist(), target=int(t)) for h, s, t in zip(hist, stamps, tgt)]
-    return items.to(DEV), ts.to(DEV), offsets.to(DEV), tgt.to(DEV), rows
 
 
 def _collate_rows_without_pads(rows, max_seq_len):
@@ -101,124 +84,6 @@ def test_jagged_bias_index_equals_the_padded_rows(pos, timed):
 
 
 # ---------------------------------------------------------------------------------------------------- one block, fp64 references
-def run_block_jagged(lengths, D, H, pos, time, idle=5, seed=1, *, p=0.0, layer=0, seed_dev=None, max_len=None, offsets=None, lead=0, canary=0):
-    """Forward and backward of one block through grb_hstu_layer_forward_jagged / _backward_jagged with a NaN-filled saved blob and
-    workspace (its scratch for the ordered sums included).  pos: ("uni", bucket) or ("fix", npos, max_distance); time: buckets or "nots".  T = sum(lengths) + idle token rows;
-    max_len defaults to the longest length.  lead: idle rows put in front of the batch (offsets[0] = lead, out of contract), the
-    other rows' inputs unchanged.  offsets (a list of B + 1) replaces the device offsets (the kernels clamp it to [0, T)).  Rows
-    outside [offsets[0], offsets[B]) are idle: pad, and dy = 0 there as the head gives it.  canary: rows of x, dy, y and dx past T
-    in the same allocations, y / dx filled with 7.0.  -> the kernel's intermediates and gradients."""
-    import genrec_b200.functional as Fn
-    from genrec_b200 import _lib
-    from genrec_b200._lib import HstuDims, HstuLayerGrads, HstuLayerParams, check, ptr, stream_ptr
-    from genrec_b200.hstu import _thresholds_on
-    lib = _lib.load()
-    g = torch.Generator().manual_seed(seed)
-    n_real = sum(lengths)
-    Tm, B = n_real + idle, len(lengths)
-    T = Tm + lead
-    max_len = max_len or max(max(lengths), 1)
-    off = torch.zeros(B + 1, dtype=torch.int64)
-    off[1:] = torch.cumsum(torch.tensor(lengths), 0)
-    off += lead
-    if offsets is not None:
-        off = torch.tensor(offsets, dtype=torch.int64)
-    lo, hi = min(max(int(off[0]), 0), T), min(max(int(off[-1]), 0), T)
-    seq = torch.zeros(T, dtype=torch.bool)
-    seq[lo:hi] = True
-    ts = 1_300_000_000 + torch.cumsum(torch.randint(1, 3 * 86400, (Tm,), generator=g), 0)
-    ts = torch.cat([torch.full((lead,), 1_300_000_000), ts])
-    pad = (~seq).to(torch.uint8)
-    uniform = pos[0] == "uni"
-    npos = 8 if uniform else pos[1]
-    pb = torch.full((max_len,), pos[1]) if uniform else pos_fixed(torch.arange(max_len), pos[1], pos[2])
-    has_time = isinstance(time, int)
-    ntime = time if has_time else 0
-    offd = off.to(DEV)
-    meta = Fn.SeqMeta(pad.to(DEV), ts.to(DEV) if has_time else None, pb.to(torch.uint8).to(DEV), _thresholds_on(DEV), ntime or 64, npos,
-                      (uniform, int(pb[0])), offsets=offd, max_len=max_len)
-    prm = _params(D, H, npos, ntime, seed + 7)
-    xa = torch.randn(Tm + canary, D, generator=g)
-    xa[:Tm:3] += 1000.0 * torch.where(torch.arange(0, Tm, 3) % 2 == 0, 1.0, -1.0)[:, None]   # LayerNorm's large-offset rows
-    dya = torch.randint(-64, 65, (Tm + canary, D), generator=g).float() / 64
-    xa = torch.cat([torch.randn(lead, D, generator=g), xa])
-    dya = torch.cat([torch.zeros(lead, D), dya])
-    dya[:T][~seq] = 0
-    xa, dya = xa.to(DEV), dya.to(DEV)
-    x, dy = xa[:T], dya[:T]
-    sdev = None if seed_dev is None else torch.tensor([seed_dev], dtype=torch.int64, device=DEV)
-    dseed = 0x1234_5678_9ABC_DEF0 + layer
-    dims = HstuDims(B, max_len, D, H, npos, ntime, float(p), dseed, ptr(sdev), layer)
-    names = ("proj_w", "proj_b", "pos_table", "time_table", "ln1_g", "ln1_b", "ffn1_w", "ffn1_b", "ffn2_w", "ffn2_b", "ln2_g", "ln2_b")
-    pstruct = HstuLayerParams(*[ptr(prm[n]) if (n != "time_table" or has_time) else None for n in names])
-    grads = {n: torch.zeros(prm[n].shape, dtype=torch.float32, device=DEV) for n in names}
-    gstruct = HstuLayerGrads(*[ptr(grads[n]) for n in names])
-    st_ = meta.struct()
-    sl, wl = hr.saved_layout(T, D), hr.work_layout(T, D)
-    nsaved, nwork = lib.grb_hstu_layer_saved_bytes_jagged(C.byref(dims), T), lib.grb_hstu_layer_workspace_bytes_jagged(C.byref(dims), T)
-    assert nsaved == sl["bytes"] and wl["bytes"] <= nwork
-    saved = torch.full((nsaved,), 0xFF, dtype=torch.uint8, device=DEV)        # NaN in bf16 and fp32
-    ws = torch.full((nwork,), 0xFF, dtype=torch.uint8, device=DEV)   # the ordered sums' scratch too: a partial never stored shows
-    ya, dxa = torch.full_like(xa, 7.0), torch.full_like(xa, 7.0)
-    st = stream_ptr(DEV)
-    check(lib.grb_hstu_layer_forward_jagged(C.byref(dims), C.byref(pstruct), C.byref(st_), ptr(offd), T, ptr(x), ptr(ya), ptr(saved), st))
-    check(lib.grb_hstu_layer_backward_jagged(C.byref(dims), C.byref(pstruct), C.byref(st_), ptr(offd), T, ptr(dy), ptr(saved), ptr(dxa),
-                                             C.byref(gstruct), ptr(ws), st))
-    torch.cuda.synchronize()
-    out = {n: hr.view(saved, sl, n) for n in sl if n != "bytes"}
-    out.update({n: hr.view(ws, wl, n) for n in wl if n != "bytes"})
-    out.update(grads=grads, prm=prm, meta=meta, off=[min(max(int(v), lo), hi) for v in off], D=D, H=H, n_real=n_real, T=T, x=x, dy=dy,
-               y=ya[:T], dx=dxa[:T], y_canary=ya[T:], dx_canary=dxa[T:], seq=seq.to(DEV), uniform=uniform, npos=npos, pb0=int(pb[0]),
-               has_time=has_time, ntime=ntime, p=p, layer=layer, seed=hr.effective_seed(dseed, p, seed_dev), max_len=max_len)
-    return out
-
-
-def attention_errors_jagged(r):
-    """The attention of a packed block against hr.attention per sequence (the sequences of one length batched; on the GPU, in fp64),
-    on the kernel's P, zp and dO.  Idle rows must hold O = 0 and dQ | dK | dV = 0.  -> ({O, dV, dQ, dK: worst error / allowance},
-    {dpos, dtime: table_excess})"""
-    D, H, prm, gr = r["D"], r["H"], r["prm"], r["grads"]
-    for n in ("P", "O", "dO", "dzp", "y", "dx"):
-        assert bool(torch.isfinite(r[n].float()).all()), f"{n} has an unwritten or non-finite element"
-    seq = r["seq"]
-    assert not bool(r["O"][~seq].any()) and not bool(r["dzp"][~seq][:, D:].any()), "idle rows of O / dQ dK dV are not zero"
-    wpos = prm["pos_table"][r["pb0"]:r["pb0"] + 1] if r["uniform"] else prm["pos_table"]
-    wtime = prm["time_table"][:r["ntime"]] if r["has_time"] else None
-    nrows = 1 if r["uniform"] else r["npos"]
-    acc = {"pos": None, "time": None}
-    worst = {k: 0.0 for k in ("O", "dV", "dQ", "dK")}
-    by_len = {}
-    for b in range(len(r["off"]) - 1):
-        lo, n = r["off"][b], min(r["off"][b + 1] - r["off"][b], r["max_len"])
-        if n > 0:
-            by_len.setdefault(n, []).append(lo)
-    for n, starts in sorted(by_len.items()):
-        step = max(1, (1 << 24) // (H * n * n))           # fp64 [seqs, H, n, n] tensors of at most 128 MB
-        for c in range(0, len(starts), step):
-            rows = (torch.tensor(starts[c:c + step])[:, None] + torch.arange(n)[None]).to(DEV)
-            w, masked, pbc, tbc = hr.cell_bias(r["meta"].bias_index[rows], wpos, wtime, nrows, H)
-            valid = hr.causal_valid(torch.zeros(rows.shape, dtype=torch.bool, device=DEV))
-            assert torch.equal(masked, ~valid.expand_as(masked)), n
-            at = hr.attention(r["P"][rows], w, valid, H, r["zp"][rows], r["dO"][rows])
-            dzp = r["dzp"][rows]
-            for name, got, ref, allow in [("O", r["O"][rows], at["O"], at["a_O"]), ("dV", dzp[..., D:2 * D], at["dV"], at["a_dV"]),
-                                          ("dQ", dzp[..., 2 * D:3 * D], at["dQ"], at["a_dQ"]), ("dK", dzp[..., 3 * D:], at["dK"], at["a_dK"])]:
-                worst[name] = max(worst[name], dr.worst(got, ref, allow))
-            bucket = torch.full_like(pbc, r["pb0"]) if r["uniform"] else pbc
-            parts = {"pos": hr.table_sums(at["dS"], valid, bucket[:, None], r["npos"])}
-            if r["has_time"]:
-                parts["time"] = hr.table_sums(at["dS"], valid, tbc[:, None], r["ntime"])
-            for k, v in parts.items():
-                acc[k] = v if acc[k] is None else tuple(a + e for a, e in zip(acc[k], v))
-            del at, w, masked, valid
-    excess = {}
-    for k, name, table in (("pos", "dpos", "pos_table"), ("time", "dtime", "time_table")):
-        if acc[k] is not None:
-            ref, mass, count = acc[k]
-            excess[name] = table_excess(gr[table], ref, mass.cpu(), count.cpu())
-        else:                                             # no time term, or no sequence at all
-            assert not bool(gr[table].any()), f"{table} gradient without a live cell"
-    return worst, excess
 
 
 def check_attention_jagged(r):
@@ -244,17 +109,6 @@ def test_jagged_attention_vs_fp64(case):
 
 
 # ---------------------------------------------------------------------------------------------------- the model
-def _model(V, blocks=2, D=64, H=2, seed=0, fixed=False):
-    from genrec_b200.hstu import HSTU
-    torch.manual_seed(seed)
-    m = HSTU(V, 200, D, H, blocks, dropout=0.0).to(DEV).train()
-    if fixed:
-        sign_fix(m)
-    with torch.no_grad():
-        for n, p in m.named_parameters():
-            if "attention_bias" in n:
-                p.normal_(0, 0.3)
-    return m
 
 
 def _grads(m):

@@ -4,7 +4,8 @@ import pytest
 import torch
 
 from tests.sign_fixed_buckets import use_sign_fixed_oracle
-from tests.test_hstu_extend_gpu import V, _absolute_ts, _check, _chunks, _model, _sign_fixed
+from tests.hstu_cases import (SERVE_V as V, _absolute_ts, _check_extend as _check, _chunks, _fill, _history_calls, _left_padded,
+                              _serve_model as _model, _sign_fixed)
 
 pytestmark = pytest.mark.gpu
 
@@ -32,14 +33,6 @@ def _same_user(pool, u, st, b):
     assert torch.equal(pool.last_hidden[u], st.last_hidden[b])
 
 
-def _fill(m, pool, users, nfill, seed):
-    """extend `users` by nfill items each (one call), to occupy pages"""
-    g = torch.Generator().manual_seed(seed)
-    ids = torch.randint(1, V + 1, (len(users), nfill), generator=g)
-    ts = 1_200_000_000 + torch.cumsum(torch.randint(1, 86400, (len(users), nfill), generator=g), 1)
-    m.extend_users(pool, torch.tensor(users), ids.cuda(), ts.cuda())
-
-
 @pytest.mark.parametrize("D,H", [(64, 2), (128, 4), (256, 8)])
 @pytest.mark.parametrize("use_time", [True, False])
 @pytest.mark.parametrize("order", ["rows", "permuted", "interleaved"])
@@ -62,44 +55,6 @@ def test_bit_identical_to_dense_state(D, H, use_time, order):
     for b in range(B):
         _same_user(pool, int(user_of[b]), st, b)
     assert not pool.overflowed().any() and int(pool.errors()) == 0
-
-
-def _history_calls(nusers, ncalls, seed):
-    """ncalls calls, each naming a different subset of users (B from 1 to nusers, random order) with a chunk of 1..9 slots per
-    row, left-padded, some rows all padding.  Timestamps increase per user."""
-    g = torch.Generator().manual_seed(seed)
-    last = torch.full((nusers,), 1_300_000_000, dtype=torch.int64)
-    calls = []
-    for c in range(ncalls):
-        B = 1 + c % nusers if c < nusers else int(torch.randint(1, nusers + 1, (1,), generator=g))
-        users = torch.randperm(nusers, generator=g)[:B]
-        w = int(torch.randint(1, 10, (1,), generator=g))
-        ids = torch.randint(1, V + 1, (B, w), generator=g)
-        gaps = torch.randint(0, 2 * 86400, (B, w), generator=g)
-        for r in range(B):
-            pads = w if (c + r) % 5 == 3 else int(torch.randint(0, w, (1,), generator=g))
-            ids[r, :pads] = 0
-        ts = torch.zeros(B, w, dtype=torch.int64)
-        for r in range(B):
-            u = int(users[r])
-            t = last[u] + torch.cumsum(gaps[r] * (ids[r] != 0), 0)
-            ts[r] = torch.where(ids[r] != 0, t, torch.zeros_like(t))
-            if (ids[r] != 0).any():
-                last[u] = int(t[-1])
-        calls.append((users, ids, ts))
-    return calls
-
-
-def _left_padded(hist, users):
-    L = max(1, max(len(hist[int(u)][0]) for u in users))
-    ids = torch.zeros(len(users), L, dtype=torch.int64)
-    ts = torch.zeros(len(users), L, dtype=torch.int64)
-    for r, u in enumerate(users.tolist()):
-        n = len(hist[u][0])
-        if n:
-            ids[r, L - n:] = torch.tensor(hist[u][0])
-            ts[r, L - n:] = torch.tensor(hist[u][1])
-    return ids, ts
 
 
 @pytest.mark.parametrize("buckets", ["reference", "sign_fixed"])

@@ -1,26 +1,13 @@
 """FlatAdam(lazy_table=True) without a GPU: an fp64 restatement of the lazy rule, checked against torch.optim.SparseAdam (eps = 0,
 where SparseAdam's form and FlatAdam's coincide) and against a dense torch.optim.Adam run whose rows are all touched at every step;
 the argument checks of the three C-ABI entry points; and the ValueErrors of the optimizer's constructor.
-tests/test_lazy_table_gpu.py checks the kernels against the same restatement."""
+tests/test_lazy_table_gpu.py checks the kernels against the same restatement (hstu_block_reference.lazy_adam_reference)."""
 import ctypes
 
 import pytest
 import torch
 
-
-def lazy_adam_reference(p, g, m, v, rows, step, lr, betas, eps, weight_decay, grad_scale=1.0, bias_corrections=None):
-    """One lazy step in fp64: FlatAdam's per-element rule (torch.optim.Adam with L2 weight decay, bias corrections of the global
-    step count `step`, already ticked) on the rows `rows` of the [C, D] tensors; every other row is copied.  -> (p, m, v).
-    ``bias_corrections`` = (1 - beta1^step, 1 - beta2^step) as the optimizer's state holds them, when given."""
-    p, g, m, v = (t.double().clone() for t in (p, g, m, v))
-    r = torch.as_tensor(sorted(set(int(i) for i in rows)), dtype=torch.long)
-    b1, b2 = betas
-    bc1, bc2 = bias_corrections if bias_corrections is not None else (1 - b1 ** step, 1 - b2 ** step)
-    gr = g[r] * grad_scale + weight_decay * p[r]
-    m[r] = b1 * m[r] + (1 - b1) * gr
-    v[r] = b2 * v[r] + (1 - b2) * gr * gr
-    p[r] = p[r] - lr / bc1 * (m[r] / (v[r].sqrt() / bc2 ** 0.5 + eps))
-    return p, m, v
+from tests.hstu_block_reference import lazy_adam_reference
 
 
 def test_reference_matches_sparse_adam_at_eps_zero():

@@ -5,7 +5,7 @@ Markov-split training run of test_sampled_head_gpu.py."""
 import pytest
 import torch
 
-from tests.test_lazy_table_cpu import lazy_adam_reference
+from tests.hstu_block_reference import lazy_adam_reference
 
 pytestmark = pytest.mark.gpu
 
@@ -368,7 +368,7 @@ def test_training_with_uniform_negatives_and_lazy_table_learns_the_markov_split(
     from genrec_b200.hstu import HSTU
     from genrec_b200.optim import FlatAdam
     from oracle import hstu as oh
-    from tests.test_recall_gpu import markov_users
+    from tests.hstu_cases import markov_users
     dev = _dev()
     V, L, D, H, NB, B, STEPS = 200, 20, 64, 2, 2, 64, 150
     seqs, stamps = markov_users(512, V, L, seed=0)

@@ -4,28 +4,9 @@ then evaluated leave-one-out exactly like genrec/trainers/hstu_trainer.py:39-83.
 import pytest
 import torch
 
+from tests.hstu_cases import markov_users
+
 pytestmark = pytest.mark.gpu
-
-
-def markov_users(num_users, V, L, seed, clusters=10):
-    """First-order Markov chain over item clusters: the next item is (mostly) drawn from the successor cluster, so the task is
-    learnable and Recall@10 is far above chance."""
-    g = torch.Generator().manual_seed(seed)
-    per = V // clusters
-    seqs, stamps = [], []
-    for _ in range(num_users):
-        c = int(torch.randint(0, clusters, (1,), generator=g))
-        items, ts, t = [], [], 1_300_000_000
-        for _ in range(L + 1):
-            if float(torch.rand(1, generator=g)) < 0.9:
-                c = (c + 1) % clusters
-            else:
-                c = int(torch.randint(0, clusters, (1,), generator=g))
-            items.append(1 + c * per + int(torch.randint(0, per, (1,), generator=g)))
-            t += int(torch.randint(60, 86400, (1,), generator=g))
-            ts.append(t)
-        seqs.append(items); stamps.append(ts)
-    return torch.tensor(seqs), torch.tensor(stamps)
 
 
 def test_recall_at_10_matches_oracle_training():

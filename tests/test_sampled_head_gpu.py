@@ -7,6 +7,7 @@ measured errors of every case."""
 import pytest
 import torch
 
+from tests.head_cases import _dev, _to_dev
 from tests.head_reference import TOL, format_table, head_errors, violations
 from tests.sampled_head_reference import make_case, reference
 
@@ -24,17 +25,6 @@ def _error_table():
         print("\n" + format_table("", {k: 0.0 for k in keys})[0] + "\n|" + "---|" * (len(keys) + 1))
         print("\n".join(line for _, line in _ROWS))
         print(format_table("max over all cases", {k: max(e[k] for e, _ in _ROWS) for k in keys})[1])
-
-
-def _dev():
-    return torch.device("cuda:0")
-
-
-def _to_dev(case):
-    from genrec_b200 import functional as Fn
-    c = {k: (v.to(_dev()).contiguous() if v is not None else None) for k, v in case.items()}
-    c["tb"] = Fn.cast_bf16(c["table"])
-    return c
 
 
 def _call(c, *, dx=None, dtable=None, dg=None, db=None, loss_only=False):
@@ -289,7 +279,7 @@ def test_training_with_uniform_negatives_learns_the_markov_split():
     from genrec_b200.hstu import HSTU
     from genrec_b200.optim import FlatAdam
     from oracle import hstu as oh
-    from tests.test_recall_gpu import markov_users
+    from tests.hstu_cases import markov_users
     dev = _dev()
     V, L, D, H, NB, B, STEPS = 200, 20, 64, 2, 2, 64, 150
     seqs, stamps = markov_users(512, V, L, seed=0)

@@ -9,7 +9,7 @@ masks are restated from (seed, site), so a backward that pairs a stage with anot
 
 Part B: Tiger.forward and forward_jagged, forward and backward, at p = 0.1 and 0.3, against tests/tiger_reference.py in fp64 on the
 same masks: torch's F.dropout masks recorded by a shim, the kernels' restated from the step's seed and sites.  The yardstick is the
-same restatement under bf16 torch.autocast (test_cfg2_parity_gpu.autocast_yardstick).
+same restatement under bf16 torch.autocast (exact_check.autocast_yardstick).
 
 `pytest -s` prints the worst error / allowance of every part A quantity and the yardstick table of every part B step."""
 import zlib
@@ -22,91 +22,27 @@ from tests import dense_reference as dr
 from tests import hstu_block_reference as hr
 from tests import tiger_params as tp
 from tests import tiger_reference as tr
-from tests.test_tiger_jagged_gpu import _geometric_lengths, _model, _padded_and_packed
+from tests.exact_check import (FTZ, Ledger, Spy, _TorchDropout, _cid, _dy, _packed_core_ref, _seeded,
+                                autocast_yardstick)
+from tests.tiger_params import _geometric_lengths, _model, _padded_and_packed
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
-_WORST = {}
 WIDTHS = [(64, 2), (128, 4), (384, 6)]
 ROWS = [1, 63, 64, 65, 129, 256 * 61]
 PS = [0.0, 0.1, 0.3]
+LEDGER = Ledger("worst error / allowance per quantity of the TIGER block stages (dense tolerance 1, attention core: "
+                "attention_reference.TOL):", width=18, floor=FTZ)
+_error_table = LEDGER.fixture()
+_check = LEDGER.check
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _error_table():
-    yield
-    if _WORST:
-        print("\nworst error / allowance per quantity of the TIGER block stages (dense tolerance 1, attention core: "
-              "attention_reference.TOL):")
-        for name, (w, case) in sorted(_WORST.items()):
-            print(f"  {name:18s} {w:8.4f}   {case}")
-
-
-def _record(case, name, w, tol=dr.TOL):
-    if name not in _WORST or w > _WORST[name][0]:
-        _WORST[name] = (w, case)
-    return None if w <= tol else f"{name} {w:.3g}"
-
-
-# fp32 flush-to-zero (--use_fast_math) of products and partial sums below 2^-126, over up to 2^26 terms: padded keys carry values
-# of 1e-37 into the K | V gradient GEMMs
-FTZ = 2.0 ** -100
-
-
-def _check(case, items):
-    """items: (name, got, ref, allowance)"""
-    bad = [_record(case, n, dr.worst(g, r, a + FTZ)) for n, g, r, a in items]
-    bad = [b for b in bad if b]
-    assert not bad, (case, bad)
-
-
-def _check_core(case, err):
-    bad = []
-    for n, (w, f) in err.items():
-        tw, tf = ar.tolerance("t5", n)
-        _record(case, "core " + n, w / tw, 1.0)
-        _record(case, "core " + n + " frob", f / tf, 1.0)
-    bad = ar.violations(err, "t5")
-    assert not bad, (case, bad)
-
-
-class _Spy:
-    """records the outputs of the functional calls of one backward, by name, in call order"""
-
-    def __init__(self, monkeypatch):
-        from genrec_b200 import functional as Fn
-        from genrec_b200 import t5_attention as t5
-        self.calls = []
-        for mod, names in ((Fn, ("cast_rows_bf16", "linear_bwd", "linear_dact_bwd")),
-                           (t5, ("attention_core_bwd", "attention_core_bwd_jagged"))):
-            for n in names:
-                monkeypatch.setattr(mod, n, self._wrap(n, getattr(mod, n)))
-
-    def _wrap(self, name, fn):
-        def spy(*a, **k):
-            out = fn(*a, **k)
-            self.calls.append((name, out))
-            return out
-        return spy
-
-    def take(self, *names):
-        got = [out for n, out in self.calls]
-        assert [n for n, _ in self.calls] == list(names), [n for n, _ in self.calls]
-        return got
-
-
-def _dy(shape, seed):
-    """small integers / 64: every masked bf16 cast of it is exact"""
-    g = torch.Generator().manual_seed(seed)
-    return (torch.randint(-64, 65, shape, generator=g).float() / 64).to(DEV)
-
-
-def _seeded(shape, seed, scale=1.0):
-    return (scale * torch.randn(shape, generator=torch.Generator().manual_seed(seed))).to(DEV)
-
-
-def _cid(c):
-    return "-".join(f"{v}" for v in c)
+def _spy(monkeypatch):
+    """the functional calls of one backward"""
+    from genrec_b200 import functional as Fn
+    from genrec_b200 import t5_attention as t5
+    return Spy(monkeypatch, {Fn: ("cast_rows_bf16", "linear_bwd", "linear_dact_bwd"),
+                             t5: ("attention_core_bwd", "attention_core_bwd_jagged")})
 
 
 # ------------------------------------------------------------------------------------------------ part A: the stages
@@ -122,7 +58,7 @@ def test_rmsnorm_and_linear_stages(case, monkeypatch):
     y = _RmsNormFn.apply(x, w)
     xc, rstd, _ = y.grad_fn.saved_tensors
     dy = _dy((R, D), R)
-    spy = _Spy(monkeypatch)
+    spy = _spy(monkeypatch)
     y.backward(dy)
     spy.take()
     fr = dr.rmsnorm_forward(xc, w.detach(), tr.EPS)
@@ -158,7 +94,7 @@ def test_ffn_stages(case, monkeypatch):
     pp, seed, site = y.grad_fn.cfg
     assert pp == p and seed == (torch.initial_seed() & (2 ** 63 - 1) if p > 0 else 0)
     dy = _dy((R, D), R + 1)
-    spy = _Spy(monkeypatch)
+    spy = _spy(monkeypatch)
     y.backward(dy)
     dyb, (_, dwo, _), dz, (dxn, dwi, _) = spy.take("cast_rows_bf16", "linear_bwd", "linear_dact_bwd", "linear_bwd")
     zero = torch.zeros(FFN_DIM, device=DEV)
@@ -196,7 +132,7 @@ def test_head_stages(case, monkeypatch):
     xb, wp = y.grad_fn.saved_tensors
     assert wp.shape == (776, D) and not bool(wp[V:].any()) and torch.equal(wp[:V], w.detach().bfloat16())
     dy = _dy((R, V), R + 2)
-    spy = _Spy(monkeypatch)
+    spy = _spy(monkeypatch)
     y.backward(dy)
     dyb, (dx, dwp, _) = spy.take("cast_rows_bf16", "linear_bwd")
     assert not bool(dyb[:, V:].any()) and not bool(dwp[V:].any()), "a pad row of the head mirror reached dw"
@@ -227,45 +163,6 @@ def _lengths(shp):
 def _aid(c):
     f, shp, Lq, D, H, p = c
     return f"{f}-{shp if isinstance(shp, str) else 'x'.join(map(str, shp))}-D{D}-H{H}-p{p}"
-
-
-def _packed_core_ref(Q, K, V, A, dAb, H, bias, offs, Lq, scale, p, seed, site):
-    """the fp64 core per sequence with the packed keys (as test_tiger_jagged_gpu._core_check) -> (ref, rows of Q / of K per seq)"""
-    from genrec_b200 import t5_attention as t5
-    mx = max(b - a for a, b in zip(offs, offs[1:]))
-    B = len(offs) - 1
-    mask = (tr.attn_mask_packed_self(Q.shape[0], H, mx, p, seed, site, DEV) if Lq == 0
-            else tr.attn_mask_packed_cross(B, H, Lq, mx, p, seed, site, DEV))
-    names = ("out", "dq", "dk", "dv")
-    ref = {k: [] for n in names for k in (n, "a_" + n)}
-    db = adb = None
-    saved = ar.attn_keep
-    try:
-        for b in range(B):
-            r0, r1 = offs[b], offs[b + 1]
-            n = r1 - r0
-            if Lq == 0:
-                keep = mask[r0:r1, :, :n].transpose(0, 1)[None]
-                q, o, do = Q[r0:r1][None], A[r0:r1][None], dAb[r0:r1][None]
-                bk = t5.relative_position_buckets(n, n).to(DEV)
-            else:
-                keep = mask[b:b + 1, :, :, :n]
-                q, o, do = Q[b:b + 1], A[b:b + 1], dAb[b:b + 1]
-                bk = None
-            ar.attn_keep = lambda *a, **k: keep
-            r = ar.t5_reference(q, K[r0:r1][None], V[r0:r1][None], H, bias, bk, None, False, scale, do, o, p, seed, site)
-            for nm in names:
-                ref[nm].append(r[nm][0])
-                ref["a_" + nm].append(r["a_" + nm][0])
-            if bias is not None:
-                db = r["dbias"] if db is None else db + r["dbias"]
-                adb = r["a_dbias"] if adb is None else adb + r["a_dbias"]
-    finally:
-        ar.attn_keep = saved
-    ref = {k: torch.cat(v) for k, v in ref.items()}
-    if bias is not None:
-        ref["dbias"], ref["a_dbias"] = db, adb
-    return ref
 
 
 @pytest.mark.parametrize("case", ATTN, ids=_aid)
@@ -321,7 +218,7 @@ def test_t5_attention_stages(case, monkeypatch):
     assert (Hc, pc) == (H, p) and seed == (torch.initial_seed() & (2 ** 63 - 1) if p > 0 else 0) and site == t5._CALLS["n"]
     bias = bias if rel is not None else None
     dy = _dy(tuple(out.shape), D + B)
-    spy = _Spy(monkeypatch)
+    spy = _spy(monkeypatch)
     out.backward(dy)
     core = "attention_core_bwd_jagged" if packed else "attention_core_bwd"
     if cross:
@@ -362,7 +259,7 @@ def test_t5_attention_stages(case, monkeypatch):
             assert bool(ref["drop"].any())
     if bias is not None:
         got["dbias"] = dbias
-    _check_core(case_id, ar.errors(got, ref, ("out", "dq", "dk", "dv", "dbias")))
+    LEDGER.check_core(case_id, ar.errors(got, ref, ("out", "dq", "dk", "dv", "dbias")), "t5")
     # backward projections
     bo = dr.linear_backward(flat(dyb), wob, flat(A))
     items += [("attn dA", flat(dA), bo["dx"], bo["a_dx"]), ("attn dwo", dwo, bo["dw"], bo["a_dw"])]
@@ -400,21 +297,6 @@ def test_edges_are_reached():
 
 
 # ------------------------------------------------------------------------------------------------ part B: the whole step
-class _TorchDropout:
-    """genrec_b200.tiger's F: dropout draws a keep-scale mask, records it and applies it; everything else is torch.nn.functional"""
-
-    def __init__(self):
-        self.masks = []
-
-    def dropout(self, x, p=0.5, training=True):
-        if not training or p == 0:
-            return x
-        m = torch.where(torch.rand(x.shape, device=x.device) >= p, ar.keep_scale(p)[1], 0.0)
-        self.masks.append(m.double())
-        return x * m
-
-    def __getattr__(self, name):
-        return getattr(torch.nn.functional, name)
 
 
 def _graph_cfgs(root):
@@ -441,7 +323,6 @@ STEPS += [("edges", p, form) for p in (0.1, 0.3) for form in ("padded", "packed"
 @pytest.mark.parametrize("case", STEPS, ids=_cid)
 def test_training_step_vs_fp64(case, monkeypatch):
     from genrec_b200 import t5_attention, tiger
-    from tests.test_cfg2_parity_gpu import autocast_yardstick
     from tests.util import frob_relerr, relerr
     shape, p, form = case
     # B = 256 throughout: the yardstick compares two realisations of bf16 noise, which a handful of users leaves too scattered

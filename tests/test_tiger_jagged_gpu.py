@@ -9,6 +9,7 @@ import pytest
 import torch
 
 from tests import attention_reference as ar
+from tests.tiger_params import _geometric_lengths, _model, _padded_and_packed
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
@@ -138,46 +139,6 @@ def test_packed_backward_is_reproducible(Lq, lengths):
 
 
 # ------------------------------------------------------------------------------------------------ models: packed against padded
-def _model(cfg, seed=7):
-    from genrec_b200.tiger import Tiger
-    from tests import tiger_params as tp
-    m = Tiger(**cfg)
-    m.load_state_dict(tp.tiger_params([(k, v.shape) for k, v in m.state_dict().items()], seed))
-    return m.to(DEV)
-
-
-def _padded_and_packed(cfg, B, n_items, seed, lengths=None, num_tokens=None):
-    """tp.batch's padded batch (or one with the given item counts) and the same users packed by data.pack_tiger (into num_tokens
-    rows, the rest idle, when given)"""
-    from genrec_b200.data import pack_tiger
-    from tests import tiger_params as tp
-    b = tp.batch(cfg, B, n_items, seed)
-    C, E = cfg["sem_id_dim"], cfg["num_item_embeddings"]
-    if lengths is not None:                        # redraw the histories at these item counts (pads: the padding id, type 0)
-        N = n_items * C
-        mask = (torch.arange(N)[None, :] < torch.tensor(lengths)[:, None] * C).long()
-        ids = torch.randint(0, E, (B, N), generator=torch.Generator().manual_seed(seed + 1))
-        types = torch.arange(N).remainder(C).unsqueeze(0).expand(B, -1)
-        b["seq_mask"] = mask
-        b["item_input_ids"] = torch.where(mask == 0, torch.full_like(ids, C * E), ids)
-        b["token_type_ids"] = torch.where(mask == 0, torch.zeros_like(ids), types)
-    lens = b["seq_mask"].sum(1)
-    toks = torch.cat([b["item_input_ids"][i, :int(lens[i])] for i in range(B)])
-    off = torch.zeros(B + 1, dtype=torch.int64)
-    off[1:] = lens.cumsum(0)
-    pk = pack_tiger(b["user_input_ids"].view(-1).to(DEV), toks.to(DEV), off.to(DEV), b["target_input_ids"].to(DEV), max_items=n_items,
-                    num_tokens=num_tokens)
-    # the padded batch at the width of its longest history, as pad_collate makes it
-    width = int(lens.max())
-    padded = {k: v.to(DEV) for k, v in b.items()}
-    for k in ("item_input_ids", "token_type_ids", "seq_mask"):
-        padded[k] = padded[k][:, :width].contiguous()
-    return padded, pk
-
-
-def _geometric_lengths(B, seed, cap=20, mean=9.0):
-    g = np.random.default_rng(seed)
-    return np.minimum(g.geometric(1.0 / mean, B), cap).tolist()
 
 
 SHAPES = {"small": ("SMALL", 5, 6), "published": ("PUBLISHED", 256, 20)}
