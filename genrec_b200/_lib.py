@@ -1,7 +1,9 @@
 """ctypes binding of include/genrec_b200.h - the reference-side stub a genrec maintainer would add (INTEGRATION.md).
 
-There is NO fallback: if the shared library is missing or the device is not sm_90, importing callers get a
-RuntimeError that says how to build.  Nothing here touches ``oracle/``.
+The package reaches the library only through ``call`` (a launch, pinned to its device and that device's current stream),
+``workspace`` / ``host_bytes`` (the ``*_bytes`` size queries) and the small host-side helpers below.  There is NO fallback: if
+the shared library is missing or the device is not sm_90, importing callers get a RuntimeError that says how to build.  Nothing
+here touches ``oracle/``.
 """
 from __future__ import annotations
 
@@ -237,9 +239,14 @@ class GrbError(RuntimeError):
     pass
 
 
+def last_error() -> str:
+    """The library's message for the last call that failed on this thread."""
+    return load().grb_last_error().decode()
+
+
 def check(rc: int) -> None:
     if rc != 0:
-        raise GrbError(f"genrec_b200 error {rc}: {load().grb_last_error().decode()}")
+        raise GrbError(f"genrec_b200 error {rc}: {last_error()}")
 
 
 def ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -248,6 +255,46 @@ def ptr(t: Optional[torch.Tensor]) -> Optional[int]:
 
 def stream_ptr(device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
+
+
+def _entry(name: str):
+    if name not in SIGNATURES:
+        raise KeyError(f"{name} is not an entry point of include/genrec_b200.h")
+    return getattr(load(), name)
+
+
+def call(device, name: str, *args) -> None:
+    """Run entry point ``name`` on ``device``: under that device, with its current stream appended as the last argument.  The
+    library launches on the current device, so the stream and the launch always belong to the same GPU."""
+    fn = _entry(name)
+    with torch.cuda.device(device):
+        check(fn(*args, stream_ptr(device)))
+
+
+def _nbytes(name: str, args, allow_empty: bool = False) -> int:
+    n = _entry(name)(*args)
+    if n == 0 and not allow_empty:
+        raise GrbError(f"genrec_b200 error -1: {name}{args} refused its arguments: {last_error()}")
+    return n
+
+
+def host_bytes(name: str, *args) -> int:
+    """Byte count of a query that depends on its arguments only (no device).  0 means unsupported arguments: GrbError."""
+    return _nbytes(name, args)
+
+
+def workspace(device, name: str, *args, allow_empty: bool = False) -> torch.Tensor:
+    """Scratch for one launch on ``device``: a uint8 tensor of the byte count query ``name`` gives under that device (sizes may
+    depend on its SM count).  0 means unsupported arguments and raises GrbError, unless ``allow_empty``: for the queries whose
+    contract makes 0 a valid size."""
+    with torch.cuda.device(device):
+        n = _nbytes(name, args, allow_empty)
+    return torch.empty(n, dtype=torch.uint8, device=device)
+
+
+def defer_weight_grads(on: bool) -> None:
+    """Send the weight-gradient GEMMs of the following calls to the library's side stream (grb_set_defer_weight_grads)."""
+    check(load().grb_set_defer_weight_grads(1 if on else 0))
 
 
 def require_cuda(*tensors: Optional[torch.Tensor]) -> None:

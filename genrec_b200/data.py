@@ -86,12 +86,11 @@ def collate_jagged(items: torch.Tensor, offsets: torch.Tensor, targets: torch.Te
     order, offsets [B+1], one held-out target per user) -> the left-padded [B, L] batch dict, without a host round trip.
     L = min(longest history, max_seq_len); pass ``max_len_in_batch`` (the loader knows it) to avoid the one device sync that reading it
     from ``offsets`` costs."""
-    from . import _lib
-    from ._lib import check, ptr, require_cuda, stream_ptr
+    from ._lib import GrbError, call, ptr, require_cuda
     require_cuda(items, offsets, targets)
     for t in (items, offsets, targets, timestamps):
         if t is not None and t.dtype != torch.int64:
-            raise _lib.GrbError(f"genrec_b200 error -1: jagged batches are int64 (got {t.dtype})")
+            raise GrbError(f"genrec_b200 error -1: jagged batches are int64 (got {t.dtype})")
     B = offsets.numel() - 1
     if max_len_in_batch is None:
         max_len_in_batch = int((offsets[1:] - offsets[:-1]).max().item())
@@ -100,10 +99,8 @@ def collate_jagged(items: torch.Tensor, offsets: torch.Tensor, targets: torch.Te
     ids = torch.empty(B, L, dtype=torch.int64, device=dev)
     tgs = torch.empty(B, L, dtype=torch.int64, device=dev)
     tss = torch.empty(B, L, dtype=torch.int64, device=dev) if timestamps is not None else None
-    with torch.cuda.device(dev):
-        check(_lib.load().grb_collate_jagged(ptr(items.contiguous()), ptr(timestamps.contiguous()) if timestamps is not None else None,
-                                             ptr(offsets.contiguous()), ptr(targets.contiguous()), B, L, ptr(ids), ptr(tgs), ptr(tss),
-                                             stream_ptr(dev)))
+    call(dev, "grb_collate_jagged", ptr(items.contiguous()), ptr(timestamps.contiguous()) if timestamps is not None else None,
+         ptr(offsets.contiguous()), ptr(targets.contiguous()), B, L, ptr(ids), ptr(tgs), ptr(tss))
     out = {"input_ids": ids, "targets": tgs}
     if tss is not None:
         out["timestamps"] = tss
@@ -124,12 +121,11 @@ def pack_jagged(items: torch.Tensor, offsets: torch.Tensor, targets: torch.Tenso
     synchronisation.  With ``num_tokens`` T = num_tokens and max_len = max_seq_len, with no synchronisation (a captured step keeps
     fixed shapes): rows past the packed total are idle (id 0, target 0, timestamp 0), and a batch that does not fit sets
     ``overflow``, is cut at T and writes nothing past it - do not train on it."""
-    from . import _lib
-    from ._lib import check, ptr, require_cuda, stream_ptr
+    from ._lib import GrbError, call, ptr, require_cuda
     require_cuda(items, offsets, targets)
     for t in (items, offsets, targets, timestamps):
         if t is not None and t.dtype != torch.int64:
-            raise _lib.GrbError(f"genrec_b200 error -1: jagged batches are int64 (got {t.dtype})")
+            raise GrbError(f"genrec_b200 error -1: jagged batches are int64 (got {t.dtype})")
     B = offsets.numel() - 1
     if B < 1 or int(max_seq_len) < 1:
         raise ValueError(f"pack_jagged needs B >= 1 and max_seq_len >= 1 (got {B}, {max_seq_len})")
@@ -147,10 +143,8 @@ def pack_jagged(items: torch.Tensor, offsets: torch.Tensor, targets: torch.Tenso
     tss = torch.empty(T, dtype=torch.int64, device=dev) if timestamps is not None else None
     out_off = torch.empty(B + 1, dtype=torch.int64, device=dev)
     info = torch.empty(2, dtype=torch.int64, device=dev)
-    with torch.cuda.device(dev):
-        check(_lib.load().grb_pack_jagged(ptr(items.contiguous()), ptr(timestamps.contiguous()) if timestamps is not None else None,
-                                          ptr(offsets.contiguous()), ptr(targets.contiguous()), B, int(max_seq_len), T, ptr(ids), ptr(tgs),
-                                          ptr(tss), ptr(out_off), ptr(info), stream_ptr(dev)))
+    call(dev, "grb_pack_jagged", ptr(items.contiguous()), ptr(timestamps.contiguous()) if timestamps is not None else None,
+         ptr(offsets.contiguous()), ptr(targets.contiguous()), B, int(max_seq_len), T, ptr(ids), ptr(tgs), ptr(tss), ptr(out_off), ptr(info))
     out = {"input_ids": ids, "targets": tgs, "offsets": out_off, "max_len": max_len, "overflow": info[0] > T}
     if tss is not None:
         out["timestamps"] = tss

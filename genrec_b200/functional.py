@@ -1,7 +1,8 @@
 """torch-facing wrappers of the C ABI: tensors in, tensors out, autograd wired by hand.
 
-Every function here hands raw device pointers + the current CUDA stream to ``libgenrec_b200.so`` (ctypes, see
-``_lib.py``); PyTorch only provides memory, streams and the autograd graph.  CPU tensors raise - there is no fallback.
+Every function here hands raw device pointers to ``libgenrec_b200.so`` through ``_lib.call``, which runs each launch under
+its tensors' device and on that device's current stream; PyTorch only provides memory, streams and the autograd graph.  CPU
+tensors raise - there is no fallback.
 """
 from __future__ import annotations
 
@@ -12,7 +13,7 @@ from typing import List, NamedTuple, Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import HstuDims, HstuLayerGrads, HstuLayerParams, HstuSeq, SasrecDims, check, ensure_device, ptr, require_cuda, stream_ptr
+from ._lib import HstuDims, HstuLayerGrads, HstuLayerParams, HstuSeq, SasrecDims, call, ensure_device, ptr, require_cuda, workspace
 
 PARAM_ORDER = ("proj_w", "proj_b", "pos_table", "time_table", "ln1_g", "ln1_b", "ffn1_w", "ffn1_b", "ffn2_w", "ffn2_b",
                "ln2_g", "ln2_b")
@@ -45,7 +46,7 @@ def set_defer_weight_grads(on: bool) -> None:
 
 def _defer_for_call(active: bool) -> bool:
     if _DEFER["c"] != active:
-        check(_lib.load().grb_set_defer_weight_grads(1 if active else 0))
+        _lib.defer_weight_grads(active)
         _DEFER["c"] = active
     return active
 
@@ -53,13 +54,8 @@ def _defer_for_call(active: bool) -> bool:
 def join_deferred(device) -> None:
     """Make the deferred dW / dE GEMMs visible to the current stream of `device` and release their operand buffers."""
     if _DEFER["c"] or _DEFER["keep"]:
-        with torch.cuda.device(device):
-            check(_lib.load().grb_join_deferred(stream_ptr(device)))
+        call(device, "grb_join_deferred")
         _DEFER["keep"].clear()
-
-
-def _u8(n, device):
-    return torch.empty(n, dtype=torch.uint8, device=device)
 
 
 def cast_bf16(src: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -69,8 +65,7 @@ def cast_bf16(src: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Te
     if out is None:
         out = torch.empty(src.shape, dtype=torch.bfloat16, device=src.device)
     require_f32(src)
-    with torch.cuda.device(src.device):
-        check(_lib.load().grb_cast_f32_to_bf16(ptr(src), ptr(out), src.numel(), stream_ptr(src.device)))
+    call(src.device, "grb_cast_f32_to_bf16", ptr(src), ptr(out), src.numel())
     return out
 
 
@@ -126,14 +121,12 @@ class SeqMeta:
             pb_arg, npos_arg = self.pos_bucket, self.num_pos_buckets
         # deferred schedule: built on the side stream, joined before the first attention launch
         _defer_for_call(_DEFER["on"] and may_defer)
-        with torch.cuda.device(dev):
-            if self.offsets is None:
-                check(_lib.load().grb_hstu_bias_index(ptr(self.timestamps), ptr(self.pad), ptr(self.time_thr), ptr(pb_arg), B, L,
-                                                      npos_arg, nt, ptr(self.bias_index), self.ld, stream_ptr(dev)))
-            else:
-                check(_lib.load().grb_hstu_bias_index_jagged(ptr(self.timestamps), ptr(self.pad), ptr(self.offsets), ptr(self.time_thr),
-                                                             ptr(pb_arg), B, self.T, L, npos_arg, nt, ptr(self.bias_index), self.ld,
-                                                             stream_ptr(dev)))
+        if self.offsets is None:
+            call(dev, "grb_hstu_bias_index", ptr(self.timestamps), ptr(self.pad), ptr(self.time_thr), ptr(pb_arg), B, L, npos_arg, nt,
+                 ptr(self.bias_index), self.ld)
+        else:
+            call(dev, "grb_hstu_bias_index_jagged", ptr(self.timestamps), ptr(self.pad), ptr(self.offsets), ptr(self.time_thr), ptr(pb_arg),
+                 B, self.T, L, npos_arg, nt, ptr(self.bias_index), self.ld)
 
     def struct(self) -> HstuSeq:
         return HstuSeq(ptr(self.bias_index), self.ld, 1 if self.timestamps is not None else 0, 1 if self.pos_uniform else 0,
@@ -155,32 +148,23 @@ def _layer_param_struct(params, bf16w: dict, has_time: bool) -> HstuLayerParams:
 
 def layer_saved_bytes(dims: HstuDims) -> int:
     """Size of the block's saved-for-backward blob (a host-side query: no device needed)."""
-    lib = _lib.load()
-    nbytes = lib.grb_hstu_layer_saved_bytes(C.byref(dims))
-    if nbytes == 0:
-        raise _lib.GrbError(lib.grb_last_error().decode())
-    return nbytes
+    return _lib.host_bytes("grb_hstu_layer_saved_bytes", C.byref(dims))
 
 
 def hstu_block_forward(dims: HstuDims, params, bf16w: dict, has_time: bool, meta: SeqMeta, x: torch.Tensor):
     """One HSTU block (grb_hstu_layer_forward): x [B, L, D] fp32 contiguous -> (y, saved-for-backward blob).  A packed ``meta``
     (offsets set) takes x [T, D] and runs grb_hstu_layer_forward_jagged."""
-    lib = _lib.load()
     if meta.offsets is None:
-        nbytes = layer_saved_bytes(dims)
+        saved = workspace(x.device, "grb_hstu_layer_saved_bytes", C.byref(dims))
     else:
-        nbytes = lib.grb_hstu_layer_saved_bytes_jagged(C.byref(dims), meta.T)
-        if nbytes == 0:
-            raise _lib.GrbError(lib.grb_last_error().decode())
-    saved = _u8(nbytes, x.device)
+        saved = workspace(x.device, "grb_hstu_layer_saved_bytes_jagged", C.byref(dims), meta.T)
     y = torch.empty_like(x)
     pstruct, seq = _layer_param_struct(params, bf16w, has_time), meta.struct()
-    with torch.cuda.device(x.device):
-        if meta.offsets is None:
-            check(lib.grb_hstu_layer_forward(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(x), ptr(y), ptr(saved), stream_ptr(x.device)))
-        else:
-            check(lib.grb_hstu_layer_forward_jagged(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(meta.offsets), meta.T, ptr(x), ptr(y),
-                                                    ptr(saved), stream_ptr(x.device)))
+    if meta.offsets is None:
+        call(x.device, "grb_hstu_layer_forward", C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(x), ptr(y), ptr(saved))
+    else:
+        call(x.device, "grb_hstu_layer_forward_jagged", C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(meta.offsets), meta.T, ptr(x),
+             ptr(y), ptr(saved))
     return y, saved
 
 
@@ -189,7 +173,6 @@ def hstu_block_backward(dims: HstuDims, params, bf16w: dict, has_time: bool, met
     """grb_hstu_layer_backward -> (dx, parameter gradients in PARAM_ORDER, None where a parameter is absent).  With a ``sink``
     (name -> view of the flat gradient buffer of genrec_b200.optim.FlatAdam) the gradients accumulate there, and the weight
     gradients follow the deferred schedule when it is on."""
-    lib = _lib.load()
     if sink is not None:
         grads = [sink[n] if q is not None else None for n, q in zip(PARAM_ORDER, params)]
     else:
@@ -198,17 +181,16 @@ def hstu_block_backward(dims: HstuDims, params, bf16w: dict, has_time: bool, met
     dyc = dy.contiguous().float()
     dx = torch.empty_like(dyc)
     if meta.offsets is None:
-        ws = _u8(lib.grb_hstu_layer_workspace_bytes(C.byref(dims)), dy.device)
+        ws = workspace(dy.device, "grb_hstu_layer_workspace_bytes", C.byref(dims))
     else:
-        ws = _u8(lib.grb_hstu_layer_workspace_bytes_jagged(C.byref(dims), meta.T), dy.device)
+        ws = workspace(dy.device, "grb_hstu_layer_workspace_bytes_jagged", C.byref(dims), meta.T)
     deferred = _defer_for_call(_DEFER["on"] and sink is not None)
-    with torch.cuda.device(dy.device):
-        if meta.offsets is None:
-            check(lib.grb_hstu_layer_backward(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(dyc), ptr(saved), ptr(dx), C.byref(gstruct),
-                                              ptr(ws), stream_ptr(dy.device)))
-        else:
-            check(lib.grb_hstu_layer_backward_jagged(C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(meta.offsets), meta.T, ptr(dyc),
-                                                     ptr(saved), ptr(dx), C.byref(gstruct), ptr(ws), stream_ptr(dy.device)))
+    if meta.offsets is None:
+        call(dy.device, "grb_hstu_layer_backward", C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(dyc), ptr(saved), ptr(dx),
+             C.byref(gstruct), ptr(ws))
+    else:
+        call(dy.device, "grb_hstu_layer_backward_jagged", C.byref(dims), C.byref(pstruct), C.byref(seq), ptr(meta.offsets), meta.T,
+             ptr(dyc), ptr(saved), ptr(dx), C.byref(gstruct), ptr(ws))
     if deferred:
         _DEFER["keep"].append((ws, saved, dyc))     # still read by the deferred dW GEMM
     return dx, grads
@@ -294,7 +276,6 @@ class EmbedFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, ids, table, pos_table, scale, mask_pad_rows, p, seed, seed_dev, sink=None, offsets=None, max_len=None):
-        lib = _lib.load()
         require_cuda(ids, table)
         require_i64(ids)
         require_f32(table, pos_table)
@@ -308,20 +289,17 @@ class EmbedFn(torch.autograd.Function):
             x = torch.empty(T, D, dtype=torch.float32, device=ids.device)
             pad = torch.empty(T, dtype=torch.uint8, device=ids.device)
             positions = torch.empty(T, dtype=torch.int32, device=ids.device)
-            with torch.cuda.device(ids.device):
-                check(lib.grb_embed_forward_jagged(ptr(ids), ptr(table.detach()), ptr(pos_table.detach()), ptr(offsets), B, T, int(max_len), D,
-                                                   float(scale), int(mask_pad_rows), float(p), int(seed), ptr(seed_dev), ptr(x), ptr(pad),
-                                                   ptr(positions), stream_ptr(ids.device)))
+            call(ids.device, "grb_embed_forward_jagged", ptr(ids), ptr(table.detach()), ptr(pos_table.detach()), ptr(offsets), B, T,
+                 int(max_len), D, float(scale), int(mask_pad_rows), float(p), int(seed), ptr(seed_dev), ptr(x), ptr(pad), ptr(positions))
             ids = torch.where(positions >= 0, ids, 0)   # the idle rows' x does not depend on the table
             ctx.jagged = (offsets, B, T, int(max_len))
         else:
             B, L = ids.shape
             x = torch.empty(B, L, D, dtype=torch.float32, device=ids.device)
             pad = torch.empty(B, L, dtype=torch.uint8, device=ids.device)
-            with torch.cuda.device(ids.device):
-                check(lib.grb_embed_forward(ptr(ids), ptr(table.detach()), ptr(pos_table.detach()) if pos_table is not None else None,
-                                            ptr(x), ptr(pad), B, L, D, float(scale), int(mask_pad_rows), float(p), int(seed), ptr(seed_dev),
-                                            stream_ptr(ids.device)))
+            call(ids.device, "grb_embed_forward", ptr(ids), ptr(table.detach()),
+                 ptr(pos_table.detach()) if pos_table is not None else None, ptr(x), ptr(pad), B, L, D, float(scale), int(mask_pad_rows),
+                 float(p), int(seed), ptr(seed_dev))
         ctx.save_for_backward(ids)
         ctx.args = (table.shape, None if pos_table is None else pos_table.shape, scale, mask_pad_rows, p, seed, seed_dev)
         ctx.mark_non_differentiable(pad)
@@ -329,7 +307,6 @@ class EmbedFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dx, _dpad):
-        lib = _lib.load()
         (ids,) = ctx.saved_tensors
         tshape, pshape, scale, mask_pad_rows, p, seed, seed_dev = ctx.args
         D = tshape[1]
@@ -341,16 +318,14 @@ class EmbedFn(torch.autograd.Function):
             dpos = torch.zeros(pshape, dtype=torch.float32, device=dx.device) if pshape is not None else None
         order = torch.sort(ids.reshape(-1), stable=True).indices   # tokens grouped by id, in token order
         scratch = torch.empty(ids.numel(), D, dtype=torch.float32, device=dx.device)
-        with torch.cuda.device(dx.device):
-            if ctx.jagged is not None:
-                offsets, B, T, max_len = ctx.jagged
-                check(lib.grb_embed_backward_jagged(ptr(ids), ptr(order), ptr(dx), ptr(dtable), ptr(dpos), ptr(offsets), B, T, max_len, D,
-                                                    float(scale), int(mask_pad_rows), float(p), int(seed), ptr(seed_dev), ptr(scratch),
-                                                    stream_ptr(dx.device)))
-            else:
-                B, L = ids.shape
-                check(lib.grb_embed_backward(ptr(ids), ptr(order), ptr(dx), ptr(dtable), ptr(dpos), B, L, D, float(scale), int(mask_pad_rows),
-                                             float(p), int(seed), ptr(seed_dev), ptr(scratch), stream_ptr(dx.device)))
+        if ctx.jagged is not None:
+            offsets, B, T, max_len = ctx.jagged
+            call(dx.device, "grb_embed_backward_jagged", ptr(ids), ptr(order), ptr(dx), ptr(dtable), ptr(dpos), ptr(offsets), B, T, max_len,
+                 D, float(scale), int(mask_pad_rows), float(p), int(seed), ptr(seed_dev), ptr(scratch))
+        else:
+            B, L = ids.shape
+            call(dx.device, "grb_embed_backward", ptr(ids), ptr(order), ptr(dx), ptr(dtable), ptr(dpos), B, L, D, float(scale),
+                 int(mask_pad_rows), float(p), int(seed), ptr(seed_dev), ptr(scratch))
         if ctx.sink is not None:
             return (None,) * 11
         return None, dtable, dpos, None, None, None, None, None, None, None, None
@@ -377,8 +352,7 @@ def _head_loss_backward(ctx, dloss, n_inputs):
     if dx is None:
         return (None,) * n_inputs
     if ctx.direct:
-        with torch.cuda.device(dx.device):
-            check(_lib.load().grb_assert_unit_scalar(ptr(dloss.detach().float().contiguous()), stream_ptr(dx.device)))
+        call(dx.device, "grb_assert_unit_scalar", ptr(dloss.detach().float().contiguous()))
         return (dx,) + (None,) * (n_inputs - 1)
     if ctx.sink is not None:
         sg, sb, st = ctx.sink
@@ -401,7 +375,6 @@ class HeadLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, ln_g, ln_b, table, table_bf16, targets, eps, sink=None, unit_loss_grad=False):
-        lib = _lib.load()
         require_cuda(x, table, targets)
         require_i64(targets)
         require_f32(ln_g, ln_b, table)
@@ -411,12 +384,10 @@ class HeadLossFn(torch.autograd.Function):
         tg = targets.contiguous()
         dx, dg, db, dtable, direct = _head_grad_buffers(ctx, xc, ln_g, ln_b, table, sink, unit_loss_grad)
         loss = torch.empty((), dtype=torch.float32, device=x.device)   # zeroed on the device by the target-count kernel
-        ws = _u8(lib.grb_head_workspace_bytes(T, D, Cn), x.device)
+        ws = workspace(x.device, "grb_head_workspace_bytes", T, D, Cn)
         deferred = _defer_for_call(_DEFER["on"] and direct)
-        with torch.cuda.device(x.device):
-            check(lib.grb_head_loss_forward_backward(ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), ptr(tg),
-                                                     T, D, Cn, ptr(loss), ptr(dx), ptr(dtable), ptr(dg), ptr(db), ptr(ws),
-                                                     stream_ptr(x.device)))
+        call(x.device, "grb_head_loss_forward_backward", ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16),
+             ptr(tg), T, D, Cn, ptr(loss), ptr(dx), ptr(dtable), ptr(dg), ptr(db), ptr(ws))
         if deferred:
             _DEFER["keep"].append((ws, xc, tg))                   # xf, the shifts and the targets are still read by the deferred dE pass
         ctx.grads = (dx, dg, db, dtable)
@@ -430,7 +401,6 @@ class HeadLossFn(torch.autograd.Function):
 def head_sampled_loss_raw(x, ln_g, ln_b, table_bf16, targets, negatives, log_q, eps, grads=None):
     """grb_head_sampled_loss_forward_backward on x [T, D]: -> loss (0-dim fp32).  ``grads = (dx, dtable, dln_g, dln_b)``: dx is
     written, the other three are accumulated into; ``None``: loss only."""
-    lib = _lib.load()
     require_cuda(x, table_bf16, targets, negatives, log_q)
     require_i64(targets, negatives)
     require_f32(x, ln_g, ln_b, log_q)
@@ -446,15 +416,10 @@ def head_sampled_loss_raw(x, ln_g, ln_b, table_bf16, targets, negatives, log_q, 
     neg = negatives.contiguous()
     lq = log_q.detach().contiguous() if log_q is not None else None
     loss = torch.empty((), dtype=torch.float32, device=x.device)   # zeroed on the device by the target-count kernel
-    with torch.cuda.device(x.device):
-        nbytes = lib.grb_head_sampled_workspace_bytes(T, D, N)
-        if nbytes == 0:
-            check(-1)
-        ws = _u8(nbytes, x.device)
-        dx, dtable, dg, db = grads if grads is not None else (None,) * 4
-        check(lib.grb_head_sampled_loss_forward_backward(ptr(x), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), ptr(targets),
-                                                         ptr(neg), ptr(lq), T, D, Cn, N, ptr(loss), ptr(dx), ptr(dtable), ptr(dg), ptr(db), ptr(ws),
-                                                         stream_ptr(x.device)))
+    ws = workspace(x.device, "grb_head_sampled_workspace_bytes", T, D, N)
+    dx, dtable, dg, db = grads if grads is not None else (None,) * 4
+    call(x.device, "grb_head_sampled_loss_forward_backward", ptr(x), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16),
+         ptr(targets), ptr(neg), ptr(lq), T, D, Cn, N, ptr(loss), ptr(dx), ptr(dtable), ptr(dg), ptr(db), ptr(ws))
     return loss
 
 
@@ -481,16 +446,14 @@ class SampledHeadLossFn(torch.autograd.Function):
 
 def head_logits(x, ln_g, ln_b, table, table_bf16, eps) -> torch.Tensor:
     """fp32 logits [B, L, C] (no autograd - inference / API parity path)."""
-    lib = _lib.load()
     require_cuda(x, table)
     B, L, D = x.shape
     T, Cn = B * L, table.shape[0]
     xc = x.detach().contiguous().float()
     logits = torch.empty(B, L, Cn, dtype=torch.float32, device=x.device)
-    ws = _u8(lib.grb_head_workspace_bytes(T, D, Cn), x.device)
-    with torch.cuda.device(x.device):
-        check(lib.grb_head_logits(ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), T, D, Cn, ptr(logits), ptr(ws),
-                                  stream_ptr(x.device)))
+    ws = workspace(x.device, "grb_head_workspace_bytes", T, D, Cn)
+    call(x.device, "grb_head_logits", ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), T, D, Cn, ptr(logits),
+         ptr(ws))
     return logits
 
 
@@ -526,36 +489,31 @@ def check_exclude_arg(exclude: Optional[torch.Tensor], rows: int, device) -> Non
         raise ValueError(f"exclude holds at most {TOPK_MAX_EXCLUDE} ids per row, got {exclude.shape[1]}")
 
 
-def _sweep_inputs(x, table_bf16, exclude, check_rows, workspace_bytes):
+def _sweep_inputs(x, table_bf16, exclude, check_rows, query, *k):
     """What head_topk and head_rank_metrics share: x must be [R, D], and ``check_rows(R)`` runs the head's own argument checks.
-    -> (x as contiguous fp32, exclude or None when it holds no ids, E, a workspace of ``workspace_bytes(R, D, C, E)`` bytes)"""
+    -> (x as contiguous fp32, exclude or None when it holds no ids, E, the workspace of size query ``query(R, D, C, *k, E)``)"""
     if x.dim() != 2:
         raise ValueError(f"x must be [R, D], got {tuple(x.shape)}")
     R, D = x.shape
     check_rows(R)
     ex = exclude.contiguous() if exclude is not None and exclude.shape[1] > 0 else None
     E = ex.shape[1] if ex is not None else 0
-    nbytes = workspace_bytes(R, D, table_bf16.shape[0], E)
-    if nbytes == 0:
-        raise _lib.GrbError(_lib.load().grb_last_error().decode())
-    return x.detach().contiguous().float(), ex, E, _u8(nbytes, x.device)
+    return x.detach().contiguous().float(), ex, E, workspace(x.device, query, R, D, table_bf16.shape[0], *k, E)
 
 
 def head_topk(x, ln_g, ln_b, table_bf16, eps, k: int, exclude: Optional[torch.Tensor] = None) -> TopItems:
     """The ``k`` best items of every row of ``x`` [R, D] under the tied head, without forming the logits (grb_head_topk): scores are
     bit-identical to ``head_logits`` of the same rows; item 0 and the row's ``exclude`` ids ([R, E] int64, any order) never appear;
     ties go to the lower item id.  Inference only (no autograd)."""
-    lib = _lib.load()
     require_cuda(x, table_bf16)
     xc, ex, E, ws = _sweep_inputs(x, table_bf16, exclude, lambda R: check_topk_args(k, exclude, R, x.device),
-                                  lambda R, D, Cn, E: lib.grb_head_topk_workspace_bytes(R, D, Cn, k, E))
+                                  "grb_head_topk_workspace_bytes", k)
     R, D = x.shape
     Cn = table_bf16.shape[0]
     scores = torch.empty(R, k, dtype=torch.float32, device=x.device)
     items = torch.empty(R, k, dtype=torch.int64, device=x.device)
-    with torch.cuda.device(x.device):
-        check(lib.grb_head_topk(ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), R, D, Cn, k, ptr(ex), E,
-                                ptr(scores), ptr(items), ptr(ws), stream_ptr(x.device)))
+    call(x.device, "grb_head_topk", ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), R, D, Cn, k, ptr(ex), E,
+         ptr(scores), ptr(items), ptr(ws))
     return TopItems(scores, items)
 
 
@@ -574,17 +532,15 @@ def head_candidates(x, ln_g, ln_b, table_bf16, eps, k: int, exclude: Optional[to
     the tied head, best first, without forming the logits.  Same rules: scores bit-identical to ``head_logits``, item 0 and the
     row's ``exclude`` ids never appear, ties go to the lower item id, (-inf, 0) where no eligible item is left.  Memory grows with
     R * k and R * E, not with the catalog.  Inference only (no autograd)."""
-    lib = _lib.load()
     require_cuda(x, table_bf16)
     xc, ex, E, ws = _sweep_inputs(x, table_bf16, exclude, lambda R: check_candidates_args(k, exclude, R, x.device),
-                                  lambda R, D, Cn, E: lib.grb_head_candidates_workspace_bytes(R, D, Cn, k, E))
+                                  "grb_head_candidates_workspace_bytes", k)
     R, D = x.shape
     Cn = table_bf16.shape[0]
     scores = torch.empty(R, k, dtype=torch.float32, device=x.device)
     items = torch.empty(R, k, dtype=torch.int64, device=x.device)
-    with torch.cuda.device(x.device):
-        check(lib.grb_head_candidates(ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), R, D, Cn, k, ptr(ex),
-                                      E, ptr(scores), ptr(items), ptr(ws), stream_ptr(x.device)))
+    call(x.device, "grb_head_candidates", ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), R, D, Cn, k,
+         ptr(ex), E, ptr(scores), ptr(items), ptr(ws))
     return TopItems(scores, items)
 
 
@@ -599,8 +555,7 @@ def eval_rank_metrics(logits_last: torch.Tensor, targets: torch.Tensor, metrics:
     if metrics is None:
         metrics = torch.zeros(6, dtype=torch.float32, device=lg.device)
     ranks = torch.empty(B, dtype=torch.int32, device=lg.device) if want_ranks else None
-    with torch.cuda.device(lg.device):
-        check(_lib.load().grb_eval_rank_metrics(ptr(lg), ptr(targets.contiguous()), B, Cn, ptr(metrics), ptr(ranks), stream_ptr(lg.device)))
+    call(lg.device, "grb_eval_rank_metrics", ptr(lg), ptr(targets.contiguous()), B, Cn, ptr(metrics), ptr(ranks))
     return (metrics, ranks) if want_ranks else metrics
 
 
@@ -612,7 +567,6 @@ def head_rank_metrics(x, ln_g, ln_b, table_bf16, eps, targets: torch.Tensor, met
     ``head_logits``, so the ranks equal ``eval_rank_metrics``' exactly.  ``exclude`` ([R, E] int64, any order, E <= 16384) removes
     ids from the count; a row whose target is 0, out of 1..C-1 or excluded gets rank 0 and adds nothing.  Memory grows with R and
     R * E, not with the catalog.  Inference only (no autograd)."""
-    lib = _lib.load()
     require_cuda(x, table_bf16, targets)
     require_i64(targets)
 
@@ -621,15 +575,14 @@ def head_rank_metrics(x, ln_g, ln_b, table_bf16, eps, targets: torch.Tensor, met
             raise ValueError(f"targets must be [{R}] (one per row of x), got {tuple(targets.shape)}")
         check_exclude_arg(exclude, R, x.device)
 
-    xc, ex, E, ws = _sweep_inputs(x, table_bf16, exclude, check_rows, lib.grb_head_rank_workspace_bytes)
+    xc, ex, E, ws = _sweep_inputs(x, table_bf16, exclude, check_rows, "grb_head_rank_workspace_bytes")
     R, D = x.shape
     Cn = table_bf16.shape[0]
     if metrics is None:
         metrics = torch.zeros(6, dtype=torch.float32, device=x.device)
     ranks = torch.empty(R, dtype=torch.int32, device=x.device) if want_ranks else None
-    with torch.cuda.device(x.device):
-        check(lib.grb_head_rank(ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), R, D, Cn,
-                                ptr(targets.contiguous()), ptr(ex), E, ptr(metrics), ptr(ranks), ptr(ws), stream_ptr(x.device)))
+    call(x.device, "grb_head_rank", ptr(xc), ptr(ln_g.detach()), ptr(ln_b.detach()), float(eps), ptr(table_bf16), R, D, Cn,
+         ptr(targets.contiguous()), ptr(ex), E, ptr(metrics), ptr(ranks), ptr(ws))
     return (metrics, ranks) if want_ranks else metrics
 
 
@@ -637,7 +590,6 @@ def head_rank_metrics(x, ln_g, ln_b, table_bf16, eps, targets: torch.Tensor, met
 def hstu_attention_fwd(P: torch.Tensor, meta: SeqMeta, H: int, pos_table: torch.Tensor, time_table: Optional[torch.Tensor],
                        ntime: int = 64) -> torch.Tensor:
     """P [B, L, 4D] bf16 = silu(x Wp^T + b) = [U | V | Q | K]  ->  O [B, L, D] bf16 (hstu.py:244-267)."""
-    lib = _lib.load()
     require_cuda(P)
     B, L, D4 = P.shape
     D = D4 // 4
@@ -645,15 +597,13 @@ def hstu_attention_fwd(P: torch.Tensor, meta: SeqMeta, H: int, pos_table: torch.
     dims = _dims(B, L, D, H, pos_table.shape[0], ntime if has_time else 0, 0.0, 0, None, 0)
     O = torch.empty(B, L, D, dtype=torch.bfloat16, device=P.device)
     seq = meta.struct()
-    with torch.cuda.device(P.device):
-        check(lib.grb_hstu_attention_forward(C.byref(dims), ptr(pos_table), ptr(time_table) if has_time else None, C.byref(seq), ptr(P), ptr(O),
-                                             stream_ptr(P.device)))
+    call(P.device, "grb_hstu_attention_forward", C.byref(dims), ptr(pos_table), ptr(time_table) if has_time else None, C.byref(seq),
+         ptr(P), ptr(O))
     return O
 
 
 def hstu_attention_bwd(P, zp, dO, meta: SeqMeta, H: int, pos_table, time_table, ntime: int = 64):
     """-> dzp [B, L, 4D] bf16 (columns V, Q, K written; U untouched = 0), dpos_table, dtime_table (fp32)."""
-    lib = _lib.load()
     B, L, D4 = P.shape
     D = D4 // 4
     has_time = time_table is not None and meta.timestamps is not None
@@ -661,11 +611,10 @@ def hstu_attention_bwd(P, zp, dO, meta: SeqMeta, H: int, pos_table, time_table, 
     dzp = torch.zeros(B, L, D4, dtype=torch.bfloat16, device=P.device)
     dpos = torch.zeros_like(pos_table, dtype=torch.float32)
     dtime = torch.zeros_like(time_table, dtype=torch.float32) if has_time else None
-    scratch = _u8(lib.grb_hstu_attention_scratch_bytes(C.byref(dims)), P.device)
+    scratch = workspace(P.device, "grb_hstu_attention_scratch_bytes", C.byref(dims))
     seq = meta.struct()
-    with torch.cuda.device(P.device):
-        check(lib.grb_hstu_attention_backward(C.byref(dims), ptr(pos_table), ptr(time_table) if has_time else None, C.byref(seq), ptr(P), ptr(zp),
-                                              ptr(dO), ptr(dzp), ptr(dpos), ptr(dtime), ptr(scratch), stream_ptr(P.device)))
+    call(P.device, "grb_hstu_attention_backward", C.byref(dims), ptr(pos_table), ptr(time_table) if has_time else None, C.byref(seq),
+         ptr(P), ptr(zp), ptr(dO), ptr(dzp), ptr(dpos), ptr(dtime), ptr(scratch))
     return dzp, dpos, dtime
 
 
@@ -680,20 +629,17 @@ def hstu_cache_append(cache: _lib.HstuCache, input_ids: torch.Tensor, timestamps
     dev = input_ids.device
     ids = input_ids.contiguous()
     ts = timestamps.contiguous() if timestamps is not None else None
-    lib = _lib.load()
     if offsets is not None:
         B, T = offsets.numel() - 1, ids.numel()
         positions = torch.empty(T, dtype=torch.int32, device=dev)
         last_row = torch.empty(B, dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            check(lib.grb_hstu_cache_append_jagged(C.byref(cache), ptr(ids), ptr(ts), ptr(offsets.contiguous()), B, T, int(max_len),
-                                                   ptr(positions), ptr(last_row), stream_ptr(dev)))
+        call(dev, "grb_hstu_cache_append_jagged", C.byref(cache), ptr(ids), ptr(ts), ptr(offsets.contiguous()), B, T, int(max_len),
+             ptr(positions), ptr(last_row))
         return positions, last_row
     B, n = input_ids.shape
     positions = torch.empty(B, n, dtype=torch.int32, device=dev)
     last_row = torch.empty(B, dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        check(lib.grb_hstu_cache_append(C.byref(cache), ptr(ids), ptr(ts), n, ptr(positions), ptr(last_row), stream_ptr(dev)))
+    call(dev, "grb_hstu_cache_append", C.byref(cache), ptr(ids), ptr(ts), n, ptr(positions), ptr(last_row))
     return positions, last_row
 
 
@@ -705,7 +651,6 @@ def hstu_layer_extend(x: torch.Tensor, cache, layer: int, positions: torch.Tenso
     (grb_hstu_layer_extend) or an ``HstuPool`` with ``users`` [B] int64 on the device (grb_hstu_layer_extend_paged).  ``params`` in
     PARAM_ORDER (time_table None or ntime = 0: no temporal term), ``bf16w`` the three bf16 weight mirrors.  With ``offsets``
     ([B+1] int64 on the device) and ``max_len`` the chunk is packed: x [T, D] -> y [T, D] (the ``_jagged`` entry points)."""
-    lib = _lib.load()
     require_cuda(x)
     require_f32(x)
     xc = x.contiguous()
@@ -718,28 +663,26 @@ def hstu_layer_extend(x: torch.Tensor, cache, layer: int, positions: torch.Tenso
     dims = _dims(B, n, D, H, npos, ntime if has_time else 0, 0.0, 0, None, layer)
     pstruct = _layer_param_struct(params, bf16w, has_time)
     paged = isinstance(cache, _lib.HstuPool)
-    if offsets is not None:
-        nbytes = (lib.grb_hstu_layer_extend_paged_workspace_bytes_jagged(C.byref(dims), C.byref(cache), T) if paged else
-                  lib.grb_hstu_layer_extend_workspace_bytes_jagged(C.byref(dims), cache.capacity, T))
+    dev = x.device
+    if offsets is not None and paged:
+        ws = workspace(dev, "grb_hstu_layer_extend_paged_workspace_bytes_jagged", C.byref(dims), C.byref(cache), T)
+    elif offsets is not None:
+        ws = workspace(dev, "grb_hstu_layer_extend_workspace_bytes_jagged", C.byref(dims), cache.capacity, T)
     elif paged:
-        nbytes = lib.grb_hstu_layer_extend_paged_workspace_bytes(C.byref(dims), C.byref(cache))
+        ws = workspace(dev, "grb_hstu_layer_extend_paged_workspace_bytes", C.byref(dims), C.byref(cache))
     else:
-        nbytes = lib.grb_hstu_layer_extend_workspace_bytes(C.byref(dims), cache.capacity)
-    if nbytes == 0:
-        raise _lib.GrbError(lib.grb_last_error().decode())
-    ws = _u8(nbytes, x.device)
+        ws = workspace(dev, "grb_hstu_layer_extend_workspace_bytes", C.byref(dims), cache.capacity)
     y = torch.empty_like(xc)
-    tail = (ptr(positions), ptr(pos_bucket), int(pos_bucket0), ptr(time_thr), ptr(xc), ptr(y), ptr(ws), stream_ptr(x.device))
-    with torch.cuda.device(x.device):
-        if offsets is not None and paged:
-            check(lib.grb_hstu_layer_extend_paged_jagged(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(users), ptr(offsets),
-                                                         T, *tail))
-        elif offsets is not None:
-            check(lib.grb_hstu_layer_extend_jagged(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(offsets), T, *tail))
-        elif paged:
-            check(lib.grb_hstu_layer_extend_paged(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, ptr(users), *tail))
-        else:
-            check(lib.grb_hstu_layer_extend(C.byref(dims), C.byref(pstruct), C.byref(cache), layer, *tail))
+    head = (C.byref(dims), C.byref(pstruct), C.byref(cache), layer)
+    tail = (ptr(positions), ptr(pos_bucket), int(pos_bucket0), ptr(time_thr), ptr(xc), ptr(y), ptr(ws))
+    if offsets is not None and paged:
+        call(dev, "grb_hstu_layer_extend_paged_jagged", *head, ptr(users), ptr(offsets), T, *tail)
+    elif offsets is not None:
+        call(dev, "grb_hstu_layer_extend_jagged", *head, ptr(offsets), T, *tail)
+    elif paged:
+        call(dev, "grb_hstu_layer_extend_paged", *head, ptr(users), *tail)
+    else:
+        call(dev, "grb_hstu_layer_extend", *head, *tail)
     return y
 
 
@@ -758,14 +701,12 @@ def hstu_pool_append(pool: _lib.HstuPool, users: torch.Tensor, input_ids: torch.
     positions = torch.empty(ids.shape, dtype=torch.int32, device=dev)
     last_row = torch.empty(B, dtype=torch.int32, device=dev)
     room = torch.empty(B, dtype=torch.int32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        if offsets is not None:
-            check(lib.grb_hstu_pool_append_jagged(C.byref(pool), ptr(users.contiguous()), B, ptr(ids), ptr(ts), ptr(offsets.contiguous()),
-                                                  ids.numel(), int(max_len), ptr(positions), ptr(last_row), ptr(room), stream_ptr(dev)))
-        else:
-            check(lib.grb_hstu_pool_append(C.byref(pool), ptr(users.contiguous()), B, ptr(ids), ptr(ts), ids.shape[1], ptr(positions),
-                                           ptr(last_row), ptr(room), stream_ptr(dev)))
+    if offsets is not None:
+        call(dev, "grb_hstu_pool_append_jagged", C.byref(pool), ptr(users.contiguous()), B, ptr(ids), ptr(ts), ptr(offsets.contiguous()),
+             ids.numel(), int(max_len), ptr(positions), ptr(last_row), ptr(room))
+    else:
+        call(dev, "grb_hstu_pool_append", C.byref(pool), ptr(users.contiguous()), B, ptr(ids), ptr(ts), ids.shape[1], ptr(positions),
+             ptr(last_row), ptr(room))
     return positions, last_row, room
 
 
@@ -774,31 +715,26 @@ def hstu_pool_release(pool: _lib.HstuPool, users: torch.Tensor, last_hidden: Opt
     require_cuda(users, last_hidden)
     require_i64(users)
     D = last_hidden.shape[1] if last_hidden is not None else 0
-    with torch.cuda.device(users.device):
-        check(_lib.load().grb_hstu_pool_release(C.byref(pool), ptr(users.contiguous()), users.numel(), ptr(last_hidden), D,
-                                                stream_ptr(users.device)))
+    call(users.device, "grb_hstu_pool_release", C.byref(pool), ptr(users.contiguous()), users.numel(), ptr(last_hidden), D)
 
 
 # ------------------------------------------------------------------------------------------------ SASRec pieces
 def layernorm_fwd(x, g, b, eps, want_bf16=True, want_f32=False):
-    lib = _lib.load()
     T, D = x.numel() // x.shape[-1], x.shape[-1]
     yb = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if want_bf16 else None
     yf = torch.empty(x.shape, dtype=torch.float32, device=x.device) if want_f32 else None
     st = torch.empty(T, 2, dtype=torch.float32, device=x.device)
-    check(lib.grb_layernorm_forward(ptr(x), ptr(g), ptr(b), float(eps), T, D, ptr(yb), ptr(yf), ptr(st), stream_ptr(x.device)))
+    call(x.device, "grb_layernorm_forward", ptr(x), ptr(g), ptr(b), float(eps), T, D, ptr(yb), ptr(yf), ptr(st))
     return yb, yf, st
 
 
 def layernorm_bwd(dy, x, st, g, residual=None):
-    lib = _lib.load()
     T, D = x.numel() // x.shape[-1], x.shape[-1]
     dx = torch.empty_like(x)
     dg = torch.zeros_like(g)
     db = torch.zeros_like(g)
-    ws = _u8(lib.grb_layernorm_backward_workspace_bytes(T, D), x.device)
-    check(lib.grb_layernorm_backward(ptr(dy), ptr(x), ptr(st), ptr(g), ptr(residual), T, D, ptr(dx), ptr(dg), ptr(db), ptr(ws),
-                                     stream_ptr(x.device)))
+    ws = workspace(x.device, "grb_layernorm_backward_workspace_bytes", T, D)
+    call(x.device, "grb_layernorm_backward", ptr(dy), ptr(x), ptr(st), ptr(g), ptr(residual), T, D, ptr(dx), ptr(dg), ptr(db), ptr(ws))
     return dx, dg, db
 
 
@@ -808,55 +744,50 @@ def rmsnorm_fwd(x, w, eps, want_bf16=True, want_f32=False):
     yb = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if want_bf16 else None
     yf = torch.empty(x.shape, dtype=torch.float32, device=x.device) if want_f32 else None
     rstd = torch.empty(T, dtype=torch.float32, device=x.device)
-    check(_lib.load().grb_rmsnorm_forward(ptr(x), ptr(w), float(eps), T, D, ptr(yb), ptr(yf), ptr(rstd), stream_ptr(x.device)))
+    call(x.device, "grb_rmsnorm_forward", ptr(x), ptr(w), float(eps), T, D, ptr(yb), ptr(yf), ptr(rstd))
     return yb, yf, rstd
 
 
 def rmsnorm_bwd(dy, x, rstd, w, residual=None):
     """-> (dx fp32 (+ residual), dw fp32), dw summed in a fixed order"""
-    lib = _lib.load()
     T, D = x.numel() // x.shape[-1], x.shape[-1]
     dx = torch.empty_like(x)
     dw = torch.zeros_like(w)
-    ws = _u8(lib.grb_rmsnorm_backward_workspace_bytes(T, D), x.device)
-    check(lib.grb_rmsnorm_backward(ptr(dy), ptr(x), ptr(rstd), ptr(w), ptr(residual), T, D, ptr(dx), ptr(dw), ptr(ws), stream_ptr(x.device)))
+    ws = workspace(x.device, "grb_rmsnorm_backward_workspace_bytes", T, D)
+    call(x.device, "grb_rmsnorm_backward", ptr(dy), ptr(x), ptr(rstd), ptr(w), ptr(residual), T, D, ptr(dx), ptr(dw), ptr(ws))
     return dx, dw
 
 
 def linear_fwd(xb, wb, bias, act, p=0.0, seed=0, seed_dev=None, site=0, out=None):
     """z = xb @ wb^T + bias (bf16) ; act: 0 none, 1 silu, 2 relu -> returns (z, act(z) with dropout); out: a contiguous bf16 tensor of
     z's shape that receives z"""
-    lib = _lib.load()
     T, K = xb.numel() // xb.shape[-1], xb.shape[-1]
     N = wb.shape[0]
     z = torch.empty(*xb.shape[:-1], N, dtype=torch.bfloat16, device=xb.device) if out is None else out
     a = torch.empty_like(z) if act else None
-    check(lib.grb_linear_forward(ptr(xb), ptr(wb), ptr(bias), T, N, K, act, ptr(z), ptr(a), float(p), int(seed), ptr(seed_dev), site,
-                                 stream_ptr(xb.device)))
+    call(xb.device, "grb_linear_forward", ptr(xb), ptr(wb), ptr(bias), T, N, K, act, ptr(z), ptr(a), float(p), int(seed), ptr(seed_dev),
+         site)
     return z, a
 
 
 def linear_residual_fwd(xb, wb, bias, residual, row_scale=None, p=0.0, seed=0, seed_dev=None, site=0):
-    lib = _lib.load()
     T, K = xb.numel() // xb.shape[-1], xb.shape[-1]
     N = wb.shape[0]
     y = torch.empty(*xb.shape[:-1], N, dtype=torch.float32, device=xb.device)
-    check(lib.grb_linear_residual_forward(ptr(xb), ptr(wb), ptr(bias), ptr(residual), ptr(row_scale), T, N, K, ptr(y), float(p), int(seed),
-                                          ptr(seed_dev), site, stream_ptr(xb.device)))
+    call(xb.device, "grb_linear_residual_forward", ptr(xb), ptr(wb), ptr(bias), ptr(residual), ptr(row_scale), T, N, K, ptr(y), float(p),
+         int(seed), ptr(seed_dev), site)
     return y
 
 
 def linear_bwd(dyb, wb, xb, need_dx=True, dx_residual=None, need_dw=True):
     """dyb [T,N] bf16 ; wb [N,K] bf16 ; xb [T,K] bf16 -> dx fp32 [T,K] (+ residual), dw fp32 [N,K], db fp32 [N]"""
-    lib = _lib.load()
     N, K = wb.shape
     T = dyb.numel() // N
     dx = torch.empty(*dyb.shape[:-1], K, dtype=torch.float32, device=dyb.device) if need_dx else None
     dw = torch.zeros(N, K, dtype=torch.float32, device=dyb.device) if need_dw else None
     db = torch.zeros(N, dtype=torch.float32, device=dyb.device) if need_dw else None
-    ws = _u8(lib.grb_linear_backward_workspace_bytes(T, N, K), dyb.device) if need_dw else None
-    check(lib.grb_linear_backward(ptr(dyb), ptr(wb), ptr(xb), T, N, K, ptr(dx), ptr(dx_residual), ptr(dw), ptr(db), ptr(ws),
-                                  stream_ptr(dyb.device)))
+    ws = workspace(dyb.device, "grb_linear_backward_workspace_bytes", T, N, K) if need_dw else None
+    call(dyb.device, "grb_linear_backward", ptr(dyb), ptr(wb), ptr(xb), T, N, K, ptr(dx), ptr(dx_residual), ptr(dw), ptr(db), ptr(ws))
     return dx, dw, db
 
 
@@ -870,32 +801,30 @@ def _sasrec_dims(q, H, p, seed, seed_dev, layer, offsets, max_len):
 def sasrec_attention_fwd(q, k, v, pad, H, p=0.0, seed=0, seed_dev=None, layer=0, offsets=None, max_len=None):
     """q, k, v [B, L, D] bf16, pad [B, L] -> (out [B, L, D] bf16, lse [B, H, L]).  With ``offsets`` ([B+1] int64 on the device) and
     ``max_len`` the batch is packed (grb_sasrec_attention_forward_jagged): q, k, v, out [T, D], pad [T], lse [H, T]."""
-    lib = _lib.load()
     dims = _sasrec_dims(q, H, p, seed, seed_dev, layer, offsets, max_len)
     out = torch.empty_like(q)
     if offsets is None:
         B, L, D = q.shape
         lse = torch.empty(B, H, L, dtype=torch.float32, device=q.device)
-        check(lib.grb_sasrec_attention_forward(C.byref(dims), ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out), ptr(lse), stream_ptr(q.device)))
+        call(q.device, "grb_sasrec_attention_forward", C.byref(dims), ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out), ptr(lse))
     else:
         T = q.shape[0]
         lse = torch.empty(H, T, dtype=torch.float32, device=q.device)
-        check(lib.grb_sasrec_attention_forward_jagged(C.byref(dims), ptr(offsets), T, ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out), ptr(lse),
-                                                      stream_ptr(q.device)))
+        call(q.device, "grb_sasrec_attention_forward_jagged", C.byref(dims), ptr(offsets), T, ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out),
+             ptr(lse))
     return out, lse
 
 
 def sasrec_attention_bwd(q, k, v, pad, out, lse, dout, H, p=0.0, seed=0, seed_dev=None, layer=0, offsets=None, max_len=None):
     """The backward of ``sasrec_attention_fwd`` -> (dq, dk, dv) shaped like q; packed with ``offsets`` and ``max_len``."""
-    lib = _lib.load()
     dims = _sasrec_dims(q, H, p, seed, seed_dev, layer, offsets, max_len)
     dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
     if offsets is None:
-        check(lib.grb_sasrec_attention_backward(C.byref(dims), ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out), ptr(lse), ptr(dout), ptr(dq),
-                                                ptr(dk), ptr(dv), stream_ptr(q.device)))
+        call(q.device, "grb_sasrec_attention_backward", C.byref(dims), ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out), ptr(lse), ptr(dout),
+             ptr(dq), ptr(dk), ptr(dv))
     else:
-        check(lib.grb_sasrec_attention_backward_jagged(C.byref(dims), ptr(offsets), q.shape[0], ptr(q), ptr(k), ptr(v), ptr(pad), ptr(out),
-                                                       ptr(lse), ptr(dout), ptr(dq), ptr(dk), ptr(dv), stream_ptr(q.device)))
+        call(q.device, "grb_sasrec_attention_backward_jagged", C.byref(dims), ptr(offsets), q.shape[0], ptr(q), ptr(k), ptr(v), ptr(pad),
+             ptr(out), ptr(lse), ptr(dout), ptr(dq), ptr(dk), ptr(dv))
     return dq, dk, dv
 
 
@@ -904,8 +833,7 @@ def linear_dact_bwd(dyb, wb, z, act, p=0.0, seed=0, seed_dev=None, site=0):
     N, K = wb.shape
     T = dyb.numel() // N
     g = torch.empty_like(z)
-    check(_lib.load().grb_linear_dact_backward(ptr(dyb), ptr(wb), ptr(z), T, N, K, act, float(p), int(seed), ptr(seed_dev), site, ptr(g),
-                                               stream_ptr(dyb.device)))
+    call(dyb.device, "grb_linear_dact_backward", ptr(dyb), ptr(wb), ptr(z), T, N, K, act, float(p), int(seed), ptr(seed_dev), site, ptr(g))
     return g
 
 
@@ -914,15 +842,13 @@ def cast_rows_bf16(x, row_scale=None, p=0.0, seed=0, seed_dev=None, site=0):
     D = x.shape[-1]
     T = x.numel() // D
     out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    check(_lib.load().grb_cast_rows_f32_to_bf16(ptr(x), ptr(out), T, D, ptr(row_scale), float(p), int(seed), ptr(seed_dev), site,
-                                                stream_ptr(x.device)))
+    call(x.device, "grb_cast_rows_f32_to_bf16", ptr(x), ptr(out), T, D, ptr(row_scale), float(p), int(seed), ptr(seed_dev), site)
     return out
 
 
 # ------------------------------------------------------------------------------------------------ RQ-VAE
 def rq_residual_argmin(x: torch.Tensor, codebooks: torch.Tensor, commitment: float = 0.25, want_aux: bool = True):
     """x [N, D] fp32, codebooks [levels, K, D] fp32 -> ids [N, levels] int64 (+ emb, res [N, D, levels], loss [N])."""
-    lib = _lib.load()
     require_cuda(x, codebooks)
     x = x.detach().contiguous().float()
     cb = codebooks.detach().contiguous().float()
@@ -936,16 +862,14 @@ def rq_residual_argmin(x: torch.Tensor, codebooks: torch.Tensor, commitment: flo
     loss = torch.empty(N, dtype=torch.float32, device=x.device) if want_aux else None
     if N == 0:
         return ids, emb, res, loss
-    with torch.cuda.device(x.device):
-        check(lib.grb_rq_residual_argmin(ptr(x), ptr(cb), N, D, K, levels, float(commitment), ptr(ids), ptr(emb), ptr(res), ptr(loss), None,
-                                         stream_ptr(x.device)))
+    call(x.device, "grb_rq_residual_argmin", ptr(x), ptr(cb), N, D, K, levels, float(commitment), ptr(ids), ptr(emb), ptr(res), ptr(loss),
+         None)
     return ids, emb, res, loss
 
 
 def rq_sinkhorn(dist: torch.Tensor, eps: float = 0.003, iters: int = 100):
     """Sinkhorn-Knopp hard assignment of the SINKHORN estimator (csrc/rq_sinkhorn.cuh): dist [B, K] fp32, 2 <= K <= 256 ->
     ids [B] int64, u [B] and v [K] fp64 (the final scalings; P = u K v)."""
-    lib = _lib.load()
     require_cuda(dist)
     require_f32(dist)
     if dist.dim() != 2:
@@ -955,9 +879,8 @@ def rq_sinkhorn(dist: torch.Tensor, eps: float = 0.003, iters: int = 100):
     ids = torch.empty(B, dtype=torch.int64, device=dist.device)
     u = torch.empty(B, dtype=torch.float64, device=dist.device)
     v = torch.empty(K, dtype=torch.float64, device=dist.device)
-    ws = _u8(lib.grb_rq_sinkhorn_workspace_bytes(B, K), dist.device)
-    with torch.cuda.device(dist.device):
-        check(lib.grb_rq_sinkhorn(ptr(dist), B, K, float(eps), int(iters), ptr(ids), ptr(u), ptr(v), ptr(ws), stream_ptr(dist.device)))
+    ws = workspace(dist.device, "grb_rq_sinkhorn_workspace_bytes", B, K, allow_empty=B == 0)     # B = 0: nothing to do, no scratch
+    call(dist.device, "grb_rq_sinkhorn", ptr(dist), B, K, float(eps), int(iters), ptr(ids), ptr(u), ptr(v), ptr(ws))
     return ids, u, v
 
 
@@ -973,9 +896,7 @@ def kmeans_update(x: torch.Tensor, assign: torch.Tensor, centroids: torch.Tensor
     B, D = x.shape
     k = centroids.shape[0]
     stats = torch.empty(2, k, dtype=torch.int32, device=x.device)
-    with torch.cuda.device(x.device):
-        check(_lib.load().grb_kmeans_update(ptr(x), ptr(assign.contiguous()), B, D, k, ptr(centroids), ptr(stats[0]), ptr(stats[1]),
-                                            stream_ptr(x.device)))
+    call(x.device, "grb_kmeans_update", ptr(x), ptr(assign.contiguous()), B, D, k, ptr(centroids), ptr(stats[0]), ptr(stats[1]))
     return stats
 
 
@@ -987,8 +908,7 @@ def split3(x: torch.Tensor, operand: int) -> torch.Tensor:
     x = x.detach().contiguous()
     rows, K = x.numel() // x.shape[-1], x.shape[-1]
     out = torch.empty(*x.shape[:-1], 6 * K, dtype=torch.bfloat16, device=x.device)
-    with torch.cuda.device(x.device):
-        check(_lib.load().grb_split3_f32_to_bf16(ptr(x), ptr(out), rows, K, operand, stream_ptr(x.device)))
+    call(x.device, "grb_split3_f32_to_bf16", ptr(x), ptr(out), rows, K, operand)
     return out
 
 
@@ -997,8 +917,7 @@ def linear_f32x3(x_split: torch.Tensor, w_split: torch.Tensor, act: int = 0) -> 
     K6 = x_split.shape[-1]
     T, N = x_split.numel() // K6, w_split.shape[0]
     y = torch.empty(*x_split.shape[:-1], N, dtype=torch.float32, device=x_split.device)
-    with torch.cuda.device(x_split.device):
-        check(_lib.load().grb_linear_f32x3_forward(ptr(x_split), ptr(w_split), T, N, K6 // 6, act, ptr(y), stream_ptr(x_split.device)))
+    call(x_split.device, "grb_linear_f32x3_forward", ptr(x_split), ptr(w_split), T, N, K6 // 6, act, ptr(y))
     return y
 
 
@@ -1011,9 +930,8 @@ def linear_f32x3_bias(x_split: torch.Tensor, w_split: torch.Tensor, bias: Option
     if residual is not None and ldy != N:
         raise _lib.GrbError("genrec_b200 error -1: residual needs N % 4 == 0")
     y = torch.empty(*x_split.shape[:-1], ldy, dtype=torch.float32, device=x_split.device)
-    with torch.cuda.device(x_split.device):
-        check(_lib.load().grb_linear_f32x3_bias_forward(ptr(x_split), ptr(w_split), ptr(bias), ptr(residual), T, N, K6 // 6, act, ptr(y), ldy,
-                                                        stream_ptr(x_split.device)))
+    call(x_split.device, "grb_linear_f32x3_bias_forward", ptr(x_split), ptr(w_split), ptr(bias), ptr(residual), T, N, K6 // 6, act, ptr(y),
+         ldy)
     return y[..., :N] if ldy != N else y
 
 
@@ -1022,9 +940,8 @@ def layernorm_f32(x: torch.Tensor, g: torch.Tensor, b: torch.Tensor, eps: float)
     require_f32(x, g, b)
     x = x.detach().contiguous()
     y = torch.empty_like(x)
-    with torch.cuda.device(x.device):
-        check(_lib.load().grb_layernorm_f32_forward(ptr(x), ptr(g.detach()), ptr(b.detach()), float(eps), x.numel() // x.shape[-1], x.shape[-1],
-                                                    ptr(y), stream_ptr(x.device)))
+    call(x.device, "grb_layernorm_f32_forward", ptr(x), ptr(g.detach()), ptr(b.detach()), float(eps), x.numel() // x.shape[-1], x.shape[-1],
+         ptr(y))
     return y
 
 
@@ -1033,7 +950,6 @@ def hstu_layer_forward_f32(x: torch.Tensor, meta: SeqMeta, H: int, npos: int, nt
     matrices pre-split by split3(w, 1); ``params`` in PARAM_ORDER.  Forward only."""
     require_cuda(x)
     require_f32(x)
-    lib = _lib.load()
     B, L, D = x.shape
     xc = x.detach().contiguous()
     (_, proj_b, pos_t, time_t, ln1_g, ln1_b, _, ffn1_b, _, ffn2_b, ln2_g, ln2_b) = params
@@ -1043,17 +959,15 @@ def hstu_layer_forward_f32(x: torch.Tensor, meta: SeqMeta, H: int, npos: int, nt
     p = _lib.HstuLayerParamsF32(ptr(split_w["proj_w"]), ptr(proj_b.detach()), ptr(pos_t.detach()), ptr(time_t.detach()) if time_t is not None else None,
                                 ptr(ln1_g.detach()), ptr(ln1_b.detach()), ptr(split_w["ffn1_w"]), ptr(ffn1_b.detach()), ptr(split_w["ffn2_w"]),
                                 ptr(ffn2_b.detach()), ptr(ln2_g.detach()), ptr(ln2_b.detach()))
-    ws = _u8(lib.grb_hstu_layer_f32_workspace_bytes(C.byref(d)), x.device)
+    ws = workspace(x.device, "grb_hstu_layer_f32_workspace_bytes", C.byref(d))
     y = torch.empty_like(xc)
-    with torch.cuda.device(x.device):
-        check(lib.grb_hstu_layer_forward_f32(C.byref(d), C.byref(p), C.byref(seq), ptr(xc), ptr(y), ptr(ws), stream_ptr(x.device)))
+    call(x.device, "grb_hstu_layer_forward_f32", C.byref(d), C.byref(p), C.byref(seq), ptr(xc), ptr(y), ptr(ws))
     return y
 
 
 def adam_step(p, g, m, v, p_bf16, state, lr, beta1, beta2, eps, weight_decay, grad_scale=1.0, zero_grad=True):
-    with torch.cuda.device(p.device):
-        check(_lib.load().grb_adam_step(ptr(p), ptr(g), ptr(m), ptr(v), ptr(p_bf16), p.numel(), ptr(state), lr, beta1, beta2, eps, weight_decay,
-                                        grad_scale, int(zero_grad), stream_ptr(p.device)))
+    call(p.device, "grb_adam_step", ptr(p), ptr(g), ptr(m), ptr(v), ptr(p_bf16), p.numel(), ptr(state), lr, beta1, beta2, eps, weight_decay,
+         grad_scale, int(zero_grad))
 
 
 def rowset_mark(ids, C, flag, rows, count):
@@ -1061,22 +975,18 @@ def rowset_mark(ids, C, flag, rows, count):
     require_cuda(ids)
     require_i64(ids)
     ids = ids.contiguous()
-    with torch.cuda.device(ids.device):
-        check(_lib.load().grb_rowset_mark(ptr(ids), ids.numel(), C, ptr(flag), ptr(rows), ptr(count), stream_ptr(ids.device)))
+    call(ids.device, "grb_rowset_mark", ptr(ids), ids.numel(), C, ptr(flag), ptr(rows), ptr(count))
 
 
 def rowset_mark_all(all_word):
-    with torch.cuda.device(all_word.device):
-        check(_lib.load().grb_rowset_mark_all(ptr(all_word), stream_ptr(all_word.device)))
+    call(all_word.device, "grb_rowset_mark_all", ptr(all_word))
 
 
 def adam_step_lazy_table(p, g, m, v, p_bf16, table_off, C, D, flag, rows, count, all_word, state, lr, beta1, beta2, eps, weight_decay,
                          grad_scale=1.0):
     """``adam_step`` with the table slot [table_off, table_off + C * D) updated on the rows of the row set only; empties the set."""
-    with torch.cuda.device(p.device):
-        check(_lib.load().grb_adam_step_lazy_table(ptr(p), ptr(g), ptr(m), ptr(v), ptr(p_bf16), p.numel(), table_off, C, D, ptr(flag), ptr(rows),
-                                                   ptr(count), ptr(all_word), ptr(state), lr, beta1, beta2, eps, weight_decay, grad_scale,
-                                                   stream_ptr(p.device)))
+    call(p.device, "grb_adam_step_lazy_table", ptr(p), ptr(g), ptr(m), ptr(v), ptr(p_bf16), p.numel(), table_off, C, D, ptr(flag), ptr(rows),
+         ptr(count), ptr(all_word), ptr(state), lr, beta1, beta2, eps, weight_decay, grad_scale)
 
 
 # ------------------------------------------------------------------------------------------------ COBRA
@@ -1085,18 +995,17 @@ def post_layernorm_fwd(x, g, b, eps):
     T, D = x.numel() // x.shape[-1], x.shape[-1]
     y = torch.empty_like(x)
     st = torch.empty(T, 2, dtype=torch.float32, device=x.device)
-    check(_lib.load().grb_post_layernorm_forward(ptr(x), ptr(g), ptr(b), float(eps), T, D, ptr(y), ptr(st), stream_ptr(x.device)))
+    call(x.device, "grb_post_layernorm_forward", ptr(x), ptr(g), ptr(b), float(eps), T, D, ptr(y), ptr(st))
     return y, st
 
 
 def post_layernorm_bwd(dy, x, st, g):
     """-> (dx, dg, db), dg / db summed in a fixed order"""
-    lib = _lib.load()
     T, D = x.numel() // x.shape[-1], x.shape[-1]
     dx = torch.empty_like(x)
     dg, db = torch.zeros_like(g), torch.zeros_like(g)
-    ws = _u8(lib.grb_layernorm_backward_workspace_bytes(T, D), x.device)
-    check(lib.grb_post_layernorm_backward(ptr(dy), ptr(x), ptr(st), ptr(g), T, D, ptr(dx), ptr(dg), ptr(db), ptr(ws), stream_ptr(x.device)))
+    ws = workspace(x.device, "grb_layernorm_backward_workspace_bytes", T, D)
+    call(x.device, "grb_post_layernorm_backward", ptr(dy), ptr(x), ptr(st), ptr(g), T, D, ptr(dx), ptr(dg), ptr(db), ptr(ws))
     return dx, dg, db
 
 
@@ -1108,7 +1017,7 @@ def cobra_pack_texts(tokens: torch.Tensor, keep: Optional[torch.Tensor] = None):
     lens = torch.empty(N, dtype=torch.int32, device=dev)
     offsets = torch.empty(N + 1, dtype=torch.int64, device=dev)
     info = torch.empty(3, dtype=torch.int64, device=dev)
-    check(_lib.load().grb_cobra_pack_texts(ptr(tokens), N, L, ptr(keep), ptr(lens), ptr(offsets), ptr(info), stream_ptr(dev)))
+    call(dev, "grb_cobra_pack_texts", ptr(tokens), N, L, ptr(keep), ptr(lens), ptr(offsets), ptr(info))
     return offsets, info
 
 
@@ -1117,7 +1026,7 @@ def cobra_text_rows(tokens: torch.Tensor, offsets: torch.Tensor, rows: int):
     N, L = tokens.shape
     tok = torch.empty(rows, dtype=torch.int64, device=tokens.device)
     pos = torch.empty(rows, dtype=torch.int64, device=tokens.device)
-    check(_lib.load().grb_cobra_text_rows(ptr(tokens), N, L, ptr(offsets), ptr(tok), ptr(pos), stream_ptr(tokens.device)))
+    call(tokens.device, "grb_cobra_text_rows", ptr(tokens), N, L, ptr(offsets), ptr(tok), ptr(pos))
     return tok, pos
 
 
@@ -1126,20 +1035,18 @@ def seg_layernorm_mean_fwd(offsets, x, g, b, eps):
     N, D = offsets.numel() - 1, g.numel()
     pooled = torch.empty(N, D, dtype=torch.float32, device=g.device)
     st = torch.empty(max(x.shape[0], 1), 2, dtype=torch.float32, device=g.device)
-    check(_lib.load().grb_seg_layernorm_mean_forward(ptr(offsets), N, ptr(x), ptr(g), ptr(b), float(eps), D, ptr(st), ptr(pooled),
-                                                     stream_ptr(g.device)))
+    call(g.device, "grb_seg_layernorm_mean_forward", ptr(offsets), N, ptr(x), ptr(g), ptr(b), float(eps), D, ptr(st), ptr(pooled))
     return pooled, st
 
 
 def seg_layernorm_mean_bwd(offsets, x, st, g, dpooled):
     """-> (dx [rows, D], dg, db [D]), dg / db summed in a fixed order"""
-    lib = _lib.load()
     N, D = offsets.numel() - 1, g.numel()
     dx = torch.empty_like(x)
     dg, db = torch.zeros_like(g), torch.zeros_like(g)
-    ws = _u8(lib.grb_seg_layernorm_mean_backward_workspace_bytes(N, D), g.device)
-    check(lib.grb_seg_layernorm_mean_backward(ptr(offsets), N, ptr(x), ptr(st), ptr(g), ptr(dpooled), D, ptr(dx), ptr(dg), ptr(db), ptr(ws),
-                                              stream_ptr(g.device)))
+    ws = workspace(g.device, "grb_seg_layernorm_mean_backward_workspace_bytes", N, D)
+    call(g.device, "grb_seg_layernorm_mean_backward", ptr(offsets), N, ptr(x), ptr(st), ptr(g), ptr(dpooled), D, ptr(dx), ptr(dg), ptr(db),
+         ptr(ws))
     return dx, dg, db
 
 
@@ -1148,14 +1055,14 @@ def l2norm_fwd(x, eps=1e-12):
     T, D = x.numel() // x.shape[-1], x.shape[-1]
     y = torch.empty_like(x)
     n = torch.empty(T, dtype=torch.float32, device=x.device)
-    check(_lib.load().grb_l2norm_forward(ptr(x), T, D, float(eps), ptr(y), ptr(n), stream_ptr(x.device)))
+    call(x.device, "grb_l2norm_forward", ptr(x), T, D, float(eps), ptr(y), ptr(n))
     return y, n
 
 
 def l2norm_bwd(dy, y, norms, eps=1e-12):
     T, D = y.numel() // y.shape[-1], y.shape[-1]
     dx = torch.empty_like(y)
-    check(_lib.load().grb_l2norm_backward(ptr(dy), ptr(y), ptr(norms), T, D, float(eps), ptr(dx), stream_ptr(y.device)))
+    call(y.device, "grb_l2norm_backward", ptr(dy), ptr(y), ptr(norms), T, D, float(eps), ptr(dx))
     return dx
 
 
@@ -1165,8 +1072,7 @@ def infonce_fwd_bwd(scores, lo, hi, inv_tau: float):
     row = torch.empty(Q, dtype=torch.float32, device=scores.device)
     loss = torch.empty(1, dtype=torch.float32, device=scores.device)
     ds = torch.empty(Q, ld, dtype=torch.bfloat16, device=scores.device)
-    check(_lib.load().grb_infonce_forward_backward(ptr(scores), Q, ld, ptr(lo), ptr(hi), float(inv_tau), ptr(row), ptr(loss), ptr(ds),
-                                                   stream_ptr(scores.device)))
+    call(scores.device, "grb_infonce_forward_backward", ptr(scores), Q, ld, ptr(lo), ptr(hi), float(inv_tau), ptr(row), ptr(loss), ptr(ds))
     return loss, ds
 
 
@@ -1176,23 +1082,20 @@ def cobra_beam_attention(q, hist_qkv, hist_len, suf_qkv, anc, S: int, H: int) ->
     step's QKV); hist_qkv [B, Li, 3D] bf16, the prefill's QKV, whose K | V are read in place, user b's keys its first hist_len[b]
     (int32 [B]) rows; suf_qkv [steps, B K, 3D] bf16, the new tokens' QKV per step; anc [B K, S - 1] int32 (None for S = 1): the row of
     step s < S - 1 a beam descends from (step S - 1 is its own row).  -> [B K, D] bf16."""
-    lib = _lib.load()
     B, Li, D3 = hist_qkv.shape
     D = D3 // 3
     R = q.shape[0]
     K = R // B
     out = torch.empty(R, D, dtype=torch.bfloat16, device=q.device)
-    ws = _u8(lib.grb_cobra_beam_attention_workspace_bytes(B, K, H, D // H, Li), q.device)
-    check(lib.grb_cobra_beam_attention(ptr(q), q.stride(0), ptr(hist_qkv[..., D:]), ptr(hist_qkv[..., 2 * D:]), D3, Li, ptr(hist_len),
-                                       ptr(suf_qkv[..., D:]), ptr(suf_qkv[..., 2 * D:]), D3, suf_qkv.stride(0), ptr(anc), S, B, K, H, D // H,
-                                       ptr(out), D, ptr(ws), stream_ptr(q.device)))
+    ws = workspace(q.device, "grb_cobra_beam_attention_workspace_bytes", B, K, H, D // H, Li)
+    call(q.device, "grb_cobra_beam_attention", ptr(q), q.stride(0), ptr(hist_qkv[..., D:]), ptr(hist_qkv[..., 2 * D:]), D3, Li, ptr(hist_len),
+         ptr(suf_qkv[..., D:]), ptr(suf_qkv[..., 2 * D:]), D3, suf_qkv.stride(0), ptr(anc), S, B, K, H, D // H, ptr(out), D, ptr(ws))
     return out
 
 
 def cobra_beam_topk(logits, scores_in, B: int, K: int, temperature: float, anc_in=None):
     """One beam step (grb_cobra_beam_topk): logits [B K_in, V] fp32, scores_in [B, K_in] or None (zero) -> (tokens [B, K] int64,
     scores [B, K], parents [B, K] int64, anc_out [B K, S_in + 1] int32: the parent's ancestry row and the parent's own row)."""
-    lib = _lib.load()
     V = logits.shape[-1]
     K_in = logits.shape[0] // B
     S_in = 0 if anc_in is None else anc_in.shape[1]
@@ -1201,23 +1104,19 @@ def cobra_beam_topk(logits, scores_in, B: int, K: int, temperature: float, anc_i
     scores = torch.empty(B, K, dtype=torch.float32, device=dev)
     parents = torch.empty(B, K, dtype=torch.int32, device=dev)
     anc_out = torch.empty(B * K, S_in + 1, dtype=torch.int32, device=dev)
-    ws = _u8(lib.grb_cobra_beam_topk_workspace_bytes(B, K_in, V, K), dev)
-    check(lib.grb_cobra_beam_topk(ptr(logits), ptr(scores_in), B, K_in, V, K, float(temperature), ptr(anc_in), S_in, ptr(tokens), ptr(scores),
-                                  ptr(parents), ptr(anc_out), ptr(ws), stream_ptr(dev)))
+    ws = workspace(dev, "grb_cobra_beam_topk_workspace_bytes", B, K_in, V, K)
+    call(dev, "grb_cobra_beam_topk", ptr(logits), ptr(scores_in), B, K_in, V, K, float(temperature), ptr(anc_in), S_in, ptr(tokens),
+         ptr(scores), ptr(parents), ptr(anc_out), ptr(ws))
     return tokens, scores, parents.long(), anc_out
 
 
 def cobra_dense_match(x_bf16, table_bf16):
     """x [R, D], table [N, D] bf16 -> (best [R] fp32, item [R] int64): each row's highest x . table_n, the lowest n among equal
     scores, without the [R, N] scores (grb_cobra_dense_match)."""
-    lib = _lib.load()
     R, D = x_bf16.shape
     N = table_bf16.shape[0]
     best = torch.empty(R, dtype=torch.float32, device=x_bf16.device)
     item = torch.empty(R, dtype=torch.int64, device=x_bf16.device)
-    nbytes = lib.grb_cobra_dense_match_workspace_bytes(R, D, N)
-    if nbytes == 0:
-        raise _lib.GrbError(lib.grb_last_error().decode())
-    ws = _u8(nbytes, x_bf16.device)
-    check(lib.grb_cobra_dense_match(ptr(x_bf16), ptr(table_bf16), R, D, N, ptr(best), ptr(item), ptr(ws), stream_ptr(x_bf16.device)))
+    ws = workspace(x_bf16.device, "grb_cobra_dense_match_workspace_bytes", R, D, N)
+    call(x_bf16.device, "grb_cobra_dense_match", ptr(x_bf16), ptr(table_bf16), R, D, N, ptr(best), ptr(item), ptr(ws))
     return best, item

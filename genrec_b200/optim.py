@@ -18,9 +18,8 @@ from typing import Optional
 import torch
 import torch.distributed as dist
 
-from . import _lib
 from . import functional as Fn
-from ._lib import check, ptr, stream_ptr
+from ._lib import call, ptr
 
 
 class FlatBuffers:
@@ -244,12 +243,10 @@ class FlatAdam:
         Fn.join_deferred(self.flat.device)
         if self.peer is not None:
             pg, pp, pmir, psig = self._peer_ptrs
-            with torch.cuda.device(self.flat.device):
-                check(_lib.load().grb_dp_adam_step(
-                    ptr(self.flat), ptr(self.grad), ptr(self.m), ptr(self.v), ptr(self.mirror), self._mc[0] or None, self._mc[1] or None,
-                    self._mc[2] or None, ptr(pg), ptr(pp), ptr(pmir), ptr(psig), ptr(self._sig), ptr(self._epoch), self.n, self.peer.rank,
-                    self.peer.world, ptr(self.state), self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay,
-                    1.0 / self.peer.world, stream_ptr(self.flat.device)))
+            call(self.flat.device, "grb_dp_adam_step",
+                 ptr(self.flat), ptr(self.grad), ptr(self.m), ptr(self.v), ptr(self.mirror), self._mc[0] or None, self._mc[1] or None,
+                 self._mc[2] or None, ptr(pg), ptr(pp), ptr(pmir), ptr(psig), ptr(self._sig), ptr(self._epoch), self.n, self.peer.rank,
+                 self.peer.world, ptr(self.state), self.lr, self.betas[0], self.betas[1], self.eps, self.weight_decay, 1.0 / self.peer.world)
             return
         if self.lazy_table:
             Fn.adam_step_lazy_table(self.flat, self.grad, self.m, self.v, self.mirror, self._table_off, self._table_rows, self._table_dim,

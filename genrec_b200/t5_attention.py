@@ -16,7 +16,7 @@ from torch import nn
 
 from . import functional as Fn
 from . import _lib
-from ._lib import check, ptr, require_cuda, stream_ptr, ensure_device
+from ._lib import call, ptr, require_cuda, ensure_device, workspace
 
 _CALLS = {"n": 0}
 _ZERO_BIAS, _BUCKETS, _CAUSAL = {}, {}, {}
@@ -75,10 +75,9 @@ def attention_core_fwd(Q, K, V, H, bias, bucket, key_pad, causal, scale, p=0.0, 
     out = torch.empty(B, Lq, D, dtype=torch.bfloat16, device=Q.device)
     lse = torch.empty(B, H, Lq, 2, dtype=torch.float32, device=Q.device)     # {row max, sum of exp(s - max)}
     nb = bias.shape[1] if bias is not None else 0
-    with torch.cuda.device(Q.device):
-        check(_lib.load().grb_t5_attention_forward(ptr(Q), ptr(K), ptr(V), B, Lq, Lk, H, D // H, Q.stride(1), K.stride(1), V.stride(1), ptr(bias),
-                                                   ptr(bucket), nb, ptr(key_pad), 1 if causal else 0, float(scale), float(p), int(seed), None,
-                                                   int(site) & 0xFFFFFFFF, ptr(out), D, ptr(lse), stream_ptr(Q.device)))
+    call(Q.device, "grb_t5_attention_forward", ptr(Q), ptr(K), ptr(V), B, Lq, Lk, H, D // H, Q.stride(1), K.stride(1), V.stride(1),
+         ptr(bias), ptr(bucket), nb, ptr(key_pad), 1 if causal else 0, float(scale), float(p), int(seed), None, int(site) & 0xFFFFFFFF,
+         ptr(out), D, ptr(lse))
     return out, lse
 
 
@@ -90,13 +89,10 @@ def attention_core_bwd(Q, K, V, H, bias, bucket, key_pad, causal, scale, out, ls
     dv = torch.empty(B, Lk, D, dtype=torch.float32, device=Q.device)
     dbias = torch.zeros_like(bias) if bias is not None else None
     nb = bias.shape[1] if bias is not None else 0
-    lib = _lib.load()
-    ws = torch.empty(lib.grb_t5_attention_backward_workspace_bytes(B, Lq, Lk, H, D // H, nb), dtype=torch.uint8, device=Q.device)
-    with torch.cuda.device(Q.device):
-        check(lib.grb_t5_attention_backward(ptr(Q), ptr(K), ptr(V), B, Lq, Lk, H, D // H, Q.stride(1), K.stride(1), V.stride(1), ptr(bias),
-                                            ptr(bucket), nb, ptr(key_pad), 1 if causal else 0, float(scale), float(p), int(seed), None,
-                                            int(site) & 0xFFFFFFFF, ptr(out), D, ptr(lse), ptr(dout), D, ptr(dq), D, ptr(dk), ptr(dv),
-                                            ptr(dbias), ptr(ws) if ws.numel() else None, stream_ptr(Q.device)))
+    ws = workspace(Q.device, "grb_t5_attention_backward_workspace_bytes", B, Lq, Lk, H, D // H, nb, allow_empty=True)
+    call(Q.device, "grb_t5_attention_backward", ptr(Q), ptr(K), ptr(V), B, Lq, Lk, H, D // H, Q.stride(1), K.stride(1), V.stride(1),
+         ptr(bias), ptr(bucket), nb, ptr(key_pad), 1 if causal else 0, float(scale), float(p), int(seed), None, int(site) & 0xFFFFFFFF,
+         ptr(out), D, ptr(lse), ptr(dout), D, ptr(dq), D, ptr(dk), ptr(dv), ptr(dbias), ptr(ws) if ws.numel() else None)
     return dq, dk, dv, dbias
 
 
@@ -116,11 +112,10 @@ def attention_core_fwd_jagged(Q, K, V, H, bias, bucket, offsets, max_len, causal
     out = torch.empty(*Q.shape[:-1], D, dtype=torch.bfloat16, device=Q.device)
     lse = torch.empty(*((H, T) if Lq == 0 else (B, H, Lq)), 2, dtype=torch.float32, device=Q.device)
     nb = bias.shape[1] if bias is not None else 0
-    with torch.cuda.device(Q.device):
-        check(_lib.load().grb_t5_attention_forward_jagged(
-            ptr(Q), ptr(K), ptr(V), ptr(offsets), B, T, int(max_len), Lq, H, D // H, Q.stride(-2), K.stride(-2), V.stride(-2), ptr(bias),
-            ptr(bucket), bucket.numel() if bucket is not None else 0, nb, 1 if causal else 0, float(scale), float(p), int(seed), None,
-            int(site) & 0xFFFFFFFF, ptr(out), D, ptr(lse), stream_ptr(Q.device)))
+    call(Q.device, "grb_t5_attention_forward_jagged",
+         ptr(Q), ptr(K), ptr(V), ptr(offsets), B, T, int(max_len), Lq, H, D // H, Q.stride(-2), K.stride(-2), V.stride(-2), ptr(bias),
+         ptr(bucket), bucket.numel() if bucket is not None else 0, nb, 1 if causal else 0, float(scale), float(p), int(seed), None,
+         int(site) & 0xFFFFFFFF, ptr(out), D, ptr(lse))
     return out, lse
 
 
@@ -134,15 +129,12 @@ def attention_core_bwd_jagged(Q, K, V, H, bias, bucket, offsets, max_len, causal
     dv = torch.empty(T, D, dtype=torch.float32, device=Q.device)
     dbias = torch.zeros_like(bias) if bias is not None else None
     nb = bias.shape[1] if bias is not None else 0
-    lib = _lib.load()
-    ws = torch.empty(lib.grb_t5_attention_backward_workspace_bytes_jagged(B, T, int(max_len), Lq, H, D // H, nb), dtype=torch.uint8,
-                     device=Q.device)
-    with torch.cuda.device(Q.device):
-        check(lib.grb_t5_attention_backward_jagged(
-            ptr(Q), ptr(K), ptr(V), ptr(offsets), B, T, int(max_len), Lq, H, D // H, Q.stride(-2), K.stride(-2), V.stride(-2), ptr(bias),
-            ptr(bucket), bucket.numel() if bucket is not None else 0, nb, 1 if causal else 0, float(scale), float(p), int(seed), None,
-            int(site) & 0xFFFFFFFF, ptr(out), D, ptr(lse), ptr(dout), D, ptr(dq), D, ptr(dk), ptr(dv), ptr(dbias),
-            ptr(ws) if ws.numel() else None, stream_ptr(Q.device)))
+    ws = workspace(Q.device, "grb_t5_attention_backward_workspace_bytes_jagged", B, T, int(max_len), Lq, H, D // H, nb, allow_empty=True)
+    call(Q.device, "grb_t5_attention_backward_jagged",
+         ptr(Q), ptr(K), ptr(V), ptr(offsets), B, T, int(max_len), Lq, H, D // H, Q.stride(-2), K.stride(-2), V.stride(-2), ptr(bias),
+         ptr(bucket), bucket.numel() if bucket is not None else 0, nb, 1 if causal else 0, float(scale), float(p), int(seed), None,
+         int(site) & 0xFFFFFFFF, ptr(out), D, ptr(lse), ptr(dout), D, ptr(dq), D, ptr(dk), ptr(dv), ptr(dbias),
+         ptr(ws) if ws.numel() else None)
     return dq, dk, dv, dbias
 
 

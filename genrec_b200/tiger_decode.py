@@ -17,8 +17,7 @@ from typing import NamedTuple, Optional
 
 import torch
 
-from . import _lib
-from ._lib import check, ptr, require_cuda, stream_ptr
+from ._lib import call, ptr, require_cuda, workspace
 
 
 class TigerGenerationOutput(NamedTuple):      # (tiger.py:78-83)
@@ -89,11 +88,9 @@ def trie_log_softmax(logits: torch.Tensor, nodes: Optional[torch.Tensor], trie: 
     use = trie is not None
     if use:
         nodes = nodes.to(torch.int32).contiguous()
-    with torch.cuda.device(x.device):
-        check(_lib.load().grb_trie_log_softmax(ptr(x), R, V, ptr(nodes) if use else None, ptr(trie.child_off) if use else None,
-                                               ptr(trie.child_tok) if use else None, trie.n_nodes if use else 0, 1 if use else 0,
-                                               int(vocab_offset), int(num_embeddings), float(temperature), ptr(probs), ptr(logp),
-                                               stream_ptr(x.device)))
+    call(x.device, "grb_trie_log_softmax", ptr(x), R, V, ptr(nodes) if use else None, ptr(trie.child_off) if use else None,
+         ptr(trie.child_tok) if use else None, trie.n_nodes if use else 0, 1 if use else 0, int(vocab_offset), int(num_embeddings),
+         float(temperature), ptr(probs), ptr(logp))
     return probs, logp
 
 
@@ -129,16 +126,14 @@ def beam_select(beam_seqs: torch.Tensor, beam_logps: torch.Tensor, cand_tok: tor
     use = trie is not None
     new_nodes = torch.empty(B, K, dtype=torch.int32, device=dev) if use else None
     nodes_c = nodes.to(torch.int32).contiguous() if use else None
-    lib = _lib.load()
     args = (ptr(seqs) if S > 0 else None, ptr(beam_logps.float().contiguous()), ptr(cand_tok.to(torch.int64).contiguous()),
             ptr(cand_logp.float().contiguous()), ptr(nodes_c), ptr(trie.child_off) if use else None, ptr(trie.child_tok) if use else None,
             ptr(trie.child_node) if use else None, trie.n_nodes if use else 0, B, K, KK, S, ptr(new_seqs), ptr(new_logps), ptr(new_nodes))
-    with torch.cuda.device(dev):
-        if K <= 32 and K * KK <= 1024:                                           # one CTA sorts a row's candidates
-            check(lib.grb_beam_select(*args, stream_ptr(dev)))
-        else:
-            ws = torch.empty(lib.grb_beam_select_wide_workspace_bytes(B, K, KK), dtype=torch.uint8, device=dev)
-            check(lib.grb_beam_select_wide(*args, ptr(ws), stream_ptr(dev)))
+    if K <= 32 and K * KK <= 1024:                                           # one CTA sorts a row's candidates
+        call(dev, "grb_beam_select", *args)
+    else:
+        ws = workspace(dev, "grb_beam_select_wide_workspace_bytes", B, K, KK)
+        call(dev, "grb_beam_select_wide", *args, ptr(ws))
     return new_seqs, new_logps, new_nodes
 
 
