@@ -126,9 +126,8 @@ class _LinearF32Fn(torch.autograd.Function):
             return x.new_zeros(*x.shape[:-1], w.shape[0], dtype=torch.float32)
         xb = Fn.cast_rows_bf16(x.detach().contiguous().float())
         wb = Fn.cast_bf16(w)
-        y, _, _ = Fn.linear_bwd(xb, wb.t().contiguous(), None, need_dw=False)
         ctx.save_for_backward(xb, wb)
-        return y + b.detach()
+        return Fn.matmul_f32(xb, wb.t().contiguous()) + b.detach()
 
     @staticmethod
     def backward(ctx, dy):
@@ -193,8 +192,8 @@ class _FfnFn(torch.autograd.Function):
         xc = x.detach().contiguous().float()
         xb = Fn.cast_rows_bf16(xc)
         w1b, w2b = Fn.cast_bf16(w1), Fn.cast_bf16(w2)
-        z, h = Fn.linear_fwd(xb, w1b, b1.detach().contiguous(), 2, p_in, seed, None, site)
-        y = Fn.linear_residual_fwd(h, w2b, b2.detach().contiguous(), xc, None, p_out, seed, None, site + 1)
+        y, z, h = Fn.ffn_fwd(xb, w1b, b1.detach().contiguous(), w2b, b2.detach().contiguous(), xc, None, p_in, p_out, seed, None, site,
+                             site + 1)
         ctx.save_for_backward(xb, z, h, w1b, w2b)
         ctx.cfg = (p_in, p_out, seed, site)
         return y
@@ -204,10 +203,7 @@ class _FfnFn(torch.autograd.Function):
         xb, z, h, w1b, w2b = ctx.saved_tensors
         p_in, p_out, seed, site = ctx.cfg
         dyc = dy.contiguous().float()
-        dyb = Fn.cast_rows_bf16(dyc, None, p_out, seed, None, site + 1)
-        _, dw2, db2 = Fn.linear_bwd(dyb, w2b, h, need_dx=False)
-        dz = Fn.linear_dact_bwd(dyb, w2b, z, 2, p_in, seed, None, site)
-        dx, dw1, db1 = Fn.linear_bwd(dz, w1b, xb, dx_residual=dyc)
+        dx, dw1, db1, dw2, db2 = Fn.ffn_bwd(dyc, w1b, w2b, xb, z, h, p_in, p_out, seed, None, site, site + 1, dx_residual=dyc)
         return dx, dw1, db1, dw2, db2, None, None, None, None
 
 
@@ -251,7 +247,7 @@ class _InfoNceFn(torch.autograd.Function):
         pb = Fn.cast_rows_bf16(pred.detach().contiguous())
         gpad = torch.zeros(Qp, d, dtype=torch.bfloat16, device=pred.device)
         gpad[:Q] = Fn.cast_rows_bf16(gt.detach().contiguous())
-        S, _, _ = Fn.linear_bwd(pb, gpad.t().contiguous(), None, need_dw=False)      # [Q, Qp] fp32 = pred gt^T
+        S = Fn.matmul_f32(pb, gpad.t().contiguous())                                # [Q, Qp] = pred gt^T
         loss, dS = Fn.infonce_fwd_bwd(S, lo, hi, inv_tau)
         ctx.save_for_backward(dS, gpad)
         return (loss / Q).reshape(())
@@ -259,8 +255,7 @@ class _InfoNceFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         dS, gpad = ctx.saved_tensors
-        dpred, _, _ = Fn.linear_bwd(dS, gpad, None, need_dw=False)
-        return dpred * g, None, None, None, None
+        return Fn.matmul_f32(dS, gpad) * g, None, None, None, None
 
 
 class _ZeroGrads(torch.autograd.Function):

@@ -7,6 +7,7 @@ tensors raise - there is no fallback.
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
 from typing import List, NamedTuple, Optional, Tuple
 
@@ -718,7 +719,7 @@ def hstu_pool_release(pool: _lib.HstuPool, users: torch.Tensor, last_hidden: Opt
     call(users.device, "grb_hstu_pool_release", C.byref(pool), ptr(users.contiguous()), users.numel(), ptr(last_hidden), D)
 
 
-# ------------------------------------------------------------------------------------------------ SASRec pieces
+# ------------------------------------------------------------------------------------------------ SASRec, TIGER and COBRA pieces
 def layernorm_fwd(x, g, b, eps, want_bf16=True, want_f32=False):
     T, D = x.numel() // x.shape[-1], x.shape[-1]
     yb = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if want_bf16 else None
@@ -844,6 +845,61 @@ def cast_rows_bf16(x, row_scale=None, p=0.0, seed=0, seed_dev=None, site=0):
     out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
     call(x.device, "grb_cast_rows_f32_to_bf16", ptr(x), ptr(out), T, D, ptr(row_scale), float(p), int(seed), ptr(seed_dev), site)
     return out
+
+
+@functools.cache
+def zero_bias(n: int, device) -> torch.Tensor:
+    """fp32 zeros [n] on ``device``, made once: the bias operand of a bias-free linear."""
+    return torch.zeros(n, dtype=torch.float32, device=device)
+
+
+def dropout_seed(p: float) -> int:
+    """The host seed of a dropout call: torch's initial seed (torch.manual_seed makes a step reproducible), 0 when p is 0."""
+    return torch.initial_seed() & 0x7FFFFFFFFFFFFFFF if p > 0 else 0
+
+
+class StepSeeds:
+    """Mixed into HSTU and SASRec, whose dropout probability is ``emb_dropout.p``: ``_seeds`` gives each training forward its
+    (host seed, device seed), (0, None) without dropout.  The device seed is an int64 counter, made by the first training forward
+    (again after ``_seed_dev = None``) and bumped by each; a CUDA graph that captures the bump draws fresh masks on every replay."""
+
+    _seed_dev = None
+
+    def _seeds(self, device):
+        if not (self.training and self.emb_dropout.p > 0):
+            return 0, None
+        if self._seed_dev is None or self._seed_dev.device != device:
+            self._seed_dev = torch.zeros(1, dtype=torch.int64, device=device)
+            self._step_seed = dropout_seed(self.emb_dropout.p)
+        self._seed_dev.add_(0x9E3779B1)
+        # per-forward snapshot: the backward re-derives the masks from the value THIS forward saw, even when another
+        # training-mode forward has bumped the counter in between
+        return self._step_seed, self._seed_dev.clone()
+
+
+def matmul_f32(xb, w_t):
+    """fp32 [R, N] = x W^T of bf16 operands, through the linear backward's dx GEMM, which writes fp32: xb [R, K] and w_t = W^T [K, N]
+    contiguous, K and N multiples of 8 (pad W with zero rows to get there, then slice the result)."""
+    y, _, _ = linear_bwd(xb, w_t, None, need_dw=False)
+    return y
+
+
+def ffn_fwd(xb, w1b, b1, w2b, b2, residual, row_scale, p_in, p_out, seed, seed_dev, site_hid, site_out):
+    """A block's feed-forward: z = x W1^T + b1, h = drop(relu(z)) at site_hid, y = (drop(h W2^T + b2) at site_out + residual) *
+    row_scale, as two fused-epilogue GEMMs on bf16 operands -> (y fp32, z, h)."""
+    z, h = linear_fwd(xb, w1b, b1, 2, p_in, seed, seed_dev, site_hid)
+    y = linear_residual_fwd(h, w2b, b2, residual, row_scale, p_out, seed, seed_dev, site_out)
+    return y, z, h
+
+
+def ffn_bwd(dy, w1b, w2b, xb, z, h, p_in, p_out, seed, seed_dev, site_hid, site_out, dx_residual=None):
+    """The backward of ``ffn_fwd`` under the same dropout arguments (the cast of dy re-applies the output mask, the dact GEMM the
+    hidden one): dy fp32 -> (dx fp32 (+ dx_residual), dw1, db1, dw2, db2).  The residual's gradient, dy, is the caller's."""
+    dyb = cast_rows_bf16(dy, None, p_out, seed, seed_dev, site_out)
+    _, dw2, db2 = linear_bwd(dyb, w2b, h, need_dx=False)
+    dz = linear_dact_bwd(dyb, w2b, z, 2, p_in, seed, seed_dev, site_hid)
+    dx, dw1, db1 = linear_bwd(dz, w1b, xb, dx_residual=dx_residual)
+    return dx, dw1, db1, dw2, db2
 
 
 # ------------------------------------------------------------------------------------------------ RQ-VAE

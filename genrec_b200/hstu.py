@@ -381,7 +381,7 @@ class HSTUPool:
                              self.free_stack.data_ptr(), self.free_top.data_ptr(), self.error_bits.data_ptr(), self.row_of.data_ptr())
 
 
-class HSTU(nn.Module):
+class HSTU(Fn.StepSeeds, nn.Module):
     """Mirror of genrec/models/hstu.py:19-157."""
 
     def __init__(self, num_items: int, max_seq_len: int = 50, embed_dim: int = 64, num_heads: int = 2, num_blocks: int = 2,
@@ -405,8 +405,6 @@ class HSTU(nn.Module):
         self._grad_sink = None
         self._unit_loss_grad = False   # FlatAdam(unit_loss_grad=True): head gradients go straight into the flat buffer (see HeadLossFn)
         self._row_marker = None        # set by FlatAdam(lazy_table=True): training forwards mark the item-table rows they touch
-        self._step_seed = 0
-        self._seed_dev = None  # device uint64 counter, bumped once per training forward (CUDA-graph-safe dropout reseeding)
         self._init_weights()
 
     def _init_weights(self):
@@ -445,17 +443,6 @@ class HSTU(nn.Module):
         if self._bf16_provider is not None:
             return self._bf16_provider(w)
         return _cached(self._table_casts, "bf16", w, Fn.cast_bf16, remake=self.training and torch.is_grad_enabled())
-
-    def _seeds(self, device):
-        if not (self.training and self.emb_dropout.p > 0):
-            return 0, None
-        if self._seed_dev is None or self._seed_dev.device != device:
-            self._seed_dev = torch.zeros(1, dtype=torch.int64, device=device)
-            self._step_seed = torch.initial_seed() & 0x7FFFFFFFFFFFFFFF
-        self._seed_dev.add_(0x9E3779B1)  # captured by CUDA graphs: every replay draws fresh masks
-        # per-forward snapshot: the backward re-derives the masks from the value THIS forward saw, even when another
-        # training-mode forward has bumped the counter in between
-        return self._step_seed, self._seed_dev.clone()
 
     def _marks_rows(self) -> bool:
         """A training forward under FlatAdam(lazy_table=True): the gradient sink is set and grad is enabled (as for esink / hsink)."""

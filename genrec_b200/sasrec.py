@@ -36,9 +36,8 @@ class _BlockFn(torch.autograd.Function):
         att, lse = Fn.sasrec_attention_fwd(Q, K, V, pad, H, p, seed, sd, layer, cfg["offsets"], cfg["max_len"])   # :206-240
         h = att.float() + qf                                                                                      # :244 residual = normalised query
         hnb, _, st2 = Fn.layernorm_fwd(h, g2.detach(), b2.detach(), 1e-8)                                        # :163 norm2
-        z1, a1 = Fn.linear_fwd(hnb, bf16w["w1"], bb1.detach(), 2, p, seed, sd, layer * 8 + SITE_HID)              # fc1 + relu + dropout
-        y = Fn.linear_residual_fwd(a1, bf16w["w2"], bb2.detach(), h, rowmask if apply_mask else None, p, seed, sd,
-                                   layer * 8 + SITE_OUT)                                                          # fc2 + dropout + residual (* mask)
+        y, z1, a1 = Fn.ffn_fwd(hnb, bf16w["w1"], bb1.detach(), bf16w["w2"], bb2.detach(), h, rowmask if apply_mask else None, p, p,
+                               seed, sd, layer * 8 + SITE_HID, layer * 8 + SITE_OUT)    # fc1 + relu + dropout, fc2 + dropout + residual (* mask)
         ctx.cfg, ctx.bf16w = cfg, bf16w
         ctx.save_for_backward(x, rowmask, pad, st1, st2, qb, xb, Q, K, V, att, lse, h, hnb, z1, a1, g1, g2)
         return y
@@ -51,10 +50,8 @@ class _BlockFn(torch.autograd.Function):
         dy = dy.contiguous().float()
         if apply_mask:
             dy = dy * rowmask.view(*dy.shape[:-1], 1)
-        dyb = Fn.cast_rows_bf16(dy, None, p, seed, sd, layer * 8 + SITE_OUT)
-        _, dw2, db2 = Fn.linear_bwd(dyb, w["w2"], a1, need_dx=False)
-        dz1 = Fn.linear_dact_bwd(dyb, w["w2"], z1, 2, p, seed, sd, layer * 8 + SITE_HID)
-        dhn, dw1, db1 = Fn.linear_bwd(dz1, w["w1"], hnb)
+        dhn, dw1, db1, dw2, db2 = Fn.ffn_bwd(dy, w["w1"], w["w2"], hnb, z1, a1, p, p, seed, sd, layer * 8 + SITE_HID,
+                                             layer * 8 + SITE_OUT)
         dh, dg2, dbt2 = Fn.layernorm_bwd(dhn, h, st2, g2, residual=dy)
         datt = Fn.cast_rows_bf16(dh)
         dQ, dK, dV = Fn.sasrec_attention_bwd(Q, K, V, pad, att, lse, datt, H, p, seed, sd, layer, cfg["offsets"], cfg["max_len"])
@@ -99,7 +96,7 @@ class _AttnFn(torch.autograd.Function):
         Q, _ = Fn.linear_fwd(qb, wqb, bq.detach(), 0)
         K, _ = Fn.linear_fwd(kvb, wkb, bk.detach(), 0)
         V, _ = Fn.linear_fwd(kvb, wvb, bv.detach(), 0)
-        seed = torch.initial_seed() & 0x7FFFFFFFFFFFFFFF if p > 0 else 0
+        seed = Fn.dropout_seed(p)
         att, lse = Fn.sasrec_attention_fwd(Q, K, V, pad, H, p, seed, None, 0)
         ctx.save_for_backward(pad, qb, kvb, Q, K, V, att, lse, wqb, wkb, wvb)
         ctx.cfg = (H, p, seed)
@@ -129,9 +126,8 @@ class _FfnFn(torch.autograd.Function):
         res = residual.detach().contiguous().float()
         w1b, w2b = Fn.cast_bf16(w1), Fn.cast_bf16(w2)
         xb = Fn.cast_rows_bf16(xf)
-        seed = torch.initial_seed() & 0x7FFFFFFFFFFFFFFF if p > 0 else 0
-        z1, a1 = Fn.linear_fwd(xb, w1b, b1.detach(), 2, p, seed, None, SITE_HID)
-        y = Fn.linear_residual_fwd(a1, w2b, b2.detach(), res, None, p, seed, None, SITE_OUT)
+        seed = Fn.dropout_seed(p)
+        y, z1, a1 = Fn.ffn_fwd(xb, w1b, b1.detach(), w2b, b2.detach(), res, None, p, p, seed, None, SITE_HID, SITE_OUT)
         ctx.save_for_backward(xb, z1, a1, w1b, w2b)
         ctx.cfg = (p, seed)
         return y
@@ -141,10 +137,7 @@ class _FfnFn(torch.autograd.Function):
         xb, z1, a1, w1b, w2b = ctx.saved_tensors
         p, seed = ctx.cfg
         dy = dy.contiguous().float()
-        dyb = Fn.cast_rows_bf16(dy, None, p, seed, None, SITE_OUT)
-        _, dw2, db2 = Fn.linear_bwd(dyb, w2b, a1, need_dx=False)
-        dz1 = Fn.linear_dact_bwd(dyb, w2b, z1, 2, p, seed, None, SITE_HID)
-        dx, dw1, db1 = Fn.linear_bwd(dz1, w1b, xb)
+        dx, dw1, db1, dw2, db2 = Fn.ffn_bwd(dy, w1b, w2b, xb, z1, a1, p, p, seed, None, SITE_HID, SITE_OUT)
         return dx, dy, None, dw1, db1, dw2, db2
 
 
@@ -199,7 +192,7 @@ class SASRecBlock(nn.Module):
         return _BlockFn.apply(x, rowmask, pad, cfg, bf16w, *self._params())
 
 
-class SASRec(nn.Module):
+class SASRec(Fn.StepSeeds, nn.Module):
     """Mirror of genrec/models/sasrec.py:18-138."""
 
     def __init__(self, num_items: int, max_seq_len: int = 50, embed_dim: int = 64, num_heads: int = 2, num_blocks: int = 2,
@@ -214,8 +207,6 @@ class SASRec(nn.Module):
             b.layer_index = i
         self.final_norm = nn.LayerNorm(embed_dim, eps=1e-8)
         self.return_train_logits = False
-        self._seed_dev = None
-        self._step_seed = 0
         self._init_weights()
 
     def _init_weights(self):
@@ -232,16 +223,6 @@ class SASRec(nn.Module):
             elif isinstance(module, nn.LayerNorm):
                 nn.init.ones_(module.weight)
                 nn.init.zeros_(module.bias)
-
-    def _seeds(self, device):
-        if not (self.training and self.emb_dropout.p > 0):
-            return 0, None
-        if self._seed_dev is None or self._seed_dev.device != device:
-            self._seed_dev = torch.zeros(1, dtype=torch.int64, device=device)
-            self._step_seed = torch.initial_seed() & 0x7FFFFFFFFFFFFFFF
-        self._seed_dev.add_(0x9E3779B1)
-        # per-forward snapshot: the backward re-derives the masks from the value THIS forward saw
-        return self._step_seed, self._seed_dev.clone()
 
     def encode(self, input_ids: torch.Tensor) -> torch.Tensor:
         """Embedding + all blocks (everything before final_norm).  sasrec.py:100-116."""

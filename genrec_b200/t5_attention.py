@@ -19,7 +19,7 @@ from . import _lib
 from ._lib import call, ptr, require_cuda, ensure_device, workspace
 
 _CALLS = {"n": 0}
-_ZERO_BIAS, _BUCKETS, _CAUSAL = {}, {}, {}
+_BUCKETS, _CAUSAL = {}, {}
 
 
 def relative_position_buckets(q_len: int, k_len: int, num_buckets: int = 32, max_distance: int = 128) -> torch.Tensor:
@@ -33,13 +33,6 @@ def relative_position_buckets(q_len: int, k_len: int, num_buckets: int = 32, max
     exact = half // 2
     large = exact + (torch.log(n.float() / exact + 1e-6) / math.log(max_distance / exact) * (half - exact)).long().clamp(max=half - exact - 1)
     return (torch.where(n < exact, n, large) + side).to(torch.int32)
-
-
-def _zero_bias(n: int, device) -> torch.Tensor:
-    key = (n, str(device))
-    if key not in _ZERO_BIAS:
-        _ZERO_BIAS[key] = torch.zeros(n, dtype=torch.float32, device=device)
-    return _ZERO_BIAS[key]
 
 
 def _bucket_map(q_len, k_len, nb, maxd, device) -> torch.Tensor:
@@ -150,10 +143,10 @@ class _T5AttnFn(torch.autograd.Function):
         D = query.shape[-1]
         xq = Fn.cast_rows_bf16(query.detach().contiguous().float())
         wqb, wob = Fn.cast_bf16(wq), Fn.cast_bf16(wo)
-        Q, _ = Fn.linear_fwd(xq, wqb, _zero_bias(D, dev), 0)
+        Q, _ = Fn.linear_fwd(xq, wqb, Fn.zero_bias(D, dev), 0)
         if fused_kv:                                   # self-attention: one [2D, D] projection of the query stream (transformer.py:121-123)
             wkb = Fn.cast_bf16(wk)                     # wk holds the kv weight
-            KV, _ = Fn.linear_fwd(xq, wkb, _zero_bias(2 * D, dev), 0)
+            KV, _ = Fn.linear_fwd(xq, wkb, Fn.zero_bias(2 * D, dev), 0)
             K, V = KV[..., :D], KV[..., D:]
             xk = xv = xq
             wvb = None
@@ -161,10 +154,10 @@ class _T5AttnFn(torch.autograd.Function):
             xk = Fn.cast_rows_bf16(key.detach().contiguous().float())
             xv = xk if value is key else Fn.cast_rows_bf16(value.detach().contiguous().float())
             wkb, wvb = Fn.cast_bf16(wk), Fn.cast_bf16(wv)
-            K, _ = Fn.linear_fwd(xk, wkb, _zero_bias(D, dev), 0)
-            V, _ = Fn.linear_fwd(xv, wvb, _zero_bias(D, dev), 0)
+            K, _ = Fn.linear_fwd(xk, wkb, Fn.zero_bias(D, dev), 0)
+            V, _ = Fn.linear_fwd(xv, wvb, Fn.zero_bias(D, dev), 0)
         bias = rel_w.detach().float().view(H, -1).contiguous() if rel_w is not None else None
-        seed = torch.initial_seed() & 0x7FFFFFFFFFFFFFFF if p > 0 else 0
+        seed = Fn.dropout_seed(p)
         _CALLS["n"] += 1
         site = _CALLS["n"]
         scale = 1.0 / math.sqrt(D // H)
@@ -172,7 +165,7 @@ class _T5AttnFn(torch.autograd.Function):
             A, lse = attention_core_fwd(Q, K, V, H, bias, bucket, key_pad, causal, scale, p, seed, site)
         else:
             A, lse = attention_core_fwd_jagged(Q, K, V, H, bias, bucket, offsets, max_len, causal, scale, p, seed, site)
-        out, _ = Fn.linear_fwd(A, wob, _zero_bias(D, dev), 0)
+        out, _ = Fn.linear_fwd(A, wob, Fn.zero_bias(D, dev), 0)
         ctx.save_for_backward(xq, xk, xv, Q, K, V, A, lse, wqb, wkb, wvb if wvb is not None else wqb, wob, bias if bias is not None else lse,
                               bucket if bucket is not None else lse, key_pad if key_pad is not None else lse,
                               offsets if offsets is not None else lse)

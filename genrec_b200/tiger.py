@@ -30,7 +30,7 @@ from torch import nn
 from . import _lib
 from . import functional as Fn
 from . import tiger_decode as td
-from .t5_attention import T5Attention, _T5AttnFn, _bucket_map, _zero_bias, attention_core_fwd, attention_core_fwd_jagged
+from .t5_attention import T5Attention, _T5AttnFn, _bucket_map, attention_core_fwd, attention_core_fwd_jagged
 from .tiger_decode import TigerGenerationOutput
 
 __all__ = ["Tiger", "TigerOutput", "TigerGenerationOutput"]
@@ -44,10 +44,6 @@ _SITES = {"n": 1 << 30}             # dropout sites of the FFN epilogues (the at
 class TigerOutput(NamedTuple):      # (tiger.py:73-78)
     logits: torch.Tensor
     loss: torch.Tensor
-
-
-def _seed(p: float) -> int:
-    return torch.initial_seed() & 0x7FFFFFFFFFFFFFFF if p > 0 else 0
 
 
 class _RmsNormFn(torch.autograd.Function):
@@ -74,7 +70,7 @@ class _LinearFn(torch.autograd.Function):
     def forward(ctx, x, w):
         xb = Fn.cast_rows_bf16(x.detach().contiguous().float())
         wb = Fn.cast_bf16(w)
-        y, _ = Fn.linear_fwd(xb, wb, _zero_bias(w.shape[0], x.device), 0)
+        y, _ = Fn.linear_fwd(xb, wb, Fn.zero_bias(w.shape[0], x.device), 0)
         ctx.save_for_backward(xb, wb)
         return y.float()
 
@@ -95,11 +91,11 @@ class _FfnFn(torch.autograd.Function):
         dev, D = xc.device, xc.shape[-1]
         xnb, _, rstd = Fn.rmsnorm_fwd(xc, nw.detach(), RMS_EPS)
         wib, wob = Fn.cast_bf16(wi), Fn.cast_bf16(wo)
-        seed = _seed(p)
+        seed = Fn.dropout_seed(p)
         _SITES["n"] += 2
         site = _SITES["n"]
-        z, h = Fn.linear_fwd(xnb, wib, _zero_bias(wi.shape[0], dev), 2, p, seed, None, site)
-        y = Fn.linear_residual_fwd(h, wob, _zero_bias(D, dev), xc, None, p, seed, None, site + 1)
+        y, z, h = Fn.ffn_fwd(xnb, wib, Fn.zero_bias(wi.shape[0], dev), wob, Fn.zero_bias(D, dev), xc, None, p, p, seed, None, site,
+                             site + 1)
         ctx.save_for_backward(xc, rstd, xnb, z, h, wib, wob, nw)
         ctx.cfg = (p, seed, site)
         return y
@@ -109,10 +105,7 @@ class _FfnFn(torch.autograd.Function):
         xc, rstd, xnb, z, h, wib, wob, nw = ctx.saved_tensors
         p, seed, site = ctx.cfg
         dyc = dy.contiguous().float()
-        dyb = Fn.cast_rows_bf16(dyc, None, p, seed, None, site + 1)
-        _, dwo, _ = Fn.linear_bwd(dyb, wob, h, need_dx=False)
-        dz = Fn.linear_dact_bwd(dyb, wob, z, 2, p, seed, None, site)
-        dxn, dwi, _ = Fn.linear_bwd(dz, wib, xnb)
+        dxn, dwi, _, dwo, _ = Fn.ffn_bwd(dyc, wib, wob, xnb, z, h, p, p, seed, None, site, site + 1)
         dx, dnw = Fn.rmsnorm_bwd(dxn, xc, rstd, nw.detach(), residual=dyc)
         return dx, dnw, dwi, dwo, None
 
@@ -126,12 +119,6 @@ def _head_mirrors(w: torch.Tensor):
     return wp, wp.t().contiguous()
 
 
-def _head_logits(xb: torch.Tensor, wpt: torch.Tensor, V: int) -> torch.Tensor:
-    """fp32 logits [R, V] = x W^T: the linear backward's dx GEMM (fp32 output) with W^T [D, Vp] as its weight operand."""
-    y, _, _ = Fn.linear_bwd(xb, wpt, None, need_dw=False)
-    return y[..., :V]
-
-
 class _HeadFn(torch.autograd.Function):
     """output_head (tiger.py:147, :207): fp32 logits [..., V] of fp32 rows."""
 
@@ -141,7 +128,7 @@ class _HeadFn(torch.autograd.Function):
         wp, wpt = _head_mirrors(w)
         ctx.save_for_backward(xb, wp)
         ctx.V = w.shape[0]
-        return _head_logits(xb, wpt, ctx.V)
+        return Fn.matmul_f32(xb, wpt)[..., :ctx.V]
 
     @staticmethod
     def backward(ctx, dy):
@@ -425,8 +412,8 @@ class Tiger(nn.Module):
         mem_kv = []                                                  # per decoder block: K, V [B, 1+N, D] (packed: [T, D]) bf16
         for blk in self.transformer.decoder.layers:
             a = blk.cross_attn.attn
-            Km, _ = Fn.linear_fwd(xm, Fn.cast_bf16(a.k.weight), _zero_bias(D, dev), 0)
-            Vm, _ = Fn.linear_fwd(xm, Fn.cast_bf16(a.v.weight), _zero_bias(D, dev), 0)
+            Km, _ = Fn.linear_fwd(xm, Fn.cast_bf16(a.k.weight), Fn.zero_bias(D, dev), 0)
+            Vm, _ = Fn.linear_fwd(xm, Fn.cast_bf16(a.v.weight), Fn.zero_bias(D, dev), 0)
             mem_kv.append((Km, Vm))
         wcache = [(Fn.cast_bf16(b.cross_attn.attn.q.weight), Fn.cast_bf16(b.cross_attn.attn.o.weight)) for b in self.transformer.decoder.layers]
         H = self.num_heads
@@ -436,12 +423,12 @@ class Tiger(nn.Module):
             # the queries of a user's beams against that user's memory: [B*R, S, D] viewed as [B, R*S, D]
             R, S = x.size(0) // B, x.size(1)
             wq, wo = wcache[i]
-            Q, _ = Fn.linear_fwd(Fn.cast_rows_bf16(blk.norm_cross(x).contiguous()), wq, _zero_bias(D, dev), 0)
+            Q, _ = Fn.linear_fwd(Fn.cast_rows_bf16(blk.norm_cross(x).contiguous()), wq, Fn.zero_bias(D, dev), 0)
             if jagged is None:
                 A, _ = attention_core_fwd(Q.view(B, R * S, D), mem_kv[i][0], mem_kv[i][1], H, None, None, kp, False, scale)
             else:
                 A, _ = attention_core_fwd_jagged(Q.view(B, R * S, D), mem_kv[i][0], mem_kv[i][1], H, None, None, *jagged, False, scale)
-            out, _ = Fn.linear_fwd(A.view(B * R, S, D), wo, _zero_bias(D, dev), 0)
+            out, _ = Fn.linear_fwd(A.view(B * R, S, D), wo, Fn.zero_bias(D, dev), 0)
             return x + out.float()
 
         wp, wpt = _head_mirrors(self.output_head.weight)
@@ -456,7 +443,7 @@ class Tiger(nn.Module):
                 x = self._decoder_input(tgt.size(0), tgt, types)
                 rows = tgt.size(0)
             out = self._decoder(x, cross)
-            logits = _head_logits(Fn.cast_rows_bf16(out[:, -1].contiguous()), wpt, V)
+            logits = Fn.matmul_f32(Fn.cast_rows_bf16(out[:, -1].contiguous()), wpt)[..., :V]
             return logits if rows == B * K else logits.unsqueeze(1).expand(B, K, V).reshape(B * K, V)
 
         run = (B, K, self.sem_id_dim, self.num_item_embeddings, dev, temperature, trie, generator)
