@@ -188,6 +188,11 @@ SIGNATURES = {
     "grb_cobra_beam_attention_workspace_bytes": (c_size_t, [c_int] * 5),
     "grb_cobra_beam_attention": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_void_p]
                                  + [c_int] * 5 + [c_void_p, c_int, c_void_p, c_void_p]),
+    "grb_cobra_paged_attention_workspace_bytes": (c_size_t, [c_int] * 4),
+    "grb_cobra_paged_attention": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                          c_void_p, c_int, c_void_p, c_void_p, c_int, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                          c_int, c_void_p, c_void_p]),
+    "grb_cobra_kv_scatter": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "grb_cobra_beam_topk_workspace_bytes": (c_size_t, [c_int] * 4),
     "grb_cobra_beam_topk": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int] + [c_void_p] * 6),
     "grb_cobra_dense_match_workspace_bytes": (c_size_t, [c_int] * 3),

@@ -35,6 +35,15 @@ whatever the batch around it.  ``beam_fusion`` (cobra.py:679-760) finds each bea
 one wgmma sweep of the bf16 catalog, without the [B, n_beam, N] similarity; the B x n_beam fusion tail stays in torch.  Both run
 without gradients and without dropout, and read two values to the host: the item-layout flag of ``_check_generate`` and the
 encoder's packing info.
+
+Serving (``new_pool`` -> ``CobraPool``, ``extend_users``, ``generate_users``, ``beam_fusion_users``, ``CobraPool.release``): every
+decoder layer's K | V rows of many users live in one paged pool.  ``extend_users`` encodes only the new items' texts and runs only
+their decoder rows, at the positions that continue each user's history: per layer the QKV GEMM, ``grb_cobra_kv_scatter`` (the new
+K | V rows into the user's pages), ``grb_cobra_paged_attention`` (each new row against everything the user has cached, read from the
+pages) and ``_layer_tail``; the final layer's row at the last dense position is kept as the user's ``last_hidden``.
+``generate_users`` runs ``generate``'s beam search (``_beams``, shared) from ``last_hidden`` with the history read through the page
+table.  The host keeps every user's item count and pages, so every refusal comes before any launch.  A user's outputs are the same
+bits however the history was split into calls and whichever users share the call or the pool.
 """
 from __future__ import annotations
 
@@ -50,7 +59,7 @@ from . import functional as Fn
 from ._lib import ensure_device, require_cuda
 from .t5_attention import attention_core_bwd, attention_core_bwd_jagged, attention_core_fwd, attention_core_fwd_jagged
 
-__all__ = ["Cobra", "CobraOutput", "CobraGenerationOutput", "BeamFusionOutput"]
+__all__ = ["Cobra", "CobraOutput", "CobraGenerationOutput", "BeamFusionOutput", "CobraPool"]
 
 LN_DIMS = (64, 128, 192, 256, 384, 768)           # widths of the LayerNorm row kernels
 POOL_DIMS = (128, 192, 256, 384, 768)             # widths of the pooled LayerNorm kernel
@@ -60,6 +69,7 @@ MAX_ATTN_ROWS = 65535                             # texts x heads (or users x he
 _MAX_BEAMS = 1024                                 # beams per user of generate (grb_cobra_beam_topk, grb_cobra_beam_attention)
 _MAX_CANDIDATES = 262144                          # beams x id_vocab_size of one beam step
 _CATALOG_CHUNK = 65536                            # catalog rows normalised at a time by beam_fusion
+_MAX_KEYS = 8192                                  # history rows of one user in the beam attention (CBA_MAX_HIST)
 
 
 class CobraGenerationOutput(NamedTuple):     # (cobra.py:29-35)
@@ -93,6 +103,62 @@ class CobraOutput(NamedTuple):      # (cobra.py:12-26)
     recall_total: torch.Tensor
     vec_cos_sim: torch.Tensor
     codebook_entropy: torch.Tensor
+
+
+class CobraPool:
+    """Paged per-user decoder cache of ``Cobra`` for serving (``Cobra.new_pool`` / ``extend_users`` / ``generate_users`` /
+    ``beam_fusion_users`` / ``CobraPool.release``).
+
+    Every decoder layer's K | V rows live in ``num_pages`` pages of ``page_size`` decoder positions shared by all users (``kv``
+    [decoder_layers, num_pages, page_size, 2 d_model] bf16); ``page_table`` [max_users, ceil(max_items (C+1) / page_size)] int32 maps
+    user u's position p to page ``page_table[u, p // page_size]`` (entries past a user's pages are 0).  ``last_hidden`` [max_users,
+    d_model] fp32 is each user's final-layer row at their last dense position, where ``generate_users`` starts.  The host keeps each
+    user's exact item count (``lengths``) and page list, and the free pages as a stack (page 0 goes out first): a call takes the pages
+    it needs in row order, and ``release`` pushes a user's pages back, first page on top.
+
+    A pool belongs to the parameters it was first written with: a later call raises once any parameter's version counter has moved
+    (a torch optimizer step, ``load_state_dict``).  ``genrec_b200.optim.FlatAdam`` writes parameters through a raw pointer and is not
+    caught, so rebuild every pool after any further training.
+    """
+
+    def __init__(self, max_users: int, num_pages: int, page_size: int, max_items: int, num_layers: int, d_model: int, C: int, device):
+        self.max_users, self.num_pages, self.page_size, self.max_items, self.C = max_users, num_pages, page_size, max_items, C
+        self.kv = torch.zeros(num_layers, num_pages, page_size, 2 * d_model, dtype=torch.bfloat16, device=device)
+        self.page_table = torch.zeros(max_users, -(-max_items * (C + 1) // page_size), dtype=torch.int32, device=device)
+        self.last_hidden = torch.zeros(max_users, d_model, dtype=torch.float32, device=device)
+        self.lengths = [0] * max_users                # items per user (host)
+        self.pages = [[] for _ in range(max_users)]   # each user's pages in position order (host)
+        self.free = list(range(num_pages - 1, -1, -1))
+        self.param_versions = None
+
+    def pages_free(self) -> int:
+        return len(self.free)
+
+    def _users(self, users, fn: str) -> list:
+        u = (users if isinstance(users, torch.Tensor) else torch.as_tensor(users)).reshape(-1).tolist()
+        if not u or not all(isinstance(x, int) for x in u):
+            raise ValueError(f"{fn}: users must be a non-empty list of integers, got {users!r}")
+        bad = [x for x in u if not 0 <= x < self.max_users]
+        if bad:
+            raise ValueError(f"{fn}: users out of range [0, {self.max_users}): {bad[:8]}")
+        if len(set(u)) != len(u):
+            raise ValueError(f"{fn}: users must be distinct within a call")
+        return u
+
+    def _pages_for(self, items: int) -> int:
+        return -(-items * (self.C + 1) // self.page_size)
+
+    def release(self, users) -> None:
+        """Forget ``users`` (distinct, any subset): their pages return to the pool, their lengths and ``last_hidden`` become zero,
+        and the next ``extend_users`` starts their histories afresh."""
+        u = self._users(users, "CobraPool.release")
+        for x in u:
+            self.free.extend(reversed(self.pages[x]))
+            self.pages[x] = []
+            self.lengths[x] = 0
+        idx = torch.tensor(u, dtype=torch.int64).to(self.kv.device)
+        self.page_table.index_fill_(0, idx, 0)
+        self.last_hidden.index_fill_(0, idx, 0.0)
 
 
 def _bad(msg: str) -> _lib.GrbError:
@@ -396,8 +462,9 @@ class Cobra(nn.Module):
         return self.encode_items(encoder_input_ids)
 
     # ---- decoder
-    def _interleave(self, input_ids, vecs, mask_items):
-        """CobraEmbedding.forward (cobra.py:75-147) for complete items: -> (h [B, T(C+1), d] fp32, mask [B, T(C+1)] bool)"""
+    def _interleave(self, input_ids, vecs, mask_items, start=None):
+        """CobraEmbedding.forward (cobra.py:75-147) for complete items: -> (h [B, T(C+1), d] fp32, mask [B, T(C+1)] bool); start [B]
+        int64: the decoder position of each row's first item (None: 0)"""
         e = self.cobra_emb
         B, L = input_ids.shape
         C, T = self.C, L // self.C
@@ -410,7 +477,11 @@ class Cobra(nn.Module):
         Li = T * (C + 1)
         types = torch.arange(Li, device=dev) % (C + 1) == C
         m = mask.unsqueeze(-1).float()
-        h = h * m + e.pos_embed.weight[:Li].unsqueeze(0) * m + F.embedding(types.long(), e.type_embed.weight).unsqueeze(0) * m
+        if start is None:
+            pos = e.pos_embed.weight[:Li].unsqueeze(0)
+        else:                                         # positions past the table only on pad rows, which m zeroes
+            pos = e.pos_embed.weight[(start[:, None] + torch.arange(Li, device=dev)).clamp_max(e.pos_embed.num_embeddings - 1)]
+        h = h * m + pos * m + F.embedding(types.long(), e.type_embed.weight).unsqueeze(0) * m
         return h, mask
 
     def _decode(self, x, mask, keep_qkv=None):
@@ -537,41 +608,45 @@ class Cobra(nn.Module):
                                   ("item_sem_ids", item_sem_ids)) if v is None]
         if missing:
             raise _MissingArguments("Cobra.beam_fusion", missing)
-        if not 1 <= n_candidates <= n_beam:
-            raise ValueError(f"Cobra.beam_fusion: n_candidates {n_candidates} must lie in 1 .. n_beam ({n_beam})")
-        if item_dense_vecs.dim() != 2 or item_dense_vecs.shape[1] != self.d_model or item_dense_vecs.shape[0] < 1:
-            raise ValueError(f"Cobra.beam_fusion: item_dense_vecs must be [N >= 1, {self.d_model}], got {tuple(item_dense_vecs.shape)}")
-        N = item_dense_vecs.shape[0]
-        if tuple(item_sem_ids.shape) != (N, self.C):
-            raise ValueError(f"Cobra.beam_fusion: item_sem_ids must be [{N}, {self.C}], got {tuple(item_sem_ids.shape)}")
+        self._check_catalog("Cobra.beam_fusion", n_candidates, n_beam, item_dense_vecs, item_sem_ids)
         self._check_generate(input_ids, encoder_input_ids, n_beam, temperature, "n_beam")
         require_cuda(item_dense_vecs, item_sem_ids)
         with torch.no_grad():
             gen = self._generate(input_ids, encoder_input_ids, n_beam, temperature)
-            B = input_ids.shape[0]
-            table = torch.empty(N, self.d_model, dtype=torch.bfloat16, device=input_ids.device)
-            for s in range(0, N, _CATALOG_CHUNK):                   # F.normalize(item_dense_vecs), bf16, a chunk of rows at a time
-                chunk = item_dense_vecs[s:s + _CATALOG_CHUNK].to(device=input_ids.device, dtype=torch.float32).contiguous()
-                table[s:s + _CATALOG_CHUNK] = Fn.cast_rows_bf16(Fn.l2norm_fwd(chunk)[0])
-            best, item = Fn.cobra_dense_match(Fn.cast_rows_bf16(gen.dense_vecs.reshape(-1, self.d_model).contiguous()), table)
-            max_sim, best_item = best.view(B, n_beam), item.view(B, n_beam)
-            fused = alpha * torch.softmax(gen.scores, dim=-1) + (1 - alpha) * ((max_sim + 1) / 2)
-            top, idx = torch.sort(fused, dim=-1, descending=True, stable=True)
-            item_ids = best_item.gather(1, idx[:, :n_candidates])
-            return BeamFusionOutput(item_ids=item_ids, sem_ids=item_sem_ids[item_ids], scores=top[:, :n_candidates].contiguous())
+            return self._fuse(gen, item_dense_vecs, item_sem_ids, n_candidates, n_beam, alpha)
+
+    def _check_catalog(self, fn, n_candidates, n_beam, item_dense_vecs, item_sem_ids):
+        if not 1 <= n_candidates <= n_beam:
+            raise ValueError(f"{fn}: n_candidates {n_candidates} must lie in 1 .. n_beam ({n_beam})")
+        if item_dense_vecs.dim() != 2 or item_dense_vecs.shape[1] != self.d_model or item_dense_vecs.shape[0] < 1:
+            raise ValueError(f"{fn}: item_dense_vecs must be [N >= 1, {self.d_model}], got {tuple(item_dense_vecs.shape)}")
+        N = item_dense_vecs.shape[0]
+        if tuple(item_sem_ids.shape) != (N, self.C):
+            raise ValueError(f"{fn}: item_sem_ids must be [{N}, {self.C}], got {tuple(item_sem_ids.shape)}")
+
+    def _fuse(self, gen, item_dense_vecs, item_sem_ids, n_candidates, n_beam, alpha) -> BeamFusionOutput:
+        """BeamFusion's catalog sweep and tail on the n_beam beams of gen"""
+        dev = gen.scores.device
+        B, N = gen.scores.shape[0], item_dense_vecs.shape[0]
+        table = torch.empty(N, self.d_model, dtype=torch.bfloat16, device=dev)
+        for s in range(0, N, _CATALOG_CHUNK):                   # F.normalize(item_dense_vecs), bf16, a chunk of rows at a time
+            chunk = item_dense_vecs[s:s + _CATALOG_CHUNK].to(device=dev, dtype=torch.float32).contiguous()
+            table[s:s + _CATALOG_CHUNK] = Fn.cast_rows_bf16(Fn.l2norm_fwd(chunk)[0])
+        best, item = Fn.cobra_dense_match(Fn.cast_rows_bf16(gen.dense_vecs.reshape(-1, self.d_model).contiguous()), table)
+        max_sim, best_item = best.view(B, n_beam), item.view(B, n_beam)
+        fused = alpha * torch.softmax(gen.scores, dim=-1) + (1 - alpha) * ((max_sim + 1) / 2)
+        top, idx = torch.sort(fused, dim=-1, descending=True, stable=True)
+        item_ids = best_item.gather(1, idx[:, :n_candidates])
+        return BeamFusionOutput(item_ids=item_ids, sem_ids=item_sem_ids[item_ids], scores=top[:, :n_candidates].contiguous())
 
     def _check_generate(self, input_ids, encoder_input_ids, K, temperature, k_name):
         """the refusals of generate / beam_fusion, before any launch; the item checks read one flag to the host"""
-        C, V = self.C, self.sparse_head[0].out_features
+        C = self.C
         if input_ids.dim() != 2 or input_ids.shape[1] % C or encoder_input_ids.dim() != 3 or \
                 tuple(encoder_input_ids.shape[:2]) != (input_ids.shape[0], input_ids.shape[1] // C) or input_ids.shape[0] < 1:
             raise ValueError(f"Cobra: input_ids [B, T*C] and encoder_input_ids [B, T, L] expected, got {tuple(input_ids.shape)} and "
                              f"{tuple(encoder_input_ids.shape)}")
-        if not 1 <= K <= min(V, _MAX_BEAMS) or K * V > _MAX_CANDIDATES:
-            raise ValueError(f"Cobra: {k_name} {K} must lie in 1 .. min(id_vocab_size, {_MAX_BEAMS}) = {min(V, _MAX_BEAMS)} with "
-                             f"{k_name} * id_vocab_size <= {_MAX_CANDIDATES}")
-        if not temperature > 0:
-            raise ValueError(f"Cobra: temperature must be positive, got {temperature}")
+        self._check_beams(K, temperature, k_name)
         T = input_ids.shape[1] // C
         if T * (C + 1) + C - 1 >= self.max_len:
             raise ValueError(f"Cobra: {T} items leave no positions for the generated tokens: T*(C+1) + C - 1 = {T * (C + 1) + C - 1} must "
@@ -582,6 +657,14 @@ class Cobra(nn.Module):
             raise ValueError("Cobra: a user has no item")
         if flag & 2:
             raise ValueError("Cobra: a real item follows a pad item; pad items must come after a user's real ones")
+
+    def _check_beams(self, K, temperature, k_name):
+        V = self.sparse_head[0].out_features
+        if not 1 <= K <= min(V, _MAX_BEAMS) or K * V > _MAX_CANDIDATES:
+            raise ValueError(f"Cobra: {k_name} {K} must lie in 1 .. min(id_vocab_size, {_MAX_BEAMS}) = {min(V, _MAX_BEAMS)} with "
+                             f"{k_name} * id_vocab_size <= {_MAX_CANDIDATES}")
+        if not temperature > 0:
+            raise ValueError(f"Cobra: temperature must be positive, got {temperature}")
 
     def _generate(self, input_ids, encoder_input_ids, K, temperature) -> CobraGenerationOutput:
         require_cuda(input_ids, encoder_input_ids)
@@ -594,9 +677,8 @@ class Cobra(nn.Module):
             self.train(training)
 
     def _beam_search(self, input_ids, encoder_input_ids, K, temperature):
-        e = self.cobra_emb
         B, TC = input_ids.shape
-        C, D, V = self.C, self.d_model, self.sparse_head[0].out_features
+        C = self.C
         T, L = TC // C, encoder_input_ids.shape[2]
         dev = input_ids.device
         # prefill: the histories once, each layer's QKV kept
@@ -608,6 +690,18 @@ class Cobra(nn.Module):
         h = self._decode(emb, seq_mask, hist_qkv)
         hist_len = (mask_items[:, :, C - 1].sum(1) * (C + 1)).to(torch.int32)
         h = h[torch.arange(B, device=dev), hist_len.long() - 1]                       # the last dense position: codebook 0
+
+        def attend(i, q, suf, anc, S, H):
+            return Fn.cobra_beam_attention(q, hist_qkv[i], hist_len, suf, anc, S, H)
+        return self._beams(h, hist_len, K, temperature, attend)
+
+    def _beams(self, h, hist_len, K, temperature, attend):
+        """The beam search from each user's codebook-0 row h [B, D] (the final layer at the last dense position) over histories of
+        hist_len [B] int32 decoder rows, whose K | V attend(layer, q, suffix QKV, ancestry, S, heads) reads."""
+        e = self.cobra_emb
+        B = h.shape[0]
+        C, D = self.C, self.d_model
+        dev = h.device
         head = self.sparse_head[0]
         tokens, scores, _, _ = Fn.cobra_beam_topk(_LinearF32Fn.apply(h, head.weight, head.bias).contiguous(), None, B, K, temperature)
         seqs = tokens.unsqueeze(-1)
@@ -623,12 +717,8 @@ class Cobra(nn.Module):
             tok = tokens.reshape(-1) + (c - 1) * e.id_vocab_size
             x = e.id_embed.weight[tok] + e.pos_embed.weight[pos + (c - 1)] + e.type_embed.weight[0]
             for i, layer in enumerate(layers):
-                sa = layer.self_attn
-                qkv = suf[i][c - 1]
-                Fn.linear_fwd(Fn.cast_rows_bf16(x.contiguous()), w[i][0], sa.in_proj_bias.detach().contiguous(), 0, out=qkv)
-                A = Fn.cobra_beam_attention(qkv[:, :D], hist_qkv[i], hist_len, suf[i], anc, c, sa.num_heads)
-                a, _ = Fn.linear_fwd(A, w[i][1], sa.out_proj.bias.detach().contiguous(), 0)
-                x = self._layer_tail(i, layer, x, a.float(), 0)
+                x = self._cached_layer(i, layer, x, w[i], lambda qkv: attend(i, qkv[:, :D], suf[i], anc, c, layer.self_attn.num_heads),
+                                       suf[i][c - 1])
             head = self.sparse_head[c]
             logits = _LinearF32Fn.apply(x, head.weight, head.bias).contiguous()
             tokens, scores, parents, anc = Fn.cobra_beam_topk(logits, scores, B, K, temperature, anc)
@@ -637,3 +727,179 @@ class Cobra(nn.Module):
                 h_last = x.view(B, K, D).gather(1, parents.unsqueeze(-1).expand(-1, -1, D))
         dense = Fn.l2norm_fwd(h_last.contiguous())[0]
         return CobraGenerationOutput(sem_ids=seqs, dense_vecs=dense, scores=scores)
+
+    def _cached_layer(self, i, layer, x, w, attend, qkv=None):
+        """decoder layer i on rows x [R, D] fp32 whose keys are cached: the QKV GEMM (into qkv when given), attend(qkv) -> the
+        attention [R, D] bf16, the out-projection and _layer_tail; w = the bf16 (in_proj, out_proj) weights"""
+        sa = layer.self_attn
+        qkv, _ = Fn.linear_fwd(Fn.cast_rows_bf16(x.contiguous()), w[0], sa.in_proj_bias.detach().contiguous(), 0, out=qkv)
+        A = attend(qkv)
+        a, _ = Fn.linear_fwd(A, w[1], sa.out_proj.bias.detach().contiguous(), 0)
+        return self._layer_tail(i, layer, x, a.float(), 0)
+
+    # ---- serving from a paged pool
+    def new_pool(self, max_users: int, num_pages: int, page_size: int = 64, max_items: Optional[int] = None) -> CobraPool:
+        """A paged K | V pool for up to ``max_users`` users of at most ``max_items`` items each; ``page_size`` counts decoder
+        positions, a positive multiple of 64.  The default and upper bound of ``max_items`` is the most items that leave generate its
+        C - 1 positions below max_len and whose n (C+1) decoder rows fit the paged attention's 8192 history keys."""
+        C = self.C
+        limit = min((self.max_len - C) // (C + 1), _MAX_KEYS // (C + 1))
+        max_items = limit if max_items is None else max_items
+        if max_users < 1 or num_pages < 1:
+            raise ValueError(f"Cobra.new_pool: max_users and num_pages must be positive, got {max_users}, {num_pages}")
+        if page_size < 64 or page_size % 64:
+            raise ValueError(f"Cobra.new_pool: page_size must be a positive multiple of 64 (one key tile), got {page_size}")
+        if not 1 <= max_items <= limit:
+            raise ValueError(f"Cobra.new_pool: max_items must lie in 1 .. {limit} (T (C+1) + C - 1 below max_len "
+                             f"{self.max_len}, at most {_MAX_KEYS} decoder rows), got {max_items}")
+        dev = self.cobra_emb.pos_embed.weight.device
+        require_cuda(self.cobra_emb.pos_embed.weight)
+        return CobraPool(max_users, num_pages, page_size, max_items, len(self.decoder.decoder.layers), self.d_model, C, dev)
+
+    def _check_pool(self, pool: CobraPool):
+        if not isinstance(pool, CobraPool) or pool.C != self.C or pool.kv.shape[0] != len(self.decoder.decoder.layers) or \
+                pool.kv.shape[3] != 2 * self.d_model:
+            raise ValueError("Cobra: the pool was not made by this model's new_pool")
+        versions = tuple(p._version for p in self.parameters())
+        if pool.param_versions is not None and pool.param_versions != versions:
+            raise RuntimeError("genrec_b200: the model's parameters changed after this pool was written; rebuild the pool")
+        return versions
+
+    def extend_users(self, pool: CobraPool, users, input_ids: torch.Tensor, encoder_input_ids: torch.Tensor) -> None:
+        """Append row b's real items to user ``users[b]``: input_ids [B, n C] with pad items after the real ones, encoder_input_ids
+        [B, n, L] right-padded with 0 (generate's layout).  Only the new items' texts are encoded and only their n_b (C+1) decoder rows
+        run through the layers, at the positions that continue the user's history; each layer writes their K | V into the user's pages
+        and then attends from the pages.  An all-pad row leaves its user untouched.  Refusals (ValueError) come before any launch."""
+        versions = self._check_pool(pool)
+        C = self.C
+        if input_ids.dim() != 2 or input_ids.shape[1] % C or input_ids.shape[1] == 0 or encoder_input_ids.dim() != 3 or \
+                tuple(encoder_input_ids.shape[:2]) != (input_ids.shape[0], input_ids.shape[1] // C) or input_ids.shape[0] < 1:
+            raise ValueError(f"Cobra.extend_users: input_ids [B, n*C] and encoder_input_ids [B, n, L] expected, got {tuple(input_ids.shape)} "
+                             f"and {tuple(encoder_input_ids.shape)}")
+        u = pool._users(users, "Cobra.extend_users")
+        B, n = input_ids.shape[0], input_ids.shape[1] // C
+        if len(u) != B:
+            raise ValueError(f"Cobra.extend_users: {len(u)} users for {B} rows")
+        # an item is real in all C codebooks or pad in all: the rows that run (every codebook's flag, _interleave) are then exactly
+        # the n_b (C+1) rows the host lays out below from the last codebook's flags
+        codes = (input_ids != self.pad_id).view(B, n, C)
+        real = codes[:, :, C - 1]
+        flags = torch.stack([(real[:, 1:] & ~real[:, :-1]).any(), (codes.any(-1) != codes.all(-1)).any()]).long()
+        *counts, gap, partial = torch.cat([real.sum(1), flags]).tolist()                                        # one host read
+        if partial:
+            raise ValueError("Cobra.extend_users: an item has pad_id in some of its codebooks but not all; an item is real in all "
+                             "C codebooks or pad in all")
+        if gap:
+            raise ValueError("Cobra.extend_users: a real item follows a pad item; pad items must come after a user's real ones")
+        over = [x for x, k in zip(u, counts) if pool.lengths[x] + k > pool.max_items]
+        if over:
+            raise ValueError(f"Cobra.extend_users: users {over[:8]} would exceed max_items ({pool.max_items}); release them first")
+        need = sum(pool._pages_for(pool.lengths[x] + k) - pool._pages_for(pool.lengths[x]) for x, k in zip(u, counts))
+        if need > len(pool.free):
+            raise ValueError(f"Cobra.extend_users: the call needs {need} pages and {len(pool.free)} are free; release users first")
+        if not any(counts):
+            return
+        require_cuda(input_ids, encoder_input_ids)
+        ensure_device(input_ids.device)
+        training = self.training
+        self.train(False)
+        try:
+            with torch.no_grad():
+                self._extend(pool, u, counts, input_ids, encoder_input_ids, versions)
+        finally:
+            self.train(training)
+
+    def _extend(self, pool, u, counts, input_ids, encoder_input_ids, versions):
+        C, D = self.C, self.d_model
+        B, n, L = encoder_input_ids.shape
+        dev = input_ids.device
+        mask_items = (input_ids != self.pad_id).view(B, n, C)
+        keep = mask_items[:, :, C - 1].reshape(-1).to(torch.uint8).contiguous()
+        vecs = self._encode(encoder_input_ids.reshape(B * n, L), keep).view(B, n, -1)   # refuses a malformed text before any write
+        # the host bookkeeping: pages in row order, then one copy of the call's index arrays
+        rows = [b for b in range(B) if counts[b]]
+        start = [pool.lengths[u[b]] * (C + 1) for b in range(B)]
+        for b in rows:
+            x = u[b]
+            for _ in range(pool._pages_for(pool.lengths[x] + counts[b]) - len(pool.pages[x])):
+                pool.pages[x].append(pool.free.pop())
+            pool.lengths[x] += counts[b]
+        pool.param_versions = versions
+        cols = pool.page_table.shape[1]
+        table = torch.zeros(len(rows), cols, dtype=torch.int32)
+        for i, b in enumerate(rows):
+            table[i, :len(pool.pages[u[b]])] = torch.tensor(pool.pages[u[b]], dtype=torch.int32)
+        new = [counts[b] * (C + 1) for b in rows]
+        q_off = [0]
+        for k in new:
+            q_off.append(q_off[-1] + k)
+        R = q_off[-1]
+        users = [u[b] for b in rows]
+        hist = [start[b] + k for b, k in zip(rows, new)]
+        row_pos = [start[b] + j for b, k in zip(rows, new) for j in range(k)]
+        row_user = [u[b] for b, k in zip(rows, new) for _ in range(k)]
+        meta = torch.tensor(users + hist + q_off + row_pos + row_user + [p + 1 for p in row_pos], dtype=torch.int32).to(dev)
+        nb = len(rows)
+        users_d, hist_d, q_off_d = meta[:nb], meta[nb:2 * nb], meta[2 * nb:3 * nb + 1]
+        pos_d, user_d, keys_d = meta[3 * nb + 1:3 * nb + 1 + R], meta[3 * nb + 1 + R:3 * nb + 1 + 2 * R], meta[3 * nb + 1 + 2 * R:]
+        pool.page_table.index_copy_(0, users_d.long(), table.to(dev))
+        # the new items' decoder rows, packed in row order, at positions that continue each history
+        emb, seq_mask = self._interleave(input_ids, vecs, mask_items, torch.tensor(start, dtype=torch.int64).to(dev))
+        x = emb[seq_mask]
+        ps, max_keys = pool.page_size, max(hist)
+        for i, layer in enumerate(self.decoder.decoder.layers):
+            sa = layer.self_attn
+            kv = pool.kv[i]
+
+            def attend(qkv):
+                Fn.cobra_kv_scatter(qkv, kv, pool.page_table, ps, user_d, pos_d)
+                return Fn.cobra_paged_attention(qkv[:, :D], kv[..., :D], kv[..., D:], pool.page_table, ps, users_d, hist_d, max_keys, q_off_d,
+                                                keys_d, sa.num_heads)
+            x = self._cached_layer(i, layer, x, (Fn.cast_bf16(sa.in_proj_weight), Fn.cast_bf16(sa.out_proj.weight)), attend)
+        pool.last_hidden.index_copy_(0, users_d.long(), x[q_off_d[1:].long() - 1])
+
+    def _check_pool_users(self, pool, users, K, temperature, k_name, fn):
+        self._check_pool(pool)
+        u = pool._users(users, fn)
+        self._check_beams(K, temperature, k_name)
+        empty = [x for x in u if pool.lengths[x] == 0]
+        if empty:
+            raise ValueError(f"{fn}: users {empty[:8]} have no item")
+        return u
+
+    def _pool_beams(self, pool, u, K, temperature) -> CobraGenerationOutput:
+        C, D = self.C, self.d_model
+        dev = pool.kv.device
+        ensure_device(dev)
+        B = len(u)
+        hist = [pool.lengths[x] * (C + 1) for x in u]
+        meta = torch.tensor(u + hist + [b * K for b in range(B + 1)], dtype=torch.int32).to(dev)
+        users_d, hist_d, q_off_d = meta[:B], meta[B:2 * B], meta[2 * B:]
+        q_keys = hist_d.repeat_interleave(K)
+        training = self.training
+        self.train(False)
+
+        def attend(i, q, suf, anc, S, H):
+            kv = pool.kv[i]
+            return Fn.cobra_paged_attention(q, kv[..., :D], kv[..., D:], pool.page_table, pool.page_size, users_d, hist_d, max(hist), q_off_d,
+                                            q_keys, H, suf, anc, S)
+        try:
+            return self._beams(pool.last_hidden[users_d.long()], hist_d, K, temperature, attend)
+        finally:
+            self.train(training)
+
+    def generate_users(self, pool: CobraPool, users, n_candidates: int = 10, temperature: float = 1.0) -> CobraGenerationOutput:
+        """generate's beam search for each of ``users`` from the pool: started from the user's ``last_hidden``, generated token j at
+        position n_u (C+1) + j, the history's K | V read from the user's pages.  Same outputs and order as generate."""
+        u = self._check_pool_users(pool, users, n_candidates, temperature, "n_candidates", "Cobra.generate_users")
+        with torch.no_grad():
+            return self._pool_beams(pool, u, n_candidates, temperature)
+
+    def beam_fusion_users(self, pool: CobraPool, users, item_dense_vecs: torch.Tensor, item_sem_ids: torch.Tensor, n_candidates: int = 10,
+                          n_beam: int = 50, temperature: float = 1.0, alpha: float = 0.5) -> BeamFusionOutput:
+        """beam_fusion on generate_users(n_beam): the same catalog sweep and fusion tail."""
+        self._check_catalog("Cobra.beam_fusion_users", n_candidates, n_beam, item_dense_vecs, item_sem_ids)
+        u = self._check_pool_users(pool, users, n_beam, temperature, "n_beam", "Cobra.beam_fusion_users")
+        require_cuda(item_dense_vecs, item_sem_ids)
+        with torch.no_grad():
+            return self._fuse(self._pool_beams(pool, u, n_beam, temperature), item_dense_vecs, item_sem_ids, n_candidates, n_beam, alpha)

@@ -2139,6 +2139,14 @@ int cobra_attn_check(int B, int K, int H, int head_dim, int hist_rows) {
     return 0;
 }
 int cobra_attn_splits(int hist_rows) { return (hist_rows + CBA_CHUNK - 1) / CBA_CHUNK; }
+int cobra_attn_launch(const CobraBeamAttnArgs& a, int head_dim, cudaStream_t st) {
+    const unsigned merge_blocks = (unsigned)(((long long)a.R * a.H + CBA_THREADS / 32 - 1) / (CBA_THREADS / 32));
+    return with_head_dim(head_dim, [&](auto DH) {
+        GRB_LAUNCH(cobra_attn_part_kernel<DH>, (unsigned)(a.B * a.H * a.splits), CBA_THREADS, 0, st, a);
+        GRB_LAUNCH(cobra_attn_merge_kernel<DH>, merge_blocks, CBA_THREADS, 0, st, a);
+        return 0;
+    });
+}
 }  // namespace
 
 size_t grb_cobra_beam_attention_workspace_bytes(int B, int K, int H, int head_dim, int hist_rows) {
@@ -2158,16 +2166,55 @@ int grb_cobra_beam_attention(const void* q, int ldq, const void* hist_k, const v
                 "leading dimensions below H * head_dim = %d, or suffix steps overlap", D);
     GRB_REQUIRE(ldq % 2 == 0 && ld_hist % 2 == 0 && aligned16(hist_k) && aligned16(hist_v) && aligned16(workspace),
                 "hist_k / hist_v / workspace must be 16-byte aligned and ldq, ld_hist even");
-    CobraBeamAttnArgs a{(const bf16*)q, ldq, (const bf16*)hist_k, (const bf16*)hist_v, ld_hist, hist_rows, hist_len, (const bf16*)suf_k,
-                        (const bf16*)suf_v, ld_suf, (long long)suf_step_stride, anc, S, B, K, H, cobra_attn_splits(hist_rows),
-                        1.f / sqrtf((float)head_dim), static_cast<float*>(workspace), static_cast<bf16*>(out), ldo};
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const unsigned merge_blocks = (unsigned)(((long long)B * K * H + CBA_THREADS / 32 - 1) / (CBA_THREADS / 32));
-    return with_head_dim(head_dim, [&](auto DH) {
-        GRB_LAUNCH(cobra_attn_part_kernel<DH>, (unsigned)(B * H * a.splits), CBA_THREADS, 0, st, a);
-        GRB_LAUNCH(cobra_attn_merge_kernel<DH>, merge_blocks, CBA_THREADS, 0, st, a);
-        return 0;
-    });
+    CobraBeamAttnArgs a{(const bf16*)q, ldq, (const bf16*)hist_k, (const bf16*)hist_v, ld_hist, KvPages{nullptr, 1, hist_rows}, nullptr,
+                        hist_len, nullptr, nullptr, (const bf16*)suf_k, (const bf16*)suf_v, ld_suf, (long long)suf_step_stride, anc, S, B, K,
+                        B * K, H, cobra_attn_splits(hist_rows), 1.f / sqrtf((float)head_dim), static_cast<float*>(workspace),
+                        static_cast<bf16*>(out), ldo};
+    return cobra_attn_launch(a, head_dim, static_cast<cudaStream_t>(stream));
+}
+
+size_t grb_cobra_paged_attention_workspace_bytes(int R, int H, int head_dim, int max_keys) {
+    if (cobra_attn_check(1, 1, H, head_dim, max_keys) || R < 1) return 0;
+    return (size_t)R * H * cobra_attn_splits(max_keys) * (head_dim + 2) * 4;
+}
+
+int grb_cobra_paged_attention(const void* q, int ldq, const void* k, const void* v, int ld_kv, const int32_t* page_table, int pt_ld,
+                              int page_size, const int32_t* users, const int32_t* hist_len, int max_keys, const int32_t* q_off,
+                              const int32_t* q_keys, int R, const void* suf_k, const void* suf_v, int ld_suf, int64_t suf_step_stride,
+                              const int32_t* anc, int S, int B, int H, int head_dim, void* out, int ldo, void* workspace, void* stream) {
+    GRB_TRY(cobra_attn_check(B, 1, H, head_dim, max_keys));
+    GRB_REQUIRE(R >= 1, "bad shape R=%d query rows", R);
+    GRB_REQUIRE(q && k && v && hist_len && q_off && q_keys && out && workspace, "null argument");
+    GRB_REQUIRE(S >= 0 && (S == 0 || (suf_k && suf_v)) && (S <= 1 || anc), "S=%d suffix keys need suf_k, suf_v (and anc for S > 1)", S);
+    if (page_table) {
+        GRB_REQUIRE(page_size >= 64 && page_size % 64 == 0, "page_size=%d must be a positive multiple of 64", page_size);
+        GRB_REQUIRE((long long)pt_ld * page_size >= max_keys, "page table rows of %d pages of %d cannot hold %d keys", pt_ld, page_size,
+                    max_keys);
+    } else {
+        GRB_REQUIRE(page_size >= max_keys, "dense rows per user page_size=%d below max_keys=%d", page_size, max_keys);
+    }
+    const int D = H * head_dim;
+    GRB_REQUIRE(ldq >= D && ld_kv >= D && ldo >= D && (S == 0 || (ld_suf >= D && suf_step_stride >= (int64_t)R * ld_suf)),
+                "leading dimensions below H * head_dim = %d, or suffix steps overlap", D);
+    GRB_REQUIRE(ldq % 2 == 0 && ld_kv % 2 == 0 && aligned16(k) && aligned16(v) && aligned16(workspace),
+                "k / v / workspace must be 16-byte aligned and ldq, ld_kv even");
+    CobraBeamAttnArgs a{(const bf16*)q, ldq, (const bf16*)k, (const bf16*)v, ld_kv, KvPages{page_table, pt_ld, page_size}, users, hist_len,
+                        q_off, q_keys, (const bf16*)suf_k, (const bf16*)suf_v, ld_suf, (long long)suf_step_stride, anc, S, B, 1, R, H,
+                        cobra_attn_splits(max_keys), 1.f / sqrtf((float)head_dim), static_cast<float*>(workspace), static_cast<bf16*>(out),
+                        ldo};
+    return cobra_attn_launch(a, head_dim, static_cast<cudaStream_t>(stream));
+}
+
+int grb_cobra_kv_scatter(const void* qkv, int ld_qkv, int R, int D, const int32_t* page_table, int pt_ld, int page_size,
+                         const int32_t* row_user, const int32_t* row_pos, void* kv, void* stream) {
+    GRB_REQUIRE(qkv && page_table && row_user && row_pos && kv, "null argument");
+    GRB_REQUIRE(R >= 1 && D >= 8 && D % 8 == 0 && pt_ld >= 1, "bad shape R=%d D=%d pt_ld=%d (D a multiple of 8)", R, D, pt_ld);
+    GRB_REQUIRE(page_size >= 64 && page_size % 64 == 0, "page_size=%d must be a positive multiple of 64", page_size);
+    GRB_REQUIRE(ld_qkv >= 3 * D && ld_qkv % 8 == 0 && aligned16(qkv) && aligned16(kv),
+                "qkv [R, ld_qkv >= 3D] with ld_qkv a multiple of 8, qkv and kv 16-byte aligned");
+    GRB_LAUNCH(cobra_kv_scatter_kernel, (unsigned)((R + 7) / 8), 256, 0, static_cast<cudaStream_t>(stream), (const bf16*)qkv, ld_qkv, R, D,
+               KvPages{page_table, pt_ld, page_size}, row_user, row_pos, static_cast<bf16*>(kv));
+    return 0;
 }
 
 namespace {

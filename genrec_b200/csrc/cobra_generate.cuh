@@ -3,10 +3,15 @@
 // The decoder runs once over each user's history (the prefill keeps every layer's QKV); each later codebook is one new token per
 // beam, whose self-attention reads the history's K | V in place and the beam's own earlier tokens through an ancestry table:
 //   cobra_attn_part_kernel     one CTA per (user, head, 128-key range of the history): the range's bf16 K / V loaded into shared
-//                              memory once and scored against every beam's query (one warp per query, one key per lane); each
-//                              query leaves its range's {acc[DH], max, sum} in the workspace
-//   cobra_attn_merge_kernel    one warp per (beam row, head): the ranges merged in range order, then the beam's suffix keys (its
+//                              memory once and scored against every query of the user (one warp per query, one key per lane);
+//                              each query leaves its range's {acc[DH], max, sum} in the workspace
+//   cobra_attn_merge_kernel    one warp per (query row, head): the ranges merged in range order, then the beam's suffix keys (its
 //                              ancestors' tokens of earlier steps and its own), softmax in fp32, bf16 out
+// The same two kernels serve the paged per-user pool (Cobra.new_pool): the history keys are addressed through KvPages (a null page
+// table is the prefill's dense layout), a user has any number of queries (packed by offsets), and each query sees the keys 0 ..
+// q_keys[r]-1.  The key ranges are fixed 128-position ranges of absolute position merged in order, so a query's result depends on
+// its key limit and the keys' contents only, not on how the history was written or which users share the call.
+//   cobra_kv_scatter_kernel    one warp per new decoder row: its K | V columns of the layer's QKV copied into the user's page row
 //   cobra_beam_topk_kernel     one CTA per user: log_softmax(logits / temperature) per row plus the parent's score, and the K best
 //                              of the user's K_in * V totals (beam_radix_topk of beam.cuh), best first, equal totals by the lower
 //                              flat index; COBRA's parents are distinct and a parent's tokens are distinct, so nothing repeats and
@@ -16,6 +21,7 @@
 //   cobra_dense_merge_kernel   the ranges' winners in range order
 // Every sum runs in a fixed order and no kernel uses atomics on values, so a user's results do not depend on the batch around it.
 #pragma once
+#include "attn_hstu_extend.cuh"
 #include "beam.cuh"
 #include "head_sweep.cuh"
 
@@ -28,18 +34,21 @@ constexpr int CBA_MAX_K = 1024;
 constexpr int CBA_MAX_HIST = 8192;
 
 struct CobraBeamAttnArgs {
-    const bf16* q; int ldq;                     // [B K, ldq]: beam row b K + k, head h at columns h DH ..
-    const bf16* hk; const bf16* hv; int ldh;    // user b's key j at hk[(b hist_rows + j) ldh + h DH] (the prefill's QKV, in place)
-    int hist_rows;
-    const int* hist_len;                        // [B]: user b's keys are rows 0 .. hist_len[b]-1
+    const bf16* q; int ldq;                     // [R, ldq]: query row r, head h at columns h DH ..
+    const bf16* hk; const bf16* hv; int ldh;    // call row b's key j at hk[pg.row(u, j) ldh + h DH], u = users[b] (b without a list)
+    KvPages pg;                                 // null page table: the prefill's QKV in place, page_size = its rows per user
+    const int* users;                           // [B] page-table row of call row b, or null
+    const int* hist_len;                        // [B]: call row b's keys are rows 0 .. hist_len[b]-1
+    const int* q_off;                           // [B + 1]: call row b's queries are rows q_off[b] .. q_off[b+1]-1; null: b K .. b K + K-1
+    const int* q_keys;                          // [R]: query r sees the keys 0 .. q_keys[r]-1 (<= hist_len of its row); null: hist_len[b]
     const bf16* sk; const bf16* sv; int lds;    // suffix step s, row r at sk[s step_stride + r lds]
     long long step_stride;
-    const int* anc;                             // [B K, S - 1]: the row of step s < S - 1 the beam descends from; step S - 1 is its own row
-    int S;
-    int B, K, H, splits;
+    const int* anc;                             // [R, S - 1]: the row of step s < S - 1 the beam descends from; step S - 1 is its own row
+    int S;                                      // suffix keys per query (0: none)
+    int B, K, R, H, splits;
     float scale;
-    float* part;                                // [B H splits, K, DH + 2] {acc[DH], max, sum}
-    bf16* out; int ldo;                         // [B K, ldo]
+    float* part;                                // [R H splits, DH + 2] {acc[DH], max, sum}
+    bf16* out; int ldo;                         // [R, ldo]
 };
 
 template <int DH>
@@ -55,23 +64,29 @@ __global__ void __launch_bounds__(CBA_THREADS) cobra_attn_part_kernel(CobraBeamA
     const int len = a.hist_len[b];
     if (j0 >= len) return;                      // the merge skips this range
     const int n = min(CBA_CHUNK, len - j0);
+    const int u = a.users ? a.users[b] : b;
     for (int e = threadIdx.x; e < n * (DH / 2); e += CBA_THREADS) {
         const int j = e / (DH / 2), d2 = e - j * (DH / 2);
-        const size_t g = ((size_t)b * a.hist_rows + j0 + j) * a.ldh + h * DH + 2 * d2;
+        const size_t g = a.pg.row(u, j0 + j) * a.ldh + h * DH + 2 * d2;
         *reinterpret_cast<uint32_t*>(&sK[j * LDS + 2 * d2]) = *reinterpret_cast<const uint32_t*>(a.hk + g);
         *reinterpret_cast<uint32_t*>(&sV[j * LDS + 2 * d2]) = *reinterpret_cast<const uint32_t*>(a.hv + g);
     }
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int k = warp; k < a.K; k += CBA_THREADS / 32) {
-        const bf16* qr = a.q + ((size_t)b * a.K + k) * a.ldq + h * DH;
+    const int r0 = a.q_off ? a.q_off[b] : b * a.K;
+    const int nq = a.q_off ? a.q_off[b + 1] - r0 : a.K;
+    for (int k = warp; k < nq; k += CBA_THREADS / 32) {
+        const int r = r0 + k;
+        const int nk = a.q_keys ? min(n, a.q_keys[r] - j0) : n;     // the keys of this range the query sees
+        if (nk <= 0) continue;                  // warp-uniform; the merge stops before this range
+        const bf16* qr = a.q + (size_t)r * a.ldq + h * DH;
 #pragma unroll
         for (int i = 0; i < DH / 32; ++i) sQ[warp][lane + 32 * i] = __bfloat162float(qr[lane + 32 * i]);
         __syncwarp();
         float m = -INFINITY, l = 0.f, acc[DH];
 #pragma unroll
         for (int d = 0; d < DH; ++d) acc[d] = 0.f;
-        for (int j = lane; j < n; j += 32) {
+        for (int j = lane; j < nk; j += 32) {
             const uint32_t* kr = reinterpret_cast<const uint32_t*>(&sK[j * LDS]);
             float s = 0.f;
 #pragma unroll
@@ -100,7 +115,7 @@ __global__ void __launch_bounds__(CBA_THREADS) cobra_attn_part_kernel(CobraBeamA
         l *= f;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
-        float* dst = a.part + ((size_t)blockIdx.x * a.K + k) * (DH + 2);
+        float* dst = a.part + (((size_t)r * a.H + h) * a.splits + sp) * (DH + 2);
 #pragma unroll
         for (int d = 0; d < DH; ++d) {
             float v = acc[d] * f;
@@ -118,19 +133,18 @@ __global__ void __launch_bounds__(CBA_THREADS) cobra_attn_merge_kernel(CobraBeam
     pdl_wait();
     constexpr int PER = DH / 32;                // dims of a lane: lane + 32 i
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const long long item = (long long)blockIdx.x * (CBA_THREADS / 32) + warp;       // (beam row, head)
-    if (item >= (long long)a.B * a.K * a.H) return;
+    const long long item = (long long)blockIdx.x * (CBA_THREADS / 32) + warp;       // (query row, head)
+    if (item >= (long long)a.R * a.H) return;
     const int h = (int)(item % a.H);
     const int r = (int)(item / a.H);
-    const int b = r / a.K, k = r - b * a.K;
     float q[PER], acc[PER];
     const bf16* qr = a.q + (size_t)r * a.ldq + h * DH;
 #pragma unroll
     for (int i = 0; i < PER; ++i) { q[i] = __bfloat162float(qr[lane + 32 * i]); acc[i] = 0.f; }
     float M = -INFINITY, L = 0.f;
-    const int len = a.hist_len[b];
+    const int len = a.q_keys ? a.q_keys[r] : a.hist_len[r / a.K];
     for (int sp = 0; sp < a.splits && sp * CBA_CHUNK < len; ++sp) {
-        const float* src = a.part + (((size_t)(b * a.H + h) * a.splits + sp) * a.K + k) * (DH + 2);
+        const float* src = a.part + (((size_t)r * a.H + h) * a.splits + sp) * (DH + 2);
         const float m = src[DH], l = src[DH + 1];
         const float Mn = fmaxf(M, m);
         const float fa = __expf(M - Mn), fb = __expf(m - Mn);
@@ -158,6 +172,19 @@ __global__ void __launch_bounds__(CBA_THREADS) cobra_attn_merge_kernel(CobraBeam
     bf16* o = a.out + (size_t)r * a.ldo + h * DH;
 #pragma unroll
     for (int i = 0; i < PER; ++i) o[lane + 32 * i] = __float2bfloat16(__fdiv_rn(acc[i], L));
+}
+
+// Row r of a layer's QKV [R, ld_qkv] (K | V at columns D .. 3D-1) goes to row pg.row(row_user[r], row_pos[r]) of that layer's pages
+// kv [pages page_size, 2D]; 16-byte copies, D a multiple of 8.
+__global__ void __launch_bounds__(256) cobra_kv_scatter_kernel(const bf16* __restrict__ qkv, int ld_qkv, int R, int D, KvPages pg,
+                                                               const int* __restrict__ row_user, const int* __restrict__ row_pos,
+                                                               bf16* __restrict__ kv) {
+    pdl_wait();
+    const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (r >= R) return;
+    const uint4* src = reinterpret_cast<const uint4*>(qkv + (size_t)r * ld_qkv + D);
+    uint4* dst = reinterpret_cast<uint4*>(kv + pg.row(row_user[r], row_pos[r]) * (size_t)(2 * D));
+    for (int i = lane; i < D / 4; i += 32) dst[i] = src[i];
 }
 
 // ------------------------------------------------------------------------------------------------ beam step

@@ -1149,6 +1149,34 @@ def cobra_beam_attention(q, hist_qkv, hist_len, suf_qkv, anc, S: int, H: int) ->
     return out
 
 
+def cobra_paged_attention(q, k, v, page_table, page_size: int, users, hist_len, max_keys: int, q_off, q_keys, H: int, suf_qkv=None,
+                          anc=None, S: int = 0) -> torch.Tensor:
+    """The attention of cobra_beam_attention for queries packed by user, history keys through a page table
+    (grb_cobra_paged_attention).  q [R, D] bf16 (a column view); k / v: column views of the key rows (the pool's [pages page_size, 2D]
+    for a layer, or with page_table None the prefill's QKV, page_size rows per user); users [B] int32 page-table rows (None: 0 .. B-1);
+    hist_len [B] int32 keys per call row; q_off [B + 1] int32; q_keys [R] int32 history keys each query sees (<= max_keys); suf_qkv
+    [steps, R, 3D] bf16, anc [R, S - 1] int32 and S suffix keys as cobra_beam_attention (S = 0: none).  -> [R, D] bf16."""
+    R, D = q.shape
+    B = hist_len.numel()
+    ld_kv = k.stride(-2)
+    pt_ld = page_table.shape[1] if page_table is not None else 1
+    out = torch.empty(R, D, dtype=torch.bfloat16, device=q.device)
+    ws = workspace(q.device, "grb_cobra_paged_attention_workspace_bytes", R, H, D // H, max_keys)
+    sk, sv = (suf_qkv[..., D:2 * D], suf_qkv[..., 2 * D:]) if S else (None, None)
+    call(q.device, "grb_cobra_paged_attention", ptr(q), q.stride(0), ptr(k), ptr(v), ld_kv, ptr(page_table), pt_ld, page_size, ptr(users),
+         ptr(hist_len), max_keys, ptr(q_off), ptr(q_keys), R, ptr(sk), ptr(sv), 3 * D, suf_qkv.stride(0) if S else 0, ptr(anc), S, B, H,
+         D // H, ptr(out), D, ptr(ws))
+    return out
+
+
+def cobra_kv_scatter(qkv, kv, page_table, page_size: int, row_user, row_pos) -> None:
+    """Row r of qkv [R, 3D] bf16 writes its K | V columns into row pg(row_user[r], row_pos[r]) of kv [pages, page_size, 2D] bf16
+    (grb_cobra_kv_scatter); row_user / row_pos int32 [R]."""
+    R, D3 = qkv.shape
+    call(qkv.device, "grb_cobra_kv_scatter", ptr(qkv), qkv.stride(0), R, D3 // 3, ptr(page_table), page_table.shape[1], page_size,
+         ptr(row_user), ptr(row_pos), ptr(kv))
+
+
 def cobra_beam_topk(logits, scores_in, B: int, K: int, temperature: float, anc_in=None):
     """One beam step (grb_cobra_beam_topk): logits [B K_in, V] fp32, scores_in [B, K_in] or None (zero) -> (tokens [B, K] int64,
     scores [B, K], parents [B, K] int64, anc_out [B K, S_in + 1] int32: the parent's ancestry row and the parent's own row)."""

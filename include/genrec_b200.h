@@ -629,6 +629,26 @@ int grb_cobra_beam_attention(const void* q, int ldq, const void* hist_k, const v
                              const int32_t* hist_len, const void* suf_k, const void* suf_v, int ld_suf, int64_t suf_step_stride,
                              const int32_t* anc, int S, int B, int K, int H, int head_dim, void* out, int ldo, void* workspace,
                              void* stream);
+/* grb_cobra_paged_attention: the attention of grb_cobra_beam_attention for queries packed by user and history keys read through a
+ * page table (Cobra.new_pool).  Call row b (pool user users[b], or b when users is NULL) has the query rows q_off[b] .. q_off[b+1]-1
+ * of the R rows of q; query r sees the history keys 0 .. q_keys[r]-1 and then S suffix keys as in grb_cobra_beam_attention (S = 0:
+ * none; anc [R, S-1]).  The kernels read these device arrays unchecked: the caller guarantees q_off[0] = 0, q_off[B] = R and
+ * q_off non-decreasing, q_keys[r] <= hist_len[b] <= max_keys <= 8192 for every query r of row b, and q_keys[r] >= 1 when S = 0 (a
+ * query with no key would divide 0 by 0).  Key j of user u, head h is at k / v + (page_table[u pt_ld
+ * + j / page_size] page_size + j % page_size) ld_kv + h head_dim; page_size a positive multiple of 64.  A NULL page table is the dense
+ * layout of grb_cobra_beam_attention with page_size rows per user (page_size >= max_keys): with q_off = b K and q_keys = hist_len[b]
+ * it gives grb_cobra_beam_attention's bits.  History keys are taken in fixed 128-position ranges merged in order, so a query's
+ * result depends on q_keys[r] and the keys' contents only.  workspace: grb_cobra_paged_attention_workspace_bytes() (0 for unsupported
+ * arguments), 16-byte aligned.
+ * grb_cobra_kv_scatter: row r of qkv [R, ld_qkv] bf16 (its K | V at columns D .. 3D-1) is copied to row
+ * page_table[u pt_ld + p / page_size] page_size + p % page_size of kv [pages page_size, 2D] bf16, u = row_user[r], p = row_pos[r]. */
+size_t grb_cobra_paged_attention_workspace_bytes(int R, int H, int head_dim, int max_keys);
+int grb_cobra_paged_attention(const void* q, int ldq, const void* k, const void* v, int ld_kv, const int32_t* page_table, int pt_ld,
+                              int page_size, const int32_t* users, const int32_t* hist_len, int max_keys, const int32_t* q_off,
+                              const int32_t* q_keys, int R, const void* suf_k, const void* suf_v, int ld_suf, int64_t suf_step_stride,
+                              const int32_t* anc, int S, int B, int H, int head_dim, void* out, int ldo, void* workspace, void* stream);
+int grb_cobra_kv_scatter(const void* qkv, int ld_qkv, int R, int D, const int32_t* page_table, int pt_ld, int page_size,
+                         const int32_t* row_user, const int32_t* row_pos, void* kv, void* stream);
 /* grb_cobra_beam_topk: one beam step.  Per row of logits [B K_in, V] fp32: log_softmax(logits / temperature), plus the parent's score
  * scores_in [B, K_in] (NULL: 0); then the K best of user b's K_in V totals, best first, equal totals by the lower flat index
  * parent V + token (NaN above every number).  Writes tokens [B, K] int64, scores [B, K], parents [B, K] int32 (the
