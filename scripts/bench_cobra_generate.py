@@ -13,46 +13,21 @@ stage."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
 import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from scripts import harness  # noqa: E402
 from tests import cobra_generate_reference as gr  # noqa: E402
 from tests import cobra_params as cp  # noqa: E402
 from tests import cobra_reference as cr  # noqa: E402
 
-STAGES = (("beam attention", ("cobra_attn",)), ("beam selection", ("cobra_beam_topk",)), ("catalog match", ("cobra_dense",)),
-          ("encoder attention (T5 core)", ("t5_attn", "<96")), ("prefill attention (T5 core)", ("t5_attn",)),
-          ("GEMMs (encoder, prefill, extension, heads)", ("tc_gemm",)), ("LayerNorms", ("ln_fwd",)), ("text pooling", ("seg_ln_mean",)),
-          ("L2 norms", ("l2norm",)), ("bf16 casts", ("cast_",)))
-
-
-def stage_of(name):
-    for stage, keys in STAGES:
-        if all(k in name for k in keys):
-            return stage
-    return "torch (gathers, embeddings, residual adds, fusion tail)"
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True,
-                           timeout=30).stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        q = "unknown"
-    return dict(gpu=torch.cuda.get_device_name(0), power_limit_and_max_sm_clock=q)
-
-
-def batch(B, items, g):
-    if items == "full":
-        n = [20] * B
-    else:
-        u = torch.rand(B, generator=g, dtype=torch.float64)
-        n = (torch.log1p(-u) / torch.log1p(torch.tensor(-1 / 9, dtype=torch.float64))).ceil().clamp(1, 20).long().tolist()
-    return cp.batch(cp.TRAINER, items=n, text_lens=[128], L=128, seed=int(torch.randint(0, 1 << 30, (1,), generator=g)))
+STAGES = (("beam attention", (("cobra_attn",),)), ("beam selection", (("cobra_beam_topk",),)), ("catalog match", (("cobra_dense",),)),
+          ("encoder attention (T5 core)", (("t5_attn", "<96"),)), ("prefill attention (T5 core)", (("t5_attn",),)),
+          ("GEMMs (encoder, prefill, extension, heads)", (("tc_gemm",),)), ("LayerNorms", (("ln_fwd",),)),
+          ("text pooling", (("seg_ln_mean",),)), ("L2 norms", (("l2norm",),)), ("bf16 casts", (("cast_",),)))
 
 
 def baseline_generate(P, cfg, ids, text, K):
@@ -85,36 +60,6 @@ def baseline_generate(P, cfg, ids, text, K):
     return seqs, F.normalize(h_last, dim=-1), scores
 
 
-def timed(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(steps):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return round(s.elapsed_time(e) / steps, 2), round(torch.cuda.max_memory_allocated() / 2**30, 2)
-
-
-def profile(fn, warmup):
-    from torch.profiler import ProfilerActivity
-    from torch.profiler import profile as tprofile
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    split = {}
-    for e in prof.events():
-        if e.device_type == torch.autograd.DeviceType.CUDA:
-            split[stage_of(e.name)] = split.get(stage_of(e.name), 0.0) + e.time_range.elapsed_us() / 1000.0
-    return {k: round(v, 2) for k, v in sorted(split.items(), key=lambda kv: -kv[1])}
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
@@ -130,12 +75,12 @@ def main():
     model.load_state_dict(P)
     model = model.to(dev).eval()
     ref = {k: v.to(dev) for k, v in P.items() if k not in ("feat_queue", "queue_ptr")}
-    info = card()
+    info = harness.card(dev)
     g = torch.Generator().manual_seed(0)
     work = [("generate", B, items, 20, None) for B in (32, 256) for items in ("full", "geometric")]
     work += [("generate", 32, "full", 256, None), ("beam_fusion", 256, "full", 20, 12101), ("beam_fusion", 256, "full", 20, 1_000_000)]
     for kind, B, items, K, N in work:
-        ids, text = (t.to(dev) for t in batch(B, items, g))
+        ids, text = (t.to(dev) for t in harness.cobra_batch(B, items, g))
         row = dict(info, call=kind, B=B, items=items, n_beam=K)
         if kind == "generate":
             def native():
@@ -148,16 +93,20 @@ def main():
             def native():
                 model.beam_fusion(ids, text, vecs, sem, n_candidates=10, n_beam=K)
         if args.profile:
-            print(json.dumps(dict(row, native_kernel_ms_by_stage=profile(native, args.warmup))), flush=True)
+            by_stage = harness.by_stage(harness.profile(native, warmup=args.warmup), STAGES,
+                                        "torch (gathers, embeddings, residual adds, fusion tail)")
+            print(json.dumps(dict(row, native_kernel_ms_by_stage=by_stage)), flush=True)
             continue
-        row["native_ms"], row["native_peak_gib"] = timed(native, args.steps, args.warmup)
+        ms, mem = harness.timed(native, args.steps, args.warmup)
+        row["native_ms"], row["native_peak_gib"] = round(ms, 2), round(mem / 2**30, 2)
         if kind == "generate" and items == "full":
             for name, autocast in (("eager_fp32", False), ("eager_bf16_autocast", True)):
                 def base():
                     with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16, enabled=autocast):
                         baseline_generate(ref, cfg, ids, text, K)
                 try:
-                    row[name + "_ms"], row[name + "_peak_gib"] = timed(base, args.baseline_steps, 1)
+                    ms, mem = harness.timed(base, args.baseline_steps, 1)
+                    row[name + "_ms"], row[name + "_peak_gib"] = round(ms, 2), round(mem / 2**30, 2)
                 except torch.cuda.OutOfMemoryError:
                     row[name + "_ms"] = "out of memory"
                     torch.cuda.empty_cache()

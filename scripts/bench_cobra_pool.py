@@ -22,53 +22,13 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from scripts.bench_cobra_generate import batch, card  # noqa: E402
+from scripts import harness  # noqa: E402
 from tests import cobra_params as cp  # noqa: E402
 
-STAGES = (("paged attention", ("cobra_attn",)), ("K | V scatter", ("cobra_kv_scatter",)), ("beam steps (selection)", ("cobra_beam_topk",)),
-          ("catalog match", ("cobra_dense",)), ("encoder attention (T5 core)", ("t5_attn",)), ("GEMMs", ("tc_gemm",)),
-          ("LayerNorms", ("ln_fwd",)), ("text pooling", ("seg_ln_mean",)), ("L2 norms", ("l2norm",)), ("bf16 casts", ("cast_",)))
-
-
-def stage_of(name):
-    for stage, keys in STAGES:
-        if all(k in name for k in keys):
-            return stage
-    return "torch (gathers, embeddings, residual adds, fusion tail)"
-
-
-def event_ms(fn):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e)
-
-
-def peak(fn):
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    fn()
-    torch.cuda.synchronize()
-    return round(torch.cuda.max_memory_allocated() / 2**30, 2)
-
-
-def profile(fn, setup):
-    from torch.profiler import ProfilerActivity
-    from torch.profiler import profile as tprofile
-    setup()
-    fn()
-    setup()
-    torch.cuda.synchronize()
-    with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    split = {}
-    for e in prof.events():
-        if e.device_type == torch.autograd.DeviceType.CUDA:
-            split[stage_of(e.name)] = split.get(stage_of(e.name), 0.0) + e.time_range.elapsed_us() / 1000.0
-    return {k: round(v, 2) for k, v in sorted(split.items(), key=lambda kv: -kv[1])}
+STAGES = (("paged attention", (("cobra_attn",),)), ("K | V scatter", (("cobra_kv_scatter",),)),
+          ("beam steps (selection)", (("cobra_beam_topk",),)), ("catalog match", (("cobra_dense",),)),
+          ("encoder attention (T5 core)", (("t5_attn",),)), ("GEMMs", (("tc_gemm",),)), ("LayerNorms", (("ln_fwd",),)),
+          ("text pooling", (("seg_ln_mean",),)), ("L2 norms", (("l2norm",),)), ("bf16 casts", (("cast_",),)))
 
 
 def main():
@@ -84,12 +44,12 @@ def main():
     model = Cobra(**cfg)
     model.load_state_dict(cp.cobra_params(cp.shapes(cfg), 0))
     model = model.to(dev).eval()
-    info = card()
+    info = harness.card(dev)
     g = torch.Generator().manual_seed(0)
     work = [("extend1", 256, "full", 20), ("extend1_k256", 32, "full", 256), ("prefill", 256, "full", 20), ("fusion_1m", 256, "full", 20),
             ("geometric", 256, "geometric", 20)]
     for name, B, items, K in work:
-        ids, text = batch(B, items, g)                               # 20 items (or geometric), plus one new item below
+        ids, text = harness.cobra_batch(B, items, g)                         # 20 items (or geometric), plus one new item below
         new_ids, new_text = cp.batch(cfg, items=[1] * B, text_lens=[128], L=128, seed=1)
         n_hist = (ids.view(B, -1, C)[:, :, C - 1] != model.pad_id).sum(1)
         # the new item right after each user's real ones, so that a geometric history stays right-padded
@@ -126,14 +86,18 @@ def main():
             held = int(n_hist.sum() + B) * (C + 1) * layers * 2 * D * 2
         row = dict(info, workload=name, B=B, items=items, n_beam=K, pool_kv_bytes=held)
         if args.profile:
-            print(json.dumps(dict(row, pool_kernel_ms_by_stage=profile(pool_call, setup))), flush=True)
+            setup()
+            pool_call()
+            setup()
+            kernels = harness.profile(pool_call, warmup=0)
+            by_stage = harness.by_stage(kernels, STAGES, "torch (gathers, embeddings, residual adds, fusion tail)")
+            print(json.dumps(dict(row, pool_kernel_ms_by_stage=by_stage)), flush=True)
             continue
         tp, tn = [], []
         for i in range(args.warmup + args.steps):
             setup()
-            torch.cuda.synchronize()
-            a = event_ms(pool_call)
-            b = event_ms(native) if native else None
+            a = harness.timed(pool_call, 1, 0)[0]
+            b = harness.timed(native, 1, 0)[0] if native else None
             if i >= args.warmup:
                 tp.append(a)
                 if native:
@@ -141,11 +105,11 @@ def main():
         setup()
         row["pool_ms"] = round(statistics.median(tp), 2)
         base = torch.cuda.memory_allocated() / 2**30
-        row["pool_peak_gib"] = peak(pool_call)
+        row["pool_peak_gib"] = round(harness.peak(pool_call) / 2**30, 2)
         row["pool_held_gib_after"] = round(base, 2)
         if native:
             row["native_ms"] = round(statistics.median(tn), 2)
-            row["native_peak_gib"] = peak(native)
+            row["native_peak_gib"] = round(harness.peak(native) / 2**30, 2)
             row["pool_over_native"] = round(row["pool_ms"] / row["native_ms"], 3)
         print(json.dumps(row), flush=True)
         del pool

@@ -16,7 +16,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -24,6 +23,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+from scripts import harness  # noqa: E402
 
 CFG2 = dict(num_items=12101, embed_dim=128, num_heads=4, num_blocks=4)
 CFG3 = dict(num_items=12101, embed_dim=256, num_heads=8, num_blocks=8)
@@ -37,21 +37,14 @@ WORKLOADS = {   # name: (geometry, pool users, max_items, B, history before the 
 }
 
 
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                       text=True)
-    return dict(gpu=torch.cuda.get_device_name(0), power_limit_and_max_sm_clock=q.stdout.strip() or "unknown")
-
-
-def lengths_of(rule, B, g):
+def user_lengths(rule, B, g):
+    """B users' item counts under a workload's (kind, lo, hi) rule; geometric has mean 4, cut at hi"""
     kind, lo, hi = rule
     if kind == "full":
         return torch.full((B,), hi, dtype=torch.int64)
     if kind == "uniform":
         return torch.randint(lo, hi + 1, (B,), generator=g)
-    p = 0.25                                           # geometric on 1, 2, ... with mean 4, cut at hi
-    u = torch.rand(B, generator=g, dtype=torch.float64)
-    return (torch.floor(torch.log1p(-u) / torch.log1p(torch.tensor(-p, dtype=torch.float64))) + 1).long().clamp(lo, hi)
+    return harness.geometric_lengths(B, 4, lo, hi, g)
 
 
 def items_of(lens, V, g, t0):
@@ -87,8 +80,8 @@ def setup(name, dev):
     m = HSTU(max_seq_len=cap, dropout=0.0, **geo).to(dev).eval()
     users = torch.randperm(nusers, generator=g)[:B]
     t0 = torch.full((B,), 1_300_000_000, dtype=torch.int64)
-    hist = lengths_of(hist_rule, B, g) if hist_rule else torch.zeros(B, dtype=torch.int64)
-    new = lengths_of(new_rule, B, g)
+    hist = user_lengths(hist_rule, B, g) if hist_rule else torch.zeros(B, dtype=torch.int64)
+    new = user_lengths(new_rule, B, g)
     pages = int(((hist + new + 63) // 64).sum()) + 8
     pool = m.new_pool(max_users=nusers, num_pages=pages, page_size=64, max_items=cap)
     if hist_rule:
@@ -98,49 +91,6 @@ def setup(name, dev):
         t0 = torch.stack([t[-1] for t in hts])
     nids, nts = items_of(new, geo["num_items"], g, t0)
     return m, pool, users.to(dev), padded(nids, nts, dev), packed(nids, nts, dev), int(new.max())
-
-
-def graphed(call, warmup=2):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(warmup):
-            call()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        out = call()
-    return g, out
-
-
-def time_graph(g, steps):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    g.replay()
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(steps):
-        g.replay()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / steps
-
-
-def kernel_us(call):
-    """device time (us) per kernel of one eager call, from torch.profiler, largest first"""
-    from torch.profiler import ProfilerActivity, profile
-    call()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        call()
-        torch.cuda.synchronize()
-    out = {}
-    for k in prof.key_averages():
-        if k.device_time_total <= 0:
-            continue
-        name = k.key.split("(")[0].replace("void ", "").replace("grb::", "")[:60]
-        out[name] = round(out.get(name, 0.0) + k.device_time_total, 1)
-    return dict(sorted(out.items(), key=lambda kv: -kv[1]))
 
 
 def run(name, steps, dev, info, profile):
@@ -167,11 +117,11 @@ def run(name, steps, dev, info, profile):
         del first
     assert torch.equal(res["padded"]["first"], res["packed"]["first"]), "the packed call's logits differ from the padded call's"
     for path, call in calls.items():
-        res[path]["graph"] = graphed(lambda call=call: (restore(), call())[1])[0]
+        res[path]["graph"] = harness.graphed(lambda call=call: (restore(), call())[1], 2)[0]
     times = {"padded": [], "packed": []}
     for _ in range(3):
         for path in ("padded", "packed"):
-            times[path].append(time_graph(res[path]["graph"], steps))
+            times[path].append(harness.timed(res[path]["graph"].replay, steps, 1)[0])
     out = dict(workload=name, desc=desc, B=B, pool_users=nusers, max_items=cap, aim=aim, padded_tokens=pi.numel(),
                packed_tokens=ids.numel(), padding_share=round(1 - ids.numel() / pi.numel(), 4), first_call_equal=True, **info)
     for path in ("padded", "packed"):
@@ -181,7 +131,8 @@ def run(name, steps, dev, info, profile):
     if profile:
         for path, call in calls.items():
             res[path]["graph"].reset()
-            out[path]["kernels_us"] = kernel_us(lambda call=call: (restore(), call())[1])
+            kernels = harness.largest_first(harness.profile(lambda call=call: (restore(), call())[1]), lambda k: harness.short_name(k)[:60])
+            out[path]["kernels_us"] = {k: round(us, 1) for k, us in kernels.items()}
     print(json.dumps(out), flush=True)
 
 
@@ -194,7 +145,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_extend_jagged.py measures on a CUDA device; none is visible")
     dev = torch.device("cuda:0")
-    info = card()
+    info = harness.card(dev)
     prof = set(args.profile.split(",")) if args.profile else set()
     for name in args.workloads.split(","):
         run(name, args.steps, dev, info, name in prof)

@@ -14,7 +14,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -22,6 +21,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+from scripts import harness  # noqa: E402
 
 CFG2 = dict(num_items=12101, max_seq_len=200, embed_dim=128, num_heads=4, num_blocks=4)
 WORKLOADS = {
@@ -33,25 +33,14 @@ WORKLOADS = {
 B = 128
 
 
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                       text=True)
-    return dict(gpu=torch.cuda.get_device_name(0), power_limit_and_max_sm_clock=q.stdout.strip() or "unknown")
-
-
-def lengths_of(kind, g):
-    if kind == "uniform":
-        return torch.randint(50, 201, (B,), generator=g)
-    if kind == "full":
-        return torch.full((B,), 200)
-    p = 1.0 / 10                                       # geometric on 1, 2, ... with mean 10
-    u = torch.rand(B, generator=g, dtype=torch.float64)
-    return (torch.floor(torch.log1p(-u) / torch.log1p(torch.tensor(-p, dtype=torch.float64))) + 1).long().clamp(1, 50)
-
-
 def jagged_batch(kind, V, seed, dev):
     g = torch.Generator().manual_seed(seed)
-    lens = lengths_of(kind, g)
+    if kind == "uniform":
+        lens = torch.randint(50, 201, (B,), generator=g)
+    elif kind == "full":
+        lens = torch.full((B,), 200)
+    else:
+        lens = harness.geometric_lengths(B, 10, 1, 50, g)
     N = int(lens.sum())
     w = torch.arange(1, V + 1, dtype=torch.float64).pow(-1.1)
     items = torch.multinomial(w, N, replacement=True, generator=g) + 1
@@ -72,47 +61,7 @@ def make(model_cfg, dev):
     return m, opt
 
 
-def graphed(step, warmup=3):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(warmup):
-            step()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        out = step()
-    return g, out
-
-
-def time_graph(g, steps):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    g.replay()
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(steps):
-        g.replay()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / steps
-
-
-def attn_us(step):
-    """device time (us) of the HSTU attention kernels, the bias index and the idle-row zeroing in one eager step, from torch.profiler"""
-    from torch.profiler import ProfilerActivity, profile
-    step()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        step()
-        torch.cuda.synchronize()
-    ev = prof.key_averages()
-    attn = {}
-    for k in ev:
-        if "hstu_attn" in k.key or "hstu_bias_index" in k.key or "hstu_idle_rows" in k.key:
-            name = k.key.split("<")[0].replace("void ", "").replace("grb::", "")
-            attn[name] = round(attn.get(name, 0.0) + k.device_time_total, 1)
-    return attn
+ATTENTION_KERNELS = ("hstu_attn", "hstu_bias_index", "hstu_idle_rows")    # the attention, its bias index and the idle-row zeroing
 
 
 def run(name, steps, dev, info):
@@ -142,14 +91,14 @@ def run(name, steps, dev, info):
                                                        # and the other path's buffers
         torch.cuda.reset_peak_memory_stats()
         loss0 = step().item()                          # the first step's loss, from the same initial parameters on both paths
-        g, _ = graphed(step)
+        g, _ = harness.graphed(step, 3)
         g.replay()
         torch.cuda.synchronize()
         res[path] = dict(model=m, opt=opt, step=step, graph=g, loss0=loss0, peak_mb=(torch.cuda.max_memory_allocated() - base) / 2 ** 20)
     times = {"padded": [], "packed": []}
     for _ in range(3):
         for path in ("padded", "packed"):
-            times[path].append(time_graph(res[path]["graph"], steps))
+            times[path].append(harness.timed(res[path]["graph"].replay, steps, 1)[0])
     out = dict(workload=name, desc=desc, B=B, **{k: model_cfg[k] for k in ("embed_dim", "num_heads", "num_blocks", "num_items")},
                padded_L=L, padded_tokens=B * L, packed_tokens=T, padding_share=round(1 - T / (B * L), 4), **info)
     for path in ("padded", "packed"):
@@ -160,7 +109,9 @@ def run(name, steps, dev, info):
     out["loss_rel_diff"] = abs(res["packed"]["loss0"] - res["padded"]["loss0"]) / abs(res["padded"]["loss0"])
     for path in ("padded", "packed"):
         res[path]["graph"].reset()
-        out[path]["attention_kernels_us"] = attn_us(res[path]["step"])
+        attn = {k: v for k, v in harness.profile(res[path]["step"]).items() if any(part in k for part in ATTENTION_KERNELS)}
+        attn = harness.largest_first(attn, lambda k: harness.short_name(k, "<"))
+        out[path]["attention_kernels_us"] = {k: round(us, 1) for k, us in attn.items()}
     print(json.dumps(out), flush=True)
     return out
 
@@ -173,7 +124,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_jagged.py measures on a CUDA device; none is visible")
     dev = torch.device("cuda:0")
-    info = card()
+    info = harness.card(dev)
     for name in args.workloads.split(","):
         run(name, args.steps, dev, info)
 

@@ -14,62 +14,20 @@ import torch
 
 import genrec_b200.functional as Fn
 from genrec_b200.hstu import HSTULayer
+from scripts import harness
 
 
-def timed(fn, iters=20, warm=5):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
+def graph_ms(fn, reps=10, iters=10):
+    """Device time (ms) per call with `reps` calls captured in one CUDA graph (no host gaps: what a small kernel really costs)."""
+    graph, _ = harness.graphed(fn, 3, calls=reps)
+    return harness.timed(graph.replay, iters, 1)[0] / reps
 
 
-def graph_timed(fn, reps=10, iters=10):
-    """Device time per call with the launches captured in a CUDA graph (no host gaps: what a small kernel really costs)."""
-    s = torch.cuda.Stream()
-    with torch.cuda.stream(s):
-        for _ in range(3):
-            fn()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, stream=s):
-            for _ in range(reps):
-                fn()
-        g.replay()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(iters):
-            g.replay()
-        e1.record()
-        torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / (reps * iters)
-
-
-def kernel_us(fn, name, iters=20):
-    """Mean device time (us) per launch of the kernels whose name contains `name`, from a torch.profiler run of its own."""
-    from torch.profiler import ProfilerActivity, profile
+def peak_mb(fn):
+    """MiB allocated at the peak of one call of fn, above what was allocated before it, after one untimed call"""
     fn()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(iters):
-            fn()
-        torch.cuda.synchronize()
-    hits = [k for k in prof.key_averages() if name in k.key]
-    total, count = sum(k.device_time_total for k in hits), sum(k.count for k in hits)
-    return total / count if count else float("nan")
-
-
-def card():
-    import subprocess
-    q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                       text=True)
-    return dict(gpu=torch.cuda.get_device_name(0), power_limit_and_max_sm_clock=q.stdout.strip() or "unknown")
+    base = torch.cuda.memory_allocated()
+    return (harness.peak(fn) - base) / 2 ** 20
 
 
 def bench_extend(dev):
@@ -78,7 +36,7 @@ def bench_extend(dev):
     The state is rewound on the device before every call (lengths.fill_, one small kernel inside the timed graph), so every call
     appends at the same position.  The chunk-attention kernel's bytes are the cache K | V and timestamps it must read."""
     from genrec_b200.hstu import HSTU
-    info = card()
+    info = harness.card(dev)
     HBM = 3.35e12   # H100 SXM data sheet, bytes/s
     geoms = (("cfg2", dict(num_items=12101, embed_dim=128, num_heads=4, num_blocks=4), 200, (1, 128)),
              ("cfg3", dict(num_items=12101, embed_dim=256, num_heads=8, num_blocks=8), 2048, (1, 32)))
@@ -103,14 +61,14 @@ def bench_extend(dev):
                 st.items_bound = 0
                 return m.extend(st, ids, ts)
 
-            full_ms = graph_timed(lambda: m.last_logits(ids, ts))
+            full_ms = graph_ms(lambda: m.last_logits(ids, ts))
             for work, fn, keys in (("extend_1", one, L), ("prefill", prefill, None)):
-                ms = graph_timed(fn)
+                ms = graph_ms(fn)
                 row = dict(kernel="hstu_extend", geometry=name, workload=work, B=B, history=L - 1 if work == "extend_1" else 0,
                            new_items=1 if work == "extend_1" else L, extend_us=ms * 1e3, last_logits_us=full_ms * 1e3,
                            speedup_vs_last_logits=full_ms / ms, **info)
                 if keys is not None:
-                    attn_us = kernel_us(fn, "hstu_attn_extend_kernel")
+                    attn_us = harness.mean_launch_us(harness.profile(fn, 20), "hstu_attn_extend_kernel")
                     byt = B * keys * (2 * D * 2 + 8)            # per layer: K | V bf16 + int64 timestamp of every cached key
                     row.update(attn_kernel_us=attn_us, attn_bytes_per_layer=byt, attn_hbm_gbs=byt / attn_us / 1e3,
                                attn_frac_of_hbm_peak=byt / (attn_us * 1e-6) / HBM, blocks=NB)
@@ -162,7 +120,7 @@ def bench_head_topk(dev):
     catalog (cfg2: D = 128, C = 12,102) and at a 1,000,000-item catalog, then extend_users(top_k=10) against extend_users + the same
     top-k on the cfg2 pool workload.  The scoring kernel's time (torch.profiler) is set against its bound, the larger of the table
     read (C D 2 bytes at 3.35 TB/s) and the GEMM (2 R C D FLOP at 989 TFLOP/s), both H100 SXM data-sheet figures."""
-    info = card()
+    info = harness.card(dev)
     HBM, BF16 = 3.35e12, 989e12
     g = torch.Generator().manual_seed(0)
     D, eps = 128, 1e-5
@@ -181,8 +139,8 @@ def bench_head_topk(dev):
                     return torch.topk(lo, k, dim=1)
 
                 assert torch.equal(fused().scores, logits_topk().values)
-                f_ms, b_ms = graph_timed(fused), graph_timed(logits_topk)
-                kern = kernel_us(fused, "head_topk_kernel")
+                f_ms, b_ms = graph_ms(fused), graph_ms(logits_topk)
+                kern = harness.mean_launch_us(harness.profile(fused, 20), "head_topk_kernel")
                 t_bytes, t_flop = C * D * 2 / HBM * 1e6, 2 * B * C * D / BF16 * 1e6
                 bound = max(t_bytes, t_flop)
                 print(json.dumps(dict(kernel="head_topk", workload="head", D=D, C=C, B=B, k=k, fused_us=f_ms * 1e3,
@@ -200,21 +158,9 @@ def bench_head_topk(dev):
         return torch.topk(lo, 10, dim=1)
 
     assert torch.equal(one(top_k=10).scores, one_topk().values)
-    f_ms, b_ms = graph_timed(lambda: one(top_k=10)), graph_timed(one_topk)
+    f_ms, b_ms = graph_ms(lambda: one(top_k=10)), graph_ms(one_topk)
     print(json.dumps(dict(kernel="head_topk", workload="extend_users", geometry=name, pool_users=nusers, B=B, k=10, max_items=cap,
                           fused_us=f_ms * 1e3, logits_topk_us=b_ms * 1e3, speedup_vs_logits_topk=b_ms / f_ms, **info)), flush=True)
-
-
-def kernels_us(fn, prefix, iters=20):
-    """Mean device time (us) per call of every kernel whose name contains `prefix`, from a torch.profiler run of its own."""
-    from torch.profiler import ProfilerActivity, profile
-    fn()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(iters):
-            fn()
-        torch.cuda.synchronize()
-    return {k.key.split("(")[0][:80]: k.device_time_total / iters for k in prof.key_averages() if prefix in k.key}
 
 
 def bench_head_candidates(dev):
@@ -225,19 +171,10 @@ def bench_head_candidates(dev):
     500) on the cfg2 pool workload against extend_users + torch.topk.  The one-sweep bound is the larger of the table read (C D 2
     bytes at 3.35 TB/s) and the GEMM (2 B C D FLOP at 989 TFLOP/s), H100 SXM data-sheet figures; peak memory is
     torch.cuda.max_memory_allocated above the inputs."""
-    info = card()
+    info = harness.card(dev)
     HBM, BF16 = 3.35e12, 989e12
     D, eps = 128, 1e-5
     gd = torch.Generator(device=dev).manual_seed(0)
-
-    def peak_mb(fn):
-        fn()
-        torch.cuda.synchronize()
-        torch.cuda.reset_peak_memory_stats()
-        base = torch.cuda.memory_allocated()
-        fn()
-        torch.cuda.synchronize()
-        return (torch.cuda.max_memory_allocated() - base) / 2 ** 20
 
     def measure(workload, x, ln_g, ln_b, tb, k, profile_kernels):
         B, C = x.shape[0], tb.shape[0]
@@ -251,15 +188,17 @@ def bench_head_candidates(dev):
             return torch.topk(lo, k, dim=1)
 
         assert torch.equal(fused().scores, logits_topk().values)
-        f_ms = graph_timed(fused)
-        b_ms = graph_timed(logits_topk, reps=2, iters=5)
+        f_ms = graph_ms(fused)
+        b_ms = graph_ms(logits_topk, reps=2, iters=5)
         t_bytes, t_flop = C * D * 2 / HBM * 1e6, 2 * B * C * D / BF16 * 1e6
         bound = max(t_bytes, t_flop)
         row = dict(kernel="head_candidates", workload=workload, D=D, C=C, B=B, k=k, fused_us=f_ms * 1e3, logits_topk_us=b_ms * 1e3,
                    speedup_vs_logits_topk=b_ms / f_ms, bound_us=bound, bound_by="table read" if t_bytes >= t_flop else "bf16 GEMM",
                    fused_over_bound=f_ms * 1e3 / bound, fused_peak_mb=peak_mb(fused), logits_topk_peak_mb=peak_mb(logits_topk))
         if profile_kernels:
-            row.update(kernels_us=kernels_us(fused, "head_" if k <= 64 else "head_cand"))
+            prefix = "head_" if k <= 64 else "head_cand"
+            kernels = harness.profile(fused, 20)
+            row.update(kernels_us={name.split("(")[0][:80]: us / 20 for name, (us, _) in kernels.items() if prefix in name})
         print(json.dumps(dict(**row, **info)), flush=True)
 
     for C in (12102, 1000001):
@@ -297,8 +236,8 @@ def bench_head_candidates(dev):
     assert torch.equal(one(num_candidates=500).scores, one_topk().values)
     runs = {"num_candidates": [], "logits_topk": []}
     for _ in range(3):
-        runs["num_candidates"].append(graph_timed(lambda: one(num_candidates=500)) * 1e3)
-        runs["logits_topk"].append(graph_timed(one_topk) * 1e3)
+        runs["num_candidates"].append(graph_ms(lambda: one(num_candidates=500)) * 1e3)
+        runs["logits_topk"].append(graph_ms(one_topk) * 1e3)
     print(json.dumps(dict(kernel="head_candidates", workload="extend_users", geometry=name, pool_users=nusers, B=B, k=500, max_items=cap,
                           us=runs, **info)), flush=True)
 
@@ -314,19 +253,10 @@ def bench_head_rank(dev):
     FLOP at 989 TFLOP/s), both H100 SXM data-sheet figures.  Peak memory is torch.cuda.max_memory_allocated above the inputs.  Last,
     HSTU.evaluate_batch at the cfg2 geometry, B = 128, against eval_rank_metrics(last_logits(...)), alternated three times."""
     from genrec_b200.hstu import HSTU
-    info = card()
+    info = harness.card(dev)
     HBM, BF16 = 3.35e12, 989e12
     D, eps = 128, 1e-5
     gd = torch.Generator(device=dev).manual_seed(0)
-
-    def peak_mb(fn):
-        fn()
-        torch.cuda.synchronize()
-        torch.cuda.reset_peak_memory_stats()
-        base = torch.cuda.memory_allocated()
-        fn()
-        torch.cuda.synchronize()
-        return (torch.cuda.max_memory_allocated() - base) / 2 ** 20
 
     for C in (12102, 1000001, 10000001):
         tb = (0.05 * torch.randn(C, D, device=dev, generator=gd)).to(torch.bfloat16)
@@ -345,8 +275,8 @@ def bench_head_rank(dev):
             logits_gb = B * C * 4 / 1e9
             t_bytes, t_flop = C * D * 2 / HBM * 1e6, 2 * B * C * D / BF16 * 1e6
             bound = max(t_bytes, t_flop)
-            f_ms = graph_timed(fused)
-            kern = kernel_us(fused, "head_rank_kernel")
+            f_ms = graph_ms(fused)
+            kern = harness.mean_launch_us(harness.profile(fused, 20), "head_rank_kernel")
             row = dict(kernel="head_rank", D=D, C=C, B=B, fused_us=f_ms * 1e3, kernel_us=kern, bound_us=bound,
                        bound_by="table read" if t_bytes >= t_flop else "bf16 GEMM", kernel_over_bound=kern / bound,
                        fused_peak_mb=peak_mb(fused), logits_gb=logits_gb)
@@ -354,7 +284,7 @@ def bench_head_rank(dev):
                 r_f = Fn.head_rank_metrics(x, ln_g, ln_b, tb, eps, tg, want_ranks=True)[1]
                 r_l = Fn.eval_rank_metrics(Fn.head_logits(x[:, None, :], ln_g, ln_b, tb, tb, eps)[:, 0, :], tg, want_ranks=True)[1]
                 assert torch.equal(r_f, r_l)
-                b_ms = graph_timed(logits_path, reps=2, iters=5)
+                b_ms = graph_ms(logits_path, reps=2, iters=5)
                 row.update(logits_path_us=b_ms * 1e3, speedup_vs_logits=b_ms / f_ms, logits_peak_mb=peak_mb(logits_path))
             else:
                 row.update(logits_path=f"not run ({logits_gb:.1f} GB of logits, cap {LOGITS_CAP_GB} GB)")
@@ -377,8 +307,8 @@ def bench_head_rank(dev):
     assert torch.equal(Fn.eval_rank_metrics(m.last_logits(ids, ts), tg)[:3], m.evaluate_batch(ids, ts, tg)[:3])
     runs = {"evaluate_batch": [], "last_logits_eval_rank": []}
     for _ in range(3):
-        runs["evaluate_batch"].append(graph_timed(new) * 1e3)
-        runs["last_logits_eval_rank"].append(graph_timed(old) * 1e3)
+        runs["evaluate_batch"].append(graph_ms(new) * 1e3)
+        runs["last_logits_eval_rank"].append(graph_ms(old) * 1e3)
     print(json.dumps(dict(kernel="head_rank", workload="HSTU.evaluate_batch", geometry="cfg2", B=B, L=L, C=V + 1, us=runs,
                           peak_mb=dict(evaluate_batch=peak_mb(new), last_logits_eval_rank=peak_mb(old)), **info)), flush=True)
 
@@ -389,18 +319,19 @@ def bench_pool(dev):
     Graph-captured with the users as a device tensor.  Every length is a non-multiple of the page size, so the timed item never
     takes a page, and the lengths are rewound on the device before every call (one small kernel inside the timed graph).  The
     allocation kernel and the chunk-attention kernel are timed on their own with torch.profiler."""
-    info = card()
+    info = harness.card(dev)
     HBM = 3.35e12
     for name, geo, nusers, cap, B, dense in POOL_GEOMS:
         m, pool, lens, hist, hts, users, one = _pool_workload(dev, name, geo, nusers, cap, B)
         D, NB, ps = geo["embed_dim"], geo["num_blocks"], pool.page_size
         ulens = lens[users].to(dev, torch.int32)
         ids1, ts1 = hist[users, -1:].to(dev), hts[users, -1:].to(dev)
-        ms = graph_timed(one)
+        ms = graph_ms(one)
         hist_u, hts_u = hist[users].to(dev), hts[users].to(dev)
-        full_ms = graph_timed(lambda: m.last_logits(hist_u, hts_u))
-        attn_us = kernel_us(one, "hstu_attn_extend_kernel")
-        alloc_us = kernel_us(one, "hstu_pool_alloc_kernel")
+        full_ms = graph_ms(lambda: m.last_logits(hist_u, hts_u))
+        kernels = harness.profile(one, 20)
+        attn_us = harness.mean_launch_us(kernels, "hstu_attn_extend_kernel")
+        alloc_us = harness.mean_launch_us(kernels, "hstu_pool_alloc_kernel")
         item = NB * 2 * D * 2 + 8                                   # cached bytes per item: K | V of every block + timestamp
         byt = int((lens[users] + 1).sum()) * (2 * D * 2 + 8)        # per layer: the keys the attention reads
         pages = int(((lens[users] + ps) // ps).sum())
@@ -418,10 +349,10 @@ def bench_pool(dev):
                 st.items_bound = cap - 1
                 return m.extend(st, ids1, ts1)
 
-            dense_ms = graph_timed(dense_one)
+            dense_ms = graph_ms(dense_one)
             assert torch.equal(one(), dense_one())                 # same users, same items: the same bits
             row.update(dense_extend_us=dense_ms * 1e3, pool_over_dense=ms / dense_ms,
-                       dense_attn_kernel_us=kernel_us(dense_one, "hstu_attn_extend_kernel"))
+                       dense_attn_kernel_us=harness.mean_launch_us(harness.profile(dense_one, 20), "hstu_attn_extend_kernel"))
         print(json.dumps(row), flush=True)
         del pool
         torch.cuda.empty_cache()
@@ -435,16 +366,16 @@ def bench_rqvae_train(dev):
     import numpy as np
     from genrec_b200.rqvae import kmeans_init_
     from tests import rqvae_train_oracle as O
-    info = card()
+    info = harness.card(dev)
     g = torch.Generator().manual_seed(3)
     for B in (1024, 20480):
         x, cb = torch.randn(B, 32, generator=g).to(dev) * 0.3, torch.randn(256, 32, generator=g).to(dev) * 0.3
         dist = O.l2_dist(x, cb)
-        ours = timed(lambda: Fn.rq_sinkhorn(dist), iters=20, warm=3)
-        ours_g = graph_timed(lambda: Fn.rq_sinkhorn(dist), reps=5, iters=4)
-        eager = timed(lambda: O.sinkhorn(dist), iters=5, warm=2)
-        graph = graph_timed(lambda: O.sinkhorn(dist), reps=2, iters=3)
-        kern = kernel_us(lambda: Fn.rq_sinkhorn(dist), "rq_sinkhorn_kernel", iters=10)
+        ours = harness.timed(lambda: Fn.rq_sinkhorn(dist), 20, 3)[0]
+        ours_g = graph_ms(lambda: Fn.rq_sinkhorn(dist), reps=5, iters=4)
+        eager = harness.timed(lambda: O.sinkhorn(dist), 5, 2)[0]
+        graph = graph_ms(lambda: O.sinkhorn(dist), reps=2, iters=3)
+        kern = harness.mean_launch_us(harness.profile(lambda: Fn.rq_sinkhorn(dist), 10), "rq_sinkhorn_kernel")
         print(json.dumps(dict(kernel="rq_sinkhorn", B=B, K=256, iters=100, kernel_us=kern, us=ours * 1e3, graph_us=ours_g * 1e3,
                               torch_fp64_eager_us=eager * 1e3, torch_fp64_graph_us=graph * 1e3, speedup_vs_torch_graph=graph / ours_g,
                               kernel_us_per_iteration=kern / 100, **info)), flush=True)
@@ -470,7 +401,7 @@ def bench_linear_bwd(dev):
     training step (forward + backward) at configs[0] geometry.  Graph-captured device time.  Only the Python API is used, so the
     script times any tree that has it."""
     from genrec_b200.sasrec import SASRec
-    info = card()
+    info = harness.card(dev)
     g = torch.Generator().manual_seed(0)
     shapes = [("sasrec", 6400, 64, 64), ("sasrec", 6400, 256, 64), ("sasrec", 6400, 64, 256),
               ("tiger_encoder", 256 * 61, 384, 384), ("tiger_encoder", 256 * 61, 768, 384),
@@ -479,7 +410,7 @@ def bench_linear_bwd(dev):
         dy = (torch.randn(T, N, generator=g) * 0.1).to(dev).bfloat16()
         w = (torch.randn(N, K, generator=g) * 0.1).to(dev).bfloat16()
         x = torch.randn(T, K, generator=g).to(dev).bfloat16()
-        ms = graph_timed(lambda: Fn.linear_bwd(dy, w, x))
+        ms = graph_ms(lambda: Fn.linear_bwd(dy, w, x))
         print(json.dumps(dict(kernel="linear_bwd", geometry=geo, T=T, N=N, K=K, us=ms * 1e3, **info)), flush=True)
     B, L, V = 128, 50, 1000
     torch.manual_seed(0)
@@ -496,7 +427,7 @@ def bench_linear_bwd(dev):
             p.grad.zero_()
         m(ids, tg)[1].backward()
 
-    ms = graph_timed(step)
+    ms = graph_ms(step)
     print(json.dumps(dict(kernel="sasrec_train_step", B=B, L=L, D=64, blocks=2, num_items=V, dropout=0.2, ms=ms, **info)), flush=True)
 
 
@@ -507,7 +438,7 @@ def bench_tiger(dev):
     from genrec_b200 import tiger_decode as td
     from genrec_b200.tiger import Tiger
     from tests import tiger_params as tp
-    info = card()
+    info = harness.card(dev)
     cfg = dict(tp.PUBLISHED, dropout=0.1)
     B, K = 256, 10
     m = Tiger(**cfg)
@@ -522,7 +453,7 @@ def bench_tiger(dev):
         opt.step()
 
     m.train()
-    ms = timed(step, iters=20, warm=5)
+    ms = harness.timed(step, 20, 5)[0]
     print(json.dumps(dict(kernel="tiger_train_step", B=B, history_items=20, dropout=0.1, optimizer="AdamW (torch fused)", ms=ms, **info)),
           flush=True)
     m.eval()
@@ -533,19 +464,12 @@ def bench_tiger(dev):
     uncached = lambda: td.generate(m, *args, n_top_k_candidates=K)          # noqa: E731
     for _ in range(2):
         eager(), uncached()
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        eager()
-    torch.cuda.current_stream().wait_stream(s)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        eager()
+    graph, _ = harness.graphed(eager, 1)
     rows = {"eager": [], "graph": [], "uncached": []}
     for _ in range(3):
-        rows["eager"].append(timed(eager, iters=10, warm=1))
-        rows["graph"].append(timed(graph.replay, iters=10, warm=1))
-        rows["uncached"].append(timed(uncached, iters=10, warm=1))
+        rows["eager"].append(harness.timed(eager, 10, 1)[0])
+        rows["graph"].append(harness.timed(graph.replay, 10, 1)[0])
+        rows["uncached"].append(harness.timed(uncached, 10, 1)[0])
     for name, v in rows.items():
         print(json.dumps(dict(kernel="tiger_generate_" + name, B=B, K=K, trie_items=12000, ms_per_round=v, ms=min(v), **info)), flush=True)
     print(json.dumps(dict(kernel="tiger_generate_speedup", eager_vs_uncached=min(rows["uncached"]) / min(rows["eager"]),
@@ -559,7 +483,7 @@ def bench_tiger_wide(dev, m, args, info):
     replayed from a CUDA graph, alternated in rounds) with its peak memory; per decode step, the device time of the beam-select
     launches next to that step's torch.multinomial (torch.profiler, a run of its own); and the beam step alone at K = 10, where
     both the one-CTA kernel and the wide path apply."""
-    from torch.profiler import ProfilerActivity, profile, record_function
+    from torch.profiler import record_function
     from genrec_b200 import _lib
     from genrec_b200 import tiger_decode as td
     from genrec_b200._lib import ptr, stream_ptr
@@ -567,25 +491,14 @@ def bench_tiger_wide(dev, m, args, info):
     for K in (10, 64, 256, 1024):
         gen = lambda: m.generate(*args, n_top_k_candidates=K)                  # noqa: E731
         gen()
-        torch.cuda.synchronize()
-        torch.cuda.reset_peak_memory_stats()
         base = torch.cuda.memory_allocated()
-        gen()
-        torch.cuda.synchronize()
-        peak = torch.cuda.max_memory_allocated() - base
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            gen()
-        torch.cuda.current_stream().wait_stream(s)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            gen()
+        peak = harness.peak(gen) - base
+        graph, _ = harness.graphed(gen, 1)
         rows = {"eager": [], "graph": []}
         iters = 10 if K <= 64 else 3
         for _ in range(3):
-            rows["eager"].append(timed(gen, iters=iters, warm=1))
-            rows["graph"].append(timed(graph.replay, iters=iters, warm=1))
+            rows["eager"].append(harness.timed(gen, iters, 1)[0])
+            rows["graph"].append(harness.timed(graph.replay, iters, 1)[0])
         del graph
         torch.cuda.empty_cache()
         if K > 10:
@@ -602,15 +515,12 @@ def bench_tiger_wide(dev, m, args, info):
 
         td.beam_select = traced
         try:
-            with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-                for _ in range(3):
-                    gen()
-                torch.cuda.synchronize()
+            prof = harness.profile(gen, 3, 0, cpu=True)
         finally:
             td.beam_select = orig
         steps = 3 * m.sem_id_dim
-        ev = {e.key: e.device_time_total / steps for e in prof.key_averages()}
-        kern = {k.split("(")[0].replace("void ", "").replace("grb::", ""): round(v, 1) for k, v in ev.items() if "beam_" in k}
+        ev = {k: us / steps for k, (us, _) in prof.items()}
+        kern = {harness.short_name(k): round(v, 1) for k, v in ev.items() if "beam_" in k}
         print(json.dumps(dict(kernel="tiger_beam_step_vs_multinomial", B=B, K=K, KK=min(6 * K, 256), us_beam_step=round(ev.get("grb_beam_step", 0), 1),
                               us_multinomial=round(ev.get("aten::multinomial", 0), 1), kernels_us_per_step=kern,
                               us_trie_log_softmax=round(sum(v for k, v in ev.items() if "trie_log_softmax_kernel" in k), 1), **info)), flush=True)
@@ -642,7 +552,7 @@ def bench_tiger_wide(dev, m, args, info):
     rows = {n: [] for n in calls}
     for _ in range(5):
         for n, fn in calls.items():
-            rows[n].append(graph_timed(fn) * 1e3)
+            rows[n].append(graph_ms(fn) * 1e3)
     for n, v in rows.items():
         print(json.dumps(dict(kernel="tiger_beam_step_k10_" + n, B=B, K=K, KK=KK, S=S, us_per_round=v, us=min(v), same_beams=same, **info)),
               flush=True)
@@ -653,8 +563,7 @@ def bench_hstu_attn(dev):
     H = 4; cfg3: B = 32, L = 2048, D = 256, H = 8), uniform position buckets, with and without the 64-bucket time table.  The call
     also clears its dzp output.  The attention kernels' device time per call comes from a torch.profiler run of its own."""
     from genrec_b200.hstu import _thresholds_on
-    from torch.profiler import ProfilerActivity, profile
-    info = card()
+    info = harness.card(dev)
     for name, B, L, D, H in (("cfg2", 128, 200, 128, 4), ("cfg3", 32, 2048, 256, 8)):
         g = torch.Generator().manual_seed(0)
         zp = (0.7 * torch.randn(B, L, 4 * D, generator=g)).bfloat16().to(dev)
@@ -671,16 +580,10 @@ def bench_hstu_attn(dev):
             def call():
                 return Fn.hstu_attention_bwd(P, zp, dO, meta, H, wpos, wt, 64)
 
-            ms = graph_timed(call)
-            call()
-            torch.cuda.synchronize()
+            ms = graph_ms(call)
             iters = 20
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                for _ in range(iters):
-                    call()
-                torch.cuda.synchronize()
-            kern = {k.key.split("<")[0].replace("void ", "").replace("grb::", ""): round(k.device_time_total / iters, 2)
-                    for k in prof.key_averages() if "hstu_attn_bwd" in k.key or "det_finish" in k.key}
+            kern = {harness.short_name(k, "<"): round(us / iters, 2) for k, (us, _) in harness.profile(call, iters).items()
+                    if "hstu_attn_bwd" in k or "det_finish" in k}
             print(json.dumps(dict(kernel="hstu_attention_bwd", geometry=name, B=B, L=L, D=D, H=H, time_table=time_table,
                                   us=ms * 1e3, kernel_us_per_call=kern, **info)), flush=True)
 
@@ -721,7 +624,7 @@ def main():
                     os.environ.pop("GRB_RQ", None)
                 else:
                     os.environ["GRB_RQ"] = mode
-                ms = graph_timed(lambda: Fn.rq_residual_argmin(x, cbs, 0.25, want_aux=aux))
+                ms = graph_ms(lambda: Fn.rq_residual_argmin(x, cbs, 0.25, want_aux=aux))
                 flops = 2 * 256 * 32 * 3 * N
                 byt = N * (32 * 4 + 3 * 8 + (2 * 32 * 3 * 4 + 4 if aux else 0))
                 print(json.dumps(dict(kernel="rq_residual_argmin", N=N, aux_outputs=aux, dispatch=mode, us=ms * 1e3, items_per_s=N / ms * 1e3,
@@ -740,7 +643,7 @@ def main():
             y = layer(x, None, pad, ts)
             y.backward(dy)
 
-        ms = timed(fb, iters=10, warm=3)
+        ms = harness.timed(fb, 10, 3)[0]
         flops = (72 * L * D * D + 6 * D * L * (L + 1)) * B
         peak = peaks.get("bf16_tflops", 989.0)   # H100 SXM data sheet, dense bf16 at 700 W
         print(json.dumps(dict(kernel="hstu_layer_fwd_bwd", B=B, L=L, D=D, H=H, ms=ms, seq_per_s=B / ms * 1e3,

@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
 from genrec_b200.rqvae import QuantizeForwardMode as M, RqVae
-from scripts.bench_kernels import card
+from scripts import harness
 from tests import rqvae_train_oracle as O
 
 GEO = dict(input_dim=768, hidden=[512, 256, 128, 64], D=32, levels=3, K=256)
@@ -41,47 +41,16 @@ def step_fn(kind, dev):
     return step
 
 
-def time_eager(fn, iters=30, warm=5):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
-
-
-def time_graph(fn, iters=30):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(3):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    g.replay()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        g.replay()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
-
-
 def main():
     dev = torch.device("cuda:0")
-    info = card()
+    info = harness.card(dev)
     for kind in ("ours", "torch_restatement"):
-        for mode, timer in (("eager", time_eager), ("cuda_graph", time_graph)):
-            ms = timer(step_fn(kind, dev))
+        for mode in ("eager", "cuda_graph"):
+            step = step_fn(kind, dev)
+            if mode == "eager":
+                ms = harness.timed(step, 30, 5)[0]
+            else:
+                ms = harness.timed(harness.graphed(step, 3)[0].replay, 30, 1)[0]
             print(json.dumps(dict(bench="rqvae_train_step", impl=kind, mode=mode, B=1024, geometry="tiger", ms=ms, **info)), flush=True)
 
 

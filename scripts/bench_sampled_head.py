@@ -15,46 +15,22 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from scripts import harness  # noqa: E402
 
 PEAK_FLOPS, PEAK_BYTES = 989e12, 3.35e12
 EPS = 1e-5
 
 
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
-    return q.stdout.strip() or torch.cuda.get_device_name(0)
-
-
 def graph_time(fn, iters=20, rounds=5):
     """median over `rounds` of the mean time (ms) of `iters` replays of fn captured in a CUDA graph"""
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(3):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    g.replay()
-    torch.cuda.synchronize()
-    out = []
-    for _ in range(rounds):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for _ in range(iters):
-            g.replay()
-        b.record()
-        torch.cuda.synchronize()
-        out.append(a.elapsed_time(b) / iters)
-    return statistics.median(out)
+    graph, _ = harness.graphed(fn, 3)
+    graph.replay()
+    return statistics.median(harness.timed(graph.replay, iters, 0)[0] for _ in range(rounds))
 
 
 class Head:
@@ -113,25 +89,15 @@ def head_alone(dev, T, res):
 
 
 def per_kernel(dev, T, res):
-    from torch.profiler import ProfilerActivity, profile
     D = 128
     h = Head(T, D, 12102, dev)
     for N in (1024, 4096):
-        fn = h.sampled(N)
-        for _ in range(3):
-            fn()
-        torch.cuda.synchronize()
         reps = 20
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(reps):
-                fn()
-            torch.cuda.synchronize()
-        for ev in prof.key_averages():
-            name = ev.key
+        kernels = harness.profile(h.sampled(N), reps, 3)
+        for name, (t, _) in kernels.items():
             for short in ("sce_gather_kernel", "sce_target_kernel", "sce_rows_kernel", "sce_table_kernel", "sce_scatter_kernel", "ln_fwd_kernel",
                           "ln_bwd_kernel"):
                 if short in name:
-                    t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0.0)
                     res[f"kernel D={D} T={T} N={N} {short} us"] = round(t / reps, 2)
         Npad = (N + 63) // 64 * 64
         flop_t = 6.0 * T * D * (N + 1) / PEAK_FLOPS
@@ -204,21 +170,19 @@ def full_step(dev, res, V):
     table = model.item_embedding.weight.numel()
     res[f"V={V} table share of the parameters"] = round(table / sum(p.numel() for p in model.parameters()), 4)
 
-    from torch.profiler import ProfilerActivity, profile
     reps, touched = 5, []
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(reps):
-            opt._mark(ids); opt._mark(tg); opt._mark(neg)
-            touched.append(opt._row_count[0].clone())
-            opt.step()
-        torch.cuda.synchronize()
+
+    def marked_step():
+        opt._mark(ids); opt._mark(tg); opt._mark(neg)
+        touched.append(opt._row_count[0].clone())
+        opt.step()
+
+    kernels = harness.profile(marked_step, reps, 0)
     rows = int(touched[0])
     res[f"V={V} touched rows per step"] = rows
-    for ev in prof.key_averages():
+    for name, (t_us, _) in kernels.items():
         for short in ("rowset_mark_kernel", "lazy_table_step_kernel", "adam_step_kernel", "rowset_reset_kernel", "adam_tick_kernel"):
-            if short in ev.key:
-                t_us = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0.0)
+            if short in name:
                 res[f"V={V} kernel {short} us per step"] = round(t_us / reps, 2)
     bound_us = 34.0 * rows * D / PEAK_BYTES * 1e6
     res[f"V={V} lazy table pass byte bound us (34 B per touched element at 3.35 TB/s)"] = round(bound_us, 2)
@@ -240,7 +204,7 @@ def main():
     from genrec_b200 import _lib
     dev = torch.device("cuda:0")
     _lib.ensure_device(dev)
-    res = {"card": card()}
+    res = harness.card(dev)
     T = 128 * 200
     if not args.skip_head:
         head_alone(dev, T, res)

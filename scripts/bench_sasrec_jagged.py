@@ -15,7 +15,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -23,6 +22,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+from scripts import harness  # noqa: E402
 
 CFG = dict(num_items=12101, max_seq_len=50, embed_dim=64, num_heads=2, num_blocks=2, ffn_dim=256)
 WORKLOADS = {   # name: (B, lengths, description, aim on packed / padded)
@@ -33,23 +33,9 @@ WORKLOADS = {   # name: (B, lengths, description, aim on packed / padded)
 EVAL_B = 256
 
 
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                       text=True)
-    return dict(gpu=torch.cuda.get_device_name(0), power_limit_and_max_sm_clock=q.stdout.strip() or "unknown")
-
-
-def lengths_of(kind, B, g):
-    if kind == "full":
-        return torch.full((B,), 50)
-    p = 1.0 / 9                                        # geometric on 1, 2, ... with mean 9
-    u = torch.rand(B, generator=g, dtype=torch.float64)
-    return (torch.floor(torch.log1p(-u) / torch.log1p(torch.tensor(-p, dtype=torch.float64))) + 1).long().clamp(1, 50)
-
-
 def jagged_batch(kind, B, V, seed, dev):
     g = torch.Generator().manual_seed(seed)
-    lens = lengths_of(kind, B, g)
+    lens = torch.full((B,), 50) if kind == "full" else harness.geometric_lengths(B, 9, 1, 50, g)
     w = torch.arange(1, V + 1, dtype=torch.float64).pow(-1.1)
     items = torch.multinomial(w, int(lens.sum()), replacement=True, generator=g) + 1
     tgt = torch.multinomial(w, B, replacement=True, generator=g) + 1
@@ -64,49 +50,6 @@ def make(dev):
     torch.manual_seed(0)
     m = SASRec(dropout=0.0, **CFG).to(dev).train()
     return m, FlatAdam(m, lr=1e-3, betas=(0.9, 0.98))
-
-
-def graphed(step, warmup=3):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(warmup):
-            step()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        out = step()
-    return g, out
-
-
-def time_graph(g, steps):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    g.replay()
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(steps):
-        g.replay()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / steps
-
-
-def kernel_us(step):
-    """device time (us) per kernel of one eager step, from torch.profiler, largest first"""
-    from torch.profiler import ProfilerActivity, profile
-    step()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        step()
-        torch.cuda.synchronize()
-    out = {}
-    for k in prof.key_averages():
-        if k.device_time_total <= 0:
-            continue
-        name = k.key.split("(")[0].replace("void ", "").replace("grb::", "")[:60]
-        out[name] = round(out.get(name, 0.0) + k.device_time_total, 1)
-    return dict(sorted(out.items(), key=lambda kv: -kv[1]))
 
 
 def batches(kind, B, dev):
@@ -139,14 +82,14 @@ def run(name, steps, dev, info, profile):
         base = torch.cuda.memory_allocated()           # step_peak_mem_mb: the step's working memory above what is already resident
         torch.cuda.reset_peak_memory_stats()
         loss0 = step().item()                          # the first step's loss, from the same initial parameters on both paths
-        g, _ = graphed(step)
+        g, _ = harness.graphed(step, 3)
         g.replay()
         torch.cuda.synchronize()
         res[path] = dict(step=step, graph=g, loss0=loss0, peak_mb=(torch.cuda.max_memory_allocated() - base) / 2 ** 20)
     times = {"padded": [], "packed": []}
     for _ in range(3):
         for path in ("padded", "packed"):
-            times[path].append(time_graph(res[path]["graph"], steps))
+            times[path].append(harness.timed(res[path]["graph"].replay, steps, 1)[0])
     out = dict(workload=name, desc=desc, B=B, aim=aim, padded_L=L, padded_tokens=B * L, packed_tokens=T,
                padding_share=round(1 - T / (B * L), 4), **info)
     for path in ("padded", "packed"):
@@ -158,7 +101,8 @@ def run(name, steps, dev, info, profile):
     if profile:
         for path in ("padded", "packed"):
             res[path]["graph"].reset()
-            out[path]["kernels_us"] = kernel_us(res[path]["step"])
+            kernels = harness.largest_first(harness.profile(res[path]["step"]), lambda k: harness.short_name(k)[:60])
+            out[path]["kernels_us"] = {k: round(us, 1) for k, us in kernels.items()}
     print(json.dumps(out), flush=True)
 
 
@@ -170,11 +114,11 @@ def run_eval(steps, dev, info):
     metrics = torch.zeros(6, device=dev)
     calls = {"padded": lambda: m.evaluate_batch(pad["input_ids"], tgt, metrics),
               "packed": lambda: m.evaluate_batch_jagged(pk["input_ids"], pk["offsets"], pk["max_len"], tgt, metrics)}
-    graphs = {k: graphed(f)[0] for k, f in calls.items()}
+    graphs = {k: harness.graphed(f, 3)[0] for k, f in calls.items()}
     times = {"padded": [], "packed": []}
     for _ in range(3):
         for k in times:
-            times[k].append(time_graph(graphs[k], steps))
+            times[k].append(harness.timed(graphs[k].replay, steps, 1)[0])
     out = dict(workload="eval256", B=EVAL_B, packed_tokens=pk["input_ids"].numel(), padded_tokens=pad["input_ids"].numel(), **info)
     for k in times:
         out[k] = dict(call_ms=round(statistics.median(times[k]), 4), runs_ms=[round(t, 4) for t in times[k]])
@@ -191,7 +135,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_sasrec_jagged.py measures on a CUDA device; none is visible")
     dev = torch.device("cuda:0")
-    info = card()
+    info = harness.card(dev)
     prof = set(args.profile.split(",")) if args.profile else set()
     for name in args.workloads.split(","):
         run(name, args.steps, dev, info, name in prof)

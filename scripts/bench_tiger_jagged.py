@@ -18,7 +18,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import tempfile
 
@@ -28,6 +27,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+from scripts import harness  # noqa: E402
 
 CFG = dict(embedding_dim=128, attn_dim=384, dropout=0.0, num_heads=6, n_layers=8, num_item_embeddings=256, num_user_embeddings=10000,
            sem_id_dim=3)
@@ -42,12 +42,6 @@ WORKLOADS = {   # name: (kind, B, lengths, aim on packed / padded)
     "gen10_full": ("generate10", 256, "full", "within 3%"),
     "gen256_full": ("generate256", 256, "full", "within 3%"),
 }
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                       text=True)
-    return dict(gpu=torch.cuda.get_device_name(0), power_limit_and_max_sm_clock=q.stdout.strip() or "unknown")
 
 
 def batch(B, kind, seed, dev):
@@ -116,55 +110,20 @@ def gen_fns(m, padded, packed, K, valid):
     return [padded_call, packed_call]
 
 
-def graphed(fn):
-    fn()
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        fn()
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        out = fn()
-    g.out = out
-    return g.replay
-
-
-def timed(fn, steps):
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(steps):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / steps
-
-
-def peak(fn):
-    torch.cuda.synchronize()
+def peak_mb(fn):
+    """MiB allocated at the peak of one call of fn, above what was allocated before it"""
     base = torch.cuda.memory_allocated()
-    torch.cuda.reset_peak_memory_stats()
-    fn()
-    torch.cuda.synchronize()
-    return (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+    return (harness.peak(fn) - base) / 2 ** 20
 
 
-def profile(fn, path):
-    from torch.profiler import ProfilerActivity, profile as prof
-    fn()
-    torch.cuda.synchronize()
-    with prof(activities=[ProfilerActivity.CUDA]) as p:
-        fn()
-        torch.cuda.synchronize()
-    rows = {}
-    for e in p.key_averages():
-        if e.device_type.name == "CUDA" or getattr(e, "device_time_total", 0) > 0:
-            rows[e.key] = rows.get(e.key, 0.0) + getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0))
+def profile_to(fn, path):
+    """one call of fn under torch.profiler, after one untimed call: writes each kernel's device us to `path`, largest first, and
+    returns their sum in ms"""
+    kernels = harness.largest_first(harness.profile(fn))
     with open(path, "w") as f:
-        for k, v in sorted(rows.items(), key=lambda kv: -kv[1]):
+        for k, v in kernels.items():
             f.write(f"{v:10.1f} us  {k}\n")
-    return sum(rows.values()) / 1000.0
+    return sum(kernels.values()) / 1000.0
 
 
 def main():
@@ -178,7 +137,7 @@ def main():
         a.out = tempfile.mkdtemp(prefix="bench_tiger_jagged_")
         print(f"profiles: {a.out}", flush=True)
     dev = torch.device("cuda:0")
-    info = card()
+    info = harness.card(dev)
     valid = torch.randint(0, CFG["num_item_embeddings"], (20000, 3), generator=torch.Generator().manual_seed(2))
     for name in a.workloads.split(","):
         kind, B, lengths, aim = WORKLOADS[name]
@@ -195,22 +154,23 @@ def main():
                                                             packed["mem_offsets"], packed["max_len"], packed["target_input_ids"],
                                                             packed["target_token_type_ids"]).loss)
             fns = train_fns(m, padded, packed)
-            res["peak_mb"] = [round(peak(f), 1) for f in fns]
+            res["peak_mb"] = [round(peak_mb(f), 1) for f in fns]
             if a.profile:
                 os.makedirs(a.out, exist_ok=True)
-                res["profiled_ms"] = [round(profile(f, os.path.join(a.out, f"prof_{name}_{p}.txt")), 3)
+                res["profiled_ms"] = [round(profile_to(f, os.path.join(a.out, f"prof_{name}_{p}.txt")), 3)
                                       for f, p in zip(fns, ("padded", "packed"))]
         else:
             m.eval()
             eager = gen_fns(m, padded, packed, 10 if kind == "generate10" else 256, valid)
-            res["peak_mb"] = [round(peak(f), 1) for f in eager]          # one eager call: a replay allocates nothing
-            fns = [graphed(f) for f in eager]
+            res["peak_mb"] = [round(peak_mb(f), 1) for f in eager]       # one eager call: a replay allocates nothing
+            fns = [harness.graphed(f, 2)[0].replay for f in eager]
         for f in fns:
-            timed(f, 3)
+            for _ in range(3):
+                f()
         t = {0: [], 1: []}
         for _ in range(3):
             for i, f in enumerate(fns):
-                t[i].append(timed(f, a.steps))
+                t[i].append(harness.timed(f, a.steps, 0)[0])
         res["ms_padded"], res["ms_packed"] = statistics.median(t[0]), statistics.median(t[1])
         res["ratio"] = round(res["ms_packed"] / res["ms_padded"], 3)
         res["runs_ms"] = {"padded": [round(x, 3) for x in t[0]], "packed": [round(x, 3) for x in t[1]]}

@@ -9,7 +9,6 @@ step's wall time, which is measured separately without the profiler.  With progr
 once every CTA of the kernel before it has started, so a kernel's time includes its wait for that kernel's last round."""
 import argparse
 import os
-import subprocess
 import sys
 from collections import defaultdict
 
@@ -17,14 +16,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
-from torch.profiler import ProfilerActivity, profile  # noqa: E402
 
 import bench  # noqa: E402
-
-
-def short_name(name):
-    name = name.split("(")[0] if not name.startswith("void ") else name[5:].split("(")[0]
-    return name.replace("grb::", "")
+from scripts import harness  # noqa: E402
 
 
 def main():
@@ -36,9 +30,8 @@ def main():
     from genrec_b200.hstu import HSTU
     from genrec_b200.optim import FlatAdam
 
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                          capture_output=True, text=True).stdout.strip().splitlines()
     dev = torch.device("cuda:0")
+    card = harness.card(dev)
     torch.cuda.set_device(dev)
     _lib.ensure_device(dev)
     c = bench.CONFIGS[args.config]
@@ -55,46 +48,22 @@ def main():
         opt.step()
         return loss
 
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        for _ in range(3):
-            step()
-    torch.cuda.current_stream().wait_stream(side)
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        step()
-    for _ in range(10):
-        graph.replay()
-    torch.cuda.synchronize()
+    graph, _ = harness.graphed(step, 3)
+    wall_us = harness.timed(graph.replay, args.steps, 10)[0] * 1e3
 
-    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0.record()
-    for _ in range(args.steps):
-        graph.replay()
-    t1.record()
-    torch.cuda.synchronize()
-    wall_us = t0.elapsed_time(t1) * 1e3 / args.steps
-
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(args.steps):
-            graph.replay()
-        torch.cuda.synchronize()
-    total, calls = defaultdict(float), defaultdict(int)
-    for e in prof.events():
-        if e.device_type == torch.autograd.DeviceType.CUDA:
-            total[short_name(e.name)] += e.time_range.elapsed_us()
-            calls[short_name(e.name)] += 1
+    kernels = harness.profile(graph.replay, args.steps, 0)
+    total, calls = harness.largest_first(kernels, harness.short_name), defaultdict(int)
+    for k, (_, n) in kernels.items():
+        calls[harness.short_name(k)] += n
     busy = sum(total.values()) / args.steps
 
-    print(f"card: {'; '.join(card)} (name, power limit, max SM clock)")
+    print(f"card: {card['gpu']}, {card['power_limit_and_max_sm_clock']} (name, power limit, max SM clock)")
     print(f"{args.config}: B={B} L={L} D={cfg['embed_dim']} blocks={cfg['num_blocks']} V={V}; {args.steps} graph replays")
     print(f"step wall time (CUDA events, no profiler): {wall_us:.1f} us; kernel time summed over both streams: {busy:.1f} us")
     print()
     print("| kernel | launches / step | us / step | share of summed kernel time |")
     print("|---|---:|---:|---:|")
-    for name, us in sorted(total.items(), key=lambda kv: -kv[1]):
+    for name, us in total.items():
         per = us / args.steps
         print(f"| `{name}` | {calls[name] / args.steps:g} | {per:.1f} | {100 * per / busy:.1f}% |")
 
