@@ -1612,16 +1612,25 @@ int check_sas_jagged(const grb_sasrec_dims* d, const int64_t* offsets, int T) {
     GRB_REQUIRE(d->B <= 65535, "B=%d exceeds 65535 sequences", d->B);
     return 0;
 }
+// a padded SASRec batch [B, L, D]: the dropout row key (b H + h) L + i and the row offsets are 32-bit, as the packed form's are
+int check_sas_padded(const grb_sasrec_dims* d) {
+    GRB_REQUIRE(d != nullptr, "null argument");
+    const long long rows = (long long)d->B * d->L;
+    GRB_REQUIRE(rows * d->H < INT32_MAX && rows * d->D <= INT32_MAX, "B*L=%lld rows out of range for H=%d, D=%d", rows, d->H, d->D);
+    return 0;
+}
 }  // namespace
 
 extern "C" {
 
 int grb_sasrec_attention_forward(const grb_sasrec_dims* d, const void* q, const void* k, const void* v, const uint8_t* pad, void* out,
                                  float* lse, void* stream) {
+    GRB_TRY(check_sas_padded(d));
     return sas_forward<false>(d, nullptr, 0, q, k, v, pad, out, lse, static_cast<cudaStream_t>(stream));
 }
 int grb_sasrec_attention_backward(const grb_sasrec_dims* d, const void* q, const void* k, const void* v, const uint8_t* pad,
                                   const void* out, const float* lse, const void* dout, void* dq, void* dk, void* dv, void* stream) {
+    GRB_TRY(check_sas_padded(d));
     return sas_backward<false>(d, nullptr, 0, q, k, v, pad, out, lse, dout, dq, dk, dv, static_cast<cudaStream_t>(stream));
 }
 int grb_sasrec_attention_forward_jagged(const grb_sasrec_dims* d, const int64_t* offsets, int T, const void* q, const void* k,

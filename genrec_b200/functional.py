@@ -859,18 +859,21 @@ def dropout_seed(p: float) -> int:
 
 
 class StepSeeds:
-    """Mixed into HSTU and SASRec, whose dropout probability is ``emb_dropout.p``: ``_seeds`` gives each training forward its
-    (host seed, device seed), (0, None) without dropout.  The device seed is an int64 counter, made by the first training forward
-    (again after ``_seed_dev = None``) and bumped by each; a CUDA graph that captures the bump draws fresh masks on every replay."""
+    """Mixed into a module whose dropout probability is its ``_dropout_p`` (the models HSTU and SASRec, and the layers a user may
+    call on their own: HSTULayer, SASRecBlock, MultiHeadAttention, PointWiseFeedForward): ``_seeds`` gives each training forward
+    its (host seed, device seed), (0, None) without dropout.  The device seed is an int64 counter, made by the first training
+    forward (again after ``_seed_dev = None``) and bumped by each; a CUDA graph that captures the bump draws fresh masks on every
+    replay."""
 
     _seed_dev = None
 
     def _seeds(self, device):
-        if not (self.training and self.emb_dropout.p > 0):
+        p = self._dropout_p
+        if not (self.training and p > 0):
             return 0, None
         if self._seed_dev is None or self._seed_dev.device != device:
             self._seed_dev = torch.zeros(1, dtype=torch.int64, device=device)
-            self._step_seed = dropout_seed(self.emb_dropout.p)
+            self._step_seed = dropout_seed(p)
         self._seed_dev.add_(0x9E3779B1)
         # per-forward snapshot: the backward re-derives the masks from the value THIS forward saw, even when another
         # training-mode forward has bumped the counter in between

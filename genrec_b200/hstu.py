@@ -155,8 +155,9 @@ class TemporalBias(nn.Module):
         return self.temporal_attention_bias(buckets).permute(0, 3, 1, 2)
 
 
-class HSTULayer(nn.Module):
-    """Mirror of genrec/models/hstu.py:160-280; forward/backward = one C-ABI call each."""
+class HSTULayer(Fn.StepSeeds, nn.Module):
+    """Mirror of genrec/models/hstu.py:160-280; forward/backward = one C-ABI call each.  HSTU passes each layer its step's seeds;
+    called on its own without them, a training layer draws fresh dropout masks on each call (``StepSeeds``)."""
 
     def __init__(self, embed_dim: int, num_heads: int, dropout: float, num_position_buckets: int, num_time_buckets: int,
                  max_position_distance: int, use_temporal_bias: bool):
@@ -179,6 +180,10 @@ class HSTULayer(nn.Module):
         self._grad_sink = None      # set by FlatAdam: param -> view of the flat gradient buffer (kernels accumulate there)
         self.precision = "bf16"     # "fp32": the fp32-exact forward path (HSTU.set_precision)
         self._split = {}            # name -> (version, tensor): three-term bf16 splits of the weight matrices (fp32 path)
+
+    @property
+    def _dropout_p(self) -> float:
+        return self.dropout.p
 
     def _weights(self) -> dict:
         """The three weight matrices, by their names in Fn.BF16_PARAMS."""
@@ -238,12 +243,15 @@ class HSTULayer(nn.Module):
         return Fn.HstuLayerFn.apply(x, meta, cfg, bf16w, *self._params())
 
     def forward(self, x: torch.Tensor, causal_mask: torch.Tensor, padding_mask: torch.Tensor,
-                timestamps: Optional[torch.Tensor] = None, _meta: Optional[Fn.SeqMeta] = None, _seed: int = 0,
+                timestamps: Optional[torch.Tensor] = None, _meta: Optional[Fn.SeqMeta] = None, _seed: Optional[int] = None,
                 _seed_dev=None) -> torch.Tensor:
         """x [B,L,D] fp32, causal_mask [L,L] bool (accepted for signature parity; causality is derived from indices),
-        padding_mask [B,L] bool (True = pad), timestamps [B,L] int64 or None  ->  [B,L,D] fp32."""
+        padding_mask [B,L] bool (True = pad), timestamps [B,L] int64 or None  ->  [B,L,D] fp32.  _seed / _seed_dev: the step's
+        seeds (HSTU passes them); None: the layer's own."""
         require_cuda(x)
         ensure_device(x.device)
+        if _seed is None:
+            _seed, _seed_dev = self._seeds(x.device)
         if _meta is None:
             _meta = self._seq_meta(padding_mask.to(torch.uint8).contiguous(), timestamps, x.shape[1], x.device)
         return self._run(x, _meta, _seed, _seed_dev)
@@ -406,6 +414,10 @@ class HSTU(Fn.StepSeeds, nn.Module):
         self._unit_loss_grad = False   # FlatAdam(unit_loss_grad=True): head gradients go straight into the flat buffer (see HeadLossFn)
         self._row_marker = None        # set by FlatAdam(lazy_table=True): training forwards mark the item-table rows they touch
         self._init_weights()
+
+    @property
+    def _dropout_p(self) -> float:
+        return self.emb_dropout.p
 
     def _init_weights(self):
         """genrec/models/hstu.py:85-97."""

@@ -62,8 +62,9 @@ class _BlockFn(torch.autograd.Function):
         return (dx, None, None, None, None, dg1, dbt1, dwq, dbq, dwk, dbk, dwv, dbv, dg2, dbt2, dw1, db1, dw2, db2)
 
 
-class MultiHeadAttention(nn.Module):
-    """Mirror of genrec/models/sasrec.py:168-246 (stand-alone use; inside SASRecBlock the fused block path is taken)."""
+class MultiHeadAttention(Fn.StepSeeds, nn.Module):
+    """Mirror of genrec/models/sasrec.py:168-246 (stand-alone use; inside SASRecBlock the fused block path is taken).  In training
+    each call draws a fresh dropout mask (``StepSeeds``), as the reference's nn.Dropout does."""
 
     def __init__(self, embed_dim: int, num_heads: int, dropout: float):
         super().__init__()
@@ -75,17 +76,23 @@ class MultiHeadAttention(nn.Module):
         self.v_proj = nn.Linear(embed_dim, embed_dim)
         self.dropout = nn.Dropout(dropout)
 
+    @property
+    def _dropout_p(self) -> float:
+        return self.dropout.p
+
     def forward(self, query: torch.Tensor, key_value: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
-        return _AttnFn.apply(query, key_value, mask, self.num_heads, self.dropout.p if self.training else 0.0,
+        seed, sd = self._seeds(query.device)
+        return _AttnFn.apply(query, key_value, mask, self.num_heads, self.dropout.p if self.training else 0.0, seed, sd,
                              self.q_proj.weight, self.q_proj.bias, self.k_proj.weight, self.k_proj.bias, self.v_proj.weight,
                              self.v_proj.bias)
 
 
 class _AttnFn(torch.autograd.Function):
-    """MultiHeadAttention.forward as a unit: projections + attention core + `+ query` residual."""
+    """MultiHeadAttention.forward as a unit: projections + attention core + `+ query` residual; dropout at site 3 under (seed,
+    seed_dev), the backward re-deriving the forward's mask from them."""
 
     @staticmethod
-    def forward(ctx, query, key_value, mask, H, p, wq, bq, wk, bk, wv, bv):
+    def forward(ctx, query, key_value, mask, H, p, seed, sd, wq, bq, wk, bk, wv, bv):
         require_cuda(query, key_value)
         ensure_device(query.device)
         q = query.detach().contiguous().float()
@@ -96,54 +103,52 @@ class _AttnFn(torch.autograd.Function):
         Q, _ = Fn.linear_fwd(qb, wqb, bq.detach(), 0)
         K, _ = Fn.linear_fwd(kvb, wkb, bk.detach(), 0)
         V, _ = Fn.linear_fwd(kvb, wvb, bv.detach(), 0)
-        seed = Fn.dropout_seed(p)
-        att, lse = Fn.sasrec_attention_fwd(Q, K, V, pad, H, p, seed, None, 0)
+        att, lse = Fn.sasrec_attention_fwd(Q, K, V, pad, H, p, seed, sd, 0)
         ctx.save_for_backward(pad, qb, kvb, Q, K, V, att, lse, wqb, wkb, wvb)
-        ctx.cfg = (H, p, seed)
+        ctx.cfg = (H, p, seed, sd)
         return att.float() + q
 
     @staticmethod
     def backward(ctx, dout):
         pad, qb, kvb, Q, K, V, att, lse, wqb, wkb, wvb = ctx.saved_tensors
-        H, p, seed = ctx.cfg
+        H, p, seed, sd = ctx.cfg
         dout = dout.contiguous().float()
-        dQ, dK, dV = Fn.sasrec_attention_bwd(Q, K, V, pad, att, lse, Fn.cast_rows_bf16(dout), H, p, seed, None, 0)
+        dQ, dK, dV = Fn.sasrec_attention_bwd(Q, K, V, pad, att, lse, Fn.cast_rows_bf16(dout), H, p, seed, sd, 0)
         dq, dwq, dbq = Fn.linear_bwd(dQ, wqb, qb, dx_residual=dout)
         dk, dwk, dbk = Fn.linear_bwd(dK, wkb, kvb)
         dkv, dwv, dbv = Fn.linear_bwd(dV, wvb, kvb, dx_residual=dk)
-        return dq, dkv, None, None, None, dwq, dbq, dwk, dbk, dwv, dbv
+        return dq, dkv, None, None, None, None, None, dwq, dbq, dwk, dbk, dwv, dbv
 
 
 class _FfnFn(torch.autograd.Function):
     """PointWiseFeedForward.forward as a unit (sasrec.py:258-266): fc1 + ReLU + dropout, fc2 + dropout + residual - the same two
-    fused-epilogue GEMMs the block path runs."""
+    fused-epilogue GEMMs the block path runs, at sites 1 and 2 under (seed, seed_dev)."""
 
     @staticmethod
-    def forward(ctx, x, residual, p, w1, b1, w2, b2):
+    def forward(ctx, x, residual, p, seed, sd, w1, b1, w2, b2):
         require_cuda(x, residual)
         ensure_device(x.device)
         xf = x.detach().contiguous().float()
         res = residual.detach().contiguous().float()
         w1b, w2b = Fn.cast_bf16(w1), Fn.cast_bf16(w2)
         xb = Fn.cast_rows_bf16(xf)
-        seed = Fn.dropout_seed(p)
-        y, z1, a1 = Fn.ffn_fwd(xb, w1b, b1.detach(), w2b, b2.detach(), res, None, p, p, seed, None, SITE_HID, SITE_OUT)
+        y, z1, a1 = Fn.ffn_fwd(xb, w1b, b1.detach(), w2b, b2.detach(), res, None, p, p, seed, sd, SITE_HID, SITE_OUT)
         ctx.save_for_backward(xb, z1, a1, w1b, w2b)
-        ctx.cfg = (p, seed)
+        ctx.cfg = (p, seed, sd)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         xb, z1, a1, w1b, w2b = ctx.saved_tensors
-        p, seed = ctx.cfg
+        p, seed, sd = ctx.cfg
         dy = dy.contiguous().float()
-        dx, dw1, db1, dw2, db2 = Fn.ffn_bwd(dy, w1b, w2b, xb, z1, a1, p, p, seed, None, SITE_HID, SITE_OUT)
-        return dx, dy, None, dw1, db1, dw2, db2
+        dx, dw1, db1, dw2, db2 = Fn.ffn_bwd(dy, w1b, w2b, xb, z1, a1, p, p, seed, sd, SITE_HID, SITE_OUT)
+        return dx, dy, None, None, None, dw1, db1, dw2, db2
 
 
-class PointWiseFeedForward(nn.Module):
+class PointWiseFeedForward(Fn.StepSeeds, nn.Module):
     """Mirror of genrec/models/sasrec.py:249-266.  Inside a SASRecBlock the fused block path runs it; called on its own it is the
-    same pair of kernels behind an autograd function."""
+    same pair of kernels behind an autograd function, drawing a fresh dropout mask on each training call (``StepSeeds``)."""
 
     def __init__(self, embed_dim: int, ffn_dim: int, dropout: float):
         super().__init__()
@@ -151,14 +156,20 @@ class PointWiseFeedForward(nn.Module):
         self.fc2 = nn.Linear(ffn_dim, embed_dim)
         self.dropout = nn.Dropout(dropout)
 
+    @property
+    def _dropout_p(self) -> float:
+        return self.dropout.p
+
     def forward(self, x: torch.Tensor, residual: torch.Tensor) -> torch.Tensor:
         """x: normalised input [B, L, D]; residual: the block input [B, L, D]  ->  fc2(drop(relu(fc1(x)))) dropped + residual."""
-        return _FfnFn.apply(x, residual, self.dropout.p if self.training else 0.0, self.fc1.weight, self.fc1.bias, self.fc2.weight,
-                            self.fc2.bias)
+        seed, sd = self._seeds(x.device)
+        return _FfnFn.apply(x, residual, self.dropout.p if self.training else 0.0, seed, sd, self.fc1.weight, self.fc1.bias,
+                            self.fc2.weight, self.fc2.bias)
 
 
-class SASRecBlock(nn.Module):
-    """Mirror of genrec/models/sasrec.py:141-165."""
+class SASRecBlock(Fn.StepSeeds, nn.Module):
+    """Mirror of genrec/models/sasrec.py:141-165.  SASRec passes each block its step's seeds; called on its own without them, a
+    training block draws fresh dropout masks on each call (``StepSeeds``)."""
 
     def __init__(self, embed_dim: int, num_heads: int, ffn_dim: int, dropout: float):
         super().__init__()
@@ -169,15 +180,23 @@ class SASRecBlock(nn.Module):
         self.layer_index = 0
         self.p = dropout
 
+    @property
+    def _dropout_p(self) -> float:
+        return self.p
+
     def _params(self):
         a, f = self.attention, self.ffn
         return (self.norm1.weight, self.norm1.bias, a.q_proj.weight, a.q_proj.bias, a.k_proj.weight, a.k_proj.bias, a.v_proj.weight,
                 a.v_proj.bias, self.norm2.weight, self.norm2.bias, f.fc1.weight, f.fc1.bias, f.fc2.weight, f.fc2.bias)
 
-    def forward(self, x: torch.Tensor, mask: torch.Tensor, _apply_mask: bool = False, _seed: int = 0, _seed_dev=None) -> torch.Tensor:
-        """x [B,L,D] fp32, mask [B,L,1] float (1 = valid)."""
+    def forward(self, x: torch.Tensor, mask: torch.Tensor, _apply_mask: bool = False, _seed: Optional[int] = None,
+                _seed_dev=None) -> torch.Tensor:
+        """x [B,L,D] fp32, mask [B,L,1] float (1 = valid).  _seed / _seed_dev: the step's seeds (SASRec passes them); None: the
+        block's own."""
         require_cuda(x)
         ensure_device(x.device)
+        if _seed is None:
+            _seed, _seed_dev = self._seeds(x.device)
         B, L, _ = x.shape
         rowmask = mask.reshape(B * L).float().contiguous()
         pad = (rowmask == 0).to(torch.uint8).view(B, L).contiguous()
@@ -208,6 +227,10 @@ class SASRec(Fn.StepSeeds, nn.Module):
         self.final_norm = nn.LayerNorm(embed_dim, eps=1e-8)
         self.return_train_logits = False
         self._init_weights()
+
+    @property
+    def _dropout_p(self) -> float:
+        return self.emb_dropout.p
 
     def _init_weights(self):
         """genrec/models/sasrec.py:64-77."""

@@ -360,7 +360,9 @@ int grb_head_rank(const float* x, const float* ln_g, const float* ln_b, float ln
 
 /* ------------------------------------------------------------------------------------------------ SASRec attention
  * Replaces MultiHeadAttention.forward (genrec/models/sasrec.py:192-246) after the three projections:
- *   out = softmax_j(mask(Q K^T * dh^-1/2)) * query_mask @ V     (residual and projections are GEMM epilogues) */
+ *   out = softmax_j(mask(Q K^T * dh^-1/2)) * query_mask @ V     (residual and projections are GEMM epilogues)
+ * A padded batch needs B*L*H < 2^31 and B*L*D <= INT32_MAX (the dropout row key (b H + h) L + i and the row offsets are 32-bit);
+ * a larger one is refused before any launch. */
 typedef struct {
     int B, L, D, H;
     float dropout_p; uint64_t seed; const uint64_t* seed_dev; int layer_index;

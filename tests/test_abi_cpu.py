@@ -57,3 +57,23 @@ def test_product_never_imports_oracle():
                 if f.endswith(".py"):
                     src = open(os.path.join(dp, f)).read()
                     assert not re.search(r"^\s*(from|import)\s+oracle\b", src, re.M), os.path.join(dp, f)
+
+
+@pytest.mark.parametrize("B,L,D,H,refused", [
+    (512, 65536, 64, 2, True),          # B L D = 2^31: the row offsets overflow int32
+    (32768, 65536, 32, 1, True),        # B L H = 2^31: the dropout row key (b H + h) L + i overflows too
+    (1801, 18631, 64, 2, False),        # B L D = 2^31 - 64: in range
+])
+def test_padded_sasrec_attention_refuses_rows_past_int32(lib, B, L, D, H, refused):
+    """The padded SASRec attention entry points check B L H and B L D before anything else: a batch past int32 is refused with the
+    bound, one inside it goes on to the next check (null pointers here, so nothing is launched and no memory is needed)."""
+    from genrec_b200._lib import SasrecDims
+    d = SasrecDims(B, L, D, H, 0.2, 1, None, 0)
+    fwd = lib.grb_sasrec_attention_forward(ctypes.byref(d), *([None] * 7))
+    fwd_msg = lib.grb_last_error()
+    bwd = lib.grb_sasrec_attention_backward(ctypes.byref(d), *([None] * 11))
+    bwd_msg = lib.grb_last_error()
+    assert fwd != 0 and bwd != 0
+    for msg in (fwd_msg, bwd_msg):
+        assert (b"out of range" in msg) == refused, msg
+        assert (b"null argument" in msg) == (not refused), msg
